@@ -1,11 +1,12 @@
 #!/usr/bin/env python
 """bench.py — UNet sampler steps/s at 1024x1024 bs=1 (BASELINE.json metric), SDXL base, synthetic weights.
 
-  python bench.py --gpus N --steps K --warmup W            our arm (libsdxl_b200.so, sm_100a kernels)
+  python bench.py --gpus N --steps K --warmup W            our arm (libsdxl_b200.so, sm_90a kernels)
   python bench.py --impl reference --gpus N --steps K ...  CPU arm: the restated oracle on the host cores
   torchrun --nproc-per-node N bench.py --gpus N ...        one process per GPU, prompt-sharded replicas
 
   ... --workload image|refiner|inpaint                     whole images through sdxl_sample_latent (BASELINE configs 3, 4, 5)
+  ... --dump-outputs DIR                                   after the timed steps, write the final latent as DIR/<name>.npy
 
 A "step" = one iteration of the reference's sampler loop body (src/model/stablediffusion/mod.rs:406-429):
 alpha lookups, forward_diffuser (conditional + unconditional UNet evaluation, CFG combine) and the DDIM
@@ -47,24 +48,12 @@ def read_peaks():
         return {"tflops": float(p["bf16_tflops_sustained"]), "tflops_burst": float(p["bf16_tflops"]), "hbm_gbs": float(p["hbm_gbs"]),
                 "src": "measured (MEASURED_PEAKS.json: cuBLAS bf16 sustained, 1350 MHz under the 1 kW cap; burst = best of 10)"}
     except Exception:
-        return {"tflops": 1400.0, "tflops_burst": 1590.0, "hbm_gbs": 6650.0, "src": "fallback (B200_PROFILING.md: ~1.4 PFLOP/s sustained, 1.59 burst)"}
-
-
-def read_parity():
-    """Final-latent parity of the CUDA path against the oracle at BASELINE's own configs (tests/test_fullsize_parity_gpu.py on a
-    B200; committed copy of the test's output)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_parity.json")) as fh:
-            d = json.load(fh)
-        c2 = d.get("config2_1024_31it_cfg7.5", {})
-        return {"final_latent_rel": c2.get("rel_err"), "bound": 1e-3, "config": "SDXL base 1024x1024, 31 iterations, cfg 7.5 vs CPU f32 oracle (parity unpinned: the reference cannot be built)",
-                "all": {k: v.get("rel_err") for k, v in d.items() if isinstance(v, dict) and "rel_err" in v}, "source": "profiles/r2_parity.json"}
-    except Exception:
-        return None
+        return {"tflops": 989.0, "tflops_burst": 989.0, "hbm_gbs": 3350.0,
+                "src": "data sheet, not measured (H100 SXM at 700 W: dense f16 989 TFLOP/s, HBM3 3.35 TB/s)"}
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons sampled (read-only query) during the timed region."""
 
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -102,6 +91,15 @@ class ClockSampler:
             except Exception:
                 pass
         return {"sm_mhz": statistics.median(sm) if sm else None, "sm_max_mhz": mx or None, "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def dump_outputs(directory: str, arrays) -> None:
+    """Writes what the timed path returned in its last step as <directory>/<name>.npy (float32), for output-by-output comparison
+    of two builds run with the same arguments (the inputs are seeded)."""
+    import numpy as np
+    os.makedirs(directory, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(directory, f"{name}.npy"), t.detach().float().cpu().numpy())
 
 
 def make_conditioning(rank: int, device):
@@ -322,6 +320,8 @@ def run_ours(args, rank: int, local_rank: int, world: int):
     torch.cuda.nvtx.range_pop()
     barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"latent": diffuser.sampler_get_latent(torch.empty(1, 4, HW // 8, HW // 8))})
     ms_total = e0.elapsed_time(e1)
     launches = ctx.launch_count - launches0
     ms_step = sharding.max_over_ranks(ms_total, dev) / args.steps   # timing rule: max over ranks of the device time
@@ -340,7 +340,7 @@ def run_ours(args, rank: int, local_rank: int, world: int):
     if args.dump_ops:
         diffuser.profile_dump(args.dump_ops)
     peaks = read_peaks()
-    ig = prof["igemm_tcgen05"]
+    ig = prof["igemm_wgmma"]
     step_flops = diffuser.plan_flops
     exec_flops = diffuser.plan_flops_executed
     total_prof_ms = sum(v["ms"] for v in prof.values())
@@ -351,15 +351,12 @@ def run_ours(args, rank: int, local_rank: int, world: int):
     ig_ms_in_step = share * ms_step
     ach = ig["flops"] / (ig_ms_in_step * 1e-3) / 1e12
     ach_eager = ig["flops"] / (ig["ms"] * 1e-3) / 1e12
-    at = prof.get("attention_tcgen05")
+    at = prof.get("attention_wgmma")
     whole = step_flops / (ms_step * 1e-3) / 1e12
     roofline = {
         "bound": "tensor", "achieved": ach, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": ach / peaks["tflops"],
         "frac_vs_burst": ach / peaks["tflops_burst"], "peak_burst": peaks["tflops_burst"],
-        # dram__bytes_read+write of the largest igemm launch (FF-in GEGLU, M=2048 N=10240 K=1280; algorithmic bytes
-        # 26.2 MB weights + 5.2 MB activations in + 21 MB out) from the ncu --set full capture under profiles/
-        "traffic": 32.63e6, "traffic_unit": "bytes/launch (ncu --set full, profiles/r2_ncu_full_igemm.csv: FF-in GEGLU launch, 31.57 MB read + 1.05 MB written, tensor pipe 72.3 % active; algorithmic operand bytes 31.4 MB: the weights stream once)",
-        "kernel": "igemm_pair_kernel / igemm_kernel (tcgen05 implicit GEMM: all Linear + conv of the step)",
+        "kernel": "igemm_kernel (wgmma implicit GEMM: all Linear + conv of the step)",
         "peak_source": peaks["src"],
         "how": "algorithmic FLOPs of the step's igemm launches / (their share of an eager CUDA-event profile of the same plan x the measured graph step)",
         "achieved_eager_events": ach_eager,
@@ -406,14 +403,13 @@ def run_ours(args, rank: int, local_rank: int, world: int):
         "ms_per_step": ms_step, "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f16", "data": "synthetic",
         "config": {"workload": "SDXL base 1024x1024, n=30 (31 DDIM iterations/image), cfg=7.5, bs=1 per GPU; step = CFG-batched UNet eval (2 forwards) + CFG + DDIM update",
                    "parallelism": f"replicas x{world} (prompt-sharded, NCCL weight broadcast at load, no in-step collective)",
-                   "weights": "synthetic N(0,1/fan_in) f16, seed 0, 2.5675 B params", "l2": "per-step working set = 5.1 GB of weights >> 126 MB L2 (no flush needed)",
+                   "weights": "synthetic N(0,1/fan_in) f16, seed 0, 2.5675 B params", "l2": "per-step working set = 5.1 GB of weights >> 50 MB L2 (no flush needed)",
                    "forwards_per_sec": 2 * value, "images_per_sec_unet_only": value / len(ts), "load_seconds": round(load_s, 2),
                    "accumulate": "f32 (operands f16, residual stream / norms / softmax / sampler f32)"},
         "clocks": clocks, "gpu_launches": int(launches),
         "e2e": {"value": e2e_value, "unit": UNIT, "h2d_bytes_per_step": lat_n * 4 + 4, "d2h_bytes_per_step": lat_n * 4, "steps": e2e_steps, "ms_per_step_median": e2e_ms, "ms_per_step_mean": e2e_mean_ms,
                 "how": "sdxl_sampler_step_host: pinned host latent -> device, CFG step, latent -> host, stream sync; wall clock per step, value = 1 / median step (mean beside it)"},
         "roofline": roofline,
-        "parity": read_parity(),
     }
     if cpu_baseline is not None:
         line["cpu_baseline"] = cpu_baseline
@@ -476,12 +472,15 @@ def run_images(args, rank, local_rank, world, ctx, base, refiner, dist, comm, lo
     launches0 = ctx.launch_count
     sampler.start()
     e0.record(ctx.stream)
+    lat = None
     for _ in range(args.steps):
-        one_image()
+        lat = one_image()
     e1.record(ctx.stream)
     ctx.synchronize()
     barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0 and lat is not None:
+        dump_outputs(args.dump_outputs, {"latent": lat})
     ms_img = sharding.max_over_ranks(e0.elapsed_time(e1), dev) / args.steps
     value = world * 1e3 / ms_img
     launches = ctx.launch_count - launches0
@@ -512,7 +511,7 @@ def run_images(args, rank, local_rank, world, ctx, base, refiner, dist, comm, lo
                                     "inpaint": "BASELINE config 5: SDXL base inpainting 1024x1024, mask = top 25 latent rows (200 px), n=100, cfg 7.5, seeded per-step noise"}[wl],
                        "parallelism": f"replicas x{world} (prompt-sharded, sdxl_unet_load_broadcast at load, no in-step collective)",
                        "iterations_per_image": iters, "sampler_steps_per_sec": value * iters, "load_seconds": round(load_s, 2),
-                       "l2": "per-step working set = 5.1 GB of weights >> 126 MB L2 (no flush needed)"},
+                       "l2": "per-step working set = 5.1 GB of weights >> 50 MB L2 (no flush needed)"},
             "clocks": clocks, "gpu_launches": int(launches),
             "roofline": {"bound": "tensor", "achieved": tf, "peak": peaks["tflops"], "unit": "TFLOP/s", "frac": tf / peaks["tflops"], "frac_vs_burst": tf / peaks["tflops_burst"],
                          "flops_per_image": fl_img, "kernel": "whole image (all launches)", "peak_source": peaks["src"]},
@@ -536,6 +535,8 @@ def main():
     ap.add_argument("--workload", default="step", choices=["step", "image", "refiner", "inpaint"],
                     help="step (default): BASELINE metric, sampler steps/s at 1024^2 bs=1; image / refiner / inpaint: whole images (configs 3 / 4 / 5)")
     ap.add_argument("--dump-ops", default=None, help="write a per-launch CSV of one step (CUDA-event times)")
+    ap.add_argument("--dump-outputs", default=None, metavar="DIR",
+                    help="after the timed steps, write what the last step computed (the final latent) as DIR/<name>.npy, float32")
     args = ap.parse_args()
     if args.warmup < 3 and args.workload == "step":
         args.warmup = 3
@@ -549,7 +550,8 @@ def main():
         # launched without torchrun: re-exec under torch.distributed.run
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", f"--nproc-per-node={args.gpus}", "--master-addr", "127.0.0.1",
                "--master-port", os.environ.get("MASTER_PORT", "29541"), os.path.abspath(__file__), "--gpus", str(args.gpus), "--steps", str(args.steps),
-               "--warmup", str(args.warmup), "--workload", args.workload] + (["--no-cpu-baseline"] if args.no_cpu_baseline else [])
+               "--warmup", str(args.warmup), "--workload", args.workload] + (["--no-cpu-baseline"] if args.no_cpu_baseline else []) + \
+              (["--dump-outputs", args.dump_outputs] if args.dump_outputs else [])
         sys.exit(subprocess.call(cmd))
     run_ours(args, rank, local_rank, world)
 

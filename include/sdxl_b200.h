@@ -1,4 +1,4 @@
-/* sdxl_b200.h — C ABI of the B200-native SDXL denoising engine (libsdxl_b200.so).
+/* sdxl_b200.h — C ABI of the H100-native (sm_90a) SDXL denoising engine (libsdxl_b200.so).
  *
  * This is the drop-in boundary for the diffusion sampling path of Gadersd/stable-diffusion-xl-burn:
  * the entry points a Rust `src/backend.rs` replacement would bind with `extern "C"` (see
@@ -17,7 +17,7 @@
  *  - One sdxl_ctx per (device, stream). A ctx and the objects created from it are not thread-safe;
  *    independent ctxs are fully concurrent. All work is enqueued on the ctx stream; functions that
  *    return results to host memory synchronise that stream, all others are asynchronous.
- *  - There is NO CPU fallback: on a machine without an sm_100 GPU sdxl_ctx_create fails.
+ *  - There is NO CPU fallback: on a machine without an sm_90 GPU sdxl_ctx_create fails.
  */
 #ifndef SDXL_B200_H_
 #define SDXL_B200_H_
@@ -158,7 +158,7 @@ SDXL_API int sdxl_unet_plan_num_ops(const sdxl_unet* unet);
  * phase-decomposed upsample convolutions at their real cost and with channel / key padding (bench: `executed_flops`). */
 SDXL_API double sdxl_unet_plan_flops_executed(const sdxl_unet* unet);
 /* Device time of ONE execution of the current launch plan, summed per kernel kind and measured with CUDA
- * events on the ctx stream (eager launches). Kind index: 0 implicit-GEMM (tcgen05), 1 attention, 2 GroupNorm,
+ * events on the ctx stream (eager launches). Kind index: 0 implicit-GEMM (wgmma), 1 attention, 2 GroupNorm,
  * 3 LayerNorm, 4 GEMV, 5 timestep-embedding, 6 first conv, 7 upsample copy, 8 phase-split copy, 9 f32->f16 cast.
  * All three arrays hold SDXL_PROFILE_KINDS entries (host). Used by bench.py for the per-kernel roofline. */
 SDXL_API int sdxl_unet_profile_plan(sdxl_unet* unet, double* ms_by_kind_host, double* flops_by_kind_host,

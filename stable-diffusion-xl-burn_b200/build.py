@@ -1,4 +1,4 @@
-"""Builds libsdxl_b200.so (hand-written sm_100a CUDA + C++ host, C ABI in include/sdxl_b200.h).
+"""Builds libsdxl_b200.so (hand-written sm_90a CUDA + C++ host, C ABI in include/sdxl_b200.h).
 
 In-tree build with plain nvcc (cross-compiles on a machine without a GPU). The .so is git-ignored but
 travels with the repo snapshot to the GPU box. `python build.py` or `build_library()`.
@@ -19,7 +19,7 @@ SOURCES = ["igemm.cu", "attention.cu", "norm.cu", "elementwise.cu", "vae_kernels
 HEADERS = ["common.cuh", "kernels.h", "engine_core.h", "unicode_tables.h", os.path.join("..", "..", "include", "sdxl_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
 ]
 
@@ -52,7 +52,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
 
     with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
         objs = list(ex.map(cc, SOURCES))
-    cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_100a,code=sm_100a", "-Xcompiler", "-fPIC", "-ldl"]
+    cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-ldl"]
     r = subprocess.run(cmd, capture_output=True, text=True)
     if r.returncode != 0:
         raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")

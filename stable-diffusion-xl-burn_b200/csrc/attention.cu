@@ -1,26 +1,13 @@
 // Fused multi-head attention for the UNet's SpatialTransformer blocks (head dim 64, no mask):
 //   out = softmax(q k^T / sqrt(64)) v            (reference src/backend.rs:4-19,32-79,88-128;
 //                                                 called from unet/mod.rs:1013-1019)
-// Flash-style on tcgen05 tensor cores; scores, probabilities and the output accumulator all live in TMEM:
-//   S_x = Q_x K^T : A = Q tile (K-major, TMA SW128 smem), B = K tile (K-major smem)        -> TMEM S_x (128 f32 columns)
-//   P_x           : written by the softmax warps straight back to TMEM as packed f16 (tcgen05.st, 64 columns)
-//   O_x += P_x V  : A = P_x FROM TMEM, B = V tile (MN-major smem: keys are the contraction)  -> TMEM O_x (64 f32 columns)
-// One CTA works on TWO 128-query tiles (slots A, B) of one head and streams the 128-key blocks once for both; two softmax
-// warpgroups (one thread per query row) ping-pong against one MMA issuer, so the tensor pipe runs slot B's P V / Q K^T while
-// slot A is in its exp phase and vice versa. O accumulates in TMEM across key blocks (no per-block read-back): the exponent
-// reference of a row is lazy (re-based only when the running max grew by more than 2^8; exact max for the first block, warp-
-// uniform overflow-safe redo), and the rare re-base rescales the row's O in TMEM in place. The CTA is persistent over a
-// contiguous range of (batch, head, query tile) work items and all barriers run with continuous phases, so the Q load, first
-// Q K^T and the output write-back of consecutive items overlap (no drain / re-initialisation between items).
-// What bounds d = 64 attention is the XU pipe (16 lanes / clk / SM): it executes both the MUFU ex2 and the F2FP f32->f16 pack
-// of P (1.5 XU instructions per score vs 4 clk of tensor time per 128 scores and row). ONE warp per scheduler cannot keep
-// that pipe busy (in-order issue, ~500 clk per 32-column chunk measured against a 384 clk pipe floor), so every query row is
-// shared by TWO threads (64 score columns each): two warps per scheduler and slot. Measured alternatives that did not pay and
-// were removed (profiles/README.md, round 2): evaluating a fraction of the exponentials on the FMA pipe (Cody-Waite +
-// degree-4 polynomial) and packing P with integer ops instead of F2FP both trade XU time for issue slots one for one.
-// Warp roles (576 threads): warp0 TMA producer, warp1 MMA issuer + TMEM owner, warps 2..9 softmax slot A, 10..17 slot B
-// (warp w of a slot: TMEM lane quarter w % 4, column half (w - 2) / 4 % 2).
-// TMEM columns: S_A [0,128) S_B [128,256) O_A [256,320) O_B [320,384) P_A [384,448) P_B [448,512).
+// Flash-style on Hopper tensor cores (wgmma); scores, probabilities and the output accumulator live in registers:
+//   S = Q K^T : wgmma m64n128k16, A = Q tile (K-major, TMA SW128 smem), B = K tile (K-major smem)     -> registers (f32)
+//   P         : online softmax on the S registers, packed to f16 in place as the A fragments of the next wgmma
+//   O += P V  : wgmma m64n64k16, A = P from registers, B = V tile (MN-major smem: keys are the contraction) -> registers (f32)
+// One CTA per (batch, head, 128-query tile): two consumer warpgroups own 64 query rows each, one producer warp streams the
+// 128-key K / V blocks through a TMA ring. The running max is exact per key block (the row is rescaled when it grows), so
+// every probability is <= 1 before the f16 rounding.
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -30,475 +17,151 @@ namespace sdxl {
 
 static constexpr int kTileBytes = 128 * 128;        // 128 rows x 64 halves (Q, K or V tile)
 static constexpr int kKvStages = 3;
-static constexpr int kQSlots = 4;                   // ring of two items x two slots
-static constexpr int kXchgBytes = 2 * 2 * 2 * 128 * 4;   // [buffer][slot][column half][row] f32
-static constexpr int kAttnSmem = kQSlots * kTileBytes + 2 * kKvStages * kTileBytes + 512 + kXchgBytes;
-static constexpr uint32_t kColS = 0, kColO = 256, kColP = 384;
+static constexpr int kConsumerWarps = 8;
+static constexpr int kAttnThreads = kConsumerWarps * 32 + 32;
+static constexpr int kAttnSmem = 1024 /*align slack*/ + kTileBytes + 2 * kKvStages * kTileBytes + 256;
 
 __device__ __forceinline__ float ex2_approx(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
+__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
+  __half2 t = __floats2half2_rn(a, b);
+  return *reinterpret_cast<uint32_t*>(&t);
 }
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, "
-      "%18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32};"
-      ::"r"(taddr), "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-        "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15]), "r"(r[16]), "r"(r[17]), "r"(r[18]), "r"(r[19]),
-        "r"(r[20]), "r"(r[21]), "r"(r[22]), "r"(r[23]), "r"(r[24]), "r"(r[25]), "r"(r[26]), "r"(r[27]), "r"(r[28]), "r"(r[29]),
-        "r"(r[30]), "r"(r[31])
-      : "memory");
-}
-__device__ __forceinline__ void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// Four K=16 MMAs of S = Q K^T (both operands in SW128 smem, 32-byte descriptor steps) + commit, one elect.
-__device__ __forceinline__ void mma_qk_commit(uint32_t d_tmem, uint32_t q_lo, uint32_t k_lo, uint32_t desc_hi, uint32_t idesc,
-                                              uint64_t* bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred e, t, f;\n\t"
-      ".reg .b64 da, db;\n\t"
-      ".reg .b32 al, bl;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      "setp.ne.b32 f, 0, 0;\n\t"
-      "mov.b64 da, {%1, %3};\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, f;\n\t"
-      "add.u32 al, %1, 2;\n\t"
-      "add.u32 bl, %2, 2;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, t;\n\t"
-      "add.u32 al, %1, 4;\n\t"
-      "add.u32 bl, %2, 4;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, t;\n\t"
-      "add.u32 al, %1, 6;\n\t"
-      "add.u32 bl, %2, 6;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, t;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%5];\n\t"
-      "}"
-      ::"r"(d_tmem), "r"(q_lo), "r"(k_lo), "r"(desc_hi), "r"(idesc), "r"(smem_u32(bar))
-      : "memory");
-}
-// Eight K=16 MMAs of O (+)= P V: A = P in TMEM (8 columns of packed f16 per step), B = V in smem (MN-major, 16 key rows =
-// 2048 B per step). `acc_first` = accumulate flag of the first MMA (0 for the first key block of a work item).
-__device__ __forceinline__ void mma_pv(uint32_t d_tmem, uint32_t p_tmem, uint32_t v_lo, uint32_t desc_hi, uint32_t idesc,
-                                       uint32_t acc_first) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred e, t, p;\n\t"
-      ".reg .b64 db;\n\t"
-      ".reg .b32 pa, bl;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], db, %4, p;\n\t"
-      "add.u32 pa, %1, 8;\n\t   add.u32 bl, %2, 128;\n\t  mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [pa], db, %4, t;\n\t"
-      "add.u32 pa, %1, 16;\n\t  add.u32 bl, %2, 256;\n\t  mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [pa], db, %4, t;\n\t"
-      "add.u32 pa, %1, 24;\n\t  add.u32 bl, %2, 384;\n\t  mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [pa], db, %4, t;\n\t"
-      "add.u32 pa, %1, 32;\n\t  add.u32 bl, %2, 512;\n\t  mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [pa], db, %4, t;\n\t"
-      "add.u32 pa, %1, 40;\n\t  add.u32 bl, %2, 640;\n\t  mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [pa], db, %4, t;\n\t"
-      "add.u32 pa, %1, 48;\n\t  add.u32 bl, %2, 768;\n\t  mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [pa], db, %4, t;\n\t"
-      "add.u32 pa, %1, 56;\n\t  add.u32 bl, %2, 896;\n\t  mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], [pa], db, %4, t;\n\t"
-      "}"
-      ::"r"(d_tmem), "r"(p_tmem), "r"(v_lo), "r"(desc_hi), "r"(idesc), "r"(acc_first)
-      : "memory");
-}
-
-// One 32-column chunk of a score row: p = 2^(s*c - mb) -> packed f16 (16 words); tracks the block max of these columns
-// (two chains) and their f32 sum.
-__device__ __forceinline__ void softmax_chunk(const uint32_t (&v)[32], uint32_t (&h)[16], float sl2e, float mb, float& b0, float& b1,
-                                              float& sum, bool ragged, int col0, int S) {
-  float s_a = 0.f, s_b = 0.f;
-#pragma unroll
-  for (int i = 0; i < 32; i += 2) {
-    float s0 = __uint_as_float(v[i]), s1 = __uint_as_float(v[i + 1]);
-    if (ragged) {
-      if (col0 + i >= S) s0 = -INFINITY;
-      if (col0 + i + 1 >= S) s1 = -INFINITY;
-    }
-    b0 = fmaxf(b0, s0);
-    b1 = fmaxf(b1, s1);
-    const float p0 = ex2_approx(fmaf(s0, sl2e, -mb));
-    const float p1 = ex2_approx(fmaf(s1, sl2e, -mb));
-    s_a += p0;
-    s_b += p1;
-    __half2 t = __floats2half2_rn(p0, p1);
-    h[i >> 1] = *reinterpret_cast<uint32_t*>(&t);
-  }
-  sum += s_a + s_b;
-}
-
-static constexpr int SPLIT = 2;   // threads per query row
-static constexpr int kAttnThreads = 64 + 256 * SPLIT;
 
 __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid_constant__ AttnParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  uint8_t* sQ = smem;                                  // [kQSlots]
-  uint8_t* sK = sQ + kQSlots * kTileBytes;             // [kKvStages]
+  extern __shared__ uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* sQ = smem;
+  uint8_t* sK = sQ + kTileBytes;                       // [kKvStages]
   uint8_t* sV = sK + kKvStages * kTileBytes;           // [kKvStages]
   uint64_t* bars = reinterpret_cast<uint64_t*>(sV + kKvStages * kTileBytes);
-  uint64_t* q_full = bars;                       // [4]
-  uint64_t* q_empty = q_full + kQSlots;          // [4]
-  uint64_t* kv_full = q_empty + kQSlots;         // [3]
-  uint64_t* kv_empty = kv_full + kKvStages;      // [3]
-  uint64_t* s_full = kv_empty + kKvStages;       // [2] per slot
-  uint64_t* p_full = s_full + 2;                 // [2] per slot, 128 arrivals
-  uint64_t* o_full = p_full + 2;                 // [2] per slot: last P V of an item retired
-  uint64_t* pv_done = o_full + 2;                // [2] per slot: P V of the block retired (O may be rescaled, P rewritten)
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(pv_done + 2);
-  float* xchg = reinterpret_cast<float*>(sV + kKvStages * kTileBytes + 512);
+  uint64_t* q_full = bars;
+  uint64_t* kv_full = q_full + 1;                      // [kKvStages]
+  uint64_t* kv_empty = kv_full + kKvStages;            // [kKvStages]
 
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform: role code stays on the uniform datapath
-  const int lane = threadIdx.x & 31;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int nblk = (p.S + 127) / 128;
-  // Persistent: the (batch, head, 128-query tile) work list is split into contiguous, balanced ranges, one per CTA; inside
-  // its range a CTA takes two consecutive tiles of the same head as a two-slot item, a single tile otherwise.
   const int nqt = (p.T + 127) / 128;
-  const long total_tiles = (long)p.B * p.n_head * nqt;
-  const int t_begin = (int)(total_tiles * blockIdx.x / gridDim.x);
-  const int t_end = (int)(total_tiles * (blockIdx.x + 1) / gridDim.x);
+  const int qt = blockIdx.x % nqt, head = (blockIdx.x / nqt) % p.n_head, b = blockIdx.x / (nqt * p.n_head);
 
   if (threadIdx.x == 0) {
-    if (smem_u32(smem) & 1023u) {
-      printf("sdxl_b200: attention smem base not 1024B aligned\n");
-      __trap();
-    }
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmV);
-    for (int i = 0; i < kQSlots; ++i) { mbar_init(&q_full[i], 1); mbar_init(&q_empty[i], 1); }
-    for (int i = 0; i < kKvStages; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&s_full[i], 1); mbar_init(&p_full[i], 128 * SPLIT); mbar_init(&o_full[i], 1); mbar_init(&pv_done[i], 1); }
+    mbar_init(q_full, 1);
+    for (int i = 0; i < kKvStages; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], kConsumerWarps); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, 512);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   griddep_wait();  // PDL: the prologue above overlapped the previous kernel's tail
   griddep_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == kConsumerWarps) {
     // ===================== TMA producer =====================
-    if (lane == 0) {
-      uint32_t qe_ph = 0;
-      int kvc = 0, item = 0;
-      for (int tile = t_begin; tile < t_end; ++item) {
-        const int qt = tile % nqt, head = (tile / nqt) % p.n_head, b = tile / (nqt * p.n_head);
-        const bool hasB = (qt + 1 < nqt) && (tile + 1 < t_end);
-        tile += hasB ? 2 : 1;
-        for (int x = 0; x < (hasB ? 2 : 1); ++x) {
-          const int qs = (item & 1) * 2 + x;
-          mbar_wait(&q_empty[qs], ((qe_ph >> qs) & 1u) ^ 1u);
-          qe_ph ^= 1u << qs;
-          mbar_expect_tx(&q_full[qs], kTileBytes);
-          tma_load_3d(sQ + qs * kTileBytes, &p.tmQ, &q_full[qs], p.q_col0 + head * 64, qt * 128 + x * 128, b);
-        }
-        for (int j = 0; j < nblk; ++j, ++kvc) {
-          const int st = kvc % kKvStages;
-          mbar_wait(&kv_empty[st], ((kvc / kKvStages) & 1) ^ 1);
-          mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
-          tma_load_3d(sK + st * kTileBytes, &p.tmK, &kv_full[st], p.k_col0 + head * 64, j * 128, b);
-          tma_load_3d(sV + st * kTileBytes, &p.tmV, &kv_full[st], p.v_col0 + head * 64, j * 128, b);
-        }
-      }
+    if (lane != 0) return;
+    mbar_expect_tx(q_full, kTileBytes);
+    tma_load_3d(sQ, &p.tmQ, q_full, p.q_col0 + head * 64, qt * 128, b);
+    for (int j = 0; j < nblk; ++j) {
+      const int st = j % kKvStages;
+      mbar_wait_nocall(&kv_empty[st], ((j / kKvStages) & 1) ^ 1);
+      mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
+      tma_load_3d(sK + st * kTileBytes, &p.tmK, &kv_full[st], p.k_col0 + head * 64, j * 128, b);
+      tma_load_3d(sV + st * kTileBytes, &p.tmV, &kv_full[st], p.v_col0 + head * 64, j * 128, b);
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: warp-convergent loop, one elected lane issues =====================
-    const uint32_t idesc_qk = make_idesc_f16(128, false);
-    const uint32_t idesc_pv = make_idesc_f16(64, true);
-    const uint32_t dhi = 64u | (1u << 14) | (2u << 29);   // SBO=1024B, version, SWIZZLE_128B
-    const uint32_t lo_flag = 1u << 16;                     // LBO(enc)=1
-    const uint32_t q_lo0 = ((smem_u32(sQ) >> 4) & 0x3FFFu) | lo_flag;
-    const uint32_t k_lo0 = ((smem_u32(sK) >> 4) & 0x3FFFu) | lo_flag;
-    const uint32_t v_lo0 = ((smem_u32(sV) >> 4) & 0x3FFFu) | lo_flag;
-    constexpr uint32_t kTile16 = kTileBytes >> 4;
-    uint32_t qf_ph = 0, pf_ph = 0;
-    int kvc = 0, item = 0;
-    int dn = 0;
-    const bool dbg = p.dbg != nullptr && blockIdx.x == 0 && lane == 0;
-    // Issue order (one in-order tensor pipe, two slots): per hand-over of slot X at block j, S_X(j+1) = Q_X K_{j+1}^T goes FIRST
-    // (it is what the softmax warps wait for; S_X(j) is dead once P_X(j) exists), then O_X += P_X(j) V_j. Starting slot B half a
-    // period behind slot A was measured and makes no difference (any offset between the slots is neutrally stable).
-    for (int tile = t_begin; tile < t_end; ++item) {
-      const int qt = tile % nqt;
-      const bool hasB = (qt + 1 < nqt) && (tile + 1 < t_end);
-      tile += hasB ? 2 : 1;
-      const int qs0 = (item & 1) * 2;
-      mbar_wait(&q_full[qs0], (qf_ph >> qs0) & 1u);
-      qf_ph ^= 1u << qs0;
-      int st = kvc % kKvStages;
-      mbar_wait(&kv_full[st], (kvc / kKvStages) & 1);
-      tc_fence_after();
-      mma_qk_commit(tmem_base + kColS, q_lo0 + qs0 * kTile16, k_lo0 + st * kTile16, dhi, idesc_qk, &s_full[0]);
-      if (hasB) {
-        mbar_wait(&q_full[qs0 + 1], (qf_ph >> (qs0 + 1)) & 1u);
-        qf_ph ^= 1u << (qs0 + 1);
-        tc_fence_after();
-        mma_qk_commit(tmem_base + kColS + 128, q_lo0 + (qs0 + 1) * kTile16, k_lo0 + st * kTile16, dhi, idesc_qk, &s_full[1]);
-      }
-      for (int j = 0; j < nblk; ++j, ++kvc) {
-        const bool more = j + 1 < nblk;
-        st = kvc % kKvStages;
-        const int stn = (kvc + 1) % kKvStages;
-        // ---- slot A hands over P_A(j)
-        mbar_wait(&p_full[0], pf_ph & 1u);
-        pf_ph ^= 1u;
-        if (dbg && dn < 256) p.dbg[2048 + dn * 4 + 0] = clock64();
-        tc_fence_after();
-        if (more) {
-          mbar_wait(&kv_full[stn], ((kvc + 1) / kKvStages) & 1);
-          tc_fence_after();
-          mma_qk_commit(tmem_base + kColS, q_lo0 + qs0 * kTile16, k_lo0 + stn * kTile16, dhi, idesc_qk, &s_full[0]);
-        }
-        mma_pv(tmem_base + kColO, tmem_base + kColP, v_lo0 + st * kTile16, dhi, idesc_pv, j > 0 ? 1u : 0u);
-        tc_commit_elect(&pv_done[0]);
-        if (!more) {
-          tc_commit_elect(&o_full[0]);
-          tc_commit_elect(&q_empty[qs0]);
-        }
-        if (dbg && dn < 256) p.dbg[2048 + dn * 4 + 1] = clock64();
-        // ---- slot B hands over P_B(j)
-        if (hasB) {
-          mbar_wait(&p_full[1], (pf_ph >> 1) & 1u);
-          pf_ph ^= 2u;
-          if (dbg && dn < 256) p.dbg[2048 + dn * 4 + 2] = clock64();
-          tc_fence_after();
-          if (more) mma_qk_commit(tmem_base + kColS + 128, q_lo0 + (qs0 + 1) * kTile16, k_lo0 + stn * kTile16, dhi, idesc_qk, &s_full[1]);
-          mma_pv(tmem_base + kColO + 64, tmem_base + kColP + 64, v_lo0 + st * kTile16, dhi, idesc_pv, j > 0 ? 1u : 0u);
-          tc_commit_elect(&pv_done[1]);
-          if (!more) {
-            tc_commit_elect(&o_full[1]);
-            tc_commit_elect(&q_empty[qs0 + 1]);
-          }
-        }
-        tc_commit_elect(&kv_empty[st]);   // K_j / V_j are free once everything issued so far retires
-        if (dbg && dn < 256) p.dbg[2048 + dn * 4 + 3] = clock64();
-        ++dn;
-      }
-    }
-  } else {
-    // ===================== softmax warps: two threads per query row =====================
-    // Each thread owns 64 of a key block's 128 score columns (and 32 of the 64 output columns). The two threads of a row agree
-    // on the row's block max (and final sum) through shared memory.
-    constexpr int NCH = 4 / SPLIT;                   // 32-column chunks per thread and key block
-    constexpr int OCOLS = 64 / SPLIT;                // output columns per thread
-    const int sw = warp - 2;
-    const int x = sw / (4 * SPLIT);                  // slot: 0 = tile A, 1 = tile B
-    const int hf = (sw >> 2) & 1;                    // column half
-    const int q = warp & 3;                          // TMEM lane quarter this warp may access (hardware: warp id % 4)
-    const int r = q * 32 + lane;                     // query row in the tile == TMEM lane
-    const uint32_t lane_off = (uint32_t)(q * 32) << 16;
-    const uint32_t tS = tmem_base + lane_off + kColS + x * 128 + hf * 64;
-    const uint32_t tO = tmem_base + lane_off + kColO + x * 64 + hf * OCOLS;
-    const uint32_t tP = tmem_base + lane_off + kColP + x * 64 + hf * 32;
-    const float sl2e = p.scale_log2e;
-    uint32_t s_ph = 0, o_ph = 0, d_ph = 0;
-    bool pv_any = false;
-    int dn = 0, xk = 0;
-    const bool dbg = p.dbg != nullptr && blockIdx.x == 0 && q == 0 && lane == 0 && hf == 0;
-    // max over the row's two halves: double-buffered slots, one 64-thread named barrier per exchange
-    auto exchange_max = [&](float v) -> float {
-      float* slot = xchg + (((xk & 1) * 2 + x) * 2) * 128;
-      slot[hf * 128 + r] = v;
-      asm volatile("bar.sync %0, 64;" ::"r"(1 + x * 4 + q) : "memory");
-      const float o = slot[(hf ^ 1) * 128 + r];
-      ++xk;
-      return fmaxf(v, o);
-    };
-    for (int tile = t_begin; tile < t_end;) {
-      const int qt = tile % nqt, head = (tile / nqt) % p.n_head, b = tile / (nqt * p.n_head);
-      const bool hasB = (qt + 1 < nqt) && (tile + 1 < t_end);
-      tile += hasB ? 2 : 1;
-      if (x == 1 && !hasB) continue;
-      float m = -INFINITY, m_prev = -INFINITY, l = 0.f;
-      for (int j = 0; j < nblk; ++j) {
-        mbar_wait(&s_full[x], s_ph);   // S(j) complete
-        s_ph ^= 1u;
-        if (dbg && dn < 256) p.dbg[x * 1024 + dn * 4 + 0] = clock64();
-        tc_fence_after();
-        const int kbase = j * 128 + hf * 64;         // first key of this thread's columns
-        const bool ragged = j * 128 + 128 > p.S;
-        // Exponent reference. Block 0: exact row max (one extra pass over S). Later blocks: the reference decided at the end
-        // of the previous block (lazy): p = 2^((s - ref) c) may exceed 1 (f16 P and the f32 sums have the head-room).
-        float ref = m;
-        if (j == 0) {
-          float m0 = -INFINITY, m1 = -INFINITY, m2 = -INFINITY, m3 = -INFINITY;
-#pragma unroll 1
-          for (int c = 0; c < NCH * 32; c += 32) {
-            if (kbase + c >= p.S) break;
-            uint32_t v[32];
-            tmem_ld32(tS + c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int i = 0; i < 32; i += 4) {
-              if (!ragged || kbase + c + i < p.S) m0 = fmaxf(m0, __uint_as_float(v[i]));
-              if (!ragged || kbase + c + i + 1 < p.S) m1 = fmaxf(m1, __uint_as_float(v[i + 1]));
-              if (!ragged || kbase + c + i + 2 < p.S) m2 = fmaxf(m2, __uint_as_float(v[i + 2]));
-              if (!ragged || kbase + c + i + 3 < p.S) m3 = fmaxf(m3, __uint_as_float(v[i + 3]));
-            }
-          }
-          ref = exchange_max(fmaxf(fmaxf(m0, m1), fmaxf(m2, m3)));
-        }
-        float sum, bmax;
-        bool redo;
-        bool pv_pending = pv_any;   // a P V of this slot was issued before this block
-        pv_any = true;
-        do {
-          const float mb = ref * sl2e;
-          sum = 0.f;
-          float b0 = -INFINITY, b1 = -INFINITY;
-          // software pipeline over the 32-column chunks: the TMEM load of chunk c+1 flies while chunk c is exponentiated
-          uint32_t va[32], vb[32], h[16];
-          tmem_ld32(tS, va);
-#pragma unroll
-          for (int c = 0; c < NCH; ++c) {
-            tmem_ld_wait();
-            const bool live = kbase + c * 32 < p.S;          // warp-uniform: chunk has at least one valid key
-            const bool next_live = c < NCH - 1 && kbase + (c + 1) * 32 < p.S;
-            if (c & 1) {
-              if (next_live) tmem_ld32(tS + (c + 1) * 32, va);
-              if (live) softmax_chunk(vb, h, sl2e, mb, b0, b1, sum, ragged, kbase + c * 32, p.S);
-            } else {
-              if (next_live) tmem_ld32(tS + (c + 1) * 32, vb);
-              if (live) softmax_chunk(va, h, sl2e, mb, b0, b1, sum, ragged, kbase + c * 32, p.S);
-            }
-            if (!live) {
-#pragma unroll
-              for (int i = 0; i < 16; ++i) h[i] = 0u;
-            }
-            if (c == 0 && pv_pending) {
-              // The previous P V of this slot (issued right after this block's Q K^T) still reads P and writes O: it must have
-              // retired before P is overwritten / O is rescaled. One exp chunk later it practically always has.
-              mbar_wait(&pv_done[x], d_ph);
-              d_ph ^= 1u;
-              tc_fence_after();
-              pv_pending = false;
-            }
-            tmem_st16(tP + c * 16, h);
-          }
-          bmax = exchange_max(fmaxf(b0, b1));   // block max of the whole row: both threads of a row take identical decisions
-          // f16 P overflows beyond 2^16: redo the whole block with the exact max (all lanes: the TMEM ops are warp-collective;
-          // the partner warp holds the same rows, hence the same vote)
-          const bool over = (bmax - ref) * sl2e > 15.0f;
-          redo = __any_sync(0xffffffffu, over);
-          if (over) ref = bmax;
-          if (redo) tmem_st_wait();
-        } while (redo);
-        if (dbg && dn < 256) p.dbg[x * 1024 + dn * 4 + 1] = clock64();
-        if (j > 0) {
-          // the row's reference moved: rescale what has been accumulated so far (rare; O(j-1) is complete: pv_done above)
-          const bool moved = ref != m_prev;
-          if (__any_sync(0xffffffffu, moved)) {
-            const float alpha = moved ? ex2_approx((m_prev - ref) * sl2e) : 1.0f;
-            l *= alpha;
-#pragma unroll 1
-            for (int c = 0; c < OCOLS; c += 32) {
-              uint32_t o[32];
-              tmem_ld32(tO + c, o);
-              tmem_ld_wait();
-#pragma unroll
-              for (int i = 0; i < 32; ++i) o[i] = __float_as_uint(__uint_as_float(o[i]) * alpha);
-              tmem_st32(tO + c, o);
-            }
-          }
-        }
-        l += sum;                                        // partial sum over this thread's columns
-        m_prev = ref;
-        m = ((bmax - ref) * sl2e > 8.0f) ? bmax : ref;   // reference for the next block
-        tmem_st_wait();
-        tc_fence_before();
-        mbar_arrive(&p_full[x]);
-        if (dbg && dn < 256) p.dbg[x * 1024 + dn * 4 + 2] = clock64();
-        ++dn;
-      }
-      // ---- write-back: O / l -> f16 (the next item's Q K^T and first exp phase overlap this)
-      {
-        float* slot = xchg + (((xk & 1) * 2 + x) * 2) * 128;
-        slot[hf * 128 + r] = l;
-        asm volatile("bar.sync %0, 64;" ::"r"(1 + x * 4 + q) : "memory");
-        l += slot[(hf ^ 1) * 128 + r];
-        ++xk;
-      }
-      mbar_wait(&o_full[x], o_ph);
-      o_ph ^= 1u;
-      tc_fence_after();
-      const int t = qt * 128 + x * 128 + r;
-      const float inv = 1.0f / l;
-      __half* o = p.out + ((size_t)b * p.T + t) * p.ldo + head * 64 + hf * OCOLS;
-#pragma unroll 1
-      for (int c = 0; c < OCOLS; c += 32) {
-        uint32_t v[32];
-        tmem_ld32(tO + c, v);
-        tmem_ld_wait();
-        if (t < p.T) {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            uint32_t hh[4];
-#pragma unroll
-            for (int i = 0; i < 4; ++i) {
-              __half2 t2 = __floats2half2_rn(__uint_as_float(v[8 * u + 2 * i]) * inv, __uint_as_float(v[8 * u + 2 * i + 1]) * inv);
-              hh[i] = *reinterpret_cast<uint32_t*>(&t2);
-            }
-            *reinterpret_cast<uint4*>(o + c + 8 * u) = make_uint4(hh[0], hh[1], hh[2], hh[3]);
-          }
-        }
-      }
-      tc_fence_before();   // the TMEM reads above are ordered before this thread's next p_full arrival
-      if (dbg && dn <= 256) p.dbg[x * 1024 + (dn - 1) * 4 + 3] = clock64();   // write-back of this item done
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();   // every role is done: all MMAs retired (o_full observed), all barriers quiescent
-  tc_fence_after();
-  if (warp == 1) tmem_dealloc(tmem_base, 512);
+  // ===================== consumers: warpgroup wg owns query rows [64 wg, 64 wg + 64) of the tile =====================
+  // Accumulator layout (m64nN): thread holds rows r and r + 8 (h = 0, 1), columns 8 j + 2 (lane & 3) + e at index 4 j + 2 h + e.
+  const int wg = warp >> 2;
+  const float sl2e = p.scale_log2e;
+  const uint32_t q_addr = smem_u32(sQ) + (uint32_t)wg * (64 * 128);
+  float o[32];
+#pragma unroll
+  for (int i = 0; i < 32; ++i) o[i] = 0.f;
+  float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  mbar_wait_nocall(q_full, 0);
+  for (int j = 0; j < nblk; ++j) {
+    const int st = j % kKvStages;
+    mbar_wait_nocall(&kv_full[st], (j / kKvStages) & 1);
+    float s[64];
+    wg_fence();
+    const uint32_t k_addr = smem_u32(sK + st * kTileBytes);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) wgmma_ss_n128(s, wg_desc_sw128(q_addr + 32 * k), wg_desc_sw128(k_addr + 32 * k), k);
+    wg_commit();
+    wg_wait<0>();
+    if (j * 128 + 128 > p.S) {   // ragged last key block: keys past S do not exist
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          if (j * 128 + 8 * jj + 2 * (lane & 3) + e >= p.S) { s[4 * jj + e] = -INFINITY; s[4 * jj + 2 + e] = -INFINITY; }
+    }
+    uint32_t pa[32];
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float mx = -INFINITY;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+      mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+      const float m_new = fmaxf(m[h], mx);
+      const float alpha = ex2_approx((m[h] - m_new) * sl2e);
+      const float mb = m_new * sl2e;
+      float sum = 0.f;
+#pragma unroll
+      for (int jj = 0; jj < 16; ++jj) {
+        const float p0 = ex2_approx(fmaf(s[4 * jj + 2 * h], sl2e, -mb));
+        const float p1 = ex2_approx(fmaf(s[4 * jj + 2 * h + 1], sl2e, -mb));
+        sum += p0 + p1;
+        // A fragment of key chunk kk = jj / 2: {row r: keys 0-7, row r+8: keys 0-7, row r: keys 8-15, row r+8: keys 8-15}
+        pa[4 * (jj >> 1) + 2 * (jj & 1) + h] = pack_half2(p0, p1);
+      }
+      l[h] = l[h] * alpha + sum;
+      m[h] = m_new;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) { o[4 * jj + 2 * h] *= alpha; o[4 * jj + 2 * h + 1] *= alpha; }
+    }
+    wg_fence();
+    const uint32_t v_addr = smem_u32(sV + st * kTileBytes);
+#pragma unroll
+    for (int kk = 0; kk < 8; ++kk)
+      wgmma_rs_n64_tb(o, *reinterpret_cast<const uint32_t(*)[4]>(pa + 4 * kk), wg_desc_sw128(v_addr + 2048 * kk));
+    wg_commit();
+    wg_wait<0>();
+    if (lane == 0) mbar_arrive(&kv_empty[st]);   // this warp is done with K_j / V_j
+  }
+  // ---- write-back: O / l -> f16
+  const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float lt = l[h];
+    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+    const float inv = 1.0f / lt;
+    const int t = qt * 128 + r + 8 * h;
+    if (t < p.T) {
+      __half* out = p.out + ((size_t)b * p.T + t) * p.ldo + head * 64 + 2 * (lane & 3);
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj)
+        *reinterpret_cast<__half2*>(out + 8 * jj) = __floats2half2_rn(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+    }
+  }
 }
 
 // Per-device launch state (several devices may be driven from one process: the opt-in to > 48 KB of dynamic shared memory
 // is a per-device function attribute).
-struct AttnDev { bool attr = false; int num_sms = 0; };
-static AttnDev g_attn_dev[64];
+static bool g_attn_attr[64];
 int attention_launch(cudaStream_t st, const AttnParams& p) {
-  int dev = 0;
-  cudaError_t e = cudaGetDevice(&dev);
-  if (e != cudaSuccess) return (int)e;
-  if (dev < 0 || dev >= 64) return 2001;
-  AttnDev& D = g_attn_dev[dev];
-  if (!D.attr) {
-    e = cudaFuncSetAttribute(attention_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kAttnSmem);
-    if (e != cudaSuccess) return (int)e;
-    cudaDeviceGetAttribute(&D.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (D.num_sms <= 0) D.num_sms = 148;
-    D.attr = true;
-  }
+  if (p.T < 1 || p.S < 1 || (p.ldo & 1)) return 2002;
+  int r = smem_optin(attention_kernel, kAttnSmem, g_attn_attr);
+  if (r) return r;
   const long tiles = (long)p.B * p.n_head * ((p.T + 127) / 128);
-  const long want = (tiles + 1) / 2;  // one two-slot item per CTA when the machine is not full
-  dim3 grid((unsigned)(want < D.num_sms ? (want > 0 ? want : 1) : D.num_sms));
-  return launch_kernel(attention_kernel, grid, dim3(kAttnThreads), (size_t)kAttnSmem, st, true, p);
+  return launch_kernel(attention_kernel, dim3((unsigned)tiles), dim3(kAttnThreads), (size_t)kAttnSmem, st, true, p);
 }
 
 }  // namespace sdxl

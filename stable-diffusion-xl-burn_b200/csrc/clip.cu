@@ -6,7 +6,7 @@
 //   CLIP / ResidualDecoderAttentionBlock / MultiHeadSelfAttention / MLP / QuickGELU
 //                                   src/model/clip/mod.rs:82-147, 176-182, 228-245, 289-305, 315-319
 //   weight names                    src/model/clip/load.rs:15-115
-// 77-token sequences: Linear layers on the tcgen05 GEMM (one M tile), causal attention / activation / embedding on
+// 77-token sequences: Linear layers on the wgmma GEMM (one M tile), causal attention / activation / embedding on
 // small CUDA-core kernels (clip_kernels.cu). Residual stream f32, GEMM operands f16 (the reference runs f32).
 // ================================================================================================
 struct CBlock {

@@ -1,5 +1,5 @@
 // Kernels that only the text encoders (Embedder: CLIP-L / OpenCLIP-bigG, reference src/model/clip/mod.rs) need. The
-// sequences are 77 tokens, so these are small CUDA-core kernels; the Linear layers run on the tcgen05 GEMM (igemm.cu).
+// sequences are 77 tokens, so these are small CUDA-core kernels; the Linear layers run on the wgmma GEMM (igemm.cu).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -153,7 +153,7 @@ __global__ void mlp_act_kernel(const float* __restrict__ x, size_t n4, int quick
 int mlp_act_launch(cudaStream_t st, const float* x, size_t n, int quick, __half* y) {
   if (n & 3) return 7103;
   int grid = cdiv((long)(n >> 2), 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   return launch_kernel(mlp_act_kernel, dim3(grid), dim3(256), (size_t)0, st, true, x, n >> 2, quick, y);
 }
 

@@ -1,5 +1,5 @@
-// Shared device-side primitives for the sm_100a kernels: mbarrier, TMA, tcgen05/TMEM wrappers
-// (inline PTX), warp reductions and small math helpers. Everything here is Blackwell-only.
+// Shared device-side primitives for the sm_90a kernels: mbarrier, TMA, wgmma wrappers (inline PTX),
+// warp reductions and small math helpers. Everything here needs Hopper (sm_90a).
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -98,7 +98,14 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
     }
   }
 }
-// generic-proxy smem writes -> visible to the async proxy (UMMA / TMA reads)
+// The same bound without the printf: for threads with wgmma in flight, where a function call would serialise the wgmma pipeline.
+__device__ __forceinline__ void mbar_wait_nocall(uint64_t* bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  const uint64_t t0 = globaltimer_ns();
+  while (!mbar_try_wait(bar, parity))
+    if (globaltimer_ns() - t0 > 4000000000ull) __trap();
+}
+// generic-proxy smem writes -> visible to the async proxy (wgmma / TMA reads)
 __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
@@ -133,186 +140,46 @@ __device__ __forceinline__ void tma_load_4d(void* dst, const void* tmap, uint64_
 }
 
 // ---------------------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// wgmma (Hopper warpgroup MMA): issued by all 128 threads of a warpgroup, accumulators in registers
 // ---------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(
-                   smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wg_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols)
-               : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void tc_fence_after() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-// tcgen05.commit: arrive(1) on the mbarrier once all previously issued MMAs of this thread retire.
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-// D[tmem] (+)= A[smem] * B[smem], f16 inputs, f32 accumulate. One thread issues.
-__device__ __forceinline__ void tc_mma_f16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc,
-                                           uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}"
-      ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Warp-convergent issue helpers: executed by ALL lanes of a converged warp with warp-uniform operands; the
-// instruction itself is predicated on elect.sync, so exactly one lane issues it. Keeping the surrounding control
-// flow convergent lets ptxas hold descriptors / addresses in uniform registers instead of emitting a per-instruction
-// ELECT + R2UR.BROADCAST waterfall (which made the single-lane issue loops the bottleneck of the GEMM main loop).
-__device__ __forceinline__ void tc_mma_f16_elect(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi,
-                                                 uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, e;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %3};\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %4, p;\n\t"
-      "}"
-      ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_pair_elect(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi,
-                                                      uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, e;\n\t"
-      ".reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %3};\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %4, p;\n\t"
-      "}"
-      ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// One K block (four K=16 MMAs on consecutive 32-byte descriptor steps) + the commit that releases its smem slot,
-// under a single elect.sync: the issue loop's cost per K block is what bounds the GEMM main loop.
-// `acc_first` = accumulate flag of the first MMA (0 only for the first K block of a tile).
-__device__ __forceinline__ void tc_mma4_commit_pair_elect(uint32_t d_tmem, uint32_t a_lo, uint32_t b_lo, uint32_t desc_hi,
-                                                          uint32_t idesc, uint32_t acc_first, uint64_t* bar) {
-  // every instruction is predicated on the elect result ONLY: ptxas then keeps the whole sequence on the uniform datapath
-  // (UTCHMMA with UR operands back to back); mixing further conditions into the predicate brings back a per-MMA
-  // ELECT / R2UR.BROADCAST waterfall loop.
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p, e, t;\n\t"
-      ".reg .b64 da, db;\n\t"
-      ".reg .b32 al, bl;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "setp.ne.b32 p, %5, 0;\n\t"
-      "setp.eq.b32 t, 0, 0;\n\t"
-      "mov.b64 da, {%1, %3};\n\t"
-      "mov.b64 db, {%2, %3};\n\t"
-      "@e tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %4, p;\n\t"
-      "add.u32 al, %1, 2;\n\t"
-      "add.u32 bl, %2, 2;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %4, t;\n\t"
-      "add.u32 al, %1, 4;\n\t"
-      "add.u32 bl, %2, 4;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %4, t;\n\t"
-      "add.u32 al, %1, 6;\n\t"
-      "add.u32 bl, %2, 6;\n\t"
-      "mov.b64 da, {al, %3};\n\t"
-      "mov.b64 db, {bl, %3};\n\t"
-      "@e tcgen05.mma.cta_group::2.kind::f16 [%0], da, db, %4, t;\n\t"
-      "@e tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%6], %7;\n\t"
-      "}"
-      ::"r"(d_tmem), "r"(a_lo), "r"(b_lo), "r"(desc_hi), "r"(idesc), "r"(acc_first), "r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];\n\t"
-      "}"
-      ::"r"(smem_u32(bar))
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_mc_elect(uint64_t* bar, uint16_t mask) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t"
-      "}"
-      ::"r"(smem_u32(bar)), "h"(mask)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair_elect(uint64_t* bar) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred e;\n\t"
-      "elect.sync _|e, 0xffffffff;\n\t"
-      "@e tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;\n\t"
-      "}"
-      ::"r"(smem_u32(bar)), "h"((uint16_t)3)
-      : "memory");
-}
-
-// Shared-memory matrix descriptor for a SWIZZLE_128B tile whose rows are 128 bytes (64 halves):
-// 8-row swizzle atoms of 1024 B stacked along the outer dimension (SBO = 1024 B). Valid both for
-// K-major operands (rows = M/N index, 64 K-elements per row) and MN-major operands (rows = K index,
-// 64 MN-elements per row); the major-ness is selected in the instruction descriptor.
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr) {
-  const uint32_t lo = ((saddr >> 4) & 0x3FFFu) | (1u << 16);           // start addr, LBO(enc)=1
-  const uint32_t hi = 64u /*SBO=1024B>>4*/ | (1u << 14) /*version*/ | (2u << 29) /*SWIZZLE_128B*/;
+// Shared-memory matrix descriptor for a SWIZZLE_128B tile whose rows are 128 bytes (64 halves): 8-row swizzle atoms of
+// 1024 B stacked along the outer dimension (SBO = 1024 B; LBO unused). Valid for K-major operands (rows = M/N index,
+// 64 K-elements per row; a K step of 16 adds 32 B to the start address) and for 64-wide MN-major operands (rows = K index;
+// a K step of 16 adds 2048 B).
+__device__ __forceinline__ uint64_t wg_desc_sw128(uint32_t saddr) {
+  const uint32_t lo = ((saddr >> 4) & 0x3FFFu) | (1u << 16);
+  const uint32_t hi = 64u /*SBO = 1024 B >> 4*/ | (1u << 30) /*layout: SWIZZLE_128B*/;
   return (static_cast<uint64_t>(hi) << 32) | lo;
 }
-// Instruction descriptor: f16 x f16 -> f32, M=128, N=n, A K-major, B K-major or MN-major.
-__device__ __forceinline__ uint32_t make_idesc_f16(uint32_t n, bool b_mn_major) {
-  return (1u << 4) | (b_mn_major ? (1u << 16) : 0u) | ((n >> 3) << 17) | ((128u >> 4) << 24);
-}
-// TMEM -> registers: this warp's 32 lanes (lane quarter = warp_id % 4), 16 consecutive columns.
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
+// D (+)= A[smem] * B[smem], m64n128k16, f16 inputs, f32 accumulators in registers; A and B K-major. scale_d = 0 overwrites D.
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t da, uint64_t db, int scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-      "%13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
+// D (+)= A[smem] * B[smem], m64n64k16, f16 inputs, f32 accumulators in registers; A and B K-major. scale_d = 0 overwrites D.
+__device__ __forceinline__ void wgmma_ss_n64(float (&d)[32], uint64_t da, uint64_t db, int scale_d) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, "
-      "%13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
-      "[%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(da), "l"(db), "r"(scale_d));
 }
-__device__ __forceinline__ void tmem_ld_wait() {
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+// D += A[registers: packed f16 fragment of the m64k16 tile, mma.m16n8k16 A layout per warp] * B[smem], m64n64k16; B MN-major.
+__device__ __forceinline__ void wgmma_rs_n64_tb(float (&d)[32], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.eq.b32 p, 0, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
 }
 
 }  // namespace sdxl

@@ -193,7 +193,7 @@ int conv_in_launch_t(cudaStream_t st, const void* x, int x_f32, int Bx, int B, i
   if (int r = smem_optin(conv_in_kernel<__half>, 200 * 1024, done_h)) return r;
   const long total = (long)B * H * ((W + kConvInPix - 1) / kConvInPix) * (Cout / 4);
   int grid = cdiv(total, 256);
-  if (grid > 148 * 4) grid = 148 * 4;
+  if (grid > 132 * 4) grid = 132 * 4;
   if (x_f32)
     conv_in_kernel<float><<<grid, 256, smem, st>>>((const float*)x, Bx, B, Cin, H, W, w, bias, Cout, y);
   else
@@ -232,7 +232,7 @@ int upsample2x_launch(cudaStream_t st, const float* x, int B, int H, int W, int 
   if (C & 3) return 2003;
   const long total = (long)B * 4 * H * W * (C / 4);
   int grid = cdiv(total, 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   upsample2x_kernel<<<grid, 256, 0, st>>>(x, B, H, W, C, y);
   return (int)cudaGetLastError();
 }
@@ -256,7 +256,7 @@ int phase_split_launch(cudaStream_t st, const float* x, int B, int H, int W, int
   if ((C & 3) || (H & 1) || (W & 1)) return 2004;
   const long total = (long)B * H * W * (C / 4);
   int grid = cdiv(total, 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   phase_split_kernel<<<grid, 256, 0, st>>>(x, B, H, W, C, y);
   return (int)cudaGetLastError();
 }
@@ -273,13 +273,13 @@ __global__ void cast_f16_f32_kernel(const __half* __restrict__ x, size_t n, floa
 }
 int cast_f32_to_f16_launch(cudaStream_t st, const float* x, size_t n, __half* y) {
   int grid = cdiv((long)n, 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   if (grid < 1) grid = 1;
   return launch_kernel(cast_f32_f16_kernel, dim3(grid), dim3(256), (size_t)0, st, true, x, n, y);
 }
 int cast_f16_to_f32_launch(cudaStream_t st, const __half* x, size_t n, float* y) {
   int grid = cdiv((long)n, 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   if (grid < 1) grid = 1;
   cast_f16_f32_kernel<<<grid, 256, 0, st>>>(x, n, y);
   return (int)cudaGetLastError();
@@ -464,7 +464,7 @@ int repack_conv_launch(cudaStream_t st, const __half* src, int O, int I, int KH,
                        int col0, int Ipad) {
   const long total = (long)O * KH * KW * Ipad;
   int grid = cdiv(total, 256);
-  if (grid > 148 * 32) grid = 148 * 32;
+  if (grid > 132 * 32) grid = 132 * 32;
   repack_conv_kernel<<<grid, 256, 0, st>>>(src, O, I, KH, KW, dst, Ktot, col0, Ipad);
   return (int)cudaGetLastError();
 }
@@ -493,7 +493,7 @@ __global__ void repack_upconv_kernel(const __half* __restrict__ src, int O, int 
 int repack_upconv_launch(cudaStream_t st, const __half* src, int O, int I, __half* dst, int Ipad) {
   const long total = (long)4 * O * 4 * Ipad;
   int grid = cdiv(total, 256);
-  if (grid > 148 * 32) grid = 148 * 32;
+  if (grid > 132 * 32) grid = 132 * 32;
   repack_upconv_kernel<<<grid, 256, 0, st>>>(src, O, I, dst, Ipad);
   return (int)cudaGetLastError();
 }

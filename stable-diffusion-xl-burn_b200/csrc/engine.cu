@@ -2,7 +2,7 @@
 // UNet launch plan, the DDIM/CFG sampler loop and the operator-level entry points of include/sdxl_b200.h. The shared
 // machinery (arena, pack parsing, launch plan, CUDA-graph replay) is in engine_core.h; the latent decoder / encoder is
 // vae.cu, the text encoders clip.cu, the tokenizers tokenizer.cpp. No torch, no cuBLAS/cuDNN: every device op is one of
-// this library's own sm_100a kernels.
+// this library's own sm_90a kernels.
 //
 // Structure mirrored from the reference (file:line relative to the reference root):
 //   UNet::forward               src/model/unet/mod.rs:449-493
@@ -27,8 +27,8 @@ extern "C" int sdxl_ctx_create(int device, void* cuda_stream, sdxl_ctx** out) {
   }
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return -3;
-  if (prop.major != 10) {
-    fprintf(stderr, "sdxl_b200: device %d is sm_%d%d; this library contains sm_100a code only\n", device,
+  if (prop.major != 9 || prop.minor != 0) {
+    fprintf(stderr, "sdxl_b200: device %d is sm_%d%d; this library contains sm_90a code only\n", device,
             prop.major, prop.minor);
     return -4;
   }
@@ -1313,7 +1313,6 @@ extern "C" int sdxl_dbg_igemm_gaps(sdxl_ctx* c, int M, int K, int N, int with_re
   IgemmOperands o{x, 1, 1, M, K, K, nullptr, 0, 0, 0, 0, 0, w, N, Kpad};
   int r = igemm_configure(p, o, M, 1, 1, IGEMM_LINEAR, 0);
   if (r) return fail(c, r, "igemm configuration failed");
-  if (!p.pair) return fail(c, 5401, "sdxl_dbg_igemm_gaps: shape does not use the 2-CTA kernel");
   for (int i = 0; i < 3; ++i) KL(c, igemm_launch(c->stream, p));
   for (int i = 0; i < n_launch; ++i) {
     p.dbg_all = dbg + (size_t)i * per;

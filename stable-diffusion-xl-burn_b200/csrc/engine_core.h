@@ -27,7 +27,7 @@ struct sdxl_ctx {
   int device = 0;
   cudaStream_t stream = nullptr;
   bool own_stream = false;
-  int num_sms = 148;
+  int num_sms = 132;
   std::string err;
   uint64_t launches = 0;
 };

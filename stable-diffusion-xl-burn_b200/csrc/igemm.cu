@@ -1,21 +1,16 @@
-// Implicit-GEMM on 5th-gen tensor cores (tcgen05.mma, accumulators in TMEM, operands staged by TMA
-// into 128B-swizzled shared memory). One kernel serves every dense contraction of the UNet step:
+// Implicit GEMM on Hopper tensor cores (wgmma, f32 accumulators in registers, operands staged by TMA into 128B-swizzled
+// shared memory). One kernel serves every dense contraction of the UNet step:
 //   * Linear layers (reference unet/mod.rs:830,839,917,944,1009-1011,1021) = 1 segment, 1x1 tap;
 //   * 3x3 / 1x1 convolutions (unet/mod.rs:1086,1096,1099,750,767-770,490): one K-segment per filter
 //     tap; the tap shift is a TMA box offset on the NHWC activation, zero padding comes from TMA
 //     out-of-bounds fill; the ResBlock skip 1x1 conv is just one more K-segment on a second tensor.
 //
-// Persistent, warp-specialised, optionally clustered:
-//   * grid = (#resident clusters) x (CM*CN CTAs); every role walks the same static super-tile sequence.
-//   * Inside a CM x CN cluster each CTA owns one 128 x BN output tile. The A tile (128 pixels) is shared by the
-//     CN CTAs of a cluster row and the B tile (BN weight rows) by the CM CTAs of a cluster column: every CTA
-//     loads only its 1/CN (1/CM) slice and TMA-multicasts it to the peers, cutting L2->SM operand traffic
-//     (the measured limiter of this kernel) by up to 2x.
-//   * The smem operand ring runs across tile boundaries and the accumulator is double-buffered in TMEM
-//     (2 x BN columns), so the epilogue of tile i overlaps the MMA main loop of tile i+1.
-//   warp 0      : TMA producer (one lane)
-//   warp 1      : TMEM owner + MMA issuer (one lane)
-//   warps 2..9  : epilogue, 2 warps per TMEM lane quarter (each takes half of the tile's columns)
+// Persistent and warp-specialised: grid = min(#tiles, #SMs), every CTA walks the tiles blockIdx.x, + gridDim.x, ...
+// (M tiles fastest, so CTAs running at the same time share the weight tile in L2).
+//   warpgroup 0     : TMA producer (one lane)
+//   warpgroups 1, 2 : consumers. Each owns 64 rows of the 128 x BN tile (wgmma.m64nNk16, N = 64 or 128 per instruction) and
+//                     runs the epilogue straight from its accumulator registers.
+// The shared-memory operand ring runs across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i.
 #include "common.cuh"
 #include "kernels.h"
 
@@ -27,1006 +22,174 @@ namespace sdxl {
 static constexpr int kTileM = 128;
 static constexpr int kBlockK = 64;                    // 64 halves = 128 B = one swizzle row
 static constexpr int kABytes = kTileM * kBlockK * 2;  // 16 KB
-// n / d with a host-computed reciprocal m = floor(2^32/d)+1 (exact while n*d < 2^32); m == 0 falls back to '/'
-__device__ __forceinline__ int fdiv(int n, int d, unsigned m) { return m ? (int)__umulhi((unsigned)n, m) : n / d; }
-static constexpr int kEpiWarps = 8;
-static constexpr int kThreads = 64 + kEpiWarps * 32;
+static constexpr int kConsumerWarps = 8;
+static constexpr int kThreads = 128 + kConsumerWarps * 32;
 
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-  uint32_t r;
-  asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-  return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-  asm volatile("barrier.cluster.arrive.release.aligned;" ::: "memory");
-  asm volatile("barrier.cluster.wait.acquire.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tma_load_4d_mc(void* dst, const void* tmap, uint64_t* bar, int c0, int c1, int c2, int c3,
-                                               uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5, "
-      "%6, %7}], [%2], %3;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_mc(void* dst, const void* tmap, uint64_t* bar, int c0, int c1, uint16_t mask) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], "
-      "[%2], %3;" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(smem_u32(bar)), "h"(mask), "r"(c0), "r"(c1)
-      : "memory");
-}
-// ---- warp-convergent (elect-predicated) producer operations: see common.cuh for the rationale ----
-#define SDXL_ELECT_BEGIN "{\n\t.reg .pred e;\n\telect.sync _|e, 0xffffffff;\n\t"
-__device__ __forceinline__ void mbar_expect_tx_elect(uint64_t* bar, uint32_t bytes) {
-  asm volatile(SDXL_ELECT_BEGIN "@e mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;\n\t}" ::"r"(smem_u32(bar)), "r"(bytes)
-               : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_elect(uint64_t* bar) {
-  asm volatile(SDXL_ELECT_BEGIN "@e mbarrier.arrive.shared::cta.b64 _, [%0];\n\t}" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_elect(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3) {
-  asm volatile(SDXL_ELECT_BEGIN
-               "@e cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];\n\t}"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_elect(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1) {
-  asm volatile(SDXL_ELECT_BEGIN
-               "@e cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];\n\t}"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_mc_elect(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, int c2, int c3,
-                                                     uint16_t mask) {
-  asm volatile(SDXL_ELECT_BEGIN
-               "@e cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, "
-               "%5, %6, %7}], [%2], %3;\n\t}"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "h"(mask), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_mc_elect(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1, uint16_t mask) {
-  asm volatile(SDXL_ELECT_BEGIN
-               "@e cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, "
-               "%5}], [%2], %3;\n\t}"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "h"(mask), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_4d_pair_elect(uint32_t dst, const void* tmap, uint32_t leader_bar, int c0, int c1, int c2,
-                                                       int c3) {
-  asm volatile(SDXL_ELECT_BEGIN
-               "@e cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, "
-               "%6}], [%2];\n\t}"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-               : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair_elect(uint32_t dst, const void* tmap, uint32_t leader_bar, int c0, int c1) {
-  asm volatile(SDXL_ELECT_BEGIN
-               "@e cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], "
-               "[%2];\n\t}"
-               ::"r"(dst), "l"(reinterpret_cast<uint64_t>(tmap)), "r"(leader_bar), "r"(c0), "r"(c1)
-               : "memory");
+__device__ __forceinline__ size_t out_pixel(const IgemmParams& p, int tb, int th, int tw, int r, bool& ok, int& bb) {
+  const int wt = r % p.Wt, ht = (r / p.Wt) % p.Ht, bt = r / (p.Wt * p.Ht);
+  bb = tb * p.Bt + bt;
+  const int hh = th * p.Ht + ht, ww = tw * p.Wt + wt;
+  ok = (bb < p.Bn) && (hh < p.H) && (ww < p.W);
+  return ok ? ((size_t)bb * p.H + hh) * (size_t)p.opix_row + (size_t)ww * p.opix_w + p.opix_off : 0;
 }
 
-// arrive(1) on the mbarrier at the same smem offset in every CTA of `mask` once the issued MMAs retire
-__device__ __forceinline__ void tc_commit_mc(uint64_t* bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"(mask)
-               : "memory");
-}
-
-// ------------------------------------------------------------------------------------------------
-// Epilogue. TMEM hands every thread one accumulator ROW (lane = row), which is the worst possible shape for global
-// memory (32 rows per warp instruction). Each epilogue warp therefore transposes 32x32-column blocks through a private
-// smem staging buffer (row pitch 36 words: conflict-free for 128-bit row-wise writes and column-group reads) and does
-// all residual loads / output stores with lanes running along the contiguous N dimension: 4 fully used 128 B lines per
-// warp instruction instead of 32 partial ones.
-//   LINEAR: out = acc + bias[batch] (+ f32 residual), f32 or f16.   GEGLU: out = value * gelu_erf(gate), f16.
-// ------------------------------------------------------------------------------------------------
-static constexpr int kStagePitch = 36;                                   // words
-static constexpr int kStageBytesPerWarp = 32 * kStagePitch * 4;           // 4608 B
-static constexpr int kEpiStageBytes = kEpiWarps * kStageBytesPerWarp;     // 36864 B (transposing epilogue)
-static constexpr int kEpiTmaBufBytes = 4096;                               // one 32-row x 128-byte box
-static constexpr int kEpiAreaBytes = kEpiWarps * 2 * kEpiTmaBufBytes;      // 65536 B: two boxes per epilogue warp (TMA epilogue); the
-                                                                          // transposing epilogue uses the first kEpiStageBytes of it
-static_assert(kEpiStageBytes <= kEpiAreaBytes, "staging area too small");
-// f16 outputs on the TMA epilogue use 32-row x 64-byte boxes: half the area (p.epi_box_bytes = 2048), which buys one more pipeline stage
-__host__ __device__ constexpr int epi_area_bytes(int box_bytes) { return kEpiWarps * 2 * box_bytes; }
-
-struct EpiRow {          // per-lane description of "my" accumulator row (lane = row within the warp's 32 rows)
-  size_t pix;            // pixel (row of the output matrix)
-  bool ok;               // inside the image / batch
-  int bb;                // batch index (selects the bias row)
-};
-
-// Global operands of one LINEAR block in the phase-2 (lanes-along-N) mapping, loaded ahead of use: lane handles
-// rows it*4 + (lane>>3), it = 0..7, columns c4 = (lane&7)*4 .. +3 of the block.
-struct EpiPrefetch {
-  float4 res[8];
-  float4 bias;            // valid when all rows of the warp share one batch (EpiRows::bb_uniform)
-};
-struct EpiRows {          // phase-2 per-lane row descriptors (constant for the whole tile)
-  uint32_t off[8];        // element offset pix*ld + c4 (outputs and residual share the leading dimension)
-  int bb[8];
-  uint32_t ok;            // bit it: row valid
-  bool bb_uniform;        // warp-uniform: every valid row has batch bb[0]-equivalent (bias row shared)
-  int bb0;
-};
-__device__ __forceinline__ EpiPrefetch epi_prefetch(const IgemmParams& p, const EpiRows& rows, int n, int ncols, int lane) {
-  EpiPrefetch f;
-  const int c4 = (lane & 7) << 2;
-  const bool col_ok = c4 < ncols && n + c4 < p.N;
-#pragma unroll
-  for (int it = 0; it < 8; ++it) {
-    const bool ok = ((rows.ok >> it) & 1u) && col_ok;
-    f.res[it] = (ok && p.res != nullptr && p.dbg_mode != 4) ? *reinterpret_cast<const float4*>(p.res + rows.off[it] + n)
-                                                             : make_float4(0.f, 0.f, 0.f, 0.f);
+__device__ __forceinline__ void store2(const IgemmParams& p, size_t off, float x0, float x1, bool two, bool vec) {
+  if (p.out_f32) {
+    float* o = reinterpret_cast<float*>(p.out) + off;
+    if (two && vec) *reinterpret_cast<float2*>(o) = make_float2(x0, x1);
+    else { o[0] = x0; if (two) o[1] = x1; }
+  } else {
+    __half* o = reinterpret_cast<__half*>(p.out) + off;
+    if (two && vec) *reinterpret_cast<__half2*>(o) = __floats2half2_rn(x0, x1);
+    else { o[0] = __float2half_rn(x0); if (two) o[1] = __float2half_rn(x1); }
   }
-  f.bias = (col_ok && p.bias != nullptr && rows.bb_uniform)
-               ? __ldg(reinterpret_cast<const float4*>(p.bias + (size_t)rows.bb0 * p.bias_bstride + n + c4))
-               : make_float4(0.f, 0.f, 0.f, 0.f);
-  return f;
 }
 
-// one 32-column block (or a 16-column tail when ncols == 16) of the LINEAR epilogue; `pf` was issued earlier
-__device__ __forceinline__ void epi_linear_block(const IgemmParams& p, float* stage, uint32_t taddr, int n, int ncols,
-                                                 const EpiRows& rows, const EpiPrefetch& pf, int lane) {
-  // ---- phase 1: TMEM -> registers -> smem, lane = row
-  const bool dbgb = p.dbg != nullptr && blockIdx.x == 0 && threadIdx.x == 64 && p.dbg[9] == 0;
-  if (dbgb) p.dbg[9] = globaltimer_ns();
-  uint32_t v[32];
-  if (ncols == 32) tmem_ld32(taddr, v);
-  else {
-    uint32_t t[16];
-    tmem_ld16(taddr, t);
+// Epilogue of one consumer thread: rows r0 and r0 + 8 of the tile, columns 8 j + 2 (lane & 3) + {0, 1} (the wgmma accumulator
+// layout: acc[4 j + 2 h + e]).
+//   LINEAR: out = acc + bias[batch] (+ f32 residual), f32 or f16.   GEGLU (reference unet/mod.rs:942-956): tile columns [0, BN/2)
+//   are values, [BN/2, BN) the matching gates; out = value * gelu_erf(gate), f16, at column nt * BN/2 + c.
+template <int BN>
+__device__ __forceinline__ void epilogue(const IgemmParams& p, const float (&acc)[BN / 2], int tb, int th, int tw, int nt, int r0,
+                                         int lane) {
+  const int cq = (lane & 3) * 2;
+  const int n0 = nt * BN;
+  const bool vec = ((p.ldo | p.ldr | p.bias_bstride) & 1) == 0 && ((reinterpret_cast<uintptr_t>(p.out) | reinterpret_cast<uintptr_t>(p.res) |
+                                                                     reinterpret_cast<uintptr_t>(p.bias)) & 7) == 0;
 #pragma unroll
-    for (int i = 0; i < 16; ++i) { v[i] = t[i]; v[16 + i] = 0u; }
-  }
-  tmem_ld_wait();
-  if (dbgb) p.dbg[10] = globaltimer_ns();
-  float* myrow = stage + lane * kStagePitch;
+  for (int h = 0; h < 2; ++h) {
+    bool ok;
+    int bb;
+    const size_t pix = out_pixel(p, tb, th, tw, r0 + 8 * h, ok, bb);
+    if (!ok) continue;
+    if (p.mode == IGEMM_LINEAR) {
+      const float* bias = p.bias ? p.bias + (size_t)bb * p.bias_bstride : nullptr;
+      const float* res = p.res ? p.res + pix * p.ldr : nullptr;
 #pragma unroll
-  for (int i = 0; i < 8; ++i)
-    *reinterpret_cast<uint4*>(myrow + 4 * i) = make_uint4(v[4 * i], v[4 * i + 1], v[4 * i + 2], v[4 * i + 3]);
-  __syncwarp();
-  if (dbgb) p.dbg[11] = globaltimer_ns();
-  // ---- phase 2: lanes run along N: 8 lanes x float4 per row, 4 rows per instruction
-  const int rr = lane >> 3, c4 = (lane & 7) << 2;
-  const bool col_ok = c4 < ncols && n + c4 < p.N;
-#pragma unroll
-  for (int it = 0; it < 8; ++it) {
-    const int row = it * 4 + rr;
-    const bool ok = ((rows.ok >> it) & 1u) && col_ok;
-    if (ok) {
-      float4 f = *reinterpret_cast<const float4*>(stage + row * kStagePitch + c4);
-      float4 b4 = pf.bias;
-      if (!rows.bb_uniform && p.bias != nullptr)  // rows of different batches in one warp tile (tiny images only)
-        b4 = __ldg(reinterpret_cast<const float4*>(p.bias + (size_t)rows.bb[it] * p.bias_bstride + n + c4));
-      f.x += b4.x + pf.res[it].x;
-      f.y += b4.y + pf.res[it].y;
-      f.z += b4.z + pf.res[it].z;
-      f.w += b4.w + pf.res[it].w;
-      const uint32_t off = rows.off[it] + (uint32_t)n;
-      if (p.dbg_mode == 3) {
-        if (f.x == 123.456f) reinterpret_cast<float*>(p.out)[0] = f.y + f.z + f.w;  // keep the math alive, no store traffic
-      } else if (p.out_f32) {
-        *reinterpret_cast<float4*>(reinterpret_cast<float*>(p.out) + off) = f;
-      } else {
-        __half2 a = __floats2half2_rn(f.x, f.y), b = __floats2half2_rn(f.z, f.w);
-        uint2 o;
-        o.x = *reinterpret_cast<uint32_t*>(&a);
-        o.y = *reinterpret_cast<uint32_t*>(&b);
-        *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out) + off) = o;
-      }
-    }
-  }
-  __syncwarp();
-  if (dbgb) p.dbg[12] = globaltimer_ns();
-}
-
-// GEGLU block: 32 value columns at taddr_v, the matching 32 gate columns at taddr_g -> 32 f16 outputs
-__device__ __forceinline__ void epi_geglu_block(const IgemmParams& p, float* stage, uint32_t taddr_v, uint32_t taddr_g, int nv,
-                                                int ng, int ncol_out, const EpiRow& me, uint32_t ok_mask, int lane) {
-  const int rr = lane >> 3, c4 = (lane & 7) << 2;
-  const uint32_t pix_lo = (uint32_t)me.pix, pix_hi = (uint32_t)(me.pix >> 32);
-  float* myrow = stage + lane * kStagePitch;
-  uint32_t v[32], g[32];
-  tmem_ld32(taddr_v, v);
-  tmem_ld32(taddr_g, g);
-  tmem_ld_wait();
-#pragma unroll
-  for (int i = 0; i < 8; ++i) {
-    float4 x = make_float4(__uint_as_float(v[4 * i]), __uint_as_float(v[4 * i + 1]), __uint_as_float(v[4 * i + 2]),
-                           __uint_as_float(v[4 * i + 3]));
-    float4 y = make_float4(__uint_as_float(g[4 * i]), __uint_as_float(g[4 * i + 1]), __uint_as_float(g[4 * i + 2]),
-                           __uint_as_float(g[4 * i + 3]));
-    if (p.bias != nullptr) {
-      const float4 bx = __ldg(reinterpret_cast<const float4*>(p.bias + nv) + i);
-      const float4 by = __ldg(reinterpret_cast<const float4*>(p.bias + ng) + i);
-      x.x += bx.x; x.y += bx.y; x.z += bx.z; x.w += bx.w;
-      y.x += by.x; y.y += by.y; y.z += by.z; y.w += by.w;
-    }
-    *reinterpret_cast<float4*>(myrow + 4 * i) =
-        make_float4(x.x * gelu_erf_f(y.x), x.y * gelu_erf_f(y.y), x.z * gelu_erf_f(y.z), x.w * gelu_erf_f(y.w));
-  }
-  __syncwarp();
-#pragma unroll
-  for (int it = 0; it < 8; ++it) {
-    const int row = it * 4 + rr;
-    const size_t pix = ((size_t)__shfl_sync(0xffffffffu, pix_hi, row) << 32) | __shfl_sync(0xffffffffu, pix_lo, row);
-    if ((ok_mask >> row) & 1u) {
-      const float4 f = *reinterpret_cast<const float4*>(stage + row * kStagePitch + c4);
-      __half2 a = __floats2half2_rn(f.x, f.y), b = __floats2half2_rn(f.z, f.w);
-      uint2 o;
-      o.x = *reinterpret_cast<uint32_t*>(&a);
-      o.y = *reinterpret_cast<uint32_t*>(&b);
-      *reinterpret_cast<uint2*>(reinterpret_cast<__half*>(p.out) + pix * p.ldo + ncol_out + c4) = o;
-    }
-  }
-  __syncwarp();
-}
-
-// ------------------------------------------------------------------------------------------------
-// Epilogue through TMA (LINEAR tiles whose 128 rows are contiguous rows of a plain [pixels, ldo] output; N, BN multiples of 32).
-// The transposing epilogue above costs ~5 us per 128 x 160 f32 tile (per-thread global loads / stores behind a smem transpose),
-// more than the main loop of the 372 single-wave transformer GEMMs of a step. Here no thread touches global memory:
-//   * the f32 residual box (32 rows x 32 columns = 32 x 128 B) of a warp's next column block is fetched by TMA into a 128B-swizzled
-//     smem box while the current block is processed (the first one while the MMAs of the tile still run);
-//   * every lane owns one row: TMEM -> registers, + bias + residual (its own 128 B of the box, conflict-free 16-byte chunks
-//     through the swizzle), result written IN PLACE;
-//   * one TMA store per box (fence.proxy.async, lane 0), two boxes per warp so that the store of block b overlaps block b + 1.
-// f16 outputs (no residual) use 32-row x 64-byte boxes with the 64B swizzle.
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ void tma_store_2d(const void* tmap, uint32_t src_smem, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(reinterpret_cast<uint64_t>(tmap)),
-               "r"(src_smem), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ void bulk_commit_group() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_group_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void bulk_wait_group_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void tma_load_2d_u32(uint32_t dst, const void* tmap, uint32_t bar, int c0, int c1) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::"r"(dst),
-               "l"(reinterpret_cast<uint64_t>(tmap)), "r"(bar), "r"(c0), "r"(c1)
-               : "memory");
-}
-__device__ __forceinline__ float4 lds128(uint32_t a) {
-  float4 v;
-  asm volatile("ld.shared.v4.f32 {%0, %1, %2, %3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a));
-  return v;
-}
-__device__ __forceinline__ void sts128(uint32_t a, float4 v) {
-  asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-}
-__device__ __forceinline__ void sts128u(uint32_t a, uint4 v) {
-  asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(a), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w) : "memory");
-}
-// per-warp state of the TMA epilogue; `kb` counts this warp's column blocks over the whole kernel (box = kb & 1)
-struct EpiTma {
-  uint32_t box[2];      // smem addresses of the warp's two boxes (1024 B aligned)
-  uint32_t bar[2];      // mbarriers of the residual loads
-  uint32_t kb;
-};
-// request the residual box of column block `n` (rows row0 .. row0 + 31) into the box that block `kb_of_block` will use. Lane 0 only.
-__device__ __forceinline__ void epi_tma_request_res(const IgemmParams& p, const EpiTma& e, uint32_t kb_of_block, int n, int row0) {
-  const uint32_t b = kb_of_block & 1u;
-  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(e.bar[b]), "r"((uint32_t)kEpiTmaBufBytes) : "memory");
-  tma_load_2d_u32(e.box[b], &p.tmRes, e.bar[b], n, row0);
-}
-// One tile for one warp: column blocks [b0, b1) of the tile (32 columns each), rows row0 .. row0 + 31 of the output matrix.
-// The residual of block b0 has been requested by the caller (epi_tma_request_res) before the accumulator was complete.
-__device__ __forceinline__ void epilogue_tile_tma(const IgemmParams& p, EpiTma& e, uint32_t trow, int n0, int b0, int b1, int row0, int bb,
-                                                  bool row_ok, int lane) {
-  const bool has_res = p.res != nullptr;
-  const float* bias_row = p.bias ? p.bias + (size_t)bb * p.bias_bstride : nullptr;
-  for (int bI = b0; bI < b1; ++bI) {
-    const int n = n0 + (bI << 5);
-    const uint32_t cur = e.kb & 1u;
-    if (lane == 0) {
-      // the box block kb+1 will use was last read by the store of block kb-1: that read must be over before it is refilled / rewritten
-      if (has_res) {
-        bulk_wait_group_read<0>();
-        if (bI + 1 < b1) epi_tma_request_res(p, e, e.kb + 1, n + 32, row0);
-      } else {
-        bulk_wait_group_read<1>();   // this block's own box: last read by the store of block kb-2
-      }
-    }
-    float4 bs[8];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) bs[j] = bias_row ? __ldg(reinterpret_cast<const float4*>(bias_row + n) + j) : make_float4(0.f, 0.f, 0.f, 0.f);
-    uint32_t v[32];
-    tmem_ld32(trow + (bI << 5), v);
-    tmem_ld_wait();
-    __syncwarp();   // lane 0's wait above covers the whole warp's writes into the box
-    if (has_res) {
-      // residual box landed? (parity: this box's barrier completes once per use of the box)
-      const uint32_t parity = (e.kb >> 1) & 1u;
-      uint32_t ok = 0;
-      for (uint32_t spin = 0; !ok; ++spin) {   // bounded: a protocol bug must trap, not hang the GPU
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(ok) : "r"(e.bar[cur]), "r"(parity) : "memory");
-        if (!ok && spin > (1u << 24)) {
-          printf("sdxl_b200: igemm residual box wait timeout (block %d thread %d)\n", blockIdx.x, threadIdx.x);
-          __trap();
+      for (int j = 0; j < BN / 8; ++j) {
+        const int n = n0 + 8 * j + cq;
+        if (n >= p.N) continue;
+        const bool two = n + 1 < p.N;
+        float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+        if (bias) {
+          if (two && vec) { const float2 b = __ldg(reinterpret_cast<const float2*>(bias + n)); x0 += b.x; x1 += b.y; }
+          else { x0 += bias[n]; if (two) x1 += bias[n + 1]; }
         }
-      }
-    }
-    if (p.out_f32) {
-      const uint32_t rowa = e.box[cur] + (uint32_t)lane * 128u;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t a = rowa + ((uint32_t)(j ^ (lane & 7)) << 4);   // SWIZZLE_128B: 16-byte chunk j of row r sits at j ^ (r & 7)
-        float4 o = make_float4(__uint_as_float(v[4 * j]) + bs[j].x, __uint_as_float(v[4 * j + 1]) + bs[j].y,
-                               __uint_as_float(v[4 * j + 2]) + bs[j].z, __uint_as_float(v[4 * j + 3]) + bs[j].w);
-        if (has_res) {
-          const float4 r = lds128(a);
-          o.x += r.x; o.y += r.y; o.z += r.z; o.w += r.w;
+        if (res) {
+          if (two && vec) { const float2 q = *reinterpret_cast<const float2*>(res + n); x0 += q.x; x1 += q.y; }
+          else { x0 += res[n]; if (two) x1 += res[n + 1]; }
         }
-        sts128(a, o);
+        store2(p, pix * p.ldo + n, x0, x1, two, vec);
       }
     } else {
-      const uint32_t rowa = e.box[cur] + (uint32_t)lane * 64u;
+      constexpr int hb = BN / 2;
 #pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const uint32_t a = rowa + ((uint32_t)(j ^ ((lane >> 1) & 3)) << 4);   // SWIZZLE_64B: chunk j of row r sits at j ^ ((r >> 1) & 3)
-        uint32_t h[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) {
-          const float4 b4 = bs[2 * j + (i >> 1)];
-          const float bx = (i & 1) ? b4.z : b4.x, by = (i & 1) ? b4.w : b4.y;
-          __half2 t = __floats2half2_rn(__uint_as_float(v[8 * j + 2 * i]) + bx, __uint_as_float(v[8 * j + 2 * i + 1]) + by);
-          h[i] = *reinterpret_cast<uint32_t*>(&t);
-        }
-        sts128u(a, make_uint4(h[0], h[1], h[2], h[3]));
-      }
-    }
-    (void)row_ok;   // rows past the end of the output are clipped by the tensor map
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      tma_store_2d(&p.tmOut, e.box[cur], n, row0);
-      bulk_commit_group();
-    }
-    ++e.kb;
-  }
-}
-
-// GEGLU tile through TMA stores: value columns [0, BN/2) and gate columns [BN/2, BN) of the accumulator -> BN/2 f16 outputs
-// (reference unet/mod.rs:942-956), 32 output columns per box (32 rows x 64 B, SWIZZLE_64B). No residual, bias on both halves.
-__device__ __forceinline__ void epilogue_tile_tma_geglu(const IgemmParams& p, EpiTma& e, uint32_t trow, int nt, int n0, int half, int row0,
-                                                        int lane) {
-  const int hb = p.BN >> 1;
-  const int nb = hb >> 5;
-  const int b0 = half == 0 ? 0 : ((nb + 1) >> 1), b1 = half == 0 ? ((nb + 1) >> 1) : nb;
-  for (int bI = b0; bI < b1; ++bI) {
-    const int c = bI << 5;
-    const uint32_t cur = e.kb & 1u;
-    if (lane == 0) bulk_wait_group_read<1>();   // this block's box: last read by the store of block kb-2
-    uint32_t v[32], g[32];
-    tmem_ld32(trow + c, v);
-    tmem_ld32(trow + hb + c, g);
-    tmem_ld_wait();
-    __syncwarp();
-    const uint32_t rowa = e.box[cur] + (uint32_t)lane * 64u;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-      uint32_t h[4];
-#pragma unroll
-      for (int i = 0; i < 4; ++i) {
-        const int k = 8 * j + 2 * i;
-        float x0 = __uint_as_float(v[k]), x1 = __uint_as_float(v[k + 1]), y0 = __uint_as_float(g[k]), y1 = __uint_as_float(g[k + 1]);
+      for (int j = 0; j < hb / 8; ++j) {
+        const int c = 8 * j + cq;
+        float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+        float y0 = acc[4 * (j + hb / 8) + 2 * h], y1 = acc[4 * (j + hb / 8) + 2 * h + 1];
         if (p.bias != nullptr) {
-          x0 += __ldg(p.bias + n0 + c + k); x1 += __ldg(p.bias + n0 + c + k + 1);
-          y0 += __ldg(p.bias + n0 + hb + c + k); y1 += __ldg(p.bias + n0 + hb + c + k + 1);
+          x0 += __ldg(p.bias + n0 + c); x1 += __ldg(p.bias + n0 + c + 1);
+          y0 += __ldg(p.bias + n0 + hb + c); y1 += __ldg(p.bias + n0 + hb + c + 1);
         }
-        __half2 t = __floats2half2_rn(x0 * gelu_erf_f(y0), x1 * gelu_erf_f(y1));
-        h[i] = *reinterpret_cast<uint32_t*>(&t);
+        reinterpret_cast<__half2*>(reinterpret_cast<__half*>(p.out) + pix * p.ldo + nt * hb + c)[0] =
+            __floats2half2_rn(x0 * gelu_erf_f(y0), x1 * gelu_erf_f(y1));
       }
-      sts128u(rowa + ((uint32_t)(j ^ ((lane >> 1) & 3)) << 4), make_uint4(h[0], h[1], h[2], h[3]));
-    }
-    fence_proxy_async_smem();
-    __syncwarp();
-    if (lane == 0) {
-      tma_store_2d(&p.tmOut, e.box[cur], nt * hb + c, row0);
-      bulk_commit_group();
-    }
-    ++e.kb;
-  }
-}
-
-// phase-2 row descriptors from the per-lane (lane = row) description
-__device__ __forceinline__ EpiRows epi_rows(const EpiRow& me, int ld, int lane) {
-  EpiRows r;
-  const uint32_t ok_mask = __ballot_sync(0xffffffffu, me.ok);
-  const uint32_t my_off = (uint32_t)(me.pix * (size_t)ld);   // host guarantees pixels*ld < 2^32
-  const int rr = lane >> 3, c4 = (lane & 7) << 2;
-  r.ok = 0;
-#pragma unroll
-  for (int it = 0; it < 8; ++it) {
-    const int row = it * 4 + rr;
-    r.off[it] = __shfl_sync(0xffffffffu, my_off, row) + (uint32_t)c4;
-    r.bb[it] = __shfl_sync(0xffffffffu, me.bb, row);
-    r.ok |= ((ok_mask >> row) & 1u) << it;
-  }
-  // batch uniformity over the warp's valid rows (lane = row view)
-  const int first = ok_mask ? (__ffs(ok_mask) - 1) : 0;
-  r.bb0 = __shfl_sync(0xffffffffu, me.bb, first);
-  r.bb_uniform = __all_sync(0xffffffffu, !me.ok || me.bb == r.bb0);
-  return r;
-}
-// column-block range [b0, b1) of this warp for a LINEAR tile
-__device__ __forceinline__ void epi_linear_range(int BN, int half, int& b0, int& b1) {
-  const int nb = (BN + 31) >> 5;
-  b0 = half == 0 ? 0 : ((nb + 1) >> 1);
-  b1 = half == 0 ? ((nb + 1) >> 1) : nb;
-}
-
-// Epilogue of one 128 x BN accumulator tile for one warp (32 rows, `half` selects which column blocks it owns).
-// `pf0` = prefetched operands of the warp's first LINEAR block (issued before the accumulator was complete).
-__device__ __forceinline__ void epilogue_tile(const IgemmParams& p, float* stage, uint32_t trow, int nt, int n0,
-                                              const EpiRow& me, const EpiRows& rows, EpiPrefetch pf0, int half, int lane) {
-  const int BN = p.BN;
-  if (p.mode == IGEMM_LINEAR) {
-    if ((p.N & 15) == 0) {
-      // column blocks of 32 (+ one 16-wide tail when BN % 32 == 16), split between the two warps of a lane quarter
-      int b0, b1;
-      epi_linear_range(BN, half, b0, b1);
-      EpiPrefetch pf = pf0;
-      for (int bI = b0; bI < b1; ++bI) {
-        const int c = bI << 5;
-        const int ncols = (BN - c) >= 32 ? 32 : 16;
-        EpiPrefetch nxt = pf;
-        if (bI + 1 < b1) {  // next block's operands fly while this block is transposed
-          const int c2 = (bI + 1) << 5;
-          nxt = epi_prefetch(p, rows, n0 + c2, (BN - c2) >= 32 ? 32 : 16, lane);
-        }
-        if (n0 + c < p.N) epi_linear_block(p, stage, trow + c, n0 + c, ncols, rows, pf, lane);
-        pf = nxt;
-      }
-    } else if (half == 0) {
-      // ragged N (e.g. the 320->4 output conv): scalar, guarded, row-per-thread
-      const float* bias = p.bias ? p.bias + (size_t)me.bb * p.bias_bstride : nullptr;
-      const float* res = p.res ? p.res + me.pix * p.ldr : nullptr;
-      for (int c = 0; c < BN; c += 16) {
-        uint32_t v[16];
-        tmem_ld16(trow + c, v);
-        tmem_ld_wait();
-        const int n = n0 + c;
-        if (me.ok) {
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            if (n + i < p.N) {
-              float x = __uint_as_float(v[i]);
-              if (bias) x += bias[n + i];
-              if (res) x += res[n + i];
-              if (p.out_f32) reinterpret_cast<float*>(p.out)[me.pix * p.ldo + n + i] = x;
-              else reinterpret_cast<__half*>(p.out)[me.pix * p.ldo + n + i] = __float2half_rn(x);
-            }
-          }
-        }
-      }
-    }
-  } else {
-    // GEGLU (reference unet/mod.rs:942-956): tile columns [0,BN/2) = value, [BN/2,BN) = matching gate
-    const uint32_t ok_mask = __ballot_sync(0xffffffffu, me.ok);
-    const int hb = BN >> 1;
-    const int nb = hb >> 5;  // hb is a multiple of 32 (geglu_bn_for)
-    const int b0 = half == 0 ? 0 : ((nb + 1) >> 1), b1 = half == 0 ? ((nb + 1) >> 1) : nb;
-    for (int bI = b0; bI < b1; ++bI) {
-      const int c = bI << 5;
-      epi_geglu_block(p, stage, trow + c, trow + hb + c, n0 + c, n0 + hb + c, nt * hb + c, me, ok_mask, lane);
     }
   }
 }
 
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
+  constexpr int NC = BN >= 128 ? 128 : 64;   // N of one wgmma
+  constexpr int NCH = BN / NC;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages x (A 16KB | B BN*128)] [full][empty][tmem_full x2][tmem_empty x2][tmem ptr]
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int BN = p.BN;
   const int nst = p.nstages;
-  const uint32_t stage_bytes = kABytes + BN * 128;
-  uint8_t* epi_area = smem + (size_t)nst * stage_bytes;   // 1024 B aligned (stage sizes are multiples of 1 KB): epilogue boxes / staging
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_area + epi_area_bytes(p.epi_box_bytes));
+  constexpr uint32_t stage_bytes = kABytes + BN * 128;
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)nst * stage_bytes);
   uint64_t* empty_bar = full_bar + nst;
-  uint64_t* tmem_full = empty_bar + nst;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;    // [2]
-  uint64_t* epi_bar = tmem_empty + 2;      // [kEpiWarps][2]: residual boxes of the TMA epilogue
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(epi_bar + 2 * kEpiWarps);
-  float* epi_stage = reinterpret_cast<float*>(epi_area);  // transposing epilogue: [kEpiWarps][32][36] f32
 
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform: role loops stay on the uniform datapath
-  const int lane = threadIdx.x & 31;
-  const int CM = p.CM, CN = p.CN, cs = CM * CN;
-  const int rank = (int)(blockIdx.x % (unsigned)cs);   // == %cluster_ctarank for 1-D clusters; blockIdx keeps it on the uniform datapath
-  const int cm_idx = rank % CM, cn_idx = rank / CM;
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tiles = p.tilesW * p.tilesH * p.tilesB;
-  const int m_super = (m_tiles + CM - 1) / CM, n_super = (p.tilesN + CN - 1) / CN;
-  const int num_super = m_super * n_super;
-  const int cluster_id = blockIdx.x / cs, num_clusters = gridDim.x / cs;
-
+  const int num_tiles = m_tiles * p.tilesN;
   int total_kb = 0;
   for (int s = 0; s < p.nseg; ++s) total_kb += p.seg[s].nkb;
 
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < (uint32_t)(2 * BN)) tmem_cols <<= 1;
-
-  if (warp == 0) {
-    // one barrier per lane; contiguous array full[nst] empty[nst] tmem_full[2] tmem_empty[2] epi_bar[16]. empty: one MMA-retire
-    // arrival from every CTA this CTA multicasts to; tmem_empty: every epilogue warp
-    const int nbar = 2 * nst + 4 + 2 * kEpiWarps;
-    for (int i = lane; i < nbar; i += 32)
-      mbar_init(&full_bar[i], (i >= nst && i < 2 * nst) ? CM + CN - 1 : (i >= 2 * nst + 2 && i < 2 * nst + 4) ? kEpiWarps : 1);
+  if (threadIdx.x == 0) {
+    for (int i = 0; i < nst; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumerWarps); }
     fence_barrier_init();
-    if (lane == 0) {
-      tma_prefetch_desc(&p.tmA0);
-      tma_prefetch_desc(&p.tmA1);
-      tma_prefetch_desc(&p.tmB);
-    }
+    tma_prefetch_desc(&p.tmA0);
+    tma_prefetch_desc(&p.tmA1);
+    tma_prefetch_desc(&p.tmB);
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, tmem_cols);
-  tc_fence_before();
   __syncthreads();
-  if (cs > 1) cluster_sync_all();  // peers' barriers are initialised before any multicast / remote arrive
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
   // PDL: everything above overlapped the previous kernel's tail; from here on we touch its outputs.
-  const bool dbg = p.dbg != nullptr && blockIdx.x == 0;
-  if (dbg && threadIdx.x == 0) p.dbg[0] = globaltimer_ns();   // prologue done (before griddep wait)
   griddep_wait();
   griddep_launch_dependents();
-  if (dbg && threadIdx.x == 0) p.dbg[1] = globaltimer_ns();   // dependencies resolved
 
-  // multicast masks (bit = CTA rank in cluster): A goes to my cluster row (same cm_idx), B to my column
-  uint16_t row_mask = 0, col_mask = 0;
-  for (int j = 0; j < CN; ++j) row_mask |= (uint16_t)(1u << (cm_idx + CM * j));
-  for (int i = 0; i < CM; ++i) col_mask |= (uint16_t)(1u << (cn_idx * CM + i));
-  const int a_rows = kTileM / CN, b_rows = BN / CM;
-
-  if (warp == 0) {
+  if (warp < 4) {
     // ===================== TMA producer =====================
-    // The whole warp walks the loop (warp-uniform control flow keeps addresses in uniform registers); one elected
-    // lane issues each TMA / barrier operation.
+    if (warp != 0 || lane != 0) return;
     uint32_t stage = 0, phase = 0;
-    const uint32_t smem_base = smem_u32(smem), full_base = smem_u32(full_bar);
-    for (int st = cluster_id; st < num_super; st += num_clusters) {
-      const int mt = (st % m_super) * CM + cm_idx, nt = (st / m_super) * CN + cn_idx;
-      const int tw = mt % p.tilesW;
-      const int th = (mt / p.tilesW) % p.tilesH;
-      const int tb = mt / (p.tilesW * p.tilesH);
-      // my slice of the A tile: offset cn_idx * a_split_ext along the split dimension
-      int w0 = tw * p.Wt, h0 = th * p.Ht, b0 = tb * p.Bt;
-      if (p.a_split_dim == 0) w0 += cn_idx * p.a_split_ext;
-      else if (p.a_split_dim == 1) h0 += cn_idx * p.a_split_ext;
-      else b0 += cn_idx * p.a_split_ext;
-      const int n0 = nt * BN + cm_idx * b_rows;
+    for (int st = blockIdx.x; st < num_tiles; st += gridDim.x) {
+      const int mt = st % m_tiles, nt = st / m_tiles;
+      const int tw = mt % p.tilesW, th = (mt / p.tilesW) % p.tilesH, tb = mt / (p.tilesW * p.tilesH);
+      const int w0 = tw * p.Wt, h0 = th * p.Ht, b0 = tb * p.Bt, n0 = nt * BN;
       int kcol = 0;
       for (int s = 0; s < p.nseg; ++s) {
         const IgemmSeg sg = p.seg[s];
         const void* mapA = sg.map ? (const void*)&p.tmA1 : (const void*)&p.tmA0;
-        const int cw = w0 + sg.dw, chh = h0 + sg.dh, cb = b0 + sg.db;
         for (int j = 0; j < sg.nkb; ++j, kcol += kBlockK) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          {
-            const uint32_t a_dst = smem_base + stage * stage_bytes + (uint32_t)(cn_idx * a_rows * 128);
-            const uint32_t b_dst = smem_base + stage * stage_bytes + kABytes + (uint32_t)(cm_idx * b_rows * 128);
-            const uint32_t fb = full_base + stage * 8;
-            if (p.dbg_mode == 1) {
-              mbar_arrive_elect(&full_bar[stage]);
-            } else {
-              mbar_expect_tx_elect(&full_bar[stage], stage_bytes);
-              if (CN > 1) tma_load_4d_mc_elect(a_dst, mapA, fb, j * kBlockK, cw, chh, cb, row_mask);
-              else tma_load_4d_elect(a_dst, mapA, fb, j * kBlockK, cw, chh, cb);
-              if (CM > 1) tma_load_2d_mc_elect(b_dst, &p.tmB, fb, kcol, n0, col_mask);
-              else tma_load_2d_elect(b_dst, &p.tmB, fb, kcol, n0);
-            }
-          }
+          mbar_wait_nocall(&empty_bar[stage], phase ^ 1);
+          uint8_t* dst = smem + stage * stage_bytes;
+          mbar_expect_tx(&full_bar[stage], stage_bytes);
+          tma_load_4d(dst, mapA, &full_bar[stage], j * kBlockK, w0 + sg.dw, h0 + sg.dh, b0 + sg.db);
+          tma_load_2d(dst + kABytes, &p.tmB, &full_bar[stage], kcol, n0);
           if (++stage == (uint32_t)nst) { stage = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: warp-uniform loop, lane 0 issues =====================
-    const uint32_t idesc = make_idesc_f16((uint32_t)BN, false);
-    const uint16_t release_mask = row_mask | col_mask;
-    const uint32_t desc_hi = 64u /*SBO=1024B>>4*/ | (1u << 14) /*version*/ | (2u << 29) /*SWIZZLE_128B*/;
-    const uint32_t a_lo0 = ((smem_u32(smem) >> 4) & 0x3FFFu) | (1u << 16);
-    const uint32_t stage_inc = stage_bytes >> 4, b_off = kABytes >> 4;
-    uint32_t stage = 0, phase = 0;
-    int lt = 0;
-    for (int st = cluster_id; st < num_super; st += num_clusters, ++lt) {
-      const int buf = lt & 1;
-      mbar_wait(&tmem_empty[buf], ((lt >> 1) & 1) ^ 1);  // epilogue drained this accumulator buffer
-      tc_fence_after();
-      const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BN);
-      for (int kb = 0; kb < total_kb; ++kb) {
-        mbar_wait(&full_bar[stage], phase);
-        if (dbg && lt == 0 && kb == 0 && lane == 0) p.dbg[2] = globaltimer_ns();  // first operands landed
-        tc_fence_after();
-        {
-          const uint32_t a_lo = a_lo0 + stage * stage_inc, b_lo = a_lo + b_off;
-          if (p.dbg_mode != 2) {
+    return;
+  }
+
+  // ===================== consumers =====================
+  const int wg = (warp >> 2) - 1;                       // 0 / 1: tile rows [64 wg, 64 wg + 64)
+  const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+  const uint32_t smem_base = smem_u32(smem);
+  uint32_t stage = 0, phase = 0;
+  float acc[BN / 2];
+  for (int st = blockIdx.x; st < num_tiles; st += gridDim.x) {
+    const int mt = st % m_tiles, nt = st / m_tiles;
+    uint32_t prev = 0;
+    for (int kb = 0; kb < total_kb; ++kb) {
+      mbar_wait_nocall(&full_bar[stage], phase);
+      wg_fence();
+      const uint32_t a = smem_base + stage * stage_bytes + (uint32_t)wg * (64 * 128);
+      const uint32_t b = smem_base + stage * stage_bytes + kABytes;
 #pragma unroll
-            for (int k = 0; k < kBlockK / 16; ++k)
-              tc_mma_f16_elect(d_tmem, a_lo + 2 * k, b_lo + 2 * k, desc_hi, idesc, (kb > 0 || k > 0) ? 1u : 0u);
-          }
-          // free the smem slot (here and in every CTA whose loads land in it) once these MMAs have read it
-          if (cs > 1) tc_commit_mc_elect(&empty_bar[stage], release_mask);
-          else tc_commit_elect(&empty_bar[stage]);
-        }
-        if (++stage == (uint32_t)nst) { stage = 0; phase ^= 1; }
-      }
-      tc_commit_elect(&tmem_full[buf]);  // accumulator of this tile complete
-    }
-  } else {
-    // ===================== epilogue warps (2..9) =====================
-    const int q = warp & 3;               // TMEM lane quarter this warp may access
-    const int half = (warp - 2) >> 2;     // which half of the tile's column blocks
-    const int r = q * 32 + lane;          // tile row == TMEM lane
-    const int wt = r % p.Wt;
-    const int ht = (r / p.Wt) % p.Ht;
-    const int bt = r / (p.Wt * p.Ht);
-    float* stage_buf = epi_stage + (warp - 2) * (32 * kStagePitch);
-    EpiTma et;
-    et.box[0] = smem_u32(epi_area) + (uint32_t)((warp - 2) * 2) * (uint32_t)p.epi_box_bytes;
-    et.box[1] = et.box[0] + (uint32_t)p.epi_box_bytes;
-    et.bar[0] = smem_u32(&epi_bar[(warp - 2) * 2]);
-    et.bar[1] = et.bar[0] + 8;
-    et.kb = 0;
-    int lt = 0;
-    for (int st = cluster_id; st < num_super; st += num_clusters, ++lt) {
-      const int mt = (st % m_super) * CM + cm_idx, nt = (st / m_super) * CN + cn_idx;
-      const int tw = mt % p.tilesW;
-      const int th = (mt / p.tilesW) % p.tilesH;
-      const int tb = mt / (p.tilesW * p.tilesH);
-      const int bb = tb * p.Bt + bt, hh = th * p.Ht + ht, ww = tw * p.Wt + wt;
-      EpiRow me;
-      me.ok = (bb < p.Bn) && (hh < p.H) && (ww < p.W);
-      me.pix = me.ok ? ((size_t)bb * p.H + hh) * (size_t)p.opix_row + (size_t)ww * p.opix_w + p.opix_off : 0;
-      me.bb = me.ok ? bb : 0;
-      const int buf = lt & 1;
-      if (p.epi_tma) {
-        // TMA epilogue: the tile's rows are contiguous rows of the output matrix, starting at the pixel of tile row 0
-        int eb0, eb1;
-        epi_linear_range(BN, half, eb0, eb1);
-        const int row0 = ((tb * p.Bt) * p.H + th * p.Ht) * p.W + tw * p.Wt + q * 32;
-        if (p.res != nullptr && eb0 < eb1 && lane == 0) {
-          bulk_wait_group_read<1>();   // the first block's box was last read by the store of block kb-2
-          epi_tma_request_res(p, et, et.kb, nt * BN + (eb0 << 5), row0);
-        }
-        mbar_wait(&tmem_full[buf], (lt >> 1) & 1);
-        tc_fence_after();
-        const uint32_t trow_t = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN);
-        if (p.mode == IGEMM_GEGLU) epilogue_tile_tma_geglu(p, et, trow_t, nt, nt * BN, half, row0, lane);
-        else epilogue_tile_tma(p, et, trow_t, nt * BN, eb0, eb1, row0, me.bb, me.ok, lane);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[buf]);
-        continue;
-      }
-      // row descriptors + the first block's residual/bias are fetched while the MMAs of this tile still run
-      const EpiRows rows = epi_rows(me, p.ldo, lane);
-      EpiPrefetch pf0;
-      {
-        int eb0, eb1;
-        epi_linear_range(BN, half, eb0, eb1);
-        const int c0 = eb0 << 5;
-        if (p.mode == IGEMM_LINEAR && (p.N & 15) == 0 && eb0 < eb1) pf0 = epi_prefetch(p, rows, nt * BN + c0, (BN - c0) >= 32 ? 32 : 16, lane);
-        else {
+      for (int k = 0; k < kBlockK / 16; ++k) {
+        const uint64_t da = wg_desc_sw128(a + 32 * k);
 #pragma unroll
-          for (int i = 0; i < 8; ++i) pf0.res[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          pf0.bias = make_float4(0.f, 0.f, 0.f, 0.f);
+        for (int c = 0; c < NCH; ++c) {
+          const uint64_t db = wg_desc_sw128(b + c * NC * 128 + 32 * k);
+          if constexpr (NC == 128) wgmma_ss_n128(*reinterpret_cast<float(*)[64]>(acc + 64 * c), da, db, (kb | k) != 0);
+          else wgmma_ss_n64(*reinterpret_cast<float(*)[32]>(acc + 32 * c), da, db, (kb | k) != 0);
         }
       }
-      mbar_wait(&tmem_full[buf], (lt >> 1) & 1);
-      if (dbg && lt == 0 && threadIdx.x == 64) p.dbg[3] = globaltimer_ns();  // first accumulator complete
-      tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN);
-      epilogue_tile(p, stage_buf, trow, nt, nt * BN, me, rows, pf0, half, lane);
-      if (dbg && lt == 0 && threadIdx.x == 64) p.dbg[4] = globaltimer_ns();  // first epilogue done
-      // all TMEM reads of this buffer are complete (tcgen05.wait::ld above): hand it back to the MMA warp
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&tmem_empty[buf]);
+      wg_commit();
+      if (kb > 0) {   // the previous K block's wgmmas have read their stage: hand it back to the producer
+        wg_wait<1>();
+        if (lane == 0) mbar_arrive(&empty_bar[prev]);
+      }
+      prev = stage;
+      if (++stage == (uint32_t)nst) { stage = 0; phase ^= 1; }
     }
+    wg_wait<0>();
+    if (lane == 0 && total_kb > 0) mbar_arrive(&empty_bar[prev]);
+    const int tw = mt % p.tilesW, th = (mt / p.tilesW) % p.tilesH, tb = mt / (p.tilesW * p.tilesH);
+    epilogue<BN>(p, acc, tb, th, tw, nt, r0, lane);
   }
-
-  if (dbg && threadIdx.x == 0) p.dbg[5] = globaltimer_ns();  // producer done issuing
-  if (p.epi_tma && warp >= 2 && lane == 0) bulk_wait_group_read<0>();   // the TMA stores have read their shared-memory boxes; the writes complete with the grid
-  tc_fence_before();
-  __syncthreads();
-  if (dbg && threadIdx.x == 0) p.dbg[6] = globaltimer_ns();  // producer warp arrived at the final barrier (the read may issue before the barrier completes)
-  if (cs > 1) cluster_sync_all();  // no CTA leaves while a peer may still signal its barriers
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, tmem_cols);
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// 2-CTA variant (tcgen05 cta_group::2): a CTA pair (cluster of 2, same TPC) computes a 256 x BN tile with one
-// MMA stream issued by the leader CTA. Each CTA stages only ITS 128 A rows and HALF of the B tile (BN/2 weight
-// rows); the tensor core reads both halves across the pair, so the bytes delivered into each SM per FLOP drop by
-// 1/3 versus the 1-CTA kernel at BN = 256 (L2->SM delivery is what bounds these GEMMs). Accumulators: each CTA's
-// TMEM holds its own 128 rows x BN columns, double-buffered; epilogues run independently in both CTAs.
-// Barriers: full[s] lives in the leader and counts the TMA bytes of BOTH CTAs; empty[s] / tmem_full[b] are
-// signalled in both CTAs by the leader's multicast tcgen05.commit; tmem_empty[b] in the leader collects the
-// epilogue warps of both CTAs (the peer arrives remotely).
-// ------------------------------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t mapa_rank(uint32_t local_addr, uint32_t rank) {
-  uint32_t r;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local_addr), "r"(rank));
-  return r;
-}
-__device__ __forceinline__ void mbar_arrive_remote(uint32_t cluster_addr) {
-  asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-// TMA load into THIS CTA's smem whose completion bytes are credited to an mbarrier in the pair's leader CTA
-__device__ __forceinline__ void tma_load_4d_pair(void* dst, const void* tmap, uint32_t leader_bar, int c0, int c1, int c2,
-                                                 int c3) {
-  asm volatile(
-      "cp.async.bulk.tensor.4d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], "
-      "[%2];" ::"r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(leader_bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
-      : "memory");
-}
-__device__ __forceinline__ void tma_load_2d_pair(void* dst, const void* tmap, uint32_t leader_bar, int c0, int c1) {
-  asm volatile(
-      "cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];" ::
-          "r"(smem_u32(dst)),
-      "l"(reinterpret_cast<uint64_t>(tmap)), "r"(leader_bar), "r"(c0), "r"(c1)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_alloc_pair(uint32_t* smem_dst, uint32_t ncols) {  // one warp in EACH CTA
-  asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc_pair(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_mma_f16_pair(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc,
-                                                uint32_t accumulate) {
-  asm volatile(
-      "{\n\t"
-      ".reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t"
-      "}" ::"r"(d_tmem),
-      "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-__device__ __forceinline__ void tc_commit_pair(uint64_t* bar) {  // arrive on `bar` in both CTAs of the pair
-  asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(
-                   smem_u32(bar)),
-               "h"((uint16_t)3)
-               : "memory");
-}
-
-__global__ void __launch_bounds__(kThreads, 1) igemm_pair_kernel(const __grid_constant__ IgemmParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  if (p.dbg_all != nullptr && threadIdx.x == 0) p.dbg_all[blockIdx.x * 8 + 0] = globaltimer_ns();
-  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
-  const int BN = p.BN;
-  const int nst = p.nstages;
-  const int b_rows = BN >> 1;                                  // this CTA's half of the B tile
-  const uint32_t stage_bytes = kABytes + b_rows * 128;
-  uint8_t* epi_area = smem + (size_t)nst * stage_bytes;   // 1024 B aligned (stage sizes are multiples of 1 KB): epilogue boxes / staging
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(epi_area + epi_area_bytes(p.epi_box_bytes));
-  uint64_t* empty_bar = full_bar + nst;
-  uint64_t* tmem_full = empty_bar + nst;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;    // [2]  (used in the leader)
-  uint64_t* epi_bar = tmem_empty + 2;      // [kEpiWarps][2]: residual boxes of the TMA epilogue
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(epi_bar + 2 * kEpiWarps);
-  float* epi_stage = reinterpret_cast<float*>(epi_area);  // transposing epilogue: [kEpiWarps][32][36] f32
-
-  const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0);   // provably warp-uniform: role loops stay on the uniform datapath
-  const int lane = threadIdx.x & 31;
-  const int rank = (int)(blockIdx.x & 1u);  // == %cluster_ctarank for the (2,1,1) cluster; 0 = leader. blockIdx keeps it on the uniform datapath
-  const int m_tiles = p.tilesW * p.tilesH * p.tilesB;
-  const int pm_tiles = m_tiles >> 1;
-  const int num_ptiles = pm_tiles * p.tilesN;
-  const int pair_id = blockIdx.x >> 1, num_pairs = gridDim.x >> 1;
-
-  int total_kb = 0;
-  for (int s = 0; s < p.nseg; ++s) total_kb += p.seg[s].nkb;
-
-  uint32_t tmem_cols = 32;
-  while (tmem_cols < (uint32_t)(2 * BN)) tmem_cols <<= 1;
-
-  if (warp == 0) {
-    // one barrier per lane (the ~30 barriers are one contiguous array: full[nst] empty[nst] tmem_full[2] tmem_empty[2] epi_bar[16]):
-    // full = the leader's producer arrives once with the byte count of both CTAs, empty = the leader's multicast commit,
-    // tmem_empty = every epilogue warp of both CTAs; a single lane initialising them one by one cost ~0.4 us of every launch
-    const int nbar = 2 * nst + 4 + 2 * kEpiWarps;
-    for (int i = lane; i < nbar; i += 32) mbar_init(&full_bar[i], (i >= 2 * nst + 2 && i < 2 * nst + 4) ? 2 * kEpiWarps : 1);
-    fence_barrier_init();
-    if (lane == 0) {
-      tma_prefetch_desc(&p.tmA0);
-      tma_prefetch_desc(&p.tmA1);
-      tma_prefetch_desc(&p.tmB);
-    }
-  }
-  __syncthreads();
-  if (p.dbg_all != nullptr && threadIdx.x == 0) p.dbg_all[blockIdx.x * 8 + 1] = globaltimer_ns();
-  cluster_sync_all();  // both CTAs' barriers exist before any cross-CTA signal
-  if (p.dbg_all != nullptr && threadIdx.x == 0) p.dbg_all[blockIdx.x * 8 + 2] = globaltimer_ns();
-  if (warp == 1) tmem_alloc_pair(tmem_ptr, tmem_cols);
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
-
-  const bool dbg = p.dbg != nullptr && blockIdx.x == 0;
-  if (dbg && threadIdx.x == 0) p.dbg[0] = globaltimer_ns();   // prologue done (before griddep wait)
-  if (p.dbg_all != nullptr && threadIdx.x == 0) p.dbg_all[blockIdx.x * 8 + 3] = globaltimer_ns();
-  griddep_wait();
-  griddep_launch_dependents();
-  if (dbg && threadIdx.x == 0) p.dbg[1] = globaltimer_ns();   // dependencies resolved
-  if (p.dbg_all != nullptr && threadIdx.x == 0) p.dbg_all[blockIdx.x * 8 + 4] = globaltimer_ns();
-
-  if (warp == 0) {
-    // ===================== TMA producer (both CTAs): warp-uniform loop, one elected lane issues =====================
-    uint32_t stage = 0, phase = 0;
-    const uint32_t smem_base = smem_u32(smem);
-    const uint32_t leader_full_base = mapa_rank(smem_u32(full_bar), 0);
-    for (int pt = pair_id; pt < num_ptiles; pt += num_pairs) {
-      // tile index -> coordinates with multiply-high reciprocals (a chain of '/' and '%' here cost ~0.8 us before the first TMA)
-      const int nt = fdiv(pt, pm_tiles, p.fd_pm);
-      const int mt = (pt - nt * pm_tiles) * 2 + rank;
-      const int q1 = fdiv(mt, p.tilesW, p.fd_w);           // mt / tilesW
-      const int tw = mt - q1 * p.tilesW;
-      const int tb = fdiv(mt, p.tilesW * p.tilesH, p.fd_wh);
-      const int th = q1 - tb * p.tilesH;                   // (mt / tilesW) % tilesH
-      const int w0 = tw * p.Wt, h0 = th * p.Ht, b0 = tb * p.Bt;
-      const int n0 = nt * BN + rank * b_rows;
-      int kcol = 0;
-      for (int s = 0; s < p.nseg; ++s) {
-        const IgemmSeg sg = p.seg[s];
-        const void* mapA = sg.map ? (const void*)&p.tmA1 : (const void*)&p.tmA0;
-        const int cw = w0 + sg.dw, chh = h0 + sg.dh, cb = b0 + sg.db;
-        for (int j = 0; j < sg.nkb; ++j, kcol += kBlockK) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          {
-            const uint32_t a_dst = smem_base + stage * stage_bytes;
-            const uint32_t b_dst = a_dst + kABytes;
-            if (p.dbg_mode == 1) {
-              if (rank == 0) mbar_arrive_elect(&full_bar[stage]);
-            } else {
-              if (rank == 0) mbar_expect_tx_elect(&full_bar[stage], 2 * stage_bytes);
-              const uint32_t lbar = leader_full_base + stage * 8;
-              tma_load_4d_pair_elect(a_dst, mapA, lbar, j * kBlockK, cw, chh, cb);
-              tma_load_2d_pair_elect(b_dst, &p.tmB, lbar, kcol, n0);
-            }
-          }
-          if (++stage == (uint32_t)nst) { stage = 0; phase ^= 1; }
-        }
-      }
-    }
-  } else if (warp == 1) {
-    // ===================== MMA issuer: leader CTA, warp-uniform loop, lane 0 issues =====================
-    if (rank == 0) {
-      // M = 256 across the pair, N = BN
-      const uint32_t idesc = (1u << 4) | (((uint32_t)BN >> 3) << 17) | ((256u >> 4) << 24);
-      const uint32_t desc_hi = 64u | (1u << 14) | (2u << 29);
-      const uint32_t a_lo0 = ((smem_u32(smem) >> 4) & 0x3FFFu) | (1u << 16);
-      const uint32_t stage_inc = stage_bytes >> 4, b_off = kABytes >> 4;
-      uint32_t stage = 0, phase = 0;
-      int lt = 0;
-      for (int pt = pair_id; pt < num_ptiles; pt += num_pairs, ++lt) {
-        const int buf = lt & 1;
-        mbar_wait(&tmem_empty[buf], ((lt >> 1) & 1) ^ 1);  // both CTAs' epilogues drained this buffer
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + (uint32_t)(buf * BN);
-        for (int kb = 0; kb < total_kb; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          if (dbg && lt == 0 && kb == 0 && lane == 0) p.dbg[2] = globaltimer_ns();  // first operands landed
-          tc_fence_after();
-          {
-            const uint32_t a_lo = a_lo0 + stage * stage_inc, b_lo = a_lo + b_off;
-            // four MMAs + the commit that frees the slot in both CTAs, one elect
-            if (p.dbg_mode != 2) tc_mma4_commit_pair_elect(d_tmem, a_lo, b_lo, desc_hi, idesc, kb > 0 ? 1u : 0u, &empty_bar[stage]);
-            else tc_commit_pair_elect(&empty_bar[stage]);   // diagnostics: loads and barriers only
-          }
-          if (++stage == (uint32_t)nst) { stage = 0; phase ^= 1; }
-        }
-        tc_commit_pair_elect(&tmem_full[buf]);  // accumulators (both halves) complete
-      }
-    }
-  } else {
-    // ===================== epilogue warps (2..9), both CTAs =====================
-    const int q = warp & 3;
-    const int half = (warp - 2) >> 2;
-    const int r = q * 32 + lane;
-    const int wt = r % p.Wt;
-    const int ht = (r / p.Wt) % p.Ht;
-    const int bt = r / (p.Wt * p.Ht);
-    float* stage_buf = epi_stage + (warp - 2) * (32 * kStagePitch);
-    EpiTma et;
-    et.box[0] = smem_u32(epi_area) + (uint32_t)((warp - 2) * 2) * (uint32_t)p.epi_box_bytes;
-    et.box[1] = et.box[0] + (uint32_t)p.epi_box_bytes;
-    et.bar[0] = smem_u32(&epi_bar[(warp - 2) * 2]);
-    et.bar[1] = et.bar[0] + 8;
-    et.kb = 0;
-    int lt = 0;
-    for (int pt = pair_id; pt < num_ptiles; pt += num_pairs, ++lt) {
-      const int mt = (pt % pm_tiles) * 2 + rank, nt = pt / pm_tiles;
-      const int tw = mt % p.tilesW;
-      const int th = (mt / p.tilesW) % p.tilesH;
-      const int tb = mt / (p.tilesW * p.tilesH);
-      const int bb = tb * p.Bt + bt, hh = th * p.Ht + ht, ww = tw * p.Wt + wt;
-      EpiRow me;
-      me.ok = (bb < p.Bn) && (hh < p.H) && (ww < p.W);
-      me.pix = me.ok ? ((size_t)bb * p.H + hh) * (size_t)p.opix_row + (size_t)ww * p.opix_w + p.opix_off : 0;
-      me.bb = me.ok ? bb : 0;
-      const int buf = lt & 1;
-      if (p.epi_tma) {
-        // TMA epilogue: the tile's rows are contiguous rows of the output matrix, starting at the pixel of tile row 0
-        int eb0, eb1;
-        epi_linear_range(BN, half, eb0, eb1);
-        const int row0 = ((tb * p.Bt) * p.H + th * p.Ht) * p.W + tw * p.Wt + q * 32;
-        if (p.res != nullptr && eb0 < eb1 && lane == 0) {
-          bulk_wait_group_read<1>();   // the first block's box was last read by the store of block kb-2
-          epi_tma_request_res(p, et, et.kb, nt * BN + (eb0 << 5), row0);
-        }
-        mbar_wait(&tmem_full[buf], (lt >> 1) & 1);
-        tc_fence_after();
-        const uint32_t trow_t = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN);
-        if (p.mode == IGEMM_GEGLU) epilogue_tile_tma_geglu(p, et, trow_t, nt, nt * BN, half, row0, lane);
-        else epilogue_tile_tma(p, et, trow_t, nt * BN, eb0, eb1, row0, me.bb, me.ok, lane);
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) {
-          if (rank == 0) mbar_arrive(&tmem_empty[buf]);
-          else mbar_arrive_remote(mapa_rank(smem_u32(&tmem_empty[buf]), 0));
-        }
-        continue;
-      }
-      // row descriptors + the first block's residual/bias are fetched while the MMAs of this tile still run
-      const EpiRows rows = epi_rows(me, p.ldo, lane);
-      EpiPrefetch pf0;
-      {
-        int eb0, eb1;
-        epi_linear_range(BN, half, eb0, eb1);
-        const int c0 = eb0 << 5;
-        if (p.mode == IGEMM_LINEAR && (p.N & 15) == 0 && eb0 < eb1) pf0 = epi_prefetch(p, rows, nt * BN + c0, (BN - c0) >= 32 ? 32 : 16, lane);
-        else {
-#pragma unroll
-          for (int i = 0; i < 8; ++i) pf0.res[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-          pf0.bias = make_float4(0.f, 0.f, 0.f, 0.f);
-        }
-      }
-      mbar_wait(&tmem_full[buf], (lt >> 1) & 1);
-      if (dbg && lt == 0 && threadIdx.x == 64) p.dbg[3] = globaltimer_ns();  // first accumulator complete
-      tc_fence_after();
-      const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(buf * BN);
-      epilogue_tile(p, stage_buf, trow, nt, nt * BN, me, rows, pf0, half, lane);
-      if (dbg && lt == 0 && threadIdx.x == 64) p.dbg[4] = globaltimer_ns();  // first epilogue done
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) {
-        if (rank == 0) mbar_arrive(&tmem_empty[buf]);
-        else mbar_arrive_remote(mapa_rank(smem_u32(&tmem_empty[buf]), 0));
-      }
-    }
-  }
-
-  if (dbg && threadIdx.x == 0) p.dbg[5] = globaltimer_ns();  // producer done issuing
-  if (p.dbg_all != nullptr && threadIdx.x == 64) p.dbg_all[blockIdx.x * 8 + 5] = globaltimer_ns();   // this warp's epilogue done
-  if (p.epi_tma && warp >= 2 && lane == 0) bulk_wait_group_read<0>();   // the TMA stores have read their shared-memory boxes; the writes complete with the grid
-  tc_fence_before();
-  __syncthreads();
-  if (p.dbg_all != nullptr && threadIdx.x == 0) p.dbg_all[blockIdx.x * 8 + 6] = globaltimer_ns();
-  if (dbg && threadIdx.x == 0) p.dbg[6] = globaltimer_ns();  // producer warp arrived at the final barrier (the read may issue before the barrier completes)
-  cluster_sync_all();  // peer finished reading its TMEM / signalling our barriers
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc_pair(tmem_base, tmem_cols);
-  }
-  if (p.dbg_all != nullptr && threadIdx.x == 0) p.dbg_all[blockIdx.x * 8 + 7] = globaltimer_ns();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1096,16 +259,6 @@ int make_tmap_rows(CUtensorMap* tm, const __half* base, int rows_per_batch, int 
   return encode(tm, base, 3, dims, str, box);
 }
 
-// 2-D row-major [rows, ld] view with 32 x 32 boxes for the TMA epilogue (f32: 128-byte box rows, f16: 64-byte box rows)
-static int make_tmap_out(CUtensorMap* tm, const void* base, uint64_t rows, int cols, int ld, bool f32) {
-  const uint64_t es = f32 ? 4 : 2;
-  uint64_t dims[2] = {(uint64_t)cols, rows};
-  uint64_t str[1] = {(uint64_t)ld * es};
-  uint32_t box[2] = {32, 32};
-  return encode(tm, base, 2, dims, str, box, f32 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
-                f32 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_64B);
-}
-
 void igemm_pick_box(int W, int H, int* Wt, int* Ht, int* Bt) {
   int wt = 1;
   while (wt * 2 <= W && wt * 2 <= 128) wt *= 2;
@@ -1117,55 +270,28 @@ void igemm_pick_box(int W, int H, int* Wt, int* Ht, int* Bt) {
 }
 
 int igemm_pick_bn(int m_tiles, int N, int num_sms, bool geglu) {
-  // candidate tiles: multiples of 16 (32 for GEGLU so both halves are x16-aligned) that divide N exactly
-  // (or cover N when N is tiny). Cost model: waves * BN (tensor time ~ BN per tile) with a mild penalty
-  // for narrow tiles (operand re-reads from smem/L2).
-  if (N <= 16) return 16;
+  // N tiles the kernel is instantiated for. Cost model: waves * BN (tensor time ~ BN per tile) with a fixed A-operand /
+  // epilogue cost per tile; a tile width that divides N wins over padding.
+  (void)geglu;
   double best = 1e30;
   int best_bn = 0;
-  const int step = geglu ? 32 : 16;
-  for (int bn = 256; bn >= 32; bn -= step) {
+  for (int bn = 256; bn >= 64; bn >>= 1) {
     if (N % bn) continue;
     const long tiles = (long)m_tiles * (N / bn);
     const long waves = (tiles + num_sms - 1) / num_sms;
-    double cost = (double)waves * (bn + 48.0);  // +48: fixed A-operand/epilogue cost per tile
+    const double cost = (double)waves * (bn + 48.0);
     if (cost < best) {
       best = cost;
       best_bn = bn;
     }
   }
-  if (!best_bn) {  // N has no suitable divisor: cover with padding
-    best_bn = N >= 256 ? 256 : ((N + 15) / 16) * 16;
-  }
-  return best_bn;
-}
-
-// N tile for the 2-CTA kernel. Measured model (tools/igemm_timeline.py, B200): one 64-deep K block costs
-// max(~420 clk issue floor, 2*BN clk tensor time, delivery at ~9000 B/clk chip-wide); the epilogue of a tile costs
-// ~2600 clk per 32-column block per warp (two warps share a lane quarter) and is exposed once per CTA.
-static int igemm_pick_bn_pair(int m_tiles, int N, int kblocks, int num_sms) {
-  double best = 1e30;
-  int best_bn = 0;
-  for (int bn = 256; bn >= 32; bn -= 32) {
-    if (N % bn) continue;
-    const long pairs = (long)(m_tiles / 2) * (N / bn);
-    const long slots = num_sms / 2;
-    const long waves = (pairs + slots - 1) / slots;
-    const long active = pairs < slots ? pairs : slots;
-    double per_kb = 420.0;
-    if (2.0 * bn > per_kb) per_kb = 2.0 * bn;
-    const double bw = (double)active * 2.0 * (16384.0 + bn * 64.0) / 9000.0;
-    if (bw > per_kb) per_kb = bw;
-    const double epi = ((bn + 31) / 32 + 1) / 2 * 2600.0;
-    const double cost = (double)waves * kblocks * per_kb + epi;
-    if (cost < best) { best = cost; best_bn = bn; }
-  }
+  if (!best_bn) best_bn = N <= 64 ? 64 : N <= 128 ? 128 : 256;   // no divisor: cover N with padding
   return best_bn;
 }
 
 // Per-device launch state: several devices may be driven from one process (one sdxl_ctx each), and the opt-in to > 48 KB of
-// dynamic shared memory, the SM count and the resident-cluster limits are all per device.
-struct IgemmDev { bool attr = false; int num_sms = 0; int max_clusters[5] = {0, 0, 0, 0, 0}; };
+// dynamic shared memory and the SM count are per device.
+struct IgemmDev { bool attr = false; int num_sms = 0; };
 static IgemmDev g_igemm_dev[64];
 static IgemmDev* igemm_dev() {
   int dev = 0;
@@ -1173,23 +299,19 @@ static IgemmDev* igemm_dev() {
   IgemmDev& D = g_igemm_dev[dev];
   if (!D.num_sms) {
     cudaDeviceGetAttribute(&D.num_sms, cudaDevAttrMultiProcessorCount, dev);
-    if (D.num_sms <= 0) D.num_sms = 148;
+    if (D.num_sms <= 0) D.num_sms = 132;
   }
   return &D;
 }
 static int device_sms() {
   IgemmDev* D = igemm_dev();
-  return D ? D->num_sms : 148;
+  return D ? D->num_sms : 132;
 }
 
-static size_t igemm_smem_bytes(int nst, int b_rows, int epi_box_bytes) {
-  return (size_t)nst * (kABytes + b_rows * 128) + 1024 /*align slack*/ + (2 * nst + 4 + 2 * kEpiWarps) * 8 + 32 + epi_area_bytes(epi_box_bytes);
-}
+static constexpr int kMaxSmem = 227 * 1024;
+static size_t igemm_smem_bytes(int nst, int BN) { return (size_t)nst * (kABytes + BN * 128) + 1024 /*align slack*/ + 2 * nst * 8; }
 
 int igemm_configure(IgemmParams& p, const IgemmOperands& o, int outW, int outH, int outB, int mode, int geglu_bn) {
-  int total_kb = 0;
-  for (int s2 = 0; s2 < p.nseg; ++s2) total_kb += p.seg[s2].nkb;
-  if (total_kb < 1) total_kb = 1;
   igemm_pick_box(outW, outH, &p.Wt, &p.Ht, &p.Bt);
   p.W = outW; p.H = outH; p.Bn = outB;
   p.opix_row = outW; p.opix_w = 1; p.opix_off = 0;
@@ -1200,141 +322,47 @@ int igemm_configure(IgemmParams& p, const IgemmOperands& o, int outW, int outH, 
   p.N = o.N;
   p.mode = mode;
   p.BN = (mode == IGEMM_GEGLU) ? geglu_bn : igemm_pick_bn(m_tiles, o.N, device_sms(), false);
-  // 2-CTA MMA (pair along M) whenever the M tile count is even and N tiles by a multiple of 32: it is the only
-  // variant that lowers the bytes delivered per SM. SDXL_B200_PAIR=0 falls back to the 1-CTA (+multicast) kernel.
-  static const bool pair_on = !(getenv("SDXL_B200_PAIR") && getenv("SDXL_B200_PAIR")[0] == '0');
-  p.pair = 0;
-  if (pair_on && m_tiles % 2 == 0 && m_tiles >= 2) {
-    if (mode == IGEMM_GEGLU) p.pair = (p.BN % 32 == 0);
-    else {
-      const int bnp = igemm_pick_bn_pair(m_tiles, o.N, total_kb, device_sms());
-      if (bnp) { p.BN = bnp; p.pair = 1; }
-    }
-  }
+  if (p.BN != 64 && p.BN != 128 && p.BN != 256) return 1010;
   p.tilesN = (mode == IGEMM_GEGLU) ? (o.N / p.BN) : ((o.N + p.BN - 1) / p.BN);
-  if ((long)m_tiles * p.tilesN < 4) p.pair = 0;
-  // cluster shape: share the A tile across 2 N-tiles and the B tile across 2 M-tiles when the tile grid is even
-  static const char* env = getenv("SDXL_B200_CLUSTER");  // "MxN" override, e.g. 1x1 to disable
-  int CM = (m_tiles % 2 == 0) ? 2 : 1, CN = (p.tilesN % 2 == 0) ? 2 : 1;
-  if ((long)m_tiles * p.tilesN < 8) CM = CN = 1;
-  if (env && env[0] && env[1] == 'x' && env[2]) {
-    const int em = env[0] - '0', en = env[2] - '0';
-    if (em >= 1 && em <= 2 && en >= 1 && en <= 2) {
-      CM = (m_tiles % em == 0) ? em : 1;
-      CN = (p.tilesN % en == 0) ? en : 1;
-    }
-  }
-  if (p.pair) { CM = 2; CN = 1; }
-  p.CM = CM; p.CN = CN;
-  // A slice (128/CN rows): split the slowest tile dimension that is >= CN
-  int sWt = p.Wt, sHt = p.Ht, sBt = p.Bt;
+  p.pair = 0;
+  p.CM = p.CN = 1;
   p.a_split_dim = 0; p.a_split_ext = 0;
-  if (CN > 1) {
-    if (p.Bt >= CN) { sBt = p.Bt / CN; p.a_split_dim = 2; p.a_split_ext = sBt; }
-    else if (p.Ht >= CN) { sHt = p.Ht / CN; p.a_split_dim = 1; p.a_split_ext = sHt; }
-    else { sWt = p.Wt / CN; p.a_split_dim = 0; p.a_split_ext = sWt; }
-  }
-  int r = make_tmap_act(&p.tmA0, o.a0, o.a0Bn, o.a0H, o.a0W, o.a0C, o.a0pitch, sWt, sHt, sBt);
-  if (!r && o.a1) r = make_tmap_act(&p.tmA1, o.a1, o.a1Bn, o.a1H, o.a1W, o.a1C, o.a1pitch, sWt, sHt, sBt);
+  p.epi_tma = 0; p.epi_box_bytes = 0;
+  int r = make_tmap_act(&p.tmA0, o.a0, o.a0Bn, o.a0H, o.a0W, o.a0C, o.a0pitch, p.Wt, p.Ht, p.Bt);
+  if (!r && o.a1) r = make_tmap_act(&p.tmA1, o.a1, o.a1Bn, o.a1H, o.a1W, o.a1C, o.a1pitch, p.Wt, p.Ht, p.Bt);
   if (!r && !o.a1) p.tmA1 = p.tmA0;
-  if (!r) r = make_tmap_wgt(&p.tmB, o.w, o.N, o.Ktot, p.BN / CM);
+  if (!r) r = make_tmap_wgt(&p.tmB, o.w, o.N, o.Ktot, p.BN);
   if (r) return r;
-  const int stage_bytes = kABytes + (p.pair ? p.BN * 64 : p.BN * 128);
-  int nst = (226 * 1024 - 1024 - 512 - kEpiAreaBytes) / stage_bytes;
+  const int stage_bytes = kABytes + p.BN * 128;
+  int nst = (kMaxSmem - 1024 - 256) / stage_bytes;
   if (nst > 8) nst = 8;
-  if (nst < 2) nst = 2;
   p.nstages = nst;
-  p.epi_box_bytes = kEpiTmaBufBytes;
-  // TMA epilogue: LINEAR tiles, 32-column blocks, tile rows = contiguous output rows (full image rows per tile and either whole
-  // images or a single image per tile), f32 output (+ optional f32 residual of the same leading dimension) or f16 output without
-  // residual. SDXL_B200_EPI_TMA=0 keeps the transposing epilogue everywhere (A/B).
-  static const bool tma_on = !(getenv("SDXL_B200_EPI_TMA") && getenv("SDXL_B200_EPI_TMA")[0] == '0');
-  p.epi_tma = 0;
-  const bool contiguous = (p.Ht == 1 && p.Bt == 1) ||   // a tile is a run of pixels inside one image row (token GEMMs: H = 1, W = M)
-                          (p.Wt == outW && (p.Ht == outH || p.Bt == 1) && outH % p.Ht == 0);   // or whole image rows
-  const bool dtype_ok = p.out_f32 ? (p.res == nullptr || p.ldr == p.ldo) : (p.res == nullptr);
-  if (tma_on && mode == IGEMM_LINEAR && contiguous && dtype_ok && p.out != nullptr && (o.N % 32) == 0 && (p.BN % 32) == 0 && (o.N % p.BN) == 0 &&
-      p.ldo >= o.N && ((size_t)p.ldo * (p.out_f32 ? 4 : 2)) % 16 == 0 && ((uintptr_t)p.out % 16) == 0 && ((uintptr_t)p.res % 16) == 0) {
-    const uint64_t rows = (uint64_t)outB * outH * outW;
-    int r2 = make_tmap_out(&p.tmOut, p.out, rows, o.N, p.ldo, p.out_f32 != 0);
-    if (!r2 && p.res) r2 = make_tmap_out(&p.tmRes, p.res, rows, o.N, p.ldr, true);
-    if (!r2 && !p.res) p.tmRes = p.tmOut;
-    if (r2) return r2;
-    p.epi_tma = 1;
-  }
-  // GEGLU tiles: [pixels, N/2] f16 output, 32-column boxes
-  if (tma_on && mode == IGEMM_GEGLU && contiguous && !p.out_f32 && p.res == nullptr && p.out != nullptr && (p.BN % 64) == 0 && (o.N % p.BN) == 0 &&
-      p.ldo >= o.N / 2 && ((size_t)p.ldo * 2) % 16 == 0 && ((uintptr_t)p.out % 16) == 0 && p.bias_bstride == 0) {
-    int r2 = make_tmap_out(&p.tmOut, p.out, (uint64_t)outB * outH * outW, o.N / 2, p.ldo, false);
-    if (r2) return r2;
-    p.tmRes = p.tmOut;
-    p.epi_tma = 1;
-  }
-  // f16 outputs through TMA boxes of 64-byte rows: half the epilogue area, one more pipeline stage (SDXL_B200_EPI_COMPACT=0: A/B)
-  static const bool compact_on = !(getenv("SDXL_B200_EPI_COMPACT") && getenv("SDXL_B200_EPI_COMPACT")[0] == '0');
-  if (compact_on && p.epi_tma && !p.out_f32) {
-    p.epi_box_bytes = kEpiTmaBufBytes / 2;
-    int n2 = (226 * 1024 - 1024 - 512 - epi_area_bytes(p.epi_box_bytes)) / stage_bytes;
-    p.nstages = n2 > 8 ? 8 : n2;
-  }
   return 0;
 }
 
 int igemm_launch(cudaStream_t st, IgemmParams& p) {
-  // the epilogue addresses outputs with 32-bit element offsets and shares the leading dimension with the residual
   if (p.res != nullptr && p.ldr != p.ldo) return 1003;
   if ((unsigned long long)p.Bn * p.H * (unsigned long long)p.opix_row * (unsigned long long)p.ldo >= (1ull << 32)) return 1004;
-  const size_t smem = igemm_smem_bytes(p.nstages, p.pair ? p.BN / 2 : p.BN, p.epi_box_bytes);
-  if (p.epi_tma && (p.opix_w != 1 || p.opix_off != 0 || p.opix_row != p.W)) {   // re-mapped output pixels (phase-decomposed upsample conv)
-    if (p.epi_box_bytes != kEpiTmaBufBytes) return 1011;   // the transposing epilogue needs the full staging area
-    p.epi_tma = 0;
-  }
+  if (p.nstages < 2) return 1011;
+  const size_t smem = igemm_smem_bytes(p.nstages, p.BN);
+  if (smem > (size_t)kMaxSmem) return 1011;
   IgemmDev* D = igemm_dev();
   if (!D) return 1009;
   if (!D->attr) {
-    cudaError_t e = cudaFuncSetAttribute(igemm_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(igemm_pair_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(igemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(igemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(igemm_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return (int)e;
     D->attr = true;
   }
-  const int cs = p.CM * p.CN;
-  const int m_tiles = p.tilesW * p.tilesH * p.tilesB;
-  const int num_super = ((m_tiles + p.CM - 1) / p.CM) * ((p.tilesN + p.CN - 1) / p.CN);
-  // resident clusters: 1 CTA per SM; cluster placement (GPC boundaries) can strand SMs for cs = 4
-  int* max_clusters = D->max_clusters;
-  if (!max_clusters[cs]) {
-    int n = D->num_sms / cs;
-    if (cs > 1) {
-      cudaLaunchConfig_t cfg{};
-      cfg.gridDim = dim3(D->num_sms / cs * cs);
-      cfg.blockDim = dim3(kThreads);
-      cfg.dynamicSmemBytes = 200 * 1024;
-      cudaLaunchAttribute at[1];
-      at[0].id = cudaLaunchAttributeClusterDimension;
-      at[0].val.clusterDim.x = cs; at[0].val.clusterDim.y = 1; at[0].val.clusterDim.z = 1;
-      cfg.attrs = at; cfg.numAttrs = 1;
-      int q = 0;
-      if (cudaOccupancyMaxActiveClusters(&q, igemm_kernel, &cfg) == cudaSuccess && q > 0) n = q;
-      else cudaGetLastError();
-    }
-    max_clusters[cs] = n;
+  const long tiles = (long)p.tilesW * p.tilesH * p.tilesB * p.tilesN;
+  const dim3 grid((unsigned)(tiles < D->num_sms ? (tiles > 0 ? tiles : 1) : D->num_sms));
+  switch (p.BN) {
+    case 64: return launch_kernel(igemm_kernel<64>, grid, dim3(kThreads), smem, st, true, p);
+    case 128: return launch_kernel(igemm_kernel<128>, grid, dim3(kThreads), smem, st, true, p);
+    case 256: return launch_kernel(igemm_kernel<256>, grid, dim3(kThreads), smem, st, true, p);
+    default: return 1010;
   }
-  const int nclusters = num_super < max_clusters[cs] ? num_super : max_clusters[cs];
-  {
-    const unsigned long long m_tiles = (unsigned long long)p.tilesW * p.tilesH * p.tilesB;
-    const unsigned long long pm = p.pair ? m_tiles / 2 : m_tiles;
-    const unsigned long long max_pt = pm * (unsigned long long)p.tilesN;
-    auto recip = [](unsigned long long max_n, unsigned long long d) -> unsigned {
-      if (d <= 1 || max_n * d >= (1ull << 32)) return 0u;   // d == 1: floor(2^32/1)+1 overflows -> plain division
-      return (unsigned)((1ull << 32) / d + 1);
-    };
-    p.fd_pm = recip(max_pt, pm);
-    p.fd_w = recip(m_tiles, (unsigned long long)p.tilesW);
-    p.fd_wh = recip(m_tiles, (unsigned long long)p.tilesW * p.tilesH);
-    p.fd_h = 0;
-  }
-  if (p.pair) return launch_kernel_cluster(igemm_pair_kernel, dim3(nclusters * 2), dim3(kThreads), smem, st, true, 2, p);
-  return launch_kernel_cluster(igemm_kernel, dim3(nclusters * cs), dim3(kThreads), smem, st, true, cs, p);
 }
 
 }  // namespace sdxl

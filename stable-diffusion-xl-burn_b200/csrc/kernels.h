@@ -1,4 +1,4 @@
-// Host-side launch API of the sm_100a kernels (internal to libsdxl_b200.so; the public boundary is
+// Host-side launch API of the sm_90a kernels (internal to libsdxl_b200.so; the public boundary is
 // include/sdxl_b200.h). All pointers are device pointers. All launchers return cudaError_t-style
 // int (0 = ok) and never synchronise.
 #pragma once
@@ -72,7 +72,7 @@ inline int smem_optin(K kernel, int bytes, bool (&done)[64]) {
 }
 
 // ------------------------------------------------------------------------------------------------
-// Implicit GEMM on tcgen05 (igemm.cu): out[pixel, n] = epilogue( sum_seg sum_c A_seg[pixel+tap, c] *
+// Implicit GEMM on wgmma (igemm.cu): out[pixel, n] = epilogue( sum_seg sum_c A_seg[pixel+tap, c] *
 // Wt[n, k(seg,c)] ). Linear layers are the 1-segment / 1x1 case of the same kernel.
 // ------------------------------------------------------------------------------------------------
 constexpr int IGEMM_MAX_SEG = 20;
@@ -90,11 +90,11 @@ struct alignas(64) IgemmParams {
   int Wt, Ht, Bt;             // A box in pixels, Wt*Ht*Bt == 128
   int W, H, Bn;               // output extents
   int tilesW, tilesH, tilesB, tilesN;
-  int pair;                   // 1: 2-CTA MMA kernel (cta_group::2), CM = 2, CN = 1
-  int CM, CN;                 // cluster shape (M x N CTAs sharing operand tiles via TMA multicast)
-  int a_split_dim, a_split_ext;  // how the A tile is sliced across the CN peers (0=W,1=H,2=B; extent per slice)
+  int pair;                   // always 0 (no paired-CTA variant); kept in the launch-plan dump
+  int CM, CN;                 // cluster shape, always 1 x 1; kept in the launch-plan dump
+  int a_split_dim, a_split_ext;  // unused (no clusters)
   int N;                      // valid output columns (GEGLU: columns of the fused [value|gate] GEMM)
-  int BN;                     // N tile (multiple of 16, <= 256)
+  int BN;                     // N tile: 64, 128 or 256
   int nstages;
   int mode;                   // IgemmMode
   void* out;                  // f16 or f32 [pixels, ldo]
@@ -108,17 +108,14 @@ struct alignas(64) IgemmParams {
   // upsample + 3x3 conv is run as four 2x2 convolutions on the original image, each writing one (row, column) parity of the
   // upsampled output: opix_row = 4W, opix_w = 2, opix_off = a*2W + b.
   int opix_row, opix_w, opix_off;
-  // TMA epilogue (igemm.cu "epilogue through TMA"): set by igemm_configure when the tile's 128 rows are contiguous rows of a plain
-  // [pixels, ldo] output (N and BN multiples of 32, LINEAR mode); igemm_launch drops it if the caller re-mapped the output pixels.
-  CUtensorMap tmOut, tmRes;   // 2-D [pixels, ldo] views, box 32 rows x 32 columns (f32: SWIZZLE_128B, f16: SWIZZLE_64B)
+  // unused: the epilogue stores from the accumulator registers
+  CUtensorMap tmOut, tmRes;
   int epi_tma;
-  int epi_box_bytes;          // bytes of one epilogue box in shared memory: 4096 (32 rows x 128 B), or 2048 for f16 outputs on the TMA epilogue
-  // host-computed reciprocals (floor(2^32/d)+1; q = umulhi(n, m), exact while n*d < 2^32; 0 = use '/') for the tile-index
-  // divisions of the producer warp: on the critical path between griddepcontrol.wait and the first TMA issue
-  unsigned fd_pm, fd_w, fd_h, fd_wh;   // divisors: pair M tiles (or M tiles), tilesW, tilesH, tilesW*tilesH
-  int dbg_mode;               // diagnostics only: 1 = skip TMA loads, 2 = skip MMAs (results are garbage)
-  unsigned long long* dbg;    // nullable: per-role %globaltimer stamps of CTA 0 (tools/igemm_timeline.py)
-  unsigned long long* dbg_all;  // nullable: [gridDim.x][4] stamps of EVERY CTA (entry, prologue done, dependencies resolved, exit): launch ramp / drain
+  int epi_box_bytes;
+  unsigned fd_pm, fd_w, fd_h, fd_wh;
+  int dbg_mode;               // unused by the wgmma kernel
+  unsigned long long* dbg;    // unused by the wgmma kernel (no per-role timestamps)
+  unsigned long long* dbg_all;  // unused by the wgmma kernel
 };
 // A operand view: NHWC f16 tensor [Bn, H, W, C] with channel pitch `pitch` (elements, multiple of 8).
 int make_tmap_act(CUtensorMap* tm, const __half* base, int Bn, int H, int W, int C, int pitch, int Wt,

@@ -241,7 +241,7 @@ int gn_launch(cudaStream_t st, GnParams& p) {
   if (R > 16) R = 16;
   // chunking depends on HW only (never on the batch size): every sample's statistics are summed in the
   // same order whatever B is, which keeps the whole forward batch-invariant bit for bit.
-  int nchunk = 148;
+  int nchunk = 132;   // one CTA per SM of an H100 SXM
   const int max_chunks = cdiv(p.HW, R);
   if (nchunk > max_chunks) nchunk = max_chunks;
   p.nchunk = nchunk;
@@ -258,7 +258,7 @@ int gn_launch(cudaStream_t st, GnParams& p) {
   if (R2 < 1) R2 = 1;
   if (R2 > 32) R2 = 32;
   int ctas = cdiv(p.HW, R2 * 4);
-  const int cap = (148 * 8) / (p.B > 0 ? p.B : 1);
+  const int cap = (132 * 8) / (p.B > 0 ? p.B : 1);
   if (ctas > cap) ctas = cap;
   if (ctas < 1) ctas = 1;
   return launch_kernel(gn_apply_kernel, dim3(ctas, p.B), dim3(V8 * R2), (size_t)0, st, true, p.x1, p.C1, p.x2, p.C2, p.HW,

@@ -9,7 +9,7 @@
 //                                   src/model/autoencoder/mod.rs:436-452, 507-524, 548-586, 298-324
 //   LatentDecoder                   src/model/stablediffusion/mod.rs:199-237, 263-266
 // Same machinery as the UNet: weights re-laid-out once on the device, a flat launch plan replayed as a CUDA graph.
-// All convolutions and the attention contractions run on the tcgen05 implicit-GEMM kernel with f16 operands and f32
+// All convolutions and the attention contractions run on the wgmma implicit-GEMM kernel with f16 operands and f32
 // accumulation; the residual stream, GroupNorm statistics, the score matrix and the softmax are f32 (the reference
 // runs this module in f32 end to end; tests/test_vae_gpu.py states the resulting tolerance).
 // The attention block is single-head with d = C (512): scores are materialised (f32 [T,T] per image, 1.07 GB at

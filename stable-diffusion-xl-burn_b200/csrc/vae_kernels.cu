@@ -1,7 +1,7 @@
 // Kernels that only the latent decoder needs (reference src/model/autoencoder/mod.rs, stablediffusion/mod.rs:199-266):
 // the single-head d=512 attention's row softmax over a materialised score matrix, an f16 matrix transpose for the
 // P·V GEMM's K-major V operand, the 1x1 post_quant_conv on the 4-channel latent, and the image converters.
-// All are HBM-bound byte movers; the contractions of the decoder run on the tcgen05 implicit-GEMM kernel (igemm.cu).
+// All are HBM-bound byte movers; the contractions of the decoder run on the wgmma implicit-GEMM kernel (igemm.cu).
 #include "common.cuh"
 #include "kernels.h"
 
@@ -143,7 +143,7 @@ int post_quant_launch(cudaStream_t st, const float* x, int B, int C, int HW, con
                       float inv_scale, float* y) {
   if (C > 8 || C < 1) return 6003;
   int grid = cdiv((long)B * HW, 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   post_quant_kernel<<<grid, 256, 0, st>>>(x, B, C, HW, w, bias, inv_scale, y);
   return (int)cudaGetLastError();
 }
@@ -165,7 +165,7 @@ __global__ void image_u8_kernel(const float* __restrict__ x, long npix, int ldx,
 }
 int image_u8_launch(cudaStream_t st, const float* x, long npix, int ldx, uint8_t* out) {
   int grid = cdiv(npix, 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   image_u8_kernel<<<grid, 256, 0, st>>>(x, npix, ldx, out);
   return (int)cudaGetLastError();
 }
@@ -185,7 +185,7 @@ __global__ void image_from_u8_kernel(const uint8_t* __restrict__ in, int B, long
 }
 int image_from_u8_launch(cudaStream_t st, const uint8_t* in, int B, long HW, float* out) {
   int grid = cdiv((long)B * HW, 256);
-  if (grid > 148 * 16) grid = 148 * 16;
+  if (grid > 132 * 16) grid = 132 * 16;
   image_from_u8_kernel<<<grid, 256, 0, st>>>(in, B, HW, out);
   return (int)cudaGetLastError();
 }
@@ -213,7 +213,7 @@ int quant_out_launch(cudaStream_t st, const float* x, int B, int Cz, int Cout, l
                      float scale, float* y) {
   if (Cz > 16 || Cout > Cz || Cout < 1) return 6004;
   int grid = cdiv((long)B * HW, 256);
-  if (grid > 148 * 8) grid = 148 * 8;
+  if (grid > 132 * 8) grid = 132 * 8;
   quant_out_kernel<<<grid, 256, 0, st>>>(x, B, Cz, Cout, HW, w, bias, scale, y);
   return (int)cudaGetLastError();
 }

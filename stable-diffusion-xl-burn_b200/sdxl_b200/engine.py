@@ -34,7 +34,7 @@ class Context:
     def __init__(self, device: int = 0):
         self.lib = _lib.load()
         if not torch.cuda.is_available():
-            raise SdxlError("sdxl_b200 needs a CUDA device (sm_100); there is no CPU fallback")
+            raise SdxlError("sdxl_b200 needs a CUDA device (sm_90); there is no CPU fallback")
         self.device = torch.device("cuda", device)
         torch.cuda.set_device(self.device)
         self.stream = torch.cuda.Stream(self.device)
@@ -317,7 +317,7 @@ class Diffuser:
     def plan_num_ops(self) -> int:
         return int(self.ctx.lib.sdxl_unet_plan_num_ops(self.h))
 
-    KIND_NAMES = ["igemm_tcgen05", "attention_tcgen05", "group_norm", "layer_norm", "gemv", "timestep_embedding",
+    KIND_NAMES = ["igemm_wgmma", "attention_wgmma", "group_norm", "layer_norm", "gemv", "timestep_embedding",
                   "conv_in", "upsample2x", "phase_split", "cast_f16"]
 
     def profile_plan(self) -> Dict[str, Dict[str, float]]:

@@ -2,7 +2,7 @@
 
 Shared by tests/golden/make_fullsize_golden.py (which runs the CPU f32 oracle once, offline, and commits the
 final latents under tests/golden/) and by tests/test_fullsize_parity_gpu.py (which runs the same inputs through
-libsdxl_b200.so on the B200 and compares). Everything is drawn from torch CPU generators, so both sides see
+libsdxl_b200.so on the GPU and compares). Everything is drawn from torch CPU generators, so both sides see
 bit-identical weights and inputs on any machine. Weights: sdxl_b200.synth_weights(cfg, seed, device="cpu").
 """
 from __future__ import annotations

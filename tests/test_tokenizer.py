@@ -2,11 +2,14 @@
 
 Pinning chain: the reference's known-answer vector (src/token/clip.rs:232-249) pins the Python oracle
 (oracle/tokenizer_oracle.py, a line-by-line restatement); the oracle generated tests/golden/tokenizer_vectors.json; the C++
-tokenizer must reproduce those vectors and agree with the oracle on a seeded fuzz corpus. Tests that need the reference's
-vocabulary files (3 MB of third-party data that is not copied into this repo) look in $SDXL_TOKENIZER_DIR or
-/root/reference/tokenizer and skip when absent; the mini-vocabulary tests run everywhere. CPU only, no GPU call.
+tokenizer must reproduce those vectors and agree with the oracle on a seeded fuzz corpus. The real vocabularies are stored
+xz-compressed under tests/golden/vocab: the OpenCLIP merges.txt / vocab.txt / tokenizer.json as shipped by the reference, and
+the CLIP merge file as the merges it reads (its bpe_simple_vocab_16e6.txt is one header line followed by exactly these merges;
+the lines past merge 48894 are never read, clip.rs:98). They are unpacked into a temporary directory per module. CPU only,
+no GPU call.
 """
 import json
+import lzma
 import os
 import random
 
@@ -18,9 +21,8 @@ from sdxl_b200 import SdxlError
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 MINI = os.path.join(GOLD, "mini_bpe")
-REF_TOK = os.environ.get("SDXL_TOKENIZER_DIR", "/root/reference/tokenizer")
-HAVE_REF = os.path.exists(os.path.join(REF_TOK, "clip", "bpe_simple_vocab_16e6.txt"))
-need_ref = pytest.mark.skipif(not HAVE_REF, reason="reference vocabulary files not present")
+VOCAB = os.path.join(GOLD, "vocab")
+CLIP_MERGES_HEADER = '"bpe_simple_vocab_16e6.txt#version: 0.2\n'
 VEC = json.load(open(os.path.join(GOLD, "tokenizer_vectors.json"), encoding="utf-8"))
 
 KAT_TEXT = "Hello world! <|startoftext|>asdf<|startoftext|>"
@@ -35,13 +37,27 @@ def mini():
 
 
 @pytest.fixture(scope="module")
-def real():
-    c = os.path.join(REF_TOK, "clip", "bpe_simple_vocab_16e6.txt")
-    m, v = os.path.join(REF_TOK, "open_clip", "merges.txt"), os.path.join(REF_TOK, "open_clip", "vocab.txt")
+def ref_dir(tmp_path_factory):
+    """The real vocabulary files, unpacked from tests/golden/vocab in the reference's directory layout."""
+    d = tmp_path_factory.mktemp("tokenizer")
+    unpack = lambda name: lzma.decompress(open(os.path.join(VOCAB, name), "rb").read())  # noqa: E731
+    merges = unpack("open_clip_merges.txt.xz")
+    (d / "open_clip").mkdir()
+    (d / "clip").mkdir()
+    (d / "open_clip" / "merges.txt").write_bytes(merges)
+    (d / "open_clip" / "vocab.txt").write_bytes(unpack("open_clip_vocab.txt.xz"))
+    (d / "clip" / "bpe_simple_vocab_16e6.txt").write_bytes(CLIP_MERGES_HEADER.encode() + merges)
+    (d / "tokenizer.json").write_bytes(unpack("open_clip_tokenizer.json.xz"))
+    return str(d)
+
+
+@pytest.fixture(scope="module")
+def real(ref_dir):
+    c = os.path.join(ref_dir, "clip", "bpe_simple_vocab_16e6.txt")
+    m, v = os.path.join(ref_dir, "open_clip", "merges.txt"), os.path.join(ref_dir, "open_clip", "vocab.txt")
     return {"clip": (ClipTokenizer(c), TO.ClipTokenizer(c)), "open_clip": (OpenClipTokenizer(m, v), TO.OpenClipTokenizer(m, v))}
 
 
-@need_ref
 def test_reference_known_answer_pins_the_oracle(real):
     """src/token/clip.rs:232-249, verbatim."""
     _, oracle = real["clip"]
@@ -50,7 +66,6 @@ def test_reference_known_answer_pins_the_oracle(real):
     assert oracle.decode(enc) == KAT_DECODE
 
 
-@need_ref
 def test_reference_known_answer_cxx(real):
     tok, _ = real["clip"]
     enc = tok.encode(KAT_TEXT, False, False)
@@ -61,7 +76,6 @@ def test_reference_known_answer_cxx(real):
     assert otok.padding_token() == 0   # open_clip.rs:218-220
 
 
-@need_ref
 @pytest.mark.parametrize("which", ["clip", "open_clip"])
 def test_real_vocab_vectors(real, which):
     tok, oracle = real[which]
@@ -125,7 +139,6 @@ def test_fuzz_cxx_equals_oracle_mini(mini):
     assert n == 400
 
 
-@need_ref
 def test_fuzz_cxx_equals_oracle_real(real):
     for which in ("clip", "open_clip"):
         tok, oracle = real[which]
@@ -175,15 +188,12 @@ def test_invalid_utf8_is_replaced_like_from_utf8_lossy(mini):
         assert list(buf[:n.value]) == oracle.encode(raw.decode("utf-8", errors="replace"), False, False), raw
 
 
-@need_ref
-def test_open_clip_ids_match_huggingface_tokenizers(real):
+def test_open_clip_ids_match_huggingface_tokenizers(real, ref_dir):
     """Independent check: the HuggingFace `tokenizers` runtime on the reference's own tokenizer.json (the file its
     vocab.txt / merges.txt were exported from, tokenizer/convert.py) gives the same ids as the oracle and the C++ tokenizer
     (NFC-stable prompts: tokenizer.json normalises with NFC, the reference's Rust code does not)."""
     tk = pytest.importorskip("tokenizers")
-    path = os.path.join(REF_TOK, "tokenizer.json")
-    if not os.path.exists(path):
-        pytest.skip("tokenizer.json not present")
+    path = os.path.join(ref_dir, "tokenizer.json")
     hf = tk.Tokenizer.from_file(path)
     tok, oracle = real["open_clip"]
     for p in ["a photo of a cat", "An astronaut riding a horse on Mars, 4k, highly-detailed!!",
