@@ -8,7 +8,7 @@
 // Persistent and warp-specialised: grid = min(#tiles, #SMs), every CTA walks the tiles blockIdx.x, + gridDim.x, ...
 // (M tiles fastest, so CTAs running at the same time share the weight tile in L2).
 //   warpgroup 0     : TMA producer (one lane)
-//   warpgroups 1, 2 : consumers. Each owns 64 rows of the 128 x BN tile (wgmma.m64nNk16, N = 64 or 128 per instruction) and
+//   warpgroups 1, 2 : consumers. Each owns 64 rows of the 128 x BN tile (wgmma.m64nNk16, N = 64, 128 or 160 per instruction) and
 //                     runs the epilogue straight from its accumulator registers.
 // The shared-memory operand ring runs across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i.
 #include "common.cuh"
@@ -101,7 +101,7 @@ __device__ __forceinline__ void epilogue(const IgemmParams& p, const float (&acc
 
 template <int BN>
 __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constant__ IgemmParams p) {
-  constexpr int NC = BN >= 128 ? 128 : 64;   // N of one wgmma
+  constexpr int NC = BN == 160 ? 160 : BN >= 128 ? 128 : 64;   // N of one wgmma
   constexpr int NCH = BN / NC;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -173,7 +173,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constan
 #pragma unroll
         for (int c = 0; c < NCH; ++c) {
           const uint64_t db = wg_desc_sw128(b + c * NC * 128 + 32 * k);
-          if constexpr (NC == 128) wgmma_ss_n128(*reinterpret_cast<float(*)[64]>(acc + 64 * c), da, db, (kb | k) != 0);
+          if constexpr (NC == 160) wgmma_ss_n160(*reinterpret_cast<float(*)[80]>(acc), da, db, (kb | k) != 0);
+          else if constexpr (NC == 128) wgmma_ss_n128(*reinterpret_cast<float(*)[64]>(acc + 64 * c), da, db, (kb | k) != 0);
           else wgmma_ss_n64(*reinterpret_cast<float(*)[32]>(acc + 32 * c), da, db, (kb | k) != 0);
         }
       }
@@ -271,11 +272,13 @@ void igemm_pick_box(int W, int H, int* Wt, int* Ht, int* Bt) {
 
 int igemm_pick_bn(int m_tiles, int N, int num_sms, bool geglu) {
   // N tiles the kernel is instantiated for. Cost model: waves * BN (tensor time ~ BN per tile) with a fixed A-operand /
-  // epilogue cost per tile; a tile width that divides N wins over padding.
+  // epilogue cost per tile; a tile width that divides N wins over padding. 160 divides the UNet's 320 * 2^k widths: at 16 M
+  // tiles and N = 1280 it fills 128 of 132 SMs where 256 fills 80. The fixed cost of 48 is the least-squares fit of
+  // log(time) to waves * (BN + c) over a sweep of every BN at the SDXL step's GEMM shapes on H100 (DESIGN §4).
   (void)geglu;
   double best = 1e30;
   int best_bn = 0;
-  for (int bn = 256; bn >= 64; bn >>= 1) {
+  for (int bn : {256, 160, 128, 64}) {
     if (N % bn) continue;
     const long tiles = (long)m_tiles * (N / bn);
     const long waves = (tiles + num_sms - 1) / num_sms;
@@ -322,7 +325,7 @@ int igemm_configure(IgemmParams& p, const IgemmOperands& o, int outW, int outH, 
   p.N = o.N;
   p.mode = mode;
   p.BN = (mode == IGEMM_GEGLU) ? geglu_bn : igemm_pick_bn(m_tiles, o.N, device_sms(), false);
-  if (p.BN != 64 && p.BN != 128 && p.BN != 256) return 1010;
+  if (p.BN != 64 && p.BN != 128 && p.BN != 160 && p.BN != 256) return 1010;
   p.tilesN = (mode == IGEMM_GEGLU) ? (o.N / p.BN) : ((o.N + p.BN - 1) / p.BN);
   p.pair = 0;
   p.CM = p.CN = 1;
@@ -351,6 +354,7 @@ int igemm_launch(cudaStream_t st, IgemmParams& p) {
   if (!D->attr) {
     cudaError_t e = cudaFuncSetAttribute(igemm_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(igemm_kernel<128>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
+    if (e == cudaSuccess) e = cudaFuncSetAttribute(igemm_kernel<160>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e == cudaSuccess) e = cudaFuncSetAttribute(igemm_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize, kMaxSmem);
     if (e != cudaSuccess) return (int)e;
     D->attr = true;
@@ -360,6 +364,7 @@ int igemm_launch(cudaStream_t st, IgemmParams& p) {
   switch (p.BN) {
     case 64: return launch_kernel(igemm_kernel<64>, grid, dim3(kThreads), smem, st, true, p);
     case 128: return launch_kernel(igemm_kernel<128>, grid, dim3(kThreads), smem, st, true, p);
+    case 160: return launch_kernel(igemm_kernel<160>, grid, dim3(kThreads), smem, st, true, p);
     case 256: return launch_kernel(igemm_kernel<256>, grid, dim3(kThreads), smem, st, true, p);
     default: return 1010;
   }

@@ -94,7 +94,7 @@ struct alignas(64) IgemmParams {
   int CM, CN;                 // cluster shape, always 1 x 1; kept in the launch-plan dump
   int a_split_dim, a_split_ext;  // unused (no clusters)
   int N;                      // valid output columns (GEGLU: columns of the fused [value|gate] GEMM)
-  int BN;                     // N tile: 64, 128 or 256
+  int BN;                     // N tile: 64, 128, 160 or 256
   int nstages;
   int mode;                   // IgemmMode
   void* out;                  // f16 or f32 [pixels, ldo]
