@@ -47,6 +47,13 @@ __device__ __forceinline__ uint64_t globaltimer_ns() {
   return t;
 }
 
+// Per-thread register budget of the executing warpgroup (all its warps must execute it): producers shrink theirs so that
+// consumers can grow.
+template <int N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // Programmatic dependent launch (PDL). wait: block until the preceding kernel in the stream has completed
 // and its memory is visible (no-op when the kernel was launched without the PDL attribute).
 // launch_dependents: allow the next kernel's CTAs to start their prologue as SM resources free up.

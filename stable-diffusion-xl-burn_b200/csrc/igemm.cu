@@ -7,7 +7,7 @@
 //
 // Persistent and warp-specialised: grid = min(#tiles, #SMs), every CTA walks the tiles blockIdx.x, + gridDim.x, ...
 // (M tiles fastest, so CTAs running at the same time share the weight tile in L2).
-//   warpgroup 0     : TMA producer (one lane)
+//   warpgroup 0     : TMA producer (one lane); gives up registers to the consumers (setmaxnreg)
 //   warpgroups 1, 2 : consumers. Each owns 64 rows of the 128 x BN tile (wgmma.m64nNk16, N = 64, 128 or 160 per instruction) and
 //                     runs the epilogue straight from its accumulator registers.
 // The shared-memory operand ring runs across tile boundaries, so the loads of tile i+1 overlap the epilogue of tile i.
@@ -49,9 +49,14 @@ __device__ __forceinline__ void store2(const IgemmParams& p, size_t off, float x
 // layout: acc[4 j + 2 h + e]).
 //   LINEAR: out = acc + bias[batch] (+ f32 residual), f32 or f16.   GEGLU (reference unet/mod.rs:942-956): tile columns [0, BN/2)
 //   are values, [BN/2, BN) the matching gates; out = value * gelu_erf(gate), f16, at column nt * BN/2 + c.
+// LINEAR runs in chunks of JC column pairs: every bias and residual load of a chunk is issued before the chunk's first add, so
+// their latencies overlap. `out` may alias `res` (in-place residual add), so no load can move above an earlier store: without
+// the chunks each column pair would pay a full load round trip.
 template <int BN>
 __device__ __forceinline__ void epilogue(const IgemmParams& p, const float (&acc)[BN / 2], int tb, int th, int tw, int nt, int r0,
                                          int lane) {
+  constexpr int JC = BN == 160 ? 10 : 8;
+  static_assert((BN / 8) % JC == 0, "column pairs must split into whole chunks");
   const int cq = (lane & 3) * 2;
   const int n0 = nt * BN;
   const bool vec = ((p.ldo | p.ldr | p.bias_bstride) & 1) == 0 && ((reinterpret_cast<uintptr_t>(p.out) | reinterpret_cast<uintptr_t>(p.res) |
@@ -66,20 +71,26 @@ __device__ __forceinline__ void epilogue(const IgemmParams& p, const float (&acc
       const float* bias = p.bias ? p.bias + (size_t)bb * p.bias_bstride : nullptr;
       const float* res = p.res ? p.res + pix * p.ldr : nullptr;
 #pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int n = n0 + 8 * j + cq;
-        if (n >= p.N) continue;
-        const bool two = n + 1 < p.N;
-        float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
-        if (bias) {
-          if (two && vec) { const float2 b = __ldg(reinterpret_cast<const float2*>(bias + n)); x0 += b.x; x1 += b.y; }
-          else { x0 += bias[n]; if (two) x1 += bias[n + 1]; }
+      for (int j0 = 0; j0 < BN / 8; j0 += JC) {
+        float2 bv[JC], rv[JC];
+#pragma unroll
+        for (int jj = 0; jj < JC; ++jj) {
+          const int n = n0 + 8 * (j0 + jj) + cq;
+          const bool two = n + 1 < p.N;
+          bv[jj] = rv[jj] = make_float2(0.f, 0.f);
+          if (n >= p.N) continue;
+          if (bias) bv[jj] = (two && vec) ? __ldg(reinterpret_cast<const float2*>(bias + n)) : make_float2(bias[n], two ? bias[n + 1] : 0.f);
+          if (res) rv[jj] = (two && vec) ? *reinterpret_cast<const float2*>(res + n) : make_float2(res[n], two ? res[n + 1] : 0.f);
         }
-        if (res) {
-          if (two && vec) { const float2 q = *reinterpret_cast<const float2*>(res + n); x0 += q.x; x1 += q.y; }
-          else { x0 += res[n]; if (two) x1 += res[n + 1]; }
+#pragma unroll
+        for (int jj = 0; jj < JC; ++jj) {
+          const int j = j0 + jj, n = n0 + 8 * j + cq;
+          if (n >= p.N) continue;
+          float x0 = acc[4 * j + 2 * h], x1 = acc[4 * j + 2 * h + 1];
+          if (bias) { x0 += bv[jj].x; x1 += bv[jj].y; }
+          if (res) { x0 += rv[jj].x; x1 += rv[jj].y; }
+          store2(p, pix * p.ldo + n, x0, x1, n + 1 < p.N, vec);
         }
-        store2(p, pix * p.ldo + n, x0, x1, two, vec);
       }
     } else {
       constexpr int hb = BN / 2;
@@ -130,6 +141,7 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constan
 
   if (warp < 4) {
     // ===================== TMA producer =====================
+    setmaxnreg_dec<40>();   // hands registers to the consumers, whose epilogue holds a chunk of loads next to the accumulators
     if (warp != 0 || lane != 0) return;
     uint32_t stage = 0, phase = 0;
     for (int st = blockIdx.x; st < num_tiles; st += gridDim.x) {
@@ -154,7 +166,8 @@ __global__ void __launch_bounds__(kThreads, 1) igemm_kernel(const __grid_constan
   }
 
   // ===================== consumers =====================
-  const int wg = (warp >> 2) - 1;                       // 0 / 1: tile rows [64 wg, 64 wg + 64)
+  setmaxnreg_inc<232>();   // 128 x 40 + 256 x 232 registers fit the SM's 64 K
+  const int wg = (warp >> 2) - 1;                      // 0 / 1: tile rows [64 wg, 64 wg + 64)
   const int r0 = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   const uint32_t smem_base = smem_u32(smem);
   uint32_t stage = 0, phase = 0;
