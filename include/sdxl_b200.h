@@ -312,6 +312,35 @@ SDXL_API int sdxl_clip_forward_hidden_pooled(sdxl_clip* clip, int B, const int32
                                              float* hidden_out, float* pooled_out, int out_on_host);
 SDXL_API double sdxl_clip_plan_flops(const sdxl_clip* clip);
 
+/* ---- LoRA adapters ----------------------------------------------------------------------------------
+ * Low-rank weight deltas merged into the device-resident weights (DESIGN.md §7). An adapter is an SDXLPK01 pack (the container
+ * of sdxl_unet_load) whose tensors are keyed by the reference's layer path (e.g.
+ * `input_blocks/4/transformer/transformer_0/attn1/query`, `output_blocks/2/upsample/conv`, `blocks/7/mlp/fc1`):
+ *   <path>/lora_down  f16 [r, in] (Linear) or [r, I, kh, kw] (conv)
+ *   <path>/lora_up    f16 [out, r] (Linear) or [O, r, 1, 1] (conv)
+ *   <path>/alpha      optional, one element (f16 or f32); missing => alpha = r
+ * With adapters a = 1..n of scales s_a active, every touched weight W (as loaded, never a previous merge) becomes
+ *   W' = f16( f32(W) + sum_a (s_a * alpha_a / r_a) * sum_r up_a[:, r] * down_a[r, :] )
+ * computed in f32 in a fixed order (adapters in array order, then rank index ascending), deterministically. In the reference's
+ * [in,out] Linear layout the delta is (up . down)^T. Exception: the 3x3 conv after a nearest-2x upsample is stored as four
+ * phase kernels whose 3x3 source is not retained; its delta is summed into the phase kernels in f32 and added to the loaded
+ * phase weights, one f16 rounding away from loading a merged pack.
+ * The call REPLACES the active set: n = 0 restores the loaded weights bit for bit and frees the backups; a new set is derived
+ * from the loaded weights again (layers no longer touched are restored). Every tensor of every adapter is validated (known
+ * layer, dtype, shapes, equal rank of down and up) before any weight is written: on failure the call returns non-zero, names the
+ * tensor in sdxl_last_error and the model is unchanged. The first touch of a layer copies it to a device backup held until
+ * n = 0 or destroy. The launch plan and its CUDA graph stay valid; for the UNet the hoisted conditioning (cross-attention K/V,
+ * label MLP) is recomputed when conditioning is set. At most SDXL_MAX_ADAPTERS adapters per call. Queued on the ctx stream. */
+#define SDXL_MAX_ADAPTERS 16
+typedef struct sdxl_adapter {
+  const void* pack;        /* SDXLPK01 pack, host or device memory (pack_on_device); borrowed for the call */
+  size_t bytes;
+  int32_t pack_on_device;
+  float scale;             /* s_a */
+} sdxl_adapter;
+SDXL_API int sdxl_unet_set_adapters(sdxl_unet* unet, int n, const sdxl_adapter* adapters);
+SDXL_API int sdxl_clip_set_adapters(sdxl_clip* clip, int n, const sdxl_adapter* adapters);
+
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),
  * ones inside the window, zero outside, inverted by crop_out; mask = 1 keeps the generated latent. Negative bound = not given

@@ -31,12 +31,14 @@ struct sdxl_clip {
   int* err_dev = nullptr;
   float* hidden = nullptr;   // [B*T, C] result of forward_hidden / h_out
   float* pooled = nullptr;   // [B, embed_dim]
+  AdapterState lora;         // LoRA-able weight slots, backups of merged layers (sdxl_clip_set_adapters)
 };
 
 static int build_clip(sdxl_clip* m, const PackView& pv, Arena& A) {
   sdxl_ctx* c = m->ctx;
   const sdxl_clip_cfg& g = m->cfg;
   Loader L{nullptr, c, &pv, &A, c->stream};
+  L.reg = &m->lora;
   const int C = g.n_state;
   m->blocks.clear();
   auto table = [&](const std::string& name, int rows, __half*& dst) {
@@ -270,6 +272,13 @@ extern "C" int sdxl_clip_forward_hidden_pooled(sdxl_clip* m, int Bn, const int32
   r = clip_copy_out(m, m->hidden, (size_t)Bn * m->cfg.n_ctx * m->cfg.n_state, hidden_out, out_on_host);
   if (r) return r;
   return clip_copy_out(m, m->pooled, (size_t)Bn * (m->has_proj ? m->cfg.embed_dim : m->cfg.n_state), pooled_out, out_on_host);
+}
+// LoRA adapters (include/sdxl_b200.h; merge in engine_core.h: adapters_apply). Nothing derived from the weights is cached
+// outside the weight arena, so the plan needs no refresh.
+extern "C" int sdxl_clip_set_adapters(sdxl_clip* m, int n, const sdxl_adapter* adapters) {
+  if (!m) return -1;
+  CU(m->ctx, cudaSetDevice(m->ctx->device));
+  return adapters_apply(m->ctx, m->lora, n, adapters);
 }
 extern "C" double sdxl_clip_plan_flops(const sdxl_clip* m) { return (m && m->plan) ? m->plan->flops : 0.0; }
 

@@ -518,4 +518,114 @@ int bias_to_f32_launch(cudaStream_t st, const __half* src, int N, float* dst, in
   return (int)cudaGetLastError();
 }
 
+// ------------------------------------------------------------------------------------------------
+// LoRA merge: one 64 x 64 tile of the delta per CTA, 256 threads, 4 x 4 outputs per thread (rows ty + 16i, columns tx + 16j).
+// up / down are staged through shared memory as f32 in chunks of 32 ranks; every output is accumulated by one thread in a
+// fixed order (terms in call order, rank index ascending): deterministic, no atomics. CUDA-core FMA (see DESIGN.md).
+// ------------------------------------------------------------------------------------------------
+constexpr int LORA_TILE = 64, LORA_RC = 32;
+__global__ void __launch_bounds__(256) lora_merge_kernel(const LoraMergeParams p) {
+  __shared__ float Us[LORA_RC][LORA_TILE + 1];   // +1: the staging stores walk rr at fixed x
+  __shared__ float Ds[LORA_RC][LORA_TILE];
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+  const int n0 = blockIdx.y * LORA_TILE, k0 = blockIdx.x * LORA_TILE;
+  float tot[4][4];
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) tot[i][j] = 0.f;
+  for (int t = 0; t < p.nterm; ++t) {
+    const LoraTerm T = p.term[t];
+    float acc[4][4];
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+    for (int r0 = 0; r0 < T.r; r0 += LORA_RC) {
+      const int rc = T.r - r0 < LORA_RC ? T.r - r0 : LORA_RC;
+      __syncthreads();
+      for (int e = tid; e < LORA_RC * LORA_TILE; e += 256) {
+        {  // up [N, r] row-major: consecutive threads read consecutive ranks of one row
+          const int x = e / LORA_RC, rr = e % LORA_RC, n = n0 + x;
+          Us[rr][x] = (rr < rc && n < p.N) ? __half2float(T.up[(size_t)n * T.r + r0 + rr]) : 0.f;
+        }
+        {
+          const int rr = e / LORA_TILE, x = e % LORA_TILE, k = k0 + x;
+          Ds[rr][x] = (rr < rc && k < p.Kd) ? __half2float(T.down[(size_t)(r0 + rr) * p.Kd + k]) : 0.f;
+        }
+      }
+      __syncthreads();
+      for (int rr = 0; rr < rc; ++rr) {
+        float a[4], b[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i) a[i] = Us[rr][ty + 16 * i];
+#pragma unroll
+        for (int j = 0; j < 4; ++j) b[j] = Ds[rr][tx + 16 * j];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+#pragma unroll
+          for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+      }
+    }
+#pragma unroll
+    for (int i = 0; i < 4; ++i)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) tot[i][j] = __fadd_rn(tot[i][j], __fmul_rn(T.coef, acc[i][j]));
+  }
+#pragma unroll
+  for (int i = 0; i < 4; ++i) {
+    const int n = n0 + ty + 16 * i;
+    if (n >= p.N) continue;
+    const size_t row = (size_t)(p.row0 + geglu_perm(n, p.N, p.geglu_bn)) * p.ld;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const int k = k0 + tx + 16 * j;
+      if (k >= p.Kd) continue;
+      const float d = tot[i][j];
+      if (p.delta_out) { p.delta_out[(size_t)n * p.Kd + k] = d; continue; }
+      const size_t off = row + p.col0 + (size_t)(k % p.taps) * p.Ipad + k / p.taps;
+      // a zero delta leaves the weight's bits alone (f32(W) + 0 would turn -0 into +0)
+      if (p.f32) {
+        const float w = ((const float*)p.src)[off];
+        ((float*)p.dst)[off] = d == 0.f ? w : __half2float(__float2half_rn(w + d));
+      } else {
+        const __half w = ((const __half*)p.src)[off];
+        ((__half*)p.dst)[off] = d == 0.f ? w : __float2half_rn(__half2float(w) + d);
+      }
+    }
+  }
+}
+int lora_merge_launch(cudaStream_t st, const LoraMergeParams& p) {
+  if (p.nterm < 1 || p.nterm > LORA_MAX_TERMS || p.taps < 1) return 1;
+  dim3 grid(cdiv(p.Kd, LORA_TILE), cdiv(p.N, LORA_TILE));
+  lora_merge_kernel<<<grid, 256, 0, st>>>(p);
+  return (int)cudaGetLastError();
+}
+// same index map and tap sets as repack_upconv_kernel; padded input channels are not written
+__global__ void lora_upconv_merge_kernel(const __half* __restrict__ src, const float* __restrict__ delta, int O, int I,
+                                         __half* __restrict__ dst, int Ipad) {
+  const long total = (long)4 * O * 4 * Ipad;
+  for (long idx = (long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
+    const int i = (int)(idx % Ipad);
+    if (i >= I) continue;
+    const int tap = (int)((idx / Ipad) % 4);
+    const int o = (int)((idx / ((long)Ipad * 4)) % O);
+    const int ph = (int)(idx / ((long)Ipad * 4 * O));
+    const int a = ph >> 1, b = ph & 1, th = tap >> 1, tw = tap & 1;
+    const int kh0 = a == 0 ? (th == 0 ? 0 : 1) : (th == 0 ? 0 : 2), kh1 = a == 0 ? (th == 0 ? 0 : 2) : (th == 0 ? 1 : 2);
+    const int kw0 = b == 0 ? (tw == 0 ? 0 : 1) : (tw == 0 ? 0 : 2), kw1 = b == 0 ? (tw == 0 ? 0 : 2) : (tw == 0 ? 1 : 2);
+    float d = 0.f;
+    for (int kh = kh0; kh <= kh1; ++kh)
+      for (int kw = kw0; kw <= kw1; ++kw) d += delta[((size_t)o * I + i) * 9 + kh * 3 + kw];
+    dst[idx] = d == 0.f ? src[idx] : __float2half_rn(__half2float(src[idx]) + d);
+  }
+}
+int lora_upconv_merge_launch(cudaStream_t st, const __half* src, const float* delta, int O, int I, __half* dst, int Ipad) {
+  const long total = (long)4 * O * 4 * Ipad;
+  int grid = cdiv(total, 256);
+  if (grid > 132 * 32) grid = 132 * 32;
+  lora_upconv_merge_kernel<<<grid, 256, 0, st>>>(src, delta, O, I, dst, Ipad);
+  return (int)cudaGetLastError();
+}
+
 }  // namespace sdxl

@@ -122,6 +122,7 @@ struct sdxl_unet {
   int* t_dev = nullptr;
   int* t_pinned = nullptr;
   int t_slot = 0;              // ring position in t_pinned (per model: independent contexts never share it)
+  AdapterState lora;           // LoRA-able weight slots, backups of merged layers (sdxl_unet_set_adapters)
 };
 
 
@@ -192,6 +193,7 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   Loader L{u, c, &pv, &A, c->stream};
+  L.reg = &u->lora;
   const int mc = g.model_channels, ted = 4 * mc;
   u->in_blocks.clear();
   u->out_blocks.clear();
@@ -220,6 +222,9 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
       if (!r) r = cast_f16_to_f32_launch(c->stream, tmp, n, u->conv0_w);
       if (r) return fail(c, r, "conv0 repack failed");
     }
+    WSlot s;
+    s.base = u->conv0_w; s.conv = 1; s.f32 = 1; s.N = mc; s.I = g.in_channels; s.ks = 3; s.ld = 9 * g.in_channels; s.Ipad = g.in_channels;
+    L.record("input_blocks/0", s, n * sizeof(float));
     u->conv0_b = L.vec_f32("input_blocks/0/bias", mc);
     if (L.err) return L.err;
   }
@@ -751,6 +756,7 @@ static int set_t(sdxl_unet* u, int t) {
 // ================================================================================================
 // conditioning (step-invariant work hoisted out of UNet::forward)
 // ================================================================================================
+static int hoist_conditioning(sdxl_unet* u);
 static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* context_dev, const __half* y_dev) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
@@ -792,6 +798,14 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
   CU(c, cudaMemcpy2DAsync(u->ctx16, (size_t)u->ctx_pitch * 2, context_dev, (size_t)g.context_dim * 2, (size_t)g.context_dim * 2,
                           (size_t)B * n_ctx, cudaMemcpyDeviceToDevice, c->stream));
   KL(c, cast_f16_to_f32_launch(c->stream, y_dev, (size_t)B * g.adm_in_channels, u->y32));
+  return hoist_conditioning(u);
+}
+
+// The step-invariant projections of the retained conditioning (ctx16, y32) under the current weights.
+static int hoist_conditioning(sdxl_unet* u) {
+  sdxl_ctx* c = u->ctx;
+  const sdxl_unet_cfg& g = u->cfg;
+  const int ted = 4 * g.model_channels, B = u->condB, n_ctx = u->n_ctx;
   // label_emb = lin2(SiLU(lin1(y)))   (unet/mod.rs:464-466)
   for (int b0 = 0; b0 < B; b0 += 8) {
     const int nb = B - b0 < 8 ? B - b0 : 8;
@@ -826,6 +840,24 @@ extern "C" int sdxl_unet_set_conditioning(sdxl_unet* u, int B, int n_ctx, const 
   if (!u || !context || !y) return -1;
   CU(u->ctx, cudaSetDevice(u->ctx->device));
   return set_conditioning_dev(u, B, n_ctx, (const __half*)context, (const __half*)y);
+}
+
+// ================================================================================================
+// LoRA adapters (include/sdxl_b200.h; merge in engine_core.h: adapters_apply)
+// ================================================================================================
+extern "C" int sdxl_unet_set_adapters(sdxl_unet* u, int n, const sdxl_adapter* adapters) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  int r = adapters_apply(c, u->lora, n, adapters);
+  if (r) return r;
+  // the head conv's duplicated [W | W] copy follows conv_out
+  const Conv& cv = u->conv_out;
+  for (int h2 = 0; h2 < 2; ++h2)
+    CU(c, cudaMemcpy2DAsync(u->conv_out_w2 + (size_t)h2 * cv.Ktot, (size_t)2 * cv.Ktot * sizeof(__half), cv.w, (size_t)cv.Ktot * sizeof(__half),
+                            (size_t)cv.Ktot * sizeof(__half), (size_t)cv.O, cudaMemcpyDeviceToDevice, c->stream));
+  // cross-attention K/V and the label MLP were computed from the previous weights
+  return u->condB > 0 ? hoist_conditioning(u) : 0;
 }
 
 // ================================================================================================

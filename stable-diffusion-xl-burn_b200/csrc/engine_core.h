@@ -125,6 +125,38 @@ struct Conv {
 };
 struct Norm { float* g = nullptr; float* b = nullptr; int C = 0; float eps = 1e-5f; };
 
+// ================================================================================================
+// LoRA: registry of the LoRA-able weight slots (filled while loading) and the merge / restore state
+// ================================================================================================
+// One weight slot = one reference layer inside a re-laid-out weight buffer. Element (n, k) of the layer's [N, I*ks*ks] delta
+// (k = i*ks*ks + tap) lives at base[(row0 + geglu_perm(n)) * ld + col0 + tap * Ipad + i] (lora_merge_kernel); `up` slots
+// are the phase kernels of an upsample conv ([4][N][4*Ipad], lora_upconv_merge_kernel).
+struct WSlot {
+  void* base = nullptr;  // weight buffer (key of AdapterState::bufs)
+  int conv = 0;          // adapter factors are conv-shaped: down [r, I, ks, ks], up [N, r, 1, 1]; else down [r, I], up [N, r]
+  int up = 0, f32 = 0;   // upsample phase kernels; f32 storage (first conv)
+  int N = 0, I = 0, ks = 1;
+  size_t ld = 0;
+  int row0 = 0, col0 = 0, Ipad = 0, geglu_bn = 0;
+};
+struct AdapterState {
+  struct Buf { size_t bytes = 0; void* backup = nullptr; bool dirty = false; };
+  std::map<std::string, WSlot> slots;   // by reference layer path
+  std::map<void*, Buf> bufs;
+  std::vector<void*> allocs;             // backup allocations (one per call that touched new buffers)
+  void add(const std::string& path, const WSlot& s, size_t buf_bytes) {
+    slots[path] = s;
+    Buf& b = bufs[s.base];
+    if (buf_bytes > b.bytes) b.bytes = buf_bytes;
+  }
+  void release() {
+    for (void* p : allocs) cudaFree(p);
+    allocs.clear();
+    for (auto& kv : bufs) { kv.second.backup = nullptr; kv.second.dirty = false; }
+  }
+  ~AdapterState() { release(); }
+};
+
 struct Loader {
   void* owner;  // unused by the helpers; kept so that front ends can tag a loader
   sdxl_ctx* c;
@@ -132,6 +164,11 @@ struct Loader {
   Arena* A;
   cudaStream_t st;
   int err = 0;
+  AdapterState* reg = nullptr;  // LoRA slot registry (recorded on the real pass only)
+
+  void record(const std::string& path, const WSlot& s, size_t buf_bytes) {
+    if (reg && !A->measure) reg->add(path, s, buf_bytes);
+  }
 
   const PackEntry* need(const std::string& name, int ndim) {
     const PackEntry* e = pv->find(name);
@@ -160,6 +197,9 @@ struct Loader {
       return err = fail(c, 4006, "weight pack: '%s/weight' is [%llu,%llu], expected [%d,%d]", path.c_str(),
                         (unsigned long long)e->shape[0], (unsigned long long)e->shape[1], expectK, expectN);
     if (!A->measure) { int r = transpose_linear_launch(st, ptr(e), expectK, expectN, dst, Kpad, row0, geglu_bn); if (r) return err = fail(c, r, "transpose_linear failed"); }
+    WSlot s;
+    s.base = dst; s.N = expectN; s.I = expectK; s.ld = Kpad; s.row0 = row0; s.Ipad = Kpad; s.geglu_bn = geglu_bn;
+    record(path, s, (size_t)(row0 + expectN) * Kpad * sizeof(__half));
     return 0;
   }
   static int pad64(int k) { return (k + 63) / 64 * 64; }
@@ -186,6 +226,11 @@ struct Loader {
       return cv;
     }
     if (!A->measure) { int r = repack_upconv_launch(st, ptr(e), O, I, cv.wup, cv.Ipad); if (r) err = fail(c, r, "repack_upconv failed"); }
+    {
+      WSlot s;
+      s.base = cv.wup; s.conv = 1; s.up = 1; s.N = O; s.I = I; s.ks = 3; s.ld = cv.Ktot; s.Ipad = cv.Ipad;
+      record(path, s, (size_t)4 * O * cv.Ktot * sizeof(__half));
+    }
     cv.b = vec_f32(path + "/bias", O);
     return cv;
   }
@@ -218,6 +263,11 @@ struct Loader {
       return cv;
     }
     if (!A->measure) { int r = repack_conv_launch(st, ptr(e), O, I, ks, ks, cv.w, cv.Ktot, 0, cv.Ipad); if (r) err = fail(c, r, "repack_conv failed"); }
+    {
+      WSlot s;
+      s.base = cv.w; s.conv = 1; s.N = O; s.I = I; s.ks = ks; s.ld = cv.Ktot; s.Ipad = cv.Ipad;
+      record(path, s, (size_t)O * cv.Ktot * sizeof(__half));
+    }
     if (rows > O) {
       const PackEntry* be = need(path + "/bias", 1);
       cv.b = A->get<float>(rows);
@@ -242,6 +292,9 @@ struct Loader {
         if (!r) r = bias_to_f32_launch(st, ptr(sb), O, cv.b, 0, 1);
         if (r) err = fail(c, r, "skip repack failed");
       }
+      WSlot sk;
+      sk.base = cv.w; sk.conv = 1; sk.N = O; sk.I = I2; sk.ks = 1; sk.ld = cv.Ktot; sk.col0 = ks * ks * cv.Ipad; sk.Ipad = cv.I2pad;
+      record(skip_path, sk, (size_t)O * cv.Ktot * sizeof(__half));
     }
     return cv;
   }
@@ -617,3 +670,134 @@ struct TmpBufs {
   }
   ~TmpBufs() { for (void* d : p) cudaFreeAsync(d, st); }
 };
+
+// Replaces the active adapter set of a model whose slots are registered in S (include/sdxl_b200.h: sdxl_unet_set_adapters).
+// Phase 1 reads and validates every adapter and allocates the backups; nothing is written before it has passed. Phase 2
+// restores the layers merged by the previous call, backs up the newly touched ones and merges. Queued on the ctx stream.
+static int adapters_apply(sdxl_ctx* c, AdapterState& S, int n, const sdxl_adapter* ad) {
+  if (n < 0 || n > SDXL_MAX_ADAPTERS) return fail(c, 4600, "set_adapters: n = %d outside [0, %d]", n, SDXL_MAX_ADAPTERS);
+  if (n > 0 && !ad) return fail(c, 4601, "set_adapters: null adapter array");
+  TmpBufs tmp(c->stream);
+  std::map<std::string, std::vector<LoraTerm>> terms;   // by layer path, adapters in call order
+  for (int a = 0; a < n; ++a) {
+    PackView pv;
+    std::vector<uint8_t> table;
+    if (!ad[a].pack) return fail(c, 4602, "set_adapters: adapter %d has a null pack", a);
+    int r = parse_pack(c, ad[a].pack, ad[a].bytes, ad[a].pack_on_device, pv, table);
+    if (r) { c->err = "adapter " + std::to_string(a) + ": " + c->err; return r; }
+    if (ad[a].pack_on_device) {
+      pv.dev = (const uint8_t*)ad[a].pack;
+    } else {
+      uint8_t* d = (uint8_t*)tmp.get(ad[a].bytes);
+      if (!d) return fail(c, 4603, "set_adapters: cannot allocate %zu bytes for adapter %d", ad[a].bytes, a);
+      CU(c, cudaMemcpyAsync(d, ad[a].pack, ad[a].bytes, cudaMemcpyHostToDevice, c->stream));
+      pv.dev = d;
+    }
+    // group the tensors by layer
+    std::map<std::string, std::map<std::string, const PackEntry*>> layers;
+    for (auto& kv : pv.t) {
+      const size_t slash = kv.first.rfind('/');
+      const std::string leaf = slash == std::string::npos ? kv.first : kv.first.substr(slash + 1);
+      if (slash == std::string::npos || (leaf != "lora_down" && leaf != "lora_up" && leaf != "alpha"))
+        return fail(c, 4604, "adapter %d: tensor '%s' is not <layer>/lora_down, <layer>/lora_up or <layer>/alpha", a, kv.first.c_str());
+      layers[kv.first.substr(0, slash)][leaf] = &kv.second;
+    }
+    for (auto& L : layers) {
+      const std::string& path = L.first;
+      auto it = S.slots.find(path);
+      if (it == S.slots.end()) return fail(c, 4605, "adapter %d: '%s' is not a LoRA-able layer of this model", a, path.c_str());
+      const WSlot& s = it->second;
+      const PackEntry* dn = L.second.count("lora_down") ? L.second["lora_down"] : nullptr;
+      const PackEntry* up = L.second.count("lora_up") ? L.second["lora_up"] : nullptr;
+      const PackEntry* al = L.second.count("alpha") ? L.second["alpha"] : nullptr;
+      if (!dn || !up) return fail(c, 4606, "adapter %d: '%s/%s' is missing", a, path.c_str(), dn ? "lora_up" : "lora_down");
+      if (dn->dtype != 0) return fail(c, 4607, "adapter %d: '%s/lora_down' must be f16", a, path.c_str());
+      if (up->dtype != 0) return fail(c, 4607, "adapter %d: '%s/lora_up' must be f16", a, path.c_str());
+      const uint64_t rank = dn->ndim ? dn->shape[0] : 0;
+      const bool dn_ok = s.conv ? (dn->ndim == 4 && dn->shape[1] == (uint64_t)s.I && dn->shape[2] == (uint64_t)s.ks && dn->shape[3] == (uint64_t)s.ks)
+                                : (dn->ndim == 2 && dn->shape[1] == (uint64_t)s.I);
+      if (!dn_ok || rank < 1 || rank > 4096)
+        return fail(c, 4608, "adapter %d: '%s/lora_down' has shape [%llu,%llu,%llu,%llu] (ndim %u), expected [r, %d%s]", a, path.c_str(),
+                    (unsigned long long)dn->shape[0], (unsigned long long)dn->shape[1], (unsigned long long)dn->shape[2],
+                    (unsigned long long)dn->shape[3], dn->ndim, s.I, s.conv ? (s.ks == 3 ? ", 3, 3" : ", 1, 1") : "");
+      const bool up_ok = s.conv ? (up->ndim == 4 && up->shape[0] == (uint64_t)s.N && up->shape[2] == 1 && up->shape[3] == 1)
+                                : (up->ndim == 2 && up->shape[0] == (uint64_t)s.N);
+      if (!up_ok) return fail(c, 4609, "adapter %d: '%s/lora_up' has shape [%llu,%llu,...] (ndim %u), expected [%d, r%s]", a, path.c_str(),
+                              (unsigned long long)up->shape[0], (unsigned long long)up->shape[1], up->ndim, s.N, s.conv ? ", 1, 1" : "");
+      if (up->shape[1] != rank)
+        return fail(c, 4610, "adapter %d: '%s': lora_down has rank %llu but lora_up has rank %llu", a, path.c_str(),
+                    (unsigned long long)rank, (unsigned long long)up->shape[1]);
+      double alpha = (double)rank;
+      if (al) {
+        const uint64_t esz = al->dtype ? 4 : 2;
+        if (al->nbytes != esz) return fail(c, 4611, "adapter %d: '%s/alpha' must have one element", a, path.c_str());
+        uint8_t raw[4] = {0, 0, 0, 0};
+        if (ad[a].pack_on_device) {
+          CU(c, cudaMemcpyAsync(raw, pv.dev + al->offset, esz, cudaMemcpyDeviceToHost, c->stream));
+          CU(c, cudaStreamSynchronize(c->stream));
+        } else {
+          memcpy(raw, (const uint8_t*)ad[a].pack + al->offset, esz);
+        }
+        if (al->dtype) { float f; memcpy(&f, raw, 4); alpha = f; }
+        else { __half_raw hr; memcpy(&hr.x, raw, 2); alpha = (double)__half2float(__half(hr)); }
+        if (!isfinite(alpha)) return fail(c, 4612, "adapter %d: '%s/alpha' is not finite", a, path.c_str());
+      }
+      LoraTerm t;
+      t.up = (const __half*)(pv.dev + up->offset);
+      t.down = (const __half*)(pv.dev + dn->offset);
+      t.r = (int)rank;
+      t.coef = (float)((double)ad[a].scale * alpha / (double)rank);
+      terms[path].push_back(t);
+    }
+  }
+  // backups of the buffers touched for the first time, one allocation (a failure leaves the model unchanged)
+  {
+    std::map<void*, size_t> fresh;   // buffer -> offset in the new allocation
+    size_t total = 0;
+    for (auto& kv : terms) {
+      void* base = S.slots[kv.first].base;
+      if (S.bufs[base].backup || fresh.count(base)) continue;
+      fresh[base] = total;
+      total += (S.bufs[base].bytes + 255) & ~size_t(255);
+    }
+    if (total) {
+      uint8_t* mem = nullptr;
+      if (cudaMalloc((void**)&mem, total) != cudaSuccess) return fail(c, 4613, "set_adapters: cannot allocate %zu bytes of weight backup", total);
+      S.allocs.push_back(mem);
+      for (auto& f : fresh) S.bufs[f.first].backup = mem + f.second;
+    }
+  }
+  // phase 2: writes
+  std::map<void*, bool> touched;
+  for (auto& kv : terms) touched[S.slots[kv.first].base] = true;
+  for (auto& kv : S.bufs) {
+    AdapterState::Buf& b = kv.second;
+    if (b.dirty) CU(c, cudaMemcpyAsync(kv.first, b.backup, b.bytes, cudaMemcpyDeviceToDevice, c->stream));
+    else if (touched.count(kv.first)) CU(c, cudaMemcpyAsync(b.backup, kv.first, b.bytes, cudaMemcpyDeviceToDevice, c->stream));
+    b.dirty = touched.count(kv.first) > 0;
+  }
+  for (auto& kv : terms) {
+    const WSlot& s = S.slots[kv.first];
+    const void* src = S.bufs[s.base].backup;
+    LoraMergeParams p{};
+    p.N = s.N; p.taps = s.ks * s.ks; p.Kd = s.I * p.taps;
+    p.nterm = (int)kv.second.size();
+    for (int i = 0; i < p.nterm; ++i) p.term[i] = kv.second[i];
+    p.src = src; p.dst = s.base; p.f32 = s.f32;
+    p.ld = s.ld; p.row0 = s.row0; p.col0 = s.col0; p.Ipad = s.Ipad; p.geglu_bn = s.geglu_bn;
+    if (s.up) {
+      float* delta = (float*)tmp.get((size_t)p.N * p.Kd * sizeof(float));
+      if (!delta) return fail(c, 4614, "set_adapters: cannot allocate the upsample delta of '%s'", kv.first.c_str());
+      p.delta_out = delta;
+      KL(c, lora_merge_launch(c->stream, p));
+      KL(c, lora_upconv_merge_launch(c->stream, (const __half*)src, delta, s.N, s.I, (__half*)s.base, s.Ipad));
+    } else {
+      KL(c, lora_merge_launch(c->stream, p));
+    }
+  }
+  if (n == 0) {   // everything is restored: the backups go
+    CU(c, cudaStreamSynchronize(c->stream));
+    S.release();
+  }
+  return 0;
+}

@@ -270,4 +270,25 @@ int vec_add_f32_launch(cudaStream_t st, float* dst, const float* src, int n);  /
 // bias f16 [N] -> f32, optional GEGLU permutation, optional accumulate (dst += src).
 int bias_to_f32_launch(cudaStream_t st, const __half* src, int N, float* dst, int geglu_bn, int accumulate);
 
+// LoRA merge (elementwise.cu). The delta of one weight slot is the [N, Kd] matrix
+//   delta = sum_t coef_t * (up_t [N, r_t] @ down_t [r_t, Kd])      (f32; terms in order, rank index ascending)
+// Kd = I * taps: column k of the delta is input channel i = k / taps, tap = k % taps (down's natural [r, I, kh, kw] order).
+// Element (n, k) is stored at dst[(row0 + geglu_perm(n)) * ld + col0 + tap * Ipad + i] as f16(src + delta), with src the
+// backed-up weight at the same offset (f32 storage: float(f16(src + delta))). With `delta_out` set the kernel writes the f32
+// delta [N, Kd] there instead (upsample convs, see lora_upconv_merge_launch).
+#define LORA_MAX_TERMS 16
+struct LoraTerm { const __half* up; const __half* down; int r; float coef; };
+struct LoraMergeParams {
+  int N, Kd, taps;
+  int nterm;
+  LoraTerm term[LORA_MAX_TERMS];
+  const void* src; void* dst; int f32;
+  size_t ld; int row0, col0, Ipad, geglu_bn;
+  float* delta_out;
+};
+int lora_merge_launch(cudaStream_t st, const LoraMergeParams& p);
+// Upsample conv: the 3x3 f32 delta [O, I*9] is summed into the four 2x2 phase kernels with the tap sets of
+// repack_upconv_kernel and added to the backed-up phase weights src (layout of repack_upconv_launch's dst).
+int lora_upconv_merge_launch(cudaStream_t st, const __half* src, const float* delta, int O, int I, __half* dst, int Ipad);
+
 }  // namespace sdxl

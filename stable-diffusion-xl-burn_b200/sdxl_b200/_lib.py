@@ -56,6 +56,13 @@ class ClipCfg(C.Structure):
     _fields_ = [(n, C.c_int32) for n in ("n_vocab", "n_state", "embed_dim", "n_head", "n_ctx", "n_layer", "quick_gelu")]
 
 
+class Adapter(C.Structure):
+    _fields_ = [("pack", C.c_void_p), ("bytes", C.c_size_t), ("pack_on_device", C.c_int32), ("scale", C.c_float)]
+
+
+MAX_ADAPTERS = 16   # SDXL_MAX_ADAPTERS (include/sdxl_b200.h)
+
+
 # name -> (restype, argtypes); every symbol include/sdxl_b200.h declares
 P = C.c_void_p
 I = C.c_int
@@ -116,6 +123,8 @@ PROTOTYPES = {
     "sdxl_clip_forward_hidden": (I, [P, I, C.POINTER(C.c_int32), I, P, I]),
     "sdxl_clip_forward_hidden_pooled": (I, [P, I, C.POINTER(C.c_int32), I, P, P, I]),
     "sdxl_clip_plan_flops": (C.c_double, [P]),
+    "sdxl_unet_set_adapters": (I, [P, I, C.POINTER(Adapter)]),
+    "sdxl_clip_set_adapters": (I, [P, I, C.POINTER(Adapter)]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),
     "sdxl_mpk_encode_u16": (C.c_size_t, [P, C.c_size_t, P]),

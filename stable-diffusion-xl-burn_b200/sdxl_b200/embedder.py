@@ -10,7 +10,7 @@ import torch
 
 from . import _lib
 from .config import ClipConfig
-from .engine import Conditioning, Context, _ptr
+from .engine import Conditioning, Context, _ptr, set_adapters
 from .tokenizer import _Tokenizer
 from .weights import build_pack
 
@@ -40,6 +40,10 @@ class ClipTextEncoder:
             self.close()
         except Exception:
             pass
+
+    def set_adapters(self, adapters) -> None:
+        """Replaces the active LoRA set with [(adapter, scale), ...] (sdxl_clip_set_adapters); [] restores the loaded weights."""
+        set_adapters(self.ctx, self.ctx.lib.sdxl_clip_set_adapters, self.h, adapters, "sdxl_clip_set_adapters")
 
     def max_sequence_length(self) -> int:
         return self.cfg.n_ctx

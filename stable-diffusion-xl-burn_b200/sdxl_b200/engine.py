@@ -174,6 +174,23 @@ class Context:
         return out
 
 
+def set_adapters(ctx: "Context", fn, h, adapters: Sequence, what: str) -> None:
+    """Calls sdxl_{unet,clip}_set_adapters with [(adapter, scale), ...]; an adapter is a reference-named tensor dict
+    (sdxl_b200.lora) or a built pack (uint8 tensor, host or device)."""
+    adapters = list(adapters)
+    if len(adapters) > _lib.MAX_ADAPTERS:
+        raise SdxlError(f"{what}: at most {_lib.MAX_ADAPTERS} adapters per call, got {len(adapters)}")
+    packs = [a if isinstance(a, torch.Tensor) else build_pack(a) for a, _ in adapters]
+    arr = (_lib.Adapter * max(1, len(packs)))()
+    for i, (pk, (_, scale)) in enumerate(zip(packs, adapters)):
+        arr[i].pack, arr[i].bytes, arr[i].pack_on_device, arr[i].scale = pk.data_ptr(), pk.numel(), int(pk.is_cuda), float(scale)
+    ctx.enter()
+    if any(pk.is_cuda for pk in packs):
+        torch.cuda.current_stream(ctx.device).synchronize()
+    ctx.check(fn(h, len(packs), arr), what)
+    ctx.leave()
+
+
 @dataclass
 class Conditioning:
     """Mirror of the reference's Conditioning record (stablediffusion/mod.rs:544-555); f16 tensors."""
@@ -270,6 +287,10 @@ class Diffuser:
             self.close()
         except Exception:
             pass
+
+    def set_adapters(self, adapters: Sequence) -> None:
+        """Replaces the active LoRA set with [(adapter, scale), ...] (sdxl_unet_set_adapters); [] restores the loaded weights."""
+        set_adapters(self.ctx, self.ctx.lib.sdxl_unet_set_adapters, self.h, adapters, "sdxl_unet_set_adapters")
 
     # ---- UNet::forward -------------------------------------------------------------------------
     def set_conditioning(self, context: torch.Tensor, label: torch.Tensor) -> None:

@@ -27,10 +27,33 @@ def make_inpaint_mask(img_hw: Tuple[int, int], latent_hw: Tuple[int, int], crop_
 
 def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_steps: int = 30, refiner=None,
            reference_rgb: Optional[torch.Tensor] = None, crop: Sequence[Optional[int]] = (None, None, None, None), crop_out: bool = False,
-           resolution: Tuple[int, int] = (1024, 1024), seed: int = 0, noise: Optional[torch.Tensor] = None) -> torch.Tensor:
+           resolution: Tuple[int, int] = (1024, 1024), seed: int = 0, noise: Optional[torch.Tensor] = None,
+           loras: Optional[Sequence] = None) -> torch.Tensor:
     """One image, like `sample --prompt ... [--reference-img ... --crop-* ...] [--use-refiner]`.
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
-    bottom) in pixels. Returns uint8 [1, H, W, 3]."""
+    bottom) in pixels. loras: [(kohya .safetensors path / bytes / tensor dict, scale), ...] merged into the base UNet and both
+    text encoders for this call (the refiner is left alone) and removed again afterwards, which also clears any adapter set
+    those models had. Returns uint8 [1, H, W, 3]."""
+    if not loras:
+        return _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
+                       seed, noise)
+    from .lora import load_kohya
+    parts = [load_kohya(src, diffuser.cfg, embedder.clip.cfg, embedder.open_clip.cfg) for src, _ in loras]
+    active = []
+    try:
+        for model, key in ((diffuser, "unet"), (embedder.clip, "te1"), (embedder.open_clip, "te2")):
+            sets = [(p[key], scale) for p, (_, scale) in zip(parts, loras) if p[key]]
+            if sets:
+                active.append(model)
+                model.set_adapters(sets)
+        return _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
+                       seed, noise)
+    finally:
+        for model in active:
+            model.set_adapters([])
+
+
+def _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution, seed, noise):
     if reference_rgb is not None:
         resolution = (int(reference_rgb.shape[1]), int(reference_rgb.shape[2]))        # main.rs:225-229: orig_dims
     size = [int(resolution[0]), int(resolution[1])]

@@ -11,7 +11,8 @@ SURVEY.md 8(d): W ~ N(0, 1/fan_in), residual-branch output projections scaled do
 gamma = 1 + N(0, 0.05^2), beta ~ N(0, 0.05^2); one master seed.
 
 Pack format ("SDXLPK01"): header {magic[8], u32 n_tensors, u32 0, u64 data_offset}, n_tensors entries
-{char name[120], u32 dtype(0=f16), u32 ndim, u64 shape[4], u64 offset, u64 nbytes}, data (256B aligned).
+{char name[120], u32 dtype(0=f16, 1=f32), u32 ndim, u64 shape[4], u64 offset, u64 nbytes}, data (256B aligned).
+Model weights are f16; f32 entries are used only by LoRA adapter packs (`alpha`).
 """
 from __future__ import annotations
 
@@ -223,7 +224,7 @@ _HEADER = struct.Struct("<8sIIQ")
 
 
 def build_pack(tensors: Dict[str, torch.Tensor], device: str | None = None, pin: bool = False) -> torch.Tensor:
-    """Serialises name->f16 tensor into one flat uint8 tensor (on `device`, default: the tensors' device)."""
+    """Serialises name->f16 (or f32) tensor into one flat uint8 tensor (on `device`, default: the tensors' device)."""
     items = list(tensors.items())
     if device is None:
         device = str(items[0][1].device)
@@ -232,11 +233,11 @@ def build_pack(tensors: Dict[str, torch.Tensor], device: str | None = None, pin:
     data_offset = off
     entries = []
     for name, t in items:
-        if t.dtype != torch.float16:
-            raise TypeError(f"{name}: pack tensors must be f16")
+        if t.dtype not in (torch.float16, torch.float32):
+            raise TypeError(f"{name}: pack tensors must be f16 or f32")
         if t.dim() > 4 or len(name.encode()) >= 120:
             raise ValueError(f"{name}: unsupported rank/name")
-        nbytes = t.numel() * 2
+        nbytes = t.numel() * t.element_size()
         shape = list(t.shape) + [0] * (4 - t.dim())
         entries.append((name, t, off, nbytes, shape))
         off = (off + nbytes + 255) // 256 * 256
@@ -247,8 +248,8 @@ def build_pack(tensors: Dict[str, torch.Tensor], device: str | None = None, pin:
         buf = torch.zeros(total, dtype=torch.uint8, device=device)
     head = bytearray(_HEADER.pack(b"SDXLPK01", len(items), 0, data_offset))
     for name, t, o, nbytes, shape in entries:
-        head += _ENTRY.pack(name.encode(), 0, t.dim(), *shape, o, nbytes)
+        head += _ENTRY.pack(name.encode(), int(t.dtype == torch.float32), t.dim(), *shape, o, nbytes)
     buf[: len(head)] = torch.frombuffer(head, dtype=torch.uint8).to(buf.device)
     for name, t, o, nbytes, shape in entries:
-        buf[o:o + nbytes] = t.contiguous().view(torch.uint8).reshape(-1).to(buf.device)
+        buf[o:o + nbytes] = t.contiguous().reshape(-1).view(torch.uint8).to(buf.device)
     return buf
