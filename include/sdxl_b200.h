@@ -341,6 +341,45 @@ typedef struct sdxl_adapter {
 SDXL_API int sdxl_unet_set_adapters(sdxl_unet* unet, int n, const sdxl_adapter* adapters);
 SDXL_API int sdxl_clip_set_adapters(sdxl_clip* clip, int n, const sdxl_adapter* adapters);
 
+/* ---- ControlNet --------------------------------------------------------------------------------------
+ * Spatial conditioning (DESIGN.md §8), the published SDXL ControlNet architecture (diffusers ControlNetModel, SGM cldm.ControlNet):
+ * a copy of the UNet's time / label MLPs, first conv, input blocks and middle block, a hint encoder and one 1x1 "zero conv" per
+ * skip tensor. Pack (SDXLPK01): the UNet's names for the encoder half (lin{1,2}_time_embed, lin{1,2}_label_embed, input_blocks/...,
+ * middle_block/...) plus input_hint_block/{0,2,...,14}/{weight,bias} (SGM indices), zero_convs/<i>/{weight,bias} [C,C,1,1] and
+ * middle_block_out/{weight,bias}. A net is built on one ctx and may be attached to any UNet of that ctx whose cfg matches. */
+typedef struct sdxl_controlnet sdxl_controlnet;
+typedef struct sdxl_controlnet_cfg {
+  sdxl_unet_cfg unet;                           /* encoder half; channels, levels, depths, context_dim, adm must equal the UNet's */
+  int32_t hint_in_channels;                     /* 3 */
+  int32_t n_hint_blocks;                        /* 4: total downscale 2^(n-1) must be 8 */
+  int32_t hint_block_channels[SDXL_MAX_LEVELS]; /* 16, 32, 96, 256 (multiples of 8) */
+} sdxl_controlnet_cfg;
+SDXL_API int sdxl_controlnet_load(sdxl_ctx* ctx, const sdxl_controlnet_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
+                                  sdxl_controlnet** out);
+/* Destroying a net that is still attached to a UNet (sdxl_unet_set_controls) is a caller error: detach first. */
+SDXL_API void sdxl_controlnet_destroy(sdxl_controlnet* net);
+#define SDXL_MAX_CONTROLS 4
+typedef struct sdxl_control {
+  const sdxl_controlnet* net;
+  const float* hint;        /* f32 NCHW [n_hint, hint_in_channels, height, width] in [0, 1]; host if hint_on_host; borrowed for the call */
+  int32_t hint_on_host;
+  int32_t n_hint;           /* UNet row b uses hint b % n_hint (CFG rows [cond | uncond] share the image's hint) */
+  int32_t height, width;    /* pixels; the latent must be height/8 x width/8 */
+  float scale;              /* residual scale s: skip_i += s * zero_conv_i(h_i) */
+} sdxl_control;
+/* Replaces the UNet's set of attached controls (n = 0 detaches all). After the UNet's middle block each control runs its own encoder
+ * on the same x, t, context and label (h0 = conv_in(x) + hint_emb) and adds s * zero_conv_i(h_i) to skip i and
+ * s * middle_block_out(mid) to the middle output, controls in array order. Everything is validated before anything changes (cfg
+ * fields, ctx, n_hint >= 1, n <= SDXL_MAX_CONTROLS): on failure the previous set stays attached. The hints are encoded during the
+ * call. A call that keeps the nets, n_hint and sizes and changes only scales or hint values rewrites buffers in place (no new
+ * launch plan); any other change rebuilds the plan at the next forward. A runtime failure after validation (device allocation or
+ * launch error) during such an in-place rewrite can leave controls 0..k-1 updated and k..n-1 not: call again, or detach. A forward or sampler_begin whose latent is not
+ * height/8 x width/8, or whose batch is not a multiple of n_hint, fails. */
+SDXL_API int sdxl_unet_set_controls(sdxl_unet* unet, int n, const sdxl_control* controls);
+/* Test aid: the hint encoder's output hint_emb f32 NCHW [n, model_channels, H/8, W/8] of hint f32 NCHW [n, 3, H, W]; both
+ * pointers are host memory if on_host. */
+SDXL_API int sdxl_controlnet_embed_hint(sdxl_controlnet* net, int n, int H, int W, const float* hint, int on_host, float* out);
+
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),
  * ones inside the window, zero outside, inverted by crop_out; mask = 1 keeps the generated latent. Negative bound = not given

@@ -134,7 +134,7 @@ constexpr int kConvInPix = 8;
 template <typename TIn>
 __global__ void __launch_bounds__(256) conv_in_kernel(const TIn* __restrict__ x, int Bx, int B, int Cin, int H, int W,
                                                       const float* __restrict__ w, const float* __restrict__ bias, int Cout,
-                                                      float* __restrict__ y) {
+                                                      float* __restrict__ y, const float* __restrict__ add, int n_add) {
   extern __shared__ float sw[];  // [9*Cin][Cout]  (k-major: lanes = consecutive output channels, conflict-free)
   const int kk = 9 * Cin;
   for (int co = threadIdx.x; co < Cout; co += blockDim.x)          // lanes = consecutive rows of w: conflict-free smem writes,
@@ -178,14 +178,23 @@ __global__ void __launch_bounds__(256) conv_in_kernel(const TIn* __restrict__ x,
       }
     }
     float* yo = y + (((size_t)b * H + hh) * W + w0) * Cout + cv * 4;
+    if (add) {   // ControlNet: h0 = conv_in(x) + hint_emb[b % n_add]
+      const float* ao = add + (((size_t)(b % n_add) * H + hh) * W + w0) * Cout + cv * 4;
+#pragma unroll
+      for (int i = 0; i < kConvInPix; ++i)
+        if (w0 + i < W) {
+          const float4 a = *reinterpret_cast<const float4*>(ao + (size_t)i * Cout);
+          acc[i].x += a.x; acc[i].y += a.y; acc[i].z += a.z; acc[i].w += a.w;
+        }
+    }
 #pragma unroll
     for (int i = 0; i < kConvInPix; ++i)
       if (w0 + i < W) *reinterpret_cast<float4*>(yo + (size_t)i * Cout) = acc[i];
   }
 }
 int conv_in_launch_t(cudaStream_t st, const void* x, int x_f32, int Bx, int B, int Cin, int H, int W, const float* w,
-                     const float* bias, int Cout, float* y) {
-  if (Cin > 8 || (Cout & 3)) return 2002;
+                     const float* bias, int Cout, float* y, const float* add, int n_add) {
+  if (Cin > 8 || (Cout & 3) || (add && n_add < 1)) return 2002;
   const size_t smem = (size_t)Cout * 9 * Cin * sizeof(float);
   static bool done_f[64], done_h[64];
   if (smem > 200 * 1024) return 2002;
@@ -195,9 +204,9 @@ int conv_in_launch_t(cudaStream_t st, const void* x, int x_f32, int Bx, int B, i
   int grid = cdiv(total, 256);
   if (grid > 132 * 4) grid = 132 * 4;
   if (x_f32)
-    conv_in_kernel<float><<<grid, 256, smem, st>>>((const float*)x, Bx, B, Cin, H, W, w, bias, Cout, y);
+    conv_in_kernel<float><<<grid, 256, smem, st>>>((const float*)x, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add);
   else
-    conv_in_kernel<__half><<<grid, 256, smem, st>>>((const __half*)x, Bx, B, Cin, H, W, w, bias, Cout, y);
+    conv_in_kernel<__half><<<grid, 256, smem, st>>>((const __half*)x, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add);
   return (int)cudaGetLastError();
 }
 int conv_in_launch(cudaStream_t st, const __half* x, int B, int Cin, int H, int W, const float* w, const float* bias,
@@ -258,6 +267,53 @@ int phase_split_launch(cudaStream_t st, const float* x, int B, int H, int W, int
   int grid = cdiv(total, 256);
   if (grid > 132 * 16) grid = 132 * 16;
   phase_split_kernel<<<grid, 256, 0, st>>>(x, B, H, W, C, y);
+  return (int)cudaGetLastError();
+}
+
+// ControlNet hint encoder, between two convs: y = f16(silu(x)), NHWC; with `phase` the output is the stride-2 phase split of
+// phase_split_kernel (the next conv has stride 2), so no f32 copy and no separate split pass.
+__global__ void silu_f16_kernel(const float* __restrict__ x, int B, int H, int W, int C, int phase, __half* __restrict__ y) {
+  const int cv = C / 4;
+  const long total = (long)B * H * W * cv;
+  for (long idx = (long)blockIdx.x * blockDim.x + threadIdx.x; idx < total; idx += (long)gridDim.x * blockDim.x) {
+    const int c = (int)(idx % cv);
+    const long pix = idx / cv;
+    float4 v = *reinterpret_cast<const float4*>(x + pix * C + c * 4);
+    v.x = silu_f(v.x); v.y = silu_f(v.y); v.z = silu_f(v.z); v.w = silu_f(v.w);
+    size_t o = pix * C + c * 4;
+    if (phase) {
+      const int w = (int)(pix % W);
+      const int h = (int)((pix / W) % H);
+      const int b = (int)(pix / ((long)W * H));
+      const int ph = (h & 1) * 2 + (w & 1);
+      o = ((((size_t)ph * B + b) * (H / 2) + (h >> 1)) * (W / 2) + (w >> 1)) * C + c * 4;
+    }
+    *reinterpret_cast<uint2*>(y + o) = pack4h(v);
+  }
+}
+int silu_f16_launch(cudaStream_t st, const float* x, int B, int H, int W, int C, int phase, __half* y) {
+  if ((C & 3) || (phase && ((H & 1) || (W & 1)))) return 2005;
+  const long total = (long)B * H * W * (C / 4);
+  int grid = cdiv(total, 256);
+  if (grid > 132 * 16) grid = 132 * 16;
+  if (grid < 1) grid = 1;
+  silu_f16_kernel<<<grid, 256, 0, st>>>(x, B, H, W, C, phase, y);
+  return (int)cudaGetLastError();
+}
+
+// ControlNet scale folded into a zero conv: wo = f16(s * w), bo = s * b (s = 1 keeps the bits).
+__global__ void scale_weights_kernel(const __half* __restrict__ w, size_t nw, const float* __restrict__ b, int nb, float s,
+                                     __half* __restrict__ wo, float* __restrict__ bo) {
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nw; i += (size_t)gridDim.x * blockDim.x)
+    wo[i] = __float2half_rn(s * __half2float(w[i]));
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < (size_t)nb; i += (size_t)gridDim.x * blockDim.x)
+    bo[i] = s * b[i];
+}
+int scale_weights_launch(cudaStream_t st, const __half* w, size_t nw, const float* b, int nb, float s, __half* wo, float* bo) {
+  int grid = cdiv((long)nw, 256);
+  if (grid > 132 * 8) grid = 132 * 8;
+  if (grid < 1) grid = 1;
+  scale_weights_kernel<<<grid, 256, 0, st>>>(w, nw, b, nb, s, wo, bo);
   return (int)cudaGetLastError();
 }
 

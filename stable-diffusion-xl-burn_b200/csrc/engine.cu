@@ -88,19 +88,32 @@ struct Block {
 
 struct Plan;
 struct Sampler;
+struct ControlAttach;
 
-struct sdxl_unet {
+// Embeddings, first conv, input blocks and middle block: the part of the UNet a ControlNet copies.
+struct EncoderHalf {
   sdxl_ctx* ctx = nullptr;
   sdxl_unet_cfg cfg{};
   Arena warena;  // re-laid-out weights
-  // embeddings
   Lin t1, t2, l1, l2;      // time / label MLPs
   Lin temb_all;            // concatenated lin_embed of every ResBlock [sumC, 4mc], bias folded with conv_in bias
   float* conv0_w = nullptr;  // first conv [mc][3][3][4] f32
   float* conv0_b = nullptr;
-  std::vector<Block> in_blocks, out_blocks;
+  std::vector<Block> in_blocks;
   Res mid_res1, mid_res2;
   STrans mid_st;
+};
+
+struct sdxl_controlnet : EncoderHalf {
+  sdxl_controlnet_cfg ncfg{};
+  float* hint0_w = nullptr;  // first hint conv [c0][3][3][hint_in] f32 (CUDA-core kernel)
+  float* hint0_b = nullptr;
+  std::vector<Conv> hint;    // the other hint convs in order: c_k -> c_k, c_k -> c_k+1 (stride 2), ..., c_last -> mc
+  std::vector<Conv> zero;    // zero_convs/0..n-1 (one per skip tensor), then middle_block_out
+};
+
+struct sdxl_unet : EncoderHalf {
+  std::vector<Block> out_blocks;
   Norm norm_out;
   Conv conv_out;
   __half* conv_out_w2 = nullptr;   // [O, 2*Ktot] = [W | W]: head conv on the hi/lo-split activation
@@ -123,6 +136,24 @@ struct sdxl_unet {
   int* t_pinned = nullptr;
   int t_slot = 0;              // ring position in t_pinned (per model: independent contexts never share it)
   AdapterState lora;           // LoRA-able weight slots, backups of merged layers (sdxl_unet_set_adapters)
+  std::vector<std::unique_ptr<ControlAttach>> controls;   // sdxl_unet_set_controls, in call order
+  uint64_t controls_version = 0;
+};
+
+// One attached ControlNet: its scaled zero convs, the encoded hint and its hoisted conditioning.
+struct ControlAttach {
+  const sdxl_controlnet* net = nullptr;
+  float scale = 1.f;
+  int n_hint = 0, h = 0, w = 0;   // latent extent
+  Arena mem;                      // zero-conv copies f16(s*W) / s*b, hint_emb f32 NHWC [n_hint, h, w, mc]
+  std::vector<Lin> zero;
+  float* hint_emb = nullptr;
+  Arena cmem;                     // conditioning of the net: label MLP, cross-attention K/V
+  int condB = 0, n_ctx = 0;
+  float* lab1 = nullptr;
+  float* label_emb = nullptr;
+  std::vector<__half*> kv;
+  ~ControlAttach() { mem.release(); cmem.release(); }
 };
 
 
@@ -188,17 +219,35 @@ static STrans load_st(Loader& L, const std::string& path, int C, int ctx_dim, in
   return s;
 }
 
-// Builds every layer (in measure mode only sizes are accumulated).
-static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
-  sdxl_ctx* c = u->ctx;
+// 3x3 conv with few input channels for the CUDA-core first-conv kernel: OIHW f16 -> [O][kh][kw][I] f32, bias f32
+static int load_conv_f32(Loader& L, const std::string& path, int I, int O, float*& w, float*& b) {
+  sdxl_ctx* c = L.c;
+  Arena& A = *L.A;
+  const PackEntry* e = L.need(path + "/weight", 4);
+  if (!e) return L.err;
+  if ((int)e->shape[0] != O || (int)e->shape[1] != I || e->shape[2] != 3 || e->shape[3] != 3)
+    return fail(c, 4010, "%s/weight bad shape", path.c_str());
+  const size_t n = (size_t)O * 9 * I;
+  __half* tmp = A.get<__half>(n);
+  w = A.get<float>(n);
+  if (!tmp || !w) return fail(c, 4005, "weight arena exhausted");
+  if (!A.measure) {
+    int r = repack_conv_launch(c->stream, L.ptr(e), O, I, 3, 3, tmp, 9 * I, 0, I);
+    if (!r) r = cast_f16_to_f32_launch(c->stream, tmp, n, w);
+    if (r) return fail(c, r, "%s repack failed", path.c_str());
+  }
+  WSlot s;
+  s.base = w; s.conv = 1; s.f32 = 1; s.N = O; s.I = I; s.ks = 3; s.ld = 9 * I; s.Ipad = I;
+  L.record(path, s, n * sizeof(float));
+  b = L.vec_f32(path + "/bias", O);
+  return L.err;
+}
+
+// Time / label MLPs, first conv, input blocks and middle block (reference unet/mod.rs:116-248), for the UNet and for a ControlNet.
+static int load_encoder(Loader& L, EncoderHalf* u, std::vector<TembItem>& tembs, int& temb_total) {
   const sdxl_unet_cfg& g = u->cfg;
-  Loader L{u, c, &pv, &A, c->stream};
-  L.reg = &u->lora;
   const int mc = g.model_channels, ted = 4 * mc;
   u->in_blocks.clear();
-  u->out_blocks.clear();
-  std::vector<TembItem> tembs;
-  int temb_total = 0;
   auto n_head = [&](int ch) { return ch / g.n_head_channels; };
 
   u->t1 = L.linear("lin1_time_embed", mc, ted, true);
@@ -206,28 +255,7 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
   u->l1 = L.linear("lin1_label_embed", g.adm_in_channels, ted, true);
   u->l2 = L.linear("lin2_label_embed", ted, ted, true);
   if (L.err) return L.err;
-
-  // first conv: OIHW f16 -> [O][kh][kw][I] f32 (CUDA-core kernel)
-  {
-    const PackEntry* e = L.need("input_blocks/0/weight", 4);
-    if (!e) return L.err;
-    if ((int)e->shape[0] != mc || (int)e->shape[1] != g.in_channels || e->shape[2] != 3 || e->shape[3] != 3)
-      return fail(c, 4010, "input_blocks/0/weight bad shape");
-    const size_t n = (size_t)mc * 9 * g.in_channels;
-    __half* tmp = A.get<__half>(n);
-    u->conv0_w = A.get<float>(n);
-    if (!tmp || !u->conv0_w) return fail(c, 4005, "weight arena exhausted");
-    if (!A.measure) {
-      int r = repack_conv_launch(c->stream, L.ptr(e), mc, g.in_channels, 3, 3, tmp, 9 * g.in_channels, 0, g.in_channels);
-      if (!r) r = cast_f16_to_f32_launch(c->stream, tmp, n, u->conv0_w);
-      if (r) return fail(c, r, "conv0 repack failed");
-    }
-    WSlot s;
-    s.base = u->conv0_w; s.conv = 1; s.f32 = 1; s.N = mc; s.I = g.in_channels; s.ks = 3; s.ld = 9 * g.in_channels; s.Ipad = g.in_channels;
-    L.record("input_blocks/0", s, n * sizeof(float));
-    u->conv0_b = L.vec_f32("input_blocks/0/bias", mc);
-    if (L.err) return L.err;
-  }
+  if (int r = load_conv_f32(L, "input_blocks/0", g.in_channels, mc, u->conv0_w, u->conv0_b)) return r;
   {
     Block b0; b0.type = BT_CONV; b0.Cout = mc;
     u->in_blocks.push_back(b0);
@@ -268,9 +296,49 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
     u->mid_st = load_st(L, "middle_block/transformer", cm, g.context_dim, n_head(cm), g.transformer_depths[g.n_levels - 1]);
     u->mid_res2 = load_res(L, "middle_block/res2", cm, cm, ted, tembs, temb_total);
   }
-  if (L.err) return L.err;
+  return L.err;
+}
+
+// concatenated lin_embed matrix (one GEMV per forward for all ResBlocks); bias += conv_in bias
+static int load_temb_all(Loader& L, EncoderHalf* u, const std::vector<TembItem>& tembs, int temb_total) {
+  sdxl_ctx* c = L.c;
+  Arena& A = *L.A;
+  const int ted = 4 * u->cfg.model_channels;
+  Lin& T = u->temb_all;
+  T.K = ted; T.Kpad = Loader::pad64(ted); T.N = temb_total;
+  T.w = A.get<__half>((size_t)temb_total * T.Kpad);
+  T.b = A.get<float>(temb_total);
+  if (!T.w || !T.b) return fail(c, 4005, "weight arena exhausted");
+  int off = 0;
+  for (auto& it : tembs) {
+    if (L.lin_into(it.path, T.w, T.Kpad, off, ted, it.Cout, 0)) return L.err;
+    const PackEntry* e = L.need(it.path + "/bias", 1);
+    if (!e) return L.err;
+    if (!A.measure) {
+      int r = bias_to_f32_launch(c->stream, L.ptr(e), it.Cout, T.b + off, 0, 0);
+      // fold the conv_in bias: h = conv_in(..) + b_conv + lin_embed(..)   (unet/mod.rs:1086-1092)
+      if (!r) r = vec_add_f32_launch(c->stream, T.b + off, it.conv_bias, it.Cout);
+      if (r) return fail(c, r, "temb bias failed");
+    }
+    off += it.Cout;
+  }
+  return 0;
+}
+
+// Builds every layer (in measure mode only sizes are accumulated).
+static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
+  sdxl_ctx* c = u->ctx;
+  const sdxl_unet_cfg& g = u->cfg;
+  Loader L{u, c, &pv, &A, c->stream};
+  L.reg = &u->lora;
+  const int mc = g.model_channels, ted = 4 * mc;
+  u->out_blocks.clear();
+  std::vector<TembItem> tembs;
+  int temb_total = 0;
+  auto n_head = [&](int ch) { return ch / g.n_head_channels; };
+  if (int r = load_encoder(L, u, tembs, temb_total)) return r;
   // output blocks (reference unet/mod.rs:250-328)
-  idx = 0;
+  int idx = 0;
   for (int level = g.n_levels - 1; level >= 0 && !L.err; --level) {
     const int next_level = (level != g.n_levels - 1) ? level + 1 : level;
     const int cout = g.channel_mults[level] * mc;
@@ -311,28 +379,7 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
         CU(c, cudaMemcpy2DAsync(u->conv_out_w2 + (size_t)h2 * cv.Ktot, (size_t)2 * cv.Ktot * sizeof(__half), cv.w, (size_t)cv.Ktot * sizeof(__half),
                                 (size_t)cv.Ktot * sizeof(__half), (size_t)cv.O, cudaMemcpyDeviceToDevice, c->stream));
   }
-
-  // concatenated lin_embed matrix (one GEMV per forward for all ResBlocks); bias += conv_in bias
-  {
-    Lin& T = u->temb_all;
-    T.K = ted; T.Kpad = Loader::pad64(ted); T.N = temb_total;
-    T.w = A.get<__half>((size_t)temb_total * T.Kpad);
-    T.b = A.get<float>(temb_total);
-    if (!T.w || !T.b) return fail(c, 4005, "weight arena exhausted");
-    int off = 0;
-    for (auto& it : tembs) {
-      if (L.lin_into(it.path, T.w, T.Kpad, off, ted, it.Cout, 0)) return L.err;
-      const PackEntry* e = L.need(it.path + "/bias", 1);
-      if (!e) return L.err;
-      if (!A.measure) {
-        int r = bias_to_f32_launch(c->stream, L.ptr(e), it.Cout, T.b + off, 0, 0);
-        // fold the conv_in bias: h = conv_in(..) + b_conv + lin_embed(..)   (unet/mod.rs:1086-1092)
-        if (!r) r = vec_add_f32_launch(c->stream, T.b + off, it.conv_bias, it.Cout);
-        if (r) return fail(c, r, "temb bias failed");
-      }
-      off += it.Cout;
-    }
-  }
+  if (int r = load_temb_all(L, u, tembs, temb_total)) return r;
   // count transformer blocks (for the hoisted K/V buffers)
   int nt = 0;
   for (auto& b : u->in_blocks) nt += (int)b.st.blocks.size();
@@ -347,6 +394,41 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
 // ================================================================================================
 
 extern "C" void sdxl_unet_destroy(sdxl_unet* u);
+
+// Parses a weight pack, makes it device-resident for the call (host packs are uploaded to a temporary copy) and runs fn(pv);
+// the stream is synchronised before the copy is freed.
+template <typename Fn>
+static int with_device_pack(sdxl_ctx* c, const void* pack, size_t bytes, int pack_on_device, Fn fn) {
+  PackView pv;
+  std::vector<uint8_t> table;
+  int r = parse_pack(c, pack, bytes, pack_on_device, pv, table);
+  if (r) return r;
+  void* dev_pack = nullptr;
+  if (pack_on_device) {
+    pv.dev = (const uint8_t*)pack;
+  } else {
+    CU(c, cudaMalloc(&dev_pack, bytes));
+    cudaError_t e = cudaMemcpyAsync(dev_pack, pack, bytes, cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) { cudaFree(dev_pack); return fail(c, (int)e, "pack upload failed"); }
+    pv.dev = (const uint8_t*)dev_pack;
+  }
+  r = fn((const PackView&)pv);
+  cudaError_t se = cudaStreamSynchronize(c->stream);
+  if (dev_pack) cudaFree(dev_pack);
+  if (!r && se != cudaSuccess) r = fail(c, (int)se, "weight re-layout failed: %s", cudaGetErrorString(se));
+  return r;
+}
+
+// pass 1: measure, pass 2: build into the model's weight arena
+template <typename M>
+static int build_two_pass(M* m, const PackView& pv, int (*build)(M*, const PackView&, Arena&)) {
+  Arena meas;
+  meas.measure = true;
+  int r = build(m, pv, meas);
+  if (!r && m->warena.init(meas.off + (1 << 20))) r = fail(m->ctx, 4203, "cannot allocate %zu bytes for weights", meas.off);
+  if (!r) r = build(m, pv, m->warena);
+  return r;
+}
 
 static int unet_load_impl(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pack, size_t bytes, int pack_on_device, sdxl_unet** out);
 
@@ -424,53 +506,170 @@ static int unet_load_impl(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pac
   std::unique_ptr<sdxl_unet> u(new sdxl_unet());
   u->ctx = c;
   u->cfg = *cfg;
-  PackView pv;
-  std::vector<uint8_t> table;
-  int r = parse_pack(c, pack, bytes, pack_on_device, pv, table);
-  if (r) return r;
-  void* dev_pack = nullptr;
-  if (pack_on_device) {
-    pv.dev = (const uint8_t*)pack;
-  } else {
-    CU(c, cudaMalloc(&dev_pack, bytes));
-    cudaError_t e = cudaMemcpyAsync(dev_pack, pack, bytes, cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) { cudaFree(dev_pack); return fail(c, (int)e, "pack upload failed"); }
-    pv.dev = (const uint8_t*)dev_pack;
-  }
-  // pass 1: measure, pass 2: build
-  Arena meas;
-  meas.measure = true;
-  r = build_model(u.get(), pv, meas);
-  if (!r) {
-    if (u->warena.init(meas.off + (1 << 20))) r = fail(c, 4203, "cannot allocate %zu bytes for weights", meas.off);
-  }
-  if (!r) r = build_model(u.get(), pv, u->warena);
-  // alphas_cumprod: f16-stored in the reference's record (HalfPrecisionSettings), read as f64 (mod.rs:485-492)
-  if (!r) {
-    const PackEntry* e = pv.find("alphas_cumprod");
-    if (!e || e->ndim != 1 || e->dtype != 0) r = fail(c, 4204, "weight pack: missing f16 'alphas_cumprod'");
-    else {
+  int r = with_device_pack(c, pack, bytes, pack_on_device, [&](const PackView& pv) {
+    int r2 = build_two_pass(u.get(), pv, build_model);
+    // alphas_cumprod: f16-stored in the reference's record (HalfPrecisionSettings), read as f64 (mod.rs:485-492)
+    if (!r2) {
+      const PackEntry* e = pv.find("alphas_cumprod");
+      if (!e || e->ndim != 1 || e->dtype != 0) return fail(c, 4204, "weight pack: missing f16 'alphas_cumprod'");
       std::vector<uint16_t> raw(e->shape[0]);
       cudaError_t ce = cudaMemcpyAsync(raw.data(), pv.dev + e->offset, raw.size() * 2, cudaMemcpyDeviceToHost, c->stream);
       if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
-      if (ce != cudaSuccess) r = fail(c, (int)ce, "alphas download failed");
-      else {
-        u->alphas.resize(raw.size());
-        for (size_t i = 0; i < raw.size(); ++i) {
-          __half_raw hr;
-          hr.x = raw[i];
-          u->alphas[i] = (double)__half2float(__half(hr));
-        }
+      if (ce != cudaSuccess) return fail(c, (int)ce, "alphas download failed");
+      u->alphas.resize(raw.size());
+      for (size_t i = 0; i < raw.size(); ++i) {
+        __half_raw hr;
+        hr.x = raw[i];
+        u->alphas[i] = (double)__half2float(__half(hr));
       }
     }
-  }
-  cudaError_t se = cudaStreamSynchronize(c->stream);
-  if (dev_pack) cudaFree(dev_pack);
-  if (!r && se != cudaSuccess) r = fail(c, (int)se, "weight re-layout failed: %s", cudaGetErrorString(se));
+    return r2;
+  });
   if (r) return r;
   CU(c, cudaMalloc((void**)&u->t_dev, 64));
   CU(c, cudaMallocHost((void**)&u->t_pinned, 4096 * sizeof(int)));
   *out = u.release();
+  return 0;
+}
+
+// ================================================================================================
+// ControlNet load
+// ================================================================================================
+static int build_controlnet(sdxl_controlnet* n, const PackView& pv, Arena& A) {
+  const sdxl_unet_cfg& g = n->cfg;
+  const sdxl_controlnet_cfg& nc = n->ncfg;
+  Loader L{n, n->ctx, &pv, &A, n->ctx->stream};   // no LoRA registry: adapters on a ControlNet are not supported
+  std::vector<TembItem> tembs;
+  int temb_total = 0;
+  if (int r = load_encoder(L, n, tembs, temb_total)) return r;
+  if (int r = load_temb_all(L, n, tembs, temb_total)) return r;
+  // hint encoder, SGM's input_hint_block indices: 0 = conv(in -> c0); 2 + 4k = conv(c_k -> c_k), 4 + 4k = conv(c_k -> c_k+1, s2);
+  // 4n - 2 = conv(c_last -> mc)
+  const int* hc = nc.hint_block_channels;
+  const int nb = nc.n_hint_blocks;
+  if (int r = load_conv_f32(L, "input_hint_block/0", nc.hint_in_channels, hc[0], n->hint0_w, n->hint0_b)) return r;
+  n->hint.clear();
+  for (int k = 0; k + 1 < nb && !L.err; ++k) {
+    n->hint.push_back(L.conv("input_hint_block/" + std::to_string(2 + 4 * k), hc[k], hc[k], 3));
+    n->hint.push_back(L.conv("input_hint_block/" + std::to_string(4 + 4 * k), hc[k], hc[k + 1], 3));
+  }
+  n->hint.push_back(L.conv("input_hint_block/" + std::to_string(4 * nb - 2), hc[nb - 1], g.model_channels, 3));
+  // zero convs: one per skip tensor (the outputs of input_blocks/0, 1, ...), then middle_block_out
+  n->zero.clear();
+  for (size_t i = 0; i < n->in_blocks.size() && !L.err; ++i)
+    n->zero.push_back(L.conv("zero_convs/" + std::to_string(i), n->in_blocks[i].Cout, n->in_blocks[i].Cout, 1));
+  const int cm = g.channel_mults[g.n_levels - 1] * g.model_channels;
+  n->zero.push_back(L.conv("middle_block_out", cm, cm, 1));
+  return L.err;
+}
+
+extern "C" int sdxl_controlnet_load(sdxl_ctx* c, const sdxl_controlnet_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
+                                    sdxl_controlnet** out) {
+  if (!c || !cfg || !pack || !out) return fail(c, -1, "sdxl_controlnet_load: null argument");
+  *out = nullptr;
+  const sdxl_unet_cfg& g = cfg->unet;
+  if (g.n_head_channels != 64) return fail(c, 4200, "n_head_channels must be 64 (got %d)", g.n_head_channels);
+  if (g.n_levels < 1 || g.n_levels > SDXL_MAX_LEVELS) return fail(c, 4201, "bad n_levels");
+  if (g.in_channels > 8 || g.model_channels % 32) return fail(c, 4202, "unsupported channel config");
+  if (cfg->hint_in_channels < 1 || cfg->hint_in_channels > 8) return fail(c, 4700, "hint_in_channels must be in [1, 8] (got %d)", cfg->hint_in_channels);
+  if (cfg->n_hint_blocks != 4) return fail(c, 4701, "n_hint_blocks must be 4 (hint downscale 2^(n-1) = 8), got %d", cfg->n_hint_blocks);
+  for (int k = 0; k < cfg->n_hint_blocks; ++k)
+    if (cfg->hint_block_channels[k] < 8 || cfg->hint_block_channels[k] % 8)
+      return fail(c, 4702, "hint_block_channels[%d] = %d must be a positive multiple of 8", k, cfg->hint_block_channels[k]);
+  CU(c, cudaSetDevice(c->device));
+  std::unique_ptr<sdxl_controlnet> n(new sdxl_controlnet());
+  n->ctx = c;
+  n->cfg = g;
+  n->ncfg = *cfg;
+  int r = with_device_pack(c, pack, bytes, pack_on_device,
+                           [&](const PackView& pv) { return build_two_pass(n.get(), pv, build_controlnet); });
+  if (r) { n->warena.release(); return r; }
+  *out = n.release();
+  return 0;
+}
+
+extern "C" void sdxl_controlnet_destroy(sdxl_controlnet* n) {
+  if (!n) return;
+  cudaStreamSynchronize(n->ctx->stream);
+  n->warena.release();
+  delete n;
+}
+
+// 3x3 pad-1 conv of an NHWC f16 image on the implicit GEMM, stride 1 or 2 (stride 2: `a` is the phase split of the input,
+// [4][Bn][H/2][W/2][C], as written by silu_f16_launch / phase_split_launch). Output f32 NHWC at H x W (stride 1) or H/2 x W/2.
+static int conv3x3_direct(sdxl_ctx* c, const __half* a, int Bn, int H, int W, int C, const Conv& cv, int stride, float* out) {
+  IgemmParams p{};
+  const int Ho = H / stride, Wo = W / stride;
+  p.nseg = 0;
+  for (int kh = 0; kh < 3; ++kh)
+    for (int kw = 0; kw < 3; ++kw) {
+      if (stride == 2) {   // tap kh -> (phase, offset), as the UNet's Downsample
+        const int ph = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
+        p.seg[p.nseg++] = {0, (int16_t)((kw == 0) ? -1 : 0), (int16_t)((kh == 0) ? -1 : 0), (int16_t)((ph * 2 + pw) * Bn), cv.Ipad / 64};
+      } else {
+        p.seg[p.nseg++] = {0, (int16_t)(kw - 1), (int16_t)(kh - 1), 0, cv.Ipad / 64};
+      }
+    }
+  p.out = out; p.out_f32 = 1; p.ldo = cv.O;
+  p.bias = cv.b; p.bias_bstride = 0; p.res = nullptr; p.ldr = 0;
+  IgemmOperands o{a, stride == 2 ? 4 * Bn : Bn, Ho, Wo, C, C, nullptr, 0, 0, 0, 0, 0, cv.w, cv.O, cv.Ktot};
+  int r = igemm_configure(p, o, Wo, Ho, Bn, IGEMM_LINEAR, 0);
+  if (r) return fail(c, r, "igemm configuration failed (hint encoder, %d -> %d)", C, cv.O);
+  KL(c, igemm_launch(c->stream, p));
+  return 0;
+}
+
+// Hint encoder (SGM input_hint_block): hint f32 NCHW [n, in, H, W] (device) -> f32 NHWC [n, H/8, W/8, mc]. Queued on the ctx stream.
+static int embed_hint(sdxl_controlnet* net, int n, int H, int W, const float* hint, float* out) {
+  sdxl_ctx* c = net->ctx;
+  const sdxl_controlnet_cfg& nc = net->ncfg;
+  const int* hc = nc.hint_block_channels;
+  const int nb = nc.n_hint_blocks;
+  if (n < 1 || H < 8 || W < 8 || H % 8 || W % 8) return fail(c, 4710, "hint must be [n >= 1, %d, H, W] with H, W multiples of 8 (got n=%d, %dx%d)", nc.hint_in_channels, n, H, W);
+  size_t maxe = 0;
+  {
+    int h = H, w = W;
+    for (int k = 0; k < nb; ++k) { maxe = std::max(maxe, (size_t)n * h * w * hc[k]); h /= 2; w /= 2; }
+  }
+  TmpBufs T(c->stream);
+  float* a = (float*)T.get(maxe * sizeof(float));
+  __half* a16 = (__half*)T.get(maxe * sizeof(__half));
+  if (!a || !a16) return fail(c, 4711, "hint encoder: cannot allocate %zu bytes of scratch", maxe * 6);
+  KL(c, conv_in_launch_t(c->stream, hint, 1, n, n, nc.hint_in_channels, H, W, net->hint0_w, net->hint0_b, hc[0], a));
+  int h = H, w = W;
+  for (int k = 0; k + 1 < nb; ++k) {
+    KL(c, silu_f16_launch(c->stream, a, n, h, w, hc[k], 0, a16));
+    if (int r = conv3x3_direct(c, a16, n, h, w, hc[k], net->hint[2 * k], 1, a)) return r;
+    KL(c, silu_f16_launch(c->stream, a, n, h, w, hc[k], 1, a16));
+    if (int r = conv3x3_direct(c, a16, n, h, w, hc[k], net->hint[2 * k + 1], 2, a)) return r;
+    h /= 2; w /= 2;
+  }
+  KL(c, silu_f16_launch(c->stream, a, n, h, w, hc[nb - 1], 0, a16));
+  return conv3x3_direct(c, a16, n, h, w, hc[nb - 1], net->hint.back(), 1, out);
+}
+
+extern "C" int sdxl_controlnet_embed_hint(sdxl_controlnet* net, int n, int H, int W, const float* hint, int on_host, float* out) {
+  if (!net || !hint || !out) return -1;
+  sdxl_ctx* c = net->ctx;
+  CU(c, cudaSetDevice(c->device));
+  const int mc = net->cfg.model_channels, h = H / 8, w = W / 8;
+  TmpBufs T(c->stream);
+  const size_t in_bytes = (size_t)n * net->ncfg.hint_in_channels * H * W * sizeof(float), out_elems = (size_t)n * h * w * mc;
+  float* x = (float*)hint;
+  if (on_host) {
+    x = (float*)T.get(in_bytes);
+    if (!x) return fail(c, 4711, "embed_hint: allocation failed");
+    CU(c, cudaMemcpyAsync(x, hint, in_bytes, cudaMemcpyHostToDevice, c->stream));
+  }
+  float* e = (float*)T.get(out_elems * sizeof(float));
+  float* o = on_host ? (float*)T.get(out_elems * sizeof(float)) : out;
+  if (!e || !o) return fail(c, 4711, "embed_hint: allocation failed");
+  if (int r = embed_hint(net, n, H, W, x, e)) return r;
+  KL(c, nhwc_to_nchw_f32_launch(c->stream, e, n, h * w, mc, mc, o));
+  if (on_host) {
+    CU(c, cudaMemcpyAsync(out, o, out_elems * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+  }
   return 0;
 }
 
@@ -481,6 +680,83 @@ static int unet_load_impl(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pac
 struct UNetPlanBuilder : PlanBuilder {
   sdxl_unet* u = nullptr;
   int kv_index = 0;
+  const std::vector<__half*>* kvs = nullptr;   // hoisted cross-attention K/V of the model being planned (UNet or ControlNet)
+
+  struct Scratch { __half *gn1, *raw; float* h; __half *gn2, *a16; float* tok; __half *qkv, *ao, *q, *ff; };
+  struct Saved { float* p; int C, H, W; };
+
+  // Time / label MLPs (on the shared timestep embedding te), first conv, input blocks and middle block of UNet::forward
+  // (unet/mod.rs:458-482) with the weights of `e`; every block output is pushed to `saved`, the middle output is returned.
+  // hint (nullable): ControlNet hint embedding f32 NHWC [n_hint, h, w, mc] added to the first conv's output.
+  float* encoder(const EncoderHalf& e, const float* label_emb, const float* te, float* t1, float* semb, float* temb_all,
+                 const Scratch& s, const float* hint, int n_hint, const std::string& prefix, std::vector<Saved>& saved) {
+    const sdxl_unet_cfg& g = e.cfg;
+    const int mc = g.model_channels, ted = 4 * mc, temb_total = e.temb_all.N;
+    gemv(te, 0, 1, e.t1, nullptr, 0, 0, 1, t1, 0);
+    gemv(t1, 0, Bf, e.t2, label_emb, ted, 0, 1, semb, ted);
+    gemv(semb, ted, Bf, e.temb_all, nullptr, 0, 0, 0, temb_all, temb_total);
+    int H = P->h, W = P->w;
+    float* x = buf<float>((size_t)Bf * H * W * mc);
+    int Cx = mc;
+    if (!err) {
+      Op op{};
+      op.kind = OP_CONV_IN;
+      op.ci = {P->x_in, P->Bx, Bf, g.in_channels, H, W, e.conv0_w, e.conv0_b, mc, x, hint, n_hint};
+      P->ops.push_back(op);
+      P->flops += 2.0 * Bf * H * W * 9.0 * g.in_channels * mc;
+    }
+    saved.push_back({x, Cx, H, W});
+    for (size_t i = 1; i < e.in_blocks.size() && !err; ++i) {
+      const Block& b = e.in_blocks[i];
+      begin_block(prefix + "input_blocks/" + std::to_string(i));
+      if (b.type == BT_RES || b.type == BT_REST) {
+        x = resblock(b.res, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s.gn1, s.raw, s.h, s.gn2);
+        Cx = b.res.Cout;
+        if (b.type == BT_REST) x = strans(b.st, x, H, W, s.a16, s.tok, s.qkv, s.ao, s.q, s.ff);
+      } else if (b.type == BT_DOWN) {
+        // 3x3 stride 2 pad 1 (unet/mod.rs:760-774) on phase-split input: tap kh -> (phase, offset)
+        __half* ph = buf<__half>((size_t)Bf * H * W * Cx);
+        Op op{};
+        op.kind = OP_PHASE;
+        op.rs = {x, Bf, H, W, Cx, ph};
+        if (!err) P->ops.push_back(op);
+        const int H2 = H / 2, W2 = W / 2;
+        ActView a{ph, 4 * Bf, H2, W2, Cx};
+        std::vector<IgemmSeg> segs;
+        for (int kh = 0; kh < 3; ++kh)
+          for (int kw = 0; kw < 3; ++kw) {
+            const int phh = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
+            const int dh = (kh == 0) ? -1 : 0, dw = (kw == 0) ? -1 : 0;
+            segs.push_back({0, (int16_t)dw, (int16_t)dh, (int16_t)((phh * 2 + pw) * Bf), b.conv.Ipad / 64});
+          }
+        float* y = buf<float>((size_t)Bf * H2 * W2 * Cx);
+        igemm(a, nullptr, segs, b.conv.w, b.conv.O, b.conv.Ktot, H2, W2, Bf, IGEMM_LINEAR, 0, y, 1, b.conv.O, b.conv.b, 0, nullptr, 0);
+        add_flops(2.0 * Bf * H2 * W2 * 9.0 * Cx * b.conv.O);
+        x = y; H = H2; W = W2;
+      }
+      end_block();
+      saved.push_back({x, Cx, H, W});
+    }
+    // --- middle
+    begin_block(prefix + "middle_block");
+    x = resblock(e.mid_res1, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s.gn1, s.raw, s.h, s.gn2);
+    x = strans(e.mid_st, x, H, W, s.a16, s.tok, s.qkv, s.ao, s.q, s.ff);
+    x = resblock(e.mid_res2, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s.gn1, s.raw, s.h, s.gn2);
+    end_block();
+    return x;
+  }
+
+  // ControlNet injection: dst += conv1x1(src) with the scaled zero conv L (f16 operand of src in `a16`, residual add in place)
+  void zero_conv(const Saved& src, const Saved& dst, const Lin& L, __half* a16) {
+    if (err) return;
+    if (src.C != dst.C || src.H != dst.H || src.W != dst.W || L.K != src.C) { err = fail(c, 5006, "control residual shape mismatch"); return; }
+    const size_t n = (size_t)Bf * src.H * src.W * src.C;
+    Op op{};
+    op.kind = OP_CAST16;
+    op.cs = {src.p, n, a16};
+    P->ops.push_back(op);
+    linear(a16, Bf * src.H * src.W, L, IGEMM_LINEAR, dst.p, 1, L.N, dst.p, L.N);
+  }
 
   // ---- ResBlock (reference unet/mod.rs:1082-1106) ----
   float* resblock(const Res& r, const float* xa, int Ca, const float* xb, int Cb, int H, int W, const float* temb_all,
@@ -519,7 +795,7 @@ struct UNetPlanBuilder : PlanBuilder {
       // x = x + attn2(norm2(x), context)   (K/V hoisted to set_conditioning)
       ln(s_tok, b.n2, M, s_a16);
       linear(s_a16, M, b.q2, IGEMM_LINEAR, s_q, 0, C, nullptr, 0);
-      const __half* kvp = A->measure ? nullptr : u->kv[kv_index];
+      const __half* kvp = A->measure ? nullptr : (*kvs)[kv_index];
       attn(s_q, C, 0, kvp, 2 * C, 0, C, T, u->n_ctx, s.n_head, s_ao, C, sl2e);
       P->flops += 2.0 * Bf * u->n_ctx * (double)b.kv2.K * b.kv2.N;  // hoisted K/V projections (algorithmic work)
       kv_index++;
@@ -621,6 +897,7 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
   __half* s_q = B.buf<__half>(Bf * max_tokC);
   __half* s_ff = B.buf<__half>(Bf * max_tokC * 4);
   if (B.err) return B.err;
+  const UNetPlanBuilder::Scratch scr{s_gn1, s_raw, s_h, s_gn2, s_a16, s_tok, s_qkv, s_ao, s_q, s_ff};
 
   // --- embeddings (unet/mod.rs:458-468): emb = time_mlp(temb(t)) + label_emb; only SiLU(emb) is consumed
   {
@@ -629,61 +906,34 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
     op.te = {u->t_dev, 1, mc, te};
     P->ops.push_back(op);
   }
-  B.gemv(te, 0, 1, u->t1, nullptr, 0, 0, 1, t1, 0);
-  B.gemv(t1, 0, Bf, u->t2, u->label_emb, ted, 0, 1, semb, ted);
-  B.gemv(semb, ted, Bf, u->temb_all, nullptr, 0, 0, 0, temb_all, temb_total);
-
-  // --- input blocks
-  struct Saved { float* p; int C, H, W; };
+  // --- embeddings, input blocks, middle
+  using Saved = UNetPlanBuilder::Saved;
   std::vector<Saved> saved;
-  int H = P->h, W = P->w;
-  float* x = B.buf<float>((size_t)Bf * H * W * mc);
-  int Cx = mc;
-  {
-    Op op{};
-    op.kind = OP_CONV_IN;
-    op.ci = {P->x_in, P->Bx, Bf, g.in_channels, H, W, u->conv0_w, u->conv0_b, mc, x};
-    P->ops.push_back(op);
-    P->flops += 2.0 * Bf * H * W * 9.0 * g.in_channels * mc;
-  }
-  saved.push_back({x, Cx, H, W});
-  for (size_t i = 1; i < u->in_blocks.size() && !B.err; ++i) {
-    const Block& b = u->in_blocks[i];
-    B.begin_block("input_blocks/" + std::to_string(i));
-    if (b.type == BT_RES || b.type == BT_REST) {
-      x = B.resblock(b.res, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s_gn1, s_raw, s_h, s_gn2);
-      Cx = b.res.Cout;
-      if (b.type == BT_REST) x = B.strans(b.st, x, H, W, s_a16, s_tok, s_qkv, s_ao, s_q, s_ff);
-    } else if (b.type == BT_DOWN) {
-      // 3x3 stride 2 pad 1 (unet/mod.rs:760-774) on phase-split input: tap kh -> (phase, offset)
-      __half* ph = B.buf<__half>((size_t)Bf * H * W * Cx);
-      Op op{};
-      op.kind = OP_PHASE;
-      op.rs = {x, Bf, H, W, Cx, ph};
-      P->ops.push_back(op);
-      const int H2 = H / 2, W2 = W / 2;
-      ActView a{ph, 4 * Bf, H2, W2, Cx};
-      std::vector<IgemmSeg> segs;
-      for (int kh = 0; kh < 3; ++kh)
-        for (int kw = 0; kw < 3; ++kw) {
-          const int phh = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
-          const int dh = (kh == 0) ? -1 : 0, dw = (kw == 0) ? -1 : 0;
-          segs.push_back({0, (int16_t)dw, (int16_t)dh, (int16_t)((phh * 2 + pw) * Bf), b.conv.Ipad / 64});
-        }
-      float* y = B.buf<float>((size_t)Bf * H2 * W2 * Cx);
-      B.igemm(a, nullptr, segs, b.conv.w, b.conv.O, b.conv.Ktot, H2, W2, Bf, IGEMM_LINEAR, 0, y, 1, b.conv.O, b.conv.b, 0, nullptr, 0);
-      B.add_flops(2.0 * Bf * H2 * W2 * 9.0 * Cx * b.conv.O);
-      x = y; H = H2; W = W2;
-    }
+  B.kvs = &u->kv;
+  float* x = B.encoder(*u, u->label_emb, te, t1, semb, temb_all, scr, nullptr, 1, "", saved);
+  int H = saved.back().H, W = saved.back().W, Cx = saved.back().C;
+  // --- ControlNets (DESIGN.md §8): each runs its own encoder on the same inputs, then skip_i += s * zero_conv_i(h_i) and
+  // mid += s * middle_block_out(mid_c), in attachment order. The UNet's own encoder above is untouched.
+  for (size_t k = 0; k < u->controls.size() && !B.err; ++k) {
+    const ControlAttach& a = *u->controls[k];
+    const EncoderHalf& e = *a.net;
+    const std::string prefix = "control" + std::to_string(k) + "/";
+    const int kv_unet = B.kv_index;
+    B.kvs = &a.kv;
+    B.kv_index = 0;
+    float* ct1 = B.buf<float>(ted);
+    float* csemb = B.buf<float>((size_t)Bf * ted);
+    float* ctemb = B.buf<float>((size_t)Bf * e.temb_all.N);
+    std::vector<Saved> cs;
+    float* cmid = B.encoder(e, a.label_emb, te, ct1, csemb, ctemb, scr, a.hint_emb, a.n_hint, prefix, cs);
+    B.kvs = &u->kv;
+    B.kv_index = kv_unet;
+    if (cs.size() != saved.size() || a.zero.size() != saved.size() + 1) return fail(c, 5006, "control %zu: skip count mismatch", k);
+    B.begin_block(prefix + "zero_convs");
+    for (size_t i = 0; i < saved.size(); ++i) B.zero_conv(cs[i], saved[i], a.zero[i], s_raw);
+    B.zero_conv({cmid, Cx, H, W}, {x, Cx, H, W}, a.zero.back(), s_raw);
     B.end_block();
-    saved.push_back({x, Cx, H, W});
   }
-  // --- middle
-  B.begin_block("middle_block");
-  x = B.resblock(u->mid_res1, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s_gn1, s_raw, s_h, s_gn2);
-  x = B.strans(u->mid_st, x, H, W, s_a16, s_tok, s_qkv, s_ao, s_q, s_ff);
-  x = B.resblock(u->mid_res2, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s_gn1, s_raw, s_h, s_gn2);
-  B.end_block();
   // --- output blocks: cat([x, saved.pop()], channel) is never materialised (GN + skip conv read both)
   for (size_t i = 0; i < u->out_blocks.size() && !B.err; ++i) {
     const Block& b = u->out_blocks[i];
@@ -727,12 +977,19 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
 static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
   sdxl_ctx* c = u->ctx;
   if (u->condB != Bf) return fail(c, 5010, "conditioning is set for batch %d but forward batch is %d (call sdxl_unet_set_conditioning first)", u->condB, Bf);
-  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan->cond_version == u->cond_version)
+  for (size_t k = 0; k < u->controls.size(); ++k) {
+    const ControlAttach& a = *u->controls[k];
+    if (a.h != h || a.w != w)
+      return fail(c, 5012, "control %zu: its hint is %dx%d pixels (latent %dx%d) but the latent is %dx%d", k, 8 * a.h, 8 * a.w, a.h, a.w, h, w);
+    if (Bf % a.n_hint) return fail(c, 5013, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bf, a.n_hint);
+  }
+  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan->cond_version == u->cond_version &&
+      u->plan->controls_version == u->controls_version)
     return 0;
   CU(c, cudaStreamSynchronize(c->stream));
   u->plan.reset(new Plan());
   Plan* P = u->plan.get();
-  P->Bf = Bf; P->Bx = Bx; P->h = h; P->w = w; P->cond_version = u->cond_version;
+  P->Bf = Bf; P->Bx = Bx; P->h = h; P->w = w; P->cond_version = u->cond_version; P->controls_version = u->controls_version;
   Arena meas;
   meas.measure = true;
   int r = build_plan_ops(u, P, &meas);
@@ -757,6 +1014,40 @@ static int set_t(sdxl_unet* u, int t) {
 // conditioning (step-invariant work hoisted out of UNet::forward)
 // ================================================================================================
 static int hoist_conditioning(sdxl_unet* u);
+
+// transformer blocks in execution order (one hoisted K/V buffer each)
+static std::vector<const TBlock*> encoder_tblocks(const EncoderHalf& e) {
+  std::vector<const TBlock*> tbs;
+  for (auto& b : e.in_blocks) for (auto& t : b.st.blocks) tbs.push_back(&t);
+  for (auto& t : e.mid_st.blocks) tbs.push_back(&t);
+  return tbs;
+}
+static std::vector<const TBlock*> unet_tblocks(const sdxl_unet* u) {
+  std::vector<const TBlock*> tbs = encoder_tblocks(*u);
+  for (auto& b : u->out_blocks) for (auto& t : b.st.blocks) tbs.push_back(&t);
+  return tbs;
+}
+
+// (Re)allocates a control's conditioning buffers for the UNet's current conditioning batch and context length.
+static int control_cond_alloc(sdxl_unet* u, ControlAttach& a) {
+  if (a.condB == u->condB && a.n_ctx == u->n_ctx) return 0;
+  const int B = u->condB, n_ctx = u->n_ctx, ted = 4 * u->cfg.model_channels;
+  const std::vector<const TBlock*> tbs = encoder_tblocks(*a.net);
+  size_t need = 0;
+  auto al = [&](size_t b) { need = ((need + 1023) & ~size_t(1023)) + b; };
+  al((size_t)B * ted * 4);
+  al((size_t)B * ted * 4);
+  for (auto* t : tbs) al((size_t)B * n_ctx * t->kv2.N * 2);
+  if (a.cmem.init(need + (1 << 16))) return fail(u->ctx, 5102, "cannot allocate ControlNet conditioning buffers");
+  a.lab1 = a.cmem.get<float>((size_t)B * ted);
+  a.label_emb = a.cmem.get<float>((size_t)B * ted);
+  a.kv.clear();
+  for (auto* t : tbs) a.kv.push_back(a.cmem.get<__half>((size_t)B * n_ctx * t->kv2.N));
+  a.condB = B;
+  a.n_ctx = n_ctx;
+  return 0;
+}
+
 static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* context_dev, const __half* y_dev) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
@@ -765,11 +1056,7 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
   if (u->condB != B || u->n_ctx != n_ctx) {
     CU(c, cudaStreamSynchronize(c->stream));
     u->plan.reset();
-    // collect transformer blocks
-    std::vector<const TBlock*> tbs;
-    for (auto& b : u->in_blocks) for (auto& t : b.st.blocks) tbs.push_back(&t);
-    for (auto& t : u->mid_st.blocks) tbs.push_back(&t);
-    for (auto& b : u->out_blocks) for (auto& t : b.st.blocks) tbs.push_back(&t);
+    const std::vector<const TBlock*> tbs = unet_tblocks(u);
     u->ctx_pitch = (g.context_dim + 7) / 8 * 8;
     size_t need = 0;
     auto al = [&](size_t b) { need = ((need + 1023) & ~size_t(1023)) + b; };
@@ -792,6 +1079,8 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
     u->condB = B;
     u->n_ctx = n_ctx;
     CU(c, cudaMemsetAsync(u->ctx16, 0, (size_t)B * n_ctx * u->ctx_pitch * 2, c->stream));
+    for (auto& a : u->controls)
+      if (int r = control_cond_alloc(u, *a)) return r;
   }
   u->cond_version++;
   if (u->plan) u->plan->cond_version = u->cond_version;  // buffers unchanged: plan stays valid
@@ -801,38 +1090,41 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
   return hoist_conditioning(u);
 }
 
-// The step-invariant projections of the retained conditioning (ctx16, y32) under the current weights.
-static int hoist_conditioning(sdxl_unet* u) {
+// label_emb = lin2(SiLU(lin1(y))) (unet/mod.rs:464-466) and the K/V projections of the context for every cross-attention
+// (unet/mod.rs:1010-1011) with the weights of `e`, from the UNet's retained conditioning.
+static int hoist_model(sdxl_unet* u, const EncoderHalf& e, const std::vector<const TBlock*>& tbs, float* lab1, float* label_emb,
+                       const std::vector<__half*>& kv) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   const int ted = 4 * g.model_channels, B = u->condB, n_ctx = u->n_ctx;
-  // label_emb = lin2(SiLU(lin1(y)))   (unet/mod.rs:464-466)
   for (int b0 = 0; b0 < B; b0 += 8) {
     const int nb = B - b0 < 8 ? B - b0 : 8;
-    KL(c, gemv_launch(c->stream, u->y32 + (size_t)b0 * g.adm_in_channels, g.adm_in_channels, nb, g.adm_in_channels, u->l1.w,
-                      u->l1.Kpad, u->l1.b, nullptr, 0, ted, 0, 1, u->lab1 + (size_t)b0 * ted, ted));
-    KL(c, gemv_launch(c->stream, u->lab1 + (size_t)b0 * ted, ted, nb, u->l2.K, u->l2.w, u->l2.Kpad, u->l2.b, nullptr, 0, ted, 0, 0,
-                      u->label_emb + (size_t)b0 * ted, ted));
+    KL(c, gemv_launch(c->stream, u->y32 + (size_t)b0 * g.adm_in_channels, g.adm_in_channels, nb, g.adm_in_channels, e.l1.w,
+                      e.l1.Kpad, e.l1.b, nullptr, 0, ted, 0, 1, lab1 + (size_t)b0 * ted, ted));
+    KL(c, gemv_launch(c->stream, lab1 + (size_t)b0 * ted, ted, nb, e.l2.K, e.l2.w, e.l2.Kpad, e.l2.b, nullptr, 0, ted, 0, 0,
+                      label_emb + (size_t)b0 * ted, ted));
   }
-  // K/V projections of the context for every cross-attention (unet/mod.rs:1010-1011)
-  {
-    std::vector<const TBlock*> tbs;
-    for (auto& b : u->in_blocks) for (auto& t : b.st.blocks) tbs.push_back(&t);
-    for (auto& t : u->mid_st.blocks) tbs.push_back(&t);
-    for (auto& b : u->out_blocks) for (auto& t : b.st.blocks) tbs.push_back(&t);
-    const int M = B * n_ctx;
-    for (size_t i = 0; i < tbs.size(); ++i) {
-      const Lin& L = tbs[i]->kv2;
-      IgemmParams p{};
-      p.nseg = 1;
-      p.seg[0] = {0, 0, 0, 0, L.Kpad / 64};
-      p.out = u->kv[i]; p.out_f32 = 0; p.ldo = L.N;
-      IgemmOperands o{u->ctx16, 1, 1, M, g.context_dim, u->ctx_pitch, nullptr, 0, 0, 0, 0, 0, L.w, L.N, L.Kpad};
-      int r = igemm_configure(p, o, M, 1, 1, IGEMM_LINEAR, 0);
-      if (r) return fail(c, r, "igemm configuration failed (kv projection)");
-      KL(c, igemm_launch(c->stream, p));
-    }
+  const int M = B * n_ctx;
+  for (size_t i = 0; i < tbs.size(); ++i) {
+    const Lin& L = tbs[i]->kv2;
+    IgemmParams p{};
+    p.nseg = 1;
+    p.seg[0] = {0, 0, 0, 0, L.Kpad / 64};
+    p.out = kv[i]; p.out_f32 = 0; p.ldo = L.N;
+    IgemmOperands o{u->ctx16, 1, 1, M, g.context_dim, u->ctx_pitch, nullptr, 0, 0, 0, 0, 0, L.w, L.N, L.Kpad};
+    int r = igemm_configure(p, o, M, 1, 1, IGEMM_LINEAR, 0);
+    if (r) return fail(c, r, "igemm configuration failed (kv projection)");
+    KL(c, igemm_launch(c->stream, p));
   }
+  return 0;
+}
+
+// The step-invariant projections of the retained conditioning (ctx16, y32) under the current weights, for the UNet and every
+// attached ControlNet.
+static int hoist_conditioning(sdxl_unet* u) {
+  if (int r = hoist_model(u, *u, unet_tblocks(u), u->lab1, u->label_emb, u->kv)) return r;
+  for (auto& a : u->controls)
+    if (int r = hoist_model(u, *a->net, encoder_tblocks(*a->net), a->lab1, a->label_emb, a->kv)) return r;
   return 0;
 }
 
@@ -840,6 +1132,107 @@ extern "C" int sdxl_unet_set_conditioning(sdxl_unet* u, int B, int n_ctx, const 
   if (!u || !context || !y) return -1;
   CU(u->ctx, cudaSetDevice(u->ctx->device));
   return set_conditioning_dev(u, B, n_ctx, (const __half*)context, (const __half*)y);
+}
+
+// ================================================================================================
+// ControlNet attachment (include/sdxl_b200.h: sdxl_unet_set_controls)
+// ================================================================================================
+// Writes the per-attachment buffers that depend on scale and hint values: f16(s*W) / s*b of every zero conv, and hint_emb.
+static int control_write(sdxl_ctx* c, ControlAttach& a, const sdxl_control& ctl) {
+  const sdxl_controlnet* n = a.net;
+  for (size_t i = 0; i < n->zero.size(); ++i) {
+    const Conv& z = n->zero[i];
+    KL(c, scale_weights_launch(c->stream, z.w, (size_t)z.O * z.Ktot, z.b, z.O, ctl.scale, a.zero[i].w, a.zero[i].b));
+  }
+  a.scale = ctl.scale;
+  TmpBufs T(c->stream);
+  const float* hint = ctl.hint;
+  if (ctl.hint_on_host) {
+    const size_t bytes = (size_t)ctl.n_hint * n->ncfg.hint_in_channels * ctl.height * ctl.width * sizeof(float);
+    float* d = (float*)T.get(bytes);
+    if (!d) return fail(c, 4720, "set_controls: cannot allocate %zu bytes for the hint", bytes);
+    CU(c, cudaMemcpyAsync(d, ctl.hint, bytes, cudaMemcpyHostToDevice, c->stream));
+    hint = d;
+  }
+  int r = embed_hint(const_cast<sdxl_controlnet*>(n), ctl.n_hint, ctl.height, ctl.width, hint, a.hint_emb);
+  if (!r && ctl.hint_on_host) CU(c, cudaStreamSynchronize(c->stream));   // the caller may reuse its host memory
+  return r;
+}
+
+extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* ctl) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  // validate everything first: on failure the attached set is unchanged
+  if (n < 0 || n > SDXL_MAX_CONTROLS) return fail(c, 4730, "set_controls: n = %d outside [0, %d]", n, SDXL_MAX_CONTROLS);
+  if (n > 0 && !ctl) return fail(c, 4731, "set_controls: null control array");
+  const sdxl_unet_cfg& g = u->cfg;
+  for (int k = 0; k < n; ++k) {
+    const sdxl_controlnet* net = ctl[k].net;
+    if (!net) return fail(c, 4732, "set_controls: control %d has a null net", k);
+    if (net->ctx != c) return fail(c, 4733, "set_controls: control %d: the net was created on another sdxl_ctx", k);
+    const sdxl_unet_cfg& h = net->cfg;
+    const char* field = nullptr;
+    if (h.model_channels != g.model_channels) field = "model_channels";
+    else if (h.n_levels != g.n_levels) field = "n_levels";
+    else if (h.in_channels != g.in_channels) field = "in_channels";
+    else if (h.context_dim != g.context_dim) field = "context_dim";
+    else if (h.adm_in_channels != g.adm_in_channels) field = "adm_in_channels";
+    else if (h.n_head_channels != g.n_head_channels) field = "n_head_channels";
+    for (int l = 0; l < g.n_levels && !field; ++l) {
+      if (h.channel_mults[l] != g.channel_mults[l]) field = "channel_mults";
+      else if (h.transformer_depths[l] != g.transformer_depths[l]) field = "transformer_depths";
+    }
+    if (field) return fail(c, 4734, "set_controls: control %d: cfg field '%s' differs from the UNet's", k, field);
+    if (ctl[k].n_hint < 1) return fail(c, 4735, "set_controls: control %d: n_hint = %d must be >= 1", k, ctl[k].n_hint);
+    if (!ctl[k].hint) return fail(c, 4736, "set_controls: control %d: null hint", k);
+    if (ctl[k].height < 8 || ctl[k].width < 8 || ctl[k].height % 8 || ctl[k].width % 8)
+      return fail(c, 4737, "set_controls: control %d: hint size %dx%d must be a positive multiple of 8", k, ctl[k].height, ctl[k].width);
+    if (!isfinite(ctl[k].scale)) return fail(c, 4738, "set_controls: control %d: scale is not finite", k);
+  }
+  // same nets, n_hint and sizes: only scales and hint values change, the launch plan stays valid
+  bool in_place = (size_t)n == u->controls.size() && n > 0;
+  for (int k = 0; k < n && in_place; ++k) {
+    const ControlAttach& a = *u->controls[k];
+    in_place = a.net == ctl[k].net && a.n_hint == ctl[k].n_hint && a.h == ctl[k].height / 8 && a.w == ctl[k].width / 8;
+  }
+  if (in_place) {   // not staged: a runtime failure of control k leaves 0..k-1 rewritten (documented in include/sdxl_b200.h)
+    for (int k = 0; k < n; ++k)
+      if (int r = control_write(c, *u->controls[k], ctl[k])) return r;
+    return 0;
+  }
+  std::vector<std::unique_ptr<ControlAttach>> fresh;
+  for (int k = 0; k < n; ++k) {
+    std::unique_ptr<ControlAttach> a(new ControlAttach());
+    const sdxl_controlnet* net = ctl[k].net;
+    a->net = net;
+    a->n_hint = ctl[k].n_hint;
+    a->h = ctl[k].height / 8;
+    a->w = ctl[k].width / 8;
+    size_t need = (size_t)a->n_hint * a->h * a->w * g.model_channels * sizeof(float) + 1024;
+    for (const Conv& z : net->zero) need += (size_t)z.O * z.Ktot * sizeof(__half) + z.O * sizeof(float) + 2048;
+    if (a->mem.init(need)) return fail(c, 4739, "set_controls: cannot allocate %zu bytes for control %d", need, k);
+    for (const Conv& z : net->zero) {
+      Lin L;
+      L.K = z.I; L.Kpad = z.Ktot; L.N = z.O;
+      L.w = a->mem.get<__half>((size_t)z.O * z.Ktot);
+      L.b = a->mem.get<float>(z.O);
+      a->zero.push_back(L);
+    }
+    a->hint_emb = a->mem.get<float>((size_t)a->n_hint * a->h * a->w * g.model_channels);
+    if (u->condB > 0)
+      if (int r = control_cond_alloc(u, *a)) return r;
+    if (int r = control_write(c, *a, ctl[k])) return r;
+    fresh.push_back(std::move(a));
+  }
+  CU(c, cudaStreamSynchronize(c->stream));   // the old plan and attachments may still be in flight
+  u->plan.reset();
+  u->controls = std::move(fresh);
+  u->controls_version++;
+  if (u->condB > 0)
+    for (auto& a : u->controls)
+      if (int r = hoist_model(u, *a->net, encoder_tblocks(*a->net), a->lab1, a->label_emb, a->kv)) return r;
+  return 0;
 }
 
 // ================================================================================================
@@ -951,6 +1344,12 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
   const sdxl_half* y_u = g.is_refiner ? cond->unconditional_channel_context_refiner : cond->unconditional_channel_context;
   if (!ctx_c || !y_c || (nfwd == 2 && (!ctx_u || !y_u))) return fail(c, 5201, "conditioning tensors for this model are null");
   if (Bimg < 1 || h < 1 || w < 1) return fail(c, 5202, "bad conditioning batch/resolution");
+  for (size_t k = 0; k < u->controls.size(); ++k) {   // rows [cond | uncond] of image b both use hint b % n_hint
+    const ControlAttach& a = *u->controls[k];
+    if (Bimg % a.n_hint) return fail(c, 5204, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bimg, a.n_hint);
+    if (a.h != h || a.w != w)
+      return fail(c, 5205, "control %zu: its hint is %dx%d pixels but the resolution is %dx%d", k, 8 * a.h, 8 * a.w, 8 * h, 8 * w);
+  }
   Sampler* S = u->sampler.get();
   const size_t lat = (size_t)Bimg * g.in_channels * h * w;
   if (n_ctx < 1) return fail(c, 5202, "bad conditioning context length");

@@ -193,9 +193,14 @@ int timestep_embedding_launch(cudaStream_t st, const int* t_dev, int nt, int dim
 // First conv: x NCHW f16 [B,Cin,H,W] (Cin<=8) -> NHWC f32 [B,H,W,Cout], 3x3 pad 1. w: [Cout][3][3][Cin] f32.
 int conv_in_launch(cudaStream_t st, const __half* x, int B, int Cin, int H, int W, const float* w,
                    const float* bias, int Cout, float* y);
-// general form: x f16 or f32 NCHW with Bx images; output batch b reads image b % Bx.
+// general form: x f16 or f32 NCHW with Bx images; output batch b reads image b % Bx. add (nullable): f32 NHWC [n_add,H,W,Cout]
+// added to the output at batch b % n_add (a ControlNet's hint embedding).
 int conv_in_launch_t(cudaStream_t st, const void* x, int x_f32, int Bx, int B, int Cin, int H, int W,
-                     const float* w, const float* bias, int Cout, float* y);
+                     const float* w, const float* bias, int Cout, float* y, const float* add = nullptr, int n_add = 1);
+// y = f16(silu(x)) of NHWC f32 [B,H,W,C]; phase != 0: written as the stride-2 phase split of phase_split_launch.
+int silu_f16_launch(cudaStream_t st, const float* x, int B, int H, int W, int C, int phase, __half* y);
+// wo[i] = f16(s * w[i]) (i < nw), bo[i] = s * b[i] (i < nb)
+int scale_weights_launch(cudaStream_t st, const __half* w, size_t nw, const float* b, int nb, float s, __half* wo, float* bo);
 // Nearest-2x upsample of NHWC: f32 [B,H,W,C] -> f16 [B,2H,2W,C] (reference unet/mod.rs:742-751).
 int upsample2x_launch(cudaStream_t st, const float* x, int B, int H, int W, int C, __half* y);
 // Stride-2 phase split: f32 [B,H,W,C] -> f16 [4(phase=ph*2+pw), B, H/2, W/2, C]; phase image

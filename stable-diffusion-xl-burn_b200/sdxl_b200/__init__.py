@@ -1,9 +1,12 @@
 """sdxl_b200 — host-side mirror of the reference's diffusion sampling surface over libsdxl_b200.so."""
 from .config import SDXL_BASE, SDXL_REFINER, TINY, TINY_REFINER, SDXL_VAE, TINY_VAE, SDXL_CLIP_L, SDXL_OPEN_CLIP_G, TINY_CLIP, TINY_OPEN_CLIP, ClipConfig, UNetConfig, VaeConfig, block_program  # noqa: F401
+from .config import SDXL_CONTROLNET, TINY_CONTROLNET, ControlNetConfig  # noqa: F401
 from .weights import alphas_cumprod, build_pack, n_params, synth_weights, unet_tensor_specs, vae_decoder_tensor_specs, vae_encoder_tensor_specs, vae_tensor_specs, clip_tensor_specs  # noqa: F401
+from .weights import controlnet_tensor_specs  # noqa: F401
 from ._lib import LIB_PATH, PROTOTYPES, SdxlError, SdxlLibraryMissing, load  # noqa: F401
 from .engine import Conditioning, Context, Diffuser, LatentDecoder, ddim_timesteps  # noqa: F401
 from .tokenizer import ClipTokenizer, OpenClipTokenizer  # noqa: F401
 from .embedder import ClipTextEncoder, Embedder, conditioning_embedding  # noqa: F401
 from .pipeline import load_models, make_inpaint_mask, sample  # noqa: F401
+from .controlnet import ControlNet  # noqa: F401
 from . import burn_record  # noqa: F401

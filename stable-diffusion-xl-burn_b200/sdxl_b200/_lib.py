@@ -63,6 +63,19 @@ class Adapter(C.Structure):
 MAX_ADAPTERS = 16   # SDXL_MAX_ADAPTERS (include/sdxl_b200.h)
 
 
+class ControlNetCfg(C.Structure):
+    _fields_ = [("unet", UnetCfg), ("hint_in_channels", C.c_int32), ("n_hint_blocks", C.c_int32),
+                ("hint_block_channels", C.c_int32 * SDXL_MAX_LEVELS)]
+
+
+class Control(C.Structure):
+    _fields_ = [("net", C.c_void_p), ("hint", C.c_void_p), ("hint_on_host", C.c_int32), ("n_hint", C.c_int32),
+                ("height", C.c_int32), ("width", C.c_int32), ("scale", C.c_float)]
+
+
+MAX_CONTROLS = 4    # SDXL_MAX_CONTROLS (include/sdxl_b200.h)
+
+
 # name -> (restype, argtypes); every symbol include/sdxl_b200.h declares
 P = C.c_void_p
 I = C.c_int
@@ -125,6 +138,10 @@ PROTOTYPES = {
     "sdxl_clip_plan_flops": (C.c_double, [P]),
     "sdxl_unet_set_adapters": (I, [P, I, C.POINTER(Adapter)]),
     "sdxl_clip_set_adapters": (I, [P, I, C.POINTER(Adapter)]),
+    "sdxl_controlnet_load": (I, [P, C.POINTER(ControlNetCfg), P, C.c_size_t, I, C.POINTER(P)]),
+    "sdxl_controlnet_destroy": (None, [P]),
+    "sdxl_unet_set_controls": (I, [P, I, C.POINTER(Control)]),
+    "sdxl_controlnet_embed_hint": (I, [P, I, I, I, P, I, P]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),
     "sdxl_mpk_encode_u16": (C.c_size_t, [P, C.c_size_t, P]),

@@ -47,6 +47,20 @@ TINY_REFINER = UNetConfig(adm_in_channels=16, model_channels=64, channel_mults=(
 
 
 @dataclass(frozen=True)
+class ControlNetConfig:
+    """An SDXL ControlNet (DESIGN.md §8): the encoder half of `unet` (which must match the UNet it is attached to) plus the hint
+    encoder: conv(hint_in -> c0), then per level conv(c_k -> c_k), conv(c_k -> c_k+1, stride 2), then conv(c_last -> mc)
+    (diffusers' conditioning_embedding_out_channels)."""
+    unet: UNetConfig
+    hint_in_channels: int = 3
+    hint_block_channels: Tuple[int, ...] = (16, 32, 96, 256)
+
+
+SDXL_CONTROLNET = ControlNetConfig(SDXL_BASE)
+TINY_CONTROLNET = ControlNetConfig(TINY, hint_block_channels=(8, 16, 24, 32))
+
+
+@dataclass(frozen=True)
 class VaeConfig:
     """Decoder half of AutoencoderConfig (reference src/model/autoencoder/mod.rs:28-45: the widths are hard-coded
     there; parameters here so a small instance can be tested) + LatentDecoder.scale_factor."""

@@ -1,0 +1,260 @@
+"""ControlNet (DESIGN.md §8): diffusers SDXL ControlNetModel files -> pack names, and the device-resident net of
+sdxl_controlnet_load. A net is attached to a UNet with Diffuser.set_controls or sample(..., controls=...)."""
+from __future__ import annotations
+
+import ctypes as C
+import json
+import os
+from typing import Dict, List, Tuple
+
+import torch
+
+from . import _lib
+from ._lib import SdxlError
+from .config import ControlNetConfig, UNetConfig
+from .engine import _cfg_struct
+from .lora import read_safetensors
+from .weights import build_pack, controlnet_tensor_specs
+
+SDXL_DOWN_BLOCK_TYPES = ["DownBlock2D", "CrossAttnDownBlock2D", "CrossAttnDownBlock2D"]
+# ControlNet variants this loader does not implement, recognised by a key prefix or substring
+_FOREIGN = [("control_model.", "an SGM/ldm ControlNet checkpoint (convert it to diffusers format)"),
+            ("task_embedding", "a ControlNet-Union checkpoint"), ("control_type_proj", "a ControlNet-Union checkpoint"),
+            ("transformer_layes", "a ControlNet-Union checkpoint"), ("lora", "a Control-LoRA checkpoint"),
+            ("adapter.", "a T2I-Adapter checkpoint"), ("body.", "a T2I-Adapter checkpoint")]
+
+_RES = {"norm1": "norm_in", "conv1": "conv_in", "time_emb_proj": "lin_embed", "norm2": "norm_out", "conv2": "conv_out",
+        "conv_shortcut": "skip_connection"}
+_ATTN = {"to_q": "query", "to_k": "key", "to_v": "value", "to_out.0": "out"}
+
+
+def config_from_diffusers(cfg: Dict) -> ControlNetConfig:
+    """ControlNetConfig of a diffusers ControlNetModel config.json; everything this engine does not run is rejected by name."""
+    if cfg.get("global_pool_conditions"):
+        raise SdxlError("controlnet config: global_pool_conditions = true is not supported")
+    dbt = list(cfg.get("down_block_types", []))
+    if dbt != SDXL_DOWN_BLOCK_TYPES:
+        raise SdxlError(f"controlnet config: down_block_types {dbt} is not SDXL base's {SDXL_DOWN_BLOCK_TYPES}")
+    ch = list(cfg["block_out_channels"])
+    mc = ch[0]
+    heads = cfg.get("num_attention_heads") or cfg.get("attention_head_dim")
+    heads = list(heads) if isinstance(heads, (list, tuple)) else [heads] * len(ch)
+    for lvl, t in enumerate(dbt):
+        if t.startswith("CrossAttn") and ch[lvl] != 64 * heads[lvl]:
+            raise SdxlError(f"controlnet config: attention_head_dim gives head dim {ch[lvl] // heads[lvl]} at level {lvl}; "
+                            "only 64 is supported")
+    tl = cfg.get("transformer_layers_per_block", 1)
+    tl = list(tl) if isinstance(tl, (list, tuple)) else [tl] * len(ch)
+    depths = tuple(tl[lvl] if t.startswith("CrossAttn") else 0 for lvl, t in enumerate(dbt))
+    unet = UNetConfig(adm_in_channels=int(cfg["projection_class_embeddings_input_dim"]), model_channels=mc,
+                      channel_mults=tuple(c // mc for c in ch), transformer_depths=depths, context_dim=int(cfg["cross_attention_dim"]),
+                      in_channels=int(cfg.get("in_channels", 4)))
+    return ControlNetConfig(unet, hint_in_channels=int(cfg.get("conditioning_channels", 3)),
+                            hint_block_channels=tuple(cfg.get("conditioning_embedding_out_channels", (16, 32, 96, 256))))
+
+
+def diffusers_name_map(cfg: ControlNetConfig) -> Dict[str, Tuple[str, bool]]:
+    """diffusers key -> (pack name, transpose): Linear weights are [out, in] in diffusers and [in, out] in the pack."""
+    m: Dict[str, Tuple[str, bool]] = {}
+
+    def put(src, dst, lin=False):
+        m[f"{src}.weight"] = (f"{dst}/weight", lin)
+        m[f"{src}.bias"] = (f"{dst}/bias", False)
+
+    def res(src, dst, has_skip):
+        for a, b in _RES.items():
+            if a != "conv_shortcut" or has_skip:
+                put(f"{src}.{a}", f"{dst}/{b}", a == "time_emb_proj")
+
+    def st(src, dst, depth):
+        put(f"{src}.norm", f"{dst}/norm")
+        put(f"{src}.proj_in", f"{dst}/proj_in", True)
+        put(f"{src}.proj_out", f"{dst}/proj_out", True)
+        for j in range(depth):
+            s, d = f"{src}.transformer_blocks.{j}", f"{dst}/transformer_{j}"
+            for n in ("norm1", "norm2", "norm3"):
+                put(f"{s}.{n}", f"{d}/{n}")
+            for a in ("attn1", "attn2"):
+                for x, y in _ATTN.items():
+                    if x == "to_out.0":
+                        put(f"{s}.{a}.{x}", f"{d}/{a}/{y}", True)
+                    else:
+                        m[f"{s}.{a}.{x}.weight"] = (f"{d}/{a}/{y}/weight", True)
+            put(f"{s}.ff.net.0.proj", f"{d}/mlp/geglu/proj", True)
+            put(f"{s}.ff.net.2", f"{d}/mlp/lin", True)
+
+    u = cfg.unet
+    put("conv_in", "input_blocks/0")
+    put("time_embedding.linear_1", "lin1_time_embed", True)
+    put("time_embedding.linear_2", "lin2_time_embed", True)
+    put("add_embedding.linear_1", "lin1_label_embed", True)
+    put("add_embedding.linear_2", "lin2_label_embed", True)
+    put("controlnet_cond_embedding.conv_in", "input_hint_block/0")
+    for k in range(2 * (len(cfg.hint_block_channels) - 1)):
+        put(f"controlnet_cond_embedding.blocks.{k}", f"input_hint_block/{2 * k + 2}")
+    put("controlnet_cond_embedding.conv_out", f"input_hint_block/{4 * len(cfg.hint_block_channels) - 2}")
+    idx = 1
+    for lvl in range(u.n_levels):
+        c_in, c_out = u.channel_mults[max(lvl - 1, 0)] * u.model_channels, u.channel_mults[lvl] * u.model_channels
+        tr = u.transformer_depths[lvl] > 0
+        for j in range(2):
+            dst = f"input_blocks/{idx}"
+            res(f"down_blocks.{lvl}.resnets.{j}", f"{dst}/res" if tr else dst, j == 0 and c_in != c_out)
+            if tr:
+                st(f"down_blocks.{lvl}.attentions.{j}", f"{dst}/transformer", u.transformer_depths[lvl])
+            idx += 1
+        if lvl != u.n_levels - 1:
+            put(f"down_blocks.{lvl}.downsamplers.0.conv", f"input_blocks/{idx}")
+            idx += 1
+    for i in range(idx):
+        put(f"controlnet_down_blocks.{i}", f"zero_convs/{i}")
+    res("mid_block.resnets.0", "middle_block/res1", False)
+    st("mid_block.attentions.0", "middle_block/transformer", u.transformer_depths[-1])
+    res("mid_block.resnets.1", "middle_block/res2", False)
+    put("controlnet_mid_block", "middle_block_out")
+    return m
+
+
+def from_diffusers(state_dict: Dict[str, torch.Tensor], config_json) -> Tuple[ControlNetConfig, Dict[str, torch.Tensor]]:
+    """A diffusers SDXL ControlNetModel (state dict + config.json as dict, JSON text or path) -> (config, pack-named f16 weights).
+    Unsupported variants raise SdxlError naming the key or config field. A "bgr" conditioning_channel_order is folded into the
+    first hint conv (its input channels are reversed), so hints are always passed as RGB."""
+    if isinstance(config_json, str):
+        if os.path.exists(config_json):
+            with open(config_json) as f:
+                config_json = json.load(f)
+        else:
+            config_json = json.loads(config_json)
+    for k in state_dict:
+        for pat, what in _FOREIGN:
+            if (k.startswith(pat) if pat.endswith(".") else pat in k):
+                raise SdxlError(f"controlnet: key '{k}' belongs to {what}, which is not supported")
+    cfg = config_from_diffusers(config_json)
+    names = diffusers_name_map(cfg)
+    out: Dict[str, torch.Tensor] = {}
+    for k, t in state_dict.items():
+        if k not in names:
+            raise SdxlError(f"controlnet: unexpected key '{k}' for an SDXL ControlNetModel")
+        dst, lin = names[k]
+        t = t.detach().to("cpu")
+        if lin:
+            t = t.reshape(t.shape[0], t.shape[1]).t()     # proj_in / proj_out may be stored as 1x1 convs
+        out[dst] = t.to(torch.float16).contiguous()
+    if config_json.get("controlnet_conditioning_channel_order", "rgb") == "bgr":
+        out["input_hint_block/0/weight"] = out["input_hint_block/0/weight"].flip(1).contiguous()
+    missing = [n for n, *_ in controlnet_tensor_specs(cfg) if n not in out]
+    if missing:
+        raise SdxlError(f"controlnet: tensor '{missing[0]}' is missing ({len(missing)} in all)")
+    return cfg, out
+
+
+def cfg_struct(cfg: ControlNetConfig) -> _lib.ControlNetCfg:
+    s = _lib.ControlNetCfg()
+    s.unet = _cfg_struct(cfg.unet)
+    s.hint_in_channels = cfg.hint_in_channels
+    s.n_hint_blocks = len(cfg.hint_block_channels)
+    for i, c in enumerate(cfg.hint_block_channels):
+        s.hint_block_channels[i] = c
+    return s
+
+
+class ControlNet:
+    """A device-resident ControlNet (sdxl_controlnet_load). weights: pack-named tensor dict or a built pack."""
+
+    def __init__(self, ctx, cfg: ControlNetConfig, weights):
+        self.ctx, self.cfg = ctx, cfg
+        pack = weights if isinstance(weights, torch.Tensor) else build_pack(weights)
+        ctx.enter()
+        if pack.is_cuda:
+            torch.cuda.current_stream(ctx.device).synchronize()
+        cs = cfg_struct(cfg)
+        h = C.c_void_p()
+        ctx.check(ctx.lib.sdxl_controlnet_load(ctx.h, C.byref(cs), pack.data_ptr(), pack.numel(), int(pack.is_cuda), C.byref(h)),
+                  "sdxl_controlnet_load")
+        self.h = h
+        self.attached = 0   # attachments to UNets (set_controls); close() refuses while > 0
+
+    @classmethod
+    def from_diffusers_dir(cls, ctx, path: str) -> "ControlNet":
+        """A diffusers ControlNetModel directory: config.json + diffusion_pytorch_model[.fp16].safetensors."""
+        files = [f for f in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors")
+                 if os.path.exists(os.path.join(path, f))]
+        if not files:
+            raise SdxlError(f"{path}: no diffusion_pytorch_model[.fp16].safetensors")
+        cfg, w = from_diffusers(read_safetensors(os.path.join(path, files[0])), os.path.join(path, "config.json"))
+        return cls(ctx, cfg, w)
+
+    def handle(self) -> int:
+        if not getattr(self, "h", None):
+            raise SdxlError("ControlNet is closed")
+        return self.h.value
+
+    def embed_hint(self, hint: torch.Tensor) -> torch.Tensor:
+        """hint_emb [n, mc, H/8, W/8] f32 of hint f32 [n, 3, H, W] in [0, 1] (test aid)."""
+        ctx = self.ctx
+        h = self.handle()
+        hint = hint_tensor(hint, self.cfg.hint_in_channels).to(ctx.device).contiguous()
+        n, _, H, W = hint.shape
+        out = torch.empty(n, self.cfg.unet.model_channels, H // 8, W // 8, device=ctx.device, dtype=torch.float32)
+        ctx.enter()
+        ctx.check(ctx.lib.sdxl_controlnet_embed_hint(h, n, H, W, hint.data_ptr(), 0, out.data_ptr()), "sdxl_controlnet_embed_hint")
+        ctx.leave()
+        return out
+
+    def close(self) -> None:
+        """Frees the device weights. Refused while the net is attached to a UNet: detach it first (set_controls([]))."""
+        if getattr(self, "attached", 0) > 0:
+            raise SdxlError("ControlNet.close: the net is still attached to a UNet (detach it with set_controls([]) first)")
+        if getattr(self, "h", None):
+            self.ctx.lib.sdxl_controlnet_destroy(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+def hint_tensor(hint: torch.Tensor, channels: int) -> torch.Tensor:
+    """A control image as the engine takes it: f32 [n, channels, H, W] in [0, 1] is used as is, u8 [n, H, W, channels] is
+    scaled by 1/255. The engine reads n * channels * H * W floats from the pointer, so any other shape is refused here."""
+    if hint.dtype == torch.uint8:
+        if hint.dim() != 4 or hint.shape[3] != channels:
+            raise SdxlError(f"u8 control image must be [n, H, W, {channels}], got {tuple(hint.shape)}")
+        return hint.permute(0, 3, 1, 2).to(torch.float32) / 255.0
+    if hint.dim() != 4 or hint.shape[1] != channels:
+        raise SdxlError(f"control image must be f32 [n, {channels}, H, W] or u8 [n, H, W, {channels}], got {tuple(hint.shape)}")
+    return hint.to(torch.float32)
+
+
+def set_controls(diffuser, controls: List) -> None:
+    """sdxl_unet_set_controls with [(ControlNet, hint, scale), ...]; [] detaches."""
+    ctx = diffuser.ctx
+    controls = list(controls)
+    if len(controls) > _lib.MAX_CONTROLS:
+        raise SdxlError(f"sdxl_unet_set_controls: at most {_lib.MAX_CONTROLS} controls, got {len(controls)}")
+    handles = [net.handle() for net, _, _ in controls]
+    hints = [hint_tensor(h, net.cfg.hint_in_channels) for net, h, _ in controls]   # every check before any device work
+    hints = [h.to(ctx.device).contiguous() for h in hints]
+    arr = (_lib.Control * max(1, len(controls)))()
+    for i, ((net, _, scale), h) in enumerate(zip(controls, hints)):
+        arr[i].net = handles[i]
+        arr[i].hint = h.data_ptr()
+        arr[i].hint_on_host = 0
+        arr[i].n_hint, arr[i].height, arr[i].width = h.shape[0], h.shape[2], h.shape[3]
+        arr[i].scale = float(scale)
+    ctx.enter()
+    ctx.check(ctx.lib.sdxl_unet_set_controls(diffuser.h, len(controls), arr), "sdxl_unet_set_controls")
+    ctx.leave()
+    release_controls(diffuser)
+    diffuser._controls = [net for net, _, _ in controls]   # the nets stay alive, and cannot be closed, while attached
+    for net in diffuser._controls:
+        net.attached += 1
+
+
+def release_controls(diffuser) -> None:
+    """Forgets the diffuser's attached nets (after a detach, or when the UNet is destroyed)."""
+    for net in getattr(diffuser, "_controls", []):
+        net.attached -= 1
+    diffuser._controls = []

@@ -281,6 +281,9 @@ class Diffuser:
         if getattr(self, "h", None):
             self.ctx.lib.sdxl_unet_destroy(self.h)
             self.h = None
+            if getattr(self, "_controls", None):   # the destroyed UNet no longer uses its ControlNets
+                from .controlnet import release_controls
+                release_controls(self)
 
     def __del__(self):
         try:
@@ -291,6 +294,12 @@ class Diffuser:
     def set_adapters(self, adapters: Sequence) -> None:
         """Replaces the active LoRA set with [(adapter, scale), ...] (sdxl_unet_set_adapters); [] restores the loaded weights."""
         set_adapters(self.ctx, self.ctx.lib.sdxl_unet_set_adapters, self.h, adapters, "sdxl_unet_set_adapters")
+
+    def set_controls(self, controls: Sequence) -> None:
+        """Replaces the attached ControlNets with [(ControlNet, hint, scale), ...] (sdxl_unet_set_controls); [] detaches.
+        hint: f32 [n, 3, H, W] in [0, 1] or u8 [n, H, W, 3]; image b of a batch uses hint b % n."""
+        from .controlnet import set_controls
+        set_controls(self, controls)
 
     # ---- UNet::forward -------------------------------------------------------------------------
     def set_conditioning(self, context: torch.Tensor, label: torch.Tensor) -> None:

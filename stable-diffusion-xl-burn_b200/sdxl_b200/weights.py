@@ -22,7 +22,7 @@ from typing import Dict, Iterable, List, Tuple
 import numpy as np
 import torch
 
-from .config import ClipConfig, UNetConfig, VaeConfig, block_program
+from .config import ClipConfig, ControlNetConfig, UNetConfig, VaeConfig, block_program
 
 Spec = Tuple[str, Tuple[int, ...], str, float]  # name, shape, kind, scale
 
@@ -95,6 +95,25 @@ def unet_tensor_specs(cfg: UNetConfig) -> List[Spec]:
     s += _res_specs("middle_block/res2", mid.c_in, mid.c_out, ted)
     s += [("norm_out/weight", (mc,), "gamma", 1.0), ("norm_out/bias", (mc,), "beta", 1.0),
           ("conv_out/weight", (cfg.out_channels, mc, 3, 3), "conv", 1.0), ("conv_out/bias", (cfg.out_channels,), "bias", 1.0)]
+    return s
+
+
+def controlnet_tensor_specs(cfg: ControlNetConfig) -> List[Spec]:
+    """A ControlNet pack (include/sdxl_b200.h): the UNet's embeddings, input blocks and middle block under the UNet's names, the
+    hint encoder (SGM indices input_hint_block/{0,2,...,14}), one 1x1 zero conv per skip tensor and middle_block_out. The
+    synthetic zero convs and last hint conv (zero-initialised in training) get the residual-output scale, so controls matter."""
+    s = [sp for sp in unet_tensor_specs(cfg.unet) if sp[0].startswith(("lin", "input_blocks/", "middle_block/"))]
+    mc, hc = cfg.unet.model_channels, cfg.hint_block_channels
+    convs = [(cfg.hint_in_channels, hc[0], 1.0)]
+    for k in range(len(hc) - 1):
+        convs += [(hc[k], hc[k], 1.0), (hc[k], hc[k + 1], 1.0)]
+    convs.append((hc[-1], mc, RESID_SCALE))
+    for i, (ci, co, sc) in enumerate(convs):
+        s += [(f"input_hint_block/{2 * i}/weight", (co, ci, 3, 3), "conv", sc), (f"input_hint_block/{2 * i}/bias", (co,), "bias", 1.0)]
+    ins, mid, _ = block_program(cfg.unet)
+    for i, b in enumerate(ins):
+        s += [(f"zero_convs/{i}/weight", (b.c_out, b.c_out, 1, 1), "conv", RESID_SCALE), (f"zero_convs/{i}/bias", (b.c_out,), "bias", 1.0)]
+    s += [("middle_block_out/weight", (mid.c_out, mid.c_out, 1, 1), "conv", RESID_SCALE), ("middle_block_out/bias", (mid.c_out,), "bias", 1.0)]
     return s
 
 
@@ -187,13 +206,15 @@ def alphas_cumprod(n_steps: int = 1000) -> torch.Tensor:
 
 def synth_weights(cfg, seed: int = 0, device: str = "cpu") -> Dict[str, torch.Tensor]:
     """Deterministic (per device type) synthetic f16 weights, reference layouts and names.
-    cfg: UNetConfig (adds alphas_cumprod), VaeConfig (decoder tensors) or ClipConfig (text encoder)."""
+    cfg: UNetConfig (adds alphas_cumprod), VaeConfig (decoder tensors), ClipConfig (text encoder) or ControlNetConfig."""
     gen = torch.Generator(device=device)
     gen.manual_seed(seed)
     out: Dict[str, torch.Tensor] = {}
     is_vae = isinstance(cfg, VaeConfig)
     is_clip = isinstance(cfg, ClipConfig)
-    specs = vae_tensor_specs(cfg) if is_vae else clip_tensor_specs(cfg) if is_clip else unet_tensor_specs(cfg)
+    is_cn = isinstance(cfg, ControlNetConfig)
+    specs = (vae_tensor_specs(cfg) if is_vae else clip_tensor_specs(cfg) if is_clip else controlnet_tensor_specs(cfg) if is_cn
+             else unet_tensor_specs(cfg))
     for name, shape, kind, scale in specs:
         if kind == "linear":
             t = torch.randn(shape, generator=gen, device=device) * (scale / shape[0] ** 0.5)
@@ -210,7 +231,7 @@ def synth_weights(cfg, seed: int = 0, device: str = "cpu") -> Dict[str, torch.Te
         else:
             raise ValueError(kind)
         out[name] = t.to(torch.float16)
-    if not is_vae and not is_clip:
+    if not is_vae and not is_clip and not is_cn:
         out["alphas_cumprod"] = alphas_cumprod(cfg.n_steps).to(device)
     return out
 
