@@ -165,14 +165,6 @@ SDXL_API int sdxl_unet_profile_plan(sdxl_unet* unet, double* ms_by_kind_host, do
                                     int* launches_by_kind_host);
 /* Same measurement, one CSV row per launch (analysis aid; written to `path_host`). */
 SDXL_API int sdxl_unet_profile_dump(sdxl_unet* unet, const char* path_host);
-/* Diagnostics: in-kernel timeline (ns, %globaltimer) of CTA 0 of one implicit-GEMM launch on a synthetic
- * [M,K]x[K,N] problem; stamps_host[9]: see csrc/engine.cu. */
-/* Diagnostics: launch ramp / drain of n_launch back-to-back launches of one Linear GEMM (see tools/igemm_gaps.py). */
-SDXL_API int sdxl_dbg_igemm_gaps(sdxl_ctx* ctx, int M, int K, int N, int with_residual, int n_launch, int64_t* out_host);
-SDXL_API int sdxl_dbg_igemm_timeline(sdxl_ctx* ctx, int M, int K, int N, int geglu, int with_residual,
-                                     uint64_t* stamps_host);
-/* Diagnostics: clock stamps of CTA 0 of one attention launch on synthetic data; stamps_host[3][256][4] (csrc/engine.cu). */
-SDXL_API int sdxl_dbg_attention_timeline(sdxl_ctx* ctx, int B, int T, int S, int n_head, long long* stamps_host);
 /* seeded N(0,1) exactly as the sampler generates it (device out). */
 SDXL_API int sdxl_randn(sdxl_ctx* ctx, float* out, size_t n, uint64_t seed, uint64_t subsequence);
 

@@ -32,12 +32,13 @@ struct sdxl_clip {
   float* hidden = nullptr;   // [B*T, C] result of forward_hidden / h_out
   float* pooled = nullptr;   // [B, embed_dim]
   AdapterState lora;         // LoRA-able weight slots, backups of merged layers (sdxl_clip_set_adapters)
+  ~sdxl_clip() { if (tokens_dev) cudaFree(tokens_dev); }
 };
 
 static int build_clip(sdxl_clip* m, const PackView& pv, Arena& A) {
   sdxl_ctx* c = m->ctx;
   const sdxl_clip_cfg& g = m->cfg;
-  Loader L{nullptr, c, &pv, &A, c->stream};
+  Loader L{c, &pv, &A, c->stream};
   L.reg = &m->lora;
   const int C = g.n_state;
   m->blocks.clear();
@@ -97,9 +98,6 @@ static int build_clip(sdxl_clip* m, const PackView& pv, Arena& A) {
 extern "C" void sdxl_clip_destroy(sdxl_clip* m) {
   if (!m) return;
   cudaStreamSynchronize(m->ctx->stream);
-  m->plan.reset();
-  m->warena.release();
-  if (m->tokens_dev) cudaFree(m->tokens_dev);
   delete m;
 }
 
@@ -112,29 +110,9 @@ extern "C" int sdxl_clip_load(sdxl_ctx* c, const sdxl_clip_cfg* cfg, const void*
   std::unique_ptr<sdxl_clip> m(new sdxl_clip());
   m->ctx = c;
   m->cfg = *cfg;
-  PackView pv;
-  std::vector<uint8_t> table;
-  int r = parse_pack(c, pack, bytes, pack_on_device, pv, table);
+  int r = with_device_pack(c, pack, bytes, pack_on_device, [&](const PackView& pv) { return build_two_pass(m.get(), pv, build_clip); });
   if (r) return r;
-  void* dev_pack = nullptr;
-  if (pack_on_device) {
-    pv.dev = (const uint8_t*)pack;
-  } else {
-    CU(c, cudaMalloc(&dev_pack, bytes));
-    cudaError_t e = cudaMemcpyAsync(dev_pack, pack, bytes, cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) { cudaFree(dev_pack); return fail(c, (int)e, "pack upload failed"); }
-    pv.dev = (const uint8_t*)dev_pack;
-  }
-  Arena meas;
-  meas.measure = true;
-  r = build_clip(m.get(), pv, meas);
-  if (!r && m->warena.init(meas.off + (1 << 20))) r = fail(c, 4203, "cannot allocate %zu bytes for weights", meas.off);
-  if (!r) r = build_clip(m.get(), pv, m->warena);
-  cudaError_t se = cudaStreamSynchronize(c->stream);
-  if (dev_pack) cudaFree(dev_pack);
-  if (!r && se != cudaSuccess) r = fail(c, (int)se, "weight re-layout failed: %s", cudaGetErrorString(se));
-  if (!r && cudaMalloc((void**)&m->tokens_dev, (size_t)(64 * cfg->n_ctx + 64 + 16) * sizeof(int)) != cudaSuccess) r = fail(c, 4412, "cudaMalloc failed");
-  if (r) { m->warena.release(); return r; }
+  if (cudaMalloc((void**)&m->tokens_dev, (size_t)(64 * cfg->n_ctx + 64 + 16) * sizeof(int)) != cudaSuccess) return fail(c, 4412, "cudaMalloc failed");
   m->eot_dev = m->tokens_dev + 64 * cfg->n_ctx;
   m->err_dev = m->eot_dev + 64;
   *out = m.release();
@@ -217,16 +195,8 @@ static int clip_run(sdxl_clip* m, int Bn, const int32_t* tokens_host, int n_run,
   if (n_run < 0 || n_run > g.n_layer) return fail(c, 5202, "hidden_idx %d out of range (n_layer %d)", n_run, g.n_layer);
   CU(c, cudaSetDevice(c->device));
   if (!m->plan || m->pB != Bn || m->p_nrun != n_run || m->p_hidden != capture || m->p_pooled != pooled) {
-    CU(c, cudaStreamSynchronize(c->stream));
-    m->plan.reset(new Plan());
-    Plan* P = m->plan.get();
-    P->Bf = Bn; P->Bx = Bn;
-    Arena meas;
-    meas.measure = true;
-    int r = build_clip_plan(m, P, &meas, n_run, capture, pooled);
-    if (!r && P->arena.init(meas.off + (1 << 20))) r = fail(c, 5011, "cannot allocate %zu bytes of workspace", meas.off);
-    if (!r) r = build_clip_plan(m, P, &P->arena, n_run, capture, pooled);
-    if (r) { m->plan.reset(); return r; }
+    if (int r = build_plan(c, m->plan, Bn, Bn, 0, 0, [&](Plan* P, Arena* A) { return build_clip_plan(m, P, A, n_run, capture, pooled); }))
+      return r;
     m->pB = Bn; m->p_nrun = n_run; m->p_hidden = capture; m->p_pooled = pooled;
   }
   // eot_indices = tokens.argmax(1): first position of the largest id (clip/mod.rs:130)

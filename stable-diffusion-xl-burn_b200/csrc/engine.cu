@@ -127,7 +127,6 @@ struct sdxl_unet : EncoderHalf {
   float* lab1 = nullptr;       // [B, 4mc]
   float* label_emb = nullptr;  // [B, 4mc]
   std::vector<__half*> kv;     // per transformer block [B*n_ctx, 2C]
-  std::vector<int> kvC;
   uint64_t cond_version = 0;
   // plan
   std::unique_ptr<Plan> plan;
@@ -138,6 +137,10 @@ struct sdxl_unet : EncoderHalf {
   AdapterState lora;           // LoRA-able weight slots, backups of merged layers (sdxl_unet_set_adapters)
   std::vector<std::unique_ptr<ControlAttach>> controls;   // sdxl_unet_set_controls, in call order
   uint64_t controls_version = 0;
+  ~sdxl_unet() {
+    if (t_dev) cudaFree(t_dev);
+    if (t_pinned) cudaFreeHost(t_pinned);
+  }
 };
 
 // One attached ControlNet: its scaled zero convs, the encoded hint and its hoisted conditioning.
@@ -153,7 +156,6 @@ struct ControlAttach {
   float* lab1 = nullptr;
   float* label_emb = nullptr;
   std::vector<__half*> kv;
-  ~ControlAttach() { mem.release(); cmem.release(); }
 };
 
 
@@ -166,7 +168,7 @@ static int geglu_bn_for(int n_out /*4C*/) {
 // temb bookkeeping while building: list of (lin_embed path, Cout, conv_in bias) in block order
 struct TembItem { std::string path; int Cout; float* conv_bias; };
 
-static Res load_res(Loader& L, const std::string& path, int Cin, int Cout, int temb_dim, std::vector<TembItem>& tembs, int& temb_total) {
+static Res load_res(Loader& L, const std::string& path, int Cin, int Cout, std::vector<TembItem>& tembs, int& temb_total) {
   Res r;
   r.Cin = Cin; r.Cout = Cout; r.has_skip = (Cin != Cout);
   r.n_in = L.norm(path + "/norm_in", Cin);
@@ -177,7 +179,6 @@ static Res load_res(Loader& L, const std::string& path, int Cin, int Cout, int t
   r.temb_off = temb_total;
   tembs.push_back({path + "/lin_embed", Cout, r.conv_in.b});
   temb_total += Cout;
-  (void)temb_dim;
   return r;
 }
 
@@ -219,30 +220,6 @@ static STrans load_st(Loader& L, const std::string& path, int C, int ctx_dim, in
   return s;
 }
 
-// 3x3 conv with few input channels for the CUDA-core first-conv kernel: OIHW f16 -> [O][kh][kw][I] f32, bias f32
-static int load_conv_f32(Loader& L, const std::string& path, int I, int O, float*& w, float*& b) {
-  sdxl_ctx* c = L.c;
-  Arena& A = *L.A;
-  const PackEntry* e = L.need(path + "/weight", 4);
-  if (!e) return L.err;
-  if ((int)e->shape[0] != O || (int)e->shape[1] != I || e->shape[2] != 3 || e->shape[3] != 3)
-    return fail(c, 4010, "%s/weight bad shape", path.c_str());
-  const size_t n = (size_t)O * 9 * I;
-  __half* tmp = A.get<__half>(n);
-  w = A.get<float>(n);
-  if (!tmp || !w) return fail(c, 4005, "weight arena exhausted");
-  if (!A.measure) {
-    int r = repack_conv_launch(c->stream, L.ptr(e), O, I, 3, 3, tmp, 9 * I, 0, I);
-    if (!r) r = cast_f16_to_f32_launch(c->stream, tmp, n, w);
-    if (r) return fail(c, r, "%s repack failed", path.c_str());
-  }
-  WSlot s;
-  s.base = w; s.conv = 1; s.f32 = 1; s.N = O; s.I = I; s.ks = 3; s.ld = 9 * I; s.Ipad = I;
-  L.record(path, s, n * sizeof(float));
-  b = L.vec_f32(path + "/bias", O);
-  return L.err;
-}
-
 // Time / label MLPs, first conv, input blocks and middle block (reference unet/mod.rs:116-248), for the UNet and for a ControlNet.
 static int load_encoder(Loader& L, EncoderHalf* u, std::vector<TembItem>& tembs, int& temb_total) {
   const sdxl_unet_cfg& g = u->cfg;
@@ -255,7 +232,7 @@ static int load_encoder(Loader& L, EncoderHalf* u, std::vector<TembItem>& tembs,
   u->l1 = L.linear("lin1_label_embed", g.adm_in_channels, ted, true);
   u->l2 = L.linear("lin2_label_embed", ted, ted, true);
   if (L.err) return L.err;
-  if (int r = load_conv_f32(L, "input_blocks/0", g.in_channels, mc, u->conv0_w, u->conv0_b)) return r;
+  if (int r = L.conv_f32("input_blocks/0", g.in_channels, mc, u->conv0_w, u->conv0_b)) return r;
   {
     Block b0; b0.type = BT_CONV; b0.Cout = mc;
     u->in_blocks.push_back(b0);
@@ -272,10 +249,10 @@ static int load_encoder(Loader& L, EncoderHalf* u, std::vector<TembItem>& tembs,
       b.Cout = cout;
       if (!tr) {
         b.type = BT_RES;
-        b.res = load_res(L, bp, k == 0 ? cin : cout, cout, ted, tembs, temb_total);
+        b.res = load_res(L, bp, k == 0 ? cin : cout, cout, tembs, temb_total);
       } else {
         b.type = BT_REST;
-        b.res = load_res(L, bp + "/res", k == 0 ? cin : cout, cout, ted, tembs, temb_total);
+        b.res = load_res(L, bp + "/res", k == 0 ? cin : cout, cout, tembs, temb_total);
         b.st = load_st(L, bp + "/transformer", cout, g.context_dim, n_head(cout), g.transformer_depths[level]);
       }
       u->in_blocks.push_back(std::move(b));
@@ -292,9 +269,9 @@ static int load_encoder(Loader& L, EncoderHalf* u, std::vector<TembItem>& tembs,
   // middle (reference unet/mod.rs:238-248)
   {
     const int cm = g.channel_mults[g.n_levels - 1] * mc;
-    u->mid_res1 = load_res(L, "middle_block/res1", cm, cm, ted, tembs, temb_total);
+    u->mid_res1 = load_res(L, "middle_block/res1", cm, cm, tembs, temb_total);
     u->mid_st = load_st(L, "middle_block/transformer", cm, g.context_dim, n_head(cm), g.transformer_depths[g.n_levels - 1]);
-    u->mid_res2 = load_res(L, "middle_block/res2", cm, cm, ted, tembs, temb_total);
+    u->mid_res2 = load_res(L, "middle_block/res2", cm, cm, tembs, temb_total);
   }
   return L.err;
 }
@@ -329,9 +306,9 @@ static int load_temb_all(Loader& L, EncoderHalf* u, const std::vector<TembItem>&
 static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
-  Loader L{u, c, &pv, &A, c->stream};
+  Loader L{c, &pv, &A, c->stream};
   L.reg = &u->lora;
-  const int mc = g.model_channels, ted = 4 * mc;
+  const int mc = g.model_channels;
   u->out_blocks.clear();
   std::vector<TembItem> tembs;
   int temb_total = 0;
@@ -354,10 +331,10 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
       const bool up = (k == 2) && (tr || level != 0);
       if (!tr) {
         b.type = up ? BT_RESU : BT_RES;
-        b.res = load_res(L, up ? bp + "/res" : bp, cins[k], cout, ted, tembs, temb_total);
+        b.res = load_res(L, up ? bp + "/res" : bp, cins[k], cout, tembs, temb_total);
       } else {
         b.type = up ? BT_RESTU : BT_REST;
-        b.res = load_res(L, bp + "/res", cins[k], cout, ted, tembs, temb_total);
+        b.res = load_res(L, bp + "/res", cins[k], cout, tembs, temb_total);
         b.st = load_st(L, bp + "/transformer", cout, g.context_dim, n_head(cout), g.transformer_depths[level]);
       }
       if (up) b.conv = L.upconv(bp + "/upsample/conv", cout, cout);
@@ -392,45 +369,47 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
 // ================================================================================================
 // load
 // ================================================================================================
+// The configurations the UNet (and a ControlNet's copy of its encoder) are built for.
+static int check_unet_cfg(sdxl_ctx* c, const sdxl_unet_cfg& g) {
+  if (g.n_head_channels != 64) return fail(c, 4200, "n_head_channels must be 64 (got %d)", g.n_head_channels);
+  if (g.n_levels < 1 || g.n_levels > SDXL_MAX_LEVELS) return fail(c, 4201, "bad n_levels");
+  if (g.in_channels > 8 || g.model_channels % 32) return fail(c, 4202, "unsupported channel config");
+  return 0;
+}
 
-extern "C" void sdxl_unet_destroy(sdxl_unet* u);
-
-// Parses a weight pack, makes it device-resident for the call (host packs are uploaded to a temporary copy) and runs fn(pv);
-// the stream is synchronised before the copy is freed.
-template <typename Fn>
-static int with_device_pack(sdxl_ctx* c, const void* pack, size_t bytes, int pack_on_device, Fn fn) {
-  PackView pv;
-  std::vector<uint8_t> table;
-  int r = parse_pack(c, pack, bytes, pack_on_device, pv, table);
+static int unet_load_impl(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pack, size_t bytes, int pack_on_device, sdxl_unet** out) {
+  if (!c || !cfg || !pack || !out) return fail(c, -1, "sdxl_unet_load: null argument");
+  *out = nullptr;
+  if (int r = check_unet_cfg(c, *cfg)) return r;
+  CU(c, cudaSetDevice(c->device));
+  std::unique_ptr<sdxl_unet> u(new sdxl_unet());
+  u->ctx = c;
+  u->cfg = *cfg;
+  int r = with_device_pack(c, pack, bytes, pack_on_device, [&](const PackView& pv) {
+    int r2 = build_two_pass(u.get(), pv, build_model);
+    // alphas_cumprod: f16-stored in the reference's record (HalfPrecisionSettings), read as f64 (mod.rs:485-492)
+    if (!r2) {
+      const PackEntry* e = pv.find("alphas_cumprod");
+      if (!e || e->ndim != 1 || e->dtype != 0) return fail(c, 4204, "weight pack: missing f16 'alphas_cumprod'");
+      std::vector<uint16_t> raw(e->shape[0]);
+      cudaError_t ce = cudaMemcpyAsync(raw.data(), pv.dev + e->offset, raw.size() * 2, cudaMemcpyDeviceToHost, c->stream);
+      if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
+      if (ce != cudaSuccess) return fail(c, (int)ce, "alphas download failed");
+      u->alphas.resize(raw.size());
+      for (size_t i = 0; i < raw.size(); ++i) {
+        __half_raw hr;
+        hr.x = raw[i];
+        u->alphas[i] = (double)__half2float(__half(hr));
+      }
+    }
+    return r2;
+  });
   if (r) return r;
-  void* dev_pack = nullptr;
-  if (pack_on_device) {
-    pv.dev = (const uint8_t*)pack;
-  } else {
-    CU(c, cudaMalloc(&dev_pack, bytes));
-    cudaError_t e = cudaMemcpyAsync(dev_pack, pack, bytes, cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) { cudaFree(dev_pack); return fail(c, (int)e, "pack upload failed"); }
-    pv.dev = (const uint8_t*)dev_pack;
-  }
-  r = fn((const PackView&)pv);
-  cudaError_t se = cudaStreamSynchronize(c->stream);
-  if (dev_pack) cudaFree(dev_pack);
-  if (!r && se != cudaSuccess) r = fail(c, (int)se, "weight re-layout failed: %s", cudaGetErrorString(se));
-  return r;
+  CU(c, cudaMalloc((void**)&u->t_dev, 64));
+  CU(c, cudaMallocHost((void**)&u->t_pinned, 4096 * sizeof(int)));
+  *out = u.release();
+  return 0;
 }
-
-// pass 1: measure, pass 2: build into the model's weight arena
-template <typename M>
-static int build_two_pass(M* m, const PackView& pv, int (*build)(M*, const PackView&, Arena&)) {
-  Arena meas;
-  meas.measure = true;
-  int r = build(m, pv, meas);
-  if (!r && m->warena.init(meas.off + (1 << 20))) r = fail(m->ctx, 4203, "cannot allocate %zu bytes for weights", meas.off);
-  if (!r) r = build(m, pv, m->warena);
-  return r;
-}
-
-static int unet_load_impl(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pack, size_t bytes, int pack_on_device, sdxl_unet** out);
 
 extern "C" int sdxl_unet_load(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
                               sdxl_unet** out) {
@@ -496,49 +475,13 @@ extern "C" int sdxl_unet_load_broadcast(sdxl_ctx* c, const sdxl_unet_cfg* cfg, c
   return r;
 }
 
-static int unet_load_impl(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pack, size_t bytes, int pack_on_device, sdxl_unet** out) {
-  if (!c || !cfg || !pack || !out) return fail(c, -1, "sdxl_unet_load: null argument");
-  *out = nullptr;
-  if (cfg->n_head_channels != 64) return fail(c, 4200, "n_head_channels must be 64 (got %d)", cfg->n_head_channels);
-  if (cfg->n_levels < 1 || cfg->n_levels > SDXL_MAX_LEVELS) return fail(c, 4201, "bad n_levels");
-  if (cfg->in_channels > 8 || cfg->model_channels % 32) return fail(c, 4202, "unsupported channel config");
-  CU(c, cudaSetDevice(c->device));
-  std::unique_ptr<sdxl_unet> u(new sdxl_unet());
-  u->ctx = c;
-  u->cfg = *cfg;
-  int r = with_device_pack(c, pack, bytes, pack_on_device, [&](const PackView& pv) {
-    int r2 = build_two_pass(u.get(), pv, build_model);
-    // alphas_cumprod: f16-stored in the reference's record (HalfPrecisionSettings), read as f64 (mod.rs:485-492)
-    if (!r2) {
-      const PackEntry* e = pv.find("alphas_cumprod");
-      if (!e || e->ndim != 1 || e->dtype != 0) return fail(c, 4204, "weight pack: missing f16 'alphas_cumprod'");
-      std::vector<uint16_t> raw(e->shape[0]);
-      cudaError_t ce = cudaMemcpyAsync(raw.data(), pv.dev + e->offset, raw.size() * 2, cudaMemcpyDeviceToHost, c->stream);
-      if (ce == cudaSuccess) ce = cudaStreamSynchronize(c->stream);
-      if (ce != cudaSuccess) return fail(c, (int)ce, "alphas download failed");
-      u->alphas.resize(raw.size());
-      for (size_t i = 0; i < raw.size(); ++i) {
-        __half_raw hr;
-        hr.x = raw[i];
-        u->alphas[i] = (double)__half2float(__half(hr));
-      }
-    }
-    return r2;
-  });
-  if (r) return r;
-  CU(c, cudaMalloc((void**)&u->t_dev, 64));
-  CU(c, cudaMallocHost((void**)&u->t_pinned, 4096 * sizeof(int)));
-  *out = u.release();
-  return 0;
-}
-
 // ================================================================================================
 // ControlNet load
 // ================================================================================================
 static int build_controlnet(sdxl_controlnet* n, const PackView& pv, Arena& A) {
   const sdxl_unet_cfg& g = n->cfg;
   const sdxl_controlnet_cfg& nc = n->ncfg;
-  Loader L{n, n->ctx, &pv, &A, n->ctx->stream};   // no LoRA registry: adapters on a ControlNet are not supported
+  Loader L{n->ctx, &pv, &A, n->ctx->stream};   // no LoRA registry: adapters on a ControlNet are not supported
   std::vector<TembItem> tembs;
   int temb_total = 0;
   if (int r = load_encoder(L, n, tembs, temb_total)) return r;
@@ -547,7 +490,7 @@ static int build_controlnet(sdxl_controlnet* n, const PackView& pv, Arena& A) {
   // 4n - 2 = conv(c_last -> mc)
   const int* hc = nc.hint_block_channels;
   const int nb = nc.n_hint_blocks;
-  if (int r = load_conv_f32(L, "input_hint_block/0", nc.hint_in_channels, hc[0], n->hint0_w, n->hint0_b)) return r;
+  if (int r = L.conv_f32("input_hint_block/0", nc.hint_in_channels, hc[0], n->hint0_w, n->hint0_b)) return r;
   n->hint.clear();
   for (int k = 0; k + 1 < nb && !L.err; ++k) {
     n->hint.push_back(L.conv("input_hint_block/" + std::to_string(2 + 4 * k), hc[k], hc[k], 3));
@@ -567,10 +510,7 @@ extern "C" int sdxl_controlnet_load(sdxl_ctx* c, const sdxl_controlnet_cfg* cfg,
                                     sdxl_controlnet** out) {
   if (!c || !cfg || !pack || !out) return fail(c, -1, "sdxl_controlnet_load: null argument");
   *out = nullptr;
-  const sdxl_unet_cfg& g = cfg->unet;
-  if (g.n_head_channels != 64) return fail(c, 4200, "n_head_channels must be 64 (got %d)", g.n_head_channels);
-  if (g.n_levels < 1 || g.n_levels > SDXL_MAX_LEVELS) return fail(c, 4201, "bad n_levels");
-  if (g.in_channels > 8 || g.model_channels % 32) return fail(c, 4202, "unsupported channel config");
+  if (int r = check_unet_cfg(c, cfg->unet)) return r;
   if (cfg->hint_in_channels < 1 || cfg->hint_in_channels > 8) return fail(c, 4700, "hint_in_channels must be in [1, 8] (got %d)", cfg->hint_in_channels);
   if (cfg->n_hint_blocks != 4) return fail(c, 4701, "n_hint_blocks must be 4 (hint downscale 2^(n-1) = 8), got %d", cfg->n_hint_blocks);
   for (int k = 0; k < cfg->n_hint_blocks; ++k)
@@ -579,11 +519,11 @@ extern "C" int sdxl_controlnet_load(sdxl_ctx* c, const sdxl_controlnet_cfg* cfg,
   CU(c, cudaSetDevice(c->device));
   std::unique_ptr<sdxl_controlnet> n(new sdxl_controlnet());
   n->ctx = c;
-  n->cfg = g;
+  n->cfg = cfg->unet;
   n->ncfg = *cfg;
   int r = with_device_pack(c, pack, bytes, pack_on_device,
                            [&](const PackView& pv) { return build_two_pass(n.get(), pv, build_controlnet); });
-  if (r) { n->warena.release(); return r; }
+  if (r) return r;
   *out = n.release();
   return 0;
 }
@@ -591,32 +531,16 @@ extern "C" int sdxl_controlnet_load(sdxl_ctx* c, const sdxl_controlnet_cfg* cfg,
 extern "C" void sdxl_controlnet_destroy(sdxl_controlnet* n) {
   if (!n) return;
   cudaStreamSynchronize(n->ctx->stream);
-  n->warena.release();
   delete n;
 }
 
 // 3x3 pad-1 conv of an NHWC f16 image on the implicit GEMM, stride 1 or 2 (stride 2: `a` is the phase split of the input,
 // [4][Bn][H/2][W/2][C], as written by silu_f16_launch / phase_split_launch). Output f32 NHWC at H x W (stride 1) or H/2 x W/2.
 static int conv3x3_direct(sdxl_ctx* c, const __half* a, int Bn, int H, int W, int C, const Conv& cv, int stride, float* out) {
-  IgemmParams p{};
   const int Ho = H / stride, Wo = W / stride;
-  p.nseg = 0;
-  for (int kh = 0; kh < 3; ++kh)
-    for (int kw = 0; kw < 3; ++kw) {
-      if (stride == 2) {   // tap kh -> (phase, offset), as the UNet's Downsample
-        const int ph = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
-        p.seg[p.nseg++] = {0, (int16_t)((kw == 0) ? -1 : 0), (int16_t)((kh == 0) ? -1 : 0), (int16_t)((ph * 2 + pw) * Bn), cv.Ipad / 64};
-      } else {
-        p.seg[p.nseg++] = {0, (int16_t)(kw - 1), (int16_t)(kh - 1), 0, cv.Ipad / 64};
-      }
-    }
-  p.out = out; p.out_f32 = 1; p.ldo = cv.O;
-  p.bias = cv.b; p.bias_bstride = 0; p.res = nullptr; p.ldr = 0;
-  IgemmOperands o{a, stride == 2 ? 4 * Bn : Bn, Ho, Wo, C, C, nullptr, 0, 0, 0, 0, 0, cv.w, cv.O, cv.Ktot};
-  int r = igemm_configure(p, o, Wo, Ho, Bn, IGEMM_LINEAR, 0);
-  if (r) return fail(c, r, "igemm configuration failed (hint encoder, %d -> %d)", C, cv.O);
-  KL(c, igemm_launch(c->stream, p));
-  return 0;
+  const IgemmOperands o{a, stride == 2 ? 4 * Bn : Bn, Ho, Wo, C, C, nullptr, 0, 0, 0, 0, 0, cv.w, cv.O, cv.Ktot};
+  return igemm_run(c, o, stride == 2 ? stride2_taps(Bn, cv.Ipad / 64) : conv_taps(3, cv.Ipad / 64), Ho, Wo, Bn, IGEMM_LINEAR, 0, out,
+                   1, cv.O, cv.b, nullptr, 0);
 }
 
 // Hint encoder (SGM input_hint_block): hint f32 NCHW [n, in, H, W] (device) -> f32 NHWC [n, H/8, W/8, mc]. Queued on the ctx stream.
@@ -714,7 +638,7 @@ struct UNetPlanBuilder : PlanBuilder {
         Cx = b.res.Cout;
         if (b.type == BT_REST) x = strans(b.st, x, H, W, s.a16, s.tok, s.qkv, s.ao, s.q, s.ff);
       } else if (b.type == BT_DOWN) {
-        // 3x3 stride 2 pad 1 (unet/mod.rs:760-774) on phase-split input: tap kh -> (phase, offset)
+        // 3x3 stride 2 pad 1 (unet/mod.rs:760-774) on phase-split input
         __half* ph = buf<__half>((size_t)Bf * H * W * Cx);
         Op op{};
         op.kind = OP_PHASE;
@@ -722,15 +646,8 @@ struct UNetPlanBuilder : PlanBuilder {
         if (!err) P->ops.push_back(op);
         const int H2 = H / 2, W2 = W / 2;
         ActView a{ph, 4 * Bf, H2, W2, Cx};
-        std::vector<IgemmSeg> segs;
-        for (int kh = 0; kh < 3; ++kh)
-          for (int kw = 0; kw < 3; ++kw) {
-            const int phh = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
-            const int dh = (kh == 0) ? -1 : 0, dw = (kw == 0) ? -1 : 0;
-            segs.push_back({0, (int16_t)dw, (int16_t)dh, (int16_t)((phh * 2 + pw) * Bf), b.conv.Ipad / 64});
-          }
         float* y = buf<float>((size_t)Bf * H2 * W2 * Cx);
-        igemm(a, nullptr, segs, b.conv.w, b.conv.O, b.conv.Ktot, H2, W2, Bf, IGEMM_LINEAR, 0, y, 1, b.conv.O, b.conv.b, 0, nullptr, 0);
+        igemm(a, nullptr, stride2_taps(Bf, b.conv.Ipad / 64), b.conv.w, b.conv.O, b.conv.Ktot, H2, W2, Bf, IGEMM_LINEAR, 0, y, 1, b.conv.O, b.conv.b, 0, nullptr, 0);
         add_flops(2.0 * Bf * H2 * W2 * 9.0 * Cx * b.conv.O);
         x = y; H = H2; W = W2;
       }
@@ -962,10 +879,8 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
   if (!B.err && !P->ops.empty()) P->ops.back().gn.y_lo = s_raw;   // rounding residue of the normalised activation (hi/lo split)
   {
     ActView a{s_gn1, Bf, H, W, Cx}, alo{s_raw, Bf, H, W, Cx};
-    std::vector<IgemmSeg> segs;
-    for (int part = 0; part < 2; ++part)   // K = [9 taps on hi | 9 taps on lo], weights [W | W]
-      for (int kh = 0; kh < 3; ++kh)
-        for (int kw = 0; kw < 3; ++kw) segs.push_back({(int16_t)part, (int16_t)(kw - 1), (int16_t)(kh - 1), 0, u->conv_out.Ipad / 64});
+    std::vector<IgemmSeg> segs = conv_taps(3, u->conv_out.Ipad / 64, 0), lo = conv_taps(3, u->conv_out.Ipad / 64, 1);
+    segs.insert(segs.end(), lo.begin(), lo.end());   // K = [9 taps on hi | 9 taps on lo], weights [W | W]
     B.igemm(a, &alo, segs, u->conv_out_w2, u->conv_out.O, 2 * u->conv_out.Ktot, H, W, Bf, IGEMM_LINEAR, 0, P->eps, 1, P->eps_ld,
             u->conv_out.b, 0, nullptr, 0);
     B.add_flops(2.0 * Bf * H * W * 9.0 * Cx * u->conv_out.O);
@@ -986,17 +901,9 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
   if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan->cond_version == u->cond_version &&
       u->plan->controls_version == u->controls_version)
     return 0;
-  CU(c, cudaStreamSynchronize(c->stream));
-  u->plan.reset(new Plan());
-  Plan* P = u->plan.get();
-  P->Bf = Bf; P->Bx = Bx; P->h = h; P->w = w; P->cond_version = u->cond_version; P->controls_version = u->controls_version;
-  Arena meas;
-  meas.measure = true;
-  int r = build_plan_ops(u, P, &meas);
-  if (r) { u->plan.reset(); return r; }
-  if (P->arena.init(meas.off + (1 << 20))) { u->plan.reset(); return fail(c, 5011, "cannot allocate %zu bytes of workspace", meas.off); }
-  r = build_plan_ops(u, P, &P->arena);
-  if (r) { u->plan.reset(); return r; }
+  if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A); })) return r;
+  u->plan->cond_version = u->cond_version;
+  u->plan->controls_version = u->controls_version;
   return 0;
 }
 
@@ -1071,11 +978,7 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
     u->lab1 = u->carena.get<float>((size_t)B * ted);
     u->label_emb = u->carena.get<float>((size_t)B * ted);
     u->kv.clear();
-    u->kvC.clear();
-    for (auto* t : tbs) {
-      u->kv.push_back(u->carena.get<__half>((size_t)B * n_ctx * t->kv2.N));
-      u->kvC.push_back(t->kv2.N / 2);
-    }
+    for (auto* t : tbs) u->kv.push_back(u->carena.get<__half>((size_t)B * n_ctx * t->kv2.N));
     u->condB = B;
     u->n_ctx = n_ctx;
     CU(c, cudaMemsetAsync(u->ctx16, 0, (size_t)B * n_ctx * u->ctx_pitch * 2, c->stream));
@@ -1107,14 +1010,8 @@ static int hoist_model(sdxl_unet* u, const EncoderHalf& e, const std::vector<con
   const int M = B * n_ctx;
   for (size_t i = 0; i < tbs.size(); ++i) {
     const Lin& L = tbs[i]->kv2;
-    IgemmParams p{};
-    p.nseg = 1;
-    p.seg[0] = {0, 0, 0, 0, L.Kpad / 64};
-    p.out = kv[i]; p.out_f32 = 0; p.ldo = L.N;
-    IgemmOperands o{u->ctx16, 1, 1, M, g.context_dim, u->ctx_pitch, nullptr, 0, 0, 0, 0, 0, L.w, L.N, L.Kpad};
-    int r = igemm_configure(p, o, M, 1, 1, IGEMM_LINEAR, 0);
-    if (r) return fail(c, r, "igemm configuration failed (kv projection)");
-    KL(c, igemm_launch(c->stream, p));
+    const IgemmOperands o{u->ctx16, 1, 1, M, g.context_dim, u->ctx_pitch, nullptr, 0, 0, 0, 0, 0, L.w, L.N, L.Kpad};
+    if (int r = igemm_run(c, o, {{0, 0, 0, 0, L.Kpad / 64}}, 1, M, 1, IGEMM_LINEAR, 0, kv[i], 0, L.N, nullptr, nullptr, 0)) return r;
   }
   return 0;
 }
@@ -1283,7 +1180,7 @@ extern "C" int sdxl_unet_forward_f32(sdxl_unet* u, int B, int h, int w, const fl
   return 0;
 }
 // Per-kernel-kind device time of one plan execution, measured with CUDA events on the ctx stream
-// (eager launches, one event pair per op). kinds: see OpKind. Arrays must hold 16 entries.
+// (eager launches, one event pair per op). kinds: see OpKind. Arrays hold SDXL_PROFILE_KINDS entries.
 extern "C" int sdxl_unet_profile_plan(sdxl_unet* u, double* ms_by_kind, double* flops_by_kind, int* launches_by_kind) {
   if (!u || !u->plan) return -1;
   return profile_plan_impl(u->ctx, u->plan.get(), ms_by_kind, flops_by_kind, launches_by_kind);
@@ -1324,7 +1221,6 @@ struct Sampler {
   size_t latent_elems = 0;
   Arena arena;
   ~Sampler() {
-    arena.release();
     if (host_stage) cudaFreeHost(host_stage);
   }
 };
@@ -1537,12 +1433,6 @@ extern "C" int sdxl_make_inpaint_mask(int img_w, int img_h, int lat_w, int lat_h
 extern "C" void sdxl_unet_destroy(sdxl_unet* u) {
   if (!u) return;
   cudaStreamSynchronize(u->ctx->stream);
-  u->plan.reset();
-  u->sampler.reset();
-  u->warena.release();
-  u->carena.release();
-  if (u->t_dev) cudaFree(u->t_dev);
-  if (u->t_pinned) cudaFreeHost(u->t_pinned);
   delete u;
 }
 
@@ -1589,19 +1479,9 @@ extern "C" int sdxl_op_linear(sdxl_ctx* c, const sdxl_half* x, const sdxl_half* 
   if (!wt || (bias && !b32)) return fail(c, 5312, "temporary allocation failed");
   KL(c, transpose_linear_launch(c->stream, (const __half*)w, K, N, wt, Kpad, 0, gbn));
   if (bias) KL(c, bias_to_f32_launch(c->stream, (const __half*)bias, N, b32, gbn, 0));
-  IgemmParams p{};
-  p.nseg = 1;
-  p.seg[0] = {0, 0, 0, 0, Kpad / 64};
-  p.out = out;
-  p.out_f32 = geglu ? 0 : !out_f16;
-  p.ldo = geglu ? N / 2 : N;
-  p.bias = b32; p.bias_bstride = 0;
-  p.res = geglu ? nullptr : residual; p.ldr = N;
-  IgemmOperands o{(const __half*)x, 1, 1, M, K, K, nullptr, 0, 0, 0, 0, 0, wt, N, Kpad};
-  int r = igemm_configure(p, o, M, 1, 1, geglu ? IGEMM_GEGLU : IGEMM_LINEAR, gbn);
-  if (r) return fail(c, r, "igemm configuration failed");
-  KL(c, igemm_launch(c->stream, p));
-  return 0;
+  const IgemmOperands o{(const __half*)x, 1, 1, M, K, K, nullptr, 0, 0, 0, 0, 0, wt, N, Kpad};
+  return igemm_run(c, o, {{0, 0, 0, 0, Kpad / 64}}, 1, M, 1, geglu ? IGEMM_GEGLU : IGEMM_LINEAR, gbn, out, geglu ? 0 : !out_f16,
+                   geglu ? N / 2 : N, b32, geglu ? nullptr : residual, N);
 }
 
 extern "C" int sdxl_op_conv2d(sdxl_ctx* c, const float* x, const sdxl_half* w, const sdxl_half* bias, int B, int H, int W, int Cin,
@@ -1619,34 +1499,20 @@ extern "C" int sdxl_op_conv2d(sdxl_ctx* c, const float* x, const sdxl_half* w, c
   if (!wt || !a16 || (bias && !b32)) return fail(c, 5322, "temporary allocation failed");
   KL(c, repack_conv_launch(c->stream, (const __half*)w, Cout, Cin, ksize, ksize, wt, Ktot, 0, Ipad));
   if (bias) KL(c, bias_to_f32_launch(c->stream, (const __half*)bias, Cout, b32, 0, 0));
-  IgemmParams p{};
-  int Ho = Hi, Wo = Wi;
-  ActView a{a16, B, Hi, Wi, Cin};
-  p.nseg = 0;
+  int Ho = Hi, Wo = Wi, Ba = B;   // output extent; images of the A operand
+  std::vector<IgemmSeg> segs;
   if (stride == 2) {
     if ((H & 1) || (W & 1)) return fail(c, 5323, "sdxl_op_conv2d: stride 2 needs even H, W");
     KL(c, phase_split_launch(c->stream, x, B, H, W, Cin, a16));
-    Ho = H / 2; Wo = W / 2;
-    a = ActView{a16, 4 * B, Ho, Wo, Cin};
-    for (int kh = 0; kh < 3; ++kh)
-      for (int kw = 0; kw < 3; ++kw) {
-        const int ph = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
-        p.seg[p.nseg++] = {0, (int16_t)((kw == 0) ? -1 : 0), (int16_t)((kh == 0) ? -1 : 0), (int16_t)((ph * 2 + pw) * B), Ipad / 64};
-      }
+    Ho = H / 2; Wo = W / 2; Ba = 4 * B;
+    segs = stride2_taps(B, Ipad / 64);
   } else {
     if (upsample) KL(c, upsample2x_launch(c->stream, x, B, H, W, Cin, a16));
     else KL(c, cast_f32_to_f16_launch(c->stream, x, (size_t)B * H * W * Cin, a16));
-    const int pad = ksize / 2;
-    for (int kh = 0; kh < ksize; ++kh)
-      for (int kw = 0; kw < ksize; ++kw) p.seg[p.nseg++] = {0, (int16_t)(kw - pad), (int16_t)(kh - pad), 0, Ipad / 64};
+    segs = conv_taps(ksize, Ipad / 64);
   }
-  p.out = out; p.out_f32 = 1; p.ldo = Cout;
-  p.bias = b32; p.bias_bstride = 0; p.res = nullptr; p.ldr = 0;
-  IgemmOperands o{a.p, a.Bn, a.H, a.W, a.C, a.C, nullptr, 0, 0, 0, 0, 0, wt, Cout, Ktot};
-  int r = igemm_configure(p, o, Wo, Ho, B, IGEMM_LINEAR, 0);
-  if (r) return fail(c, r, "igemm configuration failed");
-  KL(c, igemm_launch(c->stream, p));
-  return 0;
+  const IgemmOperands o{a16, Ba, Ho, Wo, Cin, Cin, nullptr, 0, 0, 0, 0, 0, wt, Cout, Ktot};
+  return igemm_run(c, o, segs, Ho, Wo, B, IGEMM_LINEAR, 0, out, 1, Cout, b32, nullptr, 0);
 }
 
 extern "C" int sdxl_op_group_norm(sdxl_ctx* c, const float* x1, int C1, const float* x2, int C2, int B, int HW, int n_group,
@@ -1675,147 +1541,5 @@ extern "C" int sdxl_op_timestep_embedding(sdxl_ctx* c, const int32_t* t_host, in
   CU(c, cudaMemcpyAsync(td, t_host, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
   KL(c, timestep_embedding_launch(c->stream, td, n, dim, (float)max_period, out));
   CU(c, cudaStreamSynchronize(c->stream));  // t_host is pageable caller memory
-  return 0;
-}
-
-// Diagnostics: clock64 stamps of CTA 0 of one attention launch on synthetic data (tools/attn_timeline.py).
-// stamps_host[3][256][4]: role 0/1 = softmax slot A/B (one warp's lane 0): {S ready, exp phase done, P handed over, item written
-// back}; role 2 = MMA issuer: {P_A ready, P V_A + Q K_A issued, P_B ready, P V_B + Q K_B issued}; per key block, in clocks.
-extern "C" int sdxl_dbg_attention_timeline(sdxl_ctx* c, int B, int T, int S, int n_head, long long* stamps_host) {
-  if (!c || !stamps_host) return -1;
-  CU(c, cudaSetDevice(c->device));
-  TmpBufs Tm(c->stream);
-  const int C = n_head * 64;
-  __half* q = (__half*)Tm.get((size_t)B * T * C * 2);
-  __half* k = (__half*)Tm.get((size_t)B * S * C * 2);
-  __half* v = (__half*)Tm.get((size_t)B * S * C * 2);
-  __half* o = (__half*)Tm.get((size_t)B * T * C * 2);
-  long long* dbg = (long long*)Tm.get(3 * 1024 * 8);
-  if (!q || !k || !v || !o || !dbg) return fail(c, 5400, "temporary allocation failed");
-  CU(c, cudaMemsetAsync(q, 0, (size_t)B * T * C * 2, c->stream));
-  CU(c, cudaMemsetAsync(k, 0, (size_t)B * S * C * 2, c->stream));
-  CU(c, cudaMemsetAsync(v, 0, (size_t)B * S * C * 2, c->stream));
-  CU(c, cudaMemsetAsync(dbg, 0, 3 * 1024 * 8, c->stream));
-  AttnParams p{};
-  p.T = T; p.S = S; p.n_head = n_head; p.B = B;
-  p.out = o; p.ldo = C;
-  p.scale_log2e = (float)(1.4426950408889634 / sqrt(64.0));
-  int r = make_tmap_rows(&p.tmQ, q, T, B, C, C);
-  if (!r) r = make_tmap_rows(&p.tmK, k, S, B, C, C);
-  if (!r) r = make_tmap_rows(&p.tmV, v, S, B, C, C);
-  if (r) return fail(c, r, "tensor map creation failed");
-  for (int i = 0; i < 3; ++i) KL(c, attention_launch(c->stream, p));
-  p.dbg = dbg;
-  KL(c, attention_launch(c->stream, p));
-  CU(c, cudaMemcpyAsync(stamps_host, dbg, 3 * 1024 * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  return 0;
-}
-
-// Diagnostics: in-kernel timeline (%globaltimer, ns) of CTA 0 of one igemm launch on a synthetic [M,K]x[K,N] problem.
-// stamps_host[0..6] = prologue done, dependencies resolved, first operands landed, first accumulator complete,
-// first epilogue done, producer done, all roles done; stamps_host[7] = CUDA-event duration of the launch in ns.
-// Launch ramp / drain of back-to-back launches of one GEMM (programmatic dependent launch, eager): every CTA stamps its entry, the end of
-// its prologue, the moment its dependencies are resolved and its exit. out_host: n_launch x 8 = {first, last} x {entry, prologue done,
-// dependencies resolved, exit} in ns relative to the first entry of launch 0; out_host[n_launch * 8] = grid size.
-extern "C" int sdxl_dbg_igemm_gaps(sdxl_ctx* c, int M, int K, int N, int with_residual, int n_launch, int64_t* out_host) {
-  if (!c || !out_host || n_launch < 1 || n_launch > 16) return -1;
-  TmpBufs T(c->stream);
-  const int Kpad = (K + 63) / 64 * 64;
-  __half* x = (__half*)T.get((size_t)M * K * 2);
-  __half* w = (__half*)T.get((size_t)N * Kpad * 2);
-  float* bias = (float*)T.get((size_t)N * 4);
-  float* res = (float*)T.get((size_t)M * N * 4);
-  void* out = T.get((size_t)M * N * 4);
-  const size_t per = 256 * 8;   // stamps per launch (grid <= 256 CTAs)
-  unsigned long long* dbg = (unsigned long long*)T.get((size_t)n_launch * per * 8);
-  if (!x || !w || !bias || !res || !out || !dbg) return fail(c, 5400, "temporary allocation failed");
-  CU(c, cudaMemsetAsync(x, 0, (size_t)M * K * 2, c->stream));
-  CU(c, cudaMemsetAsync(w, 0, (size_t)N * Kpad * 2, c->stream));
-  CU(c, cudaMemsetAsync(bias, 0, (size_t)N * 4, c->stream));
-  CU(c, cudaMemsetAsync(res, 0, (size_t)M * N * 4, c->stream));
-  CU(c, cudaMemsetAsync(dbg, 0, (size_t)n_launch * per * 8, c->stream));
-  IgemmParams p{};
-  p.nseg = 1;
-  p.seg[0] = {0, 0, 0, 0, Kpad / 64};
-  p.out = out; p.out_f32 = 1; p.ldo = N;
-  p.bias = bias; p.bias_bstride = 0;
-  p.res = with_residual ? res : nullptr; p.ldr = N;
-  IgemmOperands o{x, 1, 1, M, K, K, nullptr, 0, 0, 0, 0, 0, w, N, Kpad};
-  int r = igemm_configure(p, o, M, 1, 1, IGEMM_LINEAR, 0);
-  if (r) return fail(c, r, "igemm configuration failed");
-  for (int i = 0; i < 3; ++i) KL(c, igemm_launch(c->stream, p));
-  for (int i = 0; i < n_launch; ++i) {
-    p.dbg_all = dbg + (size_t)i * per;
-    KL(c, igemm_launch(c->stream, p));
-  }
-  std::vector<unsigned long long> h((size_t)n_launch * per);
-  CU(c, cudaMemcpyAsync(h.data(), dbg, h.size() * 8, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  int grid = 0;
-  while (grid < 256 && h[(size_t)grid * 8] != 0) ++grid;
-  const unsigned long long t0 = [&] { unsigned long long m = ~0ull; for (int b = 0; b < grid; ++b) m = std::min(m, h[(size_t)b * 8]); return m; }();
-  for (int i = 0; i < n_launch; ++i)
-    for (int k = 0; k < 8; ++k) {
-      unsigned long long lo = ~0ull, hi = 0;
-      for (int b = 0; b < grid; ++b) {
-        const unsigned long long v = h[(size_t)i * per + (size_t)b * 8 + k];
-        lo = std::min(lo, v); hi = std::max(hi, v);
-      }
-      out_host[i * 16 + 2 * k] = (int64_t)(lo - t0);
-      out_host[i * 16 + 2 * k + 1] = (int64_t)(hi - t0);
-    }
-  out_host[n_launch * 16] = grid;
-  return 0;
-}
-
-extern "C" int sdxl_dbg_igemm_timeline(sdxl_ctx* c, int M, int K, int N, int geglu, int with_residual, uint64_t* stamps_host) {
-  if (!c || !stamps_host) return -1;
-  TmpBufs T(c->stream);
-  const int Kpad = (K + 63) / 64 * 64;
-  int gbn = geglu ? geglu_bn_for(N / 2) : 0;
-  __half* x = (__half*)T.get((size_t)M * K * 2);
-  __half* w = (__half*)T.get((size_t)N * Kpad * 2);
-  float* bias = (float*)T.get((size_t)N * 4);
-  float* res = (float*)T.get((size_t)M * N * 4);
-  void* out = T.get((size_t)M * N * 4);
-  unsigned long long* dbg = (unsigned long long*)T.get(16 * 8);
-  if (!x || !w || !bias || !res || !out || !dbg) return fail(c, 5400, "temporary allocation failed");
-  CU(c, cudaMemsetAsync(x, 0, (size_t)M * K * 2, c->stream));
-  CU(c, cudaMemsetAsync(w, 0, (size_t)N * Kpad * 2, c->stream));
-  CU(c, cudaMemsetAsync(bias, 0, (size_t)N * 4, c->stream));
-  CU(c, cudaMemsetAsync(res, 0, (size_t)M * N * 4, c->stream));
-  CU(c, cudaMemsetAsync(dbg, 0, 128, c->stream));
-  IgemmParams p{};
-  p.nseg = 1;
-  p.seg[0] = {0, 0, 0, 0, Kpad / 64};
-  p.out = out; p.out_f32 = geglu ? 0 : 1; p.ldo = geglu ? N / 2 : N;
-  p.bias = bias; p.bias_bstride = 0;
-  p.res = (geglu || !with_residual) ? nullptr : res; p.ldr = N;
-  IgemmOperands o{x, 1, 1, M, K, K, nullptr, 0, 0, 0, 0, 0, w, N, Kpad};
-  int r = igemm_configure(p, o, M, 1, 1, geglu ? IGEMM_GEGLU : IGEMM_LINEAR, gbn);
-  if (r) return fail(c, r, "igemm configuration failed");
-  cudaEvent_t e0, e1;
-  CU(c, cudaEventCreate(&e0));
-  CU(c, cudaEventCreate(&e1));
-  if (getenv("SDXL_B200_DBG_MODE")) p.dbg_mode = atoi(getenv("SDXL_B200_DBG_MODE"));
-  if (getenv("SDXL_B200_DBG_NST")) p.nstages = atoi(getenv("SDXL_B200_DBG_NST"));
-  for (int i = 0; i < 3; ++i) KL(c, igemm_launch(c->stream, p));
-  p.dbg = dbg;
-  CU(c, cudaEventRecord(e0, c->stream));
-  KL(c, igemm_launch(c->stream, p));
-  CU(c, cudaEventRecord(e1, c->stream));
-  unsigned long long hostbuf[16];
-  CU(c, cudaMemcpyAsync(hostbuf, dbg, 128, cudaMemcpyDeviceToHost, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1);
-  for (int i = 0; i < 7; ++i) stamps_host[i] = hostbuf[i];
-  fprintf(stderr, "  epi block0: tmem_ld %llu ns, st.shared+sync %llu ns, phase2 %llu ns (since acc ready: %llu)\n",
-          hostbuf[10] - hostbuf[9], hostbuf[11] - hostbuf[10], hostbuf[12] - hostbuf[11], hostbuf[9] - hostbuf[3]);
-  stamps_host[7] = (uint64_t)(ms * 1e6);
-  stamps_host[8] = (uint64_t)p.BN | ((uint64_t)p.pair << 16) | ((uint64_t)p.CM << 20) | ((uint64_t)p.CN << 24) | ((uint64_t)p.nstages << 28);
-  cudaEventDestroy(e0);
-  cudaEventDestroy(e1);
   return 0;
 }

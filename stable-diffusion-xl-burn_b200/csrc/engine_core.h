@@ -56,12 +56,23 @@ static int fail(sdxl_ctx* c, int code, const char* fmt, ...) {
   } while (0)
 
 // ================================================================================================
-// device arena (bump allocator over one cudaMalloc)
+// device arena (bump allocator over one cudaMalloc, freed with the arena)
 // ================================================================================================
 struct Arena {
   uint8_t* base = nullptr;
   size_t cap = 0, off = 0;
   bool measure = false;  // dry run: only count
+  Arena() = default;
+  Arena(Arena&& o) noexcept : base(o.base), cap(o.cap), off(o.off), measure(o.measure) { o.base = nullptr; o.cap = o.off = 0; }
+  Arena& operator=(Arena&& o) noexcept {
+    if (this != &o) {
+      release();
+      base = o.base; cap = o.cap; off = o.off; measure = o.measure;
+      o.base = nullptr; o.cap = o.off = 0;
+    }
+    return *this;
+  }
+  ~Arena() { release(); }
   int init(size_t bytes) {
     release();
     if (cudaMalloc((void**)&base, bytes) != cudaSuccess) return 1;
@@ -158,7 +169,6 @@ struct AdapterState {
 };
 
 struct Loader {
-  void* owner;  // unused by the helpers; kept so that front ends can tag a loader
   sdxl_ctx* c;
   const PackView* pv;
   Arena* A;
@@ -175,6 +185,17 @@ struct Loader {
     if (!e) { err = fail(c, 4001, "weight pack: missing tensor '%s'", name.c_str()); return nullptr; }
     if (e->dtype != 0) { err = fail(c, 4002, "weight pack: tensor '%s' must be f16", name.c_str()); return nullptr; }
     if ((int)e->ndim != ndim) { err = fail(c, 4003, "weight pack: tensor '%s' has ndim %u, expected %d", name.c_str(), e->ndim, ndim); return nullptr; }
+    return e;
+  }
+  // `path`/weight, an OIHW f16 conv weight of shape [O, I, ks, ks]
+  const PackEntry* conv_weight(const std::string& path, int O, int I, int ks) {
+    const PackEntry* e = need(path + "/weight", 4);
+    if (e && ((int)e->shape[0] != O || (int)e->shape[1] != I || (int)e->shape[2] != ks || (int)e->shape[3] != ks)) {
+      err = fail(c, 4007, "weight pack: '%s/weight' has shape [%llu,%llu,%llu,%llu], expected [%d,%d,%d,%d]", path.c_str(),
+                 (unsigned long long)e->shape[0], (unsigned long long)e->shape[1], (unsigned long long)e->shape[2],
+                 (unsigned long long)e->shape[3], O, I, ks, ks);
+      return nullptr;
+    }
     return e;
   }
   const __half* ptr(const PackEntry* e) { return (const __half*)(pv->dev + e->offset); }
@@ -219,12 +240,8 @@ struct Loader {
     cv.I = I; cv.O = O; cv.ks = 3; cv.Ipad = pad64(I); cv.Ktot = 4 * cv.Ipad;
     cv.wup = A->get<__half>((size_t)4 * O * cv.Ktot);
     if (!cv.wup) { err = fail(c, 4005, "weight arena exhausted"); return cv; }
-    const PackEntry* e = need(path + "/weight", 4);
+    const PackEntry* e = conv_weight(path, O, I, 3);
     if (!e) return cv;
-    if ((int)e->shape[0] != O || (int)e->shape[1] != I || e->shape[2] != 3 || e->shape[3] != 3) {
-      err = fail(c, 4007, "weight pack: '%s/weight' must be [%d,%d,3,3]", path.c_str(), O, I);
-      return cv;
-    }
     if (!A->measure) { int r = repack_upconv_launch(st, ptr(e), O, I, cv.wup, cv.Ipad); if (r) err = fail(c, r, "repack_upconv failed"); }
     {
       WSlot s;
@@ -241,6 +258,35 @@ struct Loader {
     n.b = vec_f32(path + "/bias", C);
     return n;
   }
+  // 3x3 conv with few input channels for the CUDA-core first-conv kernel: OIHW f16 -> [O][kh][kw][I] f32, bias f32
+  int conv_f32(const std::string& path, int I, int O, float*& w, float*& b) {
+    const PackEntry* e = conv_weight(path, O, I, 3);
+    if (!e) return err;
+    const size_t n = (size_t)O * 9 * I;
+    __half* tmp = A->get<__half>(n);
+    w = A->get<float>(n);
+    if (!tmp || !w) return err = fail(c, 4005, "weight arena exhausted");
+    if (!A->measure) {
+      int r = repack_conv_launch(st, ptr(e), O, I, 3, 3, tmp, 9 * I, 0, I);
+      if (!r) r = cast_f16_to_f32_launch(st, tmp, n, w);
+      if (r) return err = fail(c, r, "%s repack failed", path.c_str());
+    }
+    WSlot s;
+    s.base = w; s.conv = 1; s.f32 = 1; s.N = O; s.I = I; s.ks = 3; s.ld = 9 * I; s.Ipad = I;
+    record(path, s, n * sizeof(float));
+    b = vec_f32(path + "/bias", O);
+    return err;
+  }
+  // 1x1 conv OIHW f16 [O, I, 1, 1] -> f32 matrix [O][I], bias f32 (CUDA-core kernels)
+  int mat_f32(const std::string& path, int I, int O, float*& w, float*& b) {
+    const PackEntry* e = conv_weight(path, O, I, 1);
+    if (!e) return err;
+    w = A->get<float>((size_t)O * I);
+    if (!w) return err = fail(c, 4005, "weight arena exhausted");
+    if (!A->measure) { int r = cast_f16_to_f32_launch(st, ptr(e), (size_t)O * I, w); if (r) return err = fail(c, r, "%s cast failed", path.c_str()); }
+    b = vec_f32(path + "/bias", O);
+    return err;
+  }
   // conv OIHW -> [O, ks*ks*Ipad (+ I2pad)]
   // Opad > O: the matrix (and bias) get zero rows up to Opad so the GEMM's N is a multiple of 4 (cv.O = Opad).
   Conv conv(const std::string& path, int I, int O, int ks, const std::string& skip_path = "", int I2 = 0, int Opad = 0) {
@@ -254,14 +300,8 @@ struct Loader {
       err = fail(c, 4011, "memset failed");
       return cv;
     }
-    const PackEntry* e = need(path + "/weight", 4);
+    const PackEntry* e = conv_weight(path, O, I, ks);
     if (!e) return cv;
-    if ((int)e->shape[0] != O || (int)e->shape[1] != I || (int)e->shape[2] != ks || (int)e->shape[3] != ks) {
-      err = fail(c, 4007, "weight pack: '%s/weight' has shape [%llu,%llu,%llu,%llu], expected [%d,%d,%d,%d]", path.c_str(),
-                 (unsigned long long)e->shape[0], (unsigned long long)e->shape[1], (unsigned long long)e->shape[2],
-                 (unsigned long long)e->shape[3], O, I, ks, ks);
-      return cv;
-    }
     if (!A->measure) { int r = repack_conv_launch(st, ptr(e), O, I, ks, ks, cv.w, cv.Ktot, 0, cv.Ipad); if (r) err = fail(c, r, "repack_conv failed"); }
     {
       WSlot s;
@@ -282,9 +322,8 @@ struct Loader {
       cv.b = vec_f32(path + "/bias", O);
     }
     if (I2) {
-      const PackEntry* s = need(skip_path + "/weight", 4);
+      const PackEntry* s = conv_weight(skip_path, O, I2, 1);
       if (!s) return cv;
-      if ((int)s->shape[0] != O || (int)s->shape[1] != I2 || s->shape[2] != 1 || s->shape[3] != 1) { err = fail(c, 4008, "weight pack: '%s/weight' bad shape", skip_path.c_str()); return cv; }
       const PackEntry* sb = need(skip_path + "/bias", 1);
       if (!sb) return cv;
       if (!A->measure) {
@@ -333,6 +372,41 @@ static int parse_pack(sdxl_ctx* c, const void* pack, size_t bytes, int on_device
     pv.t[name] = e[i];
   }
   return 0;
+}
+
+// Parses a weight pack, makes it device-resident for the call (host packs are uploaded to a temporary copy) and runs fn(pv);
+// the stream is synchronised before the copy is freed.
+template <typename Fn>
+static int with_device_pack(sdxl_ctx* c, const void* pack, size_t bytes, int pack_on_device, Fn fn) {
+  PackView pv;
+  std::vector<uint8_t> table;
+  int r = parse_pack(c, pack, bytes, pack_on_device, pv, table);
+  if (r) return r;
+  void* dev_pack = nullptr;
+  if (pack_on_device) {
+    pv.dev = (const uint8_t*)pack;
+  } else {
+    CU(c, cudaMalloc(&dev_pack, bytes));
+    cudaError_t e = cudaMemcpyAsync(dev_pack, pack, bytes, cudaMemcpyHostToDevice, c->stream);
+    if (e != cudaSuccess) { cudaFree(dev_pack); return fail(c, (int)e, "pack upload failed"); }
+    pv.dev = (const uint8_t*)dev_pack;
+  }
+  r = fn((const PackView&)pv);
+  cudaError_t se = cudaStreamSynchronize(c->stream);
+  if (dev_pack) cudaFree(dev_pack);
+  if (!r && se != cudaSuccess) r = fail(c, (int)se, "weight re-layout failed: %s", cudaGetErrorString(se));
+  return r;
+}
+
+// Loads a model's weights: pass 1 measures, pass 2 builds into the model's weight arena m->warena.
+template <typename M>
+static int build_two_pass(M* m, const PackView& pv, int (*build)(M*, const PackView&, Arena&)) {
+  Arena meas;
+  meas.measure = true;
+  int r = build(m, pv, meas);
+  if (!r && m->warena.init(meas.off + (1 << 20))) r = fail(m->ctx, 4203, "cannot allocate %zu bytes for weights", meas.off);
+  if (!r) r = build(m, pv, m->warena);
+  return r;
 }
 
 // ================================================================================================
@@ -386,12 +460,70 @@ struct Plan {
   ~Plan() {
     if (gexec) cudaGraphExecDestroy(gexec);
     if (graph) cudaGraphDestroy(graph);
-    arena.release();
   }
 };
 
+// (Re)builds `plan` for new shapes: build(P, A) runs once against a measuring arena, then against P->arena sized by the
+// measurement. Dims are the plan's cache keys; on failure the plan is dropped.
+template <typename Fn>
+static int build_plan(sdxl_ctx* c, std::unique_ptr<Plan>& plan, int Bf, int Bx, int h, int w, Fn build) {
+  CU(c, cudaStreamSynchronize(c->stream));   // the old plan may still be in flight
+  plan.reset(new Plan());
+  Plan* P = plan.get();
+  P->Bf = Bf; P->Bx = Bx; P->h = h; P->w = w;
+  Arena meas;
+  meas.measure = true;
+  int r = build(P, &meas);
+  if (!r && P->arena.init(meas.off + (1 << 20))) r = fail(c, 5011, "cannot allocate %zu bytes of workspace", meas.off);
+  if (!r) r = build(P, &P->arena);
+  if (r) plan.reset();
+  return r;
+}
+
 struct ActView { const __half* p; int Bn, H, W, C; };
-struct F32View { float* p; int C; };  // [Bf, HW, C]
+
+// Taps of a ks x ks stride-1 conv with padding ks/2 on A source `map`, in weight-column order (kh, kw).
+static std::vector<IgemmSeg> conv_taps(int ks, int nkb, int map = 0) {
+  std::vector<IgemmSeg> segs;
+  for (int kh = 0; kh < ks; ++kh)
+    for (int kw = 0; kw < ks; ++kw) segs.push_back({(int16_t)map, (int16_t)(kw - ks / 2), (int16_t)(kh - ks / 2), 0, nkb});
+  return segs;
+}
+// Taps of a 3x3 stride-2 pad-1 conv (the UNet's Downsample) on the phase split of its input, [4][Bn][H/2][W/2][C]
+// (phase_split_launch): tap kh reads input row 2i + kh - 1, i.e. phase (kh != 1) at row offset -1 for kh = 0; same for kw.
+static std::vector<IgemmSeg> stride2_taps(int Bn, int nkb) {
+  std::vector<IgemmSeg> segs;
+  for (int kh = 0; kh < 3; ++kh)
+    for (int kw = 0; kw < 3; ++kw) {
+      const int ph = (kh == 1) ? 0 : 1, pw = (kw == 1) ? 0 : 1;
+      segs.push_back({0, (int16_t)((kw == 0) ? -1 : 0), (int16_t)((kh == 0) ? -1 : 0), (int16_t)((ph * 2 + pw) * Bn), nkb});
+    }
+  return segs;
+}
+
+// Fills the segments and the epilogue of p and configures it for the operands o (pixel box, N tile, pipeline depth,
+// tensor maps). Output image outB x outH x outW, row pitch ldo; bias index b * bias_bstride + n.
+static int igemm_setup(sdxl_ctx* c, IgemmParams& p, const IgemmOperands& o, const std::vector<IgemmSeg>& segs, int outH, int outW,
+                       int outB, int mode, int geglu_bn, void* out, int out_f32, int ldo, const float* bias, int bias_bstride,
+                       const float* res, int ldr) {
+  if (segs.size() > (size_t)IGEMM_MAX_SEG) return fail(c, 5002, "too many igemm segments");
+  p.nseg = (int)segs.size();
+  for (int i = 0; i < p.nseg; ++i) p.seg[i] = segs[i];
+  p.out = out; p.out_f32 = out_f32; p.ldo = ldo;
+  p.bias = bias; p.bias_bstride = bias_bstride;
+  p.res = res; p.ldr = ldr;
+  int r = igemm_configure(p, o, outW, outH, outB, mode, geglu_bn);
+  if (r) return fail(c, r, "igemm configuration failed (N=%d K=%d)", o.N, o.Ktot);
+  return 0;
+}
+// One eager implicit-GEMM launch on the ctx stream (operator entry points, conditioning hoist, hint encoder).
+static int igemm_run(sdxl_ctx* c, const IgemmOperands& o, const std::vector<IgemmSeg>& segs, int outH, int outW, int outB, int mode,
+                     int geglu_bn, void* out, int out_f32, int ldo, const float* bias, const float* res, int ldr) {
+  IgemmParams p{};
+  if (int r = igemm_setup(c, p, o, segs, outH, outW, outB, mode, geglu_bn, out, out_f32, ldo, bias, 0, res, ldr)) return r;
+  KL(c, igemm_launch(c->stream, p));
+  return 0;
+}
 
 struct PlanBuilder {
   sdxl_ctx* c;
@@ -420,24 +552,14 @@ struct PlanBuilder {
     if (err) return;
     Op op{};
     op.kind = OP_IGEMM;
-    IgemmParams& p = op.ig;
-    p.nseg = (int)segs.size();
-    if (p.nseg > IGEMM_MAX_SEG) { err = fail(c, 5002, "too many igemm segments"); return; }
-    for (int i = 0; i < p.nseg; ++i) p.seg[i] = segs[i];
-    p.out = out; p.out_f32 = out_f32; p.ldo = ldo;
-    p.bias = bias; p.bias_bstride = bias_bstride;
-    p.res = res; p.ldr = ldr;
-    if (!A->measure) {
-      IgemmOperands o{a0.p, a0.Bn, a0.H, a0.W, a0.C, a0.C, a1 ? a1->p : nullptr, a1 ? a1->Bn : 0, a1 ? a1->H : 0,
-                      a1 ? a1->W : 0, a1 ? a1->C : 0, a1 ? a1->C : 0, W, N, Ktot};
-      int r = igemm_configure(p, o, outW, outH, outB, mode, geglu_bn);
-      if (r) { err = fail(c, r, "igemm configuration failed (N=%d K=%d)", N, Ktot); return; }
+    if (!A->measure) {   // a measuring arena hands out fake addresses: no tensor maps
+      const IgemmOperands o{a0.p, a0.Bn, a0.H, a0.W, a0.C, a0.C, a1 ? a1->p : nullptr, a1 ? a1->Bn : 0, a1 ? a1->H : 0,
+                            a1 ? a1->W : 0, a1 ? a1->C : 0, a1 ? a1->C : 0, W, N, Ktot};
+      if ((err = igemm_setup(c, op.ig, o, segs, outH, outW, outB, mode, geglu_bn, out, out_f32, ldo, bias, bias_bstride, res, ldr))) return;
     }
-    {
-      double kb = 0;
-      for (int i = 0; i < p.nseg; ++i) kb += p.seg[i].nkb;
-      op.flops_exec = 2.0 * outB * outH * (double)outW * N * kb * 64.0;
-    }
+    double kb = 0;
+    for (const IgemmSeg& s : segs) kb += s.nkb;
+    op.flops_exec = 2.0 * outB * outH * (double)outW * N * kb * 64.0;
     P->ops.push_back(op);
   }
   // names the reference block the following launches belong to
@@ -488,9 +610,7 @@ struct PlanBuilder {
   // 3x3 stride-1 conv (+ optional fused 1x1 skip segment on a1)
   void conv3(const ActView& a, const ActView* skip, const Conv& cv, float* out, const float* bias, int bias_bstride,
              const float* res) {
-    std::vector<IgemmSeg> segs;
-    for (int kh = 0; kh < 3; ++kh)
-      for (int kw = 0; kw < 3; ++kw) segs.push_back({0, (int16_t)(kw - 1), (int16_t)(kh - 1), 0, cv.Ipad / 64});
+    std::vector<IgemmSeg> segs = conv_taps(3, cv.Ipad / 64);
     if (skip) segs.push_back({1, 0, 0, 0, cv.I2pad / 64});
     igemm(a, skip, segs, cv.w, cv.O, cv.Ktot, a.H, a.W, a.Bn, IGEMM_LINEAR, 0, out, 1, cv.O, bias, bias_bstride, res, cv.O);
     add_flops(2.0 * a.Bn * a.H * a.W * (double)cv.O * (9.0 * cv.I + cv.I2));
@@ -593,9 +713,8 @@ static int run_plan_ops(sdxl_ctx* c, Plan* P) {
   return r;
 }
 
-// Per-kernel-kind device time of one plan execution, measured with CUDA events on the ctx stream (eager launches, one event
-// pair per op). kinds: see OpKind. Arrays must hold 16 entries.
-static int profile_plan_impl(sdxl_ctx* c, Plan* P, double* ms_by_kind, double* flops_by_kind, int* launches_by_kind) {
+// Runs every op of the plan eagerly on the ctx stream between CUDA event pairs; ms[i] = device time of op i.
+static int time_plan_ops(sdxl_ctx* c, Plan* P, std::vector<float>& ms) {
   const size_t n = P->ops.size();
   std::vector<cudaEvent_t> ev(n + 1);
   for (auto& e : ev) CU(c, cudaEventCreate(&e));
@@ -606,58 +725,49 @@ static int profile_plan_impl(sdxl_ctx* c, Plan* P, double* ms_by_kind, double* f
     if (!r && cudaEventRecord(ev[i + 1], c->stream) != cudaSuccess) r = -2;
   }
   cudaError_t se = cudaStreamSynchronize(c->stream);
-  for (int k = 0; k < SDXL_PROFILE_KINDS; ++k) { ms_by_kind[k] = 0; flops_by_kind[k] = 0; launches_by_kind[k] = 0; }
+  ms.assign(n, 0.f);
   if (!r && se == cudaSuccess)
-    for (size_t i = 0; i < n; ++i) {
-      float ms = 0;
-      cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-      const int k = (int)P->ops[i].kind;
-      if (k < 0 || k >= SDXL_PROFILE_KINDS) continue;
-      ms_by_kind[k] += ms;
-      flops_by_kind[k] += P->ops[i].flops;
-      launches_by_kind[k] += (P->ops[i].kind == OP_GN) ? 2 : 1;
-    }
+    for (size_t i = 0; i < n; ++i) cudaEventElapsedTime(&ms[i], ev[i], ev[i + 1]);
   for (auto& e : ev) cudaEventDestroy(e);
   if (se != cudaSuccess) return fail(c, (int)se, "profile run failed: %s", cudaGetErrorString(se));
   return r;
 }
 
-// Per-op dump of one eager plan execution (CUDA-event time per launch) as CSV: analysis aid for profiles/.
+// Per-kernel-kind device time of one plan execution (time_plan_ops). kinds: see OpKind. Arrays hold SDXL_PROFILE_KINDS entries.
+static int profile_plan_impl(sdxl_ctx* c, Plan* P, double* ms_by_kind, double* flops_by_kind, int* launches_by_kind) {
+  std::vector<float> ms;
+  const int r = time_plan_ops(c, P, ms);
+  for (int k = 0; k < SDXL_PROFILE_KINDS; ++k) { ms_by_kind[k] = 0; flops_by_kind[k] = 0; launches_by_kind[k] = 0; }
+  if (r) return r;
+  for (size_t i = 0; i < ms.size(); ++i) {
+    const int k = (int)P->ops[i].kind;
+    if (k < 0 || k >= SDXL_PROFILE_KINDS) continue;
+    ms_by_kind[k] += ms[i];
+    flops_by_kind[k] += P->ops[i].flops;
+    launches_by_kind[k] += (P->ops[i].kind == OP_GN) ? 2 : 1;
+  }
+  return 0;
+}
+
+// Per-op dump of one eager plan execution (time_plan_ops) as CSV: analysis aid for profiles/.
 static int profile_dump_impl(sdxl_ctx* c, Plan* P, const char* path) {
-  const size_t n = P->ops.size();
-  std::vector<cudaEvent_t> ev(n + 1);
-  for (auto& e : ev) CU(c, cudaEventCreate(&e));
-  int r = 0;
-  CU(c, cudaEventRecord(ev[0], c->stream));
-  for (size_t i = 0; i < n && !r; ++i) {
-    r = exec_op(c, P->ops[i]);
-    if (!r && cudaEventRecord(ev[i + 1], c->stream) != cudaSuccess) r = -2;
+  std::vector<float> ms;
+  if (int r = time_plan_ops(c, P, ms)) return r;
+  FILE* f = fopen(path, "w");
+  if (!f) return fail(c, -3, "cannot open %s", path);
+  fprintf(f, "op,kind,us,gflop,tflops,M_tiles,N,BN,Kblocks,T,S,heads\n");
+  for (size_t i = 0; i < ms.size(); ++i) {
+    const Op& o = P->ops[i];
+    int mt = 0, N = 0, BN = 0, kb = 0, T = 0, S = 0, H = 0;
+    if (o.kind == OP_IGEMM) {
+      mt = o.ig.tilesW * o.ig.tilesH * o.ig.tilesB; N = o.ig.N; BN = o.ig.BN;
+      for (int s2 = 0; s2 < o.ig.nseg; ++s2) kb += o.ig.seg[s2].nkb;
+    } else if (o.kind == OP_ATTN) { T = o.at.T; S = o.at.S; H = o.at.n_head; }
+    fprintf(f, "%zu,%s,%.2f,%.3f,%.1f,%d,%d,%d,%d,%d,%d,%d\n", i, kOpNames[o.kind], ms[i] * 1e3, o.flops * 1e-9,
+            ms[i] > 0 ? o.flops / (ms[i] * 1e-3) * 1e-12 : 0.0, mt, N, BN, kb, T, S, H);
   }
-  cudaError_t se = cudaStreamSynchronize(c->stream);
-  if (!r && se == cudaSuccess) {
-    FILE* f = fopen(path, "w");
-    if (!f) r = fail(c, -3, "cannot open %s", path);
-    else {
-      fprintf(f, "op,kind,us,gflop,tflops,M_tiles,N,BN,Kblocks,T,S,heads,cluster\n");
-      for (size_t i = 0; i < n; ++i) {
-        float ms = 0;
-        cudaEventElapsedTime(&ms, ev[i], ev[i + 1]);
-        const Op& o = P->ops[i];
-        int mt = 0, N = 0, BN = 0, kb = 0, T = 0, S = 0, H = 0;
-        if (o.kind == OP_IGEMM) {
-          mt = o.ig.tilesW * o.ig.tilesH * o.ig.tilesB; N = o.ig.N; BN = o.ig.BN;
-          for (int s2 = 0; s2 < o.ig.nseg; ++s2) kb += o.ig.seg[s2].nkb;
-        } else if (o.kind == OP_ATTN) { T = o.at.T; S = o.at.S; H = o.at.n_head; }
-        fprintf(f, "%zu,%s,%.2f,%.3f,%.1f,%d,%d,%d,%d,%d,%d,%d,%dx%d\n", i, kOpNames[o.kind], ms * 1e3, o.flops * 1e-9,
-                ms > 0 ? o.flops / (ms * 1e-3) * 1e-12 : 0.0, mt, N, BN, kb, T, S, H,
-                o.kind == OP_IGEMM ? (o.ig.pair ? 9 : o.ig.CM) : 0, o.kind == OP_IGEMM ? o.ig.CN : 0);
-      }
-      fclose(f);
-    }
-  }
-  for (auto& e : ev) cudaEventDestroy(e);
-  if (se != cudaSuccess) return fail(c, (int)se, "profile run failed: %s", cudaGetErrorString(se));
-  return r;
+  fclose(f);
+  return 0;
 }
 
 struct TmpBufs {

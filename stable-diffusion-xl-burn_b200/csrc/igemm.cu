@@ -340,10 +340,6 @@ int igemm_configure(IgemmParams& p, const IgemmOperands& o, int outW, int outH, 
   p.BN = (mode == IGEMM_GEGLU) ? geglu_bn : igemm_pick_bn(m_tiles, o.N, device_sms(), false);
   if (p.BN != 64 && p.BN != 128 && p.BN != 160 && p.BN != 256) return 1010;
   p.tilesN = (mode == IGEMM_GEGLU) ? (o.N / p.BN) : ((o.N + p.BN - 1) / p.BN);
-  p.pair = 0;
-  p.CM = p.CN = 1;
-  p.a_split_dim = 0; p.a_split_ext = 0;
-  p.epi_tma = 0; p.epi_box_bytes = 0;
   int r = make_tmap_act(&p.tmA0, o.a0, o.a0Bn, o.a0H, o.a0W, o.a0C, o.a0pitch, p.Wt, p.Ht, p.Bt);
   if (!r && o.a1) r = make_tmap_act(&p.tmA1, o.a1, o.a1Bn, o.a1H, o.a1W, o.a1C, o.a1pitch, p.Wt, p.Ht, p.Bt);
   if (!r && !o.a1) p.tmA1 = p.tmA0;

@@ -90,9 +90,6 @@ struct alignas(64) IgemmParams {
   int Wt, Ht, Bt;             // A box in pixels, Wt*Ht*Bt == 128
   int W, H, Bn;               // output extents
   int tilesW, tilesH, tilesB, tilesN;
-  int pair;                   // always 0 (no paired-CTA variant); kept in the launch-plan dump
-  int CM, CN;                 // cluster shape, always 1 x 1; kept in the launch-plan dump
-  int a_split_dim, a_split_ext;  // unused (no clusters)
   int N;                      // valid output columns (GEGLU: columns of the fused [value|gate] GEMM)
   int BN;                     // N tile: 64, 128, 160 or 256
   int nstages;
@@ -108,14 +105,6 @@ struct alignas(64) IgemmParams {
   // upsample + 3x3 conv is run as four 2x2 convolutions on the original image, each writing one (row, column) parity of the
   // upsampled output: opix_row = 4W, opix_w = 2, opix_off = a*2W + b.
   int opix_row, opix_w, opix_off;
-  // unused: the epilogue stores from the accumulator registers
-  CUtensorMap tmOut, tmRes;
-  int epi_tma;
-  int epi_box_bytes;
-  unsigned fd_pm, fd_w, fd_h, fd_wh;
-  int dbg_mode;               // unused by the wgmma kernel
-  unsigned long long* dbg;    // unused by the wgmma kernel (no per-role timestamps)
-  unsigned long long* dbg_all;  // unused by the wgmma kernel
 };
 // A operand view: NHWC f16 tensor [Bn, H, W, C] with channel pitch `pitch` (elements, multiple of 8).
 int make_tmap_act(CUtensorMap* tm, const __half* base, int Bn, int H, int W, int C, int pitch, int Wt,
@@ -130,7 +119,7 @@ struct IgemmOperands {
   const __half* a1; int a1Bn, a1H, a1W, a1C, a1pitch;   // nullable second source (segments with map == 1)
   const __half* w; int N, Ktot;
 };
-// Chooses the pixel box, N tile, cluster shape and pipeline depth, and builds the TMA descriptors. The caller
+// Chooses the pixel box, N tile and pipeline depth, and builds the TMA descriptors. The caller
 // fills seg[]/nseg and the epilogue fields (out, out_f32, ldo, bias, bias_bstride, res, ldr).
 int igemm_configure(IgemmParams& p, const IgemmOperands& o, int outW, int outH, int outB, int mode, int geglu_bn);
 int igemm_launch(cudaStream_t st, IgemmParams& p);
@@ -148,7 +137,6 @@ struct AttnParams {
   __half* out;                 // [B*T, ldo]
   int ldo;
   float scale_log2e;           // (1/sqrt(d)) * log2(e)
-  long long* dbg;              // nullable: clock64 stamps of CTA 0 (sdxl_dbg_attention_timeline)
 };
 int make_tmap_rows(CUtensorMap* tm, const __half* base, int rows_per_batch, int nbatch, int cols, int pitch);
 int attention_launch(cudaStream_t st, const AttnParams& p);

@@ -84,38 +84,13 @@ static VRes load_vres(Loader& L, const std::string& path, int Cin, int Cout) {
 static int build_vae(sdxl_vae* v, const PackView& pv, Arena& A) {
   sdxl_ctx* c = v->ctx;
   const sdxl_vae_cfg& g = v->cfg;
-  Loader L{nullptr, c, &pv, &A, c->stream};
+  Loader L{c, &pv, &A, c->stream};
   const int Cl = g.latent_channels;
   v->blocks.clear();
   v->C0 = g.block_in[0];
-  // post_quant_conv: OIHW [Cl,Cl,1,1] f16 -> f32 [Cl][Cl]
-  {
-    const PackEntry* e = L.need("post_quant_conv/weight", 4);
-    if (!e) return L.err;
-    if ((int)e->shape[0] != Cl || (int)e->shape[1] != Cl || e->shape[2] != 1 || e->shape[3] != 1) return fail(c, 4301, "post_quant_conv/weight bad shape");
-    v->pq_w = A.get<float>((size_t)Cl * Cl);
-    if (!v->pq_w) return fail(c, 4005, "weight arena exhausted");
-    if (!A.measure) { int r = cast_f16_to_f32_launch(c->stream, L.ptr(e), (size_t)Cl * Cl, v->pq_w); if (r) return fail(c, r, "post_quant cast failed"); }
-    v->pq_b = L.vec_f32("post_quant_conv/bias", Cl);
-    if (L.err) return L.err;
-  }
-  // decoder/conv_in: OIHW f16 -> [O][kh][kw][I] f32 (CUDA-core kernel, exact f32 like the reference)
-  {
-    const PackEntry* e = L.need("decoder/conv_in/weight", 4);
-    if (!e) return L.err;
-    if ((int)e->shape[0] != v->C0 || (int)e->shape[1] != Cl || e->shape[2] != 3 || e->shape[3] != 3) return fail(c, 4302, "decoder/conv_in/weight bad shape");
-    const size_t n = (size_t)v->C0 * 9 * Cl;
-    __half* tmp = A.get<__half>(n);
-    v->cin_w = A.get<float>(n);
-    if (!tmp || !v->cin_w) return fail(c, 4005, "weight arena exhausted");
-    if (!A.measure) {
-      int r = repack_conv_launch(c->stream, L.ptr(e), v->C0, Cl, 3, 3, tmp, 9 * Cl, 0, Cl);
-      if (!r) r = cast_f16_to_f32_launch(c->stream, tmp, n, v->cin_w);
-      if (r) return fail(c, r, "decoder conv_in repack failed");
-    }
-    v->cin_b = L.vec_f32("decoder/conv_in/bias", v->C0);
-    if (L.err) return L.err;
-  }
+  // post_quant_conv [Cl,Cl,1,1]; decoder/conv_in on the CUDA-core kernel (exact f32 like the reference)
+  if (L.mat_f32("post_quant_conv", Cl, Cl, v->pq_w, v->pq_b)) return L.err;
+  if (L.conv_f32("decoder/conv_in", Cl, v->C0, v->cin_w, v->cin_b)) return L.err;
   const int Cm = v->C0;
   v->mid1 = load_vres(L, "decoder/mid/block_1", Cm, Cm);
   v->attn_norm = L.norm("decoder/mid/attn/norm", Cm);
@@ -147,19 +122,7 @@ static int build_vae(sdxl_vae* v, const PackView& pv, Arena& A) {
   v->eblocks.clear();
   if (v->has_enc) {
     v->EC0 = g.enc_in[0];
-    const PackEntry* e = L.need("encoder/conv_in/weight", 4);
-    if (!e) return L.err;
-    if ((int)e->shape[0] != v->EC0 || e->shape[1] != 3 || e->shape[2] != 3 || e->shape[3] != 3) return fail(c, 4320, "encoder/conv_in/weight bad shape");
-    const size_t n = (size_t)v->EC0 * 27;
-    __half* tmp = A.get<__half>(n);
-    v->ecin_w = A.get<float>(n);
-    if (!tmp || !v->ecin_w) return fail(c, 4005, "weight arena exhausted");
-    if (!A.measure) {
-      int r = repack_conv_launch(c->stream, L.ptr(e), v->EC0, 3, 3, 3, tmp, 27, 0, 3);
-      if (!r) r = cast_f16_to_f32_launch(c->stream, tmp, n, v->ecin_w);
-      if (r) return fail(c, r, "encoder conv_in repack failed");
-    }
-    v->ecin_b = L.vec_f32("encoder/conv_in/bias", v->EC0);
+    if (L.conv_f32("encoder/conv_in", 3, v->EC0, v->ecin_w, v->ecin_b)) return L.err;
     for (int i = 0; i < g.n_enc_blocks && !L.err; ++i) {
       sdxl_vae::EBlock b;
       const std::string bp = "encoder/blocks/" + std::to_string(i);
@@ -183,13 +146,7 @@ static int build_vae(sdxl_vae* v, const PackView& pv, Arena& A) {
     v->enorm_out = L.norm("encoder/norm_out", Ce);
     v->econv_out = L.conv("encoder/conv_out", Ce, Cz, 3);
     if (L.err) return L.err;
-    const PackEntry* q = L.need("quant_conv/weight", 4);
-    if (!q) return L.err;
-    if ((int)q->shape[0] != Cz || (int)q->shape[1] != Cz || q->shape[2] != 1 || q->shape[3] != 1) return fail(c, 4321, "quant_conv/weight bad shape");
-    v->qc_w = A.get<float>((size_t)Cz * Cz);
-    if (!v->qc_w) return fail(c, 4005, "weight arena exhausted");
-    if (!A.measure) { int r = cast_f16_to_f32_launch(c->stream, L.ptr(q), (size_t)Cz * Cz, v->qc_w); if (r) return fail(c, r, "quant_conv cast failed"); }
-    v->qc_b = L.vec_f32("quant_conv/bias", Cz);
+    L.mat_f32("quant_conv", Cz, Cz, v->qc_w, v->qc_b);
   }
   return L.err;
 }
@@ -197,9 +154,6 @@ static int build_vae(sdxl_vae* v, const PackView& pv, Arena& A) {
 extern "C" void sdxl_vae_destroy(sdxl_vae* v) {
   if (!v) return;
   cudaStreamSynchronize(v->ctx->stream);
-  v->plan.reset();
-  v->enc_plan.reset();
-  v->warena.release();
   delete v;
 }
 
@@ -226,28 +180,8 @@ extern "C" int sdxl_vae_load(sdxl_ctx* c, const sdxl_vae_cfg* cfg, const void* p
   std::unique_ptr<sdxl_vae> v(new sdxl_vae());
   v->ctx = c;
   v->cfg = *cfg;
-  PackView pv;
-  std::vector<uint8_t> table;
-  int r = parse_pack(c, pack, bytes, pack_on_device, pv, table);
+  int r = with_device_pack(c, pack, bytes, pack_on_device, [&](const PackView& pv) { return build_two_pass(v.get(), pv, build_vae); });
   if (r) return r;
-  void* dev_pack = nullptr;
-  if (pack_on_device) {
-    pv.dev = (const uint8_t*)pack;
-  } else {
-    CU(c, cudaMalloc(&dev_pack, bytes));
-    cudaError_t e = cudaMemcpyAsync(dev_pack, pack, bytes, cudaMemcpyHostToDevice, c->stream);
-    if (e != cudaSuccess) { cudaFree(dev_pack); return fail(c, (int)e, "pack upload failed"); }
-    pv.dev = (const uint8_t*)dev_pack;
-  }
-  Arena meas;
-  meas.measure = true;
-  r = build_vae(v.get(), pv, meas);
-  if (!r && v->warena.init(meas.off + (1 << 20))) r = fail(c, 4203, "cannot allocate %zu bytes for weights", meas.off);
-  if (!r) r = build_vae(v.get(), pv, v->warena);
-  cudaError_t se = cudaStreamSynchronize(c->stream);
-  if (dev_pack) cudaFree(dev_pack);
-  if (!r && se != cudaSuccess) r = fail(c, (int)se, "weight re-layout failed: %s", cudaGetErrorString(se));
-  if (r) { v->warena.release(); return r; }
   *out = v.release();
   return 0;
 }
@@ -412,10 +346,7 @@ static int build_vae_plan(sdxl_vae* v, Plan* P, Arena* A) {
   v->img_nhwc = B.buf<float>((size_t)Bn * H * W * 4);
   {
     ActView a{st.s_gn1, Bn, H, W, Cf};
-    std::vector<IgemmSeg> segs;
-    for (int kh = 0; kh < 3; ++kh)
-      for (int kw = 0; kw < 3; ++kw) segs.push_back({0, (int16_t)(kw - 1), (int16_t)(kh - 1), 0, v->conv_out.Ipad / 64});
-    B.igemm(a, nullptr, segs, v->conv_out.w, 4, v->conv_out.Ktot, H, W, Bn, IGEMM_LINEAR, 0, v->img_nhwc, 1, 4, v->conv_out.b, 0,
+    B.igemm(a, nullptr, conv_taps(3, v->conv_out.Ipad / 64), v->conv_out.w, 4, v->conv_out.Ktot, H, W, Bn, IGEMM_LINEAR, 0, v->img_nhwc, 1, 4, v->conv_out.b, 0,
             nullptr, 0);
     B.add_flops(2.0 * Bn * H * W * 9.0 * Cf * 3);
   }
@@ -511,18 +442,8 @@ static int vae_encode_run(sdxl_vae* v, int Bn, int H, int W, const float* image,
   if (!latent_out || (!image && !rgb)) return fail(c, -1, "null argument");
   if (Bn < 1 || H < 1 || W < 1) return fail(c, 5100, "bad encode shape B=%d H=%d W=%d", Bn, H, W);
   CU(c, cudaSetDevice(c->device));
-  if (!v->enc_plan || v->enc_plan->Bf != Bn || v->enc_plan->h != H || v->enc_plan->w != W) {
-    CU(c, cudaStreamSynchronize(c->stream));
-    v->enc_plan.reset(new Plan());
-    Plan* P = v->enc_plan.get();
-    P->Bf = Bn; P->Bx = Bn; P->h = H; P->w = W;
-    Arena meas;
-    meas.measure = true;
-    int r = build_vae_enc_plan(v, P, &meas);
-    if (!r && P->arena.init(meas.off + (1 << 20))) r = fail(c, 5011, "cannot allocate %zu bytes of workspace", meas.off);
-    if (!r) r = build_vae_enc_plan(v, P, &P->arena);
-    if (r) { v->enc_plan.reset(); return r; }
-  }
+  if (!v->enc_plan || v->enc_plan->Bf != Bn || v->enc_plan->h != H || v->enc_plan->w != W)
+    if (int r = build_plan(c, v->enc_plan, Bn, Bn, H, W, [&](Plan* P, Arena* A) { return build_vae_enc_plan(v, P, A); })) return r;
   Plan* P = v->enc_plan.get();
   const size_t npix = (size_t)Bn * H * W;
   if (image) {
@@ -562,18 +483,7 @@ static int vae_ensure_plan(sdxl_vae* v, int Bn, int h, int w) {
   sdxl_ctx* c = v->ctx;
   if (Bn < 1 || h < 1 || w < 1) return fail(c, 5100, "bad decode shape B=%d h=%d w=%d", Bn, h, w);
   if (v->plan && v->plan->Bf == Bn && v->plan->h == h && v->plan->w == w) return 0;
-  CU(c, cudaStreamSynchronize(c->stream));
-  v->plan.reset(new Plan());
-  Plan* P = v->plan.get();
-  P->Bf = Bn; P->Bx = Bn; P->h = h; P->w = w;
-  Arena meas;
-  meas.measure = true;
-  int r = build_vae_plan(v, P, &meas);
-  if (r) { v->plan.reset(); return r; }
-  if (P->arena.init(meas.off + (1 << 20))) { v->plan.reset(); return fail(c, 5011, "cannot allocate %zu bytes of workspace", meas.off); }
-  r = build_vae_plan(v, P, &P->arena);
-  if (r) { v->plan.reset(); return r; }
-  return 0;
+  return build_plan(c, v->plan, Bn, Bn, h, w, [&](Plan* P, Arena* A) { return build_vae_plan(v, P, A); });
 }
 
 static int vae_run(sdxl_vae* v, int Bn, int h, int w, const float* latent, int on_host) {

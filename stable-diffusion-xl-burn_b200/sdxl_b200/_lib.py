@@ -103,9 +103,6 @@ PROTOTYPES = {
     "sdxl_unet_plan_flops_executed": (C.c_double, [P]),
     "sdxl_unet_profile_plan": (I, [P, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(C.c_int)]),
     "sdxl_unet_profile_dump": (I, [P, C.c_char_p]),
-    "sdxl_dbg_igemm_timeline": (I, [P, I, I, I, I, I, C.POINTER(C.c_uint64)]),
-    "sdxl_dbg_igemm_gaps": (I, [P, I, I, I, I, I, C.POINTER(C.c_int64)]),
-    "sdxl_dbg_attention_timeline": (I, [P, I, I, I, I, C.POINTER(C.c_longlong)]),
     "sdxl_randn": (I, [P, P, C.c_size_t, C.c_uint64, C.c_uint64]),
     "sdxl_qkv_attention": (I, [P, P, P, P, P, I, I, I, I, I, P]),
     "sdxl_op_linear": (I, [P, P, P, P, P, I, I, I, I, I, P]),
