@@ -154,6 +154,8 @@ SDXL_API double sdxl_unet_alpha(const sdxl_unet* unet, int i);
  * the launch plan currently built for this UNet (0 before the first forward). */
 SDXL_API double sdxl_unet_plan_flops(const sdxl_unet* unet);
 SDXL_API int sdxl_unet_plan_num_ops(const sdxl_unet* unet);
+/* Number of launch plans built for this UNet so far: attachment changes that keep the plan (and its CUDA graph) leave it unchanged. */
+SDXL_API uint64_t sdxl_unet_plan_builds(const sdxl_unet* unet);
 /* FLOPs the plan's tensor-core launches actually issue: without the K/V projections hoisted to set_conditioning, with the
  * phase-decomposed upsample convolutions at their real cost and with channel / key padding (bench: `executed_flops`). */
 SDXL_API double sdxl_unet_plan_flops_executed(const sdxl_unet* unet);
@@ -371,6 +373,72 @@ SDXL_API int sdxl_unet_set_controls(sdxl_unet* unet, int n, const sdxl_control* 
 /* Test aid: the hint encoder's output hint_emb f32 NCHW [n, model_channels, H/8, W/8] of hint f32 NCHW [n, 3, H, W]; both
  * pointers are host memory if on_host. */
 SDXL_API int sdxl_controlnet_embed_hint(sdxl_controlnet* net, int n, int H, int W, const float* hint, int on_host, float* out);
+
+/* ---- CLIP vision encoder (the image encoder of IP-Adapter) -------------------------------------------------
+ * HF CLIPVisionModelWithProjection (DESIGN.md §9): x = pre_layernorm([class_embedding ; patch_conv(pixels)] + position_embedding),
+ * n_layer pre-LN blocks without a mask, image_embeds = post_layernorm(x[:, 0]) @ visual_projection. Pack (SDXLPK01), Linear weights
+ * [in, out]: patch_embedding/weight [n_state, 3, p, p], class_embedding [n_state], position_embedding/weight [T, n_state],
+ * pre_layernorm/{weight,bias}, blocks/<i>/{attn_ln, mlp_ln, attn/{query,key,value,out}, mlp/{fc1,fc2}} (the text encoder's names),
+ * post_layernorm/{weight,bias}, visual_projection [n_state, proj_dim] (no bias). T = (image_size / patch_size)^2 + 1. */
+typedef struct sdxl_clip_vision sdxl_clip_vision;
+typedef struct sdxl_clip_vision_cfg {
+  int32_t n_state, n_head, n_layer;   /* head dim n_state / n_head: a multiple of 8 up to 128 (ViT-H/14: 1280/16, bigG/14: 1664/16) */
+  int32_t mlp_dim;                    /* 5120 (ViT-H), 8192 (ViT-bigG) */
+  int32_t image_size, patch_size;     /* 224, 14 */
+  int32_t proj_dim;                   /* 1024 (ViT-H), 1280 (ViT-bigG) */
+  int32_t quick_gelu;                 /* 0: exact-erf GELU */
+} sdxl_clip_vision_cfg;
+SDXL_API int sdxl_clip_vision_load(sdxl_ctx* ctx, const sdxl_clip_vision_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
+                                   sdxl_clip_vision** out);
+SDXL_API void sdxl_clip_vision_destroy(sdxl_clip_vision* v);
+/* image_embeds_out f32 [N, proj_dim] of pixels f32 NCHW [N, 3, image_size, image_size] as CLIPImageProcessor produces them (resized,
+ * centre-cropped, normalised); both host memory if on_host. */
+SDXL_API int sdxl_clip_vision_encode(sdxl_clip_vision* v, int N, const float* pixels, int on_host, float* image_embeds_out);
+
+/* ---- IP-Adapter (image prompts) -----------------------------------------------------------------------
+ * The published IP-Adapter for SDXL, base variant (DESIGN.md §9; diffusers IPAdapterAttnProcessor2_0 + ImageProjection): an
+ * image embedding e [D] (CLIP vision image_embeds) becomes tokens_per_image tokens
+ *   tokens = LayerNorm(e @ proj + b).reshape(tokens_per_image, context_dim)           (LayerNorm eps 1e-5)
+ * and every UNet cross-attention (attn2) becomes decoupled cross-attention:
+ *   h = softmax(q K_txt^T / 8) V_txt + s_blk * softmax(q K_ip^T / 8) V_ip,   K_ip = tokens @ ip_key, V_ip = tokens @ ip_value
+ * before the out projection. Pack (SDXLPK01), Linear weights [in, out]:
+ *   image_proj/proj/{weight [D, T*context_dim], bias}, image_proj/norm/{weight, bias} [context_dim],
+ *   <transformer block path>/attn2/ip_key/weight and .../ip_value/weight [context_dim, C] for every UNet transformer block, e.g.
+ *   input_blocks/4/transformer/transformer_0/attn2/ip_key/weight.
+ * An adapter is built on one ctx and may be attached to any UNet of that ctx whose cfg equals its `unet`. The refiner is not
+ * supported. */
+typedef struct sdxl_ip_adapter sdxl_ip_adapter;
+typedef struct sdxl_ip_adapter_cfg {
+  sdxl_unet_cfg unet;            /* must equal the cfg of the UNet it is attached to; context_dim a multiple of 8 */
+  int32_t image_embed_dim;       /* D: 1024 (ViT-H/14 encoder), 1280 (ViT-bigG/14 encoder) */
+  int32_t tokens_per_image;      /* 4 */
+} sdxl_ip_adapter_cfg;
+SDXL_API int sdxl_ip_adapter_load(sdxl_ctx* ctx, const sdxl_ip_adapter_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
+                                  sdxl_ip_adapter** out);
+/* Destroying an adapter that is still attached to a UNet (sdxl_unet_set_image_prompt) is a caller error: detach first. */
+SDXL_API void sdxl_ip_adapter_destroy(sdxl_ip_adapter* adapter);
+typedef struct sdxl_image_prompt {
+  const sdxl_ip_adapter* adapter;
+  const float* embeds;             /* f32 [n_batch * n_images, D]: image i of prompt b at row b * n_images + i */
+  const float* negative_embeds;    /* same shape, or NULL: the unconditional rows use the projection of zero embeddings */
+  int32_t on_host;                 /* both pointers are host memory; borrowed for the call */
+  int32_t n_batch, n_images;       /* S_ip = n_images * tokens_per_image tokens per row, images concatenated in order */
+  float scale;                     /* s_blk of every block, unless block_scales_host is given */
+  const float* block_scales_host;  /* NULL or s_blk of each UNet transformer block in execution order (input blocks, middle, output) */
+} sdxl_image_prompt;
+/* Attaches an image prompt to the UNet (NULL detaches). Row rule: in the sampler's CFG batch [cond | uncond] of n images, cond row
+ * b uses embeds prompt b % n_batch and uncond row b negative prompt b % n_batch; a direct sdxl_unet_forward of B rows uses prompt
+ * r % n_batch for row r. Everything is validated before anything changes (ctx, cfg, n_batch >= 1, n_images >= 1, finite scales, the
+ * current conditioning batch a multiple of n_batch): on failure the previous state stays. A call with the same adapter, n_batch and
+ * n_images rewrites tokens, K/V and scales in place (same launch plan and CUDA graph); any other change rebuilds the plan at the
+ * next forward. The image K/V are recomputed whenever the conditioning is set. An attached ControlNet's attentions see text only. */
+SDXL_API int sdxl_unet_set_image_prompt(sdxl_unet* unet, const sdxl_image_prompt* prompt);
+/* Test aid: tokens f16 [n * tokens_per_image, context_dim] of embeds f32 [n, D]; both host memory if on_host. */
+SDXL_API int sdxl_ip_adapter_project(sdxl_ip_adapter* adapter, int n, const float* embeds, int on_host, sdxl_half* tokens_out);
+/* Test aid: out = softmax(q k^T / 8) v + scale * softmax(q k_ip^T / 8) v_ip per head (head dim 64); q/out [B,T,C], k/v [B,S,C],
+ * k_ip/v_ip [B,S_ip,C] f16 device memory. */
+SDXL_API int sdxl_op_ip_attention(sdxl_ctx* ctx, const sdxl_half* q, const sdxl_half* k, const sdxl_half* v, const sdxl_half* k_ip,
+                                  const sdxl_half* v_ip, int B, int T, int S, int S_ip, int C, int n_head, float scale, sdxl_half* out);
 
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),

@@ -8,6 +8,7 @@
 // One CTA per (batch, head, 128-query tile): two consumer warpgroups own 64 query rows each, one producer warp streams the
 // 128-key K / V blocks through a TMA ring. The running max is exact per key block (the row is rescaled when it grows), so
 // every probability is <= 1 before the f16 rounding.
+// attention_kernel<true> adds IP-Adapter's second key/value source (DESIGN.md §9).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -31,6 +32,66 @@ __device__ __forceinline__ uint32_t pack_half2(float a, float b) {
   return *reinterpret_cast<uint32_t*>(&t);
 }
 
+// One 128-key block j (key rows kb * 128 .. of a source with S keys, ring stage st) of a consumer warpgroup: S = Q K^T, online
+// softmax update of (m, l, o), O += P V, release of the stage.
+__device__ __forceinline__ void attn_key_block(float (&o)[32], float (&m)[2], float (&l)[2], uint32_t q_addr, const uint8_t* sK,
+                                               const uint8_t* sV, uint64_t* kv_full, uint64_t* kv_empty, int j, int kb, int S,
+                                               float sl2e, int lane) {
+  const int st = j % kKvStages;
+  mbar_wait_nocall(&kv_full[st], (j / kKvStages) & 1);
+  float s[64];
+  wg_fence();
+  const uint32_t k_addr = smem_u32(sK + st * kTileBytes);
+#pragma unroll
+  for (int k = 0; k < 4; ++k) wgmma_ss_n128(s, wg_desc_sw128(q_addr + 32 * k), wg_desc_sw128(k_addr + 32 * k), k);
+  wg_commit();
+  wg_wait<0>();
+  if (kb * 128 + 128 > S) {   // ragged last key block: keys past S do not exist
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj)
+#pragma unroll
+      for (int e = 0; e < 2; ++e)
+        if (kb * 128 + 8 * jj + 2 * (lane & 3) + e >= S) { s[4 * jj + e] = -INFINITY; s[4 * jj + 2 + e] = -INFINITY; }
+  }
+  uint32_t pa[32];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    float mx = -INFINITY;
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) mx = fmaxf(mx, fmaxf(s[4 * jj + 2 * h], s[4 * jj + 2 * h + 1]));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 1));
+    mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, 2));
+    const float m_new = fmaxf(m[h], mx);
+    const float alpha = ex2_approx((m[h] - m_new) * sl2e);
+    const float mb = m_new * sl2e;
+    float sum = 0.f;
+#pragma unroll
+    for (int jj = 0; jj < 16; ++jj) {
+      const float p0 = ex2_approx(fmaf(s[4 * jj + 2 * h], sl2e, -mb));
+      const float p1 = ex2_approx(fmaf(s[4 * jj + 2 * h + 1], sl2e, -mb));
+      sum += p0 + p1;
+      // A fragment of key chunk kk = jj / 2: {row r: keys 0-7, row r+8: keys 0-7, row r: keys 8-15, row r+8: keys 8-15}
+      pa[4 * (jj >> 1) + 2 * (jj & 1) + h] = pack_half2(p0, p1);
+    }
+    l[h] = l[h] * alpha + sum;
+    m[h] = m_new;
+#pragma unroll
+    for (int jj = 0; jj < 8; ++jj) { o[4 * jj + 2 * h] *= alpha; o[4 * jj + 2 * h + 1] *= alpha; }
+  }
+  wg_fence();
+  const uint32_t v_addr = smem_u32(sV + st * kTileBytes);
+#pragma unroll
+  for (int kk = 0; kk < 8; ++kk)
+    wgmma_rs_n64_tb(o, *reinterpret_cast<const uint32_t(*)[4]>(pa + 4 * kk), wg_desc_sw128(v_addr + 2048 * kk));
+  wg_commit();
+  wg_wait<0>();
+  if (lane == 0) mbar_arrive(&kv_empty[st]);   // this warp is done with K_j / V_j
+}
+
+// kIp: decoupled cross-attention (IP-Adapter). After the text keys the producer streams the image-prompt keys (tmKip / tmVip,
+// S_ip rows) through the same ring; the consumers keep O_txt / l_txt, restart the online softmax on the image keys and write
+// f16(O_txt / l_txt + s * O_ip / l_ip), s = *ip_scale (device memory: a scale change keeps the CUDA graph valid).
+template <bool kIp>
 __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -51,6 +112,10 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
     tma_prefetch_desc(&p.tmQ);
     tma_prefetch_desc(&p.tmK);
     tma_prefetch_desc(&p.tmV);
+    if constexpr (kIp) {
+      tma_prefetch_desc(&p.tmKip);
+      tma_prefetch_desc(&p.tmVip);
+    }
     mbar_init(q_full, 1);
     for (int i = 0; i < kKvStages; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], kConsumerWarps); }
     fence_barrier_init();
@@ -71,6 +136,16 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
       tma_load_3d(sK + st * kTileBytes, &p.tmK, &kv_full[st], p.k_col0 + head * 64, j * 128, b);
       tma_load_3d(sV + st * kTileBytes, &p.tmV, &kv_full[st], p.v_col0 + head * 64, j * 128, b);
     }
+    if constexpr (kIp) {
+      const int nblk_ip = (p.S_ip + 127) / 128;
+      for (int j = nblk; j < nblk + nblk_ip; ++j) {
+        const int st = j % kKvStages;
+        mbar_wait_nocall(&kv_empty[st], ((j / kKvStages) & 1) ^ 1);
+        mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
+        tma_load_3d(sK + st * kTileBytes, &p.tmKip, &kv_full[st], p.k_ip_col0 + head * 64, (j - nblk) * 128, b);
+        tma_load_3d(sV + st * kTileBytes, &p.tmVip, &kv_full[st], p.v_ip_col0 + head * 64, (j - nblk) * 128, b);
+      }
+    }
     return;
   }
 
@@ -84,6 +159,8 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
   for (int i = 0; i < 32; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
   mbar_wait_nocall(q_full, 0);
+  // The text loop is attn_key_block written out: routed through the helper, ptxas allocates registers differently and the
+  // kernel without an image prompt would no longer compile to the code it had before the second source existed.
   for (int j = 0; j < nblk; ++j) {
     const int st = j % kKvStages;
     mbar_wait_nocall(&kv_full[st], (j / kKvStages) & 1);
@@ -135,6 +212,29 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
     wg_wait<0>();
     if (lane == 0) mbar_arrive(&kv_empty[st]);   // this warp is done with K_j / V_j
   }
+  float ot[kIp ? 32 : 1];   // O_txt / l_txt
+  float s_ip = 0.f;
+  if constexpr (kIp) {
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      float lt = l[h];
+      lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+      lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+      const float inv = 1.0f / lt;
+#pragma unroll
+      for (int jj = 0; jj < 8; ++jj) {
+        ot[4 * jj + 2 * h] = o[4 * jj + 2 * h] * inv;
+        ot[4 * jj + 2 * h + 1] = o[4 * jj + 2 * h + 1] * inv;
+      }
+      m[h] = -INFINITY;
+      l[h] = 0.f;
+    }
+#pragma unroll
+    for (int i = 0; i < 32; ++i) o[i] = 0.f;
+    const int nblk_ip = (p.S_ip + 127) / 128;
+    for (int j = nblk; j < nblk + nblk_ip; ++j) attn_key_block(o, m, l, q_addr, sK, sV, kv_full, kv_empty, j, j - nblk, p.S_ip, sl2e, lane);
+    s_ip = *p.ip_scale;
+  }
   // ---- write-back: O / l -> f16
   const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
 #pragma unroll
@@ -147,21 +247,29 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
     if (t < p.T) {
       __half* out = p.out + ((size_t)b * p.T + t) * p.ldo + head * 64 + 2 * (lane & 3);
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj)
-        *reinterpret_cast<__half2*>(out + 8 * jj) = __floats2half2_rn(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+      for (int jj = 0; jj < 8; ++jj) {
+        if constexpr (kIp)
+          *reinterpret_cast<__half2*>(out + 8 * jj) = __floats2half2_rn(fmaf(s_ip, o[4 * jj + 2 * h] * inv, ot[4 * jj + 2 * h]),
+                                                                        fmaf(s_ip, o[4 * jj + 2 * h + 1] * inv, ot[4 * jj + 2 * h + 1]));
+        else
+          *reinterpret_cast<__half2*>(out + 8 * jj) = __floats2half2_rn(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
+      }
     }
   }
 }
 
 // Per-device launch state (several devices may be driven from one process: the opt-in to > 48 KB of dynamic shared memory
 // is a per-device function attribute).
-static bool g_attn_attr[64];
+static bool g_attn_attr[2][64];
 int attention_launch(cudaStream_t st, const AttnParams& p) {
   if (p.T < 1 || p.S < 1 || (p.ldo & 1)) return 2002;
-  int r = smem_optin(attention_kernel, kAttnSmem, g_attn_attr);
+  const bool ip = p.S_ip > 0;
+  if (ip && !p.ip_scale) return 2002;
+  auto kernel = ip ? attention_kernel<true> : attention_kernel<false>;
+  int r = smem_optin(kernel, kAttnSmem, g_attn_attr[ip]);
   if (r) return r;
   const long tiles = (long)p.B * p.n_head * ((p.T + 127) / 128);
-  return launch_kernel(attention_kernel, dim3((unsigned)tiles), dim3(kAttnThreads), (size_t)kAttnSmem, st, true, p);
+  return launch_kernel(kernel, dim3((unsigned)tiles), dim3(kAttnThreads), (size_t)kAttnSmem, st, true, p);
 }
 
 }  // namespace sdxl

@@ -35,13 +35,14 @@ struct sdxl_clip {
   ~sdxl_clip() { if (tokens_dev) cudaFree(tokens_dev); }
 };
 
+static int load_clip_blocks(Loader& L, Arena& A, int n_layer, int C, int mlp, std::vector<CBlock>& blocks);
+
 static int build_clip(sdxl_clip* m, const PackView& pv, Arena& A) {
   sdxl_ctx* c = m->ctx;
   const sdxl_clip_cfg& g = m->cfg;
   Loader L{c, &pv, &A, c->stream};
   L.reg = &m->lora;
   const int C = g.n_state;
-  m->blocks.clear();
   auto table = [&](const std::string& name, int rows, __half*& dst) {
     const PackEntry* e = L.need(name, 2);
     if (!e) return;
@@ -54,8 +55,29 @@ static int build_clip(sdxl_clip* m, const PackView& pv, Arena& A) {
   table("token_embedding/weight", g.n_vocab, m->tok_emb);
   table("position_embedding/weight", g.n_ctx, m->pos_emb);
   if (L.err) return L.err;
+  if (int r = load_clip_blocks(L, A, g.n_layer, C, 4 * C, m->blocks)) return r;
+  m->ln_final = L.norm("layer_norm", C);
+  m->has_proj = pv.find("text_projection") != nullptr;
+  if (m->has_proj) {
+    const PackEntry* e = L.need("text_projection", 2);
+    if (!e) return L.err;
+    if ((int)e->shape[0] != C || (int)e->shape[1] != g.embed_dim) return fail(c, 4404, "text_projection is [%llu,%llu], expected [%d,%d]", (unsigned long long)e->shape[0], (unsigned long long)e->shape[1], C, g.embed_dim);
+    Lin& P = m->proj;
+    P.K = C; P.Kpad = Loader::pad64(C); P.N = g.embed_dim;
+    P.w = A.get<__half>((size_t)g.embed_dim * P.Kpad);
+    if (!P.w) return fail(c, 4005, "weight arena exhausted");
+    if (!A.measure) { int r = transpose_linear_launch(c->stream, L.ptr(e), C, g.embed_dim, P.w, P.Kpad, 0, 0); if (r) return fail(c, r, "text_projection re-layout failed"); }
+  }
+  return L.err;
+}
+
+// The n_layer pre-LN blocks blocks/<i>/{attn_ln, mlp_ln, attn/{query,key,value,out}, mlp/{fc1,fc2}} of width C, MLP width mlp:
+// shared by the text encoders and the vision towers.
+static int load_clip_blocks(Loader& L, Arena& A, int n_layer, int C, int mlp, std::vector<CBlock>& blocks) {
+  sdxl_ctx* c = L.c;
+  blocks.clear();
   const int Cpad = Loader::pad64(C);
-  for (int i = 0; i < g.n_layer && !L.err; ++i) {
+  for (int i = 0; i < n_layer && !L.err; ++i) {
     const std::string bp = "blocks/" + std::to_string(i);
     CBlock b;
     b.attn_ln = L.norm(bp + "/attn_ln", C);
@@ -75,22 +97,9 @@ static int build_clip(sdxl_clip* m, const PackView& pv, Arena& A) {
       if (!A.measure) { int r = bias_to_f32_launch(c->stream, L.ptr(be), C, b.qkv.b + j * C, 0, 0); if (r) L.err = fail(c, r, "bias_to_f32 failed"); }
     }
     b.out = L.linear(bp + "/attn/out", C, C, true);
-    b.fc1 = L.linear(bp + "/mlp/fc1", C, 4 * C, true);
-    b.fc2 = L.linear(bp + "/mlp/fc2", 4 * C, C, true);
-    m->blocks.push_back(b);
-  }
-  if (L.err) return L.err;
-  m->ln_final = L.norm("layer_norm", C);
-  m->has_proj = pv.find("text_projection") != nullptr;
-  if (m->has_proj) {
-    const PackEntry* e = L.need("text_projection", 2);
-    if (!e) return L.err;
-    if ((int)e->shape[0] != C || (int)e->shape[1] != g.embed_dim) return fail(c, 4404, "text_projection is [%llu,%llu], expected [%d,%d]", (unsigned long long)e->shape[0], (unsigned long long)e->shape[1], C, g.embed_dim);
-    Lin& P = m->proj;
-    P.K = C; P.Kpad = Cpad; P.N = g.embed_dim;
-    P.w = A.get<__half>((size_t)g.embed_dim * Cpad);
-    if (!P.w) return fail(c, 4005, "weight arena exhausted");
-    if (!A.measure) { int r = transpose_linear_launch(c->stream, L.ptr(e), C, g.embed_dim, P.w, Cpad, 0, 0); if (r) return fail(c, r, "text_projection re-layout failed"); }
+    b.fc1 = L.linear(bp + "/mlp/fc1", C, mlp, true);
+    b.fc2 = L.linear(bp + "/mlp/fc2", mlp, C, true);
+    blocks.push_back(b);
   }
   return L.err;
 }
@@ -119,6 +128,50 @@ extern "C" int sdxl_clip_load(sdxl_ctx* c, const sdxl_clip_cfg* cfg, const void*
   return 0;
 }
 
+// Plan buffers of the residual stream and the block operands.
+struct ClipStream { float *xa, *xb; __half *a16, *qkv16, *ao16; float* h32; __half* h16; };
+
+// Emits blocks [0, n_run) on the stream that starts in s.xa (shared by the text encoders and the vision towers). When capture >= 0
+// the stream entering block `capture` is preserved and *hidden points at it. Returns the final stream.
+static float* clip_block_ops(PlanBuilder& B, const std::vector<CBlock>& blocks, int n_run, int capture, float** hidden, const ClipStream& s,
+                             int Bn, int T, int C, int n_head, int head_dim, int mlp, int causal, int quick) {
+  Plan* P = B.P;
+  const int M = Bn * T;
+  float* x = s.xa;
+  *hidden = nullptr;
+  for (int i = 0; i < n_run && !B.err; ++i) {
+    const CBlock& b = blocks[i];
+    float* xn = x;
+    if (i == capture) {  // keep the input of this block: write the updated stream into the other buffer
+      *hidden = x;
+      xn = (x == s.xa) ? s.xb : s.xa;
+    }
+    // x = x + attn(attn_ln(x), causal mask)    (clip/mod.rs:177-179)
+    B.ln(x, b.attn_ln, M, s.a16);
+    B.linear(s.a16, M, b.qkv, IGEMM_LINEAR, s.qkv16, 0, 3 * C, nullptr, 0);
+    {
+      Op op{};
+      op.kind = OP_ATTN_SMALL;
+      op.as = {s.qkv16, 3 * C, 0, s.qkv16, s.qkv16, 3 * C, C, 2 * C, Bn, T, T, n_head, nullptr, causal, s.ao16, C, head_dim};
+      P->ops.push_back(op);
+      B.add_flops(4.0 * Bn * T * (double)T * C);
+    }
+    B.linear(s.ao16, M, b.out, IGEMM_LINEAR, xn, 1, C, x, C);
+    // x = x + mlp(mlp_ln(x))
+    B.ln(xn, b.mlp_ln, M, s.a16);
+    B.linear(s.a16, M, b.fc1, IGEMM_LINEAR, s.h32, 1, mlp, nullptr, 0);
+    {
+      Op op{};
+      op.kind = OP_ACT;
+      op.ac = {s.h32, (size_t)M * mlp, quick ? 1 : 0, s.h16};
+      P->ops.push_back(op);
+    }
+    B.linear(s.h16, M, b.fc2, IGEMM_LINEAR, xn, 1, C, xn, C);
+    x = xn;
+  }
+  return x;
+}
+
 // n_run blocks are executed; when capture >= 0 the stream entering block `capture` is preserved as the hidden output.
 static int build_clip_plan(sdxl_clip* m, Plan* P, Arena* A, int n_run, int capture, int pooled) {
   sdxl_ctx* c = m->ctx;
@@ -143,38 +196,8 @@ static int build_clip_plan(sdxl_clip* m, Plan* P, Arena* A, int n_run, int captu
     op.em = {m->tokens_dev, M, T, C, g.n_vocab, m->tok_emb, m->pos_emb, xa, m->err_dev};
     P->ops.push_back(op);
   }
-  float* x = xa;
-  m->hidden = nullptr;
-  for (int i = 0; i < n_run && !B.err; ++i) {
-    const CBlock& b = m->blocks[i];
-    float* xn = x;
-    if (i == capture) {  // keep the input of this block: write the updated stream into the other buffer
-      m->hidden = x;
-      xn = (x == xa) ? xb : xa;
-    }
-    // x = x + attn(attn_ln(x), causal mask)    (clip/mod.rs:177-179)
-    B.ln(x, b.attn_ln, M, a16);
-    B.linear(a16, M, b.qkv, IGEMM_LINEAR, qkv16, 0, 3 * C, nullptr, 0);
-    {
-      Op op{};
-      op.kind = OP_ATTN_SMALL;
-      op.as = {qkv16, 3 * C, 0, qkv16, qkv16, 3 * C, C, 2 * C, Bn, T, T, g.n_head, nullptr, 1, ao16, C};
-      P->ops.push_back(op);
-      B.add_flops(4.0 * Bn * T * (double)T * C);
-    }
-    B.linear(ao16, M, b.out, IGEMM_LINEAR, xn, 1, C, x, C);
-    // x = x + mlp(mlp_ln(x))
-    B.ln(xn, b.mlp_ln, M, a16);
-    B.linear(a16, M, b.fc1, IGEMM_LINEAR, h32, 1, 4 * C, nullptr, 0);
-    {
-      Op op{};
-      op.kind = OP_ACT;
-      op.ac = {h32, (size_t)M * 4 * C, g.quick_gelu ? 1 : 0, h16};
-      P->ops.push_back(op);
-    }
-    B.linear(h16, M, b.fc2, IGEMM_LINEAR, xn, 1, C, xn, C);
-    x = xn;
-  }
+  const ClipStream s{xa, xb, a16, qkv16, ao16, h32, h16};
+  float* x = clip_block_ops(B, m->blocks, n_run, capture, &m->hidden, s, Bn, T, C, g.n_head, 64, 4 * C, 1, g.quick_gelu);
   if (capture < 0 || capture >= n_run) m->hidden = x;
   if (pooled && !B.err) {
     // features of the end-of-text position: layer_norm(x)[b, argmax(tokens[b])] (@ text_projection)   (clip/mod.rs:130-141)
@@ -252,3 +275,168 @@ extern "C" int sdxl_clip_set_adapters(sdxl_clip* m, int n, const sdxl_adapter* a
 }
 extern "C" double sdxl_clip_plan_flops(const sdxl_clip* m) { return (m && m->plan) ? m->plan->flops : 0.0; }
 
+
+// ================================================================================================
+// CLIP vision tower (HF CLIPVisionModelWithProjection; the image encoder of IP-Adapter, DESIGN.md §9):
+//   x = pre_layrnorm([class_embedding ; patch_conv(pixels)] + position_embedding)
+//   n_layer pre-LN blocks (clip_block_ops: no causal mask, exact-erf GELU unless quick_gelu, head dim n_state / n_head)
+//   image_embeds = post_layernorm(x[:, 0]) @ visual_projection
+// The p x p stride-p patch conv is one GEMM on igemm over patchify's rows; class / position / pre_layrnorm is one kernel writing
+// the f32 residual stream; the pooled token reuses ln_gather_f32 (index 0) and gemv.
+// ================================================================================================
+struct sdxl_clip_vision {
+  sdxl_ctx* ctx = nullptr;
+  sdxl_clip_vision_cfg cfg{};
+  Arena warena;
+  Lin patch;                 // [n_state, Kpad], columns (c, kh, kw)
+  __half* cls = nullptr;     // [n_state]
+  __half* pos = nullptr;     // [T, n_state]
+  Norm pre_ln, post_ln;
+  std::vector<CBlock> blocks;
+  Lin proj;                  // visual_projection [proj_dim, n_state]
+  std::unique_ptr<Plan> plan;
+  int pN = 0;
+  __half* patch16 = nullptr; // plan buffers of the embedding steps, run before the plan
+  float* patches = nullptr;
+  float* x = nullptr;
+  float* embeds = nullptr;
+  int tokens() const { return (cfg.image_size / cfg.patch_size) * (cfg.image_size / cfg.patch_size) + 1; }
+};
+
+static int build_clip_vision(sdxl_clip_vision* m, const PackView& pv, Arena& A) {
+  sdxl_ctx* c = m->ctx;
+  const sdxl_clip_vision_cfg& g = m->cfg;
+  const int C = g.n_state, p = g.patch_size, T = m->tokens(), K = 3 * p * p;
+  Loader L{c, &pv, &A, c->stream};
+  {
+    const PackEntry* e = L.conv_weight("patch_embedding", C, 3, p);
+    if (!e) return L.err;
+    Lin& P = m->patch;
+    P.K = K; P.Kpad = Loader::pad64(K); P.N = C;
+    P.w = A.get<__half>((size_t)C * P.Kpad);
+    if (!P.w) return fail(c, 4005, "weight arena exhausted");
+    if (!A.measure) {   // OIHW rows [C, 3*p*p] into the zero-padded K-major matrix
+      CU(c, cudaMemsetAsync(P.w, 0, (size_t)C * P.Kpad * sizeof(__half), c->stream));
+      CU(c, cudaMemcpy2DAsync(P.w, (size_t)P.Kpad * sizeof(__half), L.ptr(e), (size_t)K * sizeof(__half), (size_t)K * sizeof(__half), C,
+                              cudaMemcpyDeviceToDevice, c->stream));
+    }
+  }
+  auto table = [&](const std::string& name, int ndim, int rows, __half*& dst) {
+    const PackEntry* e = L.need(name, ndim);
+    if (!e) return;
+    if ((ndim == 1 && (int)e->shape[0] != C) || (ndim == 2 && ((int)e->shape[0] != rows || (int)e->shape[1] != C))) {
+      L.err = fail(c, 4421, "weight pack: '%s' has the wrong shape (expected %d x %d)", name.c_str(), rows, C);
+      return;
+    }
+    dst = A.get<__half>((size_t)rows * C);
+    if (!dst) { L.err = fail(c, 4005, "weight arena exhausted"); return; }
+    if (!A.measure && cudaMemcpyAsync(dst, L.ptr(e), (size_t)rows * C * sizeof(__half), cudaMemcpyDeviceToDevice, c->stream) != cudaSuccess)
+      L.err = fail(c, 4402, "embedding copy failed");
+  };
+  table("class_embedding", 1, 1, m->cls);
+  table("position_embedding/weight", 2, T, m->pos);
+  if (L.err) return L.err;
+  m->pre_ln = L.norm("pre_layernorm", C);
+  if (int r = load_clip_blocks(L, A, g.n_layer, C, g.mlp_dim, m->blocks)) return r;
+  m->post_ln = L.norm("post_layernorm", C);
+  if (L.err) return L.err;
+  {   // visual_projection [n_state, proj_dim] ([in, out], no bias; named like text_projection, without /weight)
+    const PackEntry* e = L.need("visual_projection", 2);
+    if (!e) return L.err;
+    if ((int)e->shape[0] != C || (int)e->shape[1] != g.proj_dim)
+      return fail(c, 4423, "visual_projection is [%llu,%llu], expected [%d,%d]", (unsigned long long)e->shape[0], (unsigned long long)e->shape[1], C, g.proj_dim);
+    Lin& P = m->proj;
+    P.K = C; P.Kpad = Loader::pad64(C); P.N = g.proj_dim;
+    P.w = A.get<__half>((size_t)g.proj_dim * P.Kpad);
+    if (!P.w) return fail(c, 4005, "weight arena exhausted");
+    if (!A.measure) { int r = transpose_linear_launch(c->stream, L.ptr(e), C, g.proj_dim, P.w, P.Kpad, 0, 0); if (r) return fail(c, r, "visual_projection re-layout failed"); }
+  }
+  return 0;
+}
+
+extern "C" int sdxl_clip_vision_load(sdxl_ctx* c, const sdxl_clip_vision_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
+                                     sdxl_clip_vision** out) {
+  if (!c || !cfg || !pack || !out) return fail(c, -1, "sdxl_clip_vision_load: null argument");
+  *out = nullptr;
+  const int hd = cfg->n_head > 0 ? cfg->n_state / cfg->n_head : 0;
+  if (cfg->n_head < 1 || cfg->n_state != cfg->n_head * hd || hd % 8 || hd > 128)
+    return fail(c, 4420, "vision encoder head dim must be a multiple of 8 up to 128 (n_state=%d, n_head=%d)", cfg->n_state, cfg->n_head);
+  if (cfg->n_layer < 1 || cfg->mlp_dim < 8 || cfg->mlp_dim % 8 || cfg->proj_dim < 1 || cfg->patch_size < 1 ||
+      cfg->image_size < cfg->patch_size || cfg->image_size % cfg->patch_size || cfg->n_state % 8)
+    return fail(c, 4422, "bad vision encoder config");
+  CU(c, cudaSetDevice(c->device));
+  std::unique_ptr<sdxl_clip_vision> m(new sdxl_clip_vision());
+  m->ctx = c;
+  m->cfg = *cfg;
+  int r = with_device_pack(c, pack, bytes, pack_on_device, [&](const PackView& pv) { return build_two_pass(m.get(), pv, build_clip_vision); });
+  if (r) return r;
+  *out = m.release();
+  return 0;
+}
+
+extern "C" void sdxl_clip_vision_destroy(sdxl_clip_vision* m) {
+  if (!m) return;
+  cudaStreamSynchronize(m->ctx->stream);
+  delete m;
+}
+
+static int build_vision_plan(sdxl_clip_vision* m, Plan* P, Arena* A) {
+  sdxl_ctx* c = m->ctx;
+  const sdxl_clip_vision_cfg& g = m->cfg;
+  PlanBuilder B{c, P, A, P->Bf};
+  P->ops.clear();
+  P->flops = 0;
+  const int N = P->Bf, T = m->tokens(), C = g.n_state, M = N * T;
+  m->patch16 = B.buf<__half>((size_t)N * (T - 1) * m->patch.Kpad);
+  m->patches = B.buf<float>((size_t)N * (T - 1) * C);
+  const ClipStream s{B.buf<float>((size_t)M * C), B.buf<float>((size_t)M * C), B.buf<__half>((size_t)M * C), B.buf<__half>((size_t)M * 3 * C),
+                     B.buf<__half>((size_t)M * C), B.buf<float>((size_t)M * g.mlp_dim), B.buf<__half>((size_t)M * g.mlp_dim)};
+  int* idx0 = B.buf<int>(N);
+  float* pin = B.buf<float>((size_t)N * C);
+  m->embeds = B.buf<float>((size_t)N * g.proj_dim);
+  if (B.err) return B.err;
+  if (!A->measure) CU(c, cudaMemsetAsync(idx0, 0, N * sizeof(int), c->stream));   // the class token of every image
+  m->x = s.xa;
+  float* hidden = nullptr;
+  float* x = clip_block_ops(B, m->blocks, g.n_layer, -1, &hidden, s, N, T, C, g.n_head, C / g.n_head, g.mlp_dim, 0, g.quick_gelu);
+  if (B.err) return B.err;
+  Op op{};
+  op.kind = OP_LN_GATHER;
+  op.lg = {x, idx0, N, T, C, m->post_ln.g, m->post_ln.b, m->post_ln.eps, pin};
+  P->ops.push_back(op);
+  B.gemv(pin, C, N, m->proj, nullptr, 0, 0, 0, m->embeds, g.proj_dim);
+  return B.err;
+}
+
+extern "C" int sdxl_clip_vision_encode(sdxl_clip_vision* m, int N, const float* pixels, int on_host, float* image_embeds_out) {
+  if (!m || !pixels || !image_embeds_out) return fail(m ? m->ctx : nullptr, -1, "sdxl_clip_vision_encode: null argument");
+  sdxl_ctx* c = m->ctx;
+  const sdxl_clip_vision_cfg& g = m->cfg;
+  if (N < 1 || N > 256) return fail(c, 5205, "vision encoder batch must be 1..256 (got %d)", N);
+  CU(c, cudaSetDevice(c->device));
+  if (!m->plan || m->pN != N) {
+    if (int r = build_plan(c, m->plan, N, N, 0, 0, [&](Plan* P, Arena* A) { return build_vision_plan(m, P, A); })) return r;
+    m->pN = N;
+  }
+  const int S = g.image_size, T = m->tokens(), C = g.n_state;
+  const size_t in_bytes = (size_t)N * 3 * S * S * sizeof(float);
+  TmpBufs tmp(c->stream);
+  const float* px = pixels;
+  if (on_host) {
+    float* d = (float*)tmp.get(in_bytes);
+    if (!d) return fail(c, 5206, "vision encoder: cannot allocate %zu bytes for the pixels", in_bytes);
+    CU(c, cudaMemcpyAsync(d, pixels, in_bytes, cudaMemcpyHostToDevice, c->stream));
+    px = d;
+  }
+  const Lin& Pt = m->patch;
+  const int rows = N * (T - 1);
+  KL(c, patchify_launch(c->stream, px, N, S, g.patch_size, Pt.Kpad, m->patch16));
+  const IgemmOperands o{m->patch16, 1, 1, rows, Pt.Kpad, Pt.Kpad, nullptr, 0, 0, 0, 0, 0, Pt.w, Pt.N, Pt.Kpad};
+  if (int r = igemm_run(c, o, {{0, 0, 0, 0, Pt.Kpad / 64}}, 1, rows, 1, IGEMM_LINEAR, 0, m->patches, 1, C, nullptr, nullptr, 0)) return r;
+  KL(c, vision_embed_ln_launch(c->stream, m->patches, m->cls, m->pos, N, T, C, m->pre_ln.g, m->pre_ln.b, m->pre_ln.eps, m->x));
+  if (int r = run_plan_ops(c, m->plan.get())) return r;
+  const size_t out_bytes = (size_t)N * g.proj_dim * sizeof(float);
+  CU(c, cudaMemcpyAsync(image_embeds_out, m->embeds, out_bytes, on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+  if (on_host) CU(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}

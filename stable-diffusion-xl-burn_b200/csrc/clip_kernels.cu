@@ -1,4 +1,5 @@
-// Kernels that only the text encoders (Embedder: CLIP-L / OpenCLIP-bigG, reference src/model/clip/mod.rs) need. The
+// Kernels that only the CLIP towers need: the text encoders (Embedder: CLIP-L / OpenCLIP-bigG, reference src/model/clip/mod.rs)
+// and the vision encoders of IP-Adapter (HF CLIPVisionModelWithProjection). The
 // sequences are 77 tokens, so these are small CUDA-core kernels; the Linear layers run on the wgmma GEMM (igemm.cu).
 #include "common.cuh"
 #include "kernels.h"
@@ -117,13 +118,186 @@ __global__ void __launch_bounds__(128) attention_small_kernel(const __half* __re
   const float inv = l > 0.f ? 1.f / l : 0.f;
   *reinterpret_cast<__half2*>(out + ((size_t)b * T + t) * ldo + h * 64 + 2 * lane) = __floats2half2_rn(ax * inv, ay * inv);
 }
+// The same attention for head dims D other than 64 (multiples of 8 up to 128: the CLIP vision towers use 80 and 104), scale
+// 1/sqrt(D). Kept beside the d = 64 kernel so that the text encoders' kernel is unchanged. Lane l accumulates the output columns
+// 2 (l + 32 i), i < NP.
+template <int D>
+__global__ void attention_small_hd_kernel(const __half* __restrict__ q, int q_pitch, int q_col0,
+                                                                 const __half* __restrict__ k, const __half* __restrict__ v,
+                                                                 int kv_pitch, int k_col0, int v_col0, int B, int T, int S, int n_head,
+                                                                 const __half* __restrict__ mask, int causal, float scale,
+                                                                 __half* __restrict__ out, int ldo) {
+  constexpr int NP = (D / 2 + 31) / 32;
+  __shared__ float qs[4][D];
+  griddep_wait();
+  griddep_launch_dependents();
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const long item = (long)blockIdx.x * 4 + warp;
+  const long total = (long)B * n_head * T;
+  const bool active = item < total;
+  int t = 0, h = 0, b = 0;
+  if (active) {
+    t = (int)(item % T);
+    h = (int)((item / T) % n_head);
+    b = (int)(item / ((long)T * n_head));
+    for (int c = lane; c < D / 2; c += 32) {
+      const __half2 qq = *reinterpret_cast<const __half2*>(q + ((size_t)b * T + t) * q_pitch + q_col0 + h * D + 2 * c);
+      qs[warp][2 * c] = __low2float(qq) * scale;
+      qs[warp][2 * c + 1] = __high2float(qq) * scale;
+    }
+  }
+  __syncwarp();
+  if (!active) return;
+  float m = -INFINITY, l = 0.f, ax[NP], ay[NP];
+#pragma unroll
+  for (int i = 0; i < NP; ++i) ax[i] = ay[i] = 0.f;
+  const __half* kb = k + (size_t)b * S * kv_pitch + k_col0 + h * D;
+  const __half* vb = v + (size_t)b * S * kv_pitch + v_col0 + h * D;
+  const int s_end = causal ? min(S, t + 1) : S;
+  for (int j0 = 0; j0 < s_end; j0 += 32) {
+    const int j = j0 + lane;
+    float s = -INFINITY;
+    if (j < s_end) {
+      const uint4* kr = reinterpret_cast<const uint4*>(kb + (size_t)j * kv_pitch);
+      float acc = 0.f;
+#pragma unroll
+      for (int c = 0; c < D / 8; ++c) {
+        const uint4 u = kr[c];
+        const uint32_t w4[4] = {u.x, u.y, u.z, u.w};
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          __half2_raw r;
+          r.x = (unsigned short)(w4[e] & 0xffffu);
+          r.y = (unsigned short)(w4[e] >> 16);
+          const float2 f = __half22float2(__half2(r));
+          acc = fmaf(qs[warp][c * 8 + 2 * e], f.x, acc);
+          acc = fmaf(qs[warp][c * 8 + 2 * e + 1], f.y, acc);
+        }
+      }
+      s = acc;
+      if (mask) s += __half2float(mask[(size_t)t * S + j]);
+    }
+    float cm = s;
+#pragma unroll
+    for (int o = 16; o; o >>= 1) cm = fmaxf(cm, __shfl_xor_sync(0xffffffffu, cm, o));
+    const float m_new = fmaxf(m, cm);
+    if (m_new == -INFINITY) continue;  // everything so far is masked
+    const float corr = (m == -INFINITY) ? 0.f : __expf(m - m_new);
+    const float p = (s == -INFINITY) ? 0.f : __expf(s - m_new);
+    float ps = p;
+#pragma unroll
+    for (int o = 16; o; o >>= 1) ps += __shfl_xor_sync(0xffffffffu, ps, o);
+    l = l * corr + ps;
+#pragma unroll
+    for (int i = 0; i < NP; ++i) { ax[i] *= corr; ay[i] *= corr; }
+    const int nj = min(32, s_end - j0);
+    for (int jj = 0; jj < nj; ++jj) {
+      const float pj = __shfl_sync(0xffffffffu, p, jj);
+      const __half* vr = vb + (size_t)(j0 + jj) * kv_pitch;
+#pragma unroll
+      for (int i = 0; i < NP; ++i) {   // lanes past D / 2 re-read the last column and are not stored
+        const int c = min(lane + 32 * i, D / 2 - 1);
+        const float2 vv = __half22float2(*reinterpret_cast<const __half2*>(vr + 2 * c));
+        ax[i] = fmaf(pj, vv.x, ax[i]);
+        ay[i] = fmaf(pj, vv.y, ay[i]);
+      }
+    }
+    m = m_new;
+  }
+  const float inv = l > 0.f ? 1.f / l : 0.f;
+#pragma unroll
+  for (int i = 0; i < NP; ++i) {
+    const int c = lane + 32 * i;
+    if (c < D / 2)
+      *reinterpret_cast<__half2*>(out + ((size_t)b * T + t) * ldo + h * D + 2 * c) = __floats2half2_rn(ax[i] * inv, ay[i] * inv);
+  }
+}
+
 int attention_small_launch(cudaStream_t st, const __half* q, int q_pitch, int q_col0, const __half* k, const __half* v,
                            int kv_pitch, int k_col0, int v_col0, int B, int T, int S, int n_head, const __half* mask, int causal,
-                           __half* out, int ldo) {
+                           __half* out, int ldo, int head_dim) {
   if ((q_pitch & 7) || (kv_pitch & 7) || (q_col0 & 7) || (k_col0 & 7) || (v_col0 & 7) || (ldo & 1)) return 7102;
   const long total = (long)B * n_head * T;
-  return launch_kernel(attention_small_kernel, dim3(cdiv(total, 4)), dim3(128), (size_t)0, st, true, q, q_pitch, q_col0, k, v, kv_pitch,
-                       k_col0, v_col0, B, T, S, n_head, mask, causal, 0.125f, out, ldo);
+  const dim3 grid(cdiv(total, 4)), block(128);
+  const float scale = 1.f / sqrtf((float)head_dim);
+  switch (head_dim) {
+#define SDXL_ATTN_SMALL_HD(D) \
+    case D: return launch_kernel(attention_small_hd_kernel<D>, grid, block, (size_t)0, st, true, q, q_pitch, q_col0, k, v, kv_pitch, \
+                                 k_col0, v_col0, B, T, S, n_head, mask, causal, scale, out, ldo);
+    SDXL_ATTN_SMALL_HD(8) SDXL_ATTN_SMALL_HD(16) SDXL_ATTN_SMALL_HD(24) SDXL_ATTN_SMALL_HD(32) SDXL_ATTN_SMALL_HD(40)
+    SDXL_ATTN_SMALL_HD(48) SDXL_ATTN_SMALL_HD(56) SDXL_ATTN_SMALL_HD(72) SDXL_ATTN_SMALL_HD(80) SDXL_ATTN_SMALL_HD(88)
+    SDXL_ATTN_SMALL_HD(96) SDXL_ATTN_SMALL_HD(104) SDXL_ATTN_SMALL_HD(112) SDXL_ATTN_SMALL_HD(120) SDXL_ATTN_SMALL_HD(128)
+#undef SDXL_ATTN_SMALL_HD
+    case 64:
+      return launch_kernel(attention_small_kernel, grid, block, (size_t)0, st, true, q, q_pitch, q_col0, k, v, kv_pitch,
+                           k_col0, v_col0, B, T, S, n_head, mask, causal, scale, out, ldo);
+    default: return 7104;
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// CLIP vision embedding (HF CLIPVisionEmbeddings).
+// patchify: pixels f32 NCHW [N, 3, S, S] -> f16 [N * G * G, Kpad], row n * G * G + py * G + px, column (c, kh, kw) = the OIHW
+// flatten of the p x p stride-p patch conv, zero padded to Kpad (the patch conv is then one GEMM on igemm).
+// ------------------------------------------------------------------------------------------------
+__global__ void patchify_kernel(const float* __restrict__ px, int S, int p, int G, int Kpad, __half* __restrict__ y) {
+  griddep_wait();
+  griddep_launch_dependents();
+  const long row = blockIdx.x;
+  const int n = (int)(row / (G * G)), pi = (int)(row % (G * G)), py = pi / G, pxi = pi % G;
+  const int K = 3 * p * p;
+  for (int k = threadIdx.x; k < Kpad; k += blockDim.x) {
+    float v = 0.f;
+    if (k < K) {
+      const int c = k / (p * p), kh = (k / p) % p, kw = k % p;
+      v = px[(((size_t)n * 3 + c) * S + py * p + kh) * S + pxi * p + kw];
+    }
+    y[row * Kpad + k] = __float2half_rn(v);
+  }
+}
+int patchify_launch(cudaStream_t st, const float* pixels, int N, int S, int p, int Kpad, __half* y) {
+  if (p < 1 || S % p || Kpad < 3 * p * p) return 7105;
+  const int G = S / p;
+  return launch_kernel(patchify_kernel, dim3((unsigned)(N * G * G)), dim3(128), (size_t)0, st, true, pixels, S, p, G, Kpad, y);
+}
+
+// x[n*T + t, :] = pre_layrnorm((t == 0 ? class_embedding : patches[n*(T-1) + t-1, :]) + position_embedding[t, :]), the f32 residual
+// stream. One block per row; exact two-pass statistics like the other LayerNorms.
+__global__ void vision_embed_ln_kernel(const float* __restrict__ patches, const __half* __restrict__ cls, const __half* __restrict__ pos,
+                                       int T, int C, const float* __restrict__ gamma, const float* __restrict__ beta, float eps,
+                                       float* __restrict__ x) {
+  __shared__ float red[32];
+  griddep_wait();
+  griddep_launch_dependents();
+  const int row = blockIdx.x, t = row % T, n = row / T;
+  float* xr = x + (size_t)row * C;
+  const float* pr = t ? patches + ((size_t)n * (T - 1) + t - 1) * C : nullptr;
+  auto block_sum = [&](float s) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    float tot = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
+    __syncthreads();
+    return tot;
+  };
+  float s = 0.f;
+  for (int i = threadIdx.x; i < C; i += blockDim.x) {
+    const float v = (t ? pr[i] : __half2float(cls[i])) + __half2float(pos[(size_t)t * C + i]);
+    xr[i] = v;
+    s += v;
+  }
+  const float mean = block_sum(s) / C;
+  float q = 0.f;
+  for (int i = threadIdx.x; i < C; i += blockDim.x) { const float d = xr[i] - mean; q = fmaf(d, d, q); }
+  const float rstd = 1.f / sqrtf(block_sum(q) / C + eps);
+  for (int i = threadIdx.x; i < C; i += blockDim.x) xr[i] = (xr[i] - mean) * rstd * gamma[i] + beta[i];
+}
+int vision_embed_ln_launch(cudaStream_t st, const float* patches, const __half* cls, const __half* pos, int N, int T, int C,
+                           const float* gamma, const float* beta, float eps, float* x) {
+  return launch_kernel(vision_embed_ln_kernel, dim3((unsigned)(N * T)), dim3(256), (size_t)0, st, true, patches, cls, pos, T, C, gamma,
+                       beta, eps, x);
 }
 
 // ------------------------------------------------------------------------------------------------

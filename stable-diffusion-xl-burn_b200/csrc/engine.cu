@@ -14,6 +14,8 @@
 //                               src/model/stablediffusion/mod.rs:317-541
 #include "engine_core.h"
 
+#include <set>
+
 // ================================================================================================
 // context
 // ================================================================================================
@@ -65,6 +67,7 @@ extern "C" uint64_t sdxl_ctx_launch_count(const sdxl_ctx* c) { return c ? c->lau
 // model
 // ================================================================================================
 struct TBlock {
+  std::string path;   // reference path, e.g. input_blocks/4/transformer/transformer_0
   Norm n1, n2, n3;
   Lin qkv, out1;      // self-attention (fused [3C, C])
   Lin q2, kv2, out2;  // cross-attention (kv fused [2C, ctx])
@@ -89,6 +92,7 @@ struct Block {
 struct Plan;
 struct Sampler;
 struct ControlAttach;
+struct IpAttach;
 
 // Embeddings, first conv, input blocks and middle block: the part of the UNet a ControlNet copies.
 struct EncoderHalf {
@@ -137,6 +141,10 @@ struct sdxl_unet : EncoderHalf {
   AdapterState lora;           // LoRA-able weight slots, backups of merged layers (sdxl_unet_set_adapters)
   std::vector<std::unique_ptr<ControlAttach>> controls;   // sdxl_unet_set_controls, in call order
   uint64_t controls_version = 0;
+  std::unique_ptr<IpAttach> ip;   // sdxl_unet_set_image_prompt
+  uint64_t ip_version = 0;
+  uint64_t plan_builds = 0;
+  int cfg_rows = 0;               // conditioning rows are the sampler's [cond | uncond] with cfg_rows cond rows (0: plain batch)
   ~sdxl_unet() {
     if (t_dev) cudaFree(t_dev);
     if (t_pinned) cudaFreeHost(t_pinned);
@@ -156,6 +164,33 @@ struct ControlAttach {
   float* lab1 = nullptr;
   float* label_emb = nullptr;
   std::vector<__half*> kv;
+};
+
+// IP-Adapter (DESIGN.md §9): the image-token projection and, per UNet transformer block in execution order, the fused
+// [ip_key | ip_value] projection of the image tokens (N = 2C, K = context_dim).
+struct sdxl_ip_adapter {
+  sdxl_ctx* ctx = nullptr;
+  sdxl_ip_adapter_cfg cfg{};
+  Arena warena;
+  Lin proj;                 // [T * context_dim, D]
+  Norm norm;                // over context_dim, eps 1e-5
+  std::vector<Lin> kv;
+  std::vector<std::string> paths;   // the transformer block of each kv
+};
+
+// An attached image prompt: the projected tokens of the prompts and of the negatives, the per-block scales, and the image K/V
+// hoisted for the current conditioning rows.
+struct IpAttach {
+  const sdxl_ip_adapter* ad = nullptr;
+  int n_batch = 0, n_images = 0, S_ip = 0;
+  Arena mem;
+  __half* tok_pos = nullptr;   // [n_batch, S_ip, context_dim]
+  __half* tok_neg = nullptr;   // [n_batch, S_ip, context_dim]
+  float* scales = nullptr;     // [n_tblocks], read by the attention kernel
+  Arena cmem;                  // sized by the conditioning batch
+  int condB = 0;
+  __half* rows = nullptr;      // [condB, S_ip, context_dim]
+  std::vector<__half*> kv;     // per transformer block [condB * S_ip, 2C]
 };
 
 
@@ -193,6 +228,7 @@ static STrans load_st(Loader& L, const std::string& path, int C, int ctx_dim, in
   for (int j = 0; j < depth && !L.err; ++j) {
     const std::string bp = path + "/transformer_" + std::to_string(j);
     TBlock b;
+    b.path = bp;
     b.n1 = L.norm(bp + "/norm1", C);
     b.n2 = L.norm(bp + "/norm2", C);
     b.n3 = L.norm(bp + "/norm3", C);
@@ -715,6 +751,12 @@ struct UNetPlanBuilder : PlanBuilder {
       const __half* kvp = A->measure ? nullptr : (*kvs)[kv_index];
       attn(s_q, C, 0, kvp, 2 * C, 0, C, T, u->n_ctx, s.n_head, s_ao, C, sl2e);
       P->flops += 2.0 * Bf * u->n_ctx * (double)b.kv2.K * b.kv2.N;  // hoisted K/V projections (algorithmic work)
+      // an attached image prompt adds its K/V source to the UNet's own cross-attentions (a ControlNet's see text only)
+      if (u->ip && kvs == &u->kv) {
+        const IpAttach& ip = *u->ip;
+        attn_ip(A->measure ? nullptr : ip.kv[kv_index], 2 * C, 0, C, ip.S_ip, ip.scales + kv_index);
+        P->flops += 2.0 * Bf * ip.S_ip * (double)ip.ad->kv[kv_index].K * ip.ad->kv[kv_index].N;
+      }
       kv_index++;
       linear(s_ao, M, b.out2, IGEMM_LINEAR, s_tok, 1, C, s_tok, C);
       // x = x + mlp(norm3(x))
@@ -752,6 +794,20 @@ struct UNetPlanBuilder : PlanBuilder {
     op.flops_exec = 4.0 * Bf * (double)((T + 127) / 128 * 128) * (double)((S + 127) / 128 * 128) * (n_head * 64);
     P->ops.push_back(op);
     add_flops(4.0 * Bf * T * (double)S * (n_head * 64));
+  }
+  // Turns the attention just pushed into the two-source form: + (*scale) * softmax(q k_ip^T) v_ip, k_ip / v_ip column windows of
+  // kvm [Bf * S_ip, kv_pitch].
+  void attn_ip(const __half* kvm, int kv_pitch, int k_col0, int v_col0, int S_ip, const float* scale) {
+    if (err) return;
+    AttnParams& p = P->ops.back().at;
+    p.S_ip = S_ip; p.k_ip_col0 = k_col0; p.v_ip_col0 = v_col0; p.ip_scale = scale;
+    if (!A->measure) {
+      if (int r = make_tmap_rows(&p.tmKip, kvm, S_ip, Bf, kv_pitch, kv_pitch)) { err = fail(c, r, "tensor map creation failed (attention)"); return; }
+      p.tmVip = p.tmKip;
+    }
+    const int C = p.n_head * 64;
+    P->ops.back().flops_exec += 4.0 * Bf * (double)((p.T + 127) / 128 * 128) * (double)((S_ip + 127) / 128 * 128) * C;
+    add_flops(4.0 * Bf * p.T * (double)S_ip * C);
   }
 };
 
@@ -898,12 +954,15 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
       return fail(c, 5012, "control %zu: its hint is %dx%d pixels (latent %dx%d) but the latent is %dx%d", k, 8 * a.h, 8 * a.w, a.h, a.w, h, w);
     if (Bf % a.n_hint) return fail(c, 5013, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bf, a.n_hint);
   }
+  if (u->ip && u->ip->condB != Bf) return fail(c, 5014, "image prompt: its K/V are hoisted for batch %d but the batch is %d", u->ip->condB, Bf);
   if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan->cond_version == u->cond_version &&
-      u->plan->controls_version == u->controls_version)
+      u->plan->controls_version == u->controls_version && u->plan->ip_version == u->ip_version)
     return 0;
   if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A); })) return r;
+  u->plan_builds++;
   u->plan->cond_version = u->cond_version;
   u->plan->controls_version = u->controls_version;
+  u->plan->ip_version = u->ip_version;
   return 0;
 }
 
@@ -955,11 +1014,37 @@ static int control_cond_alloc(sdxl_unet* u, ControlAttach& a) {
   return 0;
 }
 
-static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* context_dev, const __half* y_dev) {
+// (Re)allocates the image prompt's row and K/V buffers for the UNet's current conditioning batch.
+static int ip_cond_alloc(sdxl_unet* u, IpAttach& a) {
+  if (a.condB == u->condB) return 0;
+  const int B = u->condB, ctx_dim = u->cfg.context_dim;
+  size_t need = 0;
+  auto al = [&](size_t b) { need = ((need + 1023) & ~size_t(1023)) + b; };
+  al((size_t)B * a.S_ip * ctx_dim * 2);
+  for (const Lin& L : a.ad->kv) al((size_t)B * a.S_ip * L.N * 2);
+  if (a.cmem.init(need + (1 << 16))) return fail(u->ctx, 5103, "cannot allocate image-prompt conditioning buffers");
+  a.rows = a.cmem.get<__half>((size_t)B * a.S_ip * ctx_dim);
+  a.kv.clear();
+  for (const Lin& L : a.ad->kv) a.kv.push_back(a.cmem.get<__half>((size_t)B * a.S_ip * L.N));
+  a.condB = B;
+  return 0;
+}
+
+// An image prompt's n_batch must divide the number of images the conditioning rows hold.
+static int ip_check_batch(sdxl_unet* u, int n_batch /* 0: no prompt */, int B, int cfg_rows) {
+  const int n_img = cfg_rows ? cfg_rows : B;
+  if (n_batch && n_img % n_batch)
+    return fail(u->ctx, 5104, "image prompt: batch %d is not a multiple of its n_batch = %d", n_img, n_batch);
+  return 0;
+}
+
+static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* context_dev, const __half* y_dev, int cfg_rows) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   const int ted = 4 * g.model_channels;
   if (B < 1 || n_ctx < 1) return fail(c, 5100, "bad conditioning shape");
+  if (int r = ip_check_batch(u, u->ip ? u->ip->n_batch : 0, B, cfg_rows)) return r;
+  u->cfg_rows = cfg_rows;
   if (u->condB != B || u->n_ctx != n_ctx) {
     CU(c, cudaStreamSynchronize(c->stream));
     u->plan.reset();
@@ -984,6 +1069,8 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
     CU(c, cudaMemsetAsync(u->ctx16, 0, (size_t)B * n_ctx * u->ctx_pitch * 2, c->stream));
     for (auto& a : u->controls)
       if (int r = control_cond_alloc(u, *a)) return r;
+    if (u->ip)
+      if (int r = ip_cond_alloc(u, *u->ip)) return r;
   }
   u->cond_version++;
   if (u->plan) u->plan->cond_version = u->cond_version;  // buffers unchanged: plan stays valid
@@ -991,6 +1078,16 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
                           (size_t)B * n_ctx, cudaMemcpyDeviceToDevice, c->stream));
   KL(c, cast_f16_to_f32_launch(c->stream, y_dev, (size_t)B * g.adm_in_channels, u->y32));
   return hoist_conditioning(u);
+}
+
+// out[i] = a @ L_i for every Lin (K/V projections of context or image tokens); a f16 [M, K] with row pitch lda.
+static int project_kv(sdxl_ctx* c, const __half* a, int M, int K, int lda, const std::vector<const Lin*>& lins, const std::vector<__half*>& out) {
+  for (size_t i = 0; i < lins.size(); ++i) {
+    const Lin& L = *lins[i];
+    const IgemmOperands o{a, 1, 1, M, K, lda, nullptr, 0, 0, 0, 0, 0, L.w, L.N, L.Kpad};
+    if (int r = igemm_run(c, o, {{0, 0, 0, 0, L.Kpad / 64}}, 1, M, 1, IGEMM_LINEAR, 0, out[i], 0, L.N, nullptr, nullptr, 0)) return r;
+  }
+  return 0;
 }
 
 // label_emb = lin2(SiLU(lin1(y))) (unet/mod.rs:464-466) and the K/V projections of the context for every cross-attention
@@ -1007,13 +1104,24 @@ static int hoist_model(sdxl_unet* u, const EncoderHalf& e, const std::vector<con
     KL(c, gemv_launch(c->stream, lab1 + (size_t)b0 * ted, ted, nb, e.l2.K, e.l2.w, e.l2.Kpad, e.l2.b, nullptr, 0, ted, 0, 0,
                       label_emb + (size_t)b0 * ted, ted));
   }
-  const int M = B * n_ctx;
-  for (size_t i = 0; i < tbs.size(); ++i) {
-    const Lin& L = tbs[i]->kv2;
-    const IgemmOperands o{u->ctx16, 1, 1, M, g.context_dim, u->ctx_pitch, nullptr, 0, 0, 0, 0, 0, L.w, L.N, L.Kpad};
-    if (int r = igemm_run(c, o, {{0, 0, 0, 0, L.Kpad / 64}}, 1, M, 1, IGEMM_LINEAR, 0, kv[i], 0, L.N, nullptr, nullptr, 0)) return r;
+  std::vector<const Lin*> lins;
+  for (auto* t : tbs) lins.push_back(&t->kv2);
+  return project_kv(c, u->ctx16, B * n_ctx, g.context_dim, u->ctx_pitch, lins, kv);
+}
+
+// The image prompt's token rows for the current conditioning rows (row rule: include/sdxl_b200.h, sdxl_unet_set_image_prompt)
+// and their K/V for every UNet cross-attention.
+static int ip_hoist(sdxl_unet* u, IpAttach& a) {
+  sdxl_ctx* c = u->ctx;
+  const int ctx_dim = u->cfg.context_dim, B = u->condB, cr = u->cfg_rows;
+  const size_t row = (size_t)a.S_ip * ctx_dim;
+  for (int r = 0; r < B; ++r) {
+    const __half* src = (cr && r >= cr) ? a.tok_neg + (size_t)((r - cr) % a.n_batch) * row : a.tok_pos + (size_t)(r % a.n_batch) * row;
+    CU(c, cudaMemcpyAsync(a.rows + (size_t)r * row, src, row * sizeof(__half), cudaMemcpyDeviceToDevice, c->stream));
   }
-  return 0;
+  std::vector<const Lin*> lins;
+  for (const Lin& L : a.ad->kv) lins.push_back(&L);
+  return project_kv(c, a.rows, B * a.S_ip, ctx_dim, ctx_dim, lins, a.kv);
 }
 
 // The step-invariant projections of the retained conditioning (ctx16, y32) under the current weights, for the UNet and every
@@ -1022,18 +1130,33 @@ static int hoist_conditioning(sdxl_unet* u) {
   if (int r = hoist_model(u, *u, unet_tblocks(u), u->lab1, u->label_emb, u->kv)) return r;
   for (auto& a : u->controls)
     if (int r = hoist_model(u, *a->net, encoder_tblocks(*a->net), a->lab1, a->label_emb, a->kv)) return r;
-  return 0;
+  return u->ip ? ip_hoist(u, *u->ip) : 0;
 }
 
 extern "C" int sdxl_unet_set_conditioning(sdxl_unet* u, int B, int n_ctx, const sdxl_half* context, const sdxl_half* y) {
   if (!u || !context || !y) return -1;
   CU(u->ctx, cudaSetDevice(u->ctx->device));
-  return set_conditioning_dev(u, B, n_ctx, (const __half*)context, (const __half*)y);
+  return set_conditioning_dev(u, B, n_ctx, (const __half*)context, (const __half*)y, 0);
 }
 
 // ================================================================================================
 // ControlNet attachment (include/sdxl_b200.h: sdxl_unet_set_controls)
 // ================================================================================================
+// The first cfg field in which an attachment built for cfg h differs from the UNet's cfg g, or null.
+static const char* unet_cfg_mismatch(const sdxl_unet_cfg& g, const sdxl_unet_cfg& h) {
+  if (h.model_channels != g.model_channels) return "model_channels";
+  if (h.n_levels != g.n_levels) return "n_levels";
+  if (h.in_channels != g.in_channels) return "in_channels";
+  if (h.context_dim != g.context_dim) return "context_dim";
+  if (h.adm_in_channels != g.adm_in_channels) return "adm_in_channels";
+  if (h.n_head_channels != g.n_head_channels) return "n_head_channels";
+  for (int l = 0; l < g.n_levels; ++l) {
+    if (h.channel_mults[l] != g.channel_mults[l]) return "channel_mults";
+    if (h.transformer_depths[l] != g.transformer_depths[l]) return "transformer_depths";
+  }
+  return nullptr;
+}
+
 // Writes the per-attachment buffers that depend on scale and hint values: f16(s*W) / s*b of every zero conv, and hint_emb.
 static int control_write(sdxl_ctx* c, ControlAttach& a, const sdxl_control& ctl) {
   const sdxl_controlnet* n = a.net;
@@ -1068,19 +1191,7 @@ extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* c
     const sdxl_controlnet* net = ctl[k].net;
     if (!net) return fail(c, 4732, "set_controls: control %d has a null net", k);
     if (net->ctx != c) return fail(c, 4733, "set_controls: control %d: the net was created on another sdxl_ctx", k);
-    const sdxl_unet_cfg& h = net->cfg;
-    const char* field = nullptr;
-    if (h.model_channels != g.model_channels) field = "model_channels";
-    else if (h.n_levels != g.n_levels) field = "n_levels";
-    else if (h.in_channels != g.in_channels) field = "in_channels";
-    else if (h.context_dim != g.context_dim) field = "context_dim";
-    else if (h.adm_in_channels != g.adm_in_channels) field = "adm_in_channels";
-    else if (h.n_head_channels != g.n_head_channels) field = "n_head_channels";
-    for (int l = 0; l < g.n_levels && !field; ++l) {
-      if (h.channel_mults[l] != g.channel_mults[l]) field = "channel_mults";
-      else if (h.transformer_depths[l] != g.transformer_depths[l]) field = "transformer_depths";
-    }
-    if (field) return fail(c, 4734, "set_controls: control %d: cfg field '%s' differs from the UNet's", k, field);
+    if (const char* field = unet_cfg_mismatch(g, net->cfg)) return fail(c, 4734, "set_controls: control %d: cfg field '%s' differs from the UNet's", k, field);
     if (ctl[k].n_hint < 1) return fail(c, 4735, "set_controls: control %d: n_hint = %d must be >= 1", k, ctl[k].n_hint);
     if (!ctl[k].hint) return fail(c, 4736, "set_controls: control %d: null hint", k);
     if (ctl[k].height < 8 || ctl[k].width < 8 || ctl[k].height % 8 || ctl[k].width % 8)
@@ -1129,6 +1240,223 @@ extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* c
   if (u->condB > 0)
     for (auto& a : u->controls)
       if (int r = hoist_model(u, *a->net, encoder_tblocks(*a->net), a->lab1, a->label_emb, a->kv)) return r;
+  return 0;
+}
+
+
+// ================================================================================================
+// IP-Adapter (include/sdxl_b200.h: sdxl_ip_adapter_load, sdxl_unet_set_image_prompt; DESIGN.md §9)
+// ================================================================================================
+// Path and width of every UNet transformer block in execution order: the block program of load_encoder / build_model. The adapter
+// loader needs it before any UNet exists; set_image_prompt checks the result against the paths the UNet recorded while loading.
+static std::vector<std::pair<std::string, int>> unet_tblock_paths(const sdxl_unet_cfg& g) {
+  std::vector<std::pair<std::string, int>> out;
+  const int mc = g.model_channels, last = g.n_levels - 1;
+  auto st = [&](const std::string& bp, int level) {
+    for (int j = 0; j < g.transformer_depths[level]; ++j) out.push_back({bp + "/transformer/transformer_" + std::to_string(j), g.channel_mults[level] * mc});
+  };
+  int idx = 1;
+  for (int level = 0; level < g.n_levels; ++level) {
+    for (int k = 0; k < 2; ++k, ++idx)
+      if (level == 1 || level == 2) st("input_blocks/" + std::to_string(idx), level);
+    if (level != last) ++idx;
+  }
+  st("middle_block", last);
+  idx = 0;
+  for (int level = last; level >= 0; --level)
+    for (int k = 0; k < 3; ++k, ++idx)
+      if (level == 1 || level == 2) st("output_blocks/" + std::to_string(idx), level);
+  return out;
+}
+
+static int build_ip_adapter(sdxl_ip_adapter* a, const PackView& pv, Arena& A) {
+  const sdxl_ip_adapter_cfg& g = a->cfg;
+  const int ctx_dim = g.unet.context_dim;
+  Loader L{a->ctx, &pv, &A, a->ctx->stream};
+  std::set<std::string> names = {"image_proj/proj/weight", "image_proj/proj/bias", "image_proj/norm/weight", "image_proj/norm/bias"};
+  a->proj = L.linear("image_proj/proj", g.image_embed_dim, g.tokens_per_image * ctx_dim, true);
+  a->norm = L.norm("image_proj/norm", ctx_dim);
+  a->kv.clear();
+  a->paths.clear();
+  for (const auto& pc : unet_tblock_paths(g.unet)) {
+    if (L.err) return L.err;
+    Lin kv;
+    kv.K = ctx_dim; kv.Kpad = Loader::pad64(ctx_dim); kv.N = 2 * pc.second;
+    kv.w = A.get<__half>((size_t)kv.N * kv.Kpad);
+    if (!kv.w) return fail(a->ctx, 4005, "weight arena exhausted");
+    L.lin_into(pc.first + "/attn2/ip_key", kv.w, kv.Kpad, 0, ctx_dim, pc.second, 0);
+    L.lin_into(pc.first + "/attn2/ip_value", kv.w, kv.Kpad, pc.second, ctx_dim, pc.second, 0);
+    names.insert(pc.first + "/attn2/ip_key/weight");
+    names.insert(pc.first + "/attn2/ip_value/weight");
+    a->kv.push_back(kv);
+    a->paths.push_back(pc.first);
+  }
+  if (L.err) return L.err;
+  for (const auto& t : pv.t)   // e.g. a pack for a UNet with more transformer blocks
+    if (!names.count(t.first)) return fail(a->ctx, 4804, "IP-Adapter pack: tensor '%s' is not part of an adapter for this UNet cfg", t.first.c_str());
+  return 0;
+}
+
+extern "C" int sdxl_ip_adapter_load(sdxl_ctx* c, const sdxl_ip_adapter_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
+                                    sdxl_ip_adapter** out) {
+  if (!c || !cfg || !pack || !out) return fail(c, -1, "sdxl_ip_adapter_load: null argument");
+  *out = nullptr;
+  if (int r = check_unet_cfg(c, cfg->unet)) return r;
+  if (cfg->unet.is_refiner) return fail(c, 4800, "IP-Adapter: the refiner is not supported");
+  if (cfg->unet.context_dim < 8 || cfg->unet.context_dim % 8)
+    return fail(c, 4801, "IP-Adapter: context_dim = %d must be a positive multiple of 8", cfg->unet.context_dim);
+  if (cfg->image_embed_dim < 1) return fail(c, 4802, "IP-Adapter: image_embed_dim = %d must be >= 1", cfg->image_embed_dim);
+  if (cfg->tokens_per_image < 1 || cfg->tokens_per_image > 64)
+    return fail(c, 4803, "IP-Adapter: tokens_per_image = %d outside [1, 64]", cfg->tokens_per_image);
+  CU(c, cudaSetDevice(c->device));
+  std::unique_ptr<sdxl_ip_adapter> a(new sdxl_ip_adapter());
+  a->ctx = c;
+  a->cfg = *cfg;
+  int r = with_device_pack(c, pack, bytes, pack_on_device,
+                           [&](const PackView& pv) { return build_two_pass(a.get(), pv, build_ip_adapter); });
+  if (r) return r;
+  *out = a.release();
+  return 0;
+}
+
+extern "C" void sdxl_ip_adapter_destroy(sdxl_ip_adapter* a) {
+  if (!a) return;
+  cudaStreamSynchronize(a->ctx->stream);
+  delete a;
+}
+
+// tokens f16 [n * T, context_dim] = LayerNorm(e @ proj + b) of embeds f32 [n, D] in device memory. Queued on the ctx stream.
+static int ip_project(const sdxl_ip_adapter* a, int n, const float* e, __half* tokens) {
+  sdxl_ctx* c = a->ctx;
+  const Lin& P = a->proj;
+  TmpBufs T(c->stream);
+  float* y = (float*)T.get((size_t)n * P.N * sizeof(float));
+  if (!y) return fail(c, 4810, "IP-Adapter projection: cannot allocate %zu bytes", (size_t)n * P.N * sizeof(float));
+  for (int b0 = 0; b0 < n; b0 += 8)
+    KL(c, gemv_launch(c->stream, e + (size_t)b0 * P.K, P.K, std::min(8, n - b0), P.K, P.w, P.Kpad, P.b, nullptr, 0, P.N, 0, 0,
+                      y + (size_t)b0 * P.N, P.N));
+  KL(c, layernorm_launch(c->stream, y, a->norm.g, a->norm.b, a->norm.eps, n * a->cfg.tokens_per_image, a->cfg.unet.context_dim, tokens));
+  return 0;
+}
+
+extern "C" int sdxl_ip_adapter_project(sdxl_ip_adapter* a, int n, const float* embeds, int on_host, sdxl_half* tokens_out) {
+  if (!a || !embeds || !tokens_out || n < 1) return -1;
+  sdxl_ctx* c = a->ctx;
+  CU(c, cudaSetDevice(c->device));
+  TmpBufs T(c->stream);
+  const size_t in_bytes = (size_t)n * a->cfg.image_embed_dim * sizeof(float);
+  const size_t out_bytes = (size_t)n * a->cfg.tokens_per_image * a->cfg.unet.context_dim * sizeof(__half);
+  const float* e = embeds;
+  __half* o = (__half*)tokens_out;
+  if (on_host) {
+    float* d = (float*)T.get(in_bytes);
+    o = (__half*)T.get(out_bytes);
+    if (!d || !o) return fail(c, 4811, "ip_adapter_project: allocation failed");
+    CU(c, cudaMemcpyAsync(d, embeds, in_bytes, cudaMemcpyHostToDevice, c->stream));
+    e = d;
+  }
+  if (int r = ip_project(a, n, e, o)) return r;
+  if (on_host) {
+    CU(c, cudaMemcpyAsync(tokens_out, o, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+  }
+  return 0;
+}
+
+// Writes the buffers that depend on the prompt's values: the tokens of prompts and negatives, and the per-block scales. Everything
+// is computed into temporaries first and copied into `a` only when all of it has succeeded, so a failure leaves `a` unchanged.
+static int ip_write(sdxl_ctx* c, IpAttach& a, const sdxl_image_prompt& p, int n_tblocks) {
+  const int n = p.n_batch * p.n_images;
+  const size_t tok_bytes = (size_t)a.n_batch * a.S_ip * a.ad->cfg.unet.context_dim * sizeof(__half);
+  const size_t bytes = (size_t)n * a.ad->cfg.image_embed_dim * sizeof(float);
+  TmpBufs T(c->stream);
+  const float* e = p.embeds;
+  const float* neg = p.negative_embeds;
+  if (p.on_host || !neg) {
+    float* d = (float*)T.get(2 * bytes);
+    if (!d) return fail(c, 4820, "set_image_prompt: cannot allocate %zu bytes for the embeddings", 2 * bytes);
+    if (p.on_host) {
+      CU(c, cudaMemcpyAsync(d, p.embeds, bytes, cudaMemcpyHostToDevice, c->stream));
+      e = d;
+    }
+    if (neg && p.on_host) CU(c, cudaMemcpyAsync(d + bytes / sizeof(float), neg, bytes, cudaMemcpyHostToDevice, c->stream));
+    else if (!neg) CU(c, cudaMemsetAsync(d + bytes / sizeof(float), 0, bytes, c->stream));   // diffusers' default negative: zeros
+    if (p.on_host || !neg) neg = d + bytes / sizeof(float);
+  }
+  __half* tp = (__half*)T.get(tok_bytes);
+  __half* tn = (__half*)T.get(tok_bytes);
+  float* ts = (float*)T.get(n_tblocks * sizeof(float));
+  if (!tp || !tn || !ts) return fail(c, 4820, "set_image_prompt: cannot allocate the token staging buffers");
+  if (int r = ip_project(a.ad, n, e, tp)) return r;
+  if (int r = ip_project(a.ad, n, neg, tn)) return r;
+  std::vector<float> s(n_tblocks, p.scale);
+  if (p.block_scales_host) s.assign(p.block_scales_host, p.block_scales_host + n_tblocks);
+  CU(c, cudaMemcpyAsync(ts, s.data(), s.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));   // s and the caller's host memory; any failure of the work above surfaces here
+  CU(c, cudaMemcpyAsync(a.tok_pos, tp, tok_bytes, cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(a.tok_neg, tn, tok_bytes, cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(a.scales, ts, n_tblocks * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  return 0;
+}
+
+extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt* p) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  if (!p) {
+    if (!u->ip) return 0;
+    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
+    u->plan.reset();
+    u->ip.reset();
+    u->ip_version++;
+    return 0;
+  }
+  // validate everything first: on failure the attached state is unchanged
+  const sdxl_ip_adapter* ad = p->adapter;
+  if (!ad) return fail(c, 4830, "set_image_prompt: null adapter");
+  if (ad->ctx != c) return fail(c, 4831, "set_image_prompt: the adapter was created on another sdxl_ctx");
+  if (u->cfg.is_refiner) return fail(c, 4832, "set_image_prompt: IP-Adapter on the refiner is not supported");
+  if (const char* field = unet_cfg_mismatch(u->cfg, ad->cfg.unet))
+    return fail(c, 4833, "set_image_prompt: adapter cfg field '%s' differs from the UNet's", field);
+  const std::vector<const TBlock*> tbs = unet_tblocks(u);
+  if (tbs.size() != ad->kv.size()) return fail(c, 4834, "set_image_prompt: adapter has %zu blocks, the UNet %zu", ad->kv.size(), tbs.size());
+  for (size_t i = 0; i < tbs.size(); ++i)   // the plan indexes the adapter's K/V by the UNet's transformer-block order
+    if (tbs[i]->path != ad->paths[i] || tbs[i]->kv2.N != ad->kv[i].N)
+      return fail(c, 4834, "set_image_prompt: block %zu: adapter has '%s' (width %d), the UNet '%s' (width %d)", i, ad->paths[i].c_str(),
+                  ad->kv[i].N / 2, tbs[i]->path.c_str(), tbs[i]->kv2.N / 2);
+  if (!p->embeds) return fail(c, 4835, "set_image_prompt: null embeds");
+  if (p->n_batch < 1 || p->n_images < 1 || p->n_images > 64)
+    return fail(c, 4836, "set_image_prompt: n_batch = %d must be >= 1 and n_images = %d in [1, 64]", p->n_batch, p->n_images);
+  if (!isfinite(p->scale)) return fail(c, 4837, "set_image_prompt: scale is not finite");
+  if (p->block_scales_host)
+    for (size_t i = 0; i < tbs.size(); ++i)
+      if (!isfinite(p->block_scales_host[i])) return fail(c, 4837, "set_image_prompt: block scale %zu is not finite", i);
+  if (u->condB > 0)
+    if (int r = ip_check_batch(u, p->n_batch, u->condB, u->cfg_rows)) return r;
+  const int n_tb = (int)tbs.size();
+  if (u->ip && u->ip->ad == ad && u->ip->n_batch == p->n_batch && u->ip->n_images == p->n_images) {   // same buffers: plan stays
+    if (int r = ip_write(c, *u->ip, *p, n_tb)) return r;
+    return u->condB > 0 ? ip_hoist(u, *u->ip) : 0;
+  }
+  std::unique_ptr<IpAttach> a(new IpAttach());
+  a->ad = ad;
+  a->n_batch = p->n_batch;
+  a->n_images = p->n_images;
+  a->S_ip = p->n_images * ad->cfg.tokens_per_image;
+  const size_t tok = (size_t)p->n_batch * a->S_ip * u->cfg.context_dim;
+  if (a->mem.init(2 * tok * sizeof(__half) + n_tb * sizeof(float) + 4096)) return fail(c, 4838, "set_image_prompt: cannot allocate token buffers");
+  a->tok_pos = a->mem.get<__half>(tok);
+  a->tok_neg = a->mem.get<__half>(tok);
+  a->scales = a->mem.get<float>(n_tb);
+  if (u->condB > 0)
+    if (int r = ip_cond_alloc(u, *a)) return r;
+  if (int r = ip_write(c, *a, *p, n_tb)) return r;
+  if (u->condB > 0)
+    if (int r = ip_hoist(u, *a)) return r;
+  CU(c, cudaStreamSynchronize(c->stream));   // the old plan and attachment may still be in flight
+  u->plan.reset();
+  u->ip = std::move(a);
+  u->ip_version++;
   return 0;
 }
 
@@ -1197,6 +1525,7 @@ extern "C" double sdxl_unet_alpha(const sdxl_unet* u, int i) {
 // algorithmic FLOPs of the current plan (debug / bench helper, not in the public header)
 extern "C" double sdxl_unet_plan_flops(const sdxl_unet* u) { return (u && u->plan) ? u->plan->flops : 0.0; }
 extern "C" int sdxl_unet_plan_num_ops(const sdxl_unet* u) { return (u && u->plan) ? (int)u->plan->ops.size() : 0; }
+extern "C" uint64_t sdxl_unet_plan_builds(const sdxl_unet* u) { return u ? u->plan_builds : 0; }
 // FLOPs the plan's tensor-core launches actually execute (see Op::flops_exec): excludes the hoisted K/V projections (not in
 // the plan), counts the phase-decomposed upsample convs at 4/9 of the algorithmic figure, includes channel / key padding.
 extern "C" double sdxl_unet_plan_flops_executed(const sdxl_unet* u) {
@@ -1246,6 +1575,7 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
     if (a.h != h || a.w != w)
       return fail(c, 5205, "control %zu: its hint is %dx%d pixels but the resolution is %dx%d", k, 8 * a.h, 8 * a.w, 8 * h, 8 * w);
   }
+  if (int r = ip_check_batch(u, u->ip ? u->ip->n_batch : 0, nfwd * Bimg, nfwd == 2 ? Bimg : 0)) return r;
   Sampler* S = u->sampler.get();
   const size_t lat = (size_t)Bimg * g.in_channels * h * w;
   if (n_ctx < 1) return fail(c, 5202, "bad conditioning context length");
@@ -1274,7 +1604,7 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
       CU(c, cudaMemcpyAsync((uint8_t*)S->cond_ctx + ctx_row * (Bimg + b), ctx_u, ctx_row, kind, c->stream));
       CU(c, cudaMemcpyAsync((uint8_t*)S->cond_y + y_row * (Bimg + b), y_u, y_row, kind, c->stream));
     }
-  int r = set_conditioning_dev(u, nfwd * Bimg, n_ctx, S->cond_ctx, S->cond_y);
+  int r = set_conditioning_dev(u, nfwd * Bimg, n_ctx, S->cond_ctx, S->cond_y, nfwd == 2 ? Bimg : 0);
   if (r) return r;
   return ensure_plan(u, nfwd * Bimg, Bimg, h, w);
 }
@@ -1460,6 +1790,32 @@ extern "C" int sdxl_qkv_attention(sdxl_ctx* c, const sdxl_half* q, const sdxl_ha
   if (!r) r = make_tmap_rows(&p.tmV, (const __half*)v, S, B, C, C);
   if (r) return fail(c, r, "tensor map creation failed");
   KL(c, attention_launch(c->stream, p));
+  return 0;
+}
+
+extern "C" int sdxl_op_ip_attention(sdxl_ctx* c, const sdxl_half* q, const sdxl_half* k, const sdxl_half* v, const sdxl_half* k_ip,
+                                    const sdxl_half* v_ip, int B, int T, int S, int S_ip, int C, int n_head, float scale, sdxl_half* out) {
+  if (!c || !q || !k || !v || !k_ip || !v_ip || !out) return -1;
+  if (n_head < 1 || C != n_head * 64) return fail(c, 5302, "sdxl_op_ip_attention: head dim must be 64 (C=%d, n_head=%d)", C, n_head);
+  if (B < 1 || S_ip < 1) return fail(c, 5303, "sdxl_op_ip_attention: B = %d and S_ip = %d must be >= 1", B, S_ip);
+  CU(c, cudaSetDevice(c->device));
+  TmpBufs tmp(c->stream);
+  float* s = (float*)tmp.get(sizeof(float));
+  if (!s) return fail(c, 5304, "temporary allocation failed");
+  CU(c, cudaMemcpyAsync(s, &scale, sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  AttnParams p{};
+  p.T = T; p.S = S; p.n_head = n_head; p.B = B;
+  p.out = (__half*)out; p.ldo = C;
+  p.scale_log2e = (float)(1.4426950408889634 / sqrt(64.0));
+  p.S_ip = S_ip; p.ip_scale = s;
+  int r = make_tmap_rows(&p.tmQ, (const __half*)q, T, B, C, C);
+  if (!r) r = make_tmap_rows(&p.tmK, (const __half*)k, S, B, C, C);
+  if (!r) r = make_tmap_rows(&p.tmV, (const __half*)v, S, B, C, C);
+  if (!r) r = make_tmap_rows(&p.tmKip, (const __half*)k_ip, S_ip, B, C, C);
+  if (!r) r = make_tmap_rows(&p.tmVip, (const __half*)v_ip, S_ip, B, C, C);
+  if (r) return fail(c, r, "tensor map creation failed");
+  KL(c, attention_launch(c->stream, p));
+  CU(c, cudaStreamSynchronize(c->stream));   // `scale` lives on the caller's stack
   return 0;
 }
 

@@ -438,7 +438,7 @@ struct Op {
   struct { const float* x; int B, C, HW; const float* w; const float* bias; float inv_scale; float* y; } pq;
   struct { const int* tokens; int rows, T, C, n_vocab; const __half* tok; const __half* pos; float* x; int* err; } em;
   struct { const __half* q; int q_pitch, q_col0; const __half* k; const __half* v; int kv_pitch, k_col0, v_col0, B, T, S, n_head;
-           const __half* mask; int causal; __half* out; int ldo; } as;
+           const __half* mask; int causal; __half* out; int ldo; int head_dim; } as;
   struct { const float* x; size_t n; int quick; __half* y; } ac;
   struct { const float* x; const int* idx; int B, T, C; const float* g; const float* b; float eps; float* y; } lg;
 };
@@ -447,6 +447,7 @@ struct Plan {
   int Bf = 0, Bx = 0, h = 0, w = 0;
   uint64_t cond_version = 0;
   uint64_t controls_version = 0;   // UNet: the attached ControlNet set the plan was built for
+  uint64_t ip_version = 0;         // UNet: the image-prompt attachment the plan was built for
   Arena arena;
   std::vector<Op> ops;
   float* x_in = nullptr;  // [Bx, Cin, h, w] f32 NCHW
@@ -669,7 +670,7 @@ static int exec_op(sdxl_ctx* c, Op& op) {
     case OP_EMBED: KL(c, embed_tokens_launch(st, op.em.tokens, op.em.rows, op.em.T, op.em.C, op.em.n_vocab, op.em.tok, op.em.pos, op.em.x, op.em.err)); break;
     case OP_ATTN_SMALL:
       KL(c, attention_small_launch(st, op.as.q, op.as.q_pitch, op.as.q_col0, op.as.k, op.as.v, op.as.kv_pitch, op.as.k_col0, op.as.v_col0,
-                                   op.as.B, op.as.T, op.as.S, op.as.n_head, op.as.mask, op.as.causal, op.as.out, op.as.ldo));
+                                   op.as.B, op.as.T, op.as.S, op.as.n_head, op.as.mask, op.as.causal, op.as.out, op.as.ldo, op.as.head_dim));
       break;
     case OP_ACT: KL(c, mlp_act_launch(st, op.ac.x, op.ac.n, op.ac.quick, op.ac.y)); break;
     case OP_LN_GATHER: KL(c, ln_gather_f32_launch(st, op.lg.x, op.lg.idx, op.lg.B, op.lg.T, op.lg.C, op.lg.g, op.lg.b, op.lg.eps, op.lg.y)); break;

@@ -127,7 +127,7 @@ int igemm_launch(cudaStream_t st, IgemmParams& p);
 int igemm_pick_bn(int m_tiles, int N, int num_sms, bool geglu);
 
 // ------------------------------------------------------------------------------------------------
-// Attention (attention.cu): out[b, t, h*64:(h+1)*64] = softmax(q k^T / 8) v, head dim 64.
+// Attention (attention.cu): out[b, t, h*64:(h+1)*64] = softmax(q k^T / 8) v, head dim 64 (+ an optional second source).
 // q/k/v are column windows of row-major f16 matrices (fused QKV / KV GEMM outputs).
 // ------------------------------------------------------------------------------------------------
 struct AttnParams {
@@ -137,6 +137,12 @@ struct AttnParams {
   __half* out;                 // [B*T, ldo]
   int ldo;
   float scale_log2e;           // (1/sqrt(d)) * log2(e)
+  // Second key/value source (IP-Adapter's decoupled cross-attention), used when S_ip > 0:
+  //   out = softmax(q k^T) v + (*ip_scale) * softmax(q k_ip^T) v_ip      (two separate softmaxes, same scale)
+  CUtensorMap tmKip, tmVip;    // 3D maps (64 cols, S_ip rows, batch)
+  int S_ip;
+  int k_ip_col0, v_ip_col0;
+  const float* ip_scale;       // device scalar
 };
 int make_tmap_rows(CUtensorMap* tm, const __half* base, int rows_per_batch, int nbatch, int cols, int pitch);
 int attention_launch(cudaStream_t st, const AttnParams& p);
@@ -238,10 +244,16 @@ int quant_out_launch(cudaStream_t st, const float* x, int B, int Cz, int Cout, l
 // x[b*T+t,:] = tok_emb[tokens[b,t],:] + pos_emb[t,:] (f16 tables -> f32); *err is set to 1 on an id outside [0, n_vocab).
 int embed_tokens_launch(cudaStream_t st, const int* tokens, int rows, int T, int C, int n_vocab, const __half* tok_emb,
                         const __half* pos_emb, float* x, int* err);
-// Masked attention for short sequences, head dim 64: additive f16 mask [T,S] (nullable) and/or causal (key <= query).
+// Masked attention for short sequences, scale 1/sqrt(head_dim): additive f16 mask [T,S] (nullable) and/or causal (key <= query).
+// head_dim: 64 (the text encoders' kernel) or another multiple of 8 up to 128.
 int attention_small_launch(cudaStream_t st, const __half* q, int q_pitch, int q_col0, const __half* k, const __half* v,
                            int kv_pitch, int k_col0, int v_col0, int B, int T, int S, int n_head, const __half* mask,
-                           int causal, __half* out, int ldo);
+                           int causal, __half* out, int ldo, int head_dim = 64);
+// CLIP vision embedding: pixels f32 NCHW [N,3,S,S] -> f16 patch rows [N*(S/p)^2, Kpad], columns in OIHW (c, kh, kw) order.
+int patchify_launch(cudaStream_t st, const float* pixels, int N, int S, int p, int Kpad, __half* y);
+// x f32 [N*T, C] = LayerNorm([class ; patches[n]] + position) (T = patches per image + 1).
+int vision_embed_ln_launch(cudaStream_t st, const float* patches, const __half* cls, const __half* pos, int N, int T, int C,
+                           const float* gamma, const float* beta, float eps, float* x);
 // y = gelu_erf(x) (quick = 0) or x * sigmoid(1.702 x) (quick = 1); f32 -> f16, n % 4 == 0.
 int mlp_act_launch(cudaStream_t st, const float* x, size_t n, int quick, __half* y);
 // y[b,:] = LayerNorm(x[b*T + idx[b], :]) in f32.

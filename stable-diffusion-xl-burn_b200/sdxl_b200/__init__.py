@@ -9,4 +9,6 @@ from .tokenizer import ClipTokenizer, OpenClipTokenizer  # noqa: F401
 from .embedder import ClipTextEncoder, Embedder, conditioning_embedding  # noqa: F401
 from .pipeline import load_models, make_inpaint_mask, sample  # noqa: F401
 from .controlnet import ControlNet  # noqa: F401
+from .ip_adapter import IPAdapter  # noqa: F401
+from .clip_vision import SDXL_VIT_BIGG, SDXL_VIT_H, ClipVisionConfig, ClipVisionEncoder, clip_preprocess  # noqa: F401
 from . import burn_record  # noqa: F401

@@ -76,6 +76,19 @@ class Control(C.Structure):
 MAX_CONTROLS = 4    # SDXL_MAX_CONTROLS (include/sdxl_b200.h)
 
 
+class ClipVisionCfg(C.Structure):
+    _fields_ = [(n, C.c_int32) for n in ("n_state", "n_head", "n_layer", "mlp_dim", "image_size", "patch_size", "proj_dim", "quick_gelu")]
+
+
+class IpAdapterCfg(C.Structure):
+    _fields_ = [("unet", UnetCfg), ("image_embed_dim", C.c_int32), ("tokens_per_image", C.c_int32)]
+
+
+class ImagePrompt(C.Structure):
+    _fields_ = [("adapter", C.c_void_p), ("embeds", C.c_void_p), ("negative_embeds", C.c_void_p), ("on_host", C.c_int32),
+                ("n_batch", C.c_int32), ("n_images", C.c_int32), ("scale", C.c_float), ("block_scales_host", C.c_void_p)]
+
+
 # name -> (restype, argtypes); every symbol include/sdxl_b200.h declares
 P = C.c_void_p
 I = C.c_int
@@ -139,6 +152,15 @@ PROTOTYPES = {
     "sdxl_controlnet_destroy": (None, [P]),
     "sdxl_unet_set_controls": (I, [P, I, C.POINTER(Control)]),
     "sdxl_controlnet_embed_hint": (I, [P, I, I, I, P, I, P]),
+    "sdxl_clip_vision_load": (I, [P, C.POINTER(ClipVisionCfg), P, C.c_size_t, I, C.POINTER(P)]),
+    "sdxl_clip_vision_destroy": (None, [P]),
+    "sdxl_clip_vision_encode": (I, [P, I, P, I, P]),
+    "sdxl_unet_plan_builds": (C.c_uint64, [P]),
+    "sdxl_ip_adapter_load": (I, [P, C.POINTER(IpAdapterCfg), P, C.c_size_t, I, C.POINTER(P)]),
+    "sdxl_ip_adapter_destroy": (None, [P]),
+    "sdxl_unet_set_image_prompt": (I, [P, C.POINTER(ImagePrompt)]),
+    "sdxl_ip_adapter_project": (I, [P, I, P, I, P]),
+    "sdxl_op_ip_attention": (I, [P, P, P, P, P, P, I, I, I, I, I, I, C.c_float, P]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),
     "sdxl_mpk_encode_u16": (C.c_size_t, [P, C.c_size_t, P]),

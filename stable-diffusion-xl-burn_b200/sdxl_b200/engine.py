@@ -284,6 +284,9 @@ class Diffuser:
             if getattr(self, "_controls", None):   # the destroyed UNet no longer uses its ControlNets
                 from .controlnet import release_controls
                 release_controls(self)
+            if getattr(self, "_image_prompt", None):
+                from .ip_adapter import release_image_prompt
+                release_image_prompt(self)
 
     def __del__(self):
         try:
@@ -300,6 +303,13 @@ class Diffuser:
         hint: f32 [n, 3, H, W] in [0, 1] or u8 [n, H, W, 3]; image b of a batch uses hint b % n."""
         from .controlnet import set_controls
         set_controls(self, controls)
+
+    def set_image_prompt(self, adapter, embeds=None, scale=1.0, negative=None) -> None:
+        """Attaches an IP-Adapter image prompt (sdxl_unet_set_image_prompt); adapter None detaches. embeds: f32 [n_batch, D] or
+        [n_batch, n_images, D] (CLIP vision image_embeds); image b of a batch uses prompt b % n_batch. scale: float, or one per
+        transformer block in execution order (ip_adapter.transformer_block_paths). negative: the CFG rows' embeddings (zeros)."""
+        from .ip_adapter import set_image_prompt
+        set_image_prompt(self, adapter, embeds, scale, negative)
 
     # ---- UNet::forward -------------------------------------------------------------------------
     def set_conditioning(self, context: torch.Tensor, label: torch.Tensor) -> None:

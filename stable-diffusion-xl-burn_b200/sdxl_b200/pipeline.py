@@ -28,13 +28,23 @@ def make_inpaint_mask(img_hw: Tuple[int, int], latent_hw: Tuple[int, int], crop_
 def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_steps: int = 30, refiner=None,
            reference_rgb: Optional[torch.Tensor] = None, crop: Sequence[Optional[int]] = (None, None, None, None), crop_out: bool = False,
            resolution: Tuple[int, int] = (1024, 1024), seed: int = 0, noise: Optional[torch.Tensor] = None,
-           loras: Optional[Sequence] = None, controls: Optional[Sequence] = None) -> torch.Tensor:
+           loras: Optional[Sequence] = None, controls: Optional[Sequence] = None, image_prompt: Optional[Sequence] = None) -> torch.Tensor:
     """One image, like `sample --prompt ... [--reference-img ... --crop-* ...] [--use-refiner]`.
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
     bottom) in pixels. loras: [(kohya .safetensors path / bytes / tensor dict, scale), ...] merged into the base UNet and both
     text encoders for this call (the refiner is left alone) and removed again afterwards, which also clears any adapter set
     those models had. controls: [(ControlNet, image u8 [1, H, W, 3] or f32 [1, 3, H, W], scale), ...] attached to the base UNet
-    for this call and detached afterwards (the refiner is left alone). Returns uint8 [1, H, W, 3]."""
+    for this call and detached afterwards (the refiner is left alone). image_prompt: (IPAdapter, ClipVisionEncoder, images u8
+    [n_images, H, W, 3], scale): the images are encoded and attached to the base UNet as one prompt of n_images images for this call
+    and detached afterwards. Returns uint8 [1, H, W, 3]."""
+    if image_prompt:
+        adapter, encoder, images, scale = image_prompt
+        diffuser.set_image_prompt(adapter, encoder.encode_images(images).unsqueeze(0), scale)
+        try:
+            return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
+                          seed, noise, loras, controls)
+        finally:
+            diffuser.set_image_prompt(None)
     if controls:
         diffuser.set_controls(controls)
         try:

@@ -1,0 +1,141 @@
+#!/usr/bin/env python
+"""Sampler step time without an image prompt, with 1 image (4 tokens) and with 4 images (16 tokens), the attention kernel's
+share of a step, the set_image_prompt time and the vision encoder's time per image (ViT-H/14, ViT-bigG/14); SDXL base + a
+ViT-H-sized IP-Adapter (synthetic weights) on one GPU.
+
+    python tools/ip_adapter_bench.py [out.json] [--steps K] [--warmup W] [--reps R]
+
+Step time: bench.py's method (sampler_begin, W warm-up steps, CUDA events around K sampler steps, CFG 7.5 at 1024^2, batch 1),
+with no prompt, 1 and 4 images alternated R times in one process; the order rotates from one alternation to the next, so a
+clock that drifts during the run does not always fall on the same configuration. Attention share: profile_plan of one step (CUDA events per
+launch, eager). set_image_prompt: host wall clock around a call that ends in a stream synchronise (embedding upload, token
+projection, K/V hoist of the 70 cross-attentions), median of R, for a new attachment (plan rebuilt at the next step) and for a
+scale change (in place). The card's name, power limit and clocks are read in the same run.
+"""
+import json
+import os
+import statistics
+import sys
+import time
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+for p in (ROOT, os.path.join(ROOT, "stable-diffusion-xl-burn_b200"), os.path.join(ROOT, "tools")):
+    sys.path.insert(0, p)
+
+import torch  # noqa: E402
+import sdxl_b200  # noqa: E402
+from sdxl_b200 import build_pack  # noqa: E402
+from sdxl_b200.clip_vision import SDXL_VIT_BIGG, SDXL_VIT_H, ClipVisionEncoder, synth_vision_weights  # noqa: E402
+from sdxl_b200.ip_adapter import synth_ip_adapter  # noqa: E402
+from controlnet_bench import gpu_info  # noqa: E402
+
+HW = 1024
+D = 1024   # ViT-H/14 image_embeds
+
+
+def main():
+    args = sys.argv[1:]
+    opt = lambda name, d: type(d)(args[args.index(name) + 1]) if name in args else d  # noqa: E731
+    steps, warmup, reps = opt("--steps", 31), opt("--warmup", 4), opt("--reps", 3)
+    out_path = args[0] if args and not args[0].startswith("--") else None
+    ctx = sdxl_b200.Context(0)
+    dev = str(ctx.device)
+    res = {"gpu": gpu_info()}
+    d = sdxl_b200.Diffuser(ctx, sdxl_b200.SDXL_BASE, sdxl_b200.build_pack(sdxl_b200.synth_weights(sdxl_b200.SDXL_BASE, seed=0, device=dev)))
+    ad = sdxl_b200.IPAdapter(ctx, sdxl_b200.SDXL_BASE, D, synth_ip_adapter(sdxl_b200.SDXL_BASE, D, seed=1))
+    torch.cuda.empty_cache()
+    g = lambda s: torch.Generator().manual_seed(s)  # noqa: E731
+    emb = {k: torch.randn(1, k, D, generator=g(10 + k)) for k in (1, 4)}
+    cond = sdxl_b200.Conditioning(
+        context_full=torch.randn(1, 77, 2048, generator=g(1)).half(), unconditional_context_full=torch.randn(77, 2048, generator=g(2)).half(),
+        channel_context=torch.randn(1, 2816, generator=g(3)).half(), unconditional_channel_context=torch.randn(2816, generator=g(4)).half(),
+        resolution=(HW, HW))
+    ts = sdxl_b200.ddim_timesteps(30)
+    step_size = 1000 // 30
+
+    def attach(k):
+        d.set_image_prompt(ad, emb[k], 1.0) if k else d.set_image_prompt(None)
+        d.sampler_begin(cond, 7.5)
+
+    def run_steps():
+        d.sampler_set_latent(ctx.randn(4 * (HW // 8) ** 2, seed=0).reshape(1, 4, HW // 8, HW // 8))
+        for i in range(warmup):
+            t = ts[i % len(ts)]
+            d.sampler_step(t, t - step_size if t >= step_size else -1)
+        ctx.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(ctx.stream)
+        for i in range(steps):
+            t = ts[i % len(ts)]
+            d.sampler_step(t, t - step_size if t >= step_size else -1)
+        e1.record(ctx.stream)
+        ctx.synchronize()
+        return e0.elapsed_time(e1) / steps
+
+    step = {0: [], 1: [], 4: []}
+    order = [0, 1, 4]
+    for r in range(reps):
+        for k in order[r % 3:] + order[:r % 3]:
+            attach(k)
+            step[k].append(round(run_steps(), 3))
+    res["step_ms"] = {f"{k}_images": {"median": statistics.median(v), "runs": v} for k, v in step.items()}
+    b = res["step_ms"]["0_images"]["median"]
+    res["step_ratio_vs_base"] = {k: round(v["median"] / b, 3) for k, v in res["step_ms"].items()}
+    res["gpu_after_steps"] = gpu_info()
+    print(json.dumps(res["step_ms"]), flush=True)
+
+    res["attention"] = {}
+    for k in (0, 1, 4):
+        attach(k)
+        run_steps()
+        prof = d.profile_plan()
+        total = sum(v["ms"] for v in prof.values())
+        a = prof.get("attention_wgmma", {"ms": 0.0, "launches": 0})
+        res["attention"][f"{k}_images"] = {"attention_ms": round(a["ms"], 3), "launches": a["launches"], "step_ms_eager": round(total, 3),
+                                           "share": round(a["ms"] / total, 4), "plan_flops": d.plan_flops}
+
+    def timed(fn, before=lambda: None):
+        ts_ = []
+        for _ in range(reps):
+            before()
+            ctx.synchronize()
+            t0 = time.perf_counter()
+            fn()
+            ctx.synchronize()
+            ts_.append((time.perf_counter() - t0) * 1e3)
+        return round(statistics.median(ts_), 2)
+
+    attach(0)
+    res["set_image_prompt_ms"] = {
+        "attach_one_image": timed(lambda: d.set_image_prompt(ad, emb[1], 1.0), before=lambda: d.set_image_prompt(None)),
+        "rescale_in_place": timed(lambda: d.set_image_prompt(ad, emb[1], 0.6)),
+    }
+    d.set_image_prompt(None)
+    res["encode_ms_per_image"] = {}
+    for name, vcfg in (("vit_h", SDXL_VIT_H), ("vit_bigg", SDXL_VIT_BIGG)):
+        enc = ClipVisionEncoder(ctx, vcfg, build_pack(synth_vision_weights(vcfg, seed=2, device=dev)))
+        px = torch.randn(4, 3, 224, 224, device=ctx.device)
+        for _ in range(3):
+            enc.encode(px)
+        ctx.synchronize()
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record(ctx.stream)
+        for _ in range(10):
+            enc.encode(px)
+        e1.record(ctx.stream)
+        ctx.synchronize()
+        res["encode_ms_per_image"][name] = round(e0.elapsed_time(e1) / 40, 3)
+        enc.close()
+        torch.cuda.empty_cache()
+    res["gpu_after"] = gpu_info()
+    print(json.dumps(res))
+    if out_path:
+        with open(out_path, "w") as f:
+            json.dump(res, f, indent=1)
+    ad.close()
+    d.close()
+    ctx.close()
+
+
+if __name__ == "__main__":
+    main()
