@@ -1,4 +1,5 @@
-"""Builds libsdxl_b200.so (hand-written sm_90a CUDA + C++ host, C ABI in include/sdxl_b200.h).
+"""Builds libsdxl_b200.so (hand-written sm_90a CUDA + C++ host, C ABI in include/sdxl_b200.h) and libsdxl_b200_testing.so
+(the same kernel objects behind the test-only entry points of csrc/testing.cu, bound by sdxl_b200/_testing.py).
 
 In-tree build with plain nvcc (cross-compiles on a machine without a GPU). The .so is git-ignored but
 travels with the repo snapshot to the GPU box. `python build.py` or `build_library()`.
@@ -15,7 +16,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "sdxl_b200", "libsdxl_b200.so")
-SOURCES = ["igemm.cu", "attention.cu", "norm.cu", "elementwise.cu", "vae_kernels.cu", "clip_kernels.cu", "engine.cu", "vae.cu", "clip.cu", "tokenizer.cpp", "mpk.cpp"]
+TEST_LIB = os.path.join(HERE, "sdxl_b200", "libsdxl_b200_testing.so")
+KERNEL_SOURCES = ["igemm.cu", "attention.cu", "norm.cu", "elementwise.cu", "vae_kernels.cu", "clip_kernels.cu"]
+SOURCES = KERNEL_SOURCES + ["engine.cu", "vae.cu", "clip.cu", "tokenizer.cpp", "mpk.cpp"]
+TEST_SOURCES = ["testing.cu"]
 HEADERS = ["common.cuh", "kernels.h", "engine_core.h", "unicode_tables.h", os.path.join("..", "..", "include", "sdxl_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
@@ -26,7 +30,7 @@ FLAGS = [
 
 def _digest() -> str:
     h = hashlib.sha256()
-    for f in SOURCES + HEADERS:
+    for f in SOURCES + TEST_SOURCES + HEADERS:
         with open(os.path.join(CSRC, f), "rb") as fh:
             h.update(fh.read())
     h.update(" ".join(FLAGS).encode())
@@ -37,7 +41,7 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
     os.makedirs(BUILD, exist_ok=True)
     stamp = os.path.join(BUILD, "stamp")
     dg = _digest()
-    if not force and os.path.exists(LIB) and os.path.exists(stamp) and open(stamp).read() == dg:
+    if not force and os.path.exists(LIB) and os.path.exists(TEST_LIB) and os.path.exists(stamp) and open(stamp).read() == dg:
         return LIB
 
     def cc(src: str) -> str:
@@ -50,12 +54,19 @@ def build_library(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed for {src}:\n{r.stdout}\n{r.stderr}")
         return obj
 
-    with ThreadPoolExecutor(max_workers=len(SOURCES)) as ex:
-        objs = list(ex.map(cc, SOURCES))
-    cmd = [NVCC, "-shared", "-o", LIB, *objs, "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler", "-fPIC", "-ldl"]
-    r = subprocess.run(cmd, capture_output=True, text=True)
-    if r.returncode != 0:
-        raise RuntimeError(f"link failed:\n{r.stdout}\n{r.stderr}")
+    with ThreadPoolExecutor(max_workers=len(SOURCES + TEST_SOURCES)) as ex:
+        objs = dict(zip(SOURCES + TEST_SOURCES, ex.map(cc, SOURCES + TEST_SOURCES)))
+
+    def link(out: str, srcs: list, extra: tuple = ()) -> None:
+        cmd = [NVCC, "-shared", "-o", out, *(objs[s] for s in srcs), "-gencode", "arch=compute_90a,code=sm_90a", "-Xcompiler",
+               "-fPIC", "-ldl", *extra]
+        r = subprocess.run(cmd, capture_output=True, text=True)
+        if r.returncode != 0:
+            raise RuntimeError(f"link of {os.path.basename(out)} failed:\n{r.stdout}\n{r.stderr}")
+
+    link(LIB, SOURCES)
+    # the kernels alone, without the engine: an unresolved symbol is a link error rather than a dlopen failure on the GPU host
+    link(TEST_LIB, TEST_SOURCES + KERNEL_SOURCES, ("-Xlinker", "--no-undefined"))
     with open(stamp, "w") as fh:
         fh.write(dg)
     return LIB

@@ -150,8 +150,8 @@ int attention_launch(cudaStream_t st, const AttnParams& p);
 // ------------------------------------------------------------------------------------------------
 // Norms (norm.cu)
 // ------------------------------------------------------------------------------------------------
-// GroupNorm over NHWC f32 input (optionally the channel-concatenation of two tensors), 32 groups,
-// biased variance, eps inside the sqrt (reference groupnorm/mod.rs:52-82). Writes f16.
+// GroupNorm over NHWC f32 input (optionally the channel-concatenation of two tensors), n_group groups (a multiple of 4 up
+// to 64; the UNet and VAE use 32), biased variance, eps inside the sqrt (reference groupnorm/mod.rs:52-82). Writes f16.
 struct GnParams {
   const float* x1; int C1;    // [B, HW, C1]
   const float* x2; int C2;    // nullable, [B, HW, C2]  (cat([x1, x2], channel))
@@ -161,7 +161,8 @@ struct GnParams {
   int silu;                   // apply x*sigmoid(x) after the affine
   __half* y;                  // [B, HW, C1+C2] normalised (+SiLU) output
   __half* raw;                // nullable: un-normalised f16 copy of cat([x1,x2]) (skip-conv operand)
-  float* partial;             // scratch of gn_scratch_floats(B, n_group) floats, initialised once with gn_scratch_init
+  float* partial;             // scratch of gn_scratch_floats(B', n_group') floats (B' >= B, n_group' >= n_group), initialised once
+                              // with gn_scratch_init and then shared by any number of GroupNorms
   int nchunk;                 // filled by gn_launch
   __half* y_lo;               // nullable: f16(t - float(y)), the rounding residue of y (hi/lo split operand of the UNet's last conv)
 };

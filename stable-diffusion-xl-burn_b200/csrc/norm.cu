@@ -13,12 +13,17 @@ namespace sdxl {
 static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 static constexpr int kGnMaxChunk = 512;
 
-// scratch layout: [B][kGnMaxChunk][G][2] chunk partials | [B][G][2] final (mean, rstd) | [B] arrival counters (zero between uses)
-size_t gn_scratch_floats(int B, int n_group) { return (size_t)B * kGnMaxChunk * n_group * 2 + (size_t)B * n_group * 2 + (size_t)B + 16; }
-static inline float* gn_final(float* scratch, int B, int n_group) { return scratch + (size_t)B * kGnMaxChunk * n_group * 2; }
-static inline unsigned* gn_counters(float* scratch, int B, int n_group) { return reinterpret_cast<unsigned*>(gn_final(scratch, B, n_group) + (size_t)B * n_group * 2); }
+// scratch layout: [B + 16, padded to 4] arrival counters (zero between uses) | [B][kGnMaxChunk][G][2] chunk partials |
+// [B][G][2] final (mean, rstd). The counters come first so that a scratch initialised for (B, G) serves every GroupNorm with
+// B' <= B and G' <= G: they sit at the same place whatever the shape, and only they must be zero on entry.
+static inline size_t gn_counter_floats(int B) { return ((size_t)B + 16 + 3) & ~(size_t)3; }
+size_t gn_scratch_floats(int B, int n_group) { return gn_counter_floats(B) + (size_t)B * kGnMaxChunk * n_group * 2 + (size_t)B * n_group * 2; }
+static inline float* gn_partials(float* scratch, int B) { return scratch + gn_counter_floats(B); }
+static inline float* gn_final(float* scratch, int B, int n_group) { return gn_partials(scratch, B) + (size_t)B * kGnMaxChunk * n_group * 2; }
+static inline unsigned* gn_counters(float* scratch) { return reinterpret_cast<unsigned*>(scratch); }
 int gn_scratch_init(cudaStream_t st, float* scratch, int B, int n_group) {
-  return (int)cudaMemsetAsync(gn_counters(scratch, B, n_group), 0, ((size_t)B + 16) * sizeof(unsigned), st);
+  (void)n_group;
+  return (int)cudaMemsetAsync(gn_counters(scratch), 0, gn_counter_floats(B) * sizeof(unsigned), st);
 }
 
 // Pivot of a (sample, group): the mean of four of its elements (first / middle channel at the first / middle pixel). Sums are
@@ -112,9 +117,12 @@ __global__ void gn_stats_kernel(const float* __restrict__ x1, int C1, const floa
   if (threadIdx.x == 0) s_ticket = atomicAdd(&counters[b], 1u);
   __syncthreads();
   if (s_ticket != (unsigned)(nchunk - 1)) return;
-  // last CTA of sample b: 8 lanes per group walk the chunk partials in chunk order (deterministic), in double precision
+  // last CTA of sample b: 8 lanes per group walk the chunk partials in chunk order (deterministic), in double precision.
+  // Only whole warps take part (blockDim.x >= 32 but not always a multiple of it) and n_group % 4 == 0 (gn_launch), so every
+  // warp either reduces four complete groups or skips the loop: the full-mask shuffles below always see all 32 lanes.
   __threadfence();
-  for (int g = threadIdx.x >> 3; g < n_group; g += blockDim.x >> 3) {
+  const int nred = blockDim.x & ~31;
+  for (int g = threadIdx.x >> 3; threadIdx.x < nred && g < n_group; g += nred >> 3) {
     const int sub = threadIdx.x & 7;
     double S = 0.0, Q = 0.0;
     for (int k0 = sub; k0 < nchunk; k0 += 64) {   // eight independent loads in flight, summed in chunk order
@@ -233,7 +241,8 @@ __global__ void gn_apply_kernel(const float* __restrict__ x1, int C1, const floa
 
 int gn_launch(cudaStream_t st, GnParams& p) {
   const int C = p.C1 + p.C2;
-  if ((p.C1 & 7) || (p.C2 & 7) || C % p.n_group || p.n_group > 64) return 3001;
+  // n_group % 4 == 0: the stats kernel's final reduction gives each group 8 lanes of a full-mask warp shuffle
+  if ((p.C1 & 7) || (p.C2 & 7) || p.n_group < 4 || (p.n_group & 3) || p.n_group > 64 || C % p.n_group) return 3001;
   const int V = C / 4;
   if (V > 1024) return 3002;
   int R = 512 / V;
@@ -249,9 +258,9 @@ int gn_launch(cudaStream_t st, GnParams& p) {
   static bool optin[64];
   if (int r = smem_optin(gn_stats_kernel, 160 * 1024, optin)) return r;
   float* fin = gn_final(p.partial, p.B, p.n_group);
-  unsigned* cnt = gn_counters(p.partial, p.B, p.n_group);
+  unsigned* cnt = gn_counters(p.partial);
   int e = launch_kernel(gn_stats_kernel, dim3(nchunk, p.B), dim3(V * R), smem1, st, true, p.x1, p.C1, p.x2, p.C2, p.HW,
-                        p.n_group, R, p.eps, p.partial, fin, cnt);
+                        p.n_group, R, p.eps, gn_partials(p.partial, p.B), fin, cnt);
   if (e) return e;
   const int V8 = C / 8;
   int R2 = 256 / V8;

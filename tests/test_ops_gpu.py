@@ -137,8 +137,10 @@ def test_qkv_attention(ctx, B, T, S, nh):
 
 @pytest.mark.parametrize("scale", [1.5, 3.0, 6.0])
 def test_qkv_attention_large_dynamic_range(ctx, scale):
-    """Scores whose row maximum jumps between key blocks — by a little (lazy reference kept), by more than 2^8 (the row's
-    O accumulator is rescaled in TMEM) and by far more than 2^15 (overflow fallback: the block is re-run with its exact max)."""
+    """Scores whose row maximum grows between 128-key blocks (keys 300 and up are doubled, so the third block takes over):
+    score spreads of a few units (scale 1.5), tens (3.0) and hundreds (6.0). The kernel keeps the exact running maximum of
+    every key block and rescales the row's O and l registers by exp(m_old - m_new) when it grows — at scale 6 that factor
+    underflows to 0 and the earlier blocks drop out — so every probability is <= 1 before its f16 rounding."""
     g = torch.Generator().manual_seed(int(scale * 10))
     B, T, S, nh = 1, 256, 640, 2
     q = h16(torch.randn(B, T, nh * 64, generator=g) * scale)
