@@ -106,7 +106,8 @@ SDXL_API int sdxl_unet_load_broadcast(sdxl_ctx* ctx, const sdxl_unet_cfg* cfg, c
 SDXL_API void sdxl_unet_destroy(sdxl_unet* unet);
 /* Step-invariant part of UNet::forward, hoisted: cross-attention K/V projections of `context`
  * (unet/mod.rs:1010-1011 for attn2) and the label-embedding MLP (unet/mod.rs:464-466).
- * context [B, n_ctx, context_dim] f16, y [B, adm_in_channels] f16. */
+ * context [B, n_ctx, context_dim] f16, y [B, adm_in_channels] f16. A call whose buffers for a new (B, n_ctx) cannot
+ * be allocated returns non-zero and leaves the previous conditioning in effect. */
 SDXL_API int sdxl_unet_set_conditioning(sdxl_unet* unet, int B, int n_ctx, const sdxl_half* context,
                                const sdxl_half* y);
 /* == UNet::forward (src/model/unet/mod.rs:449-493) with the conditioning set above.

@@ -67,7 +67,6 @@ extern "C" uint64_t sdxl_ctx_launch_count(const sdxl_ctx* c) { return c ? c->lau
 // model
 // ================================================================================================
 struct TBlock {
-  std::string path;   // reference path, e.g. input_blocks/4/transformer/transformer_0
   Norm n1, n2, n3;
   Lin qkv, out1;      // self-attention (fused [3C, C])
   Lin q2, kv2, out2;  // cross-attention (kv fused [2C, ctx])
@@ -80,14 +79,67 @@ struct Res {
   int Cin = 0, Cout = 0, temb_off = 0;
   bool has_skip = false;
 };
-enum BlockType { BT_CONV, BT_RES, BT_DOWN, BT_REST, BT_RESTU, BT_RESU };
+// BT_MID: the middle block (ResBlock, SpatialTransformer, ResBlock); the others are the Block types below.
+enum BlockType { BT_CONV, BT_RES, BT_DOWN, BT_REST, BT_RESTU, BT_RESU, BT_MID };
+static bool has_transformer(BlockType t) { return t == BT_REST || t == BT_RESTU || t == BT_MID; }
+static bool has_upsample(BlockType t) { return t == BT_RESU || t == BT_RESTU; }
+
 struct Block {
   BlockType type = BT_RES;
   Res res;
   STrans st;
-  Conv conv;  // BT_CONV (unused: first conv has its own path), BT_DOWN, upsample conv
-  int Cout = 0;
+  Conv conv;  // BT_DOWN, upsample conv (BT_CONV, the first conv, has its own fields)
 };
+
+// One block of the UNet as sdxl_b200/config.py::block_program lists it. `level` is the resolution it runs at (latent >> level);
+// a downsample reads its level and writes the next, an upsampling output block writes the previous one.
+struct BlockSpec {
+  BlockType type;
+  std::string path;
+  int c_in, c_out;
+  int depth;   // transformer depth
+  int level;
+};
+struct BlockProgram { std::vector<BlockSpec> ins; BlockSpec mid; std::vector<BlockSpec> outs; };
+
+// Input / middle / output blocks exactly as UNetConfig::init builds them (reference unet/mod.rs:115-173, 238-248, 250-328).
+static BlockProgram block_program(const sdxl_unet_cfg& g) {
+  const int mc = g.model_channels, nl = g.n_levels;
+  auto ch = [&](int level) { return g.channel_mults[level] * mc; };
+  BlockProgram p;
+  p.ins.push_back({BT_CONV, "input_blocks/0", g.in_channels, mc, 0, 0});
+  int idx = 1;
+  for (int level = 0; level < nl; ++level) {
+    const int c_in = ch(std::max(level - 1, 0)), c_out = ch(level);
+    const bool tr = level == 1 || level == 2;
+    for (int k = 0; k < 2; ++k) {
+      const int ci = k == 0 ? c_in : c_out;
+      if (tr) p.ins.push_back({BT_REST, "input_blocks/" + std::to_string(idx), ci, c_out, g.transformer_depths[level], level});
+      else p.ins.push_back({BT_RES, "input_blocks/" + std::to_string(idx), ci, c_out, 0, level});
+      idx += 1;
+    }
+    if (level != nl - 1) {
+      p.ins.push_back({BT_DOWN, "input_blocks/" + std::to_string(idx), c_out, c_out, 0, level});
+      idx += 1;
+    }
+  }
+  const int cm = ch(nl - 1);
+  p.mid = {BT_MID, "middle_block", cm, cm, g.transformer_depths[nl - 1], nl - 1};
+  idx = 0;
+  for (int level = nl - 1; level >= 0; --level) {
+    const int next_level = level != nl - 1 ? level + 1 : level;
+    const int c_out = ch(level);
+    const int cins[3] = {ch(next_level) + c_out, 2 * c_out, c_out + ch(std::max(level - 1, 0))};
+    const bool tr = level == 1 || level == 2;
+    for (int k = 0; k < 3; ++k) {
+      const bool up = k == 2 && (tr || level != 0);
+      if (tr) p.outs.push_back({up ? BT_RESTU : BT_REST, "output_blocks/" + std::to_string(idx), cins[k], c_out, g.transformer_depths[level], level});
+      else p.outs.push_back({up ? BT_RESU : BT_RES, "output_blocks/" + std::to_string(idx), cins[k], c_out, 0, level});
+      idx += 1;
+    }
+  }
+  return p;
+}
 
 struct Plan;
 struct Sampler;
@@ -106,6 +158,17 @@ struct EncoderHalf {
   std::vector<Block> in_blocks;
   Res mid_res1, mid_res2;
   STrans mid_st;
+  std::vector<const TBlock*> tblocks;   // every transformer block of the model in execution order (one hoisted K/V each)
+};
+
+// The step-invariant conditioning of one model (the UNet or an attached ControlNet) at one (B, n_ctx): the label MLP and the
+// cross-attention K/V of every transformer block, hoisted out of the plan by hoist_model.
+struct HoistedCond {
+  Arena mem;
+  int condB = 0, n_ctx = 0;
+  float* lab1 = nullptr;       // [B, 4mc]
+  float* label_emb = nullptr;  // [B, 4mc]
+  std::vector<__half*> kv;     // per transformer block [B*n_ctx, 2C]
 };
 
 struct sdxl_controlnet : EncoderHalf {
@@ -122,16 +185,12 @@ struct sdxl_unet : EncoderHalf {
   Conv conv_out;
   __half* conv_out_w2 = nullptr;   // [O, 2*Ktot] = [W | W]: head conv on the hi/lo-split activation
   std::vector<double> alphas;  // host copy (f16-stored values widened)
-  int n_tblocks = 0;
-  // conditioning state
-  Arena carena;
-  int condB = 0, n_ctx = 0, ctx_pitch = 0;
+  // conditioning state: the retained inputs and the hoisted conditioning; cond.condB / cond.n_ctx are its shape (0: not set)
+  Arena imem;
+  int ctx_pitch = 0;
   __half* ctx16 = nullptr;     // [B*n_ctx, ctx_pitch]
   float* y32 = nullptr;        // [B, adm]
-  float* lab1 = nullptr;       // [B, 4mc]
-  float* label_emb = nullptr;  // [B, 4mc]
-  std::vector<__half*> kv;     // per transformer block [B*n_ctx, 2C]
-  uint64_t cond_version = 0;
+  HoistedCond cond;
   // plan
   std::unique_ptr<Plan> plan;
   std::unique_ptr<Sampler> sampler;
@@ -140,9 +199,7 @@ struct sdxl_unet : EncoderHalf {
   int t_slot = 0;              // ring position in t_pinned (per model: independent contexts never share it)
   AdapterState lora;           // LoRA-able weight slots, backups of merged layers (sdxl_unet_set_adapters)
   std::vector<std::unique_ptr<ControlAttach>> controls;   // sdxl_unet_set_controls, in call order
-  uint64_t controls_version = 0;
   std::unique_ptr<IpAttach> ip;   // sdxl_unet_set_image_prompt
-  uint64_t ip_version = 0;
   uint64_t plan_builds = 0;
   int cfg_rows = 0;               // conditioning rows are the sampler's [cond | uncond] with cfg_rows cond rows (0: plain batch)
   ~sdxl_unet() {
@@ -159,11 +216,7 @@ struct ControlAttach {
   Arena mem;                      // zero-conv copies f16(s*W) / s*b, hint_emb f32 NHWC [n_hint, h, w, mc]
   std::vector<Lin> zero;
   float* hint_emb = nullptr;
-  Arena cmem;                     // conditioning of the net: label MLP, cross-attention K/V
-  int condB = 0, n_ctx = 0;
-  float* lab1 = nullptr;
-  float* label_emb = nullptr;
-  std::vector<__half*> kv;
+  HoistedCond cond;               // the net's own conditioning at the UNet's conditioning shape
 };
 
 // IP-Adapter (DESIGN.md §9): the image-token projection and, per UNet transformer block in execution order, the fused
@@ -175,7 +228,14 @@ struct sdxl_ip_adapter {
   Lin proj;                 // [T * context_dim, D]
   Norm norm;                // over context_dim, eps 1e-5
   std::vector<Lin> kv;
-  std::vector<std::string> paths;   // the transformer block of each kv
+};
+
+// The image prompt's token rows for one conditioning batch and their K/V.
+struct IpRows {
+  Arena mem;
+  int condB = 0;
+  __half* rows = nullptr;      // [condB, S_ip, context_dim]
+  std::vector<__half*> kv;     // per transformer block [condB * S_ip, 2C]
 };
 
 // An attached image prompt: the projected tokens of the prompts and of the negatives, the per-block scales, and the image K/V
@@ -186,11 +246,8 @@ struct IpAttach {
   Arena mem;
   __half* tok_pos = nullptr;   // [n_batch, S_ip, context_dim]
   __half* tok_neg = nullptr;   // [n_batch, S_ip, context_dim]
-  float* scales = nullptr;     // [n_tblocks], read by the attention kernel
-  Arena cmem;                  // sized by the conditioning batch
-  int condB = 0;
-  __half* rows = nullptr;      // [condB, S_ip, context_dim]
-  std::vector<__half*> kv;     // per transformer block [condB * S_ip, 2C]
+  float* scales = nullptr;     // one per transformer block, read by the attention kernel
+  IpRows cond;
 };
 
 
@@ -228,7 +285,6 @@ static STrans load_st(Loader& L, const std::string& path, int C, int ctx_dim, in
   for (int j = 0; j < depth && !L.err; ++j) {
     const std::string bp = path + "/transformer_" + std::to_string(j);
     TBlock b;
-    b.path = bp;
     b.n1 = L.norm(bp + "/norm1", C);
     b.n2 = L.norm(bp + "/norm2", C);
     b.n3 = L.norm(bp + "/norm3", C);
@@ -256,60 +312,56 @@ static STrans load_st(Loader& L, const std::string& path, int C, int ctx_dim, in
   return s;
 }
 
+// An input or output block of the block program (not the first conv).
+static Block load_block(Loader& L, const sdxl_unet_cfg& g, const BlockSpec& s, std::vector<TembItem>& tembs, int& temb_total) {
+  Block b;
+  b.type = s.type;
+  if (s.type == BT_DOWN) {
+    b.conv = L.conv(s.path, s.c_in, s.c_out, 3);
+    return b;
+  }
+  const bool tr = has_transformer(s.type), up = has_upsample(s.type);
+  b.res = load_res(L, tr || up ? s.path + "/res" : s.path, s.c_in, s.c_out, tembs, temb_total);
+  if (tr) b.st = load_st(L, s.path + "/transformer", s.c_out, g.context_dim, s.c_out / g.n_head_channels, s.depth);
+  if (up) b.conv = L.upconv(s.path + "/upsample/conv", s.c_out, s.c_out);
+  return b;
+}
+
 // Time / label MLPs, first conv, input blocks and middle block (reference unet/mod.rs:116-248), for the UNet and for a ControlNet.
-static int load_encoder(Loader& L, EncoderHalf* u, std::vector<TembItem>& tembs, int& temb_total) {
+static int load_encoder(Loader& L, EncoderHalf* u, const BlockProgram& prog, std::vector<TembItem>& tembs, int& temb_total) {
   const sdxl_unet_cfg& g = u->cfg;
   const int mc = g.model_channels, ted = 4 * mc;
   u->in_blocks.clear();
-  auto n_head = [&](int ch) { return ch / g.n_head_channels; };
-
   u->t1 = L.linear("lin1_time_embed", mc, ted, true);
   u->t2 = L.linear("lin2_time_embed", ted, ted, true);
   u->l1 = L.linear("lin1_label_embed", g.adm_in_channels, ted, true);
   u->l2 = L.linear("lin2_label_embed", ted, ted, true);
   if (L.err) return L.err;
-  if (int r = L.conv_f32("input_blocks/0", g.in_channels, mc, u->conv0_w, u->conv0_b)) return r;
-  {
-    Block b0; b0.type = BT_CONV; b0.Cout = mc;
-    u->in_blocks.push_back(b0);
-  }
-  // input blocks (reference unet/mod.rs:121-173)
-  int idx = 1;
-  for (int level = 0; level < g.n_levels && !L.err; ++level) {
-    const int cin = g.channel_mults[level > 0 ? level - 1 : 0] * mc;
-    const int cout = g.channel_mults[level] * mc;
-    const bool tr = (level == 1 || level == 2);
-    for (int k = 0; k < 2; ++k) {
-      Block b;
-      const std::string bp = "input_blocks/" + std::to_string(idx++);
-      b.Cout = cout;
-      if (!tr) {
-        b.type = BT_RES;
-        b.res = load_res(L, bp, k == 0 ? cin : cout, cout, tembs, temb_total);
-      } else {
-        b.type = BT_REST;
-        b.res = load_res(L, bp + "/res", k == 0 ? cin : cout, cout, tembs, temb_total);
-        b.st = load_st(L, bp + "/transformer", cout, g.context_dim, n_head(cout), g.transformer_depths[level]);
-      }
-      u->in_blocks.push_back(std::move(b));
-    }
-    if (level != g.n_levels - 1) {
-      Block b;
-      b.type = BT_DOWN;
-      b.Cout = cout;
-      b.conv = L.conv("input_blocks/" + std::to_string(idx++), cout, cout, 3);
-      u->in_blocks.push_back(std::move(b));
+  for (const BlockSpec& s : prog.ins) {
+    if (L.err) return L.err;
+    if (s.type == BT_CONV) {
+      if (int r = L.conv_f32(s.path, s.c_in, s.c_out, u->conv0_w, u->conv0_b)) return r;
+      Block b0;
+      b0.type = BT_CONV;
+      u->in_blocks.push_back(std::move(b0));
+    } else {
+      u->in_blocks.push_back(load_block(L, g, s, tembs, temb_total));
     }
   }
   if (L.err) return L.err;
-  // middle (reference unet/mod.rs:238-248)
-  {
-    const int cm = g.channel_mults[g.n_levels - 1] * mc;
-    u->mid_res1 = load_res(L, "middle_block/res1", cm, cm, tembs, temb_total);
-    u->mid_st = load_st(L, "middle_block/transformer", cm, g.context_dim, n_head(cm), g.transformer_depths[g.n_levels - 1]);
-    u->mid_res2 = load_res(L, "middle_block/res2", cm, cm, tembs, temb_total);
-  }
+  const BlockSpec& m = prog.mid;
+  u->mid_res1 = load_res(L, m.path + "/res1", m.c_in, m.c_out, tembs, temb_total);
+  u->mid_st = load_st(L, m.path + "/transformer", m.c_out, g.context_dim, m.c_out / g.n_head_channels, m.depth);
+  u->mid_res2 = load_res(L, m.path + "/res2", m.c_out, m.c_out, tembs, temb_total);
   return L.err;
+}
+
+// e->tblocks, after the real build pass (the block vectors no longer move): input blocks, middle, then `outs`.
+static void list_tblocks(EncoderHalf* e, const std::vector<Block>& outs) {
+  e->tblocks.clear();
+  for (auto& b : e->in_blocks) for (auto& t : b.st.blocks) e->tblocks.push_back(&t);
+  for (auto& t : e->mid_st.blocks) e->tblocks.push_back(&t);
+  for (auto& b : outs) for (auto& t : b.st.blocks) e->tblocks.push_back(&t);
 }
 
 // concatenated lin_embed matrix (one GEMV per forward for all ResBlocks); bias += conv_in bias
@@ -348,34 +400,11 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
   u->out_blocks.clear();
   std::vector<TembItem> tembs;
   int temb_total = 0;
-  auto n_head = [&](int ch) { return ch / g.n_head_channels; };
-  if (int r = load_encoder(L, u, tembs, temb_total)) return r;
-  // output blocks (reference unet/mod.rs:250-328)
-  int idx = 0;
-  for (int level = g.n_levels - 1; level >= 0 && !L.err; --level) {
-    const int next_level = (level != g.n_levels - 1) ? level + 1 : level;
-    const int cout = g.channel_mults[level] * mc;
-    const int cin1 = g.channel_mults[next_level] * mc + cout;
-    const int cin2 = 2 * cout;
-    const int cin3 = cout + g.channel_mults[level > 0 ? level - 1 : 0] * mc;
-    const bool tr = (level == 1 || level == 2);
-    const int cins[3] = {cin1, cin2, cin3};
-    for (int k = 0; k < 3; ++k) {
-      Block b;
-      const std::string bp = "output_blocks/" + std::to_string(idx++);
-      b.Cout = cout;
-      const bool up = (k == 2) && (tr || level != 0);
-      if (!tr) {
-        b.type = up ? BT_RESU : BT_RES;
-        b.res = load_res(L, up ? bp + "/res" : bp, cins[k], cout, tembs, temb_total);
-      } else {
-        b.type = up ? BT_RESTU : BT_REST;
-        b.res = load_res(L, bp + "/res", cins[k], cout, tembs, temb_total);
-        b.st = load_st(L, bp + "/transformer", cout, g.context_dim, n_head(cout), g.transformer_depths[level]);
-      }
-      if (up) b.conv = L.upconv(bp + "/upsample/conv", cout, cout);
-      u->out_blocks.push_back(std::move(b));
-    }
+  const BlockProgram prog = block_program(g);
+  if (int r = load_encoder(L, u, prog, tembs, temb_total)) return r;
+  for (const BlockSpec& s : prog.outs) {
+    if (L.err) return L.err;
+    u->out_blocks.push_back(load_block(L, g, s, tembs, temb_total));
   }
   if (L.err) return L.err;
   u->norm_out = L.norm("norm_out", mc);
@@ -393,12 +422,7 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
                                 (size_t)cv.Ktot * sizeof(__half), (size_t)cv.O, cudaMemcpyDeviceToDevice, c->stream));
   }
   if (int r = load_temb_all(L, u, tembs, temb_total)) return r;
-  // count transformer blocks (for the hoisted K/V buffers)
-  int nt = 0;
-  for (auto& b : u->in_blocks) nt += (int)b.st.blocks.size();
-  nt += (int)u->mid_st.blocks.size();
-  for (auto& b : u->out_blocks) nt += (int)b.st.blocks.size();
-  u->n_tblocks = nt;
+  if (!A.measure) list_tblocks(u, u->out_blocks);
   return 0;
 }
 
@@ -520,7 +544,8 @@ static int build_controlnet(sdxl_controlnet* n, const PackView& pv, Arena& A) {
   Loader L{n->ctx, &pv, &A, n->ctx->stream};   // no LoRA registry: adapters on a ControlNet are not supported
   std::vector<TembItem> tembs;
   int temb_total = 0;
-  if (int r = load_encoder(L, n, tembs, temb_total)) return r;
+  const BlockProgram prog = block_program(g);
+  if (int r = load_encoder(L, n, prog, tembs, temb_total)) return r;
   if (int r = load_temb_all(L, n, tembs, temb_total)) return r;
   // hint encoder, SGM's input_hint_block indices: 0 = conv(in -> c0); 2 + 4k = conv(c_k -> c_k), 4 + 4k = conv(c_k -> c_k+1, s2);
   // 4n - 2 = conv(c_last -> mc)
@@ -535,10 +560,10 @@ static int build_controlnet(sdxl_controlnet* n, const PackView& pv, Arena& A) {
   n->hint.push_back(L.conv("input_hint_block/" + std::to_string(4 * nb - 2), hc[nb - 1], g.model_channels, 3));
   // zero convs: one per skip tensor (the outputs of input_blocks/0, 1, ...), then middle_block_out
   n->zero.clear();
-  for (size_t i = 0; i < n->in_blocks.size() && !L.err; ++i)
-    n->zero.push_back(L.conv("zero_convs/" + std::to_string(i), n->in_blocks[i].Cout, n->in_blocks[i].Cout, 1));
-  const int cm = g.channel_mults[g.n_levels - 1] * g.model_channels;
-  n->zero.push_back(L.conv("middle_block_out", cm, cm, 1));
+  for (size_t i = 0; i < prog.ins.size() && !L.err; ++i)
+    n->zero.push_back(L.conv("zero_convs/" + std::to_string(i), prog.ins[i].c_out, prog.ins[i].c_out, 1));
+  n->zero.push_back(L.conv("middle_block_out", prog.mid.c_out, prog.mid.c_out, 1));
+  if (!L.err && !A.measure) list_tblocks(n, {});
   return L.err;
 }
 
@@ -640,20 +665,20 @@ extern "C" int sdxl_controlnet_embed_hint(sdxl_controlnet* net, int n, int H, in
 struct UNetPlanBuilder : PlanBuilder {
   sdxl_unet* u = nullptr;
   int kv_index = 0;
-  const std::vector<__half*>* kvs = nullptr;   // hoisted cross-attention K/V of the model being planned (UNet or ControlNet)
+  const HoistedCond* cond = nullptr;   // hoisted conditioning of the model being planned (UNet or ControlNet)
 
   struct Scratch { __half *gn1, *raw; float* h; __half *gn2, *a16; float* tok; __half *qkv, *ao, *q, *ff; };
   struct Saved { float* p; int C, H, W; };
 
   // Time / label MLPs (on the shared timestep embedding te), first conv, input blocks and middle block of UNet::forward
-  // (unet/mod.rs:458-482) with the weights of `e`; every block output is pushed to `saved`, the middle output is returned.
-  // hint (nullable): ControlNet hint embedding f32 NHWC [n_hint, h, w, mc] added to the first conv's output.
-  float* encoder(const EncoderHalf& e, const float* label_emb, const float* te, float* t1, float* semb, float* temb_all,
+  // (unet/mod.rs:458-482) with the weights of `e` and the conditioning `cond`; every block output is pushed to `saved`, the
+  // middle output is returned. hint (nullable): ControlNet hint embedding f32 NHWC [n_hint, h, w, mc] added to the first conv's output.
+  float* encoder(const EncoderHalf& e, const float* te, float* t1, float* semb, float* temb_all,
                  const Scratch& s, const float* hint, int n_hint, const std::string& prefix, std::vector<Saved>& saved) {
     const sdxl_unet_cfg& g = e.cfg;
     const int mc = g.model_channels, ted = 4 * mc, temb_total = e.temb_all.N;
     gemv(te, 0, 1, e.t1, nullptr, 0, 0, 1, t1, 0);
-    gemv(t1, 0, Bf, e.t2, label_emb, ted, 0, 1, semb, ted);
+    gemv(t1, 0, Bf, e.t2, cond->label_emb, ted, 0, 1, semb, ted);
     gemv(semb, ted, Bf, e.temb_all, nullptr, 0, 0, 0, temb_all, temb_total);
     int H = P->h, W = P->w;
     float* x = buf<float>((size_t)Bf * H * W * mc);
@@ -748,13 +773,12 @@ struct UNetPlanBuilder : PlanBuilder {
       // x = x + attn2(norm2(x), context)   (K/V hoisted to set_conditioning)
       ln(s_tok, b.n2, M, s_a16);
       linear(s_a16, M, b.q2, IGEMM_LINEAR, s_q, 0, C, nullptr, 0);
-      const __half* kvp = A->measure ? nullptr : (*kvs)[kv_index];
-      attn(s_q, C, 0, kvp, 2 * C, 0, C, T, u->n_ctx, s.n_head, s_ao, C, sl2e);
-      P->flops += 2.0 * Bf * u->n_ctx * (double)b.kv2.K * b.kv2.N;  // hoisted K/V projections (algorithmic work)
+      attn(s_q, C, 0, cond->kv[kv_index], 2 * C, 0, C, T, cond->n_ctx, s.n_head, s_ao, C, sl2e);
+      P->flops += 2.0 * Bf * cond->n_ctx * (double)b.kv2.K * b.kv2.N;  // hoisted K/V projections (algorithmic work)
       // an attached image prompt adds its K/V source to the UNet's own cross-attentions (a ControlNet's see text only)
-      if (u->ip && kvs == &u->kv) {
+      if (u->ip && cond == &u->cond) {
         const IpAttach& ip = *u->ip;
-        attn_ip(A->measure ? nullptr : ip.kv[kv_index], 2 * C, 0, C, ip.S_ip, ip.scales + kv_index);
+        attn_ip(ip.cond.kv[kv_index], 2 * C, 0, C, ip.S_ip, ip.scales + kv_index);
         P->flops += 2.0 * Bf * ip.S_ip * (double)ip.ad->kv[kv_index].K * ip.ad->kv[kv_index].N;
       }
       kv_index++;
@@ -836,28 +860,20 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
   float* semb = B.buf<float>((size_t)Bf * ted);
   float* temb_all = B.buf<float>((size_t)Bf * temb_total);
 
-  // maxima for the shared scratch buffers
-  size_t max_pixC_cat = 0, max_pixC = 0, max_tokC = 0, max_tok = 0;
+  // maxima for the shared scratch buffers over the ResBlocks and transformers of the block program, each at its level
+  size_t max_pixC_cat = 0, max_pixC = 0, max_tokC = 0;
   {
-    int H = P->h, W = P->w;
-    auto upd = [&](const Res& r, int hh, int ww) {
-      max_pixC_cat = std::max(max_pixC_cat, (size_t)hh * ww * r.Cin);
-      max_pixC = std::max(max_pixC, (size_t)hh * ww * r.Cout);
+    const BlockProgram prog = block_program(g);
+    auto upd = [&](const BlockSpec& s) {
+      if (s.type == BT_CONV || s.type == BT_DOWN) return;
+      const size_t px = (size_t)(P->h >> s.level) * (P->w >> s.level);
+      max_pixC_cat = std::max(max_pixC_cat, px * s.c_in);
+      max_pixC = std::max(max_pixC, px * s.c_out);
+      if (has_transformer(s.type)) max_tokC = std::max(max_tokC, px * s.c_out);
     };
-    for (auto& b : u->in_blocks) {
-      if (b.type == BT_RES || b.type == BT_REST) upd(b.res, H, W);
-      if (b.type == BT_REST) { max_tokC = std::max(max_tokC, (size_t)H * W * b.st.C); max_tok = std::max(max_tok, (size_t)H * W); }
-      if (b.type == BT_DOWN) { H /= 2; W /= 2; }
-    }
-    upd(u->mid_res1, H, W);
-    upd(u->mid_res2, H, W);
-    max_tokC = std::max(max_tokC, (size_t)H * W * u->mid_st.C);
-    max_tok = std::max(max_tok, (size_t)H * W);
-    for (auto& b : u->out_blocks) {
-      upd(b.res, H, W);
-      if (b.type == BT_REST || b.type == BT_RESTU) { max_tokC = std::max(max_tokC, (size_t)H * W * b.st.C); max_tok = std::max(max_tok, (size_t)H * W); }
-      if (b.type == BT_RESTU || b.type == BT_RESU) { H *= 2; W *= 2; }
-    }
+    for (const BlockSpec& s : prog.ins) upd(s);
+    upd(prog.mid);
+    for (const BlockSpec& s : prog.outs) upd(s);
   }
   __half* s_gn1 = B.buf<__half>(Bf * max_pixC_cat);
   __half* s_raw = B.buf<__half>(Bf * max_pixC_cat);
@@ -882,8 +898,8 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
   // --- embeddings, input blocks, middle
   using Saved = UNetPlanBuilder::Saved;
   std::vector<Saved> saved;
-  B.kvs = &u->kv;
-  float* x = B.encoder(*u, u->label_emb, te, t1, semb, temb_all, scr, nullptr, 1, "", saved);
+  B.cond = &u->cond;
+  float* x = B.encoder(*u, te, t1, semb, temb_all, scr, nullptr, 1, "", saved);
   int H = saved.back().H, W = saved.back().W, Cx = saved.back().C;
   // --- ControlNets (DESIGN.md §8): each runs its own encoder on the same inputs, then skip_i += s * zero_conv_i(h_i) and
   // mid += s * middle_block_out(mid_c), in attachment order. The UNet's own encoder above is untouched.
@@ -892,14 +908,14 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
     const EncoderHalf& e = *a.net;
     const std::string prefix = "control" + std::to_string(k) + "/";
     const int kv_unet = B.kv_index;
-    B.kvs = &a.kv;
+    B.cond = &a.cond;
     B.kv_index = 0;
     float* ct1 = B.buf<float>(ted);
     float* csemb = B.buf<float>((size_t)Bf * ted);
     float* ctemb = B.buf<float>((size_t)Bf * e.temb_all.N);
     std::vector<Saved> cs;
-    float* cmid = B.encoder(e, a.label_emb, te, ct1, csemb, ctemb, scr, a.hint_emb, a.n_hint, prefix, cs);
-    B.kvs = &u->kv;
+    float* cmid = B.encoder(e, te, ct1, csemb, ctemb, scr, a.hint_emb, a.n_hint, prefix, cs);
+    B.cond = &u->cond;
     B.kv_index = kv_unet;
     if (cs.size() != saved.size() || a.zero.size() != saved.size() + 1) return fail(c, 5006, "control %zu: skip count mismatch", k);
     B.begin_block(prefix + "zero_convs");
@@ -947,22 +963,18 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
 
 static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
   sdxl_ctx* c = u->ctx;
-  if (u->condB != Bf) return fail(c, 5010, "conditioning is set for batch %d but forward batch is %d (call sdxl_unet_set_conditioning first)", u->condB, Bf);
+  if (u->cond.condB != Bf) return fail(c, 5010, "conditioning is set for batch %d but forward batch is %d (call sdxl_unet_set_conditioning first)", u->cond.condB, Bf);
   for (size_t k = 0; k < u->controls.size(); ++k) {
     const ControlAttach& a = *u->controls[k];
     if (a.h != h || a.w != w)
       return fail(c, 5012, "control %zu: its hint is %dx%d pixels (latent %dx%d) but the latent is %dx%d", k, 8 * a.h, 8 * a.w, a.h, a.w, h, w);
     if (Bf % a.n_hint) return fail(c, 5013, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bf, a.n_hint);
   }
-  if (u->ip && u->ip->condB != Bf) return fail(c, 5014, "image prompt: its K/V are hoisted for batch %d but the batch is %d", u->ip->condB, Bf);
-  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan->cond_version == u->cond_version &&
-      u->plan->controls_version == u->controls_version && u->plan->ip_version == u->ip_version)
-    return 0;
+  if (u->ip && u->ip->cond.condB != Bf) return fail(c, 5014, "image prompt: its K/V are hoisted for batch %d but the batch is %d", u->ip->cond.condB, Bf);
+  // every change of the buffers or attachments a plan reads drops the plan, so the shapes are its whole cache key
+  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w) return 0;
   if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A); })) return r;
   u->plan_builds++;
-  u->plan->cond_version = u->cond_version;
-  u->plan->controls_version = u->controls_version;
-  u->plan->ip_version = u->ip_version;
   return 0;
 }
 
@@ -981,53 +993,30 @@ static int set_t(sdxl_unet* u, int t) {
 // ================================================================================================
 static int hoist_conditioning(sdxl_unet* u);
 
-// transformer blocks in execution order (one hoisted K/V buffer each)
-static std::vector<const TBlock*> encoder_tblocks(const EncoderHalf& e) {
-  std::vector<const TBlock*> tbs;
-  for (auto& b : e.in_blocks) for (auto& t : b.st.blocks) tbs.push_back(&t);
-  for (auto& t : e.mid_st.blocks) tbs.push_back(&t);
-  return tbs;
-}
-static std::vector<const TBlock*> unet_tblocks(const sdxl_unet* u) {
-  std::vector<const TBlock*> tbs = encoder_tblocks(*u);
-  for (auto& b : u->out_blocks) for (auto& t : b.st.blocks) tbs.push_back(&t);
-  return tbs;
-}
-
-// (Re)allocates a control's conditioning buffers for the UNet's current conditioning batch and context length.
-static int control_cond_alloc(sdxl_unet* u, ControlAttach& a) {
-  if (a.condB == u->condB && a.n_ctx == u->n_ctx) return 0;
-  const int B = u->condB, n_ctx = u->n_ctx, ted = 4 * u->cfg.model_channels;
-  const std::vector<const TBlock*> tbs = encoder_tblocks(*a.net);
-  size_t need = 0;
-  auto al = [&](size_t b) { need = ((need + 1023) & ~size_t(1023)) + b; };
-  al((size_t)B * ted * 4);
-  al((size_t)B * ted * 4);
-  for (auto* t : tbs) al((size_t)B * n_ctx * t->kv2.N * 2);
-  if (a.cmem.init(need + (1 << 16))) return fail(u->ctx, 5102, "cannot allocate ControlNet conditioning buffers");
-  a.lab1 = a.cmem.get<float>((size_t)B * ted);
-  a.label_emb = a.cmem.get<float>((size_t)B * ted);
-  a.kv.clear();
-  for (auto* t : tbs) a.kv.push_back(a.cmem.get<__half>((size_t)B * n_ctx * t->kv2.N));
-  a.condB = B;
-  a.n_ctx = n_ctx;
-  return 0;
+// Allocates the conditioning buffers of model e at (B, n_ctx) into h (a fresh object: callers swap it in on success).
+static int cond_alloc(sdxl_ctx* c, const EncoderHalf& e, int B, int n_ctx, HoistedCond& h) {
+  const int ted = 4 * e.cfg.model_channels;
+  h.condB = B;
+  h.n_ctx = n_ctx;
+  return carve_measured(c, h.mem, 5101, "conditioning buffers", [&](Arena& A) {
+    h.lab1 = A.get<float>((size_t)B * ted);
+    h.label_emb = A.get<float>((size_t)B * ted);
+    h.kv.clear();
+    for (const TBlock* t : e.tblocks) h.kv.push_back(A.get<__half>((size_t)B * n_ctx * t->kv2.N));
+    return 0;
+  });
 }
 
-// (Re)allocates the image prompt's row and K/V buffers for the UNet's current conditioning batch.
-static int ip_cond_alloc(sdxl_unet* u, IpAttach& a) {
-  if (a.condB == u->condB) return 0;
-  const int B = u->condB, ctx_dim = u->cfg.context_dim;
-  size_t need = 0;
-  auto al = [&](size_t b) { need = ((need + 1023) & ~size_t(1023)) + b; };
-  al((size_t)B * a.S_ip * ctx_dim * 2);
-  for (const Lin& L : a.ad->kv) al((size_t)B * a.S_ip * L.N * 2);
-  if (a.cmem.init(need + (1 << 16))) return fail(u->ctx, 5103, "cannot allocate image-prompt conditioning buffers");
-  a.rows = a.cmem.get<__half>((size_t)B * a.S_ip * ctx_dim);
-  a.kv.clear();
-  for (const Lin& L : a.ad->kv) a.kv.push_back(a.cmem.get<__half>((size_t)B * a.S_ip * L.N));
-  a.condB = B;
-  return 0;
+// Allocates the image prompt's row and K/V buffers for conditioning batch B into r (a fresh object, as above).
+static int ip_cond_alloc(sdxl_ctx* c, const IpAttach& a, int B, IpRows& r) {
+  const int ctx_dim = a.ad->cfg.unet.context_dim;
+  r.condB = B;
+  return carve_measured(c, r.mem, 5103, "image-prompt conditioning buffers", [&](Arena& A) {
+    r.rows = A.get<__half>((size_t)B * a.S_ip * ctx_dim);
+    r.kv.clear();
+    for (const Lin& L : a.ad->kv) r.kv.push_back(A.get<__half>((size_t)B * a.S_ip * L.N));
+    return 0;
+  });
 }
 
 // An image prompt's n_batch must divide the number of images the conditioning rows hold.
@@ -1041,39 +1030,39 @@ static int ip_check_batch(sdxl_unet* u, int n_batch /* 0: no prompt */, int B, i
 static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* context_dev, const __half* y_dev, int cfg_rows) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
-  const int ted = 4 * g.model_channels;
   if (B < 1 || n_ctx < 1) return fail(c, 5100, "bad conditioning shape");
   if (int r = ip_check_batch(u, u->ip ? u->ip->n_batch : 0, B, cfg_rows)) return r;
-  u->cfg_rows = cfg_rows;
-  if (u->condB != B || u->n_ctx != n_ctx) {
-    CU(c, cudaStreamSynchronize(c->stream));
+  if (u->cond.condB != B || u->cond.n_ctx != n_ctx) {
+    // everything sized by (B, n_ctx) is allocated into fresh objects and swapped in only when all of it succeeded: a failure
+    // leaves the previous conditioning, and the plan over it, in effect
+    const int pitch = (g.context_dim + 7) / 8 * 8;
+    Arena imem;
+    __half* ctx16 = nullptr;
+    float* y32 = nullptr;
+    int r = carve_measured(c, imem, 5101, "conditioning inputs", [&](Arena& A) {
+      ctx16 = A.get<__half>((size_t)B * n_ctx * pitch);
+      y32 = A.get<float>((size_t)B * g.adm_in_channels);
+      return 0;
+    });
+    HoistedCond cond;
+    if (!r) r = cond_alloc(c, *u, B, n_ctx, cond);
+    std::vector<HoistedCond> ccond(u->controls.size());
+    for (size_t k = 0; k < ccond.size() && !r; ++k) r = cond_alloc(c, *u->controls[k]->net, B, n_ctx, ccond[k]);
+    IpRows ipc;
+    if (!r && u->ip) r = ip_cond_alloc(c, *u->ip, B, ipc);
+    if (r) return r;
+    CU(c, cudaStreamSynchronize(c->stream));   // the old buffers and the plan over them may still be in flight
     u->plan.reset();
-    const std::vector<const TBlock*> tbs = unet_tblocks(u);
-    u->ctx_pitch = (g.context_dim + 7) / 8 * 8;
-    size_t need = 0;
-    auto al = [&](size_t b) { need = ((need + 1023) & ~size_t(1023)) + b; };
-    al((size_t)B * n_ctx * u->ctx_pitch * 2);
-    al((size_t)B * g.adm_in_channels * 4);
-    al((size_t)B * ted * 4);
-    al((size_t)B * ted * 4);
-    for (auto* t : tbs) al((size_t)B * n_ctx * t->kv2.N * 2);
-    if (u->carena.init(need + (1 << 16))) return fail(c, 5101, "cannot allocate conditioning buffers");
-    u->ctx16 = u->carena.get<__half>((size_t)B * n_ctx * u->ctx_pitch);
-    u->y32 = u->carena.get<float>((size_t)B * g.adm_in_channels);
-    u->lab1 = u->carena.get<float>((size_t)B * ted);
-    u->label_emb = u->carena.get<float>((size_t)B * ted);
-    u->kv.clear();
-    for (auto* t : tbs) u->kv.push_back(u->carena.get<__half>((size_t)B * n_ctx * t->kv2.N));
-    u->condB = B;
-    u->n_ctx = n_ctx;
-    CU(c, cudaMemsetAsync(u->ctx16, 0, (size_t)B * n_ctx * u->ctx_pitch * 2, c->stream));
-    for (auto& a : u->controls)
-      if (int r = control_cond_alloc(u, *a)) return r;
-    if (u->ip)
-      if (int r = ip_cond_alloc(u, *u->ip)) return r;
+    u->imem = std::move(imem);
+    u->ctx_pitch = pitch;
+    u->ctx16 = ctx16;
+    u->y32 = y32;
+    u->cond = std::move(cond);
+    for (size_t k = 0; k < ccond.size(); ++k) u->controls[k]->cond = std::move(ccond[k]);
+    if (u->ip) u->ip->cond = std::move(ipc);
+    CU(c, cudaMemsetAsync(u->ctx16, 0, (size_t)B * n_ctx * pitch * 2, c->stream));
   }
-  u->cond_version++;
-  if (u->plan) u->plan->cond_version = u->cond_version;  // buffers unchanged: plan stays valid
+  u->cfg_rows = cfg_rows;
   CU(c, cudaMemcpy2DAsync(u->ctx16, (size_t)u->ctx_pitch * 2, context_dev, (size_t)g.context_dim * 2, (size_t)g.context_dim * 2,
                           (size_t)B * n_ctx, cudaMemcpyDeviceToDevice, c->stream));
   KL(c, cast_f16_to_f32_launch(c->stream, y_dev, (size_t)B * g.adm_in_channels, u->y32));
@@ -1091,45 +1080,44 @@ static int project_kv(sdxl_ctx* c, const __half* a, int M, int K, int lda, const
 }
 
 // label_emb = lin2(SiLU(lin1(y))) (unet/mod.rs:464-466) and the K/V projections of the context for every cross-attention
-// (unet/mod.rs:1010-1011) with the weights of `e`, from the UNet's retained conditioning.
-static int hoist_model(sdxl_unet* u, const EncoderHalf& e, const std::vector<const TBlock*>& tbs, float* lab1, float* label_emb,
-                       const std::vector<__half*>& kv) {
+// (unet/mod.rs:1010-1011) with the weights of `e` into h, from the UNet's retained conditioning (h has the UNet's shape).
+static int hoist_model(sdxl_unet* u, const EncoderHalf& e, const HoistedCond& h) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
-  const int ted = 4 * g.model_channels, B = u->condB, n_ctx = u->n_ctx;
+  const int ted = 4 * g.model_channels, B = h.condB, n_ctx = h.n_ctx;
   for (int b0 = 0; b0 < B; b0 += 8) {
     const int nb = B - b0 < 8 ? B - b0 : 8;
     KL(c, gemv_launch(c->stream, u->y32 + (size_t)b0 * g.adm_in_channels, g.adm_in_channels, nb, g.adm_in_channels, e.l1.w,
-                      e.l1.Kpad, e.l1.b, nullptr, 0, ted, 0, 1, lab1 + (size_t)b0 * ted, ted));
-    KL(c, gemv_launch(c->stream, lab1 + (size_t)b0 * ted, ted, nb, e.l2.K, e.l2.w, e.l2.Kpad, e.l2.b, nullptr, 0, ted, 0, 0,
-                      label_emb + (size_t)b0 * ted, ted));
+                      e.l1.Kpad, e.l1.b, nullptr, 0, ted, 0, 1, h.lab1 + (size_t)b0 * ted, ted));
+    KL(c, gemv_launch(c->stream, h.lab1 + (size_t)b0 * ted, ted, nb, e.l2.K, e.l2.w, e.l2.Kpad, e.l2.b, nullptr, 0, ted, 0, 0,
+                      h.label_emb + (size_t)b0 * ted, ted));
   }
   std::vector<const Lin*> lins;
-  for (auto* t : tbs) lins.push_back(&t->kv2);
-  return project_kv(c, u->ctx16, B * n_ctx, g.context_dim, u->ctx_pitch, lins, kv);
+  for (const TBlock* t : e.tblocks) lins.push_back(&t->kv2);
+  return project_kv(c, u->ctx16, B * n_ctx, g.context_dim, u->ctx_pitch, lins, h.kv);
 }
 
 // The image prompt's token rows for the current conditioning rows (row rule: include/sdxl_b200.h, sdxl_unet_set_image_prompt)
 // and their K/V for every UNet cross-attention.
 static int ip_hoist(sdxl_unet* u, IpAttach& a) {
   sdxl_ctx* c = u->ctx;
-  const int ctx_dim = u->cfg.context_dim, B = u->condB, cr = u->cfg_rows;
+  const int ctx_dim = u->cfg.context_dim, B = a.cond.condB, cr = u->cfg_rows;
   const size_t row = (size_t)a.S_ip * ctx_dim;
   for (int r = 0; r < B; ++r) {
     const __half* src = (cr && r >= cr) ? a.tok_neg + (size_t)((r - cr) % a.n_batch) * row : a.tok_pos + (size_t)(r % a.n_batch) * row;
-    CU(c, cudaMemcpyAsync(a.rows + (size_t)r * row, src, row * sizeof(__half), cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync(a.cond.rows + (size_t)r * row, src, row * sizeof(__half), cudaMemcpyDeviceToDevice, c->stream));
   }
   std::vector<const Lin*> lins;
   for (const Lin& L : a.ad->kv) lins.push_back(&L);
-  return project_kv(c, a.rows, B * a.S_ip, ctx_dim, ctx_dim, lins, a.kv);
+  return project_kv(c, a.cond.rows, B * a.S_ip, ctx_dim, ctx_dim, lins, a.cond.kv);
 }
 
 // The step-invariant projections of the retained conditioning (ctx16, y32) under the current weights, for the UNet and every
 // attached ControlNet.
 static int hoist_conditioning(sdxl_unet* u) {
-  if (int r = hoist_model(u, *u, unet_tblocks(u), u->lab1, u->label_emb, u->kv)) return r;
+  if (int r = hoist_model(u, *u, u->cond)) return r;
   for (auto& a : u->controls)
-    if (int r = hoist_model(u, *a->net, encoder_tblocks(*a->net), a->lab1, a->label_emb, a->kv)) return r;
+    if (int r = hoist_model(u, *a->net, a->cond)) return r;
   return u->ip ? ip_hoist(u, *u->ip) : 0;
 }
 
@@ -1217,29 +1205,29 @@ extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* c
     a->n_hint = ctl[k].n_hint;
     a->h = ctl[k].height / 8;
     a->w = ctl[k].width / 8;
-    size_t need = (size_t)a->n_hint * a->h * a->w * g.model_channels * sizeof(float) + 1024;
-    for (const Conv& z : net->zero) need += (size_t)z.O * z.Ktot * sizeof(__half) + z.O * sizeof(float) + 2048;
-    if (a->mem.init(need)) return fail(c, 4739, "set_controls: cannot allocate %zu bytes for control %d", need, k);
-    for (const Conv& z : net->zero) {
-      Lin L;
-      L.K = z.I; L.Kpad = z.Ktot; L.N = z.O;
-      L.w = a->mem.get<__half>((size_t)z.O * z.Ktot);
-      L.b = a->mem.get<float>(z.O);
-      a->zero.push_back(L);
-    }
-    a->hint_emb = a->mem.get<float>((size_t)a->n_hint * a->h * a->w * g.model_channels);
-    if (u->condB > 0)
-      if (int r = control_cond_alloc(u, *a)) return r;
+    if (int r = carve_measured(c, a->mem, 4739, "set_controls: control buffers", [&](Arena& A) {
+          a->zero.clear();
+          for (const Conv& z : net->zero) {
+            Lin L;
+            L.K = z.I; L.Kpad = z.Ktot; L.N = z.O;
+            L.w = A.get<__half>((size_t)z.O * z.Ktot);
+            L.b = A.get<float>(z.O);
+            a->zero.push_back(L);
+          }
+          a->hint_emb = A.get<float>((size_t)a->n_hint * a->h * a->w * g.model_channels);
+          return 0;
+        }))
+      return r;
     if (int r = control_write(c, *a, ctl[k])) return r;
+    if (u->cond.condB > 0) {
+      if (int r = cond_alloc(c, *net, u->cond.condB, u->cond.n_ctx, a->cond)) return r;
+      if (int r = hoist_model(u, *net, a->cond)) return r;
+    }
     fresh.push_back(std::move(a));
   }
   CU(c, cudaStreamSynchronize(c->stream));   // the old plan and attachments may still be in flight
   u->plan.reset();
   u->controls = std::move(fresh);
-  u->controls_version++;
-  if (u->condB > 0)
-    for (auto& a : u->controls)
-      if (int r = hoist_model(u, *a->net, encoder_tblocks(*a->net), a->lab1, a->label_emb, a->kv)) return r;
   return 0;
 }
 
@@ -1247,28 +1235,6 @@ extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* c
 // ================================================================================================
 // IP-Adapter (include/sdxl_b200.h: sdxl_ip_adapter_load, sdxl_unet_set_image_prompt; DESIGN.md §9)
 // ================================================================================================
-// Path and width of every UNet transformer block in execution order: the block program of load_encoder / build_model. The adapter
-// loader needs it before any UNet exists; set_image_prompt checks the result against the paths the UNet recorded while loading.
-static std::vector<std::pair<std::string, int>> unet_tblock_paths(const sdxl_unet_cfg& g) {
-  std::vector<std::pair<std::string, int>> out;
-  const int mc = g.model_channels, last = g.n_levels - 1;
-  auto st = [&](const std::string& bp, int level) {
-    for (int j = 0; j < g.transformer_depths[level]; ++j) out.push_back({bp + "/transformer/transformer_" + std::to_string(j), g.channel_mults[level] * mc});
-  };
-  int idx = 1;
-  for (int level = 0; level < g.n_levels; ++level) {
-    for (int k = 0; k < 2; ++k, ++idx)
-      if (level == 1 || level == 2) st("input_blocks/" + std::to_string(idx), level);
-    if (level != last) ++idx;
-  }
-  st("middle_block", last);
-  idx = 0;
-  for (int level = last; level >= 0; --level)
-    for (int k = 0; k < 3; ++k, ++idx)
-      if (level == 1 || level == 2) st("output_blocks/" + std::to_string(idx), level);
-  return out;
-}
-
 static int build_ip_adapter(sdxl_ip_adapter* a, const PackView& pv, Arena& A) {
   const sdxl_ip_adapter_cfg& g = a->cfg;
   const int ctx_dim = g.unet.context_dim;
@@ -1277,19 +1243,27 @@ static int build_ip_adapter(sdxl_ip_adapter* a, const PackView& pv, Arena& A) {
   a->proj = L.linear("image_proj/proj", g.image_embed_dim, g.tokens_per_image * ctx_dim, true);
   a->norm = L.norm("image_proj/norm", ctx_dim);
   a->kv.clear();
-  a->paths.clear();
-  for (const auto& pc : unet_tblock_paths(g.unet)) {
-    if (L.err) return L.err;
-    Lin kv;
-    kv.K = ctx_dim; kv.Kpad = Loader::pad64(ctx_dim); kv.N = 2 * pc.second;
-    kv.w = A.get<__half>((size_t)kv.N * kv.Kpad);
-    if (!kv.w) return fail(a->ctx, 4005, "weight arena exhausted");
-    L.lin_into(pc.first + "/attn2/ip_key", kv.w, kv.Kpad, 0, ctx_dim, pc.second, 0);
-    L.lin_into(pc.first + "/attn2/ip_value", kv.w, kv.Kpad, pc.second, ctx_dim, pc.second, 0);
-    names.insert(pc.first + "/attn2/ip_key/weight");
-    names.insert(pc.first + "/attn2/ip_value/weight");
-    a->kv.push_back(kv);
-    a->paths.push_back(pc.first);
+  // one fused [ip_key | ip_value] per UNet transformer block, in the order of the UNet's tblocks
+  const BlockProgram prog = block_program(g.unet);
+  std::vector<BlockSpec> blocks = prog.ins;
+  blocks.push_back(prog.mid);
+  blocks.insert(blocks.end(), prog.outs.begin(), prog.outs.end());
+  for (const BlockSpec& s : blocks) {
+    if (!has_transformer(s.type)) continue;
+    const int C = s.c_out;
+    for (int j = 0; j < s.depth; ++j) {
+      if (L.err) return L.err;
+      const std::string bp = s.path + "/transformer/transformer_" + std::to_string(j);
+      Lin kv;
+      kv.K = ctx_dim; kv.Kpad = Loader::pad64(ctx_dim); kv.N = 2 * C;
+      kv.w = A.get<__half>((size_t)kv.N * kv.Kpad);
+      if (!kv.w) return fail(a->ctx, 4005, "weight arena exhausted");
+      L.lin_into(bp + "/attn2/ip_key", kv.w, kv.Kpad, 0, ctx_dim, C, 0);
+      L.lin_into(bp + "/attn2/ip_value", kv.w, kv.Kpad, C, ctx_dim, C, 0);
+      names.insert(bp + "/attn2/ip_key/weight");
+      names.insert(bp + "/attn2/ip_value/weight");
+      a->kv.push_back(kv);
+    }
   }
   if (L.err) return L.err;
   for (const auto& t : pv.t)   // e.g. a pack for a UNet with more transformer blocks
@@ -1365,8 +1339,8 @@ extern "C" int sdxl_ip_adapter_project(sdxl_ip_adapter* a, int n, const float* e
 
 // Writes the buffers that depend on the prompt's values: the tokens of prompts and negatives, and the per-block scales. Everything
 // is computed into temporaries first and copied into `a` only when all of it has succeeded, so a failure leaves `a` unchanged.
-static int ip_write(sdxl_ctx* c, IpAttach& a, const sdxl_image_prompt& p, int n_tblocks) {
-  const int n = p.n_batch * p.n_images;
+static int ip_write(sdxl_ctx* c, IpAttach& a, const sdxl_image_prompt& p) {
+  const int n = p.n_batch * p.n_images, n_tb = (int)a.ad->kv.size();
   const size_t tok_bytes = (size_t)a.n_batch * a.S_ip * a.ad->cfg.unet.context_dim * sizeof(__half);
   const size_t bytes = (size_t)n * a.ad->cfg.image_embed_dim * sizeof(float);
   TmpBufs T(c->stream);
@@ -1385,17 +1359,17 @@ static int ip_write(sdxl_ctx* c, IpAttach& a, const sdxl_image_prompt& p, int n_
   }
   __half* tp = (__half*)T.get(tok_bytes);
   __half* tn = (__half*)T.get(tok_bytes);
-  float* ts = (float*)T.get(n_tblocks * sizeof(float));
+  float* ts = (float*)T.get(n_tb * sizeof(float));
   if (!tp || !tn || !ts) return fail(c, 4820, "set_image_prompt: cannot allocate the token staging buffers");
   if (int r = ip_project(a.ad, n, e, tp)) return r;
   if (int r = ip_project(a.ad, n, neg, tn)) return r;
-  std::vector<float> s(n_tblocks, p.scale);
-  if (p.block_scales_host) s.assign(p.block_scales_host, p.block_scales_host + n_tblocks);
+  std::vector<float> s(n_tb, p.scale);
+  if (p.block_scales_host) s.assign(p.block_scales_host, p.block_scales_host + n_tb);
   CU(c, cudaMemcpyAsync(ts, s.data(), s.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
   CU(c, cudaStreamSynchronize(c->stream));   // s and the caller's host memory; any failure of the work above surfaces here
   CU(c, cudaMemcpyAsync(a.tok_pos, tp, tok_bytes, cudaMemcpyDeviceToDevice, c->stream));
   CU(c, cudaMemcpyAsync(a.tok_neg, tn, tok_bytes, cudaMemcpyDeviceToDevice, c->stream));
-  CU(c, cudaMemcpyAsync(a.scales, ts, n_tblocks * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(a.scales, ts, n_tb * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
   return 0;
 }
 
@@ -1408,7 +1382,6 @@ extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt*
     CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
     u->plan.reset();
     u->ip.reset();
-    u->ip_version++;
     return 0;
   }
   // validate everything first: on failure the attached state is unchanged
@@ -1418,25 +1391,21 @@ extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt*
   if (u->cfg.is_refiner) return fail(c, 4832, "set_image_prompt: IP-Adapter on the refiner is not supported");
   if (const char* field = unet_cfg_mismatch(u->cfg, ad->cfg.unet))
     return fail(c, 4833, "set_image_prompt: adapter cfg field '%s' differs from the UNet's", field);
-  const std::vector<const TBlock*> tbs = unet_tblocks(u);
-  if (tbs.size() != ad->kv.size()) return fail(c, 4834, "set_image_prompt: adapter has %zu blocks, the UNet %zu", ad->kv.size(), tbs.size());
-  for (size_t i = 0; i < tbs.size(); ++i)   // the plan indexes the adapter's K/V by the UNet's transformer-block order
-    if (tbs[i]->path != ad->paths[i] || tbs[i]->kv2.N != ad->kv[i].N)
-      return fail(c, 4834, "set_image_prompt: block %zu: adapter has '%s' (width %d), the UNet '%s' (width %d)", i, ad->paths[i].c_str(),
-                  ad->kv[i].N / 2, tbs[i]->path.c_str(), tbs[i]->kv2.N / 2);
+  // equal cfgs: the adapter's K/V were laid out by the same block program as the UNet's transformer blocks
+  const int n_tb = (int)ad->kv.size();
   if (!p->embeds) return fail(c, 4835, "set_image_prompt: null embeds");
   if (p->n_batch < 1 || p->n_images < 1 || p->n_images > 64)
     return fail(c, 4836, "set_image_prompt: n_batch = %d must be >= 1 and n_images = %d in [1, 64]", p->n_batch, p->n_images);
   if (!isfinite(p->scale)) return fail(c, 4837, "set_image_prompt: scale is not finite");
   if (p->block_scales_host)
-    for (size_t i = 0; i < tbs.size(); ++i)
-      if (!isfinite(p->block_scales_host[i])) return fail(c, 4837, "set_image_prompt: block scale %zu is not finite", i);
-  if (u->condB > 0)
-    if (int r = ip_check_batch(u, p->n_batch, u->condB, u->cfg_rows)) return r;
-  const int n_tb = (int)tbs.size();
+    for (int i = 0; i < n_tb; ++i)
+      if (!isfinite(p->block_scales_host[i])) return fail(c, 4837, "set_image_prompt: block scale %d is not finite", i);
+  const int condB = u->cond.condB;
+  if (condB > 0)
+    if (int r = ip_check_batch(u, p->n_batch, condB, u->cfg_rows)) return r;
   if (u->ip && u->ip->ad == ad && u->ip->n_batch == p->n_batch && u->ip->n_images == p->n_images) {   // same buffers: plan stays
-    if (int r = ip_write(c, *u->ip, *p, n_tb)) return r;
-    return u->condB > 0 ? ip_hoist(u, *u->ip) : 0;
+    if (int r = ip_write(c, *u->ip, *p)) return r;
+    return condB > 0 ? ip_hoist(u, *u->ip) : 0;
   }
   std::unique_ptr<IpAttach> a(new IpAttach());
   a->ad = ad;
@@ -1444,19 +1413,21 @@ extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt*
   a->n_images = p->n_images;
   a->S_ip = p->n_images * ad->cfg.tokens_per_image;
   const size_t tok = (size_t)p->n_batch * a->S_ip * u->cfg.context_dim;
-  if (a->mem.init(2 * tok * sizeof(__half) + n_tb * sizeof(float) + 4096)) return fail(c, 4838, "set_image_prompt: cannot allocate token buffers");
-  a->tok_pos = a->mem.get<__half>(tok);
-  a->tok_neg = a->mem.get<__half>(tok);
-  a->scales = a->mem.get<float>(n_tb);
-  if (u->condB > 0)
-    if (int r = ip_cond_alloc(u, *a)) return r;
-  if (int r = ip_write(c, *a, *p, n_tb)) return r;
-  if (u->condB > 0)
+  if (int r = carve_measured(c, a->mem, 4838, "set_image_prompt: token buffers", [&](Arena& A) {
+        a->tok_pos = A.get<__half>(tok);
+        a->tok_neg = A.get<__half>(tok);
+        a->scales = A.get<float>(n_tb);
+        return 0;
+      }))
+    return r;
+  if (condB > 0)
+    if (int r = ip_cond_alloc(c, *a, condB, a->cond)) return r;
+  if (int r = ip_write(c, *a, *p)) return r;
+  if (condB > 0)
     if (int r = ip_hoist(u, *a)) return r;
   CU(c, cudaStreamSynchronize(c->stream));   // the old plan and attachment may still be in flight
   u->plan.reset();
   u->ip = std::move(a);
-  u->ip_version++;
   return 0;
 }
 
@@ -1475,7 +1446,7 @@ extern "C" int sdxl_unet_set_adapters(sdxl_unet* u, int n, const sdxl_adapter* a
     CU(c, cudaMemcpy2DAsync(u->conv_out_w2 + (size_t)h2 * cv.Ktot, (size_t)2 * cv.Ktot * sizeof(__half), cv.w, (size_t)cv.Ktot * sizeof(__half),
                             (size_t)cv.Ktot * sizeof(__half), (size_t)cv.O, cudaMemcpyDeviceToDevice, c->stream));
   // cross-attention K/V and the label MLP were computed from the previous weights
-  return u->condB > 0 ? hoist_conditioning(u) : 0;
+  return u->cond.condB > 0 ? hoist_conditioning(u) : 0;
 }
 
 // ================================================================================================
@@ -1579,19 +1550,24 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
   Sampler* S = u->sampler.get();
   const size_t lat = (size_t)Bimg * g.in_channels * h * w;
   if (n_ctx < 1) return fail(c, 5202, "bad conditioning context length");
+  // new shapes: a fresh sampler, installed only when the conditioning and the plan for it are in place (the steps pair its
+  // shapes with the plan's buffers)
+  std::unique_ptr<Sampler> fresh;
   if (!S || S->Bimg != Bimg || S->h != h || S->w != w || S->nfwd != nfwd || S->n_ctx != n_ctx) {   // staging buffers are sized by all five
-    CU(c, cudaStreamSynchronize(c->stream));
-    u->sampler.reset(new Sampler());
-    S = u->sampler.get();
+    fresh.reset(new Sampler());
+    S = fresh.get();
     S->Bimg = Bimg; S->nfwd = nfwd; S->h = h; S->w = w; S->n_ctx = n_ctx; S->latent_elems = lat;
     const size_t ctx_elems = (size_t)nfwd * Bimg * n_ctx * g.context_dim;
     const size_t y_elems = (size_t)nfwd * Bimg * g.adm_in_channels;
-    if (S->arena.init(lat * 4 * 2 + lat + ctx_elems * 2 + y_elems * 2 + (1 << 16))) return fail(c, 5203, "cannot allocate sampler buffers");
-    S->noise = S->arena.get<float>(lat);
-    S->ref = S->arena.get<float>(lat);
-    S->mask = S->arena.get<uint8_t>(lat);
-    S->cond_ctx = S->arena.get<__half>(ctx_elems);
-    S->cond_y = S->arena.get<__half>(y_elems);
+    if (int r = carve_measured(c, S->arena, 5203, "sampler buffers", [&](Arena& A) {
+          S->noise = A.get<float>(lat);
+          S->ref = A.get<float>(lat);
+          S->mask = A.get<uint8_t>(lat);
+          S->cond_ctx = A.get<__half>(ctx_elems);
+          S->cond_y = A.get<__half>(y_elems);
+          return 0;
+        }))
+      return r;
     CU(c, cudaMallocHost((void**)&S->host_stage, lat * sizeof(float)));
   }
   S->guidance = (float)guidance;
@@ -1605,8 +1581,11 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
       CU(c, cudaMemcpyAsync((uint8_t*)S->cond_y + y_row * (Bimg + b), y_u, y_row, kind, c->stream));
     }
   int r = set_conditioning_dev(u, nfwd * Bimg, n_ctx, S->cond_ctx, S->cond_y, nfwd == 2 ? Bimg : 0);
-  if (r) return r;
-  return ensure_plan(u, nfwd * Bimg, Bimg, h, w);
+  if (!r) r = ensure_plan(u, nfwd * Bimg, Bimg, h, w);
+  if (r || !fresh) return r;
+  CU(c, cudaStreamSynchronize(c->stream));   // the old sampler's buffers may still be in flight
+  u->sampler = std::move(fresh);
+  return 0;
 }
 
 // one loop-body iteration (reference stablediffusion/mod.rs:406-429)

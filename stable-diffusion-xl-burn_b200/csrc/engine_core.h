@@ -75,7 +75,11 @@ struct Arena {
   ~Arena() { release(); }
   int init(size_t bytes) {
     release();
-    if (cudaMalloc((void**)&base, bytes) != cudaSuccess) return 1;
+    if (cudaMalloc((void**)&base, bytes) != cudaSuccess) {
+      base = nullptr;
+      cudaGetLastError();   // an oversized request is not sticky: clear it so later launch checks do not report it
+      return 1;
+    }
     cap = bytes;
     off = 0;
     return 0;
@@ -398,15 +402,21 @@ static int with_device_pack(sdxl_ctx* c, const void* pack, size_t bytes, int pac
   return r;
 }
 
-// Loads a model's weights: pass 1 measures, pass 2 builds into the model's weight arena m->warena.
-template <typename M>
-static int build_two_pass(M* m, const PackView& pv, int (*build)(M*, const PackView&, Arena&)) {
+// Sizes A by measuring: carve(Arena&) runs once against a measuring arena (placeholder pointers, no device work), A is
+// allocated to the measured size, and carve runs again against A. carve must take the same buffers on both passes.
+template <typename Fn>
+static int carve_measured(sdxl_ctx* c, Arena& A, int code, const char* what, Fn carve) {
   Arena meas;
   meas.measure = true;
-  int r = build(m, pv, meas);
-  if (!r && m->warena.init(meas.off + (1 << 20))) r = fail(m->ctx, 4203, "cannot allocate %zu bytes for weights", meas.off);
-  if (!r) r = build(m, pv, m->warena);
-  return r;
+  if (int r = carve(meas)) return r;
+  if (A.init(meas.off)) return fail(c, code, "cannot allocate %zu bytes for %s", meas.off, what);
+  return carve(A);
+}
+
+// Loads a model's weights into its weight arena m->warena.
+template <typename M>
+static int build_two_pass(M* m, const PackView& pv, int (*build)(M*, const PackView&, Arena&)) {
+  return carve_measured(m->ctx, m->warena, 4203, "weights", [&](Arena& A) { return build(m, pv, A); });
 }
 
 // ================================================================================================
@@ -445,9 +455,6 @@ struct Op {
 
 struct Plan {
   int Bf = 0, Bx = 0, h = 0, w = 0;
-  uint64_t cond_version = 0;
-  uint64_t controls_version = 0;   // UNet: the attached ControlNet set the plan was built for
-  uint64_t ip_version = 0;         // UNet: the image-prompt attachment the plan was built for
   Arena arena;
   std::vector<Op> ops;
   float* x_in = nullptr;  // [Bx, Cin, h, w] f32 NCHW
@@ -464,19 +471,15 @@ struct Plan {
   }
 };
 
-// (Re)builds `plan` for new shapes: build(P, A) runs once against a measuring arena, then against P->arena sized by the
-// measurement. Dims are the plan's cache keys; on failure the plan is dropped.
+// (Re)builds `plan` for new shapes: build(P, A) fills the plan and takes its buffers from A, P->arena sized by measuring.
+// Dims are the plan's cache keys; on failure the plan is dropped.
 template <typename Fn>
 static int build_plan(sdxl_ctx* c, std::unique_ptr<Plan>& plan, int Bf, int Bx, int h, int w, Fn build) {
   CU(c, cudaStreamSynchronize(c->stream));   // the old plan may still be in flight
   plan.reset(new Plan());
   Plan* P = plan.get();
   P->Bf = Bf; P->Bx = Bx; P->h = h; P->w = w;
-  Arena meas;
-  meas.measure = true;
-  int r = build(P, &meas);
-  if (!r && P->arena.init(meas.off + (1 << 20))) r = fail(c, 5011, "cannot allocate %zu bytes of workspace", meas.off);
-  if (!r) r = build(P, &P->arena);
+  int r = carve_measured(c, P->arena, 5011, "the plan's workspace", [&](Arena& A) { return build(P, &A); });
   if (r) plan.reset();
   return r;
 }

@@ -11,7 +11,7 @@ import torch
 
 from . import _lib
 from ._lib import SdxlError
-from .config import ControlNetConfig, UNetConfig
+from .config import ControlNetConfig, UNetConfig, block_program
 from .engine import _cfg_struct
 from .lora import read_safetensors
 from .weights import build_pack, controlnet_tensor_specs
@@ -83,8 +83,8 @@ def diffusers_name_map(cfg: ControlNetConfig) -> Dict[str, Tuple[str, bool]]:
             put(f"{s}.ff.net.0.proj", f"{d}/mlp/geglu/proj", True)
             put(f"{s}.ff.net.2", f"{d}/mlp/lin", True)
 
-    u = cfg.unet
-    put("conv_in", "input_blocks/0")
+    ins, mid, _ = block_program(cfg.unet)
+    put("conv_in", ins[0].path)
     put("time_embedding.linear_1", "lin1_time_embed", True)
     put("time_embedding.linear_2", "lin2_time_embed", True)
     put("add_embedding.linear_1", "lin1_label_embed", True)
@@ -93,24 +93,22 @@ def diffusers_name_map(cfg: ControlNetConfig) -> Dict[str, Tuple[str, bool]]:
     for k in range(2 * (len(cfg.hint_block_channels) - 1)):
         put(f"controlnet_cond_embedding.blocks.{k}", f"input_hint_block/{2 * k + 2}")
     put("controlnet_cond_embedding.conv_out", f"input_hint_block/{4 * len(cfg.hint_block_channels) - 2}")
-    idx = 1
-    for lvl in range(u.n_levels):
-        c_in, c_out = u.channel_mults[max(lvl - 1, 0)] * u.model_channels, u.channel_mults[lvl] * u.model_channels
-        tr = u.transformer_depths[lvl] > 0
-        for j in range(2):
-            dst = f"input_blocks/{idx}"
-            res(f"down_blocks.{lvl}.resnets.{j}", f"{dst}/res" if tr else dst, j == 0 and c_in != c_out)
-            if tr:
-                st(f"down_blocks.{lvl}.attentions.{j}", f"{dst}/transformer", u.transformer_depths[lvl])
-            idx += 1
-        if lvl != u.n_levels - 1:
-            put(f"down_blocks.{lvl}.downsamplers.0.conv", f"input_blocks/{idx}")
-            idx += 1
-    for i in range(idx):
+    lvl, j = 0, 0   # diffusers numbers the blocks of a level: resnets.{j} / attentions.{j}, then the level's downsampler
+    for b in ins[1:]:
+        if b.kind == "downsample":
+            put(f"down_blocks.{lvl}.downsamplers.0.conv", b.path)
+            lvl, j = lvl + 1, 0
+            continue
+        tr = b.kind == "resnet_transformer"
+        res(f"down_blocks.{lvl}.resnets.{j}", f"{b.path}/res" if tr else b.path, b.c_in != b.c_out)
+        if tr:
+            st(f"down_blocks.{lvl}.attentions.{j}", f"{b.path}/transformer", b.depth)
+        j += 1
+    for i in range(len(ins)):
         put(f"controlnet_down_blocks.{i}", f"zero_convs/{i}")
-    res("mid_block.resnets.0", "middle_block/res1", False)
-    st("mid_block.attentions.0", "middle_block/transformer", u.transformer_depths[-1])
-    res("mid_block.resnets.1", "middle_block/res2", False)
+    res("mid_block.resnets.0", f"{mid.path}/res1", False)
+    st("mid_block.attentions.0", f"{mid.path}/transformer", mid.depth)
+    res("mid_block.resnets.1", f"{mid.path}/res2", False)
     put("controlnet_mid_block", "middle_block_out")
     return m
 

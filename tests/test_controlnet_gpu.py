@@ -106,13 +106,21 @@ def test_two_controls_vs_oracle(S):
     S.d.set_controls([])
 
 
+def builds(S):
+    return int(S.ctx.lib.sdxl_unet_plan_builds(S.d.h))
+
+
 def test_detach_is_bit_identical(S):
+    S.fwd()
+    n = builds(S)
     S.d.set_controls([(S.nets[0], S.h[0], 1.0)])
     controlled = S.fwd()
     assert S.d.plan_num_ops > S.base_ops
+    assert builds(S) == n + 1                 # attaching drops the plan: rebuilt once
     S.d.set_controls([])
     assert torch.equal(S.fwd(), S.base)
     assert S.d.plan_num_ops == S.base_ops
+    assert builds(S) == n + 2                 # and so does detaching
     fresh = Diffuser(S.ctx, TINY, S.w)
     assert torch.equal(fresh.unet_forward(X, [T], S.c, S.y), S.base)
     assert fresh.plan_num_ops == S.base_ops
@@ -125,9 +133,11 @@ def test_rescale_in_place_matches_fresh_attach(S):
     S.fwd()
     S.fwd()                                   # plan built and graph captured
     n_ops = S.d.plan_num_ops
+    n_builds = builds(S)
     S.d.set_controls([(S.nets[0], S.h[0], 1.0)])   # same net, n_hint, size: buffers rewritten in place
     rescaled = S.fwd()
     assert S.d.plan_num_ops == n_ops
+    assert builds(S) == n_builds                   # the plan and its graph were kept
     S.d.set_controls([])
     S.d.set_controls([(S.nets[0], S.h[0], 1.0)])
     assert torch.equal(S.fwd(), rescaled)

@@ -116,13 +116,17 @@ def test_forward_against_oracle(S, nb, ni):
 
 
 def test_detach_restores_bit_identical(S):
+    builds = lambda: S.ctx.lib.sdxl_unet_plan_builds(S.d.h)  # noqa: E731
     base = S.fwd()
     n_ops = S.d.plan_num_ops
+    n_builds = builds()
     S.d.set_image_prompt(S.ad, embeds(2, 1, 1), 1.0)
     with_ip = S.fwd()
     assert not torch.equal(with_ip, base) and S.d.plan_num_ops == n_ops
+    assert builds() == n_builds + 1         # attaching drops the plan: rebuilt once
     S.d.set_image_prompt(None)
     assert torch.equal(S.fwd(), base) and S.d.plan_num_ops == n_ops
+    assert builds() == n_builds + 2         # and so does detaching
 
 
 def test_scale_zero_equals_no_prompt(S):

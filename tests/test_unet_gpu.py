@@ -179,6 +179,27 @@ def test_seeded_sampling_is_deterministic(tiny):
     assert not torch.equal(a, c2)
 
 
+def test_plan_follows_conditioning_shape(tiny):
+    """A same-shape set_conditioning keeps the plan and its CUDA graph and the new values reach it; a new batch or context
+    length rebuilds the plan once."""
+    d, _ = tiny
+    builds = lambda: int(d.ctx.lib.sdxl_unet_plan_builds(d.h))  # noqa: E731
+    x = arb(2, 4, 16, 16)
+    c, y = h16f(arb(2, 7, TINY.context_dim)), h16f(arb(2, TINY.adm_in_channels))
+    d.unet_forward(x, [499], c, y)
+    d.unet_forward(x, [499])                     # the second run captures the CUDA graph
+    n = builds()
+    kept = d.unet_forward(x, [499], h16f(c * 0.5), y)
+    assert builds() == n
+    d.unet_forward(x, [499], h16f(arb(2, 9, TINY.context_dim)), y)   # new n_ctx
+    assert builds() == n + 1
+    d.unet_forward(x[:1], [499], c[:1], y[:1])   # new batch
+    d.unet_forward(x[:1], [499])
+    assert builds() == n + 2
+    assert torch.equal(d.unet_forward(x, [499], h16f(c * 0.5), y), kept)   # rebuilt for batch 2: same result as the kept plan
+    assert builds() == n + 3
+
+
 def test_error_paths(ctx, tiny):
     d, _ = tiny
     from sdxl_b200 import SdxlError
