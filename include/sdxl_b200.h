@@ -395,6 +395,11 @@ SDXL_API void sdxl_clip_vision_destroy(sdxl_clip_vision* v);
 /* image_embeds_out f32 [N, proj_dim] of pixels f32 NCHW [N, 3, image_size, image_size] as CLIPImageProcessor produces them (resized,
  * centre-cropped, normalised); both host memory if on_host. */
 SDXL_API int sdxl_clip_vision_encode(sdxl_clip_vision* v, int N, const float* pixels, int on_host, float* image_embeds_out);
+/* hidden_out f32 [N, T, n_state] = HF hidden_states[hidden_idx] of the same pixels, hidden_idx in [0, n_layer]: the pre_layrnorm
+ * output for 0, else the residual stream after blocks 0..hidden_idx-1 (no post_layernorm; the convention of
+ * sdxl_clip_forward_hidden). Only hidden_idx blocks run. IP-Adapter Plus reads hidden_states[-2], i.e. hidden_idx = n_layer - 1. */
+SDXL_API int sdxl_clip_vision_encode_hidden(sdxl_clip_vision* v, int N, const float* pixels, int on_host, int hidden_idx,
+                                            float* hidden_out);
 
 /* ---- IP-Adapter (image prompts) -----------------------------------------------------------------------
  * The published IP-Adapter for SDXL, base variant (DESIGN.md §9; diffusers IPAdapterAttnProcessor2_0 + ImageProjection): an
@@ -407,12 +412,27 @@ SDXL_API int sdxl_clip_vision_encode(sdxl_clip_vision* v, int N, const float* pi
  *   <transformer block path>/attn2/ip_key/weight and .../ip_value/weight [context_dim, C] for every UNet transformer block, e.g.
  *   input_blocks/4/transformer/transformer_0/attn2/ip_key/weight.
  * An adapter is built on one ctx and may be attached to any UNet of that ctx whose cfg equals its `unet`. The refiner is not
- * supported. */
+ * supported.
+ *
+ * IP-Adapter Plus (resampler_depth > 0; h94 `ip-adapter-plus*_sdxl_vit-h`, diffusers IPAdapterPlusImageProjection): the image input
+ * is the vision encoder's penultimate hidden states h [L, D] (sdxl_clip_vision_encode_hidden, hidden_idx = n_layer - 1) and a
+ * perceiver Resampler of width W = 64 * resampler_heads turns them into Q = tokens_per_image tokens (every LayerNorm eps 1e-5):
+ *   x = h @ proj_in + b_in;  lat = latents
+ *   per layer i: kv = [LN1_i(x) ; LN2_i(lat)] (L + Q rows), q = LN2_i(lat) @ to_q, [k | v] = kv @ to_kv,
+ *                lat += (softmax(q k^T / 8) v per 64-wide head) @ to_out,  lat += gelu_erf(LNff_i(lat) @ fc1) @ fc2
+ *   tokens = LayerNorm(lat @ proj_out + b_out)                                        [Q, context_dim]
+ * Its pack holds, instead of image_proj/{proj,norm}, Linear weights [in, out] without biases unless named:
+ *   image_proj/latents [Q, W], image_proj/proj_in/{weight [D, W], bias}, image_proj/layers/<i>/attn/{norm1,norm2}/{weight,bias},
+ *   image_proj/layers/<i>/attn/{to_q [W, W], to_kv [W, 2W] (K columns, then V), to_out [W, W]}/weight,
+ *   image_proj/layers/<i>/ff/norm/{weight,bias}, image_proj/layers/<i>/ff/{fc1 [W, 4W], fc2 [4W, W]}/weight,
+ *   image_proj/proj_out/{weight [W, context_dim], bias}, image_proj/norm_out/{weight,bias}, and the same ip_key / ip_value. */
 typedef struct sdxl_ip_adapter sdxl_ip_adapter;
 typedef struct sdxl_ip_adapter_cfg {
   sdxl_unet_cfg unet;            /* must equal the cfg of the UNet it is attached to; context_dim a multiple of 8 */
-  int32_t image_embed_dim;       /* D: 1024 (ViT-H/14 encoder), 1280 (ViT-bigG/14 encoder) */
-  int32_t tokens_per_image;      /* 4 */
+  int32_t image_embed_dim;       /* D: 1024 (ViT-H/14 encoder), 1280 (ViT-bigG/14 encoder); Plus: the hidden width, 1280 for ViT-H/14 */
+  int32_t tokens_per_image;      /* 4; Plus: Q = 16 */
+  int32_t resampler_depth;       /* 0: the base adapter; Plus: the number of perceiver layers (4) */
+  int32_t resampler_heads;       /* Plus: the Resampler's heads of width 64 (20); ignored when resampler_depth = 0 */
 } sdxl_ip_adapter_cfg;
 SDXL_API int sdxl_ip_adapter_load(sdxl_ctx* ctx, const sdxl_ip_adapter_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
                                   sdxl_ip_adapter** out);
@@ -420,22 +440,31 @@ SDXL_API int sdxl_ip_adapter_load(sdxl_ctx* ctx, const sdxl_ip_adapter_cfg* cfg,
 SDXL_API void sdxl_ip_adapter_destroy(sdxl_ip_adapter* adapter);
 typedef struct sdxl_image_prompt {
   const sdxl_ip_adapter* adapter;
-  const float* embeds;             /* f32 [n_batch * n_images, D]: image i of prompt b at row b * n_images + i */
-  const float* negative_embeds;    /* same shape, or NULL: the unconditional rows use the projection of zero embeddings */
+  const float* embeds;             /* f32 [n_batch * n_images, D]: image i of prompt b at row b * n_images + i;
+                                      Plus: f32 [n_batch * n_images, seq_len, D] hidden states in the same order */
+  const float* negative_embeds;    /* same shape, or NULL: the unconditional rows use the projection of zero embeddings. Plus: required
+                                      (h94 / diffusers use the hidden states of an all-zero pixel tensor, which the library cannot
+                                      compute from the prompt); NULL is refused */
   int32_t on_host;                 /* both pointers are host memory; borrowed for the call */
   int32_t n_batch, n_images;       /* S_ip = n_images * tokens_per_image tokens per row, images concatenated in order */
   float scale;                     /* s_blk of every block, unless block_scales_host is given */
   const float* block_scales_host;  /* NULL or s_blk of each UNet transformer block in execution order (input blocks, middle, output) */
+  int32_t seq_len;                 /* Plus: L, the hidden-state rows per image (257 for ViT-H/14), in [1, 4096]; ignored otherwise */
 } sdxl_image_prompt;
 /* Attaches an image prompt to the UNet (NULL detaches). Row rule: in the sampler's CFG batch [cond | uncond] of n images, cond row
  * b uses embeds prompt b % n_batch and uncond row b negative prompt b % n_batch; a direct sdxl_unet_forward of B rows uses prompt
  * r % n_batch for row r. Everything is validated before anything changes (ctx, cfg, n_batch >= 1, n_images >= 1, finite scales, the
- * current conditioning batch a multiple of n_batch): on failure the previous state stays. A call with the same adapter, n_batch and
+ * current conditioning batch a multiple of n_batch; Plus: negative_embeds given, seq_len in range): on failure the previous state stays. A call with the same adapter, n_batch and
  * n_images rewrites tokens, K/V and scales in place (same launch plan and CUDA graph); any other change rebuilds the plan at the
  * next forward. The image K/V are recomputed whenever the conditioning is set. An attached ControlNet's attentions see text only. */
 SDXL_API int sdxl_unet_set_image_prompt(sdxl_unet* unet, const sdxl_image_prompt* prompt);
-/* Test aid: tokens f16 [n * tokens_per_image, context_dim] of embeds f32 [n, D]; both host memory if on_host. */
+/* Test aid: tokens f16 [n * tokens_per_image, context_dim] of embeds f32 [n, D]; both host memory if on_host. A Plus adapter is
+ * refused (use sdxl_ip_adapter_resample). */
 SDXL_API int sdxl_ip_adapter_project(sdxl_ip_adapter* adapter, int n, const float* embeds, int on_host, sdxl_half* tokens_out);
+/* Test aid (Plus adapters only): tokens f16 [n * tokens_per_image, context_dim] = Resampler(hidden) of hidden states f32
+ * [n, seq_len, D]; both host memory if on_host. */
+SDXL_API int sdxl_ip_adapter_resample(sdxl_ip_adapter* adapter, int n, int seq_len, const float* hidden, int on_host,
+                                      sdxl_half* tokens_out);
 /* Test aid: out = softmax(q k^T / 8) v + scale * softmax(q k_ip^T / 8) v_ip per head (head dim 64); q/out [B,T,C], k/v [B,S,C],
  * k_ip/v_ip [B,S_ip,C] f16 device memory. */
 SDXL_API int sdxl_op_ip_attention(sdxl_ctx* ctx, const sdxl_half* q, const sdxl_half* k, const sdxl_half* v, const sdxl_half* k_ip,

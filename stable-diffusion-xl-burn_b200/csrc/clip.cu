@@ -296,9 +296,11 @@ struct sdxl_clip_vision {
   Lin proj;                  // visual_projection [proj_dim, n_state]
   std::unique_ptr<Plan> plan;
   int pN = 0;
+  int p_hidden = -1;         // the plan's hidden_idx (blocks run, no pooled output), or -1: all blocks and image_embeds
   __half* patch16 = nullptr; // plan buffers of the embedding steps, run before the plan
   float* patches = nullptr;
   float* x = nullptr;
+  float* hidden = nullptr;   // the stream after the plan's blocks
   float* embeds = nullptr;
   int tokens() const { return (cfg.image_size / cfg.patch_size) * (cfg.image_size / cfg.patch_size) + 1; }
 };
@@ -380,7 +382,8 @@ extern "C" void sdxl_clip_vision_destroy(sdxl_clip_vision* m) {
   delete m;
 }
 
-static int build_vision_plan(sdxl_clip_vision* m, Plan* P, Arena* A) {
+// n_run blocks; pooled: then post_layernorm of the class token and visual_projection into m->embeds.
+static int build_vision_plan(sdxl_clip_vision* m, Plan* P, Arena* A, int n_run, int pooled) {
   sdxl_ctx* c = m->ctx;
   const sdxl_clip_vision_cfg& g = m->cfg;
   PlanBuilder B{c, P, A, P->Bf};
@@ -391,15 +394,16 @@ static int build_vision_plan(sdxl_clip_vision* m, Plan* P, Arena* A) {
   m->patches = B.buf<float>((size_t)N * (T - 1) * C);
   const ClipStream s{B.buf<float>((size_t)M * C), B.buf<float>((size_t)M * C), B.buf<__half>((size_t)M * C), B.buf<__half>((size_t)M * 3 * C),
                      B.buf<__half>((size_t)M * C), B.buf<float>((size_t)M * g.mlp_dim), B.buf<__half>((size_t)M * g.mlp_dim)};
-  int* idx0 = B.buf<int>(N);
-  float* pin = B.buf<float>((size_t)N * C);
-  m->embeds = B.buf<float>((size_t)N * g.proj_dim);
+  int* idx0 = pooled ? B.buf<int>(N) : nullptr;
+  float* pin = pooled ? B.buf<float>((size_t)N * C) : nullptr;
+  m->embeds = pooled ? B.buf<float>((size_t)N * g.proj_dim) : nullptr;
   if (B.err) return B.err;
-  if (!A->measure) CU(c, cudaMemsetAsync(idx0, 0, N * sizeof(int), c->stream));   // the class token of every image
+  if (pooled && !A->measure) CU(c, cudaMemsetAsync(idx0, 0, N * sizeof(int), c->stream));   // the class token of every image
   m->x = s.xa;
-  float* hidden = nullptr;
-  float* x = clip_block_ops(B, m->blocks, g.n_layer, -1, &hidden, s, N, T, C, g.n_head, C / g.n_head, g.mlp_dim, 0, g.quick_gelu);
-  if (B.err) return B.err;
+  float* unused = nullptr;
+  float* x = clip_block_ops(B, m->blocks, n_run, -1, &unused, s, N, T, C, g.n_head, C / g.n_head, g.mlp_dim, 0, g.quick_gelu);
+  m->hidden = x;
+  if (B.err || !pooled) return B.err;
   Op op{};
   op.kind = OP_LN_GATHER;
   op.lg = {x, idx0, N, T, C, m->post_ln.g, m->post_ln.b, m->post_ln.eps, pin};
@@ -408,15 +412,19 @@ static int build_vision_plan(sdxl_clip_vision* m, Plan* P, Arena* A) {
   return B.err;
 }
 
-extern "C" int sdxl_clip_vision_encode(sdxl_clip_vision* m, int N, const float* pixels, int on_host, float* image_embeds_out) {
-  if (!m || !pixels || !image_embeds_out) return fail(m ? m->ctx : nullptr, -1, "sdxl_clip_vision_encode: null argument");
+// Embeds the pixels and runs the plan for (N, hidden_idx); hidden_idx = -1: every block and image_embeds. The result is m->hidden
+// (and m->embeds), queued on the ctx stream.
+static int vision_run(sdxl_clip_vision* m, int N, const float* pixels, int on_host, int hidden_idx) {
   sdxl_ctx* c = m->ctx;
   const sdxl_clip_vision_cfg& g = m->cfg;
   if (N < 1 || N > 256) return fail(c, 5205, "vision encoder batch must be 1..256 (got %d)", N);
   CU(c, cudaSetDevice(c->device));
-  if (!m->plan || m->pN != N) {
-    if (int r = build_plan(c, m->plan, N, N, 0, 0, [&](Plan* P, Arena* A) { return build_vision_plan(m, P, A); })) return r;
+  if (!m->plan || m->pN != N || m->p_hidden != hidden_idx) {
+    const int n_run = hidden_idx < 0 ? g.n_layer : hidden_idx;
+    if (int r = build_plan(c, m->plan, N, N, 0, 0, [&](Plan* P, Arena* A) { return build_vision_plan(m, P, A, n_run, hidden_idx < 0); }))
+      return r;
     m->pN = N;
+    m->p_hidden = hidden_idx;
   }
   const int S = g.image_size, T = m->tokens(), C = g.n_state;
   const size_t in_bytes = (size_t)N * 3 * S * S * sizeof(float);
@@ -434,9 +442,27 @@ extern "C" int sdxl_clip_vision_encode(sdxl_clip_vision* m, int N, const float* 
   const IgemmOperands o{m->patch16, 1, 1, rows, Pt.Kpad, Pt.Kpad, nullptr, 0, 0, 0, 0, 0, Pt.w, Pt.N, Pt.Kpad};
   if (int r = igemm_run(c, o, {{0, 0, 0, 0, Pt.Kpad / 64}}, 1, rows, 1, IGEMM_LINEAR, 0, m->patches, 1, C, nullptr, nullptr, 0)) return r;
   KL(c, vision_embed_ln_launch(c->stream, m->patches, m->cls, m->pos, N, T, C, m->pre_ln.g, m->pre_ln.b, m->pre_ln.eps, m->x));
-  if (int r = run_plan_ops(c, m->plan.get())) return r;
-  const size_t out_bytes = (size_t)N * g.proj_dim * sizeof(float);
+  return m->plan->ops.empty() ? 0 : run_plan_ops(c, m->plan.get());   // hidden_idx = 0: the embedding alone
+}
+
+extern "C" int sdxl_clip_vision_encode(sdxl_clip_vision* m, int N, const float* pixels, int on_host, float* image_embeds_out) {
+  if (!m || !pixels || !image_embeds_out) return fail(m ? m->ctx : nullptr, -1, "sdxl_clip_vision_encode: null argument");
+  sdxl_ctx* c = m->ctx;
+  if (int r = vision_run(m, N, pixels, on_host, -1)) return r;
+  const size_t out_bytes = (size_t)N * m->cfg.proj_dim * sizeof(float);
   CU(c, cudaMemcpyAsync(image_embeds_out, m->embeds, out_bytes, on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+  if (on_host) CU(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+extern "C" int sdxl_clip_vision_encode_hidden(sdxl_clip_vision* m, int N, const float* pixels, int on_host, int hidden_idx, float* hidden_out) {
+  if (!m || !pixels || !hidden_out) return fail(m ? m->ctx : nullptr, -1, "sdxl_clip_vision_encode_hidden: null argument");
+  sdxl_ctx* c = m->ctx;
+  if (hidden_idx < 0 || hidden_idx > m->cfg.n_layer)
+    return fail(c, 5207, "hidden_idx %d outside [0, n_layer = %d]", hidden_idx, m->cfg.n_layer);
+  if (int r = vision_run(m, N, pixels, on_host, hidden_idx)) return r;
+  const size_t out_bytes = (size_t)N * m->tokens() * m->cfg.n_state * sizeof(float);
+  CU(c, cudaMemcpyAsync(hidden_out, m->hidden, out_bytes, on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
   if (on_host) CU(c, cudaStreamSynchronize(c->stream));
   return 0;
 }

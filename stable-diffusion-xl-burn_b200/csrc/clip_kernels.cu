@@ -359,4 +359,52 @@ int ln_gather_f32_launch(cudaStream_t st, const float* x, const int* idx, int B,
   return launch_kernel(ln_gather_f32_kernel, dim3(B), dim3(32), (size_t)0, st, true, x, idx, T, C, gamma, beta, eps, y);
 }
 
+// ------------------------------------------------------------------------------------------------
+// The two LayerNorms of one IP-Adapter Plus perceiver-attention layer (h94 resampler.py PerceiverAttention), in one launch.
+// Row r of the per-image concatenation [n, L + Q, C]: j = r % (L + Q) < L is LN1 of x[img * L + j], otherwise LN2 of
+// lat[img * Q + j - L]. Every row goes to kv (the operand of to_kv and the attention's keys / values); the LN2 rows also go to
+// q[img * Q + j - L] (the operand of to_q). One block per row, exact two-pass statistics like the other LayerNorms.
+// ------------------------------------------------------------------------------------------------
+__global__ void perceiver_ln_kernel(const float* __restrict__ x, const float* __restrict__ lat, int L, int Q, int C,
+                                    const float* __restrict__ g1, const float* __restrict__ b1, const float* __restrict__ g2,
+                                    const float* __restrict__ b2, float eps, __half* __restrict__ kv, __half* __restrict__ q) {
+  __shared__ float red[32];
+  griddep_wait();
+  griddep_launch_dependents();
+  const int row = blockIdx.x, S = L + Q, img = row / S, j = row % S;
+  const bool is_lat = j >= L;
+  const float* src = is_lat ? lat + ((size_t)img * Q + (j - L)) * C : x + ((size_t)img * L + j) * C;
+  const float* gamma = is_lat ? g2 : g1;
+  const float* beta = is_lat ? b2 : b1;
+  __half* qr = is_lat ? q + ((size_t)img * Q + (j - L)) * C : nullptr;
+  __half* kr = kv + (size_t)row * C;
+  auto block_sum = [&](float s) {
+#pragma unroll
+    for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = s;
+    __syncthreads();
+    float tot = 0.f;
+    for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += red[w];
+    __syncthreads();
+    return tot;
+  };
+  float s = 0.f;
+  for (int i = threadIdx.x; i < C; i += blockDim.x) s += src[i];
+  const float mean = block_sum(s) / C;
+  float sq = 0.f;
+  for (int i = threadIdx.x; i < C; i += blockDim.x) { const float d = src[i] - mean; sq = fmaf(d, d, sq); }
+  const float rstd = 1.f / sqrtf(block_sum(sq) / C + eps);
+  for (int i = threadIdx.x; i < C; i += blockDim.x) {
+    const __half h = __float2half_rn((src[i] - mean) * rstd * gamma[i] + beta[i]);
+    kr[i] = h;
+    if (qr) qr[i] = h;
+  }
+}
+int perceiver_ln_launch(cudaStream_t st, const float* x, const float* lat, int n, int L, int Q, int C, const float* g1,
+                        const float* b1, const float* g2, const float* b2, float eps, __half* kv, __half* q) {
+  if (n < 1 || L < 1 || Q < 1 || C < 1) return 7106;
+  return launch_kernel(perceiver_ln_kernel, dim3((unsigned)(n * (L + Q))), dim3(256), (size_t)0, st, true, x, lat, L, Q, C, g1, b1, g2,
+                       b2, eps, kv, q);
+}
+
 }  // namespace sdxl

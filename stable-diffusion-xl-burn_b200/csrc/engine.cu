@@ -219,15 +219,29 @@ struct ControlAttach {
   HoistedCond cond;               // the net's own conditioning at the UNet's conditioning shape
 };
 
-// IP-Adapter (DESIGN.md §9): the image-token projection and, per UNet transformer block in execution order, the fused
-// [ip_key | ip_value] projection of the image tokens (N = 2C, K = context_dim).
+// One perceiver layer of the IP-Adapter Plus Resampler (include/sdxl_b200.h), width W: the attention's LayerNorms of the image
+// features (ln1) and of the latents (ln2), its projections without biases, and the feed-forward block.
+struct PerceiverLayer {
+  Norm ln1, ln2, ln_ff;
+  Lin to_q, to_kv, to_out;  // [W, W], [2W, W] (K rows, then V), [W, W]
+  Lin fc1, fc2;             // [4W, W], [W, 4W]
+};
+
+// IP-Adapter (DESIGN.md §9): the image-token projection (base: proj + norm; Plus: the Resampler) and, per UNet transformer block
+// in execution order, the fused [ip_key | ip_value] projection of the image tokens (N = 2C, K = context_dim).
 struct sdxl_ip_adapter {
   sdxl_ctx* ctx = nullptr;
   sdxl_ip_adapter_cfg cfg{};
   Arena warena;
   Lin proj;                 // [T * context_dim, D]
   Norm norm;                // over context_dim, eps 1e-5
+  // Plus (cfg.resampler_depth > 0)
+  float* latents = nullptr; // [Q, W]
+  Lin proj_in, proj_out;    // [W, D], [context_dim, W]
+  Norm norm_out;            // over context_dim
+  std::vector<PerceiverLayer> layers;
   std::vector<Lin> kv;
+  bool plus() const { return cfg.resampler_depth > 0; }
 };
 
 // The image prompt's token rows for one conditioning batch and their K/V.
@@ -1239,9 +1253,52 @@ static int build_ip_adapter(sdxl_ip_adapter* a, const PackView& pv, Arena& A) {
   const sdxl_ip_adapter_cfg& g = a->cfg;
   const int ctx_dim = g.unet.context_dim;
   Loader L{a->ctx, &pv, &A, a->ctx->stream};
-  std::set<std::string> names = {"image_proj/proj/weight", "image_proj/proj/bias", "image_proj/norm/weight", "image_proj/norm/bias"};
-  a->proj = L.linear("image_proj/proj", g.image_embed_dim, g.tokens_per_image * ctx_dim, true);
-  a->norm = L.norm("image_proj/norm", ctx_dim);
+  std::set<std::string> names;
+  auto lin = [&](const std::string& path, int K, int N, bool bias) {
+    names.insert(path + "/weight");
+    if (bias) names.insert(path + "/bias");
+    return L.linear(path, K, N, bias);
+  };
+  auto norm = [&](const std::string& path, int C) {
+    names.insert(path + "/weight");
+    names.insert(path + "/bias");
+    return L.norm(path, C);
+  };
+  if (!a->plus()) {
+    a->proj = lin("image_proj/proj", g.image_embed_dim, g.tokens_per_image * ctx_dim, true);
+    a->norm = norm("image_proj/norm", ctx_dim);
+  } else {
+    const int W = 64 * g.resampler_heads, Q = g.tokens_per_image;
+    {   // latents [Q, W] f16 -> f32
+      const PackEntry* e = L.need("image_proj/latents", 2);
+      if (!e) return L.err;
+      if ((int)e->shape[0] != Q || (int)e->shape[1] != W)
+        return fail(a->ctx, 4006, "weight pack: 'image_proj/latents' is [%llu,%llu], expected [%d,%d]", (unsigned long long)e->shape[0],
+                    (unsigned long long)e->shape[1], Q, W);
+      names.insert("image_proj/latents");
+      a->latents = A.get<float>((size_t)Q * W);
+      if (!a->latents) return fail(a->ctx, 4005, "weight arena exhausted");
+      if (!A.measure) KL(a->ctx, cast_f16_to_f32_launch(a->ctx->stream, L.ptr(e), (size_t)Q * W, a->latents));
+    }
+    a->proj_in = lin("image_proj/proj_in", g.image_embed_dim, W, true);
+    a->layers.clear();
+    for (int i = 0; i < g.resampler_depth && !L.err; ++i) {
+      const std::string lp = "image_proj/layers/" + std::to_string(i);
+      PerceiverLayer l;
+      l.ln1 = norm(lp + "/attn/norm1", W);
+      l.ln2 = norm(lp + "/attn/norm2", W);
+      l.to_q = lin(lp + "/attn/to_q", W, W, false);
+      l.to_kv = lin(lp + "/attn/to_kv", W, 2 * W, false);
+      l.to_out = lin(lp + "/attn/to_out", W, W, false);
+      l.ln_ff = norm(lp + "/ff/norm", W);
+      l.fc1 = lin(lp + "/ff/fc1", W, 4 * W, false);
+      l.fc2 = lin(lp + "/ff/fc2", 4 * W, W, false);
+      a->layers.push_back(l);
+    }
+    a->proj_out = lin("image_proj/proj_out", W, ctx_dim, true);
+    a->norm_out = norm("image_proj/norm_out", ctx_dim);
+  }
+  if (L.err) return L.err;
   a->kv.clear();
   // one fused [ip_key | ip_value] per UNet transformer block, in the order of the UNet's tblocks
   const BlockProgram prog = block_program(g.unet);
@@ -1282,6 +1339,14 @@ extern "C" int sdxl_ip_adapter_load(sdxl_ctx* c, const sdxl_ip_adapter_cfg* cfg,
   if (cfg->image_embed_dim < 1) return fail(c, 4802, "IP-Adapter: image_embed_dim = %d must be >= 1", cfg->image_embed_dim);
   if (cfg->tokens_per_image < 1 || cfg->tokens_per_image > 64)
     return fail(c, 4803, "IP-Adapter: tokens_per_image = %d outside [1, 64]", cfg->tokens_per_image);
+  if (cfg->resampler_depth < 0 || cfg->resampler_depth > 64)
+    return fail(c, 4805, "IP-Adapter: resampler_depth = %d outside [0, 64]", cfg->resampler_depth);
+  if (cfg->resampler_depth > 0) {   // Plus: the LayerNorm over the width takes up to 2048 columns; the hidden states are f16 GEMM rows
+    if (cfg->resampler_heads < 1 || cfg->resampler_heads > 32)
+      return fail(c, 4806, "IP-Adapter Plus: resampler_heads = %d outside [1, 32]", cfg->resampler_heads);
+    if (cfg->image_embed_dim % 8)
+      return fail(c, 4807, "IP-Adapter Plus: image_embed_dim = %d must be a multiple of 8", cfg->image_embed_dim);
+  }
   CU(c, cudaSetDevice(c->device));
   std::unique_ptr<sdxl_ip_adapter> a(new sdxl_ip_adapter());
   a->ctx = c;
@@ -1313,9 +1378,81 @@ static int ip_project(const sdxl_ip_adapter* a, int n, const float* e, __half* t
   return 0;
 }
 
+// IP-Adapter Plus: tokens f16 [n * Q, context_dim] = Resampler(h) of hidden states f32 [n, L, D] in device memory (include/sdxl_b200.h).
+// Eager launches on the ctx stream: the GEMMs on igemm (f32 residuals into the latent stream for to_out and fc2), the per-layer
+// LayerNorms in one perceiver_ln launch, the attention of the Q latents over L + Q keys per image on attention_small.
+static int ip_resample(const sdxl_ip_adapter* a, int n, int L, const float* h, __half* tokens) {
+  sdxl_ctx* c = a->ctx;
+  const sdxl_ip_adapter_cfg& g = a->cfg;
+  const int D = g.image_embed_dim, Q = g.tokens_per_image, W = 64 * g.resampler_heads, S = L + Q, ctx_dim = g.unet.context_dim;
+  TmpBufs T(c->stream);
+  __half* h16 = (__half*)T.get((size_t)n * L * D * sizeof(__half));
+  float* x = (float*)T.get((size_t)n * L * W * sizeof(float));          // proj_in(h), read by every layer
+  float* lat = (float*)T.get((size_t)n * Q * W * sizeof(float));        // the latent stream
+  __half* kv_in = (__half*)T.get((size_t)n * S * W * sizeof(__half));   // per image [LN1(x) ; LN2(lat)]
+  __half* a16 = (__half*)T.get((size_t)n * Q * W * sizeof(__half));     // the f16 operand of the next GEMM on the latent rows
+  __half* q16 = (__half*)T.get((size_t)n * Q * W * sizeof(__half));
+  __half* kv16 = (__half*)T.get((size_t)n * S * 2 * W * sizeof(__half));
+  float* f32 = (float*)T.get((size_t)n * Q * std::max(4 * W, ctx_dim) * sizeof(float));   // fc1 output, then proj_out output
+  __half* f16 = (__half*)T.get((size_t)n * Q * 4 * W * sizeof(__half));
+  if (!h16 || !x || !lat || !kv_in || !a16 || !q16 || !kv16 || !f32 || !f16)
+    return fail(c, 4812, "IP-Adapter Plus Resampler: cannot allocate its buffers (n = %d, seq_len = %d)", n, L);
+  // out [M, Lw.N] (row pitch Lw.N) = in [M, Lw.K] (row pitch lda) @ Lw + bias (+ res, f32 output only)
+  auto linear = [&](const __half* in, int M, int lda, const Lin& Lw, void* out, int out_f32, const float* res) {
+    const IgemmOperands o{in, 1, 1, M, Lw.K, lda, nullptr, 0, 0, 0, 0, 0, Lw.w, Lw.N, Lw.Kpad};
+    return igemm_run(c, o, {{0, 0, 0, 0, Lw.Kpad / 64}}, 1, M, 1, IGEMM_LINEAR, 0, out, out_f32, Lw.N, Lw.b, res, Lw.N);
+  };
+  KL(c, cast_f32_to_f16_launch(c->stream, h, (size_t)n * L * D, h16));
+  if (int r = linear(h16, n * L, D, a->proj_in, x, 1, nullptr)) return r;
+  for (int i = 0; i < n; ++i)
+    CU(c, cudaMemcpyAsync(lat + (size_t)i * Q * W, a->latents, (size_t)Q * W * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  for (const PerceiverLayer& l : a->layers) {
+    KL(c, perceiver_ln_launch(c->stream, x, lat, n, L, Q, W, l.ln1.g, l.ln1.b, l.ln2.g, l.ln2.b, l.ln1.eps, kv_in, a16));
+    if (int r = linear(a16, n * Q, W, l.to_q, q16, 0, nullptr)) return r;
+    if (int r = linear(kv_in, n * S, W, l.to_kv, kv16, 0, nullptr)) return r;
+    KL(c, attention_small_launch(c->stream, q16, W, 0, kv16, kv16, 2 * W, 0, W, n, Q, S, g.resampler_heads, nullptr, 0, a16, W, 64));
+    if (int r = linear(a16, n * Q, W, l.to_out, lat, 1, lat)) return r;
+    KL(c, layernorm_launch(c->stream, lat, l.ln_ff.g, l.ln_ff.b, l.ln_ff.eps, n * Q, W, a16));
+    if (int r = linear(a16, n * Q, W, l.fc1, f32, 1, nullptr)) return r;
+    KL(c, mlp_act_launch(c->stream, f32, (size_t)n * Q * 4 * W, 0, f16));
+    if (int r = linear(f16, n * Q, 4 * W, l.fc2, lat, 1, lat)) return r;
+  }
+  KL(c, cast_f32_to_f16_launch(c->stream, lat, (size_t)n * Q * W, a16));
+  if (int r = linear(a16, n * Q, W, a->proj_out, f32, 1, nullptr)) return r;
+  KL(c, layernorm_launch(c->stream, f32, a->norm_out.g, a->norm_out.b, a->norm_out.eps, n * Q, ctx_dim, tokens));
+  return 0;
+}
+
+extern "C" int sdxl_ip_adapter_resample(sdxl_ip_adapter* a, int n, int seq_len, const float* hidden, int on_host, sdxl_half* tokens_out) {
+  if (!a || !hidden || !tokens_out) return fail(a ? a->ctx : nullptr, -1, "sdxl_ip_adapter_resample: null argument");
+  sdxl_ctx* c = a->ctx;
+  if (!a->plus()) return fail(c, 4813, "ip_adapter_resample: the adapter is a base IP-Adapter (use sdxl_ip_adapter_project)");
+  if (n < 1 || seq_len < 1 || seq_len > 4096) return fail(c, 4814, "ip_adapter_resample: n = %d must be >= 1 and seq_len = %d in [1, 4096]", n, seq_len);
+  CU(c, cudaSetDevice(c->device));
+  TmpBufs T(c->stream);
+  const size_t in_bytes = (size_t)n * seq_len * a->cfg.image_embed_dim * sizeof(float);
+  const size_t out_bytes = (size_t)n * a->cfg.tokens_per_image * a->cfg.unet.context_dim * sizeof(__half);
+  const float* e = hidden;
+  __half* o = (__half*)tokens_out;
+  if (on_host) {
+    float* d = (float*)T.get(in_bytes);
+    o = (__half*)T.get(out_bytes);
+    if (!d || !o) return fail(c, 4811, "ip_adapter_resample: allocation failed");
+    CU(c, cudaMemcpyAsync(d, hidden, in_bytes, cudaMemcpyHostToDevice, c->stream));
+    e = d;
+  }
+  if (int r = ip_resample(a, n, seq_len, e, o)) return r;
+  if (on_host) {
+    CU(c, cudaMemcpyAsync(tokens_out, o, out_bytes, cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+  }
+  return 0;
+}
+
 extern "C" int sdxl_ip_adapter_project(sdxl_ip_adapter* a, int n, const float* embeds, int on_host, sdxl_half* tokens_out) {
   if (!a || !embeds || !tokens_out || n < 1) return -1;
   sdxl_ctx* c = a->ctx;
+  if (a->plus()) return fail(c, 4813, "ip_adapter_project: the adapter is an IP-Adapter Plus (use sdxl_ip_adapter_resample)");
   CU(c, cudaSetDevice(c->device));
   TmpBufs T(c->stream);
   const size_t in_bytes = (size_t)n * a->cfg.image_embed_dim * sizeof(float);
@@ -1342,7 +1479,8 @@ extern "C" int sdxl_ip_adapter_project(sdxl_ip_adapter* a, int n, const float* e
 static int ip_write(sdxl_ctx* c, IpAttach& a, const sdxl_image_prompt& p) {
   const int n = p.n_batch * p.n_images, n_tb = (int)a.ad->kv.size();
   const size_t tok_bytes = (size_t)a.n_batch * a.S_ip * a.ad->cfg.unet.context_dim * sizeof(__half);
-  const size_t bytes = (size_t)n * a.ad->cfg.image_embed_dim * sizeof(float);
+  const int rows = a.ad->plus() ? p.seq_len : 1;   // input rows per image: Plus hidden states, or one embedding
+  const size_t bytes = (size_t)n * rows * a.ad->cfg.image_embed_dim * sizeof(float);
   TmpBufs T(c->stream);
   const float* e = p.embeds;
   const float* neg = p.negative_embeds;
@@ -1361,8 +1499,13 @@ static int ip_write(sdxl_ctx* c, IpAttach& a, const sdxl_image_prompt& p) {
   __half* tn = (__half*)T.get(tok_bytes);
   float* ts = (float*)T.get(n_tb * sizeof(float));
   if (!tp || !tn || !ts) return fail(c, 4820, "set_image_prompt: cannot allocate the token staging buffers");
-  if (int r = ip_project(a.ad, n, e, tp)) return r;
-  if (int r = ip_project(a.ad, n, neg, tn)) return r;
+  if (a.ad->plus()) {
+    if (int r = ip_resample(a.ad, n, p.seq_len, e, tp)) return r;
+    if (int r = ip_resample(a.ad, n, p.seq_len, neg, tn)) return r;
+  } else {
+    if (int r = ip_project(a.ad, n, e, tp)) return r;
+    if (int r = ip_project(a.ad, n, neg, tn)) return r;
+  }
   std::vector<float> s(n_tb, p.scale);
   if (p.block_scales_host) s.assign(p.block_scales_host, p.block_scales_host + n_tb);
   CU(c, cudaMemcpyAsync(ts, s.data(), s.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
@@ -1394,6 +1537,12 @@ extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt*
   // equal cfgs: the adapter's K/V were laid out by the same block program as the UNet's transformer blocks
   const int n_tb = (int)ad->kv.size();
   if (!p->embeds) return fail(c, 4835, "set_image_prompt: null embeds");
+  if (ad->plus()) {
+    if (!p->negative_embeds)
+      return fail(c, 4839, "set_image_prompt: an IP-Adapter Plus prompt needs negative_embeds (the hidden states of an all-zero "
+                           "pixel tensor; the library cannot compute them)");
+    if (p->seq_len < 1 || p->seq_len > 4096) return fail(c, 4840, "set_image_prompt: seq_len = %d outside [1, 4096]", p->seq_len);
+  }
   if (p->n_batch < 1 || p->n_images < 1 || p->n_images > 64)
     return fail(c, 4836, "set_image_prompt: n_batch = %d must be >= 1 and n_images = %d in [1, 64]", p->n_batch, p->n_images);
   if (!isfinite(p->scale)) return fail(c, 4837, "set_image_prompt: scale is not finite");

@@ -260,6 +260,10 @@ int mlp_act_launch(cudaStream_t st, const float* x, size_t n, int quick, __half*
 // y[b,:] = LayerNorm(x[b*T + idx[b], :]) in f32.
 int ln_gather_f32_launch(cudaStream_t st, const float* x, const int* idx, int B, int T, int C, const float* gamma,
                          const float* beta, float eps, float* y);
+// The LayerNorms of one IP-Adapter Plus perceiver-attention layer: x f32 [n*L, C] (LN1: g1, b1) and lat f32 [n*Q, C] (LN2: g2, b2)
+// -> kv f16 [n, L+Q, C] (per image: the L rows of LN1(x), then the Q rows of LN2(lat)) and q f16 [n*Q, C] (the LN2 rows again).
+int perceiver_ln_launch(cudaStream_t st, const float* x, const float* lat, int n, int L, int Q, int C, const float* g1,
+                        const float* b1, const float* g2, const float* b2, float eps, __half* kv, __half* q);
 
 // Weight re-layout at load time (elementwise.cu)
 // Linear [K(in), N(out)] row-major f16 -> K-major [N, Kpad] f16 (zero padded), dst row pitch Kpad;

@@ -59,6 +59,12 @@ SDXL_TEST_API int sdxl_test_attention_small(void* stream, const void* q, int q_p
                                 k_col0, v_col0, B, T, S, n_head, (const __half*)mask, causal, (__half*)out, ldo, head_dim);
 }
 
+// The IP-Adapter Plus Resampler's per-layer LayerNorms (engine.cu: ip_resample).
+SDXL_TEST_API int sdxl_test_perceiver_ln(void* stream, const float* x, const float* lat, int n, int L, int Q, int C, const float* g1,
+                                         const float* b1, const float* g2, const float* b2, float eps, void* kv, void* q) {
+  return perceiver_ln_launch((cudaStream_t)stream, x, lat, n, L, Q, C, g1, b1, g2, b2, eps, (__half*)kv, (__half*)q);
+}
+
 SDXL_TEST_API size_t sdxl_test_gn_scratch_floats(int B, int n_group) { return gn_scratch_floats(B, n_group); }
 SDXL_TEST_API int sdxl_test_gn_scratch_init(void* stream, float* scratch, int B, int n_group) {
   return gn_scratch_init((cudaStream_t)stream, scratch, B, n_group);

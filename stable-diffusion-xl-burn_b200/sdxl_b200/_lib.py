@@ -81,12 +81,14 @@ class ClipVisionCfg(C.Structure):
 
 
 class IpAdapterCfg(C.Structure):
-    _fields_ = [("unet", UnetCfg), ("image_embed_dim", C.c_int32), ("tokens_per_image", C.c_int32)]
+    _fields_ = [("unet", UnetCfg), ("image_embed_dim", C.c_int32), ("tokens_per_image", C.c_int32), ("resampler_depth", C.c_int32),
+                ("resampler_heads", C.c_int32)]
 
 
 class ImagePrompt(C.Structure):
     _fields_ = [("adapter", C.c_void_p), ("embeds", C.c_void_p), ("negative_embeds", C.c_void_p), ("on_host", C.c_int32),
-                ("n_batch", C.c_int32), ("n_images", C.c_int32), ("scale", C.c_float), ("block_scales_host", C.c_void_p)]
+                ("n_batch", C.c_int32), ("n_images", C.c_int32), ("scale", C.c_float), ("block_scales_host", C.c_void_p),
+                ("seq_len", C.c_int32)]
 
 
 # name -> (restype, argtypes); every symbol include/sdxl_b200.h declares
@@ -155,11 +157,13 @@ PROTOTYPES = {
     "sdxl_clip_vision_load": (I, [P, C.POINTER(ClipVisionCfg), P, C.c_size_t, I, C.POINTER(P)]),
     "sdxl_clip_vision_destroy": (None, [P]),
     "sdxl_clip_vision_encode": (I, [P, I, P, I, P]),
+    "sdxl_clip_vision_encode_hidden": (I, [P, I, P, I, I, P]),
     "sdxl_unet_plan_builds": (C.c_uint64, [P]),
     "sdxl_ip_adapter_load": (I, [P, C.POINTER(IpAdapterCfg), P, C.c_size_t, I, C.POINTER(P)]),
     "sdxl_ip_adapter_destroy": (None, [P]),
     "sdxl_unet_set_image_prompt": (I, [P, C.POINTER(ImagePrompt)]),
     "sdxl_ip_adapter_project": (I, [P, I, P, I, P]),
+    "sdxl_ip_adapter_resample": (I, [P, I, I, P, I, P]),
     "sdxl_op_ip_attention": (I, [P, P, P, P, P, P, I, I, I, I, I, I, C.c_float, P]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),

@@ -21,6 +21,7 @@ PROTOTYPES = {
     "sdxl_test_igemm": (I, [P, P, I, I, I, I, I, P, I, I, I, I, I, P, I, I, I, I, I, I, I, P, I, P, I, I, P, I, P, I, I, I, I]),
     "sdxl_test_attention": (I, [P, P, I, I, P, I, I, I, I, I, I, I, P, I, P, I, I, I, I, P]),
     "sdxl_test_attention_small": (I, [P, P, I, I, P, P, I, I, I, I, I, I, I, P, I, P, I, I]),
+    "sdxl_test_perceiver_ln": (I, [P, P, P, I, I, I, I, P, P, P, P, F, P, P]),
     "sdxl_test_gn_scratch_floats": (C.c_size_t, [I, I]),
     "sdxl_test_gn_scratch_init": (I, [P, P, I, I]),
     "sdxl_test_gn": (I, [P, P, I, P, I, I, I, I, P, P, F, I, P, P, P, P]),
@@ -88,6 +89,11 @@ def attention_small(q, q_pitch, q_col0, k, v, kv_pitch, k_col0, v_col0, B, T, S,
                     head_dim) -> None:
     _call("sdxl_test_attention_small", _p(q), q_pitch, q_col0, _p(k), _p(v), kv_pitch, k_col0, v_col0, B, T, S, n_head,
           _p(mask), int(causal), _p(out), ldo, head_dim)
+
+
+def perceiver_ln(x, lat, n, L, Q, C, g1, b1, g2, b2, eps, kv, q) -> None:
+    """x f32 [n*L, C], lat f32 [n*Q, C] -> kv f16 [n, L+Q, C] and q f16 [n*Q, C]."""
+    _call("sdxl_test_perceiver_ln", _p(x), _p(lat), n, L, Q, C, _p(g1), _p(b1), _p(g2), _p(b2), eps, _p(kv), _p(q))
 
 
 def gn_scratch(B: int, n_group: int) -> torch.Tensor:

@@ -5,7 +5,7 @@ from __future__ import annotations
 import ctypes as C
 import json
 from dataclasses import dataclass
-from typing import Dict, Tuple, Union
+from typing import Dict, Optional, Tuple, Union
 
 import torch
 import torch.nn.functional as F
@@ -201,6 +201,27 @@ class ClipVisionEncoder:
     def encode_images(self, rgb: torch.Tensor) -> torch.Tensor:
         """image_embeds of u8 images [N, H, W, 3]."""
         return self.encode(clip_preprocess(rgb, self.cfg.image_size))
+
+    def encode_hidden(self, pixels: torch.Tensor, hidden_idx: Optional[int] = None) -> torch.Tensor:
+        """HF hidden_states[hidden_idx] f32 [N, T, n_state] of preprocessed pixels f32 [N, 3, S, S]; hidden_idx in [0, n_layer],
+        default n_layer - 1 (hidden_states[-2], the image features of IP-Adapter Plus)."""
+        ctx, g = self.ctx, self.cfg
+        idx = g.n_layer - 1 if hidden_idx is None else int(hidden_idx)
+        if pixels.dim() != 4 or tuple(pixels.shape[1:]) != (3, g.image_size, g.image_size):
+            raise SdxlError(f"encode_hidden: pixels must be [N, 3, {g.image_size}, {g.image_size}], got {tuple(pixels.shape)}")
+        if not 0 <= idx <= g.n_layer:
+            raise SdxlError(f"encode_hidden: hidden_idx {idx} outside [0, {g.n_layer}]")
+        px = pixels.to(ctx.device, torch.float32).contiguous()
+        out = torch.empty(px.shape[0], g.n_tokens, g.n_state, device=ctx.device, dtype=torch.float32)
+        ctx.enter()
+        ctx.check(ctx.lib.sdxl_clip_vision_encode_hidden(self.h, px.shape[0], px.data_ptr(), 0, idx, out.data_ptr()),
+                  "sdxl_clip_vision_encode_hidden")
+        ctx.leave()
+        return out
+
+    def encode_images_hidden(self, rgb: torch.Tensor) -> torch.Tensor:
+        """hidden_states[-2] of u8 images [N, H, W, 3]."""
+        return self.encode_hidden(clip_preprocess(rgb, self.cfg.image_size))
 
     def close(self) -> None:
         if getattr(self, "h", None):

@@ -307,7 +307,8 @@ class Diffuser:
     def set_image_prompt(self, adapter, embeds=None, scale=1.0, negative=None) -> None:
         """Attaches an IP-Adapter image prompt (sdxl_unet_set_image_prompt); adapter None detaches. embeds: f32 [n_batch, D] or
         [n_batch, n_images, D] (CLIP vision image_embeds); image b of a batch uses prompt b % n_batch. scale: float, or one per
-        transformer block in execution order (ip_adapter.transformer_block_paths). negative: the CFG rows' embeddings (zeros)."""
+        transformer block in execution order (ip_adapter.transformer_block_paths). negative: the CFG rows' embeddings (zeros).
+        IP-Adapter Plus: embeds and negative (required) are vision hidden states [n_batch, n_images, L, D] (IPAdapter.image_embeds)."""
         from .ip_adapter import set_image_prompt
         set_image_prompt(self, adapter, embeds, scale, negative)
 

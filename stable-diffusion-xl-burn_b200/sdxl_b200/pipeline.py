@@ -35,11 +35,12 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     text encoders for this call (the refiner is left alone) and removed again afterwards, which also clears any adapter set
     those models had. controls: [(ControlNet, image u8 [1, H, W, 3] or f32 [1, 3, H, W], scale), ...] attached to the base UNet
     for this call and detached afterwards (the refiner is left alone). image_prompt: (IPAdapter, ClipVisionEncoder, images u8
-    [n_images, H, W, 3], scale): the images are encoded and attached to the base UNet as one prompt of n_images images for this call
-    and detached afterwards. Returns uint8 [1, H, W, 3]."""
+    [n_images, H, W, 3], scale): the images are encoded (IPAdapter.image_embeds: image_embeds for the base adapter, hidden states for
+    IP-Adapter Plus) and attached to the base UNet as one prompt of n_images images for this call and detached afterwards. Returns uint8 [1, H, W, 3]."""
     if image_prompt:
         adapter, encoder, images, scale = image_prompt
-        diffuser.set_image_prompt(adapter, encoder.encode_images(images).unsqueeze(0), scale)
+        e, neg = adapter.image_embeds(encoder, images)
+        diffuser.set_image_prompt(adapter, e.unsqueeze(0), scale, negative=neg.unsqueeze(0))
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
                           seed, noise, loras, controls)
