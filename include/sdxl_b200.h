@@ -162,7 +162,8 @@ SDXL_API uint64_t sdxl_unet_plan_builds(const sdxl_unet* unet);
 SDXL_API double sdxl_unet_plan_flops_executed(const sdxl_unet* unet);
 /* Device time of ONE execution of the current launch plan, summed per kernel kind and measured with CUDA
  * events on the ctx stream (eager launches). Kind index: 0 implicit-GEMM (wgmma), 1 attention, 2 GroupNorm,
- * 3 LayerNorm, 4 GEMV, 5 timestep-embedding, 6 first conv, 7 upsample copy, 8 phase-split copy, 9 f32->f16 cast.
+ * 3 LayerNorm, 4 GEMV, 5 timestep-embedding, 6 first conv, 7 upsample copy, 8 phase-split copy, 9 f32->f16 cast,
+ * 17 T2I-Adapter feature add.
  * All three arrays hold SDXL_PROFILE_KINDS entries (host). Used by bench.py for the per-kernel roofline. */
 SDXL_API int sdxl_unet_profile_plan(sdxl_unet* unet, double* ms_by_kind_host, double* flops_by_kind_host,
                                     int* launches_by_kind_host);
@@ -469,6 +470,52 @@ SDXL_API int sdxl_ip_adapter_resample(sdxl_ip_adapter* adapter, int n, int seq_l
  * k_ip/v_ip [B,S_ip,C] f16 device memory. */
 SDXL_API int sdxl_op_ip_attention(sdxl_ctx* ctx, const sdxl_half* q, const sdxl_half* k, const sdxl_half* v, const sdxl_half* k_ip,
                                   const sdxl_half* v_ip, int B, int T, int S, int S_ip, int C, int n_head, float scale, sdxl_half* out);
+
+/* ---- T2I-Adapter --------------------------------------------------------------------------------------
+ * Spatial conditioning that runs once per image (DESIGN.md §11): diffusers T2IAdapter with adapter_type "full_adapter_xl"
+ * (TencentARC t2i-adapter-*-sdxl-1.0). For a hint c f32 NCHW [n, in_channels, H, W] in [0, 1] (H, W multiples of 32) and the widths
+ * ch = (mc*m0, mc*m1, mc*m2, mc*m2) of the UNet cfg:
+ *   x = conv_in(pixel_unshuffle(c, 16))                              3x3 pad 1, in_channels*256 -> ch0
+ *   level k = 0..3: x = avg_pool2(x) if k == 2;  x = in_conv_k(x) if k in (1, 2) (1x1);
+ *                   n_res_blocks times x = x + block2(relu(block1(x))) (block1 3x3 pad 1, block2 1x1);  F_k = x
+ * F_0, F_1 are [n, ch, H/16, W/16], F_2, F_3 [n, ch, H/32, W/32]. Pack (SDXLPK01), conv weights OIHW f16, biases f16:
+ *   conv_in/{weight,bias}, body/{1,2}/in_conv/{weight,bias}, body/{k}/resnets/{j}/block{1,2}/{weight,bias}.
+ * Only SDXL-base-shaped UNet cfgs qualify: not the refiner, n_levels = 3, no transformer on level 0, and three distinct widths.
+ * An adapter is built on one ctx and may be attached to any UNet of that ctx whose cfg equals its `unet`. */
+typedef struct sdxl_t2i_adapter sdxl_t2i_adapter;
+typedef struct sdxl_t2i_adapter_cfg {
+  sdxl_unet_cfg unet;            /* must equal the cfg of the UNet it is attached to */
+  int32_t in_channels;           /* hint channels: 3 (1 allowed) */
+  int32_t n_res_blocks;          /* 2 */
+} sdxl_t2i_adapter_cfg;
+SDXL_API int sdxl_t2i_adapter_load(sdxl_ctx* ctx, const sdxl_t2i_adapter_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
+                                   sdxl_t2i_adapter** out);
+/* The UNet keeps only the features computed at attach time, so an attached adapter may be destroyed. */
+SDXL_API void sdxl_t2i_adapter_destroy(sdxl_t2i_adapter* adapter);
+#define SDXL_MAX_T2I_ADAPTERS 4
+typedef struct sdxl_t2i_control {
+  const sdxl_t2i_adapter* adapter;
+  const float* hint;        /* f32 NCHW [n_hint, in_channels, height, width] in [0, 1]; host if hint_on_host; borrowed for the call */
+  int32_t hint_on_host;
+  int32_t n_hint;           /* UNet row b uses feature set b % n_hint (CFG rows [cond | uncond] share the image's) */
+  int32_t height, width;    /* pixels, multiples of 32; the latent must be height/8 x width/8 */
+  float scale;              /* s_a */
+} sdxl_t2i_control;
+/* Replaces the UNet's attached T2I-Adapter set (n = 0 detaches). The features F_k = sum_a s_a * F_{a,k} (f32, adapters in array order,
+ * diffusers MultiAdapter with adapter_weights) are computed during the call and added in place, in the UNet's own encoder, to the
+ * output of the last input block of each level (for a level without transformers that is its Downsample: input_blocks/3, 5, 8 for
+ * SDXL base) and to the middle block's output, before any ControlNet residual; the skip saved for a block carries the feature too
+ * (diffusers down_intrablock_additional_residuals). A ControlNet's encoder does not see them. They are added only at forwards whose
+ * timestep t >= t_min (diffusers adapter_conditioning_factor; 0: always), read on the device, so the sampler and the CUDA graph honour
+ * it. Everything is validated before anything changes (ctx, cfg, n <= SDXL_MAX_T2I_ADAPTERS, n_hint >= 1, equal n_hint, height and
+ * width across items, sizes multiples of 32, finite scales): on failure the previous set stays attached. A call with the same n_hint
+ * and size as the attached set rewrites the features and t_min in place (same launch plan and CUDA graph); any other change rebuilds
+ * the plan at the next forward. A forward or sampler_begin whose latent is not height/8 x width/8, or whose batch is not a multiple
+ * of n_hint, fails. */
+SDXL_API int sdxl_unet_set_t2i_adapters(sdxl_unet* unet, int n, const sdxl_t2i_control* controls, int32_t t_min);
+/* Test aid: the four F_k of one adapter at scale 1, f32 NCHW, concatenated in k order, of hint f32 NCHW [n, in_channels, H, W]; both
+ * pointers are host memory if on_host. */
+SDXL_API int sdxl_t2i_adapter_features(sdxl_t2i_adapter* adapter, int n, int H, int W, const float* hint, int on_host, float* out);
 
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),

@@ -145,6 +145,7 @@ struct Plan;
 struct Sampler;
 struct ControlAttach;
 struct IpAttach;
+struct T2IAttach;
 
 // Embeddings, first conv, input blocks and middle block: the part of the UNet a ControlNet copies.
 struct EncoderHalf {
@@ -200,6 +201,7 @@ struct sdxl_unet : EncoderHalf {
   AdapterState lora;           // LoRA-able weight slots, backups of merged layers (sdxl_unet_set_adapters)
   std::vector<std::unique_ptr<ControlAttach>> controls;   // sdxl_unet_set_controls, in call order
   std::unique_ptr<IpAttach> ip;   // sdxl_unet_set_image_prompt
+  std::unique_ptr<T2IAttach> t2i; // sdxl_unet_set_t2i_adapters
   uint64_t plan_builds = 0;
   int cfg_rows = 0;               // conditioning rows are the sampler's [cond | uncond] with cfg_rows cond rows (0: plain batch)
   ~sdxl_unet() {
@@ -262,6 +264,29 @@ struct IpAttach {
   __half* tok_neg = nullptr;   // [n_batch, S_ip, context_dim]
   float* scales = nullptr;     // one per transformer block, read by the attention kernel
   IpRows cond;
+};
+
+// T2I-Adapter (DESIGN.md §11, diffusers FullAdapterXL): conv_in on the pixel-unshuffled hint, then per level k an optional 1x1 in_conv
+// (k = 1, 2) and n_res_blocks resnets x + block2(relu(block1(x))).
+struct T2IRes { Conv block1, block2; };
+struct sdxl_t2i_adapter {
+  sdxl_ctx* ctx = nullptr;
+  sdxl_t2i_adapter_cfg cfg{};
+  int ch[4] = {0, 0, 0, 0};   // (mc*m0, mc*m1, mc*m2, mc*m2)
+  Arena warena;
+  Conv conv_in;
+  Conv in_conv[2];            // body/1/in_conv, body/2/in_conv
+  std::vector<T2IRes> res[4];
+};
+
+// The attached T2I-Adapter set: the scaled sum of the features F_k, f32 NHWC [n_hint, Hk, Wk, Ck], and the timestep window.
+struct T2IAttach {
+  int n_hint = 0, h = 0, w = 0;     // latent extent
+  int C[4] = {}, H[4] = {}, W[4] = {};
+  size_t points[3] = {};            // input blocks (indices into the block program) after which F_0..F_2 are added; F_3 after the middle
+  Arena mem;
+  float* F[4] = {};
+  int* t_min = nullptr;             // device: features are added when t >= *t_min
 };
 
 
@@ -705,6 +730,8 @@ struct UNetPlanBuilder : PlanBuilder {
       P->flops += 2.0 * Bf * H * W * 9.0 * g.in_channels * mc;
     }
     saved.push_back({x, Cx, H, W});
+    // an attached T2I-Adapter adds its features in the UNet's own encoder (a ControlNet's does not see them)
+    const bool t2i = u->t2i && cond == &u->cond;
     for (size_t i = 1; i < e.in_blocks.size() && !err; ++i) {
       const Block& b = e.in_blocks[i];
       begin_block(prefix + "input_blocks/" + std::to_string(i));
@@ -726,6 +753,9 @@ struct UNetPlanBuilder : PlanBuilder {
         add_flops(2.0 * Bf * H2 * W2 * 9.0 * Cx * b.conv.O);
         x = y; H = H2; W = W2;
       }
+      if (t2i)
+        for (int k = 0; k < 3; ++k)
+          if (u->t2i->points[k] == i) t2i_add(x, k, Cx, H, W);
       end_block();
       saved.push_back({x, Cx, H, W});
     }
@@ -734,8 +764,20 @@ struct UNetPlanBuilder : PlanBuilder {
     x = resblock(e.mid_res1, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s.gn1, s.raw, s.h, s.gn2);
     x = strans(e.mid_st, x, H, W, s.a16, s.tok, s.qkv, s.ao, s.q, s.ff);
     x = resblock(e.mid_res2, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s.gn1, s.raw, s.h, s.gn2);
+    if (t2i) t2i_add(x, 3, Cx, H, W);
     end_block();
     return x;
+  }
+
+  // T2I-Adapter injection: x += F_k in place, so the skip saved for the block carries the feature too
+  void t2i_add(float* x, int k, int C, int H, int W) {
+    if (err) return;
+    const T2IAttach& a = *u->t2i;
+    if (a.C[k] != C || a.H[k] != H || a.W[k] != W) { err = fail(c, 5017, "T2I-Adapter feature %d shape mismatch", k); return; }
+    Op op{};
+    op.kind = OP_T2I_ADD;
+    op.ta = {x, a.F[k], (long)H * W * C, Bf, a.n_hint, u->t_dev, a.t_min};
+    P->ops.push_back(op);
   }
 
   // ControlNet injection: dst += conv1x1(src) with the scaled zero conv L (f16 operand of src in `a16`, residual add in place)
@@ -985,6 +1027,12 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
     if (Bf % a.n_hint) return fail(c, 5013, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bf, a.n_hint);
   }
   if (u->ip && u->ip->cond.condB != Bf) return fail(c, 5014, "image prompt: its K/V are hoisted for batch %d but the batch is %d", u->ip->cond.condB, Bf);
+  if (u->t2i) {
+    const T2IAttach& a = *u->t2i;
+    if (a.h != h || a.w != w)
+      return fail(c, 5015, "T2I-Adapter: its hint is %dx%d pixels (latent %dx%d) but the latent is %dx%d", 8 * a.h, 8 * a.w, a.h, a.w, h, w);
+    if (Bf % a.n_hint) return fail(c, 5016, "T2I-Adapter: batch %d is not a multiple of n_hint = %d", Bf, a.n_hint);
+  }
   // every change of the buffers or attachments a plan reads drops the plan, so the shapes are its whole cache key
   if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w) return 0;
   if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A); })) return r;
@@ -1581,6 +1629,269 @@ extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt*
 }
 
 // ================================================================================================
+// T2I-Adapter (include/sdxl_b200.h: sdxl_t2i_adapter_load, sdxl_unet_set_t2i_adapters; DESIGN.md §11)
+// ================================================================================================
+// Why a UNet cfg cannot take a T2I-Adapter, or null: FullAdapterXL's four features fit SDXL base's encoder only.
+static const char* t2i_unet_problem(const sdxl_unet_cfg& g) {
+  if (g.is_refiner) return "the refiner is not supported";
+  if (g.n_levels != 3) return "the UNet must have 3 levels";
+  if (g.transformer_depths[0] != 0) return "the UNet must have no transformer on level 0";
+  if (g.channel_mults[0] == g.channel_mults[1] || g.channel_mults[1] == g.channel_mults[2])
+    return "the widths of levels 0, 1 and 2 must differ (every in_conv of the adapter is present)";
+  return nullptr;
+}
+
+// The input blocks after which F_0, F_1, F_2 are added: per level its last block with a transformer or, on a level without one,
+// its last block (the Downsample where it has one) -- where diffusers' CrossAttnDownBlock2D and DownBlock2D add them.
+static void t2i_points(const BlockProgram& p, size_t out[3]) {
+  for (int level = 0; level < 3; ++level) {
+    size_t last = 0, last_tr = 0;
+    for (size_t i = 1; i < p.ins.size(); ++i)
+      if (p.ins[i].level == level) {
+        last = i;
+        if (has_transformer(p.ins[i].type)) last_tr = i;
+      }
+    out[level] = last_tr ? last_tr : last;
+  }
+}
+
+static int build_t2i_adapter(sdxl_t2i_adapter* a, const PackView& pv, Arena& A) {
+  const int* ch = a->ch;
+  Loader L{a->ctx, &pv, &A, a->ctx->stream};
+  std::set<std::string> names;
+  auto conv = [&](const std::string& path, int I, int O, int ks) {
+    names.insert(path + "/weight");
+    names.insert(path + "/bias");
+    return L.conv(path, I, O, ks);
+  };
+  a->conv_in = conv("conv_in", a->cfg.in_channels * 256, ch[0], 3);
+  for (int k = 1; k < 3; ++k) a->in_conv[k - 1] = conv("body/" + std::to_string(k) + "/in_conv", ch[k - 1], ch[k], 1);
+  for (int k = 0; k < 4 && !L.err; ++k) {
+    a->res[k].clear();
+    for (int j = 0; j < a->cfg.n_res_blocks; ++j) {
+      const std::string p = "body/" + std::to_string(k) + "/resnets/" + std::to_string(j);
+      T2IRes r;
+      r.block1 = conv(p + "/block1", ch[k], ch[k], 3);
+      r.block2 = conv(p + "/block2", ch[k], ch[k], 1);
+      a->res[k].push_back(r);
+    }
+  }
+  if (L.err) return L.err;
+  for (const auto& t : pv.t)
+    if (!names.count(t.first)) return fail(a->ctx, 4904, "T2I-Adapter pack: tensor '%s' is not part of an adapter for this cfg", t.first.c_str());
+  return 0;
+}
+
+extern "C" int sdxl_t2i_adapter_load(sdxl_ctx* c, const sdxl_t2i_adapter_cfg* cfg, const void* pack, size_t bytes, int pack_on_device,
+                                     sdxl_t2i_adapter** out) {
+  if (!c || !cfg || !pack || !out) return fail(c, -1, "sdxl_t2i_adapter_load: null argument");
+  *out = nullptr;
+  if (int r = check_unet_cfg(c, cfg->unet)) return r;
+  if (const char* why = t2i_unet_problem(cfg->unet)) return fail(c, 4900, "T2I-Adapter: %s", why);
+  if (cfg->in_channels < 1 || cfg->in_channels > 4) return fail(c, 4901, "T2I-Adapter: in_channels = %d outside [1, 4]", cfg->in_channels);
+  if (cfg->n_res_blocks < 1 || cfg->n_res_blocks > 8) return fail(c, 4902, "T2I-Adapter: n_res_blocks = %d outside [1, 8]", cfg->n_res_blocks);
+  CU(c, cudaSetDevice(c->device));
+  std::unique_ptr<sdxl_t2i_adapter> a(new sdxl_t2i_adapter());
+  a->ctx = c;
+  a->cfg = *cfg;
+  const sdxl_unet_cfg& g = cfg->unet;
+  for (int k = 0; k < 4; ++k) a->ch[k] = g.model_channels * g.channel_mults[k < 3 ? k : 2];
+  int r = with_device_pack(c, pack, bytes, pack_on_device,
+                           [&](const PackView& pv) { return build_two_pass(a.get(), pv, build_t2i_adapter); });
+  if (r) return r;
+  *out = a.release();
+  return 0;
+}
+
+extern "C" void sdxl_t2i_adapter_destroy(sdxl_t2i_adapter* a) {
+  if (!a) return;
+  cudaStreamSynchronize(a->ctx->stream);
+  delete a;
+}
+
+// ks x ks pad ks/2 conv of an f16 NHWC image [Bn, H, W, cv.I] on the implicit GEMM: out f32 NHWC = conv + bias (+ res, may be out).
+static int conv_nhwc(sdxl_ctx* c, const __half* a, int Bn, int H, int W, const Conv& cv, float* out, const float* res) {
+  const IgemmOperands o{a, Bn, H, W, cv.I, cv.I, nullptr, 0, 0, 0, 0, 0, cv.w, cv.O, cv.Ktot};
+  return igemm_run(c, o, conv_taps(cv.ks, cv.Ipad / 64), H, W, Bn, IGEMM_LINEAR, 0, out, 1, cv.O, cv.b, res, cv.O);
+}
+
+// Elements of F_k for n hints of H x W pixels.
+static size_t t2i_feature_elems(const sdxl_t2i_adapter* a, int k, int n, int H, int W) {
+  const int d = k < 2 ? 16 : 32;
+  return (size_t)n * (H / d) * (W / d) * a->ch[k];
+}
+
+// Adapter forward of hint f32 NCHW [n, in_channels, H, W] (device) into F[k] f32 NHWC at scale 1. Eager on the ctx stream.
+static int t2i_forward(const sdxl_t2i_adapter* a, int n, int H, int W, const float* hint, float* const F[4]) {
+  sdxl_ctx* c = a->ctx;
+  const int h2 = H / 16, w2 = W / 16, h4 = H / 32, w4 = W / 32;
+  size_t max16 = (size_t)n * h2 * w2 * a->cfg.in_channels * 256, max32 = 0;
+  for (int k = 0; k < 4; ++k) {
+    max16 = std::max(max16, t2i_feature_elems(a, k, n, H, W));
+    max32 = std::max(max32, t2i_feature_elems(a, k, n, H, W));
+  }
+  TmpBufs T(c->stream);
+  __half* a16 = (__half*)T.get(max16 * sizeof(__half));   // the f16 operand of the next conv
+  float* t32 = (float*)T.get(max32 * sizeof(float));      // block1 output
+  __half* t16 = (__half*)T.get(max32 * sizeof(__half));   // relu(block1)
+  if (!a16 || !t32 || !t16) return fail(c, 4910, "T2I-Adapter: cannot allocate its scratch (n = %d, %dx%d)", n, H, W);
+  KL(c, pixel_unshuffle_launch(c->stream, hint, n, a->cfg.in_channels, H, W, a16));
+  if (int r = conv_nhwc(c, a16, n, h2, w2, a->conv_in, F[0], nullptr)) return r;
+  for (int k = 0; k < 4; ++k) {
+    const int hk = k < 2 ? h2 : h4, wk = k < 2 ? w2 : w4;
+    const size_t e = t2i_feature_elems(a, k, n, H, W);
+    if (k == 1) {
+      KL(c, cast_f32_to_f16_launch(c->stream, F[0], t2i_feature_elems(a, 0, n, H, W), a16));
+      if (int r = conv_nhwc(c, a16, n, hk, wk, a->in_conv[0], F[1], nullptr)) return r;
+    } else if (k == 2) {
+      KL(c, avg_pool2_f16_launch(c->stream, F[1], n, h2, w2, a->ch[1], a16));
+      if (int r = conv_nhwc(c, a16, n, hk, wk, a->in_conv[1], F[2], nullptr)) return r;
+    } else if (k == 3) {
+      CU(c, cudaMemcpyAsync(F[3], F[2], e * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+    }
+    for (const T2IRes& rb : a->res[k]) {   // x = x + block2(relu(block1(x))), the residual added in block2's epilogue
+      KL(c, cast_f32_to_f16_launch(c->stream, F[k], e, a16));
+      if (int r = conv_nhwc(c, a16, n, hk, wk, rb.block1, t32, nullptr)) return r;
+      KL(c, relu_f16_launch(c->stream, t32, e, t16));
+      if (int r = conv_nhwc(c, t16, n, hk, wk, rb.block2, F[k], F[k])) return r;
+    }
+  }
+  return 0;
+}
+
+static int t2i_check_size(sdxl_ctx* c, int n, int H, int W) {
+  if (n < 1 || H < 32 || W < 32 || H % 32 || W % 32)
+    return fail(c, 4920, "T2I-Adapter: hint must be [n >= 1, C, H, W] with H, W positive multiples of 32 (got n=%d, %dx%d)", n, H, W);
+  return 0;
+}
+
+extern "C" int sdxl_t2i_adapter_features(sdxl_t2i_adapter* a, int n, int H, int W, const float* hint, int on_host, float* out) {
+  if (!a || !hint || !out) return fail(a ? a->ctx : nullptr, -1, "sdxl_t2i_adapter_features: null argument");
+  sdxl_ctx* c = a->ctx;
+  if (int r = t2i_check_size(c, n, H, W)) return r;
+  CU(c, cudaSetDevice(c->device));
+  TmpBufs T(c->stream);
+  size_t total = 0;
+  float* F[4];
+  for (int k = 0; k < 4; ++k) {
+    total += t2i_feature_elems(a, k, n, H, W);
+    F[k] = (float*)T.get(t2i_feature_elems(a, k, n, H, W) * sizeof(float));
+  }
+  const size_t in_bytes = (size_t)n * a->cfg.in_channels * H * W * sizeof(float);
+  const float* x = hint;
+  float* o = out;
+  if (on_host) {
+    float* d = (float*)T.get(in_bytes);
+    o = (float*)T.get(total * sizeof(float));
+    if (!d || !o) return fail(c, 4911, "t2i_adapter_features: allocation failed");
+    CU(c, cudaMemcpyAsync(d, hint, in_bytes, cudaMemcpyHostToDevice, c->stream));
+    x = d;
+  }
+  for (int k = 0; k < 4; ++k)
+    if (!F[k]) return fail(c, 4911, "t2i_adapter_features: allocation failed");
+  if (int r = t2i_forward(a, n, H, W, x, F)) return r;
+  size_t off = 0;
+  for (int k = 0; k < 4; ++k) {
+    const int d = k < 2 ? 16 : 32;
+    KL(c, nhwc_to_nchw_f32_launch(c->stream, F[k], n, (H / d) * (W / d), a->ch[k], a->ch[k], o + off));
+    off += t2i_feature_elems(a, k, n, H, W);
+  }
+  if (on_host) {
+    CU(c, cudaMemcpyAsync(out, o, total * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+  }
+  return 0;
+}
+
+extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_control* ctl, int32_t t_min) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  // validate everything first: on failure the attached set is unchanged
+  if (n < 0 || n > SDXL_MAX_T2I_ADAPTERS) return fail(c, 4930, "set_t2i_adapters: n = %d outside [0, %d]", n, SDXL_MAX_T2I_ADAPTERS);
+  if (n > 0 && !ctl) return fail(c, 4931, "set_t2i_adapters: null control array");
+  if (n > 0)
+    if (const char* why = t2i_unet_problem(u->cfg)) return fail(c, 4932, "set_t2i_adapters: %s", why);
+  for (int k = 0; k < n; ++k) {
+    const sdxl_t2i_adapter* a = ctl[k].adapter;
+    if (!a) return fail(c, 4933, "set_t2i_adapters: item %d has a null adapter", k);
+    if (a->ctx != c) return fail(c, 4934, "set_t2i_adapters: item %d: the adapter was created on another sdxl_ctx", k);
+    if (const char* field = unet_cfg_mismatch(u->cfg, a->cfg.unet))
+      return fail(c, 4935, "set_t2i_adapters: item %d: adapter cfg field '%s' differs from the UNet's", k, field);
+    if (!ctl[k].hint) return fail(c, 4936, "set_t2i_adapters: item %d: null hint", k);
+    if (ctl[k].n_hint < 1) return fail(c, 4937, "set_t2i_adapters: item %d: n_hint = %d must be >= 1", k, ctl[k].n_hint);
+    if (ctl[k].n_hint != ctl[0].n_hint || ctl[k].height != ctl[0].height || ctl[k].width != ctl[0].width)
+      return fail(c, 4938, "set_t2i_adapters: item %d: n_hint and size (%d, %dx%d) differ from item 0's (%d, %dx%d)", k, ctl[k].n_hint,
+                  ctl[k].height, ctl[k].width, ctl[0].n_hint, ctl[0].height, ctl[0].width);
+    if (int r = t2i_check_size(c, ctl[k].n_hint, ctl[k].height, ctl[k].width)) return r;
+    if (!isfinite(ctl[k].scale)) return fail(c, 4939, "set_t2i_adapters: item %d: scale is not finite", k);
+  }
+  if (n == 0) {
+    if (!u->t2i) return 0;
+    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
+    u->plan.reset();
+    u->t2i.reset();
+    return 0;
+  }
+  const int n_hint = ctl[0].n_hint, H = ctl[0].height, W = ctl[0].width;
+  const sdxl_t2i_adapter* a0 = ctl[0].adapter;
+  // the sum is formed in temporaries and copied into the attachment only when all of it succeeded
+  TmpBufs T(c->stream);
+  float* S[4];
+  float* Fa[4];
+  bool ok = true;
+  for (int k = 0; k < 4; ++k) {
+    S[k] = (float*)T.get(t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float));
+    Fa[k] = (float*)T.get(t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float));
+    ok = ok && S[k] && Fa[k];
+  }
+  if (!ok) return fail(c, 4940, "set_t2i_adapters: cannot allocate the feature staging buffers");
+  for (int k = 0; k < 4; ++k) CU(c, cudaMemsetAsync(S[k], 0, t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float), c->stream));
+  for (int i = 0; i < n; ++i) {
+    const float* hint = ctl[i].hint;
+    if (ctl[i].hint_on_host) {
+      const size_t bytes = (size_t)n_hint * ctl[i].adapter->cfg.in_channels * H * W * sizeof(float);
+      float* d = (float*)T.get(bytes);
+      if (!d) return fail(c, 4940, "set_t2i_adapters: cannot allocate %zu bytes for hint %d", bytes, i);
+      CU(c, cudaMemcpyAsync(d, ctl[i].hint, bytes, cudaMemcpyHostToDevice, c->stream));
+      hint = d;
+    }
+    if (int r = t2i_forward(ctl[i].adapter, n_hint, H, W, hint, Fa)) return r;
+    for (int k = 0; k < 4; ++k)   // S += s_i * F_i, adapters in array order
+      KL(c, axpby_launch(c->stream, S[k], Fa[k], t2i_feature_elems(a0, k, n_hint, H, W), 1.f, ctl[i].scale));
+  }
+  CU(c, cudaStreamSynchronize(c->stream));   // the caller's host hints; any failure of the work above surfaces here
+  T2IAttach* cur = u->t2i.get();
+  std::unique_ptr<T2IAttach> fresh;
+  if (!cur || cur->n_hint != n_hint || cur->h != H / 8 || cur->w != W / 8) {   // new shapes: new buffers and a new plan
+    fresh.reset(new T2IAttach());
+    T2IAttach& f = *fresh;
+    f.n_hint = n_hint; f.h = H / 8; f.w = W / 8;
+    t2i_points(block_program(u->cfg), f.points);
+    for (int k = 0; k < 4; ++k) {
+      const int d = k < 2 ? 16 : 32;
+      f.C[k] = a0->ch[k]; f.H[k] = H / d; f.W[k] = W / d;
+    }
+    if (int r = carve_measured(c, f.mem, 4941, "set_t2i_adapters: feature buffers", [&](Arena& A) {
+          for (int k = 0; k < 4; ++k) f.F[k] = A.get<float>(t2i_feature_elems(a0, k, n_hint, H, W));
+          f.t_min = A.get<int>(1);
+          return 0;
+        }))
+      return r;
+    cur = fresh.get();
+  }
+  for (int k = 0; k < 4; ++k)
+    CU(c, cudaMemcpyAsync(cur->F[k], S[k], t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(cur->t_min, &t_min, sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));   // t_min is on the stack; the old plan and attachment may still be in flight
+  if (fresh) {
+    u->plan.reset();
+    u->t2i = std::move(fresh);
+  }
+  return 0;
+}
+
+// ================================================================================================
 // LoRA adapters (include/sdxl_b200.h; merge in engine_core.h: adapters_apply)
 // ================================================================================================
 extern "C" int sdxl_unet_set_adapters(sdxl_unet* u, int n, const sdxl_adapter* adapters) {
@@ -1694,6 +2005,12 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
     if (Bimg % a.n_hint) return fail(c, 5204, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bimg, a.n_hint);
     if (a.h != h || a.w != w)
       return fail(c, 5205, "control %zu: its hint is %dx%d pixels but the resolution is %dx%d", k, 8 * a.h, 8 * a.w, 8 * h, 8 * w);
+  }
+  if (u->t2i) {   // the CFG rows of image b both use feature set b % n_hint
+    const T2IAttach& a = *u->t2i;
+    if (Bimg % a.n_hint) return fail(c, 5206, "T2I-Adapter: batch %d is not a multiple of n_hint = %d", Bimg, a.n_hint);
+    if (a.h != h || a.w != w)
+      return fail(c, 5207, "T2I-Adapter: its hint is %dx%d pixels but the resolution is %dx%d", 8 * a.h, 8 * a.w, 8 * h, 8 * w);
   }
   if (int r = ip_check_batch(u, u->ip ? u->ip->n_batch : 0, nfwd * Bimg, nfwd == 2 ? Bimg : 0)) return r;
   Sampler* S = u->sampler.get();

@@ -265,6 +265,16 @@ int ln_gather_f32_launch(cudaStream_t st, const float* x, const int* idx, int B,
 int perceiver_ln_launch(cudaStream_t st, const float* x, const float* lat, int n, int L, int Q, int C, const float* g1,
                         const float* b1, const float* g2, const float* b2, float eps, __half* kv, __half* q);
 
+// T2I-Adapter kernels (t2i_kernels.cu)
+// PixelUnshuffle(16): hint f32 NCHW [n, C, H, W] -> f16 NHWC [n, H/16, W/16, C*256], channel ci*256 + i*16 + j <- hint[ci, 16y+i, 16x+j].
+int pixel_unshuffle_launch(cudaStream_t st, const float* x, int n, int C, int H, int W, __half* y);
+// y = f16(relu(x)), n % 4 == 0.
+int relu_f16_launch(cudaStream_t st, const float* x, size_t n, __half* y);
+// 2x2 stride-2 average pool: f32 NHWC [n, H, W, C] -> f16 NHWC [n, H/2, W/2, C], C % 4 == 0.
+int avg_pool2_f16_launch(cudaStream_t st, const float* x, int n, int H, int W, int C, __half* y);
+// x[b] += F[b % n_hint] (f32, per_img floats per image, a multiple of 4) when *t >= *t_min; t and t_min are device ints. PDL plan op.
+int t2i_add_launch(cudaStream_t st, float* x, const float* F, long per_img, int B, int n_hint, const int* t, const int* t_min);
+
 // Weight re-layout at load time (elementwise.cu)
 // Linear [K(in), N(out)] row-major f16 -> K-major [N, Kpad] f16 (zero padded), dst row pitch Kpad;
 // rows written at dst_row0 + perm(n) where perm handles the GEGLU value/gate interleave (geglu_bn>0).

@@ -91,6 +91,18 @@ class ImagePrompt(C.Structure):
                 ("seq_len", C.c_int32)]
 
 
+class T2IAdapterCfg(C.Structure):
+    _fields_ = [("unet", UnetCfg), ("in_channels", C.c_int32), ("n_res_blocks", C.c_int32)]
+
+
+class T2IControl(C.Structure):
+    _fields_ = [("adapter", C.c_void_p), ("hint", C.c_void_p), ("hint_on_host", C.c_int32), ("n_hint", C.c_int32),
+                ("height", C.c_int32), ("width", C.c_int32), ("scale", C.c_float)]
+
+
+MAX_T2I_ADAPTERS = 4   # SDXL_MAX_T2I_ADAPTERS (include/sdxl_b200.h)
+
+
 # name -> (restype, argtypes); every symbol include/sdxl_b200.h declares
 P = C.c_void_p
 I = C.c_int
@@ -165,6 +177,10 @@ PROTOTYPES = {
     "sdxl_ip_adapter_project": (I, [P, I, P, I, P]),
     "sdxl_ip_adapter_resample": (I, [P, I, I, P, I, P]),
     "sdxl_op_ip_attention": (I, [P, P, P, P, P, P, I, I, I, I, I, I, C.c_float, P]),
+    "sdxl_t2i_adapter_load": (I, [P, C.POINTER(T2IAdapterCfg), P, C.c_size_t, I, C.POINTER(P)]),
+    "sdxl_t2i_adapter_destroy": (None, [P]),
+    "sdxl_unet_set_t2i_adapters": (I, [P, I, C.POINTER(T2IControl), C.c_int32]),
+    "sdxl_t2i_adapter_features": (I, [P, I, I, I, P, I, P]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),
     "sdxl_mpk_encode_u16": (C.c_size_t, [P, C.c_size_t, P]),

@@ -61,6 +61,24 @@ TINY_CONTROLNET = ControlNetConfig(TINY, hint_block_channels=(8, 16, 24, 32))
 
 
 @dataclass(frozen=True)
+class T2IAdapterConfig:
+    """An SDXL T2I-Adapter (DESIGN.md §11, diffusers FullAdapterXL) for `unet`, which must be SDXL-base-shaped and match the UNet it is
+    attached to. Its four feature widths follow from the UNet's."""
+    unet: UNetConfig
+    in_channels: int = 3
+    n_res_blocks: int = 2
+
+    @property
+    def channels(self) -> Tuple[int, int, int, int]:
+        mc, m = self.unet.model_channels, self.unet.channel_mults
+        return (mc * m[0], mc * m[1], mc * m[2], mc * m[2])
+
+
+SDXL_T2I_ADAPTER = T2IAdapterConfig(SDXL_BASE)
+TINY_T2I_ADAPTER = T2IAdapterConfig(TINY)
+
+
+@dataclass(frozen=True)
 class VaeConfig:
     """Decoder half of AutoencoderConfig (reference src/model/autoencoder/mod.rs:28-45: the widths are hard-coded
     there; parameters here so a small instance can be tested) + LatentDecoder.scale_factor."""

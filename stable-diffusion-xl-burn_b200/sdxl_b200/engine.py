@@ -287,6 +287,9 @@ class Diffuser:
             if getattr(self, "_image_prompt", None):
                 from .ip_adapter import release_image_prompt
                 release_image_prompt(self)
+            if getattr(self, "_t2i_adapters", None):
+                from .t2i_adapter import release_t2i_adapters
+                release_t2i_adapters(self)
 
     def __del__(self):
         try:
@@ -311,6 +314,13 @@ class Diffuser:
         IP-Adapter Plus: embeds and negative (required) are vision hidden states [n_batch, n_images, L, D] (IPAdapter.image_embeds)."""
         from .ip_adapter import set_image_prompt
         set_image_prompt(self, adapter, embeds, scale, negative)
+
+    def set_t2i_adapters(self, adapters: Sequence, t_min: int = 0) -> None:
+        """Replaces the attached T2I-Adapters with [(T2IAdapter, hint, scale), ...] (sdxl_unet_set_t2i_adapters); [] detaches.
+        hint: u8 [n, H, W, C] or f32 [n, C, H, W] in [0, 1], H and W multiples of 32; image b of a batch uses hint b % n. The features
+        are added at timesteps t >= t_min (t2i_adapter.t2i_t_min maps diffusers' adapter_conditioning_factor)."""
+        from .t2i_adapter import set_t2i_adapters
+        set_t2i_adapters(self, adapters, t_min)
 
     # ---- UNet::forward -------------------------------------------------------------------------
     def set_conditioning(self, context: torch.Tensor, label: torch.Tensor) -> None:
@@ -360,12 +370,15 @@ class Diffuser:
 
     KIND_NAMES = ["igemm_wgmma", "attention_wgmma", "group_norm", "layer_norm", "gemv", "timestep_embedding",
                   "conv_in", "upsample2x", "phase_split", "cast_f16"]
+    # kinds only the UNet plan launches, by kind index (KIND_NAMES is positional and LatentDecoder.KIND_NAMES extends it)
+    UNET_KINDS = {17: "t2i_add"}
 
     def profile_plan(self) -> Dict[str, Dict[str, float]]:
         """Per-kernel-kind device time (ms), algorithmic FLOPs and launch count of one plan execution."""
         ms, fl, ln = (C.c_double * _lib.PROFILE_KINDS)(), (C.c_double * _lib.PROFILE_KINDS)(), (C.c_int * _lib.PROFILE_KINDS)()
         self.ctx.check(self.ctx.lib.sdxl_unet_profile_plan(self.h, ms, fl, ln), "sdxl_unet_profile_plan")
-        return {n: {"ms": ms[i], "flops": fl[i], "launches": ln[i]} for i, n in enumerate(self.KIND_NAMES) if ln[i]}
+        kinds = list(enumerate(self.KIND_NAMES)) + list(self.UNET_KINDS.items())
+        return {n: {"ms": ms[i], "flops": fl[i], "launches": ln[i]} for i, n in kinds if ln[i]}
 
     def profile_dump(self, path: str) -> None:
         self.ctx.check(self.ctx.lib.sdxl_unet_profile_dump(self.h, path.encode()), "sdxl_unet_profile_dump")

@@ -28,7 +28,8 @@ def make_inpaint_mask(img_hw: Tuple[int, int], latent_hw: Tuple[int, int], crop_
 def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_steps: int = 30, refiner=None,
            reference_rgb: Optional[torch.Tensor] = None, crop: Sequence[Optional[int]] = (None, None, None, None), crop_out: bool = False,
            resolution: Tuple[int, int] = (1024, 1024), seed: int = 0, noise: Optional[torch.Tensor] = None,
-           loras: Optional[Sequence] = None, controls: Optional[Sequence] = None, image_prompt: Optional[Sequence] = None) -> torch.Tensor:
+           loras: Optional[Sequence] = None, controls: Optional[Sequence] = None, image_prompt: Optional[Sequence] = None,
+           t2i_adapters: Optional[Sequence] = None, t2i_factor: float = 1.0) -> torch.Tensor:
     """One image, like `sample --prompt ... [--reference-img ... --crop-* ...] [--use-refiner]`.
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
     bottom) in pixels. loras: [(kohya .safetensors path / bytes / tensor dict, scale), ...] merged into the base UNet and both
@@ -36,23 +37,34 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     those models had. controls: [(ControlNet, image u8 [1, H, W, 3] or f32 [1, 3, H, W], scale), ...] attached to the base UNet
     for this call and detached afterwards (the refiner is left alone). image_prompt: (IPAdapter, ClipVisionEncoder, images u8
     [n_images, H, W, 3], scale): the images are encoded (IPAdapter.image_embeds: image_embeds for the base adapter, hidden states for
-    IP-Adapter Plus) and attached to the base UNet as one prompt of n_images images for this call and detached afterwards. Returns uint8 [1, H, W, 3]."""
+    IP-Adapter Plus) and attached to the base UNet as one prompt of n_images images for this call and detached afterwards.
+    t2i_adapters: [(T2IAdapter, image u8 [1, H, W, C] or f32 [1, C, H, W], scale), ...] attached to the base UNet for this call and
+    detached afterwards, their features added on the first int(n_steps * t2i_factor) iterations (diffusers'
+    adapter_conditioning_factor). Returns uint8 [1, H, W, 3]."""
     if image_prompt:
         adapter, encoder, images, scale = image_prompt
         e, neg = adapter.image_embeds(encoder, images)
         diffuser.set_image_prompt(adapter, e.unsqueeze(0), scale, negative=neg.unsqueeze(0))
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                          seed, noise, loras, controls)
+                          seed, noise, loras, controls, t2i_adapters=t2i_adapters, t2i_factor=t2i_factor)
         finally:
             diffuser.set_image_prompt(None)
     if controls:
         diffuser.set_controls(controls)
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                          seed, noise, loras)
+                          seed, noise, loras, t2i_adapters=t2i_adapters, t2i_factor=t2i_factor)
         finally:
             diffuser.set_controls([])
+    if t2i_adapters:
+        from .t2i_adapter import t2i_t_min
+        diffuser.set_t2i_adapters(t2i_adapters, t_min=t2i_t_min(n_steps, t2i_factor))
+        try:
+            return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
+                          seed, noise, loras)
+        finally:
+            diffuser.set_t2i_adapters([])
     if not loras:
         return _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
                        seed, noise)

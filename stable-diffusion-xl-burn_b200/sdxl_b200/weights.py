@@ -22,7 +22,7 @@ from typing import Dict, Iterable, List, Tuple
 import numpy as np
 import torch
 
-from .config import ClipConfig, ControlNetConfig, UNetConfig, VaeConfig, block_program
+from .config import ClipConfig, ControlNetConfig, T2IAdapterConfig, UNetConfig, VaeConfig, block_program
 
 Spec = Tuple[str, Tuple[int, ...], str, float]  # name, shape, kind, scale
 
@@ -117,6 +117,21 @@ def controlnet_tensor_specs(cfg: ControlNetConfig) -> List[Spec]:
     return s
 
 
+def t2i_adapter_tensor_specs(cfg: T2IAdapterConfig) -> List[Spec]:
+    """A T2I-Adapter pack (include/sdxl_b200.h): diffusers FullAdapterXL's keys without `adapter.`, `/`-separated. The synthetic
+    block2 convs (the resnets' residual outputs) get the residual-output scale."""
+    ch = cfg.channels
+    s: List[Spec] = [("conv_in/weight", (ch[0], cfg.in_channels * 256, 3, 3), "conv", 1.0), ("conv_in/bias", (ch[0],), "bias", 1.0)]
+    for k in range(4):
+        if k in (1, 2):
+            s += [(f"body/{k}/in_conv/weight", (ch[k], ch[k - 1], 1, 1), "conv", 1.0), (f"body/{k}/in_conv/bias", (ch[k],), "bias", 1.0)]
+        for j in range(cfg.n_res_blocks):
+            p = f"body/{k}/resnets/{j}"
+            s += [(f"{p}/block1/weight", (ch[k], ch[k], 3, 3), "conv", 1.0), (f"{p}/block1/bias", (ch[k],), "bias", 1.0),
+                  (f"{p}/block2/weight", (ch[k], ch[k], 1, 1), "conv", RESID_SCALE), (f"{p}/block2/bias", (ch[k],), "bias", 1.0)]
+    return s
+
+
 def _vres_specs(path: str, c_in: int, c_out: int) -> List[Spec]:
     s: List[Spec] = [
         (f"{path}/norm1/weight", (c_in,), "gamma", 1.0), (f"{path}/norm1/bias", (c_in,), "beta", 1.0),
@@ -206,15 +221,17 @@ def alphas_cumprod(n_steps: int = 1000) -> torch.Tensor:
 
 def synth_weights(cfg, seed: int = 0, device: str = "cpu") -> Dict[str, torch.Tensor]:
     """Deterministic (per device type) synthetic f16 weights, reference layouts and names.
-    cfg: UNetConfig (adds alphas_cumprod), VaeConfig (decoder tensors), ClipConfig (text encoder) or ControlNetConfig."""
+    cfg: UNetConfig (adds alphas_cumprod), VaeConfig (decoder tensors), ClipConfig (text encoder), ControlNetConfig or
+    T2IAdapterConfig."""
     gen = torch.Generator(device=device)
     gen.manual_seed(seed)
     out: Dict[str, torch.Tensor] = {}
     is_vae = isinstance(cfg, VaeConfig)
     is_clip = isinstance(cfg, ClipConfig)
     is_cn = isinstance(cfg, ControlNetConfig)
+    is_t2i = isinstance(cfg, T2IAdapterConfig)
     specs = (vae_tensor_specs(cfg) if is_vae else clip_tensor_specs(cfg) if is_clip else controlnet_tensor_specs(cfg) if is_cn
-             else unet_tensor_specs(cfg))
+             else t2i_adapter_tensor_specs(cfg) if is_t2i else unet_tensor_specs(cfg))
     for name, shape, kind, scale in specs:
         if kind == "linear":
             t = torch.randn(shape, generator=gen, device=device) * (scale / shape[0] ** 0.5)
@@ -231,7 +248,7 @@ def synth_weights(cfg, seed: int = 0, device: str = "cpu") -> Dict[str, torch.Te
         else:
             raise ValueError(kind)
         out[name] = t.to(torch.float16)
-    if not is_vae and not is_clip and not is_cn:
+    if not is_vae and not is_clip and not is_cn and not is_t2i:
         out["alphas_cumprod"] = alphas_cumprod(cfg.n_steps).to(device)
     return out
 
