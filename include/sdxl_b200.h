@@ -517,6 +517,26 @@ SDXL_API int sdxl_unet_set_t2i_adapters(sdxl_unet* unet, int n, const sdxl_t2i_c
  * pointers are host memory if on_host. */
 SDXL_API int sdxl_t2i_adapter_features(sdxl_t2i_adapter* adapter, int n, int H, int W, const float* hint, int on_host, float* out);
 
+/* ---- inpainting UNet -----------------------------------------------------------------------------------
+ * A UNet cfg with in_channels = 2 * out_channels + 1 > 8 (9 for SDXL: diffusers' stable-diffusion-xl-1.0-inpainting-0.1) has the
+ * inpainting layout (DESIGN.md §12): its first conv reads the latent (out_channels), the mask (1) and the masked image's latent
+ * (out_channels), concatenated in that order. The latent the forward entry points, the sampler and sdxl_sample_latent take and return
+ * has out_channels channels; the other in_channels - out_channels come from the condition attached here, the same at every step. */
+typedef struct sdxl_inpaint_condition {
+  const float* cond;       /* f32 NCHW [n, in_channels - out_channels, height/8, width/8]: the mask (1 = repaint), then the
+                              masked image's latent (scaled like sdxl_vae_encode_image); borrowed for the call */
+  int32_t on_host;
+  int32_t n;               /* UNet row b uses row b % n */
+  int32_t height, width;   /* pixels; the latent must be height/8 x width/8 */
+} sdxl_inpaint_condition;
+/* Copies the condition into a buffer the UNet owns (NULL detaches). Everything is validated before anything changes (the UNet has the
+ * inpainting layout, cond non-null, n >= 1, height and width positive multiples of 8): on failure the previous condition stays
+ * attached. A call with the same n and size rewrites the buffer in place (same launch plan and CUDA graph); any other change rebuilds
+ * the plan at the next forward. A forward or sampler_begin on an inpainting UNet fails when no condition is attached, when the latent
+ * is not height/8 x width/8, or when the batch (the images, for the sampler: the CFG rows [cond | uncond] of image b both read row
+ * b % n) is not a multiple of n. */
+SDXL_API int sdxl_unet_set_inpaint_condition(sdxl_unet* unet, const sdxl_inpaint_condition* c);
+
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),
  * ones inside the window, zero outside, inverted by crop_out; mask = 1 keeps the generated latent. Negative bound = not given

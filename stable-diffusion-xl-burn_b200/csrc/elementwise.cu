@@ -130,11 +130,15 @@ int timestep_embedding_launch(cudaStream_t st, const int* t_dev, int nt, int dim
 // ------------------------------------------------------------------------------------------------
 // One thread = 4 output channels x 8 consecutive pixels of a row: every weight float4 read from shared memory feeds 32 FMAs
 // (at one pixel per thread the kernel was bound by the LDS.128 per 4 FMAs: 158 us for the UNet's 2x128x128x320 output).
+// kCat (the inpainting UNet): input channels [C1, Cin) come from a second source x2, f32 NCHW [n2, Cin - C1, H, W], output batch
+// b reading image b % n2. Which source a (kh, c) pair reads is the same in every lane. kCat = false compiles to the one-source
+// kernel: x2 / n2 / C1 are unused and the dead branch is removed.
 constexpr int kConvInPix = 8;
-template <typename TIn>
+template <typename TIn, bool kCat = false>
 __global__ void __launch_bounds__(256) conv_in_kernel(const TIn* __restrict__ x, int Bx, int B, int Cin, int H, int W,
                                                       const float* __restrict__ w, const float* __restrict__ bias, int Cout,
-                                                      float* __restrict__ y, const float* __restrict__ add, int n_add) {
+                                                      float* __restrict__ y, const float* __restrict__ add, int n_add,
+                                                      const float* __restrict__ x2, int n2, int C1) {
   extern __shared__ float sw[];  // [9*Cin][Cout]  (k-major: lanes = consecutive output channels, conflict-free)
   const int kk = 9 * Cin;
   for (int co = threadIdx.x; co < Cout; co += blockDim.x)          // lanes = consecutive rows of w: conflict-free smem writes,
@@ -149,7 +153,8 @@ __global__ void __launch_bounds__(256) conv_in_kernel(const TIn* __restrict__ x,
     const int w0 = (int)(seg % nseg) * kConvInPix;
     const int hh = (int)((seg / nseg) % H);
     const int b = (int)(seg / ((long)nseg * H));
-    const TIn* xb = x + (size_t)(b % Bx) * Cin * H * W;
+    const TIn* xb = x + (size_t)(b % Bx) * (kCat ? C1 : Cin) * H * W;
+    const float* x2b = kCat ? x2 + (size_t)(b % n2) * (Cin - C1) * H * W : nullptr;
     const float4 b4 = bias ? *reinterpret_cast<const float4*>(bias + cv * 4) : make_float4(0.f, 0.f, 0.f, 0.f);
     float4 acc[kConvInPix];
 #pragma unroll
@@ -158,12 +163,21 @@ __global__ void __launch_bounds__(256) conv_in_kernel(const TIn* __restrict__ x,
       const int ih = hh + kh - 1;
       if (ih < 0 || ih >= H) continue;
       for (int c = 0; c < Cin; ++c) {
-        const TIn* xr = xb + ((size_t)c * H + ih) * W;
         float xv[kConvInPix + 2];                                  // the row segment with its halo; same address in all lanes
+        if (kCat && c >= C1) {
+          const float* xr = x2b + ((size_t)(c - C1) * H + ih) * W;
 #pragma unroll
-        for (int i = 0; i < kConvInPix + 2; ++i) {
-          const int iw = w0 + i - 1;
-          xv[i] = (iw >= 0 && iw < W) ? (float)xr[iw] : 0.f;
+          for (int i = 0; i < kConvInPix + 2; ++i) {
+            const int iw = w0 + i - 1;
+            xv[i] = (iw >= 0 && iw < W) ? xr[iw] : 0.f;
+          }
+        } else {
+          const TIn* xr = xb + ((size_t)c * H + ih) * W;
+#pragma unroll
+          for (int i = 0; i < kConvInPix + 2; ++i) {
+            const int iw = w0 + i - 1;
+            xv[i] = (iw >= 0 && iw < W) ? (float)xr[iw] : 0.f;
+          }
         }
 #pragma unroll
         for (int kw = 0; kw < 3; ++kw) {
@@ -204,9 +218,27 @@ int conv_in_launch_t(cudaStream_t st, const void* x, int x_f32, int Bx, int B, i
   int grid = cdiv(total, 256);
   if (grid > 132 * 4) grid = 132 * 4;
   if (x_f32)
-    conv_in_kernel<float><<<grid, 256, smem, st>>>((const float*)x, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add);
+    conv_in_kernel<float><<<grid, 256, smem, st>>>((const float*)x, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add, nullptr, 1, Cin);
   else
-    conv_in_kernel<__half><<<grid, 256, smem, st>>>((const __half*)x, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add);
+    conv_in_kernel<__half><<<grid, 256, smem, st>>>((const __half*)x, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add, nullptr, 1, Cin);
+  return (int)cudaGetLastError();
+}
+int conv_in_cat_launch(cudaStream_t st, const void* x, int x_f32, int Bx, int B, int C1, const float* x2, int n2, int C2, int H, int W,
+                       const float* w, const float* bias, int Cout, float* y, const float* add, int n_add) {
+  const int Cin = C1 + C2;
+  if (!x2 || C1 < 1 || C2 < 1 || Cin > 9 || n2 < 1 || (Cout & 3) || (add && n_add < 1)) return 2002;
+  const size_t smem = (size_t)Cout * 9 * Cin * sizeof(float);   // 320 x 81 floats: 104 KB at SDXL's 9 channels
+  static bool done_f[64], done_h[64];
+  if (smem > 200 * 1024) return 2002;
+  if (int r = smem_optin(conv_in_kernel<float, true>, 200 * 1024, done_f)) return r;
+  if (int r = smem_optin(conv_in_kernel<__half, true>, 200 * 1024, done_h)) return r;
+  const long total = (long)B * H * ((W + kConvInPix - 1) / kConvInPix) * (Cout / 4);
+  int grid = cdiv(total, 256);
+  if (grid > 132 * 4) grid = 132 * 4;
+  if (x_f32)
+    conv_in_kernel<float, true><<<grid, 256, smem, st>>>((const float*)x, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add, x2, n2, C1);
+  else
+    conv_in_kernel<__half, true><<<grid, 256, smem, st>>>((const __half*)x, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add, x2, n2, C1);
   return (int)cudaGetLastError();
 }
 int conv_in_launch(cudaStream_t st, const __half* x, int B, int Cin, int H, int W, const float* w, const float* bias,

@@ -141,11 +141,26 @@ static BlockProgram block_program(const sdxl_unet_cfg& g) {
   return p;
 }
 
+// The inpainting UNet (DESIGN.md §12, diffusers' stable-diffusion-xl-1.0-inpainting-0.1): its input is the latent (out_channels),
+// the mask (1) and the masked image's latent (out_channels), concatenated. The one-source first conv takes at most 8 channels, so
+// no configuration loadable without this layout has it.
+static bool inpaint_layout(const sdxl_unet_cfg& g) { return g.in_channels > 8 && g.in_channels == 2 * g.out_channels + 1; }
+// Channels of the latent the forward and the sampler take: out_channels on an inpainting UNet (the rest comes from the attached
+// condition), in_channels otherwise.
+static int latent_channels(const sdxl_unet_cfg& g) { return inpaint_layout(g) ? g.out_channels : g.in_channels; }
+
 struct Plan;
 struct Sampler;
 struct ControlAttach;
 struct IpAttach;
 struct T2IAttach;
+
+// An attached inpainting condition (sdxl_unet_set_inpaint_condition): f32 NCHW [n, in_channels - out_channels, h, w], owned.
+struct InpaintAttach {
+  int n = 0, h = 0, w = 0;   // latent extent
+  Arena mem;
+  float* cond = nullptr;
+};
 
 // Embeddings, first conv, input blocks and middle block: the part of the UNet a ControlNet copies.
 struct EncoderHalf {
@@ -202,6 +217,7 @@ struct sdxl_unet : EncoderHalf {
   std::vector<std::unique_ptr<ControlAttach>> controls;   // sdxl_unet_set_controls, in call order
   std::unique_ptr<IpAttach> ip;   // sdxl_unet_set_image_prompt
   std::unique_ptr<T2IAttach> t2i; // sdxl_unet_set_t2i_adapters
+  std::unique_ptr<InpaintAttach> inpaint;   // sdxl_unet_set_inpaint_condition
   uint64_t plan_builds = 0;
   int cfg_rows = 0;               // conditioning rows are the sampler's [cond | uncond] with cfg_rows cond rows (0: plain batch)
   ~sdxl_unet() {
@@ -472,7 +488,7 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
 static int check_unet_cfg(sdxl_ctx* c, const sdxl_unet_cfg& g) {
   if (g.n_head_channels != 64) return fail(c, 4200, "n_head_channels must be 64 (got %d)", g.n_head_channels);
   if (g.n_levels < 1 || g.n_levels > SDXL_MAX_LEVELS) return fail(c, 4201, "bad n_levels");
-  if (g.in_channels > 8 || g.model_channels % 32) return fail(c, 4202, "unsupported channel config");
+  if ((g.in_channels > 8 && !inpaint_layout(g)) || g.model_channels % 32) return fail(c, 4202, "unsupported channel config");
   return 0;
 }
 
@@ -611,6 +627,7 @@ extern "C" int sdxl_controlnet_load(sdxl_ctx* c, const sdxl_controlnet_cfg* cfg,
   if (!c || !cfg || !pack || !out) return fail(c, -1, "sdxl_controlnet_load: null argument");
   *out = nullptr;
   if (int r = check_unet_cfg(c, cfg->unet)) return r;
+  if (inpaint_layout(cfg->unet)) return fail(c, 4703, "ControlNet: a UNet cfg with the inpainting layout (in_channels = %d) is not supported", cfg->unet.in_channels);
   if (cfg->hint_in_channels < 1 || cfg->hint_in_channels > 8) return fail(c, 4700, "hint_in_channels must be in [1, 8] (got %d)", cfg->hint_in_channels);
   if (cfg->n_hint_blocks != 4) return fail(c, 4701, "n_hint_blocks must be 4 (hint downscale 2^(n-1) = 8), got %d", cfg->n_hint_blocks);
   for (int k = 0; k < cfg->n_hint_blocks; ++k)
@@ -722,10 +739,14 @@ struct UNetPlanBuilder : PlanBuilder {
     int H = P->h, W = P->w;
     float* x = buf<float>((size_t)Bf * H * W * mc);
     int Cx = mc;
+    // the inpainting UNet's first conv reads the attached condition as its input channels [out_channels, in_channels)
+    const InpaintAttach* ipc = cond == &u->cond ? u->inpaint.get() : nullptr;
+    if (inpaint_layout(g) && !ipc && !err) err = fail(c, 5018, "inpainting UNet: no inpainting condition attached");
     if (!err) {
       Op op{};
       op.kind = OP_CONV_IN;
-      op.ci = {P->x_in, P->Bx, Bf, g.in_channels, H, W, e.conv0_w, e.conv0_b, mc, x, hint, n_hint};
+      op.ci = {P->x_in, P->Bx, Bf, latent_channels(g), H, W, e.conv0_w, e.conv0_b, mc, x, hint, n_hint};
+      if (inpaint_layout(g)) { op.ci.x2 = ipc->cond; op.ci.n2 = ipc->n; op.ci.C2 = g.in_channels - g.out_channels; }
       P->ops.push_back(op);
       P->flops += 2.0 * Bf * H * W * 9.0 * g.in_channels * mc;
     }
@@ -906,7 +927,7 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
   const int levels = g.n_levels;
   if ((P->h % (1 << (levels - 1))) || (P->w % (1 << (levels - 1)))) return fail(c, 5003, "latent %dx%d not divisible by %d", P->h, P->w, 1 << (levels - 1));
 
-  P->x_in = B.buf<float>((size_t)P->Bx * g.in_channels * P->h * P->w);
+  P->x_in = B.buf<float>((size_t)P->Bx * latent_channels(g) * P->h * P->w);
   P->eps_ld = g.out_channels;
   P->eps = B.buf<float>((size_t)Bf * P->h * P->w * P->eps_ld);
   B.gn_partial = B.buf<float>(gn_scratch_floats(Bf, 32));
@@ -1017,6 +1038,19 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
   return B.err;
 }
 
+// An inpainting UNet runs only with a condition attached at the latent's extent, for a batch of images that is a multiple of its n
+// (n_img: the images, so both CFG rows of image b read condition row b % n).
+static int inpaint_check(sdxl_unet* u, int n_img, int h, int w) {
+  sdxl_ctx* c = u->ctx;
+  if (!inpaint_layout(u->cfg)) return 0;
+  const InpaintAttach* a = u->inpaint.get();
+  if (!a) return fail(c, 5018, "inpainting UNet: no inpainting condition attached (call sdxl_unet_set_inpaint_condition first)");
+  if (a->h != h || a->w != w)
+    return fail(c, 5019, "inpainting condition: it is %dx%d pixels (latent %dx%d) but the latent is %dx%d", 8 * a->h, 8 * a->w, a->h, a->w, h, w);
+  if (n_img % a->n) return fail(c, 5020, "inpainting condition: batch %d is not a multiple of its n = %d", n_img, a->n);
+  return 0;
+}
+
 static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
   sdxl_ctx* c = u->ctx;
   if (u->cond.condB != Bf) return fail(c, 5010, "conditioning is set for batch %d but forward batch is %d (call sdxl_unet_set_conditioning first)", u->cond.condB, Bf);
@@ -1033,6 +1067,7 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
       return fail(c, 5015, "T2I-Adapter: its hint is %dx%d pixels (latent %dx%d) but the latent is %dx%d", 8 * a.h, 8 * a.w, a.h, a.w, h, w);
     if (Bf % a.n_hint) return fail(c, 5016, "T2I-Adapter: batch %d is not a multiple of n_hint = %d", Bf, a.n_hint);
   }
+  if (int r = inpaint_check(u, Bf, h, w)) return r;
   // every change of the buffers or attachments a plan reads drops the plan, so the shapes are its whole cache key
   if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w) return 0;
   if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A); })) return r;
@@ -1892,6 +1927,52 @@ extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_co
 }
 
 // ================================================================================================
+// inpainting UNet (include/sdxl_b200.h: sdxl_unet_set_inpaint_condition; DESIGN.md §12)
+// ================================================================================================
+extern "C" int sdxl_unet_set_inpaint_condition(sdxl_unet* u, const sdxl_inpaint_condition* ic) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  const sdxl_unet_cfg& g = u->cfg;
+  if (!ic) {
+    if (!u->inpaint) return 0;
+    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
+    u->plan.reset();
+    u->inpaint.reset();
+    return 0;
+  }
+  // validate everything first: on failure the attached condition is unchanged
+  if (!inpaint_layout(g))
+    return fail(c, 4960, "set_inpaint_condition: the UNet does not have the inpainting layout (in_channels = %d, out_channels = %d; "
+                "it needs in_channels = 2 * out_channels + 1 > 8)", g.in_channels, g.out_channels);
+  if (!ic->cond) return fail(c, 4961, "set_inpaint_condition: null cond");
+  if (ic->n < 1) return fail(c, 4962, "set_inpaint_condition: n = %d must be >= 1", ic->n);
+  if (ic->height < 8 || ic->width < 8 || ic->height % 8 || ic->width % 8)
+    return fail(c, 4963, "set_inpaint_condition: size %dx%d must be a positive multiple of 8", ic->height, ic->width);
+  const int n = ic->n, h = ic->height / 8, w = ic->width / 8;
+  const size_t bytes = (size_t)n * (g.in_channels - g.out_channels) * h * w * sizeof(float);
+  InpaintAttach* cur = u->inpaint.get();
+  std::unique_ptr<InpaintAttach> fresh;
+  if (!cur || cur->n != n || cur->h != h || cur->w != w) {   // new shape: a new buffer and a new plan
+    fresh.reset(new InpaintAttach());
+    fresh->n = n; fresh->h = h; fresh->w = w;
+    if (int r = carve_measured(c, fresh->mem, 4964, "set_inpaint_condition: condition buffer", [&](Arena& A) {
+          fresh->cond = A.get<float>(bytes / sizeof(float));
+          return 0;
+        }))
+      return r;
+    cur = fresh.get();
+  }
+  CU(c, cudaMemcpyAsync(cur->cond, ic->cond, bytes, ic->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));   // the caller's memory; the old plan and buffer may still be in flight
+  if (fresh) {
+    u->plan.reset();
+    u->inpaint = std::move(fresh);
+  }
+  return 0;
+}
+
+// ================================================================================================
 // LoRA adapters (include/sdxl_b200.h; merge in engine_core.h: adapters_apply)
 // ================================================================================================
 extern "C" int sdxl_unet_set_adapters(sdxl_unet* u, int n, const sdxl_adapter* adapters) {
@@ -1919,7 +2000,7 @@ extern "C" int sdxl_unet_forward(sdxl_unet* u, int B, int h, int w, const sdxl_h
   int r = ensure_plan(u, B, B, h, w);
   if (r) return r;
   Plan* P = u->plan.get();
-  KL(c, cast_f16_to_f32_launch(c->stream, (const __half*)x, (size_t)B * u->cfg.in_channels * h * w, P->x_in));
+  KL(c, cast_f16_to_f32_launch(c->stream, (const __half*)x, (size_t)B * latent_channels(u->cfg) * h * w, P->x_in));
   if ((r = set_t(u, t_host))) return r;
   if ((r = run_plan(u))) return r;
   KL(c, nhwc_to_nchw_f16_launch(c->stream, P->eps, B, h * w, u->cfg.out_channels, P->eps_ld, (__half*)eps_out));
@@ -1932,7 +2013,7 @@ extern "C" int sdxl_unet_forward_f32(sdxl_unet* u, int B, int h, int w, const fl
   int r = ensure_plan(u, B, B, h, w);
   if (r) return r;
   Plan* P = u->plan.get();
-  CU(c, cudaMemcpyAsync(P->x_in, x, (size_t)B * u->cfg.in_channels * h * w * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(P->x_in, x, (size_t)B * latent_channels(u->cfg) * h * w * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
   if ((r = set_t(u, t_host))) return r;
   if ((r = run_plan(u))) return r;
   KL(c, nhwc_to_nchw_f32_launch(c->stream, P->eps, B, h * w, u->cfg.out_channels, P->eps_ld, eps_out));
@@ -2013,8 +2094,9 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
       return fail(c, 5207, "T2I-Adapter: its hint is %dx%d pixels but the resolution is %dx%d", 8 * a.h, 8 * a.w, 8 * h, 8 * w);
   }
   if (int r = ip_check_batch(u, u->ip ? u->ip->n_batch : 0, nfwd * Bimg, nfwd == 2 ? Bimg : 0)) return r;
+  if (int r = inpaint_check(u, Bimg, h, w)) return r;
   Sampler* S = u->sampler.get();
-  const size_t lat = (size_t)Bimg * g.in_channels * h * w;
+  const size_t lat = (size_t)Bimg * latent_channels(g) * h * w;
   if (n_ctx < 1) return fail(c, 5202, "bad conditioning context length");
   // new shapes: a fresh sampler, installed only when the conditioning and the plan for it are in place (the steps pair its
   // shapes with the plan's buffers)
@@ -2066,7 +2148,7 @@ static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   int r = set_t(u, t);
   if (r) return r;
   if ((r = run_plan(u))) return r;
-  KL(c, cfg_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, u->cfg.in_channels, S->h * S->w, S->nfwd == 2, S->guidance,
+  KL(c, cfg_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->nfwd == 2, S->guidance,
                         (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap), P->x_in, nullptr));
   return 0;
 }

@@ -441,7 +441,9 @@ struct Op {
   struct { const float* x; const float* g; const float* b; float eps; int rows, C; __half* y; } ln;
   struct { const float* in; int in_bstride, Bv, K; const __half* W; int ldw; const float* bias; const float* add; int add_bstride, N, in_silu, out_silu; float* out; int out_bstride; } gv;
   struct { const int* t; int n, dim; float* out; } te;
-  struct { const float* x; int Bx, B, Cin, H, W; const float* w; const float* bias; int Cout; float* y; const float* add; int n_add; } ci;
+  // x2 (nullable): second input source, channels [Cin, Cin + C2) (conv_in_cat_launch)
+  struct { const float* x; int Bx, B, Cin, H, W; const float* w; const float* bias; int Cout; float* y; const float* add; int n_add;
+           const float* x2; int n2, C2; } ci;
   struct { const float* x; int B, H, W, C; __half* y; } rs;  // upsample / phase split
   struct { const float* x; size_t n; __half* y; } cs;
   struct { const float* S; size_t lds; int rows, cols; float scale; __half* P; size_t ldp; } sm;
@@ -664,8 +666,12 @@ static int exec_op(sdxl_ctx* c, Op& op) {
       break;
     case OP_TEMB: KL(c, timestep_embedding_launch(st, op.te.t, op.te.n, op.te.dim, 10000.f, op.te.out)); break;
     case OP_CONV_IN:
-      KL(c, conv_in_launch_t(st, op.ci.x, 1, op.ci.Bx, op.ci.B, op.ci.Cin, op.ci.H, op.ci.W, op.ci.w, op.ci.bias, op.ci.Cout, op.ci.y,
-                             op.ci.add, op.ci.n_add));
+      if (op.ci.x2)
+        KL(c, conv_in_cat_launch(st, op.ci.x, 1, op.ci.Bx, op.ci.B, op.ci.Cin, op.ci.x2, op.ci.n2, op.ci.C2, op.ci.H, op.ci.W, op.ci.w,
+                                 op.ci.bias, op.ci.Cout, op.ci.y, op.ci.add, op.ci.n_add));
+      else
+        KL(c, conv_in_launch_t(st, op.ci.x, 1, op.ci.Bx, op.ci.B, op.ci.Cin, op.ci.H, op.ci.W, op.ci.w, op.ci.bias, op.ci.Cout, op.ci.y,
+                               op.ci.add, op.ci.n_add));
       break;
     case OP_UPS: KL(c, upsample2x_launch(st, op.rs.x, op.rs.B, op.rs.H, op.rs.W, op.rs.C, op.rs.y)); break;
     case OP_PHASE: KL(c, phase_split_launch(st, op.rs.x, op.rs.B, op.rs.H, op.rs.W, op.rs.C, op.rs.y)); break;

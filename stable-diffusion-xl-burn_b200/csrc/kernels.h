@@ -192,6 +192,10 @@ int conv_in_launch(cudaStream_t st, const __half* x, int B, int Cin, int H, int 
 // added to the output at batch b % n_add (a ControlNet's hint embedding).
 int conv_in_launch_t(cudaStream_t st, const void* x, int x_f32, int Bx, int B, int Cin, int H, int W,
                      const float* w, const float* bias, int Cout, float* y, const float* add = nullptr, int n_add = 1);
+// two-source form (the inpainting UNet): input channels [0, C1) from x as above, [C1, C1 + C2) from x2 f32 NCHW [n2, C2, H, W]
+// at batch b % n2; C1 + C2 <= 9. w: [Cout][3][3][C1 + C2].
+int conv_in_cat_launch(cudaStream_t st, const void* x, int x_f32, int Bx, int B, int C1, const float* x2, int n2, int C2, int H, int W,
+                       const float* w, const float* bias, int Cout, float* y, const float* add = nullptr, int n_add = 1);
 // y = f16(silu(x)) of NHWC f32 [B,H,W,C]; phase != 0: written as the stride-2 phase split of phase_split_launch.
 int silu_f16_launch(cudaStream_t st, const float* x, int B, int H, int W, int C, int phase, __half* y);
 // wo[i] = f16(s * w[i]) (i < nw), bo[i] = s * b[i] (i < nb)

@@ -88,6 +88,11 @@ SDXL_TEST_API int sdxl_test_conv_in(void* stream, const void* x, int x_f32, int 
                                     const float* bias, int Cout, float* y, const float* add, int n_add) {
   return conv_in_launch_t((cudaStream_t)stream, x, x_f32, Bx, B, Cin, H, W, w, bias, Cout, y, add, n_add);
 }
+// The inpainting UNet's first conv: channels [0, C1) from x (image b % Bx), [C1, C1 + C2) from x2 f32 (image b % n2).
+SDXL_TEST_API int sdxl_test_conv_in_cat(void* stream, const void* x, int x_f32, int Bx, int B, int C1, const float* x2, int n2, int C2,
+                                        int H, int W, const float* w, const float* bias, int Cout, float* y) {
+  return conv_in_cat_launch((cudaStream_t)stream, x, x_f32, Bx, B, C1, x2, n2, C2, H, W, w, bias, Cout, y);
+}
 
 SDXL_TEST_API int sdxl_test_repack_upconv(void* stream, const void* src, int O, int I, void* dst, int Ipad) {
   return repack_upconv_launch((cudaStream_t)stream, (const __half*)src, O, I, (__half*)dst, Ipad);

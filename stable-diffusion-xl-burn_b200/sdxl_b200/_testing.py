@@ -27,6 +27,7 @@ PROTOTYPES = {
     "sdxl_test_gn": (I, [P, P, I, P, I, I, I, I, P, P, F, I, P, P, P, P]),
     "sdxl_test_gemv": (I, [P, P, I, I, I, P, I, P, P, I, I, I, I, P, I]),
     "sdxl_test_conv_in": (I, [P, P, I, I, I, I, I, I, P, P, I, P, P, I]),
+    "sdxl_test_conv_in_cat": (I, [P, P, I, I, I, I, P, I, I, I, I, P, P, I, P]),
     "sdxl_test_repack_upconv": (I, [P, P, I, I, P, I]),
     "sdxl_test_repack_conv": (I, [P, P, I, I, I, I, P, I, I, I]),
     "sdxl_test_transpose_linear": (I, [P, P, I, I, P, I, I, I]),
@@ -118,6 +119,11 @@ def gemv(inp, in_bstride, Bv, K, W, ldw, bias, add, add_bstride, N, in_silu, out
 def conv_in(x, Bx, B, Cin, H, W, w, bias, Cout, y, add=None, n_add=1) -> None:
     _call("sdxl_test_conv_in", _p(x), int(x.dtype == torch.float32), Bx, B, Cin, H, W, _p(w), _p(bias), Cout, _p(y), _p(add),
           n_add)
+
+
+def conv_in_cat(x, Bx, B, C1, x2, n2, C2, H, W, w, bias, Cout, y) -> None:
+    """The inpainting UNet's first conv: channels [0, C1) from x (f16 or f32), [C1, C1 + C2) from x2 f32 [n2, C2, H, W]."""
+    _call("sdxl_test_conv_in_cat", _p(x), int(x.dtype == torch.float32), Bx, B, C1, _p(x2), n2, C2, H, W, _p(w), _p(bias), Cout, _p(y))
 
 
 def repack_upconv(src, O, I, dst, Ipad) -> None:

@@ -6,7 +6,7 @@ are the ones SURVEY.md section 5 derives from the code and dump scripts.
 """
 from __future__ import annotations
 
-from dataclasses import dataclass, field
+from dataclasses import dataclass, field, replace
 from typing import List, Tuple
 
 
@@ -31,6 +31,16 @@ class UNetConfig:
     def time_embed_dim(self) -> int:
         return 4 * self.model_channels
 
+    @property
+    def is_inpaint(self) -> bool:
+        """The inpainting layout (DESIGN.md §12): the first conv reads the latent, a mask and the masked image's latent."""
+        return self.in_channels > 8 and self.in_channels == 2 * self.out_channels + 1
+
+    @property
+    def latent_channels(self) -> int:
+        """Channels of the latent the forward and the sampler take (the rest of an inpainting UNet's input is attached)."""
+        return self.out_channels if self.is_inpaint else self.in_channels
+
 
 # SDXL base: diffuser.cfg
 SDXL_BASE = UNetConfig(adm_in_channels=2816, model_channels=320, channel_mults=(1, 2, 4),
@@ -44,6 +54,10 @@ TINY = UNetConfig(adm_in_channels=8, model_channels=64, channel_mults=(1, 2, 4),
                   transformer_depths=(0, 1, 2), context_dim=24, is_refiner=False)
 TINY_REFINER = UNetConfig(adm_in_channels=16, model_channels=64, channel_mults=(1, 2, 4),
                           transformer_depths=(0, 1, 1), context_dim=40, is_refiner=True)
+# The inpainting UNet (diffusers stable-diffusion-xl-1.0-inpainting-0.1): SDXL base with the latent, the mask and the masked image's
+# latent as input (4 + 1 + 4 channels), and its tiny counterpart.
+SDXL_INPAINT = replace(SDXL_BASE, in_channels=9)
+TINY_INPAINT = replace(TINY, in_channels=9)
 
 
 @dataclass(frozen=True)

@@ -11,105 +11,42 @@ import torch
 
 from . import _lib
 from ._lib import SdxlError
-from .config import ControlNetConfig, UNetConfig, block_program
+from .config import ControlNetConfig, block_program
+from .diffusers_unet import SDXL_DOWN_BLOCK_TYPES, _put, encoder_config, encoder_name_map, middle_name_map  # noqa: F401
 from .engine import _cfg_struct
 from .lora import read_safetensors
 from .weights import build_pack, controlnet_tensor_specs
 
-SDXL_DOWN_BLOCK_TYPES = ["DownBlock2D", "CrossAttnDownBlock2D", "CrossAttnDownBlock2D"]
 # ControlNet variants this loader does not implement, recognised by a key prefix or substring
 _FOREIGN = [("control_model.", "an SGM/ldm ControlNet checkpoint (convert it to diffusers format)"),
             ("task_embedding", "a ControlNet-Union checkpoint"), ("control_type_proj", "a ControlNet-Union checkpoint"),
             ("transformer_layes", "a ControlNet-Union checkpoint"), ("lora", "a Control-LoRA checkpoint"),
             ("adapter.", "a T2I-Adapter checkpoint"), ("body.", "a T2I-Adapter checkpoint")]
 
-_RES = {"norm1": "norm_in", "conv1": "conv_in", "time_emb_proj": "lin_embed", "norm2": "norm_out", "conv2": "conv_out",
-        "conv_shortcut": "skip_connection"}
-_ATTN = {"to_q": "query", "to_k": "key", "to_v": "value", "to_out.0": "out"}
-
-
 def config_from_diffusers(cfg: Dict) -> ControlNetConfig:
     """ControlNetConfig of a diffusers ControlNetModel config.json; everything this engine does not run is rejected by name."""
     if cfg.get("global_pool_conditions"):
         raise SdxlError("controlnet config: global_pool_conditions = true is not supported")
-    dbt = list(cfg.get("down_block_types", []))
-    if dbt != SDXL_DOWN_BLOCK_TYPES:
-        raise SdxlError(f"controlnet config: down_block_types {dbt} is not SDXL base's {SDXL_DOWN_BLOCK_TYPES}")
-    ch = list(cfg["block_out_channels"])
-    mc = ch[0]
-    heads = cfg.get("num_attention_heads") or cfg.get("attention_head_dim")
-    heads = list(heads) if isinstance(heads, (list, tuple)) else [heads] * len(ch)
-    for lvl, t in enumerate(dbt):
-        if t.startswith("CrossAttn") and ch[lvl] != 64 * heads[lvl]:
-            raise SdxlError(f"controlnet config: attention_head_dim gives head dim {ch[lvl] // heads[lvl]} at level {lvl}; "
-                            "only 64 is supported")
-    tl = cfg.get("transformer_layers_per_block", 1)
-    tl = list(tl) if isinstance(tl, (list, tuple)) else [tl] * len(ch)
-    depths = tuple(tl[lvl] if t.startswith("CrossAttn") else 0 for lvl, t in enumerate(dbt))
-    unet = UNetConfig(adm_in_channels=int(cfg["projection_class_embeddings_input_dim"]), model_channels=mc,
-                      channel_mults=tuple(c // mc for c in ch), transformer_depths=depths, context_dim=int(cfg["cross_attention_dim"]),
-                      in_channels=int(cfg.get("in_channels", 4)))
+    unet = encoder_config(cfg, "controlnet config", int(cfg.get("in_channels", 4)))
     return ControlNetConfig(unet, hint_in_channels=int(cfg.get("conditioning_channels", 3)),
                             hint_block_channels=tuple(cfg.get("conditioning_embedding_out_channels", (16, 32, 96, 256))))
 
 
 def diffusers_name_map(cfg: ControlNetConfig) -> Dict[str, Tuple[str, bool]]:
-    """diffusers key -> (pack name, transpose): Linear weights are [out, in] in diffusers and [in, out] in the pack."""
-    m: Dict[str, Tuple[str, bool]] = {}
+    """diffusers key -> (pack name, transpose): Linear weights are [out, in] in diffusers and [in, out] in the pack. The UNet's
+    encoder half (diffusers_unet.encoder_name_map), the hint encoder, one zero conv per skip and middle_block_out."""
+    def hint_encoder(m):
+        _put(m, "controlnet_cond_embedding.conv_in", "input_hint_block/0")
+        for k in range(2 * (len(cfg.hint_block_channels) - 1)):
+            _put(m, f"controlnet_cond_embedding.blocks.{k}", f"input_hint_block/{2 * k + 2}")
+        _put(m, "controlnet_cond_embedding.conv_out", f"input_hint_block/{4 * len(cfg.hint_block_channels) - 2}")
 
-    def put(src, dst, lin=False):
-        m[f"{src}.weight"] = (f"{dst}/weight", lin)
-        m[f"{src}.bias"] = (f"{dst}/bias", False)
-
-    def res(src, dst, has_skip):
-        for a, b in _RES.items():
-            if a != "conv_shortcut" or has_skip:
-                put(f"{src}.{a}", f"{dst}/{b}", a == "time_emb_proj")
-
-    def st(src, dst, depth):
-        put(f"{src}.norm", f"{dst}/norm")
-        put(f"{src}.proj_in", f"{dst}/proj_in", True)
-        put(f"{src}.proj_out", f"{dst}/proj_out", True)
-        for j in range(depth):
-            s, d = f"{src}.transformer_blocks.{j}", f"{dst}/transformer_{j}"
-            for n in ("norm1", "norm2", "norm3"):
-                put(f"{s}.{n}", f"{d}/{n}")
-            for a in ("attn1", "attn2"):
-                for x, y in _ATTN.items():
-                    if x == "to_out.0":
-                        put(f"{s}.{a}.{x}", f"{d}/{a}/{y}", True)
-                    else:
-                        m[f"{s}.{a}.{x}.weight"] = (f"{d}/{a}/{y}/weight", True)
-            put(f"{s}.ff.net.0.proj", f"{d}/mlp/geglu/proj", True)
-            put(f"{s}.ff.net.2", f"{d}/mlp/lin", True)
-
-    ins, mid, _ = block_program(cfg.unet)
-    put("conv_in", ins[0].path)
-    put("time_embedding.linear_1", "lin1_time_embed", True)
-    put("time_embedding.linear_2", "lin2_time_embed", True)
-    put("add_embedding.linear_1", "lin1_label_embed", True)
-    put("add_embedding.linear_2", "lin2_label_embed", True)
-    put("controlnet_cond_embedding.conv_in", "input_hint_block/0")
-    for k in range(2 * (len(cfg.hint_block_channels) - 1)):
-        put(f"controlnet_cond_embedding.blocks.{k}", f"input_hint_block/{2 * k + 2}")
-    put("controlnet_cond_embedding.conv_out", f"input_hint_block/{4 * len(cfg.hint_block_channels) - 2}")
-    lvl, j = 0, 0   # diffusers numbers the blocks of a level: resnets.{j} / attentions.{j}, then the level's downsampler
-    for b in ins[1:]:
-        if b.kind == "downsample":
-            put(f"down_blocks.{lvl}.downsamplers.0.conv", b.path)
-            lvl, j = lvl + 1, 0
-            continue
-        tr = b.kind == "resnet_transformer"
-        res(f"down_blocks.{lvl}.resnets.{j}", f"{b.path}/res" if tr else b.path, b.c_in != b.c_out)
-        if tr:
-            st(f"down_blocks.{lvl}.attentions.{j}", f"{b.path}/transformer", b.depth)
-        j += 1
+    m = encoder_name_map(cfg.unet, hint_encoder)
+    ins, _, _ = block_program(cfg.unet)
     for i in range(len(ins)):
-        put(f"controlnet_down_blocks.{i}", f"zero_convs/{i}")
-    res("mid_block.resnets.0", f"{mid.path}/res1", False)
-    st("mid_block.attentions.0", f"{mid.path}/transformer", mid.depth)
-    res("mid_block.resnets.1", f"{mid.path}/res2", False)
-    put("controlnet_mid_block", "middle_block_out")
+        _put(m, f"controlnet_down_blocks.{i}", f"zero_convs/{i}")
+    middle_name_map(m, cfg.unet)
+    _put(m, "controlnet_mid_block", "middle_block_out")
     return m
 
 

@@ -322,6 +322,34 @@ class Diffuser:
         from .t2i_adapter import set_t2i_adapters
         set_t2i_adapters(self, adapters, t_min)
 
+    def set_inpaint_condition(self, cond: Optional[torch.Tensor]) -> None:
+        """Attaches the inpainting UNet's condition (sdxl_unet_set_inpaint_condition); None detaches. cond: f32
+        [n, in_channels - out_channels, h, w] (pipeline.prepare_inpaint_condition): the mask (1 = repaint), then the masked image's
+        latent; image b of a batch uses row b % n, at every step until it is replaced or detached."""
+        ctx = self.ctx
+        s = None
+        if cond is not None:
+            if cond.dim() != 4:
+                raise SdxlError(f"inpainting condition must be f32 [n, C, h, w], got {tuple(cond.shape)}")
+            if self.cfg.is_inpaint and cond.shape[1] != self.cfg.in_channels - self.cfg.out_channels:
+                raise SdxlError(f"inpainting condition must have {self.cfg.in_channels - self.cfg.out_channels} channels, got "
+                                f"{tuple(cond.shape)}")
+            cond = cond.to(ctx.device, torch.float32).contiguous()
+            s = _lib.InpaintCondition()
+            s.cond, s.on_host, s.n = cond.data_ptr(), 0, cond.shape[0]
+            s.height, s.width = 8 * cond.shape[2], 8 * cond.shape[3]
+        ctx.enter()
+        ctx.check(ctx.lib.sdxl_unet_set_inpaint_condition(self.h, None if s is None else C.byref(s)), "sdxl_unet_set_inpaint_condition")
+        ctx.leave()
+
+    @classmethod
+    def from_diffusers_dir(cls, ctx: Context, path: str) -> "Diffuser":
+        """A diffusers UNet2DConditionModel directory (the `unet/` folder of an SDXL pipeline, base or inpainting): config.json +
+        diffusion_pytorch_model[.fp16].safetensors (diffusers_unet.from_diffusers)."""
+        from .diffusers_unet import read_diffusers_dir
+        cfg, w = read_diffusers_dir(path)
+        return cls(ctx, cfg, w)
+
     # ---- UNet::forward -------------------------------------------------------------------------
     def set_conditioning(self, context: torch.Tensor, label: torch.Tensor) -> None:
         ctx = self.ctx
@@ -402,7 +430,7 @@ class Diffuser:
         ref = prep(ref, torch.float32)
         mask = prep(mask, torch.uint8)
         n_noise = 0 if noise is None else (noise.shape[0] if noise.dim() == 5 else 1)
-        out = torch.empty(s.n_batch, self.cfg.in_channels, h, w, device=dev, dtype=torch.float32)
+        out = torch.empty(s.n_batch, self.cfg.latent_channels, h, w, device=dev, dtype=torch.float32)
         ctx.enter()
         rc = ctx.lib.sdxl_sample_latent(self.h, C.byref(s), float(guidance), n_steps, step_start, _ptr(init_latent),
                                         _ptr(noise), n_noise, seed, _ptr(ref), _ptr(mask), _ptr(out))

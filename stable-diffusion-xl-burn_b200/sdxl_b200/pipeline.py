@@ -25,6 +25,30 @@ def make_inpaint_mask(img_hw: Tuple[int, int], latent_hw: Tuple[int, int], crop_
     return torch.from_numpy(out).bool().unsqueeze(0)
 
 
+def prepare_inpaint_condition(decoder, rgb: torch.Tensor, pixel_mask: torch.Tensor) -> torch.Tensor:
+    """The inpainting UNet's condition (Diffuser.set_inpaint_condition) of images rgb u8 [n, H, W, 3] and pixel_mask bool [n, 1, H, W]
+    (True = repaint), as diffusers' StableDiffusionXLInpaintPipeline.prepare_mask_latents builds it: the image normalised to [-1, 1],
+    masked = image * (mask < 0.5), the masked image's latent decoder.encode_image(masked) and the mask channel F.interpolate(mask,
+    (H/8, W/8)) (nearest: mask[8i, 8j]; the latent's extent for a VAE with another factor). Returns f32 [n, 1 + latent_channels,
+    H/8, W/8] on the decoder's device.
+    One difference: diffusers samples the VAE posterior with the call's generator, this engine's encoder returns its mean (as the
+    reference's does), so the masked latent is deterministic."""
+    import torch.nn.functional as F
+    from ._lib import SdxlError
+    if rgb.dim() != 4 or rgb.shape[3] != 3 or rgb.dtype != torch.uint8:
+        raise SdxlError(f"inpainting image must be u8 [n, H, W, 3], got {rgb.dtype} {tuple(rgb.shape)}")
+    n, H, W, _ = rgb.shape
+    if tuple(pixel_mask.shape) != (n, 1, H, W):
+        raise SdxlError(f"inpainting mask must be [{n}, 1, {H}, {W}], got {tuple(pixel_mask.shape)}")
+    dev = decoder.ctx.device
+    image = rgb.to(dev).permute(0, 3, 1, 2).to(torch.float32) / 255.0 * 2.0 - 1.0
+    mask = pixel_mask.to(dev).to(torch.float32)
+    masked = image * (mask < 0.5)
+    masked_lat = decoder.encode_image(masked.contiguous())
+    mask_lat = F.interpolate(mask, size=tuple(masked_lat.shape[2:]))   # the latent's extent: H/8 x W/8 for the SDXL VAE
+    return torch.cat([mask_lat, masked_lat], dim=1)
+
+
 def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_steps: int = 30, refiner=None,
            reference_rgb: Optional[torch.Tensor] = None, crop: Sequence[Optional[int]] = (None, None, None, None), crop_out: bool = False,
            resolution: Tuple[int, int] = (1024, 1024), seed: int = 0, noise: Optional[torch.Tensor] = None,
@@ -32,7 +56,9 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
            t2i_adapters: Optional[Sequence] = None, t2i_factor: float = 1.0) -> torch.Tensor:
     """One image, like `sample --prompt ... [--reference-img ... --crop-* ...] [--use-refiner]`.
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
-    bottom) in pixels. loras: [(kohya .safetensors path / bytes / tensor dict, scale), ...] merged into the base UNet and both
+    bottom) in pixels. With an inpainting UNet (cfg.is_inpaint, DESIGN.md §12) reference_rgb is required: the crop window becomes the
+    pixel mask (1 = repaint), prepare_inpaint_condition's condition is attached for the call and the latent is sampled from noise
+    without blending. loras: [(kohya .safetensors path / bytes / tensor dict, scale), ...] merged into the base UNet and both
     text encoders for this call (the refiner is left alone) and removed again afterwards, which also clears any adapter set
     those models had. controls: [(ControlNet, image u8 [1, H, W, 3] or f32 [1, 3, H, W], scale), ...] attached to the base UNet
     for this call and detached afterwards (the refiner is left alone). image_prompt: (IPAdapter, ClipVisionEncoder, images u8
@@ -85,11 +111,25 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
 
 
 def _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution, seed, noise):
+    inpaint_unet = diffuser.cfg.is_inpaint
+    if inpaint_unet and reference_rgb is None:
+        raise _lib.SdxlError("sample: an inpainting UNet needs reference_rgb (the image to repaint)")
     if reference_rgb is not None:
         resolution = (int(reference_rgb.shape[1]), int(reference_rgb.shape[2]))        # main.rs:225-229: orig_dims
     size = [int(resolution[0]), int(resolution[1])]
     cond = embedder.text_to_conditioning(prompt, size, [0, 0], size)                     # main.rs:231-235: size, crop = 0, ar = size
-    if reference_rgb is not None:
+    if inpaint_unet:
+        # the UNet sees the mask and the masked image at every step and samples from noise, without blending (as diffusers does
+        # for 9-channel UNets); the crop window at scale 1 is the exact pixel box, 1 = repaint
+        pixel_mask = make_inpaint_mask(resolution, resolution, *crop, crop_out=crop_out, n_channels=1)
+        c = prepare_inpaint_condition(decoder, reference_rgb, pixel_mask)
+        cond.resolution = (8 * int(c.shape[2]), 8 * int(c.shape[3]))
+        diffuser.set_inpaint_condition(c)
+        try:
+            latent = diffuser.sample_latent(cond, guidance, n_steps, noise=noise, seed=seed)
+        finally:
+            diffuser.set_inpaint_condition(None)
+    elif reference_rgb is not None:
         ref_latent = decoder.image_to_latent(reference_rgb)                              # main.rs:158
         lh, lw = int(ref_latent.shape[2]), int(ref_latent.shape[3])
         cond.resolution = (8 * lh, 8 * lw)   # the sampler's latent extent follows the encoded reference (== the image size for the x8 SDXL VAE)
