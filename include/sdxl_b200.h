@@ -459,6 +459,32 @@ typedef struct sdxl_image_prompt {
  * n_images rewrites tokens, K/V and scales in place (same launch plan and CUDA graph); any other change rebuilds the plan at the
  * next forward. The image K/V are recomputed whenever the conditioning is set. An attached ControlNet's attentions see text only. */
 SDXL_API int sdxl_unet_set_image_prompt(sdxl_unet* unet, const sdxl_image_prompt* prompt);
+/* Image-prompt sets (DESIGN.md §13): up to SDXL_MAX_IMAGE_PROMPTS prompts at once, each optionally limited to a region per image.
+ * Every UNet cross-attention computes, for query t of the T = h_l * w_l queries of its level (raster order),
+ *   h = softmax(q K_txt^T / 8) V_txt
+ *   for each prompt p in array order:
+ *     unmasked: h += s_p,blk * softmax(q K_p^T / 8) V_p                            (all its images' tokens in one softmax)
+ *     masked:   h += sum over images i of s_p,blk * m_p,i,l[t] * softmax(q K_p,i^T / 8) V_p,i   (one softmax per image)
+ * where m_p,i,l is mask plane i resized to the level as diffusers' IPAdapterMaskProcessor.downsample does: ratio = width / height,
+ * mh = int(sqrt(T / ratio)), mh += (T % mh != 0), mw = T / mh (both kept >= 1), bicubic resize (torch's, A = -0.75, align_corners
+ * false, no clamping) to (mh, mw), flattened row-major and zero-padded or cut to T. The masks are used as given: diffusers binarises
+ * them at 0.5 first. A source is one unmasked prompt or one image of a masked prompt; at most SDXL_MAX_IP_SOURCES per set. */
+#define SDXL_MAX_IMAGE_PROMPTS 4
+#define SDXL_MAX_IP_SOURCES 8
+typedef struct sdxl_ip_mask {
+  const float* mask;               /* f32 [n_images, height, width] of its prompt, shared by every batch row and both CFG halves;
+                                      NULL: the prompt is unmasked */
+  int32_t on_host;                 /* mask is host memory; borrowed for the call */
+  int32_t height, width;           /* pixels: positive multiples of 8; the latent must be height/8 x width/8 */
+} sdxl_ip_mask;
+/* Attaches n image prompts (n = 0 detaches); masks is NULL or n entries. Each prompt follows sdxl_unet_set_image_prompt's rules (its
+ * own adapter, n_batch, n_images, scales and negatives; row rule per prompt). Everything is validated before anything changes (each
+ * prompt as sdxl_unet_set_image_prompt does, n <= SDXL_MAX_IMAGE_PROMPTS, at most SDXL_MAX_IP_SOURCES sources, finite mask values,
+ * mask height and width positive multiples of 8): on failure the previous set stays. A call with the same adapters, n_batch, n_images,
+ * mask presence and mask sizes rewrites tokens, K/V, scales and masks in place (same launch plan and CUDA graph); any other call
+ * rebuilds the plan at the next forward. A forward or sampler_begin on a latent other than a masked prompt's height/8 x width/8 is
+ * refused. sdxl_unet_set_image_prompt(u, p) is sdxl_unet_set_image_prompts(u, p ? 1 : 0, p, NULL). */
+SDXL_API int sdxl_unet_set_image_prompts(sdxl_unet* unet, int n, const sdxl_image_prompt* prompts, const sdxl_ip_mask* masks);
 /* Test aid: tokens f16 [n * tokens_per_image, context_dim] of embeds f32 [n, D]; both host memory if on_host. A Plus adapter is
  * refused (use sdxl_ip_adapter_resample). */
 SDXL_API int sdxl_ip_adapter_project(sdxl_ip_adapter* adapter, int n, const float* embeds, int on_host, sdxl_half* tokens_out);

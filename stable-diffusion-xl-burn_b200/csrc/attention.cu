@@ -8,7 +8,7 @@
 // One CTA per (batch, head, 128-query tile): two consumer warpgroups own 64 query rows each, one producer warp streams the
 // 128-key K / V blocks through a TMA ring. The running max is exact per key block (the row is rescaled when it grows), so
 // every probability is <= 1 before the f16 rounding.
-// attention_kernel<true> adds IP-Adapter's second key/value source (DESIGN.md §9).
+// attention_kernel<true> adds IP-Adapter's image key/value sources (DESIGN.md §9, §13).
 #include <stdlib.h>
 
 #include "common.cuh"
@@ -88,9 +88,24 @@ __device__ __forceinline__ void attn_key_block(float (&o)[32], float (&m)[2], fl
   if (lane == 0) mbar_arrive(&kv_empty[st]);   // this warp is done with K_j / V_j
 }
 
-// kIp: decoupled cross-attention (IP-Adapter). After the text keys the producer streams the image-prompt keys (tmKip / tmVip,
-// S_ip rows) through the same ring; the consumers keep O_txt / l_txt, restart the online softmax on the image keys and write
-// f16(O_txt / l_txt + s * O_ip / l_ip), s = *ip_scale (device memory: a scale change keeps the CUDA graph valid).
+// Image source k of p (source 0 is the AttnParams fields that predate the others; K and V may have separate maps there).
+struct IpSrc {
+  const CUtensorMap* tk;
+  const CUtensorMap* tv;
+  int S, k_col0, v_col0;
+  const float* scale;
+  const float* mask;
+};
+__device__ __forceinline__ IpSrc ip_source(const AttnParams& p, int k) {
+  if (k == 0) return {&p.tmKip, &p.tmVip, p.S_ip, p.k_ip_col0, p.v_ip_col0, p.ip_scale, p.ip_mask};
+  const AttnIpSource& s = p.ip_src[k - 1];
+  return {&s.tm, &s.tm, s.S, s.k_col0, s.v_col0, s.scale, s.mask};
+}
+
+// kIp: decoupled cross-attention (IP-Adapter, DESIGN.md §9, §13). After the text keys the producer streams the keys of each of the
+// n_src image sources in turn through the same ring; the consumers keep acc = O_txt / l_txt, restart the online softmax on each
+// source's keys and add acc = fmaf(s * m[t], O_k / l_k, acc), s = *scale and m = mask[t] (1 without a mask) read from device
+// memory, so rewriting them keeps the CUDA graph valid. One unmasked source is the two-source form: f16(O_txt / l_txt + s O / l).
 template <bool kIp>
 __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid_constant__ AttnParams p) {
   extern __shared__ uint8_t smem_raw[];
@@ -115,6 +130,7 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
     if constexpr (kIp) {
       tma_prefetch_desc(&p.tmKip);
       tma_prefetch_desc(&p.tmVip);
+      for (int k = 1; k < p.n_src; ++k) tma_prefetch_desc(&p.ip_src[k - 1].tm);
     }
     mbar_init(q_full, 1);
     for (int i = 0; i < kKvStages; ++i) { mbar_init(&kv_full[i], 1); mbar_init(&kv_empty[i], kConsumerWarps); }
@@ -137,13 +153,17 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
       tma_load_3d(sV + st * kTileBytes, &p.tmV, &kv_full[st], p.v_col0 + head * 64, j * 128, b);
     }
     if constexpr (kIp) {
-      const int nblk_ip = (p.S_ip + 127) / 128;
-      for (int j = nblk; j < nblk + nblk_ip; ++j) {
-        const int st = j % kKvStages;
-        mbar_wait_nocall(&kv_empty[st], ((j / kKvStages) & 1) ^ 1);
-        mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
-        tma_load_3d(sK + st * kTileBytes, &p.tmKip, &kv_full[st], p.k_ip_col0 + head * 64, (j - nblk) * 128, b);
-        tma_load_3d(sV + st * kTileBytes, &p.tmVip, &kv_full[st], p.v_ip_col0 + head * 64, (j - nblk) * 128, b);
+      int j = nblk;
+      for (int k = 0; k < p.n_src; ++k) {
+        const IpSrc s = ip_source(p, k);
+        const int nb = (s.S + 127) / 128;
+        for (int kb = 0; kb < nb; ++kb, ++j) {
+          const int st = j % kKvStages;
+          mbar_wait_nocall(&kv_empty[st], ((j / kKvStages) & 1) ^ 1);
+          mbar_expect_tx(&kv_full[st], 2 * kTileBytes);
+          tma_load_3d(sK + st * kTileBytes, s.tk, &kv_full[st], s.k_col0 + head * 64, kb * 128, b);
+          tma_load_3d(sV + st * kTileBytes, s.tv, &kv_full[st], s.v_col0 + head * 64, kb * 128, b);
+        }
       }
     }
     return;
@@ -212,9 +232,9 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
     wg_wait<0>();
     if (lane == 0) mbar_arrive(&kv_empty[st]);   // this warp is done with K_j / V_j
   }
-  float ot[kIp ? 32 : 1];   // O_txt / l_txt
-  float s_ip = 0.f;
+  const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
   if constexpr (kIp) {
+    float acc[32];   // O_txt / l_txt, then + s_k m_k[t] O_k / l_k per source
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       float lt = l[h];
@@ -223,39 +243,94 @@ __global__ void __launch_bounds__(kAttnThreads, 1) attention_kernel(const __grid
       const float inv = 1.0f / lt;
 #pragma unroll
       for (int jj = 0; jj < 8; ++jj) {
-        ot[4 * jj + 2 * h] = o[4 * jj + 2 * h] * inv;
-        ot[4 * jj + 2 * h + 1] = o[4 * jj + 2 * h + 1] * inv;
+        acc[4 * jj + 2 * h] = o[4 * jj + 2 * h] * inv;
+        acc[4 * jj + 2 * h + 1] = o[4 * jj + 2 * h + 1] * inv;
       }
-      m[h] = -INFINITY;
-      l[h] = 0.f;
+    }
+    int j = nblk;
+    for (int k = 0; k < p.n_src; ++k) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) { m[h] = -INFINITY; l[h] = 0.f; }
+#pragma unroll
+      for (int i = 0; i < 32; ++i) o[i] = 0.f;
+      const int S = ip_source(p, k).S;
+      for (int kb = 0; kb * 128 < S; ++kb, ++j) attn_key_block(o, m, l, q_addr, sK, sV, kv_full, kv_empty, j, kb, S, sl2e, lane);
+      const IpSrc s = ip_source(p, k);   // read after the key blocks: nothing but S stays live across them
+      const float sk = *s.scale;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float lt = l[h];
+        lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+        lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+        const float inv = 1.0f / lt;
+        const int t = qt * 128 + r + 8 * h;
+        const float w = (s.mask && t < p.T) ? sk * s.mask[t] : sk;
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj) {
+          acc[4 * jj + 2 * h] = fmaf(w, o[4 * jj + 2 * h] * inv, acc[4 * jj + 2 * h]);
+          acc[4 * jj + 2 * h + 1] = fmaf(w, o[4 * jj + 2 * h + 1] * inv, acc[4 * jj + 2 * h + 1]);
+        }
+      }
     }
 #pragma unroll
-    for (int i = 0; i < 32; ++i) o[i] = 0.f;
-    const int nblk_ip = (p.S_ip + 127) / 128;
-    for (int j = nblk; j < nblk + nblk_ip; ++j) attn_key_block(o, m, l, q_addr, sK, sV, kv_full, kv_empty, j, j - nblk, p.S_ip, sl2e, lane);
-    s_ip = *p.ip_scale;
-  }
-  // ---- write-back: O / l -> f16
-  const int r = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    for (int h = 0; h < 2; ++h) {
+      const int t = qt * 128 + r + 8 * h;
+      if (t < p.T) {
+        __half* out = p.out + ((size_t)b * p.T + t) * p.ldo + head * 64 + 2 * (lane & 3);
 #pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    float lt = l[h];
-    lt += __shfl_xor_sync(0xffffffffu, lt, 1);
-    lt += __shfl_xor_sync(0xffffffffu, lt, 2);
-    const float inv = 1.0f / lt;
-    const int t = qt * 128 + r + 8 * h;
-    if (t < p.T) {
-      __half* out = p.out + ((size_t)b * p.T + t) * p.ldo + head * 64 + 2 * (lane & 3);
+        for (int jj = 0; jj < 8; ++jj)
+          *reinterpret_cast<__half2*>(out + 8 * jj) = __floats2half2_rn(acc[4 * jj + 2 * h], acc[4 * jj + 2 * h + 1]);
+      }
+    }
+  } else {
+    // ---- write-back: O / l -> f16
 #pragma unroll
-      for (int jj = 0; jj < 8; ++jj) {
-        if constexpr (kIp)
-          *reinterpret_cast<__half2*>(out + 8 * jj) = __floats2half2_rn(fmaf(s_ip, o[4 * jj + 2 * h] * inv, ot[4 * jj + 2 * h]),
-                                                                        fmaf(s_ip, o[4 * jj + 2 * h + 1] * inv, ot[4 * jj + 2 * h + 1]));
-        else
+    for (int h = 0; h < 2; ++h) {
+      float lt = l[h];
+      lt += __shfl_xor_sync(0xffffffffu, lt, 1);
+      lt += __shfl_xor_sync(0xffffffffu, lt, 2);
+      const float inv = 1.0f / lt;
+      const int t = qt * 128 + r + 8 * h;
+      if (t < p.T) {
+        __half* out = p.out + ((size_t)b * p.T + t) * p.ldo + head * 64 + 2 * (lane & 3);
+#pragma unroll
+        for (int jj = 0; jj < 8; ++jj)
           *reinterpret_cast<__half2*>(out + 8 * jj) = __floats2half2_rn(o[4 * jj + 2 * h] * inv, o[4 * jj + 2 * h + 1] * inv);
       }
     }
   }
+}
+
+// Bicubic resize of one f32 mask plane [H, W] to (mh, mw), written flat into out[T]: zero past mh * mw, cut at T. torch's
+// F.interpolate(mode="bicubic", align_corners=False): A = -0.75, source x = (W / mw) (ox + 0.5) - 0.5, taps clamped to the
+// plane, no antialias, no clamping of the result.
+__device__ __forceinline__ float cubic_w1(float x) { return ((-0.75f + 2.f) * x - (-0.75f + 3.f)) * x * x + 1.f; }
+__device__ __forceinline__ float cubic_w2(float x) { return ((-0.75f * x - 5.f * -0.75f) * x + 8.f * -0.75f) * x - 4.f * -0.75f; }
+__device__ __forceinline__ float cubic_1d(float x0, float x1, float x2, float x3, float t) {
+  return x0 * cubic_w2(t + 1.f) + x1 * cubic_w1(t) + x2 * cubic_w1(1.f - t) + x3 * cubic_w2(2.f - t);
+}
+__global__ void ip_mask_resize_kernel(const float* __restrict__ mask, int H, int W, int mh, int mw, int T, float* __restrict__ out) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= T) return;
+  if (i >= mh * mw) { out[i] = 0.f; return; }
+  const int oy = i / mw, ox = i % mw;
+  const float ry = (float)H / mh * (oy + 0.5f) - 0.5f, rx = (float)W / mw * (ox + 0.5f) - 0.5f;
+  const int iy = (int)floorf(ry), ix = (int)floorf(rx);
+  const float ty = ry - iy, tx = rx - ix;
+  float row[4];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float* m = mask + (size_t)min(max(iy - 1 + k, 0), H - 1) * W;
+    row[k] = cubic_1d(m[min(max(ix - 1, 0), W - 1)], m[min(max(ix, 0), W - 1)], m[min(max(ix + 1, 0), W - 1)],
+                      m[min(max(ix + 2, 0), W - 1)], tx);
+  }
+  out[i] = cubic_1d(row[0], row[1], row[2], row[3], ty);
+}
+
+int ip_mask_resize_launch(cudaStream_t st, const float* mask, int H, int W, int mh, int mw, int T, float* out) {
+  if (H < 1 || W < 1 || mh < 1 || mw < 1 || T < 1) return 2002;
+  ip_mask_resize_kernel<<<(T + 255) / 256, 256, 0, st>>>(mask, H, W, mh, mw, T, out);
+  return (int)cudaGetLastError();
 }
 
 // Per-device launch state (several devices may be driven from one process: the opt-in to > 48 KB of dynamic shared memory
@@ -264,7 +339,9 @@ static bool g_attn_attr[2][64];
 int attention_launch(cudaStream_t st, const AttnParams& p) {
   if (p.T < 1 || p.S < 1 || (p.ldo & 1)) return 2002;
   const bool ip = p.S_ip > 0;
-  if (ip && !p.ip_scale) return 2002;
+  if (ip && (!p.ip_scale || p.n_src < 1 || p.n_src > ATTN_MAX_SRC)) return 2002;
+  for (int k = 1; ip && k < p.n_src; ++k)
+    if (p.ip_src[k - 1].S < 1 || !p.ip_src[k - 1].scale) return 2002;
   auto kernel = ip ? attention_kernel<true> : attention_kernel<false>;
   int r = smem_optin(kernel, kAttnSmem, g_attn_attr[ip]);
   if (r) return r;

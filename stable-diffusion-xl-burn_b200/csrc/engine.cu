@@ -215,7 +215,7 @@ struct sdxl_unet : EncoderHalf {
   int t_slot = 0;              // ring position in t_pinned (per model: independent contexts never share it)
   AdapterState lora;           // LoRA-able weight slots, backups of merged layers (sdxl_unet_set_adapters)
   std::vector<std::unique_ptr<ControlAttach>> controls;   // sdxl_unet_set_controls, in call order
-  std::unique_ptr<IpAttach> ip;   // sdxl_unet_set_image_prompt
+  std::unique_ptr<IpAttach> ip;   // sdxl_unet_set_image_prompts
   std::unique_ptr<T2IAttach> t2i; // sdxl_unet_set_t2i_adapters
   std::unique_ptr<InpaintAttach> inpaint;   // sdxl_unet_set_inpaint_condition
   uint64_t plan_builds = 0;
@@ -262,25 +262,46 @@ struct sdxl_ip_adapter {
   bool plus() const { return cfg.resampler_depth > 0; }
 };
 
-// The image prompt's token rows for one conditioning batch and their K/V.
+// One image prompt's token rows for one conditioning batch and their K/V, source-major: [n_sources, condB, S_ip / n_sources, ...]
+// (an unmasked prompt is one source of S_ip tokens; a masked one is one source per image), so each source is a dense batch of rows.
 struct IpRows {
   Arena mem;
   int condB = 0;
-  __half* rows = nullptr;      // [condB, S_ip, context_dim]
+  __half* rows = nullptr;      // [condB * S_ip, context_dim]
   std::vector<__half*> kv;     // per transformer block [condB * S_ip, 2C]
 };
 
-// An attached image prompt: the projected tokens of the prompts and of the negatives, the per-block scales, and the image K/V
-// hoisted for the current conditioning rows.
-struct IpAttach {
+// One prompt of the attached image-prompt set: the projected tokens of the prompts and of the negatives, the per-block scales,
+// the masks resized to every level's queries, and the image K/V hoisted for the current conditioning rows.
+struct IpPrompt {
   const sdxl_ip_adapter* ad = nullptr;
   int n_batch = 0, n_images = 0, S_ip = 0;
-  Arena mem;
+  int mask_h = 0, mask_w = 0;  // pixel extent of the masks; 0: unmasked
   __half* tok_pos = nullptr;   // [n_batch, S_ip, context_dim]
   __half* tok_neg = nullptr;   // [n_batch, S_ip, context_dim]
   float* scales = nullptr;     // one per transformer block, read by the attention kernel
+  float* masks = nullptr;      // masked: per image, per level l the f32 [(h >> l) * (w >> l)] query weights (ip_mask_off)
   IpRows cond;
+  int n_sources() const { return mask_h ? n_images : 1; }
 };
+
+// The attached image-prompt set (sdxl_unet_set_image_prompts), in call order.
+struct IpAttach {
+  Arena mem;                   // every prompt's tokens, scales and masks
+  std::vector<IpPrompt> prompts;
+};
+
+// Offset in IpPrompt::masks of image i's weights at level l of a UNet with n_levels levels (ip_mask_off(a, n, n_images, 0): the
+// floats of all images).
+static size_t ip_mask_off(const IpPrompt& a, int n_levels, int i, int l) {
+  const int h = a.mask_h / 8, w = a.mask_w / 8;
+  size_t per = 0, off = 0;
+  for (int k = 0; k < n_levels; ++k) {
+    if (k == l) off = per;
+    per += (size_t)(h >> k) * (w >> k);
+  }
+  return (size_t)i * per + off;
+}
 
 // T2I-Adapter (DESIGN.md §11, diffusers FullAdapterXL): conv_in on the pixel-unshuffled hint, then per level k an optional 1x1 in_conv
 // (k = 1, 2) and n_res_blocks resnets x + block2(relu(block1(x))).
@@ -852,12 +873,18 @@ struct UNetPlanBuilder : PlanBuilder {
       linear(s_a16, M, b.q2, IGEMM_LINEAR, s_q, 0, C, nullptr, 0);
       attn(s_q, C, 0, cond->kv[kv_index], 2 * C, 0, C, T, cond->n_ctx, s.n_head, s_ao, C, sl2e);
       P->flops += 2.0 * Bf * cond->n_ctx * (double)b.kv2.K * b.kv2.N;  // hoisted K/V projections (algorithmic work)
-      // an attached image prompt adds its K/V source to the UNet's own cross-attentions (a ControlNet's see text only)
-      if (u->ip && cond == &u->cond) {
-        const IpAttach& ip = *u->ip;
-        attn_ip(ip.cond.kv[kv_index], 2 * C, 0, C, ip.S_ip, ip.scales + kv_index);
-        P->flops += 2.0 * Bf * ip.S_ip * (double)ip.ad->kv[kv_index].K * ip.ad->kv[kv_index].N;
-      }
+      // attached image prompts add their K/V sources to the UNet's own cross-attentions (a ControlNet's see text only)
+      if (u->ip && cond == &u->cond)
+        for (const IpPrompt& ip : u->ip->prompts) {
+          const int ns = ip.n_sources(), S = ip.S_ip / ns;
+          int level = 0;
+          while (ip.mask_h && level < u->cfg.n_levels && ((ip.mask_h / 8) >> level != H || (ip.mask_w / 8) >> level != W)) ++level;
+          if (level == u->cfg.n_levels) { err = fail(c, 5021, "image prompt: its masks do not match the latent"); return out; }
+          for (int i = 0; i < ns; ++i)
+            attn_ip(ip.cond.kv[kv_index] + (size_t)i * Bf * S * 2 * C, 2 * C, 0, C, S, ip.scales + kv_index,
+                    ip.mask_h ? ip.masks + ip_mask_off(ip, u->cfg.n_levels, i, level) : nullptr);
+          P->flops += 2.0 * Bf * ip.S_ip * (double)ip.ad->kv[kv_index].K * ip.ad->kv[kv_index].N;
+        }
       kv_index++;
       linear(s_ao, M, b.out2, IGEMM_LINEAR, s_tok, 1, C, s_tok, C);
       // x = x + mlp(norm3(x))
@@ -896,16 +923,22 @@ struct UNetPlanBuilder : PlanBuilder {
     P->ops.push_back(op);
     add_flops(4.0 * Bf * T * (double)S * (n_head * 64));
   }
-  // Turns the attention just pushed into the two-source form: + (*scale) * softmax(q k_ip^T) v_ip, k_ip / v_ip column windows of
-  // kvm [Bf * S_ip, kv_pitch].
-  void attn_ip(const __half* kvm, int kv_pitch, int k_col0, int v_col0, int S_ip, const float* scale) {
+  // Adds an image source to the attention just pushed: + (*scale) * mask[t] * softmax(q k_ip^T) v_ip (mask nullable: 1), k_ip /
+  // v_ip column windows of kvm [Bf * S_ip, kv_pitch].
+  void attn_ip(const __half* kvm, int kv_pitch, int k_col0, int v_col0, int S_ip, const float* scale, const float* mask) {
     if (err) return;
     AttnParams& p = P->ops.back().at;
-    p.S_ip = S_ip; p.k_ip_col0 = k_col0; p.v_ip_col0 = v_col0; p.ip_scale = scale;
-    if (!A->measure) {
-      if (int r = make_tmap_rows(&p.tmKip, kvm, S_ip, Bf, kv_pitch, kv_pitch)) { err = fail(c, r, "tensor map creation failed (attention)"); return; }
-      p.tmVip = p.tmKip;
+    if (p.n_src == ATTN_MAX_SRC) { err = fail(c, 5022, "image prompt: more than %d image sources", ATTN_MAX_SRC); return; }
+    CUtensorMap tm{};
+    if (!A->measure)
+      if (int r = make_tmap_rows(&tm, kvm, S_ip, Bf, kv_pitch, kv_pitch)) { err = fail(c, r, "tensor map creation failed (attention)"); return; }
+    if (p.n_src == 0) {
+      p.S_ip = S_ip; p.k_ip_col0 = k_col0; p.v_ip_col0 = v_col0; p.ip_scale = scale; p.ip_mask = mask;
+      p.tmKip = p.tmVip = tm;
+    } else {
+      p.ip_src[p.n_src - 1] = {tm, S_ip, k_col0, v_col0, scale, mask};
     }
+    p.n_src++;
     const int C = p.n_head * 64;
     P->ops.back().flops_exec += 4.0 * Bf * (double)((p.T + 127) / 128 * 128) * (double)((S_ip + 127) / 128 * 128) * C;
     add_flops(4.0 * Bf * p.T * (double)S_ip * C);
@@ -1051,6 +1084,14 @@ static int inpaint_check(sdxl_unet* u, int n_img, int h, int w) {
   return 0;
 }
 
+// A masked image prompt runs only on the latent its masks cover.
+static int ip_mask_check(sdxl_unet* u, const IpPrompt& a, int h, int w) {
+  if (a.mask_h && (a.mask_h / 8 != h || a.mask_w / 8 != w))
+    return fail(u->ctx, 5021, "image prompt: its masks are %dx%d pixels (latent %dx%d) but the latent is %dx%d", a.mask_h, a.mask_w,
+                a.mask_h / 8, a.mask_w / 8, h, w);
+  return 0;
+}
+
 static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
   sdxl_ctx* c = u->ctx;
   if (u->cond.condB != Bf) return fail(c, 5010, "conditioning is set for batch %d but forward batch is %d (call sdxl_unet_set_conditioning first)", u->cond.condB, Bf);
@@ -1060,7 +1101,11 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
       return fail(c, 5012, "control %zu: its hint is %dx%d pixels (latent %dx%d) but the latent is %dx%d", k, 8 * a.h, 8 * a.w, a.h, a.w, h, w);
     if (Bf % a.n_hint) return fail(c, 5013, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bf, a.n_hint);
   }
-  if (u->ip && u->ip->cond.condB != Bf) return fail(c, 5014, "image prompt: its K/V are hoisted for batch %d but the batch is %d", u->ip->cond.condB, Bf);
+  if (u->ip)
+    for (const IpPrompt& a : u->ip->prompts) {
+      if (a.cond.condB != Bf) return fail(c, 5014, "image prompt: its K/V are hoisted for batch %d but the batch is %d", a.cond.condB, Bf);
+      if (int r = ip_mask_check(u, a, h, w)) return r;
+    }
   if (u->t2i) {
     const T2IAttach& a = *u->t2i;
     if (a.h != h || a.w != w)
@@ -1104,8 +1149,8 @@ static int cond_alloc(sdxl_ctx* c, const EncoderHalf& e, int B, int n_ctx, Hoist
   });
 }
 
-// Allocates the image prompt's row and K/V buffers for conditioning batch B into r (a fresh object, as above).
-static int ip_cond_alloc(sdxl_ctx* c, const IpAttach& a, int B, IpRows& r) {
+// Allocates an image prompt's row and K/V buffers for conditioning batch B into r (a fresh object, as above).
+static int ip_cond_alloc(sdxl_ctx* c, const IpPrompt& a, int B, IpRows& r) {
   const int ctx_dim = a.ad->cfg.unet.context_dim;
   r.condB = B;
   return carve_measured(c, r.mem, 5103, "image-prompt conditioning buffers", [&](Arena& A) {
@@ -1123,12 +1168,18 @@ static int ip_check_batch(sdxl_unet* u, int n_batch /* 0: no prompt */, int B, i
     return fail(u->ctx, 5104, "image prompt: batch %d is not a multiple of its n_batch = %d", n_img, n_batch);
   return 0;
 }
+static int ip_check_batch_all(sdxl_unet* u, int B, int cfg_rows) {
+  if (u->ip)
+    for (const IpPrompt& a : u->ip->prompts)
+      if (int r = ip_check_batch(u, a.n_batch, B, cfg_rows)) return r;
+  return 0;
+}
 
 static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* context_dev, const __half* y_dev, int cfg_rows) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   if (B < 1 || n_ctx < 1) return fail(c, 5100, "bad conditioning shape");
-  if (int r = ip_check_batch(u, u->ip ? u->ip->n_batch : 0, B, cfg_rows)) return r;
+  if (int r = ip_check_batch_all(u, B, cfg_rows)) return r;
   if (u->cond.condB != B || u->cond.n_ctx != n_ctx) {
     // everything sized by (B, n_ctx) is allocated into fresh objects and swapped in only when all of it succeeded: a failure
     // leaves the previous conditioning, and the plan over it, in effect
@@ -1145,8 +1196,8 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
     if (!r) r = cond_alloc(c, *u, B, n_ctx, cond);
     std::vector<HoistedCond> ccond(u->controls.size());
     for (size_t k = 0; k < ccond.size() && !r; ++k) r = cond_alloc(c, *u->controls[k]->net, B, n_ctx, ccond[k]);
-    IpRows ipc;
-    if (!r && u->ip) r = ip_cond_alloc(c, *u->ip, B, ipc);
+    std::vector<IpRows> ipc(u->ip ? u->ip->prompts.size() : 0);
+    for (size_t k = 0; k < ipc.size() && !r; ++k) r = ip_cond_alloc(c, u->ip->prompts[k], B, ipc[k]);
     if (r) return r;
     CU(c, cudaStreamSynchronize(c->stream));   // the old buffers and the plan over them may still be in flight
     u->plan.reset();
@@ -1156,7 +1207,7 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
     u->y32 = y32;
     u->cond = std::move(cond);
     for (size_t k = 0; k < ccond.size(); ++k) u->controls[k]->cond = std::move(ccond[k]);
-    if (u->ip) u->ip->cond = std::move(ipc);
+    for (size_t k = 0; k < ipc.size(); ++k) u->ip->prompts[k].cond = std::move(ipc[k]);
     CU(c, cudaMemsetAsync(u->ctx16, 0, (size_t)B * n_ctx * pitch * 2, c->stream));
   }
   u->cfg_rows = cfg_rows;
@@ -1194,15 +1245,16 @@ static int hoist_model(sdxl_unet* u, const EncoderHalf& e, const HoistedCond& h)
   return project_kv(c, u->ctx16, B * n_ctx, g.context_dim, u->ctx_pitch, lins, h.kv);
 }
 
-// The image prompt's token rows for the current conditioning rows (row rule: include/sdxl_b200.h, sdxl_unet_set_image_prompt)
-// and their K/V for every UNet cross-attention.
-static int ip_hoist(sdxl_unet* u, IpAttach& a) {
+// An image prompt's token rows for the current conditioning rows (row rule: include/sdxl_b200.h, sdxl_unet_set_image_prompt),
+// source-major (IpRows), and their K/V for every UNet cross-attention.
+static int ip_hoist(sdxl_unet* u, IpPrompt& a) {
   sdxl_ctx* c = u->ctx;
-  const int ctx_dim = u->cfg.context_dim, B = a.cond.condB, cr = u->cfg_rows;
-  const size_t row = (size_t)a.S_ip * ctx_dim;
+  const int ctx_dim = u->cfg.context_dim, B = a.cond.condB, cr = u->cfg_rows, ns = a.n_sources();
+  const size_t row = (size_t)a.S_ip * ctx_dim, src_row = row / ns;   // one conditioning row's tokens; one source's part of them
   for (int r = 0; r < B; ++r) {
     const __half* src = (cr && r >= cr) ? a.tok_neg + (size_t)((r - cr) % a.n_batch) * row : a.tok_pos + (size_t)(r % a.n_batch) * row;
-    CU(c, cudaMemcpyAsync(a.cond.rows + (size_t)r * row, src, row * sizeof(__half), cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpy2DAsync(a.cond.rows + (size_t)r * src_row, B * src_row * sizeof(__half), src, src_row * sizeof(__half),
+                            src_row * sizeof(__half), ns, cudaMemcpyDeviceToDevice, c->stream));
   }
   std::vector<const Lin*> lins;
   for (const Lin& L : a.ad->kv) lins.push_back(&L);
@@ -1215,7 +1267,10 @@ static int hoist_conditioning(sdxl_unet* u) {
   if (int r = hoist_model(u, *u, u->cond)) return r;
   for (auto& a : u->controls)
     if (int r = hoist_model(u, *a->net, a->cond)) return r;
-  return u->ip ? ip_hoist(u, *u->ip) : 0;
+  if (u->ip)
+    for (IpPrompt& a : u->ip->prompts)
+      if (int r = ip_hoist(u, a)) return r;
+  return 0;
 }
 
 extern "C" int sdxl_unet_set_conditioning(sdxl_unet* u, int B, int n_ctx, const sdxl_half* context, const sdxl_half* y) {
@@ -1557,14 +1612,32 @@ extern "C" int sdxl_ip_adapter_project(sdxl_ip_adapter* a, int n, const float* e
   return 0;
 }
 
-// Writes the buffers that depend on the prompt's values: the tokens of prompts and negatives, and the per-block scales. Everything
-// is computed into temporaries first and copied into `a` only when all of it has succeeded, so a failure leaves `a` unchanged.
-static int ip_write(sdxl_ctx* c, IpAttach& a, const sdxl_image_prompt& p) {
+// One prompt's values computed into temporaries: the tokens of prompts and negatives, the per-block scales and the masks resized
+// to every level. A set is copied into its attachment (ip_commit) only when every prompt's work has succeeded, so a failure leaves
+// the attached set unchanged.
+struct IpStaged {
+  __half* tp = nullptr;
+  __half* tn = nullptr;
+  float* ts = nullptr;
+  float* tm = nullptr;
+  size_t tok_bytes = 0, mask_floats = 0;
+};
+
+// diffusers' IPAdapterMaskProcessor.downsample grid (mh, mw) for T queries and a mask of H x W pixels, computed in double; both
+// are kept >= 1 where diffusers would divide by zero or make an empty grid (levels of a few latent pixels).
+static void ip_mask_grid(int H, int W, int T, int& mh, int& mw) {
+  const double ratio = (double)W / H;
+  mh = std::max(1, (int)sqrt(T / ratio));
+  mh += T % mh != 0;
+  mw = std::max(1, T / mh);
+}
+
+static int ip_stage(sdxl_ctx* c, int n_levels, const IpPrompt& a, const sdxl_image_prompt& p, const std::vector<float>& mask,
+                    TmpBufs& T, IpStaged& s) {
   const int n = p.n_batch * p.n_images, n_tb = (int)a.ad->kv.size();
-  const size_t tok_bytes = (size_t)a.n_batch * a.S_ip * a.ad->cfg.unet.context_dim * sizeof(__half);
+  s.tok_bytes = (size_t)a.n_batch * a.S_ip * a.ad->cfg.unet.context_dim * sizeof(__half);
   const int rows = a.ad->plus() ? p.seq_len : 1;   // input rows per image: Plus hidden states, or one embedding
   const size_t bytes = (size_t)n * rows * a.ad->cfg.image_embed_dim * sizeof(float);
-  TmpBufs T(c->stream);
   const float* e = p.embeds;
   const float* neg = p.negative_embeds;
   if (p.on_host || !neg) {
@@ -1578,39 +1651,51 @@ static int ip_write(sdxl_ctx* c, IpAttach& a, const sdxl_image_prompt& p) {
     else if (!neg) CU(c, cudaMemsetAsync(d + bytes / sizeof(float), 0, bytes, c->stream));   // diffusers' default negative: zeros
     if (p.on_host || !neg) neg = d + bytes / sizeof(float);
   }
-  __half* tp = (__half*)T.get(tok_bytes);
-  __half* tn = (__half*)T.get(tok_bytes);
-  float* ts = (float*)T.get(n_tb * sizeof(float));
-  if (!tp || !tn || !ts) return fail(c, 4820, "set_image_prompt: cannot allocate the token staging buffers");
+  s.tp = (__half*)T.get(s.tok_bytes);
+  s.tn = (__half*)T.get(s.tok_bytes);
+  s.ts = (float*)T.get(n_tb * sizeof(float));
+  if (!s.tp || !s.tn || !s.ts) return fail(c, 4820, "set_image_prompt: cannot allocate the token staging buffers");
   if (a.ad->plus()) {
-    if (int r = ip_resample(a.ad, n, p.seq_len, e, tp)) return r;
-    if (int r = ip_resample(a.ad, n, p.seq_len, neg, tn)) return r;
+    if (int r = ip_resample(a.ad, n, p.seq_len, e, s.tp)) return r;
+    if (int r = ip_resample(a.ad, n, p.seq_len, neg, s.tn)) return r;
   } else {
-    if (int r = ip_project(a.ad, n, e, tp)) return r;
-    if (int r = ip_project(a.ad, n, neg, tn)) return r;
+    if (int r = ip_project(a.ad, n, e, s.tp)) return r;
+    if (int r = ip_project(a.ad, n, neg, s.tn)) return r;
   }
-  std::vector<float> s(n_tb, p.scale);
-  if (p.block_scales_host) s.assign(p.block_scales_host, p.block_scales_host + n_tb);
-  CU(c, cudaMemcpyAsync(ts, s.data(), s.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));   // s and the caller's host memory; any failure of the work above surfaces here
-  CU(c, cudaMemcpyAsync(a.tok_pos, tp, tok_bytes, cudaMemcpyDeviceToDevice, c->stream));
-  CU(c, cudaMemcpyAsync(a.tok_neg, tn, tok_bytes, cudaMemcpyDeviceToDevice, c->stream));
-  CU(c, cudaMemcpyAsync(a.scales, ts, n_tb * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  std::vector<float> sc(n_tb, p.scale);
+  if (p.block_scales_host) sc.assign(p.block_scales_host, p.block_scales_host + n_tb);
+  CU(c, cudaMemcpyAsync(s.ts, sc.data(), sc.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+  if (a.mask_h) {
+    const int H = a.mask_h, W = a.mask_w;
+    s.mask_floats = ip_mask_off(a, n_levels, a.n_images, 0);
+    float* pix = (float*)T.get(mask.size() * sizeof(float));
+    s.tm = (float*)T.get(s.mask_floats * sizeof(float));
+    if (!pix || !s.tm) return fail(c, 4820, "set_image_prompt: cannot allocate the mask staging buffers");
+    CU(c, cudaMemcpyAsync(pix, mask.data(), mask.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+    for (int i = 0; i < a.n_images; ++i)
+      for (int l = 0; l < n_levels; ++l) {
+        const int Tl = ((H / 8) >> l) * ((W / 8) >> l);
+        if (Tl < 1) continue;
+        int mh, mw;
+        ip_mask_grid(H, W, Tl, mh, mw);
+        KL(c, ip_mask_resize_launch(c->stream, pix + (size_t)i * H * W, H, W, mh, mw, Tl, s.tm + ip_mask_off(a, n_levels, i, l)));
+      }
+  }
+  CU(c, cudaStreamSynchronize(c->stream));   // sc, the mask and the caller's host memory; any failure of the work above surfaces here
   return 0;
 }
 
-extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt* p) {
-  if (!u) return -1;
+static int ip_commit(sdxl_ctx* c, IpPrompt& a, const IpStaged& s) {
+  CU(c, cudaMemcpyAsync(a.tok_pos, s.tp, s.tok_bytes, cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(a.tok_neg, s.tn, s.tok_bytes, cudaMemcpyDeviceToDevice, c->stream));
+  CU(c, cudaMemcpyAsync(a.scales, s.ts, a.ad->kv.size() * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  if (a.mask_h) CU(c, cudaMemcpyAsync(a.masks, s.tm, s.mask_floats * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  return 0;
+}
+
+// The checks of one prompt that need no device work.
+static int ip_prompt_check(sdxl_unet* u, const sdxl_image_prompt* p) {
   sdxl_ctx* c = u->ctx;
-  CU(c, cudaSetDevice(c->device));
-  if (!p) {
-    if (!u->ip) return 0;
-    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
-    u->plan.reset();
-    u->ip.reset();
-    return 0;
-  }
-  // validate everything first: on failure the attached state is unchanged
   const sdxl_ip_adapter* ad = p->adapter;
   if (!ad) return fail(c, 4830, "set_image_prompt: null adapter");
   if (ad->ctx != c) return fail(c, 4831, "set_image_prompt: the adapter was created on another sdxl_ctx");
@@ -1632,35 +1717,116 @@ extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt*
   if (p->block_scales_host)
     for (int i = 0; i < n_tb; ++i)
       if (!isfinite(p->block_scales_host[i])) return fail(c, 4837, "set_image_prompt: block scale %d is not finite", i);
+  if (u->cond.condB > 0)
+    if (int r = ip_check_batch(u, p->n_batch, u->cond.condB, u->cfg_rows)) return r;
+  return 0;
+}
+
+// Reads prompt k's mask planes [n_images, height, width] into host memory and checks them.
+static int ip_mask_read(sdxl_ctx* c, const sdxl_ip_mask& m, int n_images, int k, std::vector<float>& host) {
+  if (m.height < 8 || m.width < 8 || m.height % 8 || m.width % 8 || m.height > 16384 || m.width > 16384)
+    return fail(c, 4843, "set_image_prompts: mask %d is %dx%d pixels; height and width must be positive multiples of 8 up to 16384", k,
+                m.height, m.width);
+  host.resize((size_t)n_images * m.height * m.width);
+  if (m.on_host) {
+    memcpy(host.data(), m.mask, host.size() * sizeof(float));
+  } else {
+    CU(c, cudaMemcpyAsync(host.data(), m.mask, host.size() * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));
+  }
+  for (size_t i = 0; i < host.size(); ++i)
+    if (!isfinite(host[i])) return fail(c, 4844, "set_image_prompts: mask %d has a non-finite value at element %zu", k, i);
+  return 0;
+}
+
+extern "C" int sdxl_unet_set_image_prompts(sdxl_unet* u, int n, const sdxl_image_prompt* prompts, const sdxl_ip_mask* masks) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  if (n < 0 || n > SDXL_MAX_IMAGE_PROMPTS)
+    return fail(c, 4841, "set_image_prompts: n = %d outside [0, %d]", n, SDXL_MAX_IMAGE_PROMPTS);
+  if (n == 0) {
+    if (!u->ip) return 0;
+    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
+    u->plan.reset();
+    u->ip.reset();
+    return 0;
+  }
+  if (!prompts) return fail(c, -1, "set_image_prompts: null prompts");
+  // validate everything first: on failure the attached set is unchanged
+  const int nl = u->cfg.n_levels;
+  std::vector<IpPrompt> shape(n);
+  std::vector<std::vector<float>> mask(n);
+  int n_src = 0;
+  for (int k = 0; k < n; ++k) {
+    const sdxl_image_prompt& p = prompts[k];
+    if (int r = ip_prompt_check(u, &p)) return r;
+    const sdxl_ip_mask* m = masks && masks[k].mask ? &masks[k] : nullptr;
+    IpPrompt& a = shape[k];
+    a.ad = p.adapter;
+    a.n_batch = p.n_batch;
+    a.n_images = p.n_images;
+    a.S_ip = p.n_images * p.adapter->cfg.tokens_per_image;
+    if (m) {
+      if (int r = ip_mask_read(c, *m, p.n_images, k, mask[k])) return r;
+      a.mask_h = m->height;
+      a.mask_w = m->width;
+    }
+    n_src += a.n_sources();
+  }
+  if (n_src > SDXL_MAX_IP_SOURCES)
+    return fail(c, 4842, "set_image_prompts: %d image sources (one per unmasked prompt, one per image of a masked prompt); at most %d",
+                n_src, SDXL_MAX_IP_SOURCES);
   const int condB = u->cond.condB;
-  if (condB > 0)
-    if (int r = ip_check_batch(u, p->n_batch, condB, u->cfg_rows)) return r;
-  if (u->ip && u->ip->ad == ad && u->ip->n_batch == p->n_batch && u->ip->n_images == p->n_images) {   // same buffers: plan stays
-    if (int r = ip_write(c, *u->ip, *p)) return r;
-    return condB > 0 ? ip_hoist(u, *u->ip) : 0;
+  TmpBufs T(c->stream);
+  std::vector<IpStaged> st(n);
+  bool same = u->ip && u->ip->prompts.size() == (size_t)n;
+  for (int k = 0; same && k < n; ++k) {
+    const IpPrompt &o = u->ip->prompts[k], &a = shape[k];
+    same = o.ad == a.ad && o.n_batch == a.n_batch && o.n_images == a.n_images && o.mask_h == a.mask_h && o.mask_w == a.mask_w;
+  }
+  if (same) {   // same buffers: plan stays
+    for (int k = 0; k < n; ++k)
+      if (int r = ip_stage(c, nl, u->ip->prompts[k], prompts[k], mask[k], T, st[k])) return r;
+    for (int k = 0; k < n; ++k)
+      if (int r = ip_commit(c, u->ip->prompts[k], st[k])) return r;
+    if (condB > 0)
+      for (IpPrompt& a : u->ip->prompts)
+        if (int r = ip_hoist(u, a)) return r;
+    return 0;
   }
   std::unique_ptr<IpAttach> a(new IpAttach());
-  a->ad = ad;
-  a->n_batch = p->n_batch;
-  a->n_images = p->n_images;
-  a->S_ip = p->n_images * ad->cfg.tokens_per_image;
-  const size_t tok = (size_t)p->n_batch * a->S_ip * u->cfg.context_dim;
+  a->prompts = std::move(shape);
   if (int r = carve_measured(c, a->mem, 4838, "set_image_prompt: token buffers", [&](Arena& A) {
-        a->tok_pos = A.get<__half>(tok);
-        a->tok_neg = A.get<__half>(tok);
-        a->scales = A.get<float>(n_tb);
+        for (IpPrompt& q : a->prompts) {
+          const size_t tok = (size_t)q.n_batch * q.S_ip * u->cfg.context_dim;
+          q.tok_pos = A.get<__half>(tok);
+          q.tok_neg = A.get<__half>(tok);
+          q.scales = A.get<float>(q.ad->kv.size());
+          q.masks = q.mask_h ? A.get<float>(ip_mask_off(q, nl, q.n_images, 0)) : nullptr;
+        }
         return 0;
       }))
     return r;
+  for (int k = 0; k < n; ++k) {
+    IpPrompt& q = a->prompts[k];
+    if (condB > 0)
+      if (int r = ip_cond_alloc(c, q, condB, q.cond)) return r;
+    if (int r = ip_stage(c, nl, q, prompts[k], mask[k], T, st[k])) return r;
+  }
+  for (int k = 0; k < n; ++k)
+    if (int r = ip_commit(c, a->prompts[k], st[k])) return r;
   if (condB > 0)
-    if (int r = ip_cond_alloc(c, *a, condB, a->cond)) return r;
-  if (int r = ip_write(c, *a, *p)) return r;
-  if (condB > 0)
-    if (int r = ip_hoist(u, *a)) return r;
+    for (IpPrompt& q : a->prompts)
+      if (int r = ip_hoist(u, q)) return r;
   CU(c, cudaStreamSynchronize(c->stream));   // the old plan and attachment may still be in flight
   u->plan.reset();
   u->ip = std::move(a);
   return 0;
+}
+
+extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt* p) {
+  return sdxl_unet_set_image_prompts(u, p ? 1 : 0, p, nullptr);
 }
 
 // ================================================================================================
@@ -2093,7 +2259,10 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
     if (a.h != h || a.w != w)
       return fail(c, 5207, "T2I-Adapter: its hint is %dx%d pixels but the resolution is %dx%d", 8 * a.h, 8 * a.w, 8 * h, 8 * w);
   }
-  if (int r = ip_check_batch(u, u->ip ? u->ip->n_batch : 0, nfwd * Bimg, nfwd == 2 ? Bimg : 0)) return r;
+  if (int r = ip_check_batch_all(u, nfwd * Bimg, nfwd == 2 ? Bimg : 0)) return r;
+  if (u->ip)
+    for (const IpPrompt& a : u->ip->prompts)
+      if (int r = ip_mask_check(u, a, h, w)) return r;
   if (int r = inpaint_check(u, Bimg, h, w)) return r;
   Sampler* S = u->sampler.get();
   const size_t lat = (size_t)Bimg * latent_channels(g) * h * w;
@@ -2334,7 +2503,7 @@ extern "C" int sdxl_op_ip_attention(sdxl_ctx* c, const sdxl_half* q, const sdxl_
   p.T = T; p.S = S; p.n_head = n_head; p.B = B;
   p.out = (__half*)out; p.ldo = C;
   p.scale_log2e = (float)(1.4426950408889634 / sqrt(64.0));
-  p.S_ip = S_ip; p.ip_scale = s;
+  p.S_ip = S_ip; p.ip_scale = s; p.n_src = 1;
   int r = make_tmap_rows(&p.tmQ, (const __half*)q, T, B, C, C);
   if (!r) r = make_tmap_rows(&p.tmK, (const __half*)k, S, B, C, C);
   if (!r) r = make_tmap_rows(&p.tmV, (const __half*)v, S, B, C, C);

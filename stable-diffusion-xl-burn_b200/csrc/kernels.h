@@ -127,9 +127,16 @@ int igemm_launch(cudaStream_t st, IgemmParams& p);
 int igemm_pick_bn(int m_tiles, int N, int num_sms, bool geglu);
 
 // ------------------------------------------------------------------------------------------------
-// Attention (attention.cu): out[b, t, h*64:(h+1)*64] = softmax(q k^T / 8) v, head dim 64 (+ an optional second source).
+// Attention (attention.cu): out[b, t, h*64:(h+1)*64] = softmax(q k^T / 8) v, head dim 64 (+ optional image sources).
 // q/k/v are column windows of row-major f16 matrices (fused QKV / KV GEMM outputs).
 // ------------------------------------------------------------------------------------------------
+constexpr int ATTN_MAX_SRC = 8;   // image sources per attention (SDXL_MAX_IP_SOURCES)
+struct AttnIpSource {
+  CUtensorMap tm;              // 3D map (64 cols, S rows, batch); K and V are column windows of it
+  int S, k_col0, v_col0;
+  const float* scale;          // device scalar
+  const float* mask;           // device [T] per-query weights, or nullptr
+};
 struct AttnParams {
   CUtensorMap tmQ, tmK, tmV;  // 3D maps (64 cols, rows, batch)
   int T, S, n_head, B;
@@ -143,9 +150,18 @@ struct AttnParams {
   int S_ip;
   int k_ip_col0, v_ip_col0;
   const float* ip_scale;       // device scalar
+  // Several image sources (DESIGN.md §13): the fields above are source 0, ip_src[k - 1] is source k < n_src. Each source adds
+  //   (*scale) * mask[t] * softmax(q k_src^T) v_src          (its own softmax; mask == nullptr: 1)
+  // in source order to the text attention of query row t of every batch row.
+  int n_src;                   // 1 .. ATTN_MAX_SRC when S_ip > 0
+  const float* ip_mask;        // source 0's per-query weights [T] (device), or nullptr
+  AttnIpSource ip_src[ATTN_MAX_SRC - 1];
 };
 int make_tmap_rows(CUtensorMap* tm, const __half* base, int rows_per_batch, int nbatch, int cols, int pitch);
 int attention_launch(cudaStream_t st, const AttnParams& p);
+// An image-prompt mask plane f32 [H, W] resized to one level's queries: out[T] = bicubic resize to (mh, mw) (torch's
+// F.interpolate(mode="bicubic", align_corners=False)) flattened row-major, zero-padded or cut to T.
+int ip_mask_resize_launch(cudaStream_t st, const float* mask, int H, int W, int mh, int mw, int T, float* out);
 
 // ------------------------------------------------------------------------------------------------
 // Norms (norm.cu)

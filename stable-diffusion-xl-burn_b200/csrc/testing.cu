@@ -45,11 +45,48 @@ SDXL_TEST_API int sdxl_test_attention(void* stream, const void* q, int q_pitch, 
   if (r) return r;
   p.tmV = p.tmK;
   if (kip) {
-    p.S_ip = S_ip; p.k_ip_col0 = k_ip_col0; p.v_ip_col0 = v_ip_col0; p.ip_scale = ip_scale;
+    p.S_ip = S_ip; p.k_ip_col0 = k_ip_col0; p.v_ip_col0 = v_ip_col0; p.ip_scale = ip_scale; p.n_src = 1;
     if ((r = make_tmap_rows(&p.tmKip, (const __half*)kip, S_ip, B, kip_pitch, kip_pitch))) return r;
     p.tmVip = p.tmKip;
   }
   return attention_launch((cudaStream_t)stream, p);
+}
+
+// The same with n_src image sources as PlanBuilder::attn_ip sets them up: source k reads K / V as column windows src_info[4k + 1]
+// / src_info[4k + 2] of src_kv[k] [B * src_info[4k + 3], src_info[4k]] and adds *scales[k] * masks[k][t] (masks[k] nullable) times
+// its own softmax. The pointer and info arrays are host memory.
+SDXL_TEST_API int sdxl_test_attention_multi(void* stream, const void* q, int q_pitch, int q_col0, const void* kv, int kv_pitch, int k_col0,
+                                            int v_col0, int B, int T, int S, int n_head, void* out, int ldo, int n_src,
+                                            const void* const* src_kv, const int* src_info, const float* const* scales,
+                                            const float* const* masks) {
+  if (n_src < 1 || n_src > ATTN_MAX_SRC) return 5003;
+  AttnParams p{};
+  p.T = T; p.S = S; p.n_head = n_head; p.B = B;
+  p.q_col0 = q_col0; p.k_col0 = k_col0; p.v_col0 = v_col0;
+  p.out = (__half*)out; p.ldo = ldo;
+  p.scale_log2e = (float)(1.4426950408889634 / 8.0);
+  int r = make_tmap_rows(&p.tmQ, (const __half*)q, T, B, q_pitch, q_pitch);
+  if (!r) r = make_tmap_rows(&p.tmK, (const __half*)kv, S, B, kv_pitch, kv_pitch);
+  if (r) return r;
+  p.tmV = p.tmK;
+  p.n_src = n_src;
+  for (int k = 0; k < n_src; ++k) {
+    const int* f = src_info + 4 * k;
+    CUtensorMap tm;
+    if ((r = make_tmap_rows(&tm, (const __half*)src_kv[k], f[3], B, f[0], f[0]))) return r;
+    if (k == 0) {
+      p.tmKip = p.tmVip = tm;
+      p.S_ip = f[3]; p.k_ip_col0 = f[1]; p.v_ip_col0 = f[2]; p.ip_scale = scales[0]; p.ip_mask = masks[0];
+    } else {
+      p.ip_src[k - 1] = {tm, f[3], f[1], f[2], scales[k], masks[k]};
+    }
+  }
+  return attention_launch((cudaStream_t)stream, p);
+}
+
+// The image-prompt mask resize run when masks are attached (engine.cu: ip_stage).
+SDXL_TEST_API int sdxl_test_ip_mask_resize(void* stream, const float* mask, int H, int W, int mh, int mw, int T, float* out) {
+  return ip_mask_resize_launch((cudaStream_t)stream, mask, H, W, mh, mw, T, out);
 }
 
 SDXL_TEST_API int sdxl_test_attention_small(void* stream, const void* q, int q_pitch, int q_col0, const void* k, const void* v,

@@ -91,6 +91,10 @@ class ImagePrompt(C.Structure):
                 ("seq_len", C.c_int32)]
 
 
+class IpMask(C.Structure):
+    _fields_ = [("mask", C.c_void_p), ("on_host", C.c_int32), ("height", C.c_int32), ("width", C.c_int32)]
+
+
 class T2IAdapterCfg(C.Structure):
     _fields_ = [("unet", UnetCfg), ("in_channels", C.c_int32), ("n_res_blocks", C.c_int32)]
 
@@ -178,6 +182,7 @@ PROTOTYPES = {
     "sdxl_ip_adapter_load": (I, [P, C.POINTER(IpAdapterCfg), P, C.c_size_t, I, C.POINTER(P)]),
     "sdxl_ip_adapter_destroy": (None, [P]),
     "sdxl_unet_set_image_prompt": (I, [P, C.POINTER(ImagePrompt)]),
+    "sdxl_unet_set_image_prompts": (I, [P, I, C.POINTER(ImagePrompt), C.POINTER(IpMask)]),
     "sdxl_ip_adapter_project": (I, [P, I, P, I, P]),
     "sdxl_ip_adapter_resample": (I, [P, I, I, P, I, P]),
     "sdxl_op_ip_attention": (I, [P, P, P, P, P, P, I, I, I, I, I, I, C.c_float, P]),

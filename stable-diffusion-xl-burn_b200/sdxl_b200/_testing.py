@@ -20,6 +20,8 @@ P, I, F = C.c_void_p, C.c_int, C.c_float
 PROTOTYPES = {
     "sdxl_test_igemm": (I, [P, P, I, I, I, I, I, P, I, I, I, I, I, P, I, I, I, I, I, I, I, P, I, P, I, I, P, I, P, I, I, I, I]),
     "sdxl_test_attention": (I, [P, P, I, I, P, I, I, I, I, I, I, I, P, I, P, I, I, I, I, P]),
+    "sdxl_test_attention_multi": (I, [P, P, I, I, P, I, I, I, I, I, I, I, P, I, I, P, P, P, P]),
+    "sdxl_test_ip_mask_resize": (I, [P, P, I, I, I, I, I, P]),
     "sdxl_test_attention_small": (I, [P, P, I, I, P, P, I, I, I, I, I, I, I, P, I, P, I, I]),
     "sdxl_test_perceiver_ln": (I, [P, P, P, I, I, I, I, P, P, P, P, F, P, P]),
     "sdxl_test_gn_scratch_floats": (C.c_size_t, [I, I]),
@@ -84,6 +86,25 @@ def attention(q: torch.Tensor, q_pitch: int, q_col0: int, kv: torch.Tensor, kv_p
               ip_scale: Optional[torch.Tensor] = None) -> None:
     _call("sdxl_test_attention", _p(q), q_pitch, q_col0, _p(kv), kv_pitch, k_col0, v_col0, B, T, S, n_head, _p(out), ldo,
           _p(kip), kip_pitch, k_ip_col0, v_ip_col0, S_ip, _p(ip_scale))
+
+
+def attention_multi(q: torch.Tensor, q_pitch: int, q_col0: int, kv: torch.Tensor, kv_pitch: int, k_col0: int, v_col0: int,
+                    B: int, T: int, S: int, n_head: int, out: torch.Tensor, ldo: int, sources: Sequence[tuple]) -> None:
+    """sources: (kv [B * S_k, pitch] f16, pitch, k_col0, v_col0, S_k, scale f32 [1], mask f32 [T] or None) per image source."""
+    n = len(sources)
+    kvs = (C.c_void_p * n)(*[_p(s[0]) for s in sources])
+    info = (C.c_int * (4 * n))(*[int(v) for s in sources for v in (s[1], s[2], s[3], s[4])])
+    scales = (C.c_void_p * n)(*[_p(s[5]) for s in sources])
+    masks = (C.c_void_p * n)(*[_p(s[6]) for s in sources])
+    _call("sdxl_test_attention_multi", _p(q), q_pitch, q_col0, _p(kv), kv_pitch, k_col0, v_col0, B, T, S, n_head, _p(out), ldo, n,
+          kvs, info, scales, masks)
+
+
+def ip_mask_resize(mask: torch.Tensor, mh: int, mw: int, T: int) -> torch.Tensor:
+    """f32 [T] of a mask plane f32 [H, W]: bicubic resize to (mh, mw), flattened, zero-padded or cut to T."""
+    out = torch.empty(T, device=mask.device, dtype=torch.float32)
+    _call("sdxl_test_ip_mask_resize", _p(mask), mask.shape[0], mask.shape[1], mh, mw, T, _p(out))
+    return out
 
 
 def attention_small(q, q_pitch, q_col0, k, v, kv_pitch, k_col0, v_col0, B, T, S, n_head, mask, causal, out, ldo,

@@ -315,6 +315,13 @@ class Diffuser:
         from .ip_adapter import set_image_prompt
         set_image_prompt(self, adapter, embeds, scale, negative)
 
+    def set_image_prompts(self, prompts: Sequence) -> None:
+        """Replaces the attached image prompts with [(adapter, embeds, scale, negative, mask), ...] (sdxl_unet_set_image_prompts,
+        DESIGN.md §13); [] detaches. Up to four prompts of any adapters; mask None or [n_images, H, W] limits each image of the prompt
+        to its region (binarised at 0.5)."""
+        from .ip_adapter import set_image_prompts
+        set_image_prompts(self, prompts)
+
     def set_t2i_adapters(self, adapters: Sequence, t_min: int = 0) -> None:
         """Replaces the attached T2I-Adapters with [(T2IAdapter, hint, scale), ...] (sdxl_unet_set_t2i_adapters); [] detaches.
         hint: u8 [n, H, W, C] or f32 [n, C, H, W] in [0, 1], H and W multiples of 32; image b of a batch uses hint b % n. The features

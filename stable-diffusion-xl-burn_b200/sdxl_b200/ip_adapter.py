@@ -412,18 +412,13 @@ def _features(x: torch.Tensor, dim: int, what: str) -> torch.Tensor:
     return x.to(torch.float32)
 
 
-def set_image_prompt(diffuser, adapter: Optional[IPAdapter], embeds: Optional[torch.Tensor] = None,
-                     scale: Union[float, Sequence[float]] = 1.0, negative: Optional[torch.Tensor] = None) -> None:
-    """sdxl_unet_set_image_prompt; adapter None detaches. scale: one float, or one per UNet transformer block in execution order
-    (transformer_block_paths). negative: embeddings of the unconditional CFG rows (default: zeros). For an IP-Adapter Plus, embeds
-    and negative are image features [n_batch, n_images, L, D] (IPAdapter.image_embeds) and negative is required."""
+MAX_IMAGE_PROMPTS = 4   # SDXL_MAX_IMAGE_PROMPTS
+MAX_IP_SOURCES = 8      # SDXL_MAX_IP_SOURCES: one per unmasked prompt, one per image of a masked prompt
+
+
+def _prompt_struct(diffuser, adapter: IPAdapter, embeds, scale, negative) -> Tuple[_lib.ImagePrompt, list]:
+    """The sdxl_image_prompt of one prompt and the objects its pointers borrow; every shape is checked here."""
     ctx = diffuser.ctx
-    if adapter is None:
-        ctx.enter()
-        ctx.check(ctx.lib.sdxl_unet_set_image_prompt(diffuser.h, None), "sdxl_unet_set_image_prompt")
-        ctx.leave()
-        release_image_prompt(diffuser)
-        return
     h = adapter.handle()
     plus = getattr(adapter, "resampler", None) is not None
     if plus:
@@ -454,17 +449,86 @@ def set_image_prompt(diffuser, adapter: Optional[IPAdapter], embeds: Optional[to
     p.n_batch, p.n_images, p.scale = e.shape[0], e.shape[1], s0
     p.seq_len = e.shape[2] if plus else 0
     p.block_scales_host = C.cast(block, C.c_void_p) if block is not None else None
+    return p, [e, neg, block]
+
+
+def _mask(mask, n_images: int) -> torch.Tensor:
+    """A prompt's regional mask as f32 [n_images, H, W] of 0 / 1: bool, u8 or float, binarised at 0.5 as diffusers'
+    IPAdapterMaskProcessor does. The engine reads n_images * H * W values of a multiple-of-8 extent, so anything else is refused here."""
+    m = torch.as_tensor(mask)
+    if m.dim() != 3 or m.shape[0] != n_images or m.shape[1] < 8 or m.shape[2] < 8 or m.shape[1] % 8 or m.shape[2] % 8:
+        raise SdxlError(f"image-prompt mask must be [n_images = {n_images}, H, W] with H and W positive multiples of 8, got {tuple(m.shape)}")
+    if m.dtype == torch.uint8:
+        m = m.float() / 255.0
+    m = m.float()
+    if not bool(torch.isfinite(m).all()):
+        raise SdxlError("image-prompt mask has non-finite values")
+    return (m >= 0.5).float().contiguous()
+
+
+def set_image_prompt(diffuser, adapter: Optional[IPAdapter], embeds: Optional[torch.Tensor] = None,
+                     scale: Union[float, Sequence[float]] = 1.0, negative: Optional[torch.Tensor] = None) -> None:
+    """sdxl_unet_set_image_prompt; adapter None detaches. scale: one float, or one per UNet transformer block in execution order
+    (transformer_block_paths). negative: embeddings of the unconditional CFG rows (default: zeros). For an IP-Adapter Plus, embeds
+    and negative are image features [n_batch, n_images, L, D] (IPAdapter.image_embeds) and negative is required."""
+    ctx = diffuser.ctx
+    if adapter is None:
+        ctx.enter()
+        ctx.check(ctx.lib.sdxl_unet_set_image_prompt(diffuser.h, None), "sdxl_unet_set_image_prompt")
+        ctx.leave()
+        release_image_prompt(diffuser)
+        return
+    p, _keep = _prompt_struct(diffuser, adapter, embeds, scale, negative)
     ctx.enter()
     ctx.check(ctx.lib.sdxl_unet_set_image_prompt(diffuser.h, C.byref(p)), "sdxl_unet_set_image_prompt")
     ctx.leave()
     release_image_prompt(diffuser)
-    diffuser._image_prompt = adapter   # the adapter stays alive, and cannot be closed, while attached
+    diffuser._image_prompt = [adapter]   # the adapter stays alive, and cannot be closed, while attached
     adapter.attached += 1
 
 
+def set_image_prompts(diffuser, prompts: Sequence) -> None:
+    """sdxl_unet_set_image_prompts: replaces the attached image prompts with [(adapter, embeds, scale, negative, mask), ...] (DESIGN.md
+    §13); [] detaches. Each of the first four items is as for set_image_prompt. mask: None, or [n_images, H, W] (bool, u8 or float,
+    binarised at 0.5) limiting each image of the prompt to its region of an (H / 8) x (W / 8) latent. At most MAX_IMAGE_PROMPTS
+    prompts and MAX_IP_SOURCES sources (one per unmasked prompt, one per image of a masked prompt)."""
+    ctx = diffuser.ctx
+    prompts = list(prompts)
+    if len(prompts) > MAX_IMAGE_PROMPTS:
+        raise SdxlError(f"set_image_prompts: {len(prompts)} prompts given, at most {MAX_IMAGE_PROMPTS}")
+    structs, masks, keep = [], [], []
+    n_src = 0
+    for item in prompts:
+        if len(item) != 5:
+            raise SdxlError("set_image_prompts: each prompt is (adapter, embeds, scale, negative, mask)")
+        adapter, embeds, scale, negative, mask = item
+        p, k = _prompt_struct(diffuser, adapter, embeds, scale, negative)
+        m = _lib.IpMask()
+        if mask is not None:
+            mt = _mask(mask, p.n_images).to(ctx.device)
+            m.mask, m.on_host, m.height, m.width = mt.data_ptr(), 0, mt.shape[1], mt.shape[2]
+            k.append(mt)
+        n_src += p.n_images if mask is not None else 1
+        structs.append(p)
+        masks.append(m)
+        keep.append(k)
+    if n_src > MAX_IP_SOURCES:
+        raise SdxlError(f"set_image_prompts: {n_src} image sources (one per unmasked prompt, one per image of a masked prompt), at "
+                        f"most {MAX_IP_SOURCES}")
+    n = len(structs)
+    arr = (_lib.ImagePrompt * max(n, 1))(*structs)
+    marr = (_lib.IpMask * max(n, 1))(*masks)
+    ctx.enter()
+    ctx.check(ctx.lib.sdxl_unet_set_image_prompts(diffuser.h, n, arr, marr), "sdxl_unet_set_image_prompts")
+    ctx.leave()
+    release_image_prompt(diffuser)
+    diffuser._image_prompt = [item[0] for item in prompts]   # every adapter stays alive, and cannot be closed, while attached
+    for a in diffuser._image_prompt:
+        a.attached += 1
+
+
 def release_image_prompt(diffuser) -> None:
-    """Forgets the diffuser's attached adapter (after a detach, or when the UNet is destroyed)."""
-    a = getattr(diffuser, "_image_prompt", None)
-    if a is not None:
+    """Forgets the diffuser's attached adapters (after a detach, or when the UNet is destroyed)."""
+    for a in getattr(diffuser, "_image_prompt", None) or []:
         a.attached -= 1
     diffuser._image_prompt = None

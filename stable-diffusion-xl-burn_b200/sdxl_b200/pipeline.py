@@ -63,14 +63,26 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     those models had. controls: [(ControlNet, image u8 [1, H, W, 3] or f32 [1, 3, H, W], scale), ...] attached to the base UNet
     for this call and detached afterwards (the refiner is left alone). image_prompt: (IPAdapter, ClipVisionEncoder, images u8
     [n_images, H, W, 3], scale): the images are encoded (IPAdapter.image_embeds: image_embeds for the base adapter, hidden states for
-    IP-Adapter Plus) and attached to the base UNet as one prompt of n_images images for this call and detached afterwards.
+    IP-Adapter Plus) and attached to the base UNet as one prompt of n_images images for this call and detached afterwards; or a list
+    of up to four (IPAdapter, ClipVisionEncoder, images, scale[, mask]) attached together (Diffuser.set_image_prompts; mask None or
+    [n_images, H, W] at the output resolution).
     t2i_adapters: [(T2IAdapter, image u8 [1, H, W, C] or f32 [1, C, H, W], scale), ...] attached to the base UNet for this call and
     detached afterwards, their features added on the first int(n_steps * t2i_factor) iterations (diffusers'
     adapter_conditioning_factor). Returns uint8 [1, H, W, 3]."""
     if image_prompt:
-        adapter, encoder, images, scale = image_prompt
-        e, neg = adapter.image_embeds(encoder, images)
-        diffuser.set_image_prompt(adapter, e.unsqueeze(0), scale, negative=neg.unsqueeze(0))
+        if isinstance(image_prompt, list):
+            if len(image_prompt) > 4:
+                raise _lib.SdxlError(f"image_prompt: {len(image_prompt)} prompts given, at most 4")
+            prompts = []
+            for item in image_prompt:
+                adapter, encoder, images, scale = item[:4]
+                e, neg = adapter.image_embeds(encoder, images)
+                prompts.append((adapter, e.unsqueeze(0), scale, neg.unsqueeze(0), item[4] if len(item) > 4 else None))
+            diffuser.set_image_prompts(prompts)
+        else:
+            adapter, encoder, images, scale = image_prompt
+            e, neg = adapter.image_embeds(encoder, images)
+            diffuser.set_image_prompt(adapter, e.unsqueeze(0), scale, negative=neg.unsqueeze(0))
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
                           seed, noise, loras, controls, t2i_adapters=t2i_adapters, t2i_factor=t2i_factor)

@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Sampler step time without an image prompt, with the base adapter's 1 image (4 tokens) and 4 images (16 tokens), and with an
-IP-Adapter Plus prompt of 1 image (16 tokens) and 4 images (64 tokens), the attention kernel's share of a step, the set_image_prompt
-time (base: projection; Plus: Resampler) and the vision encoder's time per image (ViT-H/14 image_embeds and hidden states,
+IP-Adapter Plus prompt of 1 image (16 tokens) and 4 images (64 tokens), with image-prompt sets (DESIGN.md §13: base 1 image plus
+Plus 1 image, unmasked and each masked to one half; one base prompt of 2 images masked to the two halves), the attention kernel's
+share of a step, the set_image_prompt and set_image_prompts time (base: projection; Plus: Resampler) and the vision encoder's time per image (ViT-H/14 image_embeds and hidden states,
 ViT-bigG/14 image_embeds); SDXL base + ViT-H-sized base and Plus IP-Adapters (synthetic weights) on one GPU.
 
     python tools/ip_adapter_bench.py [out.json] [--steps K] [--warmup W] [--reps R]
@@ -52,7 +53,10 @@ def main():
     emb = {k: torch.randn(1, k, D, generator=g(10 + k)) for k in (1, 4)}
     hid = {k: torch.randn(1, k, L_PLUS, D_PLUS, generator=g(20 + k)) for k in (1, 4)}
     hid_neg = {k: torch.randn(1, k, L_PLUS, D_PLUS, generator=g(30 + k)) for k in (1, 4)}
-    kinds = ["none", "base_1", "base_4", "plus_1", "plus_4"]
+    kinds = ["none", "base_1", "base_4", "plus_1", "plus_4", "base_plus", "base_plus_masked", "base_2_masked"]
+    left = torch.zeros(1, HW, HW)
+    left[:, :, :HW // 2] = 1
+    emb2 = torch.randn(1, 2, D, generator=g(40))
     cond = sdxl_b200.Conditioning(
         context_full=torch.randn(1, 77, 2048, generator=g(1)).half(), unconditional_context_full=torch.randn(77, 2048, generator=g(2)).half(),
         channel_context=torch.randn(1, 2816, generator=g(3)).half(), unconditional_channel_context=torch.randn(2816, generator=g(4)).half(),
@@ -63,6 +67,12 @@ def main():
     def prompt(kind, scale=1.0):
         if kind == "none":
             d.set_image_prompt(None)
+        elif kind.startswith("base_plus"):
+            m = kind.endswith("masked")
+            d.set_image_prompts([(ad, emb[1], scale, None, left if m else None),
+                                 (plus, hid[1], scale, hid_neg[1], 1 - left if m else None)])
+        elif kind == "base_2_masked":
+            d.set_image_prompts([(ad, emb2, scale, None, torch.cat([left, 1 - left]))])
         elif kind.startswith("base"):
             d.set_image_prompt(ad, emb[int(kind[-1])], scale)
         else:
@@ -126,6 +136,10 @@ def main():
         "plus_attach_one_image": timed(lambda: prompt("plus_1"), before=lambda: prompt("none")),
         "plus_in_place_one_image": timed(lambda: prompt("plus_1", 0.6)),
         "plus_attach_four_images": timed(lambda: prompt("plus_4"), before=lambda: prompt("none")),
+    }
+    res["set_image_prompts_ms"] = {
+        "attach_base_plus_masked": timed(lambda: prompt("base_plus_masked"), before=lambda: prompt("none")),
+        "rewrite_base_plus_masked": timed(lambda: prompt("base_plus_masked", 0.6)),
     }
     d.set_image_prompt(None)
     res["encode_ms_per_image"] = {}
