@@ -163,7 +163,7 @@ SDXL_API double sdxl_unet_plan_flops_executed(const sdxl_unet* unet);
 /* Device time of ONE execution of the current launch plan, summed per kernel kind and measured with CUDA
  * events on the ctx stream (eager launches). Kind index: 0 implicit-GEMM (wgmma), 1 attention, 2 GroupNorm,
  * 3 LayerNorm, 4 GEMV, 5 timestep-embedding, 6 first conv, 7 upsample copy, 8 phase-split copy, 9 f32->f16 cast,
- * 17 T2I-Adapter feature add.
+ * 17 T2I-Adapter feature add, 18 PAG identity self-attention.
  * All three arrays hold SDXL_PROFILE_KINDS entries (host). Used by bench.py for the per-kernel roofline. */
 SDXL_API int sdxl_unet_profile_plan(sdxl_unet* unet, double* ms_by_kind_host, double* flops_by_kind_host,
                                     int* launches_by_kind_host);
@@ -453,7 +453,8 @@ typedef struct sdxl_image_prompt {
   int32_t seq_len;                 /* Plus: L, the hidden-state rows per image (257 for ViT-H/14), in [1, 4096]; ignored otherwise */
 } sdxl_image_prompt;
 /* Attaches an image prompt to the UNet (NULL detaches). Row rule: in the sampler's CFG batch [cond | uncond] of n images, cond row
- * b uses embeds prompt b % n_batch and uncond row b negative prompt b % n_batch; a direct sdxl_unet_forward of B rows uses prompt
+ * b uses embeds prompt b % n_batch and uncond row b negative prompt b % n_batch; with PAG attached the batch is [cond | uncond | ptb]
+ * and perturbed row b, a conditional row, uses embeds prompt b % n_batch; a direct sdxl_unet_forward of B rows uses prompt
  * r % n_batch for row r. Everything is validated before anything changes (ctx, cfg, n_batch >= 1, n_images >= 1, finite scales, the
  * current conditioning batch a multiple of n_batch; Plus: negative_embeds given, seq_len in range): on failure the previous state stays. A call with the same adapter, n_batch and
  * n_images rewrites tokens, K/V and scales in place (same launch plan and CUDA graph); any other change rebuilds the plan at the
@@ -562,6 +563,32 @@ typedef struct sdxl_inpaint_condition {
  * is not height/8 x width/8, or when the batch (the images, for the sampler: the CFG rows [cond | uncond] of image b both read row
  * b % n) is not a multiple of n. */
 SDXL_API int sdxl_unet_set_inpaint_condition(sdxl_unet* unet, const sdxl_inpaint_condition* c);
+
+/* ---- perturbed-attention guidance (PAG) ------------------------------------------------------------------
+ * Ahn et al. 2024, as diffusers' StableDiffusionXL*PAGPipeline runs it (DESIGN.md §14). The sampler adds a third row group to its
+ * batch: [cond | uncond | ptb] (the refiner, without CFG: [cond | ptb]). The perturbed rows repeat the conditional rows' context, pooled
+ * and time ids, image-prompt tokens and hints, but in every selected self-attention (attn1 of a transformer block) they compute
+ * to_out(to_v(x)): softmax(q k^T) is replaced by the identity. The other rows, every cross-attention and every ControlNet are unchanged.
+ * The guided noise of a step at timestep t is
+ *   e = (u + (c - u) * guidance) + p_t * (c - ptb)      resp.   e = c + p_t * (c - ptb) without CFG,
+ *   p_t = max(scale - adaptive_scale * (n_steps - t), 0)    (diffusers' pag_adaptive_scale; 0: p_t = scale),
+ * and the DDIM update is the one of sdxl_sample_latent. */
+typedef struct sdxl_pag {
+  float scale;                     /* pag_scale, finite and > 0 */
+  float adaptive_scale;            /* pag_adaptive_scale, finite and >= 0 */
+  int32_t n_layers;                /* == sdxl_unet_num_self_attentions(unet) */
+  const uint8_t* layers_host;      /* [n_layers]: 1 = identity self-attention on the perturbed rows; one per transformer block in
+                                      execution order (down blocks, middle block, up blocks); at least one set */
+  int32_t forward_perturbed_rows;  /* direct sdxl_unet_forward*: the last this-many rows of the batch are perturbed (0: none; fewer
+                                      than the batch); the sampler ignores it */
+} sdxl_pag;
+/* Self-attentions of the UNet, one per transformer block (70 for SDXL base, 44 for the refiner). */
+SDXL_API int sdxl_unet_num_self_attentions(const sdxl_unet* unet);
+/* Attaches PAG to the UNet (NULL detaches). Everything is validated before anything changes: on failure the previous attachment stays.
+ * A call that changes only scale, adaptive_scale or forward_perturbed_rows keeps the launch plan (a new perturbed row count rebuilds
+ * it at the next direct forward that uses it); a new layer set, attaching and detaching rebuild it at the next forward. Attaching or
+ * detaching between sdxl_sampler_begin and sdxl_sampler_step requires a new sdxl_sampler_begin. */
+SDXL_API int sdxl_unet_set_pag(sdxl_unet* unet, const sdxl_pag* pag);
 
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),

@@ -434,6 +434,54 @@ int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, 
                                                      sqrt_ap, sqrt_1map, x);
   return (int)cudaGetLastError();
 }
+// cfg_ddim_kernel with perturbed-attention guidance: eps rows [cond | uncond | ptb] (use_cfg) or [cond | ptb], and
+//   e = (u + (c - u) * s) + p_t * (c - ptb)      resp.   e = c + p_t * (c - ptb)
+__global__ void cfg_pag_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg, int C, int HW, int use_cfg, float g,
+                                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
+                                    float* __restrict__ x) {
+  const long total = (long)Bimg * C * HW;
+  const int ptb_row0 = (use_cfg ? 2 : 1) * Bimg;
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
+    const int p = (int)(i % HW);
+    const int c = (int)((i / HW) % C);
+    const int b = (int)(i / ((long)HW * C));
+    const float ec = eps[((size_t)b * HW + p) * ld + c];
+    const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
+    float e = ec;
+    if (use_cfg) {
+      const float eu = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
+      e = eu + (ec - eu) * g;
+    }
+    e = e + p_t * (ec - ep);
+    const float xv = x[i];
+    const float predx0 = (xv - e * sqrt_1ma) / sqrt_a;
+    x[i] = predx0 * sqrt_ap + e * sqrt_1map;
+  }
+}
+int cfg_pag_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance, float p_t,
+                        float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
+  const long total = (long)Bimg * C * HW;
+  cfg_pag_ddim_kernel<<<cdiv(total, 256), 256, 0, st>>>(eps, ld, Bimg, C, HW, use_cfg, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap,
+                                                         sqrt_1map, x);
+  return (int)cudaGetLastError();
+}
+
+// PAG's identity self-attention: out[r, 0:C] = qkv[r, 2C:3C] (the V window of the fused QKV rows), 16-byte vectors.
+__global__ void pag_identity_kernel(const uint4* __restrict__ qkv, int C8, long n, uint4* __restrict__ out) {
+  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long)gridDim.x * blockDim.x) {
+    const long r = i / C8;
+    const int c = (int)(i - r * C8);
+    out[i] = qkv[r * 3 * C8 + 2 * C8 + c];
+  }
+}
+int pag_identity_launch(cudaStream_t st, const __half* qkv, int C, long rows, __half* out) {
+  if (C % 8 || ((uintptr_t)qkv | (uintptr_t)out) % 16) return (int)cudaErrorInvalidValue;
+  const long n = rows * (C / 8);
+  if (n == 0) return 0;
+  const long blocks = cdiv(n, 256);
+  pag_identity_kernel<<<(unsigned)(blocks < 8192 ? blocks : 8192), 256, 0, st>>>((const uint4*)qkv, C / 8, n, (uint4*)out);
+  return (int)cudaGetLastError();
+}
 // x = mask ? x : (ref*sqrt_a + noise*sqrt_1ma)   (reference stablediffusion/mod.rs:463-465)
 __global__ void inpaint_blend_kernel(float* __restrict__ x, const float* __restrict__ ref,
                                      const float* __restrict__ noise, const uint8_t* __restrict__ mask, size_t n,

@@ -162,6 +162,23 @@ struct InpaintAttach {
   float* cond = nullptr;
 };
 
+// Perturbed-attention guidance (sdxl_unet_set_pag, DESIGN.md §14): the self-attentions that run as the identity on the perturbed
+// rows (one flag per transformer block in execution order), the guidance scales, and the perturbed rows of a direct forward.
+struct PagAttach {
+  float scale = 0.f, adaptive = 0.f;
+  std::vector<uint8_t> layers;
+  int forward_rows = 0;
+};
+
+// Roles of the conditioning rows. The sampler's batch is row groups of n_img rows each: [cond | uncond] with CFG, then a perturbed
+// group with PAG ([cond | uncond | ptb]; the refiner: [cond] or [cond | ptb]). The perturbed rows are conditional rows. n_img = 0:
+// a plain batch, every row conditional.
+struct RowLayout {
+  int n_img = 0;
+  bool uncond = false;   // group 1 is the unconditional one
+  bool negative(int r) const { return uncond && r / n_img == 1; }
+};
+
 // Embeddings, first conv, input blocks and middle block: the part of the UNet a ControlNet copies.
 struct EncoderHalf {
   sdxl_ctx* ctx = nullptr;
@@ -218,8 +235,10 @@ struct sdxl_unet : EncoderHalf {
   std::unique_ptr<IpAttach> ip;   // sdxl_unet_set_image_prompts
   std::unique_ptr<T2IAttach> t2i; // sdxl_unet_set_t2i_adapters
   std::unique_ptr<InpaintAttach> inpaint;   // sdxl_unet_set_inpaint_condition
+  std::unique_ptr<PagAttach> pag;           // sdxl_unet_set_pag
   uint64_t plan_builds = 0;
-  int cfg_rows = 0;               // conditioning rows are the sampler's [cond | uncond] with cfg_rows cond rows (0: plain batch)
+  int plan_ptb = 0;               // trailing rows of the current plan that take PAG's identity self-attentions
+  RowLayout rows;                 // roles of the conditioning rows
   ~sdxl_unet() {
     if (t_dev) cudaFree(t_dev);
     if (t_pinned) cudaFreeHost(t_pinned);
@@ -743,6 +762,7 @@ struct UNetPlanBuilder : PlanBuilder {
   sdxl_unet* u = nullptr;
   int kv_index = 0;
   const HoistedCond* cond = nullptr;   // hoisted conditioning of the model being planned (UNet or ControlNet)
+  int Bp = 0;                          // trailing perturbed rows: PAG's selected self-attentions of the UNet are the identity there
 
   struct Scratch { __half *gn1, *raw; float* h; __half *gn2, *a16; float* tok; __half *qkv, *ao, *q, *ff; };
   struct Saved { float* p; int C, H, W; };
@@ -866,7 +886,18 @@ struct UNetPlanBuilder : PlanBuilder {
       // x = x + attn1(norm1(x))
       ln(s_tok, b.n1, M, s_a16);
       linear(s_a16, M, b.qkv, IGEMM_LINEAR, s_qkv, 0, 3 * C, nullptr, 0);
-      attn(s_qkv, 3 * C, 0, s_qkv, 3 * C, C, 2 * C, T, T, s.n_head, s_ao, C, sl2e);
+      if (Bp && cond == &u->cond && u->pag->layers[kv_index]) {
+        // PAG: softmax attention over the attended rows, out = v on the perturbed ones (out1 and the residual run on all rows)
+        attn(s_qkv, 3 * C, 0, s_qkv, 3 * C, C, 2 * C, T, T, s.n_head, s_ao, C, sl2e, Bf - Bp);
+        if (!err) {
+          Op op{};
+          op.kind = OP_PAG_IDENTITY;
+          op.pi = {s_qkv + (size_t)(Bf - Bp) * T * 3 * C, C, (long)Bp * T, s_ao + (size_t)(Bf - Bp) * T * C};
+          P->ops.push_back(op);
+        }
+      } else {
+        attn(s_qkv, 3 * C, 0, s_qkv, 3 * C, C, 2 * C, T, T, s.n_head, s_ao, C, sl2e);
+      }
       linear(s_ao, M, b.out1, IGEMM_LINEAR, s_tok, 1, C, s_tok, C);
       // x = x + attn2(norm2(x), context)   (K/V hoisted to set_conditioning)
       ln(s_tok, b.n2, M, s_a16);
@@ -904,24 +935,26 @@ struct UNetPlanBuilder : PlanBuilder {
     linear(s_a16, M, s.proj_out, IGEMM_LINEAR, out, 1, C, x, C);
     return out;
   }
+  // over the first B rows of the batch (default: all Bf)
   void attn(const __half* qm, int q_pitch, int q_col0, const __half* kvm, int kv_pitch, int k_col0, int v_col0, int T,
-            int S, int n_head, __half* out, int ldo, float sl2e) {
+            int S, int n_head, __half* out, int ldo, float sl2e, int B = 0) {
     if (err) return;
+    if (!B) B = Bf;
     Op op{};
     op.kind = OP_ATTN;
     AttnParams& p = op.at;
-    p.T = T; p.S = S; p.n_head = n_head; p.B = Bf;
+    p.T = T; p.S = S; p.n_head = n_head; p.B = B;
     p.q_col0 = q_col0; p.k_col0 = k_col0; p.v_col0 = v_col0;
     p.out = out; p.ldo = ldo; p.scale_log2e = sl2e;
     if (!A->measure) {
-      int r = make_tmap_rows(&p.tmQ, qm, T, Bf, q_pitch, q_pitch);
-      if (!r) r = make_tmap_rows(&p.tmK, kvm, S, Bf, kv_pitch, kv_pitch);
+      int r = make_tmap_rows(&p.tmQ, qm, T, B, q_pitch, q_pitch);
+      if (!r) r = make_tmap_rows(&p.tmK, kvm, S, B, kv_pitch, kv_pitch);
       if (!r) p.tmV = p.tmK;
       if (r) { err = fail(c, r, "tensor map creation failed (attention)"); return; }
     }
-    op.flops_exec = 4.0 * Bf * (double)((T + 127) / 128 * 128) * (double)((S + 127) / 128 * 128) * (n_head * 64);
+    op.flops_exec = 4.0 * B * (double)((T + 127) / 128 * 128) * (double)((S + 127) / 128 * 128) * (n_head * 64);
     P->ops.push_back(op);
-    add_flops(4.0 * Bf * T * (double)S * (n_head * 64));
+    add_flops(4.0 * B * T * (double)S * (n_head * 64));
   }
   // Adds an image source to the attention just pushed: + (*scale) * mask[t] * softmax(q k_ip^T) v_ip (mask nullable: 1), k_ip /
   // v_ip column windows of kvm [Bf * S_ip, kv_pitch].
@@ -948,10 +981,11 @@ struct UNetPlanBuilder : PlanBuilder {
 
 
 // Builds the op list for UNet::forward (reference unet/mod.rs:449-493) at batch Bf, latent h x w.
-static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A) {
+static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   UNetPlanBuilder B{{c, P, A, P->Bf}, u};
+  B.Bp = Bp;
   P->ops.clear();
   P->block_names.clear();
   P->flops = 0;
@@ -1092,9 +1126,11 @@ static int ip_mask_check(sdxl_unet* u, const IpPrompt& a, int h, int w) {
   return 0;
 }
 
-static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
+// Bp: the trailing rows that take PAG's identity self-attentions (0: none; PAG attached when > 0).
+static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w, int Bp) {
   sdxl_ctx* c = u->ctx;
   if (u->cond.condB != Bf) return fail(c, 5010, "conditioning is set for batch %d but forward batch is %d (call sdxl_unet_set_conditioning first)", u->cond.condB, Bf);
+  if (Bp < 0 || Bp >= Bf) return fail(c, 5023, "PAG: %d perturbed rows in a batch of %d (at least one row must be attended)", Bp, Bf);
   for (size_t k = 0; k < u->controls.size(); ++k) {
     const ControlAttach& a = *u->controls[k];
     if (a.h != h || a.w != w)
@@ -1113,9 +1149,10 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w) {
     if (Bf % a.n_hint) return fail(c, 5016, "T2I-Adapter: batch %d is not a multiple of n_hint = %d", Bf, a.n_hint);
   }
   if (int r = inpaint_check(u, Bf, h, w)) return r;
-  // every change of the buffers or attachments a plan reads drops the plan, so the shapes are its whole cache key
-  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w) return 0;
-  if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A); })) return r;
+  // every change of the buffers or attachments a plan reads drops the plan, so the shapes and the perturbed rows are its whole cache key
+  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan_ptb == Bp) return 0;
+  if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A, Bp); })) return r;
+  u->plan_ptb = Bp;
   u->plan_builds++;
   return 0;
 }
@@ -1162,24 +1199,24 @@ static int ip_cond_alloc(sdxl_ctx* c, const IpPrompt& a, int B, IpRows& r) {
 }
 
 // An image prompt's n_batch must divide the number of images the conditioning rows hold.
-static int ip_check_batch(sdxl_unet* u, int n_batch /* 0: no prompt */, int B, int cfg_rows) {
-  const int n_img = cfg_rows ? cfg_rows : B;
+static int ip_check_batch(sdxl_unet* u, int n_batch /* 0: no prompt */, int B, const RowLayout& L) {
+  const int n_img = L.n_img ? L.n_img : B;
   if (n_batch && n_img % n_batch)
     return fail(u->ctx, 5104, "image prompt: batch %d is not a multiple of its n_batch = %d", n_img, n_batch);
   return 0;
 }
-static int ip_check_batch_all(sdxl_unet* u, int B, int cfg_rows) {
+static int ip_check_batch_all(sdxl_unet* u, int B, const RowLayout& L) {
   if (u->ip)
     for (const IpPrompt& a : u->ip->prompts)
-      if (int r = ip_check_batch(u, a.n_batch, B, cfg_rows)) return r;
+      if (int r = ip_check_batch(u, a.n_batch, B, L)) return r;
   return 0;
 }
 
-static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* context_dev, const __half* y_dev, int cfg_rows) {
+static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* context_dev, const __half* y_dev, const RowLayout& L) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   if (B < 1 || n_ctx < 1) return fail(c, 5100, "bad conditioning shape");
-  if (int r = ip_check_batch_all(u, B, cfg_rows)) return r;
+  if (int r = ip_check_batch_all(u, B, L)) return r;
   if (u->cond.condB != B || u->cond.n_ctx != n_ctx) {
     // everything sized by (B, n_ctx) is allocated into fresh objects and swapped in only when all of it succeeded: a failure
     // leaves the previous conditioning, and the plan over it, in effect
@@ -1210,7 +1247,7 @@ static int set_conditioning_dev(sdxl_unet* u, int B, int n_ctx, const __half* co
     for (size_t k = 0; k < ipc.size(); ++k) u->ip->prompts[k].cond = std::move(ipc[k]);
     CU(c, cudaMemsetAsync(u->ctx16, 0, (size_t)B * n_ctx * pitch * 2, c->stream));
   }
-  u->cfg_rows = cfg_rows;
+  u->rows = L;
   CU(c, cudaMemcpy2DAsync(u->ctx16, (size_t)u->ctx_pitch * 2, context_dev, (size_t)g.context_dim * 2, (size_t)g.context_dim * 2,
                           (size_t)B * n_ctx, cudaMemcpyDeviceToDevice, c->stream));
   KL(c, cast_f16_to_f32_launch(c->stream, y_dev, (size_t)B * g.adm_in_channels, u->y32));
@@ -1249,10 +1286,12 @@ static int hoist_model(sdxl_unet* u, const EncoderHalf& e, const HoistedCond& h)
 // source-major (IpRows), and their K/V for every UNet cross-attention.
 static int ip_hoist(sdxl_unet* u, IpPrompt& a) {
   sdxl_ctx* c = u->ctx;
-  const int ctx_dim = u->cfg.context_dim, B = a.cond.condB, cr = u->cfg_rows, ns = a.n_sources();
+  const int ctx_dim = u->cfg.context_dim, B = a.cond.condB, ns = a.n_sources();
+  const RowLayout& L = u->rows;
   const size_t row = (size_t)a.S_ip * ctx_dim, src_row = row / ns;   // one conditioning row's tokens; one source's part of them
   for (int r = 0; r < B; ++r) {
-    const __half* src = (cr && r >= cr) ? a.tok_neg + (size_t)((r - cr) % a.n_batch) * row : a.tok_pos + (size_t)(r % a.n_batch) * row;
+    // n_batch divides n_img (ip_check_batch), so row r of any group is image r % n_batch
+    const __half* src = L.negative(r) ? a.tok_neg + (size_t)(r % a.n_batch) * row : a.tok_pos + (size_t)(r % a.n_batch) * row;
     CU(c, cudaMemcpy2DAsync(a.cond.rows + (size_t)r * src_row, B * src_row * sizeof(__half), src, src_row * sizeof(__half),
                             src_row * sizeof(__half), ns, cudaMemcpyDeviceToDevice, c->stream));
   }
@@ -1276,7 +1315,7 @@ static int hoist_conditioning(sdxl_unet* u) {
 extern "C" int sdxl_unet_set_conditioning(sdxl_unet* u, int B, int n_ctx, const sdxl_half* context, const sdxl_half* y) {
   if (!u || !context || !y) return -1;
   CU(u->ctx, cudaSetDevice(u->ctx->device));
-  return set_conditioning_dev(u, B, n_ctx, (const __half*)context, (const __half*)y, 0);
+  return set_conditioning_dev(u, B, n_ctx, (const __half*)context, (const __half*)y, RowLayout{});
 }
 
 // ================================================================================================
@@ -1718,7 +1757,7 @@ static int ip_prompt_check(sdxl_unet* u, const sdxl_image_prompt* p) {
     for (int i = 0; i < n_tb; ++i)
       if (!isfinite(p->block_scales_host[i])) return fail(c, 4837, "set_image_prompt: block scale %d is not finite", i);
   if (u->cond.condB > 0)
-    if (int r = ip_check_batch(u, p->n_batch, u->cond.condB, u->cfg_rows)) return r;
+    if (int r = ip_check_batch(u, p->n_batch, u->cond.condB, u->rows)) return r;
   return 0;
 }
 
@@ -2157,13 +2196,54 @@ extern "C" int sdxl_unet_set_adapters(sdxl_unet* u, int n, const sdxl_adapter* a
 }
 
 // ================================================================================================
+// perturbed-attention guidance (include/sdxl_b200.h: sdxl_unet_set_pag; DESIGN.md §14)
+// ================================================================================================
+extern "C" int sdxl_unet_num_self_attentions(const sdxl_unet* u) { return u ? (int)u->tblocks.size() : -1; }
+
+extern "C" int sdxl_unet_set_pag(sdxl_unet* u, const sdxl_pag* p) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  if (!p) {
+    if (!u->pag) return 0;
+    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
+    u->plan.reset();
+    u->pag.reset();
+    return 0;
+  }
+  // validate everything first: on failure the attached state is unchanged
+  const int n = (int)u->tblocks.size();
+  if (!(isfinite(p->scale) && p->scale > 0.f)) return fail(c, 4900, "set_pag: scale = %g must be finite and > 0 (detach with NULL)", p->scale);
+  if (!(isfinite(p->adaptive_scale) && p->adaptive_scale >= 0.f))
+    return fail(c, 4901, "set_pag: adaptive_scale = %g must be finite and >= 0", p->adaptive_scale);
+  if (p->n_layers != n) return fail(c, 4902, "set_pag: n_layers = %d but the UNet has %d self-attentions", p->n_layers, n);
+  if (!p->layers_host) return fail(c, 4903, "set_pag: null layers_host");
+  int n_sel = 0;
+  for (int i = 0; i < n; ++i) n_sel += p->layers_host[i] != 0;
+  if (!n_sel) return fail(c, 4904, "set_pag: no self-attention selected");
+  if (p->forward_perturbed_rows < 0) return fail(c, 4905, "set_pag: forward_perturbed_rows = %d is negative", p->forward_perturbed_rows);
+  std::vector<uint8_t> layers(n);
+  for (int i = 0; i < n; ++i) layers[i] = p->layers_host[i] != 0;
+  if (!u->pag || u->pag->layers != layers) {   // a new layer set changes the plan; the scales and the row count do not (ensure_plan)
+    CU(c, cudaStreamSynchronize(c->stream));
+    u->plan.reset();
+    if (!u->pag) u->pag.reset(new PagAttach());
+    u->pag->layers = std::move(layers);
+  }
+  u->pag->scale = p->scale;
+  u->pag->adaptive = p->adaptive_scale;
+  u->pag->forward_rows = p->forward_perturbed_rows;
+  return 0;
+}
+
+// ================================================================================================
 // UNet::forward
 // ================================================================================================
 extern "C" int sdxl_unet_forward(sdxl_unet* u, int B, int h, int w, const sdxl_half* x, int32_t t_host, sdxl_half* eps_out) {
   if (!u || !x || !eps_out) return -1;
   sdxl_ctx* c = u->ctx;
   CU(c, cudaSetDevice(c->device));
-  int r = ensure_plan(u, B, B, h, w);
+  int r = ensure_plan(u, B, B, h, w, u->pag ? u->pag->forward_rows : 0);
   if (r) return r;
   Plan* P = u->plan.get();
   KL(c, cast_f16_to_f32_launch(c->stream, (const __half*)x, (size_t)B * latent_channels(u->cfg) * h * w, P->x_in));
@@ -2176,7 +2256,7 @@ extern "C" int sdxl_unet_forward_f32(sdxl_unet* u, int B, int h, int w, const fl
   if (!u || !x || !eps_out) return -1;
   sdxl_ctx* c = u->ctx;
   CU(c, cudaSetDevice(c->device));
-  int r = ensure_plan(u, B, B, h, w);
+  int r = ensure_plan(u, B, B, h, w, u->pag ? u->pag->forward_rows : 0);
   if (r) return r;
   Plan* P = u->plan.get();
   CU(c, cudaMemcpyAsync(P->x_in, x, (size_t)B * latent_channels(u->cfg) * h * w * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
@@ -2217,7 +2297,8 @@ extern "C" double sdxl_unet_plan_flops_executed(const sdxl_unet* u) {
 // sampler (Diffuser)
 // ================================================================================================
 struct Sampler {
-  int Bimg = 0, nfwd = 1, h = 0, w = 0, n_ctx = 0;
+  int Bimg = 0, nfwd = 1, h = 0, w = 0, n_ctx = 0;   // nfwd: row groups of Bimg rows, [cond | uncond] or [cond], then [ptb] with PAG
+  bool cfg = false, pag = false;
   float guidance = 1.f;
   float* noise = nullptr;  // scratch [Bimg,4,h,w]
   float* ref = nullptr;
@@ -2233,33 +2314,36 @@ struct Sampler {
 };
 
 // Uploads/assembles the batched conditioning: rows [0,Bimg) conditional, rows [Bimg,2*Bimg) the
-// unconditional context repeated (reference stablediffusion/mod.rs:506-537).
+// unconditional context repeated (reference stablediffusion/mod.rs:506-537). With PAG attached a last group of Bimg rows repeats
+// the conditional rows (the refiner, without CFG: [cond | ptb]).
 static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double guidance) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   if (!cond) return fail(c, 5200, "null conditioning");
   const int Bimg = cond->n_batch, n_ctx = cond->n_ctx;
   const int h = cond->resolution[0] / 8, w = cond->resolution[1] / 8;
-  const int nfwd = g.is_refiner ? 1 : 2;
+  const bool use_cfg = !g.is_refiner, pag = u->pag != nullptr;
+  const int nfwd = (use_cfg ? 2 : 1) + (pag ? 1 : 0);
+  const RowLayout layout{Bimg, use_cfg};
   const sdxl_half* ctx_c = g.is_refiner ? cond->context_open_clip : cond->context_full;
   const sdxl_half* ctx_u = g.is_refiner ? cond->unconditional_context_open_clip : cond->unconditional_context_full;
   const sdxl_half* y_c = g.is_refiner ? cond->channel_context_refiner : cond->channel_context;
   const sdxl_half* y_u = g.is_refiner ? cond->unconditional_channel_context_refiner : cond->unconditional_channel_context;
-  if (!ctx_c || !y_c || (nfwd == 2 && (!ctx_u || !y_u))) return fail(c, 5201, "conditioning tensors for this model are null");
+  if (!ctx_c || !y_c || (use_cfg && (!ctx_u || !y_u))) return fail(c, 5201, "conditioning tensors for this model are null");
   if (Bimg < 1 || h < 1 || w < 1) return fail(c, 5202, "bad conditioning batch/resolution");
-  for (size_t k = 0; k < u->controls.size(); ++k) {   // rows [cond | uncond] of image b both use hint b % n_hint
+  for (size_t k = 0; k < u->controls.size(); ++k) {   // every row group's row of image b uses hint b % n_hint
     const ControlAttach& a = *u->controls[k];
     if (Bimg % a.n_hint) return fail(c, 5204, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bimg, a.n_hint);
     if (a.h != h || a.w != w)
       return fail(c, 5205, "control %zu: its hint is %dx%d pixels but the resolution is %dx%d", k, 8 * a.h, 8 * a.w, 8 * h, 8 * w);
   }
-  if (u->t2i) {   // the CFG rows of image b both use feature set b % n_hint
+  if (u->t2i) {   // every row group's row of image b uses feature set b % n_hint
     const T2IAttach& a = *u->t2i;
     if (Bimg % a.n_hint) return fail(c, 5206, "T2I-Adapter: batch %d is not a multiple of n_hint = %d", Bimg, a.n_hint);
     if (a.h != h || a.w != w)
       return fail(c, 5207, "T2I-Adapter: its hint is %dx%d pixels but the resolution is %dx%d", 8 * a.h, 8 * a.w, 8 * h, 8 * w);
   }
-  if (int r = ip_check_batch_all(u, nfwd * Bimg, nfwd == 2 ? Bimg : 0)) return r;
+  if (int r = ip_check_batch_all(u, nfwd * Bimg, layout)) return r;
   if (u->ip)
     for (const IpPrompt& a : u->ip->prompts)
       if (int r = ip_mask_check(u, a, h, w)) return r;
@@ -2288,17 +2372,24 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
     CU(c, cudaMallocHost((void**)&S->host_stage, lat * sizeof(float)));
   }
   S->guidance = (float)guidance;
+  S->cfg = use_cfg;
+  S->pag = pag;
   const cudaMemcpyKind kind = cond->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
   const size_t ctx_row = (size_t)n_ctx * g.context_dim * 2, y_row = (size_t)g.adm_in_channels * 2;
   CU(c, cudaMemcpyAsync(S->cond_ctx, ctx_c, ctx_row * Bimg, kind, c->stream));
   CU(c, cudaMemcpyAsync(S->cond_y, y_c, y_row * Bimg, kind, c->stream));
-  if (nfwd == 2)
+  if (use_cfg)
     for (int b = 0; b < Bimg; ++b) {  // unsqueeze().repeat(0, n_batch)
       CU(c, cudaMemcpyAsync((uint8_t*)S->cond_ctx + ctx_row * (Bimg + b), ctx_u, ctx_row, kind, c->stream));
       CU(c, cudaMemcpyAsync((uint8_t*)S->cond_y + y_row * (Bimg + b), y_u, y_row, kind, c->stream));
     }
-  int r = set_conditioning_dev(u, nfwd * Bimg, n_ctx, S->cond_ctx, S->cond_y, nfwd == 2 ? Bimg : 0);
-  if (!r) r = ensure_plan(u, nfwd * Bimg, Bimg, h, w);
+  if (pag) {   // the perturbed group repeats the conditional rows
+    const int g0 = (nfwd - 1) * Bimg;
+    CU(c, cudaMemcpyAsync((uint8_t*)S->cond_ctx + ctx_row * g0, S->cond_ctx, ctx_row * Bimg, cudaMemcpyDeviceToDevice, c->stream));
+    CU(c, cudaMemcpyAsync((uint8_t*)S->cond_y + y_row * g0, S->cond_y, y_row * Bimg, cudaMemcpyDeviceToDevice, c->stream));
+  }
+  int r = set_conditioning_dev(u, nfwd * Bimg, n_ctx, S->cond_ctx, S->cond_y, layout);
+  if (!r) r = ensure_plan(u, nfwd * Bimg, Bimg, h, w, pag ? Bimg : 0);
   if (r || !fresh) return r;
   CU(c, cudaStreamSynchronize(c->stream));   // the old sampler's buffers may still be in flight
   u->sampler = std::move(fresh);
@@ -2317,6 +2408,14 @@ static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   int r = set_t(u, t);
   if (r) return r;
   if ((r = run_plan(u))) return r;
+  if (S->pag) {
+    // diffusers' adaptive scaling: p_t = max(scale - adaptive * (n_steps - t), 0)
+    const PagAttach& pg = *u->pag;
+    const float p_t = std::max(pg.scale - pg.adaptive * (float)(u->cfg.n_steps - t), 0.f);
+    KL(c, cfg_pag_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->cfg, S->guidance, p_t,
+                              (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap), P->x_in));
+    return 0;
+  }
   KL(c, cfg_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->nfwd == 2, S->guidance,
                         (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap), P->x_in, nullptr));
   return 0;

@@ -233,6 +233,13 @@ int nhwc_to_nchw_f32_launch(cudaStream_t st, const float* x, int B, int HW, int 
 int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg,
                     float guidance, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
                     float* x, __half* x16);
+// The same update with perturbed-attention guidance (DESIGN.md §14): eps rows [cond | uncond | ptb] (use_cfg) or [cond | ptb];
+// e = (u + (c - u) * guidance) + p_t * (c - ptb), resp. c + p_t * (c - ptb).
+int cfg_pag_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance, float p_t,
+                        float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x);
+// PAG's identity self-attention on `rows` token rows: out[r, 0:C] = qkv[r, 2C:3C] (qkv row pitch 3C, out row pitch C); C % 8 == 0,
+// both pointers 16-byte aligned.
+int pag_identity_launch(cudaStream_t st, const __half* qkv, int C, long rows, __half* out);
 // x = mask ? x : ref*sqrt_a + noise*sqrt_1ma ; also refreshes x16 (both forwards).
 int inpaint_blend_launch(cudaStream_t st, float* x, const float* ref, const float* noise,
                          const uint8_t* mask, size_t n_per_img_batch, int nfwd, float sqrt_a,

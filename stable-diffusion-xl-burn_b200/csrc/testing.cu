@@ -131,6 +131,16 @@ SDXL_TEST_API int sdxl_test_conv_in_cat(void* stream, const void* x, int x_f32, 
   return conv_in_cat_launch((cudaStream_t)stream, x, x_f32, Bx, B, C1, x2, n2, C2, H, W, w, bias, Cout, y);
 }
 
+// PAG's identity self-attention on `rows` rows of a fused QKV matrix (pitch 3C) into out (pitch C), as the plan's OP_PAG_IDENTITY.
+SDXL_TEST_API int sdxl_test_pag_identity(void* stream, const void* qkv, int C, long rows, void* out) {
+  return pag_identity_launch((cudaStream_t)stream, (const __half*)qkv, C, rows, (__half*)out);
+}
+// The sampler's guided DDIM update with PAG (engine.cu: sampler_step).
+SDXL_TEST_API int sdxl_test_cfg_pag_ddim(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance,
+                                         float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
+  return cfg_pag_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_cfg, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x);
+}
+
 SDXL_TEST_API int sdxl_test_repack_upconv(void* stream, const void* src, int O, int I, void* dst, int Ipad) {
   return repack_upconv_launch((cudaStream_t)stream, (const __half*)src, O, I, (__half*)dst, Ipad);
 }

@@ -14,5 +14,6 @@ from . import diffusers_unet  # noqa: F401
 from .controlnet import ControlNet  # noqa: F401
 from .ip_adapter import IPAdapter  # noqa: F401
 from .t2i_adapter import T2IAdapter, t2i_t_min  # noqa: F401
+from .pag import layer_mask as pag_layer_mask, pag_scale_at, self_attention_names  # noqa: F401
 from .clip_vision import SDXL_VIT_BIGG, SDXL_VIT_H, ClipVisionConfig, ClipVisionEncoder, clip_preprocess  # noqa: F401
 from . import burn_record  # noqa: F401

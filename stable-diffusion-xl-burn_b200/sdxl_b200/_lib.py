@@ -111,6 +111,11 @@ class InpaintCondition(C.Structure):
     _fields_ = [("cond", C.c_void_p), ("on_host", C.c_int32), ("n", C.c_int32), ("height", C.c_int32), ("width", C.c_int32)]
 
 
+class Pag(C.Structure):
+    _fields_ = [("scale", C.c_float), ("adaptive_scale", C.c_float), ("n_layers", C.c_int32), ("layers_host", C.c_void_p),
+                ("forward_perturbed_rows", C.c_int32)]
+
+
 # name -> (restype, argtypes); every symbol include/sdxl_b200.h declares
 P = C.c_void_p
 I = C.c_int
@@ -191,6 +196,8 @@ PROTOTYPES = {
     "sdxl_unet_set_t2i_adapters": (I, [P, I, C.POINTER(T2IControl), C.c_int32]),
     "sdxl_t2i_adapter_features": (I, [P, I, I, I, P, I, P]),
     "sdxl_unet_set_inpaint_condition": (I, [P, C.POINTER(InpaintCondition)]),
+    "sdxl_unet_num_self_attentions": (I, [P]),
+    "sdxl_unet_set_pag": (I, [P, C.POINTER(Pag)]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),
     "sdxl_mpk_encode_u16": (C.c_size_t, [P, C.c_size_t, P]),

@@ -30,6 +30,8 @@ PROTOTYPES = {
     "sdxl_test_gemv": (I, [P, P, I, I, I, P, I, P, P, I, I, I, I, P, I]),
     "sdxl_test_conv_in": (I, [P, P, I, I, I, I, I, I, P, P, I, P, P, I]),
     "sdxl_test_conv_in_cat": (I, [P, P, I, I, I, I, P, I, I, I, I, P, P, I, P]),
+    "sdxl_test_pag_identity": (I, [P, P, I, C.c_long, P]),
+    "sdxl_test_cfg_pag_ddim": (I, [P, P, I, I, I, I, I, F, F, F, F, F, F, P]),
     "sdxl_test_repack_upconv": (I, [P, P, I, I, P, I]),
     "sdxl_test_repack_conv": (I, [P, P, I, I, I, I, P, I, I, I]),
     "sdxl_test_transpose_linear": (I, [P, P, I, I, P, I, I, I]),
@@ -145,6 +147,16 @@ def conv_in(x, Bx, B, Cin, H, W, w, bias, Cout, y, add=None, n_add=1) -> None:
 def conv_in_cat(x, Bx, B, C1, x2, n2, C2, H, W, w, bias, Cout, y) -> None:
     """The inpainting UNet's first conv: channels [0, C1) from x (f16 or f32), [C1, C1 + C2) from x2 f32 [n2, C2, H, W]."""
     _call("sdxl_test_conv_in_cat", _p(x), int(x.dtype == torch.float32), Bx, B, C1, _p(x2), n2, C2, H, W, _p(w), _p(bias), Cout, _p(y))
+
+
+def pag_identity(qkv: torch.Tensor, C: int, rows: int, out: torch.Tensor) -> None:
+    """out[r, :C] = qkv[r, 2C:3C] for r < rows; qkv f16 [rows, 3C], out f16 [rows, C]."""
+    _call("sdxl_test_pag_identity", _p(qkv), C, rows, _p(out))
+
+
+def cfg_pag_ddim(eps, ld, Bimg, C, HW, use_cfg, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x) -> None:
+    """x f32 NCHW [Bimg, C, HW] updated in place from eps NHWC f32 [groups * Bimg, HW, ld]."""
+    _call("sdxl_test_cfg_pag_ddim", _p(eps), ld, Bimg, C, HW, int(use_cfg), guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, _p(x))
 
 
 def repack_upconv(src, O, I, dst, Ipad) -> None:

@@ -349,6 +349,30 @@ class Diffuser:
         ctx.check(ctx.lib.sdxl_unet_set_inpaint_condition(self.h, None if s is None else C.byref(s)), "sdxl_unet_set_inpaint_condition")
         ctx.leave()
 
+    def set_pag(self, layers="mid", scale: float = 3.0, adaptive_scale: float = 0.0) -> None:
+        """Attaches perturbed-attention guidance (sdxl_unet_set_pag, DESIGN.md §14); layers None or scale 0 detaches. layers: diffusers'
+        pag_applied_layers, one regular expression or a list (pag.layer_mask); the sampler then runs the row groups [cond | uncond |
+        perturbed] and adds scale * (cond - perturbed) to the guided noise (adaptive_scale: diffusers' pag_adaptive_scale)."""
+        if layers is None or scale == 0:
+            self._pag = None
+            self._set_pag(None)
+            return
+        from .pag import layer_mask
+        mask = layer_mask(self.cfg, layers)
+        self._set_pag((mask, float(scale), float(adaptive_scale), 0))
+        self._pag = (mask, float(scale), float(adaptive_scale))
+
+    def _set_pag(self, p) -> None:
+        s, keep = None, None
+        if p is not None:
+            mask, scale, adaptive, rows = p
+            keep = (C.c_uint8 * len(mask))(*mask)
+            s = _lib.Pag()
+            s.scale, s.adaptive_scale, s.n_layers, s.layers_host, s.forward_perturbed_rows = scale, adaptive, len(mask), C.addressof(keep), rows
+        self.ctx.enter()
+        self.ctx.check(self.ctx.lib.sdxl_unet_set_pag(self.h, None if s is None else C.byref(s)), "sdxl_unet_set_pag")
+        self.ctx.leave()
+
     @classmethod
     def from_diffusers_dir(cls, ctx: Context, path: str) -> "Diffuser":
         """A diffusers UNet2DConditionModel directory (the `unet/` folder of an SDXL pipeline, base or inpainting): config.json +
@@ -370,10 +394,17 @@ class Diffuser:
         self._keep = (context, label)
 
     def unet_forward(self, x: torch.Tensor, timesteps, context: Optional[torch.Tensor] = None,
-                     label: Optional[torch.Tensor] = None) -> torch.Tensor:
+                     label: Optional[torch.Tensor] = None, perturbed_rows: Optional[int] = None) -> torch.Tensor:
         """== UNet::forward(x [B,4,h,w], timesteps Int[1], context [B,77,Cctx], label [B,adm]).
-        f32 in -> f32 out (no I/O rounding), f16 in -> f16 out (the reference's tensors)."""
+        f32 in -> f32 out (no I/O rounding), f16 in -> f16 out (the reference's tensors). perturbed_rows (PAG attached, set_pag): the
+        last this-many rows of the batch run the attached layers' identity self-attention, from this forward on (0: none)."""
         ctx = self.ctx
+        if perturbed_rows is not None:
+            if getattr(self, "_pag", None) is None:
+                if perturbed_rows:
+                    raise SdxlError("unet_forward: perturbed_rows needs PAG attached (set_pag)")
+            else:
+                self._set_pag((*self._pag, int(perturbed_rows)))
         if context is not None:
             self.set_conditioning(context, label)
         t = int(timesteps[0]) if hasattr(timesteps, "__len__") else int(timesteps)
@@ -406,7 +437,7 @@ class Diffuser:
     KIND_NAMES = ["igemm_wgmma", "attention_wgmma", "group_norm", "layer_norm", "gemv", "timestep_embedding",
                   "conv_in", "upsample2x", "phase_split", "cast_f16"]
     # kinds only the UNet plan launches, by kind index (KIND_NAMES is positional and LatentDecoder.KIND_NAMES extends it)
-    UNET_KINDS = {17: "t2i_add"}
+    UNET_KINDS = {17: "t2i_add", 18: "pag_identity"}
 
     def profile_plan(self) -> Dict[str, Dict[str, float]]:
         """Per-kernel-kind device time (ms), algorithmic FLOPs and launch count of one plan execution."""
