@@ -155,9 +155,15 @@ struct ControlAttach;
 struct IpAttach;
 struct T2IAttach;
 
+// The latent extent (h, w) an attachment was made for, and its row count n: image b of a batch reads its row b % n.
+struct Extent {
+  int n = 0, h = 0, w = 0;
+  bool operator==(const Extent& o) const { return n == o.n && h == o.h && w == o.w; }
+};
+
 // An attached inpainting condition (sdxl_unet_set_inpaint_condition): f32 NCHW [n, in_channels - out_channels, h, w], owned.
 struct InpaintAttach {
-  int n = 0, h = 0, w = 0;   // latent extent
+  Extent ext;
   Arena mem;
   float* cond = nullptr;
 };
@@ -249,7 +255,7 @@ struct sdxl_unet : EncoderHalf {
 struct ControlAttach {
   const sdxl_controlnet* net = nullptr;
   float scale = 1.f;
-  int n_hint = 0, h = 0, w = 0;   // latent extent
+  Extent ext;                     // n: the hint's n_hint
   Arena mem;                      // zero-conv copies f16(s*W) / s*b, hint_emb f32 NHWC [n_hint, h, w, mc]
   std::vector<Lin> zero;
   float* hint_emb = nullptr;
@@ -337,7 +343,7 @@ struct sdxl_t2i_adapter {
 
 // The attached T2I-Adapter set: the scaled sum of the features F_k, f32 NHWC [n_hint, Hk, Wk, Ck], and the timestep window.
 struct T2IAttach {
-  int n_hint = 0, h = 0, w = 0;     // latent extent
+  Extent ext;                       // n: the hints' n_hint
   int C[4] = {}, H[4] = {}, W[4] = {};
   size_t points[3] = {};            // input blocks (indices into the block program) after which F_0..F_2 are added; F_3 after the middle
   Arena mem;
@@ -700,6 +706,26 @@ static int conv3x3_direct(sdxl_ctx* c, const __half* a, int Bn, int H, int W, in
                    1, cv.O, cv.b, nullptr, 0);
 }
 
+// Points x at a borrowed input of `bytes` in device memory: src itself, or with on_host a copy into T queued on the ctx stream (the
+// caller synchronises before it returns: src is the caller's memory). If T cannot allocate the copy, fails with code and fmt.
+template <class X, class... A>
+static int stage_in(sdxl_ctx* c, TmpBufs& T, const X* src, size_t bytes, int on_host, const X*& x, int code, const char* fmt, A... args) {
+  x = src;
+  if (!on_host) return 0;
+  X* d = (X*)T.get(bytes);
+  if (!d) return fail(c, code, fmt, args...);
+  CU(c, cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
+  x = d;
+  return 0;
+}
+
+// Copies a result from device memory to the caller's host memory and waits for it.
+static int stage_out(sdxl_ctx* c, void* host, const void* dev, size_t bytes) {
+  CU(c, cudaMemcpyAsync(host, dev, bytes, cudaMemcpyDeviceToHost, c->stream));
+  CU(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
 // Hint encoder (SGM input_hint_block): hint f32 NCHW [n, in, H, W] (device) -> f32 NHWC [n, H/8, W/8, mc]. Queued on the ctx stream.
 static int embed_hint(sdxl_controlnet* net, int n, int H, int W, const float* hint, float* out) {
   sdxl_ctx* c = net->ctx;
@@ -736,22 +762,14 @@ extern "C" int sdxl_controlnet_embed_hint(sdxl_controlnet* net, int n, int H, in
   const int mc = net->cfg.model_channels, h = H / 8, w = W / 8;
   TmpBufs T(c->stream);
   const size_t in_bytes = (size_t)n * net->ncfg.hint_in_channels * H * W * sizeof(float), out_elems = (size_t)n * h * w * mc;
-  float* x = (float*)hint;
-  if (on_host) {
-    x = (float*)T.get(in_bytes);
-    if (!x) return fail(c, 4711, "embed_hint: allocation failed");
-    CU(c, cudaMemcpyAsync(x, hint, in_bytes, cudaMemcpyHostToDevice, c->stream));
-  }
+  const float* x;
+  if (int r = stage_in(c, T, hint, in_bytes, on_host, x, 4711, "embed_hint: allocation failed")) return r;
   float* e = (float*)T.get(out_elems * sizeof(float));
   float* o = on_host ? (float*)T.get(out_elems * sizeof(float)) : out;
   if (!e || !o) return fail(c, 4711, "embed_hint: allocation failed");
   if (int r = embed_hint(net, n, H, W, x, e)) return r;
   KL(c, nhwc_to_nchw_f32_launch(c->stream, e, n, h * w, mc, mc, o));
-  if (on_host) {
-    CU(c, cudaMemcpyAsync(out, o, out_elems * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-  }
-  return 0;
+  return on_host ? stage_out(c, out, o, out_elems * sizeof(float)) : 0;
 }
 
 // ================================================================================================
@@ -787,7 +805,7 @@ struct UNetPlanBuilder : PlanBuilder {
       Op op{};
       op.kind = OP_CONV_IN;
       op.ci = {P->x_in, P->Bx, Bf, latent_channels(g), H, W, e.conv0_w, e.conv0_b, mc, x, hint, n_hint};
-      if (inpaint_layout(g)) { op.ci.x2 = ipc->cond; op.ci.n2 = ipc->n; op.ci.C2 = g.in_channels - g.out_channels; }
+      if (inpaint_layout(g)) { op.ci.x2 = ipc->cond; op.ci.n2 = ipc->ext.n; op.ci.C2 = g.in_channels - g.out_channels; }
       P->ops.push_back(op);
       P->flops += 2.0 * Bf * H * W * 9.0 * g.in_channels * mc;
     }
@@ -838,7 +856,7 @@ struct UNetPlanBuilder : PlanBuilder {
     if (a.C[k] != C || a.H[k] != H || a.W[k] != W) { err = fail(c, 5017, "T2I-Adapter feature %d shape mismatch", k); return; }
     Op op{};
     op.kind = OP_T2I_ADD;
-    op.ta = {x, a.F[k], (long)H * W * C, Bf, a.n_hint, u->t_dev, a.t_min};
+    op.ta = {x, a.F[k], (long)H * W * C, Bf, a.ext.n, u->t_dev, a.t_min};
     P->ops.push_back(op);
   }
 
@@ -1058,7 +1076,7 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
     float* csemb = B.buf<float>((size_t)Bf * ted);
     float* ctemb = B.buf<float>((size_t)Bf * e.temb_all.N);
     std::vector<Saved> cs;
-    float* cmid = B.encoder(e, te, ct1, csemb, ctemb, scr, a.hint_emb, a.n_hint, prefix, cs);
+    float* cmid = B.encoder(e, te, ct1, csemb, ctemb, scr, a.hint_emb, a.ext.n, prefix, cs);
     B.cond = &u->cond;
     B.kv_index = kv_unet;
     if (cs.size() != saved.size() || a.zero.size() != saved.size() + 1) return fail(c, 5006, "control %zu: skip count mismatch", k);
@@ -1105,50 +1123,42 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
   return B.err;
 }
 
-// An inpainting UNet runs only with a condition attached at the latent's extent, for a batch of images that is a multiple of its n
-// (n_img: the images, so both CFG rows of image b read condition row b % n).
-static int inpaint_check(sdxl_unet* u, int n_img, int h, int w) {
+// Whether every attachment fits a run of n_img images on an h x w latent: it was made for that latent, and n_img is a multiple of
+// its row count (every row group's row of image b reads attachment row b % n). An inpainting UNet runs only with a condition.
+static int attachments_fit(sdxl_unet* u, int n_img, int h, int w) {
   sdxl_ctx* c = u->ctx;
+  // what: the attachment, subject: what was sized ("its hint"), divisor: the name of its n; codes: extent, then divisor
+  auto fit = [&](const std::string& what, const char* subject, const Extent& e, const char* divisor, int code) {
+    if (e.h != h || e.w != w)
+      return fail(c, code, "%s: %s %dx%d pixels (latent %dx%d) but the latent is %dx%d", what.c_str(), subject, 8 * e.h, 8 * e.w, e.h,
+                  e.w, h, w);
+    if (n_img % e.n) return fail(c, code + 1, "%s: batch %d is not a multiple of %s = %d", what.c_str(), n_img, divisor, e.n);
+    return 0;
+  };
+  for (size_t k = 0; k < u->controls.size(); ++k)
+    if (int r = fit("control " + std::to_string(k), "its hint is", u->controls[k]->ext, "n_hint", 5012)) return r;
+  if (u->t2i)
+    if (int r = fit("T2I-Adapter", "its hint is", u->t2i->ext, "n_hint", 5015)) return r;
+  if (u->ip)
+    for (const IpPrompt& a : u->ip->prompts)
+      if (a.mask_h && (a.mask_h / 8 != h || a.mask_w / 8 != w))
+        return fail(c, 5021, "image prompt: its masks are %dx%d pixels (latent %dx%d) but the latent is %dx%d", a.mask_h, a.mask_w,
+                    a.mask_h / 8, a.mask_w / 8, h, w);
   if (!inpaint_layout(u->cfg)) return 0;
-  const InpaintAttach* a = u->inpaint.get();
-  if (!a) return fail(c, 5018, "inpainting UNet: no inpainting condition attached (call sdxl_unet_set_inpaint_condition first)");
-  if (a->h != h || a->w != w)
-    return fail(c, 5019, "inpainting condition: it is %dx%d pixels (latent %dx%d) but the latent is %dx%d", 8 * a->h, 8 * a->w, a->h, a->w, h, w);
-  if (n_img % a->n) return fail(c, 5020, "inpainting condition: batch %d is not a multiple of its n = %d", n_img, a->n);
-  return 0;
+  if (!u->inpaint) return fail(c, 5018, "inpainting UNet: no inpainting condition attached (call sdxl_unet_set_inpaint_condition first)");
+  return fit("inpainting condition", "it is", u->inpaint->ext, "its n", 5019);
 }
 
-// A masked image prompt runs only on the latent its masks cover.
-static int ip_mask_check(sdxl_unet* u, const IpPrompt& a, int h, int w) {
-  if (a.mask_h && (a.mask_h / 8 != h || a.mask_w / 8 != w))
-    return fail(u->ctx, 5021, "image prompt: its masks are %dx%d pixels (latent %dx%d) but the latent is %dx%d", a.mask_h, a.mask_w,
-                a.mask_h / 8, a.mask_w / 8, h, w);
-  return 0;
-}
-
-// Bp: the trailing rows that take PAG's identity self-attentions (0: none; PAG attached when > 0).
+// Bx: the images of the batch (the direct forward's B, the sampler's Bimg); Bp: the trailing rows that take PAG's identity
+// self-attentions (0: none; PAG attached when > 0).
 static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w, int Bp) {
   sdxl_ctx* c = u->ctx;
   if (u->cond.condB != Bf) return fail(c, 5010, "conditioning is set for batch %d but forward batch is %d (call sdxl_unet_set_conditioning first)", u->cond.condB, Bf);
   if (Bp < 0 || Bp >= Bf) return fail(c, 5023, "PAG: %d perturbed rows in a batch of %d (at least one row must be attended)", Bp, Bf);
-  for (size_t k = 0; k < u->controls.size(); ++k) {
-    const ControlAttach& a = *u->controls[k];
-    if (a.h != h || a.w != w)
-      return fail(c, 5012, "control %zu: its hint is %dx%d pixels (latent %dx%d) but the latent is %dx%d", k, 8 * a.h, 8 * a.w, a.h, a.w, h, w);
-    if (Bf % a.n_hint) return fail(c, 5013, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bf, a.n_hint);
-  }
   if (u->ip)
-    for (const IpPrompt& a : u->ip->prompts) {
+    for (const IpPrompt& a : u->ip->prompts)
       if (a.cond.condB != Bf) return fail(c, 5014, "image prompt: its K/V are hoisted for batch %d but the batch is %d", a.cond.condB, Bf);
-      if (int r = ip_mask_check(u, a, h, w)) return r;
-    }
-  if (u->t2i) {
-    const T2IAttach& a = *u->t2i;
-    if (a.h != h || a.w != w)
-      return fail(c, 5015, "T2I-Adapter: its hint is %dx%d pixels (latent %dx%d) but the latent is %dx%d", 8 * a.h, 8 * a.w, a.h, a.w, h, w);
-    if (Bf % a.n_hint) return fail(c, 5016, "T2I-Adapter: batch %d is not a multiple of n_hint = %d", Bf, a.n_hint);
-  }
-  if (int r = inpaint_check(u, Bf, h, w)) return r;
+  if (int r = attachments_fit(u, Bx, h, w)) return r;
   // every change of the buffers or attachments a plan reads drops the plan, so the shapes and the perturbed rows are its whole cache key
   if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan_ptb == Bp) return 0;
   if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A, Bp); })) return r;
@@ -1336,6 +1346,40 @@ static const char* unet_cfg_mismatch(const sdxl_unet_cfg& g, const sdxl_unet_cfg
   return nullptr;
 }
 
+static const sdxl_unet_cfg& unet_cfg_of(const sdxl_controlnet& n) { return n.cfg; }
+template <class O> static const sdxl_unet_cfg& unet_cfg_of(const O& o) { return o.cfg.unet; }
+
+// Refuses an object that cannot be attached to u: null, made on another sdxl_ctx, or built for another UNet cfg. what, k: the
+// entry point and the item, for the messages; codes: the three refusals' codes in that order.
+template <class O>
+static int attachable(sdxl_unet* u, const char* what, int k, const O* obj, const int (&codes)[3]) {
+  sdxl_ctx* c = u->ctx;
+  if (!obj) return fail(c, codes[0], "%s %d: null object", what, k);
+  if (obj->ctx != c) return fail(c, codes[1], "%s %d: created on another sdxl_ctx", what, k);
+  if (const char* field = unet_cfg_mismatch(u->cfg, unet_cfg_of(*obj)))
+    return fail(c, codes[2], "%s %d: cfg field '%s' differs from the UNet's", what, k, field);
+  return 0;
+}
+
+// Moves a new attachment into its slot of u. The plan reads the old one and may still be in flight: the stream is drained and the
+// plan dropped first.
+template <class S>
+static int attach_install(sdxl_unet* u, S& slot, S fresh) {
+  CU(u->ctx, cudaStreamSynchronize(u->ctx->stream));
+  u->plan.reset();
+  slot = std::move(fresh);
+  return 0;
+}
+
+template <class T> static bool slot_empty(const std::unique_ptr<T>& s) { return !s; }
+template <class T> static bool slot_empty(const std::vector<T>& s) { return s.empty(); }
+
+// Empties a slot of u; an empty slot keeps the plan.
+template <class S>
+static int attach_detach(sdxl_unet* u, S& slot) {
+  return slot_empty(slot) ? 0 : attach_install(u, slot, S());
+}
+
 // Writes the per-attachment buffers that depend on scale and hint values: f16(s*W) / s*b of every zero conv, and hint_emb.
 static int control_write(sdxl_ctx* c, ControlAttach& a, const sdxl_control& ctl) {
   const sdxl_controlnet* n = a.net;
@@ -1345,14 +1389,10 @@ static int control_write(sdxl_ctx* c, ControlAttach& a, const sdxl_control& ctl)
   }
   a.scale = ctl.scale;
   TmpBufs T(c->stream);
-  const float* hint = ctl.hint;
-  if (ctl.hint_on_host) {
-    const size_t bytes = (size_t)ctl.n_hint * n->ncfg.hint_in_channels * ctl.height * ctl.width * sizeof(float);
-    float* d = (float*)T.get(bytes);
-    if (!d) return fail(c, 4720, "set_controls: cannot allocate %zu bytes for the hint", bytes);
-    CU(c, cudaMemcpyAsync(d, ctl.hint, bytes, cudaMemcpyHostToDevice, c->stream));
-    hint = d;
-  }
+  const size_t bytes = (size_t)ctl.n_hint * n->ncfg.hint_in_channels * ctl.height * ctl.width * sizeof(float);
+  const float* hint;
+  if (int r = stage_in(c, T, ctl.hint, bytes, ctl.hint_on_host, hint, 4720, "set_controls: cannot allocate %zu bytes for the hint", bytes))
+    return r;
   int r = embed_hint(const_cast<sdxl_controlnet*>(n), ctl.n_hint, ctl.height, ctl.width, hint, a.hint_emb);
   if (!r && ctl.hint_on_host) CU(c, cudaStreamSynchronize(c->stream));   // the caller may reuse its host memory
   return r;
@@ -1367,22 +1407,18 @@ extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* c
   if (n > 0 && !ctl) return fail(c, 4731, "set_controls: null control array");
   const sdxl_unet_cfg& g = u->cfg;
   for (int k = 0; k < n; ++k) {
-    const sdxl_controlnet* net = ctl[k].net;
-    if (!net) return fail(c, 4732, "set_controls: control %d has a null net", k);
-    if (net->ctx != c) return fail(c, 4733, "set_controls: control %d: the net was created on another sdxl_ctx", k);
-    if (const char* field = unet_cfg_mismatch(g, net->cfg)) return fail(c, 4734, "set_controls: control %d: cfg field '%s' differs from the UNet's", k, field);
+    if (int r = attachable(u, "set_controls: control", k, ctl[k].net, {4732, 4733, 4734})) return r;
     if (ctl[k].n_hint < 1) return fail(c, 4735, "set_controls: control %d: n_hint = %d must be >= 1", k, ctl[k].n_hint);
     if (!ctl[k].hint) return fail(c, 4736, "set_controls: control %d: null hint", k);
     if (ctl[k].height < 8 || ctl[k].width < 8 || ctl[k].height % 8 || ctl[k].width % 8)
       return fail(c, 4737, "set_controls: control %d: hint size %dx%d must be a positive multiple of 8", k, ctl[k].height, ctl[k].width);
     if (!isfinite(ctl[k].scale)) return fail(c, 4738, "set_controls: control %d: scale is not finite", k);
   }
+  if (n == 0) return attach_detach(u, u->controls);
   // same nets, n_hint and sizes: only scales and hint values change, the launch plan stays valid
-  bool in_place = (size_t)n == u->controls.size() && n > 0;
-  for (int k = 0; k < n && in_place; ++k) {
-    const ControlAttach& a = *u->controls[k];
-    in_place = a.net == ctl[k].net && a.n_hint == ctl[k].n_hint && a.h == ctl[k].height / 8 && a.w == ctl[k].width / 8;
-  }
+  auto extent = [&](int k) { return Extent{ctl[k].n_hint, ctl[k].height / 8, ctl[k].width / 8}; };
+  bool in_place = (size_t)n == u->controls.size();
+  for (int k = 0; k < n && in_place; ++k) in_place = u->controls[k]->net == ctl[k].net && u->controls[k]->ext == extent(k);
   if (in_place) {   // not staged: a runtime failure of control k leaves 0..k-1 rewritten (documented in include/sdxl_b200.h)
     for (int k = 0; k < n; ++k)
       if (int r = control_write(c, *u->controls[k], ctl[k])) return r;
@@ -1393,9 +1429,7 @@ extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* c
     std::unique_ptr<ControlAttach> a(new ControlAttach());
     const sdxl_controlnet* net = ctl[k].net;
     a->net = net;
-    a->n_hint = ctl[k].n_hint;
-    a->h = ctl[k].height / 8;
-    a->w = ctl[k].width / 8;
+    a->ext = extent(k);
     if (int r = carve_measured(c, a->mem, 4739, "set_controls: control buffers", [&](Arena& A) {
           a->zero.clear();
           for (const Conv& z : net->zero) {
@@ -1405,7 +1439,7 @@ extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* c
             L.b = A.get<float>(z.O);
             a->zero.push_back(L);
           }
-          a->hint_emb = A.get<float>((size_t)a->n_hint * a->h * a->w * g.model_channels);
+          a->hint_emb = A.get<float>((size_t)a->ext.n * a->ext.h * a->ext.w * g.model_channels);
           return 0;
         }))
       return r;
@@ -1416,10 +1450,7 @@ extern "C" int sdxl_unet_set_controls(sdxl_unet* u, int n, const sdxl_control* c
     }
     fresh.push_back(std::move(a));
   }
-  CU(c, cudaStreamSynchronize(c->stream));   // the old plan and attachments may still be in flight
-  u->plan.reset();
-  u->controls = std::move(fresh);
-  return 0;
+  return attach_install(u, u->controls, std::move(fresh));
 }
 
 
@@ -1609,21 +1640,12 @@ extern "C" int sdxl_ip_adapter_resample(sdxl_ip_adapter* a, int n, int seq_len, 
   TmpBufs T(c->stream);
   const size_t in_bytes = (size_t)n * seq_len * a->cfg.image_embed_dim * sizeof(float);
   const size_t out_bytes = (size_t)n * a->cfg.tokens_per_image * a->cfg.unet.context_dim * sizeof(__half);
-  const float* e = hidden;
-  __half* o = (__half*)tokens_out;
-  if (on_host) {
-    float* d = (float*)T.get(in_bytes);
-    o = (__half*)T.get(out_bytes);
-    if (!d || !o) return fail(c, 4811, "ip_adapter_resample: allocation failed");
-    CU(c, cudaMemcpyAsync(d, hidden, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    e = d;
-  }
+  const float* e;
+  if (int r = stage_in(c, T, hidden, in_bytes, on_host, e, 4811, "ip_adapter_resample: allocation failed")) return r;
+  __half* o = on_host ? (__half*)T.get(out_bytes) : (__half*)tokens_out;
+  if (!o) return fail(c, 4811, "ip_adapter_resample: allocation failed");
   if (int r = ip_resample(a, n, seq_len, e, o)) return r;
-  if (on_host) {
-    CU(c, cudaMemcpyAsync(tokens_out, o, out_bytes, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-  }
-  return 0;
+  return on_host ? stage_out(c, tokens_out, o, out_bytes) : 0;
 }
 
 extern "C" int sdxl_ip_adapter_project(sdxl_ip_adapter* a, int n, const float* embeds, int on_host, sdxl_half* tokens_out) {
@@ -1634,21 +1656,12 @@ extern "C" int sdxl_ip_adapter_project(sdxl_ip_adapter* a, int n, const float* e
   TmpBufs T(c->stream);
   const size_t in_bytes = (size_t)n * a->cfg.image_embed_dim * sizeof(float);
   const size_t out_bytes = (size_t)n * a->cfg.tokens_per_image * a->cfg.unet.context_dim * sizeof(__half);
-  const float* e = embeds;
-  __half* o = (__half*)tokens_out;
-  if (on_host) {
-    float* d = (float*)T.get(in_bytes);
-    o = (__half*)T.get(out_bytes);
-    if (!d || !o) return fail(c, 4811, "ip_adapter_project: allocation failed");
-    CU(c, cudaMemcpyAsync(d, embeds, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    e = d;
-  }
+  const float* e;
+  if (int r = stage_in(c, T, embeds, in_bytes, on_host, e, 4811, "ip_adapter_project: allocation failed")) return r;
+  __half* o = on_host ? (__half*)T.get(out_bytes) : (__half*)tokens_out;
+  if (!o) return fail(c, 4811, "ip_adapter_project: allocation failed");
   if (int r = ip_project(a, n, e, o)) return r;
-  if (on_host) {
-    CU(c, cudaMemcpyAsync(tokens_out, o, out_bytes, cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-  }
-  return 0;
+  return on_host ? stage_out(c, tokens_out, o, out_bytes) : 0;
 }
 
 // One prompt's values computed into temporaries: the tokens of prompts and negatives, the per-block scales and the masks resized
@@ -1677,18 +1690,16 @@ static int ip_stage(sdxl_ctx* c, int n_levels, const IpPrompt& a, const sdxl_ima
   s.tok_bytes = (size_t)a.n_batch * a.S_ip * a.ad->cfg.unet.context_dim * sizeof(__half);
   const int rows = a.ad->plus() ? p.seq_len : 1;   // input rows per image: Plus hidden states, or one embedding
   const size_t bytes = (size_t)n * rows * a.ad->cfg.image_embed_dim * sizeof(float);
-  const float* e = p.embeds;
-  const float* neg = p.negative_embeds;
-  if (p.on_host || !neg) {
-    float* d = (float*)T.get(2 * bytes);
-    if (!d) return fail(c, 4820, "set_image_prompt: cannot allocate %zu bytes for the embeddings", 2 * bytes);
-    if (p.on_host) {
-      CU(c, cudaMemcpyAsync(d, p.embeds, bytes, cudaMemcpyHostToDevice, c->stream));
-      e = d;
-    }
-    if (neg && p.on_host) CU(c, cudaMemcpyAsync(d + bytes / sizeof(float), neg, bytes, cudaMemcpyHostToDevice, c->stream));
-    else if (!neg) CU(c, cudaMemsetAsync(d + bytes / sizeof(float), 0, bytes, c->stream));   // diffusers' default negative: zeros
-    if (p.on_host || !neg) neg = d + bytes / sizeof(float);
+  const char* alloc_failed = "set_image_prompt: cannot allocate %zu bytes for the embeddings";
+  const float *e, *neg;
+  if (int r = stage_in(c, T, p.embeds, bytes, p.on_host, e, 4820, alloc_failed, bytes)) return r;
+  if (p.negative_embeds) {
+    if (int r = stage_in(c, T, p.negative_embeds, bytes, p.on_host, neg, 4820, alloc_failed, bytes)) return r;
+  } else {   // diffusers' default negative: zeros
+    float* z = (float*)T.get(bytes);
+    if (!z) return fail(c, 4820, alloc_failed, bytes);
+    CU(c, cudaMemsetAsync(z, 0, bytes, c->stream));
+    neg = z;
   }
   s.tp = (__half*)T.get(s.tok_bytes);
   s.tn = (__half*)T.get(s.tok_bytes);
@@ -1733,14 +1744,11 @@ static int ip_commit(sdxl_ctx* c, IpPrompt& a, const IpStaged& s) {
 }
 
 // The checks of one prompt that need no device work.
-static int ip_prompt_check(sdxl_unet* u, const sdxl_image_prompt* p) {
+static int ip_prompt_check(sdxl_unet* u, int k, const sdxl_image_prompt* p) {
   sdxl_ctx* c = u->ctx;
   const sdxl_ip_adapter* ad = p->adapter;
-  if (!ad) return fail(c, 4830, "set_image_prompt: null adapter");
-  if (ad->ctx != c) return fail(c, 4831, "set_image_prompt: the adapter was created on another sdxl_ctx");
   if (u->cfg.is_refiner) return fail(c, 4832, "set_image_prompt: IP-Adapter on the refiner is not supported");
-  if (const char* field = unet_cfg_mismatch(u->cfg, ad->cfg.unet))
-    return fail(c, 4833, "set_image_prompt: adapter cfg field '%s' differs from the UNet's", field);
+  if (int r = attachable(u, "set_image_prompt: prompt", k, ad, {4830, 4831, 4833})) return r;
   // equal cfgs: the adapter's K/V were laid out by the same block program as the UNet's transformer blocks
   const int n_tb = (int)ad->kv.size();
   if (!p->embeds) return fail(c, 4835, "set_image_prompt: null embeds");
@@ -1784,13 +1792,7 @@ extern "C" int sdxl_unet_set_image_prompts(sdxl_unet* u, int n, const sdxl_image
   CU(c, cudaSetDevice(c->device));
   if (n < 0 || n > SDXL_MAX_IMAGE_PROMPTS)
     return fail(c, 4841, "set_image_prompts: n = %d outside [0, %d]", n, SDXL_MAX_IMAGE_PROMPTS);
-  if (n == 0) {
-    if (!u->ip) return 0;
-    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
-    u->plan.reset();
-    u->ip.reset();
-    return 0;
-  }
+  if (n == 0) return attach_detach(u, u->ip);
   if (!prompts) return fail(c, -1, "set_image_prompts: null prompts");
   // validate everything first: on failure the attached set is unchanged
   const int nl = u->cfg.n_levels;
@@ -1799,7 +1801,7 @@ extern "C" int sdxl_unet_set_image_prompts(sdxl_unet* u, int n, const sdxl_image
   int n_src = 0;
   for (int k = 0; k < n; ++k) {
     const sdxl_image_prompt& p = prompts[k];
-    if (int r = ip_prompt_check(u, &p)) return r;
+    if (int r = ip_prompt_check(u, k, &p)) return r;
     const sdxl_ip_mask* m = masks && masks[k].mask ? &masks[k] : nullptr;
     IpPrompt& a = shape[k];
     a.ad = p.adapter;
@@ -1858,10 +1860,7 @@ extern "C" int sdxl_unet_set_image_prompts(sdxl_unet* u, int n, const sdxl_image
   if (condB > 0)
     for (IpPrompt& q : a->prompts)
       if (int r = ip_hoist(u, q)) return r;
-  CU(c, cudaStreamSynchronize(c->stream));   // the old plan and attachment may still be in flight
-  u->plan.reset();
-  u->ip = std::move(a);
-  return 0;
+  return attach_install(u, u->ip, std::move(a));
 }
 
 extern "C" int sdxl_unet_set_image_prompt(sdxl_unet* u, const sdxl_image_prompt* p) {
@@ -2018,17 +2017,10 @@ extern "C" int sdxl_t2i_adapter_features(sdxl_t2i_adapter* a, int n, int H, int 
     F[k] = (float*)T.get(t2i_feature_elems(a, k, n, H, W) * sizeof(float));
   }
   const size_t in_bytes = (size_t)n * a->cfg.in_channels * H * W * sizeof(float);
-  const float* x = hint;
-  float* o = out;
-  if (on_host) {
-    float* d = (float*)T.get(in_bytes);
-    o = (float*)T.get(total * sizeof(float));
-    if (!d || !o) return fail(c, 4911, "t2i_adapter_features: allocation failed");
-    CU(c, cudaMemcpyAsync(d, hint, in_bytes, cudaMemcpyHostToDevice, c->stream));
-    x = d;
-  }
-  for (int k = 0; k < 4; ++k)
-    if (!F[k]) return fail(c, 4911, "t2i_adapter_features: allocation failed");
+  const float* x;
+  if (int r = stage_in(c, T, hint, in_bytes, on_host, x, 4911, "t2i_adapter_features: allocation failed")) return r;
+  float* o = on_host ? (float*)T.get(total * sizeof(float)) : out;
+  if (!o || !F[0] || !F[1] || !F[2] || !F[3]) return fail(c, 4911, "t2i_adapter_features: allocation failed");
   if (int r = t2i_forward(a, n, H, W, x, F)) return r;
   size_t off = 0;
   for (int k = 0; k < 4; ++k) {
@@ -2036,11 +2028,7 @@ extern "C" int sdxl_t2i_adapter_features(sdxl_t2i_adapter* a, int n, int H, int 
     KL(c, nhwc_to_nchw_f32_launch(c->stream, F[k], n, (H / d) * (W / d), a->ch[k], a->ch[k], o + off));
     off += t2i_feature_elems(a, k, n, H, W);
   }
-  if (on_host) {
-    CU(c, cudaMemcpyAsync(out, o, total * sizeof(float), cudaMemcpyDeviceToHost, c->stream));
-    CU(c, cudaStreamSynchronize(c->stream));
-  }
-  return 0;
+  return on_host ? stage_out(c, out, o, total * sizeof(float)) : 0;
 }
 
 extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_control* ctl, int32_t t_min) {
@@ -2053,11 +2041,7 @@ extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_co
   if (n > 0)
     if (const char* why = t2i_unet_problem(u->cfg)) return fail(c, 4932, "set_t2i_adapters: %s", why);
   for (int k = 0; k < n; ++k) {
-    const sdxl_t2i_adapter* a = ctl[k].adapter;
-    if (!a) return fail(c, 4933, "set_t2i_adapters: item %d has a null adapter", k);
-    if (a->ctx != c) return fail(c, 4934, "set_t2i_adapters: item %d: the adapter was created on another sdxl_ctx", k);
-    if (const char* field = unet_cfg_mismatch(u->cfg, a->cfg.unet))
-      return fail(c, 4935, "set_t2i_adapters: item %d: adapter cfg field '%s' differs from the UNet's", k, field);
+    if (int r = attachable(u, "set_t2i_adapters: item", k, ctl[k].adapter, {4933, 4934, 4935})) return r;
     if (!ctl[k].hint) return fail(c, 4936, "set_t2i_adapters: item %d: null hint", k);
     if (ctl[k].n_hint < 1) return fail(c, 4937, "set_t2i_adapters: item %d: n_hint = %d must be >= 1", k, ctl[k].n_hint);
     if (ctl[k].n_hint != ctl[0].n_hint || ctl[k].height != ctl[0].height || ctl[k].width != ctl[0].width)
@@ -2066,14 +2050,9 @@ extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_co
     if (int r = t2i_check_size(c, ctl[k].n_hint, ctl[k].height, ctl[k].width)) return r;
     if (!isfinite(ctl[k].scale)) return fail(c, 4939, "set_t2i_adapters: item %d: scale is not finite", k);
   }
-  if (n == 0) {
-    if (!u->t2i) return 0;
-    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
-    u->plan.reset();
-    u->t2i.reset();
-    return 0;
-  }
+  if (n == 0) return attach_detach(u, u->t2i);
   const int n_hint = ctl[0].n_hint, H = ctl[0].height, W = ctl[0].width;
+  const Extent ext{n_hint, H / 8, W / 8};
   const sdxl_t2i_adapter* a0 = ctl[0].adapter;
   // the sum is formed in temporaries and copied into the attachment only when all of it succeeded
   TmpBufs T(c->stream);
@@ -2088,14 +2067,11 @@ extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_co
   if (!ok) return fail(c, 4940, "set_t2i_adapters: cannot allocate the feature staging buffers");
   for (int k = 0; k < 4; ++k) CU(c, cudaMemsetAsync(S[k], 0, t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float), c->stream));
   for (int i = 0; i < n; ++i) {
-    const float* hint = ctl[i].hint;
-    if (ctl[i].hint_on_host) {
-      const size_t bytes = (size_t)n_hint * ctl[i].adapter->cfg.in_channels * H * W * sizeof(float);
-      float* d = (float*)T.get(bytes);
-      if (!d) return fail(c, 4940, "set_t2i_adapters: cannot allocate %zu bytes for hint %d", bytes, i);
-      CU(c, cudaMemcpyAsync(d, ctl[i].hint, bytes, cudaMemcpyHostToDevice, c->stream));
-      hint = d;
-    }
+    const size_t bytes = (size_t)n_hint * ctl[i].adapter->cfg.in_channels * H * W * sizeof(float);
+    const float* hint;
+    if (int r = stage_in(c, T, ctl[i].hint, bytes, ctl[i].hint_on_host, hint, 4940, "set_t2i_adapters: cannot allocate %zu bytes for hint %d",
+                         bytes, i))
+      return r;
     if (int r = t2i_forward(ctl[i].adapter, n_hint, H, W, hint, Fa)) return r;
     for (int k = 0; k < 4; ++k)   // S += s_i * F_i, adapters in array order
       KL(c, axpby_launch(c->stream, S[k], Fa[k], t2i_feature_elems(a0, k, n_hint, H, W), 1.f, ctl[i].scale));
@@ -2103,10 +2079,10 @@ extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_co
   CU(c, cudaStreamSynchronize(c->stream));   // the caller's host hints; any failure of the work above surfaces here
   T2IAttach* cur = u->t2i.get();
   std::unique_ptr<T2IAttach> fresh;
-  if (!cur || cur->n_hint != n_hint || cur->h != H / 8 || cur->w != W / 8) {   // new shapes: new buffers and a new plan
+  if (!cur || !(cur->ext == ext)) {   // new shapes: new buffers and a new plan
     fresh.reset(new T2IAttach());
     T2IAttach& f = *fresh;
-    f.n_hint = n_hint; f.h = H / 8; f.w = W / 8;
+    f.ext = ext;
     t2i_points(block_program(u->cfg), f.points);
     for (int k = 0; k < 4; ++k) {
       const int d = k < 2 ? 16 : 32;
@@ -2123,11 +2099,8 @@ extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_co
   for (int k = 0; k < 4; ++k)
     CU(c, cudaMemcpyAsync(cur->F[k], S[k], t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
   CU(c, cudaMemcpyAsync(cur->t_min, &t_min, sizeof(int), cudaMemcpyHostToDevice, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));   // t_min is on the stack; the old plan and attachment may still be in flight
-  if (fresh) {
-    u->plan.reset();
-    u->t2i = std::move(fresh);
-  }
+  if (fresh) return attach_install(u, u->t2i, std::move(fresh));
+  CU(c, cudaStreamSynchronize(c->stream));   // t_min is on the stack
   return 0;
 }
 
@@ -2139,13 +2112,7 @@ extern "C" int sdxl_unet_set_inpaint_condition(sdxl_unet* u, const sdxl_inpaint_
   sdxl_ctx* c = u->ctx;
   CU(c, cudaSetDevice(c->device));
   const sdxl_unet_cfg& g = u->cfg;
-  if (!ic) {
-    if (!u->inpaint) return 0;
-    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
-    u->plan.reset();
-    u->inpaint.reset();
-    return 0;
-  }
+  if (!ic) return attach_detach(u, u->inpaint);
   // validate everything first: on failure the attached condition is unchanged
   if (!inpaint_layout(g))
     return fail(c, 4960, "set_inpaint_condition: the UNet does not have the inpainting layout (in_channels = %d, out_channels = %d; "
@@ -2154,13 +2121,13 @@ extern "C" int sdxl_unet_set_inpaint_condition(sdxl_unet* u, const sdxl_inpaint_
   if (ic->n < 1) return fail(c, 4962, "set_inpaint_condition: n = %d must be >= 1", ic->n);
   if (ic->height < 8 || ic->width < 8 || ic->height % 8 || ic->width % 8)
     return fail(c, 4963, "set_inpaint_condition: size %dx%d must be a positive multiple of 8", ic->height, ic->width);
-  const int n = ic->n, h = ic->height / 8, w = ic->width / 8;
-  const size_t bytes = (size_t)n * (g.in_channels - g.out_channels) * h * w * sizeof(float);
+  const Extent ext{ic->n, ic->height / 8, ic->width / 8};
+  const size_t bytes = (size_t)ext.n * (g.in_channels - g.out_channels) * ext.h * ext.w * sizeof(float);
   InpaintAttach* cur = u->inpaint.get();
   std::unique_ptr<InpaintAttach> fresh;
-  if (!cur || cur->n != n || cur->h != h || cur->w != w) {   // new shape: a new buffer and a new plan
+  if (!cur || !(cur->ext == ext)) {   // new shape: a new buffer and a new plan
     fresh.reset(new InpaintAttach());
-    fresh->n = n; fresh->h = h; fresh->w = w;
+    fresh->ext = ext;
     if (int r = carve_measured(c, fresh->mem, 4964, "set_inpaint_condition: condition buffer", [&](Arena& A) {
           fresh->cond = A.get<float>(bytes / sizeof(float));
           return 0;
@@ -2169,11 +2136,8 @@ extern "C" int sdxl_unet_set_inpaint_condition(sdxl_unet* u, const sdxl_inpaint_
     cur = fresh.get();
   }
   CU(c, cudaMemcpyAsync(cur->cond, ic->cond, bytes, ic->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
-  CU(c, cudaStreamSynchronize(c->stream));   // the caller's memory; the old plan and buffer may still be in flight
-  if (fresh) {
-    u->plan.reset();
-    u->inpaint = std::move(fresh);
-  }
+  if (fresh) return attach_install(u, u->inpaint, std::move(fresh));
+  CU(c, cudaStreamSynchronize(c->stream));   // the caller's memory
   return 0;
 }
 
@@ -2204,31 +2168,24 @@ extern "C" int sdxl_unet_set_pag(sdxl_unet* u, const sdxl_pag* p) {
   if (!u) return -1;
   sdxl_ctx* c = u->ctx;
   CU(c, cudaSetDevice(c->device));
-  if (!p) {
-    if (!u->pag) return 0;
-    CU(c, cudaStreamSynchronize(c->stream));   // the plan may still be in flight
-    u->plan.reset();
-    u->pag.reset();
-    return 0;
-  }
+  if (!p) return attach_detach(u, u->pag);
   // validate everything first: on failure the attached state is unchanged
   const int n = (int)u->tblocks.size();
-  if (!(isfinite(p->scale) && p->scale > 0.f)) return fail(c, 4900, "set_pag: scale = %g must be finite and > 0 (detach with NULL)", p->scale);
+  if (!(isfinite(p->scale) && p->scale > 0.f)) return fail(c, 4970, "set_pag: scale = %g must be finite and > 0 (detach with NULL)", p->scale);
   if (!(isfinite(p->adaptive_scale) && p->adaptive_scale >= 0.f))
-    return fail(c, 4901, "set_pag: adaptive_scale = %g must be finite and >= 0", p->adaptive_scale);
-  if (p->n_layers != n) return fail(c, 4902, "set_pag: n_layers = %d but the UNet has %d self-attentions", p->n_layers, n);
-  if (!p->layers_host) return fail(c, 4903, "set_pag: null layers_host");
+    return fail(c, 4971, "set_pag: adaptive_scale = %g must be finite and >= 0", p->adaptive_scale);
+  if (p->n_layers != n) return fail(c, 4972, "set_pag: n_layers = %d but the UNet has %d self-attentions", p->n_layers, n);
+  if (!p->layers_host) return fail(c, 4973, "set_pag: null layers_host");
   int n_sel = 0;
   for (int i = 0; i < n; ++i) n_sel += p->layers_host[i] != 0;
-  if (!n_sel) return fail(c, 4904, "set_pag: no self-attention selected");
-  if (p->forward_perturbed_rows < 0) return fail(c, 4905, "set_pag: forward_perturbed_rows = %d is negative", p->forward_perturbed_rows);
+  if (!n_sel) return fail(c, 4974, "set_pag: no self-attention selected");
+  if (p->forward_perturbed_rows < 0) return fail(c, 4975, "set_pag: forward_perturbed_rows = %d is negative", p->forward_perturbed_rows);
   std::vector<uint8_t> layers(n);
   for (int i = 0; i < n; ++i) layers[i] = p->layers_host[i] != 0;
   if (!u->pag || u->pag->layers != layers) {   // a new layer set changes the plan; the scales and the row count do not (ensure_plan)
-    CU(c, cudaStreamSynchronize(c->stream));
-    u->plan.reset();
-    if (!u->pag) u->pag.reset(new PagAttach());
-    u->pag->layers = std::move(layers);
+    std::unique_ptr<PagAttach> fresh(new PagAttach());
+    fresh->layers = std::move(layers);
+    if (int r = attach_install(u, u->pag, std::move(fresh))) return r;
   }
   u->pag->scale = p->scale;
   u->pag->adaptive = p->adaptive_scale;
@@ -2331,23 +2288,8 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
   const sdxl_half* y_u = g.is_refiner ? cond->unconditional_channel_context_refiner : cond->unconditional_channel_context;
   if (!ctx_c || !y_c || (use_cfg && (!ctx_u || !y_u))) return fail(c, 5201, "conditioning tensors for this model are null");
   if (Bimg < 1 || h < 1 || w < 1) return fail(c, 5202, "bad conditioning batch/resolution");
-  for (size_t k = 0; k < u->controls.size(); ++k) {   // every row group's row of image b uses hint b % n_hint
-    const ControlAttach& a = *u->controls[k];
-    if (Bimg % a.n_hint) return fail(c, 5204, "control %zu: batch %d is not a multiple of n_hint = %d", k, Bimg, a.n_hint);
-    if (a.h != h || a.w != w)
-      return fail(c, 5205, "control %zu: its hint is %dx%d pixels but the resolution is %dx%d", k, 8 * a.h, 8 * a.w, 8 * h, 8 * w);
-  }
-  if (u->t2i) {   // every row group's row of image b uses feature set b % n_hint
-    const T2IAttach& a = *u->t2i;
-    if (Bimg % a.n_hint) return fail(c, 5206, "T2I-Adapter: batch %d is not a multiple of n_hint = %d", Bimg, a.n_hint);
-    if (a.h != h || a.w != w)
-      return fail(c, 5207, "T2I-Adapter: its hint is %dx%d pixels but the resolution is %dx%d", 8 * a.h, 8 * a.w, 8 * h, 8 * w);
-  }
+  if (int r = attachments_fit(u, Bimg, h, w)) return r;
   if (int r = ip_check_batch_all(u, nfwd * Bimg, layout)) return r;
-  if (u->ip)
-    for (const IpPrompt& a : u->ip->prompts)
-      if (int r = ip_mask_check(u, a, h, w)) return r;
-  if (int r = inpaint_check(u, Bimg, h, w)) return r;
   Sampler* S = u->sampler.get();
   const size_t lat = (size_t)Bimg * latent_channels(g) * h * w;
   if (n_ctx < 1) return fail(c, 5202, "bad conditioning context length");

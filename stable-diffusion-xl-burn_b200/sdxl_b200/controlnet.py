@@ -2,9 +2,6 @@
 sdxl_controlnet_load. A net is attached to a UNet with Diffuser.set_controls or sample(..., controls=...)."""
 from __future__ import annotations
 
-import ctypes as C
-import json
-import os
 from typing import Dict, List, Tuple
 
 import torch
@@ -12,10 +9,10 @@ import torch
 from . import _lib
 from ._lib import SdxlError
 from .config import ControlNetConfig, block_program
-from .diffusers_unet import SDXL_DOWN_BLOCK_TYPES, _put, encoder_config, encoder_name_map, middle_name_map  # noqa: F401
-from .engine import _cfg_struct
-from .lora import read_safetensors
-from .weights import build_pack, controlnet_tensor_specs
+from .diffusers_unet import (SDXL_DOWN_BLOCK_TYPES, _put, encoder_config, encoder_name_map, middle_name_map,  # noqa: F401
+                             read_config, read_model_dir)
+from .engine import AttachableModel, _cfg_struct
+from .weights import controlnet_tensor_specs
 
 # ControlNet variants this loader does not implement, recognised by a key prefix or substring
 _FOREIGN = [("control_model.", "an SGM/ldm ControlNet checkpoint (convert it to diffusers format)"),
@@ -54,12 +51,7 @@ def from_diffusers(state_dict: Dict[str, torch.Tensor], config_json) -> Tuple[Co
     """A diffusers SDXL ControlNetModel (state dict + config.json as dict, JSON text or path) -> (config, pack-named f16 weights).
     Unsupported variants raise SdxlError naming the key or config field. A "bgr" conditioning_channel_order is folded into the
     first hint conv (its input channels are reversed), so hints are always passed as RGB."""
-    if isinstance(config_json, str):
-        if os.path.exists(config_json):
-            with open(config_json) as f:
-                config_json = json.load(f)
-        else:
-            config_json = json.loads(config_json)
+    config_json = read_config(config_json)
     for k in state_dict:
         for pat, what in _FOREIGN:
             if (k.startswith(pat) if pat.endswith(".") else pat in k):
@@ -93,36 +85,18 @@ def cfg_struct(cfg: ControlNetConfig) -> _lib.ControlNetCfg:
     return s
 
 
-class ControlNet:
+class ControlNet(AttachableModel):
     """A device-resident ControlNet (sdxl_controlnet_load). weights: pack-named tensor dict or a built pack."""
+    _load_fn, _destroy_fn, _detach_call = "sdxl_controlnet_load", "sdxl_controlnet_destroy", "set_controls([])"
 
     def __init__(self, ctx, cfg: ControlNetConfig, weights):
-        self.ctx, self.cfg = ctx, cfg
-        pack = weights if isinstance(weights, torch.Tensor) else build_pack(weights)
-        ctx.enter()
-        if pack.is_cuda:
-            torch.cuda.current_stream(ctx.device).synchronize()
-        cs = cfg_struct(cfg)
-        h = C.c_void_p()
-        ctx.check(ctx.lib.sdxl_controlnet_load(ctx.h, C.byref(cs), pack.data_ptr(), pack.numel(), int(pack.is_cuda), C.byref(h)),
-                  "sdxl_controlnet_load")
-        self.h = h
-        self.attached = 0   # attachments to UNets (set_controls); close() refuses while > 0
+        self.cfg = cfg
+        self._load(ctx, cfg_struct(cfg), weights)
 
     @classmethod
     def from_diffusers_dir(cls, ctx, path: str) -> "ControlNet":
         """A diffusers ControlNetModel directory: config.json + diffusion_pytorch_model[.fp16].safetensors."""
-        files = [f for f in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors")
-                 if os.path.exists(os.path.join(path, f))]
-        if not files:
-            raise SdxlError(f"{path}: no diffusion_pytorch_model[.fp16].safetensors")
-        cfg, w = from_diffusers(read_safetensors(os.path.join(path, files[0])), os.path.join(path, "config.json"))
-        return cls(ctx, cfg, w)
-
-    def handle(self) -> int:
-        if not getattr(self, "h", None):
-            raise SdxlError("ControlNet is closed")
-        return self.h.value
+        return cls(ctx, *from_diffusers(*read_model_dir(path)))
 
     def embed_hint(self, hint: torch.Tensor) -> torch.Tensor:
         """hint_emb [n, mc, H/8, W/8] f32 of hint f32 [n, 3, H, W] in [0, 1] (test aid)."""
@@ -131,24 +105,8 @@ class ControlNet:
         hint = hint_tensor(hint, self.cfg.hint_in_channels).to(ctx.device).contiguous()
         n, _, H, W = hint.shape
         out = torch.empty(n, self.cfg.unet.model_channels, H // 8, W // 8, device=ctx.device, dtype=torch.float32)
-        ctx.enter()
-        ctx.check(ctx.lib.sdxl_controlnet_embed_hint(h, n, H, W, hint.data_ptr(), 0, out.data_ptr()), "sdxl_controlnet_embed_hint")
-        ctx.leave()
+        ctx.call("sdxl_controlnet_embed_hint", ctx.lib.sdxl_controlnet_embed_hint, h, n, H, W, hint.data_ptr(), 0, out.data_ptr())
         return out
-
-    def close(self) -> None:
-        """Frees the device weights. Refused while the net is attached to a UNet: detach it first (set_controls([]))."""
-        if getattr(self, "attached", 0) > 0:
-            raise SdxlError("ControlNet.close: the net is still attached to a UNet (detach it with set_controls([]) first)")
-        if getattr(self, "h", None):
-            self.ctx.lib.sdxl_controlnet_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def hint_tensor(hint: torch.Tensor, channels: int) -> torch.Tensor:
@@ -179,17 +137,5 @@ def set_controls(diffuser, controls: List) -> None:
         arr[i].hint_on_host = 0
         arr[i].n_hint, arr[i].height, arr[i].width = h.shape[0], h.shape[2], h.shape[3]
         arr[i].scale = float(scale)
-    ctx.enter()
-    ctx.check(ctx.lib.sdxl_unet_set_controls(diffuser.h, len(controls), arr), "sdxl_unet_set_controls")
-    ctx.leave()
-    release_controls(diffuser)
-    diffuser._controls = [net for net, _, _ in controls]   # the nets stay alive, and cannot be closed, while attached
-    for net in diffuser._controls:
-        net.attached += 1
-
-
-def release_controls(diffuser) -> None:
-    """Forgets the diffuser's attached nets (after a detach, or when the UNet is destroyed)."""
-    for net in getattr(diffuser, "_controls", []):
-        net.attached -= 1
-    diffuser._controls = []
+    ctx.call("sdxl_unet_set_controls", ctx.lib.sdxl_unet_set_controls, diffuser.h, len(controls), arr)
+    diffuser._attach("controls", [net for net, _, _ in controls])

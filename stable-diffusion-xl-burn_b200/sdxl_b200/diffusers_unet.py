@@ -193,11 +193,12 @@ def from_diffusers(state_dict: Dict[str, torch.Tensor], config_json) -> Tuple[UN
     return cfg, out
 
 
-def read_diffusers_dir(path: str) -> Tuple[UNetConfig, Dict[str, torch.Tensor]]:
-    """A diffusers UNet directory (the `unet/` folder of a pipeline): config.json + diffusion_pytorch_model[.fp16].safetensors."""
+def read_model_dir(path: str) -> Tuple[Dict[str, torch.Tensor], str]:
+    """(state dict, config.json path) of a diffusers model directory (a UNet, ControlNetModel or T2IAdapter): config.json +
+    diffusion_pytorch_model[.fp16].safetensors, the fp16 file when both are there."""
     from .lora import read_safetensors
     files = [f for f in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors")
              if os.path.exists(os.path.join(path, f))]
     if not files:
         raise SdxlError(f"{path}: no diffusion_pytorch_model[.fp16].safetensors")
-    return from_diffusers(read_safetensors(os.path.join(path, files[0])), os.path.join(path, "config.json"))
+    return read_safetensors(os.path.join(path, files[0])), os.path.join(path, "config.json")

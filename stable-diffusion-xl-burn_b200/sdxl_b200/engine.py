@@ -56,6 +56,15 @@ class Context:
     def leave(self) -> None:
         torch.cuda.current_stream(self.device).wait_stream(self.stream)
 
+    def call(self, what: str, fn, *args) -> None:
+        """fn(*args): a library call queued on the ctx stream after torch's work so far; torch's stream then waits for it, also
+        when it fails. A failure raises SdxlError naming `what`."""
+        self.enter()
+        try:
+            self.check(fn(*args), what)
+        finally:
+            self.leave()
+
     def synchronize(self) -> None:
         self.check(self.lib.sdxl_ctx_synchronize(self.h), "sdxl_ctx_synchronize")
 
@@ -87,10 +96,8 @@ class Context:
                 raise SdxlError(f"qkv_attention: mask must be [{T},{S}], got {tuple(mask.shape)}")
             mask = mask.to(self.device, torch.float16).contiguous()
         out = torch.empty_like(q)
-        self.enter()
-        self.check(self.lib.sdxl_qkv_attention(self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(mask), B, T, S, Cc, n_head, _ptr(out)),
-                   "sdxl_qkv_attention")
-        self.leave()
+        self.call("sdxl_qkv_attention", self.lib.sdxl_qkv_attention, self.h, _ptr(q), _ptr(k), _ptr(v), _ptr(mask), B, T, S, Cc,
+                  n_head, _ptr(out))
         return out
 
     def linear(self, x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None,
@@ -106,10 +113,8 @@ class Context:
             out = torch.empty(M, N // 2, device=self.device, dtype=torch.float16)
         else:
             out = torch.empty(M, N, device=self.device, dtype=torch.float16 if out_f16 else torch.float32)
-        self.enter()
-        self.check(self.lib.sdxl_op_linear(self.h, _ptr(x), _ptr(w), _ptr(bias), _ptr(residual), M, K, N, int(geglu),
-                                           int(out_f16), _ptr(out)), "sdxl_op_linear")
-        self.leave()
+        self.call("sdxl_op_linear", self.lib.sdxl_op_linear, self.h, _ptr(x), _ptr(w), _ptr(bias), _ptr(residual), M, K, N, int(geglu),
+                  int(out_f16), _ptr(out))
         return out
 
     def conv2d(self, x_nhwc: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor], stride: int = 1,
@@ -122,10 +127,8 @@ class Context:
         Cout, _, ks, _ = w.shape
         Ho, Wo = (H // 2, W // 2) if stride == 2 else ((2 * H, 2 * W) if upsample else (H, W))
         out = torch.empty(B, Ho, Wo, Cout, device=self.device, dtype=torch.float32)
-        self.enter()
-        self.check(self.lib.sdxl_op_conv2d(self.h, _ptr(x), _ptr(w), _ptr(bias), B, H, W, Cin, Cout, ks, stride,
-                                           int(upsample), _ptr(out)), "sdxl_op_conv2d")
-        self.leave()
+        self.call("sdxl_op_conv2d", self.lib.sdxl_op_conv2d, self.h, _ptr(x), _ptr(w), _ptr(bias), B, H, W, Cin, Cout, ks, stride,
+                  int(upsample), _ptr(out))
         return out
 
     def group_norm(self, x1: torch.Tensor, x2: Optional[torch.Tensor], gamma: torch.Tensor, beta: torch.Tensor,
@@ -138,10 +141,8 @@ class Context:
         gamma = gamma.to(self.device, torch.float32).contiguous()
         beta = beta.to(self.device, torch.float32).contiguous()
         out = torch.empty(B, HW, C1 + C2, device=self.device, dtype=torch.float16)
-        self.enter()
-        self.check(self.lib.sdxl_op_group_norm(self.h, _ptr(x1), C1, _ptr(x2), C2, B, HW, n_group, _ptr(gamma), _ptr(beta),
-                                               eps, int(silu), _ptr(out)), "sdxl_op_group_norm")
-        self.leave()
+        self.call("sdxl_op_group_norm", self.lib.sdxl_op_group_norm, self.h, _ptr(x1), C1, _ptr(x2), C2, B, HW, n_group, _ptr(gamma),
+                  _ptr(beta), eps, int(silu), _ptr(out))
         return out
 
     def layer_norm(self, x: torch.Tensor, gamma: torch.Tensor, beta: torch.Tensor, eps: float = 1e-5) -> torch.Tensor:
@@ -150,27 +151,19 @@ class Context:
         gamma = gamma.to(self.device, torch.float32).contiguous()
         beta = beta.to(self.device, torch.float32).contiguous()
         out = torch.empty(rows, Cc, device=self.device, dtype=torch.float16)
-        self.enter()
-        self.check(self.lib.sdxl_op_layer_norm(self.h, _ptr(x), _ptr(gamma), _ptr(beta), eps, rows, Cc, _ptr(out)),
-                   "sdxl_op_layer_norm")
-        self.leave()
+        self.call("sdxl_op_layer_norm", self.lib.sdxl_op_layer_norm, self.h, _ptr(x), _ptr(gamma), _ptr(beta), eps, rows, Cc, _ptr(out))
         return out
 
     def timestep_embedding(self, timesteps: Sequence[int], dim: int, max_period: int = 10000) -> torch.Tensor:
         n = len(timesteps)
         arr = (C.c_int32 * n)(*[int(t) for t in timesteps])
         out = torch.empty(n, dim, device=self.device, dtype=torch.float32)
-        self.enter()
-        self.check(self.lib.sdxl_op_timestep_embedding(self.h, arr, n, dim, max_period, _ptr(out)),
-                   "sdxl_op_timestep_embedding")
-        self.leave()
+        self.call("sdxl_op_timestep_embedding", self.lib.sdxl_op_timestep_embedding, self.h, arr, n, dim, max_period, _ptr(out))
         return out
 
     def randn(self, n: int, seed: int, subsequence: int = 0) -> torch.Tensor:
         out = torch.empty(n, device=self.device, dtype=torch.float32)
-        self.enter()
-        self.check(self.lib.sdxl_randn(self.h, _ptr(out), n, seed, subsequence), "sdxl_randn")
-        self.leave()
+        self.call("sdxl_randn", self.lib.sdxl_randn, self.h, _ptr(out), n, seed, subsequence)
         return out
 
 
@@ -184,11 +177,9 @@ def set_adapters(ctx: "Context", fn, h, adapters: Sequence, what: str) -> None:
     arr = (_lib.Adapter * max(1, len(packs)))()
     for i, (pk, (_, scale)) in enumerate(zip(packs, adapters)):
         arr[i].pack, arr[i].bytes, arr[i].pack_on_device, arr[i].scale = pk.data_ptr(), pk.numel(), int(pk.is_cuda), float(scale)
-    ctx.enter()
     if any(pk.is_cuda for pk in packs):
         torch.cuda.current_stream(ctx.device).synchronize()
-    ctx.check(fn(h, len(packs), arr), what)
-    ctx.leave()
+    ctx.call(what, fn, h, len(packs), arr)
 
 
 @dataclass
@@ -231,6 +222,44 @@ class Conditioning:
         return s, keep
 
 
+class AttachableModel:
+    """A device-resident model a UNet can hold (ControlNet, T2IAdapter, IPAdapter). Subclasses name their load and destroy entry
+    points and the Diffuser call that detaches them; close() is refused while a UNet holds the model."""
+    _load_fn = _destroy_fn = _detach_call = ""
+
+    def _load(self, ctx: "Context", cfg_struct, weights) -> None:
+        """Loads weights (a pack-named tensor dict or a built pack, host or device) through _load_fn with cfg_struct."""
+        self.ctx = ctx
+        pack = weights if isinstance(weights, torch.Tensor) else build_pack(weights)
+        if pack.is_cuda:
+            torch.cuda.current_stream(ctx.device).synchronize()
+        h = C.c_void_p()
+        ctx.call(self._load_fn, getattr(ctx.lib, self._load_fn), ctx.h, C.byref(cfg_struct), pack.data_ptr(), pack.numel(),
+                 int(pack.is_cuda), C.byref(h))
+        self.h = h
+        self.attached = 0   # UNets holding the model (Diffuser._attach)
+
+    def handle(self) -> int:
+        if not getattr(self, "h", None):
+            raise SdxlError(f"{type(self).__name__} is closed")
+        return self.h.value
+
+    def close(self) -> None:
+        """Frees the device weights. Refused while a UNet holds the model: detach it first."""
+        if getattr(self, "attached", 0) > 0:
+            raise SdxlError(f"{type(self).__name__}.close: the model is still attached to a UNet (detach it with "
+                            f"{self._detach_call} first)")
+        if getattr(self, "h", None):
+            getattr(self.ctx.lib, self._destroy_fn)(self.h)
+            self.h = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
 def _cfg_struct(cfg: UNetConfig) -> _lib.UnetCfg:
     s = _lib.UnetCfg()
     s.adm_in_channels = cfg.adm_in_channels
@@ -263,33 +292,33 @@ class Diffuser:
         if weights is not None:
             pack = weights if isinstance(weights, torch.Tensor) else build_pack(weights)
         on_device = bool(pack is not None and pack.is_cuda)
-        ctx.enter()
         if on_device:
             torch.cuda.current_stream(ctx.device).synchronize()
         if nccl_comm is not None:
-            rc = ctx.lib.sdxl_unet_load_broadcast(ctx.h, C.byref(cs), None if pack is None else pack.data_ptr(),
-                                                  0 if pack is None else pack.numel(), int(on_device), nccl_comm, rank, root, C.byref(h))
-            ctx.check(rc, "sdxl_unet_load_broadcast")
+            ctx.call("sdxl_unet_load_broadcast", ctx.lib.sdxl_unet_load_broadcast, ctx.h, C.byref(cs), None if pack is None else pack.data_ptr(),
+                     0 if pack is None else pack.numel(), int(on_device), nccl_comm, rank, root, C.byref(h))
         else:
-            rc = ctx.lib.sdxl_unet_load(ctx.h, C.byref(cs), pack.data_ptr(), pack.numel(), int(on_device), C.byref(h))
-            ctx.check(rc, "sdxl_unet_load")
+            ctx.call("sdxl_unet_load", ctx.lib.sdxl_unet_load, ctx.h, C.byref(cs), pack.data_ptr(), pack.numel(), int(on_device), C.byref(h))
         self.h = h
         self._cond_key = None
         self._keep = None
+        self._attached: Dict[str, list] = {}   # kind -> the AttachableModels the UNet holds (_attach)
+
+    def _attach(self, kind: str, objects: Sequence["AttachableModel"]) -> None:
+        """Records, after a successful set call, the models the UNet now holds for `kind` ("controls", "image_prompts",
+        "t2i_adapters"; [] after a detach): the ones held before are released, the new ones cannot be closed while held."""
+        for o in self._attached.get(kind, []):
+            o.attached -= 1
+        self._attached[kind] = list(objects)
+        for o in self._attached[kind]:
+            o.attached += 1
 
     def close(self) -> None:
         if getattr(self, "h", None):
             self.ctx.lib.sdxl_unet_destroy(self.h)
             self.h = None
-            if getattr(self, "_controls", None):   # the destroyed UNet no longer uses its ControlNets
-                from .controlnet import release_controls
-                release_controls(self)
-            if getattr(self, "_image_prompt", None):
-                from .ip_adapter import release_image_prompt
-                release_image_prompt(self)
-            if getattr(self, "_t2i_adapters", None):
-                from .t2i_adapter import release_t2i_adapters
-                release_t2i_adapters(self)
+            for kind in list(self._attached):   # the destroyed UNet no longer holds its models
+                self._attach(kind, [])
 
     def __del__(self):
         try:
@@ -345,9 +374,7 @@ class Diffuser:
             s = _lib.InpaintCondition()
             s.cond, s.on_host, s.n = cond.data_ptr(), 0, cond.shape[0]
             s.height, s.width = 8 * cond.shape[2], 8 * cond.shape[3]
-        ctx.enter()
-        ctx.check(ctx.lib.sdxl_unet_set_inpaint_condition(self.h, None if s is None else C.byref(s)), "sdxl_unet_set_inpaint_condition")
-        ctx.leave()
+        ctx.call("sdxl_unet_set_inpaint_condition", ctx.lib.sdxl_unet_set_inpaint_condition, self.h, None if s is None else C.byref(s))
 
     def set_pag(self, layers="mid", scale: float = 3.0, adaptive_scale: float = 0.0) -> None:
         """Attaches perturbed-attention guidance (sdxl_unet_set_pag, DESIGN.md §14); layers None or scale 0 detaches. layers: diffusers'
@@ -369,17 +396,14 @@ class Diffuser:
             keep = (C.c_uint8 * len(mask))(*mask)
             s = _lib.Pag()
             s.scale, s.adaptive_scale, s.n_layers, s.layers_host, s.forward_perturbed_rows = scale, adaptive, len(mask), C.addressof(keep), rows
-        self.ctx.enter()
-        self.ctx.check(self.ctx.lib.sdxl_unet_set_pag(self.h, None if s is None else C.byref(s)), "sdxl_unet_set_pag")
-        self.ctx.leave()
+        self.ctx.call("sdxl_unet_set_pag", self.ctx.lib.sdxl_unet_set_pag, self.h, None if s is None else C.byref(s))
 
     @classmethod
     def from_diffusers_dir(cls, ctx: Context, path: str) -> "Diffuser":
         """A diffusers UNet2DConditionModel directory (the `unet/` folder of an SDXL pipeline, base or inpainting): config.json +
         diffusion_pytorch_model[.fp16].safetensors (diffusers_unet.from_diffusers)."""
-        from .diffusers_unet import read_diffusers_dir
-        cfg, w = read_diffusers_dir(path)
-        return cls(ctx, cfg, w)
+        from .diffusers_unet import from_diffusers, read_model_dir
+        return cls(ctx, *from_diffusers(*read_model_dir(path)))
 
     # ---- UNet::forward -------------------------------------------------------------------------
     def set_conditioning(self, context: torch.Tensor, label: torch.Tensor) -> None:
@@ -387,10 +411,7 @@ class Diffuser:
         context = context.to(ctx.device, torch.float16).contiguous()
         label = label.to(ctx.device, torch.float16).contiguous()
         B, n_ctx, _ = context.shape
-        ctx.enter()
-        ctx.check(ctx.lib.sdxl_unet_set_conditioning(self.h, B, n_ctx, _ptr(context), _ptr(label)),
-                  "sdxl_unet_set_conditioning")
-        ctx.leave()
+        ctx.call("sdxl_unet_set_conditioning", ctx.lib.sdxl_unet_set_conditioning, self.h, B, n_ctx, _ptr(context), _ptr(label))
         self._keep = (context, label)
 
     def unet_forward(self, x: torch.Tensor, timesteps, context: Optional[torch.Tensor] = None,
@@ -413,13 +434,8 @@ class Diffuser:
         f16 = x.dtype == torch.float16
         x = x.to(ctx.device, torch.float16 if f16 else torch.float32).contiguous()
         out = torch.empty_like(x)
-        ctx.enter()
-        if f16:
-            rc = ctx.lib.sdxl_unet_forward(self.h, B, h, w, _ptr(x), t, _ptr(out))
-        else:
-            rc = ctx.lib.sdxl_unet_forward_f32(self.h, B, h, w, _ptr(x), t, _ptr(out))
-        ctx.check(rc, "sdxl_unet_forward")
-        ctx.leave()
+        ctx.call("sdxl_unet_forward", ctx.lib.sdxl_unet_forward if f16 else ctx.lib.sdxl_unet_forward_f32, self.h, B, h, w, _ptr(x), t,
+                 _ptr(out))
         return out
 
     @property
@@ -469,11 +485,8 @@ class Diffuser:
         mask = prep(mask, torch.uint8)
         n_noise = 0 if noise is None else (noise.shape[0] if noise.dim() == 5 else 1)
         out = torch.empty(s.n_batch, self.cfg.latent_channels, h, w, device=dev, dtype=torch.float32)
-        ctx.enter()
-        rc = ctx.lib.sdxl_sample_latent(self.h, C.byref(s), float(guidance), n_steps, step_start, _ptr(init_latent),
-                                        _ptr(noise), n_noise, seed, _ptr(ref), _ptr(mask), _ptr(out))
-        ctx.check(rc, "sdxl_sample_latent")
-        ctx.leave()
+        ctx.call("sdxl_sample_latent", ctx.lib.sdxl_sample_latent, self.h, C.byref(s), float(guidance), n_steps, step_start, _ptr(init_latent),
+                 _ptr(noise), n_noise, seed, _ptr(ref), _ptr(mask), _ptr(out))
         del keep
         return out
 
@@ -499,15 +512,13 @@ class Diffuser:
     # ---- step-wise (bench) ---------------------------------------------------------------------
     def sampler_begin(self, cond: Conditioning, guidance: float) -> None:
         s, keep = cond.to_struct(self.ctx.device)
-        self.ctx.enter()
-        self.ctx.check(self.ctx.lib.sdxl_sampler_begin(self.h, C.byref(s), float(guidance)), "sdxl_sampler_begin")
+        self.ctx.call("sdxl_sampler_begin", self.ctx.lib.sdxl_sampler_begin, self.h, C.byref(s), float(guidance))
         self.ctx.synchronize()
         del keep
 
     def sampler_set_latent(self, x: torch.Tensor) -> None:
         x = x.to(self.ctx.device, torch.float32).contiguous()
-        self.ctx.enter()
-        self.ctx.check(self.ctx.lib.sdxl_sampler_set_latent(self.h, _ptr(x), 0), "sdxl_sampler_set_latent")
+        self.ctx.call("sdxl_sampler_set_latent", self.ctx.lib.sdxl_sampler_set_latent, self.h, _ptr(x), 0)
         self.ctx.synchronize()
 
     def sampler_get_latent(self, like: torch.Tensor) -> torch.Tensor:
@@ -535,7 +546,6 @@ class LatentDecoder:
         self.ctx, self.cfg = ctx, cfg
         pack = weights if isinstance(weights, torch.Tensor) else build_pack(weights)
         on_device = pack.is_cuda
-        ctx.enter()
         if on_device:
             torch.cuda.current_stream(ctx.device).synchronize()
         cs = _lib.VaeCfg()
@@ -547,8 +557,7 @@ class LatentDecoder:
         for i, (ci, co) in enumerate(cfg.enc_block_channels):
             cs.enc_in[i], cs.enc_out[i] = ci, co
         h = C.c_void_p()
-        ctx.check(ctx.lib.sdxl_vae_load(ctx.h, C.byref(cs), pack.data_ptr(), pack.numel(), int(on_device), C.byref(h)),
-                  "sdxl_vae_load")
+        ctx.call("sdxl_vae_load", ctx.lib.sdxl_vae_load, ctx.h, C.byref(cs), pack.data_ptr(), pack.numel(), int(on_device), C.byref(h))
         self.h = h
 
     def close(self) -> None:
@@ -573,20 +582,14 @@ class LatentDecoder:
         """latent f32 [B,4,h,w] (host or device) -> image f32 [B,3,8h,8w] on the same side."""
         latent, host, B, h, w, up = self._prep(latent)
         out = torch.empty((B, 3, h * up, w * up), dtype=torch.float32, device="cpu" if host else self.ctx.device)
-        self.ctx.enter()
-        self.ctx.check(self.ctx.lib.sdxl_vae_decode_latent(self.h, B, h, w, _ptr(latent), int(host), _ptr(out)),
-                       "sdxl_vae_decode_latent")
-        self.ctx.leave()
+        self.ctx.call("sdxl_vae_decode_latent", self.ctx.lib.sdxl_vae_decode_latent, self.h, B, h, w, _ptr(latent), int(host), _ptr(out))
         return out
 
     def latent_to_image(self, latent: torch.Tensor) -> torch.Tensor:
         """RawImages buffer: u8 [B, 8h, 8w, 3]."""
         latent, host, B, h, w, up = self._prep(latent)
         out = torch.empty((B, h * up, w * up, 3), dtype=torch.uint8, device="cpu" if host else self.ctx.device)
-        self.ctx.enter()
-        self.ctx.check(self.ctx.lib.sdxl_vae_latent_to_image(self.h, B, h, w, _ptr(latent), int(host), _ptr(out)),
-                       "sdxl_vae_latent_to_image")
-        self.ctx.leave()
+        self.ctx.call("sdxl_vae_latent_to_image", self.ctx.lib.sdxl_vae_latent_to_image, self.h, B, h, w, _ptr(latent), int(host), _ptr(out))
         return out
 
     def encode_image(self, image: torch.Tensor) -> torch.Tensor:
@@ -596,9 +599,7 @@ class LatentDecoder:
         B, _, H, W = image.shape
         d = 2 ** (len(self.cfg.enc_block_channels) - 1)
         out = torch.empty((B, self.cfg.latent_channels, H // d, W // d), dtype=torch.float32, device="cpu" if host else self.ctx.device)
-        self.ctx.enter()
-        self.ctx.check(self.ctx.lib.sdxl_vae_encode_image(self.h, B, H, W, _ptr(image), int(host), _ptr(out)), "sdxl_vae_encode_image")
-        self.ctx.leave()
+        self.ctx.call("sdxl_vae_encode_image", self.ctx.lib.sdxl_vae_encode_image, self.h, B, H, W, _ptr(image), int(host), _ptr(out))
         return out
 
     def image_to_latent(self, rgb: torch.Tensor) -> torch.Tensor:
@@ -608,9 +609,7 @@ class LatentDecoder:
         B, H, W, _ = rgb.shape
         d = 2 ** (len(self.cfg.enc_block_channels) - 1)
         out = torch.empty((B, self.cfg.latent_channels, H // d, W // d), dtype=torch.float32, device="cpu" if host else self.ctx.device)
-        self.ctx.enter()
-        self.ctx.check(self.ctx.lib.sdxl_vae_image_to_latent(self.h, B, H, W, _ptr(rgb), int(host), _ptr(out)), "sdxl_vae_image_to_latent")
-        self.ctx.leave()
+        self.ctx.call("sdxl_vae_image_to_latent", self.ctx.lib.sdxl_vae_image_to_latent, self.h, B, H, W, _ptr(rgb), int(host), _ptr(out))
         return out
 
     @property

@@ -20,9 +20,8 @@ import torch
 from . import _lib
 from ._lib import SdxlError
 from .config import UNetConfig, block_program
-from .engine import _cfg_struct
+from .engine import AttachableModel, _cfg_struct
 from .lora import read_safetensors
-from .weights import build_pack
 
 TOKENS_PER_IMAGE = 4
 # keys of an IP-Adapter Plus (Resampler) image projection; in a file that also has the base projection they are refused
@@ -302,37 +301,24 @@ def cfg_struct(cfg: UNetConfig, image_embed_dim: int, resampler: Optional[Resamp
     return s
 
 
-class IPAdapter:
+class IPAdapter(AttachableModel):
     """A device-resident IP-Adapter (sdxl_ip_adapter_load). weights: pack-named tensor dict or a built pack. The kind is read from
     the weights: `image_proj/latents` makes an IP-Adapter Plus (resampler_of); a built pack is a base adapter unless `resampler`
     describes it. image_embed_dim: D of the image embeddings (base) or of the image features (Plus)."""
+    _load_fn, _destroy_fn, _detach_call = "sdxl_ip_adapter_load", "sdxl_ip_adapter_destroy", "set_image_prompt(None)"
 
     resampler: Optional[ResamplerConfig] = None   # None: the base adapter
 
     def __init__(self, ctx, cfg: UNetConfig, image_embed_dim: int, weights, resampler: Optional[ResamplerConfig] = None):
-        self.ctx, self.cfg, self.image_embed_dim = ctx, cfg, int(image_embed_dim)
+        self.cfg, self.image_embed_dim = cfg, int(image_embed_dim)
         self.resampler = resampler if isinstance(weights, torch.Tensor) else resampler_of(weights)
-        pack = weights if isinstance(weights, torch.Tensor) else build_pack(weights)
-        ctx.enter()
-        if pack.is_cuda:
-            torch.cuda.current_stream(ctx.device).synchronize()
-        cs = cfg_struct(cfg, self.image_embed_dim, self.resampler)
-        h = C.c_void_p()
-        ctx.check(ctx.lib.sdxl_ip_adapter_load(ctx.h, C.byref(cs), pack.data_ptr(), pack.numel(), int(pack.is_cuda), C.byref(h)),
-                  "sdxl_ip_adapter_load")
-        self.h = h
-        self.attached = 0   # attachments to UNets; close() refuses while > 0
+        self._load(ctx, cfg_struct(cfg, self.image_embed_dim, self.resampler), weights)
 
     @classmethod
     def from_file(cls, ctx, path: str, cfg: UNetConfig) -> "IPAdapter":
         """An h94 file, e.g. `sdxl_models/ip-adapter_sdxl_vit-h.safetensors` or `ip-adapter_sdxl.bin`."""
         dim, w = from_h94(read_h94(path), cfg)
         return cls(ctx, cfg, dim, w)
-
-    def handle(self) -> int:
-        if not getattr(self, "h", None):
-            raise SdxlError("IPAdapter is closed")
-        return self.h.value
 
     @property
     def tokens_per_image(self) -> int:
@@ -358,9 +344,7 @@ class IPAdapter:
             raise SdxlError(f"resample: needs an IP-Adapter Plus and features [n, L, {self.image_embed_dim}], got {tuple(x.shape)}")
         x = x.to(ctx.device, torch.float32).contiguous()
         out = torch.empty(x.shape[0] * self.resampler.tokens, self.cfg.context_dim, device=ctx.device, dtype=torch.float16)
-        ctx.enter()
-        ctx.check(ctx.lib.sdxl_ip_adapter_resample(h, x.shape[0], x.shape[1], x.data_ptr(), 0, out.data_ptr()), "sdxl_ip_adapter_resample")
-        ctx.leave()
+        ctx.call("sdxl_ip_adapter_resample", ctx.lib.sdxl_ip_adapter_resample, h, x.shape[0], x.shape[1], x.data_ptr(), 0, out.data_ptr())
         return out
 
     def project(self, embeds: torch.Tensor) -> torch.Tensor:
@@ -369,24 +353,8 @@ class IPAdapter:
         h = self.handle()
         e = _embeds(embeds, self.image_embed_dim).reshape(-1, self.image_embed_dim).to(ctx.device).contiguous()
         out = torch.empty(e.shape[0] * TOKENS_PER_IMAGE, self.cfg.context_dim, device=ctx.device, dtype=torch.float16)
-        ctx.enter()
-        ctx.check(ctx.lib.sdxl_ip_adapter_project(h, e.shape[0], e.data_ptr(), 0, out.data_ptr()), "sdxl_ip_adapter_project")
-        ctx.leave()
+        ctx.call("sdxl_ip_adapter_project", ctx.lib.sdxl_ip_adapter_project, h, e.shape[0], e.data_ptr(), 0, out.data_ptr())
         return out
-
-    def close(self) -> None:
-        """Frees the device weights. Refused while the adapter is attached to a UNet: detach it first."""
-        if getattr(self, "attached", 0) > 0:
-            raise SdxlError("IPAdapter.close: the adapter is still attached to a UNet (detach it with set_image_prompt(None) first)")
-        if getattr(self, "h", None):
-            self.ctx.lib.sdxl_ip_adapter_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def _embeds(e: torch.Tensor, dim: int) -> torch.Tensor:
@@ -472,19 +440,9 @@ def set_image_prompt(diffuser, adapter: Optional[IPAdapter], embeds: Optional[to
     (transformer_block_paths). negative: embeddings of the unconditional CFG rows (default: zeros). For an IP-Adapter Plus, embeds
     and negative are image features [n_batch, n_images, L, D] (IPAdapter.image_embeds) and negative is required."""
     ctx = diffuser.ctx
-    if adapter is None:
-        ctx.enter()
-        ctx.check(ctx.lib.sdxl_unet_set_image_prompt(diffuser.h, None), "sdxl_unet_set_image_prompt")
-        ctx.leave()
-        release_image_prompt(diffuser)
-        return
-    p, _keep = _prompt_struct(diffuser, adapter, embeds, scale, negative)
-    ctx.enter()
-    ctx.check(ctx.lib.sdxl_unet_set_image_prompt(diffuser.h, C.byref(p)), "sdxl_unet_set_image_prompt")
-    ctx.leave()
-    release_image_prompt(diffuser)
-    diffuser._image_prompt = [adapter]   # the adapter stays alive, and cannot be closed, while attached
-    adapter.attached += 1
+    p, _keep = (None, None) if adapter is None else _prompt_struct(diffuser, adapter, embeds, scale, negative)
+    ctx.call("sdxl_unet_set_image_prompt", ctx.lib.sdxl_unet_set_image_prompt, diffuser.h, None if p is None else C.byref(p))
+    diffuser._attach("image_prompts", [] if adapter is None else [adapter])
 
 
 def set_image_prompts(diffuser, prompts: Sequence) -> None:
@@ -518,17 +476,5 @@ def set_image_prompts(diffuser, prompts: Sequence) -> None:
     n = len(structs)
     arr = (_lib.ImagePrompt * max(n, 1))(*structs)
     marr = (_lib.IpMask * max(n, 1))(*masks)
-    ctx.enter()
-    ctx.check(ctx.lib.sdxl_unet_set_image_prompts(diffuser.h, n, arr, marr), "sdxl_unet_set_image_prompts")
-    ctx.leave()
-    release_image_prompt(diffuser)
-    diffuser._image_prompt = [item[0] for item in prompts]   # every adapter stays alive, and cannot be closed, while attached
-    for a in diffuser._image_prompt:
-        a.attached += 1
-
-
-def release_image_prompt(diffuser) -> None:
-    """Forgets the diffuser's attached adapters (after a detach, or when the UNet is destroyed)."""
-    for a in getattr(diffuser, "_image_prompt", None) or []:
-        a.attached -= 1
-    diffuser._image_prompt = None
+    ctx.call("sdxl_unet_set_image_prompts", ctx.lib.sdxl_unet_set_image_prompts, diffuser.h, n, arr, marr)
+    diffuser._attach("image_prompts", [item[0] for item in prompts])

@@ -2,9 +2,6 @@
 adapter of sdxl_t2i_adapter_load, and its attachment to a UNet with Diffuser.set_t2i_adapters or sample(..., t2i_adapters=...)."""
 from __future__ import annotations
 
-import ctypes as C
-import json
-import os
 import re
 from typing import Dict, List, Sequence, Tuple
 
@@ -14,9 +11,9 @@ from . import _lib
 from ._lib import SdxlError
 from .config import SDXL_BASE, T2IAdapterConfig, UNetConfig, block_program
 from .controlnet import hint_tensor
-from .engine import _cfg_struct, ddim_timesteps
-from .lora import read_safetensors
-from .weights import build_pack, t2i_adapter_tensor_specs
+from .diffusers_unet import read_config, read_model_dir
+from .engine import AttachableModel, _cfg_struct, ddim_timesteps
+from .weights import t2i_adapter_tensor_specs
 
 # adapter types diffusers' T2IAdapter knows that this engine does not run
 _OTHER_TYPES = {"full_adapter": "the SD1.5 full adapter", "light_adapter": "the SD1.5 light adapter",
@@ -45,13 +42,7 @@ def from_diffusers(state_dict: Dict[str, torch.Tensor], config_json, unet: UNetC
                    ) -> Tuple[T2IAdapterConfig, Dict[str, torch.Tensor]]:
     """A diffusers SDXL T2IAdapter (state dict + config.json as dict, JSON text or path) -> (config, pack-named f16 weights).
     Unknown keys, missing tensors and wrong shapes raise SdxlError naming the key."""
-    if isinstance(config_json, str):
-        if os.path.exists(config_json):
-            with open(config_json) as f:
-                config_json = json.load(f)
-        else:
-            config_json = json.loads(config_json)
-    cfg = config_from_diffusers(config_json, unet)
+    cfg = config_from_diffusers(read_config(config_json), unet)
     specs = {name: shape for name, shape, _, _ in t2i_adapter_tensor_specs(cfg)}
     out: Dict[str, torch.Tensor] = {}
     for k, t in state_dict.items():
@@ -102,36 +93,18 @@ def t2i_t_min(n_steps: int, factor: float, step_start: int = 0, total: int = 100
     return total if k <= 0 else ts[min(k, len(ts)) - 1]
 
 
-class T2IAdapter:
+class T2IAdapter(AttachableModel):
     """A device-resident T2I-Adapter (sdxl_t2i_adapter_load). weights: pack-named tensor dict or a built pack."""
+    _load_fn, _destroy_fn, _detach_call = "sdxl_t2i_adapter_load", "sdxl_t2i_adapter_destroy", "set_t2i_adapters([])"
 
     def __init__(self, ctx, cfg: T2IAdapterConfig, weights):
-        self.ctx, self.cfg = ctx, cfg
-        pack = weights if isinstance(weights, torch.Tensor) else build_pack(weights)
-        ctx.enter()
-        if pack.is_cuda:
-            torch.cuda.current_stream(ctx.device).synchronize()
-        cs = cfg_struct(cfg)
-        h = C.c_void_p()
-        ctx.check(ctx.lib.sdxl_t2i_adapter_load(ctx.h, C.byref(cs), pack.data_ptr(), pack.numel(), int(pack.is_cuda), C.byref(h)),
-                  "sdxl_t2i_adapter_load")
-        self.h = h
-        self.attached = 0   # attachments to UNets (set_t2i_adapters); close() refuses while > 0
+        self.cfg = cfg
+        self._load(ctx, cfg_struct(cfg), weights)
 
     @classmethod
     def from_diffusers_dir(cls, ctx, path: str, unet: UNetConfig = SDXL_BASE) -> "T2IAdapter":
         """A diffusers T2IAdapter directory: config.json + diffusion_pytorch_model[.fp16].safetensors."""
-        files = [f for f in ("diffusion_pytorch_model.fp16.safetensors", "diffusion_pytorch_model.safetensors")
-                 if os.path.exists(os.path.join(path, f))]
-        if not files:
-            raise SdxlError(f"{path}: no diffusion_pytorch_model[.fp16].safetensors")
-        cfg, w = from_diffusers(read_safetensors(os.path.join(path, files[0])), os.path.join(path, "config.json"), unet)
-        return cls(ctx, cfg, w)
-
-    def handle(self) -> int:
-        if not getattr(self, "h", None):
-            raise SdxlError("T2IAdapter is closed")
-        return self.h.value
+        return cls(ctx, *from_diffusers(*read_model_dir(path), unet))
 
     def features(self, hint: torch.Tensor) -> List[torch.Tensor]:
         """The four features F_k f32 [n, ch_k, H/16 or H/32, ...] of hint f32 [n, C, H, W] in [0, 1] or u8 [n, H, W, C] (test aid)."""
@@ -141,24 +114,8 @@ class T2IAdapter:
         n, _, H, W = hint.shape
         shapes = [(n, c, H // d, W // d) for c, d in zip(self.cfg.channels, (16, 16, 32, 32))]
         out = torch.empty(sum(int(torch.Size(s).numel()) for s in shapes), device=ctx.device, dtype=torch.float32)
-        ctx.enter()
-        ctx.check(ctx.lib.sdxl_t2i_adapter_features(h, n, H, W, hint.data_ptr(), 0, out.data_ptr()), "sdxl_t2i_adapter_features")
-        ctx.leave()
+        ctx.call("sdxl_t2i_adapter_features", ctx.lib.sdxl_t2i_adapter_features, h, n, H, W, hint.data_ptr(), 0, out.data_ptr())
         return [p.reshape(s) for p, s in zip(out.split([int(torch.Size(s).numel()) for s in shapes]), shapes)]
-
-    def close(self) -> None:
-        """Frees the device weights. Refused while the adapter is attached to a UNet: detach it first (set_t2i_adapters([]))."""
-        if getattr(self, "attached", 0) > 0:
-            raise SdxlError("T2IAdapter.close: the adapter is still attached to a UNet (detach it with set_t2i_adapters([]) first)")
-        if getattr(self, "h", None):
-            self.ctx.lib.sdxl_t2i_adapter_destroy(self.h)
-            self.h = None
-
-    def __del__(self):
-        try:
-            self.close()
-        except Exception:
-            pass
 
 
 def set_t2i_adapters(diffuser, items: Sequence, t_min: int = 0) -> None:
@@ -177,17 +134,5 @@ def set_t2i_adapters(diffuser, items: Sequence, t_min: int = 0) -> None:
         arr[i].hint_on_host = 0
         arr[i].n_hint, arr[i].height, arr[i].width = h.shape[0], h.shape[2], h.shape[3]
         arr[i].scale = float(scale)
-    ctx.enter()
-    ctx.check(ctx.lib.sdxl_unet_set_t2i_adapters(diffuser.h, len(items), arr, int(t_min)), "sdxl_unet_set_t2i_adapters")
-    ctx.leave()
-    release_t2i_adapters(diffuser)
-    diffuser._t2i_adapters = [ad for ad, _, _ in items]   # refused close() while attached
-    for ad in diffuser._t2i_adapters:
-        ad.attached += 1
-
-
-def release_t2i_adapters(diffuser) -> None:
-    """Forgets the diffuser's attached adapters (after a detach, or when the UNet is destroyed)."""
-    for ad in getattr(diffuser, "_t2i_adapters", []):
-        ad.attached -= 1
-    diffuser._t2i_adapters = []
+    ctx.call("sdxl_unet_set_t2i_adapters", ctx.lib.sdxl_unet_set_t2i_adapters, diffuser.h, len(items), arr, int(t_min))
+    diffuser._attach("t2i_adapters", [ad for ad, _, _ in items])
