@@ -163,7 +163,7 @@ SDXL_API double sdxl_unet_plan_flops_executed(const sdxl_unet* unet);
 /* Device time of ONE execution of the current launch plan, summed per kernel kind and measured with CUDA
  * events on the ctx stream (eager launches). Kind index: 0 implicit-GEMM (wgmma), 1 attention, 2 GroupNorm,
  * 3 LayerNorm, 4 GEMV, 5 timestep-embedding, 6 first conv, 7 upsample copy, 8 phase-split copy, 9 f32->f16 cast,
- * 17 T2I-Adapter feature add, 18 PAG identity self-attention.
+ * 17 T2I-Adapter feature add, 18 PAG identity self-attention, 19 FreeU skip filter and backbone scale.
  * All three arrays hold SDXL_PROFILE_KINDS entries (host). Used by bench.py for the per-kernel roofline. */
 SDXL_API int sdxl_unet_profile_plan(sdxl_unet* unet, double* ms_by_kind_host, double* flops_by_kind_host,
                                     int* launches_by_kind_host);
@@ -589,6 +589,22 @@ SDXL_API int sdxl_unet_num_self_attentions(const sdxl_unet* unet);
  * it at the next direct forward that uses it); a new layer set, attaching and detaching rebuild it at the next forward. Attaching or
  * detaching between sdxl_sampler_begin and sdxl_sampler_step requires a new sdxl_sampler_begin. */
 SDXL_API int sdxl_unet_set_pag(sdxl_unet* unet, const sdxl_pag* pag);
+
+/* ---- FreeU ------------------------------------------------------------------------------------------------
+ * Si et al. 2023, as diffusers' enable_freeu(s1, s2, b1, b2) runs it (DESIGN.md §15). At every skip concatenation cat([x, r]) of the
+ * output blocks of the two deepest levels (diffusers' up_blocks[0] and [1]; output_blocks/0..5) the first half of x's channels is
+ * multiplied by b and the skip r (after any ControlNet residual) becomes fourier_filter(r, threshold 1, s): the four lowest
+ * frequencies of each channel, {0, -1} x {0, -1} after fftshift's centring, are scaled by s. (s, b) is (s1, b1) at the deepest level,
+ * (s2, b2) at the one above. Every row of the batch (conditional, unconditional, perturbed) is filtered; ControlNets are not.
+ * The FreeU authors recommend s1 = 0.9, s2 = 0.2, b1 = 1.3, b2 = 1.4 for SDXL. */
+typedef struct sdxl_freeu {
+  float s1, s2, b1, b2;
+} sdxl_freeu;
+/* Attaches FreeU to the UNet. NULL detaches, and so does any value equal to 0 (diffusers enables FreeU only when all four are
+ * nonzero). A non-finite value is refused and leaves the previous state. A call that changes only the values keeps the launch plan
+ * and its CUDA graph; attaching and detaching rebuild it at the next forward. Attaching or detaching between sdxl_sampler_begin and
+ * sdxl_sampler_step requires a new sdxl_sampler_begin. */
+SDXL_API int sdxl_unet_set_freeu(sdxl_unet* unet, const sdxl_freeu* freeu);
 
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),

@@ -17,7 +17,7 @@ CSRC = os.path.join(HERE, "csrc")
 BUILD = os.path.join(HERE, "build")
 LIB = os.path.join(HERE, "sdxl_b200", "libsdxl_b200.so")
 TEST_LIB = os.path.join(HERE, "sdxl_b200", "libsdxl_b200_testing.so")
-KERNEL_SOURCES = ["igemm.cu", "attention.cu", "norm.cu", "elementwise.cu", "vae_kernels.cu", "clip_kernels.cu", "t2i_kernels.cu"]
+KERNEL_SOURCES = ["igemm.cu", "attention.cu", "norm.cu", "elementwise.cu", "vae_kernels.cu", "clip_kernels.cu", "t2i_kernels.cu", "freeu.cu"]
 SOURCES = KERNEL_SOURCES + ["engine.cu", "vae.cu", "clip.cu", "tokenizer.cpp", "mpk.cpp"]
 TEST_SOURCES = ["testing.cu"]
 HEADERS = ["common.cuh", "kernels.h", "engine_core.h", "unicode_tables.h", os.path.join("..", "..", "include", "sdxl_b200.h")]

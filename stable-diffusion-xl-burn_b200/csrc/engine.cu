@@ -176,6 +176,13 @@ struct PagAttach {
   int forward_rows = 0;
 };
 
+// FreeU (sdxl_unet_set_freeu, DESIGN.md §15): its four values on the device, [s1, s2, b1, b2], read by every OP_FREEU launch, so
+// a change of values keeps the plan and its CUDA graph.
+struct FreeuAttach {
+  Arena mem;
+  float* vals = nullptr;
+};
+
 // Roles of the conditioning rows. The sampler's batch is row groups of n_img rows each: [cond | uncond] with CFG, then a perturbed
 // group with PAG ([cond | uncond | ptb]; the refiner: [cond] or [cond | ptb]). The perturbed rows are conditional rows. n_img = 0:
 // a plain batch, every row conditional.
@@ -242,6 +249,7 @@ struct sdxl_unet : EncoderHalf {
   std::unique_ptr<T2IAttach> t2i; // sdxl_unet_set_t2i_adapters
   std::unique_ptr<InpaintAttach> inpaint;   // sdxl_unet_set_inpaint_condition
   std::unique_ptr<PagAttach> pag;           // sdxl_unet_set_pag
+  std::unique_ptr<FreeuAttach> freeu;       // sdxl_unet_set_freeu
   uint64_t plan_builds = 0;
   int plan_ptb = 0;               // trailing rows of the current plan that take PAG's identity self-attentions
   RowLayout rows;                 // roles of the conditioning rows
@@ -849,6 +857,17 @@ struct UNetPlanBuilder : PlanBuilder {
     return x;
   }
 
+  // FreeU at a decoder skip concatenation cat([x, sk]) of the UNet's level n_levels - 1 - k (k = 0, 1): x[:, :Cx / 2] *= (b1, b2)[k]
+  // and sk = fourier_filter(sk, 1, (s1, s2)[k]), both in place (the next resblock is the only reader of either). tw: the level's
+  // twiddles.
+  void freeu(const Saved& sk, float* x, int Cx, int k, const float* tw) {
+    if (err) return;
+    Op op{};
+    op.kind = OP_FREEU;
+    op.fu = {sk.p, sk.C, x, Cx, Bf, sk.H, sk.W, tw, u->freeu->vals + k, u->freeu->vals + 2 + k};
+    P->ops.push_back(op);
+  }
+
   // T2I-Adapter injection: x += F_k in place, so the skip saved for the block carries the feature too
   void t2i_add(float* x, int k, int C, int H, int W) {
     if (err) return;
@@ -1085,6 +1104,20 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
     B.zero_conv({cmid, Cx, H, W}, {x, Cx, H, W}, a.zero.back(), s_raw);
     B.end_block();
   }
+  // --- FreeU's twiddle tables of the two deepest levels, computed on the host (freeu_twiddles) into the plan's workspace
+  const float* freeu_tw[2] = {nullptr, nullptr};
+  for (int k = 0; k < 2 && u->freeu && levels - 1 - k >= 0; ++k) {
+    const int th = P->h >> (levels - 1 - k), tw = P->w >> (levels - 1 - k);
+    float* d = B.buf<float>((size_t)2 * (th + tw));
+    if (B.err) return B.err;
+    if (!A->measure) {
+      std::vector<float> host((size_t)2 * (th + tw));
+      freeu_twiddles(th, tw, host.data());
+      CU(c, cudaMemcpyAsync(d, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+      CU(c, cudaStreamSynchronize(c->stream));
+    }
+    freeu_tw[k] = d;
+  }
   // --- output blocks: cat([x, saved.pop()], channel) is never materialised (GN + skip conv read both)
   for (size_t i = 0; i < u->out_blocks.size() && !B.err; ++i) {
     const Block& b = u->out_blocks[i];
@@ -1093,6 +1126,14 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
     saved.pop_back();
     if (sk.H != H || sk.W != W || Cx + sk.C != b.res.Cin) return fail(c, 5005, "skip shape mismatch at output block %zu", i);
     B.begin_block("output_blocks/" + std::to_string(i));
+    // FreeU: the output blocks of the two deepest levels (diffusers' up_blocks[0] and [1]: three each, output block i is at level
+    // n_levels - 1 - i / 3), after the ControlNet residuals were added to the skips
+    const int k = (int)(i / 3);
+    if (u->freeu && k < 2 && k < levels) {
+      if (H != P->h >> (levels - 1 - k) || W != P->w >> (levels - 1 - k))
+        return fail(c, 5024, "FreeU: output block %zu is not at level %d", i, levels - 1 - k);
+      B.freeu(sk, x, Cx, k, freeu_tw[k]);
+    }
     x = B.resblock(b.res, x, Cx, sk.p, sk.C, H, W, temb_all, temb_total, s_gn1, s_raw, s_h, s_gn2);
     Cx = b.res.Cout;
     if (b.type == BT_REST || b.type == BT_RESTU) x = B.strans(b.st, x, H, W, s_a16, s_tok, s_qkv, s_ao, s_q, s_ff);
@@ -2191,6 +2232,37 @@ extern "C" int sdxl_unet_set_pag(sdxl_unet* u, const sdxl_pag* p) {
   u->pag->adaptive = p->adaptive_scale;
   u->pag->forward_rows = p->forward_perturbed_rows;
   return 0;
+}
+
+// ================================================================================================
+// FreeU (include/sdxl_b200.h: sdxl_unet_set_freeu; DESIGN.md §15)
+// ================================================================================================
+extern "C" int sdxl_unet_set_freeu(sdxl_unet* u, const sdxl_freeu* f) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  if (!f) return attach_detach(u, u->freeu);
+  // validate everything first: on failure the attached state is unchanged
+  const float v[4] = {f->s1, f->s2, f->b1, f->b2};
+  static const char* const names[4] = {"s1", "s2", "b1", "b2"};
+  for (int i = 0; i < 4; ++i)
+    if (!isfinite(v[i])) return fail(c, 4980 + i, "set_freeu: %s = %g must be finite", names[i], v[i]);
+  // diffusers runs FreeU only when all four values are nonzero
+  for (int i = 0; i < 4; ++i)
+    if (v[i] == 0.f) return attach_detach(u, u->freeu);
+  if (u->freeu) {   // new values only: the plan and its graph read them from the device
+    CU(c, cudaMemcpyAsync(u->freeu->vals, v, sizeof(v), cudaMemcpyHostToDevice, c->stream));
+    CU(c, cudaStreamSynchronize(c->stream));   // v is on this stack
+    return 0;
+  }
+  std::unique_ptr<FreeuAttach> fresh(new FreeuAttach());
+  if (int r = carve_measured(c, fresh->mem, 4984, "set_freeu: value buffer", [&](Arena& A) {
+        fresh->vals = A.get<float>(4);
+        return 0;
+      }))
+    return r;
+  CU(c, cudaMemcpyAsync(fresh->vals, v, sizeof(v), cudaMemcpyHostToDevice, c->stream));
+  return attach_install(u, u->freeu, std::move(fresh));   // drains the stream before v goes
 }
 
 // ================================================================================================

@@ -423,12 +423,13 @@ static int build_two_pass(M* m, const PackView& pv, int (*build)(M*, const PackV
 // launch plan
 // ================================================================================================
 enum OpKind { OP_IGEMM, OP_ATTN, OP_GN, OP_LN, OP_GEMV, OP_TEMB, OP_CONV_IN, OP_UPS, OP_PHASE, OP_CAST16,
-              OP_SOFTMAX, OP_TRANSPOSE, OP_PQ, OP_EMBED, OP_ATTN_SMALL, OP_ACT, OP_LN_GATHER, OP_T2I_ADD, OP_PAG_IDENTITY, OP_KIND_COUNT };
+              OP_SOFTMAX, OP_TRANSPOSE, OP_PQ, OP_EMBED, OP_ATTN_SMALL, OP_ACT, OP_LN_GATHER, OP_T2I_ADD, OP_PAG_IDENTITY, OP_FREEU,
+              OP_KIND_COUNT };
 // the public profile entry points take caller arrays of SDXL_PROFILE_KINDS entries (include/sdxl_b200.h)
 static_assert(OP_KIND_COUNT <= SDXL_PROFILE_KINDS, "profile arrays too small for the op kinds");
 static const char* const kOpNames[] = {"igemm", "attention", "group_norm", "layer_norm", "gemv", "temb", "conv_in", "upsample",
                                        "phase_split", "cast16", "softmax_rows", "transpose16", "post_quant", "embed_tokens",
-                                       "attention_small", "mlp_act", "ln_gather", "t2i_add", "pag_identity"};
+                                       "attention_small", "mlp_act", "ln_gather", "t2i_add", "pag_identity", "freeu"};
 static_assert(sizeof(kOpNames) / sizeof(kOpNames[0]) == OP_KIND_COUNT, "one name per op kind");
 struct Op {
   OpKind kind;
@@ -456,6 +457,7 @@ struct Op {
   struct { const float* x; const int* idx; int B, T, C; const float* g; const float* b; float eps; float* y; } lg;
   struct { float* x; const float* F; long per_img; int B, n_hint; const int* t; const int* t_min; } ta;
   struct { const __half* qkv; int C; long rows; __half* out; } pi;   // PAG identity self-attention (pag_identity_launch)
+  struct { float* r; int C; float* x; int Cx, B, H, W; const float* tw; const float* s; const float* b; } fu;   // FreeU (freeu_launch)
 };
 
 struct Plan {
@@ -689,6 +691,9 @@ static int exec_op(sdxl_ctx* c, Op& op) {
     case OP_PQ: KL(c, post_quant_launch(st, op.pq.x, op.pq.B, op.pq.C, op.pq.HW, op.pq.w, op.pq.bias, op.pq.inv_scale, op.pq.y)); break;
     case OP_T2I_ADD: KL(c, t2i_add_launch(st, op.ta.x, op.ta.F, op.ta.per_img, op.ta.B, op.ta.n_hint, op.ta.t, op.ta.t_min)); break;
     case OP_PAG_IDENTITY: KL(c, pag_identity_launch(st, op.pi.qkv, op.pi.C, op.pi.rows, op.pi.out)); break;
+    case OP_FREEU:
+      KL(c, freeu_launch(st, op.fu.r, op.fu.C, op.fu.x, op.fu.Cx, op.fu.B, op.fu.H, op.fu.W, op.fu.tw, op.fu.s, op.fu.b));
+      break;
   }
   return 0;
 }

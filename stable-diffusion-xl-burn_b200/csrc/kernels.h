@@ -302,6 +302,15 @@ int avg_pool2_f16_launch(cudaStream_t st, const float* x, int n, int H, int W, i
 // x[b] += F[b % n_hint] (f32, per_img floats per image, a multiple of 4) when *t >= *t_min; t and t_min are device ints. PDL plan op.
 int t2i_add_launch(cudaStream_t st, float* x, const float* F, long per_img, int B, int n_hint, const int* t, const int* t_min);
 
+// FreeU at one decoder skip concatenation (freeu.cu, DESIGN.md §15), in place on f32 NHWC tensors of B rows at H x W: the skip
+// r [B, H, W, C] becomes diffusers' fourier_filter(r, threshold 1, scale *s) and the channels [0, Cx / 2) of x [B, H, W, Cx] are
+// multiplied by *b. tw: freeu_twiddles(H, W) on the device; s, b: device floats. PDL plan op, one launch.
+int freeu_launch(cudaStream_t st, float* r, int C, float* x, int Cx, int B, int H, int W, const float* tw, const float* s,
+                 const float* b);
+// Host: the twiddle table of an H x W skip, 2 * (H + W) floats [cos 2 pi h / H | sin 2 pi h / H | cos 2 pi w / W | sin 2 pi w / W],
+// computed in double precision.
+void freeu_twiddles(int H, int W, float* out);
+
 // Weight re-layout at load time (elementwise.cu)
 // Linear [K(in), N(out)] row-major f16 -> K-major [N, Kpad] f16 (zero padded), dst row pitch Kpad;
 // rows written at dst_row0 + perm(n) where perm handles the GEGLU value/gate interleave (geglu_bn>0).

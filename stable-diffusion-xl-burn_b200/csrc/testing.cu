@@ -141,6 +141,13 @@ SDXL_TEST_API int sdxl_test_cfg_pag_ddim(void* stream, const float* eps, int ld,
   return cfg_pag_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_cfg, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x);
 }
 
+// FreeU at one skip concatenation, as the plan's OP_FREEU: the twiddle table (host, 2 * (H + W) floats) and the in-place launch.
+SDXL_TEST_API void sdxl_test_freeu_twiddles(int H, int W, float* out_host) { freeu_twiddles(H, W, out_host); }
+SDXL_TEST_API int sdxl_test_freeu(void* stream, float* r, int C, float* x, int Cx, int B, int H, int W, const float* tw, const float* s,
+                                  const float* b) {
+  return freeu_launch((cudaStream_t)stream, r, C, x, Cx, B, H, W, tw, s, b);
+}
+
 SDXL_TEST_API int sdxl_test_repack_upconv(void* stream, const void* src, int O, int I, void* dst, int Ipad) {
   return repack_upconv_launch((cudaStream_t)stream, (const __half*)src, O, I, (__half*)dst, Ipad);
 }

@@ -116,6 +116,10 @@ class Pag(C.Structure):
                 ("forward_perturbed_rows", C.c_int32)]
 
 
+class Freeu(C.Structure):
+    _fields_ = [("s1", C.c_float), ("s2", C.c_float), ("b1", C.c_float), ("b2", C.c_float)]
+
+
 # name -> (restype, argtypes); every symbol include/sdxl_b200.h declares
 P = C.c_void_p
 I = C.c_int
@@ -198,6 +202,7 @@ PROTOTYPES = {
     "sdxl_unet_set_inpaint_condition": (I, [P, C.POINTER(InpaintCondition)]),
     "sdxl_unet_num_self_attentions": (I, [P]),
     "sdxl_unet_set_pag": (I, [P, C.POINTER(Pag)]),
+    "sdxl_unet_set_freeu": (I, [P, C.POINTER(Freeu)]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),
     "sdxl_mpk_encode_u16": (C.c_size_t, [P, C.c_size_t, P]),

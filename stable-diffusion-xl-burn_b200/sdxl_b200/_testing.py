@@ -32,6 +32,8 @@ PROTOTYPES = {
     "sdxl_test_conv_in_cat": (I, [P, P, I, I, I, I, P, I, I, I, I, P, P, I, P]),
     "sdxl_test_pag_identity": (I, [P, P, I, C.c_long, P]),
     "sdxl_test_cfg_pag_ddim": (I, [P, P, I, I, I, I, I, F, F, F, F, F, F, P]),
+    "sdxl_test_freeu_twiddles": (None, [I, I, P]),
+    "sdxl_test_freeu": (I, [P, P, I, P, I, I, I, I, P, P, P]),
     "sdxl_test_repack_upconv": (I, [P, P, I, I, P, I]),
     "sdxl_test_repack_conv": (I, [P, P, I, I, I, I, P, I, I, I]),
     "sdxl_test_transpose_linear": (I, [P, P, I, I, P, I, I, I]),
@@ -157,6 +159,19 @@ def pag_identity(qkv: torch.Tensor, C: int, rows: int, out: torch.Tensor) -> Non
 def cfg_pag_ddim(eps, ld, Bimg, C, HW, use_cfg, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x) -> None:
     """x f32 NCHW [Bimg, C, HW] updated in place from eps NHWC f32 [groups * Bimg, HW, ld]."""
     _call("sdxl_test_cfg_pag_ddim", _p(eps), ld, Bimg, C, HW, int(use_cfg), guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, _p(x))
+
+
+def freeu_twiddles(H: int, W: int) -> torch.Tensor:
+    """The host twiddle table of an H x W skip (f32 [2 * (H + W)]: cos and sin of 2 pi h / H, then of 2 pi w / W)."""
+    out = torch.empty(2 * (H + W), dtype=torch.float32)
+    load().sdxl_test_freeu_twiddles(H, W, out.data_ptr())
+    return out
+
+
+def freeu(r, C, x, Cx, B, H, W, tw, s, b) -> None:
+    """In place: r f32 NHWC [B, H, W, C] := fourier_filter(r, 1, s[0]), x f32 NHWC [B, H, W, Cx][..., :Cx // 2] *= b[0]; tw, s, b on
+    the device."""
+    _call("sdxl_test_freeu", _p(r), C, _p(x), Cx, B, H, W, _p(tw), _p(s), _p(b))
 
 
 def repack_upconv(src, O, I, dst, Ipad) -> None:

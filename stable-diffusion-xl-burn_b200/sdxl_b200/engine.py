@@ -398,6 +398,19 @@ class Diffuser:
             s.scale, s.adaptive_scale, s.n_layers, s.layers_host, s.forward_perturbed_rows = scale, adaptive, len(mask), C.addressof(keep), rows
         self.ctx.call("sdxl_unet_set_pag", self.ctx.lib.sdxl_unet_set_pag, self.h, None if s is None else C.byref(s))
 
+    def set_freeu(self, s1: Optional[float], s2: Optional[float] = None, b1: Optional[float] = None, b2: Optional[float] = None) -> None:
+        """Attaches FreeU (sdxl_unet_set_freeu, DESIGN.md §15), diffusers' enable_freeu(s1, s2, b1, b2): in the output blocks of the
+        two deepest levels the first half of the backbone channels is scaled by b1 (deepest) / b2 and the skip's lowest frequencies
+        by s1 / s2. s1 None, or any value 0, detaches (diffusers' disable_freeu). The FreeU authors recommend
+        set_freeu(0.9, 0.2, 1.3, 1.4) for SDXL."""
+        s = None
+        if s1 is not None:
+            if s2 is None or b1 is None or b2 is None:
+                raise SdxlError("set_freeu: give all four values s1, s2, b1, b2, or None to detach")
+            s = _lib.Freeu()
+            s.s1, s.s2, s.b1, s.b2 = float(s1), float(s2), float(b1), float(b2)
+        self.ctx.call("sdxl_unet_set_freeu", self.ctx.lib.sdxl_unet_set_freeu, self.h, None if s is None else C.byref(s))
+
     @classmethod
     def from_diffusers_dir(cls, ctx: Context, path: str) -> "Diffuser":
         """A diffusers UNet2DConditionModel directory (the `unet/` folder of an SDXL pipeline, base or inpainting): config.json +
@@ -453,7 +466,7 @@ class Diffuser:
     KIND_NAMES = ["igemm_wgmma", "attention_wgmma", "group_norm", "layer_norm", "gemv", "timestep_embedding",
                   "conv_in", "upsample2x", "phase_split", "cast_f16"]
     # kinds only the UNet plan launches, by kind index (KIND_NAMES is positional and LatentDecoder.KIND_NAMES extends it)
-    UNET_KINDS = {17: "t2i_add", 18: "pag_identity"}
+    UNET_KINDS = {17: "t2i_add", 18: "pag_identity", 19: "freeu"}
 
     def profile_plan(self) -> Dict[str, Dict[str, float]]:
         """Per-kernel-kind device time (ms), algorithmic FLOPs and launch count of one plan execution."""

@@ -53,7 +53,8 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
            reference_rgb: Optional[torch.Tensor] = None, crop: Sequence[Optional[int]] = (None, None, None, None), crop_out: bool = False,
            resolution: Tuple[int, int] = (1024, 1024), seed: int = 0, noise: Optional[torch.Tensor] = None,
            loras: Optional[Sequence] = None, controls: Optional[Sequence] = None, image_prompt: Optional[Sequence] = None,
-           t2i_adapters: Optional[Sequence] = None, t2i_factor: float = 1.0, pag: Optional[Sequence] = None) -> torch.Tensor:
+           t2i_adapters: Optional[Sequence] = None, t2i_factor: float = 1.0, pag: Optional[Sequence] = None,
+           freeu: Optional[Sequence[float]] = None) -> torch.Tensor:
     """One image, like `sample --prompt ... [--reference-img ... --crop-* ...] [--use-refiner]`.
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
     bottom) in pixels. With an inpainting UNet (cfg.is_inpaint, DESIGN.md §12) reference_rgb is required: the crop window becomes the
@@ -70,7 +71,15 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     detached afterwards, their features added on the first int(n_steps * t2i_factor) iterations (diffusers'
     adapter_conditioning_factor). pag: (scale, layers[, adaptive_scale]) perturbed-attention guidance (Diffuser.set_pag, diffusers'
     pag_scale, pag_applied_layers, pag_adaptive_scale) attached to the base UNet for this call and detached afterwards (the refiner is
-    left alone). Returns uint8 [1, H, W, 3]."""
+    left alone). freeu: (s1, s2, b1, b2) FreeU (Diffuser.set_freeu, diffusers' enable_freeu) attached to the base UNet for this call
+    and detached afterwards (the refiner is left alone). Returns uint8 [1, H, W, 3]."""
+    if freeu:
+        diffuser.set_freeu(*freeu)
+        try:
+            return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
+                          seed, noise, loras, controls, image_prompt, t2i_adapters, t2i_factor, pag)
+        finally:
+            diffuser.set_freeu(None)
     if pag:
         diffuser.set_pag(pag[1], pag[0], *pag[2:3])
         try:
