@@ -235,7 +235,7 @@ SDXL_API void sdxl_vae_destroy(sdxl_vae* vae);
  * [B,3,8h,8w] NCHW (nominally in [-1,1]). `on_host` != 0: both pointers are host memory. h*w must be a multiple of 64. */
 SDXL_API int sdxl_vae_decode_latent(sdxl_vae* vae, int B, int h, int w, const float* latent, int on_host, float* image_out);
 /* == LatentDecoder::latent_to_image (stablediffusion/mod.rs:200-237): RawImages buffer, u8 [B, 8h, 8w, 3],
- * value = trunc(clamp(((x + 1) / 2) * 255, 0, 255)). */
+ * value = trunc(clamp(((x + 1) / 2) * 255, 0, 255)); a NaN pixel channel becomes 0. */
 SDXL_API int sdxl_vae_latent_to_image(sdxl_vae* vae, int B, int h, int w, const float* latent, int on_host, uint8_t* rgb_out);
 /* == LatentDecoder::encode_image (stablediffusion/mod.rs:258-261) over Autoencoder::encode_image (autoencoder/mod.rs:58-64):
  * image f32 [B,3,H,W] NCHW in [-1,1] -> latent f32 [B,latent_channels,H/8,W/8] (mean channels of quant_conv, times

@@ -228,8 +228,7 @@ int nhwc_to_nchw_f16_launch(cudaStream_t st, const float* x, int B, int HW, int 
 int nhwc_to_nchw_f32_launch(cudaStream_t st, const float* x, int B, int HW, int C, int ldx, float* y);
 // Sampler elementwise (reference stablediffusion/mod.rs:407-428, 463-465, 539-540).
 // eps layout: NHWC f32 [nfwd*Bimg, HW, ld]; cond rows first, then uncond (if cfg).
-// x: NCHW f32 master latent [Bimg,C,HW], updated in place; x16: f16 NCHW copy duplicated for the next
-// forward ([nfwd*Bimg, C, HW]).
+// x: NCHW f32 master latent [Bimg,C,HW], updated in place. x16 is unused (the next forward reads x; pass nullptr).
 int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg,
                     float guidance, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
                     float* x, __half* x16);
@@ -240,7 +239,7 @@ int cfg_pag_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int
 // PAG's identity self-attention on `rows` token rows: out[r, 0:C] = qkv[r, 2C:3C] (qkv row pitch 3C, out row pitch C); C % 8 == 0,
 // both pointers 16-byte aligned.
 int pag_identity_launch(cudaStream_t st, const __half* qkv, int C, long rows, __half* out);
-// x = mask ? x : ref*sqrt_a + noise*sqrt_1ma ; also refreshes x16 (both forwards).
+// x = mask ? x : ref*sqrt_a + noise*sqrt_1ma over n_per_img_batch elements; nfwd and x16 are unused (pass nullptr).
 int inpaint_blend_launch(cudaStream_t st, float* x, const float* ref, const float* noise,
                          const uint8_t* mask, size_t n_per_img_batch, int nfwd, float sqrt_a,
                          float sqrt_1ma, __half* x16);
@@ -259,7 +258,7 @@ int transpose_f16_launch(cudaStream_t st, const __half* x, size_t ldx, int rows,
 // 1x1 conv on the rescaled latent: y = W (x * inv_scale) + b; NCHW f32 [B, C<=8, HW]; W f32 [C, C].
 int post_quant_launch(cudaStream_t st, const float* x, int B, int C, int HW, const float* w, const float* bias,
                       float inv_scale, float* y);
-// u8[b,p,c] = trunc(clamp(((x+1)/2)*255, 0, 255)), c < 3, from NHWC f32 [npix, ldx].
+// u8[b,p,c] = trunc(clamp(((x+1)/2)*255, 0, 255)), c < 3, from NHWC f32 [npix, ldx]; NaN -> 0.
 int image_u8_launch(cudaStream_t st, const float* x, long npix, int ldx, uint8_t* out);
 
 // u8 [B,HW,3] -> f32 NCHW [B,3,HW], ((v/255)*2)-1.

@@ -2,7 +2,8 @@
 // product library). Each wrapper takes plain arguments, fills the launcher's parameter struct exactly as the UNet's launch
 // plan does (engine_core.h: PlanBuilder) and launches on `stream`, so tests can pin the fused layouts the plan uses —
 // second K sources, per-batch bias rows, scattered upsample outputs, column windows of fused QKV / KV matrices — kernel by
-// kernel against a float64 reference. All pointers are device pointers; every function returns the launcher's status.
+// kernel against a float64 reference. The VAE, text / vision encoder, T2I-Adapter and sampler kernels are reached the same
+// way. All pointers are device pointers; every function returns the launcher's status.
 #include "kernels.h"
 
 #define SDXL_TEST_API extern "C" __attribute__((visibility("default")))
@@ -178,4 +179,105 @@ SDXL_TEST_API int sdxl_test_lora_merge(void* stream, int N, int Kd, int taps, in
 }
 SDXL_TEST_API int sdxl_test_lora_upconv_merge(void* stream, const void* src, const float* delta, int O, int I, void* dst, int Ipad) {
   return lora_upconv_merge_launch((cudaStream_t)stream, (const __half*)src, delta, O, I, (__half*)dst, Ipad);
+}
+
+// The latent decoder's and encoder's small kernels (vae_kernels.cu).
+SDXL_TEST_API int sdxl_test_softmax_rows(void* stream, const float* S, size_t lds, int rows, int cols, float scale, void* P,
+                                         size_t ldp) {
+  return softmax_rows_launch((cudaStream_t)stream, S, lds, rows, cols, scale, (__half*)P, ldp);
+}
+SDXL_TEST_API int sdxl_test_transpose_f16(void* stream, const void* x, size_t ldx, int rows, int cols, void* y, size_t ldy) {
+  return transpose_f16_launch((cudaStream_t)stream, (const __half*)x, ldx, rows, cols, (__half*)y, ldy);
+}
+SDXL_TEST_API int sdxl_test_post_quant(void* stream, const float* x, int B, int C, int HW, const float* w, const float* bias,
+                                       float inv_scale, float* y) {
+  return post_quant_launch((cudaStream_t)stream, x, B, C, HW, w, bias, inv_scale, y);
+}
+SDXL_TEST_API int sdxl_test_quant_out(void* stream, const float* x, int B, int Cz, int Cout, long HW, const float* w, const float* bias,
+                                      float scale, float* y) {
+  return quant_out_launch((cudaStream_t)stream, x, B, Cz, Cout, HW, w, bias, scale, y);
+}
+SDXL_TEST_API int sdxl_test_image_u8(void* stream, const float* x, long npix, int ldx, uint8_t* out) {
+  return image_u8_launch((cudaStream_t)stream, x, npix, ldx, out);
+}
+SDXL_TEST_API int sdxl_test_image_from_u8(void* stream, const uint8_t* in, int B, long HW, float* out) {
+  return image_from_u8_launch((cudaStream_t)stream, in, B, HW, out);
+}
+
+// The CLIP text and vision towers' small kernels (clip_kernels.cu).
+SDXL_TEST_API int sdxl_test_embed_tokens(void* stream, const int* tokens, int rows, int T, int C, int n_vocab, const void* tok_emb,
+                                         const void* pos_emb, float* x, int* err) {
+  return embed_tokens_launch((cudaStream_t)stream, tokens, rows, T, C, n_vocab, (const __half*)tok_emb, (const __half*)pos_emb, x, err);
+}
+SDXL_TEST_API int sdxl_test_patchify(void* stream, const float* pixels, int N, int S, int p, int Kpad, void* y) {
+  return patchify_launch((cudaStream_t)stream, pixels, N, S, p, Kpad, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_vision_embed_ln(void* stream, const float* patches, const void* cls, const void* pos, int N, int T, int C,
+                                            const float* gamma, const float* beta, float eps, float* x) {
+  return vision_embed_ln_launch((cudaStream_t)stream, patches, (const __half*)cls, (const __half*)pos, N, T, C, gamma, beta, eps, x);
+}
+SDXL_TEST_API int sdxl_test_mlp_act(void* stream, const float* x, size_t n, int quick, void* y) {
+  return mlp_act_launch((cudaStream_t)stream, x, n, quick, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_ln_gather_f32(void* stream, const float* x, const int* idx, int B, int T, int C, const float* gamma,
+                                          const float* beta, float eps, float* y) {
+  return ln_gather_f32_launch((cudaStream_t)stream, x, idx, B, T, C, gamma, beta, eps, y);
+}
+
+// The T2I-Adapter's kernels (t2i_kernels.cu); t and t_min are device ints.
+SDXL_TEST_API int sdxl_test_pixel_unshuffle(void* stream, const float* x, int n, int C, int H, int W, void* y) {
+  return pixel_unshuffle_launch((cudaStream_t)stream, x, n, C, H, W, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_relu_f16(void* stream, const float* x, size_t n, void* y) {
+  return relu_f16_launch((cudaStream_t)stream, x, n, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_avg_pool2_f16(void* stream, const float* x, int n, int H, int W, int C, void* y) {
+  return avg_pool2_f16_launch((cudaStream_t)stream, x, n, H, W, C, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_t2i_add(void* stream, float* x, const float* F, long per_img, int B, int n_hint, const int* t,
+                                    const int* t_min) {
+  return t2i_add_launch((cudaStream_t)stream, x, F, per_img, B, n_hint, t, t_min);
+}
+
+// The sampler's elementwise kernels and the UNet's resampling copies and casts (elementwise.cu).
+SDXL_TEST_API int sdxl_test_cfg_ddim(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance,
+                                     float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
+  return cfg_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_cfg, guidance, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x, nullptr);
+}
+SDXL_TEST_API int sdxl_test_inpaint_blend(void* stream, float* x, const float* ref, const float* noise, const uint8_t* mask, size_t n,
+                                          float sqrt_a, float sqrt_1ma) {
+  return inpaint_blend_launch((cudaStream_t)stream, x, ref, noise, mask, n, 1, sqrt_a, sqrt_1ma, nullptr);
+}
+SDXL_TEST_API int sdxl_test_axpby(void* stream, float* x, const float* noise, size_t n, float sa, float sb) {
+  return axpby_launch((cudaStream_t)stream, x, noise, n, sa, sb);
+}
+SDXL_TEST_API int sdxl_test_dup_latent_f16(void* stream, const float* x, size_t n, int nfwd, void* x16) {
+  return dup_latent_f16_launch((cudaStream_t)stream, x, n, nfwd, (__half*)x16);
+}
+SDXL_TEST_API int sdxl_test_cast_f32_to_f16(void* stream, const float* x, size_t n, void* y) {
+  return cast_f32_to_f16_launch((cudaStream_t)stream, x, n, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_cast_f16_to_f32(void* stream, const void* x, size_t n, float* y) {
+  return cast_f16_to_f32_launch((cudaStream_t)stream, (const __half*)x, n, y);
+}
+SDXL_TEST_API int sdxl_test_upsample2x(void* stream, const float* x, int B, int H, int W, int C, void* y) {
+  return upsample2x_launch((cudaStream_t)stream, x, B, H, W, C, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_phase_split(void* stream, const float* x, int B, int H, int W, int C, void* y) {
+  return phase_split_launch((cudaStream_t)stream, x, B, H, W, C, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_silu_f16(void* stream, const float* x, int B, int H, int W, int C, int phase, void* y) {
+  return silu_f16_launch((cudaStream_t)stream, x, B, H, W, C, phase, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_nhwc_to_nchw_f16(void* stream, const float* x, int B, int HW, int C, int ldx, void* y) {
+  return nhwc_to_nchw_f16_launch((cudaStream_t)stream, x, B, HW, C, ldx, (__half*)y);
+}
+SDXL_TEST_API int sdxl_test_nhwc_to_nchw_f32(void* stream, const float* x, int B, int HW, int C, int ldx, float* y) {
+  return nhwc_to_nchw_f32_launch((cudaStream_t)stream, x, B, HW, C, ldx, y);
+}
+SDXL_TEST_API int sdxl_test_scale_weights(void* stream, const void* w, size_t nw, const float* b, int nb, float s, void* wo, float* bo) {
+  return scale_weights_launch((cudaStream_t)stream, (const __half*)w, nw, b, nb, s, (__half*)wo, bo);
+}
+SDXL_TEST_API int sdxl_test_vec_add_f32(void* stream, float* dst, const float* src, int n) {
+  return vec_add_f32_launch((cudaStream_t)stream, dst, src, n);
 }

@@ -14,6 +14,7 @@ static inline int cdiv(long a, long b) { return (int)((a + b - 1) / b); }
 // shared memory when it fits so S is read from HBM once. Deterministic: fixed tree reductions, no atomics.
 // ------------------------------------------------------------------------------------------------
 constexpr int kSoftmaxThreads = 256;
+constexpr int kSoftmaxRed = kSoftmaxThreads / 32;  // the kernel's static shared memory: one reduction slot per warp
 __device__ __forceinline__ float block_reduce(float v, float* red, bool is_max) {
 #pragma unroll
   for (int o = 16; o; o >>= 1) {
@@ -33,7 +34,7 @@ __global__ void __launch_bounds__(kSoftmaxThreads) softmax_rows_kernel(const flo
                                                                        float scale_log2e, __half* __restrict__ P,
                                                                        size_t ldp, int cache_row) {
   extern __shared__ float srow[];
-  __shared__ float red[kSoftmaxThreads / 32];
+  __shared__ float red[kSoftmaxRed];
   griddep_wait();
   griddep_launch_dependents();
   const float* g = S + (size_t)blockIdx.x * lds;
@@ -79,7 +80,9 @@ int softmax_rows_launch(cudaStream_t st, const float* S, size_t lds, int rows, i
   if ((cols & 3) || (lds & 3) || (ldp & 3) || rows <= 0) return 6001;
   const size_t smem = (size_t)cols * sizeof(float);
   const int cache = smem <= 160 * 1024;
-  if (cache && smem > 48 * 1024) {
+  // without the opt-in, static and dynamic shared memory together must fit in 48 KB: at cols = 12288 (a 96 x 128 latent) the
+  // row alone is 48 KB and red[] does not fit beside it
+  if (cache && smem + sizeof(float) * kSoftmaxRed > 48 * 1024) {
     static bool optin[64];
     if (int r = smem_optin(softmax_rows_kernel, 160 * 1024, optin)) return r;
   }
@@ -150,7 +153,7 @@ int post_quant_launch(cudaStream_t st, const float* x, int B, int C, int HW, con
 
 // ------------------------------------------------------------------------------------------------
 // RawImages conversion (reference stablediffusion/mod.rs:211-229): u8[b, p, c] = trunc(clamp(((x + 1) / 2) * 255, 0, 255))
-// from the decoder's NHWC f32 output [B, HW, ldx] (first 3 channels).
+// from the decoder's NHWC f32 output [B, HW, ldx] (first 3 channels); NaN -> 0.
 // ------------------------------------------------------------------------------------------------
 __global__ void image_u8_kernel(const float* __restrict__ x, long npix, int ldx, uint8_t* __restrict__ out) {
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < npix; i += (long)gridDim.x * blockDim.x) {
@@ -158,7 +161,9 @@ __global__ void image_u8_kernel(const float* __restrict__ x, long npix, int ldx,
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       float v = ((px[c] + 1.0f) / 2.0f) * 255.0f;
-      v = fmaxf(fminf(v, 255.0f), 0.0f);  // NaN -> 0 (the reference would panic on unwrap)
+      // NaN -> 0 (the reference would panic on unwrap). fminf / fmaxf return the non-NaN operand, so the clamp alone would
+      // turn NaN into 255: the comparison is false for NaN.
+      v = v >= 0.0f ? fminf(v, 255.0f) : 0.0f;
       out[(size_t)i * 3 + c] = (uint8_t)v;
     }
   }

@@ -16,7 +16,7 @@ from ._lib import SdxlError, SdxlLibraryMissing
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libsdxl_b200_testing.so")
 
-P, I, F = C.c_void_p, C.c_int, C.c_float
+P, I, F, L, Z = C.c_void_p, C.c_int, C.c_float, C.c_long, C.c_size_t
 PROTOTYPES = {
     "sdxl_test_igemm": (I, [P, P, I, I, I, I, I, P, I, I, I, I, I, P, I, I, I, I, I, I, I, P, I, P, I, I, P, I, P, I, I, I, I]),
     "sdxl_test_attention": (I, [P, P, I, I, P, I, I, I, I, I, I, I, P, I, P, I, I, I, I, P]),
@@ -40,6 +40,34 @@ PROTOTYPES = {
     "sdxl_test_bias_to_f32": (I, [P, P, I, P, I, I]),
     "sdxl_test_lora_merge": (I, [P, I, I, I, I, P, P, P, P, P, P, I, C.c_size_t, I, I, I, I, P]),
     "sdxl_test_lora_upconv_merge": (I, [P, P, P, I, I, P, I]),
+    "sdxl_test_softmax_rows": (I, [P, P, Z, I, I, F, P, Z]),
+    "sdxl_test_transpose_f16": (I, [P, P, Z, I, I, P, Z]),
+    "sdxl_test_post_quant": (I, [P, P, I, I, I, P, P, F, P]),
+    "sdxl_test_quant_out": (I, [P, P, I, I, I, L, P, P, F, P]),
+    "sdxl_test_image_u8": (I, [P, P, L, I, P]),
+    "sdxl_test_image_from_u8": (I, [P, P, I, L, P]),
+    "sdxl_test_embed_tokens": (I, [P, P, I, I, I, I, P, P, P, P]),
+    "sdxl_test_patchify": (I, [P, P, I, I, I, I, P]),
+    "sdxl_test_vision_embed_ln": (I, [P, P, P, P, I, I, I, P, P, F, P]),
+    "sdxl_test_mlp_act": (I, [P, P, Z, I, P]),
+    "sdxl_test_ln_gather_f32": (I, [P, P, P, I, I, I, P, P, F, P]),
+    "sdxl_test_pixel_unshuffle": (I, [P, P, I, I, I, I, P]),
+    "sdxl_test_relu_f16": (I, [P, P, Z, P]),
+    "sdxl_test_avg_pool2_f16": (I, [P, P, I, I, I, I, P]),
+    "sdxl_test_t2i_add": (I, [P, P, P, L, I, I, P, P]),
+    "sdxl_test_cfg_ddim": (I, [P, P, I, I, I, I, I, F, F, F, F, F, P]),
+    "sdxl_test_inpaint_blend": (I, [P, P, P, P, P, Z, F, F]),
+    "sdxl_test_axpby": (I, [P, P, P, Z, F, F]),
+    "sdxl_test_dup_latent_f16": (I, [P, P, Z, I, P]),
+    "sdxl_test_cast_f32_to_f16": (I, [P, P, Z, P]),
+    "sdxl_test_cast_f16_to_f32": (I, [P, P, Z, P]),
+    "sdxl_test_upsample2x": (I, [P, P, I, I, I, I, P]),
+    "sdxl_test_phase_split": (I, [P, P, I, I, I, I, P]),
+    "sdxl_test_silu_f16": (I, [P, P, I, I, I, I, I, P]),
+    "sdxl_test_nhwc_to_nchw_f16": (I, [P, P, I, I, I, I, P]),
+    "sdxl_test_nhwc_to_nchw_f32": (I, [P, P, I, I, I, I, P]),
+    "sdxl_test_scale_weights": (I, [P, P, Z, P, I, F, P, P]),
+    "sdxl_test_vec_add_f32": (I, [P, P, P, I]),
 }
 _lib = None
 
@@ -203,3 +231,121 @@ def lora_merge(N, Kd, taps, terms, src, dst, ld, row0=0, col0=0, Ipad=0, geglu_b
 
 def lora_upconv_merge(src, delta, O, I, dst, Ipad) -> None:
     _call("sdxl_test_lora_upconv_merge", _p(src), _p(delta), O, I, _p(dst), Ipad)
+
+
+# latent decoder / encoder (vae_kernels.cu)
+def softmax_rows(S, lds, rows, cols, scale, P, ldp) -> None:
+    """P f16 [rows, ldp][:, :cols] = softmax(scale * S f32 [rows, lds][:, :cols])."""
+    _call("sdxl_test_softmax_rows", _p(S), lds, rows, cols, scale, _p(P), ldp)
+
+
+def transpose_f16(x, ldx, rows, cols, y, ldy) -> None:
+    """y f16 [cols, ldy][:, :rows] = x f16 [rows, ldx][:, :cols] transposed."""
+    _call("sdxl_test_transpose_f16", _p(x), ldx, rows, cols, _p(y), ldy)
+
+
+def post_quant(x, B, C, HW, w, bias, inv_scale, y) -> None:
+    _call("sdxl_test_post_quant", _p(x), B, C, HW, _p(w), _p(bias), inv_scale, _p(y))
+
+
+def quant_out(x, B, Cz, Cout, HW, w, bias, scale, y) -> None:
+    _call("sdxl_test_quant_out", _p(x), B, Cz, Cout, HW, _p(w), _p(bias), scale, _p(y))
+
+
+def image_u8(x, npix, ldx, out) -> None:
+    _call("sdxl_test_image_u8", _p(x), npix, ldx, _p(out))
+
+
+def image_from_u8(inp, B, HW, out) -> None:
+    _call("sdxl_test_image_from_u8", _p(inp), B, HW, _p(out))
+
+
+# text / vision encoders (clip_kernels.cu)
+def embed_tokens(tokens, rows, T, C, n_vocab, tok_emb, pos_emb, x, err) -> None:
+    _call("sdxl_test_embed_tokens", _p(tokens), rows, T, C, n_vocab, _p(tok_emb), _p(pos_emb), _p(x), _p(err))
+
+
+def patchify(pixels, N, S, p, Kpad, y) -> None:
+    _call("sdxl_test_patchify", _p(pixels), N, S, p, Kpad, _p(y))
+
+
+def vision_embed_ln(patches, cls, pos, N, T, C, gamma, beta, eps, x) -> None:
+    _call("sdxl_test_vision_embed_ln", _p(patches), _p(cls), _p(pos), N, T, C, _p(gamma), _p(beta), eps, _p(x))
+
+
+def mlp_act(x, n, quick, y) -> None:
+    _call("sdxl_test_mlp_act", _p(x), n, int(quick), _p(y))
+
+
+def ln_gather_f32(x, idx, B, T, C, gamma, beta, eps, y) -> None:
+    _call("sdxl_test_ln_gather_f32", _p(x), _p(idx), B, T, C, _p(gamma), _p(beta), eps, _p(y))
+
+
+# T2I-Adapter (t2i_kernels.cu)
+def pixel_unshuffle(x, n, C, H, W, y) -> None:
+    _call("sdxl_test_pixel_unshuffle", _p(x), n, C, H, W, _p(y))
+
+
+def relu_f16(x, n, y) -> None:
+    _call("sdxl_test_relu_f16", _p(x), n, _p(y))
+
+
+def avg_pool2_f16(x, n, H, W, C, y) -> None:
+    _call("sdxl_test_avg_pool2_f16", _p(x), n, H, W, C, _p(y))
+
+
+def t2i_add(x, F, per_img, B, n_hint, t, t_min) -> None:
+    """x[b] += F[b % n_hint] unless *t < *t_min; t, t_min: int32 CUDA tensors of one element."""
+    _call("sdxl_test_t2i_add", _p(x), _p(F), per_img, B, n_hint, _p(t), _p(t_min))
+
+
+# sampler, resampling copies and casts (elementwise.cu)
+def cfg_ddim(eps, ld, Bimg, C, HW, use_cfg, guidance, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x) -> None:
+    """x f32 NCHW [Bimg, C, HW] updated in place from eps NHWC f32 [(1 + use_cfg) * Bimg, HW, ld]."""
+    _call("sdxl_test_cfg_ddim", _p(eps), ld, Bimg, C, HW, int(use_cfg), guidance, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, _p(x))
+
+
+def inpaint_blend(x, ref, noise, mask, n, sqrt_a, sqrt_1ma) -> None:
+    _call("sdxl_test_inpaint_blend", _p(x), _p(ref), _p(noise), _p(mask), n, sqrt_a, sqrt_1ma)
+
+
+def axpby(x, noise, n, sa, sb) -> None:
+    _call("sdxl_test_axpby", _p(x), _p(noise), n, sa, sb)
+
+
+def dup_latent_f16(x, n, nfwd, x16) -> None:
+    _call("sdxl_test_dup_latent_f16", _p(x), n, nfwd, _p(x16))
+
+
+def cast_f32_to_f16(x, n, y) -> None:
+    _call("sdxl_test_cast_f32_to_f16", _p(x), n, _p(y))
+
+
+def cast_f16_to_f32(x, n, y) -> None:
+    _call("sdxl_test_cast_f16_to_f32", _p(x), n, _p(y))
+
+
+def upsample2x(x, B, H, W, C, y) -> None:
+    _call("sdxl_test_upsample2x", _p(x), B, H, W, C, _p(y))
+
+
+def phase_split(x, B, H, W, C, y) -> None:
+    _call("sdxl_test_phase_split", _p(x), B, H, W, C, _p(y))
+
+
+def silu_f16(x, B, H, W, C, phase, y) -> None:
+    _call("sdxl_test_silu_f16", _p(x), B, H, W, C, int(phase), _p(y))
+
+
+def nhwc_to_nchw(x, B, HW, C, ldx, y) -> None:
+    """f16 or f32 y [B, C, HW] from x f32 [B, HW, ldx][..., :C], by y's dtype."""
+    name = "sdxl_test_nhwc_to_nchw_f32" if y.dtype == torch.float32 else "sdxl_test_nhwc_to_nchw_f16"
+    _call(name, _p(x), B, HW, C, ldx, _p(y))
+
+
+def scale_weights(w, nw, b, nb, s, wo, bo) -> None:
+    _call("sdxl_test_scale_weights", _p(w), nw, _p(b), nb, s, _p(wo), _p(bo))
+
+
+def vec_add_f32(dst, src, n) -> None:
+    _call("sdxl_test_vec_add_f32", _p(dst), _p(src), n)
