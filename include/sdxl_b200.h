@@ -138,6 +138,60 @@ SDXL_API int sdxl_sample_latent(sdxl_unet* unet, const sdxl_conditioning* cond, 
                        int n_noise, uint64_t seed, const float* inpaint_ref,
                        const uint8_t* inpaint_mask, float* latent_out);
 
+/* ---- samplers and noise schedules (DESIGN.md §16) --------------------------------------------------------------------
+ * sigma_i = sqrt((1 - a_i) / a_i) over the model's alphas_cumprod; a fractional timestep t has log sigma(t) linear between
+ * floor(t) and ceil(t). A schedule is n_steps pairs (t_k, sigma_k) and sigma_n = 0. The sampler state is xh = x / sqrt(a)
+ * (k-diffusion's scaling), the UNet reads xh / sqrt(sigma_k^2 + 1), D = xh - sigma_k * eps with eps the guided prediction, and
+ * step k is xh' = cx xh + cd D + ch D_prev + cn z with per-sampler coefficients computed on the host in double:
+ *   EULER            xh + (sigma' - sigma) eps, the DDIM (eta 0) update in this scaling
+ *   EULER_ANCESTRAL  k-diffusion sample_euler_ancestral (eta, s_noise)
+ *   DPMPP_2M         k-diffusion sample_dpmpp_2m; first order on the first step of a call and on the step to sigma = 0
+ *   LCM              diffusers' LCMScheduler.step (timestep scaling 10, sigma_data 0.5)
+ * Spacings over N training timesteps: REFERENCE t_k = N - 1 - k (N / n) (sdxl_sample_latent's, which runs the same n steps when n
+ * divides N); LEADING (n - 1 - k)(N / n) + 1 (diffusers, steps_offset 1); TRAILING round(N - k N / n) - 1; LINSPACE
+ * (N - 1)(1 - k / (n - 1)), fractional; KARRAS sigma_k = (smax^(1/rho) + k / (n - 1) (smin^(1/rho) - smax^(1/rho)))^rho with t_k from
+ * the interpolation; LCM diffusers' LCMScheduler.set_timesteps with original_inference_steps = 50 (n <= 50). Any sampler goes with
+ * any spacing. */
+enum { SDXL_SAMPLER_EULER = 0, SDXL_SAMPLER_EULER_ANCESTRAL = 1, SDXL_SAMPLER_DPMPP_2M = 2, SDXL_SAMPLER_LCM = 3 };
+enum { SDXL_SPACING_REFERENCE = 0, SDXL_SPACING_LEADING = 1, SDXL_SPACING_TRAILING = 2, SDXL_SPACING_LINSPACE = 3,
+       SDXL_SPACING_KARRAS = 4, SDXL_SPACING_LCM = 5 };
+typedef struct sdxl_schedule {
+  int32_t sampler;      /* SDXL_SAMPLER_* */
+  int32_t spacing;      /* SDXL_SPACING_* */
+  int32_t n_steps;      /* length of the full schedule, 1 .. N */
+  int32_t first_step;   /* 0, or k0 > 0: start from `init_latent` at sigma_k0 (img2img, refiner) */
+  int32_t last_step;    /* 0 = n_steps, or stop early and return xh at sigma_last (the base half of base -> refiner) */
+  int32_t renoise;      /* first_step > 0: 1 adds sigma_k0 * z to init_latent (img2img), 0 takes it as it is (ensemble hand-off) */
+  int32_t no_cfg;       /* 1: one conditional forward per step, guidance ignored, the unconditional tensors may be NULL */
+  float   karras_rho;   /* 0 = 7 */
+  float   eta, s_noise; /* Euler-ancestral; 0 = 1 */
+} sdxl_schedule;
+/* Pure host, needs no GPU: fills timesteps[0 .. n_steps) and sigmas[0 .. n_steps] (sigmas[n_steps] = 0) from an alphas_cumprod
+ * table of n_train entries. Non-zero on an invalid schedule; sdxl_schedule_last_error() (per thread) names the field. */
+SDXL_API int sdxl_schedule_build(const double* alphas_cumprod, int n_train, const sdxl_schedule* schedule, double* timesteps,
+                                 double* sigmas);
+SDXL_API const char* sdxl_schedule_last_error(void);
+/* sdxl_sample_latent with a sampler and a schedule; every attachment of the UNet applies as it does there. Steps
+ * [first_step, last_step) of the schedule run; latent_out is xh at sigma_last (the latent itself after the last step of the
+ * schedule, where sigma = 0).
+ *  init_latent: first_step == 0: the initial noise z (NULL => seeded), xh = sqrt(sigma_0^2 + 1) z so that the UNet's first
+ *               input is z; first_step > 0: required, the latent to start from (xh at sigma_k0 when renoise == 0).
+ *  noise / n_noise / seed: injected tensors are taken by index and the seeded Philox stream by subsequence, in this order
+ *               and only those that exist: the initial noise when init_latent is NULL; the renoise tensor; then per step, in loop
+ *               order, the inpainting blend's noise and then the sampler's (Euler-ancestral and LCM, except on their last
+ *               step). As in sdxl_sample_latent, the first tensor past the n_noise injected ones takes subsequence 0 of the seeded
+ *               stream, not its index in the order: index and subsequence coincide only for a call with no injected tensor.
+ *               Seeded noise is generated inside the step kernel and equals sdxl_randn(seed, subsequence).
+ *  inpaint_ref / inpaint_mask: as in sdxl_sample_latent: before the forward of step k, xh = mask ? xh : ref + sigma_k z.
+ * With guidance the rows are [cond | uncond]; schedule->no_cfg runs [cond] alone (few-step distilled models), half the work.
+ * The schedule is validated before any state changes; the error names the field. DPM++ 2M's history does not cross calls. */
+SDXL_API int sdxl_sample_latent_scheduled(sdxl_unet* unet, const sdxl_conditioning* cond, double guidance_scale,
+                                          const sdxl_schedule* schedule, const float* init_latent, const float* noise, int n_noise,
+                                          uint64_t seed, const float* inpaint_ref, const uint8_t* inpaint_mask, float* latent_out);
+/* sdxl_unet_forward_f32 at a fractional timestep (the timestep embedding of t; T2I-Adapter windows compare lround(t)). For an
+ * integer t the result is bit-identical to sdxl_unet_forward_f32's. t outside [0, n_steps - 1] is refused. */
+SDXL_API int sdxl_unet_forward_f32_at(sdxl_unet* unet, int B, int h, int w, const float* x, double t, float* eps_out);
+
 /* Step-wise control for benchmarking / external loops: */
 /* prepare a sampler state for cond (uploads + hoists conditioning, allocates the latent). */
 SDXL_API int sdxl_sampler_begin(sdxl_unet* unet, const sdxl_conditioning* cond, double guidance_scale);

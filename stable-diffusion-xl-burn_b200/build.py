@@ -20,7 +20,7 @@ TEST_LIB = os.path.join(HERE, "sdxl_b200", "libsdxl_b200_testing.so")
 KERNEL_SOURCES = ["igemm.cu", "attention.cu", "norm.cu", "elementwise.cu", "vae_kernels.cu", "clip_kernels.cu", "t2i_kernels.cu", "freeu.cu"]
 SOURCES = KERNEL_SOURCES + ["engine.cu", "vae.cu", "clip.cu", "tokenizer.cpp", "mpk.cpp"]
 TEST_SOURCES = ["testing.cu"]
-HEADERS = ["common.cuh", "kernels.h", "engine_core.h", "unicode_tables.h", os.path.join("..", "..", "include", "sdxl_b200.h")]
+HEADERS = ["common.cuh", "kernels.h", "engine_core.h", "schedule.h", "unicode_tables.h", os.path.join("..", "..", "include", "sdxl_b200.h")]
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
 FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",

@@ -123,6 +123,24 @@ int timestep_embedding_launch(cudaStream_t st, const int* t_dev, int nt, int dim
   timestep_embedding_kernel<<<cdiv(n, 128), 128, 0, st>>>(t_dev, nt, dim, max_period, out);
   return (int)cudaGetLastError();
 }
+// The same of a float timestep (the UNet plan's: schedules place timesteps between the training ones). For an integer-valued
+// t the arithmetic is the int kernel's after its (float) conversion, so the embedding is bit-identical.
+__global__ void timestep_embedding_f32_kernel(const float* __restrict__ t, int nt, int dim, float max_period,
+                                              float* __restrict__ out) {
+  const int half = dim / 2;
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nt * half) return;
+  const int b = i / half, j = i % half;
+  const float freq = expf((float)j * (-logf(max_period) / (float)half));
+  const float arg = t[b] * freq;
+  out[(size_t)b * dim + j] = cosf(arg);
+  out[(size_t)b * dim + half + j] = sinf(arg);
+}
+int timestep_embedding_f32_launch(cudaStream_t st, const float* t_dev, int nt, int dim, float max_period, float* out) {
+  const int n = nt * (dim / 2);
+  timestep_embedding_f32_kernel<<<cdiv(n, 128), 128, 0, st>>>(t_dev, nt, dim, max_period, out);
+  return (int)cudaGetLastError();
+}
 
 // ------------------------------------------------------------------------------------------------
 // First conv (4 -> model_channels, 3x3 pad 1; reference unet/mod.rs:116-120). K = 36: CUDA cores.
@@ -515,7 +533,9 @@ int dup_latent_f16_launch(cudaStream_t st, const float* x, size_t n, int nfwd, _
 // ------------------------------------------------------------------------------------------------
 // Philox4x32-10 counter RNG + Box-Muller. Element i of stream (seed, subseq): counter =
 // (i/4 lo32, i/4 hi32, subseq lo32, subseq hi32), key = (seed lo32, seed hi32); lane i%4 of the
-// 4 normals produced from the 4 output words. oracle/philox.py is the bit-identical restatement.
+// 4 normals produced from the 4 output words. oracle/philox.py is the bit-identical restatement, and noise4() below (the
+// scheduled samplers' in-kernel noise) repeats this arithmetic: change the three together (tests/test_schedulers_gpu.py compares
+// the two kernels bit for bit).
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void philox4x32_10(uint32_t c[4], uint32_t k0, uint32_t k1) {
 #pragma unroll
@@ -550,6 +570,124 @@ __global__ void randn_kernel(float* __restrict__ out, size_t n, uint64_t seed, u
 }
 int randn_launch(cudaStream_t st, float* out, size_t n, uint64_t seed, uint64_t subseq) {
   randn_kernel<<<cdiv((long)((n + 3) / 4), 256), 256, 0, st>>>(out, n, seed, subseq);
+  return (int)cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
+// The scheduled samplers' step (DESIGN.md §16; kernels.h: GuidedStepParams). One thread per block of four consecutive
+// elements of the NCHW state, which is the block one Philox counter produces: in-kernel noise repeats randn_kernel's
+// arithmetic on the same counter, so it equals randn_launch(seed, subseq) bit for bit. The state, history, noise and reference
+// go through 16-byte vectors when the block is whole and the pointers are aligned; the mask is read byte by byte. The eps rows
+// are NHWC and are gathered element by element: each of a thread's four loads is a warp-wide gather with stride 4 * ld floats,
+// none of them coalesced on its own (the four together cover one contiguous span, served from L1 / L2).
+// ------------------------------------------------------------------------------------------------
+__device__ __forceinline__ void noise4(const float* __restrict__ z, uint64_t seed, uint64_t subseq, size_t blk, size_t n, bool vec,
+                                       float out[4]) {
+  if (z) {
+    if (vec) {
+      const float4 v = *reinterpret_cast<const float4*>(z + blk * 4);
+      out[0] = v.x; out[1] = v.y; out[2] = v.z; out[3] = v.w;
+    } else {
+      for (int j = 0; j < 4; ++j) out[j] = blk * 4 + j < n ? z[blk * 4 + j] : 0.f;
+    }
+    return;
+  }
+  uint32_t c[4] = {(uint32_t)blk, (uint32_t)(blk >> 32), (uint32_t)subseq, (uint32_t)(subseq >> 32)};
+  philox4x32_10(c, (uint32_t)seed, (uint32_t)(seed >> 32));
+#pragma unroll
+  for (int j = 0; j < 2; ++j) {
+    const float u1 = ((float)(c[2 * j] >> 8) + 0.5f) * (1.0f / 16777216.0f);
+    const float u2 = ((float)(c[2 * j + 1] >> 8) + 0.5f) * (1.0f / 16777216.0f);
+    const float rad = sqrtf(-2.0f * logf(u1));
+    const float ang = 6.283185307179586f * u2;
+    out[2 * j] = rad * cosf(ang);
+    out[2 * j + 1] = rad * sinf(ang);
+  }
+}
+__device__ __forceinline__ void load4(const float* __restrict__ p, size_t blk, size_t n, bool vec, float out[4]) {
+  if (vec) {
+    const float4 v = *reinterpret_cast<const float4*>(p + blk * 4);
+    out[0] = v.x; out[1] = v.y; out[2] = v.z; out[3] = v.w;
+  } else {
+    for (int j = 0; j < 4; ++j) out[j] = blk * 4 + j < n ? p[blk * 4 + j] : 0.f;
+  }
+}
+__device__ __forceinline__ void store4(float* __restrict__ p, size_t blk, size_t n, bool vec, const float v[4]) {
+  if (vec) {
+    *reinterpret_cast<float4*>(p + blk * 4) = make_float4(v[0], v[1], v[2], v[3]);
+  } else {
+    for (int j = 0; j < 4; ++j)
+      if (blk * 4 + j < n) p[blk * 4 + j] = v[j];
+  }
+}
+__global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams p, int aligned) {
+  const size_t n = (size_t)p.Bimg * p.C * p.HW, nblk = (n + 3) / 4;
+  const size_t blk = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (blk >= nblk) return;
+  const bool vec = aligned && blk * 4 + 4 <= n;
+  float xh[4], D[4];
+  load4(p.xh, blk, n, vec, xh);
+  if (p.eps) {
+    const int grp_u = p.Bimg, grp_p = (p.use_cfg ? 2 : 1) * p.Bimg;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) {
+      const size_t i = blk * 4 + j;
+      D[j] = 0.f;
+      if (i >= n) continue;
+      const int px = (int)(i % p.HW);
+      const int c = (int)((i / p.HW) % p.C);
+      const int b = (int)(i / ((size_t)p.HW * p.C));
+      const float ec = p.eps[((size_t)b * p.HW + px) * p.ld + c];
+      float e = ec;
+      if (p.use_cfg) {   // u + (c - u) * s, cfg_ddim_kernel's order
+        const float eu = p.eps[((size_t)(grp_u + b) * p.HW + px) * p.ld + c];
+        e = eu + (ec - eu) * p.guidance;
+      }
+      if (p.use_pag) {   // cfg_pag_ddim_kernel's
+        const float ep = p.eps[((size_t)(grp_p + b) * p.HW + px) * p.ld + c];
+        e = e + p.p_t * (ec - ep);
+      }
+      D[j] = xh[j] - p.sigma * e;
+    }
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) D[j] = xh[j];
+  }
+  float nx[4];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) nx[j] = p.cx * xh[j] + p.cd * D[j];
+  if (p.ch != 0.f) {
+    float h[4];
+    load4(p.hist, blk, n, vec, h);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) nx[j] += p.ch * h[j];
+  }
+  if (p.write_hist) store4(p.hist, blk, n, vec, D);
+  if (p.cn != 0.f) {
+    float z[4];
+    noise4(p.z, p.seed, p.z_subseq, blk, n, vec, z);
+#pragma unroll
+    for (int j = 0; j < 4; ++j) nx[j] += p.cn * z[j];
+  }
+  if (p.mask) {   // the latent-blend inpainting of the NEXT forward: xh = mask ? xh : ref + sigma' * z
+    float z[4], r[4];
+    noise4(p.zb, p.seed, p.zb_subseq, blk, n, vec, z);
+    load4(p.ref, blk, n, vec, r);
+#pragma unroll
+    for (int j = 0; j < 4; ++j)
+      if (blk * 4 + j < n && !p.mask[blk * 4 + j]) nx[j] = r[j] + p.sigma_blend * z[j];
+  }
+  store4(p.xh, blk, n, vec, nx);
+#pragma unroll
+  for (int j = 0; j < 4; ++j) nx[j] *= p.c_in;
+  store4(p.x_in, blk, n, vec, nx);
+}
+int guided_step_launch(cudaStream_t st, const GuidedStepParams& p) {
+  const size_t n = (size_t)p.Bimg * p.C * p.HW;
+  if (!n) return 0;
+  if (!p.xh || !p.x_in || ((p.ch != 0.f || p.write_hist) && !p.hist) || (p.mask && !p.ref)) return (int)cudaErrorInvalidValue;
+  const uintptr_t a = (uintptr_t)p.xh | (uintptr_t)p.x_in | (uintptr_t)p.hist | (uintptr_t)p.z | (uintptr_t)p.zb | (uintptr_t)p.ref;
+  guided_step_kernel<<<cdiv((long)((n + 3) / 4), 256), 256, 0, st>>>(p, a % 16 == 0);
   return (int)cudaGetLastError();
 }
 

@@ -13,6 +13,7 @@
 //              forward_diffuser, get_alpha}
 //                               src/model/stablediffusion/mod.rs:317-541
 #include "engine_core.h"
+#include "schedule.h"
 
 #include <set>
 
@@ -151,6 +152,7 @@ static int latent_channels(const sdxl_unet_cfg& g) { return inpaint_layout(g) ? 
 
 struct Plan;
 struct Sampler;
+struct TimeSlot { int t; float tf; };   // one write of the timestep: lround(t) and t
 struct ControlAttach;
 struct IpAttach;
 struct T2IAttach;
@@ -240,8 +242,8 @@ struct sdxl_unet : EncoderHalf {
   // plan
   std::unique_ptr<Plan> plan;
   std::unique_ptr<Sampler> sampler;
-  int* t_dev = nullptr;
-  int* t_pinned = nullptr;
+  int* t_dev = nullptr;        // the timestep on the device: the int the T2I-Adapter window compares, then (t_dev + 1) the float the embedding reads
+  TimeSlot* t_pinned = nullptr;
   int t_slot = 0;              // ring position in t_pinned (per model: independent contexts never share it)
   AdapterState lora;           // LoRA-able weight slots, backups of merged layers (sdxl_unet_set_adapters)
   std::vector<std::unique_ptr<ControlAttach>> controls;   // sdxl_unet_set_controls, in call order
@@ -575,7 +577,7 @@ static int unet_load_impl(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pac
   });
   if (r) return r;
   CU(c, cudaMalloc((void**)&u->t_dev, 64));
-  CU(c, cudaMallocHost((void**)&u->t_pinned, 4096 * sizeof(int)));
+  CU(c, cudaMallocHost((void**)&u->t_pinned, 4096 * sizeof(TimeSlot)));
   *out = u.release();
   return 0;
 }
@@ -1073,7 +1075,7 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
   {
     Op op{};
     op.kind = OP_TEMB;
-    op.te = {u->t_dev, 1, mc, te};
+    op.te = {(const float*)(u->t_dev + 1), 1, mc, te};
     P->ops.push_back(op);
   }
   // --- embeddings, input blocks, middle
@@ -1210,11 +1212,11 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w, int Bp) {
 
 static int run_plan(sdxl_unet* u) { return run_plan_ops(u->ctx, u->plan.get()); }
 
-static int set_t(sdxl_unet* u, int t) {
+static int set_t(sdxl_unet* u, double t) {
   sdxl_ctx* c = u->ctx;
   const int slot = u->t_slot = (u->t_slot + 1) % 4096;
-  u->t_pinned[slot] = t;
-  CU(c, cudaMemcpyAsync(u->t_dev, &u->t_pinned[slot], sizeof(int), cudaMemcpyHostToDevice, c->stream));
+  u->t_pinned[slot] = {(int)lround(t), (float)t};
+  CU(c, cudaMemcpyAsync(u->t_dev, &u->t_pinned[slot], sizeof(TimeSlot), cudaMemcpyHostToDevice, c->stream));
   return 0;
 }
 
@@ -2282,9 +2284,14 @@ extern "C" int sdxl_unet_forward(sdxl_unet* u, int B, int h, int w, const sdxl_h
   return 0;
 }
 extern "C" int sdxl_unet_forward_f32(sdxl_unet* u, int B, int h, int w, const float* x, int32_t t_host, float* eps_out) {
+  return sdxl_unet_forward_f32_at(u, B, h, w, x, (double)t_host, eps_out);
+}
+extern "C" int sdxl_unet_forward_f32_at(sdxl_unet* u, int B, int h, int w, const float* x, double t_host, float* eps_out) {
   if (!u || !x || !eps_out) return -1;
   sdxl_ctx* c = u->ctx;
   CU(c, cudaSetDevice(c->device));
+  if (!(t_host >= 0.0 && t_host <= (double)(u->cfg.n_steps - 1)))   // also refuses NaN
+    return fail(c, 5024, "forward: timestep %g outside [0, %d]", t_host, u->cfg.n_steps - 1);
   int r = ensure_plan(u, B, B, h, w, u->pag ? u->pag->forward_rows : 0);
   if (r) return r;
   Plan* P = u->plan.get();
@@ -2330,6 +2337,8 @@ struct Sampler {
   bool cfg = false, pag = false;
   float guidance = 1.f;
   float* noise = nullptr;  // scratch [Bimg,4,h,w]
+  float* xh = nullptr;     // scheduled samplers: the state x / sqrt(alpha) and the previous step's denoised latent (DPM++ 2M)
+  float* hist = nullptr;
   float* ref = nullptr;
   uint8_t* mask = nullptr;
   __half* cond_ctx = nullptr;  // staged [nfwd*Bimg, n_ctx, ctx]
@@ -2344,14 +2353,14 @@ struct Sampler {
 
 // Uploads/assembles the batched conditioning: rows [0,Bimg) conditional, rows [Bimg,2*Bimg) the
 // unconditional context repeated (reference stablediffusion/mod.rs:506-537). With PAG attached a last group of Bimg rows repeats
-// the conditional rows (the refiner, without CFG: [cond | ptb]).
-static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double guidance) {
+// the conditional rows (the refiner, without CFG: [cond | ptb]). no_cfg: the base model runs its conditional rows alone too.
+static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double guidance, bool no_cfg = false) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   if (!cond) return fail(c, 5200, "null conditioning");
   const int Bimg = cond->n_batch, n_ctx = cond->n_ctx;
   const int h = cond->resolution[0] / 8, w = cond->resolution[1] / 8;
-  const bool use_cfg = !g.is_refiner, pag = u->pag != nullptr;
+  const bool use_cfg = !g.is_refiner && !no_cfg, pag = u->pag != nullptr;
   const int nfwd = (use_cfg ? 2 : 1) + (pag ? 1 : 0);
   const RowLayout layout{Bimg, use_cfg};
   const sdxl_half* ctx_c = g.is_refiner ? cond->context_open_clip : cond->context_full;
@@ -2376,6 +2385,8 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
     const size_t y_elems = (size_t)nfwd * Bimg * g.adm_in_channels;
     if (int r = carve_measured(c, S->arena, 5203, "sampler buffers", [&](Arena& A) {
           S->noise = A.get<float>(lat);
+          S->xh = A.get<float>(lat);
+          S->hist = A.get<float>(lat);
           S->ref = A.get<float>(lat);
           S->mask = A.get<uint8_t>(lat);
           S->cond_ctx = A.get<__half>(ctx_elems);
@@ -2537,6 +2548,131 @@ extern "C" int sdxl_sample_latent(sdxl_unet* u, const sdxl_conditioning* cond, d
     if ((r = sampler_step(u, t, t_prev))) return r;
   }
   CU(c, cudaMemcpyAsync(latent_out, P->x_in, bytes, cond->on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+  if (cond->on_host) CU(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
+// ================================================================================================
+// scheduled samplers (include/sdxl_b200.h: sdxl_schedule; DESIGN.md §16)
+// ================================================================================================
+static thread_local std::string g_schedule_err;
+extern "C" const char* sdxl_schedule_last_error(void) { return g_schedule_err.c_str(); }
+extern "C" int sdxl_schedule_build(const double* alphas_cumprod, int n_train, const sdxl_schedule* s, double* timesteps, double* sigmas) {
+  g_schedule_err.clear();
+  if (!alphas_cumprod || !timesteps || !sigmas) g_schedule_err = "schedule_build: null argument";
+  else if (n_train < 1) g_schedule_err = "schedule_build: n_train must be >= 1";
+  else g_schedule_err = schedule_problem(s, n_train);
+  if (g_schedule_err.empty())
+    for (int i = 0; i < n_train; ++i)
+      if (!(alphas_cumprod[i] > 0.0 && alphas_cumprod[i] < 1.0) || (i && !(alphas_cumprod[i] < alphas_cumprod[i - 1]))) {
+        g_schedule_err = "schedule_build: alphas_cumprod[" + std::to_string(i) + "] is not inside (0, 1) and below its predecessor";
+        break;
+      }
+  if (!g_schedule_err.empty()) return 5230;
+  schedule_fill(SigmaTable(alphas_cumprod, n_train), *s, timesteps, sigmas);
+  return 0;
+}
+
+extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditioning* cond, double guidance_scale, const sdxl_schedule* sch,
+                                            const float* init_latent, const float* noise, int n_noise, uint64_t seed,
+                                            const float* inpaint_ref, const uint8_t* inpaint_mask, float* latent_out) {
+  if (!u || !cond || !latent_out) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  // everything is validated before any state changes
+  const int N = (int)u->alphas.size();
+  const std::string why = schedule_problem(sch, N);
+  if (!why.empty()) return fail(c, 5230, "%s", why.c_str());
+  if ((inpaint_ref == nullptr) != (inpaint_mask == nullptr)) return fail(c, 5231, "inpaint_ref and inpaint_mask must be given together");
+  if (sch->first_step > 0 && !init_latent) return fail(c, 5232, "schedule: first_step = %d needs init_latent", sch->first_step);
+  if (n_noise < 0 || (n_noise > 0 && !noise)) return fail(c, 5233, "n_noise = %d with %s noise", n_noise, noise ? "a" : "null");
+  const int n = sch->n_steps, k0 = sch->first_step, k1 = sch->last_step ? sch->last_step : n;
+  std::vector<double> ts(n), sig(n + 1);
+  schedule_fill(SigmaTable(u->alphas.data(), N), *sch, ts.data(), sig.data());
+  for (int k = 0; k < n; ++k)
+    if (!(sig[k + 1] < sig[k])) return fail(c, 5234, "schedule: n_steps = %d gives sigmas that do not decrease at step %d", n, k);
+
+  int r = sampler_begin(u, cond, guidance_scale, sch->no_cfg != 0);
+  if (r) return r;
+  Sampler* S = u->sampler.get();
+  Plan* P = u->plan.get();
+  const size_t lat = S->latent_elems, bytes = lat * 4;
+  const cudaMemcpyKind in_kind = cond->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+  // the step kernel reads its noise in place: injected tensors from the host are staged on the device once
+  TmpBufs tmp(c->stream);
+  const float* noise_dev = noise;
+  if (n_noise && cond->on_host) {
+    float* d = (float*)tmp.get((size_t)n_noise * bytes);
+    if (!d) return fail(c, 5235, "cannot allocate %zu bytes to stage the injected noise", (size_t)n_noise * bytes);
+    CU(c, cudaMemcpyAsync(d, noise, (size_t)n_noise * bytes, cudaMemcpyHostToDevice, c->stream));
+    noise_dev = d;
+  }
+  int noise_used = 0;
+  uint64_t subseq = 0;
+  auto next_noise = [&](const float*& z, uint64_t& sub) {   // injected tensors first, then the seeded stream
+    z = nullptr;
+    sub = 0;
+    if (noise_used < n_noise) z = noise_dev + (size_t)noise_used++ * lat;
+    else sub = subseq++;
+  };
+  if (inpaint_ref) {
+    CU(c, cudaMemcpyAsync(S->ref, inpaint_ref, bytes, in_kind, c->stream));
+    CU(c, cudaMemcpyAsync(S->mask, inpaint_mask, lat, in_kind, c->stream));
+  }
+  GuidedStepParams p{};
+  p.Bimg = S->Bimg; p.C = latent_channels(u->cfg); p.HW = S->h * S->w;
+  p.xh = S->xh; p.x_in = P->x_in; p.hist = S->hist;
+  p.seed = seed;
+  if (inpaint_ref) { p.mask = S->mask; p.ref = S->ref; }
+  // entry: xh at sigma_k0, blended for the first forward
+  float* init_dev = nullptr;
+  if (init_latent && (k0 == 0 && cond->on_host)) {   // the initial noise from the host: read by the kernel as z
+    init_dev = (float*)tmp.get(bytes);
+    if (!init_dev) return fail(c, 5235, "cannot allocate %zu bytes to stage the initial noise", bytes);
+    CU(c, cudaMemcpyAsync(init_dev, init_latent, bytes, cudaMemcpyHostToDevice, c->stream));
+  }
+  if (k0 == 0) {
+    CU(c, cudaMemsetAsync(S->xh, 0, bytes, c->stream));
+    p.cx = 0.f;
+    p.cn = (float)sqrt(sig[0] * sig[0] + 1.0);
+    if (init_latent) p.z = init_dev ? init_dev : init_latent;
+    else next_noise(p.z, p.z_subseq);
+  } else {
+    CU(c, cudaMemcpyAsync(S->xh, init_latent, bytes, in_kind, c->stream));
+    p.cx = 1.f;
+    if (sch->renoise) {
+      p.cn = (float)sig[k0];
+      next_noise(p.z, p.z_subseq);
+    }
+  }
+  p.c_in = (float)(1.0 / sqrt(sig[k0] * sig[k0] + 1.0));
+  if (inpaint_ref) {
+    p.sigma_blend = (float)sig[k0];
+    next_noise(p.zb, p.zb_subseq);
+  }
+  KL(c, guided_step_launch(c->stream, p));
+  // the steps: write t, replay the plan, one launch
+  p.eps = P->eps; p.ld = P->eps_ld; p.use_cfg = S->cfg; p.use_pag = S->pag; p.guidance = S->guidance;
+  for (int k = k0; k < k1; ++k) {
+    if ((r = set_t(u, ts[k]))) return r;
+    if ((r = run_plan(u))) return r;
+    const StepCoef q = step_coef(*sch, k, ts.data(), sig.data(), k > k0);
+    p.sigma = (float)sig[k];
+    p.cx = q.cx; p.cd = q.cd; p.ch = q.ch; p.cn = q.cn; p.c_in = q.c_in;
+    p.write_hist = sampler_keeps_history(sch->sampler);
+    // diffusers' adaptive scaling (sampler_step's), at the fractional t
+    if (S->pag) p.p_t = std::max(u->pag->scale - u->pag->adaptive * (float)(u->cfg.n_steps - ts[k]), 0.f);
+    p.z = p.zb = nullptr;
+    p.mask = nullptr;
+    if (q.cn != 0.f) next_noise(p.z, p.z_subseq);
+    if (inpaint_ref && k + 1 < k1) {   // the blend before the next forward: its noise follows this step's in the call's order
+      p.mask = S->mask;
+      p.sigma_blend = (float)sig[k + 1];
+      next_noise(p.zb, p.zb_subseq);
+    }
+    KL(c, guided_step_launch(c->stream, p));
+  }
+  CU(c, cudaMemcpyAsync(latent_out, S->xh, bytes, cond->on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
   if (cond->on_host) CU(c, cudaStreamSynchronize(c->stream));
   return 0;
 }

@@ -441,7 +441,7 @@ struct Op {
   GnParams gn;
   struct { const float* x; const float* g; const float* b; float eps; int rows, C; __half* y; } ln;
   struct { const float* in; int in_bstride, Bv, K; const __half* W; int ldw; const float* bias; const float* add; int add_bstride, N, in_silu, out_silu; float* out; int out_bstride; } gv;
-  struct { const int* t; int n, dim; float* out; } te;
+  struct { const float* t; int n, dim; float* out; } te;
   // x2 (nullable): second input source, channels [Cin, Cin + C2) (conv_in_cat_launch)
   struct { const float* x; int Bx, B, Cin, H, W; const float* w; const float* bias; int Cout; float* y; const float* add; int n_add;
            const float* x2; int n2, C2; } ci;
@@ -667,7 +667,7 @@ static int exec_op(sdxl_ctx* c, Op& op) {
       KL(c, gemv_launch(st, op.gv.in, op.gv.in_bstride, op.gv.Bv, op.gv.K, op.gv.W, op.gv.ldw, op.gv.bias, op.gv.add, op.gv.add_bstride,
                         op.gv.N, op.gv.in_silu, op.gv.out_silu, op.gv.out, op.gv.out_bstride));
       break;
-    case OP_TEMB: KL(c, timestep_embedding_launch(st, op.te.t, op.te.n, op.te.dim, 10000.f, op.te.out)); break;
+    case OP_TEMB: KL(c, timestep_embedding_f32_launch(st, op.te.t, op.te.n, op.te.dim, 10000.f, op.te.out)); break;
     case OP_CONV_IN:
       if (op.ci.x2)
         KL(c, conv_in_cat_launch(st, op.ci.x, 1, op.ci.Bx, op.ci.B, op.ci.Cin, op.ci.x2, op.ci.n2, op.ci.C2, op.ci.H, op.ci.W, op.ci.w,

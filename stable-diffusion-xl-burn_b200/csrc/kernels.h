@@ -201,6 +201,8 @@ int gemv_launch(cudaStream_t st, const float* in, int in_bstride, int Bv, int K,
 // timestep_embedding (reference unet/mod.rs:21-39): out[b, :] = [cos(t*f_i), sin(t*f_i)], dim even.
 int timestep_embedding_launch(cudaStream_t st, const int* t_dev, int nt, int dim, float max_period,
                               float* out);
+// the same of float timesteps; bit-identical to the int form at integer values
+int timestep_embedding_f32_launch(cudaStream_t st, const float* t_dev, int nt, int dim, float max_period, float* out);
 // First conv: x NCHW f16 [B,Cin,H,W] (Cin<=8) -> NHWC f32 [B,H,W,Cout], 3x3 pad 1. w: [Cout][3][3][Cin] f32.
 int conv_in_launch(cudaStream_t st, const __half* x, int B, int Cin, int H, int W, const float* w,
                    const float* bias, int Cout, float* y);
@@ -247,6 +249,30 @@ int inpaint_blend_launch(cudaStream_t st, float* x, const float* ref, const floa
 int axpby_launch(cudaStream_t st, float* x, const float* noise, size_t n, float sa, float sb);
 // Standard normal noise, Philox4x32-10 + Box-Muller, element i of stream (seed, subseq).
 int randn_launch(cudaStream_t st, float* out, size_t n, uint64_t seed, uint64_t subseq);
+// One step of a scheduled sampler (DESIGN.md §16) on the k-diffusion-scaled state xh, f32 NCHW [Bimg, C, HW], in one launch:
+//   e   = guided eps of the NHWC rows [cond], [cond | uncond], [cond | ptb] or [cond | uncond | ptb] (cfg_ddim / cfg_pag_ddim's combines)
+//   D   = xh - sigma * e                          (eps == nullptr: no model output, D = xh: the entry of a call)
+//   xh' = cx * xh + cd * D + ch * hist + cn * z   (hist read when ch != 0, then D written to it when write_hist)
+//   xh' = mask ? xh' : ref + sigma_blend * zb     (mask != nullptr: the latent blend before the next forward)
+//   x_in = c_in * xh'                             (the next forward's input)
+// z and zb are read from memory when non-null, else generated in the kernel as randn_launch(seed, z_subseq / zb_subseq) would.
+struct GuidedStepParams {
+  const float* eps;
+  int ld, Bimg, C, HW, use_cfg, use_pag;
+  float guidance, p_t, sigma;
+  float cx, cd, ch, cn, c_in;
+  float* xh;
+  float* x_in;
+  float* hist;
+  int write_hist;
+  const float* z;
+  const float* zb;
+  uint64_t seed, z_subseq, zb_subseq;
+  const uint8_t* mask;
+  const float* ref;
+  float sigma_blend;
+};
+int guided_step_launch(cudaStream_t st, const GuidedStepParams& p);
 int dup_latent_f16_launch(cudaStream_t st, const float* x, size_t n, int nfwd, __half* x16);
 
 // Latent-decoder kernels (vae_kernels.cu)

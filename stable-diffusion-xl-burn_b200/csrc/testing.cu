@@ -5,6 +5,7 @@
 // kernel against a float64 reference. The VAE, text / vision encoder, T2I-Adapter and sampler kernels are reached the same
 // way. All pointers are device pointers; every function returns the launcher's status.
 #include "kernels.h"
+#include "schedule.h"
 
 #define SDXL_TEST_API extern "C" __attribute__((visibility("default")))
 
@@ -280,4 +281,29 @@ SDXL_TEST_API int sdxl_test_scale_weights(void* stream, const void* w, size_t nw
 }
 SDXL_TEST_API int sdxl_test_vec_add_f32(void* stream, float* dst, const float* src, int n) {
   return vec_add_f32_launch((cudaStream_t)stream, dst, src, n);
+}
+
+// The scheduled samplers (schedule.h, elementwise.cu): the host coefficient function, out = (cx, cd, ch, cn, c_in), the step kernel
+// with GuidedStepParams filled as sdxl_sample_latent_scheduled fills it, and the float timestep embedding of the UNet plan.
+SDXL_TEST_API void sdxl_test_step_coef(const sdxl_schedule* s, int k, const double* timesteps, const double* sigmas, int has_prev,
+                                       float* out) {
+  const StepCoef q = step_coef(*s, k, timesteps, sigmas, has_prev != 0);
+  out[0] = q.cx; out[1] = q.cd; out[2] = q.ch; out[3] = q.cn; out[4] = q.c_in;
+}
+SDXL_TEST_API int sdxl_test_guided_step(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
+                                        float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,
+                                        float* xh, float* x_in, float* hist, int write_hist, const float* z, const float* zb,
+                                        uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq, const uint8_t* mask, const float* ref,
+                                        float sigma_blend) {
+  GuidedStepParams p{};
+  p.eps = eps; p.ld = ld; p.Bimg = Bimg; p.C = C; p.HW = HW; p.use_cfg = use_cfg; p.use_pag = use_pag;
+  p.guidance = guidance; p.p_t = p_t; p.sigma = sigma;
+  p.cx = cx; p.cd = cd; p.ch = ch; p.cn = cn; p.c_in = c_in;
+  p.xh = xh; p.x_in = x_in; p.hist = hist; p.write_hist = write_hist;
+  p.z = z; p.zb = zb; p.seed = seed; p.z_subseq = z_subseq; p.zb_subseq = zb_subseq;
+  p.mask = mask; p.ref = ref; p.sigma_blend = sigma_blend;
+  return guided_step_launch((cudaStream_t)stream, p);
+}
+SDXL_TEST_API int sdxl_test_timestep_embedding_f32(void* stream, const float* t, int nt, int dim, float max_period, float* out) {
+  return timestep_embedding_f32_launch((cudaStream_t)stream, t, nt, dim, max_period, out);
 }

@@ -11,6 +11,8 @@ from .tokenizer import ClipTokenizer, OpenClipTokenizer  # noqa: F401
 from .embedder import ClipTextEncoder, Embedder, conditioning_embedding  # noqa: F401
 from .pipeline import load_models, make_inpaint_mask, prepare_inpaint_condition, sample  # noqa: F401
 from . import diffusers_unet  # noqa: F401
+from . import schedulers  # noqa: F401
+from .schedulers import Schedule  # noqa: F401
 from .controlnet import ControlNet  # noqa: F401
 from .ip_adapter import IPAdapter  # noqa: F401
 from .t2i_adapter import T2IAdapter, t2i_t_min  # noqa: F401

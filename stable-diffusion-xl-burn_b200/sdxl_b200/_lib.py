@@ -120,6 +120,12 @@ class Freeu(C.Structure):
     _fields_ = [("s1", C.c_float), ("s2", C.c_float), ("b1", C.c_float), ("b2", C.c_float)]
 
 
+class Schedule(C.Structure):
+    _fields_ = [("sampler", C.c_int32), ("spacing", C.c_int32), ("n_steps", C.c_int32), ("first_step", C.c_int32),
+                ("last_step", C.c_int32), ("renoise", C.c_int32), ("no_cfg", C.c_int32), ("karras_rho", C.c_float),
+                ("eta", C.c_float), ("s_noise", C.c_float)]
+
+
 # name -> (restype, argtypes); every symbol include/sdxl_b200.h declares
 P = C.c_void_p
 I = C.c_int
@@ -135,6 +141,10 @@ PROTOTYPES = {
     "sdxl_unet_forward": (I, [P, I, I, I, P, C.c_int32, P]),
     "sdxl_unet_forward_f32": (I, [P, I, I, I, P, C.c_int32, P]),
     "sdxl_sample_latent": (I, [P, C.POINTER(Conditioning), C.c_double, I, I, P, P, I, C.c_uint64, P, P, P]),
+    "sdxl_schedule_build": (I, [P, I, C.POINTER(Schedule), P, P]),
+    "sdxl_schedule_last_error": (C.c_char_p, []),
+    "sdxl_sample_latent_scheduled": (I, [P, C.POINTER(Conditioning), C.c_double, C.POINTER(Schedule), P, P, I, C.c_uint64, P, P, P]),
+    "sdxl_unet_forward_f32_at": (I, [P, I, I, I, P, C.c_double, P]),
     "sdxl_sampler_begin": (I, [P, C.POINTER(Conditioning), C.c_double]),
     "sdxl_sampler_step": (I, [P, I, I]),
     "sdxl_sampler_step_host": (I, [P, I, I, P]),

@@ -68,6 +68,9 @@ PROTOTYPES = {
     "sdxl_test_nhwc_to_nchw_f32": (I, [P, P, I, I, I, I, P]),
     "sdxl_test_scale_weights": (I, [P, P, Z, P, I, F, P, P]),
     "sdxl_test_vec_add_f32": (I, [P, P, P, I]),
+    "sdxl_test_step_coef": (None, [P, I, P, P, I, P]),
+    "sdxl_test_guided_step": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, F, F, P, P, P, I, P, P, C.c_uint64, C.c_uint64, C.c_uint64, P, P, F]),
+    "sdxl_test_timestep_embedding_f32": (I, [P, P, I, I, F, P]),
 }
 _lib = None
 
@@ -349,3 +352,19 @@ def scale_weights(w, nw, b, nb, s, wo, bo) -> None:
 
 def vec_add_f32(dst, src, n) -> None:
     _call("sdxl_test_vec_add_f32", _p(dst), _p(src), n)
+
+
+def guided_step(eps: Optional[torch.Tensor], ld: int, Bimg: int, Cc: int, HW: int, use_cfg: bool, use_pag: bool, guidance: float, p_t: float,
+                sigma: float, coef: Sequence[float], xh: torch.Tensor, x_in: torch.Tensor, hist: Optional[torch.Tensor] = None,
+                write_hist: bool = False, z: Optional[torch.Tensor] = None, zb: Optional[torch.Tensor] = None, seed: int = 0,
+                z_subseq: int = 0, zb_subseq: int = 0, mask: Optional[torch.Tensor] = None, ref: Optional[torch.Tensor] = None,
+                sigma_blend: float = 0.0) -> None:
+    """coef = (cx, cd, ch, cn, c_in); xh, x_in and hist are updated in place (kernels.h: GuidedStepParams)."""
+    _call("sdxl_test_guided_step", _p(eps), ld, Bimg, Cc, HW, int(use_cfg), int(use_pag), guidance, p_t, sigma, *[float(v) for v in coef],
+          _p(xh), _p(x_in), _p(hist), int(write_hist), _p(z), _p(zb), seed, z_subseq, zb_subseq, _p(mask), _p(ref), sigma_blend)
+
+
+def timestep_embedding_f32(t: torch.Tensor, dim: int, max_period: float = 10000.0) -> torch.Tensor:
+    out = torch.empty(t.numel(), dim, device=t.device, dtype=torch.float32)
+    _call("sdxl_test_timestep_embedding_f32", _p(t), t.numel(), dim, max_period, _p(out))
+    return out

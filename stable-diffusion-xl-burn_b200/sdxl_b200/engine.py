@@ -441,14 +441,18 @@ class Diffuser:
                 self._set_pag((*self._pag, int(perturbed_rows)))
         if context is not None:
             self.set_conditioning(context, label)
-        t = int(timesteps[0]) if hasattr(timesteps, "__len__") else int(timesteps)
+        t = float(timesteps[0]) if hasattr(timesteps, "__len__") else float(timesteps)   # fractional: between two training timesteps
         B, _, h, w = x.shape
         # convert first, then enter: the ctx stream must wait for the cast / copy kernels torch queues on its own stream
         f16 = x.dtype == torch.float16
         x = x.to(ctx.device, torch.float16 if f16 else torch.float32).contiguous()
         out = torch.empty_like(x)
-        ctx.call("sdxl_unet_forward", ctx.lib.sdxl_unet_forward if f16 else ctx.lib.sdxl_unet_forward_f32, self.h, B, h, w, _ptr(x), t,
-                 _ptr(out))
+        if f16:
+            if t != int(t):
+                raise SdxlError(f"unet_forward: a fractional timestep ({t}) needs an f32 latent")
+            ctx.call("sdxl_unet_forward", ctx.lib.sdxl_unet_forward, self.h, B, h, w, _ptr(x), int(t), _ptr(out))
+        else:
+            ctx.call("sdxl_unet_forward_f32_at", ctx.lib.sdxl_unet_forward_f32_at, self.h, B, h, w, _ptr(x), t, _ptr(out))
         return out
 
     @property
@@ -484,7 +488,9 @@ class Diffuser:
     # ---- Diffuser::* ---------------------------------------------------------------------------
     def _sample(self, cond: Conditioning, guidance: float, n_steps: int, step_start: int,
                 init_latent: Optional[torch.Tensor], noise: Optional[torch.Tensor], seed: int,
-                ref: Optional[torch.Tensor], mask: Optional[torch.Tensor], host: bool = False) -> torch.Tensor:
+                ref: Optional[torch.Tensor], mask: Optional[torch.Tensor], host: bool = False, schedule=None) -> torch.Tensor:
+        """schedule (schedulers.Schedule): sdxl_sample_latent_scheduled with its sampler and spacing; n_steps and step_start are
+        then unused (the schedule carries them). None: sdxl_sample_latent's DDIM loop."""
         ctx = self.ctx
         s, keep = cond.to_struct(None if host else ctx.device)
         h, w = cond.resolution[0] // 8, cond.resolution[1] // 8
@@ -498,29 +504,38 @@ class Diffuser:
         mask = prep(mask, torch.uint8)
         n_noise = 0 if noise is None else (noise.shape[0] if noise.dim() == 5 else 1)
         out = torch.empty(s.n_batch, self.cfg.latent_channels, h, w, device=dev, dtype=torch.float32)
-        ctx.call("sdxl_sample_latent", ctx.lib.sdxl_sample_latent, self.h, C.byref(s), float(guidance), n_steps, step_start, _ptr(init_latent),
-                 _ptr(noise), n_noise, seed, _ptr(ref), _ptr(mask), _ptr(out))
+        if schedule is not None:
+            sch = schedule.to_struct()
+            ctx.call("sdxl_sample_latent_scheduled", ctx.lib.sdxl_sample_latent_scheduled, self.h, C.byref(s), float(guidance), C.byref(sch),
+                     _ptr(init_latent), _ptr(noise), n_noise, seed, _ptr(ref), _ptr(mask), _ptr(out))
+        else:
+            ctx.call("sdxl_sample_latent", ctx.lib.sdxl_sample_latent, self.h, C.byref(s), float(guidance), n_steps, step_start,
+                     _ptr(init_latent), _ptr(noise), n_noise, seed, _ptr(ref), _ptr(mask), _ptr(out))
         del keep
         return out
 
     def sample_latent(self, conditioning: Conditioning, unconditional_guidance_scale: float, n_steps: int,
-                      noise: Optional[torch.Tensor] = None, seed: int = 0, host: bool = False) -> torch.Tensor:
+                      noise: Optional[torch.Tensor] = None, seed: int = 0, host: bool = False, schedule=None,
+                      step_noise: Optional[torch.Tensor] = None) -> torch.Tensor:
         """== Diffuser::sample_latent (mod.rs:317-332). `noise` injects gen_noise()'s tensor (the reference's
-        RNG is unseeded libtorch Philox; parity tests inject it)."""
-        return self._sample(conditioning, unconditional_guidance_scale, n_steps, 0, noise, None, seed, None, None, host)
+        RNG is unseeded libtorch Philox; parity tests inject it). schedule (schedulers.Schedule): its sampler, spacing and steps
+        instead of n_steps DDIM steps; step_noise [k, n, 4, h, w] then injects the sampler's per-step noise."""
+        return self._sample(conditioning, unconditional_guidance_scale, n_steps, 0, noise, step_noise, seed, None, None, host, schedule)
 
     def sample_latent_with_inpainting(self, conditioning: Conditioning, unconditional_guidance_scale: float,
                                       n_steps: int, reference: torch.Tensor, mask: torch.Tensor,
                                       init_noise: Optional[torch.Tensor] = None,
-                                      step_noise: Optional[torch.Tensor] = None, seed: int = 0) -> torch.Tensor:
-        """== Diffuser::sample_latent_with_inpainting (mod.rs:334-353); mask True keeps the generated latent."""
+                                      step_noise: Optional[torch.Tensor] = None, seed: int = 0, schedule=None) -> torch.Tensor:
+        """== Diffuser::sample_latent_with_inpainting (mod.rs:334-353); mask True keeps the generated latent. With a schedule the
+        blend is xh = mask ? xh : reference + sigma_k z before each forward."""
         return self._sample(conditioning, unconditional_guidance_scale, n_steps, 0, init_noise, step_noise, seed,
-                            reference, mask.to(torch.uint8))
+                            reference, mask.to(torch.uint8), schedule=schedule)
 
     def refine_latent(self, latent: torch.Tensor, conditioning: Conditioning, unconditional_guidance_scale: float,
-                      step_start: int, n_steps: int, noise: Optional[torch.Tensor] = None, seed: int = 0) -> torch.Tensor:
-        """== Diffuser::refine_latent (mod.rs:355-376)."""
-        return self._sample(conditioning, unconditional_guidance_scale, n_steps, step_start, latent, noise, seed, None, None)
+                      step_start: int, n_steps: int, noise: Optional[torch.Tensor] = None, seed: int = 0, schedule=None) -> torch.Tensor:
+        """== Diffuser::refine_latent (mod.rs:355-376). With a schedule its first_step / renoise say where the latent enters."""
+        return self._sample(conditioning, unconditional_guidance_scale, n_steps, step_start, latent, noise, seed, None, None,
+                            schedule=schedule)
 
     # ---- step-wise (bench) ---------------------------------------------------------------------
     def sampler_begin(self, cond: Conditioning, guidance: float) -> None:

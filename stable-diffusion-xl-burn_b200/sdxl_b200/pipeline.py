@@ -54,7 +54,8 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
            resolution: Tuple[int, int] = (1024, 1024), seed: int = 0, noise: Optional[torch.Tensor] = None,
            loras: Optional[Sequence] = None, controls: Optional[Sequence] = None, image_prompt: Optional[Sequence] = None,
            t2i_adapters: Optional[Sequence] = None, t2i_factor: float = 1.0, pag: Optional[Sequence] = None,
-           freeu: Optional[Sequence[float]] = None) -> torch.Tensor:
+           freeu: Optional[Sequence[float]] = None, sampler: Optional[str] = None, spacing: Optional[str] = None,
+           no_cfg: bool = False) -> torch.Tensor:
     """One image, like `sample --prompt ... [--reference-img ... --crop-* ...] [--use-refiner]`.
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
     bottom) in pixels. With an inpainting UNet (cfg.is_inpaint, DESIGN.md §12) reference_rgb is required: the crop window becomes the
@@ -72,19 +73,24 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     adapter_conditioning_factor). pag: (scale, layers[, adaptive_scale]) perturbed-attention guidance (Diffuser.set_pag, diffusers'
     pag_scale, pag_applied_layers, pag_adaptive_scale) attached to the base UNet for this call and detached afterwards (the refiner is
     left alone). freeu: (s1, s2, b1, b2) FreeU (Diffuser.set_freeu, diffusers' enable_freeu) attached to the base UNet for this call
-    and detached afterwards (the refiner is left alone). Returns uint8 [1, H, W, 3]."""
+    and detached afterwards (the refiner is left alone). sampler / spacing (schedulers.SAMPLERS / SPACINGS; one given, the other
+    defaults to "euler" / "leading") and no_cfg (one conditional forward per step, for few-step distilled models) build one
+    schedulers.Schedule of n_steps for the base model; a refiner then runs the same schedule from the first step whose timestep is
+    below 1000 - REFINER_STEP_START, re-noising the base latent to that step's sigma. All three None / False: the reference's DDIM
+    loop. Returns uint8 [1, H, W, 3]."""
+    sch = dict(sampler=sampler, spacing=spacing, no_cfg=no_cfg)
     if freeu:
         diffuser.set_freeu(*freeu)
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                          seed, noise, loras, controls, image_prompt, t2i_adapters, t2i_factor, pag)
+                          seed, noise, loras, controls, image_prompt, t2i_adapters, t2i_factor, pag, **sch)
         finally:
             diffuser.set_freeu(None)
     if pag:
         diffuser.set_pag(pag[1], pag[0], *pag[2:3])
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                          seed, noise, loras, controls, image_prompt, t2i_adapters, t2i_factor)
+                          seed, noise, loras, controls, image_prompt, t2i_adapters, t2i_factor, **sch)
         finally:
             diffuser.set_pag(None)
     if image_prompt:
@@ -103,27 +109,33 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
             diffuser.set_image_prompt(adapter, e.unsqueeze(0), scale, negative=neg.unsqueeze(0))
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                          seed, noise, loras, controls, t2i_adapters=t2i_adapters, t2i_factor=t2i_factor)
+                          seed, noise, loras, controls, t2i_adapters=t2i_adapters, t2i_factor=t2i_factor, **sch)
         finally:
             diffuser.set_image_prompt(None)
     if controls:
         diffuser.set_controls(controls)
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                          seed, noise, loras, t2i_adapters=t2i_adapters, t2i_factor=t2i_factor)
+                          seed, noise, loras, t2i_adapters=t2i_adapters, t2i_factor=t2i_factor, **sch)
         finally:
             diffuser.set_controls([])
     if t2i_adapters:
-        from .t2i_adapter import t2i_t_min
-        diffuser.set_t2i_adapters(t2i_adapters, t_min=t2i_t_min(n_steps, t2i_factor))
+        schedule = _schedule(n_steps, **sch)
+        if schedule is None:
+            from .t2i_adapter import t2i_t_min
+            t_min = t2i_t_min(n_steps, t2i_factor)
+        else:   # the window follows the timesteps this schedule writes
+            from .schedulers import t2i_t_min
+            t_min = t2i_t_min(_alphas(diffuser), schedule, t2i_factor)
+        diffuser.set_t2i_adapters(t2i_adapters, t_min=t_min)
         try:
             return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                          seed, noise, loras)
+                          seed, noise, loras, **sch)
         finally:
             diffuser.set_t2i_adapters([])
     if not loras:
         return _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                       seed, noise)
+                       seed, noise, **sch)
     from .lora import load_kohya
     parts = [load_kohya(src, diffuser.cfg, embedder.clip.cfg, embedder.open_clip.cfg) for src, _ in loras]
     active = []
@@ -134,13 +146,44 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
                 active.append(model)
                 model.set_adapters(sets)
         return _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
-                       seed, noise)
+                       seed, noise, **sch)
     finally:
         for model in active:
             model.set_adapters([])
 
 
-def _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution, seed, noise):
+def _schedule(n_steps, sampler=None, spacing=None, no_cfg=False):
+    """sample()'s schedule: None (the reference's DDIM loop) unless one of the three is given."""
+    if sampler is None and spacing is None and not no_cfg:
+        return None
+    from .schedulers import Schedule
+    return Schedule(sampler or "euler", spacing or "leading", n_steps, no_cfg=no_cfg)
+
+
+def _alphas(model):
+    return [model.alpha(i) for i in range(model.cfg.n_steps)]
+
+
+def refiner_schedule(refiner, schedule):
+    """The refiner's part of the base model's schedule: from the first step whose timestep is below n_steps - REFINER_STEP_START,
+    re-noising the base latent to that step's sigma. Refused when the schedule has no such step or starts below it: the hand-off
+    the caller asked for does not exist."""
+    from dataclasses import replace
+    from .schedulers import build
+    t, _ = build(_alphas(refiner), schedule)
+    limit = refiner.cfg.n_steps - REFINER_STEP_START
+    below = [k for k in range(schedule.n_steps) if t[k] < limit]
+    if not below or below[0] == 0:
+        raise _lib.SdxlError(f"sample: the refiner takes over at the first timestep below {limit}, but the {schedule.spacing} schedule of "
+                             f"{schedule.n_steps} steps runs from t = {t[0]:g} to {t[-1]:g}: {'every' if below else 'no'} step is below it")
+    return replace(schedule, first_step=below[0], renoise=True)
+
+
+def _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution, seed, noise,
+            sampler=None, spacing=None, no_cfg=False):
+    schedule = _schedule(n_steps, sampler, spacing, no_cfg)
+    kw = {} if schedule is None else {"schedule": schedule}   # None: the calls below are the reference's, argument for argument
+    refine = refiner_schedule(refiner, schedule) if refiner is not None and schedule is not None else None   # before any sampling
     inpaint_unet = diffuser.cfg.is_inpaint
     if inpaint_unet and reference_rgb is None:
         raise _lib.SdxlError("sample: an inpainting UNet needs reference_rgb (the image to repaint)")
@@ -156,7 +199,7 @@ def _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, ref
         cond.resolution = (8 * int(c.shape[2]), 8 * int(c.shape[3]))
         diffuser.set_inpaint_condition(c)
         try:
-            latent = diffuser.sample_latent(cond, guidance, n_steps, noise=noise, seed=seed)
+            latent = diffuser.sample_latent(cond, guidance, n_steps, noise=noise, seed=seed, **kw)
         finally:
             diffuser.set_inpaint_condition(None)
     elif reference_rgb is not None:
@@ -164,10 +207,12 @@ def _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, ref
         lh, lw = int(ref_latent.shape[2]), int(ref_latent.shape[3])
         cond.resolution = (8 * lh, 8 * lw)   # the sampler's latent extent follows the encoded reference (== the image size for the x8 SDXL VAE)
         mask = make_inpaint_mask(resolution, (lh, lw), *crop, crop_out=crop_out)
-        latent = diffuser.sample_latent_with_inpainting(cond, guidance, n_steps, ref_latent, mask, init_noise=noise, seed=seed)   # main.rs:246
+        latent = diffuser.sample_latent_with_inpainting(cond, guidance, n_steps, ref_latent, mask, init_noise=noise, seed=seed, **kw)   # main.rs:246
     else:
-        latent = diffuser.sample_latent(cond, guidance, n_steps, noise=noise, seed=seed)                                      # main.rs:249
-    if refiner is not None:
+        latent = diffuser.sample_latent(cond, guidance, n_steps, noise=noise, seed=seed, **kw)                                   # main.rs:249
+    if refine is not None:
+        latent = refiner.refine_latent(latent, cond, guidance, 0, n_steps, seed=seed + 1, schedule=refine)
+    elif refiner is not None:
         latent = refiner.refine_latent(latent, cond, guidance, REFINER_STEP_START, n_steps, seed=seed + 1)                    # main.rs:258-265
     return decoder.latent_to_image(latent)                                                                                   # main.rs:277
 
