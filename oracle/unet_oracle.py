@@ -22,13 +22,46 @@ python/save.py): Linear weight [in,out], conv weight OIHW.
 """
 from __future__ import annotations
 
+import dataclasses
 import math
-from typing import Dict, List, Optional, Sequence, Tuple
+from typing import Callable, Collection, Dict, List, Optional, Sequence, Tuple
 
 import torch
 import torch.nn.functional as F
 
 W = Dict[str, torch.Tensor]
+
+
+@dataclasses.dataclass
+class Attach:
+    """What is attached to the UNet, one field per attachment kind of the engine (DESIGN.md §8-15). The defaults attach nothing.
+    A row b of the UNet batch reads row b % n of every per-row tensor.
+
+    controls: [(ControlNetConfig, f32 weights, hint [n, 3, H, W], scale)], residuals added to the skips and the middle in order.
+    prompts: image prompts [(f32 adapter weights (pack names), tokens [B, S_ip, ctx], scales {transformer block path: s},
+        mask [n_images, H, W] or None)], every prompt in each attn2.
+    uncond_tokens: for forward_diffuser, the tokens of the unconditional rows, one per prompt (tokens are the conditional rows').
+    t2i: (the summed T2I features [F_0, F_1, F_2, F_3] of rows [n, ...], t_min): added while timesteps[0] >= t_min.
+    concat: the inpainting condition [n, C, h, w], concatenated to the latent before the first conv.
+    pag_layers: transformer block paths whose self-attention computes the identity out(value(x)).
+    pag_scale: for forward_diffuser, PAG's p_t of an integer timestep.
+    freeu: diffusers' (s1, s2, b1, b2), at the skip pops of output blocks 0..5 when all four are nonzero."""
+    controls: Sequence = ()
+    prompts: Sequence = ()
+    uncond_tokens: Sequence = ()
+    t2i: Optional[Tuple[Sequence[torch.Tensor], int]] = None
+    concat: Optional[torch.Tensor] = None
+    pag_layers: Collection[str] = ()
+    pag_scale: Optional[Callable[[int], float]] = None
+    freeu: Optional[Sequence[float]] = None
+
+
+NOTHING = Attach()
+
+
+def _rows(t: torch.Tensor, n: int) -> torch.Tensor:
+    """Row b of the result is row b % len(t) of t."""
+    return t[torch.arange(n) % t.shape[0]]
 
 
 # ---------------------------------------------------------------------------------------------------
@@ -143,15 +176,71 @@ def geglu(x: torch.Tensor, w: W, p: str) -> torch.Tensor:
     return projected[..., :n] * gelu_erf(projected[..., n:])
 
 
-def transformer_block(x: torch.Tensor, context: torch.Tensor, w: W, p: str, n_head: int) -> torch.Tensor:
-    """TransformerBlock::forward, src/model/unet/mod.rs:885-891."""
-    x = x + multi_head_attention(layer_norm(x, w[f"{p}/norm1/weight"], w[f"{p}/norm1/bias"]), None, w, f"{p}/attn1", n_head)
-    x = x + multi_head_attention(layer_norm(x, w[f"{p}/norm2/weight"], w[f"{p}/norm2/bias"]), context, w, f"{p}/attn2", n_head)
+def mask_grid(H: int, W: int, T: int):
+    """(mh, mw) of diffusers' IPAdapterMaskProcessor.downsample for T queries and an H x W mask, both kept >= 1 (diffusers divides
+    by zero there)."""
+    ratio = W / H
+    mh = max(1, int(math.sqrt(T / ratio)))
+    mh += int(T % mh != 0)
+    return mh, max(1, T // mh)
+
+
+def downsample_mask(mask: torch.Tensor, T: int) -> torch.Tensor:
+    """[n, H, W] -> [n, T]: bicubic to mask_grid, flattened row-major, zero-padded or cut to T."""
+    n, H, W = mask.shape
+    mh, mw = mask_grid(H, W, T)
+    m = F.interpolate(mask[:, None].float(), size=(mh, mw), mode="bicubic", align_corners=False)[:, 0].reshape(n, -1)
+    if m.shape[1] < T:
+        return torch.cat([m, m.new_zeros(n, T - m.shape[1])], 1)
+    return m[:, :T]
+
+
+def multi_attention(q, k, v, sources: Sequence, n_head: int) -> torch.Tensor:
+    """softmax(q k^T) v + sum over sources (k_s, v_s, s, m) of s * m[t] * softmax(q k_s^T) v_s (m None: 1), in order."""
+    h = qkv_attention(q, k, v, None, n_head)
+    for k_s, v_s, s, m in sources:
+        a = s * qkv_attention(q, k_s, v_s, None, n_head)
+        h = h + (a if m is None else a * m[None, :, None])
+    return h
+
+
+def prompt_sources(T: int, prompts: Sequence, a: str, p: str) -> list:
+    """The attention sources of image prompts in the attn2 `a` of transformer block `p` for T queries: one per unmasked prompt
+    (one softmax over all its tokens), one per image of a masked prompt, weighted per query by its downsampled mask."""
+    out = []
+    for wa, tokens, scales, mask in prompts:
+        k, v = linear(tokens, wa, f"{a}/ip_key"), linear(tokens, wa, f"{a}/ip_value")
+        if mask is None:
+            out.append((k, v, scales[p], None))
+            continue
+        n = mask.shape[0]
+        m = downsample_mask(mask, T)
+        per = k.shape[1] // n
+        out += [(k[:, i * per:(i + 1) * per], v[:, i * per:(i + 1) * per], scales[p], m[i]) for i in range(n)]
+    return out
+
+
+def transformer_block(x: torch.Tensor, context: torch.Tensor, w: W, p: str, n_head: int, att: Attach = NOTHING) -> torch.Tensor:
+    """TransformerBlock::forward, src/model/unet/mod.rs:885-891; PAG's identity self-attention if p is in att.pag_layers, the image
+    prompts' sources beside the text in attn2."""
+    h = layer_norm(x, w[f"{p}/norm1/weight"], w[f"{p}/norm1/bias"])
+    if p in att.pag_layers:
+        x = x + linear(linear(h, w, f"{p}/attn1/value"), w, f"{p}/attn1/out")
+    else:
+        x = x + multi_head_attention(h, None, w, f"{p}/attn1", n_head)
+    h = layer_norm(x, w[f"{p}/norm2/weight"], w[f"{p}/norm2/bias"])
+    if att.prompts:
+        a = f"{p}/attn2"
+        q, k, v = linear(h, w, f"{a}/query"), linear(context, w, f"{a}/key"), linear(context, w, f"{a}/value")
+        x = x + linear(multi_attention(q, k, v, prompt_sources(q.shape[1], att.prompts, a, p), n_head), w, f"{a}/out")
+    else:
+        x = x + multi_head_attention(h, context, w, f"{p}/attn2", n_head)
     h = layer_norm(x, w[f"{p}/norm3/weight"], w[f"{p}/norm3/bias"])
     return x + linear(geglu(h, w, f"{p}/mlp/geglu"), w, f"{p}/mlp/lin")  # MLP::forward :915-919
 
 
-def spatial_transformer(x: torch.Tensor, context: torch.Tensor, w: W, p: str, n_head: int, depth: int) -> torch.Tensor:
+def spatial_transformer(x: torch.Tensor, context: torch.Tensor, w: W, p: str, n_head: int, depth: int,
+                        att: Attach = NOTHING) -> torch.Tensor:
     """SpatialTransformer::forward, src/model/unet/mod.rs:820-845."""
     n_batch, n_channel, height, width = x.shape
     x_in = x
@@ -159,7 +248,7 @@ def spatial_transformer(x: torch.Tensor, context: torch.Tensor, w: W, p: str, n_
     x = x.reshape(n_batch, n_channel, height * width).transpose(1, 2)
     x = linear(x, w, f"{p}/proj_in")
     for j in range(depth):
-        x = transformer_block(x, context, w, f"{p}/transformer_{j}", n_head)
+        x = transformer_block(x, context, w, f"{p}/transformer_{j}", n_head, att)
     x = linear(x, w, f"{p}/proj_out").transpose(1, 2).reshape(n_batch, n_channel, height, width)
     return x_in + x
 
@@ -209,7 +298,7 @@ def unet_blocks(cfg) -> Tuple[List[tuple], tuple, List[tuple]]:
     return ins, mid, outs
 
 
-def _run_block(kind: str, p: str, n_head: int, depth: int, x, emb, context, w: W):
+def _run_block(kind: str, p: str, n_head: int, depth: int, x, emb, context, w: W, att: Attach = NOTHING):
     if kind == "conv":
         return conv2d(x, w, p)                                  # :776-780
     if kind == "downsample":
@@ -218,15 +307,14 @@ def _run_block(kind: str, p: str, n_head: int, depth: int, x, emb, context, w: W
         return res_block(x, emb, w, p)
     x = res_block(x, emb, w, f"{p}/res")                        # ResTransformer* :571-577, :657-663, ResUpsample :607-612
     if "transformer" in kind:
-        x = spatial_transformer(x, context, w, f"{p}/transformer", n_head, depth)
+        x = spatial_transformer(x, context, w, f"{p}/transformer", n_head, depth, att)
     if kind.endswith("upsample"):
         x = upsample(x, w, f"{p}/upsample")
     return x
 
 
-def unet_forward(cfg, w: W, x: torch.Tensor, timesteps: torch.Tensor, context: torch.Tensor, label: torch.Tensor) -> torch.Tensor:
-    """UNet::forward, src/model/unet/mod.rs:449-493. x [B,4,h,w], timesteps Int [1] (or [B]),
-    context [B,n_ctx,Cctx], label [B,adm]."""
+def _emb(cfg, w: W, timesteps: torch.Tensor, label: torch.Tensor) -> torch.Tensor:
+    """The time + label embedding, src/model/unet/mod.rs:449-460."""
     t_emb = timestep_embedding(timesteps, cfg.model_channels, 10000)
     t_emb = linear(t_emb, w, "lin1_time_embed")
     t_emb = silu(t_emb)
@@ -234,22 +322,127 @@ def unet_forward(cfg, w: W, x: torch.Tensor, timesteps: torch.Tensor, context: t
     label_emb = linear(label, w, "lin1_label_embed")
     label_emb = silu(label_emb)
     label_emb = linear(label_emb, w, "lin2_label_embed")
-    emb = t_emb + label_emb
-    ins, mid, outs = unet_blocks(cfg)
+    return t_emb + label_emb
+
+
+def encoder(cfg, w: W, x: torch.Tensor, emb: torch.Tensor, context: torch.Tensor, att: Attach = NOTHING,
+            adds: Optional[Dict[str, torch.Tensor]] = None) -> Tuple[torch.Tensor, List[torch.Tensor]]:
+    """The input blocks and the middle block: (the middle block's output, every input block's output). adds {block path or
+    "middle_block": tensor} is added to that block's output (T2I features, the ControlNet's hint embedding)."""
+    adds = adds or {}
+    ins, mid, _ = unet_blocks(cfg)
     saved = []
     for kind, p, nh, d in ins:
-        x = _run_block(kind, p, nh, d, x, emb, context, w)
+        x = _run_block(kind, p, nh, d, x, emb, context, w, att)
+        if p in adds:
+            x = x + adds[p]
         saved.append(x)
     _, mp, nh, d = mid                                          # ResTransformerRes::forward :713-719
     x = res_block(x, emb, w, f"{mp}/res1")
-    x = spatial_transformer(x, context, w, f"{mp}/transformer", nh, d)
+    x = spatial_transformer(x, context, w, f"{mp}/transformer", nh, d, att)
     x = res_block(x, emb, w, f"{mp}/res2")
-    for kind, p, nh, d in outs:
-        x = torch.cat([x, saved.pop()], dim=1)                  # :484
-        x = _run_block(kind, p, nh, d, x, emb, context, w)
+    if mp in adds:
+        x = x + adds[mp]
+    return x, saved
+
+
+def unet_forward(cfg, w: W, x: torch.Tensor, timesteps: torch.Tensor, context: torch.Tensor, label: torch.Tensor,
+                 att: Optional[Attach] = None) -> torch.Tensor:
+    """UNet::forward, src/model/unet/mod.rs:449-493. x [B,4,h,w], timesteps Int [1] (or [B]),
+    context [B,n_ctx,Cctx], label [B,adm]. The attachments go in where and in the order the engine's plan puts them: the
+    inpainting condition before the first conv; T2I features on the injection blocks' and the middle block's outputs; ControlNet
+    residuals (their nets see the latent without the condition, run unperturbed and without image prompts) on the skips and the
+    middle; FreeU at the skip pops; PAG and image prompts in the transformer blocks."""
+    att = att or NOTHING
+    n = x.shape[0]
+    latent = x
+    if att.concat is not None:
+        x = torch.cat([x, _rows(att.concat, n)], dim=1)
+    emb = _emb(cfg, w, timesteps, label)
+    adds = {}
+    if att.t2i is not None and int(timesteps[0]) >= att.t2i[1]:
+        adds = {p: _rows(f, n) for p, f in zip(injection_blocks(cfg) + ["middle_block"], att.t2i[0])}
+    x, saved = encoder(cfg, w, x, emb, context, att, adds)
+    for ncfg, wc, hint, scale in att.controls:
+        res, r_mid = controlnet_forward(ncfg, wc, latent, timesteps, context, label, hint_embedding(ncfg, wc, hint))
+        saved = [s + scale * r for s, r in zip(saved, res)]
+        x = x + scale * r_mid
+    for i, (kind, p, nh, d) in enumerate(unet_blocks(cfg)[2]):
+        skip = saved.pop()
+        if freeu_enabled(att.freeu) and i // 3 < 2:           # up_blocks[0] and [1]: three output blocks each
+            x, skip = apply_freeu(i // 3, x, skip, att.freeu)
+        x = torch.cat([x, skip], dim=1)                         # :484
+        x = _run_block(kind, p, nh, d, x, emb, context, w, att)
     x = group_norm(x, w["norm_out/weight"], w["norm_out/bias"])
     x = silu(x)
     return conv2d(x, w, "conv_out")
+
+
+# ---------------------------------------------------------------------------------------------------
+# attachments the forward computes
+# ---------------------------------------------------------------------------------------------------
+def hint_embedding(ncfg, w: W, hint: torch.Tensor) -> torch.Tensor:
+    """SGM input_hint_block: conv(in -> c0), then SiLU + conv after each conv, stride 2 on every second, last conv(c_last -> mc)."""
+    x = conv2d(hint, w, "input_hint_block/0")
+    idx = 2
+    for _ in range(len(ncfg.hint_block_channels) - 1):
+        x = conv2d(silu(x), w, f"input_hint_block/{idx}")
+        x = conv2d(silu(x), w, f"input_hint_block/{idx + 2}", stride=2)
+        idx += 4
+    return conv2d(silu(x), w, f"input_hint_block/{idx}")
+
+
+def controlnet_forward(ncfg, w: W, x, timesteps, context, label, hint_emb):
+    """The control branch: (residuals r_i = zero_conv_i(h_i) for every input block, r_mid = middle_block_out(mid)), the hint
+    embedding (row b reads row b % n) added to the first conv's output."""
+    cfg = ncfg.unet
+    h, saved = encoder(cfg, w, x, _emb(cfg, w, timesteps, label), context, adds={"input_blocks/0": _rows(hint_emb, x.shape[0])})
+    return [conv2d(s, w, f"zero_convs/{i}", padding=0) for i, s in enumerate(saved)], conv2d(h, w, "middle_block_out", padding=0)
+
+
+def injection_blocks(cfg) -> List[str]:
+    """Input blocks receiving the T2I features F_0..F_2: a level's last resnet+transformer block, or for a transformer-free level
+    its last block (its Downsample); F_3 follows the middle block."""
+    ins, _, _ = unet_blocks(cfg)
+    per_level, level = [[]], 0
+    for kind, p, _, _ in ins[1:]:
+        per_level[level].append((kind, p))
+        if kind == "downsample":
+            level += 1
+            per_level.append([])
+    out = []
+    for blocks in per_level:
+        tr = [p for kind, p in blocks if "transformer" in kind]
+        out.append(tr[-1] if tr else blocks[-1][1])
+    return out
+
+
+def fourier_filter(x_in: torch.Tensor, threshold: int, scale: float) -> torch.Tensor:
+    """diffusers.utils.torch_utils.fourier_filter on a real [B, C, H, W] tensor (its f16 / bf16 upcast does not apply here)."""
+    x = x_in
+    B, C, H, W = x.shape
+    x_freq = torch.fft.fftn(x, dim=(-2, -1))
+    x_freq = torch.fft.fftshift(x_freq, dim=(-2, -1))
+    mask = torch.ones((B, C, H, W), dtype=x.dtype, device=x.device)
+    crow, ccol = H // 2, W // 2
+    mask[..., crow - threshold:crow + threshold, ccol - threshold:ccol + threshold] = scale
+    x_freq = x_freq * mask
+    x_freq = torch.fft.ifftshift(x_freq, dim=(-2, -1))
+    x_filtered = torch.fft.ifftn(x_freq, dim=(-2, -1)).real
+    return x_filtered.to(dtype=x_in.dtype)
+
+
+def freeu_enabled(freeu: Optional[Sequence[float]]) -> bool:
+    """diffusers' is_freeu_enabled: all four values given and nonzero."""
+    return freeu is not None and all(freeu)
+
+
+def apply_freeu(k: int, x: torch.Tensor, res: torch.Tensor, freeu: Sequence[float]):
+    """diffusers' apply_freeu at resolution_idx k (0, 1): x's first half of channels times b, the skip filtered with s."""
+    s, b = freeu[k], freeu[2 + k]
+    half = x.shape[1] // 2
+    x = torch.cat([x[:, :half] * b, x[:, half:]], dim=1)
+    return x, fourier_filter(res, 1, s)
 
 
 def to_f32(weights: W) -> W:
@@ -275,20 +468,32 @@ class OracleConditioning:
         self.resolution = kw.get("resolution", (1024, 1024))
 
 
-def forward_diffuser(cfg, w: W, latent: torch.Tensor, timestep: torch.Tensor, c: OracleConditioning, guidance: float) -> torch.Tensor:
-    """Diffuser::forward_diffuser, src/model/stablediffusion/mod.rs:494-541."""
+def forward_diffuser(cfg, w: W, latent: torch.Tensor, timestep: torch.Tensor, c: OracleConditioning, guidance: float,
+                     att: Optional[Attach] = None) -> torch.Tensor:
+    """Diffuser::forward_diffuser, src/model/stablediffusion/mod.rs:494-541, with the attachments on every row. Image prompts: the
+    conditional (and perturbed) rows of image b see tokens b % n_batch, the unconditional rows uncond_tokens b % n_batch. PAG adds
+    p_t * (c - perturbed) to the guided noise (to the conditional noise on the refiner), the perturbed rows being the conditional
+    ones with the identity self-attention in att.pag_layers."""
     n_batch = latent.shape[0]
+    att = att or NOTHING
     if not cfg.is_refiner:
         uctx, ctx, uy, y = c.unconditional_context_full, c.context_full, c.unconditional_channel_context, c.channel_context
     else:
         uctx, ctx, uy, y = (c.unconditional_context_open_clip, c.context_open_clip,
                             c.unconditional_channel_context_refiner, c.channel_context_refiner)
-    conditional = unet_forward(cfg, w, latent, timestep, ctx, y)
-    if cfg.is_refiner:
-        return conditional                                      # :528-530
+    cond = dataclasses.replace(att, prompts=[(wa, _rows(t, n_batch), s, m) for wa, t, s, m in att.prompts], pag_layers=())
+    conditional = unet_forward(cfg, w, latent, timestep, ctx, y, cond)
+    if att.pag_layers:
+        perturbed = unet_forward(cfg, w, latent, timestep, ctx, y, dataclasses.replace(cond, pag_layers=att.pag_layers))
+        p_t = att.pag_scale(int(timestep[0]))
+    if cfg.is_refiner:                                          # :528-530
+        return conditional + p_t * (conditional - perturbed) if att.pag_layers else conditional
+    unc = dataclasses.replace(cond, prompts=[(wa, _rows(t, n_batch), s, m) for (wa, _, s, m), t in zip(att.prompts, att.uncond_tokens,
+                                                                                                      strict=True)])
     unconditional = unet_forward(cfg, w, latent, timestep, uctx.unsqueeze(0).repeat(n_batch, 1, 1),
-                                 uy.unsqueeze(0).repeat(n_batch, 1))
-    return unconditional + (conditional - unconditional) * guidance   # :539-540
+                                 uy.unsqueeze(0).repeat(n_batch, 1), unc)
+    guided = unconditional + (conditional - unconditional) * guidance   # :539-540
+    return guided + p_t * (conditional - perturbed) if att.pag_layers else guided
 
 
 def get_alpha(alphas: torch.Tensor, i: int) -> float:
@@ -298,7 +503,7 @@ def get_alpha(alphas: torch.Tensor, i: int) -> float:
 
 def diffuse_latent(cfg, w: W, alphas: torch.Tensor, latent: torch.Tensor, c: OracleConditioning, step_start: int, n_steps: int,
                    guidance: float, reference: Optional[torch.Tensor] = None, mask: Optional[torch.Tensor] = None,
-                   step_noise: Optional[Sequence[torch.Tensor]] = None, trace=None) -> torch.Tensor:
+                   step_noise: Optional[Sequence[torch.Tensor]] = None, trace=None, att: Optional[Attach] = None) -> torch.Tensor:
     """Diffuser::diffuse_latent (:390-432) and diffuse_latent_with_inpainting (:434-483); DDIM, sigma = 0.
     `trace(iteration, latent)` (test aid, not in the reference) is called after every loop iteration."""
     total = cfg.n_steps
@@ -313,7 +518,7 @@ def diffuse_latent(cfg, w: W, alphas: torch.Tensor, latent: torch.Tensor, c: Ora
             noised_reference = reference * math.sqrt(current_alpha) + step_noise[it] * sqrt_noise
             latent = torch.where(mask.bool(), latent, noised_reference)   # mask_where: mask true keeps latent
         timestep = torch.tensor([t], dtype=torch.int32)
-        pred_noise = forward_diffuser(cfg, w, latent, timestep, c, guidance)
+        pred_noise = forward_diffuser(cfg, w, latent, timestep, c, guidance, att)
         predx0 = (latent - pred_noise * sqrt_noise) / math.sqrt(current_alpha)     # :423
         dir_latent = pred_noise * math.sqrt(1.0 - prev_alpha)                      # :424
         latent = predx0 * math.sqrt(prev_alpha) + dir_latent                       # :426-428 (sigma = 0)
@@ -323,22 +528,22 @@ def diffuse_latent(cfg, w: W, alphas: torch.Tensor, latent: torch.Tensor, c: Ora
     return latent
 
 
-def sample_latent(cfg, w, alphas, noise, c, guidance, n_steps, trace=None):
+def sample_latent(cfg, w, alphas, noise, c, guidance, n_steps, trace=None, att=None):
     """Diffuser::sample_latent, :317-332 (noise = gen_noise(), injected)."""
-    return diffuse_latent(cfg, w, alphas, noise, c, 0, n_steps, guidance, trace=trace)
+    return diffuse_latent(cfg, w, alphas, noise, c, 0, n_steps, guidance, trace=trace, att=att)
 
 
-def sample_latent_with_inpainting(cfg, w, alphas, noise, c, guidance, n_steps, reference, mask, step_noise):
+def sample_latent_with_inpainting(cfg, w, alphas, noise, c, guidance, n_steps, reference, mask, step_noise, att=None):
     """Diffuser::sample_latent_with_inpainting, :334-353."""
-    return diffuse_latent(cfg, w, alphas, noise, c, 0, n_steps, guidance, reference, mask, step_noise)
+    return diffuse_latent(cfg, w, alphas, noise, c, 0, n_steps, guidance, reference, mask, step_noise, att=att)
 
 
-def refine_latent(cfg, w, alphas, latent, c, guidance, step_start, n_steps, noise):
+def refine_latent(cfg, w, alphas, latent, c, guidance, step_start, n_steps, noise, att=None):
     """Diffuser::refine_latent, :355-376."""
     t = cfg.n_steps - step_start
     start_alpha = get_alpha(alphas, t)
     noised = latent * math.sqrt(start_alpha) + noise * math.sqrt(1.0 - start_alpha)
-    return diffuse_latent(cfg, w, alphas, noised, c, step_start, n_steps, guidance)
+    return diffuse_latent(cfg, w, alphas, noised, c, step_start, n_steps, guidance, att=att)
 
 
 def make_inpaint_mask(img_w: int, img_h: int, lat_w: int, lat_h: int, crop_left: Optional[int], crop_right: Optional[int],

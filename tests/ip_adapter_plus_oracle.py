@@ -1,18 +1,12 @@
-"""f32 CPU oracle of IP-Adapter Plus image prompts (DESIGN.md §10), beside tests/ip_adapter_oracle.py, whose UNet forward with
-decoupled cross-attention it reuses: the perceiver Resampler (h94 resampler.py, diffusers IPAdapterPlusImageProjection), the Plus
-prompt tokens and the DDIM CFG sampler with a Plus prompt.
-
-The sampler takes ip = (f32 adapter weights (pack names), hidden states [n_batch, n_images, L, D], negative hidden states of the
-same shape, scales {transformer block path: s}) and applies the engine's row rule: the CFG rows of image b use prompt b % n_batch
-(cond) and negative b % n_batch (uncond)."""
+"""IP-Adapter Plus image prompts (DESIGN.md §10) for the f32 CPU oracle, beside tests/ip_adapter_oracle.py: the perceiver
+Resampler (h94 resampler.py, diffusers IPAdapterPlusImageProjection), the Plus prompt tokens and the sampler's attachment of a Plus
+prompt (f32 adapter weights (pack names), hidden states [n_batch, n_images, L, D], negative hidden states of the same shape, scales
+{transformer block path: s})."""
 from __future__ import annotations
-
-import math
 
 import torch
 
 from oracle import unet_oracle as O
-import ip_adapter_oracle as IPO
 
 
 def perceiver_attention(x, lat, wa, p: str, n_head: int) -> torch.Tensor:
@@ -51,26 +45,7 @@ def plus_prompt_tokens(wa, hidden: torch.Tensor) -> torch.Tensor:
     return resample(wa, hidden.reshape(nb * ni, L, d)).reshape(nb, -1, wa["image_proj/norm_out/weight"].shape[0])
 
 
-def forward_diffuser(cfg, w, latent, timestep, c, guidance, ip):
-    """unet_oracle.forward_diffuser (base model, CFG) with a Plus prompt (sampler form of `ip`, see the module doc)."""
-    n_batch = latent.shape[0]
-    wa, hidden, negative, scales = ip
-    sel = torch.arange(n_batch) % hidden.shape[0]
-    ipc = (wa, plus_prompt_tokens(wa, hidden)[sel], scales)
-    ipu = (wa, plus_prompt_tokens(wa, negative)[sel], scales)
-    conditional = IPO.unet_forward(cfg, w, latent, timestep, c.context_full, c.channel_context, ipc)
-    unconditional = IPO.unet_forward(cfg, w, latent, timestep, c.unconditional_context_full.unsqueeze(0).repeat(n_batch, 1, 1),
-                                     c.unconditional_channel_context.unsqueeze(0).repeat(n_batch, 1), ipu)
-    return unconditional + (conditional - unconditional) * guidance
-
-
-def sample_latent(cfg, w, alphas, latent, c, n_steps, guidance, ip):
-    """unet_oracle.sample_latent (DDIM from step 0) with a Plus prompt."""
-    step_size = cfg.n_steps // n_steps
-    for t in range(cfg.n_steps - 1, -1, -step_size):
-        current_alpha = O.get_alpha(alphas, t)
-        prev_alpha = O.get_alpha(alphas, t - step_size) if t >= step_size else 1.0
-        pred_noise = forward_diffuser(cfg, w, latent, torch.tensor([t], dtype=torch.int32), c, guidance, ip)
-        predx0 = (latent - pred_noise * math.sqrt(1.0 - current_alpha)) / math.sqrt(current_alpha)
-        latent = predx0 * math.sqrt(prev_alpha) + pred_noise * math.sqrt(1.0 - prev_alpha)
-    return latent
+def attach(wa, hidden: torch.Tensor, negative: torch.Tensor, scales) -> O.Attach:
+    """The sampler's Plus prompt: the CFG rows of image b use prompt b % n_batch (cond) and negative
+    b % n_batch (uncond)."""
+    return O.Attach(prompts=[(wa, plus_prompt_tokens(wa, hidden), scales, None)], uncond_tokens=[plus_prompt_tokens(wa, negative)])

@@ -11,7 +11,6 @@ import torch
 from sdxl_b200 import SDXL_CONTROLNET, TINY, TINY_CONTROLNET, SdxlError, _lib, controlnet_tensor_specs, synth_weights
 from sdxl_b200.controlnet import diffusers_name_map, from_diffusers
 from oracle import unet_oracle as O
-import controlnet_oracle as CN
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -110,16 +109,16 @@ def test_oracle_zero_convs_leave_unet_unchanged():
             wc[k] = torch.zeros_like(wc[k])
     x, c, y, hint = small_inputs()
     t = torch.tensor([499])
-    assert torch.equal(CN.unet_forward(TINY, wu, x, t, c, y, [(TINY_CONTROLNET, wc, hint, 1.0)]), O.unet_forward(TINY, wu, x, t, c, y))
-    assert torch.equal(CN.unet_forward(TINY, wu, x, t, c, y), O.unet_forward(TINY, wu, x, t, c, y))
+    att = O.Attach(controls=[(TINY_CONTROLNET, wc, hint, 1.0)])
+    assert torch.equal(O.unet_forward(TINY, wu, x, t, c, y, att), O.unet_forward(TINY, wu, x, t, c, y))
 
 
 def test_oracle_hint_embedding_shape():
     wc = O.to_f32(synth_weights(TINY_CONTROLNET, seed=1))
-    e = CN.hint_embedding(TINY_CONTROLNET, wc, torch.rand(3, 3, 64, 96))
+    e = O.hint_embedding(TINY_CONTROLNET, wc, torch.rand(3, 3, 64, 96))
     assert e.shape == (3, TINY.model_channels, 8, 12) and e.is_contiguous()
-    res, mid = CN.controlnet_forward(TINY_CONTROLNET, wc, torch.randn(2, 4, 8, 12), torch.tensor([9]), torch.randn(2, 5, 24),
-                                     torch.randn(2, 8), e[:1])
+    res, mid = O.controlnet_forward(TINY_CONTROLNET, wc, torch.randn(2, 4, 8, 12), torch.tensor([9]), torch.randn(2, 5, 24),
+                                    torch.randn(2, 8), e[:1])
     assert [tuple(r.shape[1:]) for r in res] == ([(64, 8, 12)] * 3 + [(64, 4, 6)] + [(128, 4, 6)] * 2 + [(128, 2, 3)] +
                                                  [(256, 2, 3)] * 2)
     assert tuple(mid.shape) == (2, 256, 2, 3)
@@ -182,23 +181,3 @@ def test_close_is_refused_while_attached():
         net.close()
     assert net.h is not None
 
-
-def test_oracle_sampler_forks_match_unet_oracle():
-    """Without controls the controlled sampler of tests/controlnet_oracle.py computes exactly what oracle/unet_oracle.py does
-    (plain and inpainting), so a change to the oracle's sampler cannot leave the controlled tests on a stale copy."""
-    from sdxl_b200 import alphas_cumprod
-    wu = O.to_f32(synth_weights(TINY, seed=0))
-    g = torch.Generator().manual_seed(2)
-    c = O.OracleConditioning(context_full=torch.randn(1, 5, TINY.context_dim, generator=g),
-                             unconditional_context_full=torch.randn(5, TINY.context_dim, generator=g),
-                             channel_context=torch.randn(1, TINY.adm_in_channels, generator=g),
-                             unconditional_channel_context=torch.randn(TINY.adm_in_channels, generator=g))
-    x = torch.randn(1, 4, 8, 8, generator=g)
-    ref, mask = torch.randn(1, 4, 8, 8, generator=g), torch.rand(1, 4, 8, 8, generator=g) > 0.5
-    noise = [torch.randn(1, 4, 8, 8, generator=g) for _ in range(2)]
-    a = alphas_cumprod(TINY.n_steps)
-    t = torch.tensor([499], dtype=torch.int32)
-    assert torch.equal(CN.forward_diffuser(TINY, wu, x, t, c, 7.5), O.forward_diffuser(TINY, wu, x, t, c, 7.5))
-    assert torch.equal(CN.diffuse_latent(TINY, wu, a, x, c, 2, 7.5), O.diffuse_latent(TINY, wu, a, x, c, 0, 2, 7.5))
-    assert torch.equal(CN.diffuse_latent(TINY, wu, a, x, c, 2, 7.5, ref, mask, noise),
-                       O.diffuse_latent(TINY, wu, a, x, c, 0, 2, 7.5, ref, mask, noise))

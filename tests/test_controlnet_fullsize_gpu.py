@@ -6,7 +6,6 @@ import torch
 import sdxl_b200
 from sdxl_b200 import SDXL_BASE, SDXL_CONTROLNET, ControlNet, Diffuser
 from oracle import unet_oracle as O
-import controlnet_oracle as CN
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -29,7 +28,7 @@ def test_controlnet_1024(ctx):
     hint = torch.rand(1, 3, 1024, 1024, generator=g)
     wcf = O.to_f32(wc)
     emb = net.embed_hint(hint)
-    emb_ref = CN.hint_embedding(SDXL_CONTROLNET, wcf, hint)
+    emb_ref = O.hint_embedding(SDXL_CONTROLNET, wcf, hint)
     e_hint = rel_err(emb, emb_ref)
     d.set_controls([(net, hint, 1.0)])          # n_hint = 1: both CFG rows use the image's hint
     got = d.unet_forward(x, [749], c, y)
@@ -37,7 +36,7 @@ def test_controlnet_1024(ctx):
     base = d.unet_forward(x, [749], c, y)
     d.close()
     net.close()
-    ref = CN.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, [(SDXL_CONTROLNET, wcf, hint, 1.0)])
+    ref = O.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, O.Attach(controls=[(SDXL_CONTROLNET, wcf, hint, 1.0)]))
     e = rel_err(got, ref)
     print(f"SDXL ControlNet 1024^2: hint_emb rel err {e_hint:.2e}, CFG-batched forward rel err {e:.2e}, "
           f"the control moves the forward by {rel_err(got, base):.2e}")

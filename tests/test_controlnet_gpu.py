@@ -1,5 +1,5 @@
-"""GPU tests of ControlNet conditioning (sdxl_unet_set_controls), tiny configs, against the f32 oracle of
-tests/controlnet_oracle.py with the bounds of tests/test_unet_gpu.py, plus the bit-exact identities of attach / detach / rescale."""
+"""GPU tests of ControlNet conditioning (sdxl_unet_set_controls), tiny configs, against the f32 oracle
+(oracle/unet_oracle.py) with the bounds of tests/test_unet_gpu.py, plus the bit-exact identities of attach / detach / rescale."""
 import ctypes as C
 
 import numpy as np
@@ -10,7 +10,6 @@ import sdxl_b200
 from sdxl_b200 import TINY, TINY_CONTROLNET, Conditioning, ControlNet, ControlNetConfig, Diffuser, SdxlError, UNetConfig, synth_weights
 from sdxl_b200 import _lib
 from oracle import unet_oracle as O
-import controlnet_oracle as CN
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
@@ -63,8 +62,8 @@ class Setup:
         return self.d.unet_forward(X, [T], self.c, self.y)
 
     def oracle_fwd(self, controls):
-        return CN.unet_forward(TINY, self.wf, X, torch.tensor([T]), self.c, self.y,
-                               [(TINY_CONTROLNET, self.wcf[i], self.h[j], s) for i, j, s in controls])
+        return O.unet_forward(TINY, self.wf, X, torch.tensor([T]), self.c, self.y,
+                              O.Attach(controls=[(TINY_CONTROLNET, self.wcf[i], self.h[j], s) for i, j, s in controls]))
 
 
 @pytest.fixture(scope="module")
@@ -81,7 +80,7 @@ def S(ctx):
 
 def test_embed_hint_vs_oracle(S):
     got = S.nets[0].embed_hint(S.h[0])
-    ref = CN.hint_embedding(TINY_CONTROLNET, S.wcf[0], S.h[0])
+    ref = O.hint_embedding(TINY_CONTROLNET, S.wcf[0], S.h[0])
     assert got.shape == ref.shape
     assert rel_err(got, ref) <= FWD_TOL
 
@@ -169,7 +168,7 @@ def test_sample_cfg_vs_oracle(S):
     S.d.set_controls([])
     alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
     c = O.OracleConditioning(**cond_kwargs(TINY))
-    ref = CN.diffuse_latent(TINY, S.wf, alphas, S.noise, c, 4, 7.5, controls=[(TINY_CONTROLNET, S.wcf[0], S.h[0], 1.0)])
+    ref = O.sample_latent(TINY, S.wf, alphas, S.noise, c, 7.5, 4, att=O.Attach(controls=[(TINY_CONTROLNET, S.wcf[0], S.h[0], 1.0)]))
     assert rel_err(got, ref) <= SAMPLE_TOL
 
 
@@ -187,8 +186,8 @@ def test_inpainting_with_control(S):
     S.d.set_controls([])
     assert torch.equal(zero, plain)
     alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
-    want = CN.diffuse_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs(TINY)), 4, 7.5, ref_lat, mask,
-                             list(step_noise), controls=[(TINY_CONTROLNET, S.wcf[0], S.h[0], 1.0)])
+    want = O.sample_latent_with_inpainting(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs(TINY)), 7.5, 4, ref_lat, mask,
+                                           list(step_noise), att=O.Attach(controls=[(TINY_CONTROLNET, S.wcf[0], S.h[0], 1.0)]))
     assert rel_err(got, want) <= SAMPLE_TOL and not torch.equal(got, plain)
 
 

@@ -1,5 +1,5 @@
 """FreeU, host side: the closed form of diffusers' fourier_filter against its torch.fft statement, the oracle's identities with
-unet_oracle, the host twiddle table and the C ABI."""
+the plain forward, the host twiddle table and the C ABI."""
 import ctypes as C
 import math
 import os
@@ -24,7 +24,7 @@ def test_closed_form_is_the_fft_filter(H, W):
     g = torch.Generator().manual_seed(H * 100 + W)
     r = torch.randn(2, 3, H, W, generator=g, dtype=torch.float64)
     for s in (0.2, 0.9, 1.0, 1.7):
-        want = FO.fourier_filter(r, 1, s)
+        want = O.fourier_filter(r, 1, s)
         got = FO.fourier_filter_closed(r, s)
         assert float((got - want).abs().max()) <= 1e-12 * max(1.0, float(want.abs().max()))
 
@@ -35,7 +35,7 @@ def test_filter_acts_on_the_lowest_bins_only():
     g = torch.Generator().manual_seed(3)
     r = torch.randn(1, 2, 8, 6, generator=g, dtype=torch.float64)
     s = 0.25
-    ratio = torch.fft.fft2(FO.fourier_filter(r, 1, s)) / torch.fft.fft2(r)
+    ratio = torch.fft.fft2(O.fourier_filter(r, 1, s)) / torch.fft.fft2(r)
     m = torch.ones(8, 6, dtype=torch.float64)
     for kh in (0, 7):
         for kw in (0, 5):
@@ -54,15 +54,14 @@ def _inputs():
 
 
 def test_oracle_identities():
-    """All four values 1 is the plain forward up to FFT round-off; no FreeU or any value 0 is the plain forward exactly; the
-    recommended values move it."""
+    """All four values 1 is the plain forward up to FFT round-off; any value 0 is the plain forward exactly; the recommended values
+    move it."""
     w, x, t, ctx, y = _inputs()
     plain = O.unet_forward(TINY, w, x, t, ctx, y)
-    assert torch.equal(FO.unet_forward(TINY, w, x, t, ctx, y), plain)
-    assert torch.equal(FO.unet_forward(TINY, w, x, t, ctx, y, (0.9, 0.0, 1.3, 1.4)), plain)
-    ones = FO.unet_forward(TINY, w, x, t, ctx, y, (1.0, 1.0, 1.0, 1.0))
+    assert torch.equal(O.unet_forward(TINY, w, x, t, ctx, y, O.Attach(freeu=(0.9, 0.0, 1.3, 1.4))), plain)
+    ones = O.unet_forward(TINY, w, x, t, ctx, y, O.Attach(freeu=(1.0, 1.0, 1.0, 1.0)))
     assert float((ones - plain).norm() / plain.norm()) < 1e-6
-    moved = FO.unet_forward(TINY, w, x, t, ctx, y, FO.RECOMMENDED_SDXL)
+    moved = O.unet_forward(TINY, w, x, t, ctx, y, O.Attach(freeu=FO.RECOMMENDED_SDXL))
     assert float((moved - plain).norm() / plain.norm()) > 1e-3
 
 

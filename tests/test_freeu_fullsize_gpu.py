@@ -1,5 +1,5 @@
 """SDXL base (synthetic weights) at 1024x1024 with FreeU at the SDXL values the FreeU authors recommend: one CFG-batched forward against
-the f32 oracle of tests/freeu_oracle.py, with the bound of the 1024^2 forward (test_fullsize_gpu)."""
+the f32 oracle (oracle/unet_oracle.py), with the bound of the 1024^2 forward (test_fullsize_gpu)."""
 import pytest
 import torch
 
@@ -29,7 +29,7 @@ def test_freeu_1024(ctx):
     d.set_freeu(None)
     base = d.unet_forward(x, [749], c, y).cpu()
     d.close()
-    ref = FO.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, FO.RECOMMENDED_SDXL)
+    ref = O.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, O.Attach(freeu=FO.RECOMMENDED_SDXL))
     err, moved = rel_err(got, ref), rel_err(got, base)
     print(f"SDXL FreeU 1024^2: forward rel err {err:.3e}; FreeU moves the forward by {moved:.3e}")
     assert err < TOL and moved > 1e-2

@@ -1,5 +1,5 @@
 """GPU tests of FreeU (sdxl_unet_set_freeu and the OP_FREEU kernel), tiny configs: the kernel against float64, forwards, a CFG sample
-and a refiner refine against the f32 oracle of tests/freeu_oracle.py with the bounds of tests/test_unet_gpu.py, its composition with
+and a refiner refine against the f32 oracle (oracle/unet_oracle.py) with the bounds of tests/test_unet_gpu.py, its composition with
 ControlNets, PAG, image prompts and the inpainting UNet, batch invariance, the bit-exact identities of detach and value 0, the plan
 kept by value-only changes, and the refusals that leave the previous state in effect."""
 import ctypes as C
@@ -13,7 +13,6 @@ from sdxl_b200 import (TINY, TINY_CONTROLNET, TINY_INPAINT, TINY_REFINER, Condit
                        _lib, _testing, pag_layer_mask, synth_weights)
 from sdxl_b200.ip_adapter import synth_ip_adapter
 from oracle import unet_oracle as O
-import controlnet_oracle as CN
 import freeu_oracle as FO
 import ip_adapter_oracle as IPO
 import pag_oracle as PO
@@ -66,7 +65,7 @@ class Setup:
 
     def ref(self, B=2, x=None, **kw):
         x = self.x[:B] if x is None else x
-        return FO.unet_forward(TINY, self.wf, x, torch.tensor([T]), self.c[:B], self.y[:B], FV, **kw)
+        return O.unet_forward(TINY, self.wf, x, torch.tensor([T]), self.c[:B], self.y[:B], O.Attach(freeu=FV, **kw))
 
     def sample(self, B=2):
         return self.d.sample_latent(Conditioning(**cond_kwargs(B)), 7.5, 4, noise=self.noise[:B]).cpu()
@@ -149,25 +148,16 @@ def _wrong_order_forward(S, wcf, hint):
     """The oracle with the filter applied to the skips before the ControlNet residuals are added (the order diffusers does not use)."""
     ts, x, c, y = torch.tensor([T]), S.x[:2], S.c[:2], S.y[:2]
     w = S.wf
-    emb = CN._emb(TINY, w, ts, y)
-    ins, mid, outs = O.unet_blocks(TINY)
-    saved = []
-    h = x
-    for kind, p, nh, d in ins:
-        h = PO._run_block(kind, p, nh, d, h, emb, c, w, (), None)
-        saved.append(h)
-    _, mp, nh, d = mid
-    h = O.res_block(h, emb, w, f"{mp}/res1")
-    h = PO._spatial_transformer(h, c, w, f"{mp}/transformer", nh, d, (), None)
-    h = O.res_block(h, emb, w, f"{mp}/res2")
-    res, r_mid = CN.controlnet_forward(TINY_CONTROLNET, wcf, x, ts, c, y, CN.hint_embedding(TINY_CONTROLNET, wcf, hint))
+    emb = O._emb(TINY, w, ts, y)
+    h, saved = O.encoder(TINY, w, x, emb, c)
+    res, r_mid = O.controlnet_forward(TINY_CONTROLNET, wcf, x, ts, c, y, O.hint_embedding(TINY_CONTROLNET, wcf, hint))
     h = h + 0.8 * r_mid
-    for i, (kind, p, nh, d) in enumerate(outs):
+    for i, (kind, p, nh, d) in enumerate(O.unet_blocks(TINY)[2]):
         skip, r = saved.pop(), res[len(saved)]
         if i // 3 < 2:
-            h, skip = FO.apply_freeu(i // 3, h, skip, FV)
+            h, skip = O.apply_freeu(i // 3, h, skip, FV)
         h = torch.cat([h, skip + 0.8 * r], dim=1)
-        h = PO._run_block(kind, p, nh, d, h, emb, c, w, (), None)
+        h = O._run_block(kind, p, nh, d, h, emb, c, w)
     h = O.group_norm(h, w["norm_out/weight"], w["norm_out/bias"])
     return O.conv2d(O.silu(h), w, "conv_out")
 
@@ -180,7 +170,7 @@ def test_forward_with_pag_vs_oracle(S):
     S.d.set_freeu(None)
     S.d.set_pag(None)
     layers = PO.paths_of_mask(TINY, pag_layer_mask(TINY, "mid"))
-    ref = torch.cat([S.ref(2), FO.unet_forward(TINY, S.wf, S.x[2:], torch.tensor([T]), S.c[2:], S.y[2:], FV, layers)])
+    ref = torch.cat([S.ref(2), O.unet_forward(TINY, S.wf, S.x[2:], torch.tensor([T]), S.c[2:], S.y[2:], O.Attach(freeu=FV, pag_layers=layers))])
     e = rel_err(got, ref)
     print(f"FreeU + PAG (mid): rel err vs oracle {e:.2e}")
     assert e <= FWD_TOL
@@ -197,7 +187,7 @@ def test_forward_with_image_prompt_vs_oracle(S, ctx):
     S.d.set_image_prompt(None)
     ad.close()
     waf = O.to_f32(wa)
-    ref = S.ref(2, ip=(waf, IPO.prompt_tokens(waf, e).expand(2, -1, -1), IPO.uniform_scales(TINY, 0.8)))
+    ref = S.ref(2, prompts=[(waf, IPO.prompt_tokens(waf, e).expand(2, -1, -1), IPO.uniform_scales(TINY, 0.8), None)])
     err = rel_err(got, ref)
     print(f"FreeU + IP-Adapter: rel err vs oracle {err:.2e}")
     assert err <= FWD_TOL
@@ -213,7 +203,7 @@ def test_inpainting_unet_vs_oracle(ctx):
     d.set_freeu(*FV)
     got = d.unet_forward(x, [T], c, y).cpu()
     d.close()
-    ref = FO.unet_forward(TINY_INPAINT, O.to_f32(w), torch.cat([x, cond.expand(2, -1, -1, -1)], 1), torch.tensor([T]), c, y, FV)
+    ref = O.unet_forward(TINY_INPAINT, O.to_f32(w), x, torch.tensor([T]), c, y, O.Attach(concat=cond, freeu=FV))
     e = rel_err(got, ref)
     print(f"FreeU, inpainting UNet: rel err vs oracle {e:.2e}")
     assert e <= FWD_TOL
@@ -228,7 +218,7 @@ def test_refiner_forward_vs_oracle(ctx):
     d.set_freeu(*FV)
     got = d.unet_forward(x, [T], c, y).cpu()
     d.close()
-    e = rel_err(got, FO.unet_forward(TINY_REFINER, O.to_f32(w), x, torch.tensor([T]), c, y, FV))
+    e = rel_err(got, O.unet_forward(TINY_REFINER, O.to_f32(w), x, torch.tensor([T]), c, y, O.Attach(freeu=FV)))
     print(f"FreeU, TINY_REFINER forward: rel err vs oracle {e:.2e}")
     assert e <= FWD_TOL
 
@@ -238,8 +228,8 @@ def test_sample_cfg_vs_oracle(S):
     S.d.set_freeu(*FV)
     got = S.sample()
     S.d.set_freeu(None)
-    ref = FO.diffuse_latent(TINY, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise, O.OracleConditioning(**cond_kwargs()), 0, 4,
-                            7.5, FV)
+    ref = O.sample_latent(TINY, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise, O.OracleConditioning(**cond_kwargs()), 7.5, 4,
+                          att=O.Attach(freeu=FV))
     e, moved = rel_err(got, ref), rel_err(got, S.sample())
     print(f"CFG sample with FreeU: rel err vs oracle {e:.2e}; FreeU moves the latent by {moved:.2e}")
     assert e <= SAMPLE_TOL and moved > 1e-3
@@ -256,8 +246,8 @@ def test_refiner_refine_vs_oracle(ctx):
     d.set_freeu(None)
     plain = d.refine_latent(latent, Conditioning(**c), 7.5, 800, 50, noise=noise).cpu()
     d.close()
-    ref = FO.refine_latent(TINY_REFINER, O.to_f32(w), sdxl_b200.alphas_cumprod(), latent, O.OracleConditioning(**c), 7.5, 800, 50,
-                           noise, FV)
+    ref = O.refine_latent(TINY_REFINER, O.to_f32(w), sdxl_b200.alphas_cumprod(), latent, O.OracleConditioning(**c), 7.5, 800, 50,
+                          noise, att=O.Attach(freeu=FV))
     e = rel_err(got, ref)
     print(f"TINY_REFINER refine with FreeU: rel err vs oracle {e:.2e}; FreeU moves it by {rel_err(got, plain):.2e}")
     assert e <= SAMPLE_TOL and not torch.equal(got, plain)

@@ -6,7 +6,6 @@ import torch
 import sdxl_b200
 from sdxl_b200 import SDXL_INPAINT, Diffuser
 from oracle import unet_oracle as O
-import inpaint_oracle as IO
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -31,7 +30,7 @@ def test_inpaint_unet_1024(ctx):
     got = d.unet_forward(x, [749], c, y)
     d.set_inpaint_condition(None)
     d.close()
-    ref = IO.unet_forward(SDXL_INPAINT, O.to_f32(w), x, torch.tensor([749]), c, y, cond)
+    ref = O.unet_forward(SDXL_INPAINT, O.to_f32(w), x, torch.tensor([749]), c, y, O.Attach(concat=cond))
     err = rel_err(got, ref)
     print(f"SDXL inpainting UNet 1024^2: CFG-batched forward rel err {err:.3e}")
     assert got.shape == (2, 4, 128, 128) and err < TOL

@@ -1,5 +1,5 @@
 """GPU tests of the inpainting UNet (sdxl_unet_set_inpaint_condition and the two-source first conv), tiny configs: the kernel against
-float64, forwards and CFG samples against the f32 oracle of tests/inpaint_oracle.py with the bounds of tests/test_unet_gpu.py, the
+float64, forwards and CFG samples against the f32 oracle (oracle/unet_oracle.py) with the bounds of tests/test_unet_gpu.py, the
 in-place rewrite, every refusal, the diffusers loader and the `sample` flow."""
 import math
 import os
@@ -99,7 +99,7 @@ class Setup:
         return self.d.unet_forward(x, [t], self.c[:x.shape[0]], self.y[:x.shape[0]])
 
     def oracle_fwd(self, cond, t=T):
-        return IO.unet_forward(TINY_INPAINT, self.wf, X, torch.tensor([t]), self.c, self.y, cond)
+        return O.unet_forward(TINY_INPAINT, self.wf, X, torch.tensor([t]), self.c, self.y, O.Attach(concat=cond))
 
 
 @pytest.fixture(scope="module")
@@ -127,8 +127,8 @@ def test_forward_vs_oracle(S, k):
 def test_sample_cfg_vs_oracle(S):
     S.d.set_inpaint_condition(S.cond[1])
     got = S.d.sample_latent(Conditioning(**cond_kwargs(TINY)), 7.5, 4, noise=S.noise)
-    ref = IO.diffuse_latent(TINY_INPAINT, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise,
-                            O.OracleConditioning(**cond_kwargs(TINY)), 4, 7.5, S.cond[1])
+    ref = O.sample_latent(TINY_INPAINT, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise,
+                          O.OracleConditioning(**cond_kwargs(TINY)), 7.5, 4, att=O.Attach(concat=S.cond[1]))
     e = rel_err(got, ref)
     print(f"CFG sample (batch 2, 4 steps) rel err vs oracle {e:.2e}")
     assert got.shape == S.noise.shape and e <= SAMPLE_TOL
@@ -268,7 +268,7 @@ def test_pipeline_sample_vs_oracle_chain(ctx):
     wvf = O.to_f32(wv)
     mask = IO.pixel_mask(32, 32, *crop, True)
     cond = IO.condition(rgb, mask, lambda im: VO.encode_image(TINY_VAE, wvf, im), 4)
-    olat = IO.diffuse_latent(ucfg, O.to_f32(wu), sdxl_b200.alphas_cumprod(), noise, ocond, 4, 5.0, cond)
+    olat = O.sample_latent(ucfg, O.to_f32(wu), sdxl_b200.alphas_cumprod(), noise, ocond, 5.0, 4, att=O.Attach(concat=cond))
     oimg = VO.latent_to_image(TINY_VAE, wvf, olat).numpy().astype("int32")
     # the library's own condition and latent on the same path
     dcond = sdxl_b200.prepare_inpaint_condition(vae, rgb, sdxl_b200.make_inpaint_mask((32, 32), (32, 32), *crop, crop_out=True, n_channels=1))

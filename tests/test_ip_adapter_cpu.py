@@ -1,6 +1,6 @@
 """CPU tests of IP-Adapter support: the h94 key map (flat and nested files, the odd attn2 indices, rejections by name), the
-oracle's decoupled attention against two scaled_dot_product_attention calls, the oracle's identity with unet_oracle without a
-prompt, the embedding-shape checks made before any library call, and a C program against the header."""
+oracle's decoupled attention against two scaled_dot_product_attention calls, the oracle at scale 0 against no prompt, the
+embedding-shape checks made before any library call, and a C program against the header."""
 import ctypes as C
 import os
 import shutil
@@ -108,14 +108,6 @@ def test_oracle_ip_attention_is_two_sdpa_calls(S_ip):
     assert float((got - want).norm() / want.norm()) < 1e-5
 
 
-def test_oracle_without_prompt_is_unet_oracle():
-    w = O.to_f32(synth_weights(TINY, seed=0))
-    x = torch.randn(2, 4, 16, 16, generator=torch.Generator().manual_seed(1))
-    c, y = torch.randn(2, 7, TINY.context_dim), torch.randn(2, TINY.adm_in_channels)
-    t = torch.tensor([499])
-    assert torch.equal(IPO.unet_forward(TINY, w, x, t, c, y), O.unet_forward(TINY, w, x, t, c, y))
-
-
 def test_oracle_zero_scale_is_no_prompt():
     from sdxl_b200.ip_adapter import synth_ip_adapter
     w = O.to_f32(synth_weights(TINY, seed=0))
@@ -124,9 +116,10 @@ def test_oracle_zero_scale_is_no_prompt():
     c, y = torch.randn(1, 7, TINY.context_dim), torch.randn(1, TINY.adm_in_channels)
     tok = IPO.prompt_tokens(wa, torch.randn(1, 2, 16))
     t = torch.tensor([499])
-    base = IPO.unet_forward(TINY, w, x, t, c, y)
-    assert torch.allclose(IPO.unet_forward(TINY, w, x, t, c, y, (wa, tok, IPO.uniform_scales(TINY, 0.0))), base, atol=1e-6)
-    assert not torch.allclose(IPO.unet_forward(TINY, w, x, t, c, y, (wa, tok, IPO.uniform_scales(TINY, 1.0))), base, atol=1e-3)
+    base = O.unet_forward(TINY, w, x, t, c, y)
+    prompt = lambda s: O.Attach(prompts=[(wa, tok, IPO.uniform_scales(TINY, s), None)])  # noqa: E731
+    assert torch.allclose(O.unet_forward(TINY, w, x, t, c, y, prompt(0.0)), base, atol=1e-6)
+    assert not torch.allclose(O.unet_forward(TINY, w, x, t, c, y, prompt(1.0)), base, atol=1e-3)
 
 
 class _NoLibrary:

@@ -35,7 +35,7 @@ def test_ip_adapter_1024(ctx):
     ad.close()
     waf = O.to_f32(wa)
     tok = IPO.prompt_tokens(waf, e).repeat(2, 1, 1)
-    ref = IPO.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, (waf, tok, IPO.uniform_scales(SDXL_BASE, 1.0)))
+    ref = O.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, O.Attach(prompts=[(waf, tok, IPO.uniform_scales(SDXL_BASE, 1.0), None)]))
     err = rel_err(got, ref)
     print(f"SDXL base + IP-Adapter 1024^2 forward: rel err {err:.3e}")
     assert err < TOL

@@ -1,5 +1,5 @@
 """GPU tests of IP-Adapter image prompts (sdxl_unet_set_image_prompt, the two-source attention kernel), tiny configs, against the
-f32 oracle of tests/ip_adapter_oracle.py with the bounds of tests/test_unet_gpu.py, plus the bit-exact identities of attach /
+f32 oracle (oracle/unet_oracle.py) with the bounds of tests/test_unet_gpu.py, plus the bit-exact identities of attach /
 detach / rescale."""
 import dataclasses
 
@@ -57,7 +57,7 @@ class Setup:
 
     def ref(self, e, scales):
         tok = IPO.prompt_tokens(self.waf, e)[torch.arange(2) % e.shape[0]]
-        return IPO.unet_forward(TINY, self.wf, self.x, torch.tensor([T]), self.c, self.y, (self.waf, tok, scales))
+        return O.unet_forward(TINY, self.wf, self.x, torch.tensor([T]), self.c, self.y, O.Attach(prompts=[(self.waf, tok, scales, None)]))
 
 
 @pytest.fixture(scope="module")
@@ -186,7 +186,7 @@ def test_cfg_sample_against_oracle(S, negative):
     finally:
         S.d.set_image_prompt(None)
     c = O.OracleConditioning(**kw)
-    ref = IPO.sample_latent(TINY, S.wf, alphas_cumprod(TINY.n_steps), noise, c, 4, 7.5, (S.waf, e, neg, IPO.uniform_scales(TINY, 0.9)))
+    ref = O.sample_latent(TINY, S.wf, alphas_cumprod(TINY.n_steps), noise, c, 7.5, 4, att=IPO.attach(S.waf, e, neg, IPO.uniform_scales(TINY, 0.9)))
     assert rel_err(out, ref) < SAMPLE_TOL
 
 

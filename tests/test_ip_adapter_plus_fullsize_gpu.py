@@ -37,7 +37,7 @@ def test_ip_adapter_plus_1024(ctx):
     ad.close()
     waf = O.to_f32(wa)
     tok = PO.plus_prompt_tokens(waf, h).repeat(2, 1, 1)
-    ref = IPO.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, (waf, tok, IPO.uniform_scales(SDXL_BASE, 1.0)))
+    ref = O.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, O.Attach(prompts=[(waf, tok, IPO.uniform_scales(SDXL_BASE, 1.0), None)]))
     err = rel_err(got, ref)
     print(f"SDXL base + IP-Adapter Plus 1024^2 forward: rel err {err:.3e}")
     assert err < TOL

@@ -121,7 +121,7 @@ def test_forward_against_oracle(S, nb, ni):
     out = S.fwd()
     S.d.set_image_prompt(None)
     tok = PO.plus_prompt_tokens(S.waf, h)[torch.arange(2) % nb]
-    ref = IPO.unet_forward(TINY, S.wf, S.x, torch.tensor([T]), S.c, S.y, (S.waf, tok, IPO.uniform_scales(TINY, 0.8)))
+    ref = O.unet_forward(TINY, S.wf, S.x, torch.tensor([T]), S.c, S.y, O.Attach(prompts=[(S.waf, tok, IPO.uniform_scales(TINY, 0.8), None)]))
     err = rel_err(out, ref)
     print(f"Plus forward n_batch={nb} n_images={ni}: rel err {err:.3e}")
     assert err < FWD_TOL
@@ -143,7 +143,7 @@ def test_cfg_sample_against_oracle(S):
     finally:
         S.d.set_image_prompt(None)
     c = O.OracleConditioning(**kw)
-    ref = PO.sample_latent(TINY, S.wf, alphas_cumprod(TINY.n_steps), noise, c, 4, 7.5, (S.waf, h, neg, IPO.uniform_scales(TINY, 0.9)))
+    ref = O.sample_latent(TINY, S.wf, alphas_cumprod(TINY.n_steps), noise, c, 7.5, 4, att=PO.attach(S.waf, h, neg, IPO.uniform_scales(TINY, 0.9)))
     err = rel_err(out, ref)
     print(f"Plus 4-step CFG sample: rel err {err:.3e}")
     assert err < SAMPLE_TOL

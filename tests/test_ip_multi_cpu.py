@@ -14,7 +14,7 @@ import torch.nn.functional as F
 from sdxl_b200 import TINY, SdxlError
 from sdxl_b200 import _lib
 from sdxl_b200.ip_adapter import set_image_prompts
-import ip_multi_oracle as MO
+from oracle import unet_oracle as O
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
@@ -26,9 +26,9 @@ def test_downsample_matching_aspect_is_the_level_grid(H, W):
     m = (torch.rand(2, H, W, generator=g) > 0.5).float()
     for l in range(3):
         hl, wl = (H // 8) >> l, (W // 8) >> l
-        assert MO.mask_grid(H, W, hl * wl) == (hl, wl)
+        assert O.mask_grid(H, W, hl * wl) == (hl, wl)
         want = F.interpolate(m[:, None], size=(hl, wl), mode="bicubic", align_corners=False)[:, 0].reshape(2, -1)
-        assert torch.equal(MO.downsample_mask(m, hl * wl), want)
+        assert torch.equal(O.downsample_mask(m, hl * wl), want)
 
 
 def test_downsample_pads_and_truncates():
@@ -36,12 +36,12 @@ def test_downsample_pads_and_truncates():
     4056 values padded with 40 zeros. mw = T // mh never overshoots T, so the cut happens only where mh alone exceeds T: a 64 x 8
     mask against T = 2 gives a 5 x 1 grid, cut to its first 2 values."""
     m = torch.rand(1, 1216, 832, generator=torch.Generator().manual_seed(1))
-    assert MO.mask_grid(1216, 832, 4096) == (78, 52)
-    assert MO.mask_grid(64, 8, 2) == (5, 1)
+    assert O.mask_grid(1216, 832, 4096) == (78, 52)
+    assert O.mask_grid(64, 8, 2) == (5, 1)
     for mask, T in ((m, 4096), (m, 1000), (m, 7), (torch.rand(1, 64, 8, generator=torch.Generator().manual_seed(2)), 2)):
-        mh, mw = MO.mask_grid(mask.shape[1], mask.shape[2], T)
+        mh, mw = O.mask_grid(mask.shape[1], mask.shape[2], T)
         full = F.interpolate(mask[:, None], size=(mh, mw), mode="bicubic", align_corners=False)[:, 0].reshape(1, -1)
-        got = MO.downsample_mask(mask, T)
+        got = O.downsample_mask(mask, T)
         assert got.shape == (1, T)
         n = min(T, mh * mw)
         assert torch.equal(got[:, :n], full[:, :n]) and bool((got[:, n:] == 0).all())
@@ -63,7 +63,7 @@ def test_multi_attention_against_softmax():
             out.append(torch.softmax(q[..., sl] @ k[..., sl].transpose(1, 2) / 8, -1) @ v[..., sl])
         return torch.cat(out, -1)
     want = att(q, k, v) + 0.7 * att(q, *srcs[0][:2]) + 1.3 * srcs[1][3][None, :, None] * att(q, *srcs[1][:2])
-    assert torch.allclose(MO.multi_attention(q, k, v, srcs, n_head), want, atol=1e-5)
+    assert torch.allclose(O.multi_attention(q, k, v, srcs, n_head), want, atol=1e-5)
 
 
 class _NoLibrary:

@@ -1,6 +1,6 @@
 """SDXL base (synthetic weights) with a ViT-H-sized base IP-Adapter and a ViT-H-sized IP-Adapter Plus (synthetic weights), masked to
-the left and right halves of the image: one CFG-batched forward with the prompt set against the f32 oracle of
-tests/ip_multi_oracle.py, with the bound of the 1024^2 forward (test_fullsize_gpu, test_ip_adapter_fullsize_gpu), at 1024 x 1024
+the left and right halves of the image: one CFG-batched forward with the prompt set against the f32 oracle
+(oracle/unet_oracle.py), with the bound of the 1024^2 forward (test_fullsize_gpu, test_ip_adapter_fullsize_gpu), at 1024 x 1024
 and at 832 x 1216."""
 import pytest
 import torch
@@ -11,7 +11,6 @@ from sdxl_b200.ip_adapter import SDXL_PLUS, synth_ip_adapter
 from oracle import unet_oracle as O
 import ip_adapter_oracle as IPO
 import ip_adapter_plus_oracle as PO
-import ip_multi_oracle as MO
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -48,7 +47,7 @@ def test_base_and_plus_masked_halves(ctx, H, W):
     waf, wpf = O.to_f32(wa), O.to_f32(wp)
     prompts = [(waf, IPO.prompt_tokens(waf, e).repeat(2, 1, 1), IPO.uniform_scales(SDXL_BASE, 0.8), left),
                (wpf, PO.plus_prompt_tokens(wpf, h).repeat(2, 1, 1), IPO.uniform_scales(SDXL_BASE, 0.7), right)]
-    ref = MO.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, prompts)
+    ref = O.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, O.Attach(prompts=prompts))
     err = rel_err(got, ref)
     print(f"SDXL base + base and Plus adapters, masked halves, {H}x{W} forward: rel err {err:.3e}")
     assert err < TOL

@@ -1,5 +1,5 @@
 """GPU tests of image-prompt sets (sdxl_unet_set_image_prompts, DESIGN.md §13): the N-source attention kernel and the mask resize
-kernel against float64 / torch, tiny UNet forwards and a CFG sample against tests/ip_multi_oracle.py with the bounds of
+kernel against float64 / torch, tiny UNet forwards and a CFG sample against oracle/unet_oracle.py with the bounds of
 tests/test_ip_adapter_gpu.py, and the bit-exact identities of the one-prompt path, detach, zero scales and in-place rewrites."""
 import numpy as np
 import pytest
@@ -147,7 +147,7 @@ class Setup:
 
     def ref(self, items):
         prompts = [(wa, tok[torch.arange(2) % tok.shape[0]], IPO.uniform_scales(TINY, s), MO.binarize(m)) for wa, tok, s, m in items]
-        return MO.unet_forward(TINY, self.wf, self.x, torch.tensor([T]), self.c, self.y, prompts)
+        return O.unet_forward(TINY, self.wf, self.x, torch.tensor([T]), self.c, self.y, O.Attach(prompts=prompts))
 
 
 @pytest.fixture(scope="module")
@@ -191,9 +191,10 @@ def test_cfg_sample_against_oracle(S):
         out = S.d.sample_latent(Conditioning(**kw), 7.5, 4, noise=noise).cpu()
     finally:
         S.d.set_image_prompts([])
-    prompts = [(S.waf, IPO.prompt_tokens(S.waf, e), IPO.prompt_tokens(S.waf, neg), IPO.uniform_scales(TINY, 0.9), halves(2)),
-               (S.wpf, PO.plus_prompt_tokens(S.wpf, h), PO.plus_prompt_tokens(S.wpf, hn), IPO.uniform_scales(TINY, 0.7), None)]
-    ref = MO.sample_latent(TINY, S.wf, alphas_cumprod(TINY.n_steps), noise, O.OracleConditioning(**kw), 4, 7.5, prompts)
+    att = O.Attach(prompts=[(S.waf, IPO.prompt_tokens(S.waf, e), IPO.uniform_scales(TINY, 0.9), halves(2)),
+                            (S.wpf, PO.plus_prompt_tokens(S.wpf, h), IPO.uniform_scales(TINY, 0.7), None)],
+                   uncond_tokens=[IPO.prompt_tokens(S.waf, neg), PO.plus_prompt_tokens(S.wpf, hn)])
+    ref = O.sample_latent(TINY, S.wf, alphas_cumprod(TINY.n_steps), noise, O.OracleConditioning(**kw), 7.5, 4, att=att)
     err = rel_err(out, ref)
     print(f"4-step CFG sample: rel err {err:.3e}")
     assert err < SAMPLE_TOL

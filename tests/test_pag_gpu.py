@@ -1,5 +1,5 @@
 """GPU tests of perturbed-attention guidance (sdxl_unet_set_pag, the identity self-attention op and the PAG-guided DDIM update), tiny
-configs, against float64 (kernels) and the f32 oracle of tests/pag_oracle.py with the bounds of tests/test_unet_gpu.py, plus the
+configs, against float64 (kernels) and the f32 oracle (oracle/unet_oracle.py) with the bounds of tests/test_unet_gpu.py, plus the
 bit-exact identities of detach and scale 0, the plan kept by scale-only changes, the composition with image prompts and ControlNets,
 and the refusals that leave the previous attachment in effect."""
 import ctypes as C
@@ -151,8 +151,8 @@ def test_forward_with_controlnet_vs_oracle(S, ctx):
     layers = PO.paths_of_mask(TINY, pag_layer_mask(TINY, "mid"))
     ctl = [(TINY_CONTROLNET, O.to_f32(wc), hint, 0.8)]
     ts = torch.tensor([T])
-    ref = torch.cat([PO.unet_forward(TINY, S.wf, S.x[:2], ts, S.c[:2], S.y[:2], controls=ctl),
-                     PO.unet_forward(TINY, S.wf, S.x[2:], ts, S.c[2:], S.y[2:], layers, controls=ctl)])
+    ref = torch.cat([O.unet_forward(TINY, S.wf, S.x[:2], ts, S.c[:2], S.y[:2], O.Attach(controls=ctl)),
+                     O.unet_forward(TINY, S.wf, S.x[2:], ts, S.c[2:], S.y[2:], O.Attach(controls=ctl, pag_layers=layers))])
     assert rel_err(got, ref) <= FWD_TOL
 
 
@@ -165,7 +165,7 @@ def test_sample_cfg_pag_vs_oracle(S, adaptive):
     S.d.set_pag(None)
     alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
     layers = PO.paths_of_mask(TINY, pag_layer_mask(TINY, "mid"))
-    ref = PO.diffuse_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs()), 0, 4, 7.5, layers, 3.0, adaptive)
+    ref = O.sample_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs()), 7.5, 4, att=PO.attach(TINY, layers, 3.0, adaptive))
     e, moved = rel_err(got, ref), rel_err(got, S.sample())
     print(f"CFG + PAG sample (adaptive {adaptive}): rel err vs oracle {e:.2e}; PAG moves the latent by {moved:.2e}")
     assert e <= SAMPLE_TOL and moved > 1e-3
@@ -183,8 +183,8 @@ def test_refiner_refine_with_pag_vs_oracle(ctx):
     plain = d.refine_latent(latent, Conditioning(**c), 7.5, 800, 50, noise=noise).cpu()
     d.close()
     layers = PO.paths_of_mask(TINY_REFINER, pag_layer_mask(TINY_REFINER, ["mid", "up_blocks.1.attentions.2"]))
-    ref = PO.refine_latent(TINY_REFINER, O.to_f32(w), sdxl_b200.alphas_cumprod(), latent, O.OracleConditioning(**c), 800, 50, noise,
-                           layers, 2.0)
+    ref = O.refine_latent(TINY_REFINER, O.to_f32(w), sdxl_b200.alphas_cumprod(), latent, O.OracleConditioning(**c), 7.5, 800, 50, noise,
+                          att=PO.attach(TINY_REFINER, layers, 2.0))
     e = rel_err(got, ref)
     print(f"TINY_REFINER refine with PAG: rel err vs oracle {e:.2e}; PAG moves it by {rel_err(got, plain):.2e}")
     assert e <= SAMPLE_TOL and not torch.equal(got, plain)
@@ -241,8 +241,9 @@ def test_sample_with_image_prompt_vs_oracle(S, ctx):
     ad.close()
     waf = O.to_f32(wa)
     layers = PO.paths_of_mask(TINY, pag_layer_mask(TINY, "mid"))
-    ref = PO.diffuse_latent(TINY, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise, O.OracleConditioning(**cond_kwargs()), 0, 4,
-                            7.5, layers, 3.0, ip=(waf, e, None, IPO.uniform_scales(TINY, 0.8)))
+    ip = IPO.attach(waf, e, None, IPO.uniform_scales(TINY, 0.8))
+    ref = O.sample_latent(TINY, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise, O.OracleConditioning(**cond_kwargs()), 7.5, 4,
+                          att=PO.attach(TINY, layers, 3.0, prompts=ip.prompts, uncond_tokens=ip.uncond_tokens))
     err = rel_err(got, ref)
     print(f"CFG + PAG + IP-Adapter sample: rel err vs oracle {err:.2e}")
     assert err <= SAMPLE_TOL

@@ -1,5 +1,5 @@
 """The scheduled samplers with each kind of attachment, and the `sample()` front end: a scheduled sample on a Karras schedule
-(fractional timesteps) against the oracle chain built from the attachment's own oracle (tests/*_oracle.py) and
+(fractional timesteps) against the oracle chain built from oracle/unet_oracle.py's guided noise with the attachment and
 tests/scheduler_oracle.py; the T2I-Adapter window derived from the schedule; sample(..., sampler=, spacing=, no_cfg=) with and
 without a refiner; Euler against the DDIM kernel on one step; the step kernel's remaining paths."""
 import ctypes as C
@@ -15,9 +15,7 @@ from sdxl_b200.ip_adapter import synth_ip_adapter
 from sdxl_b200.lora import merge_into
 from sdxl_b200.schedulers import Schedule
 from oracle import unet_oracle as O
-import controlnet_oracle as CN
 import freeu_oracle as FO
-import inpaint_oracle as IO
 import ip_adapter_oracle as IPO
 import scheduler_oracle as SO
 import t2i_adapter_oracle as TA
@@ -36,15 +34,9 @@ def S(ctx):
     s.d.close()
 
 
-def cfg_eps(fwd, oc, n=2):
-    """The guided prediction of a forward fwd(x, ts, context, label) that carries the attachment on both branches."""
-    def f(x_in, t):
-        ts = torch.tensor([float(t)], dtype=torch.float32)
-        cond = fwd(x_in.float(), ts, oc.context_full, oc.channel_context, t)
-        unc = fwd(x_in.float(), ts, oc.unconditional_context_full.unsqueeze(0).repeat(n, 1, 1),
-                  oc.unconditional_channel_context.unsqueeze(0).repeat(n, 1), t)
-        return unc + (cond - unc) * G
-    return f
+def guided_eps(cfg, w, oc, att):
+    """The guided noise prediction with the attachment att(t) at timestep t."""
+    return lambda x_in, t: O.forward_diffuser(cfg, w, x_in.float(), torch.tensor([float(t)]), oc, G, att(t))
 
 
 def chain(S, sch, eps, z):
@@ -78,8 +70,8 @@ def test_controlnet(S, ctx, plain):
     finally:
         S.d.set_controls([])
         net.close()
-    ctl = [(TINY_CONTROLNET, O.to_f32(wc), hint, 0.8)]
-    ref = chain(S, SCH, cfg_eps(lambda x, ts, c, y, t: CN.unet_forward(TINY, S.wf, x, ts, c, y, ctl), S.oc), z)
+    att = O.Attach(controls=[(TINY_CONTROLNET, O.to_f32(wc), hint, 0.8)])
+    ref = chain(S, SCH, guided_eps(TINY, S.wf, S.oc, lambda t: att), z)
     check("ControlNet", got, ref, plain)
 
 
@@ -95,9 +87,8 @@ def test_image_prompt(S, ctx, plain):
     finally:
         S.d.set_image_prompt(None)
         ad.close()
-    ip = (O.to_f32(wa), e, None, IPO.uniform_scales(TINY, 0.9))
-    eps = lambda x_in, t: IPO.forward_diffuser(TINY, S.wf, x_in.float(), torch.tensor([float(t)]), S.oc, G, ip)   # noqa: E731
-    check("image prompt", got, chain(S, SCH, eps, z), plain)
+    att = IPO.attach(O.to_f32(wa), e, None, IPO.uniform_scales(TINY, 0.9))
+    check("image prompt", got, chain(S, SCH, guided_eps(TINY, S.wf, S.oc, lambda t: att), z), plain)
 
 
 @pytest.mark.parametrize("spacing, factor", [("karras", 0.25), ("karras", 0.5), ("karras", 1.0), ("leading", 1.0), ("trailing", 0.5)])
@@ -120,11 +111,10 @@ def test_t2i_adapter_window_follows_the_schedule(S, ctx, spacing, factor):
     finally:
         S.d.set_t2i_adapters([])
         ad.close()
-    items = [(TINY_T2I_ADAPTER, O.to_f32(wa), hint, 3.0)]
+    att = O.Attach(t2i=(TA.summed_features([(TINY_T2I_ADAPTER, O.to_f32(wa), hint, 3.0)]), 0))
     first = set(float(v) for v in SO.schedule(spacing, 4, S.a64)[0][:k])
-    fwd = lambda x, ts, c, y, tk: TA.unet_forward(TINY, S.wf, x, ts, c, y, items if float(tk) in first else None)   # noqa: E731
-    ref = chain(S, sch, cfg_eps(fwd, S.oc), z)
-    always = chain(S, sch, cfg_eps(lambda x, ts, c, y, tk: TA.unet_forward(TINY, S.wf, x, ts, c, y, items), S.oc), z) if k < 4 else None
+    ref = chain(S, sch, guided_eps(TINY, S.wf, S.oc, lambda tk: att if float(tk) in first else None), z)
+    always = chain(S, sch, guided_eps(TINY, S.wf, S.oc, lambda tk: att), z) if k < 4 else None
     e = rel_err(got, ref)
     print(f"T2I-Adapter, {spacing}, factor {factor} (t = {np.round(t, 2)}, t_min {t_min}): rel err vs oracle chain {e:.2e}"
           + (f"; vs the chain with the window never closing {rel_err(got, always):.2e}" if always is not None else ""))
@@ -172,7 +162,7 @@ def test_inpainting_unet_condition(S, ctx):
     finally:
         d.close()
     wf = O.to_f32(w)
-    ref = chain(S, SCH, cfg_eps(lambda x, ts, cc, y, t: IO.unet_forward(TINY_INPAINT, wf, x, ts, cc, y, cond), oc), z)
+    ref = chain(S, SCH, guided_eps(TINY_INPAINT, wf, oc, lambda t: O.Attach(concat=cond)), z)
     check("inpainting UNet condition", got, ref, plain)
 
 
@@ -183,8 +173,8 @@ def test_freeu(S, plain):
         got = S.d.sample_latent(S.cond, G, 4, noise=z, schedule=SCH)
     finally:
         S.d.set_freeu(None)
-    eps = lambda x_in, t: FO.forward_diffuser(TINY, S.wf, x_in.float(), torch.tensor([float(t)]), S.oc, G, FO.RECOMMENDED_SDXL)   # noqa: E731
-    check("FreeU", got, chain(S, SCH, eps, z), plain)
+    att = O.Attach(freeu=FO.RECOMMENDED_SDXL)
+    check("FreeU", got, chain(S, SCH, guided_eps(TINY, S.wf, S.oc, lambda t: att), z), plain)
 
 
 def test_merged_lora(S, plain):

@@ -297,7 +297,8 @@ def test_pag_with_adaptive_scale_vs_oracle(S):
         S.d.set_pag(None)
     layers = PO.paths_of_mask(TINY, pag_layer_mask(TINY, "mid"))
     t, sig = SO.schedule("trailing", 4, S.a64)
-    f = lambda x_in, tk: PO.guided_noise(TINY, S.wf, x_in.float(), int(tk), S.oc, 7.5, layers, 3.0, 0.004, None, None)   # noqa: E731
+    att = PO.attach(TINY, layers, 3.0, 0.004)
+    f = lambda x_in, tk: O.forward_diffuser(TINY, S.wf, x_in.float(), torch.tensor([int(tk)], dtype=torch.int32), S.oc, 7.5, att)   # noqa: E731
     ref = SO.sample(f, "euler", t, sig, z * (sig[0] ** 2 + 1) ** 0.5)
     e, moved = rel_err(got, ref), rel_err(got, S.d.sample_latent(S.cond, 7.5, 4, noise=z, schedule=sch))
     print(f"CFG + PAG (adaptive) Euler trailing 4 steps: rel err vs oracle {e:.2e}; PAG moves the latent by {moved:.2e}")

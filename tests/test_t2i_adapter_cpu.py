@@ -132,7 +132,7 @@ def test_oracle_matches_module_structure(in_channels):
 def test_injection_points():
     want = ["input_blocks/3", "input_blocks/5", "input_blocks/8", "middle_block"]
     assert injection_points(SDXL_BASE) == want and injection_points(TINY) == want
-    assert TA.injection_blocks(SDXL_BASE) == want[:3] and TA.injection_blocks(TINY) == want[:3]
+    assert O.injection_blocks(SDXL_BASE) == want[:3] and O.injection_blocks(TINY) == want[:3]
     with pytest.raises(SdxlError, match="refiner"):
         injection_points(SDXL_REFINER)
 

@@ -38,7 +38,8 @@ def test_t2i_adapter_1024(ctx):
     waf = O.to_f32(wa)
     ref_feats = TA.adapter_features(SDXL_T2I_ADAPTER, waf, hint)
     feat_errs = [rel_err(a, b) for a, b in zip(feats, ref_feats)]
-    ref = TA.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, [(SDXL_T2I_ADAPTER, waf, hint, 1.0)])
+    att = O.Attach(t2i=(TA.summed_features([(SDXL_T2I_ADAPTER, waf, hint, 1.0)]), 0))
+    ref = O.unet_forward(SDXL_BASE, O.to_f32(w), x, torch.tensor([749]), c, y, att)
     err, moved = rel_err(got, ref), rel_err(got, base)
     print(f"SDXL T2I-Adapter 1024^2: feature rel errs {['%.3e' % e for e in feat_errs]}; forward rel err {err:.3e}; "
           f"the adapter moves the output by {moved:.3e}")

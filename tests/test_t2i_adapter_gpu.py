@@ -1,5 +1,5 @@
-"""GPU tests of T2I-Adapter conditioning (sdxl_t2i_adapter_load, sdxl_unet_set_t2i_adapters), tiny configs, against the f32 oracle of
-tests/t2i_adapter_oracle.py with the bounds of tests/test_unet_gpu.py, plus the bit-exact identities of detach, scale 0, the timestep
+"""GPU tests of T2I-Adapter conditioning (sdxl_t2i_adapter_load, sdxl_unet_set_t2i_adapters), tiny configs, against the f32 oracle
+(oracle/unet_oracle.py) with the bounds of tests/test_unet_gpu.py, plus the bit-exact identities of detach, scale 0, the timestep
 window and in-place rewrites, and the refusals that leave the previous set attached."""
 import pytest
 import torch
@@ -63,9 +63,9 @@ class Setup:
     def fwd(self, t=T):
         return self.d.unet_forward(X, [t], self.c, self.y)
 
-    def oracle_fwd(self, items, t=T, t_min=0, controls=None):
-        return TA.unet_forward(TINY, self.wf, X, torch.tensor([t]), self.c, self.y,
-                               [(TINY_T2I_ADAPTER, self.waf[i], self.h[j], s) for i, j, s in items], t_min, controls)
+    def oracle_fwd(self, items, t=T, t_min=0, controls=()):
+        feats = TA.summed_features([(TINY_T2I_ADAPTER, self.waf[i], self.h[j], s) for i, j, s in items])
+        return O.unet_forward(TINY, self.wf, X, torch.tensor([t]), self.c, self.y, O.Attach(t2i=(feats, t_min), controls=controls))
 
 
 @pytest.fixture(scope="module")
@@ -136,8 +136,8 @@ def test_sample_cfg_vs_oracle(S, factor):
     got = S.d.sample_latent(Conditioning(**cond_kwargs(TINY)), 7.5, 4, noise=S.noise)
     S.d.set_t2i_adapters([])
     alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
-    ref = TA.diffuse_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs(TINY)), 4, 7.5,
-                            [(TINY_T2I_ADAPTER, S.waf[0], S.h[0], 1.0)], t_min)
+    att = O.Attach(t2i=(TA.summed_features([(TINY_T2I_ADAPTER, S.waf[0], S.h[0], 1.0)]), t_min))
+    ref = O.sample_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs(TINY)), 7.5, 4, att=att)
     assert rel_err(got, ref) <= SAMPLE_TOL
 
 
