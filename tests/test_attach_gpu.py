@@ -1,35 +1,22 @@
 """GPU tests of the UNet's shared attach protocol (csrc/engine.cu: attach_install, attach_detach, attachments_fit) across the five
 kinds of attachment: a detach with nothing attached keeps the plan, and a sampler_begin on a latent an attachment does not fit is
 refused before it touches the conditioning or the plan. The per-kind in-place rewrite and detach identities are in each kind's tests."""
-import numpy as np
 import pytest
 import torch
 
 from sdxl_b200 import (TINY, TINY_CONTROLNET, TINY_INPAINT, TINY_T2I_ADAPTER, Conditioning, ControlNet, Diffuser, IPAdapter, SdxlError,
                        T2IAdapter, synth_weights)
 from sdxl_b200.ip_adapter import synth_ip_adapter
+from harness import arb, h16f, plan_builds
 
 pytestmark = pytest.mark.gpu
 T = 499
 D = 32   # image_embed_dim of the tiny adapter
 
 
-def arb(*dims):
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
-
-
 X = arb(2, 4, 16, 16)   # a 128 x 128 pixel latent
 C_CTX = h16f(arb(2, 7, TINY.context_dim))
 Y = h16f(arb(2, TINY.adm_in_channels))
-
-
-def builds(d):
-    return int(d.ctx.lib.sdxl_unet_plan_builds(d.h))
 
 
 def conditioning(res):
@@ -50,10 +37,10 @@ DETACHES = {
 def test_detach_of_nothing_keeps_the_plan(ctx, kind):
     d = Diffuser(ctx, TINY, synth_weights(TINY, seed=0))
     before = d.unet_forward(X, [T], C_CTX, Y).cpu()
-    n = builds(d)
+    n = plan_builds(d)
     DETACHES[kind](d)
     after = d.unet_forward(X, [T]).cpu()
-    assert builds(d) == n
+    assert plan_builds(d) == n
     assert torch.equal(after, before)
     d.close()
 
@@ -91,11 +78,11 @@ def test_sampler_begin_on_another_latent_is_refused_and_changes_nothing(ctx, cfg
     d = Diffuser(ctx, cfg, synth_weights(cfg, seed=0))
     models = attach(ctx, d)
     before = d.unet_forward(X, [T], C_CTX, Y).cpu()
-    n = builds(d)
+    n = plan_builds(d)
     with pytest.raises(SdxlError, match="latent"):
         d.sampler_begin(conditioning((256, 256)), 7.5)
     after = d.unet_forward(X, [T]).cpu()   # the retained conditioning: the refusal must not have replaced it
-    assert builds(d) == n
+    assert plan_builds(d) == n
     assert torch.equal(after, before)
     d.close()
     for m in models:

@@ -16,16 +16,12 @@ from sdxl_b200 import (TINY, TINY_CLIP, TINY_OPEN_CLIP, SDXL_CLIP_L, SDXL_OPEN_C
 from oracle import clip_oracle as CO
 from oracle import tokenizer_oracle as TO
 from oracle import unet_oracle as O
+from harness import rel_err
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 MINI = os.path.join(GOLD, "mini_bpe")
 TOL = 2e-3
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 @pytest.fixture(scope="module")

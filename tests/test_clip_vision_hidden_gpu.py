@@ -24,7 +24,7 @@ def _golden():
     return GP, np.load(os.path.join(HERE, "golden", "ip_adapter_vision_hidden.npz"))
 
 
-def rel_err(a, b):
+def golden_rel_err(a, b):
     a, b = a.double().cpu(), b.double().cpu()
     return float((a - b).norm() / b.norm())
 
@@ -39,11 +39,11 @@ def test_encode_hidden_against_transformers(ctx, name):
     for idx in GP.hidden_indices(cfg):
         got = enc.encode_hidden(px, idx).cpu()
         assert got.shape == (n, cfg.n_tokens, cfg.n_state)
-        err = rel_err(got.double() @ cols, torch.from_numpy(gold[f"{name}_h{idx}"]))
+        err = golden_rel_err(got.double() @ cols, torch.from_numpy(gold[f"{name}_h{idx}"]))
         print(f"{name} hidden_states[{idx}] (16 projected columns): rel err {err:.3e}")
         assert err < TOL
     if name != "vit_h":
-        err = rel_err(enc.encode_hidden(px), torch.from_numpy(gold[f"{name}_full"]))   # default: hidden_states[-2]
+        err = golden_rel_err(enc.encode_hidden(px), torch.from_numpy(gold[f"{name}_full"]))   # default: hidden_states[-2]
         print(f"{name} hidden_states[-2] (full): rel err {err:.3e}")
         assert err < TOL
     enc.close()

@@ -2,7 +2,6 @@
 (oracle/unet_oracle.py) with the bounds of tests/test_unet_gpu.py, plus the bit-exact identities of attach / detach / rescale."""
 import ctypes as C
 
-import numpy as np
 import pytest
 import torch
 
@@ -10,6 +9,7 @@ import sdxl_b200
 from sdxl_b200 import TINY, TINY_CONTROLNET, Conditioning, ControlNet, ControlNetConfig, Diffuser, SdxlError, UNetConfig, synth_weights
 from sdxl_b200 import _lib
 from oracle import unet_oracle as O
+from harness import arb, h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
@@ -17,28 +17,8 @@ SAMPLE_TOL = 5e-3
 T = 499
 
 
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
-
-
 def hint(n, seed):
     return torch.rand(n, 3, 128, 128, generator=torch.Generator().manual_seed(seed))
-
-
-def cond_kwargs(cfg, B=2, n_ctx=7, res=(128, 128)):
-    return dict(context_full=h16f(arb(B, n_ctx, cfg.context_dim) * 0.9), unconditional_context_full=h16f(arb(n_ctx, cfg.context_dim).cos()),
-                channel_context=h16f(arb(B, cfg.adm_in_channels)), unconditional_channel_context=h16f(arb(cfg.adm_in_channels).cos()),
-                resolution=res)
 
 
 X = arb(2, 4, 16, 16)
@@ -105,21 +85,17 @@ def test_two_controls_vs_oracle(S):
     S.d.set_controls([])
 
 
-def builds(S):
-    return int(S.ctx.lib.sdxl_unet_plan_builds(S.d.h))
-
-
 def test_detach_is_bit_identical(S):
     S.fwd()
-    n = builds(S)
+    n = plan_builds(S.d)
     S.d.set_controls([(S.nets[0], S.h[0], 1.0)])
     controlled = S.fwd()
     assert S.d.plan_num_ops > S.base_ops
-    assert builds(S) == n + 1                 # attaching drops the plan: rebuilt once
+    assert plan_builds(S.d) == n + 1          # attaching drops the plan: rebuilt once
     S.d.set_controls([])
     assert torch.equal(S.fwd(), S.base)
     assert S.d.plan_num_ops == S.base_ops
-    assert builds(S) == n + 2                 # and so does detaching
+    assert plan_builds(S.d) == n + 2          # and so does detaching
     fresh = Diffuser(S.ctx, TINY, S.w)
     assert torch.equal(fresh.unet_forward(X, [T], S.c, S.y), S.base)
     assert fresh.plan_num_ops == S.base_ops
@@ -132,11 +108,11 @@ def test_rescale_in_place_matches_fresh_attach(S):
     S.fwd()
     S.fwd()                                   # plan built and graph captured
     n_ops = S.d.plan_num_ops
-    n_builds = builds(S)
+    n_builds = plan_builds(S.d)
     S.d.set_controls([(S.nets[0], S.h[0], 1.0)])   # same net, n_hint, size: buffers rewritten in place
     rescaled = S.fwd()
     assert S.d.plan_num_ops == n_ops
-    assert builds(S) == n_builds                   # the plan and its graph were kept
+    assert plan_builds(S.d) == n_builds            # the plan and its graph were kept
     S.d.set_controls([])
     S.d.set_controls([(S.nets[0], S.h[0], 1.0)])
     assert torch.equal(S.fwd(), rescaled)
@@ -164,10 +140,10 @@ def test_batch_rows_use_their_own_hint(S):
 
 def test_sample_cfg_vs_oracle(S):
     S.d.set_controls([(S.nets[0], S.h[0], 1.0)])
-    got = S.d.sample_latent(Conditioning(**cond_kwargs(TINY)), 7.5, 4, noise=S.noise)
+    got = S.d.sample_latent(Conditioning(**tiny_conditioning()), 7.5, 4, noise=S.noise)
     S.d.set_controls([])
     alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
-    c = O.OracleConditioning(**cond_kwargs(TINY))
+    c = O.OracleConditioning(**tiny_conditioning())
     ref = O.sample_latent(TINY, S.wf, alphas, S.noise, c, 7.5, 4, att=O.Attach(controls=[(TINY_CONTROLNET, S.wcf[0], S.h[0], 1.0)]))
     assert rel_err(got, ref) <= SAMPLE_TOL
 
@@ -177,7 +153,7 @@ def test_inpainting_with_control(S):
     ref_lat = torch.randn(2, 4, 16, 16, generator=g)
     mask = torch.rand(2, 4, 16, 16, generator=g) > 0.5
     step_noise = torch.randn(4, 2, 4, 16, 16, generator=g)
-    cond = Conditioning(**cond_kwargs(TINY))
+    cond = Conditioning(**tiny_conditioning())
     plain = S.d.sample_latent_with_inpainting(cond, 7.5, 4, ref_lat, mask, init_noise=S.noise, step_noise=step_noise)
     S.d.set_controls([(S.nets[0], S.h[0], 0.0)])   # scale 0 adds exact zeros
     zero = S.d.sample_latent_with_inpainting(cond, 7.5, 4, ref_lat, mask, init_noise=S.noise, step_noise=step_noise)
@@ -186,7 +162,7 @@ def test_inpainting_with_control(S):
     S.d.set_controls([])
     assert torch.equal(zero, plain)
     alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
-    want = O.sample_latent_with_inpainting(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs(TINY)), 7.5, 4, ref_lat, mask,
+    want = O.sample_latent_with_inpainting(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**tiny_conditioning()), 7.5, 4, ref_lat, mask,
                                            list(step_noise), att=O.Attach(controls=[(TINY_CONTROLNET, S.wcf[0], S.h[0], 1.0)]))
     assert rel_err(got, want) <= SAMPLE_TOL and not torch.equal(got, plain)
 

@@ -16,6 +16,7 @@ from oracle import unet_oracle as O
 import freeu_oracle as FO
 import ip_adapter_oracle as IPO
 import pag_oracle as PO
+from harness import h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
@@ -23,28 +24,6 @@ SAMPLE_TOL = 5e-3
 T = 499
 FV = FO.RECOMMENDED_SDXL
 D = 32   # image_embed_dim of the tiny IP-Adapter
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
-
-
-def cond_kwargs(B=2, n_ctx=7, res=(128, 128)):
-    return dict(context_full=h16f(arb(B, n_ctx, 24) * 0.9), context_open_clip=h16f(arb(B, n_ctx, 40) * 0.8),
-                unconditional_context_full=h16f(arb(n_ctx, 24).cos()), unconditional_context_open_clip=h16f(arb(n_ctx, 40).cos()),
-                channel_context=h16f(arb(B, 8)), channel_context_refiner=h16f(arb(B, 16) * 0.5),
-                unconditional_channel_context=h16f(arb(8).cos()), unconditional_channel_context_refiner=h16f(arb(16).cos()),
-                resolution=res)
 
 
 class Setup:
@@ -68,7 +47,7 @@ class Setup:
         return O.unet_forward(TINY, self.wf, x, torch.tensor([T]), self.c[:B], self.y[:B], O.Attach(freeu=FV, **kw))
 
     def sample(self, B=2):
-        return self.d.sample_latent(Conditioning(**cond_kwargs(B)), 7.5, 4, noise=self.noise[:B]).cpu()
+        return self.d.sample_latent(Conditioning(**tiny_conditioning(B, refiner=True)), 7.5, 4, noise=self.noise[:B]).cpu()
 
 
 @pytest.fixture(scope="module")
@@ -77,10 +56,6 @@ def S(ctx):
     yield s
     s.d.set_freeu(None)
     s.d.close()
-
-
-def builds(d):
-    return int(d.ctx.lib.sdxl_unet_plan_builds(d.h))
 
 
 # ---- kernel ------------------------------------------------------------------------------------------------------------------------
@@ -228,7 +203,8 @@ def test_sample_cfg_vs_oracle(S):
     S.d.set_freeu(*FV)
     got = S.sample()
     S.d.set_freeu(None)
-    ref = O.sample_latent(TINY, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise, O.OracleConditioning(**cond_kwargs()), 7.5, 4,
+    ref = O.sample_latent(TINY, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise,
+                          O.OracleConditioning(**tiny_conditioning(refiner=True)), 7.5, 4,
                           att=O.Attach(freeu=FV))
     e, moved = rel_err(got, ref), rel_err(got, S.sample())
     print(f"CFG sample with FreeU: rel err vs oracle {e:.2e}; FreeU moves the latent by {moved:.2e}")
@@ -240,7 +216,7 @@ def test_refiner_refine_vs_oracle(ctx):
     d = Diffuser(ctx, TINY_REFINER, w)
     g = torch.Generator().manual_seed(5)
     latent, noise = torch.randn(2, 4, 8, 16, generator=g), torch.randn(2, 4, 8, 16, generator=g)
-    c = cond_kwargs(2, 6, (64, 128))
+    c = tiny_conditioning(2, 6, (64, 128), refiner=True)
     d.set_freeu(*FV)
     got = d.refine_latent(latent, Conditioning(**c), 7.5, 800, 50, noise=noise).cpu()
     d.set_freeu(None)
@@ -264,7 +240,7 @@ def test_batch_invariance(S):
 
 def test_detach_and_value_zero_are_bit_identical(S, ctx):
     fresh = Diffuser(ctx, TINY, S.w)
-    never = fresh.sample_latent(Conditioning(**cond_kwargs()), 7.5, 4, noise=S.noise).cpu()
+    never = fresh.sample_latent(Conditioning(**tiny_conditioning(refiner=True)), 7.5, 4, noise=S.noise).cpu()
     fresh_fwd = fresh.unet_forward(S.x[:2], [T], S.c[:2], S.y[:2]).cpu()
     fresh_ops = fresh.plan_num_ops
     fresh.close()
@@ -285,12 +261,12 @@ def test_detach_and_value_zero_are_bit_identical(S, ctx):
 def test_value_only_change_keeps_the_plan(S):
     S.d.set_freeu(*FV)
     S.sample()
-    n = builds(S.d)
+    n = plan_builds(S.d)
     results = []
     for v in ((1.1, 0.5, 1.2, 1.1), (0.7, 0.3, 1.5, 1.3), FV):
         S.d.set_freeu(*v)
         results.append(S.sample())
-        assert builds(S.d) == n
+        assert plan_builds(S.d) == n
     assert not torch.equal(results[0], results[2])
     S.d.set_freeu(None)
     S.d.set_freeu(1.1, 0.5, 1.2, 1.1)                         # a fresh attach with the same values computes the same latent
@@ -301,7 +277,7 @@ def test_value_only_change_keeps_the_plan(S):
 def test_refusals_leave_the_previous_state(S):
     S.d.set_freeu(*FV)
     want = S.fwd(2)
-    n = builds(S.d)
+    n = plan_builds(S.d)
     for i, name in enumerate(("s1", "s2", "b1", "b2")):
         for bad in (float("nan"), float("inf"), -float("inf")):
             f = _lib.Freeu()
@@ -312,16 +288,16 @@ def test_refusals_leave_the_previous_state(S):
             f.s1, f.s2, f.b1, f.b2 = v
             assert S.ctx.lib.sdxl_unet_set_freeu(S.d.h, C.byref(f)) != 0
             assert name in S.ctx.lib.sdxl_last_error(S.ctx.h).decode()
-            assert torch.equal(S.fwd(2), want) and builds(S.d) == n
+            assert torch.equal(S.fwd(2), want) and plan_builds(S.d) == n
     with pytest.raises(SdxlError, match="all four values"):
         S.d.set_freeu(0.9, 0.2)
-    assert torch.equal(S.fwd(2), want) and builds(S.d) == n
+    assert torch.equal(S.fwd(2), want) and plan_builds(S.d) == n
     S.d.set_freeu(None)
 
 
 def test_sampler_needs_a_new_begin_after_attach(S):
     """Attaching drops the plan: a step without a new sampler_begin is refused, and a new begin runs with FreeU."""
-    cond = Conditioning(**cond_kwargs())
+    cond = Conditioning(**tiny_conditioning(refiner=True))
     s, keep = cond.to_struct(S.ctx.device)
     lib = S.ctx.lib
     assert lib.sdxl_sampler_begin(S.d.h, C.byref(s), C.c_double(7.5)) == 0

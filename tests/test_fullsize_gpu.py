@@ -12,13 +12,9 @@ import torch
 import sdxl_b200
 from sdxl_b200 import SDXL_BASE, Diffuser
 from oracle import unet_oracle as O
+from harness import rel_err
 
 pytestmark = pytest.mark.gpu
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 @pytest.fixture(scope="module")

@@ -32,7 +32,7 @@ TARGET = 1e-3            # north_star
 RESULTS = {}
 
 
-def rel_err(a, b):
+def golden_rel_err(a, b):
     a, b = a.detach().double().cpu(), torch.as_tensor(b).double()
     return float((a - b).norm() / (b.norm() + 1e-30))
 
@@ -56,7 +56,7 @@ def test_base_forward_1024_vs_golden(base):
     x, ctx_t, y = FC.fwd_1024_inputs()
     out = base.unet_forward(x, [FC.FWD_1024_T], ctx_t, y)
     assert torch.isfinite(out).all()
-    e = rel_err(out, g["out"])
+    e = golden_rel_err(out, g["out"])
     record("base_forward_1024", e, TARGET)
     assert e < TARGET
 
@@ -66,7 +66,7 @@ def test_config1_256_4steps(base, guidance, bound):
     g = np.load(os.path.join(GOLD, "base_config1.npz"))
     c = FC.CONFIG1
     out = base.sample_latent(Conditioning(**FC.base_conditioning(c["res"])), guidance, c["n_steps"], noise=FC.base_noise(c["res"]))
-    e = rel_err(out, g[f"out_cfg{guidance}"])
+    e = golden_rel_err(out, g[f"out_cfg{guidance}"])
     record(f"config1_256_4steps_cfg{guidance}", e, bound)
     assert torch.isfinite(out).all() and e < bound
 
@@ -86,10 +86,10 @@ def test_config2_1024_31iterations(base):
     for it, t in enumerate(ts, start=1):
         base.sampler_step(t, t - step if t >= step else -1)
         if it in c["checkpoints"]:
-            traj[it] = rel_err(base.sampler_get_latent(noise), g[f"it{it}"])
+            traj[it] = golden_rel_err(base.sampler_get_latent(noise), g[f"it{it}"])
     print("config 2 error trajectory (iteration: rel err): " + ", ".join(f"{k}: {v:.2e}" for k, v in traj.items()))
     out = base.sample_latent(cond, c["guidance"], c["n_steps"], noise=noise)
-    e = rel_err(out, g["out"])
+    e = golden_rel_err(out, g["out"])
     RESULTS["config2_trajectory"] = {str(k): v for k, v in traj.items()}
     record("config2_1024_31it_cfg7.5", e, TARGET)   # measured 5.3e-4
     assert torch.isfinite(out).all()
@@ -103,7 +103,7 @@ def test_inpaint_1024_10iterations(base):
     ref, mask, init, step_noise = FC.inpaint_inputs()
     out = base.sample_latent_with_inpainting(Conditioning(**FC.base_conditioning(c["res"])), c["guidance"], c["n_steps"], ref, mask,
                                              init_noise=init, step_noise=step_noise)
-    e = rel_err(out, g["out"])
+    e = golden_rel_err(out, g["out"])
     record("inpaint_1024_10it_cfg7.5", e, 1.5e-3)   # measured 9.8e-4: at the target, bound leaves head-room for box-to-box noise
     assert torch.isfinite(out).all() and e < 1.5e-3
 
@@ -116,7 +116,7 @@ def test_refiner_1024_10iterations(ctx):
     c = FC.REFINER
     lat, noise, cond = FC.refiner_inputs()
     out = d.refine_latent(lat, Conditioning(**cond), c["guidance"], c["step_start"], c["n_steps"], noise=noise)
-    e = rel_err(out, g["out"])
+    e = golden_rel_err(out, g["out"])
     d.close()
     record("refiner_1024_10it", e, TARGET)
     assert torch.isfinite(out).all() and e < TARGET

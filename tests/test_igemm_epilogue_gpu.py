@@ -11,13 +11,9 @@ import pytest
 import torch
 
 from oracle import unet_oracle as O
+from harness import rel_err
 
 pytestmark = pytest.mark.gpu
-
-
-def rel_err(a: torch.Tensor, b: torch.Tensor) -> float:
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 def h16(t: torch.Tensor) -> torch.Tensor:

@@ -6,14 +6,10 @@ import torch
 import sdxl_b200
 from sdxl_b200 import SDXL_INPAINT, Diffuser
 from oracle import unet_oracle as O
+from harness import rel_err
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 def test_inpaint_unet_1024(ctx):

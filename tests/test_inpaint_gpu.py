@@ -19,6 +19,7 @@ from oracle import tokenizer_oracle as TO
 from oracle import unet_oracle as O
 from oracle import vae_oracle as VO
 import inpaint_oracle as IO
+from harness import arb, h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
@@ -28,32 +29,10 @@ U24 = 2.0 ** -24
 MINI = os.path.join(os.path.dirname(__file__), "golden", "mini_bpe")
 
 
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = 1
-    for d in dims:
-        n *= d
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
-
-
 def condition(n, seed, h=16, w=16):
     g = torch.Generator().manual_seed(seed)
     mask = (torch.rand(n, 1, h, w, generator=g) < 0.4).float()
     return torch.cat([mask, torch.randn(n, 4, h, w, generator=g) * (1 - mask)], dim=1)
-
-
-def cond_kwargs(cfg, B=2, n_ctx=7, res=(128, 128)):
-    return dict(context_full=h16f(arb(B, n_ctx, cfg.context_dim) * 0.9), unconditional_context_full=h16f(arb(n_ctx, cfg.context_dim).cos()),
-                channel_context=h16f(arb(B, cfg.adm_in_channels)), unconditional_channel_context=h16f(arb(cfg.adm_in_channels).cos()),
-                resolution=res)
 
 
 X = arb(2, 4, 16, 16)
@@ -110,10 +89,6 @@ def S(ctx):
     s.d.close()
 
 
-def builds(S):
-    return int(S.ctx.lib.sdxl_unet_plan_builds(S.d.h))
-
-
 @pytest.mark.parametrize("k", [0, 1], ids=["n1", "nB"])
 def test_forward_vs_oracle(S, k):
     S.d.set_inpaint_condition(S.cond[k])
@@ -126,9 +101,9 @@ def test_forward_vs_oracle(S, k):
 
 def test_sample_cfg_vs_oracle(S):
     S.d.set_inpaint_condition(S.cond[1])
-    got = S.d.sample_latent(Conditioning(**cond_kwargs(TINY)), 7.5, 4, noise=S.noise)
+    got = S.d.sample_latent(Conditioning(**tiny_conditioning()), 7.5, 4, noise=S.noise)
     ref = O.sample_latent(TINY_INPAINT, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise,
-                          O.OracleConditioning(**cond_kwargs(TINY)), 7.5, 4, att=O.Attach(concat=S.cond[1]))
+                          O.OracleConditioning(**tiny_conditioning()), 7.5, 4, att=O.Attach(concat=S.cond[1]))
     e = rel_err(got, ref)
     print(f"CFG sample (batch 2, 4 steps) rel err vs oracle {e:.2e}")
     assert got.shape == S.noise.shape and e <= SAMPLE_TOL
@@ -138,13 +113,13 @@ def test_rewrite_in_place_matches_fresh_attach(S):
     S.d.set_inpaint_condition(S.cond[1])
     S.fwd()
     S.fwd()                                                 # plan built and graph captured
-    n = builds(S)
+    n = plan_builds(S.d)
     others = [condition(2, 20), condition(2, 21)]
     results = []
     for c in others:
         S.d.set_inpaint_condition(c)                        # same n and size: rewritten in place
         results.append(S.fwd())
-        assert builds(S) == n
+        assert plan_builds(S.d) == n
     assert not torch.equal(results[0], results[1])
     for c, want in zip(others, results):
         S.d.set_inpaint_condition(None)
@@ -152,7 +127,7 @@ def test_rewrite_in_place_matches_fresh_attach(S):
         assert torch.equal(S.fwd(), want)
     S.d.set_inpaint_condition(S.cond[0])                    # a new n: a new plan
     S.fwd()
-    assert builds(S) > n
+    assert plan_builds(S.d) > n
 
 
 def test_batch_rows_use_their_own_condition(S):
@@ -168,10 +143,10 @@ def test_batch_rows_use_their_own_condition(S):
 def test_refusals_leave_the_previous_state(S):
     S.d.set_inpaint_condition(S.cond[1])
     want = S.fwd()
-    n = builds(S)
+    n = plan_builds(S.d)
 
     def unchanged():
-        assert torch.equal(S.fwd(), want) and builds(S) == n
+        assert torch.equal(S.fwd(), want) and plan_builds(S.d) == n
 
     with pytest.raises(SdxlError, match="5 channels"):
         S.d.set_inpaint_condition(condition(2, 3)[:, :4])
@@ -193,9 +168,9 @@ def test_refusals_leave_the_previous_state(S):
     with pytest.raises(SdxlError, match="latent"):
         S.d.unet_forward(arb(2, 4, 8, 8), [T], S.c, S.y)
     with pytest.raises(SdxlError, match="latent"):
-        S.d.sample_latent(Conditioning(**cond_kwargs(TINY, res=(64, 64))), 7.5, 2, noise=S.noise[:, :, :8, :8])
+        S.d.sample_latent(Conditioning(**tiny_conditioning(res=(64, 64))), 7.5, 2, noise=S.noise[:, :, :8, :8])
     with pytest.raises(SdxlError, match="multiple of its n"):
-        S.d.sample_latent(Conditioning(**cond_kwargs(TINY, B=1)), 7.5, 2, noise=S.noise[:1])
+        S.d.sample_latent(Conditioning(**tiny_conditioning(B=1)), 7.5, 2, noise=S.noise[:1])
     unchanged()
     with pytest.raises(SdxlError, match="multiple of its n"):
         S.fwd(X[:1])                                        # (its conditioning, set for batch 1 first, drops the plan)
@@ -205,7 +180,7 @@ def test_refusals_leave_the_previous_state(S):
     with pytest.raises(SdxlError, match="no inpainting condition"):
         S.fwd()
     with pytest.raises(SdxlError, match="no inpainting condition"):
-        S.d.sample_latent(Conditioning(**cond_kwargs(TINY)), 7.5, 2, noise=S.noise)
+        S.d.sample_latent(Conditioning(**tiny_conditioning()), 7.5, 2, noise=S.noise)
     S.d.set_inpaint_condition(S.cond[1])
     assert torch.equal(S.fwd(), want)
 

@@ -3,7 +3,6 @@ f32 oracle (oracle/unet_oracle.py) with the bounds of tests/test_unet_gpu.py, pl
 detach / rescale."""
 import dataclasses
 
-import numpy as np
 import pytest
 import torch
 
@@ -12,6 +11,7 @@ from sdxl_b200 import (TINY, TINY_CONTROLNET, TINY_REFINER, Conditioning, Contro
 from sdxl_b200.ip_adapter import synth_ip_adapter, transformer_block_paths
 from oracle import unet_oracle as O
 import ip_adapter_oracle as IPO
+from harness import arb, h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
@@ -19,20 +19,6 @@ SAMPLE_TOL = 5e-3
 ATTN_TOL = 2e-3
 T = 499
 D = 32   # image_embed_dim of the tiny adapter
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
 
 
 def embeds(nb, ni, seed):
@@ -116,17 +102,16 @@ def test_forward_against_oracle(S, nb, ni):
 
 
 def test_detach_restores_bit_identical(S):
-    builds = lambda: S.ctx.lib.sdxl_unet_plan_builds(S.d.h)  # noqa: E731
     base = S.fwd()
     n_ops = S.d.plan_num_ops
-    n_builds = builds()
+    n_builds = plan_builds(S.d)
     S.d.set_image_prompt(S.ad, embeds(2, 1, 1), 1.0)
     with_ip = S.fwd()
     assert not torch.equal(with_ip, base) and S.d.plan_num_ops == n_ops
-    assert builds() == n_builds + 1         # attaching drops the plan: rebuilt once
+    assert plan_builds(S.d) == n_builds + 1  # attaching drops the plan: rebuilt once
     S.d.set_image_prompt(None)
     assert torch.equal(S.fwd(), base) and S.d.plan_num_ops == n_ops
-    assert builds() == n_builds + 2         # and so does detaching
+    assert plan_builds(S.d) == n_builds + 2  # and so does detaching
 
 
 def test_scale_zero_equals_no_prompt(S):
@@ -139,18 +124,17 @@ def test_scale_zero_equals_no_prompt(S):
 
 def test_in_place_rescale_equals_fresh_attach(S):
     e1, e2 = embeds(2, 2, 3), embeds(2, 2, 4)
-    builds = lambda: S.ctx.lib.sdxl_unet_plan_builds(S.d.h)  # noqa: E731
     S.d.set_image_prompt(S.ad, e1, 0.5)
     S.fwd()
     S.fwd()                                 # the second run captures the CUDA graph
-    n_builds = builds()
+    n_builds = plan_builds(S.d)
     S.d.set_image_prompt(S.ad, e2, 1.3)    # same adapter, n_batch, n_images: buffers rewritten in place
     rewritten = S.fwd()
-    assert builds() == n_builds             # the plan (and its graph) was kept
+    assert plan_builds(S.d) == n_builds     # the plan (and its graph) was kept
     S.d.set_image_prompt(None)
     S.d.set_image_prompt(S.ad, e2, 1.3)
     fresh = S.fwd()
-    assert builds() == n_builds + 1         # a new attachment drops the plan: rebuilt at this forward
+    assert plan_builds(S.d) == n_builds + 1  # a new attachment drops the plan: rebuilt at this forward
     S.d.set_image_prompt(None)
     assert torch.equal(rewritten, fresh)
 
@@ -168,15 +152,9 @@ def test_per_block_scales(S):
         assert rel_err(out, ref) < FWD_TOL
 
 
-def _cond(B=2, n_ctx=7):
-    return dict(context_full=h16f(arb(B, n_ctx, TINY.context_dim) * 0.9), unconditional_context_full=h16f(arb(n_ctx, TINY.context_dim).cos()),
-                channel_context=h16f(arb(B, TINY.adm_in_channels)), unconditional_channel_context=h16f(arb(TINY.adm_in_channels).cos()),
-                resolution=(128, 128))
-
-
 @pytest.mark.parametrize("negative", [False, True])
 def test_cfg_sample_against_oracle(S, negative):
-    kw = _cond()
+    kw = tiny_conditioning()
     noise = torch.randn(2, 4, 16, 16, generator=torch.Generator().manual_seed(0))
     e = embeds(1, 2, 20)
     neg = embeds(1, 2, 21) if negative else None

@@ -3,7 +3,6 @@
 against the oracle with the bounds of tests/test_ip_adapter_gpu.py, and the bit-exact identities of attach / detach / rewrite."""
 import ctypes as C
 
-import numpy as np
 import pytest
 import torch
 
@@ -13,6 +12,7 @@ from sdxl_b200.ip_adapter import ResamplerConfig, synth_ip_adapter
 from oracle import unet_oracle as O
 import ip_adapter_oracle as IPO
 import ip_adapter_plus_oracle as PO
+from harness import arb, h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3      # the UNet forward bound of test_unet_gpu / test_ip_adapter_gpu
@@ -25,20 +25,6 @@ T = 499
 D = 40                                      # width of the tiny image features (a multiple of 8, not of 64)
 L = 19                                      # hidden-state rows per image
 R = ResamplerConfig(depth=2, heads=2, tokens=16)
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
 
 
 def feats(nb, ni, seed):
@@ -87,10 +73,6 @@ class Setup:
     def attach(self, h, scale, neg=None):
         self.d.set_image_prompt(self.ad, h, scale, negative=torch.zeros_like(h) if neg is None else neg)
 
-    def builds(self):
-        return self.ctx.lib.sdxl_unet_plan_builds(self.d.h)
-
-
 @pytest.fixture(scope="module")
 def S(ctx):
     s = Setup(ctx)
@@ -127,14 +109,8 @@ def test_forward_against_oracle(S, nb, ni):
     assert err < FWD_TOL
 
 
-def _cond(B=2, n_ctx=7):
-    return dict(context_full=h16f(arb(B, n_ctx, TINY.context_dim) * 0.9), unconditional_context_full=h16f(arb(n_ctx, TINY.context_dim).cos()),
-                channel_context=h16f(arb(B, TINY.adm_in_channels)), unconditional_channel_context=h16f(arb(TINY.adm_in_channels).cos()),
-                resolution=(128, 128))
-
-
 def test_cfg_sample_against_oracle(S):
-    kw = _cond()
+    kw = tiny_conditioning()
     noise = torch.randn(2, 4, 16, 16, generator=torch.Generator().manual_seed(0))
     h, neg = feats(1, 2, 20), feats(1, 2, 21) * 0.5
     S.attach(h, 0.9, neg)
@@ -166,14 +142,14 @@ def test_in_place_rewrite_equals_fresh_attach(S):
     S.attach(h1, 0.5)
     S.fwd()
     S.fwd()                                 # the second run captures the CUDA graph
-    n_builds = S.builds()
+    n_builds = plan_builds(S.d)
     S.attach(h2, 1.3, h1)                   # same adapter, n_batch, n_images: buffers rewritten in place
     rewritten = S.fwd()
-    assert S.builds() == n_builds           # the plan (and its graph) was kept
+    assert plan_builds(S.d) == n_builds     # the plan (and its graph) was kept
     S.d.set_image_prompt(None)
     S.attach(h2, 1.3, h1)
     fresh = S.fwd()
-    assert S.builds() == n_builds + 1
+    assert plan_builds(S.d) == n_builds + 1
     S.d.set_image_prompt(None)
     assert torch.equal(rewritten, fresh)
 
@@ -183,12 +159,12 @@ def test_switching_between_base_and_plus_rebuilds_the_plan(S):
     h = feats(2, 1, 9)
     S.d.set_image_prompt(S.base, e, 1.0)
     base_out = S.fwd()
-    n_builds = S.builds()
+    n_builds = plan_builds(S.d)
     S.attach(h, 1.0)
     plus_out = S.fwd()
-    assert S.builds() == n_builds + 1 and not torch.equal(plus_out, base_out)
+    assert plan_builds(S.d) == n_builds + 1 and not torch.equal(plus_out, base_out)
     S.d.set_image_prompt(S.base, e, 1.0)
-    assert torch.equal(S.fwd(), base_out) and S.builds() == n_builds + 2
+    assert torch.equal(S.fwd(), base_out) and plan_builds(S.d) == n_builds + 2
     S.d.set_image_prompt(None)
     S.attach(h, 1.0)
     assert torch.equal(S.fwd(), plus_out)
@@ -211,14 +187,14 @@ def test_null_negative_or_bad_seq_len_leaves_state(S):
     h = feats(2, 1, 30)
     S.attach(h, 1.0)
     ref = S.fwd()
-    n_builds = S.builds()
+    n_builds = plan_builds(S.d)
     other = feats(2, 1, 31).contiguous()
     rc, msg = _raw_prompt(S, other, None, L)
     assert rc != 0 and "negative" in msg
     for bad in (0, -3, 5000):
         rc, msg = _raw_prompt(S, other, torch.zeros_like(other), bad)
         assert rc != 0 and "seq_len" in msg
-    assert torch.equal(S.fwd(), ref) and S.builds() == n_builds
+    assert torch.equal(S.fwd(), ref) and plan_builds(S.d) == n_builds
     with pytest.raises(SdxlError, match="negative"):
         S.d.set_image_prompt(S.ad, other, 1.0)
     assert torch.equal(S.fwd(), ref)

@@ -1,7 +1,6 @@
 """GPU tests of image-prompt sets (sdxl_unet_set_image_prompts, DESIGN.md §13): the N-source attention kernel and the mask resize
 kernel against float64 / torch, tiny UNet forwards and a CFG sample against oracle/unet_oracle.py with the bounds of
 tests/test_ip_adapter_gpu.py, and the bit-exact identities of the one-prompt path, detach, zero scales and in-place rewrites."""
-import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
@@ -12,6 +11,7 @@ from oracle import unet_oracle as O
 import ip_adapter_oracle as IPO
 import ip_adapter_plus_oracle as PO
 import ip_multi_oracle as MO
+from harness import arb, h16f, plan_builds, rel_err
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
@@ -20,20 +20,6 @@ T = 499
 D = 32                                  # image_embed_dim of the tiny base adapter
 DP, LP = 40, 19                         # the tiny Plus adapter's feature width and rows
 R = ResamplerConfig(depth=2, heads=2, tokens=16)
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
 
 
 def embeds(nb, ni, seed):
@@ -136,9 +122,6 @@ class Setup:
     def fwd(self, x=None):
         return self.d.unet_forward(self.x if x is None else x, [T], self.c, self.y).cpu()
 
-    def builds(self):
-        return self.ctx.lib.sdxl_unet_plan_builds(self.d.h)
-
     def base_item(self, e, s, mask=None):
         return (self.ad, e, s, None, mask), (self.waf, IPO.prompt_tokens(self.waf, e), s, mask)
 
@@ -221,15 +204,15 @@ def test_rewrite_keeps_plan(S):
     h = feats(1, 1, 42)
     S.d.set_image_prompts([(S.ad, e1, 0.5, None, halves(2)), (S.plus, h, 0.6, torch.zeros_like(h), None)])
     S.fwd()
-    b = S.builds()
+    b = plan_builds(S.d)
     flipped = halves(2).flip(0)
     S.d.set_image_prompts([(S.ad, e2, 1.3, None, flipped), (S.plus, h, 0.2, torch.zeros_like(h), None)])
     out = S.fwd()
-    assert S.builds() == b                                        # same adapters, shapes and mask sizes: rewritten in place
+    assert plan_builds(S.d) == b                                  # same adapters, shapes and mask sizes: rewritten in place
     S.d.set_image_prompts([])
     S.d.set_image_prompts([(S.ad, e2, 1.3, None, flipped), (S.plus, h, 0.2, torch.zeros_like(h), None)])
     assert torch.equal(S.fwd(), out)                              # the rewrite equals a fresh attach
-    assert S.builds() == b + 1
+    assert plan_builds(S.d) == b + 1
     S.d.set_image_prompts([])
 
 

@@ -10,13 +10,9 @@ import sdxl_b200
 from sdxl_b200 import SDXL_BASE, Diffuser
 from sdxl_b200.lora import merge_into
 from lora_cases import layer_paths, make_adapter
+from harness import rel_err
 
 pytestmark = pytest.mark.gpu
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 def test_base_1024_rank32(ctx):

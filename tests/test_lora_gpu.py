@@ -7,7 +7,6 @@ weights computes. The upsample convs are the one documented exception (their 3x3
 and the delta is added after the phase sums were rounded): those are checked against the f32 oracle on host-merged weights
 with the bounds of tests/test_unet_gpu.py.
 """
-import numpy as np
 import pytest
 import torch
 
@@ -19,36 +18,17 @@ from sdxl_b200.pipeline import sample
 from oracle import clip_oracle as CO
 from oracle import unet_oracle as O
 from lora_cases import layer_paths, make_adapter, to_kohya, write_safetensors
+from harness import arb, h16f, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
 SAMPLE_TOL = 5e-3
 
 
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
-
-
 def exact_paths(cfg):
     """Every LoRA-able layer except the upsample convs: fused QKV slices, KV2, GEGLU, FF down, proj_in/out, attention out,
     ResBlock conv_in / conv_out, skip segment, downsample, lin_embed rows, time / label MLPs, first conv, head conv."""
     return [p for p in layer_paths(cfg) if "/upsample/" not in p]
-
-
-def cond_kwargs(cfg, B=2, n_ctx=7, res=(128, 128)):
-    return dict(context_full=h16f(arb(B, n_ctx, cfg.context_dim) * 0.9), unconditional_context_full=h16f(arb(n_ctx, cfg.context_dim).cos()),
-                channel_context=h16f(arb(B, cfg.adm_in_channels)), unconditional_channel_context=h16f(arb(cfg.adm_in_channels).cos()),
-                resolution=res)
 
 
 X = arb(2, 4, 16, 16)
@@ -69,7 +49,7 @@ class Tiny:
         return d.unet_forward(X, [T], self.c, self.y) if set_cond else d.unet_forward(X, [T])
 
     def smp(self, d=None):
-        return (d or self.d).sample_latent(Conditioning(**cond_kwargs(self.cfg)), 7.5, 4, noise=self.noise)
+        return (d or self.d).sample_latent(Conditioning(**tiny_conditioning(cfg=self.cfg)), 7.5, 4, noise=self.noise)
 
     def loaded(self, weights):
         return Diffuser(self.ctx, self.cfg, weights)
@@ -122,7 +102,7 @@ def test_upsample_convs_vs_oracle(tiny):
     print(f"tiny forward with every layer merged vs oracle on merged weights: rel err {e:.3e} (adapter moves it {rel_err(out, t.base_fwd):.3e})")
     assert e < FWD_TOL and rel_err(out, t.base_fwd) > 10 * FWD_TOL
     s = t.smp()
-    sref = O.sample_latent(TINY, wf, sdxl_b200.alphas_cumprod(), t.noise, O.OracleConditioning(**cond_kwargs(TINY)), 7.5, 4)
+    sref = O.sample_latent(TINY, wf, sdxl_b200.alphas_cumprod(), t.noise, O.OracleConditioning(**tiny_conditioning()), 7.5, 4)
     e = rel_err(s, sref)
     print(f"tiny 4-step CFG sample with every layer merged vs oracle: rel err {e:.3e}")
     assert e < SAMPLE_TOL

@@ -17,12 +17,9 @@ from oracle import philox
 from oracle import unet_oracle as O
 from sdxl_b200.config import SDXL_BASE, SDXL_REFINER, TINY
 from sdxl_b200.weights import alphas_cumprod, n_params, synth_weights, unet_tensor_specs
+from harness import arb
 
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
-
-
-def arb(*dims):
-    return torch.sin(torch.arange(int(np.prod(dims)), dtype=torch.float32)).reshape(*dims)
 
 
 def test_group_norm_vs_torch():

@@ -4,7 +4,6 @@ bit-exact identities of detach and scale 0, the plan kept by scale-only changes,
 and the refusals that leave the previous attachment in effect."""
 import ctypes as C
 
-import numpy as np
 import pytest
 import torch
 
@@ -15,34 +14,13 @@ from sdxl_b200.ip_adapter import synth_ip_adapter
 from oracle import unet_oracle as O
 import ip_adapter_oracle as IPO
 import pag_oracle as PO
+from harness import h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
 SAMPLE_TOL = 5e-3
 T = 499
 D = 32   # image_embed_dim of the tiny IP-Adapter
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
-
-
-def cond_kwargs(B=2, n_ctx=7, res=(128, 128)):
-    return dict(context_full=h16f(arb(B, n_ctx, 24) * 0.9), context_open_clip=h16f(arb(B, n_ctx, 40) * 0.8),
-                unconditional_context_full=h16f(arb(n_ctx, 24).cos()), unconditional_context_open_clip=h16f(arb(n_ctx, 40).cos()),
-                channel_context=h16f(arb(B, 8)), channel_context_refiner=h16f(arb(B, 16) * 0.5),
-                unconditional_channel_context=h16f(arb(8).cos()), unconditional_channel_context_refiner=h16f(arb(16).cos()),
-                resolution=res)
 
 
 class Setup:
@@ -61,7 +39,7 @@ class Setup:
         return self.d.unet_forward(self.x, [T], self.c, self.y, perturbed_rows=rows).cpu()
 
     def sample(self, B=2):
-        return self.d.sample_latent(Conditioning(**cond_kwargs(B)), 7.5, 4, noise=self.noise[:B]).cpu()
+        return self.d.sample_latent(Conditioning(**tiny_conditioning(B, refiner=True)), 7.5, 4, noise=self.noise[:B]).cpu()
 
 
 @pytest.fixture(scope="module")
@@ -70,10 +48,6 @@ def S(ctx):
     yield s
     s.d.set_pag(None)
     s.d.close()
-
-
-def builds(d):
-    return int(d.ctx.lib.sdxl_unet_plan_builds(d.h))
 
 
 # ---- kernels -----------------------------------------------------------------------------------------------------------------------
@@ -165,7 +139,8 @@ def test_sample_cfg_pag_vs_oracle(S, adaptive):
     S.d.set_pag(None)
     alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
     layers = PO.paths_of_mask(TINY, pag_layer_mask(TINY, "mid"))
-    ref = O.sample_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs()), 7.5, 4, att=PO.attach(TINY, layers, 3.0, adaptive))
+    ref = O.sample_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**tiny_conditioning(refiner=True)), 7.5, 4,
+                          att=PO.attach(TINY, layers, 3.0, adaptive))
     e, moved = rel_err(got, ref), rel_err(got, S.sample())
     print(f"CFG + PAG sample (adaptive {adaptive}): rel err vs oracle {e:.2e}; PAG moves the latent by {moved:.2e}")
     assert e <= SAMPLE_TOL and moved > 1e-3
@@ -176,7 +151,7 @@ def test_refiner_refine_with_pag_vs_oracle(ctx):
     d = Diffuser(ctx, TINY_REFINER, w)
     g = torch.Generator().manual_seed(5)
     latent, noise = torch.randn(2, 4, 8, 16, generator=g), torch.randn(2, 4, 8, 16, generator=g)
-    c = cond_kwargs(2, 6, (64, 128))
+    c = tiny_conditioning(2, 6, (64, 128), refiner=True)
     d.set_pag(["mid", "up_blocks.1.attentions.2"], 2.0)
     got = d.refine_latent(latent, Conditioning(**c), 7.5, 800, 50, noise=noise).cpu()
     d.set_pag(None)
@@ -193,7 +168,7 @@ def test_refiner_refine_with_pag_vs_oracle(ctx):
 # ---- identities --------------------------------------------------------------------------------------------------------------------
 def test_detach_and_scale_zero_are_bit_identical(S, ctx):
     fresh = Diffuser(ctx, TINY, S.w)
-    never = fresh.sample_latent(Conditioning(**cond_kwargs()), 7.5, 4, noise=S.noise).cpu()
+    never = fresh.sample_latent(Conditioning(**tiny_conditioning(refiner=True)), 7.5, 4, noise=S.noise).cpu()
     fresh_fwd = fresh.unet_forward(S.x, [T], S.c, S.y).cpu()
     fresh_ops = fresh.plan_num_ops
     fresh.close()
@@ -210,20 +185,20 @@ def test_detach_and_scale_zero_are_bit_identical(S, ctx):
 def test_scale_only_change_keeps_the_plan(S):
     S.d.set_pag("mid", 3.0)
     S.sample()
-    n = builds(S.d)
+    n = plan_builds(S.d)
     results = []
     for scale, adaptive in ((1.5, 0.0), (4.0, 0.002), (3.0, 0.0)):
         S.d.set_pag("mid", scale, adaptive)
         results.append(S.sample())
-        assert builds(S.d) == n
+        assert plan_builds(S.d) == n
     assert not torch.equal(results[0], results[2])
     S.d.set_pag(None)
     S.d.set_pag("mid", 1.5)                                   # a fresh attach at the same scale computes the same latent
     assert torch.equal(S.sample(), results[0])
-    n = builds(S.d)
+    n = plan_builds(S.d)
     S.d.set_pag(["down_blocks.1"], 1.5)                       # a new layer set rebuilds the plan
     S.sample()
-    assert builds(S.d) == n + 1
+    assert plan_builds(S.d) == n + 1
     S.d.set_pag(None)
 
 
@@ -242,7 +217,8 @@ def test_sample_with_image_prompt_vs_oracle(S, ctx):
     waf = O.to_f32(wa)
     layers = PO.paths_of_mask(TINY, pag_layer_mask(TINY, "mid"))
     ip = IPO.attach(waf, e, None, IPO.uniform_scales(TINY, 0.8))
-    ref = O.sample_latent(TINY, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise, O.OracleConditioning(**cond_kwargs()), 7.5, 4,
+    ref = O.sample_latent(TINY, S.wf, sdxl_b200.alphas_cumprod(TINY.n_steps), S.noise,
+                          O.OracleConditioning(**tiny_conditioning(refiner=True)), 7.5, 4,
                           att=PO.attach(TINY, layers, 3.0, prompts=ip.prompts, uncond_tokens=ip.uncond_tokens))
     err = rel_err(got, ref)
     print(f"CFG + PAG + IP-Adapter sample: rel err vs oracle {err:.2e}")
@@ -253,10 +229,10 @@ def test_sample_with_image_prompt_vs_oracle(S, ctx):
 def test_refusals_leave_the_previous_attachment(S):
     S.d.set_pag("mid", 2.0)
     want = S.fwd(1)
-    n = builds(S.d)
+    n = plan_builds(S.d)
 
     def unchanged():
-        assert torch.equal(S.d.unet_forward(S.x, [T], S.c, S.y).cpu(), want) and builds(S.d) == n
+        assert torch.equal(S.d.unet_forward(S.x, [T], S.c, S.y).cpu(), want) and plan_builds(S.d) == n
 
     n_sa = int(S.ctx.lib.sdxl_unet_num_self_attentions(S.d.h))
     assert n_sa == 17

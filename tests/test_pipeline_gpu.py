@@ -13,6 +13,7 @@ from oracle import clip_oracle as CO
 from oracle import tokenizer_oracle as TO
 from oracle import unet_oracle as O
 from oracle import vae_oracle as VO
+from harness import rel_err
 
 pytestmark = pytest.mark.gpu
 MINI = os.path.join(os.path.dirname(__file__), "golden", "mini_bpe")
@@ -23,11 +24,6 @@ CLIP_A = TINY_CLIP
 CLIP_B = TINY_OPEN_CLIP
 UNET = UNetConfig(adm_in_channels=CLIP_B.embed_dim + 6 * 256, model_channels=64, channel_mults=(1, 2, 4), transformer_depths=(0, 1, 1),
                   context_dim=CLIP_A.n_state + CLIP_B.n_state)
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 def test_text_to_image_and_inpaint(ctx):

@@ -20,7 +20,8 @@ import ip_adapter_oracle as IPO
 import scheduler_oracle as SO
 import t2i_adapter_oracle as TA
 from lora_cases import layer_paths, make_adapter
-from test_schedulers_gpu import LAT, Setup, cond_kwargs, noises, rel_err  # noqa: F401
+from test_schedulers_gpu import LAT, Setup, noises  # noqa: F401
+from harness import arb, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 SAMPLE_TOL = 5e-3
@@ -153,7 +154,7 @@ def test_inpainting_unet_condition(S, ctx):
     cond = torch.cat([mask, torch.randn(2, 4, 16, 16, generator=g) * (1 - mask)], dim=1)
     other = torch.cat([1 - mask, torch.randn(2, 4, 16, 16, generator=g) * mask], dim=1)
     z = noises(1)[0]
-    c, oc = Conditioning(**cond_kwargs()), O.OracleConditioning(**cond_kwargs())
+    c, oc = Conditioning(**tiny_conditioning(refiner=True)), O.OracleConditioning(**tiny_conditioning(refiner=True))
     try:
         d.set_inpaint_condition(other)
         plain = d.sample_latent(c, G, 4, noise=z, schedule=SCH)
@@ -195,7 +196,7 @@ def test_merged_lora(S, plain):
 class FixedEmbedder:
     """sample() needs text_to_conditioning only; the text encoders have their own tests."""
     def text_to_conditioning(self, prompt, size, crop, ar):
-        return Conditioning(**cond_kwargs(B=1, res=tuple(size)))
+        return Conditioning(**tiny_conditioning(B=1, res=tuple(size), refiner=True))
 
 
 class LatentOut:
@@ -208,7 +209,7 @@ def test_sample_with_a_schedule_and_a_refiner(S, ctx):
     t = 200 with the base latent re-noised to that step's sigma by seed + 1's stream."""
     wr = synth_weights(TINY_REFINER, seed=1)
     refiner = Diffuser(ctx, TINY_REFINER, wr)
-    oc = O.OracleConditioning(**cond_kwargs(B=1))
+    oc = O.OracleConditioning(**tiny_conditioning(B=1, refiner=True))
     z = noises(1, seed=6)[0][:1]
     kw = dict(guidance=G, n_steps=6, resolution=(128, 128), noise=z, seed=3)
     try:
@@ -249,9 +250,11 @@ def test_sample_derives_the_t2i_window_from_the_schedule(S, ctx):
         got = sdxl_b200.sample(FixedEmbedder(), S.d, LatentOut(), "x", guidance=G, n_steps=4, resolution=(128, 128), noise=z,
                                t2i_adapters=[(ad, hint, 1.0)], spacing="leading")
         S.d.set_t2i_adapters([(ad, hint, 1.0)], t_min=0)
-        want = S.d.sample_latent(Conditioning(**cond_kwargs(B=1)), G, 4, noise=z, schedule=Schedule("euler", "leading", 4))
+        want = S.d.sample_latent(Conditioning(**tiny_conditioning(B=1, refiner=True)), G, 4, noise=z,
+                                 schedule=Schedule("euler", "leading", 4))
         S.d.set_t2i_adapters([(ad, hint, 1.0)], t_min=sdxl_b200.t2i_t_min(4, 1.0))   # the DDIM loop's window: cuts t = 1 off
-        cut = S.d.sample_latent(Conditioning(**cond_kwargs(B=1)), G, 4, noise=z, schedule=Schedule("euler", "leading", 4))
+        cut = S.d.sample_latent(Conditioning(**tiny_conditioning(B=1, refiner=True)), G, 4, noise=z,
+                                schedule=Schedule("euler", "leading", 4))
     finally:
         S.d.set_t2i_adapters([])
         ad.close()
@@ -313,7 +316,7 @@ def test_step_kernel_blend_with_eps_rows_and_in_kernel_blend_noise(ctx):
 def test_seeded_inpainting_takes_blend_noise_before_sampler_noise(S):
     """A seeded inpainting run equals the run with sdxl_randn's tensors injected in the documented order."""
     sch = Schedule("euler_ancestral", "trailing", 4)
-    ref, mask = torch.sin(torch.arange(int(np.prod(LAT)), dtype=torch.float32)).reshape(LAT) * 0.5, noises(1, seed=12)[0] > 0.1
+    ref, mask = arb(*LAT) * 0.5, noises(1, seed=12)[0] > 0.1
     seeded = S.d.sample_latent_with_inpainting(S.cond, G, 4, ref, mask, seed=21, schedule=sch)
     k = sch.n_noise(initial=True, inpainting=True)
     assert k == 1 + 4 + 3

@@ -21,7 +21,7 @@ GOLD = os.path.join(os.path.dirname(__file__), "golden", "scheduler_1024.npz")
 BOUND = 2e-3
 
 
-def rel_err(a, b):
+def golden_rel_err(a, b):
     a, b = a.detach().double().cpu(), torch.as_tensor(b).double()
     return float((a - b).norm() / b.norm())
 
@@ -39,7 +39,7 @@ def test_dpmpp_2m_karras_8_steps_cfg(base):
     g = np.load(GOLD)
     cond = Conditioning(**FC.base_conditioning(MG.RES))
     out = base.sample_latent(cond, 7.5, 8, noise=FC.base_noise(MG.RES), schedule=Schedule("dpmpp_2m", "karras", 8))
-    e = rel_err(out, g["dpmpp_2m_karras_8"])
+    e = golden_rel_err(out, g["dpmpp_2m_karras_8"])
     print(f"SDXL base 1024^2, DPM++ 2M Karras, 8 steps, cfg 7.5: rel err vs the oracle chain {e:.3e} (bound {BOUND:.0e})")
     assert bool(torch.isfinite(out).all()) and e <= BOUND
 
@@ -49,6 +49,6 @@ def test_lcm_4_steps_no_cfg(base):
     cond = Conditioning(**FC.base_conditioning(MG.RES))
     out = base.sample_latent(cond, 1.0, 4, noise=FC.base_noise(MG.RES), step_noise=MG.lcm_step_noise(),
                              schedule=Schedule("lcm", "lcm", 4, no_cfg=True))
-    e = rel_err(out, g["lcm_4_no_cfg"])
+    e = golden_rel_err(out, g["lcm_4_no_cfg"])
     print(f"SDXL base 1024^2, LCM, 4 steps, no CFG: rel err vs the oracle chain {e:.3e} (bound {BOUND:.0e})")
     assert bool(torch.isfinite(out).all()) and e <= BOUND

@@ -13,31 +13,11 @@ from sdxl_b200.schedulers import SAMPLERS, Schedule
 from oracle import unet_oracle as O
 import pag_oracle as PO
 import scheduler_oracle as SO
+from harness import arb, h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 SAMPLE_TOL = 5e-3
 LAT = (2, 4, 16, 16)
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    return torch.sin(torch.arange(int(np.prod(dims)), dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
-
-
-def cond_kwargs(B=2, n_ctx=7, res=(128, 128)):
-    return dict(context_full=h16f(arb(B, n_ctx, 24) * 0.9), context_open_clip=h16f(arb(B, n_ctx, 40) * 0.8),
-                unconditional_context_full=h16f(arb(n_ctx, 24).cos()), unconditional_context_open_clip=h16f(arb(n_ctx, 40).cos()),
-                channel_context=h16f(arb(B, 8)), channel_context_refiner=h16f(arb(B, 16) * 0.5),
-                unconditional_channel_context=h16f(arb(8).cos()), unconditional_channel_context_refiner=h16f(arb(16).cos()),
-                resolution=res)
 
 
 def noises(n, seed=0):
@@ -52,8 +32,8 @@ class Setup:
         self.d = Diffuser(ctx, TINY, self.w)
         self.alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
         self.a64 = np.array([O.get_alpha(self.alphas, i) for i in range(TINY.n_steps)])
-        self.cond = Conditioning(**cond_kwargs())
-        self.oc = O.OracleConditioning(**cond_kwargs())
+        self.cond = Conditioning(**tiny_conditioning(refiner=True))
+        self.oc = O.OracleConditioning(**tiny_conditioning(refiner=True))
 
     def eps_fn(self, guidance, no_cfg=False):
         def f(x_in, t):
@@ -81,10 +61,6 @@ def S(ctx):
     s = Setup(ctx)
     yield s
     s.d.close()
-
-
-def builds(d):
-    return int(d.ctx.lib.sdxl_unet_plan_builds(d.h))
 
 
 # ---- kernels -----------------------------------------------------------------------------------------------------------------------
@@ -184,7 +160,7 @@ def test_euler_on_the_reference_spacing_is_sample_latent(S):
     """Ties the whole new path to the reference-derived one: same noise, n dividing 1000 so that both run n steps."""
     z = noises(1)[0]
     ddim = S.d.sample_latent(S.cond, 7.5, 10, noise=z)
-    b0 = builds(S.d)
+    b0 = plan_builds(S.d)
     got = S.d.sample_latent(S.cond, 7.5, 10, noise=z, schedule=Schedule("euler", "reference", 10))
     ref = O.sample_latent(TINY, S.wf, S.alphas, z, S.oc, 7.5, 10)
     e, e_ddim, e_euler = rel_err(got, ddim), rel_err(ddim, ref), rel_err(got, ref)
@@ -192,7 +168,7 @@ def test_euler_on_the_reference_spacing_is_sample_latent(S):
     # the two updates are the same function (tests/test_schedulers_cpu.py, 1e-12) evaluated with different f32 roundings of the state;
     # the f16 activations of ten guided forwards amplify those last bits to the order of either path's own distance to the oracle
     assert e <= 2e-3 and e_euler <= SAMPLE_TOL
-    assert builds(S.d) == b0   # the same plan serves both
+    assert plan_builds(S.d) == b0  # the same plan serves both
 
 
 @pytest.mark.parametrize("sampler", sorted(SAMPLERS))
@@ -212,18 +188,18 @@ def test_no_cfg_runs_the_conditional_rows_alone(S):
     sch = Schedule("euler", "trailing", 4, no_cfg=True)
     z = noises(1)[0]
     S.d.sample_latent(S.cond, 7.5, 4, noise=z, schedule=Schedule("euler", "trailing", 4))
-    b0, l0 = builds(S.d), S.ctx.launch_count
+    b0, l0 = plan_builds(S.d), S.ctx.launch_count
     S.d.sample_latent(S.cond, 7.5, 4, noise=z, schedule=Schedule("dpmpp_2m", "karras", 4))   # sampler and schedule: the plan stays
-    assert builds(S.d) == b0
+    assert plan_builds(S.d) == b0
     cfg_launches = S.ctx.launch_count - l0
     got = S.d.sample_latent(S.cond, 7.5, 4, noise=z, schedule=sch)
-    assert builds(S.d) == b0 + 1   # the batch is the plan's key
-    kw = cond_kwargs()
+    assert plan_builds(S.d) == b0 + 1  # the batch is the plan's key
+    kw = tiny_conditioning(refiner=True)
     kw.update(unconditional_context_full=None, unconditional_channel_context=None, unconditional_context_open_clip=None,
               unconditional_channel_context_refiner=None)
     l1 = S.ctx.launch_count
     bare = S.d.sample_latent(Conditioning(**kw), 123.0, 4, noise=z, schedule=sch)   # no unconditional tensors, guidance ignored
-    assert builds(S.d) == b0 + 1 and torch.equal(got, bare)
+    assert plan_builds(S.d) == b0 + 1 and torch.equal(got, bare)
     assert S.ctx.launch_count - l1 == cfg_launches   # the rows are one batched forward: the same launches on half the rows
     with pytest.raises(SdxlError, match="null"):
         S.d.sample_latent(Conditioning(**kw), 7.5, 4, noise=z, schedule=Schedule("euler", "trailing", 4))

@@ -10,6 +10,7 @@ from sdxl_b200 import (TINY, TINY_CONTROLNET, TINY_T2I_ADAPTER, Conditioning, Co
 from sdxl_b200 import _lib
 from oracle import unet_oracle as O
 import t2i_adapter_oracle as TA
+from harness import arb, h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 FWD_TOL = 2e-3
@@ -17,30 +18,8 @@ SAMPLE_TOL = 5e-3
 T = 499
 
 
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    n = 1
-    for d in dims:
-        n *= d
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
-
-
 def hint(n, seed, c=3, size=128):
     return torch.rand(n, c, size, size, generator=torch.Generator().manual_seed(seed))
-
-
-def cond_kwargs(cfg, B=2, n_ctx=7, res=(128, 128)):
-    return dict(context_full=h16f(arb(B, n_ctx, cfg.context_dim) * 0.9), unconditional_context_full=h16f(arb(n_ctx, cfg.context_dim).cos()),
-                channel_context=h16f(arb(B, cfg.adm_in_channels)), unconditional_channel_context=h16f(arb(cfg.adm_in_channels).cos()),
-                resolution=res)
 
 
 X = arb(2, 4, 16, 16)
@@ -78,10 +57,6 @@ def S(ctx):
     for a in s.ads:
         a.close()
     s.d.close()
-
-
-def builds(S):
-    return int(S.ctx.lib.sdxl_unet_plan_builds(S.d.h))
 
 
 @pytest.mark.parametrize("in_channels, n_hint", [(3, 1), (3, 2), (1, 1), (1, 2)])
@@ -133,11 +108,11 @@ def test_forward_adapter_and_controlnet_vs_oracle(S, ctx):
 def test_sample_cfg_vs_oracle(S, factor):
     t_min = t2i_t_min(4, factor)
     S.d.set_t2i_adapters([(S.ads[0], S.h[0], 1.0)], t_min=t_min)
-    got = S.d.sample_latent(Conditioning(**cond_kwargs(TINY)), 7.5, 4, noise=S.noise)
+    got = S.d.sample_latent(Conditioning(**tiny_conditioning()), 7.5, 4, noise=S.noise)
     S.d.set_t2i_adapters([])
     alphas = sdxl_b200.alphas_cumprod(TINY.n_steps)
     att = O.Attach(t2i=(TA.summed_features([(TINY_T2I_ADAPTER, S.waf[0], S.h[0], 1.0)]), t_min))
-    ref = O.sample_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**cond_kwargs(TINY)), 7.5, 4, att=att)
+    ref = O.sample_latent(TINY, S.wf, alphas, S.noise, O.OracleConditioning(**tiny_conditioning()), 7.5, 4, att=att)
     assert rel_err(got, ref) <= SAMPLE_TOL
 
 
@@ -164,13 +139,13 @@ def test_rewrite_in_place_matches_fresh_attach(S):
     S.d.set_t2i_adapters([(S.ads[0], S.h[0], 0.5)])
     S.fwd()
     S.fwd()                                                 # plan built and graph captured
-    n = builds(S)
+    n = plan_builds(S.d)
     results = []
     for items, t_min in (([(S.ads[0], S.h[0], 1.3)], 0), ([(S.ads[0], S.h[0].flip(3), 1.3)], 0), ([(S.ads[0], S.h[0], 1.3)], T + 1),
                          ([(S.ads[1], S.h[0], 0.7)], 0)):
         S.d.set_t2i_adapters(items, t_min=t_min)            # same n_hint and size: features and t_min rewritten in place
         results.append(S.fwd())
-        assert builds(S) == n
+        assert plan_builds(S.d) == n
     for (items, t_min), want in zip((([(S.ads[0], S.h[0], 1.3)], 0), ([(S.ads[0], S.h[0].flip(3), 1.3)], 0),
                                      ([(S.ads[0], S.h[0], 1.3)], T + 1), ([(S.ads[1], S.h[0], 0.7)], 0)), results):
         S.d.set_t2i_adapters([])
@@ -195,10 +170,10 @@ def test_batch_rows_use_their_own_features(S):
 def test_refusals_leave_the_previous_set(S, ctx):
     S.d.set_t2i_adapters([(S.ads[0], S.h[0], 1.0)])
     want = S.fwd()
-    n = builds(S)
+    n = plan_builds(S.d)
 
     def unchanged():
-        assert torch.equal(S.fwd(), want) and builds(S) == n
+        assert torch.equal(S.fwd(), want) and plan_builds(S.d) == n
 
     with pytest.raises(SdxlError, match="multiples of 32"):
         S.d.set_t2i_adapters([(S.ads[0], hint(2, 1, size=112), 1.0)])
@@ -235,7 +210,7 @@ def test_refusals_leave_the_previous_set(S, ctx):
     with pytest.raises(SdxlError, match="multiple of n_hint"):
         S.d.unet_forward(X[:1], [T], S.c[:1], S.y[:1])
     with pytest.raises(SdxlError, match="multiple of n_hint"):
-        S.d.sample_latent(Conditioning(**cond_kwargs(TINY, B=1)), 7.5, 2, noise=S.noise[:1])
+        S.d.sample_latent(Conditioning(**tiny_conditioning(B=1)), 7.5, 2, noise=S.noise[:1])
     assert torch.equal(S.fwd(), want)
     S.d.set_t2i_adapters([])
 

@@ -18,26 +18,12 @@ import torch
 import sdxl_b200
 from sdxl_b200 import TINY, TINY_REFINER, Conditioning, Diffuser, synth_weights
 from oracle import unet_oracle as O
+from harness import arb, h16f, plan_builds, rel_err, tiny_conditioning
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 FWD_TOL = 2e-3
 SAMPLE_TOL = 5e-3
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
-
-
-def arb(*dims):
-    """arb_tensor(dims) = sin(arange(prod(dims))) — the reference's probe input (src/bin/test/main.rs:51-54)."""
-    n = int(np.prod(dims))
-    return torch.sin(torch.arange(n, dtype=torch.float32)).reshape(*dims)
-
-
-def h16f(t):
-    return t.to(torch.float16).float()
 
 
 @pytest.fixture(scope="module")
@@ -98,20 +84,11 @@ def test_sample_latent_golden(tiny):
     assert e < SAMPLE_TOL
 
 
-def _tiny_cond(cfg, B, n_ctx, res):
-    return dict(
-        context_full=h16f(arb(B, n_ctx, 24) * 0.9), context_open_clip=h16f(arb(B, n_ctx, 40) * 0.8),
-        unconditional_context_full=h16f(arb(n_ctx, 24).cos()), unconditional_context_open_clip=h16f(arb(n_ctx, 40).cos()),
-        channel_context=h16f(arb(B, 8)), channel_context_refiner=h16f(arb(B, 16) * 0.5),
-        unconditional_channel_context=h16f(arb(8).cos()), unconditional_channel_context_refiner=h16f(arb(16).cos()),
-        resolution=res)
-
-
 def test_sample_latent_vs_oracle(tiny):
     """config 1 shape of BASELINE.json at tiny scale: 4 steps (t=999,749,499,249), cfg on (two forwards/step)."""
     d, wf = tiny
     B, n_ctx, res = 2, 7, (128, 128)
-    c = _tiny_cond(TINY, B, n_ctx, res)
+    c = tiny_conditioning(B, n_ctx, res, refiner=True)
     noise = torch.randn(B, 4, 16, 16, generator=torch.Generator().manual_seed(0))
     alphas = sdxl_b200.alphas_cumprod()
     for guidance, n_steps in ((7.5, 4), (1.0, 4), (5.0, 30)):
@@ -136,7 +113,7 @@ def test_iteration_counts():
 def test_inpainting_vs_oracle(tiny):
     d, wf = tiny
     B, n_ctx, res = 1, 5, (128, 128)
-    c = _tiny_cond(TINY, B, n_ctx, res)
+    c = tiny_conditioning(B, n_ctx, res, refiner=True)
     g = torch.Generator().manual_seed(3)
     n_steps = 10
     noise0 = torch.randn(B, 4, 16, 16, generator=g)
@@ -157,7 +134,7 @@ def test_inpainting_vs_oracle(tiny):
 def test_refiner_vs_oracle(tiny_refiner):
     d, wf = tiny_refiner
     B, n_ctx, res = 2, 6, (64, 128)
-    c = _tiny_cond(TINY_REFINER, B, n_ctx, res)
+    c = tiny_conditioning(B, n_ctx, res, refiner=True)
     g = torch.Generator().manual_seed(5)
     latent = torch.randn(B, 4, 8, 16, generator=g)
     noise = torch.randn(B, 4, 8, 16, generator=g)
@@ -171,7 +148,7 @@ def test_refiner_vs_oracle(tiny_refiner):
 
 def test_seeded_sampling_is_deterministic(tiny):
     d, _ = tiny
-    c = _tiny_cond(TINY, 1, 4, (64, 64))
+    c = tiny_conditioning(1, 4, (64, 64), refiner=True)
     a = d.sample_latent(Conditioning(**c), 7.5, 4, seed=42)
     b = d.sample_latent(Conditioning(**c), 7.5, 4, seed=42)
     c2 = d.sample_latent(Conditioning(**c), 7.5, 4, seed=43)
@@ -183,21 +160,20 @@ def test_plan_follows_conditioning_shape(tiny):
     """A same-shape set_conditioning keeps the plan and its CUDA graph and the new values reach it; a new batch or context
     length rebuilds the plan once."""
     d, _ = tiny
-    builds = lambda: int(d.ctx.lib.sdxl_unet_plan_builds(d.h))  # noqa: E731
     x = arb(2, 4, 16, 16)
     c, y = h16f(arb(2, 7, TINY.context_dim)), h16f(arb(2, TINY.adm_in_channels))
     d.unet_forward(x, [499], c, y)
     d.unet_forward(x, [499])                     # the second run captures the CUDA graph
-    n = builds()
+    n = plan_builds(d)
     kept = d.unet_forward(x, [499], h16f(c * 0.5), y)
-    assert builds() == n
+    assert plan_builds(d) == n
     d.unet_forward(x, [499], h16f(arb(2, 9, TINY.context_dim)), y)   # new n_ctx
-    assert builds() == n + 1
+    assert plan_builds(d) == n + 1
     d.unet_forward(x[:1], [499], c[:1], y[:1])   # new batch
     d.unet_forward(x[:1], [499])
-    assert builds() == n + 2
+    assert plan_builds(d) == n + 2
     assert torch.equal(d.unet_forward(x, [499], h16f(c * 0.5), y), kept)   # rebuilt for batch 2: same result as the kept plan
-    assert builds() == n + 3
+    assert plan_builds(d) == n + 3
 
 
 def test_error_paths(ctx, tiny):

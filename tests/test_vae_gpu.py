@@ -18,15 +18,11 @@ import torch
 from sdxl_b200 import SDXL_VAE, TINY_VAE, LatentDecoder, synth_weights
 from oracle import unet_oracle as O
 from oracle import vae_oracle as VO
+from harness import rel_err
 
 pytestmark = pytest.mark.gpu
 GOLD = os.path.join(os.path.dirname(__file__), "golden")
 TOL = 2e-3
-
-
-def rel_err(a, b):
-    a, b = a.detach().double().cpu(), b.detach().double().cpu()
-    return float((a - b).norm() / (b.norm() + 1e-30))
 
 
 @pytest.fixture(scope="module")

@@ -15,37 +15,26 @@ projection or Resampler for the prompt and its negative, K/V hoist of the 70 cro
 (plan rebuilt at the next step) and for an in-place rewrite. The card's name, power limit and clocks are read in the same run.
 """
 import json
-import os
-import statistics
-import sys
-import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for p in (ROOT, os.path.join(ROOT, "stable-diffusion-xl-burn_b200"), os.path.join(ROOT, "tools")):
-    sys.path.insert(0, p)
+import stepbench as sb
+import torch
+import sdxl_b200
+from sdxl_b200 import build_pack
+from sdxl_b200.clip_vision import SDXL_VIT_BIGG, SDXL_VIT_H, ClipVisionEncoder, synth_vision_weights
+from sdxl_b200.ip_adapter import SDXL_PLUS, synth_ip_adapter
 
-import torch  # noqa: E402
-import sdxl_b200  # noqa: E402
-from sdxl_b200 import build_pack  # noqa: E402
-from sdxl_b200.clip_vision import SDXL_VIT_BIGG, SDXL_VIT_H, ClipVisionEncoder, synth_vision_weights  # noqa: E402
-from sdxl_b200.ip_adapter import SDXL_PLUS, synth_ip_adapter  # noqa: E402
-from controlnet_bench import gpu_info  # noqa: E402
-
-HW = 1024
+HW = sb.HW
 D = 1024   # ViT-H/14 image_embeds
 D_PLUS = 1280   # ViT-H/14 hidden width
 L_PLUS = 257    # ViT-H/14 tokens per image
 
 
 def main():
-    args = sys.argv[1:]
-    opt = lambda name, d: type(d)(args[args.index(name) + 1]) if name in args else d  # noqa: E731
-    steps, warmup, reps = opt("--steps", 31), opt("--warmup", 4), opt("--reps", 3)
-    out_path = args[0] if args and not args[0].startswith("--") else None
+    out_path, steps, warmup, reps = sb.options(steps=31, warmup=4, reps=3)
     ctx = sdxl_b200.Context(0)
     dev = str(ctx.device)
-    res = {"gpu": gpu_info()}
-    d = sdxl_b200.Diffuser(ctx, sdxl_b200.SDXL_BASE, sdxl_b200.build_pack(sdxl_b200.synth_weights(sdxl_b200.SDXL_BASE, seed=0, device=dev)))
+    res = {"gpu": sb.gpu_info()}
+    d = sb.load_unet(ctx)
     ad = sdxl_b200.IPAdapter(ctx, sdxl_b200.SDXL_BASE, D, synth_ip_adapter(sdxl_b200.SDXL_BASE, D, seed=1))
     plus = sdxl_b200.IPAdapter(ctx, sdxl_b200.SDXL_BASE, D_PLUS, synth_ip_adapter(sdxl_b200.SDXL_BASE, D_PLUS, seed=1, resampler=SDXL_PLUS))
     torch.cuda.empty_cache()
@@ -57,12 +46,7 @@ def main():
     left = torch.zeros(1, HW, HW)
     left[:, :, :HW // 2] = 1
     emb2 = torch.randn(1, 2, D, generator=g(40))
-    cond = sdxl_b200.Conditioning(
-        context_full=torch.randn(1, 77, 2048, generator=g(1)).half(), unconditional_context_full=torch.randn(77, 2048, generator=g(2)).half(),
-        channel_context=torch.randn(1, 2816, generator=g(3)).half(), unconditional_channel_context=torch.randn(2816, generator=g(4)).half(),
-        resolution=(HW, HW))
-    ts = sdxl_b200.ddim_timesteps(30)
-    step_size = 1000 // 30
+    cond = sb.conditioning()
 
     def prompt(kind, scale=1.0):
         if kind == "none":
@@ -82,64 +66,37 @@ def main():
         prompt(kind)
         d.sampler_begin(cond, 7.5)
 
-    def run_steps():
-        d.sampler_set_latent(ctx.randn(4 * (HW // 8) ** 2, seed=0).reshape(1, 4, HW // 8, HW // 8))
-        for i in range(warmup):
-            t = ts[i % len(ts)]
-            d.sampler_step(t, t - step_size if t >= step_size else -1)
-        ctx.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(ctx.stream)
-        for i in range(steps):
-            t = ts[i % len(ts)]
-            d.sampler_step(t, t - step_size if t >= step_size else -1)
-        e1.record(ctx.stream)
-        ctx.synchronize()
-        return e0.elapsed_time(e1) / steps
+    def run(k):
+        attach(k)
+        return sb.run_steps(ctx, d, steps, warmup)
 
-    step = {k: [] for k in kinds}
-    for r in range(reps):
-        for k in kinds[r % len(kinds):] + kinds[:r % len(kinds)]:
-            attach(k)
-            step[k].append(round(run_steps(), 3))
-    res["step_ms"] = {k: {"median": statistics.median(v), "runs": v} for k, v in step.items()}
+    res["step_ms"] = sb.step_rounds(kinds, reps, run)
     b = res["step_ms"]["none"]["median"]
     res["step_ratio_vs_base"] = {k: round(v["median"] / b, 3) for k, v in res["step_ms"].items()}
-    res["gpu_after_steps"] = gpu_info()
+    res["gpu_after_steps"] = sb.gpu_info()
     print(json.dumps(res["step_ms"]), flush=True)
 
     res["attention"] = {}
     for k in kinds:
         attach(k)
-        run_steps()
+        sb.run_steps(ctx, d, steps, warmup)
         prof = d.profile_plan()
         total = sum(v["ms"] for v in prof.values())
         a = prof.get("attention_wgmma", {"ms": 0.0, "launches": 0})
         res["attention"][k] = {"attention_ms": round(a["ms"], 3), "launches": a["launches"], "step_ms_eager": round(total, 3),
                                            "share": round(a["ms"] / total, 4), "plan_flops": d.plan_flops}
 
-    def timed(fn, before=lambda: None):
-        ts_ = []
-        for _ in range(reps):
-            before()
-            ctx.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            ctx.synchronize()
-            ts_.append((time.perf_counter() - t0) * 1e3)
-        return round(statistics.median(ts_), 2)
-
     attach("none")
     res["set_image_prompt_ms"] = {
-        "attach_one_image": timed(lambda: prompt("base_1"), before=lambda: prompt("none")),
-        "rescale_in_place": timed(lambda: prompt("base_1", 0.6)),
-        "plus_attach_one_image": timed(lambda: prompt("plus_1"), before=lambda: prompt("none")),
-        "plus_in_place_one_image": timed(lambda: prompt("plus_1", 0.6)),
-        "plus_attach_four_images": timed(lambda: prompt("plus_4"), before=lambda: prompt("none")),
+        "attach_one_image": sb.timed(ctx, reps, lambda: prompt("base_1"), before=lambda: prompt("none")),
+        "rescale_in_place": sb.timed(ctx, reps, lambda: prompt("base_1", 0.6)),
+        "plus_attach_one_image": sb.timed(ctx, reps, lambda: prompt("plus_1"), before=lambda: prompt("none")),
+        "plus_in_place_one_image": sb.timed(ctx, reps, lambda: prompt("plus_1", 0.6)),
+        "plus_attach_four_images": sb.timed(ctx, reps, lambda: prompt("plus_4"), before=lambda: prompt("none")),
     }
     res["set_image_prompts_ms"] = {
-        "attach_base_plus_masked": timed(lambda: prompt("base_plus_masked"), before=lambda: prompt("none")),
-        "rewrite_base_plus_masked": timed(lambda: prompt("base_plus_masked", 0.6)),
+        "attach_base_plus_masked": sb.timed(ctx, reps, lambda: prompt("base_plus_masked"), before=lambda: prompt("none")),
+        "rewrite_base_plus_masked": sb.timed(ctx, reps, lambda: prompt("base_plus_masked", 0.6)),
     }
     d.set_image_prompt(None)
     res["encode_ms_per_image"] = {}
@@ -168,11 +125,8 @@ def main():
             res["encode_ms_per_image"]["vit_h_hidden"] = round(e0.elapsed_time(e1) / 40, 3)
         enc.close()
         torch.cuda.empty_cache()
-    res["gpu_after"] = gpu_info()
-    print(json.dumps(res))
-    if out_path:
-        with open(out_path, "w") as f:
-            json.dump(res, f, indent=1)
+    res["gpu_after"] = sb.gpu_info()
+    sb.report(res, out_path)
     ad.close()
     plus.close()
     d.close()

@@ -10,33 +10,15 @@ layer set of a kohya SDXL LoRA). For each rank, host wall clock around a call th
   restore_ms            n = 0: restore every layer and free the backups
 plus the re-apply timed with CUDA events alone and the merge's FLOP count (merge_tflops_lower_bound divides it by the whole
 re-apply, restore copies included). The step time uses bench.py's method (sampler_begin, W warm-up steps, CUDA events around K sampler steps,
-CFG 7.5 at 1024^2, batch 1), base and rank-32-merged alternated R times in one process.
+CFG 7.5 at 1024^2, batch 1), base and rank-32-merged alternating over R rounds in one process.
 """
-import json
-import os
 import statistics
-import subprocess
-import sys
 import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for p in (ROOT, os.path.join(ROOT, "stable-diffusion-xl-burn_b200")):
-    sys.path.insert(0, p)
-
-import torch  # noqa: E402
-import sdxl_b200  # noqa: E402
-from sdxl_b200.lora import unet_lora_modules  # noqa: E402
-
-HW = 1024
-
-
-def gpu_info():
-    try:
-        q = "name,power.limit,clocks.max.sm,clocks.sm"
-        return subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                              text=True, timeout=30).stdout.strip()
-    except Exception as e:  # noqa: BLE001
-        return f"nvidia-smi unavailable: {e}"
+import stepbench as sb
+import torch
+import sdxl_b200
+from sdxl_b200.lora import unet_lora_modules
 
 
 def adapter(cfg, paths, rank, dev, seed):
@@ -63,19 +45,16 @@ def timed(ctx, fn, reps):
 
 
 def main():
-    args = sys.argv[1:]
-    opt = lambda name, d: int(args[args.index(name) + 1]) if name in args else d  # noqa: E731
-    steps, warmup, reps = opt("--steps", 31), opt("--warmup", 4), opt("--reps", 3)
-    out_path = args[0] if args and not args[0].startswith("--") else None
+    out_path, steps, warmup, reps = sb.options(steps=31, warmup=4, reps=3)
     ctx = sdxl_b200.Context(0)
     dev = ctx.device
     cfg = sdxl_b200.SDXL_BASE
-    d = sdxl_b200.Diffuser(ctx, cfg, sdxl_b200.build_pack(sdxl_b200.synth_weights(cfg, seed=0, device=str(dev))))
+    d = sb.load_unet(ctx, cfg)
     torch.cuda.empty_cache()
     paths = [r for _, r, _ in unet_lora_modules(cfg) if "/transformer" in r]
     shapes = {n[: -len("/weight")]: s for n, s, _, _ in sdxl_b200.unet_tensor_specs(cfg) if n.endswith("/weight")}
     touched_bytes = sum(shapes[p][0] * shapes[p][1] * 2 for p in paths)
-    res = {"gpu": gpu_info(), "layers": len(paths), "touched_weight_bytes": touched_bytes, "ranks": {}}
+    res = {"gpu": sb.gpu_info(), "layers": len(paths), "touched_weight_bytes": touched_bytes, "ranks": {}}
 
     for rank in (8, 32, 128):
         pack, flops = adapter(cfg, paths, rank, dev, seed=rank)
@@ -107,44 +86,17 @@ def main():
         del pack
 
     # ---- step time, bench.py's method: base and rank-32-merged alternated
-    g = lambda s: torch.Generator().manual_seed(s)  # noqa: E731
-    cond = sdxl_b200.Conditioning(
-        context_full=torch.randn(1, 77, 2048, generator=g(1)).half(), unconditional_context_full=torch.randn(77, 2048, generator=g(2)).half(),
-        channel_context=torch.randn(1, 2816, generator=g(3)).half(), unconditional_channel_context=torch.randn(2816, generator=g(4)).half(),
-        resolution=(HW, HW))
-    d.sampler_begin(cond, 7.5)
-    ts = sdxl_b200.ddim_timesteps(30)
-    step_size = 1000 // 30
+    d.sampler_begin(sb.conditioning(), 7.5)
     pack32, _ = adapter(cfg, paths, 32, dev, seed=32)
 
-    def run_steps():
-        d.sampler_set_latent(ctx.randn(4 * (HW // 8) ** 2, seed=0).reshape(1, 4, HW // 8, HW // 8))
-        for i in range(warmup):
-            t = ts[i % len(ts)]
-            d.sampler_step(t, t - step_size if t >= step_size else -1)
-        ctx.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(ctx.stream)
-        for i in range(steps):
-            t = ts[i % len(ts)]
-            d.sampler_step(t, t - step_size if t >= step_size else -1)
-        e1.record(ctx.stream)
-        ctx.synchronize()
-        return e0.elapsed_time(e1) / steps
+    def run(name):
+        d.set_adapters([] if name == "base" else [(pack32, 1.0)])
+        return sb.run_steps(ctx, d, steps, warmup)
 
-    step = {"base": [], "rank32": []}
-    for _ in range(reps):
-        d.set_adapters([])
-        step["base"].append(round(run_steps(), 3))
-        d.set_adapters([(pack32, 1.0)])
-        step["rank32"].append(round(run_steps(), 3))
+    res["step_ms"] = sb.step_rounds(["base", "rank32"], reps, run)
     d.set_adapters([])
-    res["step_ms"] = {k: {"median": statistics.median(v), "runs": v} for k, v in step.items()}
-    res["gpu_after"] = gpu_info()
-    print(json.dumps(res))
-    if out_path:
-        with open(out_path, "w") as f:
-            json.dump(res, f, indent=1)
+    res["gpu_after"] = sb.gpu_info()
+    sb.report(res, out_path)
     d.close()
     ctx.close()
 

@@ -12,49 +12,27 @@ configuration warmed once and then run R times in rotating order in one process:
   (c) the step kernel alone: CUDA events around 200 launches at the 1024^2 latent, CFG rows, in-kernel noise.
 Also the card's name, power limit and clocks read in the same run. Fails without a GPU. Synthetic weights: times only, the latents
 say nothing about image quality."""
-import json
-import os
 import statistics
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for p in (ROOT, os.path.join(ROOT, "stable-diffusion-xl-burn_b200")):
-    sys.path.insert(0, p)
+import stepbench as sb
+import torch
+import sdxl_b200
+from sdxl_b200 import _testing
+from sdxl_b200.schedulers import Schedule
 
-import torch  # noqa: E402
-import sdxl_b200  # noqa: E402
-from sdxl_b200 import _testing  # noqa: E402
-from sdxl_b200.schedulers import Schedule  # noqa: E402
-
-HW = 1024
-
-
-def gpu_info():
-    try:
-        q = "name,power.limit,clocks.max.sm,clocks.sm"
-        return subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                              text=True, timeout=30).stdout.strip()
-    except Exception as e:  # noqa: BLE001
-        return f"nvidia-smi unavailable: {e}"
+HW = sb.HW
 
 
 def main():
-    args = sys.argv[1:]
-    opt = lambda name, d: type(d)(args[args.index(name) + 1]) if name in args else d  # noqa: E731
-    n, reps = opt("--steps", 10), max(opt("--reps", 3), 3)
-    out_path = args[0] if args and not args[0].startswith("--") else None
+    out_path, n, reps = sb.options(steps=10, reps=3)
+    reps = max(reps, 3)
     if not torch.cuda.is_available():
         raise SystemExit("sampler_bench: no CUDA device; there is nothing to measure without one")
     ctx = sdxl_b200.Context(0)
     dev = str(ctx.device)
-    res = {"gpu": gpu_info(), "resolution": HW, "steps": n, "reps": reps}
-    d = sdxl_b200.Diffuser(ctx, sdxl_b200.SDXL_BASE, sdxl_b200.build_pack(sdxl_b200.synth_weights(sdxl_b200.SDXL_BASE, seed=0, device=dev)))
-    g = lambda s: torch.Generator().manual_seed(s)  # noqa: E731
-    cond = sdxl_b200.Conditioning(
-        context_full=torch.randn(1, 77, 2048, generator=g(1)).half(), unconditional_context_full=torch.randn(77, 2048, generator=g(2)).half(),
-        channel_context=torch.randn(1, 2816, generator=g(3)).half(), unconditional_channel_context=torch.randn(2816, generator=g(4)).half(),
-        resolution=(HW, HW))
+    res = {"gpu": sb.gpu_info(), "resolution": HW, "steps": n, "reps": reps}
+    d = sb.load_unet(ctx)
+    cond = sb.conditioning()
 
     def timed(schedule, steps):
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
@@ -105,11 +83,7 @@ def main():
         res.setdefault("step_kernel_us", {})[name] = e0.elapsed_time(e1) / 200 * 1e3
     d.close()
     ctx.close()
-    print(json.dumps(res, indent=1))
-    if out_path:
-        os.makedirs(os.path.dirname(os.path.abspath(out_path)), exist_ok=True)
-        with open(out_path, "w") as fh:
-            json.dump(res, fh, indent=1)
+    sb.report(res, out_path)
 
 
 if __name__ == "__main__":

@@ -12,29 +12,13 @@ hint (the forward plus the NHWC -> NCHW copies of its outputs), median of R, and
 profile of one step with one adapter and the card's name, power limit and clocks read in the same run.
 """
 import json
-import os
 import statistics
-import subprocess
-import sys
-import time
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-for p in (ROOT, os.path.join(ROOT, "stable-diffusion-xl-burn_b200")):
-    sys.path.insert(0, p)
+import stepbench as sb
+import torch
+import sdxl_b200
 
-import torch  # noqa: E402
-import sdxl_b200  # noqa: E402
-
-HW = 1024
-
-
-def gpu_info():
-    try:
-        q = "name,power.limit,clocks.max.sm,clocks.sm"
-        return subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader", "-i", "0"], capture_output=True,
-                              text=True, timeout=30).stdout.strip()
-    except Exception as e:  # noqa: BLE001
-        return f"nvidia-smi unavailable: {e}"
+HW = sb.HW
 
 
 def adapter_flops(cfg, H, W):
@@ -51,72 +35,37 @@ def adapter_flops(cfg, H, W):
 
 
 def main():
-    args = sys.argv[1:]
-    opt = lambda name, d: type(d)(args[args.index(name) + 1]) if name in args else d  # noqa: E731
-    steps, warmup, reps = opt("--steps", 31), opt("--warmup", 4), opt("--reps", 3)
-    out_path = args[0] if args and not args[0].startswith("--") else None
+    out_path, steps, warmup, reps = sb.options(steps=31, warmup=4, reps=3)
     ctx = sdxl_b200.Context(0)
     dev = str(ctx.device)
-    res = {"gpu": gpu_info()}
+    res = {"gpu": sb.gpu_info()}
     acfg = sdxl_b200.SDXL_T2I_ADAPTER
-    d = sdxl_b200.Diffuser(ctx, sdxl_b200.SDXL_BASE, sdxl_b200.build_pack(sdxl_b200.synth_weights(sdxl_b200.SDXL_BASE, seed=0, device=dev)))
+    d = sb.load_unet(ctx)
     ads = [sdxl_b200.T2IAdapter(ctx, acfg, sdxl_b200.build_pack(sdxl_b200.synth_weights(acfg, seed=s, device=dev))) for s in (1, 2)]
     torch.cuda.empty_cache()
     g = lambda s: torch.Generator().manual_seed(s)  # noqa: E731
     hints = [torch.rand(1, 3, HW, HW, generator=g(10 + i)).to(ctx.device) for i in range(2)]
-    cond = sdxl_b200.Conditioning(
-        context_full=torch.randn(1, 77, 2048, generator=g(1)).half(), unconditional_context_full=torch.randn(77, 2048, generator=g(2)).half(),
-        channel_context=torch.randn(1, 2816, generator=g(3)).half(), unconditional_channel_context=torch.randn(2816, generator=g(4)).half(),
-        resolution=(HW, HW))
-    ts = sdxl_b200.ddim_timesteps(30)
-    step_size = 1000 // 30
+    cond = sb.conditioning()
 
     def attach(k):
         d.set_t2i_adapters([(ads[i], hints[i], 1.0) for i in range(k)])
         d.sampler_begin(cond, 7.5)
 
-    def run_steps():
-        d.sampler_set_latent(ctx.randn(4 * (HW // 8) ** 2, seed=0).reshape(1, 4, HW // 8, HW // 8))
-        for i in range(warmup):
-            t = ts[i % len(ts)]
-            d.sampler_step(t, t - step_size if t >= step_size else -1)
-        ctx.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record(ctx.stream)
-        for i in range(steps):
-            t = ts[i % len(ts)]
-            d.sampler_step(t, t - step_size if t >= step_size else -1)
-        e1.record(ctx.stream)
-        ctx.synchronize()
-        return e0.elapsed_time(e1) / steps
+    def run(k):
+        attach(k)
+        return sb.run_steps(ctx, d, steps, warmup)
 
-    step = {0: [], 1: [], 2: []}
-    for r in range(reps):
-        for j in range(3):
-            k = (r + j) % 3
-            attach(k)
-            step[k].append(round(run_steps(), 3))
-    res["step_ms"] = {f"{k}_adapters": {"median": statistics.median(v), "runs": v} for k, v in step.items()}
+    res["step_ms"] = {f"{k}_adapters": v for k, v in sb.step_rounds([0, 1, 2], reps, run).items()}
     b = res["step_ms"]["0_adapters"]["median"]
     res["step_ratio_vs_base"] = {k: round(v["median"] / b, 4) for k, v in res["step_ms"].items()}
     print(json.dumps(res["step_ms"]), flush=True)
 
-    def timed(fn, before=lambda: None):
-        ts_ = []
-        for _ in range(reps):
-            before()          # untimed set-up
-            ctx.synchronize()
-            t0 = time.perf_counter()
-            fn()
-            ctx.synchronize()
-            ts_.append((time.perf_counter() - t0) * 1e3)
-        return round(statistics.median(ts_), 2)
-
     res["set_t2i_adapters_ms"] = {
         # attach to a UNet with no adapter (the detach before it is not timed)
-        "attach_one": timed(lambda: d.set_t2i_adapters([(ads[0], hints[0], 1.0)]), before=lambda: d.set_t2i_adapters([])),
-        "rewrite_in_place": timed(lambda: d.set_t2i_adapters([(ads[0], hints[0], 0.8)])),
-        "attach_two": timed(lambda: d.set_t2i_adapters([(ads[i], hints[i], 1.0) for i in range(2)]), before=lambda: d.set_t2i_adapters([])),
+        "attach_one": sb.timed(ctx, reps, lambda: d.set_t2i_adapters([(ads[0], hints[0], 1.0)]), before=lambda: d.set_t2i_adapters([])),
+        "rewrite_in_place": sb.timed(ctx, reps, lambda: d.set_t2i_adapters([(ads[0], hints[0], 0.8)])),
+        "attach_two": sb.timed(ctx, reps, lambda: d.set_t2i_adapters([(ads[i], hints[i], 1.0) for i in range(2)]),
+                               before=lambda: d.set_t2i_adapters([])),
     }
     fw = []
     ads[0].features(hints[0])
@@ -131,16 +80,13 @@ def main():
     res["adapter_forward_ms_per_image"] = round(statistics.median(fw), 3)
     res["adapter_forward_gflop_per_image"] = round(adapter_flops(acfg, HW, HW) * 1e-9, 1)
     attach(1)
-    run_steps()
+    sb.run_steps(ctx, d, steps, warmup)
     res["profile_one_adapter"] = d.profile_plan()
     # the four adds' HBM traffic per CFG step: read x and F, write x, over 2 rows
     res["add_bytes_per_step"] = sum(2 * 3 * 4 * (HW // d_) ** 2 * c for c, d_ in zip(acfg.channels, (16, 16, 32, 32)))
     d.set_t2i_adapters([])
-    res["gpu_after"] = gpu_info()
-    print(json.dumps(res))
-    if out_path:
-        with open(out_path, "w") as f:
-            json.dump(res, f, indent=1)
+    res["gpu_after"] = sb.gpu_info()
+    sb.report(res, out_path)
     for a in ads:
         a.close()
     d.close()
