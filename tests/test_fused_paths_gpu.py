@@ -22,18 +22,12 @@ import torch.nn.functional as F
 
 from sdxl_b200 import SdxlError
 from sdxl_b200 import _testing as T
+from harness import (DEV, H11, H_SUB, U24, check, conv_taps, f16_round_bound, gn_ref, nchw, pad64, plan_upconv,
+                     repack3)
 
 pytestmark = pytest.mark.gpu
 
 U23 = 2.0 ** -23      # one f32 ulp (relative)
-U24 = 2.0 ** -24      # f32 unit roundoff
-H11 = 2.0 ** -11      # f16 unit roundoff
-H_SUB = 2.0 ** -25    # half the f16 subnormal spacing
-DEV = "cuda"
-
-
-def pad64(k: int) -> int:
-    return (k + 63) // 64 * 64
 
 
 def f16(t: torch.Tensor) -> torch.Tensor:
@@ -44,47 +38,9 @@ def randn(g, *shape, scale=1.0, shift=0.0):
     return torch.randn(*shape, generator=g) * scale + shift
 
 
-def check(out: torch.Tensor, ref: torch.Tensor, tol: torch.Tensor, what: str) -> None:
-    err = (out.double() - ref).abs()
-    bad = err > tol
-    worst = float((err / tol.clamp_min(1e-300)).max())
-    print(f"{what}: max err {float(err.max()):.3e}, worst err / bound {worst:.3f}")
-    assert not bool(bad.any()), f"{what}: {int(bad.sum())} elements outside the bound (worst err / bound {worst:.2f})"
-
-
-def f16_round_bound(ref: torch.Tensor) -> torch.Tensor:
-    return ref.abs() * H11 + H_SUB
-
-
 # ------------------------------------------------------------------------------------------------------------------------------
 # implicit GEMM: the plan's convolution forms
 # ------------------------------------------------------------------------------------------------------------------------------
-def nchw(x: torch.Tensor) -> torch.Tensor:
-    return x.permute(0, 3, 1, 2)
-
-
-def conv_taps(nkb: int, map_: int = 0):
-    return [(map_, kw - 1, kh - 1, 0, nkb) for kh in range(3) for kw in range(3)]
-
-
-def plan_upconv(x16: torch.Tensor, w: torch.Tensor, b32: torch.Tensor):
-    """PlanBuilder::upconv: repack_upconv's phase kernels, then one launch per output parity (a, b) writing the pixels
-    (2i + a, 2j + b) of the upsampled output through opix_row = 4W, opix_w = 2, opix_off = a * 2W + b."""
-    B, H, W, I = x16.shape
-    O = w.shape[0]
-    Ipad = pad64(I)
-    Ktot = 4 * Ipad
-    wup = torch.empty(4 * O * Ktot, dtype=torch.float16, device=DEV)
-    T.repack_upconv(w, O, I, wup, Ipad)
-    out = torch.full((B, 2 * H, 2 * W, O), float("nan"), dtype=torch.float32, device=DEV)
-    for pa in range(2):
-        for pb in range(2):
-            segs = [(0, tw - 1 if pb == 0 else tw, th - 1 if pa == 0 else th, 0, Ipad // 64) for th in range(2) for tw in range(2)]
-            wp = wup[(pa * 2 + pb) * O * Ktot:(pa * 2 + pb + 1) * O * Ktot]
-            T.igemm(x16, (B, H, W, I), wp, O, Ktot, (W, H, B), segs, out, O, bias=b32, opix=(4 * W, 2, pa * 2 * W + pb))
-    return out, wup.view(4, O, 4, Ipad)
-
-
 def upconv_phase_weights_host(w: torch.Tensor) -> torch.Tensor:
     """repack_upconv_kernel's summed taps, added in f32 in its (kh, kw) order and rounded once: [4 (a, b), O, 4 (th, tw), I]."""
     w = w.float().cpu()
@@ -153,14 +109,6 @@ def test_upsample_conv_plan_form(ctx, B, H, W, I, O):
     check(out, op.double(), e_plan + e_op, "upconv vs sdxl_op_conv2d(upsample=1)")
     print(f"upconv vs sdxl_op_conv2d(upsample=1): normwise rel diff "
           f"{float((out.double() - op.double()).norm() / op.double().norm()):.3e}")
-
-
-def repack3(w: torch.Tensor, Ktot: int, wt: torch.Tensor = None, col0: int = 0) -> torch.Tensor:
-    O, I, kh, _ = w.shape
-    if wt is None:
-        wt = torch.zeros(O * Ktot, dtype=torch.float16, device=DEV)
-    T.repack_conv(w, O, I, kh, kh, wt, Ktot, col0, pad64(I))
-    return wt
 
 
 @pytest.mark.parametrize("B,H,W,Cin,Cout", [(2, 12, 12, 960, 320), (3, 9, 10, 1920, 640), (2, 5, 7, 320, 320)])
@@ -241,27 +189,6 @@ def test_resnet_second_conv_identity_residual(ctx, B, H, W, C):
 # ------------------------------------------------------------------------------------------------------------------------------
 # GroupNorm
 # ------------------------------------------------------------------------------------------------------------------------------
-def gn_ref(x1, x2, B, HW, G, gam, bet, eps, silu):
-    """float64 GroupNorm (+SiLU) of cat(x1, x2): returns t, and the bound on the kernel's f32 evaluation error of t."""
-    xc = (x1 if x2 is None else torch.cat([x1, x2], dim=2)).double()
-    C = xc.shape[2]
-    xg = xc.view(B, HW, G, C // G)
-    mean = xg.mean(dim=(1, 3), keepdim=True)
-    var = ((xg - mean) ** 2).mean(dim=(1, 3), keepdim=True)
-    rstd = 1.0 / torch.sqrt(var + eps)
-    sc = (rstd * gam.double().view(1, 1, G, C // G))
-    n = ((xg - mean) * sc).view(B, HW, C) + bet.double()
-    # y = fmaf(x, sc, sh), sc = f32(rstd) * gamma, sh = fmaf(-mean, sc, beta), mean / rstd rounded from double to f32:
-    # a few f32 roundings of the terms |x sc|, |mean sc|, |beta|
-    e32 = 8 * U24 * ((xg.abs() * sc.abs()).view(B, HW, C) + (mean.abs() * sc.abs()).expand_as(xg).reshape(B, HW, C) + bet.double().abs())
-    if not silu:
-        return n, e32
-    t = n * torch.sigmoid(n)
-    # x / (1 + __expf(-x)) in f32: __expf's error grows with |x| (2^-21 + |x| 2^-23 relative); the f32 error of n passes
-    # through silu' <= 1.1
-    return t, 1.1 * e32 + 2.0 ** -20 * (1 + n.abs()) * t.abs()
-
-
 def run_gn(B, HW, C1, C2, G, silu, scratch, g):
     x1 = randn(g, B, HW, C1, scale=1.5, shift=0.3).to(DEV)
     x2 = randn(g, B, HW, C2, scale=0.7, shift=-0.2).to(DEV) if C2 else None
@@ -323,6 +250,80 @@ def test_group_norm_rejects_n_group_not_multiple_of_4(ctx):
     out = ctx.group_norm(x, None, gam, bet, n_group=12)
     t, e32 = gn_ref(x.to(DEV), None, 1, 16, 12, gam.to(DEV), bet.to(DEV), 1e-5, False)
     check(out, t, f16_round_bound(t) + e32, "op group_norm n_group=12")
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# LayerNorm
+# ------------------------------------------------------------------------------------------------------------------------------
+def ln_ref(x, gam, bet, eps, unbiased=False):
+    """float64 LayerNorm over the last dim of x [rows, C], and the bound on layernorm_kernel's f32 evaluation error (one warp per
+    row, NV = ceil(C / 128) float4 per lane, exact two-pass statistics):
+      - each warp sum: 4 NV lane-serial additions, then 5 shuffle levels: (4 NV + 5) 2^-24 sum|terms|; mean = sum / C rounds
+        once more;
+      - q = sum (x - mean32)^2: each centred value rounded (doubled by the square), each square rounded, then the same sum;
+        the mean's error d adds C d^2 exactly (sum (x - mean) = 0); var = q / C + eps: two roundings;
+      - rstd = 1 / sqrtf(var): half the variance's relative error, plus two roundings;
+      - y = (x - mean32) rstd gamma + beta: the mean's error times rstd |gamma|, the relative errors of the centred value and of
+        rstd, and three roundings.
+    The estimate is first order; a factor 2 covers the second-order terms. unbiased: the sample variance (sum / (C - 1)), a
+    reference the bound must reject."""
+    xd = x.double()
+    C = xd.shape[1]
+    n_add = 4 * ((C + 127) // 128) + 5
+    mean = xd.mean(dim=1, keepdim=True)
+    d = xd - mean
+    var = (d * d).sum(dim=1, keepdim=True) / (C - 1 if unbiased else C)
+    rstd = 1.0 / torch.sqrt(var + eps)
+    ref = d * rstd * gam.double() + bet.double()
+    e_mean = (n_add + 1) * U24 * xd.abs().mean(dim=1, keepdim=True)
+    rel_var = ((n_add + 6) * U24 * (var + e_mean ** 2) + e_mean ** 2) / (var + eps) + U24
+    rel_rstd = 0.5 * rel_var + rel_var ** 2 + 2 * U24
+    e32 = 2 * (gam.double().abs() * rstd * (e_mean + d.abs() * (rel_rstd + 4 * U24)) + 2 * U24 * (ref.abs() + bet.double().abs()))
+    return ref, e32
+
+
+def ln_rows(g, kind, rows, C):
+    if kind == "N(0.5, 2)":
+        return randn(g, rows, C, scale=2.0, shift=0.5)
+    if kind == "large mean":        # |mean| / std up to 1e3
+        std = torch.exp(randn(g, rows, 1))
+        return randn(g, rows, C) * std + (torch.rand(rows, 1, generator=g) * 2 - 1) * 1e3 * std
+    if kind == "std 1e-3":          # eps = 1e-5 is ten times the variance
+        return randn(g, rows, C, scale=1e-3, shift=0.3)
+    # constant rows of multiples of 2^-4: the sums and the mean are exact, so x - mean = 0 and y = beta
+    return (torch.randint(-64, 65, (rows, 1), generator=g).float() / 16).expand(rows, C).contiguous()
+
+
+@pytest.mark.parametrize("C", [64, 100, 320, 384, 640, 768, 1024, 1280, 1536, 1664, 2048])
+def test_layer_norm(ctx, C):
+    """layernorm_kernel through sdxl_op_layer_norm at every width class (all five NV instantiations; C = 100 and 1664 leave the
+    last float4 group of the warp partly empty), row counts that are not a multiple of the 8 warps of a CTA, and four kinds of
+    rows: N(0.5, 2), |mean| / std up to 1e3, std 1e-3 (eps comparable to the variance) and constant rows (output exactly
+    f16(beta)). At C <= 320 the bound must also reject the unbiased-variance reference (a relative change of 1 / (2C) in rstd)."""
+    g = torch.Generator().manual_seed(C)
+    gam, bet = 1 + 0.1 * randn(g, C), 0.1 * randn(g, C)
+    gd, bd = gam.to(DEV), bet.to(DEV)
+    for rows in (1, 7, 154, 2964, 8193):
+        for kind in ("N(0.5, 2)", "large mean", "std 1e-3", "constant"):
+            x = ln_rows(g, kind, rows, C).to(DEV)
+            out = ctx.layer_norm(x, gam, bet, 1e-5)
+            ref, e32 = ln_ref(x, gd, bd, 1e-5)
+            tol = f16_round_bound(ref) + e32
+            check(out, ref, tol, f"layer_norm C={C} rows={rows} {kind}")
+            if kind == "constant":
+                assert torch.equal(out, bd.half().expand(rows, C)), f"C={C}: a constant row must give exactly f16(beta)"
+            if kind == "N(0.5, 2)" and C <= 320:
+                ref_u, _ = ln_ref(x, gd, bd, 1e-5, unbiased=True)
+                assert bool(((out.double() - ref_u).abs() > tol).any()), \
+                    f"C={C} rows={rows}: the bound does not tell the biased from the unbiased variance"
+
+
+def test_layer_norm_rejects(ctx):
+    """layernorm_launch reads rows as float4 and caches at most 16 per lane: C % 4 != 0 (3003) and C > 2048 (3004) are refused."""
+    for C, code in ((102, 3003), (2052, 3004), (4096, 3004)):
+        x = torch.zeros(3, C)
+        with pytest.raises(SdxlError, match=rf"\({code}\)"):
+            ctx.layer_norm(x, torch.ones(C), torch.zeros(C))
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
