@@ -87,6 +87,10 @@ SDXL_API const char* sdxl_last_error(const sdxl_ctx* ctx);
 SDXL_API int sdxl_ctx_synchronize(sdxl_ctx* ctx);
 /* Number of this library's kernels launched on the ctx since creation (bench `gpu_launches`). */
 SDXL_API uint64_t sdxl_ctx_launch_count(const sdxl_ctx* ctx);
+/* The byte $SDXL_B200_FILL asks for, or -1 when it is unset or not a byte (0..255, decimal or 0x..). When it is set, every
+ * device buffer the library allocates for itself is filled before first use: floating-point buffers with this byte,
+ * integer and byte buffers with 0. A debugging aid: a read of memory nothing wrote then reaches the outputs. */
+SDXL_API int sdxl_debug_fill(void);
 
 /* ---- UNet / Diffuser ------------------------------------------------------------------------ */
 /* Replaces load_diffuser_model (src/bin/sample/main.rs:35-41): builds the device-resident model from

@@ -431,7 +431,7 @@ static int vision_run(sdxl_clip_vision* m, int N, const float* pixels, int on_ho
   TmpBufs tmp(c->stream);
   const float* px = pixels;
   if (on_host) {
-    float* d = (float*)tmp.get(in_bytes);
+    float* d = tmp.get<float>(in_bytes);
     if (!d) return fail(c, 5206, "vision encoder: cannot allocate %zu bytes for the pixels", in_bytes);
     CU(c, cudaMemcpyAsync(d, pixels, in_bytes, cudaMemcpyHostToDevice, c->stream));
     px = d;

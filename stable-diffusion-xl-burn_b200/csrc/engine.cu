@@ -63,6 +63,7 @@ extern "C" int sdxl_ctx_synchronize(sdxl_ctx* c) {
   return 0;
 }
 extern "C" uint64_t sdxl_ctx_launch_count(const sdxl_ctx* c) { return c ? c->launches : 0; }
+extern "C" int sdxl_debug_fill(void) { return debug_fill_byte(); }
 
 // ================================================================================================
 // model
@@ -722,7 +723,7 @@ template <class X, class... A>
 static int stage_in(sdxl_ctx* c, TmpBufs& T, const X* src, size_t bytes, int on_host, const X*& x, int code, const char* fmt, A... args) {
   x = src;
   if (!on_host) return 0;
-  X* d = (X*)T.get(bytes);
+  X* d = T.get<X>(bytes);
   if (!d) return fail(c, code, fmt, args...);
   CU(c, cudaMemcpyAsync(d, src, bytes, cudaMemcpyHostToDevice, c->stream));
   x = d;
@@ -749,8 +750,8 @@ static int embed_hint(sdxl_controlnet* net, int n, int H, int W, const float* hi
     for (int k = 0; k < nb; ++k) { maxe = std::max(maxe, (size_t)n * h * w * hc[k]); h /= 2; w /= 2; }
   }
   TmpBufs T(c->stream);
-  float* a = (float*)T.get(maxe * sizeof(float));
-  __half* a16 = (__half*)T.get(maxe * sizeof(__half));
+  float* a = T.get<float>(maxe * sizeof(float));
+  __half* a16 = T.get<__half>(maxe * sizeof(__half));
   if (!a || !a16) return fail(c, 4711, "hint encoder: cannot allocate %zu bytes of scratch", maxe * 6);
   KL(c, conv_in_launch_t(c->stream, hint, 1, n, n, nc.hint_in_channels, H, W, net->hint0_w, net->hint0_b, hc[0], a));
   int h = H, w = W;
@@ -774,8 +775,8 @@ extern "C" int sdxl_controlnet_embed_hint(sdxl_controlnet* net, int n, int H, in
   const size_t in_bytes = (size_t)n * net->ncfg.hint_in_channels * H * W * sizeof(float), out_elems = (size_t)n * h * w * mc;
   const float* x;
   if (int r = stage_in(c, T, hint, in_bytes, on_host, x, 4711, "embed_hint: allocation failed")) return r;
-  float* e = (float*)T.get(out_elems * sizeof(float));
-  float* o = on_host ? (float*)T.get(out_elems * sizeof(float)) : out;
+  float* e = T.get<float>(out_elems * sizeof(float));
+  float* o = on_host ? T.get<float>(out_elems * sizeof(float)) : out;
   if (!e || !o) return fail(c, 4711, "embed_hint: allocation failed");
   if (int r = embed_hint(net, n, H, W, x, e)) return r;
   KL(c, nhwc_to_nchw_f32_launch(c->stream, e, n, h * w, mc, mc, o));
@@ -1620,7 +1621,7 @@ static int ip_project(const sdxl_ip_adapter* a, int n, const float* e, __half* t
   sdxl_ctx* c = a->ctx;
   const Lin& P = a->proj;
   TmpBufs T(c->stream);
-  float* y = (float*)T.get((size_t)n * P.N * sizeof(float));
+  float* y = T.get<float>((size_t)n * P.N * sizeof(float));
   if (!y) return fail(c, 4810, "IP-Adapter projection: cannot allocate %zu bytes", (size_t)n * P.N * sizeof(float));
   for (int b0 = 0; b0 < n; b0 += 8)
     KL(c, gemv_launch(c->stream, e + (size_t)b0 * P.K, P.K, std::min(8, n - b0), P.K, P.w, P.Kpad, P.b, nullptr, 0, P.N, 0, 0,
@@ -1637,15 +1638,15 @@ static int ip_resample(const sdxl_ip_adapter* a, int n, int L, const float* h, _
   const sdxl_ip_adapter_cfg& g = a->cfg;
   const int D = g.image_embed_dim, Q = g.tokens_per_image, W = 64 * g.resampler_heads, S = L + Q, ctx_dim = g.unet.context_dim;
   TmpBufs T(c->stream);
-  __half* h16 = (__half*)T.get((size_t)n * L * D * sizeof(__half));
-  float* x = (float*)T.get((size_t)n * L * W * sizeof(float));          // proj_in(h), read by every layer
-  float* lat = (float*)T.get((size_t)n * Q * W * sizeof(float));        // the latent stream
-  __half* kv_in = (__half*)T.get((size_t)n * S * W * sizeof(__half));   // per image [LN1(x) ; LN2(lat)]
-  __half* a16 = (__half*)T.get((size_t)n * Q * W * sizeof(__half));     // the f16 operand of the next GEMM on the latent rows
-  __half* q16 = (__half*)T.get((size_t)n * Q * W * sizeof(__half));
-  __half* kv16 = (__half*)T.get((size_t)n * S * 2 * W * sizeof(__half));
-  float* f32 = (float*)T.get((size_t)n * Q * std::max(4 * W, ctx_dim) * sizeof(float));   // fc1 output, then proj_out output
-  __half* f16 = (__half*)T.get((size_t)n * Q * 4 * W * sizeof(__half));
+  __half* h16 = T.get<__half>((size_t)n * L * D * sizeof(__half));
+  float* x = T.get<float>((size_t)n * L * W * sizeof(float));          // proj_in(h), read by every layer
+  float* lat = T.get<float>((size_t)n * Q * W * sizeof(float));        // the latent stream
+  __half* kv_in = T.get<__half>((size_t)n * S * W * sizeof(__half));   // per image [LN1(x) ; LN2(lat)]
+  __half* a16 = T.get<__half>((size_t)n * Q * W * sizeof(__half));     // the f16 operand of the next GEMM on the latent rows
+  __half* q16 = T.get<__half>((size_t)n * Q * W * sizeof(__half));
+  __half* kv16 = T.get<__half>((size_t)n * S * 2 * W * sizeof(__half));
+  float* f32 = T.get<float>((size_t)n * Q * std::max(4 * W, ctx_dim) * sizeof(float));   // fc1 output, then proj_out output
+  __half* f16 = T.get<__half>((size_t)n * Q * 4 * W * sizeof(__half));
   if (!h16 || !x || !lat || !kv_in || !a16 || !q16 || !kv16 || !f32 || !f16)
     return fail(c, 4812, "IP-Adapter Plus Resampler: cannot allocate its buffers (n = %d, seq_len = %d)", n, L);
   // out [M, Lw.N] (row pitch Lw.N) = in [M, Lw.K] (row pitch lda) @ Lw + bias (+ res, f32 output only)
@@ -1685,7 +1686,7 @@ extern "C" int sdxl_ip_adapter_resample(sdxl_ip_adapter* a, int n, int seq_len, 
   const size_t out_bytes = (size_t)n * a->cfg.tokens_per_image * a->cfg.unet.context_dim * sizeof(__half);
   const float* e;
   if (int r = stage_in(c, T, hidden, in_bytes, on_host, e, 4811, "ip_adapter_resample: allocation failed")) return r;
-  __half* o = on_host ? (__half*)T.get(out_bytes) : (__half*)tokens_out;
+  __half* o = on_host ? T.get<__half>(out_bytes) : (__half*)tokens_out;
   if (!o) return fail(c, 4811, "ip_adapter_resample: allocation failed");
   if (int r = ip_resample(a, n, seq_len, e, o)) return r;
   return on_host ? stage_out(c, tokens_out, o, out_bytes) : 0;
@@ -1701,7 +1702,7 @@ extern "C" int sdxl_ip_adapter_project(sdxl_ip_adapter* a, int n, const float* e
   const size_t out_bytes = (size_t)n * a->cfg.tokens_per_image * a->cfg.unet.context_dim * sizeof(__half);
   const float* e;
   if (int r = stage_in(c, T, embeds, in_bytes, on_host, e, 4811, "ip_adapter_project: allocation failed")) return r;
-  __half* o = on_host ? (__half*)T.get(out_bytes) : (__half*)tokens_out;
+  __half* o = on_host ? T.get<__half>(out_bytes) : (__half*)tokens_out;
   if (!o) return fail(c, 4811, "ip_adapter_project: allocation failed");
   if (int r = ip_project(a, n, e, o)) return r;
   return on_host ? stage_out(c, tokens_out, o, out_bytes) : 0;
@@ -1739,14 +1740,14 @@ static int ip_stage(sdxl_ctx* c, int n_levels, const IpPrompt& a, const sdxl_ima
   if (p.negative_embeds) {
     if (int r = stage_in(c, T, p.negative_embeds, bytes, p.on_host, neg, 4820, alloc_failed, bytes)) return r;
   } else {   // diffusers' default negative: zeros
-    float* z = (float*)T.get(bytes);
+    float* z = T.get<float>(bytes);
     if (!z) return fail(c, 4820, alloc_failed, bytes);
     CU(c, cudaMemsetAsync(z, 0, bytes, c->stream));
     neg = z;
   }
-  s.tp = (__half*)T.get(s.tok_bytes);
-  s.tn = (__half*)T.get(s.tok_bytes);
-  s.ts = (float*)T.get(n_tb * sizeof(float));
+  s.tp = T.get<__half>(s.tok_bytes);
+  s.tn = T.get<__half>(s.tok_bytes);
+  s.ts = T.get<float>(n_tb * sizeof(float));
   if (!s.tp || !s.tn || !s.ts) return fail(c, 4820, "set_image_prompt: cannot allocate the token staging buffers");
   if (a.ad->plus()) {
     if (int r = ip_resample(a.ad, n, p.seq_len, e, s.tp)) return r;
@@ -1761,8 +1762,8 @@ static int ip_stage(sdxl_ctx* c, int n_levels, const IpPrompt& a, const sdxl_ima
   if (a.mask_h) {
     const int H = a.mask_h, W = a.mask_w;
     s.mask_floats = ip_mask_off(a, n_levels, a.n_images, 0);
-    float* pix = (float*)T.get(mask.size() * sizeof(float));
-    s.tm = (float*)T.get(s.mask_floats * sizeof(float));
+    float* pix = T.get<float>(mask.size() * sizeof(float));
+    s.tm = T.get<float>(s.mask_floats * sizeof(float));
     if (!pix || !s.tm) return fail(c, 4820, "set_image_prompt: cannot allocate the mask staging buffers");
     CU(c, cudaMemcpyAsync(pix, mask.data(), mask.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
     for (int i = 0; i < a.n_images; ++i)
@@ -2013,9 +2014,9 @@ static int t2i_forward(const sdxl_t2i_adapter* a, int n, int H, int W, const flo
     max32 = std::max(max32, t2i_feature_elems(a, k, n, H, W));
   }
   TmpBufs T(c->stream);
-  __half* a16 = (__half*)T.get(max16 * sizeof(__half));   // the f16 operand of the next conv
-  float* t32 = (float*)T.get(max32 * sizeof(float));      // block1 output
-  __half* t16 = (__half*)T.get(max32 * sizeof(__half));   // relu(block1)
+  __half* a16 = T.get<__half>(max16 * sizeof(__half));   // the f16 operand of the next conv
+  float* t32 = T.get<float>(max32 * sizeof(float));      // block1 output
+  __half* t16 = T.get<__half>(max32 * sizeof(__half));   // relu(block1)
   if (!a16 || !t32 || !t16) return fail(c, 4910, "T2I-Adapter: cannot allocate its scratch (n = %d, %dx%d)", n, H, W);
   KL(c, pixel_unshuffle_launch(c->stream, hint, n, a->cfg.in_channels, H, W, a16));
   if (int r = conv_nhwc(c, a16, n, h2, w2, a->conv_in, F[0], nullptr)) return r;
@@ -2057,12 +2058,12 @@ extern "C" int sdxl_t2i_adapter_features(sdxl_t2i_adapter* a, int n, int H, int 
   float* F[4];
   for (int k = 0; k < 4; ++k) {
     total += t2i_feature_elems(a, k, n, H, W);
-    F[k] = (float*)T.get(t2i_feature_elems(a, k, n, H, W) * sizeof(float));
+    F[k] = T.get<float>(t2i_feature_elems(a, k, n, H, W) * sizeof(float));
   }
   const size_t in_bytes = (size_t)n * a->cfg.in_channels * H * W * sizeof(float);
   const float* x;
   if (int r = stage_in(c, T, hint, in_bytes, on_host, x, 4911, "t2i_adapter_features: allocation failed")) return r;
-  float* o = on_host ? (float*)T.get(total * sizeof(float)) : out;
+  float* o = on_host ? T.get<float>(total * sizeof(float)) : out;
   if (!o || !F[0] || !F[1] || !F[2] || !F[3]) return fail(c, 4911, "t2i_adapter_features: allocation failed");
   if (int r = t2i_forward(a, n, H, W, x, F)) return r;
   size_t off = 0;
@@ -2103,8 +2104,8 @@ extern "C" int sdxl_unet_set_t2i_adapters(sdxl_unet* u, int n, const sdxl_t2i_co
   float* Fa[4];
   bool ok = true;
   for (int k = 0; k < 4; ++k) {
-    S[k] = (float*)T.get(t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float));
-    Fa[k] = (float*)T.get(t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float));
+    S[k] = T.get<float>(t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float));
+    Fa[k] = T.get<float>(t2i_feature_elems(a0, k, n_hint, H, W) * sizeof(float));
     ok = ok && S[k] && Fa[k];
   }
   if (!ok) return fail(c, 4940, "set_t2i_adapters: cannot allocate the feature staging buffers");
@@ -2602,7 +2603,7 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
   TmpBufs tmp(c->stream);
   const float* noise_dev = noise;
   if (n_noise && cond->on_host) {
-    float* d = (float*)tmp.get((size_t)n_noise * bytes);
+    float* d = tmp.get<float>((size_t)n_noise * bytes);
     if (!d) return fail(c, 5235, "cannot allocate %zu bytes to stage the injected noise", (size_t)n_noise * bytes);
     CU(c, cudaMemcpyAsync(d, noise, (size_t)n_noise * bytes, cudaMemcpyHostToDevice, c->stream));
     noise_dev = d;
@@ -2627,7 +2628,7 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
   // entry: xh at sigma_k0, blended for the first forward
   float* init_dev = nullptr;
   if (init_latent && (k0 == 0 && cond->on_host)) {   // the initial noise from the host: read by the kernel as z
-    init_dev = (float*)tmp.get(bytes);
+    init_dev = tmp.get<float>(bytes);
     if (!init_dev) return fail(c, 5235, "cannot allocate %zu bytes to stage the initial noise", bytes);
     CU(c, cudaMemcpyAsync(init_dev, init_latent, bytes, cudaMemcpyHostToDevice, c->stream));
   }
@@ -2745,7 +2746,7 @@ extern "C" int sdxl_op_ip_attention(sdxl_ctx* c, const sdxl_half* q, const sdxl_
   if (B < 1 || S_ip < 1) return fail(c, 5303, "sdxl_op_ip_attention: B = %d and S_ip = %d must be >= 1", B, S_ip);
   CU(c, cudaSetDevice(c->device));
   TmpBufs tmp(c->stream);
-  float* s = (float*)tmp.get(sizeof(float));
+  float* s = tmp.get<float>(sizeof(float));
   if (!s) return fail(c, 5304, "temporary allocation failed");
   CU(c, cudaMemcpyAsync(s, &scale, sizeof(float), cudaMemcpyHostToDevice, c->stream));
   AttnParams p{};
@@ -2775,8 +2776,8 @@ extern "C" int sdxl_op_linear(sdxl_ctx* c, const sdxl_half* x, const sdxl_half* 
     gbn = geglu_bn_for(N / 2);
     if (!gbn || (N & 1)) return fail(c, 5311, "sdxl_op_linear: GEGLU width not tileable");
   }
-  __half* wt = (__half*)T.get((size_t)N * Kpad * 2);
-  float* b32 = bias ? (float*)T.get((size_t)N * 4) : nullptr;
+  __half* wt = T.get<__half>((size_t)N * Kpad * 2);
+  float* b32 = bias ? T.get<float>((size_t)N * 4) : nullptr;
   if (!wt || (bias && !b32)) return fail(c, 5312, "temporary allocation failed");
   KL(c, transpose_linear_launch(c->stream, (const __half*)w, K, N, wt, Kpad, 0, gbn));
   if (bias) KL(c, bias_to_f32_launch(c->stream, (const __half*)bias, N, b32, gbn, 0));
@@ -2793,10 +2794,10 @@ extern "C" int sdxl_op_conv2d(sdxl_ctx* c, const float* x, const sdxl_half* w, c
   if (Cin % 8) return fail(c, 5321, "sdxl_op_conv2d: Cin must be a multiple of 8");
   TmpBufs T(c->stream);
   const int Ipad = (Cin + 63) / 64 * 64, Ktot = ksize * ksize * Ipad;
-  __half* wt = (__half*)T.get((size_t)Cout * Ktot * 2);
-  float* b32 = bias ? (float*)T.get((size_t)Cout * 4) : nullptr;
+  __half* wt = T.get<__half>((size_t)Cout * Ktot * 2);
+  float* b32 = bias ? T.get<float>((size_t)Cout * 4) : nullptr;
   const int Hi = upsample ? 2 * H : H, Wi = upsample ? 2 * W : W;  // conv input extent
-  __half* a16 = (__half*)T.get((size_t)B * Hi * Wi * Cin * 2);
+  __half* a16 = T.get<__half>((size_t)B * Hi * Wi * Cin * 2);
   if (!wt || !a16 || (bias && !b32)) return fail(c, 5322, "temporary allocation failed");
   KL(c, repack_conv_launch(c->stream, (const __half*)w, Cout, Cin, ksize, ksize, wt, Ktot, 0, Ipad));
   if (bias) KL(c, bias_to_f32_launch(c->stream, (const __half*)bias, Cout, b32, 0, 0));
@@ -2820,7 +2821,7 @@ extern "C" int sdxl_op_group_norm(sdxl_ctx* c, const float* x1, int C1, const fl
                                   const float* gamma, const float* beta, float eps, int silu, sdxl_half* out) {
   if (!c || !x1 || !gamma || !beta || !out) return -1;
   TmpBufs T(c->stream);
-  float* part = (float*)T.get(gn_scratch_floats(B, n_group) * 4);
+  float* part = T.get<float>(gn_scratch_floats(B, n_group) * 4);
   if (part && gn_scratch_init(c->stream, part, B, n_group)) return fail(c, 5007, "GroupNorm scratch init failed");
   if (!part) return fail(c, 5330, "temporary allocation failed");
   GnParams p{x1, C1, x2, x2 ? C2 : 0, B, HW, n_group, gamma, beta, eps, silu, (__half*)out, nullptr, part, 0};
@@ -2837,7 +2838,7 @@ extern "C" int sdxl_op_layer_norm(sdxl_ctx* c, const float* x, const float* gamm
 extern "C" int sdxl_op_timestep_embedding(sdxl_ctx* c, const int32_t* t_host, int n, int dim, int max_period, float* out) {
   if (!c || !t_host || !out || n < 1 || (dim & 1)) return -1;
   TmpBufs T(c->stream);
-  int* td = (int*)T.get((size_t)n * 4);
+  int* td = T.get<int>((size_t)n * 4);
   if (!td) return fail(c, 5340, "temporary allocation failed");
   CU(c, cudaMemcpyAsync(td, t_host, (size_t)n * 4, cudaMemcpyHostToDevice, c->stream));
   KL(c, timestep_embedding_launch(c->stream, td, n, dim, (float)max_period, out));

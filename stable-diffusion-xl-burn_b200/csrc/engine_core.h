@@ -16,6 +16,7 @@
 #include <map>
 #include <memory>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 using namespace sdxl;
@@ -56,18 +57,44 @@ static int fail(sdxl_ctx* c, int code, const char* fmt, ...) {
   } while (0)
 
 // ================================================================================================
+// fresh-memory fill (SDXL_B200_FILL)
+// ================================================================================================
+// SDXL_B200_FILL=<byte> (decimal or 0x..): every device buffer the library carves for itself is memset on its stream before
+// anything writes to it, so that a read of memory nothing wrote reaches the outputs instead of whatever the allocator left
+// there. Floating-point buffers get the byte (0xff: NaN in f16 and f32; 0x7b: large finite values); integer and byte buffers
+// get 0, so that an index or a count is never poisoned into an address. -1 when unset or not a byte (sdxl_debug_fill).
+static int debug_fill_byte() {
+  static const int b = [] {
+    const char* s = getenv("SDXL_B200_FILL");
+    if (!s || !*s) return -1;
+    char* end = nullptr;
+    const long v = strtol(s, &end, 0);
+    return (*end || v < 0 || v > 255) ? -1 : (int)v;
+  }();
+  return b;
+}
+// Queues the fill of n fresh elements of T at p on st; fill = debug_fill_byte(), nothing when it is negative.
+template <typename T>
+static void debug_fill(T* p, size_t n, cudaStream_t st, int fill) {
+  constexpr bool fp = std::is_floating_point<T>::value || std::is_same<T, __half>::value;
+  if (fill >= 0 && p && n) cudaMemsetAsync(p, fp ? fill : 0, n * sizeof(T), st);
+}
+
+// ================================================================================================
 // device arena (bump allocator over one cudaMalloc, freed with the arena)
 // ================================================================================================
 struct Arena {
   uint8_t* base = nullptr;
   size_t cap = 0, off = 0;
   bool measure = false;  // dry run: only count
+  cudaStream_t stream = nullptr;   // the stream that writes the arena: fresh-memory fills are queued on it
+  int fill = -1;                   // debug_fill_byte() for a real arena, -1 for none
   Arena() = default;
-  Arena(Arena&& o) noexcept : base(o.base), cap(o.cap), off(o.off), measure(o.measure) { o.base = nullptr; o.cap = o.off = 0; }
+  Arena(Arena&& o) noexcept : base(o.base), cap(o.cap), off(o.off), measure(o.measure), stream(o.stream), fill(o.fill) { o.base = nullptr; o.cap = o.off = 0; }
   Arena& operator=(Arena&& o) noexcept {
     if (this != &o) {
       release();
-      base = o.base; cap = o.cap; off = o.off; measure = o.measure;
+      base = o.base; cap = o.cap; off = o.off; measure = o.measure; stream = o.stream; fill = o.fill;
       o.base = nullptr; o.cap = o.off = 0;
     }
     return *this;
@@ -96,7 +123,11 @@ struct Arena {
     return measure ? (void*)(uintptr_t)(0x1000 + a) : (void*)(base + a);
   }
   template <typename T>
-  T* get(size_t n) { return (T*)alloc(n * sizeof(T)); }
+  T* get(size_t n) {
+    T* p = (T*)alloc(n * sizeof(T));
+    if (fill >= 0 && !measure) debug_fill(p, n, stream, fill);
+    return p;
+  }
 };
 
 // ================================================================================================
@@ -403,13 +434,16 @@ static int with_device_pack(sdxl_ctx* c, const void* pack, size_t bytes, int pac
 }
 
 // Sizes A by measuring: carve(Arena&) runs once against a measuring arena (placeholder pointers, no device work), A is
-// allocated to the measured size, and carve runs again against A. carve must take the same buffers on both passes.
+// allocated to the measured size, and carve runs again against A. carve must take the same buffers on both passes and write
+// them on the ctx stream (A's fresh-memory fills are queued there).
 template <typename Fn>
 static int carve_measured(sdxl_ctx* c, Arena& A, int code, const char* what, Fn carve) {
   Arena meas;
   meas.measure = true;
   if (int r = carve(meas)) return r;
   if (A.init(meas.off)) return fail(c, code, "cannot allocate %zu bytes for %s", meas.off, what);
+  A.stream = c->stream;
+  A.fill = debug_fill_byte();
   return carve(A);
 }
 
@@ -790,15 +824,20 @@ static int profile_dump_impl(sdxl_ctx* c, Plan* P, const char* path) {
   return 0;
 }
 
+// Stream-ordered staging buffers of one call, freed on the stream when it returns. get<T>(bytes): T says how a fresh buffer
+// is filled under SDXL_B200_FILL (debug_fill).
 struct TmpBufs {
   std::vector<void*> p;
   cudaStream_t st;
+  int fill = debug_fill_byte();
   explicit TmpBufs(cudaStream_t s) : st(s) {}
-  void* get(size_t bytes) {
+  template <typename T>
+  T* get(size_t bytes) {
     void* d = nullptr;
     if (cudaMallocAsync(&d, bytes ? bytes : 16, st) != cudaSuccess) return nullptr;
     p.push_back(d);
-    return d;
+    if (fill >= 0) debug_fill((T*)d, bytes / sizeof(T), st, fill);
+    return (T*)d;
   }
   ~TmpBufs() { for (void* d : p) cudaFreeAsync(d, st); }
 };
@@ -820,7 +859,7 @@ static int adapters_apply(sdxl_ctx* c, AdapterState& S, int n, const sdxl_adapte
     if (ad[a].pack_on_device) {
       pv.dev = (const uint8_t*)ad[a].pack;
     } else {
-      uint8_t* d = (uint8_t*)tmp.get(ad[a].bytes);
+      uint8_t* d = tmp.get<uint8_t>(ad[a].bytes);
       if (!d) return fail(c, 4603, "set_adapters: cannot allocate %zu bytes for adapter %d", ad[a].bytes, a);
       CU(c, cudaMemcpyAsync(d, ad[a].pack, ad[a].bytes, cudaMemcpyHostToDevice, c->stream));
       pv.dev = d;
@@ -918,7 +957,7 @@ static int adapters_apply(sdxl_ctx* c, AdapterState& S, int n, const sdxl_adapte
     p.src = src; p.dst = s.base; p.f32 = s.f32;
     p.ld = s.ld; p.row0 = s.row0; p.col0 = s.col0; p.Ipad = s.Ipad; p.geglu_bn = s.geglu_bn;
     if (s.up) {
-      float* delta = (float*)tmp.get((size_t)p.N * p.Kd * sizeof(float));
+      float* delta = tmp.get<float>((size_t)p.N * p.Kd * sizeof(float));
       if (!delta) return fail(c, 4614, "set_adapters: cannot allocate the upsample delta of '%s'", kv.first.c_str());
       p.delta_out = delta;
       KL(c, lora_merge_launch(c->stream, p));

@@ -135,6 +135,7 @@ PROTOTYPES = {
     "sdxl_last_error": (C.c_char_p, [P]),
     "sdxl_ctx_synchronize": (I, [P]),
     "sdxl_ctx_launch_count": (C.c_uint64, [P]),
+    "sdxl_debug_fill": (I, []),
     "sdxl_unet_load": (I, [P, C.POINTER(UnetCfg), P, C.c_size_t, I, C.POINTER(P)]),
     "sdxl_unet_destroy": (None, [P]),
     "sdxl_unet_set_conditioning": (I, [P, I, I, P, P]),

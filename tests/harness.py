@@ -1,5 +1,5 @@
 """Helpers the tests share: the relative error they bound, the reference's probe input, f16 rounding, the tiny-config CFG
-conditioning, the UNet's plan-build counter, and the kernel-level pieces of the implicit-GEMM and GroupNorm tests (elementwise
+conditioning, a report of where two tensors differ, the UNet's plan-build counter, and the kernel-level pieces of the implicit-GEMM and GroupNorm tests (elementwise
 bound check, the plan's conv tap segments and weight repacks, float64 GroupNorm)."""
 import numpy as np
 import torch
@@ -42,6 +42,21 @@ def tiny_conditioning(B=2, n_ctx=7, res=(128, 128), cfg=TINY, refiner=False):
                   channel_context_refiner=h16f(arb(B, r.adm_in_channels) * 0.5),
                   unconditional_channel_context_refiner=h16f(arb(r.adm_in_channels).cos()))
     return kw
+
+
+def first_difference(a: torch.Tensor, b: torch.Tensor) -> str:
+    """Where b differs bit for bit from a: how many elements, the non-finite counts of each, and the largest |a - b| with its index
+    (a NaN or an infinity on either side counts as the largest)."""
+    if a.shape != b.shape or a.dtype != b.dtype:
+        return f"shape / dtype {tuple(a.shape)} {a.dtype} vs {tuple(b.shape)} {b.dtype}"
+    a64, b64 = a.double(), b.double()
+    d = (a64 - b64).abs().nan_to_num(nan=float("inf"))
+    d[a64 == b64] = 0
+    i = int(d.flatten().argmax())
+    idx = tuple(int(k) for k in torch.unravel_index(torch.tensor(i), a.shape))
+    return (f"{int((a64 != b64).sum())} of {a.numel()} elements differ; non-finite: {int((~torch.isfinite(a64)).sum())} vs "
+            f"{int((~torch.isfinite(b64)).sum())}; max |delta| {float(d.flatten()[i]):.3e} at {idx} "
+            f"({float(a64.flatten()[i])!r} vs {float(b64.flatten()[i])!r})")
 
 
 def plan_builds(d):
