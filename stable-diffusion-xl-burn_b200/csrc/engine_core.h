@@ -809,16 +809,17 @@ static int profile_dump_impl(sdxl_ctx* c, Plan* P, const char* path) {
   if (int r = time_plan_ops(c, P, ms)) return r;
   FILE* f = fopen(path, "w");
   if (!f) return fail(c, -3, "cannot open %s", path);
-  fprintf(f, "op,kind,us,gflop,tflops,M_tiles,N,BN,Kblocks,T,S,heads\n");
+  fprintf(f, "op,kind,us,gflop,tflops,M_tiles,N,BN,Kblocks,T,S,heads,mode,out_f32,res\n");
   for (size_t i = 0; i < ms.size(); ++i) {
     const Op& o = P->ops[i];
-    int mt = 0, N = 0, BN = 0, kb = 0, T = 0, S = 0, H = 0;
+    int mt = 0, N = 0, BN = 0, kb = 0, T = 0, S = 0, H = 0, mode = 0, of32 = 0, res = 0;
     if (o.kind == OP_IGEMM) {
       mt = o.ig.tilesW * o.ig.tilesH * o.ig.tilesB; N = o.ig.N; BN = o.ig.BN;
+      mode = o.ig.mode; of32 = o.ig.out_f32; res = o.ig.res != nullptr;
       for (int s2 = 0; s2 < o.ig.nseg; ++s2) kb += o.ig.seg[s2].nkb;
     } else if (o.kind == OP_ATTN) { T = o.at.T; S = o.at.S; H = o.at.n_head; }
-    fprintf(f, "%zu,%s,%.2f,%.3f,%.1f,%d,%d,%d,%d,%d,%d,%d\n", i, kOpNames[o.kind], ms[i] * 1e3, o.flops * 1e-9,
-            ms[i] > 0 ? o.flops / (ms[i] * 1e-3) * 1e-12 : 0.0, mt, N, BN, kb, T, S, H);
+    fprintf(f, "%zu,%s,%.2f,%.3f,%.1f,%d,%d,%d,%d,%d,%d,%d,%d,%d,%d\n", i, kOpNames[o.kind], ms[i] * 1e3, o.flops * 1e-9,
+            ms[i] > 0 ? o.flops / (ms[i] * 1e-3) * 1e-12 : 0.0, mt, N, BN, kb, T, S, H, mode, of32, res);
   }
   fclose(f);
   return 0;

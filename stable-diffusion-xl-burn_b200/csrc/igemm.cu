@@ -289,6 +289,10 @@ int igemm_pick_bn(int m_tiles, int N, int num_sms, bool geglu) {
   // tiles and N = 1280 it fills 128 of 132 SMs where 256 fills 80. The fixed cost of 48 is the least-squares fit of
   // log(time) to waves * (BN + c) over a sweep of every BN at the SDXL step's GEMM shapes on H100 (DESIGN §4).
   (void)geglu;
+  // The one shape the model gets wrong: the base UNet's level-2 QKV (16 M tiles, N = 3840) costs 608 at BN = 256 (2 waves)
+  // against 624 at 160 (3 waves), but 160 took 3.8 % off the whole step on H100 (DESIGN §4, §6). The refiner's level-2 QKV
+  // (N = 4608) and its N = 1536 GEMMs keep the model's choice. The tile width does not change any result.
+  if (m_tiles == 16 && N == 3840) return 160;
   double best = 1e30;
   int best_bn = 0;
   for (int bn : {256, 160, 128, 64}) {
