@@ -221,7 +221,8 @@ SDXL_API double sdxl_unet_plan_flops_executed(const sdxl_unet* unet);
 /* Device time of ONE execution of the current launch plan, summed per kernel kind and measured with CUDA
  * events on the ctx stream (eager launches). Kind index: 0 implicit-GEMM (wgmma), 1 attention, 2 GroupNorm,
  * 3 LayerNorm, 4 GEMV, 5 timestep-embedding, 6 first conv, 7 upsample copy, 8 phase-split copy, 9 f32->f16 cast,
- * 17 T2I-Adapter feature add, 18 PAG identity self-attention, 19 FreeU skip filter and backbone scale.
+ * 17 T2I-Adapter feature add, 18 PAG identity self-attention, 19 FreeU skip filter and backbone scale, 20 device-to-device copy
+ * (DeepCache's feature where FreeU scales it in place).
  * All three arrays hold SDXL_PROFILE_KINDS entries (host). Used by bench.py for the per-kernel roofline. */
 SDXL_API int sdxl_unet_profile_plan(sdxl_unet* unet, double* ms_by_kind_host, double* flops_by_kind_host,
                                     int* launches_by_kind_host);
@@ -663,6 +664,37 @@ typedef struct sdxl_freeu {
  * and its CUDA graph; attaching and detaching rebuild it at the next forward. Attaching or detaching between sdxl_sampler_begin and
  * sdxl_sampler_step requires a new sdxl_sampler_begin. */
 SDXL_API int sdxl_unet_set_freeu(sdxl_unet* unet, const sdxl_freeu* freeu);
+
+/* ---- DeepCache ---------------------------------------------------------------------------------------------
+ * Ma et al., CVPR 2024, uniform schedule (DESIGN.md §17). The UNet has 3 * n_levels input and 3 * n_levels output blocks (9 and 9
+ * for SDXL base, 12 and 12 for the refiner); output block j pops the skip of input block 3 * n_levels - 1 - j. For the branch b and
+ * e = 3 * n_levels - 1 - b:
+ *   full forward    the whole UNet, unchanged. The tensor entering output block e as its backbone input x (the output of output block
+ *                   e - 1, or of the middle block when e = 0, after any ControlNet or T2I-Adapter addition) is kept as the feature,
+ *                   before FreeU scales it.
+ *   cached forward  the time and label MLPs at the current t, the first conv and input blocks 1..b (with the T2I-Adapter features
+ *                   that fall in them), then output blocks e..3 * n_levels - 1 with x = feature at block e (FreeU there if it
+ *                   applies), then the head. The skips are the fresh outputs of input blocks b..0. Each attached ControlNet runs its
+ *                   time and label MLPs, hint, first conv and input blocks 1..b and adds its zero-conv residuals to skips 0..b; its
+ *                   middle residual belongs to the part that is skipped. Image prompts, PAG rows and the inpainting condition act
+ *                   wherever their layers fall in the blocks that run.
+ * Sampling (sdxl_sample_latent, sdxl_sample_latent_scheduled, sdxl_sampler_step and sdxl_sampler_step_host): UNet evaluation j since
+ * the last sdxl_sampler_begin (j = 0, 1, ...) is full when j % interval == 0 and cached otherwise, for every row of the batch. Every
+ * sampling entry point calls sdxl_sampler_begin, so each call's first step is full.
+ * The feature is what the last full forward computed from its inputs: a full forward after a change of the conditioning or of an
+ * attachment's values is what refreshes it. */
+typedef struct sdxl_deepcache {
+  int32_t interval;        /* >= 1: a full forward every interval-th sampler step, cached ones in between; 1 = every step full */
+  int32_t branch;          /* b in [0, 3 * n_levels - 1]: the shallow branch (0 = input_blocks/0 with the last output block) */
+  int32_t forward_cached;  /* direct sdxl_unet_forward*: 1 runs the cached forward on the feature the last full forward kept;
+                              0 runs the full forward, which keeps it; the samplers ignore it */
+} sdxl_deepcache;
+/* Attaches DeepCache to the UNet (NULL detaches). Everything is validated before anything changes: on failure the previous state stays
+ * and the error names the field. A call that changes only interval or forward_cached keeps the launch plan and its CUDA graphs; a new
+ * branch, attaching and detaching rebuild it at the next forward. Attaching or detaching between sdxl_sampler_begin and
+ * sdxl_sampler_step requires a new sdxl_sampler_begin. A cached direct forward is refused when no full forward has kept a feature
+ * since the plan was last built (a new branch, batch or latent size, or any attachment change rebuilds it). */
+SDXL_API int sdxl_unet_set_deepcache(sdxl_unet* unet, const sdxl_deepcache* dc);
 
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),

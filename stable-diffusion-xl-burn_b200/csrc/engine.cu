@@ -186,6 +186,13 @@ struct FreeuAttach {
   float* vals = nullptr;
 };
 
+// DeepCache (sdxl_unet_set_deepcache, DESIGN.md §17): the shallow branch the plan's cached list runs, the sampler's full-step interval
+// and the kind of forward a direct sdxl_unet_forward* runs.
+struct DeepcacheAttach {
+  int branch = 0, interval = 1;
+  bool forward_cached = false;
+};
+
 // Roles of the conditioning rows. The sampler's batch is row groups of n_img rows each: [cond | uncond] with CFG, then a perturbed
 // group with PAG ([cond | uncond | ptb]; the refiner: [cond] or [cond | ptb]). The perturbed rows are conditional rows. n_img = 0:
 // a plain batch, every row conditional.
@@ -253,8 +260,11 @@ struct sdxl_unet : EncoderHalf {
   std::unique_ptr<InpaintAttach> inpaint;   // sdxl_unet_set_inpaint_condition
   std::unique_ptr<PagAttach> pag;           // sdxl_unet_set_pag
   std::unique_ptr<FreeuAttach> freeu;       // sdxl_unet_set_freeu
+  std::unique_ptr<DeepcacheAttach> deepcache;   // sdxl_unet_set_deepcache
   uint64_t plan_builds = 0;
   int plan_ptb = 0;               // trailing rows of the current plan that take PAG's identity self-attentions
+  int plan_dc = -1;               // DeepCache branch of the current plan's cached list (-1: none)
+  bool dc_feature = false;        // a full run of the current plan has kept DeepCache's feature
   RowLayout rows;                 // roles of the conditioning rows
   ~sdxl_unet() {
     if (t_dev) cudaFree(t_dev);
@@ -799,8 +809,10 @@ struct UNetPlanBuilder : PlanBuilder {
   // Time / label MLPs (on the shared timestep embedding te), first conv, input blocks and middle block of UNet::forward
   // (unet/mod.rs:458-482) with the weights of `e` and the conditioning `cond`; every block output is pushed to `saved`, the
   // middle output is returned. hint (nullable): ControlNet hint embedding f32 NHWC [n_hint, h, w, mc] added to the first conv's output.
+  // last_in < in_blocks.size(): DeepCache's shallow branch, which stops after input block last_in and returns null.
   float* encoder(const EncoderHalf& e, const float* te, float* t1, float* semb, float* temb_all,
-                 const Scratch& s, const float* hint, int n_hint, const std::string& prefix, std::vector<Saved>& saved) {
+                 const Scratch& s, const float* hint, int n_hint, const std::string& prefix, std::vector<Saved>& saved,
+                 size_t last_in) {
     const sdxl_unet_cfg& g = e.cfg;
     const int mc = g.model_channels, ted = 4 * mc, temb_total = e.temb_all.N;
     gemv(te, 0, 1, e.t1, nullptr, 0, 0, 1, t1, 0);
@@ -823,7 +835,7 @@ struct UNetPlanBuilder : PlanBuilder {
     saved.push_back({x, Cx, H, W});
     // an attached T2I-Adapter adds its features in the UNet's own encoder (a ControlNet's does not see them)
     const bool t2i = u->t2i && cond == &u->cond;
-    for (size_t i = 1; i < e.in_blocks.size() && !err; ++i) {
+    for (size_t i = 1; i < e.in_blocks.size() && i <= last_in && !err; ++i) {
       const Block& b = e.in_blocks[i];
       begin_block(prefix + "input_blocks/" + std::to_string(i));
       if (b.type == BT_RES || b.type == BT_REST) {
@@ -850,6 +862,7 @@ struct UNetPlanBuilder : PlanBuilder {
       end_block();
       saved.push_back({x, Cx, H, W});
     }
+    if (last_in < e.in_blocks.size()) return nullptr;
     // --- middle
     begin_block(prefix + "middle_block");
     x = resblock(e.mid_res1, x, Cx, nullptr, 0, H, W, temb_all, temb_total, s.gn1, s.raw, s.h, s.gn2);
@@ -1020,7 +1033,155 @@ struct UNetPlanBuilder : PlanBuilder {
 
 
 
-// Builds the op list for UNet::forward (reference unet/mod.rs:449-493) at batch Bf, latent h x w.
+// Transformer blocks that run before output block e in a full forward: the index of e's first one in UNet::tblocks (list_tblocks).
+static int tblocks_before_output(const sdxl_unet* u, size_t e) {
+  size_t n = u->mid_st.blocks.size();
+  for (const Block& b : u->in_blocks) n += b.st.blocks.size();
+  for (size_t i = 0; i < e; ++i) n += u->out_blocks[i].st.blocks.size();
+  return (int)n;
+}
+
+// Buffers that every op list of a plan shares (build_plan_ops).
+struct UNetPlanShared {
+  UNetPlanBuilder::Scratch scr;
+  float *te, *t1, *semb, *temb_all;
+  const float* freeu_tw[2] = {nullptr, nullptr};   // FreeU's twiddles of the two deepest levels, made by the first list
+};
+
+// Emits one forward into B's op list. branch < 0: no DeepCache. Full list (cached false): UNet::forward (reference
+// unet/mod.rs:449-493); with a branch, the backbone input of output block e = 3 * n_levels - 1 - branch is kept in `feature` (a copy
+// made before FreeU scales it in place, when FreeU runs there). Cached list: the shallow branch on `feature` (DESIGN.md §17).
+static int plan_forward(sdxl_unet* u, UNetPlanBuilder& B, UNetPlanShared& sh, int branch, bool cached, UNetPlanBuilder::Saved& feature) {
+  sdxl_ctx* c = u->ctx;
+  const sdxl_unet_cfg& g = u->cfg;
+  Plan* P = B.P;
+  Arena* A = B.A;
+  const int Bf = P->Bf, mc = g.model_channels, ted = 4 * mc;
+  const int temb_total = u->temb_all.N;
+  const int levels = g.n_levels;
+  const size_t n_out = u->out_blocks.size();
+  const size_t e = branch >= 0 ? n_out - 1 - (size_t)branch : 0;
+  const size_t last_in = cached ? (size_t)branch : SIZE_MAX;   // the encoder's bound: SIZE_MAX runs all of it
+  const UNetPlanBuilder::Scratch& scr = sh.scr;
+  float *te = sh.te, *t1 = sh.t1, *semb = sh.semb, *temb_all = sh.temb_all;
+
+  // --- embeddings (unet/mod.rs:458-468): emb = time_mlp(temb(t)) + label_emb; only SiLU(emb) is consumed
+  {
+    Op op{};
+    op.kind = OP_TEMB;
+    op.te = {(const float*)(u->t_dev + 1), 1, mc, te};
+    P->ops.push_back(op);
+  }
+  // --- embeddings, input blocks, middle
+  using Saved = UNetPlanBuilder::Saved;
+  std::vector<Saved> saved;
+  B.cond = &u->cond;
+  float* x = B.encoder(*u, te, t1, semb, temb_all, scr, nullptr, 1, "", saved, last_in);
+  int H = saved.back().H, W = saved.back().W, Cx = saved.back().C;
+  // --- ControlNets (DESIGN.md §8): each runs its own encoder on the same inputs, then skip_i += s * zero_conv_i(h_i) and
+  // mid += s * middle_block_out(mid_c), in attachment order. The UNet's own encoder above is untouched. The cached list has no middle.
+  for (size_t k = 0; k < u->controls.size() && !B.err; ++k) {
+    const ControlAttach& a = *u->controls[k];
+    const EncoderHalf& en = *a.net;
+    const std::string prefix = "control" + std::to_string(k) + "/";
+    const int kv_unet = B.kv_index;
+    B.cond = &a.cond;
+    B.kv_index = 0;
+    float* ct1 = B.buf<float>(ted);
+    float* csemb = B.buf<float>((size_t)Bf * ted);
+    float* ctemb = B.buf<float>((size_t)Bf * en.temb_all.N);
+    std::vector<Saved> cs;
+    float* cmid = B.encoder(en, te, ct1, csemb, ctemb, scr, a.hint_emb, a.ext.n, prefix, cs, last_in);
+    B.cond = &u->cond;
+    B.kv_index = kv_unet;
+    if (cs.size() != saved.size() || a.zero.size() != u->in_blocks.size() + 1) return fail(c, 5006, "control %zu: skip count mismatch", k);
+    B.begin_block(prefix + "zero_convs");
+    for (size_t i = 0; i < saved.size(); ++i) B.zero_conv(cs[i], saved[i], a.zero[i], scr.raw);
+    if (!cached) B.zero_conv({cmid, Cx, H, W}, {x, Cx, H, W}, a.zero.back(), scr.raw);
+    B.end_block();
+  }
+  // --- FreeU's twiddle tables of the two deepest levels, computed on the host (freeu_twiddles) into the plan's workspace
+  for (int k = 0; k < 2 && u->freeu && !sh.freeu_tw[k] && levels - 1 - k >= 0; ++k) {
+    const int th = P->h >> (levels - 1 - k), tw = P->w >> (levels - 1 - k);
+    float* d = B.buf<float>((size_t)2 * (th + tw));
+    if (B.err) return B.err;
+    if (!A->measure) {
+      std::vector<float> host((size_t)2 * (th + tw));
+      freeu_twiddles(th, tw, host.data());
+      CU(c, cudaMemcpyAsync(d, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
+      CU(c, cudaStreamSynchronize(c->stream));
+    }
+    sh.freeu_tw[k] = d;
+  }
+  if (cached) {   // the deep part is the kept feature
+    x = feature.p; Cx = feature.C; H = feature.H; W = feature.W;
+    B.kv_index = tblocks_before_output(u, e);
+  }
+  // DeepCache's copy of a feature that FreeU scales in place: made in the full list, and in the cached list for FreeU to scale
+  auto copy = [&](const Saved& src) -> Saved {
+    const size_t n = (size_t)Bf * src.H * src.W * src.C;
+    float* d = B.buf<float>(n);
+    if (!B.err) {
+      Op op{};
+      op.kind = OP_COPY;
+      op.cp = {src.p, d, n * sizeof(float)};
+      P->ops.push_back(op);
+    }
+    return {d, src.C, src.H, src.W};
+  };
+  // --- output blocks: cat([x, saved.pop()], channel) is never materialised (GN + skip conv read both)
+  for (size_t i = cached ? e : 0; i < n_out && !B.err; ++i) {
+    const Block& b = u->out_blocks[i];
+    if (saved.empty()) return fail(c, 5004, "skip stack underflow");
+    Saved sk = saved.back();
+    saved.pop_back();
+    if (sk.H != H || sk.W != W || Cx + sk.C != b.res.Cin) return fail(c, 5005, "skip shape mismatch at output block %zu", i);
+    B.begin_block("output_blocks/" + std::to_string(i));
+    // FreeU: the output blocks of the two deepest levels (diffusers' up_blocks[0] and [1]: three each, output block i is at level
+    // n_levels - 1 - i / 3), after the ControlNet residuals were added to the skips
+    const int k = (int)(i / 3);
+    const bool fu = u->freeu && k < 2 && k < levels;
+    if (branch >= 0 && i == e) {
+      if (cached && fu) x = copy(feature).p;
+      else if (!cached) feature = fu ? copy({x, Cx, H, W}) : Saved{x, Cx, H, W};
+    }
+    if (fu) {
+      if (H != P->h >> (levels - 1 - k) || W != P->w >> (levels - 1 - k))
+        return fail(c, 5024, "FreeU: output block %zu is not at level %d", i, levels - 1 - k);
+      B.freeu(sk, x, Cx, k, sh.freeu_tw[k]);
+    }
+    x = B.resblock(b.res, x, Cx, sk.p, sk.C, H, W, temb_all, temb_total, scr.gn1, scr.raw, scr.h, scr.gn2);
+    Cx = b.res.Cout;
+    if (b.type == BT_REST || b.type == BT_RESTU) x = B.strans(b.st, x, H, W, scr.a16, scr.tok, scr.qkv, scr.ao, scr.q, scr.ff);
+    if (b.type == BT_RESTU || b.type == BT_RESU) {
+      // nearest-2x then 3x3 conv (unet/mod.rs:742-751), as four 2x2 phase convolutions of the source image
+      __half* x16 = B.buf<__half>((size_t)Bf * H * W * Cx);
+      float* y = B.buf<float>((size_t)Bf * 4 * H * W * Cx);
+      B.upconv(x, Bf, H, W, b.conv, x16, y);
+      H *= 2; W *= 2;
+      x = y;
+    }
+    B.end_block();
+  }
+  if (B.err) return B.err;
+  B.begin_block("norm_out+conv_out");
+  // --- head: GN -> SiLU -> conv 3x3 (unet/mod.rs:488-490)
+  B.gn(x, Cx, nullptr, 0, H * W, u->norm_out, 1, scr.gn1, nullptr);
+  if (!B.err && !P->ops.empty()) P->ops.back().gn.y_lo = scr.raw;   // rounding residue of the normalised activation (hi/lo split)
+  {
+    ActView a{scr.gn1, Bf, H, W, Cx}, alo{scr.raw, Bf, H, W, Cx};
+    std::vector<IgemmSeg> segs = conv_taps(3, u->conv_out.Ipad / 64, 0), lo = conv_taps(3, u->conv_out.Ipad / 64, 1);
+    segs.insert(segs.end(), lo.begin(), lo.end());   // K = [9 taps on hi | 9 taps on lo], weights [W | W]
+    B.igemm(a, &alo, segs, u->conv_out_w2, u->conv_out.O, 2 * u->conv_out.Ktot, H, W, Bf, IGEMM_LINEAR, 0, P->eps, 1, P->eps_ld,
+            u->conv_out.b, 0, nullptr, 0);
+    B.add_flops(2.0 * Bf * H * W * 9.0 * Cx * u->conv_out.O);
+  }
+  B.end_block();
+  return B.err;
+}
+
+// Builds the op list for UNet::forward at batch Bf, latent h x w and, with DeepCache attached, the cached list (Plan::cached) after
+// it, over the same shared buffers.
 static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
@@ -1029,6 +1190,7 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
   P->ops.clear();
   P->block_names.clear();
   P->flops = 0;
+  P->cached.reset();
   const int Bf = P->Bf, mc = g.model_channels, ted = 4 * mc;
   const int temb_total = u->temb_all.N;
   const int levels = g.n_levels;
@@ -1039,10 +1201,11 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
   P->eps = B.buf<float>((size_t)Bf * P->h * P->w * P->eps_ld);
   B.gn_partial = B.buf<float>(gn_scratch_floats(Bf, 32));
   if (B.gn_partial && !A->measure && gn_scratch_init(c->stream, B.gn_partial, Bf, 32)) return fail(c, 5007, "GroupNorm scratch init failed");
-  float* te = B.buf<float>(mc);
-  float* t1 = B.buf<float>(ted);
-  float* semb = B.buf<float>((size_t)Bf * ted);
-  float* temb_all = B.buf<float>((size_t)Bf * temb_total);
+  UNetPlanShared sh;
+  sh.te = B.buf<float>(mc);
+  sh.t1 = B.buf<float>(ted);
+  sh.semb = B.buf<float>((size_t)Bf * ted);
+  sh.temb_all = B.buf<float>((size_t)Bf * temb_total);
 
   // maxima for the shared scratch buffers over the ResBlocks and transformers of the block program, each at its level
   size_t max_pixC_cat = 0, max_pixC = 0, max_tokC = 0;
@@ -1070,101 +1233,21 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
   __half* s_q = B.buf<__half>(Bf * max_tokC);
   __half* s_ff = B.buf<__half>(Bf * max_tokC * 4);
   if (B.err) return B.err;
-  const UNetPlanBuilder::Scratch scr{s_gn1, s_raw, s_h, s_gn2, s_a16, s_tok, s_qkv, s_ao, s_q, s_ff};
+  sh.scr = {s_gn1, s_raw, s_h, s_gn2, s_a16, s_tok, s_qkv, s_ao, s_q, s_ff};
 
-  // --- embeddings (unet/mod.rs:458-468): emb = time_mlp(temb(t)) + label_emb; only SiLU(emb) is consumed
-  {
-    Op op{};
-    op.kind = OP_TEMB;
-    op.te = {(const float*)(u->t_dev + 1), 1, mc, te};
-    P->ops.push_back(op);
-  }
-  // --- embeddings, input blocks, middle
-  using Saved = UNetPlanBuilder::Saved;
-  std::vector<Saved> saved;
-  B.cond = &u->cond;
-  float* x = B.encoder(*u, te, t1, semb, temb_all, scr, nullptr, 1, "", saved);
-  int H = saved.back().H, W = saved.back().W, Cx = saved.back().C;
-  // --- ControlNets (DESIGN.md §8): each runs its own encoder on the same inputs, then skip_i += s * zero_conv_i(h_i) and
-  // mid += s * middle_block_out(mid_c), in attachment order. The UNet's own encoder above is untouched.
-  for (size_t k = 0; k < u->controls.size() && !B.err; ++k) {
-    const ControlAttach& a = *u->controls[k];
-    const EncoderHalf& e = *a.net;
-    const std::string prefix = "control" + std::to_string(k) + "/";
-    const int kv_unet = B.kv_index;
-    B.cond = &a.cond;
-    B.kv_index = 0;
-    float* ct1 = B.buf<float>(ted);
-    float* csemb = B.buf<float>((size_t)Bf * ted);
-    float* ctemb = B.buf<float>((size_t)Bf * e.temb_all.N);
-    std::vector<Saved> cs;
-    float* cmid = B.encoder(e, te, ct1, csemb, ctemb, scr, a.hint_emb, a.ext.n, prefix, cs);
-    B.cond = &u->cond;
-    B.kv_index = kv_unet;
-    if (cs.size() != saved.size() || a.zero.size() != saved.size() + 1) return fail(c, 5006, "control %zu: skip count mismatch", k);
-    B.begin_block(prefix + "zero_convs");
-    for (size_t i = 0; i < saved.size(); ++i) B.zero_conv(cs[i], saved[i], a.zero[i], s_raw);
-    B.zero_conv({cmid, Cx, H, W}, {x, Cx, H, W}, a.zero.back(), s_raw);
-    B.end_block();
-  }
-  // --- FreeU's twiddle tables of the two deepest levels, computed on the host (freeu_twiddles) into the plan's workspace
-  const float* freeu_tw[2] = {nullptr, nullptr};
-  for (int k = 0; k < 2 && u->freeu && levels - 1 - k >= 0; ++k) {
-    const int th = P->h >> (levels - 1 - k), tw = P->w >> (levels - 1 - k);
-    float* d = B.buf<float>((size_t)2 * (th + tw));
-    if (B.err) return B.err;
-    if (!A->measure) {
-      std::vector<float> host((size_t)2 * (th + tw));
-      freeu_twiddles(th, tw, host.data());
-      CU(c, cudaMemcpyAsync(d, host.data(), host.size() * sizeof(float), cudaMemcpyHostToDevice, c->stream));
-      CU(c, cudaStreamSynchronize(c->stream));
-    }
-    freeu_tw[k] = d;
-  }
-  // --- output blocks: cat([x, saved.pop()], channel) is never materialised (GN + skip conv read both)
-  for (size_t i = 0; i < u->out_blocks.size() && !B.err; ++i) {
-    const Block& b = u->out_blocks[i];
-    if (saved.empty()) return fail(c, 5004, "skip stack underflow");
-    Saved sk = saved.back();
-    saved.pop_back();
-    if (sk.H != H || sk.W != W || Cx + sk.C != b.res.Cin) return fail(c, 5005, "skip shape mismatch at output block %zu", i);
-    B.begin_block("output_blocks/" + std::to_string(i));
-    // FreeU: the output blocks of the two deepest levels (diffusers' up_blocks[0] and [1]: three each, output block i is at level
-    // n_levels - 1 - i / 3), after the ControlNet residuals were added to the skips
-    const int k = (int)(i / 3);
-    if (u->freeu && k < 2 && k < levels) {
-      if (H != P->h >> (levels - 1 - k) || W != P->w >> (levels - 1 - k))
-        return fail(c, 5024, "FreeU: output block %zu is not at level %d", i, levels - 1 - k);
-      B.freeu(sk, x, Cx, k, freeu_tw[k]);
-    }
-    x = B.resblock(b.res, x, Cx, sk.p, sk.C, H, W, temb_all, temb_total, s_gn1, s_raw, s_h, s_gn2);
-    Cx = b.res.Cout;
-    if (b.type == BT_REST || b.type == BT_RESTU) x = B.strans(b.st, x, H, W, s_a16, s_tok, s_qkv, s_ao, s_q, s_ff);
-    if (b.type == BT_RESTU || b.type == BT_RESU) {
-      // nearest-2x then 3x3 conv (unet/mod.rs:742-751), as four 2x2 phase convolutions of the source image
-      __half* x16 = B.buf<__half>((size_t)Bf * H * W * Cx);
-      float* y = B.buf<float>((size_t)Bf * 4 * H * W * Cx);
-      B.upconv(x, Bf, H, W, b.conv, x16, y);
-      H *= 2; W *= 2;
-      x = y;
-    }
-    B.end_block();
-  }
-  if (B.err) return B.err;
-  B.begin_block("norm_out+conv_out");
-  // --- head: GN -> SiLU -> conv 3x3 (unet/mod.rs:488-490)
-  B.gn(x, Cx, nullptr, 0, H * W, u->norm_out, 1, s_gn1, nullptr);
-  if (!B.err && !P->ops.empty()) P->ops.back().gn.y_lo = s_raw;   // rounding residue of the normalised activation (hi/lo split)
-  {
-    ActView a{s_gn1, Bf, H, W, Cx}, alo{s_raw, Bf, H, W, Cx};
-    std::vector<IgemmSeg> segs = conv_taps(3, u->conv_out.Ipad / 64, 0), lo = conv_taps(3, u->conv_out.Ipad / 64, 1);
-    segs.insert(segs.end(), lo.begin(), lo.end());   // K = [9 taps on hi | 9 taps on lo], weights [W | W]
-    B.igemm(a, &alo, segs, u->conv_out_w2, u->conv_out.O, 2 * u->conv_out.Ktot, H, W, Bf, IGEMM_LINEAR, 0, P->eps, 1, P->eps_ld,
-            u->conv_out.b, 0, nullptr, 0);
-    B.add_flops(2.0 * Bf * H * W * 9.0 * Cx * u->conv_out.O);
-  }
-  B.end_block();
-  return B.err;
+  const int branch = u->deepcache ? u->deepcache->branch : -1;
+  UNetPlanBuilder::Saved feature{};
+  if (int r = plan_forward(u, B, sh, branch, false, feature)) return r;
+  if (branch < 0) return 0;
+  // DeepCache's cached list: its own ops, graph and run count; every buffer from this plan's arena
+  P->cached.reset(new Plan());
+  Plan* Q = P->cached.get();
+  Q->Bf = P->Bf; Q->Bx = P->Bx; Q->h = P->h; Q->w = P->w;
+  Q->x_in = P->x_in; Q->eps = P->eps; Q->eps_ld = P->eps_ld;
+  UNetPlanBuilder Bc{{c, Q, A, Bf}, u};
+  Bc.Bp = Bp;
+  Bc.gn_partial = B.gn_partial;
+  return plan_forward(u, Bc, sh, branch, true, feature);
 }
 
 // Whether every attachment fits a run of n_img images on an h x w latent: it was made for that latent, and n_img is a multiple of
@@ -1203,15 +1286,35 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w, int Bp) {
     for (const IpPrompt& a : u->ip->prompts)
       if (a.cond.condB != Bf) return fail(c, 5014, "image prompt: its K/V are hoisted for batch %d but the batch is %d", a.cond.condB, Bf);
   if (int r = attachments_fit(u, Bx, h, w)) return r;
-  // every change of the buffers or attachments a plan reads drops the plan, so the shapes and the perturbed rows are its whole cache key
-  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan_ptb == Bp) return 0;
+  // every change of the buffers or attachments a plan reads drops the plan, so the shapes, the perturbed rows and the DeepCache
+  // branch are its whole cache key
+  const int dc = u->deepcache ? u->deepcache->branch : -1;
+  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan_ptb == Bp && u->plan_dc == dc)
+    return 0;
+  u->dc_feature = false;
   if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A, Bp); })) return r;
   u->plan_ptb = Bp;
+  u->plan_dc = dc;
   u->plan_builds++;
   return 0;
 }
 
-static int run_plan(sdxl_unet* u) { return run_plan_ops(u->ctx, u->plan.get()); }
+// Refuses DeepCache's cached forward until a full run of the current plan has kept the feature it reads.
+static int cached_ready(sdxl_unet* u) {
+  if (u->plan && u->plan->cached && u->dc_feature) return 0;
+  return fail(u->ctx, 5025, "DeepCache: no full forward has kept a feature since the plan was built (run one with forward_cached = 0)");
+}
+
+// Runs the plan's full list, which keeps DeepCache's feature when it is attached, or (cached) its cached list on that feature.
+static int run_plan(sdxl_unet* u, bool cached = false) {
+  if (cached) {
+    if (int r = cached_ready(u)) return r;
+    return run_plan_ops(u->ctx, u->plan->cached.get());
+  }
+  const int r = run_plan_ops(u->ctx, u->plan.get());
+  u->dc_feature = !r && u->plan->cached;
+  return r;
+}
 
 static int set_t(sdxl_unet* u, double t) {
   sdxl_ctx* c = u->ctx;
@@ -2269,6 +2372,30 @@ extern "C" int sdxl_unet_set_freeu(sdxl_unet* u, const sdxl_freeu* f) {
 }
 
 // ================================================================================================
+// DeepCache (include/sdxl_b200.h: sdxl_unet_set_deepcache; DESIGN.md §17)
+// ================================================================================================
+extern "C" int sdxl_unet_set_deepcache(sdxl_unet* u, const sdxl_deepcache* d) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  if (!d) return attach_detach(u, u->deepcache);
+  // validate everything first: on failure the attached state is unchanged
+  const int n = (int)u->out_blocks.size();
+  if (d->interval < 1) return fail(c, 4990, "set_deepcache: interval = %d must be >= 1", d->interval);
+  if (d->branch < 0 || d->branch >= n) return fail(c, 4991, "set_deepcache: branch = %d outside [0, %d]", d->branch, n - 1);
+  if (d->forward_cached != 0 && d->forward_cached != 1)
+    return fail(c, 4992, "set_deepcache: forward_cached = %d must be 0 or 1", d->forward_cached);
+  if (!u->deepcache || u->deepcache->branch != d->branch) {   // a new branch changes the plan; the interval and the forward kind do not
+    std::unique_ptr<DeepcacheAttach> fresh(new DeepcacheAttach());
+    fresh->branch = d->branch;
+    if (int r = attach_install(u, u->deepcache, std::move(fresh))) return r;
+  }
+  u->deepcache->interval = d->interval;
+  u->deepcache->forward_cached = d->forward_cached != 0;
+  return 0;
+}
+
+// ================================================================================================
 // UNet::forward
 // ================================================================================================
 extern "C" int sdxl_unet_forward(sdxl_unet* u, int B, int h, int w, const sdxl_half* x, int32_t t_host, sdxl_half* eps_out) {
@@ -2277,10 +2404,12 @@ extern "C" int sdxl_unet_forward(sdxl_unet* u, int B, int h, int w, const sdxl_h
   CU(c, cudaSetDevice(c->device));
   int r = ensure_plan(u, B, B, h, w, u->pag ? u->pag->forward_rows : 0);
   if (r) return r;
+  const bool cached = u->deepcache && u->deepcache->forward_cached;
+  if (cached && (r = cached_ready(u))) return r;
   Plan* P = u->plan.get();
   KL(c, cast_f16_to_f32_launch(c->stream, (const __half*)x, (size_t)B * latent_channels(u->cfg) * h * w, P->x_in));
   if ((r = set_t(u, t_host))) return r;
-  if ((r = run_plan(u))) return r;
+  if ((r = run_plan(u, cached))) return r;
   KL(c, nhwc_to_nchw_f16_launch(c->stream, P->eps, B, h * w, u->cfg.out_channels, P->eps_ld, (__half*)eps_out));
   return 0;
 }
@@ -2295,10 +2424,12 @@ extern "C" int sdxl_unet_forward_f32_at(sdxl_unet* u, int B, int h, int w, const
     return fail(c, 5024, "forward: timestep %g outside [0, %d]", t_host, u->cfg.n_steps - 1);
   int r = ensure_plan(u, B, B, h, w, u->pag ? u->pag->forward_rows : 0);
   if (r) return r;
+  const bool cached = u->deepcache && u->deepcache->forward_cached;
+  if (cached && (r = cached_ready(u))) return r;
   Plan* P = u->plan.get();
   CU(c, cudaMemcpyAsync(P->x_in, x, (size_t)B * latent_channels(u->cfg) * h * w * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
   if ((r = set_t(u, t_host))) return r;
-  if ((r = run_plan(u))) return r;
+  if ((r = run_plan(u, cached))) return r;
   KL(c, nhwc_to_nchw_f32_launch(c->stream, P->eps, B, h * w, u->cfg.out_channels, P->eps_ld, eps_out));
   return 0;
 }
@@ -2336,6 +2467,7 @@ extern "C" double sdxl_unet_plan_flops_executed(const sdxl_unet* u) {
 struct Sampler {
   int Bimg = 0, nfwd = 1, h = 0, w = 0, n_ctx = 0;   // nfwd: row groups of Bimg rows, [cond | uncond] or [cond], then [ptb] with PAG
   bool cfg = false, pag = false;
+  int evals = 0;           // UNet evaluations since sampler_begin (DeepCache: evaluation j is full when j % interval == 0)
   float guidance = 1.f;
   float* noise = nullptr;  // scratch [Bimg,4,h,w]
   float* xh = nullptr;     // scheduled samplers: the state x / sqrt(alpha) and the previous step's denoised latent (DPM++ 2M)
@@ -2400,6 +2532,7 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
   S->guidance = (float)guidance;
   S->cfg = use_cfg;
   S->pag = pag;
+  S->evals = 0;
   const cudaMemcpyKind kind = cond->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
   const size_t ctx_row = (size_t)n_ctx * g.context_dim * 2, y_row = (size_t)g.adm_in_channels * 2;
   CU(c, cudaMemcpyAsync(S->cond_ctx, ctx_c, ctx_row * Bimg, kind, c->stream));
@@ -2422,6 +2555,15 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
   return 0;
 }
 
+// One UNet evaluation of a sampling loop: with DeepCache, the full list on every interval-th evaluation since sampler_begin and the
+// cached list between.
+static int run_sampler_plan(sdxl_unet* u) {
+  Sampler* S = u->sampler.get();
+  const int r = run_plan(u, u->deepcache && S->evals % u->deepcache->interval != 0);
+  if (!r) S->evals++;
+  return r;
+}
+
 // one loop-body iteration (reference stablediffusion/mod.rs:406-429)
 static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   sdxl_ctx* c = u->ctx;
@@ -2433,7 +2575,7 @@ static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   const double ap = t_prev >= 0 ? u->alphas[t_prev] : 1.0;
   int r = set_t(u, t);
   if (r) return r;
-  if ((r = run_plan(u))) return r;
+  if ((r = run_sampler_plan(u))) return r;
   if (S->pag) {
     // diffusers' adaptive scaling: p_t = max(scale - adaptive * (n_steps - t), 0)
     const PagAttach& pg = *u->pag;
@@ -2656,7 +2798,7 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
   p.eps = P->eps; p.ld = P->eps_ld; p.use_cfg = S->cfg; p.use_pag = S->pag; p.guidance = S->guidance;
   for (int k = k0; k < k1; ++k) {
     if ((r = set_t(u, ts[k]))) return r;
-    if ((r = run_plan(u))) return r;
+    if ((r = run_sampler_plan(u))) return r;
     const StepCoef q = step_coef(*sch, k, ts.data(), sig.data(), k > k0);
     p.sigma = (float)sig[k];
     p.cx = q.cx; p.cd = q.cd; p.ch = q.ch; p.cn = q.cn; p.c_in = q.c_in;

@@ -458,12 +458,12 @@ static int build_two_pass(M* m, const PackView& pv, int (*build)(M*, const PackV
 // ================================================================================================
 enum OpKind { OP_IGEMM, OP_ATTN, OP_GN, OP_LN, OP_GEMV, OP_TEMB, OP_CONV_IN, OP_UPS, OP_PHASE, OP_CAST16,
               OP_SOFTMAX, OP_TRANSPOSE, OP_PQ, OP_EMBED, OP_ATTN_SMALL, OP_ACT, OP_LN_GATHER, OP_T2I_ADD, OP_PAG_IDENTITY, OP_FREEU,
-              OP_KIND_COUNT };
+              OP_COPY, OP_KIND_COUNT };
 // the public profile entry points take caller arrays of SDXL_PROFILE_KINDS entries (include/sdxl_b200.h)
 static_assert(OP_KIND_COUNT <= SDXL_PROFILE_KINDS, "profile arrays too small for the op kinds");
 static const char* const kOpNames[] = {"igemm", "attention", "group_norm", "layer_norm", "gemv", "temb", "conv_in", "upsample",
                                        "phase_split", "cast16", "softmax_rows", "transpose16", "post_quant", "embed_tokens",
-                                       "attention_small", "mlp_act", "ln_gather", "t2i_add", "pag_identity", "freeu"};
+                                       "attention_small", "mlp_act", "ln_gather", "t2i_add", "pag_identity", "freeu", "copy"};
 static_assert(sizeof(kOpNames) / sizeof(kOpNames[0]) == OP_KIND_COUNT, "one name per op kind");
 struct Op {
   OpKind kind;
@@ -492,6 +492,7 @@ struct Op {
   struct { float* x; const float* F; long per_img; int B, n_hint; const int* t; const int* t_min; } ta;
   struct { const __half* qkv; int C; long rows; __half* out; } pi;   // PAG identity self-attention (pag_identity_launch)
   struct { float* r; int C; float* x; int Cx, B, H, W; const float* tw; const float* s; const float* b; } fu;   // FreeU (freeu_launch)
+  struct { const void* src; void* dst; size_t bytes; } cp;   // device-to-device copy (a memcpy node in the graph)
 };
 
 struct Plan {
@@ -506,6 +507,9 @@ struct Plan {
   int runs = 0;
   double flops = 0;  // algorithmic FLOPs of one run (2*MAC over Linear/conv/attention)
   std::vector<std::string> block_names;   // reference blocks in execution order (input_blocks/3, middle_block, ...)
+  // DeepCache's cached forward (engine.cu, DESIGN.md §17): a second op list with its own graph and run count over this plan's
+  // buffers. Its arena stays empty; its shapes, x_in and eps are this plan's.
+  std::unique_ptr<Plan> cached;
   ~Plan() {
     if (gexec) cudaGraphExecDestroy(gexec);
     if (graph) cudaGraphDestroy(graph);
@@ -728,6 +732,7 @@ static int exec_op(sdxl_ctx* c, Op& op) {
     case OP_FREEU:
       KL(c, freeu_launch(st, op.fu.r, op.fu.C, op.fu.x, op.fu.Cx, op.fu.B, op.fu.H, op.fu.W, op.fu.tw, op.fu.s, op.fu.b));
       break;
+    case OP_COPY: KL(c, (int)cudaMemcpyAsync(op.cp.dst, op.cp.src, op.cp.bytes, cudaMemcpyDeviceToDevice, st)); break;
   }
   return 0;
 }

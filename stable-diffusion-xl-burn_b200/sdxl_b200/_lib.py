@@ -120,6 +120,10 @@ class Freeu(C.Structure):
     _fields_ = [("s1", C.c_float), ("s2", C.c_float), ("b1", C.c_float), ("b2", C.c_float)]
 
 
+class Deepcache(C.Structure):
+    _fields_ = [("interval", C.c_int32), ("branch", C.c_int32), ("forward_cached", C.c_int32)]
+
+
 class Schedule(C.Structure):
     _fields_ = [("sampler", C.c_int32), ("spacing", C.c_int32), ("n_steps", C.c_int32), ("first_step", C.c_int32),
                 ("last_step", C.c_int32), ("renoise", C.c_int32), ("no_cfg", C.c_int32), ("karras_rho", C.c_float),
@@ -214,6 +218,7 @@ PROTOTYPES = {
     "sdxl_unet_num_self_attentions": (I, [P]),
     "sdxl_unet_set_pag": (I, [P, C.POINTER(Pag)]),
     "sdxl_unet_set_freeu": (I, [P, C.POINTER(Freeu)]),
+    "sdxl_unet_set_deepcache": (I, [P, C.POINTER(Deepcache)]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),
     "sdxl_mpk_encode_u16": (C.c_size_t, [P, C.c_size_t, P]),

@@ -411,6 +411,25 @@ class Diffuser:
             s.s1, s.s2, s.b1, s.b2 = float(s1), float(s2), float(b1), float(b2)
         self.ctx.call("sdxl_unet_set_freeu", self.ctx.lib.sdxl_unet_set_freeu, self.h, None if s is None else C.byref(s))
 
+    def set_deepcache(self, interval: Optional[int], branch: int = 0) -> None:
+        """Attaches DeepCache (sdxl_unet_set_deepcache, DESIGN.md §17; Ma et al. 2024, uniform schedule): every sampling call runs the
+        whole UNet on its first step and every interval-th one after it, and on the steps between only the shallow branch (the first
+        conv and input blocks 1..branch, then the last branch + 1 output blocks and the head) on the deep feature the last full step
+        kept. interval None detaches. Direct unet_forward calls run the full forward unless unet_forward(cached=True)."""
+        if interval is None:
+            self._deepcache = None
+            self._set_deepcache(None)
+            return
+        self._set_deepcache((int(interval), int(branch), 0))
+        self._deepcache = (int(interval), int(branch))
+
+    def _set_deepcache(self, d) -> None:
+        s = None
+        if d is not None:
+            s = _lib.Deepcache()
+            s.interval, s.branch, s.forward_cached = d
+        self.ctx.call("sdxl_unet_set_deepcache", self.ctx.lib.sdxl_unet_set_deepcache, self.h, None if s is None else C.byref(s))
+
     @classmethod
     def from_diffusers_dir(cls, ctx: Context, path: str) -> "Diffuser":
         """A diffusers UNet2DConditionModel directory (the `unet/` folder of an SDXL pipeline, base or inpainting): config.json +
@@ -428,11 +447,20 @@ class Diffuser:
         self._keep = (context, label)
 
     def unet_forward(self, x: torch.Tensor, timesteps, context: Optional[torch.Tensor] = None,
-                     label: Optional[torch.Tensor] = None, perturbed_rows: Optional[int] = None) -> torch.Tensor:
+                     label: Optional[torch.Tensor] = None, perturbed_rows: Optional[int] = None,
+                     cached: Optional[bool] = None) -> torch.Tensor:
         """== UNet::forward(x [B,4,h,w], timesteps Int[1], context [B,77,Cctx], label [B,adm]).
         f32 in -> f32 out (no I/O rounding), f16 in -> f16 out (the reference's tensors). perturbed_rows (PAG attached, set_pag): the
-        last this-many rows of the batch run the attached layers' identity self-attention, from this forward on (0: none)."""
+        last this-many rows of the batch run the attached layers' identity self-attention, from this forward on (0: none). cached
+        (DeepCache attached, set_deepcache): True runs the cached forward on the feature the last full forward kept, False the full
+        forward, from this forward on."""
         ctx = self.ctx
+        if cached is not None:
+            if getattr(self, "_deepcache", None) is None:
+                if cached:
+                    raise SdxlError("unet_forward: cached needs DeepCache attached (set_deepcache)")
+            else:
+                self._set_deepcache((*self._deepcache, int(bool(cached))))
         if perturbed_rows is not None:
             if getattr(self, "_pag", None) is None:
                 if perturbed_rows:
@@ -470,7 +498,7 @@ class Diffuser:
     KIND_NAMES = ["igemm_wgmma", "attention_wgmma", "group_norm", "layer_norm", "gemv", "timestep_embedding",
                   "conv_in", "upsample2x", "phase_split", "cast_f16"]
     # kinds only the UNet plan launches, by kind index (KIND_NAMES is positional and LatentDecoder.KIND_NAMES extends it)
-    UNET_KINDS = {17: "t2i_add", 18: "pag_identity", 19: "freeu"}
+    UNET_KINDS = {17: "t2i_add", 18: "pag_identity", 19: "freeu", 20: "copy"}
 
     def profile_plan(self) -> Dict[str, Dict[str, float]]:
         """Per-kernel-kind device time (ms), algorithmic FLOPs and launch count of one plan execution."""
