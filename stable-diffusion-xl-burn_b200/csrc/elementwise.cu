@@ -424,10 +424,13 @@ int nhwc_to_nchw_f16_launch(cudaStream_t st, const float* x, int B, int HW, int 
 // ------------------------------------------------------------------------------------------------
 // sampler elementwise math. All latents are f32 NCHW [Bimg, C, HW].
 // ------------------------------------------------------------------------------------------------
-__global__ void cfg_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg, int C, int HW, int use_cfg,
-                                float g, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
+// DDIM eta=0 on the guided eps of the NHWC rows [cond], [cond | uncond], [cond | ptb] or [cond | uncond | ptb]:
+//   e = u + (c - u) * g (use_cfg) or c;  then, with perturbed-attention guidance, e = e + p_t * (c - ptb)
+__global__ void cfg_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
+                                float g, float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
                                 float* __restrict__ x) {
   const long total = (long)Bimg * C * HW;
+  const int ptb_row0 = (use_cfg ? 2 : 1) * Bimg;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
     const int p = (int)(i % HW);
     const int c = (int)((i / HW) % C);
@@ -439,48 +442,21 @@ __global__ void cfg_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg,
       const float eu = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
       e = eu + (ec - eu) * g;
     }
+    if (use_pag) {
+      const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
+      e = e + p_t * (ec - ep);
+    }
     // DDIM eta=0 (reference stablediffusion/mod.rs:423-428)
     const float xv = x[i];
     const float predx0 = (xv - e * sqrt_1ma) / sqrt_a;
     x[i] = predx0 * sqrt_ap + e * sqrt_1map;
   }
 }
-int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance,
-                    float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x, __half* /*x16*/) {
+int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag, float guidance,
+                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
   const long total = (long)Bimg * C * HW;
-  cfg_ddim_kernel<<<cdiv(total, 256), 256, 0, st>>>(eps, ld, Bimg, C, HW, use_cfg, guidance, sqrt_a, sqrt_1ma,
+  cfg_ddim_kernel<<<cdiv(total, 256), 256, 0, st>>>(eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sqrt_a, sqrt_1ma,
                                                      sqrt_ap, sqrt_1map, x);
-  return (int)cudaGetLastError();
-}
-// cfg_ddim_kernel with perturbed-attention guidance: eps rows [cond | uncond | ptb] (use_cfg) or [cond | ptb], and
-//   e = (u + (c - u) * s) + p_t * (c - ptb)      resp.   e = c + p_t * (c - ptb)
-__global__ void cfg_pag_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg, int C, int HW, int use_cfg, float g,
-                                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
-                                    float* __restrict__ x) {
-  const long total = (long)Bimg * C * HW;
-  const int ptb_row0 = (use_cfg ? 2 : 1) * Bimg;
-  for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-    const int p = (int)(i % HW);
-    const int c = (int)((i / HW) % C);
-    const int b = (int)(i / ((long)HW * C));
-    const float ec = eps[((size_t)b * HW + p) * ld + c];
-    const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
-    float e = ec;
-    if (use_cfg) {
-      const float eu = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
-      e = eu + (ec - eu) * g;
-    }
-    e = e + p_t * (ec - ep);
-    const float xv = x[i];
-    const float predx0 = (xv - e * sqrt_1ma) / sqrt_a;
-    x[i] = predx0 * sqrt_ap + e * sqrt_1map;
-  }
-}
-int cfg_pag_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance, float p_t,
-                        float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
-  const long total = (long)Bimg * C * HW;
-  cfg_pag_ddim_kernel<<<cdiv(total, 256), 256, 0, st>>>(eps, ld, Bimg, C, HW, use_cfg, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap,
-                                                         sqrt_1map, x);
   return (int)cudaGetLastError();
 }
 
@@ -509,8 +485,8 @@ __global__ void inpaint_blend_kernel(float* __restrict__ x, const float* __restr
     x[i] = mask[i] ? x[i] : nr;
   }
 }
-int inpaint_blend_launch(cudaStream_t st, float* x, const float* ref, const float* noise, const uint8_t* mask,
-                         size_t n, int /*nfwd*/, float sqrt_a, float sqrt_1ma, __half* /*x16*/) {
+int inpaint_blend_launch(cudaStream_t st, float* x, const float* ref, const float* noise, const uint8_t* mask, size_t n,
+                         float sqrt_a, float sqrt_1ma) {
   inpaint_blend_kernel<<<cdiv((long)n, 256), 256, 0, st>>>(x, ref, noise, mask, n, sqrt_a, sqrt_1ma);
   return (int)cudaGetLastError();
 }
@@ -521,13 +497,6 @@ __global__ void axpby_kernel(float* __restrict__ x, const float* __restrict__ no
 int axpby_launch(cudaStream_t st, float* x, const float* noise, size_t n, float sa, float sb) {
   axpby_kernel<<<cdiv((long)n, 256), 256, 0, st>>>(x, noise, n, sa, sb);
   return (int)cudaGetLastError();
-}
-int dup_latent_f16_launch(cudaStream_t st, const float* x, size_t n, int nfwd, __half* x16) {
-  for (int f = 0; f < nfwd; ++f) {
-    int e = cast_f32_to_f16_launch(st, x, n, x16 + (size_t)f * n);
-    if (e) return e;
-  }
-  return 0;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -643,7 +612,7 @@ __global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams
         const float eu = p.eps[((size_t)(grp_u + b) * p.HW + px) * p.ld + c];
         e = eu + (ec - eu) * p.guidance;
       }
-      if (p.use_pag) {   // cfg_pag_ddim_kernel's
+      if (p.use_pag) {   // cfg_ddim_kernel's
         const float ep = p.eps[((size_t)(grp_p + b) * p.HW + px) * p.ld + c];
         e = e + p.p_t * (ec - ep);
       }

@@ -2398,20 +2398,27 @@ extern "C" int sdxl_unet_set_deepcache(sdxl_unet* u, const sdxl_deepcache* d) {
 // ================================================================================================
 // UNet::forward
 // ================================================================================================
-extern "C" int sdxl_unet_forward(sdxl_unet* u, int B, int h, int w, const sdxl_half* x, int32_t t_host, sdxl_half* eps_out) {
-  if (!u || !x || !eps_out) return -1;
+// The direct forwards' body: x NCHW [B, C, h, w] in, eps NCHW out, both f16 (sdxl_unet_forward) or both f32.
+static int unet_forward(sdxl_unet* u, int B, int h, int w, const void* x, bool f16, double t, void* eps_out) {
   sdxl_ctx* c = u->ctx;
-  CU(c, cudaSetDevice(c->device));
   int r = ensure_plan(u, B, B, h, w, u->pag ? u->pag->forward_rows : 0);
   if (r) return r;
   const bool cached = u->deepcache && u->deepcache->forward_cached;
   if (cached && (r = cached_ready(u))) return r;
   Plan* P = u->plan.get();
-  KL(c, cast_f16_to_f32_launch(c->stream, (const __half*)x, (size_t)B * latent_channels(u->cfg) * h * w, P->x_in));
-  if ((r = set_t(u, t_host))) return r;
+  const size_t n = (size_t)B * latent_channels(u->cfg) * h * w;
+  if (f16) KL(c, cast_f16_to_f32_launch(c->stream, (const __half*)x, n, P->x_in));
+  else CU(c, cudaMemcpyAsync(P->x_in, x, n * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
+  if ((r = set_t(u, t))) return r;
   if ((r = run_plan(u, cached))) return r;
-  KL(c, nhwc_to_nchw_f16_launch(c->stream, P->eps, B, h * w, u->cfg.out_channels, P->eps_ld, (__half*)eps_out));
+  if (f16) KL(c, nhwc_to_nchw_f16_launch(c->stream, P->eps, B, h * w, u->cfg.out_channels, P->eps_ld, (__half*)eps_out));
+  else KL(c, nhwc_to_nchw_f32_launch(c->stream, P->eps, B, h * w, u->cfg.out_channels, P->eps_ld, (float*)eps_out));
   return 0;
+}
+extern "C" int sdxl_unet_forward(sdxl_unet* u, int B, int h, int w, const sdxl_half* x, int32_t t_host, sdxl_half* eps_out) {
+  if (!u || !x || !eps_out) return -1;
+  CU(u->ctx, cudaSetDevice(u->ctx->device));
+  return unet_forward(u, B, h, w, x, true, t_host, eps_out);
 }
 extern "C" int sdxl_unet_forward_f32(sdxl_unet* u, int B, int h, int w, const float* x, int32_t t_host, float* eps_out) {
   return sdxl_unet_forward_f32_at(u, B, h, w, x, (double)t_host, eps_out);
@@ -2422,16 +2429,7 @@ extern "C" int sdxl_unet_forward_f32_at(sdxl_unet* u, int B, int h, int w, const
   CU(c, cudaSetDevice(c->device));
   if (!(t_host >= 0.0 && t_host <= (double)(u->cfg.n_steps - 1)))   // also refuses NaN
     return fail(c, 5024, "forward: timestep %g outside [0, %d]", t_host, u->cfg.n_steps - 1);
-  int r = ensure_plan(u, B, B, h, w, u->pag ? u->pag->forward_rows : 0);
-  if (r) return r;
-  const bool cached = u->deepcache && u->deepcache->forward_cached;
-  if (cached && (r = cached_ready(u))) return r;
-  Plan* P = u->plan.get();
-  CU(c, cudaMemcpyAsync(P->x_in, x, (size_t)B * latent_channels(u->cfg) * h * w * sizeof(float), cudaMemcpyDeviceToDevice, c->stream));
-  if ((r = set_t(u, t_host))) return r;
-  if ((r = run_plan(u, cached))) return r;
-  KL(c, nhwc_to_nchw_f32_launch(c->stream, P->eps, B, h * w, u->cfg.out_channels, P->eps_ld, eps_out));
-  return 0;
+  return unet_forward(u, B, h, w, x, false, t_host, eps_out);
 }
 // Per-kernel-kind device time of one plan execution, measured with CUDA events on the ctx stream
 // (eager launches, one event pair per op). kinds: see OpKind. Arrays hold SDXL_PROFILE_KINDS entries.
@@ -2564,6 +2562,11 @@ static int run_sampler_plan(sdxl_unet* u) {
   return r;
 }
 
+// PAG's scale at timestep t, with diffusers' adaptive scaling: p_t = max(scale - adaptive * (n_steps - t), 0)
+static float pag_scale(const sdxl_unet* u, double t) {
+  return std::max(u->pag->scale - u->pag->adaptive * (float)(u->cfg.n_steps - t), 0.f);
+}
+
 // one loop-body iteration (reference stablediffusion/mod.rs:406-429)
 static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   sdxl_ctx* c = u->ctx;
@@ -2576,16 +2579,9 @@ static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   int r = set_t(u, t);
   if (r) return r;
   if ((r = run_sampler_plan(u))) return r;
-  if (S->pag) {
-    // diffusers' adaptive scaling: p_t = max(scale - adaptive * (n_steps - t), 0)
-    const PagAttach& pg = *u->pag;
-    const float p_t = std::max(pg.scale - pg.adaptive * (float)(u->cfg.n_steps - t), 0.f);
-    KL(c, cfg_pag_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->cfg, S->guidance, p_t,
-                              (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap), P->x_in));
-    return 0;
-  }
-  KL(c, cfg_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->nfwd == 2, S->guidance,
-                        (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap), P->x_in, nullptr));
+  KL(c, cfg_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->cfg, S->pag, S->guidance,
+                        S->pag ? pag_scale(u, t) : 0.f, (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap),
+                        P->x_in));
   return 0;
 }
 
@@ -2637,6 +2633,66 @@ extern "C" int sdxl_randn(sdxl_ctx* c, float* out, size_t n, uint64_t seed, uint
   return 0;
 }
 
+// The noise draws of a sampling call, in the call's order: the injected tensors first, then subsequences 0, 1, 2, ... of the
+// seeded Philox stream. Injected tensors from the host are staged on the device once, so that every draw is read in place.
+struct NoiseFeed {
+  const float* injected = nullptr;   // device, n_injected tensors of lat elements
+  int n_injected = 0, used = 0;
+  size_t lat = 0;
+  uint64_t seed = 0, subseq = 0;
+  int init(sdxl_ctx* c, TmpBufs& tmp, const float* noise, int n_noise, bool on_host, size_t lat_, uint64_t seed_) {
+    lat = lat_; seed = seed_;
+    injected = noise; n_injected = noise ? n_noise : 0;
+    if (n_injected > 0 && on_host) {
+      const size_t bytes = (size_t)n_injected * lat * sizeof(float);
+      float* d = tmp.get<float>(bytes);
+      if (!d) return fail(c, 5235, "cannot allocate %zu bytes to stage the injected noise", bytes);
+      CU(c, cudaMemcpyAsync(d, noise, bytes, cudaMemcpyHostToDevice, c->stream));
+      injected = d;
+    }
+    return 0;
+  }
+  // the next draw: an injected tensor z, or (z null) subsequence sub of the seeded stream
+  void next(const float*& z, uint64_t& sub) {
+    z = nullptr;
+    sub = 0;
+    if (used < n_injected) z = injected + (size_t)used++ * lat;
+    else sub = subseq++;
+  }
+  // the next draw in memory, for kernels that read their noise: an injected tensor in place, or the seeded one generated into dst
+  int next_in(sdxl_ctx* c, float* dst, const float*& z) {
+    uint64_t sub;
+    next(z, sub);
+    if (!z) {
+      KL(c, randn_launch(c->stream, dst, lat, seed, sub));
+      z = dst;
+    }
+    return 0;
+  }
+};
+
+// The start of a sampling call whose arguments have been checked: the sampler, then the inpainting reference and mask.
+static int sample_begin(sdxl_unet* u, const sdxl_conditioning* cond, double guidance, bool no_cfg, const float* inpaint_ref,
+                        const uint8_t* inpaint_mask) {
+  if (int r = sampler_begin(u, cond, guidance, no_cfg)) return r;
+  if (inpaint_ref) {
+    sdxl_ctx* c = u->ctx;
+    Sampler* S = u->sampler.get();
+    const cudaMemcpyKind kind = cond->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
+    CU(c, cudaMemcpyAsync(S->ref, inpaint_ref, S->latent_elems * sizeof(float), kind, c->stream));
+    CU(c, cudaMemcpyAsync(S->mask, inpaint_mask, S->latent_elems, kind, c->stream));
+  }
+  return 0;
+}
+// The end of a sampling call: the latent to the caller's memory, synchronised when that is host memory.
+static int sample_end(sdxl_unet* u, const sdxl_conditioning* cond, const float* latent, float* latent_out) {
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaMemcpyAsync(latent_out, latent, u->sampler->latent_elems * sizeof(float),
+                        cond->on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
+  if (cond->on_host) CU(c, cudaStreamSynchronize(c->stream));
+  return 0;
+}
+
 extern "C" int sdxl_sample_latent(sdxl_unet* u, const sdxl_conditioning* cond, double guidance_scale, int n_steps,
                                   int step_start, const float* init_latent, const float* noise, int n_noise, uint64_t seed,
                                   const float* inpaint_ref, const uint8_t* inpaint_mask, float* latent_out) {
@@ -2648,7 +2704,7 @@ extern "C" int sdxl_sample_latent(sdxl_unet* u, const sdxl_conditioning* cond, d
   if (step_start < 0 || step_start >= total) return fail(c, 5221, "bad step_start");
   if ((inpaint_ref == nullptr) != (inpaint_mask == nullptr)) return fail(c, 5222, "inpaint_ref and inpaint_mask must be given together");
   if (step_start > 0 && !init_latent) return fail(c, 5223, "refine (step_start>0) needs init_latent");
-  int r = sampler_begin(u, cond, guidance_scale);
+  int r = sample_begin(u, cond, guidance_scale, false, inpaint_ref, inpaint_mask);
   if (r) return r;
   Sampler* S = u->sampler.get();
   Plan* P = u->plan.get();
@@ -2656,43 +2712,34 @@ extern "C" int sdxl_sample_latent(sdxl_unet* u, const sdxl_conditioning* cond, d
   const cudaMemcpyKind in_kind = cond->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
   const int step_size = total / n_steps;      // mod.rs:400
   const int t_begin = total - step_start;     // mod.rs:404
-  int noise_used = 0;
-  uint64_t subseq = 0;
-  auto next_noise = [&](float* dst) -> int {  // injected noise first, then the seeded stream
-    if (noise && noise_used < n_noise) {
-      CU(c, cudaMemcpyAsync(dst, noise + (size_t)noise_used * lat, bytes, in_kind, c->stream));
-      noise_used++;
-      return 0;
-    }
-    KL(c, randn_launch(c->stream, dst, lat, seed, subseq++));
-    return 0;
-  };
+  TmpBufs tmp(c->stream);
+  NoiseFeed feed;
+  if ((r = feed.init(c, tmp, noise, n_noise, cond->on_host, lat, seed))) return r;
+  const float* z;
   // initial latent
-  if (init_latent) CU(c, cudaMemcpyAsync(P->x_in, init_latent, bytes, in_kind, c->stream));
-  else if ((r = next_noise(P->x_in))) return r;
+  if (init_latent) {
+    CU(c, cudaMemcpyAsync(P->x_in, init_latent, bytes, in_kind, c->stream));
+  } else {
+    if ((r = feed.next_in(c, P->x_in, z))) return r;
+    if (z != P->x_in) CU(c, cudaMemcpyAsync(P->x_in, z, bytes, cudaMemcpyDeviceToDevice, c->stream));
+  }
   if (step_start > 0) {
     // refine_latent entry (mod.rs:363-367): x = x*sqrt(a_t0) + noise*sqrt(1-a_t0), t0 = n_steps_total - step_start
     const double a0 = u->alphas[t_begin];
-    if ((r = next_noise(S->noise))) return r;
-    KL(c, axpby_launch(c->stream, P->x_in, S->noise, lat, (float)sqrt(a0), (float)sqrt(1.0 - a0)));
-  }
-  if (inpaint_ref) {
-    CU(c, cudaMemcpyAsync(S->ref, inpaint_ref, bytes, in_kind, c->stream));
-    CU(c, cudaMemcpyAsync(S->mask, inpaint_mask, lat, in_kind, c->stream));
+    if ((r = feed.next_in(c, S->noise, z))) return r;
+    KL(c, axpby_launch(c->stream, P->x_in, z, lat, (float)sqrt(a0), (float)sqrt(1.0 - a0)));
   }
   // for t in (0..t_begin).rev().step_by(step_size)   (mod.rs:406, 452)
   for (int t = t_begin - 1; t >= 0; t -= step_size) {
     const int t_prev = (t >= step_size) ? t - step_size : -1;
     if (inpaint_ref) {
       const double a = u->alphas[t];
-      if ((r = next_noise(S->noise))) return r;
-      KL(c, inpaint_blend_launch(c->stream, P->x_in, S->ref, S->noise, S->mask, lat, S->nfwd, (float)sqrt(a), (float)sqrt(1.0 - a), nullptr));
+      if ((r = feed.next_in(c, S->noise, z))) return r;
+      KL(c, inpaint_blend_launch(c->stream, P->x_in, S->ref, z, S->mask, lat, (float)sqrt(a), (float)sqrt(1.0 - a)));
     }
     if ((r = sampler_step(u, t, t_prev))) return r;
   }
-  CU(c, cudaMemcpyAsync(latent_out, P->x_in, bytes, cond->on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
-  if (cond->on_host) CU(c, cudaStreamSynchronize(c->stream));
-  return 0;
+  return sample_end(u, cond, P->x_in, latent_out);
 }
 
 // ================================================================================================
@@ -2735,33 +2782,15 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
   for (int k = 0; k < n; ++k)
     if (!(sig[k + 1] < sig[k])) return fail(c, 5234, "schedule: n_steps = %d gives sigmas that do not decrease at step %d", n, k);
 
-  int r = sampler_begin(u, cond, guidance_scale, sch->no_cfg != 0);
+  int r = sample_begin(u, cond, guidance_scale, sch->no_cfg != 0, inpaint_ref, inpaint_mask);
   if (r) return r;
   Sampler* S = u->sampler.get();
   Plan* P = u->plan.get();
   const size_t lat = S->latent_elems, bytes = lat * 4;
   const cudaMemcpyKind in_kind = cond->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
-  // the step kernel reads its noise in place: injected tensors from the host are staged on the device once
   TmpBufs tmp(c->stream);
-  const float* noise_dev = noise;
-  if (n_noise && cond->on_host) {
-    float* d = tmp.get<float>((size_t)n_noise * bytes);
-    if (!d) return fail(c, 5235, "cannot allocate %zu bytes to stage the injected noise", (size_t)n_noise * bytes);
-    CU(c, cudaMemcpyAsync(d, noise, (size_t)n_noise * bytes, cudaMemcpyHostToDevice, c->stream));
-    noise_dev = d;
-  }
-  int noise_used = 0;
-  uint64_t subseq = 0;
-  auto next_noise = [&](const float*& z, uint64_t& sub) {   // injected tensors first, then the seeded stream
-    z = nullptr;
-    sub = 0;
-    if (noise_used < n_noise) z = noise_dev + (size_t)noise_used++ * lat;
-    else sub = subseq++;
-  };
-  if (inpaint_ref) {
-    CU(c, cudaMemcpyAsync(S->ref, inpaint_ref, bytes, in_kind, c->stream));
-    CU(c, cudaMemcpyAsync(S->mask, inpaint_mask, lat, in_kind, c->stream));
-  }
+  NoiseFeed feed;   // the step kernel reads an injected draw in place and generates a seeded one
+  if ((r = feed.init(c, tmp, noise, n_noise, cond->on_host, lat, seed))) return r;
   GuidedStepParams p{};
   p.Bimg = S->Bimg; p.C = latent_channels(u->cfg); p.HW = S->h * S->w;
   p.xh = S->xh; p.x_in = P->x_in; p.hist = S->hist;
@@ -2779,19 +2808,19 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
     p.cx = 0.f;
     p.cn = (float)sqrt(sig[0] * sig[0] + 1.0);
     if (init_latent) p.z = init_dev ? init_dev : init_latent;
-    else next_noise(p.z, p.z_subseq);
+    else feed.next(p.z, p.z_subseq);
   } else {
     CU(c, cudaMemcpyAsync(S->xh, init_latent, bytes, in_kind, c->stream));
     p.cx = 1.f;
     if (sch->renoise) {
       p.cn = (float)sig[k0];
-      next_noise(p.z, p.z_subseq);
+      feed.next(p.z, p.z_subseq);
     }
   }
   p.c_in = (float)(1.0 / sqrt(sig[k0] * sig[k0] + 1.0));
   if (inpaint_ref) {
     p.sigma_blend = (float)sig[k0];
-    next_noise(p.zb, p.zb_subseq);
+    feed.next(p.zb, p.zb_subseq);
   }
   KL(c, guided_step_launch(c->stream, p));
   // the steps: write t, replay the plan, one launch
@@ -2803,21 +2832,18 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
     p.sigma = (float)sig[k];
     p.cx = q.cx; p.cd = q.cd; p.ch = q.ch; p.cn = q.cn; p.c_in = q.c_in;
     p.write_hist = sampler_keeps_history(sch->sampler);
-    // diffusers' adaptive scaling (sampler_step's), at the fractional t
-    if (S->pag) p.p_t = std::max(u->pag->scale - u->pag->adaptive * (float)(u->cfg.n_steps - ts[k]), 0.f);
+    if (S->pag) p.p_t = pag_scale(u, ts[k]);
     p.z = p.zb = nullptr;
     p.mask = nullptr;
-    if (q.cn != 0.f) next_noise(p.z, p.z_subseq);
+    if (q.cn != 0.f) feed.next(p.z, p.z_subseq);
     if (inpaint_ref && k + 1 < k1) {   // the blend before the next forward: its noise follows this step's in the call's order
       p.mask = S->mask;
       p.sigma_blend = (float)sig[k + 1];
-      next_noise(p.zb, p.zb_subseq);
+      feed.next(p.zb, p.zb_subseq);
     }
     KL(c, guided_step_launch(c->stream, p));
   }
-  CU(c, cudaMemcpyAsync(latent_out, S->xh, bytes, cond->on_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice, c->stream));
-  if (cond->on_host) CU(c, cudaStreamSynchronize(c->stream));
-  return 0;
+  return sample_end(u, cond, S->xh, latent_out);
 }
 
 // ================================================================================================

@@ -230,27 +230,22 @@ int nhwc_to_nchw_f16_launch(cudaStream_t st, const float* x, int B, int HW, int 
 int nhwc_to_nchw_f32_launch(cudaStream_t st, const float* x, int B, int HW, int C, int ldx, float* y);
 // Sampler elementwise (reference stablediffusion/mod.rs:407-428, 463-465, 539-540).
 // eps layout: NHWC f32 [nfwd*Bimg, HW, ld]; cond rows first, then uncond (if cfg).
-// x: NCHW f32 master latent [Bimg,C,HW], updated in place. x16 is unused (the next forward reads x; pass nullptr).
-int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg,
-                    float guidance, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
-                    float* x, __half* x16);
-// The same update with perturbed-attention guidance (DESIGN.md §14): eps rows [cond | uncond | ptb] (use_cfg) or [cond | ptb];
-// e = (u + (c - u) * guidance) + p_t * (c - ptb), resp. c + p_t * (c - ptb).
-int cfg_pag_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance, float p_t,
-                        float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x);
+// x: NCHW f32 master latent [Bimg,C,HW], updated in place. use_pag (DESIGN.md §14): a last group of Bimg perturbed rows follows,
+// eps rows [cond | uncond | ptb] (use_cfg) or [cond | ptb], and e = (u + (c - u) * guidance) + p_t * (c - ptb), resp. c + p_t * (c - ptb).
+int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag, float guidance,
+                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x);
 // PAG's identity self-attention on `rows` token rows: out[r, 0:C] = qkv[r, 2C:3C] (qkv row pitch 3C, out row pitch C); C % 8 == 0,
 // both pointers 16-byte aligned.
 int pag_identity_launch(cudaStream_t st, const __half* qkv, int C, long rows, __half* out);
-// x = mask ? x : ref*sqrt_a + noise*sqrt_1ma over n_per_img_batch elements; nfwd and x16 are unused (pass nullptr).
-int inpaint_blend_launch(cudaStream_t st, float* x, const float* ref, const float* noise,
-                         const uint8_t* mask, size_t n_per_img_batch, int nfwd, float sqrt_a,
-                         float sqrt_1ma, __half* x16);
+// x = mask ? x : ref*sqrt_a + noise*sqrt_1ma over n_per_img_batch elements.
+int inpaint_blend_launch(cudaStream_t st, float* x, const float* ref, const float* noise, const uint8_t* mask,
+                         size_t n_per_img_batch, float sqrt_a, float sqrt_1ma);
 // x = x*sa + noise*sb  (refine_latent entry, reference stablediffusion/mod.rs:363-367)
 int axpby_launch(cudaStream_t st, float* x, const float* noise, size_t n, float sa, float sb);
 // Standard normal noise, Philox4x32-10 + Box-Muller, element i of stream (seed, subseq).
 int randn_launch(cudaStream_t st, float* out, size_t n, uint64_t seed, uint64_t subseq);
 // One step of a scheduled sampler (DESIGN.md §16) on the k-diffusion-scaled state xh, f32 NCHW [Bimg, C, HW], in one launch:
-//   e   = guided eps of the NHWC rows [cond], [cond | uncond], [cond | ptb] or [cond | uncond | ptb] (cfg_ddim / cfg_pag_ddim's combines)
+//   e   = guided eps of the NHWC rows [cond], [cond | uncond], [cond | ptb] or [cond | uncond | ptb] (cfg_ddim's combines)
 //   D   = xh - sigma * e                          (eps == nullptr: no model output, D = xh: the entry of a call)
 //   xh' = cx * xh + cd * D + ch * hist + cn * z   (hist read when ch != 0, then D written to it when write_hist)
 //   xh' = mask ? xh' : ref + sigma_blend * zb     (mask != nullptr: the latent blend before the next forward)
@@ -273,7 +268,6 @@ struct GuidedStepParams {
   float sigma_blend;
 };
 int guided_step_launch(cudaStream_t st, const GuidedStepParams& p);
-int dup_latent_f16_launch(cudaStream_t st, const float* x, size_t n, int nfwd, __half* x16);
 
 // Latent-decoder kernels (vae_kernels.cu)
 // P[r,:] = softmax(scale * S[r,:]); S f32 [rows, lds] -> P f16 [rows, ldp]; cols % 4 == 0.

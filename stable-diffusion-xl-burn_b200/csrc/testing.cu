@@ -137,11 +137,6 @@ SDXL_TEST_API int sdxl_test_conv_in_cat(void* stream, const void* x, int x_f32, 
 SDXL_TEST_API int sdxl_test_pag_identity(void* stream, const void* qkv, int C, long rows, void* out) {
   return pag_identity_launch((cudaStream_t)stream, (const __half*)qkv, C, rows, (__half*)out);
 }
-// The sampler's guided DDIM update with PAG (engine.cu: sampler_step).
-SDXL_TEST_API int sdxl_test_cfg_pag_ddim(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance,
-                                         float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
-  return cfg_pag_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_cfg, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x);
-}
 
 // FreeU at one skip concatenation, as the plan's OP_FREEU: the twiddle table (host, 2 * (H + W) floats) and the in-place launch.
 SDXL_TEST_API void sdxl_test_freeu_twiddles(int H, int W, float* out_host) { freeu_twiddles(H, W, out_host); }
@@ -241,19 +236,18 @@ SDXL_TEST_API int sdxl_test_t2i_add(void* stream, float* x, const float* F, long
 }
 
 // The sampler's elementwise kernels and the UNet's resampling copies and casts (elementwise.cu).
-SDXL_TEST_API int sdxl_test_cfg_ddim(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, float guidance,
-                                     float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
-  return cfg_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_cfg, guidance, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x, nullptr);
+// The sampler's guided DDIM update, with or without PAG (engine.cu: sampler_step).
+SDXL_TEST_API int sdxl_test_cfg_ddim(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
+                                     float guidance, float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
+  return cfg_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap,
+                         sqrt_1map, x);
 }
 SDXL_TEST_API int sdxl_test_inpaint_blend(void* stream, float* x, const float* ref, const float* noise, const uint8_t* mask, size_t n,
                                           float sqrt_a, float sqrt_1ma) {
-  return inpaint_blend_launch((cudaStream_t)stream, x, ref, noise, mask, n, 1, sqrt_a, sqrt_1ma, nullptr);
+  return inpaint_blend_launch((cudaStream_t)stream, x, ref, noise, mask, n, sqrt_a, sqrt_1ma);
 }
 SDXL_TEST_API int sdxl_test_axpby(void* stream, float* x, const float* noise, size_t n, float sa, float sb) {
   return axpby_launch((cudaStream_t)stream, x, noise, n, sa, sb);
-}
-SDXL_TEST_API int sdxl_test_dup_latent_f16(void* stream, const float* x, size_t n, int nfwd, void* x16) {
-  return dup_latent_f16_launch((cudaStream_t)stream, x, n, nfwd, (__half*)x16);
 }
 SDXL_TEST_API int sdxl_test_cast_f32_to_f16(void* stream, const float* x, size_t n, void* y) {
   return cast_f32_to_f16_launch((cudaStream_t)stream, x, n, (__half*)y);

@@ -31,7 +31,6 @@ PROTOTYPES = {
     "sdxl_test_conv_in": (I, [P, P, I, I, I, I, I, I, P, P, I, P, P, I]),
     "sdxl_test_conv_in_cat": (I, [P, P, I, I, I, I, P, I, I, I, I, P, P, I, P]),
     "sdxl_test_pag_identity": (I, [P, P, I, C.c_long, P]),
-    "sdxl_test_cfg_pag_ddim": (I, [P, P, I, I, I, I, I, F, F, F, F, F, F, P]),
     "sdxl_test_freeu_twiddles": (None, [I, I, P]),
     "sdxl_test_freeu": (I, [P, P, I, P, I, I, I, I, P, P, P]),
     "sdxl_test_repack_upconv": (I, [P, P, I, I, P, I]),
@@ -55,10 +54,9 @@ PROTOTYPES = {
     "sdxl_test_relu_f16": (I, [P, P, Z, P]),
     "sdxl_test_avg_pool2_f16": (I, [P, P, I, I, I, I, P]),
     "sdxl_test_t2i_add": (I, [P, P, P, L, I, I, P, P]),
-    "sdxl_test_cfg_ddim": (I, [P, P, I, I, I, I, I, F, F, F, F, F, P]),
+    "sdxl_test_cfg_ddim": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, P]),
     "sdxl_test_inpaint_blend": (I, [P, P, P, P, P, Z, F, F]),
     "sdxl_test_axpby": (I, [P, P, P, Z, F, F]),
-    "sdxl_test_dup_latent_f16": (I, [P, P, Z, I, P]),
     "sdxl_test_cast_f32_to_f16": (I, [P, P, Z, P]),
     "sdxl_test_cast_f16_to_f32": (I, [P, P, Z, P]),
     "sdxl_test_upsample2x": (I, [P, P, I, I, I, I, P]),
@@ -187,11 +185,6 @@ def pag_identity(qkv: torch.Tensor, C: int, rows: int, out: torch.Tensor) -> Non
     _call("sdxl_test_pag_identity", _p(qkv), C, rows, _p(out))
 
 
-def cfg_pag_ddim(eps, ld, Bimg, C, HW, use_cfg, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x) -> None:
-    """x f32 NCHW [Bimg, C, HW] updated in place from eps NHWC f32 [groups * Bimg, HW, ld]."""
-    _call("sdxl_test_cfg_pag_ddim", _p(eps), ld, Bimg, C, HW, int(use_cfg), guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, _p(x))
-
-
 def freeu_twiddles(H: int, W: int) -> torch.Tensor:
     """The host twiddle table of an H x W skip (f32 [2 * (H + W)]: cos and sin of 2 pi h / H, then of 2 pi w / W)."""
     out = torch.empty(2 * (H + W), dtype=torch.float32)
@@ -303,9 +296,11 @@ def t2i_add(x, F, per_img, B, n_hint, t, t_min) -> None:
 
 
 # sampler, resampling copies and casts (elementwise.cu)
-def cfg_ddim(eps, ld, Bimg, C, HW, use_cfg, guidance, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x) -> None:
-    """x f32 NCHW [Bimg, C, HW] updated in place from eps NHWC f32 [(1 + use_cfg) * Bimg, HW, ld]."""
-    _call("sdxl_test_cfg_ddim", _p(eps), ld, Bimg, C, HW, int(use_cfg), guidance, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, _p(x))
+def cfg_ddim(eps, ld, Bimg, C, HW, use_cfg, guidance, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x, use_pag=False, p_t=0.0) -> None:
+    """x f32 NCHW [Bimg, C, HW] updated in place from eps NHWC f32 [(1 + use_cfg + use_pag) * Bimg, HW, ld]; use_pag: the last
+    group is the perturbed rows, weighted by p_t."""
+    _call("sdxl_test_cfg_ddim", _p(eps), ld, Bimg, C, HW, int(use_cfg), int(use_pag), guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map,
+          _p(x))
 
 
 def inpaint_blend(x, ref, noise, mask, n, sqrt_a, sqrt_1ma) -> None:
@@ -314,10 +309,6 @@ def inpaint_blend(x, ref, noise, mask, n, sqrt_a, sqrt_1ma) -> None:
 
 def axpby(x, noise, n, sa, sb) -> None:
     _call("sdxl_test_axpby", _p(x), _p(noise), n, sa, sb)
-
-
-def dup_latent_f16(x, n, nfwd, x16) -> None:
-    _call("sdxl_test_dup_latent_f16", _p(x), n, nfwd, _p(x16))
 
 
 def cast_f32_to_f16(x, n, y) -> None:

@@ -616,20 +616,6 @@ F16_EDGES = [0.0, -0.0, 65504.0, 65519.99, 65520.0, -65520.0, 2.0 ** -24, 2.0 **
              1e-30, float("inf"), float("-inf"), 1.0 + 2.0 ** -11, 1.0 + 3 * 2.0 ** -11]
 
 
-@pytest.mark.parametrize("nfwd", [2, 3])
-@pytest.mark.parametrize("n", [1000, CAP16 + 1001])
-def test_dup_latent_f16(nfwd, n):
-    """x16[f n + i] = f16(x[i]) for each of nfwd forwards, bit-exact (round-to-nearest-even, overflow to inf, subnormals)."""
-    g = gen(n + nfwd)
-    x = randn(g, n, scale=100.0)
-    x[:len(F16_EDGES)] = torch.tensor(F16_EDGES)
-    y = buf(nfwd * n, torch.float16)
-    T.dup_latent_f16(on_dev(x), n, nfwd, y)
-    torch.cuda.synchronize()
-    same_bits(y[:nfwd * n].view(nfwd, n), x.half()[None].expand(nfwd, n), f"dup_latent_f16 n={n} nfwd={nfwd}")
-    untouched(y[nfwd * n:], "dup_latent_f16: after x16")
-
-
 def test_casts():
     """cast_f32_to_f16 over n above the grid cap with the rounding edges, bit-exact; cast_f16_to_f32 of every f16 bit pattern,
     bit-exact (NaN stays NaN)."""

@@ -69,8 +69,9 @@ def test_identity_kernel(ctx, C_, Tq, Bp):
 
 
 @pytest.mark.parametrize("use_cfg, Bimg", [(True, 1), (True, 2), (False, 2)])
-def test_cfg_pag_ddim_kernel(ctx, use_cfg, Bimg):
-    """The guided update against float64, for the base layout [cond | uncond | ptb] and the refiner's [cond | ptb]."""
+def test_cfg_ddim_kernel_pag(ctx, use_cfg, Bimg):
+    """cfg_ddim_kernel's guided update with PAG against float64, for the base layout [cond | uncond | ptb] and the refiner's
+    [cond | ptb]."""
     Cc, HW, ld = 4, 37 * 5, 4
     groups = 3 if use_cfg else 2
     g = torch.Generator().manual_seed(Bimg)
@@ -78,7 +79,8 @@ def test_cfg_pag_ddim_kernel(ctx, use_cfg, Bimg):
     x0 = torch.randn(Bimg, Cc, HW, generator=g)
     s, p_t, a, ap = 7.5, 2.25, 0.31, 0.55
     x = x0.clone().cuda()
-    _testing.cfg_pag_ddim(eps.cuda(), ld, Bimg, Cc, HW, use_cfg, s, p_t, a ** 0.5, (1 - a) ** 0.5, ap ** 0.5, (1 - ap) ** 0.5, x)
+    _testing.cfg_ddim(eps.cuda(), ld, Bimg, Cc, HW, use_cfg, s, a ** 0.5, (1 - a) ** 0.5, ap ** 0.5, (1 - ap) ** 0.5, x,
+                      use_pag=True, p_t=p_t)
     torch.cuda.synchronize()
     e = eps.double().permute(0, 2, 1)[:, :Cc]
     c, ptb = e[:Bimg], e[(groups - 1) * Bimg:]
