@@ -207,7 +207,8 @@ SDXL_API int sdxl_sampler_step(sdxl_unet* unet, int t, int t_prev);
 SDXL_API int sdxl_sampler_step_host(sdxl_unet* unet, int t, int t_prev, float* latent_host);
 SDXL_API int sdxl_sampler_set_latent(sdxl_unet* unet, const float* latent, int on_host);
 SDXL_API int sdxl_sampler_get_latent(sdxl_unet* unet, float* latent, int on_host);
-/* alphas_cumprod[i] as the sampler sees it (f16-stored like the reference's .mpk, widened). */
+/* alphas_cumprod[i] as the sampler sees it: the loaded table (f16-stored like the reference's .mpk, widened), or the one
+ * sdxl_unet_set_prediction put in effect. */
 SDXL_API double sdxl_unet_alpha(const sdxl_unet* unet, int i);
 /* Algorithmic FLOPs (2*MAC over Linear/conv/attention, SURVEY 8(d) counting rule) and kernel-op count of
  * the launch plan currently built for this UNet (0 before the first forward). */
@@ -695,6 +696,33 @@ typedef struct sdxl_deepcache {
  * sdxl_sampler_step requires a new sdxl_sampler_begin. A cached direct forward is refused when no full forward has kept a feature
  * since the plan was last built (a new branch, batch or latent size, or any attachment change rebuilds it). */
 SDXL_API int sdxl_unet_set_deepcache(sdxl_unet* unet, const sdxl_deepcache* dc);
+
+/* ---- prediction type, guidance rescale and the noise table ------------------------------------------------------------
+ * DESIGN.md §18. What the sampling loops (sdxl_sample_latent, sdxl_sample_latent_scheduled, sdxl_sampler_step and
+ * sdxl_sampler_step_host) read the UNet's output as. With the rows [cond | uncond | ptb], m the output of a row, the guided output is
+ * g = u + (c - u) * s, plus p_t * (c - ptb) with PAG, and then:
+ *   guidance rescale (phi > 0, calls with CFG rows only; diffusers' rescale_noise_cfg, Lin et al. 2023): for each image b,
+ *                    g <- phi * g * std(c_b) / std(g_b) + (1 - phi) * g, both std unbiased over the C * H * W elements of the image,
+ *                    the ratio read as 1 when std(g_b) = 0. It acts on the model output, v for a v model. no_cfg calls and the refiner,
+ *                    which run without CFG, ignore phi.
+ *   epsilon          g is the noise: the DDIM loop x' = sqrt(a') * (x - sqrt(1 - a) * g) / sqrt(a) + sqrt(1 - a') * g, the
+ *                    scheduled samplers D = xh - sigma * g.
+ *   v                g is v (Salimans & Ho 2022): the DDIM loop x0 = sqrt(a) * x - sqrt(1 - a) * g, eps = sqrt(a) * g + sqrt(1 - a) * x,
+ *                    x' = sqrt(a') * x0 + sqrt(1 - a') * eps; the scheduled samplers D = xh / (sigma^2 + 1) - sigma / sqrt(sigma^2 + 1) * g.
+ * The table: every loop, sdxl_unet_alpha and so every sdxl_schedule_build on it use the one in effect. A zero-terminal-SNR table
+ * (Lin et al. 2023, Algorithm 1) is computed by the caller, as diffusers does it in float32 with the last entry set to 2^-24
+ * (sdxl_b200.schedulers.alphas_cumprod); the loaded table is f16-rounded and is not rescaled here. */
+enum { SDXL_PREDICTION_EPSILON = 0, SDXL_PREDICTION_V = 1 };
+typedef struct sdxl_prediction {
+  int32_t type;                       /* SDXL_PREDICTION_* */
+  float   guidance_rescale;           /* phi in [0, 1]; 0 = off */
+  int32_t n_alphas;                   /* 0: keep the loaded alphas_cumprod; else cfg.n_steps */
+  const double* alphas_cumprod_host;  /* n_alphas entries, strictly decreasing inside (0, 1) */
+} sdxl_prediction;
+/* Sets the UNet's prediction type, guidance rescale and noise table. NULL restores epsilon, phi 0 and the loaded table, bit for bit.
+ * Everything is validated before anything changes: a refusal (5600..5604) names the field and leaves the previous state. Nothing here
+ * rebuilds the launch plan, and a change between sdxl_sampler_begin and sdxl_sampler_step applies from the next step. */
+SDXL_API int sdxl_unet_set_prediction(sdxl_unet* unet, const sdxl_prediction* p);
 
 /* ---- `sample` front-end helpers --------------------------------------------------------------------- */
 /* Inpainting mask from a crop window in pixels (src/bin/sample/main.rs:144-190): latent coordinates = pixel / (img_h / lat_h),

@@ -426,9 +426,11 @@ int nhwc_to_nchw_f16_launch(cudaStream_t st, const float* x, int B, int HW, int 
 // ------------------------------------------------------------------------------------------------
 // DDIM eta=0 on the guided eps of the NHWC rows [cond], [cond | uncond], [cond | ptb] or [cond | uncond | ptb]:
 //   e = u + (c - u) * g (use_cfg) or c;  then, with perturbed-attention guidance, e = e + p_t * (c - ptb)
+// kV, kRescale: kernels.h Prediction; <false, false> is the epsilon step and never reads `factor`.
+template <bool kV, bool kRescale>
 __global__ void cfg_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
                                 float g, float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
-                                float* __restrict__ x) {
+                                float* __restrict__ x, const float* __restrict__ factor) {
   const long total = (long)Bimg * C * HW;
   const int ptb_row0 = (use_cfg ? 2 : 1) * Bimg;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -446,17 +448,138 @@ __global__ void cfg_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg,
       const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
       e = e + p_t * (ec - ep);
     }
-    // DDIM eta=0 (reference stablediffusion/mod.rs:423-428)
+    if constexpr (kRescale) e *= factor[b];
     const float xv = x[i];
-    const float predx0 = (xv - e * sqrt_1ma) / sqrt_a;
-    x[i] = predx0 * sqrt_ap + e * sqrt_1map;
+    if constexpr (kV) {   // x0 and eps of the v prediction, then the same DDIM step
+      const float predx0 = sqrt_a * xv - sqrt_1ma * e;
+      const float pred_eps = sqrt_a * e + sqrt_1ma * xv;
+      x[i] = predx0 * sqrt_ap + pred_eps * sqrt_1map;
+    } else {
+      // DDIM eta=0 (reference stablediffusion/mod.rs:423-428)
+      const float predx0 = (xv - e * sqrt_1ma) / sqrt_a;
+      x[i] = predx0 * sqrt_ap + e * sqrt_1map;
+    }
   }
 }
 int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag, float guidance,
-                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x) {
+                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x, const Prediction& pr) {
   const long total = (long)Bimg * C * HW;
-  cfg_ddim_kernel<<<cdiv(total, 256), 256, 0, st>>>(eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sqrt_a, sqrt_1ma,
-                                                     sqrt_ap, sqrt_1map, x);
+  auto kernel = pr.v ? (pr.factor ? cfg_ddim_kernel<true, true> : cfg_ddim_kernel<true, false>)
+                     : (pr.factor ? cfg_ddim_kernel<false, true> : cfg_ddim_kernel<false, false>);
+  kernel<<<cdiv(total, 256), 256, 0, st>>>(eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map,
+                                           x, pr.factor);
+  return (int)cudaGetLastError();
+}
+
+// ------------------------------------------------------------------------------------------------
+// Guidance rescale statistics (kernels.h: guidance_stats_launch). Grid (blocks per image, Bimg); each thread runs Welford's update in
+// double over a fixed set of elements of its image, then warps and blocks merge (n, mean, M2) with Chan et al.'s formula in a fixed
+// order (the last block's warp 0 merges the block partials), so the result is the same on every run and stays exact when
+// |mean| >> std. The guided value repeats the step kernels'
+// expressions (cfg_ddim_kernel, guided_step_kernel) term for term, so it is the value the step then scales.
+// ------------------------------------------------------------------------------------------------
+static constexpr int kGsThreads = 256, kGsMaxBlocks = 128, kGsPerThread = 2;
+struct Moments {
+  double n, mean, m2;
+};
+__device__ __forceinline__ void welford(Moments& m, double x) {
+  m.n += 1.0;
+  const double d = x - m.mean;
+  m.mean += d / m.n;
+  m.m2 += d * (x - m.mean);
+}
+__device__ __forceinline__ Moments chan_merge(const Moments& a, const Moments& b) {
+  const double n = a.n + b.n;
+  if (n == 0.0) return a;
+  const double d = b.mean - a.mean;
+  return {n, a.mean + d * (b.n / n), a.m2 + b.m2 + d * d * (a.n * b.n / n)};
+}
+__device__ __forceinline__ Moments shfl_down(const Moments& m, int o) {
+  return {__shfl_down_sync(0xffffffffu, m.n, o), __shfl_down_sync(0xffffffffu, m.mean, o), __shfl_down_sync(0xffffffffu, m.m2, o)};
+}
+// scratch layout: [Bimg] arrival counters (zero between launches), padded to 16 bytes | [Bimg][kGsMaxBlocks][2] block partials (c, g)
+static inline size_t gs_counter_bytes(int Bimg) { return ((size_t)Bimg * sizeof(unsigned) + 15) & ~(size_t)15; }
+size_t guidance_stats_scratch_bytes(int Bimg) { return gs_counter_bytes(Bimg) + (size_t)Bimg * kGsMaxBlocks * 2 * sizeof(Moments); }
+int guidance_stats_scratch_init(cudaStream_t st, void* scratch, int Bimg) {
+  return (int)cudaMemsetAsync(scratch, 0, gs_counter_bytes(Bimg), st);
+}
+__global__ void __launch_bounds__(kGsThreads) guidance_stats_kernel(const float* __restrict__ eps, int ld, int Bimg, int C, int HW,
+                                                                     int use_pag, float g, float p_t, float phi, unsigned* counters,
+                                                                     Moments* partial, float* __restrict__ factor) {
+  const int b = blockIdx.y, nb = gridDim.x;
+  const long n = (long)C * HW;
+  const int ptb_row0 = 2 * Bimg;
+  Moments mc{0, 0, 0}, mg{0, 0, 0};
+  for (long i = (long)blockIdx.x * kGsThreads + threadIdx.x; i < n; i += (long)nb * kGsThreads) {   // NHWC order within the image
+    const int p = (int)(i / C);
+    const int c = (int)(i % C);
+    const float ec = eps[((size_t)b * HW + p) * ld + c];
+    const float eu = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
+    float e = eu + (ec - eu) * g;
+    if (use_pag) {
+      const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
+      e = e + p_t * (ec - ep);
+    }
+    welford(mc, ec);
+    welford(mg, e);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const Moments oc = shfl_down(mc, o), og = shfl_down(mg, o);
+    mc = chan_merge(mc, oc);
+    mg = chan_merge(mg, og);
+  }
+  __shared__ Moments s_warp[kGsThreads / 32][2];
+  __shared__ unsigned s_ticket;
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  if (lane == 0) {
+    s_warp[warp][0] = mc;
+    s_warp[warp][1] = mg;
+  }
+  __syncthreads();
+  Moments* mine = partial + ((size_t)b * kGsMaxBlocks + blockIdx.x) * 2;
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kGsThreads / 32; ++w) {
+      mc = chan_merge(mc, s_warp[w][0]);
+      mg = chan_merge(mg, s_warp[w][1]);
+    }
+    mine[0] = mc;
+    mine[1] = mg;
+    __threadfence();   // this block's partials are visible device-wide before it takes its ticket
+    s_ticket = atomicAdd(&counters[b], 1u);
+  }
+  __syncthreads();
+  if (s_ticket != (unsigned)(nb - 1) || warp != 0) return;
+  // the last block of image b: lane l merges block partials [l * per, (l + 1) * per) in order, then the lanes merge as above
+  __threadfence();
+  const Moments* all = partial + (size_t)b * kGsMaxBlocks * 2;
+  const int per = (nb + 31) / 32;
+  Moments c_all{0, 0, 0}, g_all{0, 0, 0};
+  for (int k = lane * per; k < (lane + 1) * per && k < nb; ++k) {
+    const Moments pc{__ldcg(&all[2 * k].n), __ldcg(&all[2 * k].mean), __ldcg(&all[2 * k].m2)};
+    const Moments pg{__ldcg(&all[2 * k + 1].n), __ldcg(&all[2 * k + 1].mean), __ldcg(&all[2 * k + 1].m2)};
+    c_all = chan_merge(c_all, pc);
+    g_all = chan_merge(g_all, pg);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const Moments oc = shfl_down(c_all, o), og = shfl_down(g_all, o);
+    c_all = chan_merge(c_all, oc);
+    g_all = chan_merge(g_all, og);
+  }
+  if (lane != 0) return;
+  double ratio = 1.0;
+  if (n > 1 && g_all.m2 > 0.0) ratio = sqrt(c_all.m2 / g_all.m2);   // std(c) / std(g): the (n - 1) divisors cancel
+  factor[b] = (float)((double)phi * ratio + (1.0 - (double)phi));
+  counters[b] = 0u;   // ready for the next launch
+}
+int guidance_stats_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_pag, float guidance, float p_t,
+                          float phi, void* scratch, float* factor) {
+  const long n = (long)C * HW;
+  if (Bimg < 1 || n < 1) return (int)cudaErrorInvalidValue;
+  const int want = cdiv(n, (long)kGsThreads * kGsPerThread), nb = want < kGsMaxBlocks ? want : kGsMaxBlocks;
+  guidance_stats_kernel<<<dim3(nb, Bimg), kGsThreads, 0, st>>>(eps, ld, Bimg, C, HW, use_pag, guidance, p_t, phi, (unsigned*)scratch,
+                                                               (Moments*)((uint8_t*)scratch + gs_counter_bytes(Bimg)), factor);
   return (int)cudaGetLastError();
 }
 
@@ -589,7 +712,9 @@ __device__ __forceinline__ void store4(float* __restrict__ p, size_t blk, size_t
       if (blk * 4 + j < n) p[blk * 4 + j] = v[j];
   }
 }
-__global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams p, int aligned) {
+// kV, kRescale: kernels.h Prediction; <false, false> is the epsilon step and never reads `pr`.
+template <bool kV, bool kRescale>
+__global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams p, int aligned, const Prediction pr) {
   const size_t n = (size_t)p.Bimg * p.C * p.HW, nblk = (n + 3) / 4;
   const size_t blk = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (blk >= nblk) return;
@@ -616,7 +741,9 @@ __global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams
         const float ep = p.eps[((size_t)(grp_p + b) * p.HW + px) * p.ld + c];
         e = e + p.p_t * (ec - ep);
       }
-      D[j] = xh[j] - p.sigma * e;
+      if constexpr (kRescale) e *= pr.factor[b];
+      if constexpr (kV) D[j] = pr.dx * xh[j] - pr.de * e;
+      else D[j] = xh[j] - p.sigma * e;
     }
   } else {
 #pragma unroll
@@ -651,12 +778,14 @@ __global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams
   for (int j = 0; j < 4; ++j) nx[j] *= p.c_in;
   store4(p.x_in, blk, n, vec, nx);
 }
-int guided_step_launch(cudaStream_t st, const GuidedStepParams& p) {
+int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr) {
   const size_t n = (size_t)p.Bimg * p.C * p.HW;
   if (!n) return 0;
   if (!p.xh || !p.x_in || ((p.ch != 0.f || p.write_hist) && !p.hist) || (p.mask && !p.ref)) return (int)cudaErrorInvalidValue;
   const uintptr_t a = (uintptr_t)p.xh | (uintptr_t)p.x_in | (uintptr_t)p.hist | (uintptr_t)p.z | (uintptr_t)p.zb | (uintptr_t)p.ref;
-  guided_step_kernel<<<cdiv((long)((n + 3) / 4), 256), 256, 0, st>>>(p, a % 16 == 0);
+  auto kernel = pr.v ? (pr.factor ? guided_step_kernel<true, true> : guided_step_kernel<true, false>)
+                     : (pr.factor ? guided_step_kernel<false, true> : guided_step_kernel<false, false>);
+  kernel<<<cdiv((long)((n + 3) / 4), 256), 256, 0, st>>>(p, a % 16 == 0, pr);
   return (int)cudaGetLastError();
 }
 

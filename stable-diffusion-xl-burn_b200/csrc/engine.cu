@@ -240,7 +240,10 @@ struct sdxl_unet : EncoderHalf {
   Norm norm_out;
   Conv conv_out;
   __half* conv_out_w2 = nullptr;   // [O, 2*Ktot] = [W | W]: head conv on the hi/lo-split activation
-  std::vector<double> alphas;  // host copy (f16-stored values widened)
+  std::vector<double> alphas;  // the alphas_cumprod table in effect: alphas_loaded, or the one sdxl_unet_set_prediction gave
+  std::vector<double> alphas_loaded;   // host copy of the record's table (f16-stored values widened)
+  int prediction = SDXL_PREDICTION_EPSILON;   // sdxl_unet_set_prediction: what the UNet's output is, and guidance rescale's phi
+  float guidance_rescale = 0.f;
   // conditioning state: the retained inputs and the hoisted conditioning; cond.condB / cond.n_ctx are its shape (0: not set)
   Arena imem;
   int ctx_pitch = 0;
@@ -583,6 +586,7 @@ static int unet_load_impl(sdxl_ctx* c, const sdxl_unet_cfg* cfg, const void* pac
         hr.x = raw[i];
         u->alphas[i] = (double)__half2float(__half(hr));
       }
+      u->alphas_loaded = u->alphas;
     }
     return r2;
   });
@@ -2396,6 +2400,39 @@ extern "C" int sdxl_unet_set_deepcache(sdxl_unet* u, const sdxl_deepcache* d) {
 }
 
 // ================================================================================================
+// prediction type, guidance rescale and the noise table (include/sdxl_b200.h: sdxl_unet_set_prediction; DESIGN.md §18)
+// ================================================================================================
+extern "C" int sdxl_unet_set_prediction(sdxl_unet* u, const sdxl_prediction* p) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  if (!p) {
+    u->prediction = SDXL_PREDICTION_EPSILON;
+    u->guidance_rescale = 0.f;
+    u->alphas = u->alphas_loaded;
+    return 0;
+  }
+  // validate everything first: on failure the previous state is unchanged
+  const int N = (int)u->alphas_loaded.size();
+  if (p->type != SDXL_PREDICTION_EPSILON && p->type != SDXL_PREDICTION_V)
+    return fail(c, 5600, "set_prediction: type = %d must be SDXL_PREDICTION_EPSILON (0) or SDXL_PREDICTION_V (1)", p->type);
+  if (!(p->guidance_rescale >= 0.f && p->guidance_rescale <= 1.f))   // also refuses NaN
+    return fail(c, 5601, "set_prediction: guidance_rescale = %g outside [0, 1]", p->guidance_rescale);
+  if (p->n_alphas != 0 && p->n_alphas != N)
+    return fail(c, 5602, "set_prediction: n_alphas = %d must be 0 (the loaded table) or the UNet's %d timesteps", p->n_alphas, N);
+  if (p->n_alphas && !p->alphas_cumprod_host) return fail(c, 5603, "set_prediction: null alphas_cumprod_host with n_alphas = %d", p->n_alphas);
+  for (int i = 0; i < p->n_alphas; ++i) {
+    const double a = p->alphas_cumprod_host[i];
+    if (!(a > 0.0 && a < 1.0) || (i && !(a < p->alphas_cumprod_host[i - 1])))
+      return fail(c, 5604, "set_prediction: alphas_cumprod_host[%d] = %g is not inside (0, 1) and below its predecessor", i, a);
+  }
+  u->prediction = p->type;
+  u->guidance_rescale = p->guidance_rescale;
+  if (p->n_alphas) u->alphas.assign(p->alphas_cumprod_host, p->alphas_cumprod_host + N);
+  else u->alphas = u->alphas_loaded;
+  return 0;
+}
+
+// ================================================================================================
 // UNet::forward
 // ================================================================================================
 // The direct forwards' body: x NCHW [B, C, h, w] in, eps NCHW out, both f16 (sdxl_unet_forward) or both f32.
@@ -2472,6 +2509,8 @@ struct Sampler {
   float* hist = nullptr;
   float* ref = nullptr;
   uint8_t* mask = nullptr;
+  float* rescale = nullptr;    // guidance rescale: the per-image factors [Bimg] and the statistics kernel's scratch
+  void* stats = nullptr;
   __half* cond_ctx = nullptr;  // staged [nfwd*Bimg, n_ctx, ctx]
   __half* cond_y = nullptr;
   float* host_stage = nullptr;  // pinned
@@ -2520,11 +2559,14 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
           S->hist = A.get<float>(lat);
           S->ref = A.get<float>(lat);
           S->mask = A.get<uint8_t>(lat);
+          S->rescale = A.get<float>(Bimg);
+          S->stats = A.get<uint8_t>(guidance_stats_scratch_bytes(Bimg));
           S->cond_ctx = A.get<__half>(ctx_elems);
           S->cond_y = A.get<__half>(y_elems);
           return 0;
         }))
       return r;
+    KL(c, guidance_stats_scratch_init(c->stream, S->stats, Bimg));
     CU(c, cudaMallocHost((void**)&S->host_stage, lat * sizeof(float)));
   }
   S->guidance = (float)guidance;
@@ -2567,6 +2609,27 @@ static float pag_scale(const sdxl_unet* u, double t) {
   return std::max(u->pag->scale - u->pag->adaptive * (float)(u->cfg.n_steps - t), 0.f);
 }
 
+// What the step kernel after this evaluation reads the UNet's output as (kernels.h: Prediction), at noise level sigma for the guided
+// step. With guidance rescale on a call that has CFG rows, the statistics kernel first writes the per-image factors.
+static int step_prediction(sdxl_unet* u, float p_t, double sigma, Prediction& pr) {
+  sdxl_ctx* c = u->ctx;
+  Sampler* S = u->sampler.get();
+  Plan* P = u->plan.get();
+  pr = Prediction{};
+  if (u->guidance_rescale > 0.f && S->cfg) {
+    KL(c, guidance_stats_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->pag, S->guidance, p_t,
+                                u->guidance_rescale, S->stats, S->rescale));
+    pr.factor = S->rescale;
+  }
+  if (u->prediction == SDXL_PREDICTION_V) {
+    const DScale q = d_scale(SDXL_PREDICTION_V, sigma);
+    pr.v = 1;
+    pr.dx = q.dx;
+    pr.de = q.de;
+  }
+  return 0;
+}
+
 // one loop-body iteration (reference stablediffusion/mod.rs:406-429)
 static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   sdxl_ctx* c = u->ctx;
@@ -2579,9 +2642,11 @@ static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   int r = set_t(u, t);
   if (r) return r;
   if ((r = run_sampler_plan(u))) return r;
-  KL(c, cfg_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->cfg, S->pag, S->guidance,
-                        S->pag ? pag_scale(u, t) : 0.f, (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap),
-                        P->x_in));
+  const float p_t = S->pag ? pag_scale(u, t) : 0.f;
+  Prediction pr;
+  if ((r = step_prediction(u, p_t, sqrt((1.0 - a) / a), pr))) return r;
+  KL(c, cfg_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->cfg, S->pag, S->guidance, p_t,
+                        (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap), P->x_in, pr));
   return 0;
 }
 
@@ -2841,7 +2906,9 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
       p.sigma_blend = (float)sig[k + 1];
       feed.next(p.zb, p.zb_subseq);
     }
-    KL(c, guided_step_launch(c->stream, p));
+    Prediction pr;
+    if ((r = step_prediction(u, p.p_t, sig[k], pr))) return r;
+    KL(c, guided_step_launch(c->stream, p, pr));
   }
   return sample_end(u, cond, S->xh, latent_out);
 }

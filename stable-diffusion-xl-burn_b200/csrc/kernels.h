@@ -232,8 +232,28 @@ int nhwc_to_nchw_f32_launch(cudaStream_t st, const float* x, int B, int HW, int 
 // eps layout: NHWC f32 [nfwd*Bimg, HW, ld]; cond rows first, then uncond (if cfg).
 // x: NCHW f32 master latent [Bimg,C,HW], updated in place. use_pag (DESIGN.md §14): a last group of Bimg perturbed rows follows,
 // eps rows [cond | uncond | ptb] (use_cfg) or [cond | ptb], and e = (u + (c - u) * guidance) + p_t * (c - ptb), resp. c + p_t * (c - ptb).
+// What the guided model output g of the two step kernels is (DESIGN.md §18). The default is the epsilon prediction without
+// guidance rescale, the kernels' first instantiation.
+//   v       g is the v prediction: cfg_ddim takes x0 = sqrt_a * x - sqrt_1ma * g and eps = sqrt_a * g + sqrt_1ma * x, the guided
+//           step D = dx * xh - de * g (schedule.h: d_scale)
+//   factor  per-image guidance-rescale factors [Bimg] on the device (guidance_stats_launch): g = g * factor[b] before its use
+struct Prediction {
+  int v = 0;
+  const float* factor = nullptr;
+  float dx = 0.f, de = 0.f;
+};
 int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag, float guidance,
-                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x);
+                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x, const Prediction& pr = {});
+// Guidance rescale (diffusers' rescale_noise_cfg, Lin et al. 2023): for each image b of the rows [cond | uncond] or
+// [cond | uncond | ptb], with c_b its conditional output and g_b its guided output as the step kernels compute them,
+//   factor[b] = phi * std(c_b) / std(g_b) + (1 - phi)   (unbiased std over C * HW; std(c_b) / std(g_b) read as 1 when std(g_b) = 0)
+// One launch: per-block (n, mean, M2) partials in double, merged in block order by the last block of each image (an arrival
+// counter orders the blocks; no value goes through an atomic). scratch: guidance_stats_scratch_bytes(Bimg) bytes, initialised once
+// with guidance_stats_scratch_init.
+size_t guidance_stats_scratch_bytes(int Bimg);
+int guidance_stats_scratch_init(cudaStream_t st, void* scratch, int Bimg);
+int guidance_stats_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_pag, float guidance, float p_t,
+                          float phi, void* scratch, float* factor);
 // PAG's identity self-attention on `rows` token rows: out[r, 0:C] = qkv[r, 2C:3C] (qkv row pitch 3C, out row pitch C); C % 8 == 0,
 // both pointers 16-byte aligned.
 int pag_identity_launch(cudaStream_t st, const __half* qkv, int C, long rows, __half* out);
@@ -246,7 +266,7 @@ int axpby_launch(cudaStream_t st, float* x, const float* noise, size_t n, float 
 int randn_launch(cudaStream_t st, float* out, size_t n, uint64_t seed, uint64_t subseq);
 // One step of a scheduled sampler (DESIGN.md §16) on the k-diffusion-scaled state xh, f32 NCHW [Bimg, C, HW], in one launch:
 //   e   = guided eps of the NHWC rows [cond], [cond | uncond], [cond | ptb] or [cond | uncond | ptb] (cfg_ddim's combines)
-//   D   = xh - sigma * e                          (eps == nullptr: no model output, D = xh: the entry of a call)
+//   D   = xh - sigma * e                          (eps == nullptr: no model output, D = xh: the entry of a call; v: Prediction)
 //   xh' = cx * xh + cd * D + ch * hist + cn * z   (hist read when ch != 0, then D written to it when write_hist)
 //   xh' = mask ? xh' : ref + sigma_blend * zb     (mask != nullptr: the latent blend before the next forward)
 //   x_in = c_in * xh'                             (the next forward's input)
@@ -267,7 +287,7 @@ struct GuidedStepParams {
   const float* ref;
   float sigma_blend;
 };
-int guided_step_launch(cudaStream_t st, const GuidedStepParams& p);
+int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr = {});
 
 // Latent-decoder kernels (vae_kernels.cu)
 // P[r,:] = softmax(scale * S[r,:]); S f32 [rows, lds] -> P f16 [rows, ldp]; cols % 4 == 0.

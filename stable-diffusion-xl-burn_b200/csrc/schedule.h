@@ -95,8 +95,17 @@ inline void schedule_fill(const SigmaTable& T, const sdxl_schedule& s, double* t
 }
 
 // The sampler layer. Step k of the schedule takes the state xh at sigma_k to sigma_{k+1}:
-//   xh' = cx * xh + cd * D + ch * D_prev + cn * z,   D = xh - sigma_k * eps,   x_in' = c_in * xh'
+//   xh' = cx * xh + cd * D + ch * D_prev + cn * z,   D = xh - sigma_k * eps (d_scale),   x_in' = c_in * xh'
 // `has_prev`: D of step k - 1 is in the history buffer (false on the first step of a call).
+// The denoised latent D = dx * xh - de * g of the model output g at sigma (DESIGN.md §18), in double: an epsilon model gives
+// D = xh - sigma * eps (the step kernel's own expression, dx = 1, de = sigma), a v model D = xh / (sigma^2 + 1) - sigma / sqrt(sigma^2 + 1) * v.
+struct DScale {
+  float dx, de;
+};
+inline DScale d_scale(int prediction, double sigma) {
+  if (prediction != SDXL_PREDICTION_V) return {1.f, (float)sigma};
+  return {(float)(1.0 / (sigma * sigma + 1.0)), (float)(sigma / sqrt(sigma * sigma + 1.0))};
+}
 struct StepCoef {
   float cx, cd, ch, cn, c_in;
 };

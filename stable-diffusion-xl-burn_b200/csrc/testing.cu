@@ -242,6 +242,25 @@ SDXL_TEST_API int sdxl_test_cfg_ddim(void* stream, const float* eps, int ld, int
   return cfg_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap,
                          sqrt_1map, x);
 }
+// The same with the v prediction (v != 0) and the per-image guidance-rescale factors (factor nullable), kernels.h: Prediction.
+SDXL_TEST_API int sdxl_test_cfg_ddim_pred(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
+                                          float guidance, float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
+                                          float* x, int v, const float* factor) {
+  Prediction pr;
+  pr.v = v;
+  pr.factor = factor;
+  return cfg_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap,
+                         sqrt_1map, x, pr);
+}
+// Guidance rescale's statistics kernel (engine.cu: step_prediction) on a scratch initialised once, as the sampler's; factor [Bimg] out.
+SDXL_TEST_API size_t sdxl_test_guidance_stats_scratch_bytes(int Bimg) { return guidance_stats_scratch_bytes(Bimg); }
+SDXL_TEST_API int sdxl_test_guidance_stats_scratch_init(void* stream, void* scratch, int Bimg) {
+  return guidance_stats_scratch_init((cudaStream_t)stream, scratch, Bimg);
+}
+SDXL_TEST_API int sdxl_test_guidance_stats(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_pag, float guidance,
+                                           float p_t, float phi, void* scratch, float* factor) {
+  return guidance_stats_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_pag, guidance, p_t, phi, scratch, factor);
+}
 SDXL_TEST_API int sdxl_test_inpaint_blend(void* stream, float* x, const float* ref, const float* noise, const uint8_t* mask, size_t n,
                                           float sqrt_a, float sqrt_1ma) {
   return inpaint_blend_launch((cudaStream_t)stream, x, ref, noise, mask, n, sqrt_a, sqrt_1ma);
@@ -284,11 +303,13 @@ SDXL_TEST_API void sdxl_test_step_coef(const sdxl_schedule* s, int k, const doub
   const StepCoef q = step_coef(*s, k, timesteps, sigmas, has_prev != 0);
   out[0] = q.cx; out[1] = q.cd; out[2] = q.ch; out[3] = q.cn; out[4] = q.c_in;
 }
-SDXL_TEST_API int sdxl_test_guided_step(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
-                                        float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,
-                                        float* xh, float* x_in, float* hist, int write_hist, const float* z, const float* zb,
-                                        uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq, const uint8_t* mask, const float* ref,
-                                        float sigma_blend) {
+// The same with the prediction type (SDXL_PREDICTION_*: v takes schedule.h's d_scale at sigma, as the engine does) and the per-image
+// guidance-rescale factors (factor nullable).
+SDXL_TEST_API int sdxl_test_guided_step_pred(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
+                                             float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,
+                                             float* xh, float* x_in, float* hist, int write_hist, const float* z, const float* zb,
+                                             uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq, const uint8_t* mask, const float* ref,
+                                             float sigma_blend, int prediction, const float* factor) {
   GuidedStepParams p{};
   p.eps = eps; p.ld = ld; p.Bimg = Bimg; p.C = C; p.HW = HW; p.use_cfg = use_cfg; p.use_pag = use_pag;
   p.guidance = guidance; p.p_t = p_t; p.sigma = sigma;
@@ -296,7 +317,22 @@ SDXL_TEST_API int sdxl_test_guided_step(void* stream, const float* eps, int ld, 
   p.xh = xh; p.x_in = x_in; p.hist = hist; p.write_hist = write_hist;
   p.z = z; p.zb = zb; p.seed = seed; p.z_subseq = z_subseq; p.zb_subseq = zb_subseq;
   p.mask = mask; p.ref = ref; p.sigma_blend = sigma_blend;
-  return guided_step_launch((cudaStream_t)stream, p);
+  Prediction pr;
+  pr.factor = factor;
+  if (prediction == SDXL_PREDICTION_V) {
+    const DScale q = d_scale(prediction, sigma);
+    pr.v = 1; pr.dx = q.dx; pr.de = q.de;
+  }
+  return guided_step_launch((cudaStream_t)stream, p, pr);
+}
+SDXL_TEST_API int sdxl_test_guided_step(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
+                                        float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,
+                                        float* xh, float* x_in, float* hist, int write_hist, const float* z, const float* zb,
+                                        uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq, const uint8_t* mask, const float* ref,
+                                        float sigma_blend) {
+  return sdxl_test_guided_step_pred(stream, eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sigma, cx, cd, ch, cn, c_in, xh, x_in,
+                                    hist, write_hist, z, zb, seed, z_subseq, zb_subseq, mask, ref, sigma_blend, SDXL_PREDICTION_EPSILON,
+                                    nullptr);
 }
 SDXL_TEST_API int sdxl_test_timestep_embedding_f32(void* stream, const float* t, int nt, int dim, float max_period, float* out) {
   return timestep_embedding_f32_launch((cudaStream_t)stream, t, nt, dim, max_period, out);

@@ -124,6 +124,13 @@ class Deepcache(C.Structure):
     _fields_ = [("interval", C.c_int32), ("branch", C.c_int32), ("forward_cached", C.c_int32)]
 
 
+class Prediction(C.Structure):
+    _fields_ = [("type", C.c_int32), ("guidance_rescale", C.c_float), ("n_alphas", C.c_int32), ("alphas_cumprod_host", C.c_void_p)]
+
+
+PREDICTIONS = {"epsilon": 0, "v_prediction": 1}   # SDXL_PREDICTION_* (include/sdxl_b200.h), by diffusers' prediction_type
+
+
 class Schedule(C.Structure):
     _fields_ = [("sampler", C.c_int32), ("spacing", C.c_int32), ("n_steps", C.c_int32), ("first_step", C.c_int32),
                 ("last_step", C.c_int32), ("renoise", C.c_int32), ("no_cfg", C.c_int32), ("karras_rho", C.c_float),
@@ -219,6 +226,7 @@ PROTOTYPES = {
     "sdxl_unet_set_pag": (I, [P, C.POINTER(Pag)]),
     "sdxl_unet_set_freeu": (I, [P, C.POINTER(Freeu)]),
     "sdxl_unet_set_deepcache": (I, [P, C.POINTER(Deepcache)]),
+    "sdxl_unet_set_prediction": (I, [P, C.POINTER(Prediction)]),
     "sdxl_make_inpaint_mask": (I, [I, I, I, I, I, I, I, I, I, I, P]),
     "sdxl_mpk_decode_u16": (I, [P, C.c_size_t, C.c_size_t, P, C.POINTER(C.c_size_t)]),
     "sdxl_mpk_encode_u16": (C.c_size_t, [P, C.c_size_t, P]),

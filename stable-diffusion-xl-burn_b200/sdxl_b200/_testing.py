@@ -69,6 +69,12 @@ PROTOTYPES = {
     "sdxl_test_step_coef": (None, [P, I, P, P, I, P]),
     "sdxl_test_guided_step": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, F, F, P, P, P, I, P, P, C.c_uint64, C.c_uint64, C.c_uint64, P, P, F]),
     "sdxl_test_timestep_embedding_f32": (I, [P, P, I, I, F, P]),
+    "sdxl_test_cfg_ddim_pred": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, P, I, P]),
+    "sdxl_test_guidance_stats_scratch_bytes": (Z, [I]),
+    "sdxl_test_guidance_stats_scratch_init": (I, [P, P, I]),
+    "sdxl_test_guidance_stats": (I, [P, P, I, I, I, I, I, F, F, F, P, P]),
+    "sdxl_test_guided_step_pred": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, F, F, P, P, P, I, P, P, C.c_uint64, C.c_uint64, C.c_uint64, P,
+                                       P, F, I, P]),
 }
 _lib = None
 
@@ -303,6 +309,25 @@ def cfg_ddim(eps, ld, Bimg, C, HW, use_cfg, guidance, sqrt_a, sqrt_1ma, sqrt_ap,
           _p(x))
 
 
+def cfg_ddim_pred(eps, ld, Bimg, C, HW, use_cfg, guidance, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x, use_pag=False, p_t=0.0, v=False,
+                  factor=None) -> None:
+    """cfg_ddim with the v prediction (v) and the per-image guidance-rescale factors (factor: f32 CUDA [Bimg] or None)."""
+    _call("sdxl_test_cfg_ddim_pred", _p(eps), ld, Bimg, C, HW, int(use_cfg), int(use_pag), guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap,
+          sqrt_1map, _p(x), int(v), _p(factor))
+
+
+def guidance_stats_scratch(Bimg, device="cuda") -> torch.Tensor:
+    """The statistics kernel's scratch for Bimg images, initialised (its arrival counters zero)."""
+    s = torch.empty(int(load().sdxl_test_guidance_stats_scratch_bytes(Bimg)), dtype=torch.uint8, device=device)
+    _call("sdxl_test_guidance_stats_scratch_init", _p(s), Bimg)
+    return s
+
+
+def guidance_stats(eps, ld, Bimg, C, HW, use_pag, guidance, p_t, phi, scratch, factor) -> None:
+    """factor f32 [Bimg] = phi * std(c_b) / std(g_b) + (1 - phi) of the rows [cond | uncond (| ptb)] of eps (kernels.h)."""
+    _call("sdxl_test_guidance_stats", _p(eps), ld, Bimg, C, HW, int(use_pag), guidance, p_t, phi, _p(scratch), _p(factor))
+
+
 def inpaint_blend(x, ref, noise, mask, n, sqrt_a, sqrt_1ma) -> None:
     _call("sdxl_test_inpaint_blend", _p(x), _p(ref), _p(noise), _p(mask), n, sqrt_a, sqrt_1ma)
 
@@ -353,6 +378,14 @@ def guided_step(eps: Optional[torch.Tensor], ld: int, Bimg: int, Cc: int, HW: in
     """coef = (cx, cd, ch, cn, c_in); xh, x_in and hist are updated in place (kernels.h: GuidedStepParams)."""
     _call("sdxl_test_guided_step", _p(eps), ld, Bimg, Cc, HW, int(use_cfg), int(use_pag), guidance, p_t, sigma, *[float(v) for v in coef],
           _p(xh), _p(x_in), _p(hist), int(write_hist), _p(z), _p(zb), seed, z_subseq, zb_subseq, _p(mask), _p(ref), sigma_blend)
+
+
+def guided_step_pred(eps, ld, Bimg, Cc, HW, use_cfg, use_pag, guidance, p_t, sigma, coef, xh, x_in, hist=None, write_hist=False, z=None,
+                     zb=None, seed=0, z_subseq=0, zb_subseq=0, mask=None, ref=None, sigma_blend=0.0, v=False, factor=None) -> None:
+    """guided_step with the v prediction (v: D from schedule.h's d_scale at sigma) and the per-image guidance-rescale factors."""
+    _call("sdxl_test_guided_step_pred", _p(eps), ld, Bimg, Cc, HW, int(use_cfg), int(use_pag), guidance, p_t, sigma,
+          *[float(c) for c in coef], _p(xh), _p(x_in), _p(hist), int(write_hist), _p(z), _p(zb), seed, z_subseq, zb_subseq, _p(mask),
+          _p(ref), sigma_blend, int(v), _p(factor))
 
 
 def timestep_embedding_f32(t: torch.Tensor, dim: int, max_period: float = 10000.0) -> torch.Tensor:

@@ -16,6 +16,7 @@ import ctypes as C
 from dataclasses import dataclass
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -430,12 +431,60 @@ class Diffuser:
             s.interval, s.branch, s.forward_cached = d
         self.ctx.call("sdxl_unet_set_deepcache", self.ctx.lib.sdxl_unet_set_deepcache, self.h, None if s is None else C.byref(s))
 
+    def set_prediction(self, prediction: str = "epsilon", guidance_rescale: float = 0.0, zero_terminal_snr: bool = False,
+                       alphas=None) -> None:
+        """What the sampling loops read the UNet's output as (sdxl_unet_set_prediction, DESIGN.md §18): diffusers' prediction_type
+        ("epsilon" or "v_prediction"), guidance_rescale (phi in [0, 1], diffusers' pipeline argument; calls with CFG rows only) and the
+        noise table: alphas (f64 [cfg.n_steps]) if given, else with zero_terminal_snr schedulers.alphas_cumprod(cfg.n_steps,
+        zero_terminal_snr=True), else the loaded table. The default arguments detach: epsilon, phi 0 and the loaded table."""
+        if prediction not in _lib.PREDICTIONS:
+            raise SdxlError(f"set_prediction: prediction = {prediction!r} is not one of {sorted(_lib.PREDICTIONS)}")
+        if alphas is None and zero_terminal_snr:
+            from .schedulers import alphas_cumprod
+            alphas = alphas_cumprod(self.cfg.n_steps, zero_terminal_snr=True)
+        self._set_prediction((prediction, float(guidance_rescale), None if alphas is None else np.asarray(alphas, dtype=np.float64)))
+
+    def _set_prediction(self, p) -> None:
+        prediction, phi, alphas = p
+        s, a = None, None
+        if prediction != "epsilon" or phi != 0.0 or alphas is not None:
+            s = _lib.Prediction()
+            s.type, s.guidance_rescale = _lib.PREDICTIONS[prediction], phi
+            if alphas is not None:
+                a = np.ascontiguousarray(alphas, dtype=np.float64)
+                s.n_alphas, s.alphas_cumprod_host = a.size, a.ctypes.data
+        self.ctx.call("sdxl_unet_set_prediction", self.ctx.lib.sdxl_unet_set_prediction, self.h, None if s is None else C.byref(s))
+        self._prediction = (prediction, phi, alphas)
+
+    @property
+    def prediction(self):
+        """(prediction, guidance_rescale, alphas or None) as set_prediction last set them."""
+        return getattr(self, "_prediction", ("epsilon", 0.0, None))
+
     @classmethod
     def from_diffusers_dir(cls, ctx: Context, path: str) -> "Diffuser":
         """A diffusers UNet2DConditionModel directory (the `unet/` folder of an SDXL pipeline, base or inpainting): config.json +
-        diffusion_pytorch_model[.fp16].safetensors (diffusers_unet.from_diffusers)."""
+        diffusion_pytorch_model[.fp16].safetensors (diffusers_unet.from_diffusers). When the pipeline's scheduler/scheduler_config.json
+        sits next to it and says prediction_type "v_prediction" or rescale_betas_zero_snr true, the model is set to that prediction
+        and noise table (schedulers.prediction_of_config, set_prediction); prediction_type "sample" and a beta_schedule other than
+        "scaled_linear" are refused."""
+        import json
+        import os
         from .diffusers_unet import from_diffusers, read_model_dir
-        return cls(ctx, *from_diffusers(*read_model_dir(path)))
+        from .schedulers import prediction_of_config
+        sched = os.path.join(os.path.dirname(os.path.normpath(path)), "scheduler", "scheduler_config.json")
+        pred = None
+        if os.path.exists(sched):
+            with open(sched) as f:
+                pred = prediction_of_config(json.load(f))
+        d = cls(ctx, *from_diffusers(*read_model_dir(path)))
+        if pred is not None:
+            try:
+                d.set_prediction(**pred)
+            except Exception:
+                d.close()
+                raise
+        return d
 
     # ---- UNet::forward -------------------------------------------------------------------------
     def set_conditioning(self, context: torch.Tensor, label: torch.Tensor) -> None:

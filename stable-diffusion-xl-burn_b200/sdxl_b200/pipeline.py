@@ -55,7 +55,7 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
            loras: Optional[Sequence] = None, controls: Optional[Sequence] = None, image_prompt: Optional[Sequence] = None,
            t2i_adapters: Optional[Sequence] = None, t2i_factor: float = 1.0, pag: Optional[Sequence] = None,
            freeu: Optional[Sequence[float]] = None, sampler: Optional[str] = None, spacing: Optional[str] = None,
-           no_cfg: bool = False, deepcache: Optional[Sequence[int]] = None) -> torch.Tensor:
+           no_cfg: bool = False, deepcache: Optional[Sequence[int]] = None, guidance_rescale: float = 0.0) -> torch.Tensor:
     """One image, like `sample --prompt ... [--reference-img ... --crop-* ...] [--use-refiner]`.
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
     bottom) in pixels. With an inpainting UNet (cfg.is_inpaint, DESIGN.md §12) reference_rgb is required: the crop window becomes the
@@ -78,8 +78,18 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     schedulers.Schedule of n_steps for the base model; a refiner then runs the same schedule from the first step whose timestep is
     below 1000 - REFINER_STEP_START, re-noising the base latent to that step's sigma. All three None / False: the reference's DDIM
     loop. deepcache: (interval[, branch]) DeepCache (Diffuser.set_deepcache) attached to the base UNet for this call and detached
-    afterwards (the refiner is left alone). Returns uint8 [1, H, W, 3]."""
+    afterwards (the refiner is left alone). guidance_rescale: diffusers' guidance_rescale (phi, DESIGN.md §18) set on the base UNet
+    for this call, with the prediction type and noise table the model has (Diffuser.set_prediction), and the previous phi restored
+    afterwards. Returns uint8 [1, H, W, 3]."""
     sch = dict(sampler=sampler, spacing=spacing, no_cfg=no_cfg)
+    if guidance_rescale:
+        prev = diffuser.prediction
+        diffuser.set_prediction(prev[0], guidance_rescale, alphas=prev[2])
+        try:
+            return sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
+                          seed, noise, loras, controls, image_prompt, t2i_adapters, t2i_factor, pag, freeu, deepcache=deepcache, **sch)
+        finally:
+            diffuser.set_prediction(prev[0], prev[1], alphas=prev[2])
     if deepcache:
         diffuser.set_deepcache(*deepcache)
         try:

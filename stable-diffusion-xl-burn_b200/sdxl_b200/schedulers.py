@@ -56,6 +56,44 @@ class Schedule:
         return n
 
 
+def alphas_cumprod(n: int = 1000, beta_start: float = 0.00085, beta_end: float = 0.012, zero_terminal_snr: bool = False) -> np.ndarray:
+    """alphas_cumprod f64 [n] of diffusers' scaled-linear betas, computed as diffusers computes it, in float32. zero_terminal_snr:
+    the betas rescaled to zero terminal SNR first (Lin et al. 2023, Algorithm 1: diffusers' rescale_zero_terminal_snr) and the last
+    entry set to 2^-24, as diffusers' Euler and DPM-Solver schedulers do (rescale_betas_zero_snr=True). For
+    Diffuser.set_prediction (DESIGN.md §18)."""
+    import torch
+    betas = torch.linspace(beta_start ** 0.5, beta_end ** 0.5, n, dtype=torch.float32) ** 2
+    if zero_terminal_snr:
+        sqrt_bar = torch.cumprod(1.0 - betas, dim=0).sqrt()
+        first, last = sqrt_bar[0].clone(), sqrt_bar[-1].clone()
+        sqrt_bar = (sqrt_bar - last) * (first / (first - last))   # sqrt(alpha_bar) from sqrt(alpha_bar_0) down to 0
+        bar = sqrt_bar ** 2
+        betas = 1.0 - torch.cat([bar[0:1], bar[1:] / bar[:-1]])
+    a = torch.cumprod(1.0 - betas, dim=0)
+    if zero_terminal_snr:
+        a[-1] = 2.0 ** -24
+    return a.double().numpy()
+
+
+def prediction_of_config(config: dict):
+    """Diffuser.set_prediction's keyword arguments for a diffusers scheduler_config.json (read as a dict), or None when the model is
+    an epsilon model on the loaded noise table. Attaches only for prediction_type "v_prediction" or rescale_betas_zero_snr true, with
+    the file's betas (diffusers' defaults where a key is missing). Refuses prediction_type "sample" and any other unknown type, and a
+    beta_schedule other than "scaled_linear" when it attaches, naming the key."""
+    kind = config.get("prediction_type", "epsilon")
+    if kind not in _lib.PREDICTIONS:
+        raise _lib.SdxlError(f"scheduler config: prediction_type = {kind!r} is not supported (one of {sorted(_lib.PREDICTIONS)})")
+    zero_snr = bool(config.get("rescale_betas_zero_snr", False))
+    if kind == "epsilon" and not zero_snr:
+        return None
+    if config.get("beta_schedule", "linear") != "scaled_linear":
+        raise _lib.SdxlError(f"scheduler config: beta_schedule = {config.get('beta_schedule', 'linear')!r} is not supported (only "
+                             f"'scaled_linear')")
+    alphas = alphas_cumprod(int(config.get("num_train_timesteps", 1000)), float(config.get("beta_start", 0.0001)),
+                            float(config.get("beta_end", 0.02)), zero_snr)
+    return dict(prediction=kind, zero_terminal_snr=zero_snr, alphas=alphas)
+
+
 def build(alphas: Sequence[float], schedule: Schedule) -> Tuple[np.ndarray, np.ndarray]:
     """(timesteps f64 [n_steps], sigmas f64 [n_steps + 1]) of `schedule` over an alphas_cumprod table (sdxl_schedule_build)."""
     lib = _lib.load()
