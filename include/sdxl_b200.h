@@ -386,7 +386,27 @@ SDXL_API double sdxl_clip_plan_flops(const sdxl_clip* clip);
  * layer, dtype, shapes, equal rank of down and up) before any weight is written: on failure the call returns non-zero, names the
  * tensor in sdxl_last_error and the model is unchanged. The first touch of a layer copies it to a device backup held until
  * n = 0 or destroy. The launch plan and its CUDA graph stay valid; for the UNet the hoisted conditioning (cross-attention K/V,
- * label MLP) is recomputed when conditioning is set. At most SDXL_MAX_ADAPTERS adapters per call. Queued on the ctx stream. */
+ * label MLP) is recomputed when conditioning is set. At most SDXL_MAX_ADAPTERS adapters per call. Queued on the ctx stream.
+ * Other families (DESIGN.md §19). Per layer an adapter holds exactly one delta family and optional modifiers; logical shapes are
+ * [N, Kd], Kd = I*kh*kw in PyTorch order (i, kh, kw):
+ *   LoRA   lora_down, lora_up (above)                                  P = up @ down                     c = alpha / r
+ *   LoHa   hada_w1_a [N, r], hada_w1_b [r, Kd] or [r, I, kh, kw],      P = (w1_a @ w1_b) * (w2_a @ w2_b)  c = alpha / r
+ *          hada_w2_a [N, r'], hada_w2_b [r', Kd] or [r', I, kh, kw]                                         (r: rows of hada_w1_b)
+ *   LoKr   lokr_w1 [a, b] or lokr_w1_a [a, r] + lokr_w1_b [r, b];      P[i*c+j, (p*d+q)*taps+t] = w1[i,p] * w2[j, q*taps+t],
+ *          lokr_w2 [c, d(,kh,kw)] or lokr_w2_a [c, r] + lokr_w2_b      a*c = N, b*d = I;  c = alpha / r if a factor is a
+ *          [r, d(,kh,kw)] or [r, d*kh*kw]                              product (r its rank), else 1 (alpha ignored)
+ *   full   diff [N, I(,kh,kw)] or [N, Kd]                              P = diff                          c = 1
+ * all f16. Modifiers: alpha (one element; missing => alpha = r) and dora_scale m (f32; LoRA, LoHa, LoKr): [N], [N,1] or [N,1,1,1]
+ * takes the norm n per output row over Kd; [1,I] or [1,I,1,1] per input channel over N and the taps. With scale s_a:
+ *   C_a = s_a * c_a * P_a                              (no dora_scale: the LoRA term above; a negative alpha is used as given)
+ *   C_a = s_a * (m_a * V_a / n_a - W), V_a = W + c_a * P_a   (dora_scale; 0 where n_a = 0; no epsilon)
+ *   W'  = f16(f32(W) + sum C), non-DoRA terms in call order, then DoRA terms in call order; a zero sum keeps W's bits.
+ * Norms and DoRA terms are computed in double in a fixed order. Refused, with nothing changed and the layer and tensor named:
+ * 4615 two families on one layer, 4616 an incomplete family, 4617 a factor of the wrong shape, 4618 ranks that do not agree
+ * (within a factor pair, or the two LoKr factors when both are given as products: alpha / r needs one r),
+ * 4619 LoKr factors whose Kronecker product is not [N, I], 4620 a dora_scale of another shape, 4621 a dora_scale on a layer
+ * without a delta, 4622 a dora_scale on an upsample conv (its 3x3 weight is not retained, so n cannot be taken), 4623 a
+ * dora_scale that is not f32, 4624 scratch that cannot be allocated. Factors other than f16 are refused with 4607. */
 #define SDXL_MAX_ADAPTERS 16
 typedef struct sdxl_adapter {
   const void* pack;        /* SDXLPK01 pack, host or device memory (pack_on_device); borrowed for the call */

@@ -896,6 +896,44 @@ int bias_to_f32_launch(cudaStream_t st, const __half* src, int N, float* dst, in
 // fixed order (terms in call order, rank index ascending): deterministic, no atomics. CUDA-core FMA (see DESIGN.md).
 // ------------------------------------------------------------------------------------------------
 constexpr int LORA_TILE = 64, LORA_RC = 32;
+// acc[i][j] = sum_r up[n, r] * down[r, k] over the tile's outputs, rank index ascending
+__device__ __forceinline__ void lora_rank_product(float (&acc)[4][4], float (*Us)[LORA_TILE + 1], float (*Ds)[LORA_TILE],
+                                                  const __half* __restrict__ up, const __half* __restrict__ down, int R,
+                                                  int N, int Kd, int n0, int k0) {
+  const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
+#pragma unroll
+  for (int i = 0; i < 4; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+  for (int r0 = 0; r0 < R; r0 += LORA_RC) {
+    const int rc = R - r0 < LORA_RC ? R - r0 : LORA_RC;
+    __syncthreads();
+    for (int e = tid; e < LORA_RC * LORA_TILE; e += 256) {
+      {  // up [N, r] row-major: consecutive threads read consecutive ranks of one row
+        const int x = e / LORA_RC, rr = e % LORA_RC, n = n0 + x;
+        Us[rr][x] = (rr < rc && n < N) ? __half2float(up[(size_t)n * R + r0 + rr]) : 0.f;
+      }
+      {
+        const int rr = e / LORA_TILE, x = e % LORA_TILE, k = k0 + x;
+        Ds[rr][x] = (rr < rc && k < Kd) ? __half2float(down[(size_t)(r0 + rr) * Kd + k]) : 0.f;
+      }
+    }
+    __syncthreads();
+    for (int rr = 0; rr < rc; ++rr) {
+      float a[4], b[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) a[i] = Us[rr][ty + 16 * i];
+#pragma unroll
+      for (int j = 0; j < 4; ++j) b[j] = Ds[rr][tx + 16 * j];
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+    }
+  }
+}
+// kMixed = false: every term is LORA_LORA (the kind field is not read).
+template <bool kMixed>
 __global__ void __launch_bounds__(256) lora_merge_kernel(const LoraMergeParams p) {
   __shared__ float Us[LORA_RC][LORA_TILE + 1];   // +1: the staging stores walk rr at fixed x
   __shared__ float Ds[LORA_RC][LORA_TILE];
@@ -909,35 +947,36 @@ __global__ void __launch_bounds__(256) lora_merge_kernel(const LoraMergeParams p
   for (int t = 0; t < p.nterm; ++t) {
     const LoraTerm T = p.term[t];
     float acc[4][4];
-#pragma unroll
-    for (int i = 0; i < 4; ++i)
-#pragma unroll
-      for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
-    for (int r0 = 0; r0 < T.r; r0 += LORA_RC) {
-      const int rc = T.r - r0 < LORA_RC ? T.r - r0 : LORA_RC;
-      __syncthreads();
-      for (int e = tid; e < LORA_RC * LORA_TILE; e += 256) {
-        {  // up [N, r] row-major: consecutive threads read consecutive ranks of one row
-          const int x = e / LORA_RC, rr = e % LORA_RC, n = n0 + x;
-          Us[rr][x] = (rr < rc && n < p.N) ? __half2float(T.up[(size_t)n * T.r + r0 + rr]) : 0.f;
-        }
-        {
-          const int rr = e / LORA_TILE, x = e % LORA_TILE, k = k0 + x;
-          Ds[rr][x] = (rr < rc && k < p.Kd) ? __half2float(T.down[(size_t)(r0 + rr) * p.Kd + k]) : 0.f;
-        }
-      }
-      __syncthreads();
-      for (int rr = 0; rr < rc; ++rr) {
-        float a[4], b[4];
-#pragma unroll
-        for (int i = 0; i < 4; ++i) a[i] = Us[rr][ty + 16 * i];
-#pragma unroll
-        for (int j = 0; j < 4; ++j) b[j] = Ds[rr][tx + 16 * j];
+    if (!kMixed || T.kind == LORA_LORA || T.kind == LORA_LOHA) {
+      lora_rank_product(acc, Us, Ds, T.up, T.down, T.r, p.N, p.Kd, n0, k0);
+      if (kMixed && T.kind == LORA_LOHA) {
+        float acc2[4][4];
+        lora_rank_product(acc2, Us, Ds, T.up2, T.down2, T.r2, p.N, p.Kd, n0, k0);
 #pragma unroll
         for (int i = 0; i < 4; ++i)
 #pragma unroll
-          for (int j = 0; j < 4; ++j) acc[i][j] = fmaf(a[i], b[j], acc[i][j]);
+          for (int j = 0; j < 4; ++j) acc[i][j] = __fmul_rn(acc[i][j], acc2[i][j]);
       }
+    } else {
+      const int b = p.Kd / p.taps / (T.d > 0 ? T.d : 1);   // LORA_LOKR: columns of w1
+#pragma unroll
+      for (int i = 0; i < 4; ++i)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          const int n = n0 + ty + 16 * i, k = k0 + tx + 16 * j;
+          float v = 0.f;
+          if (n < p.N && k < p.Kd) {
+            if (T.kind == LORA_FULL) {
+              v = __half2float(T.down[(size_t)n * p.Kd + k]);
+            } else if (T.kind == LORA_F32) {
+              v = T.w1[(size_t)n * p.Kd + k];
+            } else {   // LORA_LOKR
+              const int ich = k / p.taps, tap = k % p.taps;
+              v = __fmul_rn(T.w1[(size_t)(n / T.c) * b + ich / T.d], T.w2[(size_t)(n % T.c) * T.d * p.taps + (ich % T.d) * p.taps + tap]);
+            }
+          }
+          acc[i][j] = v;
+        }
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i)
@@ -969,8 +1008,70 @@ __global__ void __launch_bounds__(256) lora_merge_kernel(const LoraMergeParams p
 }
 int lora_merge_launch(cudaStream_t st, const LoraMergeParams& p) {
   if (p.nterm < 1 || p.nterm > LORA_MAX_TERMS || p.taps < 1) return 1;
+  bool mixed = false;
+  for (int t = 0; t < p.nterm; ++t) {
+    const LoraTerm& T = p.term[t];
+    if (T.kind < LORA_LORA || T.kind > LORA_F32) return 1;
+    if (T.kind == LORA_LOKR && (T.c < 1 || T.d < 1 || p.N % T.c || (p.Kd / p.taps) % T.d)) return 1;
+    mixed |= T.kind != LORA_LORA;
+  }
   dim3 grid(cdiv(p.Kd, LORA_TILE), cdiv(p.N, LORA_TILE));
-  lora_merge_kernel<<<grid, 256, 0, st>>>(p);
+  if (mixed) lora_merge_kernel<true><<<grid, 256, 0, st>>>(p);
+  else lora_merge_kernel<false><<<grid, 256, 0, st>>>(p);
+  return (int)cudaGetLastError();
+}
+
+// W of element (n, k) of a slot's logical [N, Kd] matrix (the lora_merge_kernel map), read from p.src
+__device__ __forceinline__ double dora_w(const LoraMergeParams& p, int n, int k) {
+  const size_t off = (size_t)(p.row0 + geglu_perm(n, p.N, p.geglu_bn)) * p.ld + p.col0 + (size_t)(k % p.taps) * p.Ipad + k / p.taps;
+  return p.f32 ? (double)((const float*)p.src)[off] : (double)__half2float(((const __half*)p.src)[off]);
+}
+constexpr int DORA_THREADS = 256;
+// one CTA per norm: thread x sums (W + dw)^2 over the elements x, x + 256, ... of its row (axis 0: k ascending) or input
+// channel (axis 1: e = n * taps + tap ascending) in double, then a fixed tree reduction. No atomics.
+__global__ void __launch_bounds__(DORA_THREADS) dora_norm_kernel(const LoraMergeParams p, const float* __restrict__ dw, int axis,
+                                                                   double* __restrict__ norm) {
+  __shared__ double red[DORA_THREADS];
+  const int j = blockIdx.x;
+  const int len = axis == 0 ? p.Kd : p.N * p.taps;
+  double s = 0.0;
+  for (int e = threadIdx.x; e < len; e += DORA_THREADS) {
+    const int n = axis == 0 ? j : e / p.taps, k = axis == 0 ? e : j * p.taps + e % p.taps;
+    const double v = dora_w(p, n, k) + (double)dw[(size_t)n * p.Kd + k];
+    s = fma(v, v, s);
+  }
+  red[threadIdx.x] = s;
+  __syncthreads();
+  for (int h = DORA_THREADS / 2; h > 0; h >>= 1) {
+    if ((int)threadIdx.x < h) red[threadIdx.x] += red[threadIdx.x + h];
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) norm[j] = sqrt(red[0]);
+}
+int dora_norm_launch(cudaStream_t st, const LoraMergeParams& slot, const float* dw, int axis, double* norm) {
+  if (slot.taps < 1 || slot.N < 1 || slot.Kd < 1) return 1;
+  dora_norm_kernel<<<axis == 0 ? slot.N : slot.Kd / slot.taps, DORA_THREADS, 0, st>>>(slot, dw, axis, norm);
+  return (int)cudaGetLastError();
+}
+__global__ void dora_accum_kernel(const LoraMergeParams p, const float* __restrict__ dw, const float* __restrict__ m,
+                                  const double* __restrict__ norm, int axis, float s, float* __restrict__ acc) {
+  const long total = (long)p.N * p.Kd;
+  for (long e = (long)blockIdx.x * blockDim.x + threadIdx.x; e < total; e += (long)gridDim.x * blockDim.x) {
+    const int n = (int)(e / p.Kd), k = (int)(e % p.Kd);
+    const int j = axis == 0 ? n : k / p.taps;
+    const double nj = norm[j];
+    if (nj == 0.0) continue;
+    const double w = dora_w(p, n, k);
+    const double c = (double)s * ((double)m[j] * (w + (double)dw[e]) / nj - w);
+    acc[e] = __fadd_rn(acc[e], (float)c);
+  }
+}
+int dora_accum_launch(cudaStream_t st, const LoraMergeParams& slot, const float* dw, const float* m, const double* norm, int axis,
+                      float s, float* acc) {
+  if (slot.taps < 1) return 1;
+  const long total = (long)slot.N * slot.Kd;
+  if (total < 1) return 1;
+  dora_accum_kernel<<<(unsigned)cdiv(total, 256), 256, 0, st>>>(slot, dw, m, norm, axis, s, acc);
   return (int)cudaGetLastError();
 }
 // same index map and tap sets as repack_upconv_kernel; padded input channels are not written

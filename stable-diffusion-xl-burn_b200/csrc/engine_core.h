@@ -13,6 +13,7 @@
 #include <stdlib.h>
 #include <string.h>
 
+#include <algorithm>
 #include <map>
 #include <memory>
 #include <string>
@@ -848,14 +849,32 @@ struct TmpBufs {
   ~TmpBufs() { for (void* d : p) cudaFreeAsync(d, st); }
 };
 
+// One adapter's term of one layer: the merge kernel's term (coef = s * c, or c alone for a DoRA term) and, for DoRA, the
+// magnitude m (f32 [N] for axis 0, [I] for axis 1) and the user scale s (DESIGN.md §19).
+struct AdapterTerm {
+  LoraTerm t{};
+  const float* m = nullptr;   // dora_scale; null: not a DoRA term
+  int axis = 0;
+  float s = 0.f;
+};
+
+static std::string shape_str(const PackEntry* e) {
+  std::string r = "[";
+  for (uint32_t i = 0; i < e->ndim && i < 4; ++i) r += (i ? "," : "") + std::to_string((unsigned long long)e->shape[i]);
+  return r + "]";
+}
+
 // Replaces the active adapter set of a model whose slots are registered in S (include/sdxl_b200.h: sdxl_unet_set_adapters).
-// Phase 1 reads and validates every adapter and allocates the backups; nothing is written before it has passed. Phase 2
-// restores the layers merged by the previous call, backs up the newly touched ones and merges. Queued on the ctx stream.
+// Phase 1 reads and validates every adapter, expands LoKr factors given as products into scratch and allocates the backups and
+// the scratch; nothing in the model is written before it has passed. Phase 2 restores the layers merged by the previous call,
+// backs up the newly touched ones and merges. Queued on the ctx stream.
 static int adapters_apply(sdxl_ctx* c, AdapterState& S, int n, const sdxl_adapter* ad) {
   if (n < 0 || n > SDXL_MAX_ADAPTERS) return fail(c, 4600, "set_adapters: n = %d outside [0, %d]", n, SDXL_MAX_ADAPTERS);
   if (n > 0 && !ad) return fail(c, 4601, "set_adapters: null adapter array");
   TmpBufs tmp(c->stream);
-  std::map<std::string, std::vector<LoraTerm>> terms;   // by layer path, adapters in call order
+  std::map<std::string, std::vector<AdapterTerm>> terms;   // by layer path, adapters in call order
+  static const char* kLeaves[] = {"lora_down", "lora_up", "alpha", "dora_scale", "diff", "hada_w1_a", "hada_w1_b", "hada_w2_a",
+                                  "hada_w2_b", "lokr_w1", "lokr_w1_a", "lokr_w1_b", "lokr_w2", "lokr_w2_a", "lokr_w2_b"};
   for (int a = 0; a < n; ++a) {
     PackView pv;
     std::vector<uint8_t> table;
@@ -875,8 +894,11 @@ static int adapters_apply(sdxl_ctx* c, AdapterState& S, int n, const sdxl_adapte
     for (auto& kv : pv.t) {
       const size_t slash = kv.first.rfind('/');
       const std::string leaf = slash == std::string::npos ? kv.first : kv.first.substr(slash + 1);
-      if (slash == std::string::npos || (leaf != "lora_down" && leaf != "lora_up" && leaf != "alpha"))
-        return fail(c, 4604, "adapter %d: tensor '%s' is not <layer>/lora_down, <layer>/lora_up or <layer>/alpha", a, kv.first.c_str());
+      bool known = false;
+      for (const char* l : kLeaves) known |= leaf == l;
+      if (slash == std::string::npos || !known)
+        return fail(c, 4604, "adapter %d: tensor '%s' is not <layer>/lora_down, <layer>/lora_up or <layer>/alpha, nor a LoHa, LoKr, "
+                    "full-delta or dora_scale tensor (DESIGN.md §19)", a, kv.first.c_str());
       layers[kv.first.substr(0, slash)][leaf] = &kv.second;
     }
     for (auto& L : layers) {
@@ -884,27 +906,30 @@ static int adapters_apply(sdxl_ctx* c, AdapterState& S, int n, const sdxl_adapte
       auto it = S.slots.find(path);
       if (it == S.slots.end()) return fail(c, 4605, "adapter %d: '%s' is not a LoRA-able layer of this model", a, path.c_str());
       const WSlot& s = it->second;
-      const PackEntry* dn = L.second.count("lora_down") ? L.second["lora_down"] : nullptr;
-      const PackEntry* up = L.second.count("lora_up") ? L.second["lora_up"] : nullptr;
-      const PackEntry* al = L.second.count("alpha") ? L.second["alpha"] : nullptr;
-      if (!dn || !up) return fail(c, 4606, "adapter %d: '%s/%s' is missing", a, path.c_str(), dn ? "lora_up" : "lora_down");
-      if (dn->dtype != 0) return fail(c, 4607, "adapter %d: '%s/lora_down' must be f16", a, path.c_str());
-      if (up->dtype != 0) return fail(c, 4607, "adapter %d: '%s/lora_up' must be f16", a, path.c_str());
-      const uint64_t rank = dn->ndim ? dn->shape[0] : 0;
-      const bool dn_ok = s.conv ? (dn->ndim == 4 && dn->shape[1] == (uint64_t)s.I && dn->shape[2] == (uint64_t)s.ks && dn->shape[3] == (uint64_t)s.ks)
-                                : (dn->ndim == 2 && dn->shape[1] == (uint64_t)s.I);
-      if (!dn_ok || rank < 1 || rank > 4096)
-        return fail(c, 4608, "adapter %d: '%s/lora_down' has shape [%llu,%llu,%llu,%llu] (ndim %u), expected [r, %d%s]", a, path.c_str(),
-                    (unsigned long long)dn->shape[0], (unsigned long long)dn->shape[1], (unsigned long long)dn->shape[2],
-                    (unsigned long long)dn->shape[3], dn->ndim, s.I, s.conv ? (s.ks == 3 ? ", 3, 3" : ", 1, 1") : "");
-      const bool up_ok = s.conv ? (up->ndim == 4 && up->shape[0] == (uint64_t)s.N && up->shape[2] == 1 && up->shape[3] == 1)
-                                : (up->ndim == 2 && up->shape[0] == (uint64_t)s.N);
-      if (!up_ok) return fail(c, 4609, "adapter %d: '%s/lora_up' has shape [%llu,%llu,...] (ndim %u), expected [%d, r%s]", a, path.c_str(),
-                              (unsigned long long)up->shape[0], (unsigned long long)up->shape[1], up->ndim, s.N, s.conv ? ", 1, 1" : "");
-      if (up->shape[1] != rank)
-        return fail(c, 4610, "adapter %d: '%s': lora_down has rank %llu but lora_up has rank %llu", a, path.c_str(),
-                    (unsigned long long)rank, (unsigned long long)up->shape[1]);
-      double alpha = (double)rank;
+      const int taps = s.ks * s.ks;
+      auto get = [&](const char* leaf) -> const PackEntry* { auto f = L.second.find(leaf); return f == L.second.end() ? nullptr : f->second; };
+      const char* fams[4][6] = {{"lora_down", "lora_up"}, {"hada_w1_a", "hada_w1_b", "hada_w2_a", "hada_w2_b"},
+                                {"lokr_w1", "lokr_w1_a", "lokr_w1_b", "lokr_w2", "lokr_w2_a", "lokr_w2_b"}, {"diff"}};
+      int fam = -1;
+      const char* first = nullptr;
+      for (int f = 0; f < 4; ++f)
+        for (int i = 0; i < 6 && fams[f][i]; ++i)
+          if (get(fams[f][i])) {
+            if (fam >= 0 && fam != f)
+              return fail(c, 4615, "adapter %d: '%s' holds two delta families ('%s' and '%s')", a, path.c_str(), first, fams[f][i]);
+            fam = f; first = fams[f][i];
+          }
+      const PackEntry* al = get("alpha");
+      const PackEntry* ds = get("dora_scale");
+      if (fam < 0 && ds) return fail(c, 4621, "adapter %d: '%s/dora_scale' is on a layer without a delta", a, path.c_str());
+      if (fam < 0) fam = 0;   // alpha alone: reported as a LoRA without factors
+      for (int f = 0; f < 4; ++f)
+        for (int i = 0; i < 6 && fams[f][i]; ++i) {
+          const PackEntry* e = get(fams[f][i]);
+          if (e && e->dtype != 0) return fail(c, 4607, "adapter %d: '%s/%s' must be f16", a, path.c_str(), fams[f][i]);
+        }
+      double alpha = 0.0;    // read when have_alpha; a finite negative alpha is used as given
+      const bool have_alpha = al != nullptr;
       if (al) {
         const uint64_t esz = al->dtype ? 4 : 2;
         if (al->nbytes != esz) return fail(c, 4611, "adapter %d: '%s/alpha' must have one element", a, path.c_str());
@@ -919,13 +944,164 @@ static int adapters_apply(sdxl_ctx* c, AdapterState& S, int n, const sdxl_adapte
         else { __half_raw hr; memcpy(&hr.x, raw, 2); alpha = (double)__half2float(__half(hr)); }
         if (!isfinite(alpha)) return fail(c, 4612, "adapter %d: '%s/alpha' is not finite", a, path.c_str());
       }
-      LoraTerm t;
-      t.up = (const __half*)(pv.dev + up->offset);
-      t.down = (const __half*)(pv.dev + dn->offset);
-      t.r = (int)rank;
-      t.coef = (float)((double)ad[a].scale * alpha / (double)rank);
-      terms[path].push_back(t);
+      auto dev16 = [&](const PackEntry* e) { return (const __half*)(pv.dev + e->offset); };
+      // columns of a [rows, I(, ks, ks)] factor as input channels: 2-D [rows, I * taps] or (convs) 4-D [rows, I, ks, ks]; -1 otherwise
+      auto in_ch = [&](const PackEntry* e) -> long long {
+        if (e->ndim == 2) return e->shape[1] % taps ? -1 : (long long)(e->shape[1] / taps);
+        if (e->ndim == 4 && s.conv && e->shape[2] == (uint64_t)s.ks && e->shape[3] == (uint64_t)s.ks) return (long long)e->shape[1];
+        return -1;
+      };
+      auto need = [&](const char* leaf) -> const PackEntry* {
+        const PackEntry* e = get(leaf);
+        if (!e) fail(c, 4616, "adapter %d: '%s/%s' is missing (%s)", a, path.c_str(), leaf, first);
+        return e;
+      };
+      auto bad_shape = [&](const char* leaf, const char* want) {
+        return fail(c, 4617, "adapter %d: '%s/%s' has shape %s, expected %s (N = %d, I = %d%s)", a, path.c_str(), leaf,
+                    shape_str(get(leaf)).c_str(), want, s.N, s.I, s.conv ? (s.ks == 3 ? ", 3x3 conv" : ", 1x1 conv") : "");
+      };
+      AdapterTerm T;
+      double rank = 1.0;       // the r of alpha / r
+      bool use_alpha = true;
+      if (fam == 0) {   // LoRA: the original checks and codes
+        const PackEntry* dn = get("lora_down");
+        const PackEntry* up = get("lora_up");
+        if (!dn || !up) return fail(c, 4606, "adapter %d: '%s/%s' is missing", a, path.c_str(), dn ? "lora_up" : "lora_down");
+        const uint64_t rk = dn->ndim ? dn->shape[0] : 0;
+        const bool dn_ok = s.conv ? (dn->ndim == 4 && dn->shape[1] == (uint64_t)s.I && dn->shape[2] == (uint64_t)s.ks && dn->shape[3] == (uint64_t)s.ks)
+                                  : (dn->ndim == 2 && dn->shape[1] == (uint64_t)s.I);
+        if (!dn_ok || rk < 1 || rk > 4096)
+          return fail(c, 4608, "adapter %d: '%s/lora_down' has shape [%llu,%llu,%llu,%llu] (ndim %u), expected [r, %d%s]", a, path.c_str(),
+                      (unsigned long long)dn->shape[0], (unsigned long long)dn->shape[1], (unsigned long long)dn->shape[2],
+                      (unsigned long long)dn->shape[3], dn->ndim, s.I, s.conv ? (s.ks == 3 ? ", 3, 3" : ", 1, 1") : "");
+        const bool up_ok = s.conv ? (up->ndim == 4 && up->shape[0] == (uint64_t)s.N && up->shape[2] == 1 && up->shape[3] == 1)
+                                  : (up->ndim == 2 && up->shape[0] == (uint64_t)s.N);
+        if (!up_ok) return fail(c, 4609, "adapter %d: '%s/lora_up' has shape [%llu,%llu,...] (ndim %u), expected [%d, r%s]", a, path.c_str(),
+                                (unsigned long long)up->shape[0], (unsigned long long)up->shape[1], up->ndim, s.N, s.conv ? ", 1, 1" : "");
+        if (up->shape[1] != rk)
+          return fail(c, 4610, "adapter %d: '%s': lora_down has rank %llu but lora_up has rank %llu", a, path.c_str(),
+                      (unsigned long long)rk, (unsigned long long)up->shape[1]);
+        T.t.kind = LORA_LORA; T.t.up = dev16(up); T.t.down = dev16(dn); T.t.r = (int)rk;
+        rank = (double)rk;
+      } else if (fam == 1) {   // LoHa
+        const PackEntry* f[4];
+        const char* nm[4] = {"hada_w1_a", "hada_w1_b", "hada_w2_a", "hada_w2_b"};
+        for (int i = 0; i < 4; ++i) if (!(f[i] = need(nm[i]))) return 4616;
+        uint64_t rk[2];
+        for (int p = 0; p < 2; ++p) {
+          const PackEntry* A = f[2 * p];
+          const PackEntry* B = f[2 * p + 1];
+          if (A->ndim != 2 || A->shape[0] != (uint64_t)s.N || A->shape[1] < 1 || A->shape[1] > 4096) return bad_shape(nm[2 * p], "[N, r]");
+          if (in_ch(B) != s.I) return bad_shape(nm[2 * p + 1], s.conv ? "[r, I, kh, kw] or [r, I*kh*kw]" : "[r, I]");
+          if (B->shape[0] != A->shape[1])
+            return fail(c, 4618, "adapter %d: '%s': %s has rank %llu but %s has rank %llu", a, path.c_str(), nm[2 * p],
+                        (unsigned long long)A->shape[1], nm[2 * p + 1], (unsigned long long)B->shape[0]);
+          rk[p] = B->shape[0];
+        }
+        T.t.kind = LORA_LOHA;
+        T.t.up = dev16(f[0]); T.t.down = dev16(f[1]); T.t.r = (int)rk[0];
+        T.t.up2 = dev16(f[2]); T.t.down2 = dev16(f[3]); T.t.r2 = (int)rk[1];
+        rank = (double)rk[0];
+      } else if (fam == 2) {   // LoKr: each factor is staged as f32 (a product is expanded with coefficient 1)
+        uint64_t prod_rank[2] = {0, 0};
+        uint64_t rows[2], cols[2];       // w1 [a, b]; w2 [c, d * taps]
+        float* fx[2];
+        for (int w = 0; w < 2; ++w) {
+          const std::string base = w ? "lokr_w2" : "lokr_w1";
+          const PackEntry* full = get(base.c_str());
+          const PackEntry* A = get((base + "_a").c_str());
+          const PackEntry* B = get((base + "_b").c_str());
+          if (full && (A || B))
+            return fail(c, 4615, "adapter %d: '%s' holds both '%s' and '%s_%s'", a, path.c_str(), base.c_str(), base.c_str(), A ? "a" : "b");
+          if (!full && !(A && B)) return fail(c, 4616, "adapter %d: '%s/%s%s' is missing (%s)", a, path.c_str(), base.c_str(),
+                                              A ? "_b" : B ? "_a" : "", first);
+          LoraMergeParams q{};
+          q.nterm = 1; q.taps = 1; q.term[0].coef = 1.f;
+          long long ich;
+          if (full) {
+            ich = w ? in_ch(full) : (full->ndim == 2 ? (long long)full->shape[1] : -1);
+            if (ich < 1) return bad_shape(base.c_str(), w ? (s.conv ? "[c, d, kh, kw] or [c, d*kh*kw]" : "[c, d]") : "[a, b]");
+            rows[w] = full->shape[0];
+            q.term[0].kind = LORA_FULL; q.term[0].down = dev16(full);
+          } else {
+            const std::string an = base + "_a", bn = base + "_b";
+            if (A->ndim != 2 || A->shape[1] < 1 || A->shape[1] > 4096) return bad_shape(an.c_str(), "[rows, r]");
+            ich = w ? in_ch(B) : (B->ndim == 2 ? (long long)B->shape[1] : -1);
+            if (ich < 1) return bad_shape(bn.c_str(), w ? (s.conv ? "[r, d, kh, kw] or [r, d*kh*kw]" : "[r, d]") : "[r, b]");
+            if (B->shape[0] != A->shape[1])
+              return fail(c, 4618, "adapter %d: '%s': %s has rank %llu but %s has rank %llu", a, path.c_str(), an.c_str(),
+                          (unsigned long long)A->shape[1], bn.c_str(), (unsigned long long)B->shape[0]);
+            rows[w] = A->shape[0];
+            prod_rank[w] = A->shape[1];
+            q.term[0].kind = LORA_LORA; q.term[0].up = dev16(A); q.term[0].down = dev16(B); q.term[0].r = (int)A->shape[1];
+          }
+          cols[w] = (uint64_t)ich * (w ? (uint64_t)taps : 1);
+          if (rows[w] < 1 || rows[w] > (uint64_t)s.N || cols[w] < 1 || cols[w] > (uint64_t)s.I * taps)
+            return fail(c, 4619, "adapter %d: '%s': the LoKr factor %s is larger than the layer (N = %d, I = %d)", a, path.c_str(),
+                        base.c_str(), s.N, s.I);
+          fx[w] = tmp.get<float>((size_t)rows[w] * cols[w] * sizeof(float));
+          if (!fx[w]) return fail(c, 4624, "set_adapters: cannot allocate the LoKr factor %s of '%s'", base.c_str(), path.c_str());
+          q.N = (int)rows[w]; q.Kd = (int)cols[w]; q.delta_out = fx[w];
+          KL(c, lora_merge_launch(c->stream, q));
+        }
+        const uint64_t d = cols[1] / taps;
+        if (rows[0] * rows[1] != (uint64_t)s.N || cols[0] * d != (uint64_t)s.I)
+          return fail(c, 4619, "adapter %d: '%s': kron(lokr_w1 [%llu, %llu], lokr_w2 [%llu, %llu]) is not [N = %d, I = %d]", a, path.c_str(),
+                      (unsigned long long)rows[0], (unsigned long long)cols[0], (unsigned long long)rows[1], (unsigned long long)d, s.N, s.I);
+        if (prod_rank[0] && prod_rank[1] && prod_rank[0] != prod_rank[1])
+          return fail(c, 4618, "adapter %d: '%s': lokr_w1_a has rank %llu but lokr_w2_a has rank %llu (LoKr factors given as "
+                      "products must share the rank r of alpha / r)", a, path.c_str(),
+                      (unsigned long long)prod_rank[0], (unsigned long long)prod_rank[1]);
+        T.t.kind = LORA_LOKR; T.t.w1 = fx[0]; T.t.w2 = fx[1]; T.t.c = (int)rows[1]; T.t.d = (int)d;
+        use_alpha = prod_rank[0] || prod_rank[1];
+        rank = (double)(prod_rank[0] ? prod_rank[0] : prod_rank[1]);
+      } else {   // full delta
+        const PackEntry* e = get("diff");
+        if (e->shape[0] != (uint64_t)s.N || in_ch(e) != s.I) return bad_shape("diff", s.conv ? "[N, I, kh, kw] or [N, I*kh*kw]" : "[N, I]");
+        T.t.kind = LORA_FULL; T.t.down = dev16(e);
+        use_alpha = false;
+      }
+      // c = alpha / r; the LoRA term's coefficient s * alpha / r is evaluated in that order, as before this family table
+      const double num = use_alpha ? (have_alpha ? alpha : rank) : 1.0, den = use_alpha ? rank : 1.0;
+      T.t.coef = (float)((double)ad[a].scale * num / den);
+      if (ds) {
+        if (s.up) return fail(c, 4622, "adapter %d: '%s/dora_scale': DoRA on an upsample conv is not supported (its 3x3 weight is not "
+                              "retained, so the norm cannot be taken)", a, path.c_str());
+        if (ds->dtype != 1) return fail(c, 4623, "adapter %d: '%s/dora_scale' must be f32", a, path.c_str());
+        const uint64_t* sh = ds->shape;
+        const bool row = (ds->ndim == 1 && sh[0] == (uint64_t)s.N) || (ds->ndim == 2 && sh[0] == (uint64_t)s.N && sh[1] == 1) ||
+                         (ds->ndim == 4 && sh[0] == (uint64_t)s.N && sh[1] == 1 && sh[2] == 1 && sh[3] == 1);
+        const bool col = (ds->ndim == 2 && sh[0] == 1 && sh[1] == (uint64_t)s.I) ||
+                         (ds->ndim == 4 && sh[0] == 1 && sh[1] == (uint64_t)s.I && sh[2] == 1 && sh[3] == 1);
+        if (!row && !col)
+          return fail(c, 4620, "adapter %d: '%s/dora_scale' has shape %s, expected [%d], [%d,1], [%d,1,1,1] (rows) or [1,%d], [1,%d,1,1] "
+                      "(input channels)", a, path.c_str(), shape_str(ds).c_str(), s.N, s.N, s.N, s.I, s.I);
+        T.m = (const float*)(pv.dev + ds->offset);
+        T.axis = row ? 0 : 1;
+        T.s = ad[a].scale;
+        T.t.coef = (float)(num / den);
+      }
+      terms[path].push_back(T);
     }
+  }
+  // scratch of the layers merged through an f32 delta (upsample convs, DoRA), sized for the largest, reused layer by layer
+  float* delta = nullptr;   // the layer's summed delta
+  float* ddw = nullptr;     // one DoRA term's delta
+  double* dnorm = nullptr;
+  {
+    size_t nd = 0, nw = 0, nn = 0;
+    for (auto& kv : terms) {
+      const WSlot& s = S.slots[kv.first];
+      const size_t e = (size_t)s.N * s.I * s.ks * s.ks;
+      bool dora = false;
+      for (auto& T : kv.second) dora |= T.m != nullptr;
+      if (s.up || dora) nd = std::max(nd, e);
+      if (dora) { nw = std::max(nw, e); nn = std::max(nn, (size_t)std::max(s.N, s.I)); }
+    }
+    if (nd && !(delta = tmp.get<float>(nd * sizeof(float))))
+      return fail(c, 4614, "set_adapters: cannot allocate %zu bytes of merge scratch", nd * sizeof(float));
+    if (nw && (!(ddw = tmp.get<float>(nw * sizeof(float))) || !(dnorm = tmp.get<double>(nn * sizeof(double)))))
+      return fail(c, 4624, "set_adapters: cannot allocate %zu bytes of DoRA scratch", nw * sizeof(float) + nn * sizeof(double));
   }
   // backups of the buffers touched for the first time, one allocation (a failure leaves the model unchanged)
   {
@@ -958,19 +1134,35 @@ static int adapters_apply(sdxl_ctx* c, AdapterState& S, int n, const sdxl_adapte
     const void* src = S.bufs[s.base].backup;
     LoraMergeParams p{};
     p.N = s.N; p.taps = s.ks * s.ks; p.Kd = s.I * p.taps;
-    p.nterm = (int)kv.second.size();
-    for (int i = 0; i < p.nterm; ++i) p.term[i] = kv.second[i];
     p.src = src; p.dst = s.base; p.f32 = s.f32;
     p.ld = s.ld; p.row0 = s.row0; p.col0 = s.col0; p.Ipad = s.Ipad; p.geglu_bn = s.geglu_bn;
-    if (s.up) {
-      float* delta = tmp.get<float>((size_t)p.N * p.Kd * sizeof(float));
-      if (!delta) return fail(c, 4614, "set_adapters: cannot allocate the upsample delta of '%s'", kv.first.c_str());
-      p.delta_out = delta;
+    std::vector<const AdapterTerm*> plain, dora;   // non-DoRA terms, then DoRA terms, each in call order
+    for (auto& T : kv.second) (T.m ? dora : plain).push_back(&T);
+    p.nterm = (int)plain.size();
+    for (int i = 0; i < p.nterm; ++i) p.term[i] = plain[i]->t;
+    if (dora.empty() && !s.up) {
       KL(c, lora_merge_launch(c->stream, p));
-      KL(c, lora_upconv_merge_launch(c->stream, (const __half*)src, delta, s.N, s.I, (__half*)s.base, s.Ipad));
-    } else {
-      KL(c, lora_merge_launch(c->stream, p));
+      continue;
     }
+    LoraMergeParams q = p;
+    q.delta_out = delta;
+    if (p.nterm) KL(c, lora_merge_launch(c->stream, q));
+    else CU(c, cudaMemsetAsync(delta, 0, (size_t)p.N * p.Kd * sizeof(float), c->stream));
+    if (s.up) {
+      KL(c, lora_upconv_merge_launch(c->stream, (const __half*)src, delta, s.N, s.I, (__half*)s.base, s.Ipad));
+      continue;
+    }
+    for (const AdapterTerm* T : dora) {
+      LoraMergeParams w = p;
+      w.nterm = 1; w.term[0] = T->t; w.delta_out = ddw;
+      KL(c, lora_merge_launch(c->stream, w));
+      KL(c, dora_norm_launch(c->stream, p, ddw, T->axis, dnorm));
+      KL(c, dora_accum_launch(c->stream, p, ddw, T->m, dnorm, T->axis, T->s, delta));
+    }
+    p.nterm = 1;
+    p.term[0] = LoraTerm{};
+    p.term[0].kind = LORA_F32; p.term[0].w1 = delta; p.term[0].coef = 1.f;
+    KL(c, lora_merge_launch(c->stream, p));
   }
   if (n == 0) {   // everything is restored: the backups go
     CU(c, cudaStreamSynchronize(c->stream));

@@ -370,9 +370,22 @@ int bias_to_f32_launch(cudaStream_t st, const __half* src, int N, float* dst, in
 // Kd = I * taps: column k of the delta is input channel i = k / taps, tap = k % taps (down's natural [r, I, kh, kw] order).
 // Element (n, k) is stored at dst[(row0 + geglu_perm(n)) * ld + col0 + tap * Ipad + i] as f16(src + delta), with src the
 // backed-up weight at the same offset (f32 storage: float(f16(src + delta))). With `delta_out` set the kernel writes the f32
-// delta [N, Kd] there instead (upsample convs, see lora_upconv_merge_launch).
+// delta [N, Kd] there instead (upsample convs, DoRA layers and LoKr factors; see lora_upconv_merge_launch, dora_*_launch).
+// A term's product P (the `up @ down` above) depends on its kind (DESIGN.md §19):
+//   LORA_LORA   P = up [N, r] @ down [r, Kd]
+//   LORA_LOHA   P = (up @ down) * (up2 [N, r2] @ down2 [r2, Kd])            (both pairs staged like LORA, then multiplied)
+//   LORA_LOKR   P[i*c + j, (p*d + q)*taps + t] = w1[i, p] * w2[j, q*taps + t]  (w1 f32 [N/c, I/d], w2 f32 [c, d*taps])
+//   LORA_FULL   P = down as f16 [N, Kd]
+//   LORA_F32    P = w1 as f32 [N, Kd] (a delta staged by an earlier launch; with coef 1 the kernel just applies it)
+// A set of LORA_LORA terms only runs the kernel's original instantiation.
 #define LORA_MAX_TERMS 16
-struct LoraTerm { const __half* up; const __half* down; int r; float coef; };
+enum { LORA_LORA = 0, LORA_LOHA = 1, LORA_LOKR = 2, LORA_FULL = 3, LORA_F32 = 4 };
+struct LoraTerm {
+  const __half* up; const __half* down; int r; float coef;
+  int kind;
+  const __half* up2; const __half* down2; int r2;   // LORA_LOHA
+  const float* w1; const float* w2; int c, d;       // LORA_LOKR (w2 rows c, w2 input channels d); LORA_F32: w1
+};
 struct LoraMergeParams {
   int N, Kd, taps;
   int nterm;
@@ -385,5 +398,14 @@ int lora_merge_launch(cudaStream_t st, const LoraMergeParams& p);
 // Upsample conv: the 3x3 f32 delta [O, I*9] is summed into the four 2x2 phase kernels with the tap sets of
 // repack_upconv_kernel and added to the backed-up phase weights src (layout of repack_upconv_launch's dst).
 int lora_upconv_merge_launch(cudaStream_t st, const __half* src, const float* delta, int O, int I, __half* dst, int Ipad);
+// DoRA (DESIGN.md §19). `slot` gives the weight W through its slot map (src, f32, ld, row0, col0, Ipad, geglu_bn, N, Kd, taps;
+// its terms are not read); dw is the adapter's f32 delta [N, Kd] (coef included, scale not). axis 0: one norm per output row n
+// over all Kd; axis 1: one norm per input channel i over N and the taps.
+//   dora_norm:  norm[j] = sqrt(sum (W + dw)^2) in double, one CTA per row or input channel, fixed order and tree reduction.
+//               No atomics.
+//   dora_accum: acc[n, k] += f32(s * (m[j] * (W + dw) / norm[j] - W)) computed in double; 0 where norm[j] == 0.
+int dora_norm_launch(cudaStream_t st, const LoraMergeParams& slot, const float* dw, int axis, double* norm);
+int dora_accum_launch(cudaStream_t st, const LoraMergeParams& slot, const float* dw, const float* m, const double* norm, int axis,
+                      float s, float* acc);
 
 }  // namespace sdxl

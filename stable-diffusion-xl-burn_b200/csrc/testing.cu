@@ -173,6 +173,43 @@ SDXL_TEST_API int sdxl_test_lora_merge(void* stream, int N, int Kd, int taps, in
   p.delta_out = delta_out;
   return lora_merge_launch((cudaStream_t)stream, p);
 }
+// nterm terms of any kind (kernels.h: LORA_*): per term ints[5 t ..] = kind, r, r2, c, d and ptrs[6 t ..] = up, down, up2,
+// down2, w1, w2.
+SDXL_TEST_API int sdxl_test_lora_merge_kinds(void* stream, int N, int Kd, int taps, int nterm, const int* ints, const void* const* ptrs,
+                                             const float* coef, const void* src, void* dst, int f32, size_t ld, int row0, int col0,
+                                             int Ipad, int geglu_bn, float* delta_out) {
+  if (nterm < 1 || nterm > LORA_MAX_TERMS) return 1;
+  LoraMergeParams p{};
+  p.N = N; p.Kd = Kd; p.taps = taps; p.nterm = nterm;
+  for (int i = 0; i < nterm; ++i) {
+    LoraTerm& T = p.term[i];
+    const int* v = ints + 5 * i;
+    const void* const* q = ptrs + 6 * i;
+    T.kind = v[0]; T.r = v[1]; T.r2 = v[2]; T.c = v[3]; T.d = v[4]; T.coef = coef[i];
+    T.up = (const __half*)q[0]; T.down = (const __half*)q[1]; T.up2 = (const __half*)q[2]; T.down2 = (const __half*)q[3];
+    T.w1 = (const float*)q[4]; T.w2 = (const float*)q[5];
+  }
+  p.src = src; p.dst = dst; p.f32 = f32;
+  p.ld = ld; p.row0 = row0; p.col0 = col0; p.Ipad = Ipad; p.geglu_bn = geglu_bn;
+  p.delta_out = delta_out;
+  return lora_merge_launch((cudaStream_t)stream, p);
+}
+static LoraMergeParams dora_slot(int N, int Kd, int taps, const void* src, int f32, size_t ld, int row0, int col0, int Ipad, int geglu_bn) {
+  LoraMergeParams p{};
+  p.N = N; p.Kd = Kd; p.taps = taps; p.src = src; p.f32 = f32;
+  p.ld = ld; p.row0 = row0; p.col0 = col0; p.Ipad = Ipad; p.geglu_bn = geglu_bn;
+  return p;
+}
+SDXL_TEST_API int sdxl_test_dora_norm(void* stream, int N, int Kd, int taps, const void* src, int f32, size_t ld, int row0, int col0,
+                                      int Ipad, int geglu_bn, const float* dw, int axis, double* norm) {
+  return dora_norm_launch((cudaStream_t)stream, dora_slot(N, Kd, taps, src, f32, ld, row0, col0, Ipad, geglu_bn), dw, axis, norm);
+}
+SDXL_TEST_API int sdxl_test_dora_accum(void* stream, int N, int Kd, int taps, const void* src, int f32, size_t ld, int row0, int col0,
+                                       int Ipad, int geglu_bn, const float* dw, const float* m, const double* norm, int axis, float s,
+                                       float* acc) {
+  return dora_accum_launch((cudaStream_t)stream, dora_slot(N, Kd, taps, src, f32, ld, row0, col0, Ipad, geglu_bn), dw, m, norm, axis,
+                           s, acc);
+}
 SDXL_TEST_API int sdxl_test_lora_upconv_merge(void* stream, const void* src, const float* delta, int O, int I, void* dst, int Ipad) {
   return lora_upconv_merge_launch((cudaStream_t)stream, (const __half*)src, delta, O, I, (__half*)dst, Ipad);
 }

@@ -39,6 +39,9 @@ PROTOTYPES = {
     "sdxl_test_bias_to_f32": (I, [P, P, I, P, I, I]),
     "sdxl_test_lora_merge": (I, [P, I, I, I, I, P, P, P, P, P, P, I, C.c_size_t, I, I, I, I, P]),
     "sdxl_test_lora_upconv_merge": (I, [P, P, P, I, I, P, I]),
+    "sdxl_test_lora_merge_kinds": (I, [P, I, I, I, I, P, P, P, P, P, I, C.c_size_t, I, I, I, I, P]),
+    "sdxl_test_dora_norm": (I, [P, I, I, I, P, I, C.c_size_t, I, I, I, I, P, I, P]),
+    "sdxl_test_dora_accum": (I, [P, I, I, I, P, I, C.c_size_t, I, I, I, I, P, P, P, I, F, P]),
     "sdxl_test_softmax_rows": (I, [P, P, Z, I, I, F, P, Z]),
     "sdxl_test_transpose_f16": (I, [P, P, Z, I, I, P, Z]),
     "sdxl_test_post_quant": (I, [P, P, I, I, I, P, P, F, P]),
@@ -233,6 +236,49 @@ def lora_merge(N, Kd, taps, terms, src, dst, ld, row0=0, col0=0, Ipad=0, geglu_b
 
 def lora_upconv_merge(src, delta, O, I, dst, Ipad) -> None:
     _call("sdxl_test_lora_upconv_merge", _p(src), _p(delta), O, I, _p(dst), Ipad)
+
+
+LORA_KINDS = {"lora": 0, "loha": 1, "lokr": 2, "full": 3, "f32": 4}
+
+
+def lora_merge_kinds(N, Kd, taps, terms, src, dst, ld, row0=0, col0=0, Ipad=0, geglu_bn=0, delta_out=None) -> None:
+    """terms: [(kind, coef, tensors)] with kind a LORA_KINDS key and tensors by kind: lora (up [N, r], down [r, Kd]); loha (up, down,
+    up2, down2); lokr (w1 f32 [N / c, I / d], w2 f32 [c, d * taps]); full (diff f16 [N, Kd]); f32 (delta f32 [N, Kd])."""
+    n = len(terms)
+    ints, ptrs = [], []
+    for kind, _, ts in terms:
+        z = [None] * 6
+        r = r2 = c = d = 0
+        if kind in ("lora", "loha"):
+            z[0], z[1] = ts[0], ts[1]
+            r = ts[0].shape[1]
+            if kind == "loha":
+                z[2], z[3] = ts[2], ts[3]
+                r2 = ts[2].shape[1]
+        elif kind == "lokr":
+            z[4], z[5] = ts[0], ts[1]
+            c, d = ts[1].shape[0], ts[1].shape[1] // taps
+        elif kind == "full":
+            z[1] = ts[0]
+        else:
+            z[4] = ts[0]
+        ints += [LORA_KINDS[kind], r, r2, c, d]
+        ptrs += [_p(x) for x in z]
+    coefs = (C.c_float * n)(*[float(cf) for _, cf, _ in terms])
+    _call("sdxl_test_lora_merge_kinds", N, Kd, taps, n, (C.c_int * len(ints))(*ints), (C.c_void_p * len(ptrs))(*ptrs), coefs, _p(src),
+          _p(dst), int(dst.dtype == torch.float32), ld, row0, col0, Ipad, geglu_bn, _p(delta_out))
+
+
+def dora_norm(N, Kd, taps, src, ld, dw, axis, norm, row0=0, col0=0, Ipad=0, geglu_bn=0) -> None:
+    """norm f64 [N] (axis 0) or [Kd / taps] (axis 1) of W (src through the slot map) + dw f32 [N, Kd]."""
+    _call("sdxl_test_dora_norm", N, Kd, taps, _p(src), int(src.dtype == torch.float32), ld, row0, col0, Ipad, geglu_bn, _p(dw), axis,
+          _p(norm))
+
+
+def dora_accum(N, Kd, taps, src, ld, dw, m, norm, axis, s, acc, row0=0, col0=0, Ipad=0, geglu_bn=0) -> None:
+    """acc f32 [N, Kd] += s * (m * (W + dw) / norm - W), m f32 and norm f64 along `axis`."""
+    _call("sdxl_test_dora_accum", N, Kd, taps, _p(src), int(src.dtype == torch.float32), ld, row0, col0, Ipad, geglu_bn, _p(dw), _p(m),
+          _p(norm), axis, float(s), _p(acc))
 
 
 # latent decoder / encoder (vae_kernels.cu)

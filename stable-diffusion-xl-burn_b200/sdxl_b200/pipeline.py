@@ -60,7 +60,7 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
     bottom) in pixels. With an inpainting UNet (cfg.is_inpaint, DESIGN.md §12) reference_rgb is required: the crop window becomes the
     pixel mask (1 = repaint), prepare_inpaint_condition's condition is attached for the call and the latent is sampled from noise
-    without blending. loras: [(kohya .safetensors path / bytes / tensor dict, scale), ...] merged into the base UNet and both
+    without blending. loras: [(adapter .safetensors path / bytes / tensor dict, scale), ...] (any format lora.load_adapter reads) merged into the base UNet and both
     text encoders for this call (the refiner is left alone) and removed again afterwards, which also clears any adapter set
     those models had. controls: [(ControlNet, image u8 [1, H, W, 3] or f32 [1, 3, H, W], scale), ...] attached to the base UNet
     for this call and detached afterwards (the refiner is left alone). image_prompt: (IPAdapter, ClipVisionEncoder, images u8
@@ -154,8 +154,8 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     if not loras:
         return _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
                        seed, noise, **sch)
-    from .lora import load_kohya
-    parts = [load_kohya(src, diffuser.cfg, embedder.clip.cfg, embedder.open_clip.cfg) for src, _ in loras]
+    from .lora import load_adapter
+    parts = [load_adapter(src, diffuser.cfg, embedder.clip.cfg, embedder.open_clip.cfg) for src, _ in loras]
     active = []
     try:
         for model, key in ((diffuser, "unet"), (embedder.clip, "te1"), (embedder.open_clip, "te2")):
