@@ -26,29 +26,69 @@ int gn_scratch_init(cudaStream_t st, float* scratch, int B, int n_group) {
   return (int)cudaMemsetAsync(gn_counters(scratch), 0, gn_counter_floats(B) * sizeof(unsigned), st);
 }
 
-// Pivot of a (sample, group): the mean of four of its elements (first / middle channel at the first / middle pixel). Sums are
-// taken of (x - pivot), so that var = E[(x-K)^2] - E[x-K]^2 has no cancellation when |mean| >> sigma (the reference centres
-// first, groupnorm/mod.rs:75-82; real activations have groups with |mean| / sigma in the hundreds). Same value in every CTA.
-__device__ __forceinline__ float gn_pivot(const float* __restrict__ x1, int C1, const float* __restrict__ x2, int C2, int b, int HW,
-                                          int c0, int cpg) {
-  float k = 0.f;
-#pragma unroll
-  for (int i = 0; i < 2; ++i) {
-    const int c = c0 + i * (cpg >> 1);
-    const float* src = c < C1 ? x1 + (size_t)b * HW * C1 + c : x2 + (size_t)b * HW * C2 + (c - C1);
-    const int Cs = c < C1 ? C1 : C2;
-    k += __ldg(src) + __ldg(src + (size_t)(HW >> 1) * Cs);
+// Running statistics of one channel column of a thread: the count n (shared by the four channels of a float4), and per channel
+// a centre K, the offset r of the running mean from K, and m2, the sum of squared deviations from the running mean K + r.
+// merge() adds k <= N rows: it centres them on their own mean (two-pass, in registers), adds them by Chan's pairwise update and
+// then moves K to the new mean, keeping in r what the move rounded away (exactly, by Fast2Sum, when |r| <= |K|; otherwise, for a
+// mean near zero or a first row far from the rest, within one f32 rounding of the move). So the sums add deviations from the
+// running mean, never |mean| itself, and no statistic depends on which row a thread happens to read first.
+struct GnRun {
+  float n = 0.f;
+  float4 K, r = make_float4(0, 0, 0, 0), m2 = make_float4(0, 0, 0, 0);
+
+  // a[0 .. k-1] are the rows (1 <= k <= N); the rest are ignored
+  template <int N>
+  __device__ __forceinline__ void merge(float4 (&a)[N], int k) {
+    const float fk = (float)k, nn = n + fk, kinv = fk * __frcp_rn(nn), w = n * kinv, inv_k = k == N ? 1.f / (float)N : __frcp_rn(fk);
+    merge1(a, k, &float4::x, kinv, w, inv_k);
+    merge1(a, k, &float4::y, kinv, w, inv_k);
+    merge1(a, k, &float4::z, kinv, w, inv_k);
+    merge1(a, k, &float4::w, kinv, w, inv_k);
+    n = nn;
   }
-  return 0.25f * k;
-}
+  // kinv = k / (n + k), w = n k / (n + k): Chan's weights (both 0 / 1 on the first merge, where n = 0)
+  template <int N>
+  __device__ __forceinline__ void merge1(float4 (&a)[N], int k, float float4::*f, float kinv, float w, float inv_k) {
+    float& Kf = K.*f;
+    float& rf = r.*f;
+    float sb = 0.f;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      a[u].*f = u < k ? a[u].*f - Kf : 0.f;
+      sb += a[u].*f;
+    }
+    const float mb = sb * inv_k;
+    float m2b = 0.f;
+#pragma unroll
+    for (int u = 0; u < N; ++u) {
+      const float e = u < k ? a[u].*f - mb : 0.f;
+      m2b = fmaf(e, e, m2b);
+    }
+    const float delta = mb - rf;                     // block mean - running mean
+    m2.*f += fmaf(w * delta, delta, m2b);
+    rf = fmaf(kinv, delta, rf);                      // new mean - K
+    const float Kn = Kf + rf;                        // re-centre on the new mean
+    rf -= Kn - Kf;
+    Kf = Kn;
+  }
+  __device__ __forceinline__ float mean(float float4::*f) const { return K.*f + r.*f; }
+};
 
 // ---- stats: grid (nchunk, B); block = V*R threads, V = C/4 float4 columns, R pixel rows in flight.
-// The last CTA of a sample to finish (arrival counter; control only, the arithmetic order is fixed) turns the chunk partials
-// into the sample's (mean, rstd) per group, so the apply kernel does not repeat that in every CTA.
-__global__ void gn_stats_kernel(const float* __restrict__ x1, int C1, const float* __restrict__ x2, int C2, int HW,
-                                int n_group, int R, float eps, float* __restrict__ partial, float* __restrict__ final_stats,
-                                unsigned* __restrict__ counters) {
-  extern __shared__ float sm[];  // [R][C][2]
+// Each thread keeps a GnRun of its column over the rows p0 + rr, p0 + rr + R, ... of its chunk; the CTA folds its R * cpg
+// (count, mean, m2) partials per group in double (sum of count * mean, then the centred second moment around that mean), and the
+// last CTA of a sample to finish (arrival counter; control only, the arithmetic order is fixed) merges the chunks' (mean, m2)
+// the same way in double and writes the sample's (mean, rstd) per group, so the apply kernel does not repeat that in every CTA.
+// No statistic depends on which element a thread happens to read first (the reference centres first, groupnorm/mod.rs:75-82;
+// real activations have groups with |mean| / sigma in the hundreds, and outliers anywhere).
+// kMaxThreads / kMinBlocks / kRows: the UNet's GroupNorms (blocks of <= 512 threads, HW < 64k) are compiled for two CTAs per SM,
+// so a B = 2 grid of 2 x 132 CTAs runs in one wave; at the 64 registers that allows, a thread keeps 6 rows in flight (8 spill).
+// The rest run one CTA per SM with 8 rows in flight (gn_launch).
+template <int kMaxThreads, int kMinBlocks, int kRows>
+__global__ void __launch_bounds__(kMaxThreads, kMinBlocks)
+gn_stats_kernel(const float* __restrict__ x1, int C1, const float* __restrict__ x2, int C2, int HW, int n_group, int R, float eps,
+                float* __restrict__ partial, float* __restrict__ final_stats, unsigned* __restrict__ counters) {
+  extern __shared__ float sm[];  // [R][C][2]: (mean, m2) of each thread's column
   __shared__ unsigned s_ticket;
   griddep_wait();
   griddep_launch_dependents();
@@ -58,96 +98,97 @@ __global__ void gn_stats_kernel(const float* __restrict__ x1, int C1, const floa
   const int b = blockIdx.y, chunk = blockIdx.x, nchunk = gridDim.x;
   const int per = (HW + nchunk - 1) / nchunk;
   const int p0 = chunk * per;
-  const int p1 = min(HW, p0 + per);
+  const int p1 = min(HW, p0 + per);   // p1 <= p0: an empty chunk (nchunk * per may exceed HW by up to per - 1)
   const int c = v * 4;
   const float* src;
   int cc, Cs;
   if (c < C1) { src = x1; cc = c; Cs = C1; } else { src = x2; cc = c - C1; Cs = C2; }
   src += (size_t)b * HW * Cs + cc;
   const int cpg = C / n_group;
-  // per-channel pivot = pivot of the channel's group (a float4 may straddle two groups)
-  float4 K;
-  {
-    const int g0 = c / cpg, g3 = (c + 3) / cpg;
-    const float k0 = gn_pivot(x1, C1, x2, C2, b, HW, g0 * cpg, cpg);
-    const float k3 = g3 == g0 ? k0 : gn_pivot(x1, C1, x2, C2, b, HW, g3 * cpg, cpg);
-    K.x = k0;
-    K.y = (c + 1) / cpg == g0 ? k0 : k3;
-    K.z = (c + 2) / cpg == g0 ? k0 : k3;
-    K.w = k3;
-  }
-  float4 s = make_float4(0, 0, 0, 0), q = make_float4(0, 0, 0, 0);
+  GnRun run;
   int p = p0 + rr;
-  for (; p + 7 * R < p1; p += 8 * R) {  // eight independent 128-bit loads in flight per thread
-    float4 a[8];
+  run.K = p < p1 ? *reinterpret_cast<const float4*>(src + (size_t)p * Cs) : make_float4(0, 0, 0, 0);   // any start will do
+  for (; p < p1; p += kRows * R) {  // kRows independent 128-bit loads in flight per thread; the last block may be partial
+    const int k = min(kRows, (p1 - p + R - 1) / R);
+    float4 a[kRows];
 #pragma unroll
-    for (int u = 0; u < 8; ++u) a[u] = *reinterpret_cast<const float4*>(src + (size_t)(p + u * R) * Cs);
-#pragma unroll
-    for (int u = 0; u < 8; ++u) {
-      const float dx = a[u].x - K.x, dy = a[u].y - K.y, dz = a[u].z - K.z, dw = a[u].w - K.w;
-      s.x += dx; s.y += dy; s.z += dz; s.w += dw;
-      q.x = fmaf(dx, dx, q.x); q.y = fmaf(dy, dy, q.y);
-      q.z = fmaf(dz, dz, q.z); q.w = fmaf(dw, dw, q.w);
-    }
-  }
-  for (; p < p1; p += R) {
-    const float4 a = *reinterpret_cast<const float4*>(src + (size_t)p * Cs);
-    const float dx = a.x - K.x, dy = a.y - K.y, dz = a.z - K.z, dw = a.w - K.w;
-    s.x += dx; s.y += dy; s.z += dz; s.w += dw;
-    q.x = fmaf(dx, dx, q.x); q.y = fmaf(dy, dy, q.y); q.z = fmaf(dz, dz, q.z); q.w = fmaf(dw, dw, q.w);
+    for (int u = 0; u < kRows; ++u) a[u] = u < k ? *reinterpret_cast<const float4*>(src + (size_t)(p + u * R) * Cs) : make_float4(0, 0, 0, 0);
+    run.merge(a, k);
   }
   float* row = sm + ((size_t)rr * C + c) * 2;
-  row[0] = s.x; row[1] = q.x; row[2] = s.y; row[3] = q.y; row[4] = s.z; row[5] = q.z; row[6] = s.w; row[7] = q.w;
+  row[0] = run.mean(&float4::x); row[1] = run.m2.x; row[2] = run.mean(&float4::y); row[3] = run.m2.y;
+  row[4] = run.mean(&float4::z); row[5] = run.m2.z; row[6] = run.mean(&float4::w); row[7] = run.m2.w;
   __syncthreads();
   if (threadIdx.x < n_group) {
     const int g = threadIdx.x;
-    float S = 0.f, Q = 0.f;
-    for (int r = 0; r < R; ++r)
+    const int np = p1 - p0;   // rows of this chunk; thread row r holds ceil((np - r) / R) of them
+    double S = 0.0;
+    for (int r = 0; r < R && r < np; ++r) {
+      double Sr = 0.0;
+      for (int j = 0; j < cpg; ++j) Sr += (double)sm[((size_t)r * C + g * cpg + j) * 2];
+      S += (double)((np - r + R - 1) / R) * Sr;
+    }
+    const double n = (double)cpg * (double)max(np, 0);
+    const double m = n > 0.0 ? S / n : 0.0;
+    double M2 = 0.0;
+    for (int r = 0; r < R && r < np; ++r) {
+      const double cnt = (double)((np - r + R - 1) / R);
       for (int j = 0; j < cpg; ++j) {
         const float* e = sm + ((size_t)r * C + g * cpg + j) * 2;
-        S += e[0];
-        Q += e[1];
+        const double d = (double)e[0] - m;
+        M2 += fma(cnt * d, d, (double)e[1]);
       }
+    }
     float* o = partial + (((size_t)b * nchunk + chunk) * n_group + g) * 2;
-    o[0] = S;
-    o[1] = Q;
+    o[0] = (float)m;
+    o[1] = (float)M2;
     __threadfence();  // this CTA's partials are visible device-wide before it takes its ticket
   }
   __syncthreads();
   if (threadIdx.x == 0) s_ticket = atomicAdd(&counters[b], 1u);
   __syncthreads();
   if (s_ticket != (unsigned)(nchunk - 1)) return;
-  // last CTA of sample b: 8 lanes per group walk the chunk partials in chunk order (deterministic), in double precision.
+  // last CTA of sample b: 8 lanes per group walk the chunk partials in chunk order (deterministic), in double precision: the
+  // count-weighted sum of the chunk means, then the chunks' m2 plus count * (chunk mean - mean)^2.
   // Only whole warps take part (blockDim.x >= 32 but not always a multiple of it) and n_group % 4 == 0 (gn_launch), so every
   // warp either reduces four complete groups or skips the loop: the full-mask shuffles below always see all 32 lanes.
   __threadfence();
   const int nred = blockDim.x & ~31;
   for (int g = threadIdx.x >> 3; threadIdx.x < nred && g < n_group; g += nred >> 3) {
     const int sub = threadIdx.x & 7;
-    double S = 0.0, Q = 0.0;
+    auto load = [&](int k) {   // chunk k's (mean, m2); (0, 0) past the last chunk
+      return k < nchunk ? __ldcg(reinterpret_cast<const float2*>(partial + (((size_t)b * nchunk + k) * n_group + g) * 2))
+                        : make_float2(0.f, 0.f);
+    };
+    auto count = [&](int k) { return (double)cpg * (double)max(min(HW - k * per, per), 0); };   // 0 for an empty chunk
+    double S = 0.0;
     for (int k0 = sub; k0 < nchunk; k0 += 64) {   // eight independent loads in flight, summed in chunk order
       float2 e[8];
 #pragma unroll
+      for (int j = 0; j < 8; ++j) e[j] = load(k0 + 8 * j);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) S = fma(count(k0 + 8 * j), (double)e[j].x, S);
+    }
+#pragma unroll
+    for (int o = 4; o > 0; o >>= 1) S += __shfl_xor_sync(0xffffffffu, S, o);
+    const double n = (double)cpg * HW;
+    const double m = S / n;
+    double M2 = 0.0;
+    for (int k0 = sub; k0 < nchunk; k0 += 64) {
+      float2 e[8];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) e[j] = load(k0 + 8 * j);
+#pragma unroll
       for (int j = 0; j < 8; ++j) {
-        const int k = k0 + 8 * j;
-        e[j] = k < nchunk ? __ldcg(reinterpret_cast<const float2*>(partial + (((size_t)b * nchunk + k) * n_group + g) * 2))
-                          : make_float2(0.f, 0.f);
+        const double d = (double)e[j].x - m;
+        M2 += fma(count(k0 + 8 * j) * d, d, (double)e[j].y);
       }
-#pragma unroll
-      for (int j = 0; j < 8; ++j) { S += (double)e[j].x; Q += (double)e[j].y; }
     }
 #pragma unroll
-    for (int o = 4; o > 0; o >>= 1) {
-      S += __shfl_xor_sync(0xffffffffu, S, o);
-      Q += __shfl_xor_sync(0xffffffffu, Q, o);
-    }
+    for (int o = 4; o > 0; o >>= 1) M2 += __shfl_xor_sync(0xffffffffu, M2, o);
     if (sub == 0) {
-      const double n = (double)cpg * HW;
-      const double m = S / n;               // mean of (x - pivot): O(sigma), so the subtraction below does not cancel
-      double var = Q / n - m * m;
-      if (var < 0.0) var = 0.0;
-      final_stats[((size_t)b * n_group + g) * 2] = (float)((double)gn_pivot(x1, C1, x2, C2, b, HW, g * cpg, cpg) + m);
-      final_stats[((size_t)b * n_group + g) * 2 + 1] = (float)(1.0 / sqrt(var + (double)eps));
+      final_stats[((size_t)b * n_group + g) * 2] = (float)m;
+      final_stats[((size_t)b * n_group + g) * 2 + 1] = (float)(1.0 / sqrt(M2 / n + (double)eps));
     }
   }
   if (threadIdx.x == 0) counters[b] = 0u;  // ready for the next GroupNorm that uses this scratch
@@ -244,7 +285,7 @@ int gn_launch(cudaStream_t st, GnParams& p) {
   // n_group % 4 == 0: the stats kernel's final reduction gives each group 8 lanes of a full-mask warp shuffle
   if ((p.C1 & 7) || (p.C2 & 7) || p.n_group < 4 || (p.n_group & 3) || p.n_group > 64 || C % p.n_group) return 3001;
   const int V = C / 4;
-  if (V > 1024) return 3002;
+  if (V > 768) return 3002;   // gn_stats_kernel's launch bound (C <= 3072: the refiner's widest concatenation)
   int R = 512 / V;
   if (R < 1) R = 1;
   if (R > 16) R = 16;
@@ -255,11 +296,16 @@ int gn_launch(cudaStream_t st, GnParams& p) {
   if (nchunk > max_chunks) nchunk = max_chunks;
   p.nchunk = nchunk;
   const size_t smem1 = (size_t)R * C * 2 * sizeof(float);
-  static bool optin[64];
-  if (int r = smem_optin(gn_stats_kernel, 160 * 1024, optin)) return r;
+  static bool optin_narrow[64], optin_wide[64];
+  // two CTAs per SM (6 rows in flight) where the grid is short, one with 8 rows in flight where each CTA streams many rows
+  // (HW >= 64k: the VAE's larger GroupNorms, HBM-bound) or the block is wider than 512 threads. Chosen by shape only, never by
+  // B, so the summation order stays batch-invariant.
+  const bool narrow = V * R <= 512 && p.HW < 65536;
+  auto kernel = narrow ? gn_stats_kernel<512, 2, 6> : gn_stats_kernel<768, 1, 8>;
+  if (int r = smem_optin(kernel, 160 * 1024, narrow ? optin_narrow : optin_wide)) return r;
   float* fin = gn_final(p.partial, p.B, p.n_group);
   unsigned* cnt = gn_counters(p.partial);
-  int e = launch_kernel(gn_stats_kernel, dim3(nchunk, p.B), dim3(V * R), smem1, st, true, p.x1, p.C1, p.x2, p.C2, p.HW,
+  int e = launch_kernel(kernel, dim3(nchunk, p.B), dim3(V * R), smem1, st, true, p.x1, p.C1, p.x2, p.C2, p.HW,
                         p.n_group, R, p.eps, gn_partials(p.partial, p.B), fin, cnt);
   if (e) return e;
   const int V8 = C / 8;
