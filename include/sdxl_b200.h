@@ -151,12 +151,27 @@ SDXL_API int sdxl_sample_latent(sdxl_unet* unet, const sdxl_conditioning* cond, 
  *   EULER_ANCESTRAL  k-diffusion sample_euler_ancestral (eta, s_noise)
  *   DPMPP_2M         k-diffusion sample_dpmpp_2m; first order on the first step of a call and on the step to sigma = 0
  *   LCM              diffusers' LCMScheduler.step (timestep scaling 10, sigma_data 0.5)
+ * and (DESIGN.md §20; lambda = -log sigma, h = lambda' - lambda, D_j the denoised latent of step j; each step to sigma' = 0 returns
+ * D exactly, with one evaluation):
+ *   DPMPP_2M_SDE     k-diffusion sample_dpmpp_2m_sde, midpoint: with eta_h = eta h and phi = -expm1(-h - eta_h),
+ *                    xh' = (sigma' / sigma) e^(-eta_h) xh + phi D [+ 0.5 phi (D - D_{k-1}) h / h_{k-1}] + s_noise sigma'
+ *                    sqrt(-expm1(-2 eta_h)) z; the bracket once D_{k-1} exists in the call
+ *   DPMPP_3M_SDE     k-diffusion sample_dpmpp_3m_sde: order 1, 2, 3 as D_{k-1}, D_{k-2} exist in the call; the same noise term
+ *   UNIPC            diffusers' UniPCMultistepScheduler (solver_order 2, x0 prediction, bh2, corrector on, lower_order_final): UniC
+ *                    corrects the current state from x_{k-1}, D_{k-1}, D_{k-2} and D_k (no extra evaluation, none on the first
+ *                    step of a call), then UniP of order min(2, steps done in the call + 1, steps left) runs from it
+ *   HEUN             k-diffusion sample_heun (s_churn 0): an Euler step to sigma', a second evaluation there, the trapezoid
+ *   DPM_2            k-diffusion sample_dpm_2: an Euler step to sigma_mid = sqrt(sigma sigma'), a second evaluation there at the
+ *                    fractional t of sigma_mid, then xh' = xh + (sigma' - sigma) d_mid
+ * HEUN and DPM_2 evaluate the UNet twice per step (once on the step to sigma = 0); every attachment applies per evaluation, at its t.
  * Spacings over N training timesteps: REFERENCE t_k = N - 1 - k (N / n) (sdxl_sample_latent's, which runs the same n steps when n
  * divides N); LEADING (n - 1 - k)(N / n) + 1 (diffusers, steps_offset 1); TRAILING round(N - k N / n) - 1; LINSPACE
  * (N - 1)(1 - k / (n - 1)), fractional; KARRAS sigma_k = (smax^(1/rho) + k / (n - 1) (smin^(1/rho) - smax^(1/rho)))^rho with t_k from
  * the interpolation; LCM diffusers' LCMScheduler.set_timesteps with original_inference_steps = 50 (n <= 50). Any sampler goes with
  * any spacing. */
-enum { SDXL_SAMPLER_EULER = 0, SDXL_SAMPLER_EULER_ANCESTRAL = 1, SDXL_SAMPLER_DPMPP_2M = 2, SDXL_SAMPLER_LCM = 3 };
+/* 4 is not assigned: sdxl_schedule_build refuses it, as it always has. */
+enum { SDXL_SAMPLER_EULER = 0, SDXL_SAMPLER_EULER_ANCESTRAL = 1, SDXL_SAMPLER_DPMPP_2M = 2, SDXL_SAMPLER_LCM = 3,
+       SDXL_SAMPLER_DPMPP_2M_SDE = 5, SDXL_SAMPLER_DPMPP_3M_SDE = 6, SDXL_SAMPLER_UNIPC = 7, SDXL_SAMPLER_HEUN = 8, SDXL_SAMPLER_DPM_2 = 9 };
 enum { SDXL_SPACING_REFERENCE = 0, SDXL_SPACING_LEADING = 1, SDXL_SPACING_TRAILING = 2, SDXL_SPACING_LINSPACE = 3,
        SDXL_SPACING_KARRAS = 4, SDXL_SPACING_LCM = 5 };
 typedef struct sdxl_schedule {
@@ -168,7 +183,7 @@ typedef struct sdxl_schedule {
   int32_t renoise;      /* first_step > 0: 1 adds sigma_k0 * z to init_latent (img2img), 0 takes it as it is (ensemble hand-off) */
   int32_t no_cfg;       /* 1: one conditional forward per step, guidance ignored, the unconditional tensors may be NULL */
   float   karras_rho;   /* 0 = 7 */
-  float   eta, s_noise; /* Euler-ancestral; 0 = 1 */
+  float   eta, s_noise; /* Euler-ancestral, DPM++ 2M SDE and 3M SDE; 0 = 1 */
 } sdxl_schedule;
 /* Pure host, needs no GPU: fills timesteps[0 .. n_steps) and sigmas[0 .. n_steps] (sigmas[n_steps] = 0) from an alphas_cumprod
  * table of n_train entries. Non-zero on an invalid schedule; sdxl_schedule_last_error() (per thread) names the field. */
@@ -182,13 +197,13 @@ SDXL_API const char* sdxl_schedule_last_error(void);
  *               input is z; first_step > 0: required, the latent to start from (xh at sigma_k0 when renoise == 0).
  *  noise / n_noise / seed: injected tensors are taken by index and the seeded Philox stream by subsequence, in this order
  *               and only those that exist: the initial noise when init_latent is NULL; the renoise tensor; then per step, in loop
- *               order, the inpainting blend's noise and then the sampler's (Euler-ancestral and LCM, except on their last
- *               step). As in sdxl_sample_latent, the first tensor past the n_noise injected ones takes subsequence 0 of the seeded
+ *               order, the inpainting blend's noise of each of the step's evaluations and then the sampler's (Euler-ancestral, LCM,
+ *               DPM++ 2M SDE and 3M SDE, except on the step to sigma = 0). As in sdxl_sample_latent, the first tensor past the n_noise injected ones takes subsequence 0 of the seeded
  *               stream, not its index in the order: index and subsequence coincide only for a call with no injected tensor.
  *               Seeded noise is generated inside the step kernel and equals sdxl_randn(seed, subsequence).
- *  inpaint_ref / inpaint_mask: as in sdxl_sample_latent: before the forward of step k, xh = mask ? xh : ref + sigma_k z.
+ *  inpaint_ref / inpaint_mask: as in sdxl_sample_latent: before each forward, xh = mask ? xh : ref + sigma z at that forward's sigma.
  * With guidance the rows are [cond | uncond]; schedule->no_cfg runs [cond] alone (few-step distilled models), half the work.
- * The schedule is validated before any state changes; the error names the field. DPM++ 2M's history does not cross calls. */
+ * The schedule is validated before any state changes; the error names the field. Multistep history does not cross calls. */
 SDXL_API int sdxl_sample_latent_scheduled(sdxl_unet* unet, const sdxl_conditioning* cond, double guidance_scale,
                                           const sdxl_schedule* schedule, const float* init_latent, const float* noise, int n_noise,
                                           uint64_t seed, const float* inpaint_ref, const uint8_t* inpaint_mask, float* latent_out);
@@ -701,7 +716,8 @@ SDXL_API int sdxl_unet_set_freeu(sdxl_unet* unet, const sdxl_freeu* freeu);
  *                   wherever their layers fall in the blocks that run.
  * Sampling (sdxl_sample_latent, sdxl_sample_latent_scheduled, sdxl_sampler_step and sdxl_sampler_step_host): UNet evaluation j since
  * the last sdxl_sampler_begin (j = 0, 1, ...) is full when j % interval == 0 and cached otherwise, for every row of the batch. Every
- * sampling entry point calls sdxl_sampler_begin, so each call's first step is full.
+ * sampling entry point calls sdxl_sampler_begin, so each call's first step is full. Evaluations, not steps, are counted: with a
+ * two-evaluation sampler (SDXL_SAMPLER_HEUN, SDXL_SAMPLER_DPM_2) at interval 2, each step runs one full and one cached evaluation.
  * The feature is what the last full forward computed from its inputs: a full forward after a change of the conditioning or of an
  * attachment's values is what refreshes it. */
 typedef struct sdxl_deepcache {

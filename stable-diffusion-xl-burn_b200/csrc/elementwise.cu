@@ -712,9 +712,10 @@ __device__ __forceinline__ void store4(float* __restrict__ p, size_t blk, size_t
       if (blk * 4 + j < n) p[blk * 4 + j] = v[j];
   }
 }
-// kV, kRescale: kernels.h Prediction; <false, false> is the epsilon step and never reads `pr`.
-template <bool kV, bool kRescale>
-__global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams p, int aligned, const Prediction pr) {
+// kV, kRescale: kernels.h Prediction; <false, false> is the epsilon step and never reads `pr`. kRows: kernels.h StepRows, the
+// two-row form; without it `r` is never read.
+template <bool kV, bool kRescale, bool kRows>
+__global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams p, int aligned, const Prediction pr, const StepRows r) {
   const size_t n = (size_t)p.Bimg * p.C * p.HW, nblk = (n + 3) / 4;
   const size_t blk = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (blk >= nblk) return;
@@ -750,13 +751,29 @@ __global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams
     for (int j = 0; j < 4; ++j) D[j] = xh[j];
   }
   float nx[4];
+  if constexpr (kRows) {   // every operand is read before anything is written: both rows see the values before the launch
+    float xs[4] = {0.f, 0.f, 0.f, 0.f}, h1[4] = {0.f, 0.f, 0.f, 0.f}, h2[4] = {0.f, 0.f, 0.f, 0.f};
+    if (r.cs != 0.f || r.ss != 0.f) load4(r.xs, blk, n, vec, xs);
+    if (p.ch != 0.f || r.sh != 0.f || r.shift) load4(p.hist, blk, n, vec, h1);
+    if (r.ch2 != 0.f || r.sh2 != 0.f) load4(r.h2, blk, n, vec, h2);
 #pragma unroll
-  for (int j = 0; j < 4; ++j) nx[j] = p.cx * xh[j] + p.cd * D[j];
-  if (p.ch != 0.f) {
-    float h[4];
-    load4(p.hist, blk, n, vec, h);
+    for (int j = 0; j < 4; ++j) nx[j] = p.cx * xh[j] + r.cs * xs[j] + p.cd * D[j] + p.ch * h1[j] + r.ch2 * h2[j];
+    if (r.write_xs) {
+      float s[4];
 #pragma unroll
-    for (int j = 0; j < 4; ++j) nx[j] += p.ch * h[j];
+      for (int j = 0; j < 4; ++j) s[j] = r.sx * xh[j] + r.ss * xs[j] + r.sd * D[j] + r.sh * h1[j] + r.sh2 * h2[j];
+      store4(r.xs, blk, n, vec, s);
+    }
+    if (r.shift) store4(r.h2, blk, n, vec, h1);
+  } else {
+#pragma unroll
+    for (int j = 0; j < 4; ++j) nx[j] = p.cx * xh[j] + p.cd * D[j];
+    if (p.ch != 0.f) {
+      float h[4];
+      load4(p.hist, blk, n, vec, h);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) nx[j] += p.ch * h[j];
+    }
   }
   if (p.write_hist) store4(p.hist, blk, n, vec, D);
   if (p.cn != 0.f) {
@@ -778,14 +795,26 @@ __global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams
   for (int j = 0; j < 4; ++j) nx[j] *= p.c_in;
   store4(p.x_in, blk, n, vec, nx);
 }
-int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr) {
+int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr, const StepRows* rows) {
   const size_t n = (size_t)p.Bimg * p.C * p.HW;
   if (!n) return 0;
   if (!p.xh || !p.x_in || ((p.ch != 0.f || p.write_hist) && !p.hist) || (p.mask && !p.ref)) return (int)cudaErrorInvalidValue;
-  const uintptr_t a = (uintptr_t)p.xh | (uintptr_t)p.x_in | (uintptr_t)p.hist | (uintptr_t)p.z | (uintptr_t)p.zb | (uintptr_t)p.ref;
-  auto kernel = pr.v ? (pr.factor ? guided_step_kernel<true, true> : guided_step_kernel<true, false>)
-                     : (pr.factor ? guided_step_kernel<false, true> : guided_step_kernel<false, false>);
-  kernel<<<cdiv((long)((n + 3) / 4), 256), 256, 0, st>>>(p, a % 16 == 0, pr);
+  uintptr_t a = (uintptr_t)p.xh | (uintptr_t)p.x_in | (uintptr_t)p.hist | (uintptr_t)p.z | (uintptr_t)p.zb | (uintptr_t)p.ref;
+  const unsigned grid = cdiv((long)((n + 3) / 4), 256);
+  if (rows) {
+    const StepRows& r = *rows;
+    if (((r.cs != 0.f || r.ss != 0.f || r.write_xs) && !r.xs) || ((r.sh != 0.f || r.shift) && !p.hist) ||
+        ((r.ch2 != 0.f || r.sh2 != 0.f || r.shift) && !r.h2))
+      return (int)cudaErrorInvalidValue;
+    a |= (uintptr_t)r.xs | (uintptr_t)r.h2;
+    auto kernel = pr.v ? (pr.factor ? guided_step_kernel<true, true, true> : guided_step_kernel<true, false, true>)
+                       : (pr.factor ? guided_step_kernel<false, true, true> : guided_step_kernel<false, false, true>);
+    kernel<<<grid, 256, 0, st>>>(p, a % 16 == 0, pr, r);
+    return (int)cudaGetLastError();
+  }
+  auto kernel = pr.v ? (pr.factor ? guided_step_kernel<true, true, false> : guided_step_kernel<true, false, false>)
+                     : (pr.factor ? guided_step_kernel<false, true, false> : guided_step_kernel<false, false, false>);
+  kernel<<<grid, 256, 0, st>>>(p, a % 16 == 0, pr, StepRows{});
   return (int)cudaGetLastError();
 }
 

@@ -2505,8 +2505,10 @@ struct Sampler {
   int evals = 0;           // UNet evaluations since sampler_begin (DeepCache: evaluation j is full when j % interval == 0)
   float guidance = 1.f;
   float* noise = nullptr;  // scratch [Bimg,4,h,w]
-  float* xh = nullptr;     // scheduled samplers: the state x / sqrt(alpha) and the previous step's denoised latent (DPM++ 2M)
-  float* hist = nullptr;
+  float* xh = nullptr;     // scheduled samplers: the state x / sqrt(alpha), the denoised-latent history slots H1 and H2 and the
+  float* hist = nullptr;   // saved state xs (DESIGN.md §16, §20)
+  float* h2 = nullptr;
+  float* xs = nullptr;
   float* ref = nullptr;
   uint8_t* mask = nullptr;
   float* rescale = nullptr;    // guidance rescale: the per-image factors [Bimg] and the statistics kernel's scratch
@@ -2557,6 +2559,8 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
           S->noise = A.get<float>(lat);
           S->xh = A.get<float>(lat);
           S->hist = A.get<float>(lat);
+          S->h2 = A.get<float>(lat);
+          S->xs = A.get<float>(lat);
           S->ref = A.get<float>(lat);
           S->mask = A.get<uint8_t>(lat);
           S->rescale = A.get<float>(Bimg);
@@ -2843,7 +2847,8 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
   if (n_noise < 0 || (n_noise > 0 && !noise)) return fail(c, 5233, "n_noise = %d with %s noise", n_noise, noise ? "a" : "null");
   const int n = sch->n_steps, k0 = sch->first_step, k1 = sch->last_step ? sch->last_step : n;
   std::vector<double> ts(n), sig(n + 1);
-  schedule_fill(SigmaTable(u->alphas.data(), N), *sch, ts.data(), sig.data());
+  const SigmaTable table(u->alphas.data(), N);
+  schedule_fill(table, *sch, ts.data(), sig.data());
   for (int k = 0; k < n; ++k)
     if (!(sig[k + 1] < sig[k])) return fail(c, 5234, "schedule: n_steps = %d gives sigmas that do not decrease at step %d", n, k);
 
@@ -2888,27 +2893,35 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
     feed.next(p.zb, p.zb_subseq);
   }
   KL(c, guided_step_launch(c->stream, p));
-  // the steps: write t, replay the plan, one launch
+  // the steps: per evaluation, write t, replay the plan, one launch
   p.eps = P->eps; p.ld = P->eps_ld; p.use_cfg = S->cfg; p.use_pag = S->pag; p.guidance = S->guidance;
+  StepRows rows;
+  rows.xs = S->xs; rows.h2 = S->h2;
   for (int k = k0; k < k1; ++k) {
-    if ((r = set_t(u, ts[k]))) return r;
-    if ((r = run_sampler_plan(u))) return r;
-    const StepCoef q = step_coef(*sch, k, ts.data(), sig.data(), k > k0);
-    p.sigma = (float)sig[k];
-    p.cx = q.cx; p.cd = q.cd; p.ch = q.ch; p.cn = q.cn; p.c_in = q.c_in;
-    p.write_hist = sampler_keeps_history(sch->sampler);
-    if (S->pag) p.p_t = pag_scale(u, ts[k]);
-    p.z = p.zb = nullptr;
-    p.mask = nullptr;
-    if (q.cn != 0.f) feed.next(p.z, p.z_subseq);
-    if (inpaint_ref && k + 1 < k1) {   // the blend before the next forward: its noise follows this step's in the call's order
-      p.mask = S->mask;
-      p.sigma_blend = (float)sig[k + 1];
-      feed.next(p.zb, p.zb_subseq);
+    const StepStages ss = step_stages(&table, *sch, k, ts.data(), sig.data(), std::min(k - k0, 2));
+    for (int i = 0; i < ss.n; ++i) {
+      const Stage& q = ss.st[i];
+      if ((r = set_t(u, q.t))) return r;
+      if ((r = run_sampler_plan(u))) return r;
+      p.sigma = (float)q.sigma;
+      p.cx = q.cx; p.cd = q.cd; p.ch = q.ch; p.cn = q.cn; p.c_in = q.c_in;
+      p.write_hist = q.write_hist;
+      rows.cs = q.cs; rows.ch2 = q.ch2;
+      rows.sx = q.sx; rows.ss = q.ss; rows.sd = q.sd; rows.sh = q.sh; rows.sh2 = q.sh2;
+      rows.write_xs = q.write_xs; rows.shift = q.shift;
+      if (S->pag) p.p_t = pag_scale(u, q.t);
+      p.z = p.zb = nullptr;
+      p.mask = nullptr;
+      if (q.cn != 0.f) feed.next(p.z, p.z_subseq);
+      if (inpaint_ref && (i + 1 < ss.n || k + 1 < k1)) {   // the blend before the next forward: its noise follows this launch's
+        p.mask = S->mask;
+        p.sigma_blend = (float)q.sigma_next;
+        feed.next(p.zb, p.zb_subseq);
+      }
+      Prediction pr;
+      if ((r = step_prediction(u, p.p_t, q.sigma, pr))) return r;
+      KL(c, guided_step_launch(c->stream, p, pr, q.rows() ? &rows : nullptr));
     }
-    Prediction pr;
-    if ((r = step_prediction(u, p.p_t, sig[k], pr))) return r;
-    KL(c, guided_step_launch(c->stream, p, pr));
   }
   return sample_end(u, cond, S->xh, latent_out);
 }

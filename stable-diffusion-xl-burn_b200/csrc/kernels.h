@@ -287,7 +287,21 @@ struct GuidedStepParams {
   const float* ref;
   float sigma_blend;
 };
-int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr = {});
+// The two-row form of the step (DESIGN.md §20), for samplers that keep a saved state xs and a second history slot h2 (each f32 NCHW
+// like xh). With it, from the values before the launch:
+//   xh' = cx xh + cs xs + cd D + ch hist + ch2 h2 + cn z                    (then the blend and x_in as above)
+//   xs' = sx xh + ss xs + sd D + sh hist + sh2 h2                           (write_xs)
+//   h2' = hist (shift), hist' = D (write_hist)
+// xs is read when cs or ss is non-zero, hist when ch or sh is or shift is asked, h2 when ch2 or sh2 is.
+struct StepRows {
+  float* xs = nullptr;
+  float* h2 = nullptr;
+  float cs = 0.f, ch2 = 0.f;
+  float sx = 0.f, ss = 0.f, sd = 0.f, sh = 0.f, sh2 = 0.f;
+  int write_xs = 0, shift = 0;
+};
+// rows == nullptr: the one-row form above.
+int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr = {}, const StepRows* rows = nullptr);
 
 // Latent-decoder kernels (vae_kernels.cu)
 // P[r,:] = softmax(scale * S[r,:]); S f32 [rows, lds] -> P f16 [rows, ldp]; cols % 4 == 0.

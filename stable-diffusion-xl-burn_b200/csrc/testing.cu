@@ -337,16 +337,31 @@ SDXL_TEST_API int sdxl_test_vec_add_f32(void* stream, float* dst, const float* s
 // with GuidedStepParams filled as sdxl_sample_latent_scheduled fills it, and the float timestep embedding of the UNet plan.
 SDXL_TEST_API void sdxl_test_step_coef(const sdxl_schedule* s, int k, const double* timesteps, const double* sigmas, int has_prev,
                                        float* out) {
-  const StepCoef q = step_coef(*s, k, timesteps, sigmas, has_prev != 0);
+  const Stage q = step_stages(nullptr, *s, k, timesteps, sigmas, has_prev ? 1 : 0).st[0];
   out[0] = q.cx; out[1] = q.cd; out[2] = q.ch; out[3] = q.cn; out[4] = q.c_in;
 }
+// Every stage of step k with n_hist history slots filled (schedule.h: step_stages) over an alphas_cumprod table of n_train
+// entries; returns the number of stages. out[2][17] per stage: t, sigma, sigma_next, cx, cs, cd, ch, ch2, cn, sx, ss, sd, sh, sh2,
+// c_in, write_xs, write_hist + 2 * shift.
+SDXL_TEST_API int sdxl_test_step_stages(const double* alphas, int n_train, const sdxl_schedule* s, int k, const double* timesteps,
+                                        const double* sigmas, int n_hist, double* out) {
+  const SigmaTable T(alphas, n_train);
+  const StepStages ss = step_stages(&T, *s, k, timesteps, sigmas, n_hist);
+  for (int i = 0; i < ss.n; ++i) {
+    const Stage& q = ss.st[i];
+    const double v[17] = {q.t, q.sigma, q.sigma_next, q.cx, q.cs, q.cd, q.ch, q.ch2, q.cn, q.sx, q.ss, q.sd, q.sh, q.sh2, q.c_in,
+                          (double)q.write_xs, (double)q.write_hist + 2.0 * q.shift};
+    for (int j = 0; j < 17; ++j) out[17 * i + j] = v[j];
+  }
+  return ss.n;
+}
 // The same with the prediction type (SDXL_PREDICTION_*: v takes schedule.h's d_scale at sigma, as the engine does) and the per-image
-// guidance-rescale factors (factor nullable).
-SDXL_TEST_API int sdxl_test_guided_step_pred(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
-                                             float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,
-                                             float* xh, float* x_in, float* hist, int write_hist, const float* z, const float* zb,
-                                             uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq, const uint8_t* mask, const float* ref,
-                                             float sigma_blend, int prediction, const float* factor) {
+// guidance-rescale factors (factor nullable); with rows, the two-row form (kernels.h: StepRows).
+static int guided_step_test(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag, float guidance,
+                            float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in, float* xh, float* x_in, float* hist,
+                            int write_hist, const float* z, const float* zb, uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq,
+                            const uint8_t* mask, const float* ref, float sigma_blend, int prediction, const float* factor,
+                            const StepRows* rows) {
   GuidedStepParams p{};
   p.eps = eps; p.ld = ld; p.Bimg = Bimg; p.C = C; p.HW = HW; p.use_cfg = use_cfg; p.use_pag = use_pag;
   p.guidance = guidance; p.p_t = p_t; p.sigma = sigma;
@@ -360,7 +375,31 @@ SDXL_TEST_API int sdxl_test_guided_step_pred(void* stream, const float* eps, int
     const DScale q = d_scale(prediction, sigma);
     pr.v = 1; pr.dx = q.dx; pr.de = q.de;
   }
-  return guided_step_launch((cudaStream_t)stream, p, pr);
+  return guided_step_launch((cudaStream_t)stream, p, pr, rows);
+}
+SDXL_TEST_API int sdxl_test_guided_step_pred(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
+                                             float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,
+                                             float* xh, float* x_in, float* hist, int write_hist, const float* z, const float* zb,
+                                             uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq, const uint8_t* mask, const float* ref,
+                                             float sigma_blend, int prediction, const float* factor) {
+  return guided_step_test(stream, eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sigma, cx, cd, ch, cn, c_in, xh, x_in, hist,
+                          write_hist, z, zb, seed, z_subseq, zb_subseq, mask, ref, sigma_blend, prediction, factor, nullptr);
+}
+// sdxl_test_guided_step_pred's arguments, then the saved state xs, the second history slot h2, rc = (cs, ch2),
+// sr = (sx, ss, sd, sh, sh2) and the write_xs and shift flags.
+SDXL_TEST_API int sdxl_test_guided_step_rows(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
+                                             float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,
+                                             float* xh, float* x_in, float* hist, int write_hist, const float* z, const float* zb,
+                                             uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq, const uint8_t* mask, const float* ref,
+                                             float sigma_blend, int prediction, const float* factor, float* xs, float* h2,
+                                             const float* rc, const float* sr, int write_xs, int shift) {
+  StepRows r;
+  r.xs = xs; r.h2 = h2;
+  r.cs = rc[0]; r.ch2 = rc[1];
+  r.sx = sr[0]; r.ss = sr[1]; r.sd = sr[2]; r.sh = sr[3]; r.sh2 = sr[4];
+  r.write_xs = write_xs; r.shift = shift;
+  return guided_step_test(stream, eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sigma, cx, cd, ch, cn, c_in, xh, x_in, hist,
+                          write_hist, z, zb, seed, z_subseq, zb_subseq, mask, ref, sigma_blend, prediction, factor, &r);
 }
 SDXL_TEST_API int sdxl_test_guided_step(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
                                         float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,

@@ -78,6 +78,9 @@ PROTOTYPES = {
     "sdxl_test_guidance_stats": (I, [P, P, I, I, I, I, I, F, F, F, P, P]),
     "sdxl_test_guided_step_pred": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, F, F, P, P, P, I, P, P, C.c_uint64, C.c_uint64, C.c_uint64, P,
                                        P, F, I, P]),
+    "sdxl_test_guided_step_rows": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, F, F, P, P, P, I, P, P, C.c_uint64, C.c_uint64, C.c_uint64, P,
+                                       P, F, I, P, P, P, P, P, I, I]),
+    "sdxl_test_step_stages": (I, [P, I, P, I, P, P, I, P]),
 }
 _lib = None
 
@@ -438,3 +441,28 @@ def timestep_embedding_f32(t: torch.Tensor, dim: int, max_period: float = 10000.
     out = torch.empty(t.numel(), dim, device=t.device, dtype=torch.float32)
     _call("sdxl_test_timestep_embedding_f32", _p(t), t.numel(), dim, max_period, _p(out))
     return out
+
+
+def guided_step_rows(eps, ld, Bimg, Cc, HW, use_cfg, use_pag, guidance, p_t, sigma, coef, rows, xh, x_in, hist=None, h2=None, xs=None,
+                     write_hist=False, write_xs=False, shift=False, z=None, zb=None, seed=0, z_subseq=0, zb_subseq=0, mask=None, ref=None,
+                     sigma_blend=0.0, v=False, factor=None) -> None:
+    """The step kernel's two-row form (kernels.h: StepRows): coef = (cx, cs, cd, ch, ch2, cn, c_in), rows = (sx, ss, sd, sh, sh2);
+    xh, x_in, xs, hist and h2 are updated in place."""
+    cx, cs, cd, ch, ch2, cn, c_in = [float(c) for c in coef]
+    rc, sr = (C.c_float * 2)(cs, ch2), (C.c_float * 5)(*[float(c) for c in rows])
+    _call("sdxl_test_guided_step_rows", _p(eps), ld, Bimg, Cc, HW, int(use_cfg), int(use_pag), guidance, p_t, sigma, cx, cd, ch, cn, c_in,
+          _p(xh), _p(x_in), _p(hist), int(write_hist), _p(z), _p(zb), seed, z_subseq, zb_subseq, _p(mask), _p(ref), sigma_blend, int(v),
+          _p(factor), _p(xs), _p(h2), rc, sr, int(write_xs), int(shift))
+
+
+STAGE_FIELDS = ("t", "sigma", "sigma_next", "cx", "cs", "cd", "ch", "ch2", "cn", "sx", "ss", "sd", "sh", "sh2", "c_in", "write_xs", "hist")
+
+
+def step_stages(alphas, schedule_struct, k: int, t, sig, n_hist: int) -> list:
+    """schedule.h's step_stages on the host: one dict of STAGE_FIELDS per stage; "hist" is write_hist + 2 * shift. Needs no GPU."""
+    import numpy as np
+    a = np.ascontiguousarray(alphas, dtype=np.float64)
+    t, sig = np.ascontiguousarray(t, dtype=np.float64), np.ascontiguousarray(sig, dtype=np.float64)
+    out = (C.c_double * 34)()
+    n = load().sdxl_test_step_stages(a.ctypes.data, a.size, C.byref(schedule_struct), k, t.ctypes.data, sig.ctypes.data, n_hist, out)
+    return [dict(zip(STAGE_FIELDS, out[17 * i:17 * (i + 1)])) for i in range(n)]

@@ -416,7 +416,8 @@ class Diffuser:
         """Attaches DeepCache (sdxl_unet_set_deepcache, DESIGN.md §17; Ma et al. 2024, uniform schedule): every sampling call runs the
         whole UNet on its first step and every interval-th one after it, and on the steps between only the shallow branch (the first
         conv and input blocks 1..branch, then the last branch + 1 output blocks and the head) on the deep feature the last full step
-        kept. interval None detaches. Direct unet_forward calls run the full forward unless unet_forward(cached=True)."""
+        kept. The count is of UNet evaluations: a Heun or DPM2 step at interval 2 runs one full and one cached evaluation (DESIGN.md
+        §20). interval None detaches. Direct unet_forward calls run the full forward unless unet_forward(cached=True)."""
         if interval is None:
             self._deepcache = None
             self._set_deepcache(None)

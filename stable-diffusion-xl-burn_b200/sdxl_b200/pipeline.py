@@ -73,7 +73,7 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     adapter_conditioning_factor). pag: (scale, layers[, adaptive_scale]) perturbed-attention guidance (Diffuser.set_pag, diffusers'
     pag_scale, pag_applied_layers, pag_adaptive_scale) attached to the base UNet for this call and detached afterwards (the refiner is
     left alone). freeu: (s1, s2, b1, b2) FreeU (Diffuser.set_freeu, diffusers' enable_freeu) attached to the base UNet for this call
-    and detached afterwards (the refiner is left alone). sampler / spacing (schedulers.SAMPLERS / SPACINGS; one given, the other
+    and detached afterwards (the refiner is left alone). sampler / spacing (schedulers.ALL_SAMPLERS / SPACINGS; one given, the other
     defaults to "euler" / "leading") and no_cfg (one conditional forward per step, for few-step distilled models) build one
     schedulers.Schedule of n_steps for the base model; a refiner then runs the same schedule from the first step whose timestep is
     below 1000 - REFINER_STEP_START, re-noising the base latent to that step's sigma. All three None / False: the reference's DDIM

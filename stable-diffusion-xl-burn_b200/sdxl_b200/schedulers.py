@@ -1,4 +1,4 @@
-"""Samplers and noise schedules (include/sdxl_b200.h: sdxl_schedule; DESIGN.md §16): the ctypes mirror with string names and
+"""Samplers and noise schedules (include/sdxl_b200.h: sdxl_schedule; DESIGN.md §16, §20): the ctypes mirror with string names and
 `build`, the host-only timestep / sigma table of a schedule. Needs no GPU."""
 from __future__ import annotations
 
@@ -10,13 +10,18 @@ import numpy as np
 
 from . import _lib
 
-SAMPLERS = {"euler": 0, "euler_ancestral": 1, "dpmpp_2m": 2, "lcm": 3}
+SAMPLERS = {"euler": 0, "euler_ancestral": 1, "dpmpp_2m": 2, "lcm": 3}   # one evaluation and at most one history slot (§16)
+# DESIGN.md §20: the SDE multistep samplers, UniPC, and the two-evaluation Heun (diffusers' HeunDiscreteScheduler, k-diffusion's
+# sample_heun) and DPM2
+MORE_SAMPLERS = {"dpmpp_2m_sde": 5, "dpmpp_3m_sde": 6, "unipc": 7, "heun_discrete": 8, "dpm_2": 9}
+ALL_SAMPLERS = {**SAMPLERS, **MORE_SAMPLERS}
+TWO_EVALUATIONS = ("heun_discrete", "dpm_2")   # UNet evaluations per step: two, except on the step to sigma = 0
 SPACINGS = {"reference": 0, "leading": 1, "trailing": 2, "linspace": 3, "karras": 4, "lcm": 5}
 
 
 @dataclass
 class Schedule:
-    """sampler: one of SAMPLERS; spacing: one of SPACINGS; the other fields as sdxl_schedule documents them."""
+    """sampler: one of ALL_SAMPLERS; spacing: one of SPACINGS; the other fields as sdxl_schedule documents them."""
     sampler: str = "euler"
     spacing: str = "leading"
     n_steps: int = 30
@@ -39,10 +44,10 @@ class Schedule:
         return cls(n_steps=n_steps, first_step=first, renoise=first > 0, **kw)
 
     def to_struct(self) -> "_lib.Schedule":
-        for what, table, v in (("sampler", SAMPLERS, self.sampler), ("spacing", SPACINGS, self.spacing)):
+        for what, table, v in (("sampler", ALL_SAMPLERS, self.sampler), ("spacing", SPACINGS, self.spacing)):
             if v not in table:
                 raise _lib.SdxlError(f"Schedule: {what} = {v!r} is not one of {sorted(table)}")
-        return _lib.Schedule(SAMPLERS[self.sampler], SPACINGS[self.spacing], int(self.n_steps), int(self.first_step), int(self.last_step),
+        return _lib.Schedule(ALL_SAMPLERS[self.sampler], SPACINGS[self.spacing], int(self.n_steps), int(self.first_step), int(self.last_step),
                              int(self.renoise), int(self.no_cfg), float(self.karras_rho), float(self.eta), float(self.s_noise))
 
     def n_noise(self, initial: bool, inpainting: bool = False) -> int:
@@ -50,10 +55,17 @@ class Schedule:
         call draws its initial noise, i.e. first_step == 0 and no init tensor is passed)."""
         last = self.last_step or self.n_steps
         steps = last - self.first_step
-        n = int(initial) + int(self.renoise) + (steps if inpainting else 0)
-        if self.sampler in ("euler_ancestral", "lcm"):   # none on the step to sigma = 0
-            n += steps - (1 if last == self.n_steps else 0)
+        to_zero = 1 if last == self.n_steps else 0   # the call runs the step to sigma = 0
+        n = int(initial) + int(self.renoise) + (self.n_evaluations() if inpainting else 0)   # a blend before every evaluation
+        if self.sampler in ("euler_ancestral", "lcm", "dpmpp_2m_sde", "dpmpp_3m_sde"):   # none on the step to sigma = 0
+            n += steps - to_zero
         return n
+
+    def n_evaluations(self) -> int:
+        """UNet evaluations of a call with this schedule (DeepCache counts these)."""
+        last = self.last_step or self.n_steps
+        steps = last - self.first_step
+        return steps + (steps - (1 if last == self.n_steps else 0) if self.sampler in TWO_EVALUATIONS else 0)
 
 
 def alphas_cumprod(n: int = 1000, beta_start: float = 0.00085, beta_end: float = 0.012, zero_terminal_snr: bool = False) -> np.ndarray:
