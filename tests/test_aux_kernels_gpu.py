@@ -122,7 +122,7 @@ def softmax_logits(g, rows: int, cols: int) -> torch.Tensor:
     return S
 
 
-@pytest.mark.parametrize("cols", [4, 12280, 12284, 12288, 12292, 40960, 40964])
+@pytest.mark.parametrize("cols", [4, 12280, 12284, 12288, 12292, 40960, 40964, 15360, 15808, 16128, 16384])
 def test_softmax_rows(cols):
     """softmax_rows at the columns on both sides of its two branches: the row is cached in shared memory when cols * 4 <= 160 KB
     (40960 cached, 40964 not), with the opt-in when the cached row and the kernel's 32-byte reduction buffer exceed the 48 KB

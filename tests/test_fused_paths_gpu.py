@@ -542,30 +542,32 @@ def test_gemv(ctx, Bv, K):
 
 
 @pytest.mark.parametrize("x_f32", [0, 1])
-@pytest.mark.parametrize("Cin", [4, 8])
+@pytest.mark.parametrize("Cin", [4, 8, 3])
 @pytest.mark.parametrize("W", [8, 13])
 def test_conv_in(ctx, x_f32, Cin, W):
     """The first conv (CUDA cores, f32): one latent broadcast to B = 4 output images (Bx = 1), plus a ControlNet hint
-    embedding added per batch b % n_add (n_add = 2); W = 13 leaves a partial 8-pixel segment."""
-    g = torch.Generator().manual_seed(x_f32 + Cin + W)
-    Bx, B, H, Cout, n_add = 1, 4, 6, 320, 2
-    x = randn(g, Bx, Cin, H, W)
-    x = x.to(DEV) if x_f32 else f16(x)
-    w = randn(g, Cout, Cin, 3, 3, scale=1 / math.sqrt(9 * Cin)).to(DEV)
-    wk = w.permute(0, 2, 3, 1).contiguous()                             # [Cout][kh][kw][Cin]
-    bias = randn(g, Cout, scale=0.1).to(DEV)
-    add = randn(g, n_add, H, W, Cout).to(DEV)
-    for use_add in (False, True):
-        y = torch.full((B, H, W, Cout), float("nan"), device=DEV)
-        T.conv_in(x, Bx, B, Cin, H, W, wk, bias, Cout, y, add if use_add else None, n_add)
-        xb = x.double()[[b % Bx for b in range(B)]]
-        ref = F.conv2d(xb, w.double(), bias.double(), padding=1).permute(0, 2, 3, 1)
-        mag = F.conv2d(xb.abs(), w.double().abs(), bias.double().abs(), padding=1).permute(0, 2, 3, 1)
-        if use_add:
-            a = add.double()[[b % n_add for b in range(B)]]
-            ref, mag = ref + a, mag + a.abs()
-        # fmaf chain of 9 Cin products onto the bias, then the add: one f32 rounding each
-        check(y, ref, (9 * Cin + 2) * U24 * mag, f"conv_in x_f32={x_f32} Cin={Cin} W={W} add={use_add}")
+    embedding added per batch b % n_add (n_add = 2); W = 13 leaves a partial 8-pixel segment. Cin = 3 is the RGB stem of the VAE
+    encoder (Cout = 128) and of the ControlNet hint encoder (Cout = 16), and Cout = 512 the decoder's width."""
+    for Cout in (16, 128, 512) if Cin == 3 else (320,):
+        g = torch.Generator().manual_seed(x_f32 + Cin + W + (Cout if Cin == 3 else 0))
+        Bx, B, H, n_add = 1, 4, 6, 2
+        x = randn(g, Bx, Cin, H, W)
+        x = x.to(DEV) if x_f32 else f16(x)
+        w = randn(g, Cout, Cin, 3, 3, scale=1 / math.sqrt(9 * Cin)).to(DEV)
+        wk = w.permute(0, 2, 3, 1).contiguous()                             # [Cout][kh][kw][Cin]
+        bias = randn(g, Cout, scale=0.1).to(DEV)
+        add = randn(g, n_add, H, W, Cout).to(DEV)
+        for use_add in (False, True):
+            y = torch.full((B, H, W, Cout), float("nan"), device=DEV)
+            T.conv_in(x, Bx, B, Cin, H, W, wk, bias, Cout, y, add if use_add else None, n_add)
+            xb = x.double()[[b % Bx for b in range(B)]]
+            ref = F.conv2d(xb, w.double(), bias.double(), padding=1).permute(0, 2, 3, 1)
+            mag = F.conv2d(xb.abs(), w.double().abs(), bias.double().abs(), padding=1).permute(0, 2, 3, 1)
+            if use_add:
+                a = add.double()[[b % n_add for b in range(B)]]
+                ref, mag = ref + a, mag + a.abs()
+            # fmaf chain of 9 Cin products onto the bias, then the add: one f32 rounding each
+            check(y, ref, (9 * Cin + 2) * U24 * mag, f"conv_in x_f32={x_f32} Cin={Cin} Cout={Cout} W={W} add={use_add}")
 
 
 # ------------------------------------------------------------------------------------------------------------------------------

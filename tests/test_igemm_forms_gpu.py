@@ -24,118 +24,19 @@ import math
 
 import pytest
 import torch
-import torch.nn.functional as F
 
 from sdxl_b200 import _testing as T
-from harness import DEV, H11, H_SUB, check, conv_taps, gn_ref, pad64, plan_upconv, repack3
+from harness import (DEV, GEGLU, GRID_B, H11, H_SUB, assert_exact, assert_exact_range, bias_f32, check, conv_bound, conv_ref,
+                     conv_taps, gen, gn_ref, grid, grid_f32, grid_w, grid_x, guarded, in_place_residual, lin_weights, linear, pad64,
+                     plan_upconv, repack3, stride2_taps)
 
 pytestmark = pytest.mark.gpu
 
 U23 = 2.0 ** -23
-GRID_X, GRID_W, GRID_B = 2.0 ** -3, 2.0 ** -6, 2.0 ** -9
-EXACT_SUM = 2.0 ** 22 * GRID_B    # below this, every sum of multiples of 2^-9 is exact in f32
-GUARD = 4096                      # elements after each output that must stay NaN
-LINEAR, GEGLU = 0, 1              # kernels.h: IgemmMode
 GEGLU_BN = 256                    # engine.cu geglu_bn_for(4C): 4C is a multiple of 128 at every UNet width
 # erf_as (common.cuh): Abramowitz-Stegun 7.1.26 (1.5e-7 absolute) evaluated in f32 with rcp.approx / ex2.approx
 E_GELU = 5e-7
 HEAD_LO_TOL = 5.5e-5              # normwise error of the hi / lo head conv (test_head_conv_hi_lo)
-
-
-def gen(*key) -> torch.Generator:
-    return torch.Generator(device=DEV).manual_seed(sum((i + 1) * 7919 * int(k) for i, k in enumerate(key)) % (2 ** 31))
-
-
-def grid(g, shape, step, lim, dtype=torch.float16) -> torch.Tensor:
-    """Random integers in [-lim, lim] times step, exact in dtype."""
-    return (torch.randint(-lim, lim + 1, tuple(shape), generator=g, device=DEV).double() * step).to(dtype)
-
-
-def grid_x(g, *shape):
-    return grid(g, shape, GRID_X, 8)
-
-
-def grid_w(g, *shape):
-    return grid(g, shape, GRID_W, 8)
-
-
-def grid_f32(g, *shape):
-    """Bias / residual values: f32 multiples of 2^-9 with magnitude <= 2^11."""
-    return grid(g, shape, GRID_B, 2 ** 20, torch.float32)
-
-
-def bias_f32(g, N, geglu_bn=0):
-    """A grid f16 bias (magnitude <= 2047 * 2^-9, exact in f16) and its plan copy: bias_to_f32 (Loader::vec_f32)."""
-    b16 = grid(g, (N,), GRID_B, 2047)
-    b32 = torch.empty(N, dtype=torch.float32, device=DEV)
-    T.bias_to_f32(b16, N, b32, geglu_bn=geglu_bn)
-    return b16, b32
-
-
-def guarded(shape, dtype=torch.float32, fill=None):
-    """An output of `shape`, NaN-filled (or holding `fill`), followed by GUARD NaN elements: (output view, guard view)."""
-    n = math.prod(shape)
-    buf = torch.full((n + GUARD,), float("nan"), dtype=dtype, device=DEV)
-    if fill is not None:
-        buf[:n] = fill.reshape(-1)
-    return buf[:n].view(shape), buf[n:]
-
-
-def assert_exact_range(what, *bounds) -> None:
-    """bounds: upper bounds of sum |x w| per output and of every added |bias| / |res|, taken from the operands."""
-    tot = sum(float(b) for b in bounds)
-    assert tot < EXACT_SUM, f"{what}: operands reach {tot} >= 2^22 * 2^-9, partial sums would not be exact in f32"
-
-
-def conv_bound(x, w) -> float:
-    """max |x| * max_o sum |w[o]|: bounds sum |x w| of every output of a conv (or Linear, w [N, K]) of x with w."""
-    return float(x.abs().max()) * float(w.double().abs().reshape(w.shape[0], -1).sum(dim=1).max())
-
-
-def assert_exact(out, ref, guard, what) -> None:
-    """out (f32 or f16) equals the exact float64 value ref rounded once (f32(ref) is exact, so f16(f32(ref)) is RN-even); the
-    guard after it (if any) is still NaN."""
-    want = ref.float() if out.dtype == torch.float32 else ref.float().half()
-    bad = out != want
-    n_bad = int(bad.sum())
-    first = tuple(bad.nonzero()[0].tolist()) if n_bad else None
-    print(f"{what}: {bad.numel() - n_bad} / {bad.numel()} exact")
-    assert n_bad == 0, (f"{what}: {n_bad} elements differ from the exact value, first at {first}: "
-                        f"{float(out[first])} != {float(want[first])}")
-    assert guard is None or bool(guard.isnan().all()), f"{what}: elements after the output were written"
-
-
-def conv_ref(x, w, stride=1):
-    """Exact float64 conv (padding k // 2) of x [B, H, W, I] with w [O, I, k, k]: one matmul per tap over a shifted (strided)
-    view of the zero-padded input. [B, Ho, Wo, O]."""
-    B, H, W, I = x.shape
-    O, _, k, _ = w.shape
-    p = k // 2
-    xp = F.pad(x.double(), (0, 0, p, p, p, p))
-    Ho, Wo = (H + 2 * p - k) // stride + 1, (W + 2 * p - k) // stride + 1
-    wd = w.double()
-    out = torch.zeros(B, Ho, Wo, O, dtype=torch.float64, device=x.device)
-    for kh in range(k):
-        for kw in range(k):
-            out += xp[:, kh:kh + stride * (Ho - 1) + 1:stride, kw:kw + stride * (Wo - 1) + 1:stride] @ wd[:, :, kh, kw].t()
-    return out
-
-
-def linear(x16, wt, N, Kpad, out, ldo, bias=None, res=None, mode=LINEAR, geglu_bn=0) -> None:
-    """PlanBuilder::linear: x [M, K] as a (1, 1, M, K) image, one 1x1 segment over the padded K."""
-    M, K = x16.shape
-    T.igemm(x16, (1, 1, M, K), wt, N, Kpad, (M, 1, 1), [(0, 0, 0, 0, Kpad // 64)], out, ldo, bias=bias, res=res,
-            ldr=ldo if res is not None else 0, mode=mode, geglu_bn=geglu_bn)
-
-
-def lin_weights(g, K, N, geglu_bn=0, wt=None, row0=0):
-    """A grid Linear weight [K, N] (stored [in, out]) and its plan layout (Loader::lin_into): transpose_linear's K-major
-    [N, Kpad], rows from row0 of wt (a fused matrix) or of a new one."""
-    w = grid_w(g, K, N)
-    if wt is None:
-        wt = torch.empty(N * pad64(K), dtype=torch.float16, device=DEV)
-    T.transpose_linear(w, K, N, wt, pad64(K), row0, geglu_bn)
-    return w, wt
 
 
 # ------------------------------------------------------------------------------------------------------------------------------
@@ -218,13 +119,6 @@ def test_resblock_conv_out_identity(ctx, B, H, W, C):
     assert_exact_range("conv_out + identity", conv_bound(a0, w), b16.abs().max(), res.abs().max())
     T.igemm(a0, (B, H, W, C), wt, C, Ktot, (W, H, B), conv_taps(pad64(C) // 64), out, C, bias=b32, res=res, ldr=C)
     assert_exact(out, conv_ref(a0, w) + b16.double() + res.double(), guard, f"resblock conv_out + identity {B}x{H}x{W}x{C}")
-
-
-def stride2_taps(Bn: int, nkb: int):
-    """engine_core.h stride2_taps: tap (kh, kw) reads phase (kh != 1, kw != 1) of the phase split, one row / column back
-    for kh / kw = 0."""
-    return [(0, -1 if kw == 0 else 0, -1 if kh == 0 else 0, ((kh != 1) * 2 + (kw != 1)) * Bn, nkb)
-            for kh in range(3) for kw in range(3)]
 
 
 @pytest.mark.parametrize("B,H,W,C", [(2, 128, 128, 320), (3, 152, 104, 320), (2, 64, 64, 640), (3, 76, 52, 640),
@@ -320,20 +214,6 @@ def test_strans_proj_in_proj_out(ctx, M, C):
         linear(x, wt, C, pad64(C), out, C, bias=b32, res=res)
         ref = x.double() @ w.double() + b16.double() + (0 if res is None else res.double())
         assert_exact(out, ref, guard, f"strans {name} M={M} C={C}")
-
-
-def in_place_residual(g, x, w, wt, b16, b32, what) -> None:
-    """out == res: the f32 residual stream updated in place, against the exact value and, bit for bit, against the same launch
-    writing a separate output."""
-    M, N = x.shape[0], w.shape[1]
-    res = grid_f32(g, M, N)
-    assert_exact_range(what, conv_bound(x, w.t()), b16.abs().max(), res.abs().max())
-    inplace, guard = guarded((M, N), fill=res)
-    linear(x, wt, N, pad64(x.shape[1]), inplace, N, bias=b32, res=inplace)
-    sep, _ = guarded((M, N))
-    linear(x, wt, N, pad64(x.shape[1]), sep, N, bias=b32, res=res)
-    assert_exact(inplace, x.double() @ w.double() + b16.double() + res.double(), guard, what)
-    assert torch.equal(inplace, sep), f"{what}: the in-place launch differs from the one with a separate output"
 
 
 @pytest.mark.parametrize("M,C", LIN_SHAPES)
