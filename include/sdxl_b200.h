@@ -58,6 +58,7 @@ typedef struct sdxl_unet_cfg {
   int32_t context_dim;                        /* 2048 base / 1280 refiner */
   int32_t is_refiner;                         /* Diffuser.is_refiner: single forward, no CFG */
   int32_t n_steps;                            /* 1000 (stablediffusion/mod.rs:282) */
+  int32_t edit_layout;                        /* 0; 1: the instruction-editing layout (sdxl_unet_set_edit_image, DESIGN.md §21) */
 } sdxl_unet_cfg;
 
 /* Mirrors Conditioning (src/model/stablediffusion/mod.rs:544-555); f16 like the reference's
@@ -659,6 +660,35 @@ typedef struct sdxl_inpaint_condition {
  * b % n) is not a multiple of n. */
 SDXL_API int sdxl_unet_set_inpaint_condition(sdxl_unet* unet, const sdxl_inpaint_condition* c);
 
+/* ---- instruction-based editing (InstructPix2Pix) ------------------------------------------------------------
+ * diffusers' StableDiffusionXLInstructPix2PixPipeline (DESIGN.md §21; diffusers/sdxl-instructpix2pix-768). A cfg with edit_layout = 1
+ * has in_channels = 2 * out_channels: its first conv reads the latent (out_channels) and the source image's latent L (out_channels),
+ * concatenated in that order. The latent the forward entry points and the samplers take and return has out_channels channels; L is
+ * attached here, unscaled by the sampler's input scaling. Refused at load: edit_layout other than 0 or 1 (5700), in_channels other than
+ * 2 * out_channels (5701), with is_refiner (5702); a ControlNet cfg with the edit layout (5703).
+ * Rows. A direct forward of B rows: row r reads image r % n. The sampling loops with CFG run three row groups of the n_batch images,
+ * [cond | img | uncond], with context and pooled/time ids [c | n | n] (the negative prompt twice) and first-conv condition
+ * [L | L | 0]; the guided output (diffusers' order of terms, f32 in that order) is
+ *   g = (u + s * (c - i)) + s_img * (i - u)          s = guidance_scale, s_img = image_guidance
+ * and guidance rescale, v-prediction and every sampler take this g (sdxl_unet_set_prediction). no_cfg runs [c] with L alone.
+ * Refused at a forward or sampler_begin on an edit UNet, each leaving every state as it was: nothing attached (5720), an image of another
+ * size (5721), a batch that is not a multiple of n (5722), PAG attached (5723; it would need a fourth group), ControlNets (5724),
+ * T2I-Adapters (5725) or image prompts (5726) attached; and the latent-blend arguments inpaint_ref / inpaint_mask of the sampling calls
+ * (5727). */
+typedef struct sdxl_edit_image {
+  const float* latent;     /* f32 NCHW [n, out_channels, height/8, width/8]: the source image's VAE latent (posterior mean, not scaled by
+                              the VAE scaling factor); borrowed for the call */
+  int32_t on_host;
+  int32_t n;               /* row rule above */
+  int32_t height, width;   /* pixels; the latent must be height/8 x width/8 */
+  float image_guidance;    /* s_img, finite */
+} sdxl_edit_image;
+/* Copies the source latent into a buffer the UNet owns (NULL detaches). Everything is validated before anything changes (the UNet has
+ * the edit layout 5710, latent non-null 5711, n >= 1 5712, height and width positive multiples of 8 5713, image_guidance finite 5714;
+ * 5715: the buffer cannot be allocated): on failure the previous image stays attached. A call with the same n and size rewrites the
+ * image and s_img in place (same launch plan and CUDA graph); any other change rebuilds the plan at the next forward. */
+SDXL_API int sdxl_unet_set_edit_image(sdxl_unet* unet, const sdxl_edit_image* e);
+
 /* ---- perturbed-attention guidance (PAG) ------------------------------------------------------------------
  * Ahn et al. 2024, as diffusers' StableDiffusionXL*PAGPipeline runs it (DESIGN.md §14). The sampler adds a third row group to its
  * batch: [cond | uncond | ptb] (the refiner, without CFG: [cond | ptb]). The perturbed rows repeat the conditional rows' context, pooled
@@ -736,7 +766,7 @@ SDXL_API int sdxl_unet_set_deepcache(sdxl_unet* unet, const sdxl_deepcache* dc);
 /* ---- prediction type, guidance rescale and the noise table ------------------------------------------------------------
  * DESIGN.md §18. What the sampling loops (sdxl_sample_latent, sdxl_sample_latent_scheduled, sdxl_sampler_step and
  * sdxl_sampler_step_host) read the UNet's output as. With the rows [cond | uncond | ptb], m the output of a row, the guided output is
- * g = u + (c - u) * s, plus p_t * (c - ptb) with PAG, and then:
+ * g = u + (c - u) * s, plus p_t * (c - ptb) with PAG (an edit UNet's rows [cond | img | uncond]: sdxl_unet_set_edit_image's g), and then:
  *   guidance rescale (phi > 0, calls with CFG rows only; diffusers' rescale_noise_cfg, Lin et al. 2023): for each image b,
  *                    g <- phi * g * std(c_b) / std(g_b) + (1 - phi) * g, both std unbiased over the C * H * W elements of the image,
  *                    the ratio read as 1 when std(g_b) = 0. It acts on the model output, v for a v model. no_cfg calls and the refiner,

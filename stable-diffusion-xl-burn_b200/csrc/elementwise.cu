@@ -426,11 +426,12 @@ int nhwc_to_nchw_f16_launch(cudaStream_t st, const float* x, int B, int HW, int 
 // ------------------------------------------------------------------------------------------------
 // DDIM eta=0 on the guided eps of the NHWC rows [cond], [cond | uncond], [cond | ptb] or [cond | uncond | ptb]:
 //   e = u + (c - u) * g (use_cfg) or c;  then, with perturbed-attention guidance, e = e + p_t * (c - ptb)
-// kV, kRescale: kernels.h Prediction; <false, false> is the epsilon step and never reads `factor`.
-template <bool kV, bool kRescale>
+// kV, kRescale: kernels.h Prediction; <false, false> is the epsilon step and never reads `factor`. kImg: image guidance (DESIGN.md §21)
+// on the rows [cond | img | uncond], e = (u + (c - i) * g) + s_img * (i - u); use_cfg and use_pag are not read.
+template <bool kV, bool kRescale, bool kImg = false>
 __global__ void cfg_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
                                 float g, float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map,
-                                float* __restrict__ x, const float* __restrict__ factor) {
+                                float* __restrict__ x, const float* __restrict__ factor, float s_img) {
   const long total = (long)Bimg * C * HW;
   const int ptb_row0 = (use_cfg ? 2 : 1) * Bimg;
   for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
@@ -439,14 +440,20 @@ __global__ void cfg_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg,
     const int b = (int)(i / ((long)HW * C));
     const float ec = eps[((size_t)b * HW + p) * ld + c];
     float e = ec;
-    if (use_cfg) {
-      // u + (c - u) * s   (reference stablediffusion/mod.rs:539-540)
-      const float eu = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
-      e = eu + (ec - eu) * g;
-    }
-    if (use_pag) {
-      const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
-      e = e + p_t * (ec - ep);
+    if constexpr (kImg) {
+      const float ei = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
+      const float eu = eps[((size_t)(2 * Bimg + b) * HW + p) * ld + c];
+      e = (eu + (ec - ei) * g) + s_img * (ei - eu);
+    } else {
+      if (use_cfg) {
+        // u + (c - u) * s   (reference stablediffusion/mod.rs:539-540)
+        const float eu = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
+        e = eu + (ec - eu) * g;
+      }
+      if (use_pag) {
+        const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
+        e = e + p_t * (ec - ep);
+      }
     }
     if constexpr (kRescale) e *= factor[b];
     const float xv = x[i];
@@ -462,12 +469,16 @@ __global__ void cfg_ddim_kernel(const float* __restrict__ eps, int ld, int Bimg,
   }
 }
 int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag, float guidance,
-                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x, const Prediction& pr) {
+                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x, const Prediction& pr, int use_img,
+                    float img_guidance) {
   const long total = (long)Bimg * C * HW;
   auto kernel = pr.v ? (pr.factor ? cfg_ddim_kernel<true, true> : cfg_ddim_kernel<true, false>)
                      : (pr.factor ? cfg_ddim_kernel<false, true> : cfg_ddim_kernel<false, false>);
+  if (use_img)
+    kernel = pr.v ? (pr.factor ? cfg_ddim_kernel<true, true, true> : cfg_ddim_kernel<true, false, true>)
+                  : (pr.factor ? cfg_ddim_kernel<false, true, true> : cfg_ddim_kernel<false, false, true>);
   kernel<<<cdiv(total, 256), 256, 0, st>>>(eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map,
-                                           x, pr.factor);
+                                           x, pr.factor, img_guidance);
   return (int)cudaGetLastError();
 }
 
@@ -503,9 +514,11 @@ size_t guidance_stats_scratch_bytes(int Bimg) { return gs_counter_bytes(Bimg) + 
 int guidance_stats_scratch_init(cudaStream_t st, void* scratch, int Bimg) {
   return (int)cudaMemsetAsync(scratch, 0, gs_counter_bytes(Bimg), st);
 }
+// kImg: the image-guidance combine of cfg_ddim_kernel<.., .., true> on the rows [cond | img | uncond]; use_pag is not read.
+template <bool kImg = false>
 __global__ void __launch_bounds__(kGsThreads) guidance_stats_kernel(const float* __restrict__ eps, int ld, int Bimg, int C, int HW,
                                                                      int use_pag, float g, float p_t, float phi, unsigned* counters,
-                                                                     Moments* partial, float* __restrict__ factor) {
+                                                                     Moments* partial, float* __restrict__ factor, float s_img) {
   const int b = blockIdx.y, nb = gridDim.x;
   const long n = (long)C * HW;
   const int ptb_row0 = 2 * Bimg;
@@ -514,11 +527,18 @@ __global__ void __launch_bounds__(kGsThreads) guidance_stats_kernel(const float*
     const int p = (int)(i / C);
     const int c = (int)(i % C);
     const float ec = eps[((size_t)b * HW + p) * ld + c];
-    const float eu = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
-    float e = eu + (ec - eu) * g;
-    if (use_pag) {
-      const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
-      e = e + p_t * (ec - ep);
+    float e;
+    if constexpr (kImg) {
+      const float ei = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
+      const float eu = eps[((size_t)(2 * Bimg + b) * HW + p) * ld + c];
+      e = (eu + (ec - ei) * g) + s_img * (ei - eu);
+    } else {
+      const float eu = eps[((size_t)(Bimg + b) * HW + p) * ld + c];
+      e = eu + (ec - eu) * g;
+      if (use_pag) {
+        const float ep = eps[((size_t)(ptb_row0 + b) * HW + p) * ld + c];
+        e = e + p_t * (ec - ep);
+      }
     }
     welford(mc, ec);
     welford(mg, e);
@@ -574,12 +594,13 @@ __global__ void __launch_bounds__(kGsThreads) guidance_stats_kernel(const float*
   counters[b] = 0u;   // ready for the next launch
 }
 int guidance_stats_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_pag, float guidance, float p_t,
-                          float phi, void* scratch, float* factor) {
+                          float phi, void* scratch, float* factor, int use_img, float img_guidance) {
   const long n = (long)C * HW;
   if (Bimg < 1 || n < 1) return (int)cudaErrorInvalidValue;
   const int want = cdiv(n, (long)kGsThreads * kGsPerThread), nb = want < kGsMaxBlocks ? want : kGsMaxBlocks;
-  guidance_stats_kernel<<<dim3(nb, Bimg), kGsThreads, 0, st>>>(eps, ld, Bimg, C, HW, use_pag, guidance, p_t, phi, (unsigned*)scratch,
-                                                               (Moments*)((uint8_t*)scratch + gs_counter_bytes(Bimg)), factor);
+  auto kernel = use_img ? guidance_stats_kernel<true> : guidance_stats_kernel<false>;
+  kernel<<<dim3(nb, Bimg), kGsThreads, 0, st>>>(eps, ld, Bimg, C, HW, use_pag, guidance, p_t, phi, (unsigned*)scratch,
+                                                (Moments*)((uint8_t*)scratch + gs_counter_bytes(Bimg)), factor, img_guidance);
   return (int)cudaGetLastError();
 }
 
@@ -713,9 +734,9 @@ __device__ __forceinline__ void store4(float* __restrict__ p, size_t blk, size_t
   }
 }
 // kV, kRescale: kernels.h Prediction; <false, false> is the epsilon step and never reads `pr`. kRows: kernels.h StepRows, the
-// two-row form; without it `r` is never read.
-template <bool kV, bool kRescale, bool kRows>
-__global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams p, int aligned, const Prediction pr, const StepRows r) {
+// two-row form; without it `r` is never read. kImg: cfg_ddim_kernel's image-guidance combine with scale s_img (guided_step_img_kernel).
+template <bool kV, bool kRescale, bool kRows, bool kImg>
+__device__ __forceinline__ void guided_step(const GuidedStepParams& p, int aligned, const Prediction& pr, const StepRows& r, float s_img) {
   const size_t n = (size_t)p.Bimg * p.C * p.HW, nblk = (n + 3) / 4;
   const size_t blk = (size_t)blockIdx.x * blockDim.x + threadIdx.x;
   if (blk >= nblk) return;
@@ -734,13 +755,19 @@ __global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams
       const int b = (int)(i / ((size_t)p.HW * p.C));
       const float ec = p.eps[((size_t)b * p.HW + px) * p.ld + c];
       float e = ec;
-      if (p.use_cfg) {   // u + (c - u) * s, cfg_ddim_kernel's order
-        const float eu = p.eps[((size_t)(grp_u + b) * p.HW + px) * p.ld + c];
-        e = eu + (ec - eu) * p.guidance;
-      }
-      if (p.use_pag) {   // cfg_ddim_kernel's
-        const float ep = p.eps[((size_t)(grp_p + b) * p.HW + px) * p.ld + c];
-        e = e + p.p_t * (ec - ep);
+      if constexpr (kImg) {   // cfg_ddim_kernel's, rows [cond | img | uncond]
+        const float ei = p.eps[((size_t)(p.Bimg + b) * p.HW + px) * p.ld + c];
+        const float eu = p.eps[((size_t)(2 * p.Bimg + b) * p.HW + px) * p.ld + c];
+        e = (eu + (ec - ei) * p.guidance) + s_img * (ei - eu);
+      } else {
+        if (p.use_cfg) {   // u + (c - u) * s, cfg_ddim_kernel's order
+          const float eu = p.eps[((size_t)(grp_u + b) * p.HW + px) * p.ld + c];
+          e = eu + (ec - eu) * p.guidance;
+        }
+        if (p.use_pag) {   // cfg_ddim_kernel's
+          const float ep = p.eps[((size_t)(grp_p + b) * p.HW + px) * p.ld + c];
+          e = e + p.p_t * (ec - ep);
+        }
       }
       if constexpr (kRescale) e *= pr.factor[b];
       if constexpr (kV) D[j] = pr.dx * xh[j] - pr.de * e;
@@ -795,26 +822,46 @@ __global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams
   for (int j = 0; j < 4; ++j) nx[j] *= p.c_in;
   store4(p.x_in, blk, n, vec, nx);
 }
-int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr, const StepRows* rows) {
+template <bool kV, bool kRescale, bool kRows>
+__global__ void __launch_bounds__(256) guided_step_kernel(const GuidedStepParams p, int aligned, const Prediction pr, const StepRows r) {
+  guided_step<kV, kRescale, kRows, false>(p, aligned, pr, r, 0.f);
+}
+template <bool kV, bool kRescale, bool kRows>
+__global__ void __launch_bounds__(256) guided_step_img_kernel(const GuidedStepParams p, int aligned, const Prediction pr, const StepRows r,
+                                                              float s_img) {
+  guided_step<kV, kRescale, kRows, true>(p, aligned, pr, r, s_img);
+}
+// The instantiation of (kV, kRescale) = (pr.v, pr.factor) at the given kRows, without and with image guidance.
+template <bool kRows>
+static auto guided_step_pick(const Prediction& pr) {
+  return pr.v ? (pr.factor ? guided_step_kernel<true, true, kRows> : guided_step_kernel<true, false, kRows>)
+              : (pr.factor ? guided_step_kernel<false, true, kRows> : guided_step_kernel<false, false, kRows>);
+}
+template <bool kRows>
+static auto guided_step_img_pick(const Prediction& pr) {
+  return pr.v ? (pr.factor ? guided_step_img_kernel<true, true, kRows> : guided_step_img_kernel<true, false, kRows>)
+              : (pr.factor ? guided_step_img_kernel<false, true, kRows> : guided_step_img_kernel<false, false, kRows>);
+}
+int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr, const StepRows* rows, int use_img,
+                       float img_guidance) {
   const size_t n = (size_t)p.Bimg * p.C * p.HW;
   if (!n) return 0;
   if (!p.xh || !p.x_in || ((p.ch != 0.f || p.write_hist) && !p.hist) || (p.mask && !p.ref)) return (int)cudaErrorInvalidValue;
   uintptr_t a = (uintptr_t)p.xh | (uintptr_t)p.x_in | (uintptr_t)p.hist | (uintptr_t)p.z | (uintptr_t)p.zb | (uintptr_t)p.ref;
   const unsigned grid = cdiv((long)((n + 3) / 4), 256);
+  const bool img = use_img && p.eps;
   if (rows) {
     const StepRows& r = *rows;
     if (((r.cs != 0.f || r.ss != 0.f || r.write_xs) && !r.xs) || ((r.sh != 0.f || r.shift) && !p.hist) ||
         ((r.ch2 != 0.f || r.sh2 != 0.f || r.shift) && !r.h2))
       return (int)cudaErrorInvalidValue;
     a |= (uintptr_t)r.xs | (uintptr_t)r.h2;
-    auto kernel = pr.v ? (pr.factor ? guided_step_kernel<true, true, true> : guided_step_kernel<true, false, true>)
-                       : (pr.factor ? guided_step_kernel<false, true, true> : guided_step_kernel<false, false, true>);
-    kernel<<<grid, 256, 0, st>>>(p, a % 16 == 0, pr, r);
+    if (img) guided_step_img_pick<true>(pr)<<<grid, 256, 0, st>>>(p, a % 16 == 0, pr, r, img_guidance);
+    else guided_step_pick<true>(pr)<<<grid, 256, 0, st>>>(p, a % 16 == 0, pr, r);
     return (int)cudaGetLastError();
   }
-  auto kernel = pr.v ? (pr.factor ? guided_step_kernel<true, true, false> : guided_step_kernel<true, false, false>)
-                     : (pr.factor ? guided_step_kernel<false, true, false> : guided_step_kernel<false, false, false>);
-  kernel<<<grid, 256, 0, st>>>(p, a % 16 == 0, pr, StepRows{});
+  if (img) guided_step_img_pick<false>(pr)<<<grid, 256, 0, st>>>(p, a % 16 == 0, pr, StepRows{}, img_guidance);
+  else guided_step_pick<false>(pr)<<<grid, 256, 0, st>>>(p, a % 16 == 0, pr, StepRows{});
   return (int)cudaGetLastError();
 }
 

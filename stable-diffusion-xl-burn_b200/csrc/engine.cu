@@ -147,9 +147,12 @@ static BlockProgram block_program(const sdxl_unet_cfg& g) {
 // the mask (1) and the masked image's latent (out_channels), concatenated. The one-source first conv takes at most 8 channels, so
 // no configuration loadable without this layout has it.
 static bool inpaint_layout(const sdxl_unet_cfg& g) { return g.in_channels > 8 && g.in_channels == 2 * g.out_channels + 1; }
-// Channels of the latent the forward and the sampler take: out_channels on an inpainting UNet (the rest comes from the attached
-// condition), in_channels otherwise.
-static int latent_channels(const sdxl_unet_cfg& g) { return inpaint_layout(g) ? g.out_channels : g.in_channels; }
+// The instruction-editing UNet (DESIGN.md §21, diffusers' sdxl-instructpix2pix-768): its input is the latent and the source image's
+// latent (out_channels each), concatenated. Only the explicit flag selects it: an 8 -> 4 cfg without it keeps its 8-channel latent.
+static bool edit_layout(const sdxl_unet_cfg& g) { return g.edit_layout != 0; }
+// Channels of the latent the forward and the sampler take: out_channels on an inpainting or edit UNet (the rest comes from the
+// attachment), in_channels otherwise.
+static int latent_channels(const sdxl_unet_cfg& g) { return inpaint_layout(g) || edit_layout(g) ? g.out_channels : g.in_channels; }
 
 struct Plan;
 struct Sampler;
@@ -169,6 +172,15 @@ struct InpaintAttach {
   Extent ext;
   Arena mem;
   float* cond = nullptr;
+};
+
+// An attached source image of an edit UNet (sdxl_unet_set_edit_image): its latent f32 NCHW [n, out_channels, h, w], owned, and s_img.
+// The first conv reads the plan's per-row copy (sdxl_unet::plan_edit), refreshed from here whenever either changes.
+struct EditAttach {
+  Extent ext;
+  float image_guidance = 0.f;
+  Arena mem;
+  float* latent = nullptr;
 };
 
 // Perturbed-attention guidance (sdxl_unet_set_pag, DESIGN.md §14): the self-attentions that run as the identity on the perturbed
@@ -194,12 +206,13 @@ struct DeepcacheAttach {
 };
 
 // Roles of the conditioning rows. The sampler's batch is row groups of n_img rows each: [cond | uncond] with CFG, then a perturbed
-// group with PAG ([cond | uncond | ptb]; the refiner: [cond] or [cond | ptb]). The perturbed rows are conditional rows. n_img = 0:
-// a plain batch, every row conditional.
+// group with PAG ([cond | uncond | ptb]; the refiner: [cond] or [cond | ptb]). The perturbed rows are conditional rows. An edit UNet
+// with CFG runs [cond | img | uncond], both of the last two with the negative prompt. n_img = 0: a plain batch, every row conditional.
 struct RowLayout {
   int n_img = 0;
   bool uncond = false;   // group 1 is the unconditional one
-  bool negative(int r) const { return uncond && r / n_img == 1; }
+  bool uncond2 = false;  // so is group 2 (image guidance)
+  bool negative(int r) const { return (uncond && r / n_img == 1) || (uncond2 && r / n_img == 2); }
 };
 
 // Embeddings, first conv, input blocks and middle block: the part of the UNet a ControlNet copies.
@@ -261,6 +274,7 @@ struct sdxl_unet : EncoderHalf {
   std::unique_ptr<IpAttach> ip;   // sdxl_unet_set_image_prompts
   std::unique_ptr<T2IAttach> t2i; // sdxl_unet_set_t2i_adapters
   std::unique_ptr<InpaintAttach> inpaint;   // sdxl_unet_set_inpaint_condition
+  std::unique_ptr<EditAttach> edit;         // sdxl_unet_set_edit_image
   std::unique_ptr<PagAttach> pag;           // sdxl_unet_set_pag
   std::unique_ptr<FreeuAttach> freeu;       // sdxl_unet_set_freeu
   std::unique_ptr<DeepcacheAttach> deepcache;   // sdxl_unet_set_deepcache
@@ -268,6 +282,8 @@ struct sdxl_unet : EncoderHalf {
   int plan_ptb = 0;               // trailing rows of the current plan that take PAG's identity self-attentions
   int plan_dc = -1;               // DeepCache branch of the current plan's cached list (-1: none)
   bool dc_feature = false;        // a full run of the current plan has kept DeepCache's feature
+  float* plan_edit = nullptr;     // edit UNet: the first conv's condition per row of the current plan, f32 NCHW [Bf, out_channels, h, w]
+  int plan_edit_zero = 0;         // its trailing rows that are zero (the sampler's unconditional group with image guidance)
   RowLayout rows;                 // roles of the conditioning rows
   ~sdxl_unet() {
     if (t_dev) cudaFree(t_dev);
@@ -556,6 +572,10 @@ static int build_model(sdxl_unet* u, const PackView& pv, Arena& A) {
 // ================================================================================================
 // The configurations the UNet (and a ControlNet's copy of its encoder) are built for.
 static int check_unet_cfg(sdxl_ctx* c, const sdxl_unet_cfg& g) {
+  if (g.edit_layout != 0 && g.edit_layout != 1) return fail(c, 5700, "edit_layout = %d must be 0 or 1", g.edit_layout);
+  if (edit_layout(g) && g.in_channels != 2 * g.out_channels)
+    return fail(c, 5701, "edit_layout: in_channels = %d must be 2 * out_channels = %d", g.in_channels, 2 * g.out_channels);
+  if (edit_layout(g) && g.is_refiner) return fail(c, 5702, "edit_layout: not supported with is_refiner");
   if (g.n_head_channels != 64) return fail(c, 4200, "n_head_channels must be 64 (got %d)", g.n_head_channels);
   if (g.n_levels < 1 || g.n_levels > SDXL_MAX_LEVELS) return fail(c, 4201, "bad n_levels");
   if ((g.in_channels > 8 && !inpaint_layout(g)) || g.model_channels % 32) return fail(c, 4202, "unsupported channel config");
@@ -699,6 +719,7 @@ extern "C" int sdxl_controlnet_load(sdxl_ctx* c, const sdxl_controlnet_cfg* cfg,
   *out = nullptr;
   if (int r = check_unet_cfg(c, cfg->unet)) return r;
   if (inpaint_layout(cfg->unet)) return fail(c, 4703, "ControlNet: a UNet cfg with the inpainting layout (in_channels = %d) is not supported", cfg->unet.in_channels);
+  if (edit_layout(cfg->unet)) return fail(c, 5703, "ControlNet: a UNet cfg with the edit layout is not supported");
   if (cfg->hint_in_channels < 1 || cfg->hint_in_channels > 8) return fail(c, 4700, "hint_in_channels must be in [1, 8] (got %d)", cfg->hint_in_channels);
   if (cfg->n_hint_blocks != 4) return fail(c, 4701, "n_hint_blocks must be 4 (hint downscale 2^(n-1) = 8), got %d", cfg->n_hint_blocks);
   for (int k = 0; k < cfg->n_hint_blocks; ++k)
@@ -833,6 +854,7 @@ struct UNetPlanBuilder : PlanBuilder {
       op.kind = OP_CONV_IN;
       op.ci = {P->x_in, P->Bx, Bf, latent_channels(g), H, W, e.conv0_w, e.conv0_b, mc, x, hint, n_hint};
       if (inpaint_layout(g)) { op.ci.x2 = ipc->cond; op.ci.n2 = ipc->ext.n; op.ci.C2 = g.in_channels - g.out_channels; }
+      if (edit_layout(g) && cond == &u->cond) { op.ci.x2 = u->plan_edit; op.ci.n2 = Bf; op.ci.C2 = g.out_channels; }
       P->ops.push_back(op);
       P->flops += 2.0 * Bf * H * W * 9.0 * g.in_channels * mc;
     }
@@ -1201,6 +1223,7 @@ static int build_plan_ops(sdxl_unet* u, Plan* P, Arena* A, int Bp) {
   if ((P->h % (1 << (levels - 1))) || (P->w % (1 << (levels - 1)))) return fail(c, 5003, "latent %dx%d not divisible by %d", P->h, P->w, 1 << (levels - 1));
 
   P->x_in = B.buf<float>((size_t)P->Bx * latent_channels(g) * P->h * P->w);
+  if (edit_layout(g)) u->plan_edit = B.buf<float>((size_t)Bf * g.out_channels * P->h * P->w);
   P->eps_ld = g.out_channels;
   P->eps = B.buf<float>((size_t)Bf * P->h * P->w * P->eps_ld);
   B.gn_partial = B.buf<float>(gn_scratch_floats(Bf, 32));
@@ -1275,14 +1298,36 @@ static int attachments_fit(sdxl_unet* u, int n_img, int h, int w) {
       if (a.mask_h && (a.mask_h / 8 != h || a.mask_w / 8 != w))
         return fail(c, 5021, "image prompt: its masks are %dx%d pixels (latent %dx%d) but the latent is %dx%d", a.mask_h, a.mask_w,
                     a.mask_h / 8, a.mask_w / 8, h, w);
+  if (edit_layout(u->cfg)) {   // image guidance takes the third row group and the first conv's second source
+    if (!u->edit) return fail(c, 5720, "edit UNet: no source image attached (call sdxl_unet_set_edit_image first)");
+    if (u->pag) return fail(c, 5723, "edit UNet: PAG is attached; image guidance and PAG would need a fourth row group");
+    if (!u->controls.empty()) return fail(c, 5724, "edit UNet: ControlNets are attached; they are not supported with image guidance");
+    if (u->t2i) return fail(c, 5725, "edit UNet: T2I-Adapters are attached; they are not supported with image guidance");
+    if (u->ip) return fail(c, 5726, "edit UNet: image prompts are attached; they are not supported with image guidance");
+    return fit("edit image", "it is", u->edit->ext, "its n", 5721);
+  }
   if (!inpaint_layout(u->cfg)) return 0;
   if (!u->inpaint) return fail(c, 5018, "inpainting UNet: no inpainting condition attached (call sdxl_unet_set_inpaint_condition first)");
   return fit("inpainting condition", "it is", u->inpaint->ext, "its n", 5019);
 }
 
+// An edit UNet's per-row first-conv condition of the current plan (plan_edit), from the attached image: row r of the first
+// Bf - plan_edit_zero reads image r % n, the rest are zero. Called when the plan is built and when the image is rewritten in place.
+static int edit_rows_fill(sdxl_unet* u) {
+  sdxl_ctx* c = u->ctx;
+  if (!edit_layout(u->cfg) || !u->plan || !u->edit) return 0;
+  const Plan* P = u->plan.get();
+  const size_t img = (size_t)u->cfg.out_channels * P->h * P->w * sizeof(float);
+  const int n = u->edit->ext.n, lit = P->Bf - u->plan_edit_zero;
+  for (int r = 0; r < lit; r += n)   // lit is a multiple of n (attachments_fit)
+    CU(c, cudaMemcpyAsync((uint8_t*)u->plan_edit + r * img, u->edit->latent, n * img, cudaMemcpyDeviceToDevice, c->stream));
+  if (u->plan_edit_zero) CU(c, cudaMemsetAsync((uint8_t*)u->plan_edit + lit * img, 0, u->plan_edit_zero * img, c->stream));
+  return 0;
+}
+
 // Bx: the images of the batch (the direct forward's B, the sampler's Bimg); Bp: the trailing rows that take PAG's identity
-// self-attentions (0: none; PAG attached when > 0).
-static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w, int Bp) {
+// self-attentions (0: none; PAG attached when > 0); Bz: an edit UNet's trailing rows whose first-conv condition is zero.
+static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w, int Bp, int Bz = 0) {
   sdxl_ctx* c = u->ctx;
   if (u->cond.condB != Bf) return fail(c, 5010, "conditioning is set for batch %d but forward batch is %d (call sdxl_unet_set_conditioning first)", u->cond.condB, Bf);
   if (Bp < 0 || Bp >= Bf) return fail(c, 5023, "PAG: %d perturbed rows in a batch of %d (at least one row must be attended)", Bp, Bf);
@@ -1293,14 +1338,16 @@ static int ensure_plan(sdxl_unet* u, int Bf, int Bx, int h, int w, int Bp) {
   // every change of the buffers or attachments a plan reads drops the plan, so the shapes, the perturbed rows and the DeepCache
   // branch are its whole cache key
   const int dc = u->deepcache ? u->deepcache->branch : -1;
-  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan_ptb == Bp && u->plan_dc == dc)
+  if (u->plan && u->plan->Bf == Bf && u->plan->Bx == Bx && u->plan->h == h && u->plan->w == w && u->plan_ptb == Bp && u->plan_dc == dc &&
+      u->plan_edit_zero == Bz)
     return 0;
   u->dc_feature = false;
   if (int r = build_plan(c, u->plan, Bf, Bx, h, w, [&](Plan* P, Arena* A) { return build_plan_ops(u, P, A, Bp); })) return r;
   u->plan_ptb = Bp;
   u->plan_dc = dc;
+  u->plan_edit_zero = Bz;
   u->plan_builds++;
-  return 0;
+  return edit_rows_fill(u);
 }
 
 // Refuses DeepCache's cached forward until a full run of the current plan has kept the feature it reads.
@@ -2293,6 +2340,44 @@ extern "C" int sdxl_unet_set_inpaint_condition(sdxl_unet* u, const sdxl_inpaint_
 }
 
 // ================================================================================================
+// instruction-based editing (include/sdxl_b200.h: sdxl_unet_set_edit_image; DESIGN.md §21)
+// ================================================================================================
+extern "C" int sdxl_unet_set_edit_image(sdxl_unet* u, const sdxl_edit_image* e) {
+  if (!u) return -1;
+  sdxl_ctx* c = u->ctx;
+  CU(c, cudaSetDevice(c->device));
+  const sdxl_unet_cfg& g = u->cfg;
+  if (!e) return attach_detach(u, u->edit);
+  // validate everything first: on failure the attached image is unchanged
+  if (!edit_layout(g)) return fail(c, 5710, "set_edit_image: the UNet does not have the edit layout (cfg edit_layout = 0)");
+  if (!e->latent) return fail(c, 5711, "set_edit_image: null latent");
+  if (e->n < 1) return fail(c, 5712, "set_edit_image: n = %d must be >= 1", e->n);
+  if (e->height < 8 || e->width < 8 || e->height % 8 || e->width % 8)
+    return fail(c, 5713, "set_edit_image: size %dx%d must be a positive multiple of 8", e->height, e->width);
+  if (!isfinite(e->image_guidance)) return fail(c, 5714, "set_edit_image: image_guidance = %g must be finite", e->image_guidance);
+  const Extent ext{e->n, e->height / 8, e->width / 8};
+  const size_t bytes = (size_t)ext.n * g.out_channels * ext.h * ext.w * sizeof(float);
+  EditAttach* cur = u->edit.get();
+  std::unique_ptr<EditAttach> fresh;
+  if (!cur || !(cur->ext == ext)) {   // new shape: a new buffer and a new plan
+    fresh.reset(new EditAttach());
+    fresh->ext = ext;
+    if (int r = carve_measured(c, fresh->mem, 5715, "set_edit_image: image buffer", [&](Arena& A) {
+          fresh->latent = A.get<float>(bytes / sizeof(float));
+          return 0;
+        }))
+      return r;
+    cur = fresh.get();
+  }
+  cur->image_guidance = e->image_guidance;
+  CU(c, cudaMemcpyAsync(cur->latent, e->latent, bytes, e->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice, c->stream));
+  if (fresh) return attach_install(u, u->edit, std::move(fresh));
+  if (int r = edit_rows_fill(u)) return r;   // the same plan and graph read the new values
+  CU(c, cudaStreamSynchronize(c->stream));   // the caller's memory
+  return 0;
+}
+
+// ================================================================================================
 // LoRA adapters (include/sdxl_b200.h; merge in engine_core.h: adapters_apply)
 // ================================================================================================
 extern "C" int sdxl_unet_set_adapters(sdxl_unet* u, int n, const sdxl_adapter* adapters) {
@@ -2502,6 +2587,7 @@ extern "C" double sdxl_unet_plan_flops_executed(const sdxl_unet* u) {
 struct Sampler {
   int Bimg = 0, nfwd = 1, h = 0, w = 0, n_ctx = 0;   // nfwd: row groups of Bimg rows, [cond | uncond] or [cond], then [ptb] with PAG
   bool cfg = false, pag = false;
+  bool img = false;        // image guidance: the rows are [cond | img | uncond] (an edit UNet with CFG)
   int evals = 0;           // UNet evaluations since sampler_begin (DeepCache: evaluation j is full when j % interval == 0)
   float guidance = 1.f;
   float* noise = nullptr;  // scratch [Bimg,4,h,w]
@@ -2525,16 +2611,17 @@ struct Sampler {
 
 // Uploads/assembles the batched conditioning: rows [0,Bimg) conditional, rows [Bimg,2*Bimg) the
 // unconditional context repeated (reference stablediffusion/mod.rs:506-537). With PAG attached a last group of Bimg rows repeats
-// the conditional rows (the refiner, without CFG: [cond | ptb]). no_cfg: the base model runs its conditional rows alone too.
+// the conditional rows (the refiner, without CFG: [cond | ptb]); an edit UNet with CFG repeats the unconditional rows there
+// ([cond | img | uncond], DESIGN.md §21), its first-conv condition zero. no_cfg: the base model runs its conditional rows alone too.
 static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double guidance, bool no_cfg = false) {
   sdxl_ctx* c = u->ctx;
   const sdxl_unet_cfg& g = u->cfg;
   if (!cond) return fail(c, 5200, "null conditioning");
   const int Bimg = cond->n_batch, n_ctx = cond->n_ctx;
   const int h = cond->resolution[0] / 8, w = cond->resolution[1] / 8;
-  const bool use_cfg = !g.is_refiner && !no_cfg, pag = u->pag != nullptr;
-  const int nfwd = (use_cfg ? 2 : 1) + (pag ? 1 : 0);
-  const RowLayout layout{Bimg, use_cfg};
+  const bool use_cfg = !g.is_refiner && !no_cfg, pag = u->pag != nullptr, img = edit_layout(g) && use_cfg;
+  const int nfwd = (use_cfg ? 2 : 1) + (pag || img ? 1 : 0);   // attachments_fit refuses PAG on an edit UNet
+  const RowLayout layout{Bimg, use_cfg, img};
   const sdxl_half* ctx_c = g.is_refiner ? cond->context_open_clip : cond->context_full;
   const sdxl_half* ctx_u = g.is_refiner ? cond->unconditional_context_open_clip : cond->unconditional_context_full;
   const sdxl_half* y_c = g.is_refiner ? cond->channel_context_refiner : cond->channel_context;
@@ -2576,6 +2663,7 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
   S->guidance = (float)guidance;
   S->cfg = use_cfg;
   S->pag = pag;
+  S->img = img;
   S->evals = 0;
   const cudaMemcpyKind kind = cond->on_host ? cudaMemcpyHostToDevice : cudaMemcpyDeviceToDevice;
   const size_t ctx_row = (size_t)n_ctx * g.context_dim * 2, y_row = (size_t)g.adm_in_channels * 2;
@@ -2586,13 +2674,15 @@ static int sampler_begin(sdxl_unet* u, const sdxl_conditioning* cond, double gui
       CU(c, cudaMemcpyAsync((uint8_t*)S->cond_ctx + ctx_row * (Bimg + b), ctx_u, ctx_row, kind, c->stream));
       CU(c, cudaMemcpyAsync((uint8_t*)S->cond_y + y_row * (Bimg + b), y_u, y_row, kind, c->stream));
     }
-  if (pag) {   // the perturbed group repeats the conditional rows
-    const int g0 = (nfwd - 1) * Bimg;
-    CU(c, cudaMemcpyAsync((uint8_t*)S->cond_ctx + ctx_row * g0, S->cond_ctx, ctx_row * Bimg, cudaMemcpyDeviceToDevice, c->stream));
-    CU(c, cudaMemcpyAsync((uint8_t*)S->cond_y + y_row * g0, S->cond_y, y_row * Bimg, cudaMemcpyDeviceToDevice, c->stream));
+  if (pag || img) {   // the perturbed group repeats the conditional rows, image guidance's third group the unconditional ones
+    const int g0 = (nfwd - 1) * Bimg, src = pag ? 0 : Bimg;
+    CU(c, cudaMemcpyAsync((uint8_t*)S->cond_ctx + ctx_row * g0, (uint8_t*)S->cond_ctx + ctx_row * src, ctx_row * Bimg, cudaMemcpyDeviceToDevice,
+                          c->stream));
+    CU(c, cudaMemcpyAsync((uint8_t*)S->cond_y + y_row * g0, (uint8_t*)S->cond_y + y_row * src, y_row * Bimg, cudaMemcpyDeviceToDevice,
+                          c->stream));
   }
   int r = set_conditioning_dev(u, nfwd * Bimg, n_ctx, S->cond_ctx, S->cond_y, layout);
-  if (!r) r = ensure_plan(u, nfwd * Bimg, Bimg, h, w, pag ? Bimg : 0);
+  if (!r) r = ensure_plan(u, nfwd * Bimg, Bimg, h, w, pag ? Bimg : 0, img ? Bimg : 0);
   if (r || !fresh) return r;
   CU(c, cudaStreamSynchronize(c->stream));   // the old sampler's buffers may still be in flight
   u->sampler = std::move(fresh);
@@ -2608,6 +2698,9 @@ static int run_sampler_plan(sdxl_unet* u) {
   return r;
 }
 
+// s_img of a sampler with image guidance (0 otherwise: the kernels do not read it)
+static float img_scale(const sdxl_unet* u) { return u->sampler->img ? u->edit->image_guidance : 0.f; }
+
 // PAG's scale at timestep t, with diffusers' adaptive scaling: p_t = max(scale - adaptive * (n_steps - t), 0)
 static float pag_scale(const sdxl_unet* u, double t) {
   return std::max(u->pag->scale - u->pag->adaptive * (float)(u->cfg.n_steps - t), 0.f);
@@ -2622,7 +2715,7 @@ static int step_prediction(sdxl_unet* u, float p_t, double sigma, Prediction& pr
   pr = Prediction{};
   if (u->guidance_rescale > 0.f && S->cfg) {
     KL(c, guidance_stats_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->pag, S->guidance, p_t,
-                                u->guidance_rescale, S->stats, S->rescale));
+                                u->guidance_rescale, S->stats, S->rescale, S->img, img_scale(u)));
     pr.factor = S->rescale;
   }
   if (u->prediction == SDXL_PREDICTION_V) {
@@ -2650,7 +2743,7 @@ static int sampler_step(sdxl_unet* u, int t, int t_prev) {
   Prediction pr;
   if ((r = step_prediction(u, p_t, sqrt((1.0 - a) / a), pr))) return r;
   KL(c, cfg_ddim_launch(c->stream, P->eps, P->eps_ld, S->Bimg, latent_channels(u->cfg), S->h * S->w, S->cfg, S->pag, S->guidance, p_t,
-                        (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap), P->x_in, pr));
+                        (float)sqrt(a), (float)sqrt(1.0 - a), (float)sqrt(ap), (float)sqrt(1.0 - ap), P->x_in, pr, S->img, img_scale(u)));
   return 0;
 }
 
@@ -2772,6 +2865,7 @@ extern "C" int sdxl_sample_latent(sdxl_unet* u, const sdxl_conditioning* cond, d
   if (n_steps < 1 || n_steps > total) return fail(c, 5220, "n_steps must be in [1,%d]", total);
   if (step_start < 0 || step_start >= total) return fail(c, 5221, "bad step_start");
   if ((inpaint_ref == nullptr) != (inpaint_mask == nullptr)) return fail(c, 5222, "inpaint_ref and inpaint_mask must be given together");
+  if (inpaint_ref && edit_layout(u->cfg)) return fail(c, 5727, "edit UNet: the latent-blend inpainting arguments are not supported");
   if (step_start > 0 && !init_latent) return fail(c, 5223, "refine (step_start>0) needs init_latent");
   int r = sample_begin(u, cond, guidance_scale, false, inpaint_ref, inpaint_mask);
   if (r) return r;
@@ -2843,6 +2937,7 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
   const std::string why = schedule_problem(sch, N);
   if (!why.empty()) return fail(c, 5230, "%s", why.c_str());
   if ((inpaint_ref == nullptr) != (inpaint_mask == nullptr)) return fail(c, 5231, "inpaint_ref and inpaint_mask must be given together");
+  if (inpaint_ref && edit_layout(u->cfg)) return fail(c, 5727, "edit UNet: the latent-blend inpainting arguments are not supported");
   if (sch->first_step > 0 && !init_latent) return fail(c, 5232, "schedule: first_step = %d needs init_latent", sch->first_step);
   if (n_noise < 0 || (n_noise > 0 && !noise)) return fail(c, 5233, "n_noise = %d with %s noise", n_noise, noise ? "a" : "null");
   const int n = sch->n_steps, k0 = sch->first_step, k1 = sch->last_step ? sch->last_step : n;
@@ -2920,7 +3015,7 @@ extern "C" int sdxl_sample_latent_scheduled(sdxl_unet* u, const sdxl_conditionin
       }
       Prediction pr;
       if ((r = step_prediction(u, p.p_t, q.sigma, pr))) return r;
-      KL(c, guided_step_launch(c->stream, p, pr, q.rows() ? &rows : nullptr));
+      KL(c, guided_step_launch(c->stream, p, pr, q.rows() ? &rows : nullptr, S->img, img_scale(u)));
     }
   }
   return sample_end(u, cond, S->xh, latent_out);

@@ -242,8 +242,11 @@ struct Prediction {
   const float* factor = nullptr;
   float dx = 0.f, de = 0.f;
 };
+// use_img (image guidance, DESIGN.md §21): the eps rows are [cond | img | uncond] and e = (u + (c - i) * guidance) + img_guidance * (i - u)
+// in that order; use_cfg and use_pag are then not read. The step kernels and guidance_stats_launch take it the same way.
 int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag, float guidance,
-                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x, const Prediction& pr = {});
+                    float p_t, float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x, const Prediction& pr = {},
+                    int use_img = 0, float img_guidance = 0.f);
 // Guidance rescale (diffusers' rescale_noise_cfg, Lin et al. 2023): for each image b of the rows [cond | uncond] or
 // [cond | uncond | ptb], with c_b its conditional output and g_b its guided output as the step kernels compute them,
 //   factor[b] = phi * std(c_b) / std(g_b) + (1 - phi)   (unbiased std over C * HW; std(c_b) / std(g_b) read as 1 when std(g_b) = 0)
@@ -253,7 +256,7 @@ int cfg_ddim_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, 
 size_t guidance_stats_scratch_bytes(int Bimg);
 int guidance_stats_scratch_init(cudaStream_t st, void* scratch, int Bimg);
 int guidance_stats_launch(cudaStream_t st, const float* eps, int ld, int Bimg, int C, int HW, int use_pag, float guidance, float p_t,
-                          float phi, void* scratch, float* factor);
+                          float phi, void* scratch, float* factor, int use_img = 0, float img_guidance = 0.f);
 // PAG's identity self-attention on `rows` token rows: out[r, 0:C] = qkv[r, 2C:3C] (qkv row pitch 3C, out row pitch C); C % 8 == 0,
 // both pointers 16-byte aligned.
 int pag_identity_launch(cudaStream_t st, const __half* qkv, int C, long rows, __half* out);
@@ -300,8 +303,9 @@ struct StepRows {
   float sx = 0.f, ss = 0.f, sd = 0.f, sh = 0.f, sh2 = 0.f;
   int write_xs = 0, shift = 0;
 };
-// rows == nullptr: the one-row form above.
-int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr = {}, const StepRows* rows = nullptr);
+// rows == nullptr: the one-row form above. use_img: cfg_ddim_launch's image-guidance combine of the rows [cond | img | uncond].
+int guided_step_launch(cudaStream_t st, const GuidedStepParams& p, const Prediction& pr = {}, const StepRows* rows = nullptr,
+                       int use_img = 0, float img_guidance = 0.f);
 
 // Latent-decoder kernels (vae_kernels.cu)
 // P[r,:] = softmax(scale * S[r,:]); S f32 [rows, lds] -> P f16 [rows, ldp]; cols % 4 == 0.

@@ -298,6 +298,19 @@ SDXL_TEST_API int sdxl_test_guidance_stats(void* stream, const float* eps, int l
                                            float p_t, float phi, void* scratch, float* factor) {
   return guidance_stats_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, use_pag, guidance, p_t, phi, scratch, factor);
 }
+// Image guidance (DESIGN.md §21): the v / rescale forms above with the combine of the rows [cond | img | uncond] at scale s_img.
+SDXL_TEST_API int sdxl_test_cfg_ddim_img(void* stream, const float* eps, int ld, int Bimg, int C, int HW, float guidance, float s_img,
+                                         float sqrt_a, float sqrt_1ma, float sqrt_ap, float sqrt_1map, float* x, int v, const float* factor) {
+  Prediction pr;
+  pr.v = v;
+  pr.factor = factor;
+  return cfg_ddim_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, 1, 0, guidance, 0.f, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x, pr, 1,
+                         s_img);
+}
+SDXL_TEST_API int sdxl_test_guidance_stats_img(void* stream, const float* eps, int ld, int Bimg, int C, int HW, float guidance, float s_img,
+                                               float phi, void* scratch, float* factor) {
+  return guidance_stats_launch((cudaStream_t)stream, eps, ld, Bimg, C, HW, 0, guidance, 0.f, phi, scratch, factor, 1, s_img);
+}
 SDXL_TEST_API int sdxl_test_inpaint_blend(void* stream, float* x, const float* ref, const float* noise, const uint8_t* mask, size_t n,
                                           float sqrt_a, float sqrt_1ma) {
   return inpaint_blend_launch((cudaStream_t)stream, x, ref, noise, mask, n, sqrt_a, sqrt_1ma);
@@ -361,7 +374,7 @@ static int guided_step_test(void* stream, const float* eps, int ld, int Bimg, in
                             float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in, float* xh, float* x_in, float* hist,
                             int write_hist, const float* z, const float* zb, uint64_t seed, uint64_t z_subseq, uint64_t zb_subseq,
                             const uint8_t* mask, const float* ref, float sigma_blend, int prediction, const float* factor,
-                            const StepRows* rows) {
+                            const StepRows* rows, int use_img = 0, float s_img = 0.f) {
   GuidedStepParams p{};
   p.eps = eps; p.ld = ld; p.Bimg = Bimg; p.C = C; p.HW = HW; p.use_cfg = use_cfg; p.use_pag = use_pag;
   p.guidance = guidance; p.p_t = p_t; p.sigma = sigma;
@@ -375,7 +388,7 @@ static int guided_step_test(void* stream, const float* eps, int ld, int Bimg, in
     const DScale q = d_scale(prediction, sigma);
     pr.v = 1; pr.dx = q.dx; pr.de = q.de;
   }
-  return guided_step_launch((cudaStream_t)stream, p, pr, rows);
+  return guided_step_launch((cudaStream_t)stream, p, pr, rows, use_img, s_img);
 }
 SDXL_TEST_API int sdxl_test_guided_step_pred(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
                                              float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,
@@ -400,6 +413,23 @@ SDXL_TEST_API int sdxl_test_guided_step_rows(void* stream, const float* eps, int
   r.write_xs = write_xs; r.shift = shift;
   return guided_step_test(stream, eps, ld, Bimg, C, HW, use_cfg, use_pag, guidance, p_t, sigma, cx, cd, ch, cn, c_in, xh, x_in, hist,
                           write_hist, z, zb, seed, z_subseq, zb_subseq, mask, ref, sigma_blend, prediction, factor, &r);
+}
+// sdxl_test_guided_step_rows's arguments (use_cfg = 1, no PAG) with the image-guidance combine at s_img; use_rows = 0: the one-row
+// form, xs, h2, rc, sr, write_xs and shift unread.
+SDXL_TEST_API int sdxl_test_guided_step_img(void* stream, const float* eps, int ld, int Bimg, int C, int HW, float guidance, float s_img,
+                                            float sigma, float cx, float cd, float ch, float cn, float c_in, float* xh, float* x_in,
+                                            float* hist, int write_hist, const float* z, uint64_t seed, uint64_t z_subseq, int prediction,
+                                            const float* factor, int use_rows, float* xs, float* h2, const float* rc, const float* sr,
+                                            int write_xs, int shift) {
+  StepRows r;
+  if (use_rows) {
+    r.xs = xs; r.h2 = h2;
+    r.cs = rc[0]; r.ch2 = rc[1];
+    r.sx = sr[0]; r.ss = sr[1]; r.sd = sr[2]; r.sh = sr[3]; r.sh2 = sr[4];
+    r.write_xs = write_xs; r.shift = shift;
+  }
+  return guided_step_test(stream, eps, ld, Bimg, C, HW, 1, 0, guidance, 0.f, sigma, cx, cd, ch, cn, c_in, xh, x_in, hist, write_hist, z,
+                          nullptr, seed, z_subseq, 0, nullptr, nullptr, 0.f, prediction, factor, use_rows ? &r : nullptr, 1, s_img);
 }
 SDXL_TEST_API int sdxl_test_guided_step(void* stream, const float* eps, int ld, int Bimg, int C, int HW, int use_cfg, int use_pag,
                                         float guidance, float p_t, float sigma, float cx, float cd, float ch, float cn, float c_in,

@@ -3,13 +3,14 @@ from .config import SDXL_BASE, SDXL_REFINER, TINY, TINY_REFINER, SDXL_VAE, TINY_
 from .config import SDXL_CONTROLNET, TINY_CONTROLNET, ControlNetConfig  # noqa: F401
 from .config import SDXL_T2I_ADAPTER, TINY_T2I_ADAPTER, T2IAdapterConfig  # noqa: F401
 from .config import SDXL_INPAINT, TINY_INPAINT  # noqa: F401
+from .config import SDXL_EDIT, TINY_EDIT  # noqa: F401
 from .weights import alphas_cumprod, build_pack, n_params, synth_weights, unet_tensor_specs, vae_decoder_tensor_specs, vae_encoder_tensor_specs, vae_tensor_specs, clip_tensor_specs  # noqa: F401
 from .weights import controlnet_tensor_specs, t2i_adapter_tensor_specs  # noqa: F401
 from ._lib import LIB_PATH, PROTOTYPES, SdxlError, SdxlLibraryMissing, load  # noqa: F401
 from .engine import Conditioning, Context, Diffuser, LatentDecoder, ddim_timesteps  # noqa: F401
 from .tokenizer import ClipTokenizer, OpenClipTokenizer  # noqa: F401
 from .embedder import ClipTextEncoder, Embedder, conditioning_embedding  # noqa: F401
-from .pipeline import load_models, make_inpaint_mask, prepare_inpaint_condition, sample  # noqa: F401
+from .pipeline import load_models, make_inpaint_mask, prepare_edit_latent, prepare_inpaint_condition, sample  # noqa: F401
 from . import diffusers_unet  # noqa: F401
 from . import schedulers  # noqa: F401
 from .schedulers import Schedule  # noqa: F401

@@ -27,7 +27,7 @@ class UnetCfg(C.Structure):
         ("adm_in_channels", C.c_int32), ("in_channels", C.c_int32), ("out_channels", C.c_int32),
         ("model_channels", C.c_int32), ("n_levels", C.c_int32), ("channel_mults", C.c_int32 * SDXL_MAX_LEVELS),
         ("n_head_channels", C.c_int32), ("transformer_depths", C.c_int32 * SDXL_MAX_LEVELS),
-        ("context_dim", C.c_int32), ("is_refiner", C.c_int32), ("n_steps", C.c_int32),
+        ("context_dim", C.c_int32), ("is_refiner", C.c_int32), ("n_steps", C.c_int32), ("edit_layout", C.c_int32),
     ]
 
 
@@ -109,6 +109,11 @@ MAX_T2I_ADAPTERS = 4   # SDXL_MAX_T2I_ADAPTERS (include/sdxl_b200.h)
 
 class InpaintCondition(C.Structure):
     _fields_ = [("cond", C.c_void_p), ("on_host", C.c_int32), ("n", C.c_int32), ("height", C.c_int32), ("width", C.c_int32)]
+
+
+class EditImage(C.Structure):
+    _fields_ = [("latent", C.c_void_p), ("on_host", C.c_int32), ("n", C.c_int32), ("height", C.c_int32), ("width", C.c_int32),
+                ("image_guidance", C.c_float)]
 
 
 class Pag(C.Structure):
@@ -222,6 +227,7 @@ PROTOTYPES = {
     "sdxl_unet_set_t2i_adapters": (I, [P, I, C.POINTER(T2IControl), C.c_int32]),
     "sdxl_t2i_adapter_features": (I, [P, I, I, I, P, I, P]),
     "sdxl_unet_set_inpaint_condition": (I, [P, C.POINTER(InpaintCondition)]),
+    "sdxl_unet_set_edit_image": (I, [P, C.POINTER(EditImage)]),
     "sdxl_unet_num_self_attentions": (I, [P]),
     "sdxl_unet_set_pag": (I, [P, C.POINTER(Pag)]),
     "sdxl_unet_set_freeu": (I, [P, C.POINTER(Freeu)]),

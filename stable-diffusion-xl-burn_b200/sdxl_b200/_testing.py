@@ -76,6 +76,10 @@ PROTOTYPES = {
     "sdxl_test_guidance_stats_scratch_bytes": (Z, [I]),
     "sdxl_test_guidance_stats_scratch_init": (I, [P, P, I]),
     "sdxl_test_guidance_stats": (I, [P, P, I, I, I, I, I, F, F, F, P, P]),
+    "sdxl_test_cfg_ddim_img": (I, [P, P, I, I, I, I, F, F, F, F, F, F, P, I, P]),
+    "sdxl_test_guidance_stats_img": (I, [P, P, I, I, I, I, F, F, F, P, P]),
+    "sdxl_test_guided_step_img": (I, [P, P, I, I, I, I, F, F, F, F, F, F, F, F, P, P, P, I, P, C.c_uint64, C.c_uint64, I, P, I, P, P, P, P,
+                                      I, I]),
     "sdxl_test_guided_step_pred": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, F, F, P, P, P, I, P, P, C.c_uint64, C.c_uint64, C.c_uint64, P,
                                        P, F, I, P]),
     "sdxl_test_guided_step_rows": (I, [P, P, I, I, I, I, I, I, F, F, F, F, F, F, F, F, P, P, P, I, P, P, C.c_uint64, C.c_uint64, C.c_uint64, P,
@@ -377,6 +381,17 @@ def guidance_stats(eps, ld, Bimg, C, HW, use_pag, guidance, p_t, phi, scratch, f
     _call("sdxl_test_guidance_stats", _p(eps), ld, Bimg, C, HW, int(use_pag), guidance, p_t, phi, _p(scratch), _p(factor))
 
 
+def cfg_ddim_img(eps, ld, Bimg, C, HW, guidance, s_img, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, x, v=False, factor=None) -> None:
+    """cfg_ddim_pred with image guidance (DESIGN.md §21): eps rows [cond | img | uncond], e = (u + (c - i) * guidance) + s_img * (i - u)."""
+    _call("sdxl_test_cfg_ddim_img", _p(eps), ld, Bimg, C, HW, guidance, s_img, sqrt_a, sqrt_1ma, sqrt_ap, sqrt_1map, _p(x), int(v),
+          _p(factor))
+
+
+def guidance_stats_img(eps, ld, Bimg, C, HW, guidance, s_img, phi, scratch, factor) -> None:
+    """guidance_stats of the image-guidance combine of the rows [cond | img | uncond]."""
+    _call("sdxl_test_guidance_stats_img", _p(eps), ld, Bimg, C, HW, guidance, s_img, phi, _p(scratch), _p(factor))
+
+
 def inpaint_blend(x, ref, noise, mask, n, sqrt_a, sqrt_1ma) -> None:
     _call("sdxl_test_inpaint_blend", _p(x), _p(ref), _p(noise), _p(mask), n, sqrt_a, sqrt_1ma)
 
@@ -453,6 +468,23 @@ def guided_step_rows(eps, ld, Bimg, Cc, HW, use_cfg, use_pag, guidance, p_t, sig
     _call("sdxl_test_guided_step_rows", _p(eps), ld, Bimg, Cc, HW, int(use_cfg), int(use_pag), guidance, p_t, sigma, cx, cd, ch, cn, c_in,
           _p(xh), _p(x_in), _p(hist), int(write_hist), _p(z), _p(zb), seed, z_subseq, zb_subseq, _p(mask), _p(ref), sigma_blend, int(v),
           _p(factor), _p(xs), _p(h2), rc, sr, int(write_xs), int(shift))
+
+
+def guided_step_img(eps, ld, Bimg, Cc, HW, guidance, s_img, sigma, coef, xh, x_in, hist=None, write_hist=False, z=None, seed=0, z_subseq=0,
+                    v=False, factor=None, rows=None, h2=None, xs=None, write_xs=False, shift=False) -> None:
+    """The step kernel with image guidance on the eps rows [cond | img | uncond]. rows None: the one-row form, coef = (cx, cd, ch, cn,
+    c_in); else the two-row form as guided_step_rows, coef = (cx, cs, cd, ch, ch2, cn, c_in), rows = (sx, ss, sd, sh, sh2)."""
+    if rows is None:
+        cx, cd, ch, cn, c_in = [float(c) for c in coef]
+        cs = ch2 = 0.0
+        rows = (0.0,) * 5
+        use_rows = 0
+    else:
+        cx, cs, cd, ch, ch2, cn, c_in = [float(c) for c in coef]
+        use_rows = 1
+    rc, sr = (C.c_float * 2)(cs, ch2), (C.c_float * 5)(*[float(c) for c in rows])
+    _call("sdxl_test_guided_step_img", _p(eps), ld, Bimg, Cc, HW, guidance, s_img, sigma, cx, cd, ch, cn, c_in, _p(xh), _p(x_in), _p(hist),
+          int(write_hist), _p(z), seed, z_subseq, int(v), _p(factor), use_rows, _p(xs), _p(h2), rc, sr, int(write_xs), int(shift))
 
 
 STAGE_FIELDS = ("t", "sigma", "sigma_next", "cx", "cs", "cd", "ch", "ch2", "cn", "sx", "ss", "sd", "sh", "sh2", "c_in", "write_xs", "hist")

@@ -408,6 +408,10 @@ def read_diffuser_cfg(path: str) -> UNetConfig:
 
 
 def write_diffuser_cfg(path: str, cfg: UNetConfig) -> None:
+    """Refuses an edit UNet (cfg.is_edit): DiffuserConfig has no field for the edit layout, and a record read back without it would
+    load as a plain UNet with an 8-channel latent."""
+    if cfg.is_edit:
+        raise BurnRecordError(f"{path}: DiffuserConfig cannot record the edit layout (is_edit); keep edit UNets in the diffusers format")
     with open(path, "w") as fh:
         json.dump({"adm_in_channels": cfg.adm_in_channels, "model_channels": cfg.model_channels, "channel_mults": list(cfg.channel_mults),
                    "num_head_channels": cfg.n_head_channels, "transformer_depths": list(cfg.transformer_depths), "context_dim": cfg.context_dim,

@@ -22,6 +22,7 @@ class UNetConfig:
     out_channels: int = 4
     n_head_channels: int = 64
     n_steps: int = 1000
+    is_edit: bool = False   # the instruction-editing layout (DESIGN.md §21): in_channels = 2 * out_channels, the second half attached
 
     @property
     def n_levels(self) -> int:
@@ -38,8 +39,8 @@ class UNetConfig:
 
     @property
     def latent_channels(self) -> int:
-        """Channels of the latent the forward and the sampler take (the rest of an inpainting UNet's input is attached)."""
-        return self.out_channels if self.is_inpaint else self.in_channels
+        """Channels of the latent the forward and the sampler take (the rest of an inpainting or edit UNet's input is attached)."""
+        return self.out_channels if self.is_inpaint or self.is_edit else self.in_channels
 
 
 # SDXL base: diffuser.cfg
@@ -58,6 +59,10 @@ TINY_REFINER = UNetConfig(adm_in_channels=16, model_channels=64, channel_mults=(
 # latent as input (4 + 1 + 4 channels), and its tiny counterpart.
 SDXL_INPAINT = replace(SDXL_BASE, in_channels=9)
 TINY_INPAINT = replace(TINY, in_channels=9)
+# The instruction-editing UNet (diffusers/sdxl-instructpix2pix-768): SDXL base with the latent and the source image's latent as input
+# (4 + 4 channels), and its tiny counterpart.
+SDXL_EDIT = replace(SDXL_BASE, in_channels=8, is_edit=True)
+TINY_EDIT = replace(TINY, in_channels=8, is_edit=True)
 
 
 @dataclass(frozen=True)

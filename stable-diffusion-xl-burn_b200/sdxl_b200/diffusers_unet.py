@@ -6,6 +6,7 @@ from __future__ import annotations
 
 import json
 import os
+from dataclasses import replace
 from typing import Callable, Dict, Tuple
 
 import torch
@@ -64,8 +65,8 @@ def encoder_config(cfg: Dict, what: str, in_channels: int, out_channels: int = 4
 
 def config_from_diffusers(config_json) -> UNetConfig:
     """UNetConfig of a diffusers UNet2DConditionModel config.json (dict, JSON text or path). SDXL-base-shaped UNets with
-    in_channels = out_channels (4) or 2 * out_channels + 1 (9, the inpainting layout) are accepted; every other field this engine does
-    not run is refused by name."""
+    in_channels = out_channels (4), 2 * out_channels + 1 (9, the inpainting layout) or 2 * out_channels (8, the InstructPix2Pix edit
+    layout) are accepted; every other field this engine does not run is refused by name."""
     cfg = read_config(config_json)
     what = "unet config"
     ubt = list(cfg.get("up_block_types", []))
@@ -82,9 +83,10 @@ def config_from_diffusers(config_json) -> UNetConfig:
     in_ch = int(cfg.get("in_channels", 4))
     if out_ch != 4:
         raise SdxlError(f"{what}: out_channels = {out_ch} is not supported (only 4)")
-    if in_ch not in (out_ch, 2 * out_ch + 1):
-        raise SdxlError(f"{what}: in_channels = {in_ch} is not supported (only {out_ch}, or {2 * out_ch + 1} for inpainting)")
-    return encoder_config(cfg, what, in_ch, out_ch)
+    if in_ch not in (out_ch, 2 * out_ch + 1, 2 * out_ch):
+        raise SdxlError(f"{what}: in_channels = {in_ch} is not supported (only {out_ch}, {2 * out_ch + 1} for inpainting or "
+                        f"{2 * out_ch} for editing)")
+    return replace(encoder_config(cfg, what, in_ch, out_ch), is_edit=in_ch == 2 * out_ch)
 
 
 def _put(m: Names, src: str, dst: str, lin: bool = False) -> None:

@@ -276,6 +276,7 @@ def _cfg_struct(cfg: UNetConfig) -> _lib.UnetCfg:
     s.context_dim = cfg.context_dim
     s.is_refiner = int(cfg.is_refiner)
     s.n_steps = cfg.n_steps
+    s.edit_layout = int(cfg.is_edit)
     return s
 
 
@@ -377,6 +378,22 @@ class Diffuser:
             s.height, s.width = 8 * cond.shape[2], 8 * cond.shape[3]
         ctx.call("sdxl_unet_set_inpaint_condition", ctx.lib.sdxl_unet_set_inpaint_condition, self.h, None if s is None else C.byref(s))
 
+    def set_edit_image(self, latent: Optional[torch.Tensor], image_guidance: float = 1.5) -> None:
+        """Attaches the edit UNet's source image (sdxl_unet_set_edit_image, DESIGN.md §21); None detaches. latent: f32
+        [n, out_channels, h, w] (pipeline.prepare_edit_latent), image b of a batch uses row b % n; image_guidance: diffusers'
+        image_guidance_scale. The sampling loops with CFG then run [cond | img | uncond] and guide with
+        (u + s * (c - i)) + image_guidance * (i - u)."""
+        ctx = self.ctx
+        s = None
+        if latent is not None:
+            if latent.dim() != 4 or latent.shape[1] != self.cfg.out_channels:
+                raise SdxlError(f"edit image latent must be f32 [n, {self.cfg.out_channels}, h, w], got {tuple(latent.shape)}")
+            latent = latent.to(ctx.device, torch.float32).contiguous()
+            s = _lib.EditImage()
+            s.latent, s.on_host, s.n = latent.data_ptr(), 0, latent.shape[0]
+            s.height, s.width, s.image_guidance = 8 * latent.shape[2], 8 * latent.shape[3], float(image_guidance)
+        ctx.call("sdxl_unet_set_edit_image", ctx.lib.sdxl_unet_set_edit_image, self.h, None if s is None else C.byref(s))
+
     def set_pag(self, layers="mid", scale: float = 3.0, adaptive_scale: float = 0.0) -> None:
         """Attaches perturbed-attention guidance (sdxl_unet_set_pag, DESIGN.md §14); layers None or scale 0 detaches. layers: diffusers'
         pag_applied_layers, one regular expression or a list (pag.layer_mask); the sampler then runs the row groups [cond | uncond |
@@ -464,7 +481,8 @@ class Diffuser:
 
     @classmethod
     def from_diffusers_dir(cls, ctx: Context, path: str) -> "Diffuser":
-        """A diffusers UNet2DConditionModel directory (the `unet/` folder of an SDXL pipeline, base or inpainting): config.json +
+        """A diffusers UNet2DConditionModel directory (the `unet/` folder of an SDXL pipeline: base, inpainting or InstructPix2Pix
+        edit): config.json +
         diffusion_pytorch_model[.fp16].safetensors (diffusers_unet.from_diffusers). When the pipeline's scheduler/scheduler_config.json
         sits next to it and says prediction_type "v_prediction" or rescale_betas_zero_snr true, the model is set to that prediction
         and noise table (schedulers.prediction_of_config, set_prediction); prediction_type "sample" and a beta_schedule other than

@@ -49,13 +49,30 @@ def prepare_inpaint_condition(decoder, rgb: torch.Tensor, pixel_mask: torch.Tens
     return torch.cat([mask_lat, masked_lat], dim=1)
 
 
+def prepare_edit_latent(decoder, rgb: torch.Tensor, size: Optional[Tuple[int, int]] = None) -> torch.Tensor:
+    """The edit UNet's source latent (Diffuser.set_edit_image) of images rgb u8 [n, H, W, 3], as diffusers'
+    StableDiffusionXLInstructPix2PixPipeline.prepare_image_latents makes it: the image (resized bilinearly to size = (height, width)
+    when given and different) mapped to [-1, 1] and encoded to the VAE posterior mean (retrieve_latents(..., sample_mode="argmax")),
+    without the VAE scaling factor: decoder.encode_image's scaled latent divided by it again. Returns f32 [n, latent_channels, H/8, W/8]
+    on the decoder's device."""
+    import torch.nn.functional as F
+    from ._lib import SdxlError
+    if rgb.dim() != 4 or rgb.shape[3] != 3 or rgb.dtype != torch.uint8:
+        raise SdxlError(f"edit image must be u8 [n, H, W, 3], got {rgb.dtype} {tuple(rgb.shape)}")
+    image = rgb.to(decoder.ctx.device).permute(0, 3, 1, 2).to(torch.float32) / 255.0 * 2.0 - 1.0
+    if size is not None and tuple(size) != tuple(image.shape[2:]):
+        image = F.interpolate(image, size=(int(size[0]), int(size[1])), mode="bilinear", align_corners=False)
+    return decoder.encode_image(image.contiguous()) / decoder.cfg.scale_factor
+
+
 def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_steps: int = 30, refiner=None,
            reference_rgb: Optional[torch.Tensor] = None, crop: Sequence[Optional[int]] = (None, None, None, None), crop_out: bool = False,
            resolution: Tuple[int, int] = (1024, 1024), seed: int = 0, noise: Optional[torch.Tensor] = None,
            loras: Optional[Sequence] = None, controls: Optional[Sequence] = None, image_prompt: Optional[Sequence] = None,
            t2i_adapters: Optional[Sequence] = None, t2i_factor: float = 1.0, pag: Optional[Sequence] = None,
            freeu: Optional[Sequence[float]] = None, sampler: Optional[str] = None, spacing: Optional[str] = None,
-           no_cfg: bool = False, deepcache: Optional[Sequence[int]] = None, guidance_rescale: float = 0.0) -> torch.Tensor:
+           no_cfg: bool = False, deepcache: Optional[Sequence[int]] = None, guidance_rescale: float = 0.0,
+           edit_image: Optional[torch.Tensor] = None, image_guidance: float = 1.5) -> torch.Tensor:
     """One image, like `sample --prompt ... [--reference-img ... --crop-* ...] [--use-refiner]`.
     reference_rgb: uint8 [1, H, W, 3] (the reference image: switches to inpainting, main.rs:131-197); crop = (left, right, top,
     bottom) in pixels. With an inpainting UNet (cfg.is_inpaint, DESIGN.md §12) reference_rgb is required: the crop window becomes the
@@ -80,8 +97,12 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
     loop. deepcache: (interval[, branch]) DeepCache (Diffuser.set_deepcache) attached to the base UNet for this call and detached
     afterwards (the refiner is left alone). guidance_rescale: diffusers' guidance_rescale (phi, DESIGN.md §18) set on the base UNet
     for this call, with the prediction type and noise table the model has (Diffuser.set_prediction), and the previous phi restored
-    afterwards. Returns uint8 [1, H, W, 3]."""
-    sch = dict(sampler=sampler, spacing=spacing, no_cfg=no_cfg)
+    afterwards. edit_image: u8 [1, H, W, 3], required with an edit UNet (cfg.is_edit, DESIGN.md §21) and refused otherwise: the output
+    has the image's size, its latent (prepare_edit_latent) is attached for the call with image_guidance (diffusers'
+    image_guidance_scale) and detached afterwards. As diffusers does, the call runs without CFG (no_cfg) when guidance <= 1 or
+    image_guidance < 1; without a sampler or spacing that is the reference's DDIM update (Euler on the reference spacing). Returns
+    uint8 [1, H, W, 3]."""
+    sch = dict(sampler=sampler, spacing=spacing, no_cfg=no_cfg, edit_image=edit_image, image_guidance=image_guidance)
     if guidance_rescale:
         prev = diffuser.prediction
         diffuser.set_prediction(prev[0], guidance_rescale, alphas=prev[2])
@@ -138,7 +159,7 @@ def sample(embedder, diffuser, decoder, prompt: str, guidance: float = 7.5, n_st
         finally:
             diffuser.set_controls([])
     if t2i_adapters:
-        schedule = _schedule(n_steps, **sch)
+        schedule = _schedule(n_steps, sampler, spacing, no_cfg)
         if schedule is None:
             from .t2i_adapter import t2i_t_min
             t_min = t2i_t_min(n_steps, t2i_factor)
@@ -198,7 +219,31 @@ def refiner_schedule(refiner, schedule):
 
 
 def _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution, seed, noise,
-            sampler=None, spacing=None, no_cfg=False):
+            sampler=None, spacing=None, no_cfg=False, edit_image=None, image_guidance=1.5):
+    if diffuser.cfg.is_edit != (edit_image is not None):
+        raise _lib.SdxlError("sample: an edit UNet needs edit_image (the image to edit)" if diffuser.cfg.is_edit else
+                             "sample: edit_image needs an edit UNet (cfg.is_edit)")
+    if edit_image is None:
+        return _sample_image(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution,
+                             seed, noise, sampler, spacing, no_cfg)
+    if refiner is not None or reference_rgb is not None:
+        raise _lib.SdxlError("sample: edit_image does not go with a refiner or reference_rgb")
+    if guidance <= 1 or image_guidance < 1:   # diffusers' do_classifier_free_guidance is off
+        no_cfg = True
+        spacing = spacing or (None if sampler else "reference")
+    resolution = (int(edit_image.shape[1]), int(edit_image.shape[2]))
+    latent = prepare_edit_latent(decoder, edit_image, resolution)
+    diffuser.set_edit_image(latent, image_guidance)
+    try:
+        return _sample_image(embedder, diffuser, decoder, prompt, guidance, n_steps, None, None, crop, crop_out, resolution, seed, noise,
+                             sampler, spacing, no_cfg, tuple(latent.shape[2:]))
+    finally:
+        diffuser.set_edit_image(None)
+
+
+def _sample_image(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, reference_rgb, crop, crop_out, resolution, seed, noise,
+                  sampler=None, spacing=None, no_cfg=False, latent_hw=None):
+    """latent_hw: the extent of an attached edit image's latent, which the sampled latent takes (the image size / the VAE's factor)."""
     schedule = _schedule(n_steps, sampler, spacing, no_cfg)
     kw = {} if schedule is None else {"schedule": schedule}   # None: the calls below are the reference's, argument for argument
     refine = refiner_schedule(refiner, schedule) if refiner is not None and schedule is not None else None   # before any sampling
@@ -209,6 +254,8 @@ def _sample(embedder, diffuser, decoder, prompt, guidance, n_steps, refiner, ref
         resolution = (int(reference_rgb.shape[1]), int(reference_rgb.shape[2]))        # main.rs:225-229: orig_dims
     size = [int(resolution[0]), int(resolution[1])]
     cond = embedder.text_to_conditioning(prompt, size, [0, 0], size)                     # main.rs:231-235: size, crop = 0, ar = size
+    if latent_hw is not None:
+        cond.resolution = (8 * int(latent_hw[0]), 8 * int(latent_hw[1]))
     if inpaint_unet:
         # the UNet sees the mask and the masked image at every step and samples from noise, without blending (as diffusers does
         # for 9-channel UNets); the crop window at scale 1 is the exact pixel box, 1 = repaint
