@@ -11,6 +11,7 @@ import torch.nn.functional as F
 from sdxl_b200 import TINY, TINY_REFINER
 from sdxl_b200 import _testing as T
 
+U23 = 2.0 ** -23      # one f32 ulp (relative)
 U24 = 2.0 ** -24      # f32 unit roundoff
 H11 = 2.0 ** -11      # f16 unit roundoff
 H_SUB = 2.0 ** -25    # half the f16 subnormal spacing
@@ -72,12 +73,14 @@ def pad64(k: int) -> int:
     return (k + 63) // 64 * 64
 
 
-def check(out: torch.Tensor, ref: torch.Tensor, tol: torch.Tensor, what: str) -> None:
+def check(out: torch.Tensor, ref: torch.Tensor, tol: torch.Tensor, what: str) -> float:
+    """Every element of out within tol of ref; a NaN in out, ref or tol counts as outside. Returns the worst err / bound."""
     err = (out.double() - ref).abs()
-    bad = err > tol
-    worst = float((err / tol.clamp_min(1e-300)).max())
+    bad = ~(err <= tol)
+    worst = float((err / tol.clamp_min(1e-300)).nan_to_num(nan=float("inf")).max())
     print(f"{what}: max err {float(err.max()):.3e}, worst err / bound {worst:.3f}")
     assert not bool(bad.any()), f"{what}: {int(bad.sum())} elements outside the bound (worst err / bound {worst:.2f})"
+    return worst
 
 
 def f16_round_bound(ref: torch.Tensor) -> torch.Tensor:
@@ -86,6 +89,46 @@ def f16_round_bound(ref: torch.Tensor) -> torch.Tensor:
 
 def nchw(x: torch.Tensor) -> torch.Tensor:
     return x.permute(0, 3, 1, 2)
+
+
+# ------------------------------------------------------------------------------------------------------------------------------
+# attention (test_fused_paths_gpu.py, test_attention_plans_gpu.py): head views of the plan's row-major matrices, float64 softmax
+# ------------------------------------------------------------------------------------------------------------------------------
+def heads(m: torch.Tensor, B: int, rows: int, col0: int, nh: int, d: int) -> torch.Tensor:
+    """[B * rows, pitch] -> [B, nh, rows, d] float64 view of the column window starting at col0."""
+    return m.view(B, rows, -1)[:, :, col0:col0 + nh * d].double().reshape(B, rows, nh, d).permute(0, 2, 1, 3)
+
+
+def attn_ref(q, k, v, scale, mask=None, causal=False, p_f16=True):
+    """float64 softmax(q k^T scale + mask) v, and the bound on the kernel's error before its f16 output rounding:
+    - the f32 score: (d + 1) 2^-23 sum_i |q_i k_i| scale, plus exp's argument rounding and its approximation 2^-21
+      (relative error of each p, and of l);
+    - P rounded to f16 (flash kernel): 2^-11 p, or 2^-25 absolute for a subnormal p (p <= 1, so l >= 1);
+    - f32 accumulation of S terms of p v and of l."""
+    d, S = q.shape[-1], k.shape[-2]
+    s = q @ k.transpose(-1, -2) * scale
+    sabs = q.abs() @ k.abs().transpose(-1, -2) * scale
+    if mask is not None:
+        s = s + mask
+    if causal:
+        T_ = q.shape[-2]
+        s = s.masked_fill(torch.ones(T_, S, dtype=torch.bool, device=s.device).triu(1), float("-inf"))
+    m = s.amax(dim=-1, keepdim=True)
+    P = torch.softmax(s, dim=-1)
+    ref = P @ v
+    pv = P @ v.abs()
+    eps_s = ((d + 1) * U23 * sabs.amax(dim=-1, keepdim=True) + 2 * U24 * (s.abs().masked_fill(s.isinf(), 0).amax(dim=-1, keepdim=True)
+             + m.abs().nan_to_num(0)) + 2.0 ** -21)
+    tol = (2 * eps_s + S * U23) * pv + (eps_s + S * U24) * ref.abs()
+    if p_f16:
+        tol = tol + H11 * pv + H_SUB * v.abs().sum(dim=-2, keepdim=True)
+    return ref, tol
+
+
+def to_rows(x: torch.Tensor) -> torch.Tensor:
+    """[B, nh, rows, d] -> [B * rows, nh * d]"""
+    B, nh, rows, d = x.shape
+    return x.permute(0, 2, 1, 3).reshape(B * rows, nh * d)
 
 
 def conv_taps(nkb: int, map_: int = 0):

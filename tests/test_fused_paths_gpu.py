@@ -22,12 +22,10 @@ import torch.nn.functional as F
 
 from sdxl_b200 import SdxlError
 from sdxl_b200 import _testing as T
-from harness import (DEV, H11, H_SUB, U24, check, conv_taps, f16_round_bound, gn_ref, nchw, pad64, plan_upconv,
-                     repack3)
+from harness import (DEV, H11, H_SUB, U23, U24, attn_ref, check, conv_taps, f16_round_bound, gn_ref, heads, nchw, pad64,
+                     plan_upconv, repack3, to_rows)
 
 pytestmark = pytest.mark.gpu
-
-U23 = 2.0 ** -23      # one f32 ulp (relative)
 
 
 def f16(t: torch.Tensor) -> torch.Tensor:
@@ -329,43 +327,6 @@ def test_layer_norm_rejects(ctx):
 # ------------------------------------------------------------------------------------------------------------------------------
 # attention
 # ------------------------------------------------------------------------------------------------------------------------------
-def heads(m: torch.Tensor, B: int, rows: int, col0: int, nh: int, d: int) -> torch.Tensor:
-    """[B * rows, pitch] -> [B, nh, rows, d] float64 view of the column window starting at col0."""
-    return m.view(B, rows, -1)[:, :, col0:col0 + nh * d].double().reshape(B, rows, nh, d).permute(0, 2, 1, 3)
-
-
-def attn_ref(q, k, v, scale, mask=None, causal=False, p_f16=True):
-    """float64 softmax(q k^T scale + mask) v, and the bound on the kernel's error before its f16 output rounding:
-    - the f32 score: (d + 1) 2^-23 sum_i |q_i k_i| scale, plus exp's argument rounding and its approximation 2^-21
-      (relative error of each p, and of l);
-    - P rounded to f16 (flash kernel): 2^-11 p, or 2^-25 absolute for a subnormal p (p <= 1, so l >= 1);
-    - f32 accumulation of S terms of p v and of l."""
-    d, S = q.shape[-1], k.shape[-2]
-    s = q @ k.transpose(-1, -2) * scale
-    sabs = q.abs() @ k.abs().transpose(-1, -2) * scale
-    if mask is not None:
-        s = s + mask
-    if causal:
-        T_ = q.shape[-2]
-        s = s.masked_fill(torch.ones(T_, S, dtype=torch.bool, device=s.device).triu(1), float("-inf"))
-    m = s.amax(dim=-1, keepdim=True)
-    P = torch.softmax(s, dim=-1)
-    ref = P @ v
-    pv = P @ v.abs()
-    eps_s = ((d + 1) * U23 * sabs.amax(dim=-1, keepdim=True) + 2 * U24 * (s.abs().masked_fill(s.isinf(), 0).amax(dim=-1, keepdim=True)
-             + m.abs().nan_to_num(0)) + 2.0 ** -21)
-    tol = (2 * eps_s + S * U23) * pv + (eps_s + S * U24) * ref.abs()
-    if p_f16:
-        tol = tol + H11 * pv + H_SUB * v.abs().sum(dim=-2, keepdim=True)
-    return ref, tol
-
-
-def to_rows(x: torch.Tensor) -> torch.Tensor:
-    """[B, nh, rows, d] -> [B * rows, nh * d]"""
-    B, nh, rows, d = x.shape
-    return x.permute(0, 2, 1, 3).reshape(B * rows, nh * d)
-
-
 @pytest.mark.parametrize("B,T_,nh", [(1, 1, 1), (3, 129, 5), (1, 128, 1), (3, 127, 20), (1, 4096, 5)])
 def test_flash_attention_fused_qkv(ctx, B, T_, nh):
     """Self-attention as strans runs it: q, k and v are the column windows 0, C, 2C of one [B*T, 3C] QKV matrix."""
